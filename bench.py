@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- moment-match rollout steps/s of the B200-native PILCO engine (BASELINE.json metric).
+"""bench.py -- moment-match rollout steps/s of the H100-native PILCO engine (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                     [--config metric|inverted_pendulum|inv_double_pendulum|smgpr|swimmer|test_cascade]
-                    [--restarts R] [--through-api]
+                    [--restarts R] [--through-api] [--dump-outputs DIR]
 
 One bench "step" = one pass of the hot path over one batch: an H-step moment-matching rollout
 (policy moment match -> squash -> joint -> dynamics moment match -> glue -> reward, pilco.py:118-153)
@@ -15,6 +15,10 @@ H=40, RBF policy with 50 basis functions, fp64, synthetic seeded data, R=32 rest
 `--through-api` (any config) drives `PILCO.optimize_policy(restarts=R*N)` itself -- lock-step L-BFGS-B,
 taped forward + reverse sweep per evaluation, one all_gather of [loss | params] -- and reports wall-clock
 loss-evaluations x R x H / s.
+
+Every timed arm runs W untimed and K timed steps.  `--dump-outputs DIR` writes, after the timed steps, what each timed
+arm computed in its last step as DIR/<name>.npy (float64; inputs are seeded, so two builds can be compared output for
+output).
 
 Rank 0 prints ONE JSON line.  `--impl reference` times the reference-equivalent CPU path
 (oracle/torch_port.py, all host threads it can use) on bounded samples of the same workload.
@@ -52,6 +56,7 @@ CONFIGS = {
                     name="swimmer.py: N=500 E=8 D=10 H=50, RBF bf=40, 256 restarts over 8 GPUs (32 per GPU)"),
 }
 UNIT = "rollout-steps/s"
+DUMP_LIMIT = 64 * 1024 * 1024   # bytes of --dump-outputs; beyond it a fixed, seeded sample of the restarts is written
 EXP_FLOP_EQ = 14.0          # fp64 flop-equivalents of one exp: exp_shifted()'s 7 fp64-pipe instructions (3 DADD, 3 DFMA, DMUL), 2 each
 
 
@@ -381,17 +386,24 @@ def run_through_api(args, cfg):
     wl = make_workload(cfg)
     p = build_pilco(cfg, wl, make_policies(cfg, [0]))
     sink = io.StringIO()
+    # one bench step = one PILCO.optimize_policy(maxiter, restarts) call; the first (warm-up) call builds the evaluator and
+    # captures its graph
+    evals = rollout_steps = 0
     with contextlib.redirect_stdout(sink):                 # (randomize() / optimize_policy() print per restart)
-        p.optimize_policy(maxiter=2, restarts=R * world)   # warm-up: builds the evaluator, captures its graph
+        for _ in range(args.warmup):
+            p.optimize_policy(maxiter=args.maxiter, restarts=R * world)
         torch.cuda.synchronize()
         if world > 1:
             dist.barrier()
         t0 = time.perf_counter()
-        reward = p.optimize_policy(maxiter=args.maxiter, restarts=R * world)
+        for _ in range(args.steps):
+            reward = p.optimize_policy(maxiter=args.maxiter, restarts=R * world)
+            st = dict(policy_opt.LAST_STATS)
+            evals += st["evals"]
+            rollout_steps += st.get("rollout_steps", st["evals"] * st["restarts_local"] * st["horizon"])
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
-    st = dict(policy_opt.LAST_STATS)
-    tt = torch.tensor([dt, float(st.get("rollout_steps", st["evals"] * st["restarts_local"] * st["horizon"]))], dtype=torch.float64, device="cuda")
+    tt = torch.tensor([dt, float(rollout_steps)], dtype=torch.float64, device="cuda")
     if world > 1:
         tmax = tt.clone(); dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
         tsum = tt.clone(); dist.all_reduce(tsum, op=dist.ReduceOp.SUM)
@@ -401,12 +413,15 @@ def run_through_api(args, cfg):
     if rank == 0:
         print(json.dumps({
             "metric": metric_name(cfg) + " through PILCO.optimize_policy", "value": steps / dt, "unit": UNIT, "n_gpus": world,
-            "steps": args.maxiter, "warmup": 2, "ms_per_step": 1e3 * dt / max(st["evals"], 1), "higher_is_better": True,
+            "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
-            "config": {"workload": "%s; PILCO.optimize_policy(maxiter=%d, restarts=%d): lock-step L-BFGS-B, forward + reverse sweep per evaluation, wall clock incl. SciPy and host<->device copies"
+            "config": {"workload": "%s; each step one PILCO.optimize_policy(maxiter=%d, restarts=%d): lock-step L-BFGS-B, forward + reverse sweep per evaluation, wall clock incl. SciPy and host<->device copies"
                                    % (cfg["name"], args.maxiter, R * world), "restarts_per_gpu": R},
-            "loss_evaluations": st["evals"], "lockstep_groups": st.get("groups", 1), "wall_s": dt, "best_reward": float(reward),
+            "loss_evaluations": evals, "ms_per_loss_evaluation": 1e3 * dt / max(evals, 1), "lockstep_groups": st.get("groups", 1),
+            "wall_s": dt, "best_reward": float(reward),
         }))
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"best_reward": np.array([float(reward)])}, 1)
     if world > 1:
         dist.destroy_process_group()
 
@@ -468,7 +483,7 @@ def run_ours(args, cfg):
         return engine.RolloutPlan(gp, policy_spec(lo, hi, pgps), rew, wl["m0"], wl["S0"], H, R=hi - lo, grad=grad)
 
     split = engine.SplitRollout(make_plan, R, nsplit=nsplit)
-    flush = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device=d)       # > L2 (126 MB)
+    flush = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device=d)       # > L2 (50 MB on H100)
     gathered = [torch.empty(R, dtype=torch.float64, device=d) for _ in range(world)]
 
     def step_resident():
@@ -640,19 +655,32 @@ def run_ours(args, cfg):
     sampler = ClockSampler(local) if rank == 0 else None
     if sampler:
         sampler.start()
+    outputs = {}                                           # --dump-outputs: each timed arm's results of its last step
+
+    def plan_outputs(sp, prefix, grad_keys=()):
+        outputs[prefix + "reward"] = sp.reward.cpu().numpy()
+        for k in grad_keys:
+            outputs[prefix + "grad_" + k] = torch.cat([p.gbuf[k] for p in sp.plans]).cpu().numpy()
     ms_res = timed(step_resident, args.steps, args.warmup)
     ok = int(split.info.max().item()) == 0 and bool(torch.isfinite(split.reward).all().item())
+    plan_outputs(split, "")
+    outputs["traj_m"] = torch.cat([p.traj_m for p in split.plans]).cpu().numpy()
+    outputs["traj_S"] = torch.cat([p.traj_S for p in split.plans]).cpu().numpy()
     ms_e2e = timed(step_e2e, args.steps, args.warmup)
+    outputs["e2e_reward"] = h_out.numpy().copy()
     ms_fb = ms_fb_e2e = ms_fbg = ms_fbg_e2e = None
     if split3 is not None:
-        kb = max(3, args.steps // 2)
-        ms_fb = timed(step_fwd_bwd, kb, 3)
-        ms_fb_e2e = timed(step_fwd_bwd_e2e, kb, 3)
+        ms_fb = timed(step_fwd_bwd, args.steps, args.warmup)
+        plan_outputs(split3, "fwd_bwd_", gkeys)
+        ms_fb_e2e = timed(step_fwd_bwd_e2e, args.steps, args.warmup)
+        outputs["fwd_bwd_e2e_reward_grad"] = h_grad.numpy().copy()
         if G > 1:
-            pipeline(3, False)
+            pipeline(args.warmup, False)
             ms_fbg = pipeline(args.steps, False) / args.steps
-            pipeline(3, True)
+            outputs["fwd_bwd_grouped_reward"] = torch.cat([g_.reward for g_ in gsplit3]).cpu().numpy()
+            pipeline(args.warmup, True)
             ms_fbg_e2e = pipeline(args.steps, True) / args.steps
+            outputs["fwd_bwd_grouped_e2e_reward_grad"] = h_grad.numpy().copy()
     if sampler:
         sampler.stop_flag = True
         sampler.join(timeout=2)
@@ -713,11 +741,18 @@ def run_ours(args, cfg):
     # 256 FMA = 512 flop each
     sink = torch.zeros(8, dtype=torch.float64, device=d)
     msf = C.c_float()
-    iters, blocks = 20000, 148 * 4
+    iters, blocks = 20000, torch.cuda.get_device_properties(d).multi_processor_count * 4
     _lib.check(lib.pilco_microbench_fp64(0, iters, blocks, ptr(sink), C.byref(msf), stream_ptr()))
     dfma_tf = 2 * blocks * 256 * iters * 8.0 / (msf.value * 1e-3) / 1e12
     _lib.check(lib.pilco_microbench_fp64(1, iters, blocks, ptr(sink), C.byref(msf), stream_ptr()))
     dmma_tf = blocks * 8 * iters * 8.0 * 512 / (msf.value * 1e-3) / 1e12
+    # Hopper's native fp64 MMA shapes (DMMA.16x8x8 / 16x8x16, 2048 / 4096 flop per warp instruction): the fp64 tensor rate
+    # the tile kernels' DMMA.8x8x4 is compared against
+    native_tf = {}
+    for which, shape, flop in ((5, "m16n8k8", 2048), (6, "m16n8k16", 4096)):
+        _lib.check(lib.pilco_microbench_fp64(which, iters // 4, blocks, ptr(sink), C.byref(msf), stream_ptr()))
+        native_tf[shape] = blocks * 8 * (iters // 4) * 8.0 * flop / (msf.value * 1e-3) / 1e12
+    tensor_peak = max(native_tf.values())
     # independent library denominator (NOT on the product path): cuBLAS DGEMM through torch.matmul
     lib_tf, nmm = None, 6144
     try:
@@ -754,29 +789,23 @@ def run_ours(args, cfg):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    traffic = tsrc = None                # dram bytes per launch of the same kernel/config from the committed ncu --set full capture
-    if cfg is CONFIGS["metric"] and R == 32:
-        for fn in ("r02_tile_traffic.json", "r01_tile_traffic.json"):
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", fn)))["dram_bytes_per_launch"]
-                tsrc = "profiles/" + fn + " (ncu --set full, same kernel and config; cold caches: in the pipeline the operands written by the setup kernel are L2 hits)"
-                break
-            except Exception:
-                pass
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)                    # H100 SXM data sheet: 3.35 TB/s HBM3
     roofline = dict(rf)
     roofline.update({
-        "bound": "tensor", "traffic": traffic, "traffic_source": tsrc,
-        "algorithmic_bytes": alg_bytes, "traffic_over_algorithmic": (traffic / alg_bytes) if traffic else None,
+        "bound": "tensor", "algorithmic_bytes": alg_bytes,
         "peak_source": "fp64 pipe measured live by pilco_microbench_fp64 (DFMA %.1f, DMMA %.1f TFLOP/s: 512 flop per warp-level DMMA.8x8x4), "
                        "time-weighted for this kernel's op mix; MEASURED_PEAKS.json holds no fp64 figure" % (dfma_tf, dmma_tf),
         "fp64_library_tflops": lib_tf,
         "fp64_library_note": "cuBLAS DGEMM %d^3 through torch.matmul in this process: independent denominator only, not on the product path" % nmm,
         "frac_of_library": (rf["achieved"] / lib_tf) if lib_tf else None,
+        "fp64_tensor_native_tflops": native_tf,
+        "frac_of_fp64_tensor_peak": rf["achieved"] / tensor_peak,
+        "fp64_tensor_note": "the Q-contraction runs on DMMA.8x8x4 (mma.sync m8n8k4), which reaches %.1f TFLOP/s; Hopper's native fp64 "
+                            "shapes reach %.1f (m16n8k8) / %.1f (m16n8k16)" % (dmma_tf, native_tf["m16n8k8"], native_tf["m16n8k16"]),
         "setup_kernel_ms": setup_ms,
         "hbm": {"achieved_gbs": alg_bytes / (tile_ms * 1e-3) / 1e9, "peak_gbs": hbm_peak,
                 "frac": alg_bytes / (tile_ms * 1e-3) / 1e9 / hbm_peak,
-                "peak_source": "MEASURED_PEAKS.json" if peaks else "fallback"},
+                "peak_source": "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet"},
     })
     # whole step: SURVEY 8d flop + exp count of one rollout step x steps / measured time
     F, Xe, Bs = step_counts(cfg)
@@ -802,7 +831,7 @@ def run_ours(args, cfg):
                                "(x %d sub-batches on parallel streams), each group's evaluations back to back on its own stream, "
                                "groups %.1f ms out of phase (offset inside the timed region) -- the schedule policy_opt.optimize runs"
                                % (G, R // G, nsplit_b, stagger_ms),
-                       "l2": "no flush between the pipelined steps: a step writes and re-reads its tape (%.1f GB per step over all restarts), far beyond the 126 MB L2"
+                       "l2": "no flush between the pipelined steps: a step writes and re-reads its tape (%.1f GB per step over all restarts), far beyond the 50 MB L2"
                              % (1e-9 * sum(pl.tape.numel() * 8 for sp in gsplit3 for pl in sp.plans if pl.tape is not None))})
             fb["e2e"].update({"value": total_steps / (ms_fbg_e2e * 1e-3), "ms_per_step": ms_fbg_e2e,
                               "what": fb["e2e"]["what"] + "; one host thread per group, stream-synchronised after every evaluation"})
@@ -812,6 +841,7 @@ def run_ours(args, cfg):
             fb["roofline"] = tile_block(ttile_ms, float(P) * nn * R, 2.0 * (D + 1), 4.0,
                                         "mm_tape_tile_kernel<%d> (taped dynamics pass: Q-contraction + exp + H.[Z,1] product + column sums)" % ks, 0.0)
             fb["roofline"]["bound"] = "tensor"
+            fb["roofline"]["frac_of_fp64_tensor_peak"] = fb["roofline"]["achieved"] / tensor_peak
     cpu = {"value": None, "unit": UNIT, "cores": 0, "kind": "port", "sample": "skipped (--no-cpu-baseline)"}
     if args.cpu_baseline:
         cr = CpuRollout(cfg, wl)
@@ -840,8 +870,23 @@ def run_ours(args, cfg):
         "clocks": sampler.summary() if sampler else None,
     }
     print(json.dumps(line))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs, R)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path, arrays, R):
+    """arrays: name -> ndarray with the R restarts of this rank first.  Written as float64 .npy; over DUMP_LIMIT bytes,
+    the same seeded sample of restarts is taken from every array (its indices go to restart_index.npy)."""
+    os.makedirs(path, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        keep = np.sort(np.random.RandomState(0).choice(R, max(1, int(R * DUMP_LIMIT // total)), replace=False))
+        arrays = {k: a[keep] for k, a in arrays.items()}
+        arrays["restart_index"] = keep
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), np.asarray(a, dtype=np.float64))
 
 
 def main():
@@ -860,8 +905,14 @@ def main():
     ap.add_argument("--groups", type=int, default=2, help="lock-step groups of the forward+backward arms (policy_opt.GROUPS); 1 = one batch")
     ap.add_argument("--stagger-ms", type=float, default=0.0, help="phase offset between the groups (default: one group's evaluation time / groups)")
     ap.add_argument("--through-api", action="store_true", help="drive PILCO.optimize_policy itself (lock-step L-BFGS-B, sharded restarts)")
-    ap.add_argument("--maxiter", type=int, default=10, help="--through-api: L-BFGS-B iterations")
+    ap.add_argument("--maxiter", type=int, default=10, help="--through-api: L-BFGS-B iterations per optimize_policy call (one bench step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write each timed arm's last-step results as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU arms' results; the reference arm has none")
     cfg = CONFIGS[args.config]
     # Exactly ONE line on stdout (the JSON): everything any library writes to file descriptor 1 meanwhile (NCCL's
     # "NCCL version ..." banner is written by C code, not through sys.stdout) is sent to stderr; the JSON line is

@@ -5,7 +5,7 @@ examples/utils.py:7-36): collect (x,u)->dx data with random actions, then iterat
   optimize_models -> optimize_policy (batched restarts on the device) -> rollout with the learnt policy ->
   append data -> set_data.
 The environment is a stand-in for gym/mujoco (not installable offline); everything from ``pilco`` is the
-B200-native engine.  Usage:  python examples/pendulum_numpy.py [--iters 3]"""
+H100-native engine.  Usage:  python examples/pendulum_numpy.py [--iters 3]"""
 import argparse
 import os
 import sys

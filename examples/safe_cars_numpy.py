@@ -7,7 +7,7 @@ additive LinearReward (progress) and a multiplicative RiskOfCollision (both cars
 per iteration: optimize_models, optimize_policy, predicted per-step risks along the planned trajectory
 (``pilco.predict`` for every prefix + ``RiskOfCollision.compute_reward``), act with ``compute_action`` only when the
 predicted overall risk is below the threshold, adapt ``mu``.  Everything imported from ``pilco`` /
-``safe_pilco_extension`` is the B200-native engine.  Usage:  python examples/safe_cars_numpy.py [--iters 3]"""
+``safe_pilco_extension`` is the H100-native engine.  Usage:  python examples/safe_cars_numpy.py [--iters 3]"""
 import argparse
 import os
 import sys

@@ -1,9 +1,9 @@
 /*
- * pilco_b200.h -- C ABI of the B200-native PILCO moment-matching rollout engine.
+ * pilco_b200.h -- C ABI of the H100-native PILCO moment-matching rollout engine.
  *
  * The reference (nrontsis/PILCO) has no FFI: its hot path is TensorFlow ops composed in Python.
  * This ABI is therefore the boundary placed directly beneath the reference's Python class API;
- * each entry point names the reference function (file:line under /root/reference) it replaces.
+ * each entry point names the reference function (file:line in nrontsis/PILCO) it replaces.
  *
  * Rules (all entry points):
  *   - every pointer is a DEVICE pointer to contiguous fp64 (or int32 for `info`), owned by the caller
@@ -278,8 +278,8 @@ int    pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad*
 
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
- * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp; 8 ops/thread/iteration (16 DMMA for
- * which=1,2 counted as 8 pairs).  Synchronises (it times itself with CUDA events) -- never call it in a
+ * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;
+ * 8 ops/thread/iteration (16 DMMA for which=1,2 counted as 8 pairs; 8 MMAs per warp for which=5,6).  Synchronises (it times itself with CUDA events) -- never call it in a
  * captured region. */
 /* pilco_mm_forward with CUDA events around its three launches: ms_out[0..2] = setup, tile, finish.
  * Synchronises. */

@@ -1,4 +1,4 @@
-"""Drop-in alias: ``import pilco`` resolves to the B200-native engine (``pilco_b200``), so the reference's
+"""Drop-in alias: ``import pilco`` resolves to the H100-native engine (``pilco_b200``), so the reference's
 ``tests/`` and ``examples/`` import lines (``from pilco.models import MGPR`` ...) work unchanged."""
 import sys
 

@@ -1,8 +1,8 @@
-"""Build the sm_100a shared library in-tree with nvcc (cross-compiles without a GPU).
+"""Build the sm_90a (H100) shared library in-tree with nvcc (cross-compiles without a GPU).
 
     python -m pilco_b200.build
 
-Produces ``pilco_b200/libpilco_b200.so`` (git-ignored; travels to the GPU box with the snapshot).
+Produces ``pilco_b200/libpilco_b200.so`` (git-ignored build product).
 """
 import os
 import subprocess
@@ -13,7 +13,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpilco_b200.so")
 SOURCES = ["abi.cu", "mm_forward.cu", "mm_backward.cu", "mm_tape.cu", "closed_forms.cu", "factorize.cu", "rollout.cu",
            "rollout_bwd.cu", "microbench.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 (Hopper)
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-rdc=false"]
 
 
@@ -57,7 +58,7 @@ def build(force=False, verbose=False, extra_flags=(), lib=None, build_dir=None):
         if verbose and out:
             sys.stderr.write(out)
     out_lib = lib or LIB
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out_lib] + objs + ["-lcudart"]
+    cmd = [nvcc, "-shared"] + GENCODE + ["-o", out_lib] + objs + ["-lcudart"]
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if res.returncode != 0:
         raise RuntimeError("link failed:\n" + res.stdout)

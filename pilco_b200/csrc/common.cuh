@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the PILCO B200 engine (sm_100a).
+// common.cuh -- shared device helpers for the PILCO engine (sm_90a).
 //
 // Small dense linear algebra on D<=16 matrices held in shared memory (one warp cooperates),
 // the table-driven fp64 exp used by the tile kernels, DMMA wrappers, TMA bulk-copy wrappers.
@@ -19,7 +19,7 @@
 #define MAXD PILCO_MAX_D
 #define MAXE PILCO_MAX_E
 #define SLD  17                 // leading dimension of small smem matrices (odd -> conflict-light)
-#define PILCO_MAX_SMEM_OPTIN (227 * 1024)   // dynamic shared memory a CTA can opt in to on sm_100
+#define PILCO_MAX_SMEM_OPTIN (227 * 1024)   // dynamic shared memory a CTA can opt in to on sm_90
 #define NEG_PAD (-1.0e9)        // (scaled) exponent of padded rows/cols: exp_scaled() clamps it to ~1e-304
 
 #define CUDA_LAUNCH_CHECK() do { cudaError_t e__ = cudaGetLastError(); if (e__ != cudaSuccess) return PILCO_ERR_LAUNCH; } while (0)
@@ -199,6 +199,17 @@ static inline int pilco_current_device() {
     if (cudaGetDevice(&d) != cudaSuccess || d < 0) d = 0;
     return d < PILCO_MAX_DEVICES ? d : PILCO_MAX_DEVICES - 1;
 }
+// SMs of the current device (cached per device): the launch heuristics size grids against the machine
+static inline int pilco_sm_count() {
+    static int count[PILCO_MAX_DEVICES] = {0};
+    int& c = count[pilco_current_device()];
+    if (c == 0) {
+        int d = 0, v = 0;
+        cudaGetDevice(&d);
+        c = (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d) == cudaSuccess && v > 0) ? v : 132;
+    }
+    return c;
+}
 static inline int exp_table_upload() { return PILCO_OK; }
 
 // ---------------------------------------------------------------------------------------------
@@ -227,8 +238,7 @@ static inline int pilco_hi_priority() {
 // (lets the NEXT grid's CTAs be scheduled early; they park in their own pdl_wait).  With the stream-serialisation
 // attribute the launch latency and grid drain/fill gaps between the ~15 dependent kernels of a rollout step overlap
 // instead of adding up.  Stream capture turns these into programmatic graph edges.
-// MEASURED (round 2): no latency gain at R = 1 (45.3 -> 44.8 us per step) and 5-7 % LOWER throughput at R = 32 (the
-// early-scheduled CTAs of the dependents hold SM resources the tile kernels of the other sub-batches could use), so
+// The early-scheduled CTAs of the dependents hold SM resources the tile kernels of the other sub-batches could use, so
 // it is OFF by default; PILCO_PDL=1 enables it (the device-side instructions are no-ops without the attribute).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -275,7 +285,7 @@ __device__ __forceinline__ bool last_cta_arrives(unsigned* counter, unsigned cou
 }
 
 // tile-type kernels: "glue" (high priority) while the whole grid fits the machine once, bulk work otherwise
-static inline bool pilco_small_grid(dim3 g) { return (long long)g.x * g.y * g.z < 296; }
+static inline bool pilco_small_grid(dim3 g) { return (long long)g.x * g.y * g.z < 2LL * pilco_sm_count(); }
 #endif       // (kept for the launchers: nothing to upload)
 
 __device__ __forceinline__ void exp_table_init(double* tab) {
@@ -285,7 +295,7 @@ __device__ __forceinline__ void exp_table_init(double* tab) {
 // (exp_scaled, exp_shifted, exp_row_split: exp_table.cuh -- shared with the host test build)
 
 // ---------------------------------------------------------------------------------------------
-// DMMA: D(8x8) = A(8x4) * B(4x8) + C, fp64 (legacy mma.sync path -- tcgen05 has no f64 kind).
+// DMMA: D(8x8) = A(8x4) * B(4x8) + C, fp64 (mma.sync: wgmma has no f64 kind).
 // lane = 4*g + t:  a = A[g][t],  b = B[t][g],  c0/c1 = C[g][2t], C[g][2t+1].
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {

@@ -17,8 +17,7 @@ template <int KS>
 static int launch_tile(const MMParams& p, cudaStream_t st) {
     static bool configured_dev[PILCO_MAX_DEVICES] = {false};      // function attributes are per device
     // 3 (default): 3 CTAs/SM, two row octets per warp on off-diagonal pairs (80 registers); 1: 3 CTAs/SM, one octet per warp (the round-1
-    // kernel); 0: 2 CTAs/SM, two octets; 2: 4 CTAs/SM, one octet.  PILCO_TILE_VARIANT selects (tuning switch).  Measured at the metric
-    // shape, R = 32 (one launch / forward bench): 1: 0.2519 ms / 101.8 k steps/s, 0: 0.2498 / 101.5 k, 3: 0.2517 / 103.2 k, 2: 0.2599 / --.
+    // kernel); 0: 2 CTAs/SM, two octets; 2: 4 CTAs/SM, one octet.  PILCO_TILE_VARIANT selects (tuning switch).
     static int variant = 3;
     static int rpc_env = 0;          // 0: automatic
     bool& configured = configured_dev[pilco_current_device()];
@@ -40,10 +39,10 @@ static int launch_tile(const MMParams& p, cudaStream_t st) {
     // row blocks per CTA: a CTA's fixed cost (TMA staging of the columns and the exp table, barrier, first-load
     // latency: ~5 k cycles against ~16 k per 64-row sweep at the metric shape) is paid once for all its row blocks.
     // All of a pair's row blocks go to one CTA as soon as pairs x restarts still give every SM a CTA; smaller
-    // launches keep enough CTAs to fill the machine (2 x 148).
+    // launches keep enough CTAs to fill the machine (2 CTAs per SM).
     int rpc = p.L.NB;
-    const long long pr = (long long)p.L.P * p.R;
-    if (pr < 148) { rpc = (int)(((long long)p.L.NB * pr) / 296); if (rpc < 1) rpc = 1; }
+    const long long pr = (long long)p.L.P * p.R, nsm = pilco_sm_count();
+    if (pr < nsm) { rpc = (int)(((long long)p.L.NB * pr) / (2 * nsm)); if (rpc < 1) rpc = 1; }
     if (rpc_env > 0) rpc = rpc_env;
     if (rpc > p.L.NB) rpc = p.L.NB;
     dim3 grid((p.L.NB + rpc - 1) / rpc, p.L.P, p.R);

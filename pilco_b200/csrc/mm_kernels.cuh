@@ -560,13 +560,12 @@ static inline void mm_setup_launch(const MMParams& p, cudaStream_t st) {
     // ONE launch while the whole launch is small -- at most half the SMs' worth of CTAs: a single restart, or the RBF
     // policy's few tasks -- (latency regime: every launch on the serial path of a rollout step counts); anything bigger keeps
     // the two-stage form: stage 1 is register-hungry (218 registers at D = 12), fused it caps the occupancy of the throughput
-    // stage, and in a sub-batch of a larger job its CTAs take SM slots from the other sub-batches' tile kernels (measured,
-    // inv_double_pendulum R = 32 in 8 sub-batches of 27 tasks x 4: fused 194 k, two-stage 206 k steps/s).
+    // stage, and in a sub-batch of a larger job its CTAs take SM slots from the other sub-batches' tile kernels.
     // PILCO_SETUP_FUSED=0/1 forces either (tuning switch).
     {
         static int mode = -1;
         if (mode < 0) { const char* e = getenv("PILCO_SETUP_FUSED"); mode = (e && (e[0] == '0' || e[0] == '1')) ? e[0] - '0' : 2; }
-        const bool fused = mode == 2 ? (long long)ntask * p.R <= 74 : mode == 1;
+        const bool fused = mode == 2 ? (long long)ntask * p.R <= pilco_sm_count() / 2 : mode == 1;
         if (fused) {
             // pair tasks are split over up to 3 CTAs, one 128-row chunk each (the stage-2 sweep is what the step waits for)
             int split = (p.L.np + 127) / 128;
@@ -782,8 +781,8 @@ __device__ __forceinline__ void mm_tile_body(const MMParams& p, int rpc) {
 // Off-diagonal pairs with TWO row octets per warp (the 2 CTAs/SM instantiation): the warp takes its octet of two
 // consecutive row blocks at a time, so every column operand it reads from shared memory -- the DMMA B fragments of
 // zeta, B_q, beta_b -- feeds two tiles instead of one: 36 instead of 56 LDS per 8 tiles, and twice the independent
-// DMMA -> exp chains in flight per warp.  Measured on the instruction mix alone (scripts/ubench/fp64_mix.cu, `full16`
-// against `full`): 0.82 of the fp64 issue-path ideal at 4 warps per sub-partition against 0.77 at 6.  An odd last row
+// DMMA -> exp chains in flight per warp (scripts/ubench/fp64_mix.cu, `full16` against `full`, times the instruction
+// mix alone).  An odd last row
 // block runs the one-octet form of the same code.  Every group is fully unrolled (1-4 column tiles): no per-tile
 // branches anywhere.  Same staging (TMA bulk copies on one mbarrier), same per-octet outputs (Tpart) as mm_tile_body.
 // -------------------------------------------------------------------------------------------------

@@ -19,18 +19,21 @@
 #include "mm_kernels.cuh"
 
 // row splits of one pair over CTAs: 1 once pairs x restarts fill the machine twice over
-static inline __host__ __device__ int mm_tape_splits(int n, int P, int R) {
+// (host only: depends on the current device's SM count.  A tape lives in one device's memory and its forward pass and
+// reverse sweep run on that device, so both derive the same layout; every entry point also checks tape_bytes against the
+// layout of the current device, so a tape sized on a device with fewer splits is rejected, never overrun.)
+static inline int mm_tape_splits(int n, int P, int R) {
     const int NO = (n + 7) / 8;
-    const long long pr = (long long)P * R;
+    const long long pr = (long long)P * R, fill = 2LL * pilco_sm_count();
     int cs = 1;
-    if (pr < 296) cs = (int)((296 + pr - 1) / pr);
+    if (pr < fill) cs = (int)((fill + pr - 1) / pr);
     int cap = NO / 8;
     if (cap < 1) cap = 1;
     if (cap > 4) cap = 4;
     return cs < cap ? cs : cap;
 }
 
-static inline __host__ __device__ MMTapeL mm_tape_layout(int n, int D, int E, int R) {
+static inline MMTapeL mm_tape_layout(int n, int D, int E, int R) {
     MMTapeL T;
     T.np = pad64(n); T.P = npairs_of(E);
     T.ldh = ldz_of(D);            // row stride of HZ: 4 / 12 / 20, bank-conflict free as a DMMA B operand (like zeta)

@@ -17,7 +17,7 @@ F64 = torch.float64
 
 def device():
     if not torch.cuda.is_available():
-        raise RuntimeError("pilco_b200: a CUDA device (B200, sm_100a) is required; "
+        raise RuntimeError("pilco_b200: a CUDA device (H100, sm_90a) is required; "
                            "there is no CPU fallback for the moment-matching path")
     return torch.device("cuda", torch.cuda.current_device())
 

@@ -8,8 +8,7 @@
 * The restarts of a rank are independent optimisation problems, so they are dealt to ``GROUPS`` lock-step groups
   that only wait for THEIR OWN previous evaluation: each group has its own evaluator (captured graph, stream, pinned
   buffers) and driver thread, started half an evaluation apart, so the latency-bound reverse sweep and the SciPy
-  host work of one group run under the tile kernels of the other (measured, metric shape, R = 32:
-  46.1 k -> 49.7 k rollout steps/s forward + backward).
+  host work of one group run under the tile kernels of the other.
 * Multi-GPU: restart r belongs to rank r % world; after the local optimisations a single
   ``all_gather`` of ``[loss | flat parameters]`` lets every rank pick the same winner (ties -> lowest
   restart index, the sequential ``>`` comparison of pilco.py:105).  No other collective is used.
@@ -43,8 +42,7 @@ class PolicyEvaluator:
 
     The R restarts are dealt to ``nsplit`` sub-batches, each with its own RolloutPlan (taped forward + reverse sweep)
     on its own stream inside ONE captured CUDA graph: the latency-bound glue kernels of one sub-batch overlap the tile
-    kernels of the others (measured at the metric shape, R = 32: 40.5 k / 43.3 k / 46.0 k rollout steps/s forward +
-    backward with 1 / 2 / 4 sub-batches; 8 is slower for the reverse sweep)."""
+    kernels of the others."""
 
     NSPLIT = 4
 

@@ -1,4 +1,4 @@
-"""First-light diagnostics on the B200 box: fp64 pipe microbenchmarks + raw timing of the moment-match
+"""First-light diagnostics on the GPU: fp64 pipe microbenchmarks + raw timing of the moment-match
 kernels at the metric configuration.  Writes gpurun_out/diag.json."""
 import ctypes as C
 import json
@@ -22,7 +22,7 @@ print(torch.cuda.get_device_name(0))
 sink = torch.zeros(8, dtype=torch.float64, device=d)
 ms = C.c_float()
 names = {0: "dfma", 1: "dmma", 2: "dfma+dmma", 3: "exp_tab", 4: "exp_libdevice"}
-iters, blocks = 20000, 148 * 4
+iters, blocks = 20000, torch.cuda.get_device_properties(0).multi_processor_count * 4
 for which in range(5):
     _lib.check(lib.pilco_microbench_fp64(which, iters, blocks, engine.ptr(sink), C.byref(ms), engine.stream_ptr()))
     thread_ops = blocks * 256 * iters * 8.0

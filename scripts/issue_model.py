@@ -1,13 +1,15 @@
 """Static issue-path model of the tile kernels' hot loops, read from the SASS of the built library (no GPU needed).
 
-For every innermost loop that holds DMMA instructions it counts the instruction classes and prices them with the rates
-measured by scripts/ubench/fp64_mix.cu on a B200 (profiles/r02_ubench_fp64_mix.txt):
+For every innermost loop that holds DMMA instructions it counts the instruction classes and prices them per warp on one
+SM sub-partition with the rates measured on an H100 SXM (80GB HBM3, 700 W, 1980 MHz): DMMA.8x8x4 from bench.py's
+pilco_microbench_fp64 (31.7 TFLOP/s over 132 SMs x 4 sub-partitions), the fp64 instructions from scripts/ubench/fp64_mix.cu:
 
-    DMMA.8x8x4                                  16 cycles of the fp64 pipe per warp
+    DMMA.8x8x4 (512 flop)                       17 cycles of the fp64 pipe per warp (about half the H100's fp64 tensor
+                                                rate: the native DMMA.16x8x16 reaches 54.8 TFLOP/s in the same process)
     DADD / DMUL / DFMA, <= 2 distinct registers  2 cycles
     DFMA with three distinct register sources    3 cycles   (operand bandwidth)
-    everything else                              not priced (co-issues; what it really costs is the gap between this model
-                                                 and the measurement -- shuffles and the table gather, DESIGN.md section 6)
+    everything else                             not priced (co-issues; what it really costs is the gap between this model
+                                                and the measurement -- shuffles and the table gather, DESIGN.md section 6)
 
     python scripts/issue_model.py [kernel-regex ...]      default: the forward and the taped tile kernel at the metric shape
 
@@ -90,7 +92,7 @@ def model(code, lo, hi):
             c["shfl"] += 1
         elif op != "NOP":
             c["other"] += 1
-    c["cycles"] = 16 * c["dmma"] + 2 * c["fp64"] + 3 * c["fp64_3"]
+    c["cycles"] = 17 * c["dmma"] + 2 * c["fp64"] + 3 * c["fp64_3"]
     return c
 
 

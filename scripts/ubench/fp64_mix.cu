@@ -1,13 +1,14 @@
-// fp64_mix.cu -- stand-alone microbenchmarks of the fp64 issue path on sm_100a: what does the tile kernels' instruction
+// fp64_mix.cu -- stand-alone microbenchmarks of the fp64 issue path on sm_90a: what does the tile kernels' instruction
 // mix (DMMA.8x8x4 + DADD/DFMA/DMUL + integer + LDS) cost per warp, and which restructurings of the inner loop pay.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -o scripts/ubench/fp64_mix scripts/ubench/fp64_mix.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o scripts/ubench/fp64_mix scripts/ubench/fp64_mix.cu
 //   scripts/ubench/fp64_mix            (prints one line per pattern x occupancy)
 //
-// Every pattern runs ONE wave of 148 x bpsm CTAs of 256 threads (bpsm x 2 warps per SM sub-partition); elapsed SM cycles
+// Every pattern runs ONE wave of (SMs x bpsm) CTAs of 256 threads (bpsm x 2 warps per SM sub-partition); elapsed SM cycles
 // are read with clock64() in CTA 0.  `cyc/it` = elapsed cycles / (iterations x warps per sub-partition): the sub-partition
 // cycles one warp-iteration costs at that occupancy.  `ideal` = 17 x DMMA + 2 x fp64 instructions of the iteration
-// (fp64 pipe time at the measured peak rates).  Diagnostics only: not part of the library.
+// (fp64 pipe time at the peak rates measured on an H100 SXM at 1980 MHz: DMMA.8x8x4 31.7 TFLOP/s = 17 cycles per warp
+// and sub-partition, DFMA / DADD / DMUL 2 cycles).  Diagnostics only: not part of the library.
 #include <cstdio>
 #include <cstdlib>
 #include <vector>

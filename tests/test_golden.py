@@ -70,16 +70,19 @@ def test_oracle_cascade_matches_reference_m_files():
     assert scaled_err(Mp[0], g["Mtraj"][:, -1]) < 1e-10 and scaled_err(Sp, g["Straj"][:, :, -1]) < 1e-9
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/tests/Matlab Code"), reason="reference tree not present")
 def test_golden_regenerates_from_reference_sources():
-    """Re-execute two of the reference's .m files with oracle/mrun.py and compare with the committed vectors."""
+    """Re-execute two of the reference's .m files (the checksummed copies under tests/reference_tests) with
+    oracle/mrun.py and compare with the committed vectors."""
     from oracle import mrun
     g = load("gp0_a")
     M, S, V = mrun.run("gp0", dict(hyp=hyp_of(g["ell"], g["sf2"], g["sn2"]), inputs=g["X"], targets=g["Y"]), g["m"].T, g["s"], nout=3)
-    assert np.array_equal(M, g["M"]) and np.array_equal(S, g["S"]) and np.array_equal(V, g["V"])
+    # round-off only: numpy's BLAS takes a different kernel on another CPU than where the vectors were made (S moves by
+    # ~2e-12 of its scale between OpenBLAS core types)
+    same = lambda a, b: scaled_err(a, b) < 1e-11
+    assert same(M, g["M"]) and same(S, g["S"]) and same(V, g["V"])
     g = load("gSin")
     M, S, C = mrun.run("gSin", g["m"].T, g["s"], float(g["e"]), nout=3)
-    assert np.array_equal(M, g["M"]) and np.array_equal(S, g["S"])
+    assert same(M, g["M"]) and same(S, g["S"])
 
 
 # ---------------------------------------------------------------------------------------------- GPU

@@ -1,7 +1,7 @@
 """Build-time evidence that the hot kernels are what DESIGN.md says they are, read from the SASS of the built
 library with cuobjdump (no GPU needed): the forward and backward tile kernels use the fp64 tensor-core path
 (DMMA.8x8x4), stage their operands with TMA bulk copies completing on an mbarrier (UBLKCP / SYNCS) and keep
-everything in registers (no local-memory loads/stores); every device cubin targets sm_100a."""
+everything in registers (no local-memory loads/stores); every device cubin targets sm_90a (H100)."""
 import os
 import re
 import shutil
@@ -31,10 +31,10 @@ def _sass(pattern):
     return {k: "\n".join(v) for k, v in funcs.items()}
 
 
-def test_device_code_targets_sm_100a():
+def test_device_code_targets_sm_90a():
     out = subprocess.run([CUOBJDUMP, "-lelf", LIB], capture_output=True, text=True, timeout=120).stdout
     cubins = re.findall(r"ELF file\s+\d+: (\S+)", out)
-    assert len(cubins) >= 9 and all(c.endswith(".sm_100a.cubin") for c in cubins), cubins
+    assert len(cubins) >= 9 and all(c.endswith(".sm_90a.cubin") for c in cubins), cubins
 
 
 def test_tile_kernels_use_dmma_tma_and_no_local_memory():
@@ -103,8 +103,8 @@ def test_session3_shuffle_and_chain_properties():
 def test_issue_model_of_the_hot_loops():
     """scripts/issue_model.py on the built library: the structure of the innermost DMMA loops DESIGN.md section 6 reasons about.
     Forward tile kernel (metric shape): the two-octet loop issues 24 DMMA per 8 tiles with 36 LDS (one octet: 12 per 4 tiles,
-    28 LDS) and not one shuffle; priced with the measured rates (DMMA 16 cycles, fp64 2, three-register DFMA 3) that is
-    82 cycles per 8x8 tile.  Taped tile kernel: 14 DMMA per tile and octet pair; 6 shuffles in the loops of the non-symmetric
+    28 LDS) and not one shuffle; priced with the rates measured on an H100 (DMMA.8x8x4 17 cycles, fp64 2, three-register
+    DFMA 3) that is 85 cycles per 8x8 tile.  Taped tile kernel: 14 DMMA per tile and octet pair; 6 shuffles in the loops of the non-symmetric
     pairs, none in those of the symmetric diagonal pairs."""
     import sys
     sys.path.insert(0, os.path.join(ROOT, "scripts"))
@@ -116,7 +116,7 @@ def test_issue_model_of_the_hot_loops():
     assert len(two) == 1 and len(one) == 1
     assert two[0]["shfl"] == 0 and one[0]["shfl"] == 0
     assert two[0]["lds"] <= 36 and one[0]["lds"] <= 28
-    assert two[0]["cycles"] == 2 * one[0]["cycles"] and 80 <= two[0]["cycles"] / 8.0 <= 84      # 12*16 + 8*(7*2+3) = 328 per 4 tiles
+    assert two[0]["cycles"] == 2 * one[0]["cycles"] and 83 <= two[0]["cycles"] / 8.0 <= 87      # 12*17 + 8*(7*2+3) = 340 per 4 tiles
     tape = list(issue_model.analyse(r"mm_tape_tile_kernelILi3ELi256E").values())
     assert len(tape) == 1
     pair_loops = [c for _, c in tape[0] if c["dmma"] == 14]
