@@ -304,6 +304,55 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
 }
 
 // ---------------------------------------------------------------------------------------------
+// Hopper's native fp64 MMA shapes: D(16x8) = A(16xK) * B(Kx8) + C, K = 4, 8, 16 (SASS DMMA.16x8x4 / 16x8x8 / 16x8x16).
+// lane = 4*g + t:  a[2i] = A[g][t + 4i],  a[2i+1] = A[g + 8][t + 4i],  b[i] = B[t + 4i][g],
+//                  c[0], c[1] = C[g][2t], C[g][2t+1],  c[2], c[3] = C[g + 8][2t], C[g + 8][2t+1].
+// Two 8x8x4 problems on row octets that share their B operand are ONE 16x8x4 problem: A rows 0-7 are the first octet's
+// A fragment, rows 8-15 the second's, and the C fragment is the two octets' C fragments side by side.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void dmma1684(double (&c)[4], double a0, double a1, double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a0), "d"(a1), "d"(b));
+}
+__device__ __forceinline__ void dmma1688(double (&c)[4], const double (&a)[4], double b0, double b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b0), "d"(b1));
+}
+__device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                   "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
+// C(16x8) += A(16 x 4KS) B(4KS x 8) with the A fragment af[2ks + o] = A[8o + g][4ks + t] (two row octets, k-step ks)
+// and the B fragment bf[ks] = B[4ks + t][g]: one MMA per K chunk, K = 4KS on Hopper's 16x8 shapes -- KS = 3 as
+// 16x8x8 + 16x8x4 (PILCO_M16_K16PAD: one 16x8x16 whose fourth k-step has a zero A fragment; the B operand of that
+// k-step repeats bf[2], finite, so the product adds exact zeros).
+template <int KS>
+__device__ __forceinline__ void mma16_k(double (&c)[4], const double (&af)[2 * KS], const double (&bf)[KS]) {
+    if constexpr (KS == 1) {
+        dmma1684(c, af[0], af[1], bf[0]);
+    } else if constexpr (KS == 2) {
+        dmma1688(c, af, bf[0], bf[1]);
+    } else if constexpr (KS == 3) {
+#ifdef PILCO_M16_K16PAD
+        const double a8[8] = {af[0], af[1], af[2], af[3], af[4], af[5], 0.0, 0.0};
+        const double b4[4] = {bf[0], bf[1], bf[2], bf[2]};
+        dmma16816(c, a8, b4);
+#else
+        const double a4[4] = {af[0], af[1], af[2], af[3]};
+        dmma1688(c, a4, bf[0], bf[1]);
+        dmma1684(c, af[4], af[5], bf[2]);
+#endif
+    } else {
+        static_assert(KS == 4, "K = 4 KS <= 16");
+        const double b4[4] = {bf[0], bf[1], bf[2], bf[3]};
+        dmma16816(c, af, b4);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // TMA bulk copy (1-D cp.async.bulk, SASS UBLKCP) global -> shared, completion on an mbarrier.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

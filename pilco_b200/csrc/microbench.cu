@@ -1,21 +1,13 @@
 // microbench.cu -- fp64 pipe diagnostics used to set the roofline denominators:
 //   which=0: DFMA only, 1: DMMA (m8n8k4) only, 2: DFMA+DMMA interleaved 1:1 (per-warp instruction counts),
 //   3: exp_tab only, 4: libdevice exp only, 5: DMMA m16n8k8 only, 6: DMMA m16n8k16 only (Hopper's native fp64 MMA shapes:
-//   what the fp64 tensor cores reach, against which the m8n8k4 rate of the tile kernels is compared).
+//   what the fp64 tensor cores reach, against which the m8n8k4 rate of the tile kernels is compared), 7: DMMA m16n8k4 only,
+//   8: DFMA+DMMA m16n8k16 interleaved 1:1, 9: DFMA+DMMA m16n8k8 interleaved 1:1 (does the 16x8 tensor path block DFMA issue
+//   the way the 8x8x4 one does?).
 // Returns achieved warp-instructions/s through *rate (DFMA or DMMA or exp evaluations per second, chip-wide).
 #include "common.cuh"
 
-// D(16x8) += A(16xK) B(Kx8), fp64, K = 8 or 16 (sm_90)
-__device__ __forceinline__ void dmma1688(double (&c)[4], const double (&a)[4], double b0, double b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b0), "d"(b1));
-}
-__device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
-                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
-                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
-                   "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
-}
+// (dmma1684 / dmma1688 / dmma16816: common.cuh)
 
 template <int WHICH>
 __global__ void __launch_bounds__(256) fp64_pipe_kernel(int iters, double* sink) {
@@ -28,7 +20,7 @@ __global__ void __launch_bounds__(256) fp64_pipe_kernel(int iters, double* sink)
     double c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0, c5 = 0, c6 = 0, c7 = 0;
     const double m = 0.999999, b = 1e-7;
     for (int it = 0; it < iters; ++it) {
-        if (WHICH == 0 || WHICH == 2) {
+        if (WHICH == 0 || WHICH == 2 || WHICH == 8 || WHICH == 9) {
             a0 = fma(a0, m, b); a1 = fma(a1, m, b); a2 = fma(a2, m, b); a3 = fma(a3, m, b);
             a4 = fma(a4, m, b); a5 = fma(a5, m, b); a6 = fma(a6, m, b); a7 = fma(a7, m, b);
         }
@@ -39,13 +31,15 @@ __global__ void __launch_bounds__(256) fp64_pipe_kernel(int iters, double* sink)
             dmma884(c0, c1, a1, a2); dmma884(c2, c3, a3, a4); dmma884(c4, c5, a5, a6); dmma884(c6, c7, a7, a0);
             if (WHICH == 1) { a0 += c1 * 1e-300; a3 += c2 * 1e-300; }
         }
-        if (WHICH == 5 || WHICH == 6) {
+        if (WHICH == 5 || WHICH == 6 || WHICH == 7 || WHICH == 8 || WHICH == 9) {
             // 8 MMAs per iteration into 4 independent accumulators, operands rotated (no identical-operand fast path)
             double x[8] = {a0, a1, a2, a3, a4, a5, a6, a7};
             double acc[4][4] = {{c0, c1, c2, c3}, {c4, c5, c6, c7}, {c1, c2, c3, c4}, {c5, c6, c7, c0}};
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
-                if (WHICH == 5) {
+                if (WHICH == 7) {
+                    dmma1684(acc[k & 3], x[k & 7], x[(k + 1) & 7], x[(k + 4) & 7]);
+                } else if (WHICH == 5 || WHICH == 9) {
                     const double av[4] = {x[k & 7], x[(k + 1) & 7], x[(k + 2) & 7], x[(k + 3) & 7]};
                     dmma1688(acc[k & 3], av, x[(k + 4) & 7], x[(k + 5) & 7]);
                 } else {
@@ -86,6 +80,9 @@ extern "C" int pilco_microbench_fp64(int which, int iters, int blocks, double* s
             case 3: fp64_pipe_kernel<3><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
             case 5: fp64_pipe_kernel<5><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
             case 6: fp64_pipe_kernel<6><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
+            case 7: fp64_pipe_kernel<7><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
+            case 8: fp64_pipe_kernel<8><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
+            case 9: fp64_pipe_kernel<9><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
             default: fp64_pipe_kernel<4><<<blocks, 256, 0, st>>>(iters, sink_dev); break;
         }
         cudaEventRecord(e1, st);

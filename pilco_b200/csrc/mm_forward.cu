@@ -16,14 +16,15 @@ int mm_check_model(const pilco_gp_model* gp) {
 template <int KS>
 static int launch_tile(const MMParams& p, cudaStream_t st) {
     static bool configured_dev[PILCO_MAX_DEVICES] = {false};      // function attributes are per device
-    // 3 (default): 3 CTAs/SM, two row octets per warp on off-diagonal pairs (80 registers); 1: 3 CTAs/SM, one octet per warp (the round-1
-    // kernel); 0: 2 CTAs/SM, two octets; 2: 4 CTAs/SM, one octet.  PILCO_TILE_VARIANT selects (tuning switch).
-    static int variant = 3;
+    // 4 (default): 3 CTAs/SM, two row octets per warp on off-diagonal pairs as ONE 16-row tile on the 16x8 MMA shapes
+    // (mm_tile_m16_kernel); 3: 3 CTAs/SM, two row octets per warp on DMMA.8x8x4 (80 registers); 1: 3 CTAs/SM, one octet per
+    // warp (the round-1 kernel); 0: 2 CTAs/SM, two octets; 2: 4 CTAs/SM, one octet.  PILCO_TILE_VARIANT selects (tuning switch).
+    static int variant = 4;
     static int rpc_env = 0;          // 0: automatic
     bool& configured = configured_dev[pilco_current_device()];
     if (!configured) {
         const char* e = getenv("PILCO_TILE_VARIANT");       // tuning switches
-        if (e && e[0] >= '0' && e[0] <= '3') variant = e[0] - '0';
+        if (e && e[0] >= '0' && e[0] <= '4') variant = e[0] - '0';
         const char* e2 = getenv("PILCO_TILE_RPC");
         if (e2) rpc_env = atoi(e2);
         const int big = (int)mm_tile_smem_bytes(TILE_CM, 20);
@@ -31,6 +32,7 @@ static int launch_tile(const MMParams& p, cudaStream_t st) {
         if (cudaFuncSetAttribute(mm_tile_kernel<KS, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
         if (cudaFuncSetAttribute(mm_tile_kernel<KS, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
         if (cudaFuncSetAttribute(mm_tile_kernel<KS, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
+        if (cudaFuncSetAttribute(mm_tile_m16_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
         configured = true;
     }
     int rc = exp_table_upload();
@@ -47,7 +49,8 @@ static int launch_tile(const MMParams& p, cudaStream_t st) {
     if (rpc > p.L.NB) rpc = p.L.NB;
     dim3 grid((p.L.NB + rpc - 1) / rpc, p.L.P, p.R);
     const bool hi = pilco_small_grid(grid);          // e.g. the RBF policy's 3 pairs: glue, not bulk work
-    if (variant == 3) launch_pri(hi, mm_tile_kernel<KS, 3, true>, grid, dim3(256), smem, st, p, rpc);
+    if (variant == 4) launch_pri(hi, mm_tile_m16_kernel<KS>, grid, dim3(256), smem, st, p, rpc);
+    else if (variant == 3) launch_pri(hi, mm_tile_kernel<KS, 3, true>, grid, dim3(256), smem, st, p, rpc);
     else if (variant == 2) launch_pri(hi, mm_tile_kernel<KS, 4>, grid, dim3(256), smem, st, p, rpc);
     else if (variant == 1) launch_pri(hi, mm_tile_kernel<KS, 3>, grid, dim3(256), smem, st, p, rpc);
     else launch_pri(hi, mm_tile_kernel<KS, 2>, grid, dim3(256), smem, st, p, rpc);

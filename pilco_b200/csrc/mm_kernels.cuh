@@ -6,7 +6,8 @@
 //                                                 per-centre A'_ab[n], B_ab[n], U'_ab[n][:]
 //   tile    grid (NB, P, R): T_ab = sum_{n,m} (beta_a[n] beta_b[m] - d_ab iK_a[n,m])
 //                                              * exp(A'[n] + B[m] + U'[n].zeta[m])
-//                            8 rows per warp, DMMA m8n8k4 for U'.zeta, table exp, TMA-staged columns
+//                            off-diagonal pairs: 16 rows per warp, one 16x8 MMA per K chunk for U'.zeta
+//                            (mm_tile_m16_kernel); diagonal pairs: 8 rows per warp, DMMA m8n8k4; table exp, TMA-staged columns
 //   finish  grid (R)       : S_ab = T_ab + d_ab*diag_add - M_a M_b
 // Reference: pilco/models/mgpr.py:91-149 (gp0.m:63-104, gp2.m:69-106).
 #pragma once
@@ -938,6 +939,172 @@ __global__ void __launch_bounds__(256, MINB) mm_tile_kernel(MMParams p, int rpc)
         if (TWO) mm_tile_body16<KS>(p, rpc);                // two row octets per warp (the default instantiation)
         else mm_tile_body<KS, false, false>(p, rpc);
     }
+    else if (p.gp.mode == 0 && p.gp.iK != nullptr) mm_tile_body<KS, true, true>(p, rpc);
+    else mm_tile_body<KS, true, false>(p, rpc);
+}
+
+// -------------------------------------------------------------------------------------------------
+// Off-diagonal pairs on Hopper's native 16x8 MMA shapes.  The two row octets of mm_tile_body16 share every B fragment,
+// so their two 8x8 exponent tiles are ONE 16x8 tile: A = the two octets' U' fragments (rows g and g + 8), C = the two
+// octets' C fragments side by side, K = DP in one MMA per K chunk (mma16_k) instead of 2 KS DMMA.8x8x4.  Same staging,
+// same exp and weighted sums, same per-octet outputs (Tpart) as mm_tile_body16.
+// A pass with ONE row block left (an odd last block) keeps the 16-row shape too: warps 0-3 take the octet pairs
+// {2w, 2w + 1} of that block over all columns, warps 4-7 have no rows in that pass (the other CTAs on the SM use the
+// pipe).  An octet's sum is the same whichever pass form it ran in -- the row blocks per CTA, and with them the odd
+// blocks, follow the batch size, and a restart's result must not.
+// -------------------------------------------------------------------------------------------------
+template <int KS>
+__device__ __forceinline__ void tile_sweep_m16(const double* __restrict__ sZ, const double* __restrict__ sBq,
+                                               const double* __restrict__ sBe, const double* __restrict__ ltab, int cbeg, int cend,
+                                               const double (&af)[2 * KS], const double (&am)[2], double (&acc)[2], int g, int t) {
+    constexpr int ldz = KS == 1 ? 4 : (KS <= 3 ? 12 : 20);
+    int cg = cbeg;
+    auto group = [&](auto nt_c) {
+        constexpr int NTL = decltype(nt_c)::value;
+        double e[NTL][4];
+#pragma unroll
+        for (int j = 0; j < NTL; ++j) {
+            const double2 bq = *reinterpret_cast<const double2*>(sBq + cg + 8 * j + 2 * t);
+            e[j][0] = bq.x; e[j][1] = bq.y; e[j][2] = bq.x; e[j][3] = bq.y;
+        }
+#pragma unroll
+        for (int j = 0; j < NTL; ++j) {
+            double bf[KS];
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) bf[ks] = sZ[(size_t)(cg + 8 * j + g) * ldz + 4 * ks + t];
+            mma16_k<KS>(e[j], af, bf);
+        }
+#pragma unroll
+        for (int j = 0; j < NTL; ++j) {
+            const double2 bb = *reinterpret_cast<const double2*>(sBe + cg + 8 * j + 2 * t);
+#pragma unroll
+            for (int o = 0; o < 2; ++o) {
+                const double l0 = exp_shifted(e[j][2 * o], am[o], ltab), l1 = exp_shifted(e[j][2 * o + 1], am[o], ltab);
+                acc[o] = fma(bb.x, l0, acc[o]); acc[o] = fma(bb.y, l1, acc[o]);
+            }
+        }
+    };
+    // groups of 4 column tiles (KS = 3: 3, KS = 4: 2 -- with the wider A fragments larger groups spill at 80 registers)
+    constexpr int GM = KS == 4 ? 2 : (KS == 3 ? 3 : 4);
+    for (; cg + 8 * GM <= cend; cg += 8 * GM) group(std::integral_constant<int, GM>{});
+    const int ntl = (cend - cg) >> 3;                                   // 0 .. GM - 1 tiles left (cend - cbeg is a multiple of 8)
+    if (GM == 4 && ntl == 3) group(std::integral_constant<int, 3>{});
+    else if (ntl == 2) group(std::integral_constant<int, 2>{});
+    else if (ntl == 1) group(std::integral_constant<int, 1>{});
+}
+
+template <int KS>
+__device__ __forceinline__ void mm_tile_body_m16(const MMParams& p, int rpc) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    TILE_STAMP(0);
+    const MMWs& L = p.L;
+    constexpr int ldz = KS == 1 ? 4 : (KS <= 3 ? 12 : 20);
+    const int np = L.np, n = p.gp.n;
+    const int CM = np < TILE_CM ? np : TILE_CM;
+    double* sZ = reinterpret_cast<double*>(smem_raw);
+    double* sBq = sZ + (size_t)CM * ldz;
+    double* sBe = sBq + CM;
+    double* tab = sBe + CM;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(tab + EXP_TAB_DOUBLES);
+
+    const int r = blockIdx.z, q = blockIdx.y;
+    const int rb0 = blockIdx.x * rpc;
+    const int rb1 = (rb0 + rpc) < L.NB ? (rb0 + rpc) : L.NB;
+    int a, b;
+    pair_decode(q, a, b);
+    const double* wsr = p.ws + (size_t)r * L.per_r;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const double* ltab = EXP_LANE_TAB(tab, lane);
+    const int ncol8 = (n + 7) & ~7;
+    const bool single = ncol8 <= CM;
+
+    if (tid == 0) { mbar_init(bar, 1); mbar_fence_init(); }
+    auto issue_chunk = [&](int c0, bool with_table) {
+        const int cm = (np - c0) < CM ? (np - c0) : CM;
+        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        mbar_expect_tx(bar, (unsigned)(cm * ldz * 8 + cm * 16 + (with_table ? EXP_TAB_DOUBLES * 8 : 0)));
+        tma_bulk_g2s(sZ, wsr + L.zeta + (size_t)c0 * ldz, (unsigned)(cm * ldz * 8), bar);
+        tma_bulk_g2s(sBq, wsr + L.Bq + (size_t)q * np + c0, (unsigned)(cm * 8), bar);
+        tma_bulk_g2s(sBe, wsr + L.betap + (size_t)b * np + c0, (unsigned)(cm * 8), bar);
+        if (with_table) tma_bulk_g2s(tab, g_exp_tab, (unsigned)(EXP_TAB_DOUBLES * 8), bar);
+    };
+    if (tid == 0) issue_chunk(0, true);
+    TILE_STAMP(1);
+    __syncthreads();                                    // barrier initialisation visible to the waiting warps
+
+    unsigned phase = 0;
+    bool staged = true;                                 // the chunk issued at entry has not been consumed yet
+    for (int rb = rb0; rb < rb1; rb += 2) {
+        const bool odd = rb + 1 >= rb1;                 // one row block left (uniform over the CTA)
+        // this warp's two octets (global octet indices): octet w of both row blocks, or octets 2w, 2w + 1 of the odd block
+        const int oct0 = odd ? rb * 8 + 2 * (warp & 3) : rb * 8 + warp;
+        const int ostep = odd ? 1 : 8;
+        const bool mine = !odd || warp < 4;             // warp-uniform: does this warp own rows in this pass
+        int row0[2];
+        bool act[2];
+        double af[2 * KS], am[2], ba[2], acc[2];
+#pragma unroll
+        for (int o = 0; o < 2; ++o) {
+            row0[o] = 8 * (oct0 + o * ostep);
+            act[o] = mine && row0[o] < n;               // warp-uniform; act[1] implies act[0]
+            am[o] = EXP_MAGIC; ba[o] = 0.0; acc[o] = 0.0;
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) af[2 * ks + o] = 0.0;
+            if (act[o]) {
+                // row operands (materialised by setup stage 2): U' fragments of the octet as rows 8o + g of the 16x8 A
+                // operand, and the scalar A' (integer part -> exp rounding constant, fractional part -> row factor)
+                const int row = row0[o] + g;
+                const double* uf = wsr + L.Ufrag + ((size_t)q * (np >> 3) + (row0[o] >> 3)) * (KS * 32);
+#pragma unroll
+                for (int ks = 0; ks < KS; ++ks) af[2 * ks + o] = uf[ks * 32 + lane];
+                double rowfac;
+                exp_row_split(wsr[L.Arow + (size_t)q * np + row], am[o], rowfac);
+                ba[o] = wsr[L.betap + (size_t)a * np + row] * rowfac;
+            }
+        }
+        for (int c0 = 0; c0 < ncol8; c0 += CM) {
+            const int cm = (np - c0) < CM ? (np - c0) : CM;
+            const int cend = (ncol8 - c0) < cm ? (ncol8 - c0) : cm;        // chunk-local end of valid columns
+            if (staged) {                                                  // chunk issued at CTA entry
+                mbar_wait(bar, phase);
+                phase ^= 1;
+                staged = false;
+                TILE_STAMP(2);
+            } else if (!single) {
+                __syncthreads();                                           // all warps done with the previous chunk
+                if (tid == 0) issue_chunk(c0, false);
+                mbar_wait(bar, phase);
+                phase ^= 1;
+            }
+            if (act[0]) tile_sweep_m16<KS>(sZ, sBq, sBe, ltab, 0, cend, af, am, acc, g, t);
+        }
+        if (rb + 2 >= rb1) TILE_STAMP(3);
+        // row sums -> beta_a-weighted totals, one partial per row octet
+        double* Tp = p.ws + (size_t)r * L.per_r + L.Tpart + (size_t)q * mm_tile_slots(np);
+        double v[2];
+#pragma unroll
+        for (int o = 0; o < 2; ++o) {
+            double s = acc[o];
+            s += __shfl_xor_sync(0xffffffffu, s, 1);
+            s += __shfl_xor_sync(0xffffffffu, s, 2);
+            v[o] = warp_sum((t == 0) ? ba[o] * s : 0.0);
+        }
+        if (mine && lane == 0) {
+            Tp[oct0] = act[0] ? v[0] : 0.0;
+            Tp[oct0 + ostep] = act[1] ? v[1] : 0.0;
+        }
+    }
+    TILE_STAMP(4);
+}
+
+// 3 CTAs/SM (<= 80 registers); diagonal pairs keep the one-octet 8x8x4 body (triangle + trace bookkeeping)
+template <int KS>
+__global__ void __launch_bounds__(256, 3) mm_tile_m16_kernel(MMParams p, int rpc) {
+    PDL_ENTRY();
+    int a, b;
+    pair_decode(blockIdx.y, a, b);
+    if (a != b) mm_tile_body_m16<KS>(p, rpc);
     else if (p.gp.mode == 0 && p.gp.iK != nullptr) mm_tile_body<KS, true, true>(p, rpc);
     else mm_tile_body<KS, true, false>(p, rpc);
 }

@@ -8,13 +8,16 @@
 template <int KS>
 static int launch_tape_tile(const MMParams& p, cudaStream_t st) {
     static bool configured_dev[PILCO_MAX_DEVICES] = {false};      // function attributes are per device
-    static int variant = 0;        // 0: <=128 regs (default: fastest tile pass, measured); 1: <=96 regs, 2 CTAs/SM; 2: <=80 regs, 2 CTAs/SM (padded smem); 3: <=80 regs, 3 CTAs/SM
+    // 4 (default): the 16x8-MMA kernel (mm_tape_tile_m16_kernel, <=128 regs); 0: the DMMA.8x8x4 kernel, <=128 regs; 1: <=96 regs,
+    // 2 CTAs/SM; 2: <=80 regs, 2 CTAs/SM (padded smem); 3: <=80 regs, 3 CTAs/SM
+    static int variant = 4;
     bool& configured = configured_dev[pilco_current_device()];
     if (!configured) {
         const char* e = getenv("PILCO_TAPE_VARIANT");           // tuning switch
-        if (e && e[0] >= '0' && e[0] <= '3') variant = e[0] - '0';
+        if (e && e[0] >= '0' && e[0] <= '4') variant = e[0] - '0';
         const int big = PILCO_MAX_SMEM_OPTIN;
-        if (cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
+        if (cudaFuncSetAttribute(mm_tape_tile_m16_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
+            cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
             cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 304>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
             cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 352>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
             return PILCO_ERR_LAUNCH;
@@ -24,7 +27,8 @@ static int launch_tape_tile(const MMParams& p, cudaStream_t st) {
     if (p.L.np > TAPE_MAX_NP || smem > PILCO_MAX_SMEM_OPTIN) return PILCO_ERR_UNSUPPORTED;
     const dim3 grid(p.TL.cs, p.L.P, p.R);
     const bool hi = pilco_small_grid(grid);
-    if (variant == 0) launch_pri(hi, mm_tape_tile_kernel<KS, 256>, grid, dim3(256), smem, st, p);
+    if (variant == 4) launch_pri(hi, mm_tape_tile_m16_kernel<KS>, grid, dim3(256), smem, st, p);
+    else if (variant == 0) launch_pri(hi, mm_tape_tile_kernel<KS, 256>, grid, dim3(256), smem, st, p);
     else if (variant == 1) launch_pri(hi, mm_tape_tile_kernel<KS, 304>, grid, dim3(256), smem, st, p);
     else {
         if (variant == 2 && smem < 80 * 1024) smem = 80 * 1024;    // 2 CTAs per SM

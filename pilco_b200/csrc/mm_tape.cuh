@@ -272,6 +272,220 @@ __global__ void __launch_bounds__(LB, 2) mm_tape_tile_kernel(MMParams p) {
     else mm_tape_body<KS, false>(p);
 }
 
+// -------------------------------------------------------------------------------------------------
+// The same taped pass on Hopper's native 16x8 MMA shapes: the warp's two row octets are one 16-row tile.
+//   exponent  C(16x8) = [B, B] + [U'_o0; U'_o1] . zeta[pi(cols)]   one MMA per K chunk (mma16_k)
+//   H.[Z,1]   the exponent's C fragment (c0, c2, c1, c3) of the weighted tile w is the A fragment of m16n8k8 -- (g, t),
+//             (g + 8, t), (g, t + 4), (g + 8, t + 4) -- because the exponent's B fragment takes the centres in the order
+//             pi; its B fragments are tape_sweep's zb[0][nt], zb[1][nt]: ONE DMMA.16x8x8 per n-tile, no shuffles.
+// hz[nt][0..1] = row g of octet 0, hz[nt][2..3] = row g of octet 1 (columns 8 nt + 2t, 8 nt + 2t + 1).  A dead second
+// octet (ua = 0, rf = 0) rides along; its sums are dropped.
+// -------------------------------------------------------------------------------------------------
+template <int KS, bool DIAG>
+__device__ __forceinline__ void tape_sweep_m16(const double* __restrict__ sZ, const double* __restrict__ sBq,
+                                               const double* __restrict__ sBe, const double* __restrict__ tab,
+                                               int cbeg, int cend, int c0,
+                                               const double (&af)[2 * KS], const double (&am)[2], const double (&rf)[2],
+                                               const double (&bn)[2], const double* const (&ikrow)[2],
+                                               double (&hl)[2], double (&hz)[(4 * KS + 7) / 8][4],
+                                               double* __restrict__ sCsw, int lane) {
+    constexpr int ldz = KS == 1 ? 4 : (KS <= 3 ? 12 : 20);
+    constexpr int NT = (4 * KS + 7) / 8;
+    constexpr bool ONES = (KS & 1) != 0;                       // DP = 4 KS = 4 (mod 8)
+    const int g = lane >> 2, t = lane & 3;
+    const int pg = (g >> 1) | ((g & 1) << 2);                  // pi(g)
+    const double* ltab = EXP_LANE_TAB(tab, lane);
+    for (int cg = cbeg; cg < cend; cg += 8) {
+        const double bq0 = sBq[cg + t], bq1 = sBq[cg + 4 + t];
+        const double bb0 = sBe[cg + t], bb1 = sBe[cg + 4 + t];
+        double bf[KS];
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) bf[ks] = sZ[(size_t)(cg + pg) * ldz + 4 * ks + t];
+        double zb[2][NT];
+#pragma unroll
+        for (int k2 = 0; k2 < 2; ++k2)
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) zb[k2][nt] = sZ[(size_t)(cg + 4 * k2 + t) * ldz + 8 * nt + g];
+        if (ONES && g == 4) { zb[0][NT - 1] = 1.0; zb[1][NT - 1] = 1.0; }   // ones column: row sums as HZ[:, DP]
+        double e[4] = {bq0, bq1, bq0, bq1};
+        mma16_k<KS>(e, af, bf);
+        double w[4];                                            // A fragment of H.[Z,1]: w0(o0), w0(o1), w1(o0), w1(o1)
+        double cs0 = 0.0, cs1 = 0.0;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            const double l0 = exp_shifted(e[2 * j], am[j], ltab), l1 = exp_shifted(e[2 * j + 1], am[j], ltab);
+            double w0, w1;
+            if (DIAG) {
+                const double ik0 = ikrow[j][c0 + cg + t], ik1 = ikrow[j][c0 + cg + 4 + t];   // zero padded: in bounds
+                w0 = fma(bn[j], bb0, -ik0) * l0;
+                w1 = fma(bn[j], bb1, -ik1) * l1;
+            } else {
+                w0 = bb0 * l0; w1 = bb1 * l1;
+            }
+            if (!ONES) hl[j] += w0 + w1;
+            if (!DIAG) { cs0 = fma(rf[j], w0, cs0); cs1 = fma(rf[j], w1, cs1); }
+            w[j] = w0; w[2 + j] = w1;
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) dmma1688(hz[nt], w, zb[0][nt], zb[1][nt]);
+        if (!DIAG) {                                            // column sums: the reduce-scatter butterfly of tape_sweep
+            const bool up = (g & 4) != 0;
+            double keep = up ? cs1 : cs0;
+            const double send = up ? cs0 : cs1;
+            keep += __shfl_xor_sync(0xffffffffu, send, 16);
+            keep += __shfl_xor_sync(0xffffffffu, keep, 8);
+            keep += __shfl_xor_sync(0xffffffffu, keep, 4);
+            if ((g & 3) == 0) sCsw[c0 + cg + (up ? 4 : 0) + t] += keep;
+        }
+    }
+}
+
+// CTA = (row split, pair, restart) as mm_tape_body.  A pass whose second block of octets is past the last row (at the
+// bench shapes: the last pass of every pair) does not fall back to one octet per warp: warps 0-3 take the octet pairs
+// {2w, 2w + 1} of the remaining block over all columns, warps 4-7 have no rows in that pass.  An octet's row-side results
+// (hr, HZ, T) are the same whichever pass form it ran in, so they do not depend on the row splits (i.e. the batch size).
+template <int KS, bool DIAG>
+__device__ __forceinline__ void mm_tape_body_m16(const MMParams& p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr int ldz = KS == 1 ? 4 : (KS <= 3 ? 12 : 20);
+    constexpr int NT = (4 * KS + 7) / 8;
+    const MMWs& L = p.L;
+    const MMTapeL& TL = p.TL;
+    const int np = L.np, n = p.gp.n;
+    const int CM = np < TILE_CM ? np : TILE_CM;
+    double* sZ = reinterpret_cast<double*>(smem_raw);
+    double* sBq = sZ + (size_t)CM * ldz;
+    double* sBe = sBq + CM;
+    double* tab = sBe + CM;
+    uint64_t* bar = reinterpret_cast<uint64_t*>(tab + EXP_TAB_DOUBLES);
+    double* sCs = reinterpret_cast<double*>(bar + 2);          // [8 warps][np] column-sum partials
+
+    const int r = blockIdx.z, q = blockIdx.y, sidx = blockIdx.x, cs = gridDim.x;
+    int a, b;
+    pair_decode(q, a, b);
+    const double* wsr = p.ws + (size_t)r * L.per_r;
+    double* tpr = p.tape + (size_t)r * TL.per_r;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int NO = (n + 7) >> 3, NS = np >> 3;                 // live row octets / partial-sum slots of a pair
+    const int ncol8 = (n + 7) & ~7;
+    const bool single = ncol8 <= CM;
+    double* sCsw = sCs + (size_t)warp * np;
+
+    if (tid == 0) { mbar_init(bar, 1); mbar_fence_init(); }
+    for (int c = lane; c < np; c += 32) sCsw[c] = 0.0;
+    auto issue_chunk = [&](int c0, bool with_table) {
+        const int cm = (np - c0) < CM ? (np - c0) : CM;
+        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        mbar_expect_tx(bar, (unsigned)(cm * ldz * 8 + cm * 16 + (with_table ? EXP_TAB_DOUBLES * 8 : 0)));
+        tma_bulk_g2s(sZ, wsr + L.zeta + (size_t)c0 * ldz, (unsigned)(cm * ldz * 8), bar);
+        tma_bulk_g2s(sBq, wsr + L.Bq + (size_t)q * np + c0, (unsigned)(cm * 8), bar);
+        tma_bulk_g2s(sBe, wsr + L.betap + (size_t)b * np + c0, (unsigned)(cm * 8), bar);
+        if (with_table) tma_bulk_g2s(tab, g_exp_tab, (unsigned)(EXP_TAB_DOUBLES * 8), bar);
+    };
+    __syncthreads();                                    // barrier initialised before the first arrive / wait
+    if (tid == 0) issue_chunk(0, true);
+
+    const int GW = cs * 8, gw = sidx * 8 + warp;
+    const int npass = (NS + 2 * GW - 1) / (2 * GW);     // uniform over the CTA (barriers inside when !single)
+    unsigned phase = 0;
+    bool staged = true;
+    for (int pass = 0; pass < npass; ++pass) {
+        // octet blocks of this pass: sidx * 8 + (2 pass) GW + [0, 8) and sidx * 8 + (2 pass + 1) GW + [0, 8)
+        const int base0 = sidx * 8 + (2 * pass) * GW;
+        const bool odd = base0 < NO && base0 + GW >= NO;       // uniform over the CTA: the second block is past the rows
+        int oct[2];
+        if (!odd) { oct[0] = gw + (2 * pass) * GW; oct[1] = gw + (2 * pass + 1) * GW; }
+        else if (warp < 4) { oct[0] = base0 + 2 * warp; oct[1] = oct[0] + 1; }
+        else { oct[0] = oct[1] = NS; }                         // no rows (no loads, no sweep, no outputs)
+        double af[2 * KS], am[2], rf[2], bn[2], hl[2], hz[NT][4];
+        const double* ikrow[2];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) { hz[nt][0] = hz[nt][1] = hz[nt][2] = hz[nt][3] = 0.0; }
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            hl[j] = 0.0; bn[j] = 0.0; rf[j] = 0.0; am[j] = EXP_MAGIC; ikrow[j] = nullptr;
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) af[2 * ks + j] = 0.0;
+            if (oct[j] < NO) {
+                const int row = 8 * oct[j] + g;
+                const double* uf = wsr + L.Ufrag + ((size_t)q * NS + oct[j]) * (KS * 32);
+#pragma unroll
+                for (int ks = 0; ks < KS; ++ks) af[2 * ks + j] = uf[ks * 32 + lane];
+                double rowfac;
+                exp_row_split(wsr[L.Arow + (size_t)q * np + row], am[j], rowfac);
+                const double ba = wsr[L.betap + (size_t)a * np + row];
+                if (DIAG) { bn[j] = ba; rf[j] = rowfac; ikrow[j] = p.gp.iK + ((size_t)a * p.gp.ldk + row) * p.gp.ldk; }
+                else rf[j] = ba * rowfac;
+            }
+        }
+        if (DIAG && ikrow[1] == nullptr) ikrow[1] = ikrow[0];  // dead second octet: any readable row (its sums are dropped)
+        const bool live = oct[0] < NO;                         // warp-uniform
+        for (int c0 = 0; c0 < ncol8; c0 += CM) {
+            const int cm = (np - c0) < CM ? (np - c0) : CM;
+            const int cend = (ncol8 - c0) < cm ? (ncol8 - c0) : cm;
+            if (staged) {
+                mbar_wait(bar, phase); phase ^= 1; staged = false;
+            } else if (!single) {
+                __syncthreads();
+                if (tid == 0) issue_chunk(c0, false);
+                mbar_wait(bar, phase); phase ^= 1;
+            }
+            if (live) tape_sweep_m16<KS, DIAG>(sZ, sBq, sBe, tab, 0, cend, c0, af, am, rf, bn, ikrow, hl, hz, sCsw, lane);
+        }
+        // row-side results of this pass
+        {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                if (oct[j] >= NS) continue;                     // warp-uniform
+                double v = 0.0;
+                if (oct[j] < NO) {
+                    const int row = 8 * oct[j] + g;
+                    constexpr bool ONES = (KS & 1) != 0;
+                    constexpr int tsum = ONES ? 2 : 0;          // lane of the quad that holds the row sum
+                    double h;
+                    if (ONES) h = hz[NT - 1][2 * j];            // HZ[:, DP] (ones column of the second product)
+                    else {
+                        h = hl[j];
+                        h += __shfl_xor_sync(0xffffffffu, h, 1);
+                        h += __shfl_xor_sync(0xffffffffu, h, 2);
+                    }
+                    const double hrv = rf[j] * h;
+                    if (t == tsum) { tpr[TL.hr + (size_t)q * np + row] = hrv; v = hrv; }
+                    double* hzrow = tpr + TL.HZ + ((size_t)q * np + row) * ldz;      // (TL.ldh == ldz)
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+                        if (8 * nt + 2 * t < ldz)                                // columns beyond the row stride: not stored
+                            *reinterpret_cast<double2*>(hzrow + 8 * nt + 2 * t) = make_double2(rf[j] * hz[nt][2 * j], rf[j] * hz[nt][2 * j + 1]);
+                    v = warp_sum(v);
+                }
+                if (lane == 0) p.ws[(size_t)r * L.per_r + L.Tpart + (size_t)q * NS + oct[j]] = v;
+            }
+        }
+    }
+    // column sums of this CTA's rows: fixed order over the warps (deterministic); none for the diagonal pairs of an exact GP
+    if (!DIAG) {
+        __syncthreads();
+        double* hc = tpr + TL.hc + ((size_t)q * cs + sidx) * np;
+        for (int c = tid; c < np; c += blockDim.x) {
+            double v = 0.0;
+#pragma unroll
+            for (int w = 0; w < 8; ++w) v += sCs[(size_t)w * np + c];
+            hc[c] = v;
+        }
+    }
+}
+
+// 2 CTAs/SM (<= 128 registers, as mm_tape_tile_kernel<KS, 256>)
+template <int KS>
+__global__ void __launch_bounds__(256, 2) mm_tape_tile_m16_kernel(MMParams p) {
+    PDL_ENTRY();
+    int a, b;
+    pair_decode(blockIdx.y, a, b);
+    if (a == b && p.gp.mode == 0 && p.gp.iK != nullptr) mm_tape_body_m16<KS, true>(p);
+    else mm_tape_body_m16<KS, false>(p);
+}
+
 #endif  // __CUDACC__
 
 // taped tile pass in place of mm_tile_kernel (p.tape != nullptr); defined in mm_tape.cu

@@ -6,6 +6,7 @@ pilco_microbench_fp64 (31.7 TFLOP/s over 132 SMs x 4 sub-partitions), the fp64 i
 
     DMMA.8x8x4 (512 flop)                       17 cycles of the fp64 pipe per warp (about half the H100's fp64 tensor
                                                 rate: the native DMMA.16x8x16 reaches 54.8 TFLOP/s in the same process)
+    DMMA.16x8x4 / 16x8x8 / 16x8x16              the same pipe time per flop as their measured rates say (DMMA_CYCLES)
     DADD / DMUL / DFMA, <= 2 distinct registers  2 cycles
     DFMA with three distinct register sources    3 cycles   (operand bandwidth)
     everything else                             not priced (co-issues; what it really costs is the gap between this model
@@ -13,8 +14,9 @@ pilco_microbench_fp64 (31.7 TFLOP/s over 132 SMs x 4 sub-partitions), the fp64 i
 
     python scripts/issue_model.py [kernel-regex ...]      default: the forward and the taped tile kernel at the metric shape
 
-Output: one line per loop -- SASS address range, DMMA / fp64 (3-register ones apart) / LDS / SHFL / other counts, model
-cycles per iteration.  tests/test_sass_properties.py::test_issue_model_of_the_hot_loops pins the structure it finds.
+Output: one line per loop -- SASS address range, DMMA (by shape) / fp64 (3-register ones apart) / LDS / SHFL / other counts, model
+cycles per iteration.  tests/test_sass_properties.py::test_issue_model_of_the_hot_loops and tests/test_sass_m16.py pin the
+structure it finds.
 """
 import os
 import re
@@ -25,7 +27,12 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")
 CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-DEFAULT = [r"mm_tile_kernelILi3ELi3ELb1E", r"mm_tape_tile_kernelILi3ELi256E"]
+DEFAULT = [r"mm_tile_m16_kernelILi3E", r"mm_tape_tile_m16_kernelILi3E", r"mm_tile_kernelILi3ELi3ELb1E", r"mm_tape_tile_kernelILi3ELi256E"]
+
+# fp64-pipe cycles per warp instruction and SM sub-partition, by DMMA shape: 17 for DMMA.8x8x4 (31.7 TFLOP/s), the 16x8
+# shapes scaled by flop / rate against it (pilco_microbench_fp64 which = 7, 5, 6 on an H100 SXM: 16x8x8 51.3 and 16x8x16
+# 54.8 TFLOP/s at 700 W; 16x8x4 49.1 TFLOP/s at 400 W, where 8x8x4 also measured 31.7)
+DMMA_CYCLES = {"8x8x4": 17, "16x8x4": 22, "16x8x8": 42, "16x8x16": 79}
 
 INS = re.compile(r"^\s+/\*([0-9a-f]{4,})\*/\s+(.*?);")
 
@@ -73,7 +80,7 @@ def loops(code):
 
 
 def model(code, lo, hi):
-    c = dict(dmma=0, fp64=0, fp64_3=0, lds=0, shfl=0, other=0)
+    c = dict(dmma=0, fp64=0, fp64_3=0, lds=0, shfl=0, other=0, dmma_cycles=0, shapes={})
     for a, t in code:
         if a < lo or a > hi:
             continue
@@ -81,6 +88,9 @@ def model(code, lo, hi):
         op = body.split()[0]
         if op.startswith("DMMA"):
             c["dmma"] += 1
+            shape = op.split(".")[1] if "." in op else "8x8x4"
+            c["shapes"][shape] = c["shapes"].get(shape, 0) + 1
+            c["dmma_cycles"] += DMMA_CYCLES[shape]
         elif op.split(".")[0] in ("DADD", "DMUL", "DFMA"):
             if op.startswith("DFMA") and distinct_registers(body) >= 3:
                 c["fp64_3"] += 1
@@ -92,7 +102,7 @@ def model(code, lo, hi):
             c["shfl"] += 1
         elif op != "NOP":
             c["other"] += 1
-    c["cycles"] = 17 * c["dmma"] + 2 * c["fp64"] + 3 * c["fp64_3"]
+    c["cycles"] = c["dmma_cycles"] + 2 * c["fp64"] + 3 * c["fp64_3"]
     return c
 
 
@@ -114,5 +124,6 @@ if __name__ == "__main__":
         for name, rows in analyse(pat).items():
             print(name)
             for (lo, hi), c in rows:
-                print("  loop %05x-%05x  DMMA %3d  fp64 %3d (+%2d three-register)  LDS %3d  SHFL %2d  other %3d  -> model %4d cycles/iteration"
-                      % (lo, hi, c["dmma"], c["fp64"], c["fp64_3"], c["lds"], c["shfl"], c["other"], c["cycles"]))
+                print("  loop %05x-%05x  DMMA %3d (%s)  fp64 %3d (+%2d three-register)  LDS %3d  SHFL %2d  other %3d  -> model %4d cycles/iteration"
+                      % (lo, hi, c["dmma"], " ".join("%sx%d" % kv for kv in sorted(c["shapes"].items())), c["fp64"], c["fp64_3"],
+                         c["lds"], c["shfl"], c["other"], c["cycles"]))
