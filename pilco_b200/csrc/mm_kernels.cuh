@@ -181,6 +181,8 @@ __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int tas
             wsr[L.Wc + a] = sf2[a] * sqrt(pl) * pip;           // c_a = sf2 sqrt(prod ell^2 / det(s + Lambda^2))
             if (!ok && p.info) atomicOr(&p.info[r], 1);
         }
+        const double* beta = gp.beta + (size_t)r * gp.beta_bs; // betap row a: beta_a zero-padded to np (tile kernels' columns)
+        for (int nn = lane; nn < L.np; nn += 32) wsr[L.betap + (size_t)a * L.np + nn] = nn < gp.n ? beta[(size_t)a * gp.n + nn] : 0.0;
         return;
     }
 
@@ -252,7 +254,25 @@ __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int tas
     }
 }
 
-// stage 1 as its own launch (ordered-pair backward mode; forward mode uses mm_setup_fused_kernel)
+// zeta = X - m of restart r ([np][ldz], zero outside rows [0, n) and columns [0, D)) with coalesced 16-byte stores:
+// thread `first` of the `stride` threads writing it takes every stride-th 16-byte pair (forward mode: once per restart)
+template <int DP>
+__device__ __forceinline__ void setup_publish_zeta(const MMParams& p, int r, int first, int stride) {
+    constexpr int ldz = DP <= 4 ? 4 : (DP <= 12 ? 12 : 20);   // == L.ldz
+    const int n = p.gp.n, D = p.gp.D;
+    const double* X = p.gp.X + (size_t)r * p.gp.X_bs;
+    const double* mr = p.m + (size_t)r * p.m_rs;
+    double2* dst = reinterpret_cast<double2*>(p.ws + (size_t)r * p.L.per_r + p.L.zeta);
+    for (int e = first; e < p.L.np * ldz / 2; e += stride) {
+        const int rr = (2 * e) / ldz, cc = (2 * e) % ldz;
+        const double z0 = (rr < n && cc < D) ? X[(size_t)rr * D + cc] - mr[cc] : 0.0;
+        const double z1 = (rr < n && cc + 1 < D) ? X[(size_t)rr * D + cc + 1] - mr[cc + 1] : 0.0;
+        dst[e] = make_double2(z0, z1);
+    }
+}
+
+// stage 1 as its own launch (the two-stage form of mm_setup_launch).  Forward mode: output tasks also write their betap
+// row, and all CTAs of the restart share writing zeta -- both read by stage 2 and the tile kernels.
 template <int DP, bool BWD>
 __global__ void __launch_bounds__(32 * SETUP_WARPS) mm_setup1_kernel(MMParams p) {
     PDL_ENTRY();
@@ -267,16 +287,186 @@ __global__ void __launch_bounds__(32 * SETUP_WARPS) mm_setup1_kernel(MMParams p)
     __shared__ double spw[SETUP_WARPS][3][MAXD];
     setup_stage_s<DP>(p, r, s_s);
     __syncthreads();
-    if (task0 >= ntask) return;
-    mm_setup1_task<DP, BWD>(p, r, task, lane, s_s, sLw[warp], sQw[warp], spw[warp][0], spw[warp][1], spw[warp][2]);
+    if (task0 < ntask)
+        mm_setup1_task<DP, BWD>(p, r, task, lane, s_s, sLw[warp], sQw[warp], spw[warp][0], spw[warp][1], spw[warp][2]);
+    if (!BWD) setup_publish_zeta<DP>(p, r, blockIdx.x * blockDim.x + tid, gridDim.x * blockDim.x);
 }
 
-template <int KS> struct RowOpConsts;
+// Row-side operands of a warp's row octets for the pair block `blk`: DMMA A fragments ua[ks] = U'[row][4ks+t] with
+// U' = 2 EXP_SC p_b o (Qa zeta_row), and the scalar A'[row] = EXP_SC (log sf2_a - 0.5 sum p_a zeta^2 + z_a'Q z_a
+// - 0.5 log det R).  2*ceil(DP/8)*KS DMMA + ONE quad reduction per 8 rows (no layout shuffles: permuted B fragments).  The pair constants (this lane's B fragments
+// of Qa and its slices of p_a, p_b) are loaded once (RowOpConsts) and reused for every row octet.
 template <int KS>
-__device__ __forceinline__ void row_operands_compute(const RowOpConsts<KS>& c, const double* __restrict__ zr,
-                                                     bool live, int lane, double (&ua)[KS], double& Apv);
+struct RowOpConsts {
+    static constexpr int DP = 4 * KS, NT = (DP + 7) / 8;
+    // B fragments of Qa with PERMUTED columns: column c of n-tile nt is Qa row 8 nt + pi(c), pi = (0,4,1,5,2,6,3,7), so
+    // that the C fragment of Z.Qa' (row g; this lane's two columns = actual columns 8 nt + t and 8 nt + 4 + t) IS the
+    // A-fragment layout of k-steps 2 nt and 2 nt + 1 -- U' leaves the product without a single shuffle (the same
+    // trick as the taped tile kernel's second product)
+    double bq[KS][NT];
+    double pak[KS];             // p_a[4 ks + t]
+    double pac[NT][2], pbc[NT][2];   // p_a, p_b at this lane's C-fragment columns 8 nt + t, 8 nt + 4 + t
+    double lsa, hld;            // log sf2_a, 0.5 log det R
+    __device__ __forceinline__ void load(const double* __restrict__ blk, int lane) {
+        const int g = lane >> 2, t = lane & 3;
+        const int pg = (g >> 1) | ((g & 1) << 2);              // pi(g)
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            pak[ks] = blk[PAIR_PA + 4 * ks + t];
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const int i = 8 * nt + pg;
+                bq[ks][nt] = i < DP ? blk[PAIR_QA + i * DP + 4 * ks + t] : 0.0;
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int c = 8 * nt + 4 * h + t;
+                pac[nt][h] = c < DP ? blk[PAIR_PA + c] : 0.0;
+                pbc[nt][h] = c < DP ? blk[PAIR_PB + c] : 0.0;
+            }
+        }
+        lsa = blk[PAIR_SC + 1]; hld = blk[PAIR_SC + 0];
+    }
+};
 
-// stage 2: the throughput part: one CTA (128 threads) per task sweeps the centres
+// NO row octets at once (independent DMMA chains in flight; every octet's arithmetic is the same whatever NO is).
+// zr[o] = zeta row of this lane's centre (row g of octet o), readable at [0, ldz)
+template <int KS, int NO>
+__device__ __forceinline__ void row_operands_octets(const RowOpConsts<KS>& c, const double* const (&zr)[NO], const bool (&live)[NO],
+                                                    int lane, double (&ua)[NO][KS], double (&Apv)[NO]) {
+    constexpr int DP = 4 * KS, NT = (DP + 7) / 8;
+    const int t = lane & 3;
+    double z[NO][KS], va[NO][NT][2];
+    double x[NO];                                               // this lane's share of z_a'Q z_a - 0.5 sum p_a zeta^2
+#pragma unroll
+    for (int o = 0; o < NO; ++o) {
+        x[o] = 0.0;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            z[o][ks] = zr[o][4 * ks + t];
+            x[o] = fma(-0.5 * c.pak[ks] * z[o][ks], z[o][ks], x[o]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) { va[o][nt][0] = va[o][nt][1] = 0.0; }
+    }
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int o = 0; o < NO; ++o) dmma884(va[o][nt][0], va[o][nt][1], z[o][ks], c.bq[ks][nt]);
+    // va[nt][h] = (Qa zeta)[8 nt + 4 h + t] of row g: column 4 ks + t with ks = 2 nt + h, i.e. A-fragment layout already
+#pragma unroll
+    for (int o = 0; o < NO; ++o)
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            const int nt = ks >> 1, h = ks & 1;
+            x[o] = fma(c.pac[nt][h] * z[o][ks], va[o][nt][h], x[o]);      // (zeta at that column is this lane's z[ks])
+            ua[o][ks] = (2.0 * EXP_SC) * c.pbc[nt][h] * va[o][nt][h];
+        }
+#pragma unroll
+    for (int o = 0; o < NO; ++o) x[o] += __shfl_xor_sync(0xffffffffu, x[o], 1);     // one quad reduction for both terms
+#pragma unroll
+    for (int o = 0; o < NO; ++o) x[o] += __shfl_xor_sync(0xffffffffu, x[o], 2);
+#pragma unroll
+    for (int o = 0; o < NO; ++o) Apv[o] = live[o] ? EXP_SC * (c.lsa + x[o] - c.hld) : NEG_PAD;
+}
+
+// one-shot form (backward tile kernel prologue): zeta rows are read from the workspace (L2 resident)
+template <int KS>
+__device__ __forceinline__ void tile_row_operands(const double* __restrict__ blk, const double* __restrict__ zeta,
+                                                  int ldz, int row, bool live, int lane,
+                                                  double (&ua)[KS], double& Apv) {
+    RowOpConsts<KS> c;
+    c.load(blk, lane);
+    const double* const zr[1] = {zeta + (size_t)row * ldz};
+    const bool l1[1] = {live};
+    double u1[1][KS], a1[1];
+    row_operands_octets<KS, 1>(c, zr, l1, lane, u1, a1);
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) ua[ks] = u1[0][ks];
+    Apv = a1[0];
+}
+
+// Column-side exponent piece of NO row octets of a pair: B_ab[m] = EXP_SC (log sf2_b + z'(Q diag p_b) z - 0.5 sum p_b z^2)
+// of this lane's centre (row g of octet o, zeta row zr[o]), (Q diag p_b) zeta as the DMMA mini-GEMM Z[8 x DP] . Qb^T
+// with the B fragments bqb[ks][nt] = Qb[8 nt + g][4 ks + t], and one quad reduction; NEG_PAD for padding rows.  As in
+// row_operands_octets, every octet's arithmetic is the same whatever NO is.
+template <int KS, int NO>
+__device__ __forceinline__ void pair_b_octets(const double (&bqb)[KS][(4 * KS + 7) / 8], const double* __restrict__ pb, double lsb,
+                                              const double* const (&zr)[NO], const bool (&live)[NO], int lane, double (&bv)[NO]) {
+    constexpr int DP = 4 * KS, NT = (DP + 7) / 8;
+    const int t = lane & 3;
+    double z[NO][KS], vb[NO][NT][2], kbp[NO], xb[NO];
+#pragma unroll
+    for (int o = 0; o < NO; ++o) {
+        kbp[o] = 0.0;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            z[o][ks] = zr[o][4 * ks + t];
+            kbp[o] = fma(pb[4 * ks + t] * z[o][ks], z[o][ks], kbp[o]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) { vb[o][nt][0] = vb[o][nt][1] = 0.0; }
+    }
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int o = 0; o < NO; ++o) dmma884(vb[o][nt][0], vb[o][nt][1], z[o][ks], bqb[ks][nt]);
+#pragma unroll
+    for (int o = 0; o < NO; ++o) {
+        double qbp = 0.0;
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            const int i0 = 8 * nt + 2 * t;                      // this lane's two columns of the C fragment
+            if (i0 < DP) qbp = fma(pb[i0] * zr[o][i0], vb[o][nt][0], fma(pb[i0 + 1] * zr[o][i0 + 1], vb[o][nt][1], qbp));
+        }
+        xb[o] = fma(-0.5, kbp[o], qbp);                         // one quad reduction for both terms
+    }
+#pragma unroll
+    for (int o = 0; o < NO; ++o) xb[o] += __shfl_xor_sync(0xffffffffu, xb[o], 1);
+#pragma unroll
+    for (int o = 0; o < NO; ++o) xb[o] += __shfl_xor_sync(0xffffffffu, xb[o], 2);
+#pragma unroll
+    for (int o = 0; o < NO; ++o) bv[o] = live[o] ? EXP_SC * (lsb + xb[o]) : NEG_PAD;
+}
+
+// Output task a, one centre: t = W_a z, w = beta_a[m] exp(-z'W_a z / 2); acc[i] += w t_i, acc[DP] += w
+template <int DP>
+__device__ __forceinline__ void out_centre(const double* __restrict__ sW, const double (&z)[DP], double bw, double (&acc)[DP + 1]) {
+    double t[DP], e = 0.0;
+#pragma unroll
+    for (int i = 0; i < DP; ++i) {
+        double v = 0.0;
+#pragma unroll
+        for (int j = 0; j < DP; ++j) v = fma(sW[i * DP + j], z[j], v);
+        t[i] = v; e = fma(z[i], v, e);
+    }
+    const double w = bw * exp(-0.5 * e);
+    acc[DP] += w;
+#pragma unroll
+    for (int i = 0; i < DP; ++i) acc[i] = fma(w, t[i], acc[i]);
+}
+
+// Output task a: the CTA's fixed-order reduction of the per-thread sums (thread tid of 128 holds centres tid + 128 k),
+// then M_a = c_a sum w and V_a = c_a sum w W_a z
+template <int DP>
+__device__ __forceinline__ void out_task_store(const MMParams& p, int r, int a, double (&acc)[DP + 1], double* sred, double* sout) {
+    const int tid = threadIdx.x, D = p.gp.D, E = p.gp.E;
+    const double c = p.ws[(size_t)r * p.L.per_r + p.L.Wc + a];
+    block_sum<DP + 1>(acc, DP + 1, sred, sout);
+    if (tid == 0) p.M[(size_t)r * E + a] = c * sout[DP];
+    if (tid < D) p.V[((size_t)r * D + tid) * E + a] = c * sout[tid];
+}
+
+// stage 2 of one task by one CTA of 128 threads, as the fused setup kernel runs it (both modes) and the ordered-pair
+// backward mode's stage-2 launch.  The forward two-stage form splits it into mm_setup2_out_kernel and
+// mm_setup2_pair_kernel (below), which run the same per-centre and per-octet arithmetic.
 template <int DP, bool BWD>
 __device__ __forceinline__ void mm_setup2_task(const MMParams& p, int r, int task, int part = 0, int nparts = 1) {
     const pilco_gp_model& gp = p.gp;
@@ -287,31 +477,28 @@ __device__ __forceinline__ void mm_setup2_task(const MMParams& p, int r, int tas
     const int tid = threadIdx.x;
 
     __shared__ double sQa[MAXD * MAXD], sQb[MAXD * MAXD];
-    __shared__ double sm[MAXD], pa[MAXD], pb[MAXD];
-    __shared__ __align__(16) double sStage[128 * (MAXD + 5)];   // [128][ldz|1] staging: X block in, U'/zeta block out
+    __shared__ double sm[MAXD], pb[MAXD];
+    __shared__ __align__(16) double sStage[128 * (MAXD + 5)];   // [128][ldz|1] staging: X block in
     __shared__ double sred[(MAXD + 1) * 4], sout[MAXD + 1];
 
     const double* X = gp.X + (size_t)r * gp.X_bs;
-    const double* ell = gp.ell + (size_t)r * gp.ell_bs;
-    const double* sf2 = gp.sf2 + (size_t)r * gp.sf2_bs;
     const double* beta = gp.beta + (size_t)r * gp.beta_bs;
     const double* mr = p.m + (size_t)r * p.m_rs;
     double* wsr = p.ws + (size_t)r * L.per_r;
     if (tid < DP) sm[tid] = tid < D ? mr[tid] : 0.0;
 
     if (!BWD && task < E) {
-        // ---------------- output task: mean M_a and V_a; betap and zeta ----------------
+        // ---------------- output task: mean M_a and V_a (betap and zeta: stage 1) ----------------
         const int a = task;
         const double* Wg = wsr + L.Wm + (size_t)a * MAXD * MAXD;
         for (int e = tid; e < DP * DP; e += blockDim.x) sQa[e] = Wg[e];
         __syncthreads();
-        const double c = wsr[L.Wc + a];
         double acc[DP + 1];
 #pragma unroll
         for (int i = 0; i <= DP; ++i) acc[i] = 0.0;
         const int lds = ldz | 1;
-        for (int n0 = 0; n0 < np; n0 += 128) {
-            const int rows = (n - n0) < 128 ? ((n - n0) > 0 ? (n - n0) : 0) : 128;
+        for (int n0 = 0; n0 < n; n0 += 128) {
+            const int rows = (n - n0) < 128 ? (n - n0) : 128;
             __syncthreads();
             for (int e = tid; e < rows * ldz; e += blockDim.x) {
                 const int rr = e / ldz, cc = e % ldz;
@@ -319,46 +506,14 @@ __device__ __forceinline__ void mm_setup2_task(const MMParams& p, int r, int tas
             }
             __syncthreads();
             const int nn = n0 + tid;
-            double z[DP];
-            double bw = 0.0;
             if (nn < n) {
+                double z[DP];
 #pragma unroll
                 for (int d = 0; d < DP; ++d) z[d] = d < D ? sStage[tid * lds + d] - sm[d] : 0.0;
-                double t[DP], e = 0.0;
-#pragma unroll
-                for (int i = 0; i < DP; ++i) {
-                    double v = 0.0;
-#pragma unroll
-                    for (int j = 0; j < DP; ++j) v = fma(sQa[i * DP + j], z[j], v);
-                    t[i] = v; e = fma(z[i], v, e);
-                }
-                bw = beta[(size_t)a * n + nn];
-                const double w = bw * exp(-0.5 * e);
-                acc[DP] += w;
-#pragma unroll
-                for (int i = 0; i < DP; ++i) acc[i] = fma(w, t[i], acc[i]);
-            } else {
-#pragma unroll
-                for (int d = 0; d < DP; ++d) z[d] = 0.0;
-            }
-            if (nn < np) wsr[L.betap + (size_t)a * np + nn] = bw;
-            if (a == 0) {                                       // zeta block: smem -> coalesced double2 stores
-                __syncthreads();
-#pragma unroll
-                for (int d = 0; d < DP; ++d) sStage[tid * lds + d] = z[d];
-                for (int d = DP; d < ldz; ++d) sStage[tid * lds + d] = 0.0;
-                __syncthreads();
-                const int rows_out = (np - n0) < 128 ? (np - n0) : 128;
-                double2* dst = reinterpret_cast<double2*>(wsr + L.zeta + (size_t)n0 * ldz);
-                for (int e = tid; e < rows_out * ldz / 2; e += blockDim.x) {
-                    const int rr = (2 * e) / ldz, cc = (2 * e) % ldz;
-                    dst[e] = make_double2(sStage[rr * lds + cc], sStage[rr * lds + cc + 1]);
-                }
+                out_centre<DP>(sQa, z, beta[(size_t)a * n + nn], acc);
             }
         }
-        block_sum<DP + 1>(acc, DP + 1, sred, sout);
-        if (tid == 0) p.M[(size_t)r * E + a] = c * sout[DP];
-        if (tid < D) p.V[((size_t)r * D + tid) * E + a] = c * sout[tid];
+        out_task_store<DP>(p, r, a, acc, sred, sout);
         return;
     }
 
@@ -407,47 +562,149 @@ __device__ __forceinline__ void mm_setup2_task(const MMParams& p, int r, int tas
         for (int grp = warp; grp < 16; grp += 4) {
             const int row = n0 + 8 * grp + g;
             if (n0 + 8 * grp >= np) break;                      // warp-uniform
-            const double* zr = sStage + (size_t)(8 * grp + g) * ldz;
-            double z[KS], vb[NT][2];
-            double kbp = 0.0;
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks) {
-                z[ks] = zr[4 * ks + t];
-                kbp = fma(pb[4 * ks + t] * z[ks], z[ks], kbp);
-            }
-#pragma unroll
-            for (int nt = 0; nt < NT; ++nt) { vb[nt][0] = vb[nt][1] = 0.0; }
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-                for (int nt = 0; nt < NT; ++nt) dmma884(vb[nt][0], vb[nt][1], z[ks], bqb[ks][nt]);
-            double qbp = 0.0;
-#pragma unroll
-            for (int nt = 0; nt < NT; ++nt) {
-                const int i0 = 8 * nt + 2 * t;                  // this lane's two columns of the C fragment
-                if (i0 < DP) qbp = fma(pb[i0] * zr[i0], vb[nt][0], fma(pb[i0 + 1] * zr[i0 + 1], vb[nt][1], qbp));
-            }
-            double xb = fma(-0.5, kbp, qbp);                     // one quad reduction for both terms
-            xb += __shfl_xor_sync(0xffffffffu, xb, 1); xb += __shfl_xor_sync(0xffffffffu, xb, 2);
-            if (t == 0) wsr[L.Bq + (size_t)q * np + row] = row < n ? EXP_SC * (lsb + xb) : NEG_PAD;
+            const double* const zr[1] = {sStage + (size_t)(8 * grp + g) * ldz};
+            const bool live[1] = {row < n};
+            double bv[1];
+            pair_b_octets<KS, 1>(bqb, pb, lsb, zr, live, lane, bv);
+            if (t == 0) wsr[L.Bq + (size_t)q * np + row] = bv[0];
             if (!BWD) {
-                // row side of the same 8 centres: DMMA A fragments of U' and the scalar A' (see tile_row_operands),
+                // row side of the same 8 centres: DMMA A fragments of U' and the scalar A' (see row_operands_octets),
                 // written in the layout the tile kernel's prologue loads with three coalesced 8-byte loads per lane
-                double ua[KS], Apv;
-                row_operands_compute<KS>(roc, zr, row < n, lane, ua, Apv);
+                double ua[1][KS], Apv[1];
+                row_operands_octets<KS, 1>(roc, zr, live, lane, ua, Apv);
                 double* uf = wsr + L.Ufrag + ((size_t)q * (np >> 3) + ((n0 >> 3) + grp)) * (KS * 32);
 #pragma unroll
-                for (int ks = 0; ks < KS; ++ks) uf[ks * 32 + lane] = ua[ks];
-                if (t == 0) wsr[L.Arow + (size_t)q * np + row] = Apv;
+                for (int ks = 0; ks < KS; ++ks) uf[ks * 32 + lane] = ua[0][ks];
+                if (t == 0) wsr[L.Arow + (size_t)q * np + row] = Apv[0];
             }
         }
     }
 }
 
-template <int DP, bool BWD>
-__global__ void __launch_bounds__(128) mm_setup2_kernel(MMParams p) {
+// stage 2 of the ordered-pair backward mode: one CTA per (ordered pair, restart)
+template <int DP>
+__global__ void __launch_bounds__(128) mm_setup2_bwd_kernel(MMParams p) {
     PDL_ENTRY();
-    mm_setup2_task<DP, BWD>(p, blockIdx.y, BWD ? blockIdx.x + p.gp.E : blockIdx.x);
+    mm_setup2_task<DP, true>(p, blockIdx.y, blockIdx.x + p.gp.E);
+}
+
+// Forward stage 2, output tasks: M_a and V_a, one CTA of 128 threads per (output, restart).  The zeta rows written by
+// stage 1 are read straight from the workspace (each thread's row is DP/2 contiguous 16-byte loads), one centre ahead.
+// Register cap (launched with 128 threads): the prefetched row without spills, and 3 CTAs per SM at D <= 12.
+template <int DP>
+__global__ void __maxnreg__(DP <= 12 ? 168 : 232) mm_setup2_out_kernel(MMParams p) {
+    PDL_ENTRY();
+    constexpr int ldz = DP <= 4 ? 4 : (DP <= 12 ? 12 : 20);   // == L.ldz
+    const int a = blockIdx.x, r = blockIdx.y, tid = threadIdx.x;
+    const int n = p.gp.n;
+    __shared__ double sW[DP * DP];
+    __shared__ double sred[(DP + 1) * 4], sout[DP + 1];
+    const double* wsr = p.ws + (size_t)r * p.L.per_r;
+    const double* beta = p.gp.beta + (size_t)r * p.gp.beta_bs + (size_t)a * n;
+    for (int e = tid; e < DP * DP; e += blockDim.x) sW[e] = wsr[p.L.Wm + (size_t)a * MAXD * MAXD + e];
+    __syncthreads();
+    double acc[DP + 1];
+#pragma unroll
+    for (int i = 0; i <= DP; ++i) acc[i] = 0.0;
+    // thread tid takes centres tid, tid + 128, ...; the next centre's zeta row and beta are loaded before this one's sums
+    const double2* zg = reinterpret_cast<const double2*>(wsr + p.L.zeta);
+    double2 zn[DP / 2];
+    double bn = 0.0;
+    if (tid < n) {
+#pragma unroll
+        for (int d = 0; d < DP / 2; ++d) zn[d] = zg[(size_t)tid * (ldz / 2) + d];
+        bn = beta[tid];
+    }
+    for (int n0 = 0; n0 < n; n0 += 128) {
+        const int nn = n0 + tid;
+        double z[DP];
+#pragma unroll
+        for (int d = 0; d < DP / 2; ++d) { z[2 * d] = zn[d].x; z[2 * d + 1] = zn[d].y; }
+        const double bw = bn;
+        if (nn + 128 < n) {
+#pragma unroll
+            for (int d = 0; d < DP / 2; ++d) zn[d] = zg[(size_t)(nn + 128) * (ldz / 2) + d];
+            bn = beta[nn + 128];
+        }
+        __syncwarp();                                          // W stays in shared memory: it is not hoisted into DP^2 registers
+        if (nn < n) out_centre<DP>(sW, z, bw, acc);
+    }
+    out_task_store<DP>(p, r, a, acc, sred, sout);
+}
+
+// rows of zeta per pair-kernel CTA: all np rows while zeta, the pair block and the barrier fit 48 KB of shared memory
+// (np <= 448 at ldz = 12), else an even split in multiples of 64 rows
+static inline __host__ __device__ int setup_pair_rows(int np, int ldz) {
+    const int cap = ((48 * 1024 - 16 - PAIR_BLK * 8) / (ldz * 8)) & ~63;
+    const int nch = (np + cap - 1) / cap;
+    return ((np + nch - 1) / nch + 63) & ~63;
+}
+static inline __host__ __device__ size_t setup_pair_smem_bytes(int rows, int ldz) { return 16 + (size_t)PAIR_BLK * 8 + (size_t)rows * ldz * 8; }
+
+// Forward stage 2, pair tasks: one CTA per (pair, row chunk, restart).  One TMA bulk copy each brings the pair block
+// and the chunk's zeta rows (written by stage 1) into shared memory on one mbarrier; after that single wait no CTA-wide
+// barrier.  Each warp sweeps octet pairs {2j, 2j+1}, j = warp, warp + 8, ..., the two octets as independent DMMA chains:
+// first their B pieces, then their row operands.  Writes B_ab, U' (DMMA A fragments) and A' in the layout the tile kernels read.
+#define SETUP_PAIR_WARPS 8
+template <int DP>
+__global__ void __launch_bounds__(32 * SETUP_PAIR_WARPS, 3) mm_setup2_pair_kernel(MMParams p, int rows) {
+    PDL_ENTRY();
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr int KS = DP / 4, NT = (DP + 7) / 8;
+    constexpr int ldz = DP <= 4 ? 4 : (DP <= 12 ? 12 : 20);   // == L.ldz
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
+    double* sblk = reinterpret_cast<double*>(smem_raw + 16);   // pair block (PAIR_*)
+    double* sZ = sblk + PAIR_BLK;                              // zeta rows [c0, c0 + cm)
+    const MMWs& L = p.L;
+    const int n = p.gp.n, np = L.np;
+    const int q = blockIdx.x, r = blockIdx.z, c0 = blockIdx.y * rows;
+    const int cm = (np - c0) < rows ? (np - c0) : rows;        // multiple of 64
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+    double* wsr = p.ws + (size_t)r * L.per_r;
+    if (tid == 0) {
+        mbar_init(bar, 1); mbar_fence_init();
+        mbar_expect_tx(bar, (unsigned)(PAIR_BLK * 8 + cm * ldz * 8));
+        tma_bulk_g2s(sblk, wsr + L.Qab + (size_t)q * PAIR_BLK, (unsigned)(PAIR_BLK * 8), bar);
+        tma_bulk_g2s(sZ, wsr + L.zeta + (size_t)c0 * ldz, (unsigned)(cm * ldz * 8), bar);
+    }
+    __syncthreads();                                           // barrier initialisation visible to the waiting warps
+    mbar_wait(bar, 0);
+    double* Bq = wsr + L.Bq + (size_t)q * np + c0;
+    double* Ar = wsr + L.Arow + (size_t)q * np + c0;
+    double* uf = wsr + L.Ufrag + ((size_t)q * (np >> 3) + (c0 >> 3)) * (KS * 32);
+    // two sweeps over the warp's octet pairs, so that only one sweep's pair constants are held in registers
+    {
+        double bqb[KS][NT];                                    // B fragments: B[k][n] = Qb[n][k]
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                const int i = 8 * nt + g;
+                bqb[ks][nt] = i < DP ? sblk[PAIR_QB + i * DP + 4 * ks + t] : 0.0;
+            }
+        const double* pb = sblk + PAIR_PB;
+        const double lsb = sblk[PAIR_SC + 2];
+        for (int j = warp; 16 * j < cm; j += SETUP_PAIR_WARPS) {
+            const double* const zr[2] = {sZ + (size_t)(16 * j + g) * ldz, sZ + (size_t)(16 * j + 8 + g) * ldz};
+            const bool live[2] = {c0 + 16 * j + g < n, c0 + 16 * j + 8 + g < n};
+            double bv[2];
+            pair_b_octets<KS, 2>(bqb, pb, lsb, zr, live, lane, bv);
+            if (t == 0) { Bq[16 * j + g] = bv[0]; Bq[16 * j + 8 + g] = bv[1]; }
+        }
+    }
+    RowOpConsts<KS> roc;
+    roc.load(sblk, lane);
+    for (int j = warp; 16 * j < cm; j += SETUP_PAIR_WARPS) {
+        const double* const zr[2] = {sZ + (size_t)(16 * j + g) * ldz, sZ + (size_t)(16 * j + 8 + g) * ldz};
+        const bool live[2] = {c0 + 16 * j + g < n, c0 + 16 * j + 8 + g < n};
+        double ua[2][KS], Apv[2];
+        row_operands_octets<KS, 2>(roc, zr, live, lane, ua, Apv);
+        if (t == 0) { Ar[16 * j + g] = Apv[0]; Ar[16 * j + 8 + g] = Apv[1]; }
+#pragma unroll
+        for (int o = 0; o < 2; ++o)
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) uf[(size_t)(2 * j + o) * (KS * 32) + ks * 32 + lane] = ua[o][ks];
+    }
 }
 
 // both stages of one task in ONE launch -- stage 2 only consumes the stage-1 output of its own task,
@@ -472,86 +729,7 @@ __global__ void __launch_bounds__(128, 2) mm_setup_fused_kernel(MMParams p, int 
     if (threadIdx.x < 32) mm_setup1_task<DP, BWD>(p, r, task, threadIdx.x, f_s, f_L, f_Q, f_p[0], f_p[1], f_p[2]);
     __syncthreads();
     mm_setup2_task<DP, BWD>(p, r, task, part, nparts);
-}
-
-// Row-side operands of one warp's 8 rows for the pair block `blk`: DMMA A fragments ua[ks] = U'[row][4ks+t] with
-// U' = 2 EXP_SC p_b o (Qa zeta_row), and the scalar A'[row] = EXP_SC (log sf2_a - 0.5 sum p_a zeta^2 + z_a'Q z_a
-// - 0.5 log det R).  2*ceil(DP/8)*KS DMMA + ONE quad reduction per 8 rows (no layout shuffles: permuted B fragments).  The pair constants (this lane's B fragments
-// of Qa and its slices of p_a, p_b) are loaded once (RowOpConsts) and reused for every row octet.
-template <int KS>
-struct RowOpConsts {
-    static constexpr int DP = 4 * KS, NT = (DP + 7) / 8;
-    // B fragments of Qa with PERMUTED columns: column c of n-tile nt is Qa row 8 nt + pi(c), pi = (0,4,1,5,2,6,3,7), so
-    // that the C fragment of Z.Qa' (row g; this lane's two columns = actual columns 8 nt + t and 8 nt + 4 + t) IS the
-    // A-fragment layout of k-steps 2 nt and 2 nt + 1 -- U' leaves the product without a single shuffle (the same
-    // trick as the taped tile kernel's second product)
-    double bq[KS][NT];
-    double pak[KS];             // p_a[4 ks + t]
-    double pac[NT][2], pbc[NT][2];   // p_a, p_b at this lane's C-fragment columns 8 nt + t, 8 nt + 4 + t
-    double lsa, hld;            // log sf2_a, 0.5 log det R
-    __device__ __forceinline__ void load(const double* __restrict__ blk, int lane) {
-        const int g = lane >> 2, t = lane & 3;
-        const int pg = (g >> 1) | ((g & 1) << 2);              // pi(g)
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-            pak[ks] = blk[PAIR_PA + 4 * ks + t];
-#pragma unroll
-            for (int nt = 0; nt < NT; ++nt) {
-                const int i = 8 * nt + pg;
-                bq[ks][nt] = i < DP ? blk[PAIR_QA + i * DP + 4 * ks + t] : 0.0;
-            }
-        }
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int c = 8 * nt + 4 * h + t;
-                pac[nt][h] = c < DP ? blk[PAIR_PA + c] : 0.0;
-                pbc[nt][h] = c < DP ? blk[PAIR_PB + c] : 0.0;
-            }
-        }
-        lsa = blk[PAIR_SC + 1]; hld = blk[PAIR_SC + 0];
-    }
-};
-
-// zr = zeta row of this lane's centre (row g of the octet), readable at [0, ldz)
-template <int KS>
-__device__ __forceinline__ void row_operands_compute(const RowOpConsts<KS>& c, const double* __restrict__ zr,
-                                                     bool live, int lane, double (&ua)[KS], double& Apv) {
-    constexpr int DP = 4 * KS, NT = (DP + 7) / 8;
-    const int t = lane & 3;
-    double z[KS], va[NT][2];
-    double x = 0.0;                                             // this lane's share of z_a'Q z_a - 0.5 sum p_a zeta^2
-#pragma unroll
-    for (int ks = 0; ks < KS; ++ks) {
-        z[ks] = zr[4 * ks + t];
-        x = fma(-0.5 * c.pak[ks] * z[ks], z[ks], x);
-    }
-#pragma unroll
-    for (int nt = 0; nt < NT; ++nt) { va[nt][0] = va[nt][1] = 0.0; }
-#pragma unroll
-    for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) dmma884(va[nt][0], va[nt][1], z[ks], c.bq[ks][nt]);
-    // va[nt][h] = (Qa zeta)[8 nt + 4 h + t] of row g: column 4 ks + t with ks = 2 nt + h, i.e. A-fragment layout already
-#pragma unroll
-    for (int ks = 0; ks < KS; ++ks) {
-        const int nt = ks >> 1, h = ks & 1;
-        x = fma(c.pac[nt][h] * z[ks], va[nt][h], x);            // (zeta at that column is this lane's z[ks])
-        ua[ks] = (2.0 * EXP_SC) * c.pbc[nt][h] * va[nt][h];
-    }
-    x += __shfl_xor_sync(0xffffffffu, x, 1); x += __shfl_xor_sync(0xffffffffu, x, 2);       // one quad reduction for both terms
-    Apv = live ? EXP_SC * (c.lsa + x - c.hld) : NEG_PAD;
-}
-
-// one-shot form (backward tile kernel prologue): zeta rows are read from the workspace (L2 resident)
-template <int KS>
-__device__ __forceinline__ void tile_row_operands(const double* __restrict__ blk, const double* __restrict__ zeta,
-                                                  int ldz, int row, bool live, int lane,
-                                                  double (&ua)[KS], double& Apv) {
-    RowOpConsts<KS> c;
-    c.load(blk, lane);
-    row_operands_compute<KS>(c, zeta + (size_t)row * ldz, live, lane, ua, Apv);
+    if (!BWD && blockIdx.x == 0) setup_publish_zeta<DP>(p, r, threadIdx.x, blockDim.x);   // forward: output task 0's CTA
 }
 
 // both stages
@@ -577,7 +755,14 @@ static inline void mm_setup_launch(const MMParams& p, cudaStream_t st) {
         }
     }
     launch_hi(mm_setup1_kernel<DP, BWD>, dim3((ntask + SETUP_WARPS - 1) / SETUP_WARPS, p.R), dim3(32 * SETUP_WARPS), 0, st, p);
-    launch_hi(mm_setup2_kernel<DP, BWD>, dim3(ntask, p.R), dim3(128), 0, st, p);
+    if constexpr (BWD) {
+        launch_hi(mm_setup2_bwd_kernel<DP>, dim3(ntask, p.R), dim3(128), 0, st, p);
+    } else {
+        const int rows = setup_pair_rows(p.L.np, p.L.ldz);
+        launch_hi(mm_setup2_out_kernel<DP>, dim3(p.gp.E, p.R), dim3(128), 0, st, p);
+        launch_hi(mm_setup2_pair_kernel<DP>, dim3(p.L.P, (p.L.np + rows - 1) / rows, p.R), dim3(32 * SETUP_PAIR_WARPS),
+                  setup_pair_smem_bytes(rows, p.L.ldz), st, p, rows);
+    }
 }
 
 // -------------------------------------------------------------------------------------------------
