@@ -164,6 +164,21 @@ int pilco_fitc_factorize(int N, int Mi, int D, int E,
                          double* iK, int ldk, double* beta,
                          int* info, void* ws, size_t ws_bytes, pilco_stream_t stream);
 
+/* ---- prediction at deterministic inputs -------------------------------------------------------
+ * Stands in for gpflow GPR.predict_f / GPRFITC.predict_f, which the reference's users call on the output models of
+ * MGPR / SMGPR (pilco/models/mgpr.py:28-36, smgpr.py:16-22) to check the learnt dynamics: the posterior of outputs
+ * e0 .. e0+ne-1 of an unbatched mode-0 model with iK (pilco_gp_factorize, pilco_gp_append or pilco_fitc_factorize) at
+ * T inputs Xs [T,D]:  mean = k*' beta_e,  var = sf2_e - k*' iK_e k*  (latent f; the caller adds sn2 for y), or with
+ * full_cov the [ne,T,T] covariance K** - K* iK_e K*'.  A point's mean and variance do not depend on T, on its row in
+ * Xs or on which outputs are requested (fixed-order reductions; diagonal path).  PILCO_ERR_UNSUPPORTED: mode != 0,
+ * no iK, or a batched model; PILCO_ERR_ALIGN: iK or ws not 16-byte aligned, or ldk odd. */
+size_t pilco_gp_predict_workspace_bytes(int n, int D, int E, int T, int full_cov);   /* 0: unsupported arguments */
+int    pilco_gp_predict(const pilco_gp_model* gp, int e0, int ne, int T,
+                        const double* Xs,      /* [T,D] deterministic inputs */
+                        double* mean,          /* [T,ne] */
+                        double* var,           /* full_cov ? [ne,T,T] : [T,ne] */
+                        int full_cov, void* ws, size_t ws_bytes, pilco_stream_t stream);
+
 /* ---- closed-form moments ---------------------------------------------------------------------
  * squash_sin (pilco/controllers.py:13-36; gSin.m:33-48), LinearController.compute_action
  * (controllers.py:46-58; conlin.m:50-62), ExponentialReward.compute_reward (rewards.py:19-51;

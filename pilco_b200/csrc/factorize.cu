@@ -1082,3 +1082,23 @@ int pilco_fitc_factorize(int N, int Mi, int D, int E, const double* X, const dou
 }
 
 }  // extern "C"
+
+// pilco_gp_predict with full_cov (predict.cu validates): ne outputs whose ell, sf2, beta, iK start at the first requested
+// one.  ws: K* [ne,T,np] (zero in columns n..np) then W = K* iK [ne,T,np].  mean [T,ne], cov [ne,T,T].
+int gp_predict_full_cov(cudaStream_t st, int n, int D, int ne, int T, const double* C, const double* ell, const double* sf2,
+                        const double* beta, const double* iK, int ldk, const double* Xs, double* mean, double* cov, double* ws) {
+    const int np = pad64(n);
+    const long long ts = (long long)T * np, cs = (long long)T * T, ks = (long long)ldk * ldk;
+    double* Ks = ws;
+    double* W = Ks + (size_t)ne * ts;
+    GramArgs gs{T, n, D, ne, Xs, 0, C, 0, ell, 0, sf2, 0, nullptr, 0, 0.0, Ks, np, ts, T, np, 0};
+    launch_hi(gram_kernel, dim3((np + 31) / 32, (T + 7) / 8, ne), dim3(32, 8), 0, st, gs);
+    GramArgs gss{T, T, D, ne, Xs, 0, Xs, 0, ell, 0, sf2, 0, nullptr, 0, 0.0, cov, T, cs, T, T, 0};
+    launch_hi(gram_kernel, dim3((T + 31) / 32, (T + 7) / 8, ne), dim3(32, 8), 0, st, gss);
+    CUDA_LAUNCH_CHECK();
+    int rc = gemm(st, ne, T, 1, n, 0, 0, 1.0, Ks, np, ts, beta, 1, n, 0.0, mean, ne, 1);            // mean = K* beta
+    if (rc) return rc;
+    rc = gemm(st, ne, T, np, np, 0, 0, 1.0, Ks, np, ts, iK, ldk, ks, 0.0, W, np, ts);              // W = K* iK
+    if (rc) return rc;
+    return gemm(st, ne, T, T, np, 0, 1, -1.0, W, np, ts, Ks, np, ts, 1.0, cov, T, cs);            // K** - W K*'
+}

@@ -217,6 +217,27 @@ def fitc_factorize(X, Z, Y, ell, sf2, sn2):
     return gp
 
 
+def gp_predict(gp, Xnew, e0=0, ne=None, full_cov=False):
+    """pilco_gp_predict: posterior of outputs e0 .. e0+ne-1 of the factorised model ``gp`` at deterministic inputs
+    Xnew [T,D] -> mean [T,ne] and the latent variance, [T,ne] or with ``full_cov`` the covariance [ne,T,T]."""
+    Xs = dev(Xnew)
+    if Xs.dim() != 2 or Xs.shape[1] != gp.D:
+        raise ValueError("gp_predict: Xnew must be [T, %d], got %s" % (gp.D, tuple(Xs.shape)))
+    T = int(Xs.shape[0])
+    ne = gp.E - int(e0) if ne is None else int(ne)
+    if T < 1 or ne < 1:
+        raise ValueError("gp_predict: needs at least one input row and one output (T=%d, ne=%d)" % (T, ne))
+    d = device()
+    mean = torch.empty((T, ne), dtype=F64, device=d)
+    var = torch.empty((ne, T, T) if full_cov else (T, ne), dtype=F64, device=d)
+    wsb = lib.pilco_gp_predict_workspace_bytes(gp.n, gp.D, ne, T, 1 if full_cov else 0)
+    ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+    g = gp.struct()
+    check(lib.pilco_gp_predict(C.byref(g), int(e0), ne, T, ptr(Xs), ptr(mean), ptr(var), 1 if full_cov else 0,
+                               ptr(ws), wsb, stream_ptr()), "gp_predict")
+    return mean, var
+
+
 def mm_forward(gp, m, s):
     """pilco_mm_forward: m [R,D], s [R,D,D] -> M [R,E], S [R,E,E], V [R,D,E], info [R]."""
     m, s = dev(m), dev(s)

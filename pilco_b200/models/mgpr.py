@@ -64,6 +64,75 @@ class GPRModel:
     def optimize(self, maxiter=None):
         return gp_training.minimize(self._loss, self.parameters, maxiter=maxiter)
 
+    # ---- prediction at deterministic inputs (gpflow.models.GPR.predict_f / predict_y / predict_log_density) -----------
+    _owner = None           # (MGPR, output index) of the models an MGPR creates
+
+    def _hypers(self):
+        return (np.asarray(self.kernel.lengthscales, dtype=np.float64).reshape(1, -1),
+                np.asarray(self.kernel.variance, dtype=np.float64).reshape(1),
+                np.asarray(self.likelihood.variance, dtype=np.float64).reshape(1))
+
+    def _own_key(self):
+        parts = [np.asarray(self.data[0], dtype=np.float64), np.asarray(self.data[1], dtype=np.float64), *self._hypers()]
+        return hash(tuple(np.ascontiguousarray(p).tobytes() for p in parts))
+
+    def _own_factorize(self):
+        ell, sf2, sn2 = self._hypers()
+        return engine.gp_factorize(np.asarray(self.data[0]), np.asarray(self.data[1]).reshape(-1, 1), ell, sf2, sn2)
+
+    def _predict_source(self):
+        """(DeviceGP, output index) holding this model's posterior.  A model of an MGPR whose inputs are the MGPR's
+        uses the MGPR's resident factorisation (the one the rollout uses, appended rows included); any other model
+        factorises its own data, cached until data or hyper-parameters change."""
+        engine.device()
+        if self._owner is not None:
+            mgpr, i = self._owner
+            if mgpr.mm_mode == 0 and i < len(mgpr.models) and mgpr.models[i] is self:
+                try:
+                    same = np.array_equal(np.asarray(self.data[0], dtype=np.float64), mgpr.X) and mgpr.Y.shape[1] == len(mgpr.models)
+                except ValueError:                  # outputs with different row counts: no common factorisation
+                    same = False
+                if same:
+                    return mgpr.device_gp(), i
+        return self._own_device_gp(), 0
+
+    def _own_device_gp(self):
+        key = self._own_key()
+        cached = getattr(self, "_own_gp", None)
+        if cached is None or cached[0] != key:
+            gp = self._own_factorize()
+            if int(gp.info.max().item()):
+                raise RuntimeError("Cholesky decomposition was not successful (matrix not positive definite)")
+            self._own_gp = (key, gp)
+        return self._own_gp[1]
+
+    def _predict_device(self, Xnew, full_cov, full_output_cov):
+        if full_output_cov:
+            raise NotImplementedError("full_output_cov: a GPRModel has a single output")
+        gp, e = self._predict_source()
+        return engine.gp_predict(gp, Xnew, e0=e, ne=1, full_cov=full_cov)
+
+    def predict_f(self, Xnew, full_cov=False, full_output_cov=False):
+        """Latent posterior at Xnew [T,D]: mean [T,1] and variance [T,1] ([1,T,T] with ``full_cov``)."""
+        mean, var = self._predict_device(Xnew, full_cov, full_output_cov)
+        return host(mean), host(var)
+
+    def predict_y(self, Xnew, full_cov=False, full_output_cov=False):
+        """Predictive of the observations: predict_f's mean and variance + the likelihood variance."""
+        if full_cov:
+            raise NotImplementedError("predict_y with full_cov=True: add the likelihood variance to predict_f's diagonal")
+        mean, var = self._predict_device(Xnew, False, full_output_cov)
+        return host(mean), host(var + float(self.likelihood.variance))
+
+    def predict_log_density(self, data, full_cov=False, full_output_cov=False):
+        """log N(Y | mean, var_f + sn2) at each row of data = (X [T,D], Y [T,1]) -> [T]."""
+        if full_cov:
+            raise NotImplementedError("predict_log_density with full_cov=True")
+        mean, var = self._predict_device(data[0], False, full_output_cov)
+        Y = engine.dev(data[1]).reshape(mean.shape)
+        vy = var + float(self.likelihood.variance)
+        return host((-0.5 * (np.log(2.0 * np.pi) + torch.log(vy) + (Y - mean) ** 2 / vy)).sum(-1))
+
 
 def randomize(model, mean=1, sigma=0.01):
     """pilco/models/mgpr.py:8-15"""
@@ -94,6 +163,7 @@ class MGPR:
             kern.lengthscales.prior = (1.1, 1.0 / 10.0)        # Gamma(alpha, rate)   mgpr.py:33
             kern.variance.prior = (1.5, 1.0 / 2.0)             # mgpr.py:34
             self.models.append(GPRModel((data[0], data[1][:, i:i + 1]), kern))
+            self.models[-1]._owner = (self, i)              # predict_f uses this MGPR's factorisation
 
     def set_data(self, data):
         for i, model in enumerate(self.models):

@@ -31,6 +31,20 @@ class GPRFITCModel(GPRModel):
         ell, sf2, sn2, Z = vals
         return gp_training.fitc_loss(X, y, Z, ell, sf2, sn2)
 
+    # predict_f / predict_y / predict_log_density (GPRModel) over this model's OWN inducing inputs, as
+    # gpflow.models.GPRFITC.predict_f does; the moment match of SMGPR uses output 0's (smgpr.py:50-52)
+    def _own_key(self):
+        return hash((GPRModel._own_key(self), np.ascontiguousarray(np.asarray(self.inducing_variable.Z, dtype=np.float64)).tobytes()))
+
+    def _own_factorize(self):
+        ell, sf2, sn2 = self._hypers()
+        return engine.fitc_factorize(np.asarray(self.data[0]), np.asarray(self.inducing_variable.Z, dtype=np.float64),
+                                     np.asarray(self.data[1]).reshape(-1, 1), ell, sf2, sn2)
+
+    def _predict_source(self):
+        engine.device()
+        return self._own_device_gp(), 0
+
 
 class SMGPR(MGPR):
     def __init__(self, data, num_induced_points, name=None):
