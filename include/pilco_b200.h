@@ -291,6 +291,36 @@ typedef struct pilco_rollout_grad {
 size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro);
 int    pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream);
 
+/* ---- particle rollout -------------------------------------------------------------------------
+ * Monte Carlo check of the moment-matching cascade (nothing in the reference; the PILCO papers validate moment
+ * matching against particle rollouts of the same model).  P particles follow the Markov chain whose Gaussian
+ * marginals pilco_rollout_forward approximates, with the caller's standard normals eps:
+ *   u_t = pi(x_t)  (linear: W x + b; RBF: sum_i beta_i k(x, c_i), the mean action at a point), squashed as
+ *         squash_sin does at the policy's output variance (0 linear, 1e-6 RBF, as compute_action),
+ *   x_{t+1} = x_t + mu(x~_t) + sqrt(max(var(x~_t), 0)) o eps_t,  x~_t = [x_t, u_t]  (latent posterior, no noise),
+ *   step_reward / step_risk = the ADD / MULT terms at the point x_t (t < H), ret = sum_t step_reward
+ *   (+ mult_mu (1 - prod_t (1 - step_risk)) with MULT terms).
+ * H+1 step launches and H pilco_gp_predict calls on `stream`; every argument, the predict step's included, is
+ * validated before anything is enqueued.  A particle's outputs do not depend on P or on its row.
+ * PILCO_ERR_UNSUPPORTED: dyn not an unbatched mode-0 model with iK, a batched policy, an RBF policy not in mode 1,
+ * unknown kinds or channels. */
+typedef struct pilco_particles {
+    int P, H;
+    pilco_gp_model dyn;             /* mode 0 with iK, unbatched; D = Ds+U, E = Ds */
+    pilco_policy   pol;             /* unbatched: every *_bs of the policy is 0 */
+    int n_rewards; pilco_reward_term rewards[8]; double mult_mu;
+    const double* x0;               /* [P,Ds]   initial particles (the caller samples them) */
+    const double* eps;              /* [P,H,Ds] standard normals (the caller draws them) */
+    double* traj;                   /* [P,H+1,Ds] */
+    double* act;                    /* [P,H,U]  squashed actions */
+    double* step_reward;            /* [P,H]    additive channel */
+    double* step_risk;              /* [P,H]    MULT channel (zeros without MULT terms) */
+    double* ret;                    /* [P] */
+    void* ws; size_t ws_bytes;
+} pilco_particles;
+size_t pilco_particles_workspace_bytes(const pilco_particles* pr);   /* 0: unsupported sizes */
+int    pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

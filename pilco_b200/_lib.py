@@ -54,6 +54,16 @@ class RolloutGrad(C.Structure):
                 ("gm0", c_dp), ("gS0", c_dp), ("ws", c_dp), ("ws_bytes", C.c_size_t)]
 
 
+class Particles(C.Structure):
+    """mirror of ``pilco_particles``"""
+    _fields_ = [("P", C.c_int), ("H", C.c_int),
+                ("dyn", GpModel), ("pol", Policy),
+                ("n_rewards", C.c_int), ("rewards", RewardTerm * 8), ("mult_mu", C.c_double),
+                ("x0", c_dp), ("eps", c_dp),
+                ("traj", c_dp), ("act", c_dp), ("step_reward", c_dp), ("step_risk", c_dp), ("ret", c_dp),
+                ("ws", c_dp), ("ws_bytes", C.c_size_t)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 CHANNEL_ADD, CHANNEL_MULT = 0, 1
@@ -100,6 +110,8 @@ SIGNATURES = {
     "pilco_mm_backward": (C.c_int, [C.POINTER(GpModel), C.c_int] + [c_dp] * 11 + [c_dp, C.c_size_t, c_dp]),
     "pilco_rollout_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout)]),
     "pilco_rollout_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(RolloutGrad), c_dp]),
+    "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
+    "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),
     "pilco_mm_forward_taped_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,

@@ -56,3 +56,16 @@ RISK_HD double risk_box_eval(int Ds, const double* prm, const double* m, const d
     }
     return inside ? val : 1.0 - val;
 }
+
+// the same box at a point x (risk_box_eval as s -> 0, used by the particle rollout): the indicator that every
+// constrained dimension lies strictly inside (low_k, high_k), complemented when inside = 0
+RISK_HD double risk_box_point(const double* prm, const double* x) {
+    const int nd = (int)prm[0];
+    const bool inside = prm[1] != 0.0;
+    bool in = true;
+    for (int k = 0; k < nd; ++k) {
+        const double v = x[(int)prm[3 + 3 * k]];
+        in = in && prm[4 + 3 * k] < v && v < prm[5 + 3 * k];
+    }
+    return (in == inside) ? 1.0 : 0.0;
+}

@@ -493,6 +493,94 @@ class RolloutPlan:
         return self.gbuf
 
 
+class ParticlePlan:
+    """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
+
+    ``x0`` [P,Ds] and ``eps`` [P,H,Ds] are static device buffers: fill them (``set_inputs``) and ``launch()``, or
+    capture ``launch()`` in a CUDA graph.  Policy and reward terms as for ``RolloutPlan``; the policy must be unbatched."""
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0):
+        d = device()
+        self.P, self.H = int(P), int(H)
+        self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
+        P, H, Ds, U = self.P, self.H, self.Ds, self.U
+        if P < 1 or H < 0:
+            raise ValueError("particles: needs P >= 1 and H >= 0 (P=%d, H=%d)" % (P, H))
+        self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
+        pr = _lib.Particles()
+        pr.P, pr.H = P, H
+        pr.dyn = dyn.struct()
+        pol = pr.pol
+        pol.kind = policy_spec["kind"]
+        pol.Ds, pol.U = Ds, U
+        pol.squash = 1 if policy_spec.get("squash", True) else 0
+        self.max_action = dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(),
+                                              (U,)).copy())
+        pol.max_action = self.max_action.data_ptr()
+        if pol.kind == _lib.POLICY_LINEAR:
+            self.W, self.b = dev(policy_spec["W"]), dev(policy_spec["b"])
+            if self.W.numel() != U * Ds or self.b.numel() != U:
+                raise ValueError("particles: the policy must be unbatched (W [U,Ds], b [U])")
+            pol.W, pol.b = self.W.data_ptr(), self.b.data_ptr()
+        else:
+            self.rbf = policy_spec["gp"]
+            if self.rbf.batched:
+                raise ValueError("particles: the policy must be unbatched")
+            pol.rbf = self.rbf.struct()
+        self.rw = []
+        pr.n_rewards = len(reward_terms)
+        for k, rt in enumerate(reward_terms):
+            W = dev(rt["W"]); t = dev(rt["t"]) if rt.get("t") is not None else None
+            self.rw.append((W, t))
+            pr.rewards[k].kind = rt["kind"]
+            pr.rewards[k].channel = int(rt.get("channel", _lib.CHANNEL_ADD))
+            pr.rewards[k].coef = float(rt.get("coef", 1.0))
+            pr.rewards[k].W = W.data_ptr()
+            pr.rewards[k].t = t.data_ptr() if t is not None else None
+        pr.mult_mu = float(mult_mu)
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
+        Hb = max(H, 1)                                          # H = 0: every buffer still has an address
+        self.x0, self.eps_buf = mk(P, Ds), mk(P, Hb, Ds)
+        self.traj, self.act_buf = mk(P, H + 1, Ds), mk(P, Hb, U)
+        self.rew_buf, self.risk_buf, self.ret = mk(P, Hb), mk(P, Hb), mk(P)
+        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
+        pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
+        pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
+        wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
+        if wsb == 0:
+            raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+        self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+        pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        self.pr = pr
+
+    def set_inputs(self, x0, eps):
+        self.x0.copy_(dev(x0).reshape(self.P, self.Ds))
+        if self.H > 0:
+            self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
+
+    def launch(self):
+        check(lib.pilco_particles_rollout(C.byref(self.pr), stream_ptr()), "particles_rollout")
+
+    def outputs(self):
+        """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views)"""
+        H = self.H
+        return self.traj, self.act_buf[:, :H], self.rew_buf[:, :H], self.risk_buf[:, :H], self.ret
+
+
+def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0):
+    """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
+    factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
+    step_risk [P,H], ret [P]) device tensors."""
+    x0, eps = dev(x0), dev(eps)
+    if x0.dim() != 2 or eps.dim() != 3 or eps.shape[0] != x0.shape[0] or eps.shape[2] != x0.shape[1]:
+        raise ValueError("particles_rollout: x0 must be [P,Ds] and eps [P,H,Ds], got %s and %s"
+                         % (tuple(x0.shape), tuple(eps.shape)))
+    plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu)
+    plan.set_inputs(x0, eps)
+    plan.launch()
+    return plan.outputs()
+
+
 class PredictPlan:
     """``PILCO.predict(m, S, n)`` as ONE graph launch: host moments -> device, n-step cascade (R = 1), final
     moments + reward + status -> pinned host memory.  Built once per (model, policy, reward, n) state by

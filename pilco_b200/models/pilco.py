@@ -4,6 +4,7 @@ The H-step moment-matching cascade (``predict``/``propagate``, pilco.py:118-153)
 objective with its gradient run on the device through ``pilco_rollout_*``; policy optimisation batches
 the random restarts (pilco.py:98-107) in one device rollout and shards them across ranks
 (``pilco_b200.policy_opt``)."""
+import collections
 import time
 
 import numpy as np
@@ -13,6 +14,22 @@ from .. import controllers, rewards, engine, _lib
 from ..params import host, set_trainable
 from .mgpr import MGPR
 from .smgpr import SMGPR
+
+ParticleTrajectories = collections.namedtuple("ParticleTrajectories", ["states", "actions", "rewards", "risks", "returns"])
+
+
+def _sqrt_factor(S):
+    """F with F F' = S: the Cholesky factor, or for a positive semi-definite S (S = 0 included) the eigen-factor
+    Q diag(sqrt(max(lambda, 0))).  ValueError when S has an eigenvalue below -1e-12 max|lambda|."""
+    import torch
+    St = torch.as_tensor(S, dtype=torch.float64)
+    L, info = torch.linalg.cholesky_ex(St)
+    if int(info) == 0:
+        return L.numpy()
+    lam, Q = torch.linalg.eigh(St)
+    if float(lam.min()) < -1e-12 * float(lam.abs().max()):
+        raise ValueError("sample_trajectories: s_x is not positive semi-definite (smallest eigenvalue %.3e)" % float(lam.min()))
+    return (Q * lam.clamp(min=0.0).sqrt()[None, :]).numpy()
 
 
 class PILCO:
@@ -113,6 +130,41 @@ class PILCO:
         """one step (pilco.py:138-153) -> (M_x [1,Ds], S_x [Ds,Ds])"""
         M, S, _ = self.predict(m_x, s_x, 1)
         return M, S
+
+    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None):
+        """Monte Carlo rollouts of the learnt dynamics under the policy, to check what ``predict``'s moment matching
+        approximates: ``num_samples`` particles start at x0 ~ N(m_x, s_x) and take n steps of
+        x_{t+1} = x_t + mu(x_t, u_t) + sqrt(var(x_t, u_t)) eps_t with the latent GP posterior mean and variance,
+        u_t = compute_action(x_t).  Rewards are the reward terms at the particle's state (the expectation of
+        ``predict``'s reward is their mean).  Every draw comes from one device ``torch.Generator``; with
+        ``seed=None`` its seed is drawn from ``np.random``.  s_x may be singular (a known start state: s_x = 0).
+
+        -> ParticleTrajectories(states [S,n+1,Ds], actions [S,n,U], rewards [S,n], risks [S,n], returns [S]) of
+        host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
+        returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
+        import torch
+        from ..params import HostArray
+        n, S = int(n), int(num_samples)
+        if n < 0 or S < 1:
+            raise ValueError("sample_trajectories: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (n, S))
+        dyn = self.mgpr.device_gp()
+        Ds = self.state_dim
+        m = np.asarray(m_x, dtype=np.float64).reshape(Ds)
+        F = _sqrt_factor(np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds))
+        d = engine.device()
+        if seed is None:
+            seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+        g = torch.Generator(device=d)
+        g.manual_seed(int(seed))
+        terms, mult_mu = self.reward_spec()
+        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, S, n, mult_mu=mult_mu)
+        eps0 = torch.randn((S, Ds), dtype=engine.F64, device=d, generator=g)
+        plan.x0.copy_(engine.dev(m)[None] + eps0 @ engine.dev(F).T)
+        if n > 0:
+            plan.eps_buf.copy_(torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g))
+        plan.launch()
+        out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
+        return ParticleTrajectories(*out)
 
     def training_loss(self):
         return -self.predict(self.m_init, self.S_init, self.horizon)[2]
