@@ -178,6 +178,17 @@ int    pilco_gp_predict(const pilco_gp_model* gp, int e0, int ne, int T,
                         double* mean,          /* [T,ne] */
                         double* var,           /* full_cov ? [ne,T,T] : [T,ne] */
                         int full_cov, void* ws, size_t ws_bytes, pilco_stream_t stream);
+/* Vector-Jacobian product of the diagonal posterior of ALL E outputs at the inputs:
+ *   gXs[t] = d/dXs[t] sum_e (gmean[t,e] mean_e(Xs[t]) + gvar[t,e] var_e(Xs[t]))
+ * over the same models and with the same validation and limits as pilco_gp_predict (full_cov = 0).  A point's result
+ * does not depend on T or on its row in Xs (fixed-order reductions). */
+size_t pilco_gp_predict_vjp_workspace_bytes(int n, int D, int E, int T);             /* 0: unsupported arguments */
+int    pilco_gp_predict_vjp(const pilco_gp_model* gp, int T,
+                            const double* Xs,      /* [T,D] */
+                            const double* gmean,   /* [T,E] */
+                            const double* gvar,    /* [T,E] */
+                            double* gXs,           /* [T,D] */
+                            void* ws, size_t ws_bytes, pilco_stream_t stream);
 
 /* ---- closed-form moments ---------------------------------------------------------------------
  * squash_sin (pilco/controllers.py:13-36; gSin.m:33-48), LinearController.compute_action
@@ -320,6 +331,25 @@ typedef struct pilco_particles {
 } pilco_particles;
 size_t pilco_particles_workspace_bytes(const pilco_particles* pr);   /* 0: unsupported sizes */
 int    pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream);
+
+/* Pathwise (reparameterisation) gradient of the particle return: runs the particle rollout of `pr` (its outputs are
+ * bitwise those of pilco_particles_rollout; pr->ws is not used, g->ws holds every buffer) and then a reverse sweep
+ * with x0 and eps held fixed.  value[0] = (1/P) sum_p ret_p and the gradient of value w.r.t. the policy parameters:
+ * linear gW [U,Ds], gb [U]; RBF gXc [bf,Ds] centres, gYc [bf,U] targets, gell [U,Ds] lengthscales (constrained),
+ * through beta = (K + sn2 I)^-1 Yc with pol_L = the Cholesky factors pilco_gp_factorize leaves (as
+ * pilco_rollout_grad).  Box terms are flat almost everywhere: they enter value but not the gradient, so for them the
+ * estimator is biased as an estimate of d E[return].  Where a predicted variance is close to 0 the derivative of its
+ * square root is large (exact, not clamped); where it is <= 0 it is taken as 0.  Every argument, the forward's
+ * included, is validated before anything is enqueued; no host synchronisation (graph-capturable). */
+typedef struct pilco_particles_grad {
+    double* gW; double* gb;                             /* linear policy */
+    double* gXc; double* gYc; double* gell;             /* RBF policy */
+    const double* pol_L;
+    double* value;                                      /* [1] */
+    void* ws; size_t ws_bytes;
+} pilco_particles_grad;
+size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr);  /* 0: unsupported sizes */
+int    pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,

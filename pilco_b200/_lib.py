@@ -64,6 +64,12 @@ class Particles(C.Structure):
                 ("ws", c_dp), ("ws_bytes", C.c_size_t)]
 
 
+class ParticlesGrad(C.Structure):
+    """mirror of ``pilco_particles_grad``"""
+    _fields_ = [("gW", c_dp), ("gb", c_dp), ("gXc", c_dp), ("gYc", c_dp), ("gell", c_dp), ("pol_L", c_dp),
+                ("value", c_dp), ("ws", c_dp), ("ws_bytes", C.c_size_t)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 CHANNEL_ADD, CHANNEL_MULT = 0, 1
@@ -112,6 +118,10 @@ SIGNATURES = {
     "pilco_rollout_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(RolloutGrad), c_dp]),
     "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
     "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
+    "pilco_gp_predict_vjp_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "pilco_gp_predict_vjp": (C.c_int, [C.POINTER(GpModel), C.c_int] + [c_dp] * 5 + [C.c_size_t, c_dp]),
+    "pilco_particles_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
+    "pilco_particles_rollout_grad": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesGrad), c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),
     "pilco_mm_forward_taped_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,

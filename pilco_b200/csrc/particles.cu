@@ -137,6 +137,255 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     }
 }
 
+// ---- reverse sweep of pilco_particles_rollout_grad (DESIGN.md section 12) ---------------------------------------------
+// Per particle, x_bar_H = 0 and t = H-1 .. 0 (s_t = sqrt(max(var_t, 0)), z_t the pre-squash action):
+//   mu_bar_t = x_bar_{t+1},  var_bar_t = x_bar_{t+1} o eps_t / (2 s_t) where var_t > 0, else 0
+//   x~_bar_t = pilco_gp_predict_vjp at x~_t;  z_bar_t = x~_bar_t[Ds:] o maxa e^{-su/2} cos(z_t)  (when squashed)
+//   x_bar_t  = x_bar_{t+1} + x~_bar_t[:Ds] + (d pi / dx)' z_bar_t + sum_k a_kt grad v_k(x_t)
+// a_kt = coef_k (ADD) or coef_k mult_mu prod_{s != t} (1 - risk_s) (MULT).  x_H carries no reward, so the sweep
+// starts at t = H-1 with x_bar_H = 0 and x~_bar_{H-1} = 0: H-1 VJP calls.
+struct PgDev {
+    int P, H, Ds, U, t;
+    int pol_kind, squash;
+    const double* maxa;
+    const double* W; const double* b;
+    const double* C; const double* ell; const double* sf2; const double* beta; int bf;
+    int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
+    const double* eps; const double* traj; const double* step_risk;
+    const double* gxt;          // VJP of step t at x~_t [P,D]; NULL at t = H-1
+    const double* var_prev;     // var_{t-1} [P,Ds] (t > 0)
+    double* gx;                 // [P,Ds] x_bar_{t+1} in, x_bar_t out (= the gmean of step t-1's VJP)
+    double* gvar;               // [P,Ds] the gvar of step t-1's VJP
+    double* zbar;               // [P,H,U]
+};
+
+// grid ceil(P / 128), one thread per particle: step t of the reverse sweep
+__global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
+    PDL_ENTRY();
+    const int p = blockIdx.x * PT_THREADS + threadIdx.x;
+    if (p >= a.P) return;
+    const int Ds = a.Ds, U = a.U, t = a.t, H = a.H;
+    const double* xg = a.traj + ((size_t)p * (H + 1) + t) * Ds;
+    const double* gxt = a.gxt ? a.gxt + (size_t)p * (Ds + U) : nullptr;
+    double x[MAXD], xb[MAXD];
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) {
+        x[d] = d < Ds ? xg[d] : 0.0;
+        xb[d] = (d < Ds && gxt) ? a.gx[(size_t)p * Ds + d] + gxt[d] : 0.0;
+    }
+    // reward terms at x_t (box: flat almost everywhere, no gradient)
+    double wmult = 0.0;
+    if (a.n_mult > 0) {                                 // mult_mu prod_{s != t} (1 - risk_s): prefix x suffix, no division
+        const double* rk = a.step_risk + (size_t)p * H;
+        double pre = 1.0, suf = 1.0;
+        for (int s = 0; s < t; ++s) pre *= 1.0 - rk[s];
+        for (int s = t + 1; s < H; ++s) suf *= 1.0 - rk[s];
+        wmult = a.mult_mu * (pre * suf);
+    }
+    for (int k = 0; k < a.n_rewards; ++k) {
+        const pilco_reward_term& rt = a.rewards[k];
+        if (rt.kind == PILCO_REWARD_BOX) continue;
+        const double w = rt.channel == PILCO_CHANNEL_MULT ? rt.coef * wmult : rt.coef;
+        if (rt.kind == PILCO_REWARD_LINEAR) {
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(w, rt.W[d], xb[d]);
+            continue;
+        }
+        // exp(-0.5 v' W v), v = x - t:  gradient -value (W + W') v / 2
+        double v[MAXD], gv[MAXD];
+#pragma unroll
+        for (int i = 0; i < MAXD; ++i) v[i] = i < Ds ? x[i] - rt.t[i] : 0.0;
+        double quad = 0.0;
+#pragma unroll
+        for (int i = 0; i < MAXD; ++i) {
+            gv[i] = 0.0;
+            if (i < Ds) {
+                double wy = 0.0, wty = 0.0;
+#pragma unroll
+                for (int k2 = 0; k2 < MAXD; ++k2)
+                    if (k2 < Ds) { wy = fma(rt.W[i * Ds + k2], v[k2], wy); wty = fma(rt.W[k2 * Ds + i], v[k2], wty); }
+                quad = fma(v[i], wy, quad);
+                gv[i] = wy + wty;
+            }
+        }
+        const double f = -0.5 * w * exp(-0.5 * quad);
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(f, gv[d], xb[d]);
+    }
+    // policy: z_bar_t and (d pi / dx)' z_bar_t; z_t recomputed in the forward's order
+    double* zb = a.zbar + ((size_t)p * H + t) * U;
+    const double su = a.pol_kind == PILCO_POLICY_RBF ? PT_RBF_VAR : 0.0;
+    for (int j = 0; j < U; ++j) {
+        if (!gxt) { zb[j] = 0.0; continue; }
+        double jx[MAXD], z;
+        if (a.pol_kind == PILCO_POLICY_LINEAR) {
+            z = a.b[j];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) {
+                jx[d] = d < Ds ? a.W[j * Ds + d] : 0.0;
+                if (d < Ds) z = fma(a.W[j * Ds + d], x[d], z);
+            }
+        } else {                                        // d z_j / dx = sum_i beta_ji k_ji (c_i - x) / ell_j^2
+            double il[MAXD];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) { il[d] = d < Ds ? 1.0 / a.ell[j * Ds + d] : 0.0; jx[d] = 0.0; }
+            const double sf2 = a.sf2[j];
+            const double* be = a.beta + (size_t)j * a.bf;
+            z = 0.0;
+            for (int i = 0; i < a.bf; ++i) {
+                const double* c = a.C + (size_t)i * Ds;
+                double d2 = 0.0;
+#pragma unroll
+                for (int d = 0; d < MAXD; ++d) if (d < Ds) { const double q = (x[d] - c[d]) * il[d]; d2 = fma(q, q, d2); }
+                const double kb = sf2 * exp(-0.5 * d2);
+                z = fma(kb, be[i], z);
+                const double f = kb * be[i];
+#pragma unroll
+                for (int d = 0; d < MAXD; ++d) if (d < Ds) jx[d] = fma(f, (c[d] - x[d]) * (il[d] * il[d]), jx[d]);
+            }
+        }
+        double zbj = gxt[Ds + j];
+        // cos(z) as cospi(z / pi): no Payne-Hanek slow path (and its local-memory table), as the forward's sinpi
+        if (a.squash) zbj *= a.maxa[j] * exp(-0.5 * su) * cospi(z * PT_INV_PI);
+        zb[j] = zbj;
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(zbj, jx[d], xb[d]);
+    }
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) if (d < Ds) a.gx[(size_t)p * Ds + d] = xb[d];
+    if (t > 0) {                                        // cotangents of step t-1's predict outputs
+        const double* vp = a.var_prev + (size_t)p * Ds;
+        const double* ep = a.eps + ((size_t)p * H + (t - 1)) * Ds;
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) {
+            if (d < Ds) {
+                const double v = vp[d];
+                a.gvar[(size_t)p * Ds + d] = v > 0.0 ? xb[d] * ep[d] / (2.0 * sqrt(v)) : 0.0;
+            }
+        }
+    }
+}
+
+// fixed-order block sum of NV values per thread (256 threads): warp butterflies, then warps in order -> out[0..NV)
+template <int NV>
+__device__ __forceinline__ void pg_block_sum(double (&v)[NV], double* red, double* out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+        const double s = warp_sum(v[c]);
+        if (lane == 0) red[c * 8 + warp] = s;
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < NV; c += 256) {
+        double s = 0.0;
+        for (int w = 0; w < 8; ++w) s += red[c * 8 + w];
+        out[c] = s;
+    }
+    __syncthreads();
+}
+
+struct PgRed {
+    int P, H, Ds, U, bf, pol_kind;
+    const double* traj; const double* zbar; const double* ret;
+    const double* C; const double* ell; const double* sf2; const double* beta;
+    double* gW; double* gb;                             // linear
+    double* s1; double* s2; double* gbeta;              // RBF per (output j, centre i): [U,bf,Ds], [U,bf,Ds], [U,bf]
+    double* gXc; double* gell;                          // RBF direct terms (pg_rbf_finish_kernel)
+    double* value;
+};
+
+// The policy-parameter gradient over all P H points (x_t, z_bar_t) and the value, each CTA one fixed-order sum:
+// grid (linear: U, RBF: U bf) + 1, 256 threads; thread q takes the points q, q + 256, ... in order.
+//   linear j:    gW[j] = sum z_bar_j x / P,  gb[j] = sum z_bar_j / P
+//   RBF (j, i):  a = z_bar_j beta_ji k_ji:  s1 = sum a (x - c_i),  s2 = sum a (x - c_i)^2,  gbeta_ji = sum z_bar_j k_ji / P
+__global__ void __launch_bounds__(256) pg_param_kernel(PgRed a) {
+    PDL_ENTRY();
+    __shared__ double red[(2 * MAXD + 1) * 8], out[2 * MAXD + 1];
+    const int Ds = a.Ds, U = a.U, H = a.H, tid = threadIdx.x;
+    const size_t npts = (size_t)a.P * H;
+    const int nblk = a.pol_kind == PILCO_POLICY_LINEAR ? U : U * a.bf;
+    const double invP = 1.0 / a.P;
+    if ((int)blockIdx.x == nblk) {                      // value = mean return
+        double v[1] = {0.0};
+        for (int p = tid; p < a.P; p += 256) v[0] += a.ret[p];
+        pg_block_sum<1>(v, red, out);
+        if (tid == 0) a.value[0] = out[0] * invP;
+        return;
+    }
+    if (a.pol_kind == PILCO_POLICY_LINEAR) {
+        const int j = blockIdx.x;
+        double v[MAXD + 1];
+#pragma unroll
+        for (int d = 0; d <= MAXD; ++d) v[d] = 0.0;
+        for (size_t q = tid; q < npts; q += 256) {
+            const size_t p = q / H, t = q % H;
+            const double* x = a.traj + (p * (H + 1) + t) * Ds;
+            const double zb = a.zbar[q * U + j];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < Ds) v[d] = fma(zb, x[d], v[d]);
+            v[MAXD] += zb;
+        }
+        pg_block_sum<MAXD + 1>(v, red, out);
+        if (tid < Ds) a.gW[j * Ds + tid] = out[tid] * invP;
+        if (tid == 0) a.gb[j] = out[MAXD] * invP;
+        return;
+    }
+    const int j = blockIdx.x / a.bf, i = blockIdx.x % a.bf;
+    double c[MAXD], il[MAXD], v[2 * MAXD + 1];
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) {
+        c[d] = d < Ds ? a.C[(size_t)i * Ds + d] : 0.0;
+        il[d] = d < Ds ? 1.0 / a.ell[j * Ds + d] : 0.0;
+    }
+#pragma unroll
+    for (int k = 0; k <= 2 * MAXD; ++k) v[k] = 0.0;
+    const double sf2 = a.sf2[j], bji = a.beta[(size_t)j * a.bf + i];
+    for (size_t q = tid; q < npts; q += 256) {
+        const size_t p = q / H, t = q % H;
+        const double* x = a.traj + (p * (H + 1) + t) * Ds;
+        const double zb = a.zbar[q * U + j];
+        double df[MAXD], d2 = 0.0;
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) {
+            df[d] = d < Ds ? x[d] - c[d] : 0.0;
+            const double s = df[d] * il[d];
+            d2 = fma(s, s, d2);
+        }
+        const double k = sf2 * exp(-0.5 * d2), w = zb * bji * k;
+        v[2 * MAXD] = fma(zb, k, v[2 * MAXD]);
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) { v[d] = fma(w, df[d], v[d]); v[MAXD + d] = fma(w * df[d], df[d], v[MAXD + d]); }
+    }
+    pg_block_sum<2 * MAXD + 1>(v, red, out);
+    const size_t ji = (size_t)j * a.bf + i;
+    if (tid < Ds) { a.s1[ji * Ds + tid] = out[tid]; a.s2[ji * Ds + tid] = out[MAXD + tid]; }
+    if (tid == 0) a.gbeta[ji] = out[2 * MAXD] * invP;
+}
+
+// direct RBF gradients from the per-(j, i) sums, in fixed order:
+//   gXc[i,d] = sum_j s1[j,i,d] / ell_jd^2 / P,   gell[j,d] = sum_i s2[j,i,d] / ell_jd^3 / P
+__global__ void __launch_bounds__(128) pg_rbf_finish_kernel(PgRed a) {
+    PDL_ENTRY();
+    const int Ds = a.Ds, U = a.U, bf = a.bf;
+    const double invP = 1.0 / a.P;
+    for (int q = threadIdx.x; q < bf * Ds; q += 128) {
+        const int i = q / Ds, d = q % Ds;
+        double s = 0.0;
+        for (int j = 0; j < U; ++j) {
+            const double l = a.ell[j * Ds + d];
+            s += a.s1[((size_t)j * bf + i) * Ds + d] / (l * l);
+        }
+        a.gXc[q] = s * invP;
+    }
+    for (int q = threadIdx.x; q < U * Ds; q += 128) {
+        const int j = q / Ds, d = q % Ds;
+        double s = 0.0;
+        for (int i = 0; i < bf; ++i) s += a.s2[((size_t)j * bf + i) * Ds + d];
+        const double l = a.ell[q];
+        a.gell[q] = s / (l * l * l) * invP;
+    }
+}
+
 struct PtWs { size_t xt, mean, var, pws, pws_bytes, total; };     // offsets in doubles; total and pws_bytes in bytes
 
 static PtWs pt_ws_layout(const pilco_particles* pr) {
@@ -155,7 +404,8 @@ static bool pt_sizes_ok(const pilco_particles* pr) {
            pr->pol.Ds >= 1 && pr->pol.U >= 1 && pr->pol.Ds <= MAXE;
 }
 
-static int pt_check(const pilco_particles* pr) {
+// everything but the workspace (pilco_particles_rollout_grad brings its own)
+static int pt_check_desc(const pilco_particles* pr) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
     const pilco_gp_model& g = pr->dyn;
@@ -183,14 +433,65 @@ static int pt_check(const pilco_particles* pr) {
         if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
         if (rt.kind == PILCO_REWARD_EXP && !rt.t) return PILCO_ERR_NULL;
     }
-    if (!pr->x0 || !pr->eps || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret || !pr->ws)
+    if (!pr->x0 || !pr->eps || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret)
         return PILCO_ERR_NULL;
-    if (((uintptr_t)g.iK & 15) || (g.ldk & 1) || ((uintptr_t)pr->ws & 15)) return PILCO_ERR_ALIGN;   // predict's TMA rows
+    if (((uintptr_t)g.iK & 15) || (g.ldk & 1)) return PILCO_ERR_ALIGN;                  // predict's TMA rows
+    return PILCO_OK;
+}
+
+static int pt_check(const pilco_particles* pr) {
+    const int rc = pt_check_desc(pr);
+    if (rc) return rc;
+    if (!pr->ws) return PILCO_ERR_NULL;
+    if ((uintptr_t)pr->ws & 15) return PILCO_ERR_ALIGN;
     const PtWs L = pt_ws_layout(pr);
     if (L.pws_bytes == 0) return PILCO_ERR_DIM;
     if (pr->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
     return PILCO_OK;
 }
+
+static PtDev pt_dev(const pilco_particles* pr) {
+    const pilco_policy& pol = pr->pol;
+    PtDev a;
+    a.P = pr->P; a.H = pr->H; a.Ds = pol.Ds; a.U = pol.U; a.t = 0;
+    a.pol_kind = pol.kind; a.squash = pol.squash; a.maxa = pol.max_action;
+    a.W = pol.W; a.b = pol.b;
+    a.C = pol.rbf.X; a.ell = pol.rbf.ell; a.sf2 = pol.rbf.sf2; a.beta = pol.rbf.beta; a.bf = pol.rbf.n;
+    a.n_rewards = pr->n_rewards; a.n_mult = 0;
+    for (int k = 0; k < 8; ++k) a.rewards[k] = pr->rewards[k];
+    for (int k = 0; k < pr->n_rewards; ++k) a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
+    a.mult_mu = pr->mult_mu;
+    a.x0 = pr->x0; a.eps = pr->eps;
+    a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
+    return a;
+}
+
+// workspace of pilco_particles_rollout_grad (offsets in doubles; total and pws_bytes in bytes): the forward's predict
+// inputs and variances of EVERY step (the reverse sweep needs them), the state cotangent, the VJP's cotangents and
+// output, z_bar of every point, the RBF sums, and one predict / VJP workspace (never in use at the same time)
+struct PgWs { size_t xt, mean, var, gx, gvar, gxt, zbar, s1, s2, gbeta, gy, pws, pws_bytes, total; };
+
+static PgWs pg_ws_layout(const pilco_particles* pr) {
+    const size_t P = pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+    const size_t bf = pr->pol.kind == PILCO_POLICY_RBF ? pr->pol.rbf.n : 0;
+    PgWs L; size_t o = 0;
+    auto take = [&](size_t len) { const size_t at = o; o += (len + 1) & ~(size_t)1; return at; };
+    L.xt = take(H * P * D); L.mean = take(P * Ds); L.var = take(H * P * Ds);
+    L.gx = take(P * Ds); L.gvar = take(P * Ds); L.gxt = take(P * D); L.zbar = take(P * H * U);
+    L.s1 = take(U * bf * Ds); L.s2 = take(U * bf * Ds); L.gbeta = take(U * bf); L.gy = take(U * bf);
+    L.pws = o;
+    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
+    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, pr->P);
+    L.pws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
+    L.total = o * sizeof(double) + L.pws_bytes;
+    return L;
+}
+
+void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
+                           const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
+int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, const double* ell,
+                          const double* sf2, long long sf2_bs, const double* beta, const double* gy,
+                          double* gX, double* gY, double* gell);
 
 extern "C" {
 
@@ -207,17 +508,7 @@ int pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream) {
     cudaStream_t st = (cudaStream_t)stream;
     double* ws = (double*)pr->ws;
     const pilco_policy& pol = pr->pol;
-    PtDev a;
-    a.P = pr->P; a.H = pr->H; a.Ds = pol.Ds; a.U = pol.U;
-    a.pol_kind = pol.kind; a.squash = pol.squash; a.maxa = pol.max_action;
-    a.W = pol.W; a.b = pol.b;
-    a.C = pol.rbf.X; a.ell = pol.rbf.ell; a.sf2 = pol.rbf.sf2; a.beta = pol.rbf.beta; a.bf = pol.rbf.n;
-    a.n_rewards = pr->n_rewards; a.n_mult = 0;
-    for (int k = 0; k < 8; ++k) a.rewards[k] = pr->rewards[k];
-    for (int k = 0; k < pr->n_rewards; ++k) a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
-    a.mult_mu = pr->mult_mu;
-    a.x0 = pr->x0; a.eps = pr->eps;
-    a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
+    PtDev a = pt_dev(pr);
     a.xt = ws + L.xt; a.mean = ws + L.mean; a.var = ws + L.var;
     const dim3 grid((pr->P + PT_THREADS - 1) / PT_THREADS);
     for (int t = 0; t <= pr->H; ++t) {
@@ -227,6 +518,89 @@ int pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream) {
         if (t == pr->H) break;
         const int rc = pilco_gp_predict(&pr->dyn, 0, pol.Ds, pr->P, ws + L.xt, ws + L.mean, ws + L.var, 0,
                                         ws + L.pws, L.pws_bytes, stream);
+        if (rc) return rc;
+    }
+    return PILCO_OK;
+}
+
+size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr) {
+    if (!pr || !pt_sizes_ok(pr)) return 0;
+    const PgWs L = pg_ws_layout(pr);
+    return L.pws_bytes ? L.total : 0;
+}
+
+int pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream) {
+    int rc = pt_check_desc(pr);
+    if (rc) return rc;
+    if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
+    const pilco_policy& pol = pr->pol;
+    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    if (rbf ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
+    if ((uintptr_t)g->ws & 15) return PILCO_ERR_ALIGN;
+    const PgWs L = pg_ws_layout(pr);
+    if (L.pws_bytes == 0) return PILCO_ERR_DIM;
+    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)g->ws;
+    const int P = pr->P, H = pr->H, Ds = pol.Ds, U = pol.U, D = Ds + U;
+    const size_t PD = (size_t)P * D, PDs = (size_t)P * Ds;
+    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS);
+    // forward: pilco_particles_rollout's launches, with the predict inputs and variances of every step kept
+    PtDev a = pt_dev(pr);
+    a.mean = ws + L.mean;
+    for (int t = 0; t <= H; ++t) {
+        a.t = t;
+        a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * PD;
+        a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * PDs;
+        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        if (t == H) break;
+        rc = pilco_gp_predict(&pr->dyn, 0, Ds, P, a.xt, ws + L.mean, ws + L.var + (size_t)t * PDs, 0,
+                              ws + L.pws, L.pws_bytes, stream);
+        if (rc) return rc;
+    }
+    // reverse sweep
+    PgDev b;
+    b.P = P; b.H = H; b.Ds = Ds; b.U = U;
+    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
+    b.W = pol.W; b.b = pol.b;
+    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
+    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
+    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
+    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
+    b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
+    for (int t = H - 1; t >= 0; --t) {
+        b.t = t;
+        b.gxt = nullptr;
+        if (t < H - 1) {
+            rc = pilco_gp_predict_vjp(&pr->dyn, P, ws + L.xt + (size_t)t * PD, b.gx, b.gvar, ws + L.gxt,
+                                      ws + L.pws, L.pws_bytes, stream);
+            if (rc) return rc;
+            b.gxt = ws + L.gxt;
+        }
+        b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * PDs : nullptr;
+        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
+        CUDA_LAUNCH_CHECK();
+    }
+    // value and the policy-parameter gradient over all P H points, fixed order
+    PgRed r;
+    r.P = P; r.H = H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
+    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
+    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
+    r.gW = g->gW; r.gb = g->gb;
+    r.s1 = ws + L.s1; r.s2 = ws + L.s2; r.gbeta = ws + L.gbeta;
+    r.gXc = g->gXc; r.gell = g->gell;
+    r.value = g->value;
+    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1), dim3(256), 0, st, r);
+    CUDA_LAUNCH_CHECK();
+    if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
+        const int bf = r.bf, ldw = pad64(bf);
+        launch_hi(pg_rbf_finish_kernel, dim3(1), dim3(128), 0, st, r);
+        CUDA_LAUNCH_CHECK();
+        chol_solve_vec_launch(st, U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
+                              ws + L.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
+        rc = rbf_factor_bwd_launch(st, 1, bf, Ds, U, pol.rbf.X, pol.rbf.ell, pol.rbf.sf2, 0, pol.rbf.beta, ws + L.gy,
+                                   g->gXc, g->gYc, g->gell);
         if (rc) return rc;
     }
     return PILCO_OK;

@@ -157,6 +157,174 @@ __global__ void __launch_bounds__(256, 2) gp_predict_kernel(PredictArgs a) {
     }
 }
 
+// ---- VJP of the diagonal posterior at the inputs (pilco_gp_predict_vjp, DESIGN.md section 12) ----------------------
+//   gx = sum_e ell_e^-2 o sum_n c_en (c_n - x),   c_en = k_en (gmean_e beta_en - 2 gvar_e w_en),   w_e = iK_e k_e
+// (d k_en / dx = k_en (c_n - x) / ell_e^2; d var / d k = -2 w since iK is symmetric).  The difference form c_n - x is
+// summed directly: the expanded sum_n c_n c_n - (sum_n c_n) x would cancel when |x| >> |c_n - x|.
+struct VjpArgs {
+    int n, D, np, nj, nrb, T, E;
+    const double* C; const double* ell; const double* sf2; const double* beta;
+    const double* iK; int ldk;
+    const double* Xs;           // [T,D]
+    const double* gmean;        // [T,E]
+    const double* gvar;         // [T,E]
+    double* gXs;                // [T,D]
+    double* part;               // [E, nrb, nj, PR_TR, D] per-(output, j block) sums of c_en (c_n - x)
+    unsigned* cnt;              // [nrb] arrival counters over the nj * E CTAs of a row block (zeroed by the launcher)
+};
+
+struct VjpSmem {
+    double B[2][PR_KC * PR_LDB];        // iK[i chunk, j block] (TMA destination); after the main loop c [PR_TR][PR_LDB]
+    double A[2][PR_TR * PR_LDA];        // K*[rows, i chunk]
+    double x[PR_TR * MAXD];
+    double il[MAXD];
+    double gm[PR_TR], gv[PR_TR];        // the rows' cotangents of output e
+    uint64_t bar[2];
+};
+static_assert(2 * PR_KC >= PR_TR, "c of the CTA's rows x j block fits the iK double buffer");
+
+// grid (nj, nrb, E), 256 threads.  The main loop is gp_predict_kernel's (W = K* iK[:, j block] on DMMA.16x8x16 from
+// TMA-staged iK tiles); only the epilogue differs: c for the CTA's (rows, j block) goes to the free iK buffer, then
+// 8 lanes per row sum c (c_n - x) over the block's columns in a fixed order and the last of the row block's nj * E
+// CTAs applies ell_e^-2 and sums the outputs and j blocks in a fixed order.
+__global__ void __launch_bounds__(256, 2) gp_predict_vjp_kernel(VjpArgs a) {
+    PDL_ENTRY();
+    extern __shared__ __align__(16) unsigned char pr_smem_raw[];
+    VjpSmem& sm = *reinterpret_cast<VjpSmem*>(pr_smem_raw);
+    const int jb = blockIdx.x, rb = blockIdx.y, e = blockIdx.z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int wm = (warp >> 2) * 16, wc = warp & 3, wn = wc * 64;
+    const int D = a.D, r0 = rb * PR_TR, j0 = jb * PR_JB;
+    const int jw = min(PR_JB, a.np - j0);
+    const bool active = wn < jw;
+    const double sf2 = a.sf2[e];
+    const double* iK = a.iK + (size_t)e * a.ldk * a.ldk;
+    for (int i = tid; i < PR_TR * MAXD; i += 256) {
+        const int r = i / MAXD, d = i % MAXD;
+        sm.x[i] = (r0 + r < a.T && d < D) ? a.Xs[(size_t)(r0 + r) * D + d] : 0.0;
+    }
+    if (tid < MAXD) sm.il[tid] = tid < D ? 1.0 / a.ell[(size_t)e * D + tid] : 0.0;
+    if (tid < PR_TR) {
+        const bool in = r0 + tid < a.T;
+        sm.gm[tid] = in ? a.gmean[(size_t)(r0 + tid) * a.E + e] : 0.0;
+        sm.gv[tid] = in ? a.gvar[(size_t)(r0 + tid) * a.E + e] : 0.0;
+    }
+    if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
+    __syncthreads();
+    // main loop: gp_predict_kernel's, kept as its own copy so that the predict kernel's code is not touched
+    const int nc = a.np / PR_KC;
+    auto issue = [&](int c) {
+        uint64_t* bar = &sm.bar[c & 1];
+        mbar_expect_tx(bar, (unsigned)(PR_KC * jw * sizeof(double)));
+        for (int k = 0; k < PR_KC; ++k)
+            tma_bulk_g2s(&sm.B[c & 1][k * PR_LDB], iK + (size_t)(c * PR_KC + k) * a.ldk + j0, (unsigned)(jw * sizeof(double)), bar);
+    };
+    auto kchunk = [&](int c) {
+        double* A = sm.A[c & 1];
+        for (int q = tid; q < PR_TR * PR_KC; q += 256) {
+            const int r = q / PR_KC, k = q % PR_KC, i = c * PR_KC + k;
+            double v = 0.0;
+            if (i < a.n && r0 + r < a.T) v = pr_kstar(&sm.x[r * MAXD], a.C + (size_t)i * D, sm.il, D, sf2);
+            A[r * PR_LDA + k] = v;
+        }
+    };
+    if (tid == 0) { issue(0); if (nc > 1) issue(1); }
+    kchunk(0);
+    double acc[8][4];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.0;
+    for (int c = 0; c < nc; ++c) {
+        __syncthreads();
+        if (tid == 0 && c >= 1 && c + 1 < nc) issue(c + 1);
+        if (c + 1 < nc) kchunk(c + 1);
+        mbar_wait(&sm.bar[c & 1], (unsigned)((c >> 1) & 1));
+        if (active) {
+            const double* A = sm.A[c & 1];
+            const double* B = sm.B[c & 1];
+            double af[8];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                af[2 * i] = A[(wm + g) * PR_LDA + t + 4 * i];
+                af[2 * i + 1] = A[(wm + g + 8) * PR_LDA + t + 4 * i];
+            }
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                double bf[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) bf[i] = B[(t + 4 * i) * PR_LDB + wn + 8 * q + g];
+                dmma16816(acc[q], af, bf);
+            }
+        }
+    }
+    __syncthreads();                                            // every warp is done with the last iK tile
+    double* cs = &sm.B[0][0];                                   // c [PR_TR][PR_LDB]
+    const double* be = a.beta + (size_t)e * a.n;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = wm + g + 8 * h;
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+#pragma unroll
+            for (int o = 0; o < 2; ++o) {
+                const int jl = wn + 8 * q + 2 * t + o, j = j0 + jl;
+                double c = 0.0;
+                if (active && r0 + r < a.T && j < a.n) {
+                    const double k = pr_kstar(&sm.x[r * MAXD], a.C + (size_t)j * D, sm.il, D, sf2);
+                    c = k * fma(-2.0 * sm.gv[r], acc[q][2 * h + o], sm.gm[r] * be[j]);
+                }
+                cs[r * PR_LDB + jl] = c;
+            }
+    }
+    __syncthreads();
+    {                                                           // row r = tid / 8; lane s sums columns s, s + 8, ...
+        const int r = tid >> 3, s = tid & 7;
+        const int jend = min(PR_JB, a.n - j0);
+        const double* xr = &sm.x[r * MAXD];
+        double gs[MAXD];
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) gs[d] = 0.0;
+        for (int jl = s; jl < jend; jl += 8) {
+            const double c = cs[r * PR_LDB + jl];
+            const double* cj = a.C + (size_t)(j0 + jl) * D;
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < D) gs[d] = fma(c, cj[d] - xr[d], gs[d]);
+        }
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) {                        // over the 8 lanes of a row: fixed butterfly
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 1);
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 2);
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 4);
+        }
+        if (s == 0 && r0 + r < a.T) {
+            double* pr = a.part + ((((size_t)e * a.nrb + rb) * a.nj + jb) * PR_TR + r) * D;
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < D) pr[d] = gs[d];
+        }
+    }
+    if (!last_cta_arrives(a.cnt + rb, (unsigned)(a.nj * a.E))) return;
+    for (int q = tid; q < PR_TR * D; q += 256) {                // outputs, then j blocks, in fixed order
+        const int r = q / D, d = q % D;
+        if (r0 + r >= a.T) continue;
+        double sum = 0.0;
+        for (int ee = 0; ee < a.E; ++ee) {
+            const double* pe = a.part + (((size_t)ee * a.nrb + rb) * a.nj * PR_TR + r) * D + d;
+            double se = 0.0;
+            for (int b = 0; b < a.nj; ++b) se += pe[(size_t)b * PR_TR * D];
+            const double il = 1.0 / a.ell[(size_t)ee * D + d];
+            sum = fma(se, il * il, sum);
+        }
+        a.gXs[(size_t)(r0 + r) * D + d] = sum;
+    }
+}
+
+static size_t pr_vjp_bytes(int np, int D, int E, int T) {
+    const size_t nj = (size_t)(np + PR_JB - 1) / PR_JB, nrb = (size_t)(T + PR_TR - 1) / PR_TR;
+    const size_t part = (size_t)E * nrb * nj * PR_TR * D * sizeof(double);
+    const size_t cnt = (nrb * sizeof(unsigned) + 15) & ~(size_t)15;
+    return part + cnt;
+}
+
 // full covariance (factorize.cu): K*, K** (gram_kernel), W = K* iK, K** - W K*' and K* beta (gemm)
 int gp_predict_full_cov(cudaStream_t st, int n, int D, int ne, int T, const double* C, const double* ell, const double* sf2,
                         const double* beta, const double* iK, int ldk, const double* Xs, double* mean, double* cov, double* ws);
@@ -210,6 +378,45 @@ int pilco_gp_predict(const pilco_gp_model* gp, int e0, int ne, int T, const doub
     }
     const dim3 grid(nj, nrb, ne);
     launch_pri(pilco_small_grid(grid), gp_predict_kernel, grid, dim3(256), smem, st, a);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
+size_t pilco_gp_predict_vjp_workspace_bytes(int n, int D, int E, int T) {
+    if (n < 1 || D < 1 || D > MAXD || E < 1 || E > MAXE || T < 1 || T > 65535 * PR_TR) return 0;
+    return pr_vjp_bytes(pad64(n), D, E, T);
+}
+
+int pilco_gp_predict_vjp(const pilco_gp_model* gp, int T, const double* Xs, const double* gmean, const double* gvar,
+                         double* gXs, void* ws, size_t ws_bytes, pilco_stream_t stream) {
+    if (!gp || !Xs || !gmean || !gvar || !gXs || !ws) return PILCO_ERR_NULL;
+    if (!gp->X || !gp->ell || !gp->sf2 || !gp->beta) return PILCO_ERR_NULL;
+    if (gp->mode != 0 || !gp->iK || gp->X_bs || gp->ell_bs || gp->sf2_bs || gp->beta_bs) return PILCO_ERR_UNSUPPORTED;
+    const int n = gp->n, D = gp->D, E = gp->E;
+    if (n < 1 || D < 1 || D > MAXD || E < 1 || E > MAXE) return PILCO_ERR_DIM;
+    if (T < 1 || T > 65535 * PR_TR) return PILCO_ERR_DIM;
+    if (gp->ldk < pad64(n)) return PILCO_ERR_DIM;
+    if (((uintptr_t)gp->iK & 15) || (gp->ldk & 1) || ((uintptr_t)ws & 15)) return PILCO_ERR_ALIGN;
+    if (ws_bytes < pilco_gp_predict_vjp_workspace_bytes(n, D, E, T)) return PILCO_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int np = pad64(n), nj = (np + PR_JB - 1) / PR_JB, nrb = (T + PR_TR - 1) / PR_TR;
+    VjpArgs a;
+    a.n = n; a.D = D; a.np = np; a.nj = nj; a.nrb = nrb; a.T = T; a.E = E;
+    a.C = gp->X; a.ell = gp->ell; a.sf2 = gp->sf2; a.beta = gp->beta; a.iK = gp->iK; a.ldk = gp->ldk;
+    a.Xs = Xs; a.gmean = gmean; a.gvar = gvar; a.gXs = gXs;
+    a.part = (double*)ws;
+    a.cnt = (unsigned*)((char*)ws + (size_t)E * nrb * nj * PR_TR * D * sizeof(double));
+    cudaMemsetAsync(a.cnt, 0, (size_t)nrb * sizeof(unsigned), st);
+    const size_t smem = sizeof(VjpSmem);
+    static bool attr_set[PILCO_MAX_DEVICES] = {false};
+    bool& set = attr_set[pilco_current_device()];
+    if (!set) {
+        if (cudaFuncSetAttribute(gp_predict_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+            return PILCO_ERR_LAUNCH;
+        set = true;
+    }
+    const dim3 grid(nj, nrb, E);
+    launch_pri(pilco_small_grid(grid), gp_predict_vjp_kernel, grid, dim3(256), smem, st, a);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }

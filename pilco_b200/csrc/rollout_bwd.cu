@@ -297,6 +297,15 @@ __global__ void __launch_bounds__(128) rbf_factor_bwd_kernel(int bf, int Ds, int
     }
 }
 
+// rbf_factor_bwd_kernel for callers in other translation units (the particle gradient, particles.cu)
+int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, const double* ell,
+                          const double* sf2, long long sf2_bs, const double* beta, const double* gy,
+                          double* gX, double* gY, double* gell) {
+    launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, X, ell, sf2, sf2_bs, beta, gy, gX, gY, gell);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
 extern "C" {
 
 size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro) {

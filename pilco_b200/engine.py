@@ -497,9 +497,10 @@ class ParticlePlan:
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
 
     ``x0`` [P,Ds] and ``eps`` [P,H,Ds] are static device buffers: fill them (``set_inputs``) and ``launch()``, or
-    capture ``launch()`` in a CUDA graph.  Policy and reward terms as for ``RolloutPlan``; the policy must be unbatched."""
+    capture ``launch()`` in a CUDA graph.  Policy and reward terms as for ``RolloutPlan``; the policy must be unbatched.
+    ``grad=True`` also allocates the buffers of ``launch_grad()`` (pilco_particles_rollout_grad)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0):
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False):
         d = device()
         self.P, self.H = int(P), int(H)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
@@ -552,6 +553,35 @@ class ParticlePlan:
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         self.pr = pr
+        self.grad = None
+        if grad:
+            g = _lib.ParticlesGrad()
+            if pol.kind == _lib.POLICY_LINEAR:
+                self.gbuf = {"W": mk(U, Ds), "b": mk(U)}
+                g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
+            else:
+                bf = self.rbf.n
+                self.gbuf = {"X": mk(bf, Ds), "Y": mk(bf, U), "ell": mk(U, Ds)}
+                g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
+                g.pol_L = self.rbf.fact_ws.data_ptr()
+            self.gbuf["value"] = mk(1)
+            g.value = self.gbuf["value"].data_ptr()
+            gwsb = lib.pilco_particles_grad_workspace_bytes(C.byref(pr))
+            if gwsb == 0:
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+            self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
+            g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
+            self.grad = g
+
+    def launch_grad(self):
+        """pilco_particles_rollout_grad: the rollout (``outputs()`` as after ``launch()``, bitwise) and the pathwise
+        gradient of value = mean return w.r.t. the policy parameters with x0 and eps fixed.  Returns the device tensors
+        {'value' [1], 'W' [U,Ds], 'b' [U]} (linear) or {'value', 'X' [bf,Ds], 'Y' [bf,U], 'ell' [U,Ds]} (RBF, constrained
+        lengthscales), like ``RolloutPlan.backward``."""
+        if self.grad is None:
+            raise RuntimeError("ParticlePlan: constructed without grad=True")
+        check(lib.pilco_particles_rollout_grad(C.byref(self.pr), C.byref(self.grad), stream_ptr()), "particles_rollout_grad")
+        return self.gbuf
 
     def set_inputs(self, x0, eps):
         self.x0.copy_(dev(x0).reshape(self.P, self.Ds))
@@ -565,6 +595,24 @@ class ParticlePlan:
         """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views)"""
         H = self.H
         return self.traj, self.act_buf[:, :H], self.rew_buf[:, :H], self.risk_buf[:, :H], self.ret
+
+
+def gp_predict_vjp(gp, Xs, gmean, gvar):
+    """pilco_gp_predict_vjp: d/dXs of sum(gmean * mean + gvar * var) over all E outputs of the (unbatched, mode-0)
+    factorised model ``gp`` at Xs [T,D]; gmean, gvar [T,E] -> [T,D] device tensor."""
+    Xs, gmean, gvar = dev(Xs), dev(gmean), dev(gvar)
+    T = int(Xs.shape[0])
+    if Xs.shape != (T, gp.D) or gmean.shape != (T, gp.E) or gvar.shape != (T, gp.E):
+        raise ValueError("gp_predict_vjp: expected Xs [T,%d], gmean and gvar [T,%d]" % (gp.D, gp.E))
+    out = torch.empty((T, gp.D), dtype=F64, device=device())
+    wsb = lib.pilco_gp_predict_vjp_workspace_bytes(gp.n, gp.D, gp.E, T)
+    if wsb == 0:
+        raise ValueError("gp_predict_vjp: unsupported sizes (n=%d, D=%d, E=%d, T=%d)" % (gp.n, gp.D, gp.E, T))
+    ws = torch.empty(wsb // 8, dtype=F64, device=device())
+    g = gp.struct()
+    check(lib.pilco_gp_predict_vjp(C.byref(g), T, ptr(Xs), ptr(gmean), ptr(gvar), ptr(out), ptr(ws), wsb,
+                                   stream_ptr()), "gp_predict_vjp")
+    return out
 
 
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0):

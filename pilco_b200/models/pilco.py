@@ -16,6 +16,7 @@ from .mgpr import MGPR
 from .smgpr import SMGPR
 
 ParticleTrajectories = collections.namedtuple("ParticleTrajectories", ["states", "actions", "rewards", "risks", "returns"])
+ParticlePolicyGradient = collections.namedtuple("ParticlePolicyGradient", ["value", "grad", "returns"])
 
 
 def _sqrt_factor(S):
@@ -142,11 +143,19 @@ class PILCO:
         -> ParticleTrajectories(states [S,n+1,Ds], actions [S,n,U], rewards [S,n], risks [S,n], returns [S]) of
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
-        import torch
         from ..params import HostArray
+        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_trajectories")
+        plan.launch()
+        out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
+        return ParticleTrajectories(*out)
+
+    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False):
+        """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
+        (from ``np.random`` when None): the same seed gives the same particles to every caller."""
+        import torch
         n, S = int(n), int(num_samples)
         if n < 0 or S < 1:
-            raise ValueError("sample_trajectories: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (n, S))
+            raise ValueError("%s: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (what, n, S))
         dyn = self.mgpr.device_gp()
         Ds = self.state_dim
         m = np.asarray(m_x, dtype=np.float64).reshape(Ds)
@@ -157,14 +166,53 @@ class PILCO:
         g = torch.Generator(device=d)
         g.manual_seed(int(seed))
         terms, mult_mu = self.reward_spec()
-        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, S, n, mult_mu=mult_mu)
+        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, S, n, mult_mu=mult_mu, grad=grad)
         eps0 = torch.randn((S, Ds), dtype=engine.F64, device=d, generator=g)
         plan.x0.copy_(engine.dev(m)[None] + eps0 @ engine.dev(F).T)
         if n > 0:
             plan.eps_buf.copy_(torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g))
-        plan.launch()
-        out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
-        return ParticleTrajectories(*out)
+        return plan
+
+    def _flat_grad(self, g):
+        """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
+        derivative of the softplus transform, sigmoid(theta), as policy_opt applies it"""
+        c = self.controller
+        if isinstance(c, controllers.LinearController):
+            return np.concatenate([g["W"].cpu().numpy().ravel(), g["b"].cpu().numpy().ravel()])
+        bf, Ds, U = c.policy_shapes
+        th = c.get_flat()[bf * Ds + bf * U:]
+        return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
+                               g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
+
+    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None):
+        """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
+        are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
+        d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
+        sampled return, to compare with ``policy_gradient``.  Box (risk) terms enter value but not grad: their
+        indicator is flat almost everywhere, so for them the estimate of d E[return] is biased.
+
+        -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
+        from ..params import HostArray
+        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True)
+        g = plan.launch_grad()
+        return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
+                                      plan.ret.cpu().numpy().view(HostArray))
+
+    def policy_gradient(self, m_x=None, s_x=None, n=None):
+        """The moment-matching reward of ``predict`` (n steps from N(m_x, s_x); defaults m_init, S_init, horizon) and
+        its gradient d reward / d controller.get_flat() for the current policy: the direction ``optimize_policy``
+        ascends, in the layout of ``sample_policy_gradient``.  -> (reward (float), grad host array)."""
+        from ..params import HostArray
+        m_x = self.m_init if m_x is None else m_x
+        s_x = self.S_init if s_x is None else s_x
+        n = self.horizon if n is None else n
+        terms, mult_mu = self.reward_spec()
+        plan = engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
+                                  np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
+                                  int(n), R=1, mult_mu=mult_mu, grad=True)
+        plan.forward()
+        g = plan.backward()
+        return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
     def training_loss(self):
         return -self.predict(self.m_init, self.S_init, self.horizon)[2]
