@@ -351,6 +351,19 @@ typedef struct pilco_particles_grad {
 size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr);  /* 0: unsupported sizes */
 int    pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* The particle gradient of R policies at once (policy optimisation on the sampled return, random restarts in one call):
+ * restart r runs the policy at r times the policy's batch strides (W_bs, b_bs, rbf.X_bs / ell_bs / sf2_bs / beta_bs;
+ * a stride of 0 shares that array) over the SAME x0 [P,Ds] and eps [P,H,Ds] (common random numbers: the restarts are
+ * compared on one sample), through the one unbatched dynamics model.  Outputs are restart-major: traj [R,P,H+1,Ds],
+ * act [R,P,H,U], step_reward / step_risk [R,P,H], ret [R,P], value [R], gW [R,U,Ds], gb [R,U], gXc [R,bf,Ds],
+ * gYc [R,bf,U], gell [R,U,Ds]; pol_L = the [R,U,ldw,ldw] Cholesky factors a batched pilco_gp_factorize leaves.
+ * Restart r's outputs are bitwise those of pilco_particles_rollout_grad with policy r.  One predict / VJP call per
+ * step at T = R P.  Validation as pilco_particles_rollout_grad, plus PILCO_ERR_DIM for R < 1, R > 65535,
+ * R P > 65535 * 32 (the predict limit) or a negative stride; no host synchronisation (graph-capturable). */
+size_t pilco_particles_batch_grad_workspace_bytes(const pilco_particles* pr, int R);   /* 0: unsupported sizes */
+int    pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R,
+                                          const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

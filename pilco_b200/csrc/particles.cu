@@ -7,6 +7,11 @@
 // pt_step_kernel is one thread per particle: it closes the previous step from the predict outputs, writes traj[:, t],
 // and for t < H evaluates the reward terms at the point x_t, the policy and the predict input x~_t; at t = H it sums
 // the return.  The O(n^2) work per step is pilco_gp_predict (predict.cu) at T = P.
+// pilco_particles_rollout_batch_grad runs R policies over the same x0 and eps (DESIGN.md section 13): restart r is
+// blockIdx.y of the per-particle kernels, its particle p is row r P + p of every output and of the predict calls
+// (T = R P), and its policy arrays are offset by r times their batch strides.  The unbatched entry points are the
+// same launches at R = 1.
+#include <initializer_list>
 #include "common.cuh"
 #include "risk_math.cuh"
 
@@ -21,11 +26,12 @@ struct PtDev {
     const double* maxa;
     const double* W; const double* b;                   // linear policy [U,Ds], [U]
     const double* C; const double* ell; const double* sf2; const double* beta; int bf;   // RBF policy
+    long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;   // per-restart policy strides (0: shared)
     int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
-    const double* x0; const double* eps;
-    double* traj; double* act; double* step_reward; double* step_risk; double* ret;
-    double* xt;                                         // predict input [P,D]
-    const double* mean; const double* var;              // predict outputs [P,Ds]
+    const double* x0; const double* eps;                // [P,Ds], [P,H,Ds]: shared by the restarts
+    double* traj; double* act; double* step_reward; double* step_risk; double* ret;   // rows r P + p
+    double* xt;                                         // predict input [R P,D]
+    const double* mean; const double* var;              // predict outputs [R P,Ds]
 };
 
 // one reward term at the point x (registers; xg = the same point in global memory, for the box's indexed reads):
@@ -55,21 +61,22 @@ __device__ __forceinline__ double pt_reward_value(const pilco_reward_term& rt, c
     return exp(-0.5 * quad);
 }
 
-// grid ceil(P / 128), one thread per particle
+// grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y
 __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     PDL_ENTRY();
-    const int p = blockIdx.x * PT_THREADS + threadIdx.x;
+    const int p = blockIdx.x * PT_THREADS + threadIdx.x, r = blockIdx.y;
     if (p >= a.P) return;
     const int Ds = a.Ds, U = a.U, D = Ds + U, t = a.t, H = a.H;
-    double* tr = a.traj + ((size_t)p * (H + 1) + t) * Ds;
+    const size_t row = (size_t)r * a.P + p;
+    double* tr = a.traj + (row * (H + 1) + t) * Ds;
     double x[MAXD];
     if (t == 0) {
 #pragma unroll
         for (int d = 0; d < MAXD; ++d) x[d] = d < Ds ? a.x0[(size_t)p * Ds + d] : 0.0;
     } else {                                            // close step t-1
         const double* xp = tr - Ds;
-        const double* mu = a.mean + (size_t)p * Ds;
-        const double* var = a.var + (size_t)p * Ds;
+        const double* mu = a.mean + row * Ds;
+        const double* var = a.var + row * Ds;
         const double* ep = a.eps + ((size_t)p * H + (t - 1)) * Ds;
 #pragma unroll
         for (int d = 0; d < MAXD; ++d) {
@@ -81,7 +88,7 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     }
 #pragma unroll
     for (int d = 0; d < MAXD; ++d) if (d < Ds) tr[d] = x[d];
-    const size_t ph = (size_t)p * H;
+    const size_t ph = row * H;
     if (t == H) {                                       // return: step order, as ro_reward_sum_kernel
         double s = 0.0;
         for (int tt = 0; tt < H; ++tt) s += a.step_reward[ph + tt];
@@ -90,7 +97,7 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
             for (int tt = 0; tt < H; ++tt) mult *= 1.0 - a.step_risk[ph + tt];
             s += a.mult_mu * (1.0 - mult);
         }
-        a.ret[p] = s;
+        a.ret[row] = s;
         return;
     }
     double rew = 0.0, risk = 0.0;                       // at the pre-step state (pilco.py:130-134)
@@ -102,7 +109,7 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     }
     a.step_reward[ph + t] = rew;
     a.step_risk[ph + t] = risk;
-    double* xo = a.xt + (size_t)p * D;
+    double* xo = a.xt + row * D;
 #pragma unroll
     for (int d = 0; d < MAXD; ++d) if (d < Ds) xo[d] = x[d];
     double* ao = a.act + (ph + t) * U;
@@ -113,18 +120,21 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     for (int j = 0; j < U; ++j) {
         double u;
         if (a.pol_kind == PILCO_POLICY_LINEAR) {        // dev_linear_action's order
-            u = a.b[j];
+            const double* W = a.W + r * a.W_bs;
+            u = a.b[r * a.b_bs + j];
 #pragma unroll
-            for (int d = 0; d < MAXD; ++d) if (d < Ds) u = fma(a.W[j * Ds + d], x[d], u);
+            for (int d = 0; d < MAXD; ++d) if (d < Ds) u = fma(W[j * Ds + d], x[d], u);
         } else {                                        // sum_i beta_ji sf2_j exp(-0.5 |(x - c_i) / ell_j|^2)
+            const double* ell = a.ell + r * a.ell_bs;
             double il[MAXD];
 #pragma unroll
-            for (int d = 0; d < MAXD; ++d) il[d] = d < Ds ? 1.0 / a.ell[j * Ds + d] : 0.0;
-            const double sf2 = a.sf2[j];
-            const double* be = a.beta + (size_t)j * a.bf;
+            for (int d = 0; d < MAXD; ++d) il[d] = d < Ds ? 1.0 / ell[j * Ds + d] : 0.0;
+            const double sf2 = a.sf2[r * a.sf2_bs + j];
+            const double* be = a.beta + r * a.beta_bs + (size_t)j * a.bf;
+            const double* C = a.C + r * a.C_bs;
             u = 0.0;
             for (int i = 0; i < a.bf; ++i) {
-                const double* c = a.C + (size_t)i * Ds;
+                const double* c = C + (size_t)i * Ds;
                 double d2 = 0.0;
 #pragma unroll
                 for (int d = 0; d < MAXD; ++d) if (d < Ds) { const double q = (x[d] - c[d]) * il[d]; d2 = fma(q, q, d2); }
@@ -150,33 +160,35 @@ struct PgDev {
     const double* maxa;
     const double* W; const double* b;
     const double* C; const double* ell; const double* sf2; const double* beta; int bf;
+    long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;
     int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
     const double* eps; const double* traj; const double* step_risk;
-    const double* gxt;          // VJP of step t at x~_t [P,D]; NULL at t = H-1
-    const double* var_prev;     // var_{t-1} [P,Ds] (t > 0)
-    double* gx;                 // [P,Ds] x_bar_{t+1} in, x_bar_t out (= the gmean of step t-1's VJP)
-    double* gvar;               // [P,Ds] the gvar of step t-1's VJP
-    double* zbar;               // [P,H,U]
+    const double* gxt;          // VJP of step t at x~_t [R P,D]; NULL at t = H-1
+    const double* var_prev;     // var_{t-1} [R P,Ds] (t > 0)
+    double* gx;                 // [R P,Ds] x_bar_{t+1} in, x_bar_t out (= the gmean of step t-1's VJP)
+    double* gvar;               // [R P,Ds] the gvar of step t-1's VJP
+    double* zbar;               // [R P,H,U]
 };
 
-// grid ceil(P / 128), one thread per particle: step t of the reverse sweep
+// grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y: step t of the reverse sweep
 __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
     PDL_ENTRY();
-    const int p = blockIdx.x * PT_THREADS + threadIdx.x;
+    const int p = blockIdx.x * PT_THREADS + threadIdx.x, r = blockIdx.y;
     if (p >= a.P) return;
     const int Ds = a.Ds, U = a.U, t = a.t, H = a.H;
-    const double* xg = a.traj + ((size_t)p * (H + 1) + t) * Ds;
-    const double* gxt = a.gxt ? a.gxt + (size_t)p * (Ds + U) : nullptr;
+    const size_t row = (size_t)r * a.P + p;
+    const double* xg = a.traj + (row * (H + 1) + t) * Ds;
+    const double* gxt = a.gxt ? a.gxt + row * (Ds + U) : nullptr;
     double x[MAXD], xb[MAXD];
 #pragma unroll
     for (int d = 0; d < MAXD; ++d) {
         x[d] = d < Ds ? xg[d] : 0.0;
-        xb[d] = (d < Ds && gxt) ? a.gx[(size_t)p * Ds + d] + gxt[d] : 0.0;
+        xb[d] = (d < Ds && gxt) ? a.gx[row * Ds + d] + gxt[d] : 0.0;
     }
     // reward terms at x_t (box: flat almost everywhere, no gradient)
     double wmult = 0.0;
     if (a.n_mult > 0) {                                 // mult_mu prod_{s != t} (1 - risk_s): prefix x suffix, no division
-        const double* rk = a.step_risk + (size_t)p * H;
+        const double* rk = a.step_risk + row * H;
         double pre = 1.0, suf = 1.0;
         for (int s = 0; s < t; ++s) pre *= 1.0 - rk[s];
         for (int s = t + 1; s < H; ++s) suf *= 1.0 - rk[s];
@@ -213,27 +225,30 @@ __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
         for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(f, gv[d], xb[d]);
     }
     // policy: z_bar_t and (d pi / dx)' z_bar_t; z_t recomputed in the forward's order
-    double* zb = a.zbar + ((size_t)p * H + t) * U;
+    double* zb = a.zbar + (row * H + t) * U;
     const double su = a.pol_kind == PILCO_POLICY_RBF ? PT_RBF_VAR : 0.0;
     for (int j = 0; j < U; ++j) {
         if (!gxt) { zb[j] = 0.0; continue; }
         double jx[MAXD], z;
         if (a.pol_kind == PILCO_POLICY_LINEAR) {
-            z = a.b[j];
+            const double* W = a.W + r * a.W_bs;
+            z = a.b[r * a.b_bs + j];
 #pragma unroll
             for (int d = 0; d < MAXD; ++d) {
-                jx[d] = d < Ds ? a.W[j * Ds + d] : 0.0;
-                if (d < Ds) z = fma(a.W[j * Ds + d], x[d], z);
+                jx[d] = d < Ds ? W[j * Ds + d] : 0.0;
+                if (d < Ds) z = fma(W[j * Ds + d], x[d], z);
             }
         } else {                                        // d z_j / dx = sum_i beta_ji k_ji (c_i - x) / ell_j^2
+            const double* ell = a.ell + r * a.ell_bs;
             double il[MAXD];
 #pragma unroll
-            for (int d = 0; d < MAXD; ++d) { il[d] = d < Ds ? 1.0 / a.ell[j * Ds + d] : 0.0; jx[d] = 0.0; }
-            const double sf2 = a.sf2[j];
-            const double* be = a.beta + (size_t)j * a.bf;
+            for (int d = 0; d < MAXD; ++d) { il[d] = d < Ds ? 1.0 / ell[j * Ds + d] : 0.0; jx[d] = 0.0; }
+            const double sf2 = a.sf2[r * a.sf2_bs + j];
+            const double* be = a.beta + r * a.beta_bs + (size_t)j * a.bf;
+            const double* C = a.C + r * a.C_bs;
             z = 0.0;
             for (int i = 0; i < a.bf; ++i) {
-                const double* c = a.C + (size_t)i * Ds;
+                const double* c = C + (size_t)i * Ds;
                 double d2 = 0.0;
 #pragma unroll
                 for (int d = 0; d < MAXD; ++d) if (d < Ds) { const double q = (x[d] - c[d]) * il[d]; d2 = fma(q, q, d2); }
@@ -252,15 +267,15 @@ __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
         for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(zbj, jx[d], xb[d]);
     }
 #pragma unroll
-    for (int d = 0; d < MAXD; ++d) if (d < Ds) a.gx[(size_t)p * Ds + d] = xb[d];
+    for (int d = 0; d < MAXD; ++d) if (d < Ds) a.gx[row * Ds + d] = xb[d];
     if (t > 0) {                                        // cotangents of step t-1's predict outputs
-        const double* vp = a.var_prev + (size_t)p * Ds;
+        const double* vp = a.var_prev + row * Ds;
         const double* ep = a.eps + ((size_t)p * H + (t - 1)) * Ds;
 #pragma unroll
         for (int d = 0; d < MAXD; ++d) {
             if (d < Ds) {
                 const double v = vp[d];
-                a.gvar[(size_t)p * Ds + d] = v > 0.0 ? xb[d] * ep[d] / (2.0 * sqrt(v)) : 0.0;
+                a.gvar[row * Ds + d] = v > 0.0 ? xb[d] * ep[d] / (2.0 * sqrt(v)) : 0.0;
             }
         }
     }
@@ -288,28 +303,32 @@ struct PgRed {
     int P, H, Ds, U, bf, pol_kind;
     const double* traj; const double* zbar; const double* ret;
     const double* C; const double* ell; const double* sf2; const double* beta;
-    double* gW; double* gb;                             // linear
-    double* s1; double* s2; double* gbeta;              // RBF per (output j, centre i): [U,bf,Ds], [U,bf,Ds], [U,bf]
-    double* gXc; double* gell;                          // RBF direct terms (pg_rbf_finish_kernel)
-    double* value;
+    long long C_bs, ell_bs, sf2_bs, beta_bs;            // per-restart RBF policy strides (0: shared)
+    double* gW; double* gb;                             // linear [R,U,Ds], [R,U]
+    double* s1; double* s2; double* gbeta;              // RBF per (r, output j, centre i): [R,U,bf,Ds] (x2), [R,U,bf]
+    double* gXc; double* gell;                          // RBF direct terms (pg_rbf_finish_kernel) [R,bf,Ds], [R,U,Ds]
+    double* value;                                      // [R]
 };
 
-// The policy-parameter gradient over all P H points (x_t, z_bar_t) and the value, each CTA one fixed-order sum:
-// grid (linear: U, RBF: U bf) + 1, 256 threads; thread q takes the points q, q + 256, ... in order.
+// The policy-parameter gradient over all P H points (x_t, z_bar_t) of restart r = blockIdx.y and its value, each CTA
+// one fixed-order sum: grid ((linear: U, RBF: U bf) + 1, R), 256 threads; thread q takes the points q, q + 256, ...
+// of the restart in order (so a restart's sums do not depend on R).
 //   linear j:    gW[j] = sum z_bar_j x / P,  gb[j] = sum z_bar_j / P
 //   RBF (j, i):  a = z_bar_j beta_ji k_ji:  s1 = sum a (x - c_i),  s2 = sum a (x - c_i)^2,  gbeta_ji = sum z_bar_j k_ji / P
 __global__ void __launch_bounds__(256) pg_param_kernel(PgRed a) {
     PDL_ENTRY();
     __shared__ double red[(2 * MAXD + 1) * 8], out[2 * MAXD + 1];
-    const int Ds = a.Ds, U = a.U, H = a.H, tid = threadIdx.x;
-    const size_t npts = (size_t)a.P * H;
+    const int Ds = a.Ds, U = a.U, H = a.H, tid = threadIdx.x, r = blockIdx.y;
+    const size_t npts = (size_t)a.P * H, r0 = (size_t)r * a.P;       // r0: the restart's first row
+    const double* traj = a.traj + r0 * (H + 1) * Ds;
+    const double* zbar = a.zbar + r0 * H * U;
     const int nblk = a.pol_kind == PILCO_POLICY_LINEAR ? U : U * a.bf;
     const double invP = 1.0 / a.P;
     if ((int)blockIdx.x == nblk) {                      // value = mean return
         double v[1] = {0.0};
-        for (int p = tid; p < a.P; p += 256) v[0] += a.ret[p];
+        for (int p = tid; p < a.P; p += 256) v[0] += a.ret[r0 + p];
         pg_block_sum<1>(v, red, out);
-        if (tid == 0) a.value[0] = out[0] * invP;
+        if (tid == 0) a.value[r] = out[0] * invP;
         return;
     }
     if (a.pol_kind == PILCO_POLICY_LINEAR) {
@@ -319,31 +338,33 @@ __global__ void __launch_bounds__(256) pg_param_kernel(PgRed a) {
         for (int d = 0; d <= MAXD; ++d) v[d] = 0.0;
         for (size_t q = tid; q < npts; q += 256) {
             const size_t p = q / H, t = q % H;
-            const double* x = a.traj + (p * (H + 1) + t) * Ds;
-            const double zb = a.zbar[q * U + j];
+            const double* x = traj + (p * (H + 1) + t) * Ds;
+            const double zb = zbar[q * U + j];
 #pragma unroll
             for (int d = 0; d < MAXD; ++d) if (d < Ds) v[d] = fma(zb, x[d], v[d]);
             v[MAXD] += zb;
         }
         pg_block_sum<MAXD + 1>(v, red, out);
-        if (tid < Ds) a.gW[j * Ds + tid] = out[tid] * invP;
-        if (tid == 0) a.gb[j] = out[MAXD] * invP;
+        if (tid < Ds) a.gW[((size_t)r * U + j) * Ds + tid] = out[tid] * invP;
+        if (tid == 0) a.gb[(size_t)r * U + j] = out[MAXD] * invP;
         return;
     }
     const int j = blockIdx.x / a.bf, i = blockIdx.x % a.bf;
+    const double* C = a.C + r * a.C_bs;
+    const double* ell = a.ell + r * a.ell_bs;
     double c[MAXD], il[MAXD], v[2 * MAXD + 1];
 #pragma unroll
     for (int d = 0; d < MAXD; ++d) {
-        c[d] = d < Ds ? a.C[(size_t)i * Ds + d] : 0.0;
-        il[d] = d < Ds ? 1.0 / a.ell[j * Ds + d] : 0.0;
+        c[d] = d < Ds ? C[(size_t)i * Ds + d] : 0.0;
+        il[d] = d < Ds ? 1.0 / ell[j * Ds + d] : 0.0;
     }
 #pragma unroll
     for (int k = 0; k <= 2 * MAXD; ++k) v[k] = 0.0;
-    const double sf2 = a.sf2[j], bji = a.beta[(size_t)j * a.bf + i];
+    const double sf2 = a.sf2[r * a.sf2_bs + j], bji = a.beta[r * a.beta_bs + (size_t)j * a.bf + i];
     for (size_t q = tid; q < npts; q += 256) {
         const size_t p = q / H, t = q % H;
-        const double* x = a.traj + (p * (H + 1) + t) * Ds;
-        const double zb = a.zbar[q * U + j];
+        const double* x = traj + (p * (H + 1) + t) * Ds;
+        const double zb = zbar[q * U + j];
         double df[MAXD], d2 = 0.0;
 #pragma unroll
         for (int d = 0; d < MAXD; ++d) {
@@ -357,32 +378,33 @@ __global__ void __launch_bounds__(256) pg_param_kernel(PgRed a) {
         for (int d = 0; d < MAXD; ++d) { v[d] = fma(w, df[d], v[d]); v[MAXD + d] = fma(w * df[d], df[d], v[MAXD + d]); }
     }
     pg_block_sum<2 * MAXD + 1>(v, red, out);
-    const size_t ji = (size_t)j * a.bf + i;
+    const size_t ji = ((size_t)r * U + j) * a.bf + i;
     if (tid < Ds) { a.s1[ji * Ds + tid] = out[tid]; a.s2[ji * Ds + tid] = out[MAXD + tid]; }
     if (tid == 0) a.gbeta[ji] = out[2 * MAXD] * invP;
 }
 
-// direct RBF gradients from the per-(j, i) sums, in fixed order:
+// direct RBF gradients from the per-(j, i) sums, in fixed order; one CTA per restart r = blockIdx.x:
 //   gXc[i,d] = sum_j s1[j,i,d] / ell_jd^2 / P,   gell[j,d] = sum_i s2[j,i,d] / ell_jd^3 / P
 __global__ void __launch_bounds__(128) pg_rbf_finish_kernel(PgRed a) {
     PDL_ENTRY();
-    const int Ds = a.Ds, U = a.U, bf = a.bf;
+    const int Ds = a.Ds, U = a.U, bf = a.bf, r = blockIdx.x;
     const double invP = 1.0 / a.P;
+    const size_t rU = (size_t)r * U;                    // restart r's first (output, centre) block
     for (int q = threadIdx.x; q < bf * Ds; q += 128) {
         const int i = q / Ds, d = q % Ds;
         double s = 0.0;
         for (int j = 0; j < U; ++j) {
-            const double l = a.ell[j * Ds + d];
-            s += a.s1[((size_t)j * bf + i) * Ds + d] / (l * l);
+            const double l = a.ell[r * a.ell_bs + j * Ds + d];
+            s += a.s1[((rU + j) * bf + i) * Ds + d] / (l * l);
         }
-        a.gXc[q] = s * invP;
+        a.gXc[(size_t)r * bf * Ds + q] = s * invP;
     }
     for (int q = threadIdx.x; q < U * Ds; q += 128) {
         const int j = q / Ds, d = q % Ds;
         double s = 0.0;
-        for (int i = 0; i < bf; ++i) s += a.s2[((size_t)j * bf + i) * Ds + d];
-        const double l = a.ell[q];
-        a.gell[q] = s / (l * l * l) * invP;
+        for (int i = 0; i < bf; ++i) s += a.s2[((rU + j) * bf + i) * Ds + d];
+        const double l = a.ell[r * a.ell_bs + q];
+        a.gell[rU * Ds + q] = s / (l * l * l) * invP;
     }
 }
 
@@ -404,8 +426,14 @@ static bool pt_sizes_ok(const pilco_particles* pr) {
            pr->pol.Ds >= 1 && pr->pol.U >= 1 && pr->pol.Ds <= MAXE;
 }
 
-// everything but the workspace (pilco_particles_rollout_grad brings its own)
-static int pt_check_desc(const pilco_particles* pr) {
+// R restarts of P particles: one CTA row per restart (gridDim.y) and R P predict points
+static bool pt_batch_ok(int P, int R) {
+    return R >= 1 && R <= 65535 && (long long)R * P <= PT_MAX_P;
+}
+
+// everything but the workspace (pilco_particles_rollout_grad brings its own).  batched: the policy's batch strides
+// are honoured (pilco_particles_rollout_batch_grad); otherwise a batched policy is unsupported.
+static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
     const pilco_gp_model& g = pr->dyn;
@@ -415,13 +443,21 @@ static int pt_check_desc(const pilco_particles* pr) {
     const pilco_policy& pol = pr->pol;
     const int Ds = pol.Ds, U = pol.U;
     if (Ds < 1 || U < 1 || Ds + U != g.D || g.E != Ds) return PILCO_ERR_DIM;
+    auto strides = [batched](std::initializer_list<long long> bs) {
+        for (long long b : bs) {
+            if (b && !batched) return PILCO_ERR_UNSUPPORTED;
+            if (b < 0) return PILCO_ERR_DIM;
+        }
+        return PILCO_OK;
+    };
     if (pol.kind == PILCO_POLICY_LINEAR) {
         if (!pol.W || !pol.b) return PILCO_ERR_NULL;
-        if (pol.W_bs || pol.b_bs) return PILCO_ERR_UNSUPPORTED;
+        if (const int rc = strides({pol.W_bs, pol.b_bs})) return rc;
     } else if (pol.kind == PILCO_POLICY_RBF) {
         const pilco_gp_model& r = pol.rbf;
         if (!r.X || !r.ell || !r.sf2 || !r.beta) return PILCO_ERR_NULL;
-        if (r.mode != 1 || r.X_bs || r.ell_bs || r.sf2_bs || r.beta_bs) return PILCO_ERR_UNSUPPORTED;
+        if (r.mode != 1) return PILCO_ERR_UNSUPPORTED;
+        if (const int rc = strides({r.X_bs, r.ell_bs, r.sf2_bs, r.beta_bs})) return rc;
         if (r.n < 1 || r.D != Ds || r.E != U) return PILCO_ERR_DIM;
     } else return PILCO_ERR_UNSUPPORTED;
     if (pol.squash && !pol.max_action) return PILCO_ERR_NULL;
@@ -457,6 +493,10 @@ static PtDev pt_dev(const pilco_particles* pr) {
     a.pol_kind = pol.kind; a.squash = pol.squash; a.maxa = pol.max_action;
     a.W = pol.W; a.b = pol.b;
     a.C = pol.rbf.X; a.ell = pol.rbf.ell; a.sf2 = pol.rbf.sf2; a.beta = pol.rbf.beta; a.bf = pol.rbf.n;
+    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    a.W_bs = rbf ? 0 : pol.W_bs; a.b_bs = rbf ? 0 : pol.b_bs;
+    a.C_bs = rbf ? pol.rbf.X_bs : 0; a.ell_bs = rbf ? pol.rbf.ell_bs : 0;
+    a.sf2_bs = rbf ? pol.rbf.sf2_bs : 0; a.beta_bs = rbf ? pol.rbf.beta_bs : 0;
     a.n_rewards = pr->n_rewards; a.n_mult = 0;
     for (int k = 0; k < 8; ++k) a.rewards[k] = pr->rewards[k];
     for (int k = 0; k < pr->n_rewards; ++k) a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
@@ -466,22 +506,23 @@ static PtDev pt_dev(const pilco_particles* pr) {
     return a;
 }
 
-// workspace of pilco_particles_rollout_grad (offsets in doubles; total and pws_bytes in bytes): the forward's predict
-// inputs and variances of EVERY step (the reverse sweep needs them), the state cotangent, the VJP's cotangents and
-// output, z_bar of every point, the RBF sums, and one predict / VJP workspace (never in use at the same time)
+// workspace of the particle gradient for R restarts (offsets in doubles; total and pws_bytes in bytes): the forward's
+// predict inputs and variances of EVERY step (the reverse sweep needs them), the state cotangent, the VJP's cotangents
+// and output, z_bar of every point, the RBF sums, and one predict / VJP workspace at T = R P (never in use at the same
+// time).  Rows are restart-major (row r P + p); nothing of size [., n] is kept.
 struct PgWs { size_t xt, mean, var, gx, gvar, gxt, zbar, s1, s2, gbeta, gy, pws, pws_bytes, total; };
 
-static PgWs pg_ws_layout(const pilco_particles* pr) {
-    const size_t P = pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+static PgWs pg_ws_layout(const pilco_particles* pr, int R) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pr->pol.kind == PILCO_POLICY_RBF ? pr->pol.rbf.n : 0;
     PgWs L; size_t o = 0;
     auto take = [&](size_t len) { const size_t at = o; o += (len + 1) & ~(size_t)1; return at; };
-    L.xt = take(H * P * D); L.mean = take(P * Ds); L.var = take(H * P * Ds);
-    L.gx = take(P * Ds); L.gvar = take(P * Ds); L.gxt = take(P * D); L.zbar = take(P * H * U);
-    L.s1 = take(U * bf * Ds); L.s2 = take(U * bf * Ds); L.gbeta = take(U * bf); L.gy = take(U * bf);
+    L.xt = take(H * T * D); L.mean = take(T * Ds); L.var = take(H * T * Ds);
+    L.gx = take(T * Ds); L.gvar = take(T * Ds); L.gxt = take(T * D); L.zbar = take(T * H * U);
+    L.s1 = take(R * U * bf * Ds); L.s2 = take(R * U * bf * Ds); L.gbeta = take(R * U * bf); L.gy = take(R * U * bf);
     L.pws = o;
-    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
-    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, pr->P);
+    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
+    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
     L.pws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.total = o * sizeof(double) + L.pws_bytes;
     return L;
@@ -489,9 +530,96 @@ static PgWs pg_ws_layout(const pilco_particles* pr) {
 
 void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
                            const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
-int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, const double* ell,
-                          const double* sf2, long long sf2_bs, const double* beta, const double* gy,
+int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
+                          const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
+                          const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
+
+// the gradient's arguments and workspace, after pt_check_desc
+static int pg_check(const pilco_particles* pr, int R, const pilco_particles_grad* g) {
+    if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
+    const bool rbf = pr->pol.kind == PILCO_POLICY_RBF;
+    if (rbf ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
+    if ((uintptr_t)g->ws & 15) return PILCO_ERR_ALIGN;
+    const PgWs L = pg_ws_layout(pr, R);
+    if (L.pws_bytes == 0) return PILCO_ERR_DIM;
+    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
+    return PILCO_OK;
+}
+
+// forward rollout and reverse sweep of R restarts (validated): R = 1 is pilco_particles_rollout_grad
+static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
+    const PgWs L = pg_ws_layout(pr, R);
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)g->ws;
+    const pilco_policy& pol = pr->pol;
+    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    const int P = pr->P, H = pr->H, Ds = pol.Ds, U = pol.U, D = Ds + U, T = R * P;
+    const size_t PD = (size_t)T * D, PDs = (size_t)T * Ds;
+    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R);
+    int rc;
+    // forward: pilco_particles_rollout's launches, with the predict inputs and variances of every step kept
+    PtDev a = pt_dev(pr);
+    a.mean = ws + L.mean;
+    for (int t = 0; t <= H; ++t) {
+        a.t = t;
+        a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * PD;
+        a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * PDs;
+        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        if (t == H) break;
+        rc = pilco_gp_predict(&pr->dyn, 0, Ds, T, a.xt, ws + L.mean, ws + L.var + (size_t)t * PDs, 0,
+                              ws + L.pws, L.pws_bytes, stream);
+        if (rc) return rc;
+    }
+    // reverse sweep
+    PgDev b;
+    b.P = P; b.H = H; b.Ds = Ds; b.U = U;
+    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
+    b.W = pol.W; b.b = pol.b;
+    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
+    b.W_bs = a.W_bs; b.b_bs = a.b_bs; b.C_bs = a.C_bs; b.ell_bs = a.ell_bs; b.sf2_bs = a.sf2_bs; b.beta_bs = a.beta_bs;
+    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
+    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
+    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
+    b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
+    for (int t = H - 1; t >= 0; --t) {
+        b.t = t;
+        b.gxt = nullptr;
+        if (t < H - 1) {
+            rc = pilco_gp_predict_vjp(&pr->dyn, T, ws + L.xt + (size_t)t * PD, b.gx, b.gvar, ws + L.gxt,
+                                      ws + L.pws, L.pws_bytes, stream);
+            if (rc) return rc;
+            b.gxt = ws + L.gxt;
+        }
+        b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * PDs : nullptr;
+        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
+        CUDA_LAUNCH_CHECK();
+    }
+    // value and the policy-parameter gradient over all P H points of each restart, fixed order
+    PgRed r;
+    r.P = P; r.H = H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
+    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
+    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
+    r.C_bs = a.C_bs; r.ell_bs = a.ell_bs; r.sf2_bs = a.sf2_bs; r.beta_bs = a.beta_bs;
+    r.gW = g->gW; r.gb = g->gb;
+    r.s1 = ws + L.s1; r.s2 = ws + L.s2; r.gbeta = ws + L.gbeta;
+    r.gXc = g->gXc; r.gell = g->gell;
+    r.value = g->value;
+    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1, R), dim3(256), 0, st, r);
+    CUDA_LAUNCH_CHECK();
+    if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
+        const int bf = r.bf, ldw = pad64(bf);
+        launch_hi(pg_rbf_finish_kernel, dim3(R), dim3(128), 0, st, r);
+        CUDA_LAUNCH_CHECK();
+        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
+                              ws + L.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
+        rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, pol.rbf.X, a.C_bs, pol.rbf.ell, a.ell_bs, pol.rbf.sf2, a.sf2_bs,
+                                   pol.rbf.beta, a.beta_bs, ws + L.gy, g->gXc, g->gYc, g->gell);
+        if (rc) return rc;
+    }
+    return PILCO_OK;
+}
 
 extern "C" {
 
@@ -525,85 +653,32 @@ int pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream) {
 
 size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr) {
     if (!pr || !pt_sizes_ok(pr)) return 0;
-    const PgWs L = pg_ws_layout(pr);
+    const PgWs L = pg_ws_layout(pr, 1);
     return L.pws_bytes ? L.total : 0;
 }
 
 int pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream) {
     int rc = pt_check_desc(pr);
     if (rc) return rc;
-    if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
-    const pilco_policy& pol = pr->pol;
-    const bool rbf = pol.kind == PILCO_POLICY_RBF;
-    if (rbf ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
-    if ((uintptr_t)g->ws & 15) return PILCO_ERR_ALIGN;
-    const PgWs L = pg_ws_layout(pr);
-    if (L.pws_bytes == 0) return PILCO_ERR_DIM;
-    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)g->ws;
-    const int P = pr->P, H = pr->H, Ds = pol.Ds, U = pol.U, D = Ds + U;
-    const size_t PD = (size_t)P * D, PDs = (size_t)P * Ds;
-    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS);
-    // forward: pilco_particles_rollout's launches, with the predict inputs and variances of every step kept
-    PtDev a = pt_dev(pr);
-    a.mean = ws + L.mean;
-    for (int t = 0; t <= H; ++t) {
-        a.t = t;
-        a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * PD;
-        a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * PDs;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        if (t == H) break;
-        rc = pilco_gp_predict(&pr->dyn, 0, Ds, P, a.xt, ws + L.mean, ws + L.var + (size_t)t * PDs, 0,
-                              ws + L.pws, L.pws_bytes, stream);
-        if (rc) return rc;
-    }
-    // reverse sweep
-    PgDev b;
-    b.P = P; b.H = H; b.Ds = Ds; b.U = U;
-    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
-    b.W = pol.W; b.b = pol.b;
-    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
-    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
-    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
-    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
-    b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
-    for (int t = H - 1; t >= 0; --t) {
-        b.t = t;
-        b.gxt = nullptr;
-        if (t < H - 1) {
-            rc = pilco_gp_predict_vjp(&pr->dyn, P, ws + L.xt + (size_t)t * PD, b.gx, b.gvar, ws + L.gxt,
-                                      ws + L.pws, L.pws_bytes, stream);
-            if (rc) return rc;
-            b.gxt = ws + L.gxt;
-        }
-        b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * PDs : nullptr;
-        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
-        CUDA_LAUNCH_CHECK();
-    }
-    // value and the policy-parameter gradient over all P H points, fixed order
-    PgRed r;
-    r.P = P; r.H = H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
-    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
-    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
-    r.gW = g->gW; r.gb = g->gb;
-    r.s1 = ws + L.s1; r.s2 = ws + L.s2; r.gbeta = ws + L.gbeta;
-    r.gXc = g->gXc; r.gell = g->gell;
-    r.value = g->value;
-    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1), dim3(256), 0, st, r);
-    CUDA_LAUNCH_CHECK();
-    if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
-        const int bf = r.bf, ldw = pad64(bf);
-        launch_hi(pg_rbf_finish_kernel, dim3(1), dim3(128), 0, st, r);
-        CUDA_LAUNCH_CHECK();
-        chol_solve_vec_launch(st, U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              ws + L.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
-        rc = rbf_factor_bwd_launch(st, 1, bf, Ds, U, pol.rbf.X, pol.rbf.ell, pol.rbf.sf2, 0, pol.rbf.beta, ws + L.gy,
-                                   g->gXc, g->gYc, g->gell);
-        if (rc) return rc;
-    }
-    return PILCO_OK;
+    rc = pg_check(pr, 1, g);
+    if (rc) return rc;
+    return pg_run(pr, 1, g, stream);
+}
+
+size_t pilco_particles_batch_grad_workspace_bytes(const pilco_particles* pr, int R) {
+    if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    const PgWs L = pg_ws_layout(pr, R);
+    return L.pws_bytes ? L.total : 0;
+}
+
+int pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
+                                       pilco_stream_t stream) {
+    int rc = pt_check_desc(pr, true);
+    if (rc) return rc;
+    if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
+    rc = pg_check(pr, R, g);
+    if (rc) return rc;
+    return pg_run(pr, R, g, stream);
 }
 
 }  // extern "C"

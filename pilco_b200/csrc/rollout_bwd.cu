@@ -249,16 +249,18 @@ static int launch_dyn_finish(const MMTapeBwd& tb, const RbDev& d, cudaStream_t s
 
 // VJP through beta_a = (K_a + sn2 I)^-1 y_a for the RBF policy (sf2 frozen, controllers.py:91-93): given gy_a = (K_a+sn2 I)^-1 gbeta_a,
 //   gY[:,a] = gy_a ;  gK = -gy beta^T ;  gX += ..., gell += ...   (oracle/staged.py: rbf_factor_backward)
-__global__ void __launch_bounds__(128) rbf_factor_bwd_kernel(int bf, int Ds, int U, const double* X, const double* ell,
+// X, ell, sf2, beta: the policy's arrays with their per-restart strides; gy, gX, gY, gell: contiguous [R, ...]
+__global__ void __launch_bounds__(128) rbf_factor_bwd_kernel(int bf, int Ds, int U, const double* X, long long X_bs,
+                                                             const double* ell, long long ell_bs,
                                                              const double* sf2, long long sf2_bs,
-                                                             const double* beta, const double* gy,
+                                                             const double* beta, long long beta_bs, const double* gy,
                                                              double* gX, double* gY, double* gell) {
     PDL_ENTRY();
     // one CTA per restart, thread n owns centre n: K[n][m] is evaluated once per (n, m, a)
     const int r = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-    const double* Xr = X + (size_t)r * bf * Ds;
-    const double* lr = ell + (size_t)r * U * Ds;
-    const double* br = beta + (size_t)r * U * bf;
+    const double* Xr = X + (size_t)r * X_bs;
+    const double* lr = ell + (size_t)r * ell_bs;
+    const double* br = beta + (size_t)r * beta_bs;
     const double* gr = gy + (size_t)r * U * bf;
     __shared__ double sgl[MAXD * 4], sglo[MAXD];
     for (int e = tid; e < bf * U; e += nt) { const int n = e / U, a = e % U; gY[(size_t)r * bf * U + e] = gr[a * bf + n]; }
@@ -298,10 +300,12 @@ __global__ void __launch_bounds__(128) rbf_factor_bwd_kernel(int bf, int Ds, int
 }
 
 // rbf_factor_bwd_kernel for callers in other translation units (the particle gradient, particles.cu)
-int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, const double* ell,
-                          const double* sf2, long long sf2_bs, const double* beta, const double* gy,
+int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
+                          const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
+                          const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell) {
-    launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, X, ell, sf2, sf2_bs, beta, gy, gX, gY, gell);
+    launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, X, X_bs, ell, ell_bs, sf2, sf2_bs, beta, beta_bs,
+              gy, gX, gY, gell);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
@@ -422,8 +426,9 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
         const int ldw = pad64(bf);
         chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
                               buf(BL.gbeta), (long long)U * bf, bf, 1, buf(BL.gy), bf);
-        launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, ro->pol.rbf.X, ro->pol.rbf.ell, ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs,
-                                                  ro->pol.rbf.beta,
+        launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, ro->pol.rbf.X, (long long)bf * Ds,
+                                                  ro->pol.rbf.ell, (long long)U * Ds, ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs,
+                                                  ro->pol.rbf.beta, (long long)U * bf,
                                                   buf(BL.gy), g->gXc, g->gYc, g->gell);
         CUDA_LAUNCH_CHECK();
     }

@@ -497,16 +497,25 @@ class ParticlePlan:
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
 
     ``x0`` [P,Ds] and ``eps`` [P,H,Ds] are static device buffers: fill them (``set_inputs``) and ``launch()``, or
-    capture ``launch()`` in a CUDA graph.  Policy and reward terms as for ``RolloutPlan``; the policy must be unbatched.
-    ``grad=True`` also allocates the buffers of ``launch_grad()`` (pilco_particles_rollout_grad)."""
+    capture ``launch()`` in a CUDA graph.  Policy and reward terms as for ``RolloutPlan``; one policy is unbatched.
+    ``grad=True`` also allocates the buffers of ``launch_grad()`` (pilco_particles_rollout_grad).
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False):
+    A batch of policies (``R > 1``, or an RBF policy factorised with a leading batch dimension) takes a policy spec
+    with a leading R, as ``RolloutPlan`` does, and needs ``grad=True``: ``launch_grad()`` then runs the R policies over
+    the same x0 and eps (pilco_particles_rollout_batch_grad) and every output has a leading R."""
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1):
         d = device()
-        self.P, self.H = int(P), int(H)
+        self.P, self.H, self.R = int(P), int(H), int(R)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
-        P, H, Ds, U = self.P, self.H, self.Ds, self.U
-        if P < 1 or H < 0:
-            raise ValueError("particles: needs P >= 1 and H >= 0 (P=%d, H=%d)" % (P, H))
+        P, H, Ds, U, R = self.P, self.H, self.Ds, self.U, self.R
+        if P < 1 or H < 0 or R < 1:
+            raise ValueError("particles: needs P >= 1, H >= 0 and R >= 1 (P=%d, H=%d, R=%d)" % (P, H, R))
+        rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
+        self.batched = R > 1 or rbf_batched
+        if self.batched and not grad:
+            raise ValueError("particles: a batch of policies runs the gradient path only (grad=True)")
+        lead = (R,) if self.batched else ()
         self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
         pr = _lib.Particles()
         pr.P, pr.H = P, H
@@ -520,13 +529,15 @@ class ParticlePlan:
         pol.max_action = self.max_action.data_ptr()
         if pol.kind == _lib.POLICY_LINEAR:
             self.W, self.b = dev(policy_spec["W"]), dev(policy_spec["b"])
-            if self.W.numel() != U * Ds or self.b.numel() != U:
-                raise ValueError("particles: the policy must be unbatched (W [U,Ds], b [U])")
+            if self.W.numel() != R * U * Ds or self.b.numel() != R * U:
+                raise ValueError("particles: expected W [R,U,Ds] and b [R,U] with R=%d (unbatched: [U,Ds], [U])" % R)
             pol.W, pol.b = self.W.data_ptr(), self.b.data_ptr()
+            if self.batched:
+                pol.W_bs, pol.b_bs = U * Ds, U
         else:
             self.rbf = policy_spec["gp"]
-            if self.rbf.batched:
-                raise ValueError("particles: the policy must be unbatched")
+            if self.rbf.batched != self.batched or (self.batched and self.rbf.X.shape[0] != R):
+                raise ValueError("particles: the RBF policy must be factorised with a leading R=%d (unbatched: none)" % R)
             pol.rbf = self.rbf.struct()
         self.rw = []
         pr.n_rewards = len(reward_terms)
@@ -541,34 +552,38 @@ class ParticlePlan:
         pr.mult_mu = float(mult_mu)
         mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
         Hb = max(H, 1)                                          # H = 0: every buffer still has an address
-        self.x0, self.eps_buf = mk(P, Ds), mk(P, Hb, Ds)
-        self.traj, self.act_buf = mk(P, H + 1, Ds), mk(P, Hb, U)
-        self.rew_buf, self.risk_buf, self.ret = mk(P, Hb), mk(P, Hb), mk(P)
+        self.x0, self.eps_buf = mk(P, Ds), mk(P, Hb, Ds)                  # shared by the R policies
+        self.traj, self.act_buf = mk(*lead, P, H + 1, Ds), mk(*lead, P, Hb, U)
+        self.rew_buf, self.risk_buf, self.ret = mk(*lead, P, Hb), mk(*lead, P, Hb), mk(*lead, P)
         pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
         pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
         pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
-        wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
-        if wsb == 0:
-            raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
-        self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
-        pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        if not self.batched:                                    # the forward-only rollout (a batch has none)
+            wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
+            if wsb == 0:
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         self.pr = pr
         self.grad = None
         if grad:
             g = _lib.ParticlesGrad()
             if pol.kind == _lib.POLICY_LINEAR:
-                self.gbuf = {"W": mk(U, Ds), "b": mk(U)}
+                self.gbuf = {"W": mk(*lead, U, Ds), "b": mk(*lead, U)}
                 g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
             else:
                 bf = self.rbf.n
-                self.gbuf = {"X": mk(bf, Ds), "Y": mk(bf, U), "ell": mk(U, Ds)}
+                self.gbuf = {"X": mk(*lead, bf, Ds), "Y": mk(*lead, bf, U), "ell": mk(*lead, U, Ds)}
                 g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
                 g.pol_L = self.rbf.fact_ws.data_ptr()
-            self.gbuf["value"] = mk(1)
+            self.gbuf["value"] = mk(R if self.batched else 1)
             g.value = self.gbuf["value"].data_ptr()
-            gwsb = lib.pilco_particles_grad_workspace_bytes(C.byref(pr))
+            if self.batched:
+                gwsb = lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), R)
+            else:
+                gwsb = lib.pilco_particles_grad_workspace_bytes(C.byref(pr))
             if gwsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (P, H, dyn.D, R))
             self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
             self.grad = g
@@ -577,10 +592,15 @@ class ParticlePlan:
         """pilco_particles_rollout_grad: the rollout (``outputs()`` as after ``launch()``, bitwise) and the pathwise
         gradient of value = mean return w.r.t. the policy parameters with x0 and eps fixed.  Returns the device tensors
         {'value' [1], 'W' [U,Ds], 'b' [U]} (linear) or {'value', 'X' [bf,Ds], 'Y' [bf,U], 'ell' [U,Ds]} (RBF, constrained
-        lengthscales), like ``RolloutPlan.backward``."""
+        lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R])."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        check(lib.pilco_particles_rollout_grad(C.byref(self.pr), C.byref(self.grad), stream_ptr()), "particles_rollout_grad")
+        if self.batched:
+            check(lib.pilco_particles_rollout_batch_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
+                  "particles_rollout_batch_grad")
+        else:
+            check(lib.pilco_particles_rollout_grad(C.byref(self.pr), C.byref(self.grad), stream_ptr()),
+                  "particles_rollout_grad")
         return self.gbuf
 
     def set_inputs(self, x0, eps):
@@ -589,12 +609,15 @@ class ParticlePlan:
             self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
 
     def launch(self):
+        if self.batched:
+            raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
         check(lib.pilco_particles_rollout(C.byref(self.pr), stream_ptr()), "particles_rollout")
 
     def outputs(self):
-        """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views)"""
+        """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views), each
+        with a leading R for a batched plan"""
         H = self.H
-        return self.traj, self.act_buf[:, :H], self.rew_buf[:, :H], self.risk_buf[:, :H], self.ret
+        return self.traj, self.act_buf[..., :H, :], self.rew_buf[..., :H], self.risk_buf[..., :H], self.ret
 
 
 def gp_predict_vjp(gp, Xs, gmean, gvar):

@@ -152,11 +152,20 @@ class PILCO:
     def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
         (from ``np.random`` when None): the same seed gives the same particles to every caller."""
+        dyn = self.mgpr.device_gp()
+        x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, what)
+        terms, mult_mu = self.reward_spec()
+        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu, grad=grad)
+        plan.set_inputs(x0, eps)
+        return plan
+
+    def _particle_inputs(self, m_x, s_x, n, num_samples, seed, what):
+        """(x0 [S,Ds], eps [S,n,Ds]) device tensors of ``_particle_plan``: x0 = m + F eps0, then the step normals, from
+        one device generator seeded with ``seed`` (from ``np.random`` when None)."""
         import torch
         n, S = int(n), int(num_samples)
         if n < 0 or S < 1:
             raise ValueError("%s: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (what, n, S))
-        dyn = self.mgpr.device_gp()
         Ds = self.state_dim
         m = np.asarray(m_x, dtype=np.float64).reshape(Ds)
         F = _sqrt_factor(np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds))
@@ -165,13 +174,10 @@ class PILCO:
             seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
         g = torch.Generator(device=d)
         g.manual_seed(int(seed))
-        terms, mult_mu = self.reward_spec()
-        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, S, n, mult_mu=mult_mu, grad=grad)
         eps0 = torch.randn((S, Ds), dtype=engine.F64, device=d, generator=g)
-        plan.x0.copy_(engine.dev(m)[None] + eps0 @ engine.dev(F).T)
-        if n > 0:
-            plan.eps_buf.copy_(torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g))
-        return plan
+        x0 = engine.dev(m)[None] + eps0 @ engine.dev(F).T
+        eps = torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g) if n > 0 else None
+        return x0, eps
 
     def _flat_grad(self, g):
         """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
@@ -213,6 +219,44 @@ class PILCO:
         plan.forward()
         g = plan.backward()
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
+
+    def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None):
+        """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
+        objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
+        over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
+        ``sample_policy_gradient`` draw them for the same ``seed`` (from ``np.random`` when None, drawn after the
+        restarts' starting points).  With the random numbers held fixed the objective is a deterministic, smooth
+        function of the policy parameters, which is why L-BFGS-B applies; its gradient is the pathwise one of
+        ``sample_policy_gradient``.  Restarts are chosen, batched, sharded over ranks and selected as in
+        ``optimize_policy``, evaluated on the same particles.  The controller is set to the winner.
+
+        Returns the winner's sampled value: an in-sample estimate, biased upwards by the optimisation; for an
+        out-of-sample estimate run ``sample_trajectories`` with another seed.  A reward with box (risk) terms is
+        rejected, because they carry no pathwise gradient and the optimiser would ignore the constraint."""
+        from functools import partial
+        from .. import policy_opt
+        if int(num_samples) < 1:
+            raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
+        terms, _ = self.reward_spec()
+        if any(t["kind"] == _lib.REWARD_BOX for t in terms):
+            raise ValueError("optimize_policy_sampled: the reward has box (risk) terms, which carry no pathwise "
+                             "gradient; use optimize_policy")
+        restarts = max(int(restarts), 1)
+        mgpr_trainable = self.mgpr.trainable_parameters
+        for p in mgpr_trainable:
+            set_trainable(p, False)
+        try:
+            flats0 = policy_opt.initial_flats(self.controller, restarts)
+            x0, eps = self._particle_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed,
+                                            "optimize_policy_sampled")
+            best_flat, best_value, _ = policy_opt.optimize(
+                self, maxiter=maxiter, restarts=restarts, flats0=flats0,
+                evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps))
+            self.controller.set_flat(best_flat)
+        finally:
+            for p in mgpr_trainable:
+                set_trainable(p, True)
+        return best_value
 
     def training_loss(self):
         return -self.predict(self.m_init, self.S_init, self.horizon)[2]

@@ -37,41 +37,28 @@ def group_bounds(R, groups=None):
     return [(b[k], b[k + 1]) for k in range(g)]
 
 
-class PolicyEvaluator:
-    """loss(flat) = -sum_t E[r(x_t)] and its gradient for a batch of flat policy parameter vectors.
+class _FlatEvaluator:
+    """What the evaluators share: loss and gradient for R flat policy parameter vectors (``controller.get_flat()``
+    layout), served through pinned host buffers, on the evaluator's own stream, with the whole evaluation captured in
+    one CUDA graph.  A subclass builds its plans, then calls ``_setup_io()``, and implements ``_enqueue()`` with
+    ``_unpack`` (flat parameters -> policy buffers) and ``_pack`` (loss, status and gradient -> ``d_out``)."""
 
-    The R restarts are dealt to ``nsplit`` sub-batches, each with its own RolloutPlan (taped forward + reverse sweep)
-    on its own stream inside ONE captured CUDA graph: the latency-bound glue kernels of one sub-batch overlap the tile
-    kernels of the others."""
-
-    NSPLIT = 4
-
-    def __init__(self, pilco, R, nsplit=None):
+    def __init__(self, pilco, R):
         self.pilco, self.R = pilco, R
         c = pilco.controller
         self.c = c
         self.linear = isinstance(c, controllers.LinearController)
-        flat0 = np.tile(c.get_flat(), (R, 1))
-        self.P = flat0.shape[1]
+        self.flat0 = np.tile(c.get_flat(), (R, 1))
+        self.P = self.flat0.shape[1]
         if self.linear:
             U, Ds = c.W.shape
         else:
             bf, Ds, U = c.policy_shapes
             self.ell_lower = float(c.models[0].kernel.lengthscales.transform.lower)
         self.shape = (Ds, U)
-        terms, mult_mu = pilco.reward_spec()
-        nsplit = max(1, min(int(self.NSPLIT if nsplit is None else nsplit), R // 4 if R >= 8 else 1))
-        bounds = [round(k * R / nsplit) for k in range(nsplit + 1)]
-        self.slices = [(bounds[k], bounds[k + 1]) for k in range(nsplit) if bounds[k + 1] > bounds[k]]
-        self.plans, self.gps = [], []
-        dyn = pilco.mgpr.device_gp()
-        for lo, hi in self.slices:
-            spec = c.policy_spec(flat0[lo:hi]) if self.linear else pilco.policy_spec(flat0[lo:hi])
-            self.gps.append(None if self.linear else spec["gp"])
-            self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
-                                                 np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
-                                                 mult_mu=mult_mu, grad=True))
-        self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
+
+    def _setup_io(self):
+        R = self.R
         self.stream = torch.cuda.Stream()                      # the group's own stream: evaluations of different
         self.done = torch.cuda.Event()                         # groups overlap on the device
         self.graph, self.ncalls, self.cache, self.eval_s = None, 0, None, 0.0
@@ -83,8 +70,8 @@ class PolicyEvaluator:
     def __call__(self, flats):
         """flats [R,P] (numpy) -> loss [R], grad [R,P]; non-finite restarts get (BIG, 0).
         The first call runs eagerly (warm-up), the second captures the whole evaluation -- parameter unpacking,
-        policy factorisation, H-step forward cascade, reverse sweep, gradient packing -- into one CUDA graph
-        that every later L-BFGS evaluation replays."""
+        policy factorisation, forward, reverse sweep, gradient packing -- into one CUDA graph that every later
+        L-BFGS evaluation replays."""
         flats = np.asarray(flats, dtype=np.float64)
         if self.cache is not None and np.array_equal(flats, self.cache[0]):     # the point prepare() evaluated
             return self.cache[1].copy(), self.cache[2].copy()
@@ -125,6 +112,69 @@ class PolicyEvaluator:
         self.eval_s = time.perf_counter() - t0
         self.cache = (np.array(flats, dtype=np.float64), loss, grad)
 
+    def _unpack(self, flat, plan, gp):
+        """flat [R,P] device rows -> the plan's linear policy buffers, or the RBF policy ``gp`` (refactorised);
+        returns the lengthscales' unconstrained theta [R,U,Ds] (RBF) or None"""
+        R = flat.shape[0]
+        Ds, U = self.shape
+        if self.linear:
+            plan.W.copy_(flat[:, :U * Ds].reshape(plan.W.shape))
+            plan.b.copy_(flat[:, U * Ds:].reshape(plan.b.shape))
+            return None
+        bf = gp.n
+        th = flat[:, bf * Ds + bf * U:].reshape(R, U, Ds)
+        gp.X.copy_(flat[:, :bf * Ds].reshape(R, bf, Ds))
+        gp.Y.copy_(flat[:, bf * Ds:bf * Ds + bf * U].reshape(R, bf, U))
+        # ell = lower + log(1 + e^theta): the controller's own transform (controllers.py:100), same formula as
+        # params.Softplus.forward on the host (np.logaddexp)
+        gp.ell.copy_(self.ell_lower + torch.logaddexp(th, torch.zeros_like(th)))
+        engine.gp_refactorize(gp)
+        return th
+
+    def _pack(self, out, value, info, g, th):
+        """out [R,P+2] = [-value | status | -gradient in the flat layout]; the lengthscale block goes through the
+        softplus: d ell / d theta = sigmoid(theta)"""
+        R = out.shape[0]
+        Ds, U = self.shape
+        out[:, 0] = -value
+        out[:, 1] = info.to(torch.float64)
+        if self.linear:
+            out[:, 2:2 + U * Ds] = -g["W"].reshape(R, -1)
+            out[:, 2 + U * Ds:] = -g["b"].reshape(R, -1)
+        else:
+            bf = g["X"].shape[-2]
+            out[:, 2:2 + bf * Ds] = -g["X"].reshape(R, -1)
+            out[:, 2 + bf * Ds:2 + bf * Ds + bf * U] = -g["Y"].reshape(R, -1)
+            out[:, 2 + bf * Ds + bf * U:] = -(g["ell"].reshape(R, U, Ds) * torch.sigmoid(th)).reshape(R, -1)
+
+
+class PolicyEvaluator(_FlatEvaluator):
+    """loss(flat) = -sum_t E[r(x_t)] and its gradient for a batch of flat policy parameter vectors.
+
+    The R restarts are dealt to ``nsplit`` sub-batches, each with its own RolloutPlan (taped forward + reverse sweep)
+    on its own stream inside ONE captured CUDA graph: the latency-bound glue kernels of one sub-batch overlap the tile
+    kernels of the others."""
+
+    NSPLIT = 4
+
+    def __init__(self, pilco, R, nsplit=None):
+        super().__init__(pilco, R)
+        c, flat0 = self.c, self.flat0
+        terms, mult_mu = pilco.reward_spec()
+        nsplit = max(1, min(int(self.NSPLIT if nsplit is None else nsplit), R // 4 if R >= 8 else 1))
+        bounds = [round(k * R / nsplit) for k in range(nsplit + 1)]
+        self.slices = [(bounds[k], bounds[k + 1]) for k in range(nsplit) if bounds[k + 1] > bounds[k]]
+        self.plans, self.gps = [], []
+        dyn = pilco.mgpr.device_gp()
+        for lo, hi in self.slices:
+            spec = c.policy_spec(flat0[lo:hi]) if self.linear else pilco.policy_spec(flat0[lo:hi])
+            self.gps.append(None if self.linear else spec["gp"])
+            self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
+                                                 np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
+                                                 mult_mu=mult_mu, grad=True))
+        self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
+        self._setup_io()
+
     def _enqueue(self):
         self.d_flat.copy_(self.h_flat, non_blocking=True)
         cur = torch.cuda.current_stream()
@@ -140,34 +190,44 @@ class PolicyEvaluator:
 
     def _enqueue_slice(self, k):
         (lo, hi), plan, gp = self.slices[k], self.plans[k], self.gps[k]
-        R = hi - lo
-        Ds, U = self.shape
-        flat = self.d_flat[lo:hi]
-        if self.linear:
-            plan.W.copy_(flat[:, :U * Ds].reshape(R, U, Ds))
-            plan.b.copy_(flat[:, U * Ds:].reshape(R, U))
-        else:
-            bf = gp.n
-            th = flat[:, bf * Ds + bf * U:].reshape(R, U, Ds)
-            gp.X.copy_(flat[:, :bf * Ds].reshape(R, bf, Ds))
-            gp.Y.copy_(flat[:, bf * Ds:bf * Ds + bf * U].reshape(R, bf, U))
-            # ell = lower + log(1 + e^theta): the controller's own transform (controllers.py:100), same formula as
-            # params.Softplus.forward on the host (np.logaddexp)
-            gp.ell.copy_(self.ell_lower + torch.logaddexp(th, torch.zeros_like(th)))
-            engine.gp_refactorize(gp)
+        th = self._unpack(self.d_flat[lo:hi], plan, gp)
         plan.forward()
         g = plan.backward()
-        out = self.d_out[lo:hi]
-        out[:, 0] = -plan.reward
-        out[:, 1] = torch.maximum(plan.info, gp.info if not self.linear else plan.info).to(torch.float64)
-        if self.linear:
-            out[:, 2:2 + U * Ds] = -g["W"].reshape(R, -1)
-            out[:, 2 + U * Ds:] = -g["b"].reshape(R, -1)
-        else:
-            bf = gp.n
-            out[:, 2:2 + bf * Ds] = -g["X"].reshape(R, -1)
-            out[:, 2 + bf * Ds:2 + bf * Ds + bf * U] = -g["Y"].reshape(R, -1)
-            out[:, 2 + bf * Ds + bf * U:] = -(g["ell"] * torch.sigmoid(th)).reshape(R, -1)
+        self._pack(self.d_out[lo:hi], plan.reward, torch.maximum(plan.info, gp.info if not self.linear else plan.info),
+                   g, th)
+
+
+class ParticleEvaluator(_FlatEvaluator):
+    """loss(flat) = -(mean return of P particles) and its pathwise gradient for a batch of flat policy parameter
+    vectors, in ``PolicyEvaluator``'s contract.
+
+    The R policies run over the same particles ``x0`` [P,Ds] and standard normals ``eps`` [P,H,Ds] (H = the horizon),
+    held fixed, so the objective is a deterministic function of the parameters: one batched device call
+    (pilco_particles_rollout_batch_grad) evaluates every restart.  Box terms carry no pathwise gradient, so a reward
+    with them is rejected."""
+
+    def __init__(self, pilco, R, x0, eps):
+        terms, mult_mu = pilco.reward_spec()
+        if any(t["kind"] == _lib.REWARD_BOX for t in terms):
+            raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
+                             "almost everywhere, so optimising it would ignore the constraint")
+        super().__init__(pilco, R)
+        c, flat0 = self.c, self.flat0
+        spec = c.policy_spec(flat0) if self.linear else pilco.policy_spec(flat0)
+        self.gp = None if self.linear else spec["gp"]
+        x0 = engine.dev(x0)
+        self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
+                                        mult_mu=mult_mu, grad=True, R=R)
+        self.plan.set_inputs(x0, eps)
+        self._setup_io()
+
+    def _enqueue(self):
+        self.d_flat.copy_(self.h_flat, non_blocking=True)
+        th = self._unpack(self.d_flat, self.plan, self.gp)
+        g = self.plan.launch_grad()
+        info = self.gp.info if not self.linear else torch.zeros_like(g["value"])
+        self._pack(self.d_out, g["value"].reshape(self.R), info.reshape(self.R), g, th)
+        self.h_out.copy_(self.d_out, non_blocking=True)
 
 
 class LockstepLBFGS:
@@ -297,18 +357,20 @@ def initial_flats(controller, restarts):
     return np.stack(flats)
 
 
-def optimize(pilco, maxiter=50, restarts=1):
-    """Returns (best_flat, best_reward, per-restart rewards)."""
+def optimize(pilco, maxiter=50, restarts=1, evaluator=PolicyEvaluator, flats0=None):
+    """Returns (best_flat, best_reward, per-restart rewards).  ``evaluator(pilco, R)`` builds the evaluator of one
+    lock-step group of R restarts (``PolicyEvaluator``: the moment-matching reward); ``flats0`` [restarts, P] are the
+    starting points (default ``initial_flats``)."""
     restarts = max(int(restarts), 1)
     dist, rank, world = _dist()
-    flats0 = initial_flats(pilco.controller, restarts)
+    flats0 = initial_flats(pilco.controller, restarts) if flats0 is None else np.asarray(flats0, dtype=np.float64)
     mine = shard_restarts(restarts, rank, world)
     P = flats0.shape[1]
     local = np.full((restarts, 1 + P), np.nan)
     if mine:
         x0 = flats0[mine]
         bounds = group_bounds(len(mine))
-        evs = [PolicyEvaluator(pilco, hi - lo) for lo, hi in bounds]
+        evs = [evaluator(pilco, hi - lo) for lo, hi in bounds]
         for ev, (lo, hi) in zip(evs, bounds):
             ev.prepare(x0[lo:hi])
         xs, loss = np.empty_like(x0), np.empty(len(mine))
