@@ -364,6 +364,17 @@ size_t pilco_particles_batch_grad_workspace_bytes(const pilco_particles* pr, int
 int    pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R,
                                           const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* The particle rollout with ONE function drawn per particle from the latent posterior of each dynamics output, instead
+ * of fresh noise at every step: f_t = mu(x~_t) + sum_{s<t} l_s eps_s + sqrt(max(d2, 0)) eps_t, where l and d2 come
+ * from conditioning on the particle's own earlier inputs (k_post(a,b) = k(a,b) - k(a,C) iK k(C,b); forward
+ * substitution in the particle's running Cholesky factor; a pivot d2 <= 1e-10 sf2_e leaves its column out of later
+ * substitutions, so a revisited input reproduces its value).  Same description, outputs, validation and status codes
+ * as pilco_particles_rollout, with pr->ws sized by pilco_particles_consistent_workspace_bytes: O(P H E n) (the K*
+ * history) + O(P H^2 E).  Step 0 is bitwise pilco_particles_rollout's.  A particle's outputs do not depend on P or
+ * on its row; no host synchronisation (graph-capturable). */
+size_t pilco_particles_consistent_workspace_bytes(const pilco_particles* pr);   /* 0: unsupported sizes or overflow */
+int    pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

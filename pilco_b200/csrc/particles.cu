@@ -11,6 +11,9 @@
 // blockIdx.y of the per-particle kernels, its particle p is row r P + p of every output and of the predict calls
 // (T = R P), and its policy arrays are offset by r times their batch strides.  The unbatched entry points are the
 // same launches at R = 1.
+// pilco_particles_rollout_consistent draws ONE posterior function per particle (DESIGN.md section 14): after each step's
+// predict (fs_predict_kernel, predict.cu, which also keeps W_t = K*_t iK and K*_t) fs_cond_kernel conditions the draw
+// on the particle's earlier inputs, and pt_step_kernel closes the step unchanged from the mean and variance it leaves.
 #include <initializer_list>
 #include "common.cuh"
 #include "risk_math.cuh"
@@ -408,6 +411,93 @@ __global__ void __launch_bounds__(128) pg_rbf_finish_kernel(PgRed a) {
     }
 }
 
+// ---- consistent function samples (pilco_particles_rollout_consistent, DESIGN.md section 14) ------------------------
+// Particle p follows x_{t+1} = x_t + f(x~_t) with ONE draw f per particle and output from the latent posterior
+// k_post(a, b) = k_e(a, b) - k(a, C) iK_e k(C, b), sampled sequentially (exact for a GP with path-dependent inputs):
+//   c_s  = k_post(x~_t, x~_s), s < t;   l = L_{<t}^-1 c;   d2 = var(x~_t) - sum_s l_s^2
+//   f_t  = mu(x~_t) + sum_{s<t} l_s eps_s + sqrt(max(d2, 0)) eps_t
+// A pivot with d2 <= FS_TAU sf2_e (conditional sd below 1e-5 sigma_f: no visible randomness, and d2 in the rounding
+// noise of var) leaves its column out of every later substitution: the semidefinite Cholesky, so a revisited input
+// reproduces its earlier value.  The step's own noise is sqrt(max(d2, 0)) in every case.
+#define FS_TAU   1e-10
+#define FS_WARPS 8                      // warps (particles) per CTA of fs_cond_kernel
+
+struct FsCond {
+    int P, H, D, Ds, n, np, t;
+    const double* ell; const double* sf2;               // dynamics [E,D], [E]
+    const double* xh;                                   // [H,P,D] predict inputs of the steps so far
+    const double* mu; const double* s2;                 // [P,Ds] the posterior mean and variance at x~_t
+    const double* W;                                    // [E,P,np] W_t = K*_t iK
+    const double* Kh;                                   // [H,E,P,np] K*_s of every step
+    const double* eps;                                  // [P,H,Ds]
+    double* L;                                          // [H(H+1)/2, E, P] packed rows; (s, r) at s(s+1)/2 + r
+    double* mean; double* var;                          // [P,Ds] what pt_step_kernel closes the step with
+};
+
+__device__ __forceinline__ double fs_bfly(double v) {   // fixed butterfly: every lane ends with the same bits
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// grid (ceil(P / FS_WARPS), E), one warp per (particle p, output e): step t's conditioning on the particle's past.
+// The packed diagonal holds the pivot later substitutions divide by: sqrt(d2), or 0 for a degenerate column.
+__global__ void __launch_bounds__(FS_WARPS * 32, 4) fs_cond_kernel(FsCond a) {
+    PDL_ENTRY();
+    const int lane = threadIdx.x & 31, p = blockIdx.x * FS_WARPS + (threadIdx.x >> 5), e = blockIdx.y;
+    if (p >= a.P) return;
+    const int D = a.D, Ds = a.Ds, t = a.t, n = a.n;
+    const size_t P = a.P, EP = (size_t)Ds * P, pe = (size_t)e * P + p;
+    const double sf2 = a.sf2[e];
+    // lane d < D holds dimension d of x~_t and 1 / ell_ed
+    const bool dl = lane < D;
+    const double xd = dl ? a.xh[((size_t)t * P + p) * D + lane] : 0.0;
+    const double ild = dl ? 1.0 / a.ell[(size_t)e * D + lane] : 0.0;
+    double* Lt = a.L + (size_t)t * (t + 1) / 2 * EP + pe;              // row t: entry s at Lt[s EP]
+    const double* __restrict__ Wr = a.W + pe * a.np;
+    // c_s = k_e(x~_t, x~_s) - W_t . K*_s: lanes stride the columns (and the dimensions) in order, then the butterfly
+    for (int s = 0; s < t; ++s) {
+        const double* __restrict__ Kr = a.Kh + ((size_t)s * EP + pe) * a.np;
+        double dot = 0.0;
+#pragma unroll 4
+        for (int j = lane; j < n; j += 32) dot = fma(Wr[j], Kr[j], dot);
+        const double q = dl ? (xd - a.xh[((size_t)s * P + p) * D + lane]) * ild : 0.0;
+        dot = fs_bfly(dot);
+        const double d2 = fs_bfly(q * q);
+        const double c = sf2 * exp(-0.5 * d2) - dot;
+        if (lane == 0) Lt[(size_t)s * EP] = c;
+    }
+    __syncwarp();
+    // forward substitution in the particle's running factor, in place: Lt[s] = c_s -> l_s
+    for (int s = 0; s < t; ++s) {
+        const double* Ls = a.L + (size_t)s * (s + 1) / 2 * EP + pe;
+        double sub = 0.0;
+        for (int r = lane; r < s; r += 32) sub = fma(Ls[(size_t)r * EP], Lt[(size_t)r * EP], sub);
+        sub = fs_bfly(sub);
+        const double piv = Ls[(size_t)s * EP];
+        const double l = piv > 0.0 ? (Lt[(size_t)s * EP] - sub) / piv : 0.0;
+        __syncwarp();                                   // every lane has read c_s before it is overwritten
+        if (lane == 0) Lt[(size_t)s * EP] = l;
+        __syncwarp();
+    }
+    double ssq = 0.0, sme = 0.0;
+    const double* ep = a.eps + (size_t)p * a.H * Ds + e;
+    for (int s = lane; s < t; s += 32) {
+        const double l = Lt[(size_t)s * EP];
+        ssq = fma(l, l, ssq);
+        sme = fma(l, ep[(size_t)s * Ds], sme);
+    }
+    ssq = fs_bfly(ssq);
+    sme = fs_bfly(sme);
+    if (lane == 0) {
+        const size_t o = (size_t)p * Ds + e;
+        const double mu = a.mu[o], d2 = a.s2[o] - ssq;
+        Lt[(size_t)t * EP] = d2 > FS_TAU * sf2 ? sqrt(d2) : 0.0;
+        a.mean[o] = t > 0 ? mu + sme : mu;              // t = 0: the marginal sampler's step exactly
+        a.var[o] = d2 < 0.0 ? 0.0 : d2;                 // NaN stays NaN
+    }
+}
+
 struct PtWs { size_t xt, mean, var, pws, pws_bytes, total; };     // offsets in doubles; total and pws_bytes in bytes
 
 static PtWs pt_ws_layout(const pilco_particles* pr) {
@@ -505,6 +595,39 @@ static PtDev pt_dev(const pilco_particles* pr) {
     a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
     return a;
 }
+
+// workspace of the consistent rollout (offsets in doubles; total and pws_bytes in bytes; ok = false on size_t
+// overflow): x~ of every step [H,P,D], the predict outputs mu and var and the step closure's mean and var [P,Ds],
+// W_t [E,P,np], the K* history [H,E,P,np], the packed factor rows [H(H+1)/2,E,P], one predict workspace at T = P
+struct FsWs { size_t xh, mu, s2, mean, var, W, Kh, L, pws, pws_bytes, total; bool ok; };
+
+static bool fs_mul(size_t x, size_t y, size_t& r) { return !__builtin_mul_overflow(x, y, &r); }
+
+static FsWs fs_ws_layout(const pilco_particles* pr) {
+    FsWs L = {};
+    const size_t P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
+    size_t xh, pd, w, kh, rows, lp;
+    L.ok = fs_mul(H * P, D, xh) && fs_mul(P, Ds, pd) && fs_mul(pd, np, w) && fs_mul(H, w, kh) &&
+           fs_mul(H, H + 1, rows) && fs_mul(rows / 2, pd, lp);
+    if (!L.ok) return L;
+    size_t o = 0;
+    auto take = [&](size_t len) {
+        const size_t at = o;
+        if (len == SIZE_MAX || __builtin_add_overflow(o, len + (len & 1), &o)) L.ok = false;
+        return at;
+    };
+    L.xh = take(xh); L.mu = take(pd); L.s2 = take(pd); L.mean = take(pd); L.var = take(pd);
+    L.W = take(w); L.Kh = take(kh); L.L = take(lp);
+    L.pws = o;
+    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
+    size_t b = 0;
+    if (!L.ok || !fs_mul(o, sizeof(double), b) || __builtin_add_overflow(b, L.pws_bytes, &L.total)) L.ok = false;
+    return L;
+}
+
+int fs_predict_prepare();
+int fs_predict_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, double* mean, double* var,
+                      double* W, double* Ks, void* ws);
 
 // workspace of the particle gradient for R restarts (offsets in doubles; total and pws_bytes in bytes): the forward's
 // predict inputs and variances of EVERY step (the reverse sweep needs them), the state cotangent, the VJP's cotangents
@@ -679,6 +802,52 @@ int pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R, const p
     rc = pg_check(pr, R, g);
     if (rc) return rc;
     return pg_run(pr, R, g, stream);
+}
+
+size_t pilco_particles_consistent_workspace_bytes(const pilco_particles* pr) {
+    if (!pr || !pt_sizes_ok(pr)) return 0;
+    const FsWs L = fs_ws_layout(pr);
+    return L.ok && L.pws_bytes ? L.total : 0;
+}
+
+// pt_step<0>, fs_predict<0>, fs_cond<0>, pt_step<1>, ..., fs_cond<H-1>, pt_step<H>: pt_step_kernel unchanged, reading
+// the step closure (mean, var) fs_cond_kernel leaves
+int pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t stream) {
+    int rc = pt_check_desc(pr);
+    if (rc) return rc;
+    if (!pr->ws) return PILCO_ERR_NULL;
+    if ((uintptr_t)pr->ws & 15) return PILCO_ERR_ALIGN;
+    const FsWs L = fs_ws_layout(pr);
+    if (!L.ok || L.pws_bytes == 0) return PILCO_ERR_DIM;
+    if (pr->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
+    rc = fs_predict_prepare();
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)pr->ws;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D;
+    const size_t PD = (size_t)P * D, slot = (size_t)Ds * P * pad64(pr->dyn.n);
+    PtDev a = pt_dev(pr);
+    a.mean = ws + L.mean; a.var = ws + L.var;
+    FsCond c;
+    c.P = P; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = pad64(pr->dyn.n); c.t = 0;
+    c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
+    c.xh = ws + L.xh; c.mu = ws + L.mu; c.s2 = ws + L.s2; c.W = ws + L.W; c.Kh = ws + L.Kh;
+    c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean; c.var = ws + L.var;
+    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds);
+    for (int t = 0; t <= H; ++t) {
+        a.t = t;
+        a.xt = ws + L.xh + (size_t)(t < H ? t : 0) * PD;
+        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        if (t == H) break;
+        rc = fs_predict_launch(st, &pr->dyn, P, a.xt, ws + L.mu, ws + L.s2, ws + L.W, ws + L.Kh + (size_t)t * slot,
+                               ws + L.pws);
+        if (rc) return rc;
+        c.t = t;
+        launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
+        CUDA_LAUNCH_CHECK();
+    }
+    return PILCO_OK;
 }
 
 }  // extern "C"

@@ -318,6 +318,194 @@ __global__ void __launch_bounds__(256, 2) gp_predict_vjp_kernel(VjpArgs a) {
     }
 }
 
+// ---- predict for the consistent particle sampler (pilco_particles_rollout_consistent, DESIGN.md section 14) ---------
+// gp_predict_kernel with two extra epilogue stores of values it already holds: W = K* iK (the C fragments) to
+// W[e, row, :] and the recomputed K* to Ks[e, row, :], both [ne, T, np] with zeros past n.  mean and var are bitwise
+// those of pilco_gp_predict at the same inputs (same main loop, same epilogue order, same reductions).
+struct FsPredArgs {
+    PredictArgs p;
+    double* W;                  // [ne, T, np]  K* iK
+    double* Ks;                 // [ne, T, np]  K*
+};
+
+// grid (nj, nrb, ne), 256 threads: gp_predict_kernel's decomposition
+__global__ void __launch_bounds__(256, 2) fs_predict_kernel(FsPredArgs fa) {
+    PDL_ENTRY();
+    const PredictArgs& a = fa.p;
+    extern __shared__ __align__(16) unsigned char pr_smem_raw[];
+    PredictSmem& sm = *reinterpret_cast<PredictSmem*>(pr_smem_raw);
+    const int jb = blockIdx.x, rb = blockIdx.y, z = blockIdx.z, e = a.e0 + z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int wm = (warp >> 2) * 16, wc = warp & 3, wn = wc * 64;
+    const int D = a.D, r0 = rb * PR_TR, j0 = jb * PR_JB;
+    const int jw = min(PR_JB, a.np - j0);
+    const bool active = wn < jw;
+    const double sf2 = a.sf2[e];
+    const double* iK = a.iK + (size_t)e * a.ldk * a.ldk;
+    for (int i = tid; i < PR_TR * MAXD; i += 256) {
+        const int r = i / MAXD, d = i % MAXD;
+        sm.x[i] = (r0 + r < a.T && d < D) ? a.Xs[(size_t)(r0 + r) * D + d] : 0.0;
+    }
+    if (tid < MAXD) sm.il[tid] = tid < D ? 1.0 / a.ell[(size_t)e * D + tid] : 0.0;
+    if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
+    __syncthreads();
+    // main loop: gp_predict_kernel's, kept as its own copy so that the predict kernel's code is not touched
+    const int nc = a.np / PR_KC;
+    auto issue = [&](int c) {
+        uint64_t* bar = &sm.bar[c & 1];
+        mbar_expect_tx(bar, (unsigned)(PR_KC * jw * sizeof(double)));
+        for (int k = 0; k < PR_KC; ++k)
+            tma_bulk_g2s(&sm.B[c & 1][k * PR_LDB], iK + (size_t)(c * PR_KC + k) * a.ldk + j0, (unsigned)(jw * sizeof(double)), bar);
+    };
+    auto kchunk = [&](int c) {
+        double* A = sm.A[c & 1];
+        for (int q = tid; q < PR_TR * PR_KC; q += 256) {
+            const int r = q / PR_KC, k = q % PR_KC, i = c * PR_KC + k;
+            double v = 0.0;
+            if (i < a.n && r0 + r < a.T) v = pr_kstar(&sm.x[r * MAXD], a.C + (size_t)i * D, sm.il, D, sf2);
+            A[r * PR_LDA + k] = v;
+        }
+    };
+    if (tid == 0) { issue(0); if (nc > 1) issue(1); }
+    kchunk(0);
+    double acc[8][4];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.0;
+    for (int c = 0; c < nc; ++c) {
+        __syncthreads();
+        if (tid == 0 && c >= 1 && c + 1 < nc) issue(c + 1);
+        if (c + 1 < nc) kchunk(c + 1);
+        mbar_wait(&sm.bar[c & 1], (unsigned)((c >> 1) & 1));
+        if (active) {
+            const double* A = sm.A[c & 1];
+            const double* B = sm.B[c & 1];
+            double af[8];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                af[2 * i] = A[(wm + g) * PR_LDA + t + 4 * i];
+                af[2 * i + 1] = A[(wm + g + 8) * PR_LDA + t + 4 * i];
+            }
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                double bf[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) bf[i] = B[(t + 4 * i) * PR_LDB + wn + 8 * q + g];
+                dmma16816(acc[q], af, bf);
+            }
+        }
+    }
+    // epilogue.  W (0 past n) goes to the free iK buffer and out to global memory as coalesced 16-byte rows; then
+    // gp_predict_kernel's sums in its order, with each thread's W entries read back from the buffer (the same values)
+    // and overwritten by K*, which goes out the same way.
+    __syncthreads();                                            // every warp is done with the last iK tile
+    double* cs = &sm.B[0][0];                                   // [PR_TR][PR_LDB]
+    const int jw2 = jw >> 1;
+    auto store_tile = [&](double* dst) {                        // cs rows < T, columns [0, jw) -> dst[z, r0 + r, j0 ..]
+        for (int i = tid; i < PR_TR * jw2; i += 256) {
+            const int r = i / jw2, c2 = i % jw2;
+            if (r0 + r < a.T)
+                *reinterpret_cast<double2*>(dst + ((size_t)z * a.T + r0 + r) * a.np + j0 + 2 * c2) =
+                    *reinterpret_cast<const double2*>(cs + r * PR_LDB + 2 * c2);
+        }
+    };
+    if (active) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+#pragma unroll
+                for (int o = 0; o < 2; ++o) {
+                    const int jl = wn + 8 * q + 2 * t + o;
+                    cs[(wm + g + 8 * h) * PR_LDB + jl] = j0 + jl < a.n ? acc[q][2 * h + o] : 0.0;
+                }
+    }
+    __syncthreads();
+    store_tile(fa.W);
+    __syncthreads();                                            // W is out before K* overwrites it
+    double qf[2] = {0.0, 0.0}, mp[2] = {0.0, 0.0};
+    if (active) {
+        const double* be = a.beta + (size_t)e * a.n;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = wm + g + 8 * h;
+            if (r0 + r < a.T) {
+                for (int q = 0; q < 8; ++q)
+#pragma unroll
+                    for (int o = 0; o < 2; ++o) {
+                        const int j = j0 + wn + 8 * q + 2 * t + o;
+                        double* c = &cs[r * PR_LDB + wn + 8 * q + 2 * t + o];
+                        double k = 0.0;
+                        if (j < a.n) {
+                            k = pr_kstar(&sm.x[r * MAXD], a.C + (size_t)j * D, sm.il, D, sf2);
+                            qf[h] = fma(*c, k, qf[h]);
+                            mp[h] = fma(k, be[j], mp[h]);
+                        }
+                        *c = k;
+                    }
+            }
+        }
+    }
+    __syncthreads();
+    store_tile(fa.Ks);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        qf[h] += __shfl_xor_sync(0xffffffffu, qf[h], 1);
+        qf[h] += __shfl_xor_sync(0xffffffffu, qf[h], 2);
+        mp[h] += __shfl_xor_sync(0xffffffffu, mp[h], 1);
+        mp[h] += __shfl_xor_sync(0xffffffffu, mp[h], 2);
+    }
+    if (t == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) { sm.red[wc][0][wm + g + 8 * h] = qf[h]; sm.red[wc][1][wm + g + 8 * h] = mp[h]; }
+    }
+    __syncthreads();
+    double* part = a.part + (((size_t)z * a.nrb + rb) * a.nj) * 2 * PR_TR;
+    if (tid < 2 * PR_TR) {
+        const int w = tid / PR_TR, r = tid % PR_TR;
+        part[(size_t)jb * 2 * PR_TR + tid] = ((sm.red[0][w][r] + sm.red[1][w][r]) + sm.red[2][w][r]) + sm.red[3][w][r];
+    }
+    if (!last_cta_arrives(a.cnt + (size_t)z * a.nrb + rb, (unsigned)a.nj)) return;
+    if (tid < PR_TR && r0 + tid < a.T) {
+        double qs = 0.0, ms = 0.0;
+        for (int b = 0; b < a.nj; ++b) { qs += part[(size_t)b * 2 * PR_TR + tid]; ms += part[(size_t)b * 2 * PR_TR + PR_TR + tid]; }
+        a.mean[(size_t)(r0 + tid) * a.ne + z] = ms;
+        a.var[(size_t)(r0 + tid) * a.ne + z] = sf2 - qs;
+    }
+}
+
+// one-time kernel attribute of fs_predict_kernel (before the consistent rollout enqueues anything)
+int fs_predict_prepare() {
+    static bool attr_set[PILCO_MAX_DEVICES] = {false};
+    bool& set = attr_set[pilco_current_device()];
+    if (!set) {
+        if (cudaFuncSetAttribute(fs_predict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PredictSmem))
+            != cudaSuccess)
+            return PILCO_ERR_LAUNCH;
+        set = true;
+    }
+    return PILCO_OK;
+}
+
+// all ne = E outputs of the validated model at T points (T <= 65535 * PR_TR); ws: pilco_gp_predict's diagonal workspace
+int fs_predict_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, double* mean, double* var,
+                      double* W, double* Ks, void* ws) {
+    const int n = gp->n, E = gp->E, np = pad64(n), nj = (np + PR_JB - 1) / PR_JB, nrb = (T + PR_TR - 1) / PR_TR;
+    FsPredArgs fa;
+    PredictArgs& a = fa.p;
+    a.n = n; a.D = gp->D; a.np = np; a.nj = nj; a.nrb = nrb; a.T = T; a.e0 = 0;
+    a.C = gp->X; a.ell = gp->ell; a.sf2 = gp->sf2; a.beta = gp->beta; a.iK = gp->iK; a.ldk = gp->ldk;
+    a.Xs = Xs; a.mean = mean; a.var = var; a.ne = E;
+    a.part = (double*)ws;
+    a.cnt = (unsigned*)((char*)ws + (size_t)E * nrb * nj * 2 * PR_TR * sizeof(double));
+    fa.W = W; fa.Ks = Ks;
+    cudaMemsetAsync(a.cnt, 0, (size_t)E * nrb * sizeof(unsigned), st);
+    const dim3 grid(nj, nrb, E);
+    launch_pri(pilco_small_grid(grid), fs_predict_kernel, grid, dim3(256), sizeof(PredictSmem), st, fa);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
 static size_t pr_vjp_bytes(int np, int D, int E, int T) {
     const size_t nj = (size_t)(np + PR_JB - 1) / PR_JB, nrb = (size_t)(T + PR_TR - 1) / PR_TR;
     const size_t part = (size_t)E * nrb * nj * PR_TR * D * sizeof(double);

@@ -502,15 +502,22 @@ class ParticlePlan:
 
     A batch of policies (``R > 1``, or an RBF policy factorised with a leading batch dimension) takes a policy spec
     with a leading R, as ``RolloutPlan`` does, and needs ``grad=True``: ``launch_grad()`` then runs the R policies over
-    the same x0 and eps (pilco_particles_rollout_batch_grad) and every output has a leading R."""
+    the same x0 and eps (pilco_particles_rollout_batch_grad) and every output has a leading R.
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1):
+    ``consistent=True``: ``launch()`` samples each particle's dynamics as ONE function drawn from the GP posterior
+    (pilco_particles_rollout_consistent, DESIGN.md section 14) instead of fresh noise at every step; its workspace is
+    O(P H E n).  It has no gradient path: ``grad=True`` with ``consistent=True`` is a ValueError."""
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False):
         d = device()
         self.P, self.H, self.R = int(P), int(H), int(R)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
         P, H, Ds, U, R = self.P, self.H, self.Ds, self.U, self.R
         if P < 1 or H < 0 or R < 1:
             raise ValueError("particles: needs P >= 1, H >= 0 and R >= 1 (P=%d, H=%d, R=%d)" % (P, H, R))
+        self.consistent = bool(consistent)
+        if self.consistent and grad:
+            raise ValueError("particles: the consistent (function-sample) rollout has no gradient path (grad=True)")
         rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
         self.batched = R > 1 or rbf_batched
         if self.batched and not grad:
@@ -558,7 +565,13 @@ class ParticlePlan:
         pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
         pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
         pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
-        if not self.batched:                                    # the forward-only rollout (a batch has none)
+        if self.consistent:
+            wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
+            if wsb == 0:
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        elif not self.batched:                                  # the forward-only rollout (a batch has none)
             wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
@@ -611,6 +624,9 @@ class ParticlePlan:
     def launch(self):
         if self.batched:
             raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
+        if self.consistent:
+            check(lib.pilco_particles_rollout_consistent(C.byref(self.pr), stream_ptr()), "particles_rollout_consistent")
+            return
         check(lib.pilco_particles_rollout(C.byref(self.pr), stream_ptr()), "particles_rollout")
 
     def outputs(self):
@@ -638,18 +654,70 @@ def gp_predict_vjp(gp, Xs, gmean, gvar):
     return out
 
 
-def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0):
+def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
-    step_risk [P,H], ret [P]) device tensors."""
+    step_risk [P,H], ret [P]) device tensors.
+
+    ``consistent=True``: pilco_particles_rollout_consistent, one posterior function per particle.  Its workspace is
+    O(P H E n), so the particles run in chunks whose workspace fits ``max_ws_bytes`` (default: half the free device
+    memory).  A particle's outputs do not depend on its batch, so the chunking does not change them."""
     x0, eps = dev(x0), dev(eps)
     if x0.dim() != 2 or eps.dim() != 3 or eps.shape[0] != x0.shape[0] or eps.shape[2] != x0.shape[1]:
         raise ValueError("particles_rollout: x0 must be [P,Ds] and eps [P,H,Ds], got %s and %s"
                          % (tuple(x0.shape), tuple(eps.shape)))
+    if consistent:
+        return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes)
     plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu)
     plan.set_inputs(x0, eps)
     plan.launch()
     return plan.outputs()
+
+
+def consistent_workspace_bytes(dyn, Ds, U, P, H):
+    """pilco_particles_consistent_workspace_bytes of P particles over H steps (0: unsupported sizes)"""
+    pr = _lib.Particles()
+    pr.P, pr.H = int(P), int(H)
+    pr.dyn = dyn.struct()
+    pr.pol.Ds, pr.pol.U = int(Ds), int(U)
+    return int(lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)))
+
+
+def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes):
+    P, H = int(x0.shape[0]), int(eps.shape[1])
+    Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
+    if max_ws_bytes is None:
+        max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+    fits = lambda p: 0 < consistent_workspace_bytes(dyn, Ds, U, p, H) <= max_ws_bytes
+    if not fits(1):
+        raise ValueError("particles_rollout: the consistent rollout of one particle (H=%d, n=%d) needs %d workspace "
+                         "bytes, more than max_ws_bytes=%d" % (H, dyn.n, consistent_workspace_bytes(dyn, Ds, U, 1, H),
+                                                               max_ws_bytes))
+    lo, hi = 1, P                                           # the largest chunk that fits: bisection
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    if lo == P:
+        plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True)
+        plan.set_inputs(x0, eps)
+        plan.launch()
+        return plan.outputs()
+    d = device()
+    Hb = max(H, 1)
+    out = (torch.empty((P, H + 1, Ds), dtype=F64, device=d), torch.empty((P, Hb, U), dtype=F64, device=d)[:, :H],
+           torch.empty((P, Hb), dtype=F64, device=d)[:, :H], torch.empty((P, Hb), dtype=F64, device=d)[:, :H],
+           torch.empty(P, dtype=F64, device=d))
+    plan = None
+    for p0 in range(0, P, lo):
+        p1 = min(P, p0 + lo)
+        if plan is None or plan.P != p1 - p0:
+            plan = None                                     # free the previous chunk's workspace first
+            plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True)
+        plan.set_inputs(x0[p0:p1], eps[p0:p1])
+        plan.launch()
+        for o, c in zip(out, plan.outputs()):
+            o[p0:p1].copy_(c)
+    return out
 
 
 class PredictPlan:

@@ -132,7 +132,7 @@ class PILCO:
         M, S, _ = self.predict(m_x, s_x, 1)
         return M, S
 
-    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None):
+    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
         """Monte Carlo rollouts of the learnt dynamics under the policy, to check what ``predict``'s moment matching
         approximates: ``num_samples`` particles start at x0 ~ N(m_x, s_x) and take n steps of
         x_{t+1} = x_t + mu(x_t, u_t) + sqrt(var(x_t, u_t)) eps_t with the latent GP posterior mean and variance,
@@ -140,10 +140,25 @@ class PILCO:
         ``predict``'s reward is their mean).  Every draw comes from one device ``torch.Generator``; with
         ``seed=None`` its seed is drawn from ``np.random``.  s_x may be singular (a known start state: s_x = 0).
 
+        ``consistent=True``: each particle follows ONE function drawn from the GP posterior, conditioned at every step
+        on the particle's own earlier inputs (a state region visited twice has the same dynamics both times), as the
+        PILCO papers' sampled trajectories do; the step-wise default draws fresh noise at every step.  The same seed
+        gives the same x0 and normals, so step 0 is the same in both.  Its device workspace grows as
+        num_samples n^2 (and n times the model's centres); large batches run in chunks.
+
         -> ParticleTrajectories(states [S,n+1,Ds], actions [S,n,U], rewards [S,n], risks [S,n], returns [S]) of
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
         from ..params import HostArray
+        if consistent:
+            import torch
+            dyn = self.mgpr.device_gp()
+            x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, "sample_trajectories")
+            if eps is None:                                     # n = 0
+                eps = torch.zeros((int(num_samples), 0, self.state_dim), dtype=engine.F64, device=x0.device)
+            terms, mult_mu = self.reward_spec()
+            out = engine.particles_rollout(dyn, self.policy_spec(), terms, x0, eps, mult_mu=mult_mu, consistent=True)
+            return ParticleTrajectories(*[t.cpu().numpy().view(HostArray) for t in out])
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_trajectories")
         plan.launch()
         out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
