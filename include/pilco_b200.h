@@ -375,6 +375,19 @@ int    pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R,
 size_t pilco_particles_consistent_workspace_bytes(const pilco_particles* pr);   /* 0: unsupported sizes or overflow */
 int    pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t stream);
 
+/* The consistent rollout of R policies and the pathwise gradient of each one's mean return (DESIGN.md section 15):
+ * pilco_particles_rollout_batch_grad's contract (shared x0 and eps, the policy's batch strides honoured, 0 sharing an
+ * array, restart-major outputs, the gradient in pilco_particles_grad) with the particles of
+ * pilco_particles_rollout_consistent.  Its forward outputs are bitwise those of pilco_particles_rollout_consistent with
+ * the same policy; R = 1 with an unbatched policy is the single-policy call.  Validation and status codes are those of
+ * pilco_particles_rollout_batch_grad and pilco_particles_rollout_consistent; g->ws is sized by
+ * pilco_particles_consistent_grad_workspace_bytes: the consistent forward's at R P particles + O(R P H^2 E).  Every
+ * sum has a fixed order, so a restart's results are bitwise independent of R and reproducible run to run; a pivot the
+ * forward declares degenerate holds its step's own noise constant.  No host synchronisation (graph-capturable). */
+size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr, int R);  /* 0: unsupported / overflow */
+int    pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
+                                               pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -422,16 +422,17 @@ __global__ void __launch_bounds__(128) pg_rbf_finish_kernel(PgRed a) {
 #define FS_TAU   1e-10
 #define FS_WARPS 8                      // warps (particles) per CTA of fs_cond_kernel
 
+// Buffers have T = R P rows (restart r's particle p is row r P + p, as section 13); eps is shared by the restarts.
 struct FsCond {
-    int P, H, D, Ds, n, np, t;
+    int P, T, H, D, Ds, n, np, t;
     const double* ell; const double* sf2;               // dynamics [E,D], [E]
-    const double* xh;                                   // [H,P,D] predict inputs of the steps so far
-    const double* mu; const double* s2;                 // [P,Ds] the posterior mean and variance at x~_t
-    const double* W;                                    // [E,P,np] W_t = K*_t iK
-    const double* Kh;                                   // [H,E,P,np] K*_s of every step
+    const double* xh;                                   // [H,T,D] predict inputs of the steps so far
+    const double* mu; const double* s2;                 // [T,Ds] the posterior mean and variance at x~_t
+    const double* W;                                    // [E,T,np] W_t = K*_t iK
+    const double* Kh;                                   // [H,E,T,np] K*_s of every step
     const double* eps;                                  // [P,H,Ds]
-    double* L;                                          // [H(H+1)/2, E, P] packed rows; (s, r) at s(s+1)/2 + r
-    double* mean; double* var;                          // [P,Ds] what pt_step_kernel closes the step with
+    double* L;                                          // [H(H+1)/2, E, T] packed rows; (s, r) at s(s+1)/2 + r
+    double* mean; double* var;                          // [T,Ds] what pt_step_kernel closes the step with
 };
 
 __device__ __forceinline__ double fs_bfly(double v) {   // fixed butterfly: every lane ends with the same bits
@@ -440,18 +441,19 @@ __device__ __forceinline__ double fs_bfly(double v) {   // fixed butterfly: ever
     return v;
 }
 
-// grid (ceil(P / FS_WARPS), E), one warp per (particle p, output e): step t's conditioning on the particle's past.
-// The packed diagonal holds the pivot later substitutions divide by: sqrt(d2), or 0 for a degenerate column.
+// grid (ceil(P / FS_WARPS), E, R), one warp per (particle p of restart r = blockIdx.z, output e): step t's conditioning
+// on the particle's past.  The packed diagonal holds the pivot later substitutions divide by: sqrt(d2), or 0 for a
+// degenerate column.
 __global__ void __launch_bounds__(FS_WARPS * 32, 4) fs_cond_kernel(FsCond a) {
     PDL_ENTRY();
     const int lane = threadIdx.x & 31, p = blockIdx.x * FS_WARPS + (threadIdx.x >> 5), e = blockIdx.y;
     if (p >= a.P) return;
     const int D = a.D, Ds = a.Ds, t = a.t, n = a.n;
-    const size_t P = a.P, EP = (size_t)Ds * P, pe = (size_t)e * P + p;
+    const size_t T = a.T, row = (size_t)blockIdx.z * a.P + p, EP = (size_t)Ds * T, pe = (size_t)e * T + row;
     const double sf2 = a.sf2[e];
     // lane d < D holds dimension d of x~_t and 1 / ell_ed
     const bool dl = lane < D;
-    const double xd = dl ? a.xh[((size_t)t * P + p) * D + lane] : 0.0;
+    const double xd = dl ? a.xh[((size_t)t * T + row) * D + lane] : 0.0;
     const double ild = dl ? 1.0 / a.ell[(size_t)e * D + lane] : 0.0;
     double* Lt = a.L + (size_t)t * (t + 1) / 2 * EP + pe;              // row t: entry s at Lt[s EP]
     const double* __restrict__ Wr = a.W + pe * a.np;
@@ -461,7 +463,7 @@ __global__ void __launch_bounds__(FS_WARPS * 32, 4) fs_cond_kernel(FsCond a) {
         double dot = 0.0;
 #pragma unroll 4
         for (int j = lane; j < n; j += 32) dot = fma(Wr[j], Kr[j], dot);
-        const double q = dl ? (xd - a.xh[((size_t)s * P + p) * D + lane]) * ild : 0.0;
+        const double q = dl ? (xd - a.xh[((size_t)s * T + row) * D + lane]) * ild : 0.0;
         dot = fs_bfly(dot);
         const double d2 = fs_bfly(q * q);
         const double c = sf2 * exp(-0.5 * d2) - dot;
@@ -490,12 +492,103 @@ __global__ void __launch_bounds__(FS_WARPS * 32, 4) fs_cond_kernel(FsCond a) {
     ssq = fs_bfly(ssq);
     sme = fs_bfly(sme);
     if (lane == 0) {
-        const size_t o = (size_t)p * Ds + e;
+        const size_t o = row * Ds + e;
         const double mu = a.mu[o], d2 = a.s2[o] - ssq;
         Lt[(size_t)t * EP] = d2 > FS_TAU * sf2 ? sqrt(d2) : 0.0;
         a.mean[o] = t > 0 ? mu + sme : mu;              // t = 0: the marginal sampler's step exactly
         a.var[o] = d2 < 0.0 ? 0.0 : d2;                 // NaN stays NaN
     }
+}
+
+// ---- reverse of the conditioning (pilco_particles_rollout_consistent_grad, DESIGN.md section 15) -------------------
+// Per (particle, output) at reverse step t, given m_bar = the cotangent of mean'_t and v_bar = that of var'_t, with the
+// packed cotangent rows G (Lambda of the factor rows, accumulated by the later steps; zero at the start):
+//   d2_bar = piv_t > 0 ? v_bar + Lambda_tt / (2 piv_t) : 0         (tau rule: a degenerate step's own noise is constant)
+//   l_bar_s = Lambda_ts + m_bar eps_s - 2 d2_bar l_ts
+//   s = t-1 .. 0:  c_s = l_bar_s / piv_s (0 where piv_s = 0);  Lambda_ss -= c_s l_ts;
+//                  r < s:  l_bar_r -= c_s l_sr,  Lambda_sr -= c_s l_tr
+// Row t of G then holds c_t. = G_t., the cotangent of the cross-covariance k_post(x~_t, x~_s); the entries s > t are in
+// rows s (written by the earlier reverse steps).  Out: a_t = -2 d2_bar K*_t - sum_{s != t} G_ts K*_s and the direct
+// sum sum_{s != t} G_ts k_e(x~_t, x~_s) (x~_s - x~_t), for fs_predict_vjp_kernel.
+struct FsBwd {
+    int P, T, H, D, Ds, np, t;
+    const double* ell; const double* sf2;               // dynamics [E,D], [E]
+    const double* xh;                                   // [H,T,D] predict inputs of every step
+    const double* Kh;                                   // [H,E,T,np] K*_s of every step
+    const double* L;                                    // [H(H+1)/2, E, T] the forward's packed rows
+    const double* eps;                                  // [P,H,Ds]
+    const double* gx; const double* gvar;               // [T,Ds] m_bar_t, v_bar_t
+    double* G;                                          // [H(H+1)/2, E, T] Lambda, then c (one buffer)
+    double* A;                                          // [E,T,np] a_t
+    double* dir;                                        // [E,T,D] the direct sums
+};
+
+// grid (ceil(P / FS_WARPS), E, R), one warp per (particle p of restart r = blockIdx.z, output e), as fs_cond_kernel
+__global__ void __launch_bounds__(FS_WARPS * 32, 3) fs_cond_bwd_kernel(FsBwd a) {
+    PDL_ENTRY();
+    const int lane = threadIdx.x & 31, p = blockIdx.x * FS_WARPS + (threadIdx.x >> 5), e = blockIdx.y;
+    if (p >= a.P) return;
+    const int D = a.D, Ds = a.Ds, t = a.t, H = a.H, np = a.np;
+    const size_t T = a.T, row = (size_t)blockIdx.z * a.P + p, EP = (size_t)Ds * T, pe = (size_t)e * T + row;
+    const double* Lt = a.L + (size_t)t * (t + 1) / 2 * EP + pe;        // row t: entry s at [s EP]
+    double* Gt = a.G + (size_t)t * (t + 1) / 2 * EP + pe;
+    const double piv = Lt[(size_t)t * EP];
+    const size_t o = row * Ds + e;
+    const double mb = a.gx[o];
+    const double db = piv > 0.0 ? a.gvar[o] + Gt[(size_t)t * EP] / (2.0 * piv) : 0.0;
+    const double* ep = a.eps + (size_t)p * H * Ds + e;
+    for (int s = lane; s < t; s += 32)
+        Gt[(size_t)s * EP] = fma(-2.0 * db, Lt[(size_t)s * EP], fma(mb, ep[(size_t)s * Ds], Gt[(size_t)s * EP]));
+    __syncwarp();
+    // reverse of the forward substitution, s = t-1 .. 0
+    for (int s = t - 1; s >= 0; --s) {
+        const double* Ls = a.L + (size_t)s * (s + 1) / 2 * EP + pe;
+        double* Gs = a.G + (size_t)s * (s + 1) / 2 * EP + pe;
+        const double ps = Ls[(size_t)s * EP];
+        const double c = ps > 0.0 ? Gt[(size_t)s * EP] / ps : 0.0;
+        for (int r = lane; r < s; r += 32) {
+            Gt[(size_t)r * EP] = fma(-c, Ls[(size_t)r * EP], Gt[(size_t)r * EP]);
+            Gs[(size_t)r * EP] = fma(-c, Lt[(size_t)r * EP], Gs[(size_t)r * EP]);
+        }
+        __syncwarp();                                   // every lane has read l_bar_s before it is overwritten
+        if (lane == 0) {
+            Gs[(size_t)s * EP] = fma(-c, Lt[(size_t)s * EP], Gs[(size_t)s * EP]);
+            Gt[(size_t)s * EP] = c;
+        }
+        __syncwarp();
+    }
+    // G_ts of step s (s < t: row t; s > t: row s, entry t); 0 at s = t
+    auto gts = [&](int s) -> double {
+        return s < t ? Gt[(size_t)s * EP] : s > t ? a.G[((size_t)s * (s + 1) / 2 + t) * EP + pe] : 0.0;
+    };
+    // a_t: lanes stride the columns, 128 at a time; the slots are summed in order
+    const double* Kp = a.Kh + pe * np;
+    double* Ar = a.A + pe * np;
+    for (int j0 = 0; j0 < np; j0 += 128) {
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};
+        for (int s = 0; s < H; ++s) {
+            const double gs = s == t ? -2.0 * db : -gts(s);
+            const double* Kr = Kp + (size_t)s * EP * np + j0 + lane;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) if (j0 + 32 * i + lane < np) acc[i] = fma(gs, Kr[32 * i], acc[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) if (j0 + 32 * i + lane < np) Ar[j0 + 32 * i + lane] = acc[i];
+    }
+    // the direct sum: lane d < D holds dimension d, the kernel distance is fs_cond_kernel's butterfly
+    const bool dl = lane < D;
+    const double xd = dl ? a.xh[((size_t)t * T + row) * D + lane] : 0.0;
+    const double ild = dl ? 1.0 / a.ell[(size_t)e * D + lane] : 0.0;
+    const double sf2 = a.sf2[e];
+    double ds = 0.0;
+    for (int s = 0; s < H; ++s) {
+        if (s == t) continue;
+        const double xs = dl ? a.xh[((size_t)s * T + row) * D + lane] : 0.0;
+        const double q = dl ? (xd - xs) * ild : 0.0;
+        const double k = sf2 * exp(-0.5 * fs_bfly(q * q));
+        ds = fma(gts(s) * k, xs - xd, ds);
+    }
+    if (dl) a.dir[pe * D + lane] = ds;
 }
 
 struct PtWs { size_t xt, mean, var, pws, pws_bytes, total; };     // offsets in doubles; total and pws_bytes in bytes
@@ -658,12 +751,63 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
                           const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
 
-// the gradient's arguments and workspace, after pt_check_desc
-static int pg_check(const pilco_particles* pr, int R, const pilco_particles_grad* g) {
+// the reverse sweep's per-particle arguments (everything but the step, the workspace buffers and gxt / var_prev)
+static PgDev pg_dev(const pilco_particles* pr, const PtDev& a) {
+    const pilco_policy& pol = pr->pol;
+    PgDev b;
+    b.P = pr->P; b.H = pr->H; b.Ds = pol.Ds; b.U = pol.U;
+    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
+    b.W = pol.W; b.b = pol.b;
+    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
+    b.W_bs = a.W_bs; b.b_bs = a.b_bs; b.C_bs = a.C_bs; b.ell_bs = a.ell_bs; b.sf2_bs = a.sf2_bs; b.beta_bs = a.beta_bs;
+    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
+    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
+    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
+    return b;
+}
+
+// value and the policy-parameter gradient over all P H points of each restart, fixed order, from z_bar [R P,H,U]
+static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtDev& a, double* zbar,
+                     double* s1, double* s2, double* gbeta, double* gy, cudaStream_t st) {
+    const pilco_policy& pol = pr->pol;
+    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    const int Ds = pol.Ds, U = pol.U;
+    PgRed r;
+    r.P = pr->P; r.H = pr->H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
+    r.traj = pr->traj; r.zbar = zbar; r.ret = pr->ret;
+    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
+    r.C_bs = a.C_bs; r.ell_bs = a.ell_bs; r.sf2_bs = a.sf2_bs; r.beta_bs = a.beta_bs;
+    r.gW = g->gW; r.gb = g->gb;
+    r.s1 = s1; r.s2 = s2; r.gbeta = gbeta;
+    r.gXc = g->gXc; r.gell = g->gell;
+    r.value = g->value;
+    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1, R), dim3(256), 0, st, r);
+    CUDA_LAUNCH_CHECK();
+    if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
+        const int bf = r.bf, ldw = pad64(bf);
+        launch_hi(pg_rbf_finish_kernel, dim3(R), dim3(128), 0, st, r);
+        CUDA_LAUNCH_CHECK();
+        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
+                              gbeta, (long long)U * bf, bf, 1, gy, bf);
+        const int rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, pol.rbf.X, a.C_bs, pol.rbf.ell, a.ell_bs, pol.rbf.sf2,
+                                             a.sf2_bs, pol.rbf.beta, a.beta_bs, gy, g->gXc, g->gYc, g->gell);
+        if (rc) return rc;
+    }
+    return PILCO_OK;
+}
+
+// the gradient's output and workspace pointers, after pt_check_desc
+static int pg_check_ptrs(const pilco_particles* pr, const pilco_particles_grad* g) {
     if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
     const bool rbf = pr->pol.kind == PILCO_POLICY_RBF;
     if (rbf ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
     if ((uintptr_t)g->ws & 15) return PILCO_ERR_ALIGN;
+    return PILCO_OK;
+}
+
+// the gradient's arguments and workspace, after pt_check_desc
+static int pg_check(const pilco_particles* pr, int R, const pilco_particles_grad* g) {
+    if (const int rc = pg_check_ptrs(pr, g)) return rc;
     const PgWs L = pg_ws_layout(pr, R);
     if (L.pws_bytes == 0) return PILCO_ERR_DIM;
     if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
@@ -676,7 +820,6 @@ static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
     cudaStream_t st = (cudaStream_t)stream;
     double* ws = (double*)g->ws;
     const pilco_policy& pol = pr->pol;
-    const bool rbf = pol.kind == PILCO_POLICY_RBF;
     const int P = pr->P, H = pr->H, Ds = pol.Ds, U = pol.U, D = Ds + U, T = R * P;
     const size_t PD = (size_t)T * D, PDs = (size_t)T * Ds;
     const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R);
@@ -696,15 +839,7 @@ static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
         if (rc) return rc;
     }
     // reverse sweep
-    PgDev b;
-    b.P = P; b.H = H; b.Ds = Ds; b.U = U;
-    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
-    b.W = pol.W; b.b = pol.b;
-    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
-    b.W_bs = a.W_bs; b.b_bs = a.b_bs; b.C_bs = a.C_bs; b.ell_bs = a.ell_bs; b.sf2_bs = a.sf2_bs; b.beta_bs = a.beta_bs;
-    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
-    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
-    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
+    PgDev b = pg_dev(pr, a);
     b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
     for (int t = H - 1; t >= 0; --t) {
         b.t = t;
@@ -719,29 +854,106 @@ static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
         launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
         CUDA_LAUNCH_CHECK();
     }
-    // value and the policy-parameter gradient over all P H points of each restart, fixed order
-    PgRed r;
-    r.P = P; r.H = H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
-    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
-    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
-    r.C_bs = a.C_bs; r.ell_bs = a.ell_bs; r.sf2_bs = a.sf2_bs; r.beta_bs = a.beta_bs;
-    r.gW = g->gW; r.gb = g->gb;
-    r.s1 = ws + L.s1; r.s2 = ws + L.s2; r.gbeta = ws + L.gbeta;
-    r.gXc = g->gXc; r.gell = g->gell;
-    r.value = g->value;
-    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1, R), dim3(256), 0, st, r);
-    CUDA_LAUNCH_CHECK();
-    if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
-        const int bf = r.bf, ldw = pad64(bf);
-        launch_hi(pg_rbf_finish_kernel, dim3(R), dim3(128), 0, st, r);
+    return pg_reduce(pr, R, g, a, ws + L.zbar, ws + L.s1, ws + L.s2, ws + L.gbeta, ws + L.gy, st);
+}
+
+int fs_vjp_prepare();
+int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, const double* gmean,
+                  const double* A, const double* dir, double* gXs, void* ws);
+
+// workspace of the consistent gradient for R restarts (offsets in doubles; total and vws_bytes in bytes; ok = false on
+// size_t overflow): the consistent forward's at T = R P (its W slot holds a_t in the reverse sweep), then the var'
+// history [H,T,Ds], the packed cotangent rows [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the
+// VJP output [T,D], z_bar [T,H,U], the RBF sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T
+struct FgWs { FsWs f; size_t varh, G, dir, gx, gvar, gxt, zbar, s1, s2, gbeta, gy, vws, vws_bytes, total; bool ok; };
+
+static FgWs fg_ws_layout(const pilco_particles* pr, int R) {
+    FgWs L = {};
+    pilco_particles q = *pr;
+    q.P = R * pr->P;                                    // pt_batch_ok: R P <= PT_MAX_P
+    L.f = fs_ws_layout(&q);
+    L.ok = L.f.ok && L.f.pws_bytes;
+    if (!L.ok) return L;
+    const size_t T = q.P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+    const size_t bf = pr->pol.kind == PILCO_POLICY_RBF ? pr->pol.rbf.n : 0;
+    size_t vh, gl, dr, zb, rb, rs;
+    L.ok = fs_mul(H * T, Ds, vh) && fs_mul(H * (H + 1) / 2, T * Ds, gl) && fs_mul(T * Ds, D, dr) &&
+           fs_mul(T * H, U, zb) && fs_mul((size_t)R * U, bf, rb) && fs_mul(rb, Ds, rs);
+    if (!L.ok) return L;
+    size_t o = L.f.total / sizeof(double);              // f.total: a multiple of 16 bytes
+    auto take = [&](size_t len) {
+        const size_t at = o;
+        if (len == SIZE_MAX || __builtin_add_overflow(o, len + (len & 1), &o)) L.ok = false;
+        return at;
+    };
+    L.varh = take(vh); L.G = take(gl); L.dir = take(dr);
+    L.gx = take(T * Ds); L.gvar = take(T * Ds); L.gxt = take(T * D); L.zbar = take(zb);
+    L.s1 = take(rs); L.s2 = take(rs); L.gbeta = take(rb); L.gy = take(rb);
+    L.vws = o;
+    L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
+    size_t b = 0;
+    if (!L.ok || !L.vws_bytes || !fs_mul(o, sizeof(double), b) || __builtin_add_overflow(b, L.vws_bytes, &L.total))
+        L.ok = false;
+    return L;
+}
+
+// the consistent forward at T = R P with var' kept per step, then the reverse sweep (DESIGN.md section 15):
+//   pg_step<H-1>, [fs_cond_bwd<t>, fs_vjp<t>, pg_step<t>] for t = H-2 .. 0, then pg_reduce's launches
+static int fg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
+    const FgWs L = fg_ws_layout(pr, R);
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)g->ws;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
+    const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = (size_t)Ds * T * np;
+    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
+    int rc;
+    PtDev a = pt_dev(pr);
+    a.mean = ws + L.f.mean;
+    FsCond c;
+    c.P = P; c.T = T; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = np; c.t = 0;
+    c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
+    c.xh = ws + L.f.xh; c.mu = ws + L.f.mu; c.s2 = ws + L.f.s2; c.W = ws + L.f.W; c.Kh = ws + L.f.Kh;
+    c.eps = pr->eps; c.L = ws + L.f.L; c.mean = ws + L.f.mean;
+    for (int t = 0; t <= H; ++t) {
+        a.t = t;
+        a.xt = ws + L.f.xh + (size_t)(t < H ? t : 0) * TD;
+        a.var = ws + L.varh + (size_t)(t > 0 ? t - 1 : 0) * TDs;
+        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
-        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              ws + L.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
-        rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, pol.rbf.X, a.C_bs, pol.rbf.ell, a.ell_bs, pol.rbf.sf2, a.sf2_bs,
-                                   pol.rbf.beta, a.beta_bs, ws + L.gy, g->gXc, g->gYc, g->gell);
+        if (t == H) break;
+        rc = fs_predict_launch(st, &pr->dyn, T, a.xt, ws + L.f.mu, ws + L.f.s2, ws + L.f.W, ws + L.f.Kh + (size_t)t * slot,
+                               ws + L.f.pws);
         if (rc) return rc;
+        c.t = t;
+        c.var = ws + L.varh + (size_t)t * TDs;
+        launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
+        CUDA_LAUNCH_CHECK();
     }
-    return PILCO_OK;
+    // reverse sweep; the cotangent rows accumulate from zero
+    if (H > 1) cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TDs * sizeof(double), st);
+    PgDev b = pg_dev(pr, a);
+    b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
+    FsBwd q;
+    q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = Ds; q.np = np; q.t = 0;
+    q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
+    q.xh = ws + L.f.xh; q.Kh = ws + L.f.Kh; q.L = ws + L.f.L; q.eps = pr->eps;
+    q.gx = b.gx; q.gvar = b.gvar; q.G = ws + L.G; q.A = ws + L.f.W; q.dir = ws + L.dir;
+    for (int t = H - 1; t >= 0; --t) {
+        b.t = t;
+        b.gxt = nullptr;
+        if (t < H - 1) {
+            q.t = t;
+            launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
+            CUDA_LAUNCH_CHECK();
+            rc = fs_vjp_launch(st, &pr->dyn, T, ws + L.f.xh + (size_t)t * TD, b.gx, q.A, q.dir, ws + L.gxt, ws + L.vws);
+            if (rc) return rc;
+            b.gxt = ws + L.gxt;
+        }
+        b.var_prev = t > 0 ? ws + L.varh + (size_t)(t - 1) * TDs : nullptr;
+        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
+        CUDA_LAUNCH_CHECK();
+    }
+    return pg_reduce(pr, R, g, a, ws + L.zbar, ws + L.s1, ws + L.s2, ws + L.gbeta, ws + L.gy, st);
 }
 
 extern "C" {
@@ -829,7 +1041,7 @@ int pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t
     PtDev a = pt_dev(pr);
     a.mean = ws + L.mean; a.var = ws + L.var;
     FsCond c;
-    c.P = P; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = pad64(pr->dyn.n); c.t = 0;
+    c.P = P; c.T = P; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = pad64(pr->dyn.n); c.t = 0;
     c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
     c.xh = ws + L.xh; c.mu = ws + L.mu; c.s2 = ws + L.s2; c.W = ws + L.W; c.Kh = ws + L.Kh;
     c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean; c.var = ws + L.var;
@@ -848,6 +1060,29 @@ int pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t
         CUDA_LAUNCH_CHECK();
     }
     return PILCO_OK;
+}
+
+size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr, int R) {
+    if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    const FgWs L = fg_ws_layout(pr, R);
+    return L.ok ? L.total : 0;
+}
+
+int pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
+                                            pilco_stream_t stream) {
+    int rc = pt_check_desc(pr, true);
+    if (rc) return rc;
+    if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
+    rc = pg_check_ptrs(pr, g);
+    if (rc) return rc;
+    const FgWs L = fg_ws_layout(pr, R);
+    if (!L.ok) return PILCO_ERR_DIM;
+    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
+    rc = fs_predict_prepare();
+    if (rc) return rc;
+    rc = fs_vjp_prepare();
+    if (rc) return rc;
+    return fg_run(pr, R, g, stream);
 }
 
 }  // extern "C"

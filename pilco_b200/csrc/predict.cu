@@ -506,6 +506,178 @@ int fs_predict_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const do
     return PILCO_OK;
 }
 
+// ---- VJP for the gradient of the consistent sampler (pilco_particles_rollout_consistent_grad, DESIGN.md section 15) --
+//   gx = sum_e ell_e^-2 o (sum_n c_en (c_n - x) + dir_e),   c_en = k_en (gmean_e beta_en + [a_e iK_e]_n)
+// gp_predict_vjp_kernel with the row a_e (fs_cond_bwd_kernel: -2 var_bar K* - sum_s G_s K*_s) as the A operand of the
+// main loop instead of K*, so the contraction gives a iK directly, and the per-output direct sums dir_e of the
+// cross-covariance terms added by the last-arriving CTA before ell_e^-2.
+struct FsVjpArgs {
+    VjpArgs v;                  // gvar unused: it is folded into A
+    const double* A;            // [E, T, np]  a rows, zeros past n
+    const double* dir;          // [E, T, D]   direct sums
+};
+
+// grid (nj, nrb, E), 256 threads: gp_predict_vjp_kernel's decomposition
+__global__ void __launch_bounds__(256, 2) fs_predict_vjp_kernel(FsVjpArgs fa) {
+    PDL_ENTRY();
+    const VjpArgs& a = fa.v;
+    extern __shared__ __align__(16) unsigned char pr_smem_raw[];
+    VjpSmem& sm = *reinterpret_cast<VjpSmem*>(pr_smem_raw);
+    const int jb = blockIdx.x, rb = blockIdx.y, e = blockIdx.z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    const int wm = (warp >> 2) * 16, wc = warp & 3, wn = wc * 64;
+    const int D = a.D, r0 = rb * PR_TR, j0 = jb * PR_JB;
+    const int jw = min(PR_JB, a.np - j0);
+    const bool active = wn < jw;
+    const double sf2 = a.sf2[e];
+    const double* iK = a.iK + (size_t)e * a.ldk * a.ldk;
+    const double* Ae = fa.A + (size_t)e * a.T * a.np;
+    for (int i = tid; i < PR_TR * MAXD; i += 256) {
+        const int r = i / MAXD, d = i % MAXD;
+        sm.x[i] = (r0 + r < a.T && d < D) ? a.Xs[(size_t)(r0 + r) * D + d] : 0.0;
+    }
+    if (tid < MAXD) sm.il[tid] = tid < D ? 1.0 / a.ell[(size_t)e * D + tid] : 0.0;
+    if (tid < PR_TR) sm.gm[tid] = r0 + tid < a.T ? a.gmean[(size_t)(r0 + tid) * a.E + e] : 0.0;
+    if (tid == 0) { mbar_init(&sm.bar[0], 1); mbar_init(&sm.bar[1], 1); mbar_fence_init(); }
+    __syncthreads();
+    const int nc = a.np / PR_KC;
+    auto issue = [&](int c) {
+        uint64_t* bar = &sm.bar[c & 1];
+        mbar_expect_tx(bar, (unsigned)(PR_KC * jw * sizeof(double)));
+        for (int k = 0; k < PR_KC; ++k)
+            tma_bulk_g2s(&sm.B[c & 1][k * PR_LDB], iK + (size_t)(c * PR_KC + k) * a.ldk + j0, (unsigned)(jw * sizeof(double)), bar);
+    };
+    auto achunk = [&](int c) {                                  // a[rows, c KC .. (c+1) KC) -> A[c & 1]; 0 past n or T
+        double* A = sm.A[c & 1];
+        for (int q = tid; q < PR_TR * PR_KC; q += 256) {
+            const int r = q / PR_KC, k = q % PR_KC, i = c * PR_KC + k;
+            A[r * PR_LDA + k] = (i < a.n && r0 + r < a.T) ? Ae[(size_t)(r0 + r) * a.np + i] : 0.0;
+        }
+    };
+    if (tid == 0) { issue(0); if (nc > 1) issue(1); }
+    achunk(0);
+    double acc[8][4];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.0;
+    for (int c = 0; c < nc; ++c) {
+        __syncthreads();
+        if (tid == 0 && c >= 1 && c + 1 < nc) issue(c + 1);
+        if (c + 1 < nc) achunk(c + 1);
+        mbar_wait(&sm.bar[c & 1], (unsigned)((c >> 1) & 1));
+        if (active) {
+            const double* A = sm.A[c & 1];
+            const double* B = sm.B[c & 1];
+            double af[8];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                af[2 * i] = A[(wm + g) * PR_LDA + t + 4 * i];
+                af[2 * i + 1] = A[(wm + g + 8) * PR_LDA + t + 4 * i];
+            }
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                double bf[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) bf[i] = B[(t + 4 * i) * PR_LDB + wn + 8 * q + g];
+                dmma16816(acc[q], af, bf);
+            }
+        }
+    }
+    __syncthreads();                                            // every warp is done with the last iK tile
+    double* cs = &sm.B[0][0];                                   // c [PR_TR][PR_LDB]
+    const double* be = a.beta + (size_t)e * a.n;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = wm + g + 8 * h;
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+#pragma unroll
+            for (int o = 0; o < 2; ++o) {
+                const int jl = wn + 8 * q + 2 * t + o, j = j0 + jl;
+                double c = 0.0;
+                if (active && r0 + r < a.T && j < a.n) {
+                    const double k = pr_kstar(&sm.x[r * MAXD], a.C + (size_t)j * D, sm.il, D, sf2);
+                    c = k * fma(sm.gm[r], be[j], acc[q][2 * h + o]);
+                }
+                cs[r * PR_LDB + jl] = c;
+            }
+    }
+    __syncthreads();
+    {                                                           // row r = tid / 8; lane s sums columns s, s + 8, ...
+        const int r = tid >> 3, s = tid & 7;
+        const int jend = min(PR_JB, a.n - j0);
+        const double* xr = &sm.x[r * MAXD];
+        double gs[MAXD];
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) gs[d] = 0.0;
+        for (int jl = s; jl < jend; jl += 8) {
+            const double c = cs[r * PR_LDB + jl];
+            const double* cj = a.C + (size_t)(j0 + jl) * D;
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < D) gs[d] = fma(c, cj[d] - xr[d], gs[d]);
+        }
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) {
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 1);
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 2);
+            gs[d] += __shfl_xor_sync(0xffffffffu, gs[d], 4);
+        }
+        if (s == 0 && r0 + r < a.T) {
+            double* pr = a.part + ((((size_t)e * a.nrb + rb) * a.nj + jb) * PR_TR + r) * D;
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < D) pr[d] = gs[d];
+        }
+    }
+    if (!last_cta_arrives(a.cnt + rb, (unsigned)(a.nj * a.E))) return;
+    for (int q = tid; q < PR_TR * D; q += 256) {                // outputs, then j blocks, then the direct sum
+        const int r = q / D, d = q % D;
+        if (r0 + r >= a.T) continue;
+        double sum = 0.0;
+        for (int ee = 0; ee < a.E; ++ee) {
+            const double* pe = a.part + (((size_t)ee * a.nrb + rb) * a.nj * PR_TR + r) * D + d;
+            double se = 0.0;
+            for (int b = 0; b < a.nj; ++b) se += pe[(size_t)b * PR_TR * D];
+            se += fa.dir[((size_t)ee * a.T + r0 + r) * D + d];
+            const double il = 1.0 / a.ell[(size_t)ee * D + d];
+            sum = fma(se, il * il, sum);
+        }
+        a.gXs[(size_t)(r0 + r) * D + d] = sum;
+    }
+}
+
+// one-time kernel attribute of fs_predict_vjp_kernel (before the consistent gradient enqueues anything)
+int fs_vjp_prepare() {
+    static bool attr_set[PILCO_MAX_DEVICES] = {false};
+    bool& set = attr_set[pilco_current_device()];
+    if (!set) {
+        if (cudaFuncSetAttribute(fs_predict_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VjpSmem))
+            != cudaSuccess)
+            return PILCO_ERR_LAUNCH;
+        set = true;
+    }
+    return PILCO_OK;
+}
+
+// d/dXs of the validated model at T points given gmean [T,E], the a rows [E,T,np] and the direct sums [E,T,D];
+// ws: pilco_gp_predict_vjp's workspace at T
+int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, const double* gmean,
+                  const double* A, const double* dir, double* gXs, void* ws) {
+    const int n = gp->n, D = gp->D, E = gp->E, np = pad64(n), nj = (np + PR_JB - 1) / PR_JB, nrb = (T + PR_TR - 1) / PR_TR;
+    FsVjpArgs fa;
+    VjpArgs& a = fa.v;
+    a.n = n; a.D = D; a.np = np; a.nj = nj; a.nrb = nrb; a.T = T; a.E = E;
+    a.C = gp->X; a.ell = gp->ell; a.sf2 = gp->sf2; a.beta = gp->beta; a.iK = gp->iK; a.ldk = gp->ldk;
+    a.Xs = Xs; a.gmean = gmean; a.gvar = nullptr; a.gXs = gXs;
+    a.part = (double*)ws;
+    a.cnt = (unsigned*)((char*)ws + (size_t)E * nrb * nj * PR_TR * D * sizeof(double));
+    fa.A = A; fa.dir = dir;
+    cudaMemsetAsync(a.cnt, 0, (size_t)nrb * sizeof(unsigned), st);
+    const dim3 grid(nj, nrb, E);
+    launch_pri(pilco_small_grid(grid), fs_predict_vjp_kernel, grid, dim3(256), sizeof(VjpSmem), st, fa);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
 static size_t pr_vjp_bytes(int np, int D, int E, int T) {
     const size_t nj = (size_t)(np + PR_JB - 1) / PR_JB, nrb = (size_t)(T + PR_TR - 1) / PR_TR;
     const size_t part = (size_t)E * nrb * nj * PR_TR * D * sizeof(double);

@@ -506,23 +506,54 @@ class ParticlePlan:
 
     ``consistent=True``: ``launch()`` samples each particle's dynamics as ONE function drawn from the GP posterior
     (pilco_particles_rollout_consistent, DESIGN.md section 14) instead of fresh noise at every step; its workspace is
-    O(P H E n).  It has no gradient path: ``grad=True`` with ``consistent=True`` is a ValueError."""
+    O(P H E n).  Its gradient is ``ConsistentGradPlan``; ``grad=True`` with ``consistent=True`` is a ValueError."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False):
+        if consistent and grad:
+            raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
+                             "ConsistentGradPlan, not ParticlePlan(grad=True)")
+        self.consistent = bool(consistent)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad)
+        pr, d = self.pr, device()
+        P, H = self.P, self.H
+        if self.consistent:
+            wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
+            if wsb == 0:
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        elif not self.batched:                                  # the forward-only rollout (a batch has none)
+            wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
+            if wsb == 0:
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        self.grad = None
+        if grad:
+            self._grad_buffers(self._grad_ws_bytes(P))
+
+    def _grad_ws_bytes(self, P):
+        """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
+        pr = _lib.Particles.from_buffer_copy(self.pr)
+        pr.P = int(P)
+        if self.batched:
+            return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
+        return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
+
+    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad):
+        """the pilco_particles description, its input and output buffers (self.pr)"""
         d = device()
         self.P, self.H, self.R = int(P), int(H), int(R)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
         P, H, Ds, U, R = self.P, self.H, self.Ds, self.U, self.R
         if P < 1 or H < 0 or R < 1:
             raise ValueError("particles: needs P >= 1, H >= 0 and R >= 1 (P=%d, H=%d, R=%d)" % (P, H, R))
-        self.consistent = bool(consistent)
-        if self.consistent and grad:
-            raise ValueError("particles: the consistent (function-sample) rollout has no gradient path (grad=True)")
         rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
         self.batched = R > 1 or rbf_batched
         if self.batched and not grad:
             raise ValueError("particles: a batch of policies runs the gradient path only (grad=True)")
         lead = (R,) if self.batched else ()
+        self.lead = lead
         self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
         pr = _lib.Particles()
         pr.P, pr.H = P, H
@@ -565,41 +596,28 @@ class ParticlePlan:
         pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
         pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
         pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
-        if self.consistent:
-            wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
-            if wsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
-            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
-            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
-        elif not self.batched:                                  # the forward-only rollout (a batch has none)
-            wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
-            if wsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
-            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
-            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         self.pr = pr
-        self.grad = None
-        if grad:
-            g = _lib.ParticlesGrad()
-            if pol.kind == _lib.POLICY_LINEAR:
-                self.gbuf = {"W": mk(*lead, U, Ds), "b": mk(*lead, U)}
-                g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
-            else:
-                bf = self.rbf.n
-                self.gbuf = {"X": mk(*lead, bf, Ds), "Y": mk(*lead, bf, U), "ell": mk(*lead, U, Ds)}
-                g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
-                g.pol_L = self.rbf.fact_ws.data_ptr()
-            self.gbuf["value"] = mk(R if self.batched else 1)
-            g.value = self.gbuf["value"].data_ptr()
-            if self.batched:
-                gwsb = lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), R)
-            else:
-                gwsb = lib.pilco_particles_grad_workspace_bytes(C.byref(pr))
-            if gwsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (P, H, dyn.D, R))
-            self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
-            g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
-            self.grad = g
+
+    def _grad_buffers(self, gwsb):
+        """the pilco_particles_grad outputs and a gradient workspace of gwsb bytes (self.grad)"""
+        d, lead, Ds, U, pr = device(), self.lead, self.Ds, self.U, self.pr
+        if gwsb == 0:
+            raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, pr.dyn.D, self.R))
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
+        g = _lib.ParticlesGrad()
+        if pr.pol.kind == _lib.POLICY_LINEAR:
+            self.gbuf = {"W": mk(*lead, U, Ds), "b": mk(*lead, U)}
+            g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
+        else:
+            bf = self.rbf.n
+            self.gbuf = {"X": mk(*lead, bf, Ds), "Y": mk(*lead, bf, U), "ell": mk(*lead, U, Ds)}
+            g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
+            g.pol_L = self.rbf.fact_ws.data_ptr()
+        self.gbuf["value"] = mk(self.R if self.batched else 1)
+        g.value = self.gbuf["value"].data_ptr()
+        self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
+        g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
+        self.grad = g
 
     def launch_grad(self):
         """pilco_particles_rollout_grad: the rollout (``outputs()`` as after ``launch()``, bitwise) and the pathwise
@@ -634,6 +652,54 @@ class ParticlePlan:
         with a leading R for a batched plan"""
         H = self.H
         return self.traj, self.act_buf[..., :H, :], self.rew_buf[..., :H], self.risk_buf[..., :H], self.ret
+
+
+class ConsistentGradPlan(ParticlePlan):
+    """The consistent (function-sample) rollout of ``ParticlePlan(consistent=True)`` and the pathwise gradient of its
+    mean return w.r.t. the policy parameters with x0 and eps fixed (pilco_particles_rollout_consistent_grad, DESIGN.md
+    section 15): ``set_inputs``, ``launch_grad()`` and ``outputs()`` in ``ParticlePlan``'s layout, each with a leading
+    R for a batch of policies (``R > 1`` or a batched RBF policy; the R policies share x0 and eps).  The forward
+    outputs are bitwise those of ``ParticlePlan(consistent=True).launch()`` with the same policy.
+
+    The workspace is O(R P H E n) and is not chunked: chunking the particles would reorder the gradient's fixed-order
+    sums.  A plan whose workspace exceeds ``max_ws_bytes`` (default: half the free device memory) is a ValueError
+    that names the bytes needed and the number of particles that would fit, raised before anything is allocated."""
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None):
+        self.consistent = True
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True)
+        need = self._grad_ws_bytes(self.P)
+        if need == 0:
+            raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
+        if max_ws_bytes is None:
+            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+        if need > max_ws_bytes:
+            fits = lambda p: 0 < self._grad_ws_bytes(p) <= max_ws_bytes
+            lo, hi = 0, self.P - 1                              # the largest P that fits: bisection
+            while lo < hi:
+                mid = (lo + hi + 1) // 2
+                lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+            raise ValueError("particles: the consistent gradient of %d restarts x %d particles over H=%d steps needs %d "
+                             "workspace bytes, more than max_ws_bytes=%d (half the free device memory by default); "
+                             "num_samples=%d would fit" % (self.R, self.P, self.H, need, max_ws_bytes, lo))
+        self._grad_buffers(need)
+
+    def _grad_ws_bytes(self, P):
+        if P < 1:
+            return 0
+        pr = _lib.Particles.from_buffer_copy(self.pr)
+        pr.P = int(P)
+        return int(lib.pilco_particles_consistent_grad_workspace_bytes(C.byref(pr), self.R))
+
+    def launch(self):
+        raise RuntimeError("ConsistentGradPlan: the rollout runs with its gradient, launch_grad()")
+
+    def launch_grad(self):
+        """pilco_particles_rollout_consistent_grad: the consistent rollout (``outputs()``) and the pathwise gradient
+        of value = mean return, returned as ``ParticlePlan.launch_grad`` returns it"""
+        check(lib.pilco_particles_rollout_consistent_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
+              "particles_rollout_consistent_grad")
+        return self.gbuf
 
 
 def gp_predict_vjp(gp, Xs, gmean, gvar):

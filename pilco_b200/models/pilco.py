@@ -164,13 +164,18 @@ class PILCO:
         out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
         return ParticleTrajectories(*out)
 
-    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False):
+    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
-        (from ``np.random`` when None): the same seed gives the same particles to every caller."""
+        (from ``np.random`` when None): the same seed gives the same particles to every caller.  ``consistent``
+        (with ``grad``): the ConsistentGradPlan over the same particles."""
         dyn = self.mgpr.device_gp()
         x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, what)
         terms, mult_mu = self.reward_spec()
-        plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu, grad=grad)
+        if consistent:
+            plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu)
+        else:
+            plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
+                                       grad=grad)
         plan.set_inputs(x0, eps)
         return plan
 
@@ -205,16 +210,20 @@ class PILCO:
         return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
                                g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
 
-    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None):
+    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
         """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
         are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
         d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
         sampled return, to compare with ``policy_gradient``.  Box (risk) terms enter value but not grad: their
-        indicator is flat almost everywhere, so for them the estimate of d E[return] is biased.
+        indicator is flat almost everywhere, so for them the estimate of d E[return] is biased.  ``consistent=True``:
+        the particles of ``sample_trajectories(..., consistent=True)``, each following one function drawn from the
+        dynamics posterior (DESIGN.md section 15); its workspace grows as num_samples n E N (N training points)
+        and is not chunked.
 
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
-        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True)
+        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
+                                   consistent=consistent)
         g = plan.launch_grad()
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
@@ -235,7 +244,7 @@ class PILCO:
         g = plan.backward()
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
-    def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None):
+    def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -247,7 +256,12 @@ class PILCO:
 
         Returns the winner's sampled value: an in-sample estimate, biased upwards by the optimisation; for an
         out-of-sample estimate run ``sample_trajectories`` with another seed.  A reward with box (risk) terms is
-        rejected, because they carry no pathwise gradient and the optimiser would ignore the constraint."""
+        rejected, because they carry no pathwise gradient and the optimiser would ignore the constraint.
+
+        ``consistent=True``: the particles follow one function drawn from the dynamics posterior each, as
+        ``sample_trajectories(..., consistent=True)`` (Deep PILCO's objective), so model errors do not average out
+        along a trajectory.  A lock-step group's workspace is O(restarts num_samples horizon^2 E n); a group that
+        needs more than half the free device memory is a ValueError naming the num_samples that would fit."""
         from functools import partial
         from .. import policy_opt
         if int(num_samples) < 1:
@@ -266,7 +280,7 @@ class PILCO:
                                             "optimize_policy_sampled")
             best_flat, best_value, _ = policy_opt.optimize(
                 self, maxiter=maxiter, restarts=restarts, flats0=flats0,
-                evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps))
+                evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent))
             self.controller.set_flat(best_flat)
         finally:
             for p in mgpr_trainable:

@@ -203,10 +203,11 @@ class ParticleEvaluator(_FlatEvaluator):
 
     The R policies run over the same particles ``x0`` [P,Ds] and standard normals ``eps`` [P,H,Ds] (H = the horizon),
     held fixed, so the objective is a deterministic function of the parameters: one batched device call
-    (pilco_particles_rollout_batch_grad) evaluates every restart.  Box terms carry no pathwise gradient, so a reward
-    with them is rejected."""
+    (pilco_particles_rollout_batch_grad) evaluates every restart.  ``consistent=True``: each particle follows one
+    function drawn from the dynamics posterior (pilco_particles_rollout_consistent_grad through
+    ``engine.ConsistentGradPlan``).  Box terms carry no pathwise gradient, so a reward with them is rejected."""
 
-    def __init__(self, pilco, R, x0, eps):
+    def __init__(self, pilco, R, x0, eps, consistent=False):
         terms, mult_mu = pilco.reward_spec()
         if any(t["kind"] == _lib.REWARD_BOX for t in terms):
             raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
@@ -216,8 +217,12 @@ class ParticleEvaluator(_FlatEvaluator):
         spec = c.policy_spec(flat0) if self.linear else pilco.policy_spec(flat0)
         self.gp = None if self.linear else spec["gp"]
         x0 = engine.dev(x0)
-        self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
-                                        mult_mu=mult_mu, grad=True, R=R)
+        if consistent:
+            self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
+                                                  int(pilco.horizon), mult_mu=mult_mu, R=R)
+        else:
+            self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
+                                            mult_mu=mult_mu, grad=True, R=R)
         self.plan.set_inputs(x0, eps)
         self._setup_io()
 
