@@ -23,14 +23,19 @@
 #define PT_RBF_VAR 1e-6                 // output variance of the deterministic-GP policy (mode 1, mm_finish_device)
 #define PT_INV_PI  0.31830988618379067154
 
-struct PtDev {
-    int P, H, Ds, U, t;
+// the policy and the rewards, as every per-particle kernel reads them (pt_policy)
+struct PtPolicy {
+    int P, H, Ds, U;
     int pol_kind, squash;
     const double* maxa;
     const double* W; const double* b;                   // linear policy [U,Ds], [U]
-    const double* C; const double* ell; const double* sf2; const double* beta; int bf;   // RBF policy
+    const double* C; const double* ell; const double* sf2; const double* beta; int bf;   // RBF policy (bf = 0: linear)
     long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;   // per-restart policy strides (0: shared)
     int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
+};
+
+struct PtDev : PtPolicy {
+    int t;
     const double* x0; const double* eps;                // [P,Ds], [P,H,Ds]: shared by the restarts
     double* traj; double* act; double* step_reward; double* step_risk; double* ret;   // rows r P + p
     double* xt;                                         // predict input [R P,D]
@@ -157,14 +162,8 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
 //   x_bar_t  = x_bar_{t+1} + x~_bar_t[:Ds] + (d pi / dx)' z_bar_t + sum_k a_kt grad v_k(x_t)
 // a_kt = coef_k (ADD) or coef_k mult_mu prod_{s != t} (1 - risk_s) (MULT).  x_H carries no reward, so the sweep
 // starts at t = H-1 with x_bar_H = 0 and x~_bar_{H-1} = 0: H-1 VJP calls.
-struct PgDev {
-    int P, H, Ds, U, t;
-    int pol_kind, squash;
-    const double* maxa;
-    const double* W; const double* b;
-    const double* C; const double* ell; const double* sf2; const double* beta; int bf;
-    long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;
-    int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
+struct PgDev : PtPolicy {
+    int t;
     const double* eps; const double* traj; const double* step_risk;
     const double* gxt;          // VJP of step t at x~_t [R P,D]; NULL at t = H-1
     const double* var_prev;     // var_{t-1} [R P,Ds] (t > 0)
@@ -227,7 +226,9 @@ __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
 #pragma unroll
         for (int d = 0; d < MAXD; ++d) if (d < Ds) xb[d] = fma(f, gv[d], xb[d]);
     }
-    // policy: z_bar_t and (d pi / dx)' z_bar_t; z_t recomputed in the forward's order
+    // policy: z_bar_t and (d pi / dx)' z_bar_t; z_t recomputed in the forward's order.  This is pt_step_kernel's
+    // policy code with the Jacobian row added: one shared function changes pt_step_kernel's code (127 -> 96 registers)
+    // and makes the rollout slower at small P, so the two stay separate and must be kept in the same order.
     double* zb = a.zbar + (row * H + t) * U;
     const double su = a.pol_kind == PILCO_POLICY_RBF ? PT_RBF_VAR : 0.0;
     for (int j = 0; j < U; ++j) {
@@ -302,11 +303,8 @@ __device__ __forceinline__ void pg_block_sum(double (&v)[NV], double* red, doubl
     __syncthreads();
 }
 
-struct PgRed {
-    int P, H, Ds, U, bf, pol_kind;
+struct PgRed : PtPolicy {
     const double* traj; const double* zbar; const double* ret;
-    const double* C; const double* ell; const double* sf2; const double* beta;
-    long long C_bs, ell_bs, sf2_bs, beta_bs;            // per-restart RBF policy strides (0: shared)
     double* gW; double* gb;                             // linear [R,U,Ds], [R,U]
     double* s1; double* s2; double* gbeta;              // RBF per (r, output j, centre i): [R,U,bf,Ds] (x2), [R,U,bf]
     double* gXc; double* gell;                          // RBF direct terms (pg_rbf_finish_kernel) [R,bf,Ds], [R,U,Ds]
@@ -591,16 +589,99 @@ __global__ void __launch_bounds__(FS_WARPS * 32, 3) fs_cond_bwd_kernel(FsBwd a) 
     if (dl) a.dir[pe * D + lane] = ds;
 }
 
-struct PtWs { size_t xt, mean, var, pws, pws_bytes, total; };     // offsets in doubles; total and pws_bytes in bytes
+// ---- host side ------------------------------------------------------------------------------------------------------
+// Offsets in doubles into a particle workspace, for all four layouts (a slot a layout does not have stays 0); the
+// predict (pws) and VJP (vws) workspaces are one slot when one call needs both.  total in bytes; 0 for unsupported
+// sizes and on size_t overflow.
+struct PtWs {
+    size_t xt, mean, var;                               // forward: x~ [H or 1,T,D], step closure mean [T,Ds], var
+    size_t mu, s2, W, Kh, L;                            // consistent forward: predict outputs, W_t, K* history, factor
+    size_t gx, gvar, gxt, zbar, s1, s2r, gbeta, gy;     // reverse sweep and the policy-parameter reduction
+    size_t G, dir;                                      // reverse of the conditioning
+    size_t pws, pws_bytes, vws, vws_bytes, total;
+};
 
+// slots of dims[0] x dims[1] x ... doubles, each rounded up to an even count (16 bytes); ok = false on size_t overflow
+struct PtTake {
+    size_t o = 0;
+    bool ok = true;
+    size_t operator()(std::initializer_list<size_t> dims) {
+        size_t len = 1;
+        for (size_t d : dims) ok = ok && !__builtin_mul_overflow(len, d, &len);
+        const size_t at = o;
+        ok = ok && !__builtin_add_overflow(len, len & 1, &len) && !__builtin_add_overflow(o, len, &o);
+        return at;
+    }
+    size_t bytes() { size_t b = 0; return ok && !__builtin_mul_overflow(o, sizeof(double), &b) ? b : 0; }
+};
+
+static bool pt_rbf(const pilco_particles* pr) { return pr->pol.kind == PILCO_POLICY_RBF; }
+
+// the marginal rollout: x~, the predict outputs and one predict workspace at T = P
 static PtWs pt_ws_layout(const pilco_particles* pr) {
     const size_t P = pr->P, Ds = pr->pol.Ds, D = pr->dyn.D;
-    PtWs L; size_t o = 0;
-    auto take = [&](size_t len) { const size_t at = o; o += (len + 1) & ~(size_t)1; return at; };
-    L.xt = take(P * D); L.mean = take(P * Ds); L.var = take(P * Ds);
-    L.pws = o;
+    PtWs L = {}; PtTake take;
+    L.xt = take({P, D}); L.mean = take({P, Ds}); L.var = take({P, Ds});
     L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
-    L.total = o * sizeof(double) + L.pws_bytes;
+    L.pws = take({L.pws_bytes / sizeof(double)});
+    L.total = L.pws_bytes ? take.bytes() : 0;
+    return L;
+}
+
+// the gradient for R restarts: the forward's predict inputs and variances of EVERY step (the reverse sweep needs
+// them), the state cotangent, the VJP's cotangents and output, z_bar of every point, the RBF sums, and one predict /
+// VJP workspace at T = R P (never in use at the same time).  Rows are restart-major (row r P + p); nothing of size
+// [., n] is kept.
+static PtWs pg_ws_layout(const pilco_particles* pr, int R) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+    const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+    PtWs L = {}; PtTake take;
+    L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
+    L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
+    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
+    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
+    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
+    L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
+    L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
+    L.total = L.pws_bytes ? take.bytes() : 0;
+    return L;
+}
+
+// the consistent rollout at T rows: x~ of every step [H,T,D], the predict outputs mu and var and the step closure's
+// mean and var [T,Ds], W_t [E,T,np], the K* history [H,E,T,np], the packed factor rows [H(H+1)/2,E,T], one predict
+// workspace at T
+static void fs_take(const pilco_particles* pr, size_t T, PtWs& L, PtTake& take) {
+    const size_t H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
+    L.xt = take({H, T, D}); L.mu = take({T, Ds}); L.s2 = take({T, Ds}); L.mean = take({T, Ds}); L.var = take({T, Ds});
+    L.W = take({T, Ds, np}); L.Kh = take({H, T, Ds, np}); L.L = take({H * (H + 1) / 2, T, Ds});
+    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
+    L.pws = take({L.pws_bytes / sizeof(double)});
+}
+
+static PtWs fs_ws_layout(const pilco_particles* pr) {
+    PtWs L = {}; PtTake take;
+    fs_take(pr, pr->P, L, take);
+    L.total = L.pws_bytes ? take.bytes() : 0;
+    return L;
+}
+
+// the consistent gradient for R restarts: the consistent forward's at T = R P (its W slot holds a_t in the reverse
+// sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
+// [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
+// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T
+static PtWs fg_ws_layout(const pilco_particles* pr, int R) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+    const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+    PtWs L = {}; PtTake take;
+    fs_take(pr, T, L, take);                            // pt_batch_ok: R P <= PT_MAX_P
+    L.var = take({H, T, Ds}); L.G = take({H * (H + 1) / 2, T, Ds}); L.dir = take({T, Ds, D});
+    L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
+    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
+    L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
+    L.vws = take({L.vws_bytes / sizeof(double)});
+    L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
     return L;
 }
 
@@ -614,8 +695,8 @@ static bool pt_batch_ok(int P, int R) {
     return R >= 1 && R <= 65535 && (long long)R * P <= PT_MAX_P;
 }
 
-// everything but the workspace (pilco_particles_rollout_grad brings its own).  batched: the policy's batch strides
-// are honoured (pilco_particles_rollout_batch_grad); otherwise a batched policy is unsupported.
+// everything but the workspace (the gradients bring their own).  batched: the policy's batch strides are honoured
+// (the batch_grad and consistent_grad entry points); otherwise a batched policy is unsupported.
 static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
@@ -658,25 +739,30 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
     return PILCO_OK;
 }
 
-static int pt_check(const pilco_particles* pr) {
-    const int rc = pt_check_desc(pr);
-    if (rc) return rc;
-    if (!pr->ws) return PILCO_ERR_NULL;
-    if ((uintptr_t)pr->ws & 15) return PILCO_ERR_ALIGN;
-    const PtWs L = pt_ws_layout(pr);
-    if (L.pws_bytes == 0) return PILCO_ERR_DIM;
-    if (pr->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
+// a workspace against its layout's total (0: unsupported sizes)
+static int pt_check_ws(const void* ws, size_t ws_bytes, size_t total) {
+    if (!ws) return PILCO_ERR_NULL;
+    if ((uintptr_t)ws & 15) return PILCO_ERR_ALIGN;
+    if (total == 0) return PILCO_ERR_DIM;
+    if (ws_bytes < total) return PILCO_ERR_WORKSPACE;
     return PILCO_OK;
 }
 
-static PtDev pt_dev(const pilco_particles* pr) {
+// the gradient's output pointers, after pt_check_desc
+static int pg_check(const pilco_particles* pr, const pilco_particles_grad* g) {
+    if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
+    if (pt_rbf(pr) ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
+    return PILCO_OK;
+}
+
+static PtPolicy pt_policy(const pilco_particles* pr) {
     const pilco_policy& pol = pr->pol;
-    PtDev a;
-    a.P = pr->P; a.H = pr->H; a.Ds = pol.Ds; a.U = pol.U; a.t = 0;
+    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    PtPolicy a;
+    a.P = pr->P; a.H = pr->H; a.Ds = pol.Ds; a.U = pol.U;
     a.pol_kind = pol.kind; a.squash = pol.squash; a.maxa = pol.max_action;
     a.W = pol.W; a.b = pol.b;
-    a.C = pol.rbf.X; a.ell = pol.rbf.ell; a.sf2 = pol.rbf.sf2; a.beta = pol.rbf.beta; a.bf = pol.rbf.n;
-    const bool rbf = pol.kind == PILCO_POLICY_RBF;
+    a.C = pol.rbf.X; a.ell = pol.rbf.ell; a.sf2 = pol.rbf.sf2; a.beta = pol.rbf.beta; a.bf = rbf ? pol.rbf.n : 0;
     a.W_bs = rbf ? 0 : pol.W_bs; a.b_bs = rbf ? 0 : pol.b_bs;
     a.C_bs = rbf ? pol.rbf.X_bs : 0; a.ell_bs = rbf ? pol.rbf.ell_bs : 0;
     a.sf2_bs = rbf ? pol.rbf.sf2_bs : 0; a.beta_bs = rbf ? pol.rbf.beta_bs : 0;
@@ -684,64 +770,58 @@ static PtDev pt_dev(const pilco_particles* pr) {
     for (int k = 0; k < 8; ++k) a.rewards[k] = pr->rewards[k];
     for (int k = 0; k < pr->n_rewards; ++k) a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
     a.mult_mu = pr->mult_mu;
-    a.x0 = pr->x0; a.eps = pr->eps;
-    a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
     return a;
-}
-
-// workspace of the consistent rollout (offsets in doubles; total and pws_bytes in bytes; ok = false on size_t
-// overflow): x~ of every step [H,P,D], the predict outputs mu and var and the step closure's mean and var [P,Ds],
-// W_t [E,P,np], the K* history [H,E,P,np], the packed factor rows [H(H+1)/2,E,P], one predict workspace at T = P
-struct FsWs { size_t xh, mu, s2, mean, var, W, Kh, L, pws, pws_bytes, total; bool ok; };
-
-static bool fs_mul(size_t x, size_t y, size_t& r) { return !__builtin_mul_overflow(x, y, &r); }
-
-static FsWs fs_ws_layout(const pilco_particles* pr) {
-    FsWs L = {};
-    const size_t P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
-    size_t xh, pd, w, kh, rows, lp;
-    L.ok = fs_mul(H * P, D, xh) && fs_mul(P, Ds, pd) && fs_mul(pd, np, w) && fs_mul(H, w, kh) &&
-           fs_mul(H, H + 1, rows) && fs_mul(rows / 2, pd, lp);
-    if (!L.ok) return L;
-    size_t o = 0;
-    auto take = [&](size_t len) {
-        const size_t at = o;
-        if (len == SIZE_MAX || __builtin_add_overflow(o, len + (len & 1), &o)) L.ok = false;
-        return at;
-    };
-    L.xh = take(xh); L.mu = take(pd); L.s2 = take(pd); L.mean = take(pd); L.var = take(pd);
-    L.W = take(w); L.Kh = take(kh); L.L = take(lp);
-    L.pws = o;
-    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
-    size_t b = 0;
-    if (!L.ok || !fs_mul(o, sizeof(double), b) || __builtin_add_overflow(b, L.pws_bytes, &L.total)) L.ok = false;
-    return L;
 }
 
 int fs_predict_prepare();
 int fs_predict_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, double* mean, double* var,
                       double* W, double* Ks, void* ws);
+int fs_vjp_prepare();
+int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, const double* gmean,
+                  const double* A, const double* dir, double* gXs, void* ws);
 
-// workspace of the particle gradient for R restarts (offsets in doubles; total and pws_bytes in bytes): the forward's
-// predict inputs and variances of EVERY step (the reverse sweep needs them), the state cotangent, the VJP's cotangents
-// and output, z_bar of every point, the RBF sums, and one predict / VJP workspace at T = R P (never in use at the same
-// time).  Rows are restart-major (row r P + p); nothing of size [., n] is kept.
-struct PgWs { size_t xt, mean, var, gx, gvar, gxt, zbar, s1, s2, gbeta, gy, pws, pws_bytes, total; };
-
-static PgWs pg_ws_layout(const pilco_particles* pr, int R) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
-    const size_t bf = pr->pol.kind == PILCO_POLICY_RBF ? pr->pol.rbf.n : 0;
-    PgWs L; size_t o = 0;
-    auto take = [&](size_t len) { const size_t at = o; o += (len + 1) & ~(size_t)1; return at; };
-    L.xt = take(H * T * D); L.mean = take(T * Ds); L.var = take(H * T * Ds);
-    L.gx = take(T * Ds); L.gvar = take(T * Ds); L.gxt = take(T * D); L.zbar = take(T * H * U);
-    L.s1 = take(R * U * bf * Ds); L.s2 = take(R * U * bf * Ds); L.gbeta = take(R * U * bf); L.gy = take(R * U * bf);
-    L.pws = o;
-    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
-    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
-    L.pws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
-    L.total = o * sizeof(double) + L.pws_bytes;
-    return L;
+// The forward of every entry point, R restarts (validated; T = R P rows):
+//   pt_step<0>, predict<0>, [fs_cond<0>,] pt_step<1>, ..., pt_step<H>
+// consistent: the predict is fs_predict_kernel and fs_cond_kernel leaves the step closure (mean, var) that
+// pt_step_kernel reads unchanged.  history: var of every step is kept (the reverse sweep needs it); x~ of every step is
+// kept when either needs it.
+static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
+                      cudaStream_t st) {
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
+    const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
+    const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
+    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
+    PtDev a;
+    static_cast<PtPolicy&>(a) = pt_policy(pr);
+    a.x0 = pr->x0; a.eps = pr->eps;
+    a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
+    a.mean = ws + L.mean;
+    FsCond c;
+    c.P = P; c.T = T; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = np; c.t = 0;
+    c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
+    c.xh = ws + L.xt; c.mu = ws + L.mu; c.s2 = ws + L.s2; c.W = ws + L.W; c.Kh = ws + L.Kh;
+    c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean;
+    for (int t = 0; t <= H; ++t) {
+        a.t = t;
+        a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
+        a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
+        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        if (t == H) break;
+        double* var = ws + L.var + (size_t)t * vstep;
+        if (consistent) {
+            const int rc = fs_predict_launch(st, &pr->dyn, T, a.xt, ws + L.mu, ws + L.s2, ws + L.W, ws + L.Kh + t * slot,
+                                             ws + L.pws);
+            if (rc) return rc;
+            c.t = t; c.var = var;
+            launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
+            CUDA_LAUNCH_CHECK();
+        } else {
+            const int rc = pilco_gp_predict(&pr->dyn, 0, Ds, T, a.xt, ws + L.mean, var, 0, ws + L.pws, L.pws_bytes, st);
+            if (rc) return rc;
+        }
+    }
+    return PILCO_OK;
 }
 
 void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
@@ -751,338 +831,151 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
                           const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
 
-// the reverse sweep's per-particle arguments (everything but the step, the workspace buffers and gxt / var_prev)
-static PgDev pg_dev(const pilco_particles* pr, const PtDev& a) {
-    const pilco_policy& pol = pr->pol;
-    PgDev b;
-    b.P = pr->P; b.H = pr->H; b.Ds = pol.Ds; b.U = pol.U;
-    b.pol_kind = pol.kind; b.squash = pol.squash; b.maxa = pol.max_action;
-    b.W = pol.W; b.b = pol.b;
-    b.C = pol.rbf.X; b.ell = pol.rbf.ell; b.sf2 = pol.rbf.sf2; b.beta = pol.rbf.beta; b.bf = pol.rbf.n;
-    b.W_bs = a.W_bs; b.b_bs = a.b_bs; b.C_bs = a.C_bs; b.ell_bs = a.ell_bs; b.sf2_bs = a.sf2_bs; b.beta_bs = a.beta_bs;
-    b.n_rewards = a.n_rewards; b.n_mult = a.n_mult; b.mult_mu = a.mult_mu;
-    for (int k = 0; k < 8; ++k) b.rewards[k] = a.rewards[k];
-    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
-    return b;
-}
-
 // value and the policy-parameter gradient over all P H points of each restart, fixed order, from z_bar [R P,H,U]
-static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtDev& a, double* zbar,
-                     double* s1, double* s2, double* gbeta, double* gy, cudaStream_t st) {
-    const pilco_policy& pol = pr->pol;
-    const bool rbf = pol.kind == PILCO_POLICY_RBF;
-    const int Ds = pol.Ds, U = pol.U;
+static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_grad* g, double* ws, const PtWs& L,
+                     cudaStream_t st) {
     PgRed r;
-    r.P = pr->P; r.H = pr->H; r.Ds = Ds; r.U = U; r.bf = rbf ? pol.rbf.n : 0; r.pol_kind = pol.kind;
-    r.traj = pr->traj; r.zbar = zbar; r.ret = pr->ret;
-    r.C = pol.rbf.X; r.ell = pol.rbf.ell; r.sf2 = pol.rbf.sf2; r.beta = pol.rbf.beta;
-    r.C_bs = a.C_bs; r.ell_bs = a.ell_bs; r.sf2_bs = a.sf2_bs; r.beta_bs = a.beta_bs;
+    static_cast<PtPolicy&>(r) = pt_policy(pr);
+    const bool rbf = r.pol_kind == PILCO_POLICY_RBF;
+    const int Ds = r.Ds, U = r.U, bf = r.bf;
+    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
     r.gW = g->gW; r.gb = g->gb;
-    r.s1 = s1; r.s2 = s2; r.gbeta = gbeta;
+    r.s1 = ws + L.s1; r.s2 = ws + L.s2r; r.gbeta = ws + L.gbeta;
     r.gXc = g->gXc; r.gell = g->gell;
     r.value = g->value;
-    launch_hi(pg_param_kernel, dim3((rbf ? U * r.bf : U) + 1, R), dim3(256), 0, st, r);
+    launch_hi(pg_param_kernel, dim3((rbf ? U * bf : U) + 1, R), dim3(256), 0, st, r);
     CUDA_LAUNCH_CHECK();
     if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
-        const int bf = r.bf, ldw = pad64(bf);
+        const int ldw = pad64(bf);
         launch_hi(pg_rbf_finish_kernel, dim3(R), dim3(128), 0, st, r);
         CUDA_LAUNCH_CHECK();
         chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              gbeta, (long long)U * bf, bf, 1, gy, bf);
-        const int rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, pol.rbf.X, a.C_bs, pol.rbf.ell, a.ell_bs, pol.rbf.sf2,
-                                             a.sf2_bs, pol.rbf.beta, a.beta_bs, gy, g->gXc, g->gYc, g->gell);
+                              r.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
+        const int rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, r.C, r.C_bs, r.ell, r.ell_bs, r.sf2, r.sf2_bs,
+                                             r.beta, r.beta_bs, ws + L.gy, g->gXc, g->gYc, g->gell);
         if (rc) return rc;
     }
     return PILCO_OK;
 }
 
-// the gradient's output and workspace pointers, after pt_check_desc
-static int pg_check_ptrs(const pilco_particles* pr, const pilco_particles_grad* g) {
-    if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
-    const bool rbf = pr->pol.kind == PILCO_POLICY_RBF;
-    if (rbf ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
-    if ((uintptr_t)g->ws & 15) return PILCO_ERR_ALIGN;
-    return PILCO_OK;
-}
-
-// the gradient's arguments and workspace, after pt_check_desc
-static int pg_check(const pilco_particles* pr, int R, const pilco_particles_grad* g) {
-    if (const int rc = pg_check_ptrs(pr, g)) return rc;
-    const PgWs L = pg_ws_layout(pr, R);
-    if (L.pws_bytes == 0) return PILCO_ERR_DIM;
-    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
-    return PILCO_OK;
-}
-
-// forward rollout and reverse sweep of R restarts (validated): R = 1 is pilco_particles_rollout_grad
-static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
-    const PgWs L = pg_ws_layout(pr, R);
-    cudaStream_t st = (cudaStream_t)stream;
+// The reverse sweep after pt_forward(history) and the reduction (DESIGN.md sections 12, 15):
+//   pg_step<H-1>, [VJP<t>, pg_step<t>] for t = H-2 .. 0, then pg_reduce's launches
+// The step's VJP is pilco_gp_predict_vjp, or (consistent) fs_cond_bwd_kernel followed by fs_predict_vjp_kernel.
+static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
+                      cudaStream_t st) {
     double* ws = (double*)g->ws;
-    const pilco_policy& pol = pr->pol;
-    const int P = pr->P, H = pr->H, Ds = pol.Ds, U = pol.U, D = Ds + U, T = R * P;
-    const size_t PD = (size_t)T * D, PDs = (size_t)T * Ds;
-    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R);
-    int rc;
-    // forward: pilco_particles_rollout's launches, with the predict inputs and variances of every step kept
-    PtDev a = pt_dev(pr);
-    a.mean = ws + L.mean;
-    for (int t = 0; t <= H; ++t) {
-        a.t = t;
-        a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * PD;
-        a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * PDs;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        if (t == H) break;
-        rc = pilco_gp_predict(&pr->dyn, 0, Ds, T, a.xt, ws + L.mean, ws + L.var + (size_t)t * PDs, 0,
-                              ws + L.pws, L.pws_bytes, stream);
-        if (rc) return rc;
-    }
-    // reverse sweep
-    PgDev b = pg_dev(pr, a);
-    b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
-    for (int t = H - 1; t >= 0; --t) {
-        b.t = t;
-        b.gxt = nullptr;
-        if (t < H - 1) {
-            rc = pilco_gp_predict_vjp(&pr->dyn, T, ws + L.xt + (size_t)t * PD, b.gx, b.gvar, ws + L.gxt,
-                                      ws + L.pws, L.pws_bytes, stream);
-            if (rc) return rc;
-            b.gxt = ws + L.gxt;
-        }
-        b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * PDs : nullptr;
-        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
-        CUDA_LAUNCH_CHECK();
-    }
-    return pg_reduce(pr, R, g, a, ws + L.zbar, ws + L.s1, ws + L.s2, ws + L.gbeta, ws + L.gy, st);
-}
-
-int fs_vjp_prepare();
-int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, const double* gmean,
-                  const double* A, const double* dir, double* gXs, void* ws);
-
-// workspace of the consistent gradient for R restarts (offsets in doubles; total and vws_bytes in bytes; ok = false on
-// size_t overflow): the consistent forward's at T = R P (its W slot holds a_t in the reverse sweep), then the var'
-// history [H,T,Ds], the packed cotangent rows [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the
-// VJP output [T,D], z_bar [T,H,U], the RBF sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T
-struct FgWs { FsWs f; size_t varh, G, dir, gx, gvar, gxt, zbar, s1, s2, gbeta, gy, vws, vws_bytes, total; bool ok; };
-
-static FgWs fg_ws_layout(const pilco_particles* pr, int R) {
-    FgWs L = {};
-    pilco_particles q = *pr;
-    q.P = R * pr->P;                                    // pt_batch_ok: R P <= PT_MAX_P
-    L.f = fs_ws_layout(&q);
-    L.ok = L.f.ok && L.f.pws_bytes;
-    if (!L.ok) return L;
-    const size_t T = q.P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
-    const size_t bf = pr->pol.kind == PILCO_POLICY_RBF ? pr->pol.rbf.n : 0;
-    size_t vh, gl, dr, zb, rb, rs;
-    L.ok = fs_mul(H * T, Ds, vh) && fs_mul(H * (H + 1) / 2, T * Ds, gl) && fs_mul(T * Ds, D, dr) &&
-           fs_mul(T * H, U, zb) && fs_mul((size_t)R * U, bf, rb) && fs_mul(rb, Ds, rs);
-    if (!L.ok) return L;
-    size_t o = L.f.total / sizeof(double);              // f.total: a multiple of 16 bytes
-    auto take = [&](size_t len) {
-        const size_t at = o;
-        if (len == SIZE_MAX || __builtin_add_overflow(o, len + (len & 1), &o)) L.ok = false;
-        return at;
-    };
-    L.varh = take(vh); L.G = take(gl); L.dir = take(dr);
-    L.gx = take(T * Ds); L.gvar = take(T * Ds); L.gxt = take(T * D); L.zbar = take(zb);
-    L.s1 = take(rs); L.s2 = take(rs); L.gbeta = take(rb); L.gy = take(rb);
-    L.vws = o;
-    L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
-    size_t b = 0;
-    if (!L.ok || !L.vws_bytes || !fs_mul(o, sizeof(double), b) || __builtin_add_overflow(b, L.vws_bytes, &L.total))
-        L.ok = false;
-    return L;
-}
-
-// the consistent forward at T = R P with var' kept per step, then the reverse sweep (DESIGN.md section 15):
-//   pg_step<H-1>, [fs_cond_bwd<t>, fs_vjp<t>, pg_step<t>] for t = H-2 .. 0, then pg_reduce's launches
-static int fg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
-    const FgWs L = fg_ws_layout(pr, R);
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)g->ws;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
-    const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = (size_t)Ds * T * np;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P;
+    const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
     const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
-    int rc;
-    PtDev a = pt_dev(pr);
-    a.mean = ws + L.f.mean;
-    FsCond c;
-    c.P = P; c.T = T; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = np; c.t = 0;
-    c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
-    c.xh = ws + L.f.xh; c.mu = ws + L.f.mu; c.s2 = ws + L.f.s2; c.W = ws + L.f.W; c.Kh = ws + L.f.Kh;
-    c.eps = pr->eps; c.L = ws + L.f.L; c.mean = ws + L.f.mean;
-    for (int t = 0; t <= H; ++t) {
-        a.t = t;
-        a.xt = ws + L.f.xh + (size_t)(t < H ? t : 0) * TD;
-        a.var = ws + L.varh + (size_t)(t > 0 ? t - 1 : 0) * TDs;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        if (t == H) break;
-        rc = fs_predict_launch(st, &pr->dyn, T, a.xt, ws + L.f.mu, ws + L.f.s2, ws + L.f.W, ws + L.f.Kh + (size_t)t * slot,
-                               ws + L.f.pws);
-        if (rc) return rc;
-        c.t = t;
-        c.var = ws + L.varh + (size_t)t * TDs;
-        launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
-        CUDA_LAUNCH_CHECK();
-    }
-    // reverse sweep; the cotangent rows accumulate from zero
-    if (H > 1) cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TDs * sizeof(double), st);
-    PgDev b = pg_dev(pr, a);
+    if (consistent && H > 1) cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TDs * sizeof(double), st);
+    PgDev b;
+    static_cast<PtPolicy&>(b) = pt_policy(pr);
+    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
     b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
-    FsBwd q;
-    q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = Ds; q.np = np; q.t = 0;
+    FsBwd q;                                            // the cotangent rows G accumulate from zero
+    q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = Ds; q.np = pad64(pr->dyn.n); q.t = 0;
     q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
-    q.xh = ws + L.f.xh; q.Kh = ws + L.f.Kh; q.L = ws + L.f.L; q.eps = pr->eps;
-    q.gx = b.gx; q.gvar = b.gvar; q.G = ws + L.G; q.A = ws + L.f.W; q.dir = ws + L.dir;
+    q.xh = ws + L.xt; q.Kh = ws + L.Kh; q.L = ws + L.L; q.eps = pr->eps;
+    q.gx = b.gx; q.gvar = b.gvar; q.G = ws + L.G; q.A = ws + L.W; q.dir = ws + L.dir;
     for (int t = H - 1; t >= 0; --t) {
         b.t = t;
         b.gxt = nullptr;
         if (t < H - 1) {
-            q.t = t;
-            launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
-            CUDA_LAUNCH_CHECK();
-            rc = fs_vjp_launch(st, &pr->dyn, T, ws + L.f.xh + (size_t)t * TD, b.gx, q.A, q.dir, ws + L.gxt, ws + L.vws);
+            const double* xt = ws + L.xt + (size_t)t * TD;
+            int rc;
+            if (consistent) {
+                q.t = t;
+                launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
+                CUDA_LAUNCH_CHECK();
+                rc = fs_vjp_launch(st, &pr->dyn, T, xt, b.gx, q.A, q.dir, ws + L.gxt, ws + L.vws);
+            } else {
+                rc = pilco_gp_predict_vjp(&pr->dyn, T, xt, b.gx, b.gvar, ws + L.gxt, ws + L.vws, L.vws_bytes, st);
+            }
             if (rc) return rc;
             b.gxt = ws + L.gxt;
         }
-        b.var_prev = t > 0 ? ws + L.varh + (size_t)(t - 1) * TDs : nullptr;
+        b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * TDs : nullptr;
         launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
         CUDA_LAUNCH_CHECK();
     }
-    return pg_reduce(pr, R, g, a, ws + L.zbar, ws + L.s1, ws + L.s2, ws + L.gbeta, ws + L.gy, st);
+    return pg_reduce(pr, R, g, ws, L, st);
+}
+
+// the validated gradient of R restarts: the forward with its history, then the reverse sweep
+static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool consistent,
+                  pilco_stream_t stream) {
+    const PtWs L = consistent ? fg_ws_layout(pr, R) : pg_ws_layout(pr, R);
+    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
+    if (consistent) {
+        if (const int rc = fs_predict_prepare()) return rc;
+        if (const int rc = fs_vjp_prepare()) return rc;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st)) return rc;
+    return pg_reverse(pr, R, g, L, consistent, st);
+}
+
+// the forward alone, R = 1
+static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream) {
+    if (const int rc = pt_check_desc(pr)) return rc;
+    const PtWs L = consistent ? fs_ws_layout(pr) : pt_ws_layout(pr);
+    if (const int rc = pt_check_ws(pr->ws, pr->ws_bytes, L.total)) return rc;
+    if (consistent)
+        if (const int rc = fs_predict_prepare()) return rc;
+    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream);
+}
+
+// the gradient entry points: batched honours the policy's batch strides
+static int pg_entry(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, bool consistent,
+                    pilco_stream_t stream) {
+    if (const int rc = pt_check_desc(pr, batched)) return rc;
+    if (batched && !pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
+    if (const int rc = pg_check(pr, g)) return rc;
+    return pg_run(pr, R, g, consistent, stream);
 }
 
 extern "C" {
 
 size_t pilco_particles_workspace_bytes(const pilco_particles* pr) {
-    if (!pr || !pt_sizes_ok(pr)) return 0;
-    const PtWs L = pt_ws_layout(pr);
-    return L.pws_bytes ? L.total : 0;
+    return pr && pt_sizes_ok(pr) ? pt_ws_layout(pr).total : 0;
 }
 
 int pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream) {
-    const int rc0 = pt_check(pr);
-    if (rc0) return rc0;
-    const PtWs L = pt_ws_layout(pr);
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)pr->ws;
-    const pilco_policy& pol = pr->pol;
-    PtDev a = pt_dev(pr);
-    a.xt = ws + L.xt; a.mean = ws + L.mean; a.var = ws + L.var;
-    const dim3 grid((pr->P + PT_THREADS - 1) / PT_THREADS);
-    for (int t = 0; t <= pr->H; ++t) {
-        a.t = t;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        if (t == pr->H) break;
-        const int rc = pilco_gp_predict(&pr->dyn, 0, pol.Ds, pr->P, ws + L.xt, ws + L.mean, ws + L.var, 0,
-                                        ws + L.pws, L.pws_bytes, stream);
-        if (rc) return rc;
-    }
-    return PILCO_OK;
+    return pt_run(pr, false, stream);
 }
 
 size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr) {
-    if (!pr || !pt_sizes_ok(pr)) return 0;
-    const PgWs L = pg_ws_layout(pr, 1);
-    return L.pws_bytes ? L.total : 0;
+    return pr && pt_sizes_ok(pr) ? pg_ws_layout(pr, 1).total : 0;
 }
 
 int pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream) {
-    int rc = pt_check_desc(pr);
-    if (rc) return rc;
-    rc = pg_check(pr, 1, g);
-    if (rc) return rc;
-    return pg_run(pr, 1, g, stream);
+    return pg_entry(pr, 1, g, false, false, stream);
 }
 
 size_t pilco_particles_batch_grad_workspace_bytes(const pilco_particles* pr, int R) {
-    if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
-    const PgWs L = pg_ws_layout(pr, R);
-    return L.pws_bytes ? L.total : 0;
+    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R).total : 0;
 }
 
 int pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                        pilco_stream_t stream) {
-    int rc = pt_check_desc(pr, true);
-    if (rc) return rc;
-    if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
-    rc = pg_check(pr, R, g);
-    if (rc) return rc;
-    return pg_run(pr, R, g, stream);
+    return pg_entry(pr, R, g, true, false, stream);
 }
 
 size_t pilco_particles_consistent_workspace_bytes(const pilco_particles* pr) {
-    if (!pr || !pt_sizes_ok(pr)) return 0;
-    const FsWs L = fs_ws_layout(pr);
-    return L.ok && L.pws_bytes ? L.total : 0;
+    return pr && pt_sizes_ok(pr) ? fs_ws_layout(pr).total : 0;
 }
 
-// pt_step<0>, fs_predict<0>, fs_cond<0>, pt_step<1>, ..., fs_cond<H-1>, pt_step<H>: pt_step_kernel unchanged, reading
-// the step closure (mean, var) fs_cond_kernel leaves
 int pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t stream) {
-    int rc = pt_check_desc(pr);
-    if (rc) return rc;
-    if (!pr->ws) return PILCO_ERR_NULL;
-    if ((uintptr_t)pr->ws & 15) return PILCO_ERR_ALIGN;
-    const FsWs L = fs_ws_layout(pr);
-    if (!L.ok || L.pws_bytes == 0) return PILCO_ERR_DIM;
-    if (pr->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
-    rc = fs_predict_prepare();
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)pr->ws;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D;
-    const size_t PD = (size_t)P * D, slot = (size_t)Ds * P * pad64(pr->dyn.n);
-    PtDev a = pt_dev(pr);
-    a.mean = ws + L.mean; a.var = ws + L.var;
-    FsCond c;
-    c.P = P; c.T = P; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = pad64(pr->dyn.n); c.t = 0;
-    c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
-    c.xh = ws + L.xh; c.mu = ws + L.mu; c.s2 = ws + L.s2; c.W = ws + L.W; c.Kh = ws + L.Kh;
-    c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean; c.var = ws + L.var;
-    const dim3 grid((P + PT_THREADS - 1) / PT_THREADS), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds);
-    for (int t = 0; t <= H; ++t) {
-        a.t = t;
-        a.xt = ws + L.xh + (size_t)(t < H ? t : 0) * PD;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        if (t == H) break;
-        rc = fs_predict_launch(st, &pr->dyn, P, a.xt, ws + L.mu, ws + L.s2, ws + L.W, ws + L.Kh + (size_t)t * slot,
-                               ws + L.pws);
-        if (rc) return rc;
-        c.t = t;
-        launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
-        CUDA_LAUNCH_CHECK();
-    }
-    return PILCO_OK;
+    return pt_run(pr, true, stream);
 }
 
 size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr, int R) {
-    if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
-    const FgWs L = fg_ws_layout(pr, R);
-    return L.ok ? L.total : 0;
+    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R).total : 0;
 }
 
 int pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                             pilco_stream_t stream) {
-    int rc = pt_check_desc(pr, true);
-    if (rc) return rc;
-    if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
-    rc = pg_check_ptrs(pr, g);
-    if (rc) return rc;
-    const FgWs L = fg_ws_layout(pr, R);
-    if (!L.ok) return PILCO_ERR_DIM;
-    if (g->ws_bytes < L.total) return PILCO_ERR_WORKSPACE;
-    rc = fs_predict_prepare();
-    if (rc) return rc;
-    rc = fs_vjp_prepare();
-    if (rc) return rc;
-    return fg_run(pr, R, g, stream);
+    return pg_entry(pr, R, g, true, true, stream);
 }
 
 }  // extern "C"

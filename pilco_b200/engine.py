@@ -674,11 +674,7 @@ class ConsistentGradPlan(ParticlePlan):
         if max_ws_bytes is None:
             max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
         if need > max_ws_bytes:
-            fits = lambda p: 0 < self._grad_ws_bytes(p) <= max_ws_bytes
-            lo, hi = 0, self.P - 1                              # the largest P that fits: bisection
-            while lo < hi:
-                mid = (lo + hi + 1) // 2
-                lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+            lo = _largest_fitting(lambda p: 0 < self._grad_ws_bytes(p) <= max_ws_bytes, 0, self.P - 1)
             raise ValueError("particles: the consistent gradient of %d restarts x %d particles over H=%d steps needs %d "
                              "workspace bytes, more than max_ws_bytes=%d (half the free device memory by default); "
                              "num_samples=%d would fit" % (self.R, self.P, self.H, need, max_ws_bytes, lo))
@@ -700,6 +696,14 @@ class ConsistentGradPlan(ParticlePlan):
         check(lib.pilco_particles_rollout_consistent_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
               "particles_rollout_consistent_grad")
         return self.gbuf
+
+
+def _largest_fitting(fits, lo, hi):
+    """the largest p in [lo, hi] with fits(p), by bisection; fits must be monotone and hold at lo (or lo is returned)"""
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    return lo
 
 
 def gp_predict_vjp(gp, Xs, gmean, gvar):
@@ -759,10 +763,7 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         raise ValueError("particles_rollout: the consistent rollout of one particle (H=%d, n=%d) needs %d workspace "
                          "bytes, more than max_ws_bytes=%d" % (H, dyn.n, consistent_workspace_bytes(dyn, Ds, U, 1, H),
                                                                max_ws_bytes))
-    lo, hi = 1, P                                           # the largest chunk that fits: bisection
-    while lo < hi:
-        mid = (lo + hi + 1) // 2
-        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    lo = _largest_fitting(fits, 1, P)
     if lo == P:
         plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True)
         plan.set_inputs(x0, eps)

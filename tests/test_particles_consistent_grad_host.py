@@ -218,21 +218,23 @@ def test_consistent_grad_workspace_bytes():
         assert _ws(_particles(P=P, H=H), R) == 0, (P, H, R)
 
 
-SASS_GOLDEN = os.path.join(ROOT, "tests", "golden", "consistent_grad_sass.json")
+SASS_GOLDEN = os.path.join(ROOT, "tests", "golden", "predict_sass.json")
 
 
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
-def test_consistent_grad_kernels_sass():
-    names = ["fs_cond_bwd_kernel", "fs_predict_vjp_kernel", "fs_cond_kernel", "pg_step_kernel", "pg_param_kernel",
-             "pg_rbf_finish_kernel", "gp_predict_vjp_kernel", "fs_predict_kernel"]
+def test_consistent_grad_and_predict_kernels_sass():
+    predict = ["gp_predict_kernel", "gp_predict_vjp_kernel", "fs_predict_kernel", "fs_predict_vjp_kernel"]
+    names = ["fs_cond_bwd_kernel", "fs_cond_kernel", "pg_step_kernel", "pg_param_kernel", "pg_rbf_finish_kernel"] + predict
     sass = _sass(names)
     assert set(sass) == set(names)
     for k, text in sass.items():
         assert not re.search(r"\b(STL|LDL)\b", text), k
     assert "DMMA.16x8x16" in sass["fs_predict_vjp_kernel"] and "UBLKCP" in sass["fs_predict_vjp_kernel"]
-    # the predict VJP and the consistent forward's predict are separate copies, untouched by their new sibling
+    # the four predict-family kernels share their main loop and tails (predict.cu): each is pinned by hash, so a change
+    # to the shared code, or to one kernel's own part, shows up here
     with open(SASS_GOLDEN) as f:
         golden = json.load(f)
+    assert sorted(golden) == sorted(predict)
     for k, h in golden.items():
         assert hashlib.sha256(sass[k].encode()).hexdigest() == h, k
 

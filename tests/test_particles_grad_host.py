@@ -236,7 +236,9 @@ def _sass(names):
     funcs, name = {}, None
     for line in out.splitlines():
         m = re.match(r"\s*Function : (\S+)", line)
-        if m:
+        if line.startswith("Fatbin"):       # the next module's header (its source path) is not the last function's
+            name = None
+        elif m:
             name = next((k for k in names if k in m.group(1)), None)
             if name:
                 funcs[name] = []
