@@ -210,7 +210,6 @@ static inline int pilco_sm_count() {
     }
     return c;
 }
-static inline int exp_table_upload() { return PILCO_OK; }
 
 // ---------------------------------------------------------------------------------------------
 // Launch priorities.  A rollout step is a chain of ~15 small latency-bound kernels around one (or two) big tile
@@ -221,6 +220,7 @@ static inline int exp_table_upload() { return PILCO_OK; }
 // PILCO_NO_PRIORITY=1 disables (A/B tuning switch).
 // ---------------------------------------------------------------------------------------------
 #include <stdlib.h>
+#include <type_traits>
 #include <utility>
 static inline int pilco_hi_priority() {
     static int hi = 0x7fffffff;
@@ -286,7 +286,32 @@ __device__ __forceinline__ bool last_cta_arrives(unsigned* counter, unsigned cou
 
 // tile-type kernels: "glue" (high priority) while the whole grid fits the machine once, bulk work otherwise
 static inline bool pilco_small_grid(dim3 g) { return (long long)g.x * g.y * g.z < 2LL * pilco_sm_count(); }
-#endif       // (kept for the launchers: nothing to upload)
+
+// Calls f(std::integral_constant<int, KS>()) with the moment-match kernels' k-step count KS = ksteps_of(D) (1..4; 4
+// beyond): the one map from a model's D to the template KS (or DP = 4 KS) the host launches.
+template <class F>
+static inline decltype(auto) ks_dispatch(int D, F&& f) {
+    const int ks = ksteps_of(D);
+    if (ks == 1) return f(std::integral_constant<int, 1>());
+    if (ks == 2) return f(std::integral_constant<int, 2>());
+    if (ks == 3) return f(std::integral_constant<int, 3>());
+    return f(std::integral_constant<int, 4>());
+}
+
+// Opts the kernels Ks in to `bytes` of dynamic shared memory, in order, once per device (function attributes are per
+// device; one flag per instantiation).  PILCO_ERR_LAUNCH if an attribute call fails.
+template <auto... Ks>
+static inline int pilco_smem_optin(int bytes) {
+    static bool configured[PILCO_MAX_DEVICES] = {false};
+    bool& done = configured[pilco_current_device()];
+    if (!done) {
+        if ((... || (cudaFuncSetAttribute(Ks, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)))
+            return PILCO_ERR_LAUNCH;
+        done = true;
+    }
+    return PILCO_OK;
+}
+#endif
 
 __device__ __forceinline__ void exp_table_init(double* tab) {
     for (int j = threadIdx.x; j < EXP_TAB_DOUBLES; j += blockDim.x) tab[j] = g_exp_tab[j];

@@ -68,7 +68,6 @@ __global__ void __launch_bounds__(256) fp64_pipe_kernel(int iters, double* sink)
 
 extern "C" int pilco_microbench_fp64(int which, int iters, int blocks, double* sink_dev, float* ms_out, pilco_stream_t stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (exp_table_upload()) return PILCO_ERR_LAUNCH;
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int rep = 0; rep < 2; ++rep) {

@@ -493,15 +493,8 @@ __global__ void __launch_bounds__(128, 2) mm_bfinish_kernel(MMBwdParams bp) {
 template <int KS>
 static int launch_btile(const MMBwdParams& bp, cudaStream_t st) {
     const size_t smem = mm_btile_smem_bytes(bp.B.F.np, bp.B.F.ldz);
-    { int rc0 = exp_table_upload(); if (rc0) return rc0; }
-    static bool configured_dev[PILCO_MAX_DEVICES] = {false};      // function attributes are per device
-    bool& configured = configured_dev[pilco_current_device()];
-    if (!configured) {
-        const int big = (int)mm_btile_smem_bytes(TILE_CM, 20);
-        if (cudaFuncSetAttribute(mm_btile_kernel<KS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
-        if (cudaFuncSetAttribute(mm_btile_kernel<KS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
-        configured = true;
-    }
+    if (pilco_smem_optin<mm_btile_kernel<KS, false>, mm_btile_kernel<KS, true>>((int)mm_btile_smem_bytes(TILE_CM, 20)))
+        return PILCO_ERR_LAUNCH;
     const int E = bp.f.gp.E;
     { const dim3 gb(bp.B.F.NB, bp.B.P2, bp.f.R); launch_pri(pilco_small_grid(gb), mm_btile_kernel<KS, false>, gb, dim3(256), smem, st, bp); }
     if (bp.f.gp.mode == 0 && bp.f.gp.iK != nullptr)
@@ -510,35 +503,18 @@ static int launch_btile(const MMBwdParams& bp, cudaStream_t st) {
 }
 
 int mm_backward_launch(MMBwdParams bp, cudaStream_t st) {
-    const int E = bp.f.gp.E, R = bp.f.R;
-    const int ks = ksteps_of(bp.f.gp.D);
+    const int E = bp.f.gp.E, R = bp.f.R, D = bp.f.gp.D;
     MMParams sp = bp.f;                       // setup in ordered/backward mode on the same workspace
     sp.L = bp.B.F; sp.bwd = 1; sp.oQ = bp.B.oQ; sp.oC = bp.B.oC; sp.oLd = bp.B.oLd;
     // per-restart stride of the setup arrays must be the backward stride
     sp.L.per_r = bp.B.per_r;
-    switch (ks) {
-        case 1: mm_setup_launch<4, true>(sp, st); break;
-        case 2: mm_setup_launch<8, true>(sp, st); break;
-        case 3: mm_setup_launch<12, true>(sp, st); break;
-        default: mm_setup_launch<16, true>(sp, st); break;
-    }
+    ks_dispatch(D, [&](auto ks) { mm_setup_launch<4 * ks, true>(sp, st); });
     CUDA_LAUNCH_CHECK();
-    int rc;
-    switch (ks) {
-        case 1: rc = launch_btile<1>(bp, st); break;
-        case 2: rc = launch_btile<2>(bp, st); break;
-        case 3: rc = launch_btile<3>(bp, st); break;
-        default: rc = launch_btile<4>(bp, st); break;
-    }
+    const int rc = ks_dispatch(D, [&](auto ks) { return launch_btile<ks>(bp, st); });
     if (rc) return rc;
     CUDA_LAUNCH_CHECK();
-    dim3 gf(E + E * E, R);
-    switch (ks) {
-        case 1: launch_hi(mm_bfinish_kernel<4>, dim3(gf), dim3(128), 0, st, bp); break;
-        case 2: launch_hi(mm_bfinish_kernel<8>, dim3(gf), dim3(128), 0, st, bp); break;
-        case 3: launch_hi(mm_bfinish_kernel<12>, dim3(gf), dim3(128), 0, st, bp); break;
-        default: launch_hi(mm_bfinish_kernel<16>, dim3(gf), dim3(128), 0, st, bp); break;
-    }
+    const dim3 gf(E + E * E, R);
+    ks_dispatch(D, [&](auto ks) { launch_hi(mm_bfinish_kernel<4 * ks>, gf, dim3(128), 0, st, bp); });
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
@@ -550,9 +526,8 @@ MMBwdParams mm_bwd_params(const pilco_gp_model* gp, int R, const double* m, long
     MMBwdParams bp;
     bp.need_param = (gX && gbeta && gell) ? 1 : 0;
     bp.B = mm_bws_layout(gp->n, gp->D, gp->E, bp.need_param);
-    bp.f.gp = *gp; bp.f.R = R; bp.f.m = m; bp.f.s = s; bp.f.m_rs = m_rs; bp.f.s_rs = s_rs;
-    bp.f.M = const_cast<double*>(Mfwd); bp.f.S = nullptr; bp.f.V = nullptr; bp.f.info = nullptr;
-    bp.f.ws = ws; bp.f.L = bp.B.F; bp.f.bwd = 1; bp.f.oQ = bp.B.oQ; bp.f.oC = bp.B.oC; bp.f.oLd = bp.B.oLd;
+    bp.f = mm_params(gp, R, m, m_rs, s, s_rs, const_cast<double*>(Mfwd), nullptr, nullptr, nullptr, ws);
+    bp.f.L = bp.B.F; bp.f.bwd = 1; bp.f.oQ = bp.B.oQ; bp.f.oC = bp.B.oC; bp.f.oLd = bp.B.oLd;
     bp.gM = gM; bp.gS = gS; bp.gV = gV;
     bp.gm = gm; bp.gs = gs; bp.gm_rs = gm_rs; bp.gs_rs = gs_rs;
     bp.gX = gX; bp.gbeta = gbeta; bp.gell = gell; bp.accumulate = accumulate;

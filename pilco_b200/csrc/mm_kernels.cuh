@@ -73,6 +73,17 @@ struct MMParams {
     MMTapeL TL;
 };
 
+// the parameter block of one forward moment match on the forward workspace layout; with a tape, the taped tile pass
+// writing tape layout TL.  Value-initialised: the backward-mode fields and TL are defined whatever the caller sets.
+static inline MMParams mm_params(const pilco_gp_model* gp, int R, const double* m, long long m_rs, const double* s,
+                                 long long s_rs, double* M, double* S, double* V, int* info, double* ws,
+                                 double* tape = nullptr, const MMTapeL& TL = MMTapeL()) {
+    MMParams p{};
+    p.gp = *gp; p.R = R; p.m = m; p.m_rs = m_rs; p.s = s; p.s_rs = s_rs; p.M = M; p.S = S; p.V = V; p.info = info;
+    p.ws = ws; p.L = mm_ws_layout(gp->n, gp->D, gp->E); p.tape = tape; p.TL = TL;
+    return p;
+}
+
 
 #ifdef __CUDACC__
 
@@ -1334,6 +1345,7 @@ static __global__ void __launch_bounds__(128) mm_finish_kernel(MMParams p) {
 
 #endif  // __CUDACC__
 
-// host-side launcher shared by mm_forward.cu and rollout.cu
-int mm_forward_launch(const MMParams& p, cudaStream_t st, bool with_finish);
+// host-side launcher shared by mm_forward.cu and rollout.cu: setup, tile (taped when p.tape), finish (with_finish).
+// ev: null, or 4 events recorded before the setup, the tile pass and the finish and after the finish.
+int mm_forward_launch(const MMParams& p, cudaStream_t st, bool with_finish, cudaEvent_t* ev = nullptr);
 int mm_check_model(const pilco_gp_model* gp);

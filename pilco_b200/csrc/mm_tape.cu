@@ -7,22 +7,15 @@
 
 template <int KS>
 static int launch_tape_tile(const MMParams& p, cudaStream_t st) {
-    static bool configured_dev[PILCO_MAX_DEVICES] = {false};      // function attributes are per device
     // 4 (default): the 16x8-MMA kernel (mm_tape_tile_m16_kernel, <=128 regs); 0: the DMMA.8x8x4 kernel, <=128 regs; 1: <=96 regs,
-    // 2 CTAs/SM; 2: <=80 regs, 2 CTAs/SM (padded smem); 3: <=80 regs, 3 CTAs/SM
-    static int variant = 4;
-    bool& configured = configured_dev[pilco_current_device()];
-    if (!configured) {
-        const char* e = getenv("PILCO_TAPE_VARIANT");           // tuning switch
-        if (e && e[0] >= '0' && e[0] <= '4') variant = e[0] - '0';
-        const int big = PILCO_MAX_SMEM_OPTIN;
-        if (cudaFuncSetAttribute(mm_tape_tile_m16_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 304>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_tile_kernel<KS, 352>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
-            return PILCO_ERR_LAUNCH;
-        configured = true;
-    }
+    // 2 CTAs/SM; 2: <=80 regs, 2 CTAs/SM (padded smem); 3: <=80 regs, 3 CTAs/SM.  PILCO_TAPE_VARIANT selects (tuning switch).
+    static const int variant = [] {
+        const char* e = getenv("PILCO_TAPE_VARIANT");
+        return e && e[0] >= '0' && e[0] <= '4' ? e[0] - '0' : 4;
+    }();
+    if (pilco_smem_optin<mm_tape_tile_m16_kernel<KS>, mm_tape_tile_kernel<KS, 256>, mm_tape_tile_kernel<KS, 304>,
+                         mm_tape_tile_kernel<KS, 352>>(PILCO_MAX_SMEM_OPTIN))
+        return PILCO_ERR_LAUNCH;
     size_t smem = mm_tape_smem_bytes(p.L.np, p.L.ldz);
     if (p.L.np > TAPE_MAX_NP || smem > PILCO_MAX_SMEM_OPTIN) return PILCO_ERR_UNSUPPORTED;
     const dim3 grid(p.TL.cs, p.L.P, p.R);
@@ -38,12 +31,7 @@ static int launch_tape_tile(const MMParams& p, cudaStream_t st) {
 }
 
 int mm_tape_tile_launch(const MMParams& p, cudaStream_t st) {
-    switch (ksteps_of(p.gp.D)) {
-        case 1: return launch_tape_tile<1>(p, st);
-        case 2: return launch_tape_tile<2>(p, st);
-        case 3: return launch_tape_tile<3>(p, st);
-        default: return launch_tape_tile<4>(p, st);
-    }
+    return ks_dispatch(p.gp.D, [&](auto ks) { return launch_tape_tile<ks>(p, st); });
 }
 
 template <int DP>
@@ -65,23 +53,11 @@ int mm_tape_backward_launch(const MMTapeBwd& bp, cudaStream_t st, bool with_redu
     const int E = bp.gp.E, R = bp.R;
     dim3 gf(E + bp.TL.P, R);
     const size_t smem = mm_tape_bfinish_smem_bytes(bp.TL.np, bp.gp.D);
-    static bool configured_dev[PILCO_MAX_DEVICES] = {false};
-    bool& configured = configured_dev[pilco_current_device()];
-    if (!configured) {                                          // large n: static + dynamic shared memory > 48 KB
-        const int big = 196 * 1024;
-        if (cudaFuncSetAttribute(mm_tape_bfinish_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_bfinish_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_bfinish_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(mm_tape_bfinish_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
-            return PILCO_ERR_LAUNCH;
-        configured = true;
-    }
-    switch (ksteps_of(bp.gp.D)) {
-        case 1: launch_hi(mm_tape_bfinish_kernel<4>, dim3(gf), dim3(TB_THREADS), smem, st, bp); break;
-        case 2: launch_hi(mm_tape_bfinish_kernel<8>, dim3(gf), dim3(TB_THREADS), smem, st, bp); break;
-        case 3: launch_hi(mm_tape_bfinish_kernel<12>, dim3(gf), dim3(TB_THREADS), smem, st, bp); break;
-        default: launch_hi(mm_tape_bfinish_kernel<16>, dim3(gf), dim3(TB_THREADS), smem, st, bp); break;
-    }
+    // large n: static + dynamic shared memory > 48 KB
+    if (pilco_smem_optin<mm_tape_bfinish_kernel<4>, mm_tape_bfinish_kernel<8>, mm_tape_bfinish_kernel<12>,
+                         mm_tape_bfinish_kernel<16>>(196 * 1024))
+        return PILCO_ERR_LAUNCH;
+    ks_dispatch(bp.gp.D, [&](auto ks) { launch_hi(mm_tape_bfinish_kernel<4 * ks>, gf, dim3(TB_THREADS), smem, st, bp); });
     CUDA_LAUNCH_CHECK();
     if (with_reduce) {
         launch_hi(mm_tape_breduce_kernel, dim3(R), dim3(128), 0, st, bp);
@@ -102,24 +78,6 @@ size_t pilco_mm_tape_bwd_workspace_bytes(int D, int E, int R) {
     return mm_tape_bwd_part_doubles(D, E) * (size_t)R * sizeof(double);
 }
 
-int pilco_mm_forward_taped(const pilco_gp_model* gp, int R, const double* m, const double* s,
-                           double* M, double* S, double* V, int* info,
-                           void* ws, size_t ws_bytes, void* tape, size_t tape_bytes, pilco_stream_t stream) {
-    int rc = mm_check_model(gp);
-    if (rc) return rc;
-    if (!m || !s || !M || !S || !V || !ws || !tape) return PILCO_ERR_NULL;
-    if (R < 1) return PILCO_ERR_DIM;
-    if (!mm_tape_supported(gp->n, gp->D)) return PILCO_ERR_UNSUPPORTED;
-    if (ws_bytes < pilco_mm_workspace_bytes(gp->n, gp->D, gp->E, R)) return PILCO_ERR_WORKSPACE;
-    if (tape_bytes < pilco_mm_tape_bytes(gp->n, gp->D, gp->E, R)) return PILCO_ERR_WORKSPACE;
-    if ((((uintptr_t)ws) | ((uintptr_t)tape)) & 15) return PILCO_ERR_ALIGN;
-    MMParams p;
-    p.gp = *gp; p.R = R; p.m = m; p.s = s; p.m_rs = gp->D; p.s_rs = (long long)gp->D * gp->D; p.M = M; p.S = S; p.V = V; p.info = info;
-    p.ws = (double*)ws; p.L = mm_ws_layout(gp->n, gp->D, gp->E); p.bwd = 0; p.oQ = p.oC = p.oLd = 0;
-    p.tape = (double*)tape; p.TL = mm_tape_layout(gp->n, gp->D, gp->E, R);
-    return mm_forward_launch(p, (cudaStream_t)stream, true);
-}
-
 int pilco_mm_backward_taped(const pilco_gp_model* gp, int R, const double* m, const double* s, const double* M,
                             const double* gM, const double* gS, const double* gV,
                             const void* tape, size_t tape_bytes, double* gm, double* gs,
@@ -132,12 +90,9 @@ int pilco_mm_backward_taped(const pilco_gp_model* gp, int R, const double* m, co
     if (tape_bytes < pilco_mm_tape_bytes(gp->n, gp->D, gp->E, R)) return PILCO_ERR_WORKSPACE;
     if (ws_bytes < pilco_mm_tape_bwd_workspace_bytes(gp->D, gp->E, R)) return PILCO_ERR_WORKSPACE;
     if ((((uintptr_t)ws) | ((uintptr_t)tape)) & 15) return PILCO_ERR_ALIGN;
-    MMTapeBwd bp;
-    bp.gp = *gp; bp.R = R; bp.m = m; bp.s = s; bp.m_rs = gp->D; bp.s_rs = (long long)gp->D * gp->D;
-    bp.Mfwd = M; bp.gM = gM; bp.gS = gS; bp.gV = gV;
-    bp.tape = (const double*)tape; bp.TL = mm_tape_layout(gp->n, gp->D, gp->E, R);
-    bp.part = (double*)ws; bp.gm = gm; bp.gs = gs; bp.gm_rs = gp->D; bp.gs_rs = (long long)gp->D * gp->D;
-    bp.accumulate = 0;
+    const int D = gp->D;
+    const MMTapeBwd bp = mm_tape_bwd_params(gp, R, m, D, s, (long long)D * D, M, gM, gS, gV, (const double*)tape,
+                                            mm_tape_layout(gp->n, D, gp->E, R), (double*)ws, gm, D, gs, (long long)D * D);
     return mm_tape_backward_launch(bp, (cudaStream_t)stream, true);
 }
 

@@ -502,6 +502,18 @@ struct MMTapeBwd {
     double* gm; double* gs; long long gm_rs, gs_rs;
     int accumulate;
 };
+// the reverse sweep of one taped moment match: cotangents gM, gS, gV of its outputs -> gm, gs (overwritten); tape and its
+// layout TL as the forward wrote them, part: task partials
+static inline MMTapeBwd mm_tape_bwd_params(const pilco_gp_model* gp, int R, const double* m, long long m_rs,
+                                           const double* s, long long s_rs, const double* Mfwd, const double* gM,
+                                           const double* gS, const double* gV, const double* tape, const MMTapeL& TL,
+                                           double* part, double* gm, long long gm_rs, double* gs, long long gs_rs) {
+    MMTapeBwd bp{};
+    bp.gp = *gp; bp.R = R; bp.m = m; bp.s = s; bp.m_rs = m_rs; bp.s_rs = s_rs;
+    bp.Mfwd = Mfwd; bp.gM = gM; bp.gS = gS; bp.gV = gV; bp.tape = tape; bp.TL = TL;
+    bp.part = part; bp.gm = gm; bp.gs = gs; bp.gm_rs = gm_rs; bp.gs_rs = gs_rs; bp.accumulate = 0;
+    return bp;
+}
 static inline __host__ __device__ size_t mm_tape_bwd_part_doubles(int D, int E) {
     return (size_t)(E + npairs_of(E)) * (MAXD + (size_t)D * D);
 }

@@ -473,23 +473,10 @@ static PrArgs pr_args(const pilco_gp_model* gp, int T, const double* Xs, const P
     return a;
 }
 
-// one-time dynamic-shared-memory attribute of kernel K, per device
-template <auto K, size_t SMEM>
-static int pr_prepare() {
-    static bool attr_set[PILCO_MAX_DEVICES] = {false};
-    bool& set = attr_set[pilco_current_device()];
-    if (!set) {
-        if (cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM) != cudaSuccess)
-            return PILCO_ERR_LAUNCH;
-        set = true;
-    }
-    return PILCO_OK;
-}
-
 // zero the counters and launch K on grid (nj, nrb, nz), 256 threads
 template <auto K, size_t SMEM, class Args>
 static int pr_launch(cudaStream_t st, const PrWs& w, int nz, const Args& a) {
-    if (const int rc = pr_prepare<K, SMEM>()) return rc;
+    if (const int rc = pilco_smem_optin<K>((int)SMEM)) return rc;
     cudaMemsetAsync(w.cnt, 0, w.ncnt * sizeof(unsigned), st);
     const dim3 grid(w.nj, w.nrb, nz);
     launch_pri(pilco_small_grid(grid), K, grid, dim3(256), SMEM, st, a);
@@ -498,8 +485,8 @@ static int pr_launch(cudaStream_t st, const PrWs& w, int nz, const Args& a) {
 }
 
 // the consistent rollout and its gradient set the attributes before they enqueue anything
-int fs_predict_prepare() { return pr_prepare<fs_predict_kernel, sizeof(PredictSmem)>(); }
-int fs_vjp_prepare() { return pr_prepare<fs_predict_vjp_kernel, sizeof(VjpSmem)>(); }
+int fs_predict_prepare() { return pilco_smem_optin<fs_predict_kernel>((int)sizeof(PredictSmem)); }
+int fs_vjp_prepare() { return pilco_smem_optin<fs_predict_vjp_kernel>((int)sizeof(VjpSmem)); }
 
 // all ne = E outputs of the validated model at T points (T <= 65535 * PR_TR); ws: pilco_gp_predict's diagonal workspace
 int fs_predict_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double* Xs, double* mean, double* var,

@@ -201,26 +201,16 @@ int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
     d.risk = ws + L.risk; d.rew = ws + L.rew; d.step_risk = ro->step_risk; d.mult_mu = ro->mult_mu; d.n_mult = ro_count_mult(ro);
 
     auto slot = [&](size_t base, size_t len, int t) { return ws + base + (size_t)t * RR * len; };
-    auto dyn_params = [&](int t) {
-        MMParams p;
-        p.gp = ro->dyn; p.R = R;
-        p.m = slot(L.mj, D, t); p.s = slot(L.sj, (size_t)D * D, t); p.m_rs = D; p.s_rs = (long long)D * D;
-        p.M = slot(L.Md, Ds, t); p.S = slot(L.Sd, (size_t)Ds * Ds, t); p.V = slot(L.Vd, (size_t)D * Ds, t);
-        p.info = ro->info; p.ws = ws + L.dynws; p.L = mm_ws_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E); p.bwd = 0; p.oQ = p.oC = p.oLd = 0;
-        if (ro->tape) {                                  // taped tile pass: slot (t, :) of the rollout's tape
-            p.TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
-            p.tape = (double*)ro->tape + (size_t)t * RR * p.TL.per_r;
-        }
-        return p;
+    const MMTapeL TL = ro->tape ? mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R) : MMTapeL();
+    auto dyn_params = [&](int t) {                   // taped: the tile pass writes slot (t, :) of the rollout's tape
+        return mm_params(&ro->dyn, R, slot(L.mj, D, t), D, slot(L.sj, (size_t)D * D, t), (long long)D * D,
+                         slot(L.Md, Ds, t), slot(L.Sd, (size_t)Ds * Ds, t), slot(L.Vd, (size_t)D * Ds, t), ro->info,
+                         ws + L.dynws, ro->tape ? (double*)ro->tape + (size_t)t * RR * TL.per_r : nullptr, TL);
     };
     auto pol_params = [&](int t) {
-        MMParams p;
-        p.gp = ro->pol.rbf; p.R = R;
-        p.m = ro->traj_m + (size_t)t * Ds; p.s = ro->traj_S + (size_t)t * Ds * Ds;
-        p.m_rs = (long long)(H + 1) * Ds; p.s_rs = (long long)(H + 1) * Ds * Ds;
-        p.M = slot(L.Mp, U, t); p.S = slot(L.Sp, (size_t)U * U, t); p.V = slot(L.Vp, (size_t)Ds * U, t);
-        p.info = ro->info; p.ws = ws + L.polws; p.L = mm_ws_layout(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E); p.bwd = 0; p.oQ = p.oC = p.oLd = 0;
-        return p;
+        return mm_params(&ro->pol.rbf, R, ro->traj_m + (size_t)t * Ds, (long long)(H + 1) * Ds,
+                         ro->traj_S + (size_t)t * Ds * Ds, (long long)(H + 1) * Ds * Ds, slot(L.Mp, U, t),
+                         slot(L.Sp, (size_t)U * U, t), slot(L.Vp, (size_t)Ds * U, t), ro->info, ws + L.polws);
     };
 
     if (ro->info) cudaMemsetAsync(ro->info, 0, sizeof(int) * RR, st);

@@ -236,13 +236,7 @@ template <int DP>
 static int launch_dyn_finish(const MMTapeBwd& tb, const RbDev& d, cudaStream_t st) {
     size_t smem = mm_tape_bfinish_smem_bytes(tb.TL.np, tb.gp.D);
     if (smem < sizeof(RbPostSmem)) smem = sizeof(RbPostSmem);
-    static bool configured_dev[PILCO_MAX_DEVICES] = {false};
-    bool& configured = configured_dev[pilco_current_device()];
-    if (!configured) {
-        const int big = 196 * 1024;
-        if (cudaFuncSetAttribute(rb_dyn_finish_kernel<DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess) return PILCO_ERR_LAUNCH;
-        configured = true;
-    }
+    if (pilco_smem_optin<rb_dyn_finish_kernel<DP>>(196 * 1024)) return PILCO_ERR_LAUNCH;
     launch_hi(rb_dyn_finish_kernel<DP>, dim3(tb.gp.E + tb.TL.P, tb.R), dim3(TB_THREADS), smem, st, tb, d);
     return PILCO_OK;
 }
@@ -383,21 +377,13 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
         d.Mu = slot(FL.Mu, U, t); d.Su = slot(FL.Su, (size_t)U * U, t); d.Cq = slot(FL.Cq, (size_t)U * U, t);
         d.Vu = slot(FL.Vu, (size_t)Ds * U, t);
         if (ro->tape) {                              // consume the tape of step t: no exponential is recomputed
-            MMTapeBwd tb;
-            tb.gp = ro->dyn; tb.R = R;
-            tb.m = slot(FL.mj, D, t); tb.m_rs = D; tb.s = slot(FL.sj, (size_t)D * D, t); tb.s_rs = (long long)D * D;
-            tb.Mfwd = slot(FL.Md, Ds, t);
-            tb.gM = d.gm; tb.gS = d.gS; tb.gV = nullptr;       // seeds straight from the state cotangent; gV = s1'(gS+gS') inline
-            tb.TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
-            tb.tape = (const double*)ro->tape + (size_t)t * RR * tb.TL.per_r;
-            tb.part = bws + BL.dynb;
-            tb.gm = d.gmj; tb.gm_rs = D; tb.gs = d.gsj; tb.gs_rs = (long long)D * D; tb.accumulate = 0;
-            switch (ksteps_of(D)) {
-                case 1: rc = launch_dyn_finish<4>(tb, d, st); break;
-                case 2: rc = launch_dyn_finish<8>(tb, d, st); break;
-                case 3: rc = launch_dyn_finish<12>(tb, d, st); break;
-                default: rc = launch_dyn_finish<16>(tb, d, st); break;
-            }
+            // seeds straight from the state cotangent (gV = s1'(gS+gS') inline); tape slot (t, :)
+            const MMTapeL TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
+            const MMTapeBwd tb = mm_tape_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t),
+                                                    (long long)D * D, slot(FL.Md, Ds, t), d.gm, d.gS, nullptr,
+                                                    (const double*)ro->tape + (size_t)t * RR * TL.per_r, TL,
+                                                    bws + BL.dynb, d.gmj, D, d.gsj, (long long)D * D);
+            rc = ks_dispatch(D, [&](auto ks) { return launch_dyn_finish<4 * ks>(tb, d, st); });
             if (rc) return rc;
             CUDA_LAUNCH_CHECK();
         } else {

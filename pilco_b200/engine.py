@@ -361,6 +361,64 @@ def box_risk(prm, m, s, grad=False):
     return (risk, dm, dv) if grad else risk
 
 
+def _max_action(policy_spec, U):
+    """the policy spec's max_action (scalar or [U]) as a [U] device tensor"""
+    return dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(), (U,)).copy())
+
+
+def _fill_policy(pol, policy_spec, batched=None):
+    """Fill the pilco_policy ``pol`` from a policy spec: kind, Ds, U, squash, max_action and either the linear W/b
+    (batch strides when ``batched``; None: when W has a leading batch dimension) or the RBF policy GP.  Returns the
+    device tensors and the policy GP it points to: (max_action, W, b, rbf), W and b None for an RBF policy, rbf None
+    for a linear one."""
+    pol.kind = policy_spec["kind"]
+    pol.Ds, pol.U = Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
+    pol.squash = 1 if policy_spec.get("squash", True) else 0
+    max_action, W, b, rbf = _max_action(policy_spec, U), None, None, None
+    pol.max_action = max_action.data_ptr()
+    if pol.kind == _lib.POLICY_LINEAR:
+        W, b = dev(policy_spec["W"]), dev(policy_spec["b"])
+        bat = W.dim() == 3 if batched is None else batched
+        pol.W, pol.W_bs = W.data_ptr(), U * Ds if bat else 0
+        pol.b, pol.b_bs = b.data_ptr(), U if bat else 0
+    else:
+        rbf = policy_spec["gp"]
+        pol.rbf = rbf.struct()
+    return max_action, W, b, rbf
+
+
+def _fill_rewards(desc, reward_terms):
+    """Fill ``desc.n_rewards`` and ``desc.rewards`` from reward-term dicts; returns the device tensors [(W, t)] they
+    point to"""
+    rw = []
+    desc.n_rewards = len(reward_terms)
+    for k, rt in enumerate(reward_terms):
+        W = dev(rt["W"]); t = dev(rt["t"]) if rt.get("t") is not None else None
+        rw.append((W, t))
+        desc.rewards[k].kind = rt["kind"]
+        desc.rewards[k].channel = int(rt.get("channel", _lib.CHANNEL_ADD))
+        desc.rewards[k].coef = float(rt.get("coef", 1.0))
+        desc.rewards[k].W = W.data_ptr()
+        desc.rewards[k].t = t.data_ptr() if t is not None else None
+    return rw
+
+
+def _policy_grad_buffers(g, pol, rbf, lead):
+    """the policy-gradient outputs of ``g`` (pilco_rollout_grad / pilco_particles_grad) for the policy ``pol``, with
+    leading dimensions ``lead``: {'W', 'b'} (linear) or {'X', 'Y', 'ell'} and the factors pol_L (RBF policy GP
+    ``rbf``).  Zero-filled; the C code overwrites or zeroes them itself."""
+    mk = lambda *shape: torch.zeros(shape, dtype=F64, device=device())
+    Ds, U = pol.Ds, pol.U
+    if pol.kind == _lib.POLICY_LINEAR:
+        buf = {"W": mk(*lead, U, Ds), "b": mk(*lead, U)}
+        g.gW, g.gb = buf["W"].data_ptr(), buf["b"].data_ptr()
+    else:
+        buf = {"X": mk(*lead, rbf.n, Ds), "Y": mk(*lead, rbf.n, U), "ell": mk(*lead, U, Ds)}
+        g.gXc, g.gYc, g.gell = (buf[k].data_ptr() for k in ("X", "Y", "ell"))
+        g.pol_L = rbf.fact_ws.data_ptr()
+    return buf
+
+
 class RolloutPlan:
     """Owns the buffers of one ``pilco_rollout`` description (batch R, horizon H) and launches it.
 
@@ -379,31 +437,8 @@ class RolloutPlan:
         ro = _lib.Rollout()
         ro.R, ro.H = self.R, self.H
         ro.dyn = dyn.struct()
-        pol = ro.pol
-        pol.kind = policy_spec["kind"]
-        pol.Ds, pol.U = self.Ds, self.U
-        pol.squash = 1 if policy_spec.get("squash", True) else 0
-        self.max_action = dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(),
-                                              (self.U,)).copy())
-        pol.max_action = self.max_action.data_ptr()
-        if pol.kind == _lib.POLICY_LINEAR:
-            self.W, self.b = dev(policy_spec["W"]), dev(policy_spec["b"])
-            bat = self.W.dim() == 3
-            pol.W = self.W.data_ptr(); pol.W_bs = self.U * self.Ds if bat else 0
-            pol.b = self.b.data_ptr(); pol.b_bs = self.U if bat else 0
-        else:
-            self.rbf = policy_spec["gp"]
-            pol.rbf = self.rbf.struct()
-        self.rw = []
-        ro.n_rewards = len(reward_terms)
-        for k, rt in enumerate(reward_terms):
-            W = dev(rt["W"]); t = dev(rt["t"]) if rt.get("t") is not None else None
-            self.rw.append((W, t))
-            ro.rewards[k].kind = rt["kind"]
-            ro.rewards[k].channel = int(rt.get("channel", _lib.CHANNEL_ADD))
-            ro.rewards[k].coef = float(rt.get("coef", 1.0))
-            ro.rewards[k].W = W.data_ptr()
-            ro.rewards[k].t = t.data_ptr() if t is not None else None
+        self.max_action, self.W, self.b, self.rbf = _fill_policy(ro.pol, policy_spec)
+        self.rw = _fill_rewards(ro, reward_terms)
         self.m0, self.S0 = dev(m0), dev(S0)
         # per-restart initial moments: leading dimension R (and R > 1); [1, ...] or unbatched = shared by the batch
         def _batched(t, tail, what):
@@ -447,7 +482,7 @@ class RolloutPlan:
     def capture(self, backward=False):
         """Capture forward (and optionally the reverse sweep) into a CUDA graph.  Buffers are static, the C
         entry points only enqueue work on the current stream, so stream capture records every launch."""
-        self.forward()                       # warm-up: one-time function attributes / table upload happen here
+        self.forward()                       # warm-up: one-time function attributes are set here
         if backward:
             self.backward()
         torch.cuda.synchronize()
@@ -469,19 +504,8 @@ class RolloutPlan:
         d = device()
         if not hasattr(self, "grad"):
             g = _lib.RolloutGrad()
-            R, Ds, U = self.R, self.Ds, self.U
-            self.gbuf = {}
-            if self.ro.pol.kind == _lib.POLICY_LINEAR:
-                self.gbuf["W"] = torch.empty((R, U, Ds), dtype=F64, device=d)
-                self.gbuf["b"] = torch.empty((R, U), dtype=F64, device=d)
-                g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
-            else:
-                bf = self.rbf.n
-                self.gbuf["X"] = torch.empty((R, bf, Ds), dtype=F64, device=d)
-                self.gbuf["Y"] = torch.empty((R, bf, U), dtype=F64, device=d)
-                self.gbuf["ell"] = torch.empty((R, U, Ds), dtype=F64, device=d)
-                g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
-                g.pol_L = self.rbf.fact_ws.data_ptr()
+            R, Ds = self.R, self.Ds
+            self.gbuf = _policy_grad_buffers(g, self.ro.pol, self.rbf, (R,))
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
@@ -558,35 +582,13 @@ class ParticlePlan:
         pr = _lib.Particles()
         pr.P, pr.H = P, H
         pr.dyn = dyn.struct()
-        pol = pr.pol
-        pol.kind = policy_spec["kind"]
-        pol.Ds, pol.U = Ds, U
-        pol.squash = 1 if policy_spec.get("squash", True) else 0
-        self.max_action = dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(),
-                                              (U,)).copy())
-        pol.max_action = self.max_action.data_ptr()
-        if pol.kind == _lib.POLICY_LINEAR:
-            self.W, self.b = dev(policy_spec["W"]), dev(policy_spec["b"])
+        self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, policy_spec, self.batched)
+        if pr.pol.kind == _lib.POLICY_LINEAR:
             if self.W.numel() != R * U * Ds or self.b.numel() != R * U:
                 raise ValueError("particles: expected W [R,U,Ds] and b [R,U] with R=%d (unbatched: [U,Ds], [U])" % R)
-            pol.W, pol.b = self.W.data_ptr(), self.b.data_ptr()
-            if self.batched:
-                pol.W_bs, pol.b_bs = U * Ds, U
-        else:
-            self.rbf = policy_spec["gp"]
-            if self.rbf.batched != self.batched or (self.batched and self.rbf.X.shape[0] != R):
-                raise ValueError("particles: the RBF policy must be factorised with a leading R=%d (unbatched: none)" % R)
-            pol.rbf = self.rbf.struct()
-        self.rw = []
-        pr.n_rewards = len(reward_terms)
-        for k, rt in enumerate(reward_terms):
-            W = dev(rt["W"]); t = dev(rt["t"]) if rt.get("t") is not None else None
-            self.rw.append((W, t))
-            pr.rewards[k].kind = rt["kind"]
-            pr.rewards[k].channel = int(rt.get("channel", _lib.CHANNEL_ADD))
-            pr.rewards[k].coef = float(rt.get("coef", 1.0))
-            pr.rewards[k].W = W.data_ptr()
-            pr.rewards[k].t = t.data_ptr() if t is not None else None
+        elif self.rbf.batched != self.batched or (self.batched and self.rbf.X.shape[0] != R):
+            raise ValueError("particles: the RBF policy must be factorised with a leading R=%d (unbatched: none)" % R)
+        self.rw = _fill_rewards(pr, reward_terms)
         pr.mult_mu = float(mult_mu)
         mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
         Hb = max(H, 1)                                          # H = 0: every buffer still has an address
@@ -600,20 +602,12 @@ class ParticlePlan:
 
     def _grad_buffers(self, gwsb):
         """the pilco_particles_grad outputs and a gradient workspace of gwsb bytes (self.grad)"""
-        d, lead, Ds, U, pr = device(), self.lead, self.Ds, self.U, self.pr
+        d, pr = device(), self.pr
         if gwsb == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, pr.dyn.D, self.R))
-        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
         g = _lib.ParticlesGrad()
-        if pr.pol.kind == _lib.POLICY_LINEAR:
-            self.gbuf = {"W": mk(*lead, U, Ds), "b": mk(*lead, U)}
-            g.gW, g.gb = self.gbuf["W"].data_ptr(), self.gbuf["b"].data_ptr()
-        else:
-            bf = self.rbf.n
-            self.gbuf = {"X": mk(*lead, bf, Ds), "Y": mk(*lead, bf, U), "ell": mk(*lead, U, Ds)}
-            g.gXc, g.gYc, g.gell = (self.gbuf[k].data_ptr() for k in ("X", "Y", "ell"))
-            g.pol_L = self.rbf.fact_ws.data_ptr()
-        self.gbuf["value"] = mk(self.R if self.batched else 1)
+        self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead)
+        self.gbuf["value"] = torch.zeros(self.R if self.batched else 1, dtype=F64, device=d)
         g.value = self.gbuf["value"].data_ptr()
         self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
         g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
@@ -913,8 +907,7 @@ class ActionPlan:
         self.Cq = torch.empty((1, U, U), dtype=F64, device=d)
         self.out = torch.zeros((1, U + 1), dtype=F64, device=d)
         self.info = torch.zeros(1, dtype=torch.int32, device=d)
-        self.maxa = dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(),
-                                        (U,)).copy())
+        self.maxa = _max_action(policy_spec, U)
         if self.kind == _lib.POLICY_LINEAR:
             self.W, self.b = dev(policy_spec["W"]).reshape(U, Ds), dev(policy_spec["b"]).reshape(U)
         else:

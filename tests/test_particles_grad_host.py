@@ -6,7 +6,6 @@ only), the kernels' SASS and the failure without a GPU."""
 import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -17,6 +16,7 @@ from pilco_b200 import _lib
 from pilco_b200._lib import lib
 from particle_oracle import particle_rollout
 from particle_grad_oracle import predict_vjp, rbf_pol_np, value_and_grad
+from util import CUOBJDUMP, sass
 from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, ROOT, _gp, _particles
 
 
@@ -227,24 +227,9 @@ def test_predict_vjp_argument_validation():
     assert lib.pilco_gp_predict_vjp_workspace_bytes(50, 17, 3, 10) == 0
 
 
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-
-
 def _sass(names):
-    out = subprocess.run([CUOBJDUMP, "-sass", os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")],
-                         capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if line.startswith("Fatbin"):       # the next module's header (its source path) is not the last function's
-            name = None
-        elif m:
-            name = next((k for k in names if k in m.group(1)), None)
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items()}
+    """{name: SASS text} of the kernels whose mangled names contain one of ``names`` (keyed by the first that does)"""
+    return {next(k for k in names if k in m): text for m, text in sass("|".join(map(re.escape, names))).items()}
 
 
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")

@@ -6,7 +6,6 @@ exact."""
 import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -17,6 +16,7 @@ from oracle import python_port as pp
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
 from particle_oracle import moment_check, particle_rollout
+from util import CUOBJDUMP, sass
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_UNSUP = -1, -2, -3, -4, -6
@@ -179,24 +179,11 @@ def test_box_point_formula_on_host(tmp_path):
         assert h.box_point(c(prm), c(x)) == float(not bool(inside))
 
 
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-
-
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 def test_particle_step_kernel_has_no_local_memory():
-    out = subprocess.run([CUOBJDUMP, "-sass", os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")],
-                         capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if "pt_step_kernel" in m.group(1) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
+    funcs = sass(r"pt_step_kernel")
     assert len(funcs) == 1
-    text = "\n".join(next(iter(funcs.values())))
+    text = next(iter(funcs.values()))
     assert not re.search(r"\b(STL|LDL)\b", text)
 
 

@@ -6,8 +6,6 @@ import ctypes as C
 import inspect
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -17,9 +15,8 @@ from oracle import python_port as pp
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
 from predict_oracle import fitc_predict_f, gpr_predict_f, ik_beta_predict
-from util import scaled_err
+from util import CUOBJDUMP, sass, scaled_err
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_UNSUP = -1, -2, -3, -4, -6
 FAKE = 0x10000
 
@@ -133,26 +130,13 @@ def test_predict_methods_fail_loudly_without_gpu(monkeypatch):
         m.predict_y(X[:4], full_cov=True)
 
 
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-
-
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 def test_predict_kernel_sass():
     """The quadratic form runs on DMMA.16x8x16 (no 8x8x4), the iK tiles arrive by TMA bulk copy on an mbarrier, and
     nothing touches local memory."""
-    out = subprocess.run([CUOBJDUMP, "-sass", os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")],
-                         capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if "gp_predict_kernel" in m.group(1) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
+    funcs = sass(r"gp_predict_kernel")
     assert len(funcs) == 1
-    text = "\n".join(next(iter(funcs.values())))
+    text = next(iter(funcs.values()))
     assert re.search(r"DMMA\.16x8x\d+", text) and "DMMA.8x8x4" not in text
     assert "UBLKCP" in text and "SYNCS.ARRIVE.TRANS64" in text and "TRYWAIT" in text
     assert not re.search(r"\b(STL|LDL)\b", text)

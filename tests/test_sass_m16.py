@@ -4,34 +4,16 @@ loops issue DMMA.16x8x* only, the columns are TMA-staged, nothing lives in local
 and the hot loops keep the structure DESIGN.md section 6 prices (scripts/issue_model.py)."""
 import os
 import re
-import shutil
-import subprocess
 import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+from util import CUOBJDUMP, ROOT, sass
 
 pytestmark = pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 
 # K decomposition of the exponent per KS (k-steps of 4): one MMA per K chunk
 EXPONENT_SHAPES = {1: ["16x8x4"], 2: ["16x8x8"], 3: ["16x8x8", "16x8x4"], 4: ["16x8x16"]}
-
-
-def _sass(pattern):
-    out = subprocess.run([CUOBJDUMP, "-sass", LIB], capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if re.search(pattern, m.group(1)) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items()}
 
 
 def _issue_model():
@@ -45,8 +27,8 @@ def _ks(name):
 
 
 def test_m16_kernels_use_16x8_dmma_tma_and_no_local_memory():
-    fwd = _sass(r"mm_tile_m16_kernelILi\dE")
-    tape = _sass(r"mm_tape_tile_m16_kernelILi\dE")
+    fwd = sass(r"mm_tile_m16_kernelILi\dE")
+    tape = sass(r"mm_tape_tile_m16_kernelILi\dE")
     assert len(fwd) == 4 and len(tape) == 4                                    # KS = 1..4
     for name, text in list(fwd.items()) + list(tape.items()):
         for shape in EXPONENT_SHAPES[_ks(name)]:

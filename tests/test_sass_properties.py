@@ -4,31 +4,15 @@ library with cuobjdump (no GPU needed): the forward and backward tile kernels us
 everything in registers (no local-memory loads/stores); every device cubin targets sm_90a (H100)."""
 import os
 import re
-import shutil
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from util import CUOBJDUMP, ROOT, sass
+
 LIB = os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
 
 pytestmark = pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
-
-
-def _sass(pattern):
-    """{mangled name: SASS text} of every kernel whose name matches ``pattern``"""
-    out = subprocess.run([CUOBJDUMP, "-sass", LIB], capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if re.search(pattern, m.group(1)) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items()}
 
 
 def test_device_code_targets_sm_90a():
@@ -38,8 +22,8 @@ def test_device_code_targets_sm_90a():
 
 
 def test_tile_kernels_use_dmma_tma_and_no_local_memory():
-    fwd = _sass(r"mm_tile_kernelILi\dELi3ELb1E")                              # the launched instantiation: 3 CTAs/SM, two row octets per warp
-    bwd = _sass(r"mm_btile_kernel")
+    fwd = sass(r"mm_tile_kernelILi\dELi3ELb1E")                              # the launched instantiation: 3 CTAs/SM, two row octets per warp
+    bwd = sass(r"mm_btile_kernel")
     assert len(fwd) == 4 and len(bwd) == 8                                     # KS = 1..4 (x DIAG for the backward)
     for name, text in list(fwd.items()) + list(bwd.items()):
         assert "DMMA.8x8x4" in text, name
@@ -57,7 +41,7 @@ def test_taped_path_kernels_use_dmma_and_stay_in_registers():
     Tile: DMMA for both products (exponent + H.[Z,1]), TMA-staged columns, no local memory in the launched register variant,
     table exp.  Finish: the weighted moment sums are DMMA (no DFMA inner product loops), metric-shape instantiation
     spill-free apart from a few bytes."""
-    tile = _sass(r"mm_tape_tile_kernelILi\d")
+    tile = sass(r"mm_tape_tile_kernelILi\d")
     assert len(tile) == 12                                                     # KS = 1..4 x 3 register variants
     for name, text in tile.items():
         assert "DMMA.8x8x4" in text and "UBLKCP" in text and "TRYWAIT" in text, name
@@ -67,7 +51,7 @@ def test_taped_path_kernels_use_dmma_and_stay_in_registers():
     metric = [t for n, t in tile.items() if "ILi3ELi256E" in n][0]             # D = 12, default register variant
     # per octet and 8-column tile: 3 (exponent) + 4 (H.[Z,1]) DMMA; two octets per pass, x 2 pair kinds x {1, 2 live octets}
     assert metric.count("DMMA.8x8x4") >= 2 * (7 + 14)
-    fin = _sass(r"rb_dyn_finish_kernelILi12E|mm_tape_bfinish_kernelILi12E")
+    fin = sass(r"rb_dyn_finish_kernelILi12E|mm_tape_bfinish_kernelILi12E")
     assert len(fin) == 2
     for name, text in fin.items():
         assert text.count("DMMA.8x8x4") >= 10, name                            # 3 + 3 symmetric tiles + 4 (Z'HZ) per k-step
@@ -77,7 +61,7 @@ def test_taped_path_kernels_use_dmma_and_stay_in_registers():
 def test_reverse_sweep_policy_kernels_present():
     """The recomputing VJP kernels that remain on the path (RBF policy, need_param) exist in every instantiation,
     finish + reduce are one kernel (no mm_breduce_kernel launch any more)."""
-    names = _sass(r"mm_bfinish_kernel|mm_breduce_kernel|mm_setup_fused_kernel")
+    names = sass(r"mm_bfinish_kernel|mm_breduce_kernel|mm_setup_fused_kernel")
     assert sum("mm_bfinish_kernel" in n for n in names) == 4
     assert not any("mm_breduce_kernel" in n for n in names)
     assert sum("mm_setup_fused_kernel" in n for n in names) == 8               # DP = 4..16 x {forward, ordered-pair backward}
@@ -89,10 +73,10 @@ def test_session3_shuffle_and_chain_properties():
     reductions -- holds fewer than 100 SHFL (it was 128 with the 6-shuffle butterfly in every loop); (2) the expected rewards
     are their own kernels, off the per-step chain: ro_state carries no LU / reward code any more (two shuffles: the
     partial-sum pairs of mm_finish)."""
-    tile = _sass(r"mm_tape_tile_kernelILi3ELi256E")
+    tile = sass(r"mm_tape_tile_kernelILi3ELi256E")
     assert len(tile) == 1
     assert sum(t.count("SHFL") for t in tile.values()) < 100
-    ro = _sass(r"ro_state_kernel|ro_reward_kernel|ro_reward_sum_kernel")
+    ro = sass(r"ro_state_kernel|ro_reward_kernel|ro_reward_sum_kernel")
     assert len(ro) == 3
     state = [t for n, t in ro.items() if "ro_state" in n][0]
     assert state.count("SHFL") <= 4

@@ -7,36 +7,17 @@ batch-position test (R=32 two-stage against R=1 fused; its swimmer case, np=512 
 row chunks per pair)."""
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")
-CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+from util import CUOBJDUMP, sass
 
 pytestmark = pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 
 
-def _sass(pattern):
-    """{mangled name: SASS text} of every kernel whose name matches ``pattern``"""
-    out = subprocess.run([CUOBJDUMP, "-sass", LIB], capture_output=True, text=True, timeout=600).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if re.search(pattern, m.group(1)) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
-    return {k: "\n".join(v) for k, v in funcs.items()}
-
-
 def test_forward_stage2_kernels_stay_in_registers_and_pair_kernel_uses_tma():
-    pair = _sass(r"mm_setup2_pair_kernel")
-    out = _sass(r"mm_setup2_out_kernel")
+    pair = sass(r"mm_setup2_pair_kernel")
+    out = sass(r"mm_setup2_out_kernel")
     assert len(pair) == 4 and len(out) == 4                                    # DP = 4, 8, 12, 16
     for name, text in list(pair.items()) + list(out.items()):
         assert not re.search(r"\b(STL|LDL)\b", text), "local memory traffic in %s" % name
@@ -49,6 +30,6 @@ def test_forward_stage2_kernels_stay_in_registers_and_pair_kernel_uses_tma():
 
 
 def test_combined_forward_stage2_kernel_is_gone():
-    names = _sass(r"mm_setup2")
+    names = sass(r"mm_setup2")
     assert not any(re.search(r"mm_setup2_kernel", n) for n in names)
     assert sum("mm_setup2_bwd_kernel" in n for n in names) == 4

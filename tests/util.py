@@ -1,5 +1,39 @@
-"""Shared test helpers: seeded synthetic problems (SURVEY.md section 8d recipe) and error metrics."""
+"""Shared test helpers: seeded synthetic problems (SURVEY.md section 8d recipe), error metrics and the SASS of the
+built library."""
+import functools
+import os
+import re
+import shutil
+import subprocess
+
 import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CUOBJDUMP = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+
+
+@functools.lru_cache(maxsize=None)
+def _sass_functions():
+    """[(mangled name, SASS text)] of every function of the built library, from one cuobjdump run per process.  A
+    function's text ends at the next function or at the next module's Fatbin header, which holds the source path."""
+    lib = os.path.join(ROOT, "pilco_b200", "libpilco_b200.so")
+    out = subprocess.run([CUOBJDUMP, "-sass", lib], capture_output=True, text=True, timeout=600).stdout
+    funcs, name, lines = [], None, []
+    for line in out.splitlines() + ["Fatbin"]:
+        m = re.match(r"\s*Function : (\S+)", line)
+        if m or line.startswith("Fatbin"):
+            if name:
+                funcs.append((name, "\n".join(lines)))
+            name, lines = (m.group(1) if m else None), []
+        elif name:
+            lines.append(line)
+    return funcs
+
+
+def sass(pattern):
+    """{mangled name: SASS text} of every function whose name matches the regular expression ``pattern`` (a static
+    kernel that several modules hold: the last module's copy)"""
+    return {name: text for name, text in _sass_functions() if re.search(pattern, name)}
 
 
 def relerr(a, b):
