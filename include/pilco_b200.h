@@ -388,6 +388,23 @@ size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr
 int    pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                                pilco_stream_t stream);
 
+/* Score-function (likelihood-ratio) gradient of the particle return (DESIGN.md section 16): the contract of
+ * pilco_particles_rollout_batch_grad (R policies through the batch strides, 0 sharing an array, shared x0 and eps,
+ * restart-major outputs, R = 1 with an unbatched policy the single-policy call, the same validation and status codes,
+ * all checked before anything is enqueued), with g->ws sized by pilco_particles_score_grad_workspace_bytes.  The
+ * forward outputs and value are bitwise those of pilco_particles_rollout_batch_grad; the gradient, in the same layout,
+ * is that of (1/P) sum_p sum_{t<H-1} w_pt log N(x_{t+1} - x_t; mu(x~_t), var(x~_t)) with x_t, x_{t+1} held fixed:
+ *   d/d mu = eps / s,  d/d var = (eps^2 - 1) / (2 var)   (both 0 where var <= 0; not clamped near 0),
+ *   w_pt = G_pt - (S_t - G_pt) / (P - 1), G_pt the part of particle p's return that transition t can affect
+ *   (the step rewards after t, and mult_mu prod_{s<=t} (1 - risk_s) (1 - prod_{s>t} (1 - risk_s))), S_t = sum_q G_qt
+ *   over the restart's particles (a leave-one-out baseline; P = 1: w = G).
+ * Its expectation is d E[return] for every reward kind, box terms included; it differentiates no trajectory, and its
+ * variance grows as 1/var where the model is confident.  H <= 1 gives a zero gradient.  A restart's results are
+ * bitwise independent of R and reproducible run to run; no host synchronisation (graph-capturable). */
+size_t pilco_particles_score_grad_workspace_bytes(const pilco_particles* pr, int R);   /* 0: unsupported / overflow */
+int    pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
+                                          pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -129,6 +129,8 @@ SIGNATURES = {
     "pilco_particles_consistent_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.c_int]),
     "pilco_particles_rollout_consistent_grad": (C.c_int, [C.POINTER(Particles), C.c_int, C.POINTER(ParticlesGrad),
                                                           c_dp]),
+    "pilco_particles_score_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.c_int]),
+    "pilco_particles_rollout_score_grad": (C.c_int, [C.POINTER(Particles), C.c_int, C.POINTER(ParticlesGrad), c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),
     "pilco_mm_forward_taped_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,

@@ -14,6 +14,8 @@
 // pilco_particles_rollout_consistent draws ONE posterior function per particle (DESIGN.md section 14): after each step's
 // predict (fs_predict_kernel, predict.cu, which also keeps W_t = K*_t iK and K*_t) fs_cond_kernel conditions the draw
 // on the particle's earlier inputs, and pt_step_kernel closes the step unchanged from the mean and variance it leaves.
+// pilco_particles_rollout_score_grad runs the batched forward and then the score-function gradient (DESIGN.md section
+// 16): per-transition weights and score cotangents, one VJP pass over all steps, z_bar, and the pathwise reduction.
 #include <initializer_list>
 #include "common.cuh"
 #include "risk_math.cuh"
@@ -589,6 +591,135 @@ __global__ void __launch_bounds__(FS_WARPS * 32, 3) fs_cond_bwd_kernel(FsBwd a) 
     if (dl) a.dir[pe * D + lane] = ds;
 }
 
+// ---- score-function gradient (pilco_particles_rollout_score_grad, DESIGN.md section 16) ----------------------------
+// The likelihood-ratio estimator over the forward's transitions, x_t and x_{t+1} held fixed (s_t = sqrt(var_t)):
+//   G_t  = sum_{t' > t} step_reward_t' + mult_mu prod_{s <= t} (1 - risk_s) (1 - prod_{s > t} (1 - risk_s)),  t < H-1
+//   w_t  = G_t - (S_t - G_t) / (P - 1),  S_t = sum_q G_qt over the restart's particles  (P = 1: w_t = G_t)
+//   gmean_t = w_t eps_t / s_t,  gvar_t = w_t (eps_t^2 - 1) / (2 var_t)   (0 where var_t <= 0)
+//   x~_bar_t = pilco_gp_predict_vjp at x~_t (the steps do not depend on one another: whole groups of steps per call)
+//   z_bar_t = x~_bar_t[Ds:] o maxa e^{-su/2} cos(z_t) (when squashed),  z_bar_{H-1} = 0
+// then pg_reduce as after the pathwise sweep.  Box terms enter G, so they enter the gradient.
+struct PsDev : PtPolicy {
+    long long T;                                        // R P rows
+    const double* eps; const double* traj; const double* step_reward; const double* step_risk;
+    const double* var;                                  // [H,T,Ds] the forward's predicted variances
+    double* G;                                          // [H-1,T] return-to-go
+    double* S;                                          // [R,H] per-(restart, step) sums of G
+    double* gmean; double* gvar;                        // [H-1,T,Ds] the VJP's cotangents
+    const double* gxt;                                  // [H-1,T,D] the VJP's outputs
+    double* zbar;                                       // [T,H,U]
+};
+
+// grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y: G_t for t = H-2 .. 0 (H > 1).  The
+// prefix products are parked in G on the way up; suffix sum and product on the way down, no division.
+__global__ void __launch_bounds__(PT_THREADS) ps_togo_kernel(PsDev a) {
+    PDL_ENTRY();
+    const int p = blockIdx.x * PT_THREADS + threadIdx.x;
+    if (p >= a.P) return;
+    const int H = a.H;
+    const size_t row = (size_t)blockIdx.y * a.P + p, T = a.T;
+    const double* rw = a.step_reward + row * H;
+    const double* rk = a.step_risk + row * H;
+    double* G = a.G + row;                              // G_t at G[t T]
+    const bool mult = a.n_mult > 0;
+    if (mult) {
+        double pre = 1.0;
+        for (int t = 0; t < H - 1; ++t) { pre *= 1.0 - rk[t]; G[t * T] = pre; }
+    }
+    double sum = 0.0, suf = 1.0;
+    for (int t = H - 2; t >= 0; --t) {
+        sum += rw[t + 1];
+        double g = sum;
+        if (mult) { suf *= 1.0 - rk[t + 1]; g = sum + a.mult_mu * (G[t * T] * (1.0 - suf)); }
+        G[t * T] = g;
+    }
+}
+
+// grid (H-1, R), 256 threads: S_t of restart r = blockIdx.y, step t = blockIdx.x; thread q takes p = q, q + 256, ...
+// in order, then pg_block_sum (so a restart's sums do not depend on R)
+__global__ void __launch_bounds__(256) ps_base_kernel(PsDev a) {
+    PDL_ENTRY();
+    __shared__ double red[8], out[1];
+    const int t = blockIdx.x, r = blockIdx.y;
+    const double* G = a.G + (size_t)t * a.T + (size_t)r * a.P;
+    double v[1] = {0.0};
+    for (int p = threadIdx.x; p < a.P; p += 256) v[0] += G[p];
+    pg_block_sum<1>(v, red, out);
+    if (threadIdx.x == 0) a.S[(size_t)r * a.H + t] = out[0];
+}
+
+// grid (ceil(P / 128) (H-1), R), one thread per (step t, particle p of restart r = blockIdx.y): the cotangents of
+// step t's predict outputs.  eps of particle p is shared by the restarts.
+__global__ void __launch_bounds__(PT_THREADS) ps_cot_kernel(PsDev a) {
+    PDL_ENTRY();
+    const int nb = (a.P + PT_THREADS - 1) / PT_THREADS;
+    const int t = blockIdx.x / nb, p = (blockIdx.x % nb) * PT_THREADS + threadIdx.x, r = blockIdx.y;
+    if (p >= a.P) return;
+    const int Ds = a.Ds;
+    const size_t row = (size_t)r * a.P + p, tr = (size_t)t * a.T + row;
+    const double G = a.G[tr];
+    const double w = a.P > 1 ? G - (a.S[(size_t)r * a.H + t] - G) / (a.P - 1) : G;
+    const double* ep = a.eps + ((size_t)p * a.H + t) * Ds;
+    for (int e = 0; e < Ds; ++e) {
+        const double v = a.var[tr * Ds + e], ee = ep[e];
+        a.gmean[tr * Ds + e] = v > 0.0 ? w * ee / sqrt(v) : 0.0;
+        a.gvar[tr * Ds + e] = v > 0.0 ? w * (ee * ee - 1.0) / (2.0 * v) : 0.0;
+    }
+}
+
+// grid (ceil(P / 128) H, R), one thread per (step t, particle p of restart r = blockIdx.y): z_bar_t.  z_t is recomputed
+// from x_t in pt_step_kernel's order (its policy code, kept as a separate copy for the reason pg_step_kernel gives).
+__global__ void __launch_bounds__(PT_THREADS) ps_zbar_kernel(PsDev a) {
+    PDL_ENTRY();
+    const int nb = (a.P + PT_THREADS - 1) / PT_THREADS;
+    const int t = blockIdx.x / nb, p = (blockIdx.x % nb) * PT_THREADS + threadIdx.x, r = blockIdx.y;
+    if (p >= a.P) return;
+    const int Ds = a.Ds, U = a.U, H = a.H;
+    const size_t row = (size_t)r * a.P + p;
+    double* zb = a.zbar + (row * H + t) * U;
+    if (t == H - 1) {                                   // x_H carries no reward
+        for (int j = 0; j < U; ++j) zb[j] = 0.0;
+        return;
+    }
+    const double* gx = a.gxt + ((size_t)t * a.T + row) * (Ds + U) + Ds;
+    if (!a.squash) {
+        for (int j = 0; j < U; ++j) zb[j] = gx[j];
+        return;
+    }
+    const double* xg = a.traj + (row * (H + 1) + t) * Ds;
+    double x[MAXD];
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) x[d] = d < Ds ? xg[d] : 0.0;
+    const double su = a.pol_kind == PILCO_POLICY_RBF ? PT_RBF_VAR : 0.0;
+    for (int j = 0; j < U; ++j) {
+        double z;
+        if (a.pol_kind == PILCO_POLICY_LINEAR) {
+            const double* W = a.W + r * a.W_bs;
+            z = a.b[r * a.b_bs + j];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < Ds) z = fma(W[j * Ds + d], x[d], z);
+        } else {
+            const double* ell = a.ell + r * a.ell_bs;
+            double il[MAXD];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) il[d] = d < Ds ? 1.0 / ell[j * Ds + d] : 0.0;
+            const double sf2 = a.sf2[r * a.sf2_bs + j];
+            const double* be = a.beta + r * a.beta_bs + (size_t)j * a.bf;
+            const double* C = a.C + r * a.C_bs;
+            z = 0.0;
+            for (int i = 0; i < a.bf; ++i) {
+                const double* c = C + (size_t)i * Ds;
+                double d2 = 0.0;
+#pragma unroll
+                for (int d = 0; d < MAXD; ++d) if (d < Ds) { const double q = (x[d] - c[d]) * il[d]; d2 = fma(q, q, d2); }
+                z = fma(sf2 * exp(-0.5 * d2), be[i], z);
+            }
+        }
+        // cos(z) as cospi(z / pi), as pg_step_kernel: no Payne-Hanek slow path and its local-memory table
+        zb[j] = gx[j] * (a.maxa[j] * exp(-0.5 * su) * cospi(z * PT_INV_PI));
+    }
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 // Offsets in doubles into a particle workspace, for all four layouts (a slot a layout does not have stays 0); the
 // predict (pws) and VJP (vws) workspaces are one slot when one call needs both.  total in bytes; 0 for unsupported
@@ -597,7 +728,8 @@ struct PtWs {
     size_t xt, mean, var;                               // forward: x~ [H or 1,T,D], step closure mean [T,Ds], var
     size_t mu, s2, W, Kh, L;                            // consistent forward: predict outputs, W_t, K* history, factor
     size_t gx, gvar, gxt, zbar, s1, s2r, gbeta, gy;     // reverse sweep and the policy-parameter reduction
-    size_t G, dir;                                      // reverse of the conditioning
+    size_t G, dir;                                      // reverse of the conditioning (score: G = the return-to-go)
+    size_t gsum;                                        // score: the per-(restart, step) sums of G
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -682,6 +814,35 @@ static PtWs fg_ws_layout(const pilco_particles* pr, int R) {
     L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
     L.vws = take({L.vws_bytes / sizeof(double)});
     L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
+    return L;
+}
+
+// steps per pilco_gp_predict_vjp call of the score gradient: whole steps of T rows, at most PT_MAX_P rows (T <= PT_MAX_P)
+static int ps_group(long long T, int H) {
+    const long long k = PT_MAX_P / T;
+    return H - 1 < k ? H - 1 : (int)k;
+}
+
+// the score gradient for R restarts: pg_ws_layout's forward part (x~ [H,T,D], mean [T,Ds], var [H,T,Ds]), then G
+// [H-1,T], the sums [R,H], gmean and gvar [H-1,T,Ds], the VJP output [H-1,T,D], z_bar [T,H,U], the RBF sums
+// [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one predict / VJP workspace for the predict at T and the largest VJP group.
+// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.
+static PtWs ps_ws_layout(const pilco_particles* pr, int R) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Ds = pr->pol.Ds, U = pr->pol.U;
+    const size_t D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+    PtWs L = {}; PtTake take;
+    L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
+    L.G = take({Hm, T}); L.gsum = take({(size_t)R, H});
+    L.gx = take({Hm, T, Ds}); L.gvar = take({Hm, T, Ds}); L.gxt = take({Hm, T, D}); L.zbar = take({T, H, U});
+    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
+    const int grp = ps_group((long long)T, (int)H);
+    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
+    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T * (grp > 1 ? grp : 1));
+    L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
+    L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
+    const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
+    L.total = L.pws_bytes && nb * H <= 0x7fffffff ? take.bytes() : 0;
     return L;
 }
 
@@ -925,12 +1086,56 @@ static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t str
     return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream);
 }
 
-// the gradient entry points: batched honours the policy's batch strides
-static int pg_entry(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, bool consistent,
-                    pilco_stream_t stream) {
+// The score-function gradient of R restarts (validated; DESIGN.md section 16):
+//   pt_forward(history), ps_togo, ps_base, ps_cot, VJP of steps 0..H-2 in groups of whole steps, ps_zbar, pg_reduce
+// The x~ history [H-1,T,D] and the cotangents [H-1,T,Ds] are contiguous, so a group of k steps is one VJP call at k T
+// rows; a point's VJP does not depend on T or on its row, so the grouping changes no bit.
+static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
+    const PtWs L = ps_ws_layout(pr, R);
+    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)g->ws;
+    if (const int rc = pt_forward(pr, R, ws, L, false, true, st)) return rc;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, nb = (P + PT_THREADS - 1) / PT_THREADS;
+    PsDev a;
+    static_cast<PtPolicy&>(a) = pt_policy(pr);
+    a.T = T;
+    a.eps = pr->eps; a.traj = pr->traj; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
+    a.var = ws + L.var; a.G = ws + L.G; a.S = ws + L.gsum; a.gmean = ws + L.gx; a.gvar = ws + L.gvar;
+    a.gxt = ws + L.gxt; a.zbar = ws + L.zbar;
+    if (H > 1) {
+        launch_hi(ps_togo_kernel, dim3(nb, R), dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        launch_hi(ps_base_kernel, dim3(H - 1, R), dim3(256), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        launch_hi(ps_cot_kernel, dim3(nb * (H - 1), R), dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        const int grp = ps_group(T, H);
+        for (int t0 = 0; t0 < H - 1; t0 += grp) {
+            const int k = grp < H - 1 - t0 ? grp : H - 1 - t0;
+            const size_t o = (size_t)t0 * T;
+            const int rc = pilco_gp_predict_vjp(&pr->dyn, k * T, ws + L.xt + o * D, ws + L.gx + o * Ds,
+                                                ws + L.gvar + o * Ds, ws + L.gxt + o * D, ws + L.vws, L.vws_bytes, st);
+            if (rc) return rc;
+        }
+    }
+    if (H > 0) {
+        launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+    }
+    return pg_reduce(pr, R, g, ws, L, st);
+}
+
+// everything a gradient entry point checks before its workspace: batched honours the policy's batch strides
+static int pg_validate(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched) {
     if (const int rc = pt_check_desc(pr, batched)) return rc;
     if (batched && !pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
-    if (const int rc = pg_check(pr, g)) return rc;
+    return pg_check(pr, g);
+}
+
+static int pg_entry(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, bool consistent,
+                    pilco_stream_t stream) {
+    if (const int rc = pg_validate(pr, R, g, batched)) return rc;
     return pg_run(pr, R, g, consistent, stream);
 }
 
@@ -976,6 +1181,16 @@ size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr
 int pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                             pilco_stream_t stream) {
     return pg_entry(pr, R, g, true, true, stream);
+}
+
+size_t pilco_particles_score_grad_workspace_bytes(const pilco_particles* pr, int R) {
+    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R).total : 0;
+}
+
+int pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
+                                       pilco_stream_t stream) {
+    if (const int rc = pg_validate(pr, R, g, true)) return rc;
+    return ps_run(pr, R, g, stream);
 }
 
 }  // extern "C"

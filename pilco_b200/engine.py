@@ -530,9 +530,23 @@ class ParticlePlan:
 
     ``consistent=True``: ``launch()`` samples each particle's dynamics as ONE function drawn from the GP posterior
     (pilco_particles_rollout_consistent, DESIGN.md section 14) instead of fresh noise at every step; its workspace is
-    O(P H E n).  Its gradient is ``ConsistentGradPlan``; ``grad=True`` with ``consistent=True`` is a ValueError."""
+    O(P H E n).  Its gradient is ``ConsistentGradPlan``; ``grad=True`` with ``consistent=True`` is a ValueError.
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False):
+    ``estimator`` picks what ``launch_grad()`` estimates d E[return] with: ``"pathwise"`` (the default) differentiates
+    the sampled trajectories; ``"score"`` is the score-function estimator (pilco_particles_rollout_score_grad, DESIGN.md
+    section 16), which differentiates no trajectory, so box terms enter its gradient.  Both give the same rollout and
+    value.  ``"score"`` with ``consistent=True``, or an unknown estimator, is a ValueError."""
+
+    ESTIMATORS = ("pathwise", "score")
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
+                 estimator="pathwise"):
+        if estimator not in self.ESTIMATORS:
+            raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
+        if consistent and estimator == "score":
+            raise ValueError("particles: the score-function gradient of the consistent (function-sample) rollout "
+                             "is not available; use estimator='pathwise'")
+        self.estimator = estimator
         if consistent and grad:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
@@ -560,6 +574,8 @@ class ParticlePlan:
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.estimator == "score":
+            return int(lib.pilco_particles_score_grad_workspace_bytes(C.byref(pr), self.R))
         if self.batched:
             return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
         return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
@@ -617,10 +633,14 @@ class ParticlePlan:
         """pilco_particles_rollout_grad: the rollout (``outputs()`` as after ``launch()``, bitwise) and the pathwise
         gradient of value = mean return w.r.t. the policy parameters with x0 and eps fixed.  Returns the device tensors
         {'value' [1], 'W' [U,Ds], 'b' [U]} (linear) or {'value', 'X' [bf,Ds], 'Y' [bf,U], 'ell' [U,Ds]} (RBF, constrained
-        lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R])."""
+        lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R]).
+        ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        if self.batched:
+        if self.estimator == "score":
+            check(lib.pilco_particles_rollout_score_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
+                  "particles_rollout_score_grad")
+        elif self.batched:
             check(lib.pilco_particles_rollout_batch_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
                   "particles_rollout_batch_grad")
         else:

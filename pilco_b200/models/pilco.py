@@ -164,10 +164,10 @@ class PILCO:
         out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
         return ParticleTrajectories(*out)
 
-    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False):
+    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False, estimator="pathwise"):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
         (from ``np.random`` when None): the same seed gives the same particles to every caller.  ``consistent``
-        (with ``grad``): the ConsistentGradPlan over the same particles."""
+        (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``: ParticlePlan's."""
         dyn = self.mgpr.device_gp()
         x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, what)
         terms, mult_mu = self.reward_spec()
@@ -175,7 +175,7 @@ class PILCO:
             plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu)
         else:
             plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
-                                       grad=grad)
+                                       grad=grad, estimator=estimator)
         plan.set_inputs(x0, eps)
         return plan
 
@@ -210,7 +210,7 @@ class PILCO:
         return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
                                g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
 
-    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
+    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, estimator="pathwise"):
         """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
         are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
         d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
@@ -220,10 +220,22 @@ class PILCO:
         dynamics posterior (DESIGN.md section 15); its workspace grows as num_samples n E N (N training points)
         and is not chunked.
 
+        ``estimator="score"``: the score-function (likelihood-ratio) estimate over the same particles instead (DESIGN.md
+        section 16), with a leave-one-out baseline.  It differentiates no trajectory, so box terms enter grad and the
+        estimate is unbiased for every reward; value and returns are the pathwise call's.  Its variance scales as
+        1 / sigma^2 where the model is confident (a small predicted variance), so it can need many more samples than
+        the pathwise estimate on smooth rewards.  ``consistent=True`` with ``estimator="score"`` is a ValueError.
+
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
+        if estimator not in engine.ParticlePlan.ESTIMATORS:
+            raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
+                             % (engine.ParticlePlan.ESTIMATORS, estimator))
+        if consistent and estimator == "score":
+            raise ValueError("sample_policy_gradient: the score-function estimator is not available for the consistent "
+                             "(function-sample) particles; use estimator='pathwise'")
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
-                                   consistent=consistent)
+                                   consistent=consistent, estimator=estimator)
         g = plan.launch_grad()
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
