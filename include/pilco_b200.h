@@ -178,6 +178,23 @@ int    pilco_gp_predict(const pilco_gp_model* gp, int e0, int ne, int T,
                         double* mean,          /* [T,ne] */
                         double* var,           /* full_cov ? [ne,T,T] : [T,ne] */
                         int full_cov, void* ws, size_t ws_bytes, pilco_stream_t stream);
+/* Posterior function samples at the same inputs (gpflow GPModel.predict_f_samples), given the caller's standard normals:
+ *   full_cov = 1:  samples[s,:,e] = mean_e + L_e eps[s,:,e],  L_e = chol(cov_e + jitter I)  (pilco_gp_predict's covariance)
+ *   full_cov = 0:  samples[s,t,e] = mean[t,e] + sqrt(max(var[t,e], 0)) eps[s,t,e]           (jitter unused)
+ * Same models, validation, status codes and T limits as pilco_gp_predict, plus PILCO_ERR_DIM for S < 1 or a negative
+ * or non-finite jitter.  info[e] is set on the stream: nonzero where cov_e + jitter I is not positive definite (always 0
+ * for full_cov = 0).  Workspace (0: unsupported sizes or size_t overflow):
+ *   full_cov = 0:  pilco_gp_predict's (rounded up to 16 bytes) + 2 T ne doubles  -- O(T)
+ *   full_cov = 1:  max(pilco_gp_predict's, 2 S T ne doubles) + ne T^2 + T ne doubles
+ * No host synchronisation (graph-capturable).  The first S' samples do not depend on S. */
+size_t pilco_gp_predict_samples_workspace_bytes(int n, int D, int E, int T, int S, int full_cov);
+int    pilco_gp_predict_samples(const pilco_gp_model* gp, int e0, int ne, int T, int S,
+                                const double* Xs,      /* [T,D]     */
+                                const double* eps,     /* [S,T,ne]  standard normals */
+                                double* samples,       /* [S,T,ne]  */
+                                int full_cov, double jitter,
+                                int* info,             /* [ne] */
+                                void* ws, size_t ws_bytes, pilco_stream_t stream);
 /* Vector-Jacobian product of the diagonal posterior of ALL E outputs at the inputs:
  *   gXs[t] = d/dXs[t] sum_e (gmean[t,e] mean_e(Xs[t]) + gvar[t,e] var_e(Xs[t]))
  * over the same models and with the same validation and limits as pilco_gp_predict (full_cov = 0).  A point's result

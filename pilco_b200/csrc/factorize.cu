@@ -1102,3 +1102,123 @@ int gp_predict_full_cov(cudaStream_t st, int n, int D, int ne, int T, const doub
     if (rc) return rc;
     return gemm(st, ne, T, T, np, 0, 1, -1.0, W, np, ts, Ks, np, ts, 1.0, cov, T, cs);            // K** - W K*'
 }
+
+// ---- posterior function samples at deterministic inputs (gpflow GPModel.predict_f_samples; DESIGN.md section 17) ----
+//   full_cov = 0:  samples[s,t,e] = mean[t,e] + sqrt(max(var[t,e], 0)) eps[s,t,e]             (one diagonal predict)
+//   full_cov = 1:  samples[s,:,e] = mean[:,e] + L_e eps[s,:,e],  L_e L_e' = cov_e + jitter I     (covariance, Cholesky, GEMM)
+// The GEMM contracts over the full T x T square of L (the strict upper triangle is zeroed first): a triangular product
+// would halve its flops.
+__global__ void __launch_bounds__(256) gp_sample_diag_kernel(long long count, int tn, const double* mean, const double* var,
+                                                             const double* eps, double* out) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) {
+        const int j = (int)(i % tn);
+        out[i] = __dadd_rn(mean[j], __dmul_rn(sqrt(fmax(var[j], 0.0)), eps[i]));     // no FMA: mean + sd * eps as written
+    }
+}
+
+// zero the strict upper triangle of ne [T,T] matrices (the Cholesky leaves the input there); grid (rows, ne)
+__global__ void __launch_bounds__(256) gp_sample_tril_kernel(int T, double* A) {
+    double* Ae = A + (size_t)blockIdx.y * T * T;
+    for (int r = blockIdx.x; r < T; r += gridDim.x)
+        for (int c = r + 1 + threadIdx.x; c < T; c += 256) Ae[(size_t)r * T + c] = 0.0;
+}
+
+// out[c][r] = in[r][c] (+ radd[r]) for an [rows, cols] matrix, 32 x 32 tiles through shared memory, block (32, 8)
+__global__ void __launch_bounds__(256) gp_sample_transpose_kernel(long long rows, long long cols, const double* in,
+                                                                  double* out, const double* radd) {
+    __shared__ double tile[32][33];
+    const long long tr = (rows + 31) / 32, ntile = tr * ((cols + 31) / 32);
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    for (long long b = blockIdx.x; b < ntile; b += gridDim.x) {
+        const long long r0 = (b % tr) * 32, c0 = (b / tr) * 32;
+        __syncthreads();
+        for (int k = ty; k < 32; k += 8) {
+            const long long r = r0 + k, c = c0 + tx;
+            if (r < rows && c < cols) {
+                const double v = in[r * cols + c];
+                tile[k][tx] = radd ? radd[r] + v : v;
+            }
+        }
+        __syncthreads();
+        for (int k = ty; k < 32; k += 8) {
+            const long long c = c0 + k, r = r0 + tx;
+            if (r < rows && c < cols) out[c * rows + r] = tile[tx][k];
+        }
+    }
+}
+
+static unsigned sample_grid(long long work, long long per_block) {
+    const long long b = (work + per_block - 1) / per_block;
+    return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
+}
+
+extern "C" {
+
+size_t pilco_gp_predict_samples_workspace_bytes(int n, int D, int E, int T, int S, int full_cov) {
+    const size_t pb = pilco_gp_predict_workspace_bytes(n, D, E, T, full_cov ? 1 : 0);
+    if (pb == 0 || S < 1) return 0;
+    size_t te = 0, b = 0;
+    if (__builtin_mul_overflow((size_t)T, (size_t)E, &te)) return 0;
+    if (!full_cov) {                                            // predict workspace, then mean and var [T,E]
+        if (__builtin_mul_overflow(te, 2 * sizeof(double), &b) || __builtin_add_overflow(b, (pb + 15) & ~(size_t)15, &b)) return 0;
+        return b;
+    }
+    // max(K* and W of the predict, eps' and L eps [T,E,S] each), then cov [E,T,T] and mean [T,E]
+    size_t es = 0, cov = 0;
+    if ((long long)E * S > 0x7fffffff) return 0;                // leading dimension E S of the GEMM operands
+    if (__builtin_mul_overflow(te, (size_t)S * 2 * sizeof(double), &es)) return 0;
+    if (__builtin_mul_overflow(te, (size_t)T * sizeof(double), &cov)) return 0;
+    b = pb > es ? pb : es;
+    if (__builtin_add_overflow(b, cov, &b) || __builtin_add_overflow(b, te * sizeof(double), &b)) return 0;
+    return b;
+}
+
+int pilco_gp_predict_samples(const pilco_gp_model* gp, int e0, int ne, int T, int S, const double* Xs, const double* eps,
+                             double* samples, int full_cov, double jitter, int* info, void* ws, size_t ws_bytes,
+                             pilco_stream_t stream) {
+    if (!gp || !Xs || !eps || !samples || !info || !ws) return PILCO_ERR_NULL;
+    if (!gp->X || !gp->ell || !gp->sf2 || !gp->beta) return PILCO_ERR_NULL;
+    if (gp->mode != 0 || !gp->iK || gp->X_bs || gp->ell_bs || gp->sf2_bs || gp->beta_bs) return PILCO_ERR_UNSUPPORTED;
+    const int n = gp->n, D = gp->D, E = gp->E;
+    if (n < 1 || D < 1 || D > MAXD || E < 1 || E > MAXE) return PILCO_ERR_DIM;
+    if (T < 1 || T > (full_cov ? 65535 * 8 : 65535 * 32) || ne < 1 || e0 < 0 || e0 + ne > E || S < 1) return PILCO_ERR_DIM;
+    if (!(jitter >= 0.0) || !isfinite(jitter)) return PILCO_ERR_DIM;
+    if (gp->ldk < pad64(n)) return PILCO_ERR_DIM;
+    if (((uintptr_t)gp->iK & 15) || (gp->ldk & 1) || ((uintptr_t)ws & 15)) return PILCO_ERR_ALIGN;
+    const size_t need = pilco_gp_predict_samples_workspace_bytes(n, D, ne, T, S, full_cov);
+    if (need == 0) return PILCO_ERR_DIM;
+    if (ws_bytes < need) return PILCO_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaMemsetAsync(info, 0, sizeof(int) * ne, st);
+    const long long te = (long long)T * ne;
+    const size_t pb = pilco_gp_predict_workspace_bytes(n, D, ne, T, full_cov ? 1 : 0);
+    if (!full_cov) {
+        double* mean = (double*)((char*)ws + ((pb + 15) & ~(size_t)15));
+        double* var = mean + te;
+        if (const int rc = pilco_gp_predict(gp, e0, ne, T, Xs, mean, var, 0, ws, pb, stream)) return rc;
+        const long long count = te * S;
+        gp_sample_diag_kernel<<<sample_grid(count, 256), 256, 0, st>>>(count, (int)te, mean, var, eps, samples);
+        CUDA_LAUNCH_CHECK();
+        return PILCO_OK;
+    }
+    const long long es = te * S;
+    double* epsT = (double*)ws;                                 // [T,ne,S], after the predict is done with K* and W
+    double* Z = epsT + es;                                      // L eps [T,ne,S]
+    double* cov = (double*)((char*)ws + (pb > (size_t)es * 2 * sizeof(double) ? pb : (size_t)es * 2 * sizeof(double)));
+    double* mean = cov + (size_t)ne * T * T;
+    if (const int rc = pilco_gp_predict(gp, e0, ne, T, Xs, mean, cov, 1, ws, pb, stream)) return rc;
+    const long long ms = (long long)T * T;
+    add_diag_const_kernel<<<dim3((T + 127) / 128, ne), 128, 0, st>>>(T, cov, T, ms, jitter);
+    CUDA_LAUNCH_CHECK();
+    if (const int rc = chol_launch(st, ne, T, cov, T, ms, 1, info)) return rc;
+    gp_sample_tril_kernel<<<dim3(T < 4096 ? T : 4096, ne), 256, 0, st>>>(T, cov);
+    gp_sample_transpose_kernel<<<sample_grid(es, 1024), dim3(32, 8), 0, st>>>(S, te, eps, epsT, nullptr);
+    CUDA_LAUNCH_CHECK();
+    // Z_e [T,S] = L_e eps'_e: column block e of the [T, ne S] arrays
+    if (const int rc = gemm(st, ne, T, S, T, 0, 0, 1.0, cov, T, ms, epsT, ne * S, S, 0.0, Z, ne * S, S)) return rc;
+    gp_sample_transpose_kernel<<<sample_grid(es, 1024), dim3(32, 8), 0, st>>>(te, S, Z, samples, mean);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
+}  // extern "C"

@@ -238,6 +238,50 @@ def gp_predict(gp, Xnew, e0=0, ne=None, full_cov=False):
     return mean, var
 
 
+def predict_samples_workspace_bytes(gp, T, S, ne=None, full_cov=True):
+    """pilco_gp_predict_samples_workspace_bytes (0: unsupported sizes)"""
+    ne = gp.E if ne is None else int(ne)
+    return int(lib.pilco_gp_predict_samples_workspace_bytes(gp.n, gp.D, ne, int(T), int(S), 1 if full_cov else 0))
+
+
+def gp_predict_samples(gp, Xnew, eps, e0=0, ne=None, full_cov=True, jitter=1e-6, max_ws_bytes=None):
+    """pilco_gp_predict_samples: posterior function samples of outputs e0 .. e0+ne-1 of the factorised model ``gp`` at
+    Xnew [T,D] given standard normals eps [S,T,ne] -> (samples [S,T,ne], info [ne]) device tensors; info[e] != 0 where
+    the covariance + jitter I of output e is not positive definite.  ``full_cov=False`` draws each point independently
+    from its marginal.  A workspace above ``max_ws_bytes`` (default: half the free device memory) is a ValueError that
+    names the bytes needed and the largest T that would fit, raised before anything is allocated."""
+    Xs, eps = dev(Xnew), dev(eps)
+    if Xs.dim() != 2 or Xs.shape[1] != gp.D:
+        raise ValueError("gp_predict_samples: Xnew must be [T, %d], got %s" % (gp.D, tuple(Xs.shape)))
+    T = int(Xs.shape[0])
+    ne = gp.E - int(e0) if ne is None else int(ne)
+    if eps.dim() != 3 or eps.shape[1:] != (T, ne):
+        raise ValueError("gp_predict_samples: eps must be [S, %d, %d], got %s" % (T, ne, tuple(eps.shape)))
+    S = int(eps.shape[0])
+    if T < 1 or ne < 1 or S < 1:
+        raise ValueError("gp_predict_samples: needs T, ne, S >= 1 (T=%d, ne=%d, S=%d)" % (T, ne, S))
+    wsb = predict_samples_workspace_bytes(gp, T, S, ne, full_cov)
+    if wsb == 0:
+        raise ValueError("gp_predict_samples: unsupported sizes (n=%d, D=%d, ne=%d, T=%d, S=%d)" % (gp.n, gp.D, ne, T, S))
+    d = device()
+    if max_ws_bytes is None:
+        max_ws_bytes = torch.cuda.mem_get_info(d)[0] // 2
+    if wsb > max_ws_bytes:
+        lo = _largest_fitting(lambda t: 0 < predict_samples_workspace_bytes(gp, t, S, ne, full_cov) <= max_ws_bytes,
+                              0, T - 1)
+        raise ValueError("gp_predict_samples: %d samples of %d outputs at T=%d points (full_cov=%s) need %d workspace "
+                         "bytes, more than max_ws_bytes=%d (half the free device memory by default); T=%d would fit"
+                         % (S, ne, T, bool(full_cov), wsb, max_ws_bytes, lo))
+    samples = torch.empty((S, T, ne), dtype=F64, device=d)
+    info = torch.empty(ne, dtype=torch.int32, device=d)
+    ws = torch.empty(wsb // 8, dtype=F64, device=d)
+    g = gp.struct()
+    check(lib.pilco_gp_predict_samples(C.byref(g), int(e0), ne, T, S, ptr(Xs), ptr(eps), ptr(samples),
+                                       1 if full_cov else 0, float(jitter), ptr(info), ptr(ws), wsb, stream_ptr()),
+          "gp_predict_samples")
+    return samples, info
+
+
 def mm_forward(gp, m, s):
     """pilco_mm_forward: m [R,D], s [R,D,D] -> M [R,E], S [R,E,E], V [R,D,E], info [R]."""
     m, s = dev(m), dev(s)

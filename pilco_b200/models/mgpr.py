@@ -6,6 +6,8 @@ Device side: ``pilco_gp_factorize`` (mgpr.py:81-89) and ``pilco_mm_forward`` (mg
 ``pilco_b200.engine``.  Factorisations are cached per (data, hyper-parameter) state instead of being
 recomputed on every call as the reference does (mgpr.py:77-79).
 """
+import numbers
+
 import numpy as np
 import torch
 
@@ -123,6 +125,30 @@ class GPRModel:
             raise NotImplementedError("predict_y with full_cov=True: add the likelihood variance to predict_f's diagonal")
         mean, var = self._predict_device(Xnew, False, full_output_cov)
         return host(mean), host(var + float(self.likelihood.variance))
+
+    def predict_f_samples(self, Xnew, num_samples=None, full_cov=True, full_output_cov=False, *, seed=None):
+        """Latent functions drawn from the posterior at Xnew [T,D]: [num_samples,T,1] ([T,1] when num_samples is None).
+        ``full_cov=True`` draws mean + L eps with L = chol(cov + 1e-6 I), the correlated function values at the T
+        points; ``full_cov=False`` draws each point from its own marginal.  The standard normals come from one device
+        ``torch.Generator`` seeded with ``seed`` (from ``np.random`` when None): the same seed gives the same draw."""
+        if num_samples is not None and (isinstance(num_samples, bool) or not isinstance(num_samples, numbers.Integral)
+                                        or num_samples < 1):
+            raise ValueError("predict_f_samples: num_samples must be None or an integer >= 1, got %r" % (num_samples,))
+        if full_output_cov:
+            raise NotImplementedError("full_output_cov: a GPRModel has a single output")
+        gp, e = self._predict_source()
+        Xs = engine.dev(Xnew)
+        S = 1 if num_samples is None else int(num_samples)
+        if seed is None:
+            seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+        g = torch.Generator(device=Xs.device)
+        g.manual_seed(int(seed))
+        eps = torch.randn((S, Xs.shape[0], 1), dtype=engine.F64, device=Xs.device, generator=g)
+        samples, info = engine.gp_predict_samples(gp, Xs, eps, e0=e, ne=1, full_cov=full_cov)
+        if int(info.max().item()):
+            raise RuntimeError("Cholesky decomposition was not successful (posterior covariance + jitter not positive "
+                               "definite)")
+        return host(samples[0] if num_samples is None else samples)
 
     def predict_log_density(self, data, full_cov=False, full_output_cov=False):
         """log N(Y | mean, var_f + sn2) at each row of data = (X [T,D], Y [T,1]) -> [T]."""
