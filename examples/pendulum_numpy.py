@@ -56,7 +56,7 @@ def rollout(env, policy, timesteps):
     return np.stack(X), np.stack(Y)
 
 
-def run(iters=3, T=25, restarts=4, maxiter=20, bf=10, verbose=True, seed=0):
+def run(iters=3, T=25, restarts=4, maxiter=20, bf=10, verbose=True, seed=0, action_cost=0.0):
     np.random.seed(seed)
     env = PendulumEnv(seed=seed)
     X, Y = rollout(env, lambda x: env.sample_action(), T)
@@ -66,6 +66,9 @@ def run(iters=3, T=25, restarts=4, maxiter=20, bf=10, verbose=True, seed=0):
     state_dim, control_dim = 2, 1
     controller = RbfController(state_dim, control_dim, bf, max_action=env.max_torque)
     reward = ExponentialReward(state_dim, W=np.diag([1.0, 0.1]), t=np.array([np.pi / 3, 0.0]))   # swing to 60 degrees
+    if action_cost:       # a torque cost action_cost (1 - exp(-u^2 / 2)) beside the swing-up reward (a reward on [x, u])
+        from pilco.rewards import CombinedRewards, action_cost as effort
+        reward = CombinedRewards(state_dim, [reward, effort(state_dim, control_dim, [[1.0]])], coefs=[1.0, action_cost])
     pilco = PILCO((X, Y), controller=controller, horizon=T, reward=reward,
                   m_init=np.zeros((1, state_dim)), S_init=np.diag([0.01, 0.01]))
     history = []
@@ -86,5 +89,6 @@ def run(iters=3, T=25, restarts=4, maxiter=20, bf=10, verbose=True, seed=0):
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=3)
+    ap.add_argument("--action-cost", type=float, default=0.0, help="weight of a saturating torque cost (0: none)")
     a = ap.parse_args()
-    run(iters=a.iters)
+    run(iters=a.iters, action_cost=a.action_cost)

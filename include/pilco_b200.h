@@ -224,6 +224,8 @@ int pilco_linear_action(int Ds, int U, int R,
                         double* M /*[R,U]*/, double* S /*[R,U,U]*/, double* V /*[R,Ds,U]*/,
                         pilco_stream_t stream);
 
+/* Ds is the dimension of whatever Gaussian is handed in: the state's, or D = Ds + U for joint state-action moments
+ * (the closed form of PILCO_REWARD_EXP_SA). */
 int pilco_exp_reward(int Ds, int R, const double* W /*[Ds,Ds]*/, const double* t /*[Ds]*/,
                      const double* m /*[R,Ds]*/, const double* s /*[R,Ds,Ds]*/,
                      double* muR /*[R]*/, double* sR /*[R] or NULL*/, int* info,
@@ -248,6 +250,12 @@ int pilco_box_risk(int Ds, int R, const double* prm, const double* m /*[R,Ds]*/,
 #define PILCO_REWARD_EXP    0
 #define PILCO_REWARD_LINEAR 1
 #define PILCO_REWARD_BOX    2   /* pilco_box_risk; W = its prm block, t unused */
+/* Terms on the joint Gaussian of the state and the APPLIED action, x~_t = [x_t, u_t] (D = Ds + U): term k at step t
+ * (t = 0 .. H-1) is evaluated at the (m~, s~) handed to the dynamics moment match of step t, i.e. u_t after squash_sin
+ * when pol.squash.  The final state x_H has no action and gets no joint term.  Control-effort costs live here.
+ * Within a step the state terms are accumulated first, in order, then the joint terms, in order (every path). */
+#define PILCO_REWARD_EXP_SA     3   /* exp(-1/2 (x~-t)' W (x~-t)) moments over the joint:  W [D,D], t [D] */
+#define PILCO_REWARD_LINEAR_SA  4   /* x~' W:  W [D] */
 /* accumulation channel of a reward term (safe_pilco_extension/safe_pilco.py:29-50, SafePILCO.predict):
  *   ADD : reward_add  += coef * value(x_t)                       (PILCO.predict, pilco.py:130-134)
  *   MULT: reward_mult *= 1 - sum_k coef_k * value_k(x_t)          (the terms of this channel form the risk)
@@ -271,8 +279,8 @@ typedef struct pilco_reward_term {
     int kind;                   /* PILCO_REWARD_* */
     int channel;                /* PILCO_CHANNEL_* */
     double coef;                /* CombinedRewards weight (rewards.py:64-81) */
-    const double* W;            /* exp: [Ds,Ds]; linear: [Ds]; box: prm block */
-    const double* t;            /* exp: [Ds] target; linear: unused */
+    const double* W;            /* exp: [Ds,Ds]; linear: [Ds]; box: prm block; exp_sa: [D,D]; linear_sa: [D] */
+    const double* t;            /* exp: [Ds] target; exp_sa: [D] target; otherwise unused */
 } pilco_reward_term;
 
 typedef struct pilco_rollout {
@@ -327,7 +335,8 @@ int    pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad*
  *         squash_sin does at the policy's output variance (0 linear, 1e-6 RBF, as compute_action),
  *   x_{t+1} = x_t + mu(x~_t) + sqrt(max(var(x~_t), 0)) o eps_t,  x~_t = [x_t, u_t]  (latent posterior, no noise),
  *   step_reward / step_risk = the ADD / MULT terms at the point x_t (t < H), ret = sum_t step_reward
- *   (+ mult_mu (1 - prod_t (1 - step_risk)) with MULT terms).
+ *   (+ mult_mu (1 - prod_t (1 - step_risk)) with MULT terms).  Joint terms (PILCO_REWARD_*_SA) are evaluated at the
+ *   point x~_t; within a step the state terms are accumulated first, in order, then the joint terms, in order.
  * H+1 step launches and H pilco_gp_predict calls on `stream`; every argument, the predict step's included, is
  * validated before anything is enqueued.  A particle's outputs do not depend on P or on its row.
  * PILCO_ERR_UNSUPPORTED: dyn not an unbatched mode-0 model with iK, a batched policy, an RBF policy not in mode 1,
@@ -354,7 +363,8 @@ int    pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream)
  * with x0 and eps held fixed.  value[0] = (1/P) sum_p ret_p and the gradient of value w.r.t. the policy parameters:
  * linear gW [U,Ds], gb [U]; RBF gXc [bf,Ds] centres, gYc [bf,U] targets, gell [U,Ds] lengthscales (constrained),
  * through beta = (K + sn2 I)^-1 Yc with pol_L = the Cholesky factors pilco_gp_factorize leaves (as
- * pilco_rollout_grad).  Box terms are flat almost everywhere: they enter value but not the gradient, so for them the
+ * pilco_rollout_grad).  A joint term adds a_kt d v_k / d u_t to the action cotangent and a_kt d v_k / d x_t to the
+ * state cotangent of step t, a_kt the weight the step's state terms carry (step H-1 included).  Box terms are flat almost everywhere: they enter value but not the gradient, so for them the
  * estimator is biased as an estimate of d E[return].  Where a predicted variance is close to 0 the derivative of its
  * square root is large (exact, not clamped); where it is <= 0 it is taken as 0.  Every argument, the forward's
  * included, is validated before anything is enqueued; no host synchronisation (graph-capturable). */
@@ -415,8 +425,13 @@ int    pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R,
  *   w_pt = G_pt - (S_t - G_pt) / (P - 1), G_pt the part of particle p's return that transition t can affect
  *   (the step rewards after t, and mult_mu prod_{s<=t} (1 - risk_s) (1 - prod_{s>t} (1 - risk_s))), S_t = sum_q G_qt
  *   over the restart's particles (a leave-one-out baseline; P = 1: w = G).
+ * With the states held fixed a joint term (PILCO_REWARD_*_SA) still depends on the parameters directly, through
+ * u_t = pi(x_t), so the estimator adds (1/P) sum_p sum_{t<H} a_kt d v_k / d u_t d pi(x_pt) / d theta (a_kt = coef_k, or
+ * coef_k mult_mu prod_{s != t} (1 - risk_s) in the MULT channel; t = H-1 included): without it the gradient would be
+ * biased as soon as a joint term is present.  G_pt needs no change: the step rewards contain the joint terms.
  * Its expectation is d E[return] for every reward kind, box terms included; it differentiates no trajectory, and its
- * variance grows as 1/var where the model is confident.  H <= 1 gives a zero gradient.  A restart's results are
+ * variance grows as 1/var where the model is confident.  H <= 1 gives a zero gradient (H = 1 with joint terms: the
+ * direct term alone).  A restart's results are
  * bitwise independent of R and reproducible run to run; no host synchronisation (graph-capturable). */
 size_t pilco_particles_score_grad_workspace_bytes(const pilco_particles* pr, int R);   /* 0: unsupported / overflow */
 int    pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,

@@ -72,6 +72,8 @@ class ParticlesGrad(C.Structure):
 
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
+REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
+JOINT_REWARDS = (REWARD_EXP_SA, REWARD_LINEAR_SA)
 CHANNEL_ADD, CHANNEL_MULT = 0, 1
 ABI_VERSION = 3
 

@@ -25,6 +25,11 @@
 #define CUDA_LAUNCH_CHECK() do { cudaError_t e__ = cudaGetLastError(); if (e__ != cudaSuccess) return PILCO_ERR_LAUNCH; } while (0)
 
 static inline __host__ __device__ int pad64(int n) { return (n + 63) & ~63; }
+// reward kinds: the *_SA ones are evaluated on the joint state-action Gaussian / point (dimension D), the others on
+// the state (dimension Ds); the exponential ones carry a target t
+static inline __host__ __device__ bool reward_on_joint(int kind) { return kind == PILCO_REWARD_EXP_SA || kind == PILCO_REWARD_LINEAR_SA; }
+static inline bool reward_kind_known(int kind) { return kind >= PILCO_REWARD_EXP && kind <= PILCO_REWARD_LINEAR_SA; }
+static inline bool reward_needs_t(int kind) { return kind == PILCO_REWARD_EXP || kind == PILCO_REWARD_EXP_SA; }
 // row stride (in doubles) of zeta/U rows: multiple of 4 (DMMA k-step) and == 4 or 12 (mod 16) so
 // that the 8-column x 4-k B-fragment read is shared-memory bank-conflict free.
 static inline __host__ __device__ int ldz_of(int D) { return D <= 4 ? 4 : (D <= 12 ? 12 : 20); }

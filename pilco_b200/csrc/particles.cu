@@ -16,6 +16,11 @@
 // on the particle's earlier inputs, and pt_step_kernel closes the step unchanged from the mean and variance it leaves.
 // pilco_particles_rollout_score_grad runs the batched forward and then the score-function gradient (DESIGN.md section
 // 16): per-transition weights and score cotangents, one VJP pass over all steps, z_bar, and the pathwise reduction.
+// Joint state-action reward terms (PILCO_REWARD_*_SA, DESIGN.md section 18) have kernels of their own, launched beside
+// the per-particle ones only when such a term is present: pt_joint_kernel adds their values at x~_t to the step's
+// reward and risk after pt_step<t>, pj_grad_kernel adds their gradients to the VJP output x~_bar_t before pg_step<t> /
+// ps_zbar.  The state kernels see the state terms only (pt_policy), so they are untouched: pt_step_kernel and
+// pg_step_kernel sit at their register limits (127 and 255), and the joint terms would have spilled them.
 #include <initializer_list>
 #include "common.cuh"
 #include "risk_math.cuh"
@@ -157,13 +162,96 @@ __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
     }
 }
 
+// ---- joint state-action reward terms (DESIGN.md section 18) --------------------------------------------------------
+// rewards[] = the joint terms only; n_mult counts the MULT terms of both kinds.  Buffers have T = R P rows.
+struct PjDev : PtPolicy {
+    long long T;
+    int t;                                              // pt_joint: the step; pj_grad: the first step of the grid
+    const double* xh;                                   // pt_joint: x~_t [T,D]; pj_grad: x~ of every step [H,T,D]
+    double* step_reward; double* step_risk;             // [T,H]
+    double* gxt; long long gstep;                       // x~_bar of step t at gxt + t gstep (0: one [T,D] buffer)
+    int first;                                          // first dimension of x~_bar that receives (0, or Ds: actions only)
+};
+
+// exp(-0.5 v' W v), v = x~ - t, or x~' W, at the point xq [D] in global memory: plain loops, a handful of registers
+__device__ __forceinline__ double pj_value(const pilco_reward_term& rt, const double* xq, int D) {
+    double acc = 0.0;
+    if (rt.kind == PILCO_REWARD_LINEAR_SA) {
+        for (int i = 0; i < D; ++i) acc = fma(xq[i], rt.W[i], acc);
+        return acc;
+    }
+    for (int i = 0; i < D; ++i) {
+        double wy = 0.0;
+        for (int k = 0; k < D; ++k) wy = fma(rt.W[i * D + k], xq[k] - rt.t[k], wy);
+        acc = fma(xq[i] - rt.t[i], wy, acc);
+    }
+    return exp(-0.5 * acc);
+}
+
+// grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y, after pt_step<t>: the joint terms at
+// x~_t join the step's reward and risk (state terms first, then these, each in term order)
+__global__ void __launch_bounds__(PT_THREADS) pt_joint_kernel(PjDev a) {
+    PDL_ENTRY();
+    const int p = blockIdx.x * PT_THREADS + threadIdx.x;
+    if (p >= a.P) return;
+    const int D = a.Ds + a.U;
+    const size_t row = (size_t)blockIdx.y * a.P + p, o = row * a.H + a.t;
+    const double* xq = a.xh + row * D;
+    double rew = a.step_reward[o], risk = a.step_risk[o];
+    for (int k = 0; k < a.n_rewards; ++k) {
+        const pilco_reward_term& rt = a.rewards[k];
+        const double v = pj_value(rt, xq, D);
+        if (rt.channel == PILCO_CHANNEL_MULT) risk = fma(rt.coef, v, risk);
+        else rew = fma(rt.coef, v, rew);
+    }
+    a.step_reward[o] = rew;
+    a.step_risk[o] = risk;
+}
+
+// grid (ceil(P / 128) nsteps, R), one thread per (step t = a.t + blockIdx.x / nb, particle p of restart r = blockIdx.y):
+// x~_bar_t[first:] += sum_k a_kt grad v_k(x~_t), a_kt as in the reverse sweep below (coef_k, or coef_k mult_mu
+// prod_{s != t} (1 - risk_s) in the MULT channel)
+__global__ void __launch_bounds__(PT_THREADS) pj_grad_kernel(PjDev a) {
+    PDL_ENTRY();
+    const int nb = (a.P + PT_THREADS - 1) / PT_THREADS;
+    const int t = a.t + blockIdx.x / nb, p = (blockIdx.x % nb) * PT_THREADS + threadIdx.x;
+    if (p >= a.P) return;
+    const int D = a.Ds + a.U, H = a.H;
+    const size_t row = (size_t)blockIdx.y * a.P + p;
+    const double* xq = a.xh + ((size_t)t * a.T + row) * D;
+    double* g = a.gxt + (size_t)t * a.gstep + row * D;
+    double wmult = 0.0;
+    if (a.n_mult > 0) {                                 // as pg_step_kernel
+        const double* rk = a.step_risk + row * H;
+        double pre = 1.0, suf = 1.0;
+        for (int s = 0; s < t; ++s) pre *= 1.0 - rk[s];
+        for (int s = t + 1; s < H; ++s) suf *= 1.0 - rk[s];
+        wmult = a.mult_mu * (pre * suf);
+    }
+    for (int k = 0; k < a.n_rewards; ++k) {
+        const pilco_reward_term& rt = a.rewards[k];
+        const double w = rt.channel == PILCO_CHANNEL_MULT ? rt.coef * wmult : rt.coef;
+        if (rt.kind == PILCO_REWARD_LINEAR_SA) {
+            for (int i = a.first; i < D; ++i) g[i] = fma(w, rt.W[i], g[i]);
+            continue;
+        }
+        const double f = -0.5 * w * pj_value(rt, xq, D);        // gradient -value (W + W') v / 2
+        for (int i = a.first; i < D; ++i) {
+            double wv = 0.0;
+            for (int k2 = 0; k2 < D; ++k2) wv = fma(rt.W[i * D + k2] + rt.W[k2 * D + i], xq[k2] - rt.t[k2], wv);
+            g[i] = fma(f, wv, g[i]);
+        }
+    }
+}
+
 // ---- reverse sweep of pilco_particles_rollout_grad (DESIGN.md section 12) ---------------------------------------------
 // Per particle, x_bar_H = 0 and t = H-1 .. 0 (s_t = sqrt(max(var_t, 0)), z_t the pre-squash action):
 //   mu_bar_t = x_bar_{t+1},  var_bar_t = x_bar_{t+1} o eps_t / (2 s_t) where var_t > 0, else 0
 //   x~_bar_t = pilco_gp_predict_vjp at x~_t;  z_bar_t = x~_bar_t[Ds:] o maxa e^{-su/2} cos(z_t)  (when squashed)
 //   x_bar_t  = x_bar_{t+1} + x~_bar_t[:Ds] + (d pi / dx)' z_bar_t + sum_k a_kt grad v_k(x_t)
 // a_kt = coef_k (ADD) or coef_k mult_mu prod_{s != t} (1 - risk_s) (MULT).  x_H carries no reward, so the sweep
-// starts at t = H-1 with x_bar_H = 0 and x~_bar_{H-1} = 0: H-1 VJP calls.
+// starts at t = H-1 with x_bar_H = 0 and x~_bar_{H-1} = 0: H-1 VJP calls.  With joint terms pj_grad_kernel has added
+// sum_k a_kt grad v_k(x~_t) to x~_bar_t beforehand (at t = H-1 to a zeroed one, which this kernel then reads).
 struct PgDev : PtPolicy {
     int t;
     const double* eps; const double* traj; const double* step_risk;
@@ -598,7 +686,9 @@ __global__ void __launch_bounds__(FS_WARPS * 32, 3) fs_cond_bwd_kernel(FsBwd a) 
 //   gmean_t = w_t eps_t / s_t,  gvar_t = w_t (eps_t^2 - 1) / (2 var_t)   (0 where var_t <= 0)
 //   x~_bar_t = pilco_gp_predict_vjp at x~_t (the steps do not depend on one another: whole groups of steps per call)
 //   z_bar_t = x~_bar_t[Ds:] o maxa e^{-su/2} cos(z_t) (when squashed),  z_bar_{H-1} = 0
-// then pg_reduce as after the pathwise sweep.  Box terms enter G, so they enter the gradient.
+// then pg_reduce as after the pathwise sweep.  Box terms enter G, so they enter the gradient.  Joint terms depend on
+// the parameters directly through u_t = pi(x_t) even with the states held fixed: pj_grad_kernel adds
+// sum_k a_kt d v_k / d u_t to x~_bar_t[Ds:] for every t < H (x~_bar_{H-1} = 0 before it), so z_bar carries the direct term.
 struct PsDev : PtPolicy {
     long long T;                                        // R P rows
     const double* eps; const double* traj; const double* step_reward; const double* step_risk;
@@ -608,6 +698,7 @@ struct PsDev : PtPolicy {
     double* gmean; double* gvar;                        // [H-1,T,Ds] the VJP's cotangents
     const double* gxt;                                  // [H-1,T,D] the VJP's outputs
     double* zbar;                                       // [T,H,U]
+    int direct;                                         // joint terms present: gxt has H steps, z_bar_{H-1} is not 0
 };
 
 // grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y: G_t for t = H-2 .. 0 (H > 1).  The
@@ -677,7 +768,7 @@ __global__ void __launch_bounds__(PT_THREADS) ps_zbar_kernel(PsDev a) {
     const int Ds = a.Ds, U = a.U, H = a.H;
     const size_t row = (size_t)r * a.P + p;
     double* zb = a.zbar + (row * H + t) * U;
-    if (t == H - 1) {                                   // x_H carries no reward
+    if (t == H - 1 && !a.direct) {                      // x_H carries no reward
         for (int j = 0; j < U; ++j) zb[j] = 0.0;
         return;
     }
@@ -748,6 +839,10 @@ struct PtTake {
 };
 
 static bool pt_rbf(const pilco_particles* pr) { return pr->pol.kind == PILCO_POLICY_RBF; }
+static bool pt_has_joint(const pilco_particles* pr) {
+    for (int k = 0; k < pr->n_rewards && k < 8; ++k) if (reward_on_joint(pr->rewards[k].kind)) return true;
+    return false;
+}
 
 // the marginal rollout: x~, the predict outputs and one predict workspace at T = P
 static PtWs pt_ws_layout(const pilco_particles* pr) {
@@ -833,7 +928,9 @@ static PtWs ps_ws_layout(const pilco_particles* pr, int R) {
     PtWs L = {}; PtTake take;
     L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
     L.G = take({Hm, T}); L.gsum = take({(size_t)R, H});
-    L.gx = take({Hm, T, Ds}); L.gvar = take({Hm, T, Ds}); L.gxt = take({Hm, T, D}); L.zbar = take({T, H, U});
+    L.gx = take({Hm, T, Ds}); L.gvar = take({Hm, T, Ds});
+    L.gxt = take({pt_has_joint(pr) ? H : Hm, T, D});    // joint terms: step H-1 too, for their direct term
+    L.zbar = take({T, H, U});
     L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
     L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
     const int grp = ps_group((long long)T, (int)H);
@@ -890,9 +987,9 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
     for (int k = 0; k < pr->n_rewards; ++k) {
         const pilco_reward_term& rt = pr->rewards[k];
         if (!rt.W) return PILCO_ERR_NULL;
-        if (rt.kind != PILCO_REWARD_EXP && rt.kind != PILCO_REWARD_LINEAR && rt.kind != PILCO_REWARD_BOX) return PILCO_ERR_UNSUPPORTED;
+        if (!reward_kind_known(rt.kind)) return PILCO_ERR_UNSUPPORTED;
         if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
-        if (rt.kind == PILCO_REWARD_EXP && !rt.t) return PILCO_ERR_NULL;
+        if (reward_needs_t(rt.kind) && !rt.t) return PILCO_ERR_NULL;
     }
     if (!pr->x0 || !pr->eps || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret)
         return PILCO_ERR_NULL;
@@ -916,7 +1013,9 @@ static int pg_check(const pilco_particles* pr, const pilco_particles_grad* g) {
     return PILCO_OK;
 }
 
-static PtPolicy pt_policy(const pilco_particles* pr) {
+// joint = false: the state terms, for the per-particle state kernels; true: the joint state-action terms, for
+// pt_joint_kernel / pj_grad_kernel.  n_mult counts the MULT terms of both.
+static PtPolicy pt_policy(const pilco_particles* pr, bool joint = false) {
     const pilco_policy& pol = pr->pol;
     const bool rbf = pol.kind == PILCO_POLICY_RBF;
     PtPolicy a;
@@ -927,11 +1026,23 @@ static PtPolicy pt_policy(const pilco_particles* pr) {
     a.W_bs = rbf ? 0 : pol.W_bs; a.b_bs = rbf ? 0 : pol.b_bs;
     a.C_bs = rbf ? pol.rbf.X_bs : 0; a.ell_bs = rbf ? pol.rbf.ell_bs : 0;
     a.sf2_bs = rbf ? pol.rbf.sf2_bs : 0; a.beta_bs = rbf ? pol.rbf.beta_bs : 0;
-    a.n_rewards = pr->n_rewards; a.n_mult = 0;
-    for (int k = 0; k < 8; ++k) a.rewards[k] = pr->rewards[k];
-    for (int k = 0; k < pr->n_rewards; ++k) a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
+    a.n_rewards = 0; a.n_mult = 0;
+    for (int k = 0; k < 8; ++k) a.rewards[k] = pilco_reward_term();
+    for (int k = 0; k < pr->n_rewards; ++k) {
+        if (reward_on_joint(pr->rewards[k].kind) == joint) a.rewards[a.n_rewards++] = pr->rewards[k];
+        a.n_mult += pr->rewards[k].channel == PILCO_CHANNEL_MULT;
+    }
     a.mult_mu = pr->mult_mu;
     return a;
+}
+
+static PjDev pj_dev(const pilco_particles* pr, int R) {
+    PjDev j;
+    static_cast<PtPolicy&>(j) = pt_policy(pr, true);
+    j.T = (long long)R * pr->P; j.t = 0; j.xh = nullptr;
+    j.step_reward = pr->step_reward; j.step_risk = pr->step_risk;
+    j.gxt = nullptr; j.gstep = 0; j.first = 0;
+    return j;
 }
 
 int fs_predict_prepare();
@@ -962,6 +1073,8 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
     c.xh = ws + L.xt; c.mu = ws + L.mu; c.s2 = ws + L.s2; c.W = ws + L.W; c.Kh = ws + L.Kh;
     c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean;
+    const bool joint = pt_has_joint(pr);
+    PjDev j = pj_dev(pr, R);
     for (int t = 0; t <= H; ++t) {
         a.t = t;
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
@@ -969,6 +1082,11 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
         launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
         if (t == H) break;
+        if (joint) {
+            j.t = t; j.xh = a.xt;
+            launch_hi(pt_joint_kernel, grid, dim3(PT_THREADS), 0, st, j);
+            CUDA_LAUNCH_CHECK();
+        }
         double* var = ws + L.var + (size_t)t * vstep;
         if (consistent) {
             const int rc = fs_predict_launch(st, &pr->dyn, T, a.xt, ws + L.mu, ws + L.s2, ws + L.W, ws + L.Kh + t * slot,
@@ -1038,9 +1156,16 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
     q.xh = ws + L.xt; q.Kh = ws + L.Kh; q.L = ws + L.L; q.eps = pr->eps;
     q.gx = b.gx; q.gvar = b.gvar; q.G = ws + L.G; q.A = ws + L.W; q.dir = ws + L.dir;
+    const bool joint = pt_has_joint(pr);
+    PjDev j = pj_dev(pr, R);
+    j.xh = ws + L.xt; j.gxt = ws + L.gxt;
+    if (joint && H > 0) {                               // x_bar_H = 0 and x~_bar_{H-1} = 0, then the joint terms' share
+        cudaMemsetAsync(b.gx, 0, TDs * sizeof(double), st);
+        cudaMemsetAsync(ws + L.gxt, 0, TD * sizeof(double), st);
+    }
     for (int t = H - 1; t >= 0; --t) {
         b.t = t;
-        b.gxt = nullptr;
+        b.gxt = joint ? ws + L.gxt : nullptr;
         if (t < H - 1) {
             const double* xt = ws + L.xt + (size_t)t * TD;
             int rc;
@@ -1054,6 +1179,11 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             }
             if (rc) return rc;
             b.gxt = ws + L.gxt;
+        }
+        if (joint) {
+            j.t = t;
+            launch_hi(pj_grad_kernel, grid, dim3(PT_THREADS), 0, st, j);
+            CUDA_LAUNCH_CHECK();
         }
         b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * TDs : nullptr;
         launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
@@ -1103,6 +1233,7 @@ static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
     a.eps = pr->eps; a.traj = pr->traj; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
     a.var = ws + L.var; a.G = ws + L.G; a.S = ws + L.gsum; a.gmean = ws + L.gx; a.gvar = ws + L.gvar;
     a.gxt = ws + L.gxt; a.zbar = ws + L.zbar;
+    a.direct = pt_has_joint(pr);
     if (H > 1) {
         launch_hi(ps_togo_kernel, dim3(nb, R), dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
@@ -1118,6 +1249,14 @@ static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
                                                 ws + L.gvar + o * Ds, ws + L.gxt + o * D, ws + L.vws, L.vws_bytes, st);
             if (rc) return rc;
         }
+    }
+    if (H > 0 && a.direct) {                            // the direct term: d v_k / d u_t of every step, on top of the VJP's
+        const size_t TD = (size_t)T * D;
+        cudaMemsetAsync(ws + L.gxt + (size_t)(H - 1) * TD, 0, TD * sizeof(double), st);
+        PjDev j = pj_dev(pr, R);
+        j.xh = ws + L.xt; j.gxt = ws + L.gxt; j.gstep = (long long)TD; j.first = Ds;
+        launch_hi(pj_grad_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, j);
+        CUDA_LAUNCH_CHECK();
     }
     if (H > 0) {
         launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);

@@ -9,7 +9,10 @@
 // and a final ro_state<H> that closes the last step.  The expected rewards depend on the trajectory only, so they are
 // NOT on this chain (an LU factorisation per step and restart would sit on the serial path of every step): one
 // ro_reward launch over all (t, r) after the last step, then ro_reward_sum adds them in step order (same summation
-// order, hence the same bits, as a running sum).
+// order, hence the same bits, as a running sum).  Terms on the joint state-action Gaussian (PILCO_REWARD_*_SA) read
+// the per-step joints the cascade keeps in the workspace for the reverse sweep: ro_reward_joint, launched between the two
+// only when such a term is present, adds them to each step's reward and risk (state terms first, then joint terms, each in
+// term order).  ro_reward sees the state terms only, so a rollout without joint terms runs exactly the kernels it always ran.
 #include "rollout.cuh"
 #include "mm_tape.cuh"
 #include "small_kernels.cuh"
@@ -119,6 +122,32 @@ __global__ void __launch_bounds__(128) ro_reward_kernel(RoDev p) {
     }
 }
 
+// the joint state-action terms of every step, CTA = (step t, restart r): p.rewards holds those terms only and p.mj, p.sj
+// the joint Gaussians of step 0 (step t is R D, R D D doubles further on): what the dynamics moment match of step t received
+__global__ void __launch_bounds__(128) ro_reward_joint_kernel(RoDev p) {
+    PDL_ENTRY();
+    __shared__ SmallScratch sc;
+    const int t = blockIdx.x, r = blockIdx.y, D = p.Ds + p.U;
+    const double* mj = p.mj + ((size_t)t * p.R + r) * D;
+    const double* sj = p.sj + ((size_t)t * p.R + r) * D * D;
+    const size_t o = (size_t)t * p.R + r;
+    double rew = p.rew[o], risk = p.n_mult > 0 ? p.risk[o] : 0.0;
+    for (int k = 0; k < p.n_rewards; ++k) {
+        const pilco_reward_term& rt = p.rewards[k];
+        const double mu = dev_joint_reward_value(D, rt, mj, sj, sc);
+        if (rt.channel == PILCO_CHANNEL_MULT) risk = fma(rt.coef, mu, risk);
+        else rew = fma(rt.coef, mu, rew);
+    }
+    if (threadIdx.x == 0) {
+        p.rew[o] = rew;
+        if (p.step_reward) p.step_reward[(size_t)r * p.H + t] = rew;
+        if (p.n_mult > 0) {
+            p.risk[o] = risk;
+            if (p.step_risk) p.step_risk[(size_t)r * p.H + t] = risk;
+        }
+    }
+}
+
 // reward[r] = sum_t rew[t, r] in step order  (+ SafePILCO.predict, safe_pilco.py:49: mu (1 - prod_t (1 - risk_t)))
 __global__ void __launch_bounds__(128) ro_reward_sum_kernel(RoDev p) {
     PDL_ENTRY();
@@ -152,8 +181,8 @@ int ro_check(const pilco_rollout* ro) {
     for (int k = 0; k < ro->n_rewards; ++k) {
         if (!ro->rewards[k].W) return PILCO_ERR_NULL;
         const int kind = ro->rewards[k].kind, ch = ro->rewards[k].channel;
-        if (kind == PILCO_REWARD_EXP && !ro->rewards[k].t) return PILCO_ERR_NULL;
-        if (kind != PILCO_REWARD_EXP && kind != PILCO_REWARD_LINEAR && kind != PILCO_REWARD_BOX) return PILCO_ERR_UNSUPPORTED;
+        if (reward_needs_t(kind) && !ro->rewards[k].t) return PILCO_ERR_NULL;
+        if (!reward_kind_known(kind)) return PILCO_ERR_UNSUPPORTED;
         if (ch != PILCO_CHANNEL_ADD && ch != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
     }
     if (!ro->m0 || !ro->S0 || !ro->traj_m || !ro->traj_S || !ro->reward || !ro->ws) return PILCO_ERR_NULL;
@@ -194,8 +223,14 @@ int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
     d.R = R; d.H = H; d.Ds = Ds; d.U = U;
     d.pol_kind = ro->pol.kind; d.squash = ro->pol.squash; d.maxa = ro->pol.max_action;
     d.W = ro->pol.W; d.W_bs = ro->pol.W_bs; d.b = ro->pol.b; d.b_bs = ro->pol.b_bs;
-    d.n_rewards = ro->n_rewards;
-    for (int k = 0; k < 8; ++k) d.rewards[k] = ro->rewards[k];
+    int n_joint = 0;                                  // the state terms go to ro_reward, the joint ones to ro_reward_joint
+    pilco_reward_term joint_terms[8];
+    d.n_rewards = 0;
+    for (int k = 0; k < 8; ++k) d.rewards[k] = joint_terms[k] = pilco_reward_term();
+    for (int k = 0; k < ro->n_rewards; ++k) {
+        if (reward_on_joint(ro->rewards[k].kind)) joint_terms[n_joint++] = ro->rewards[k];
+        else d.rewards[d.n_rewards++] = ro->rewards[k];
+    }
     d.m0 = ro->m0; d.m0_bs = ro->m0_bs; d.S0 = ro->S0; d.S0_bs = ro->S0_bs;
     d.traj_m = ro->traj_m; d.traj_S = ro->traj_S; d.reward = ro->reward; d.step_reward = ro->step_reward;
     d.risk = ws + L.risk; d.rew = ws + L.rew; d.step_risk = ro->step_risk; d.mult_mu = ro->mult_mu; d.n_mult = ro_count_mult(ro);
@@ -245,6 +280,14 @@ int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
     }
     if (H > 0) {
         launch_hi(ro_reward_kernel, dim3(H, R), dim3(128), 0, st, d);
+        CUDA_LAUNCH_CHECK();
+    }
+    if (H > 0 && n_joint > 0) {
+        RoDev dj = d;
+        dj.n_rewards = n_joint;
+        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
+        dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
+        launch_hi(ro_reward_joint_kernel, dim3(H, R), dim3(128), 0, st, dj);
         CUDA_LAUNCH_CHECK();
     }
     launch_hi(ro_reward_sum_kernel, dim3((R + 127) / 128), dim3(128), 0, st, d);

@@ -5,7 +5,9 @@
 //
 // The sweep is a strictly serial chain over the H steps, so its cost at small batches is (kernels per step) x
 // (latency of each): the chain is kept short.
-//   once      rb_reward  grid (R,H): d reward_t / d(m_t, S_t) of EVERY step -- it depends on the saved trajectory only
+//   once      rb_reward  grid (R,H): d reward_t / d(m_t, S_t) of EVERY step -- it depends on the saved trajectory only;
+//                        with joint state-action terms rb_reward_joint likewise: d reward_t / d(m~_t, s~_t) at the saved joint
+//                        Gaussians, which rb_post adds to the joint's cotangent before the joint VJP hands it on
 //   per step t = H-1 .. 0, with a tape (pilco_rollout.tape):
 //     rb_dyn_finish  grid (E+P, R): tape-driven VJP of the dynamics moment match (mm_tape_bfinish_task; the glue seeds
 //                    gM = gm, gS, gV = s1'(gS+gS') are formed inline); the LAST CTA of a restart to arrive then runs
@@ -24,8 +26,13 @@ void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, i
                            const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
 
 struct RbWs {            // backward workspace (offsets in doubles)
-    size_t gm, gS, gMd, gSd, gVd, gmj, gsj, gsjx, gMp, gSp, gVp, gbeta, gy, rgm, rgS, cnt, dynb, polb, total;
+    size_t gm, gS, gMd, gSd, gVd, gmj, gsj, gsjx, gMp, gSp, gVp, gbeta, gy, rgm, rgS, jgm, jgS, cnt, dynb, polb, total;
 };
+
+static bool rb_has_joint(const pilco_rollout* ro) {
+    for (int k = 0; k < ro->n_rewards && k < 8; ++k) if (reward_on_joint(ro->rewards[k].kind)) return true;
+    return false;
+}
 
 static RbWs rb_ws_layout(const pilco_rollout* ro) {
     const size_t R = ro->R, H = ro->H, Ds = ro->pol.Ds, U = ro->pol.U, D = Ds + U;
@@ -39,6 +46,9 @@ static RbWs rb_ws_layout(const pilco_rollout* ro) {
     L.gbeta = take(U * bf); L.gy = take(U * bf);
     // reward gradients of every step, per channel (0: additive, 1: multiplicative): [H][2][R][Ds], [H][2][R][Ds*Ds]
     L.rgm = take(H * 2 * Ds); L.rgS = take(H * 2 * Ds * Ds);
+    // likewise for the joint state-action terms, only when there is one: [H][2][R][D], [H][2][R][D*D]
+    const size_t Hj = rb_has_joint(ro) ? H : 0;
+    L.jgm = take(Hj * 2 * D); L.jgS = take(Hj * 2 * D * D);
     L.cnt = take(1);                                           // arrival counters of rb_dyn_finish (one per restart)
     // dynamics GP: task partials of the tape-driven reverse sweep, or the workspace of the recomputing one
     L.dynb = o;
@@ -65,6 +75,8 @@ struct RbDev {
     double *gm, *gS, *gMd, *gSd, *gVd, *gmj, *gsj, *gsjx, *gMp, *gSp, *gVp;
     double *gW, *gb;      // linear policy gradient accumulators [R,U,Ds], [R,U]
     double *rgm, *rgS;    // reward gradients of every step (rb_reward_kernel)
+    double *jgm, *jgS;    // the joint state-action terms' gradients of every step, NULL without such terms
+    const double *mj0, *sj0;  // forward joint Gaussians of step 0; step t is R D (R D D) doubles further on
     // taped dynamics VJP: task partials [R][ntask][MAXD + D*D] that rb_post sums into gmj / gsj itself (else NULL);
     // then the glue cotangent gsjx is formed in shared memory too (no rb_pre launch)
     const double* tpart; int tp_ntask;
@@ -93,6 +105,29 @@ __global__ void __launch_bounds__(128) rb_reward_kernel(RbDev p) {
         const pilco_reward_term& rt = p.rewards[k];
         const bool mult = rt.channel == PILCO_CHANNEL_MULT;
         dev_reward_bwd(Ds, rt, mx, sx, rt.coef, mult ? gm1 : gm0, mult ? gS1 : gS0, sc);
+    }
+}
+
+// the same for the joint state-action terms, at the forward's joint Gaussian (m~_t, s~_t) of every step: p.rewards holds
+// those terms only, jgm / jgS their per-channel gradients [H][2][R][D], [H][2][R][D*D]
+__global__ void __launch_bounds__(128) rb_reward_joint_kernel(RbDev p) {
+    PDL_ENTRY();
+    __shared__ SmallScratch sc;
+    const int r = blockIdx.x, t = blockIdx.y, D = p.Ds + p.U;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const double* mj = p.mj0 + ((size_t)t * p.R + r) * D;
+    const double* sj = p.sj0 + ((size_t)t * p.R + r) * D * D;
+    double* gm0 = p.jgm + (((size_t)t * 2) * p.R + r) * D;
+    double* gS0 = p.jgS + (((size_t)t * 2) * p.R + r) * D * D;
+    double* gm1 = gm0 + (size_t)p.R * D;
+    double* gS1 = gS0 + (size_t)p.R * D * D;
+    for (int i = tid; i < D; i += nt) { gm0[i] = 0.0; gm1[i] = 0.0; }
+    for (int e = tid; e < D * D; e += nt) { gS0[e] = 0.0; gS1[e] = 0.0; }
+    __syncthreads();
+    for (int k = 0; k < p.n_rewards; ++k) {
+        const pilco_reward_term& rt = p.rewards[k];
+        const bool mult = rt.channel == PILCO_CHANNEL_MULT;
+        dev_joint_reward_bwd(D, rt, mj, sj, rt.coef, mult ? gm1 : gm0, mult ? gS1 : gS0, sc);
     }
 }
 
@@ -144,6 +179,23 @@ __device__ __forceinline__ void rb_post_body(const RbDev& p, int r, RbPostSmem& 
             sm.gsjx[e] = v;
         }
         gsjx = sm.gsjx;
+        __syncthreads();
+    }
+    // MULT channel (safe_pilco.py:44-49): d[mu (1 - prod_t' (1 - risk_t'))] / d risk_t = mu prod_{t' != t} (1 - risk_t')
+    double wmult = p.mult_mu;
+    if (wmult != 0.0)
+        for (int tt = 0; tt < p.H; ++tt) if (tt != t) wmult *= 1.0 - p.risk[(size_t)tt * p.R + r];
+    if (p.jgm) {
+        // joint state-action terms: their gradients at (m~_t, s~_t) join the cotangent the dynamics VJP left, with the
+        // state terms' per-channel weights, so the joint VJP below distributes them to (m_x, S_x) and the policy moments
+        double* gmj_w = p.gmj + (size_t)r * D;
+        double* gsj_w = p.gsj + (size_t)r * D * D;
+        const double* ja_m = p.jgm + (((size_t)t * 2) * p.R + r) * D;
+        const double* ja_S = p.jgS + (((size_t)t * 2) * p.R + r) * D * D;
+        const double* jm_m = ja_m + (size_t)p.R * D;
+        const double* jm_S = ja_S + (size_t)p.R * D * D;
+        for (int i = tid; i < D; i += nt) gmj_w[i] += ja_m[i] + wmult * jm_m[i];
+        for (int e = tid; e < D * D; e += nt) gsj_w[e] += ja_S[e] + wmult * jm_S[e];
         __syncthreads();
     }
     const double* gmj = p.gmj + (size_t)r * D;
@@ -203,11 +255,7 @@ __device__ __forceinline__ void rb_post_body(const RbDev& p, int r, RbPostSmem& 
         dev_linear_bwd(Ds, U, p.W + (size_t)r * p.W_bs, mx, sx, gMp, gSp, gVp,
                        p.gW + (size_t)r * U * Ds, p.gb + (size_t)r * U, gm, gS, sc);
     }
-    // ---- reward VJP at state t (pilco.py:133): precomputed per channel by rb_reward_kernel ----
-    // MULT channel (safe_pilco.py:44-49): d[mu (1 - prod_t' (1 - risk_t'))] / d risk_t = mu prod_{t' != t} (1 - risk_t')
-    double wmult = p.mult_mu;
-    if (wmult != 0.0)
-        for (int tt = 0; tt < p.H; ++tt) if (tt != t) wmult *= 1.0 - p.risk[(size_t)tt * p.R + r];
+    // ---- reward VJP at state t (pilco.py:133): precomputed per channel by rb_reward_kernel, weighted by wmult ----
     const double* ra_m = p.rgm + (((size_t)t * 2) * p.R + r) * Ds;
     const double* ra_S = p.rgS + (((size_t)t * 2) * p.R + r) * Ds * Ds;
     const double* rm_m = ra_m + (size_t)p.R * Ds;
@@ -351,8 +399,14 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
     d.R = R; d.H = H; d.Ds = Ds; d.U = U;
     d.pol_kind = ro->pol.kind; d.squash = ro->pol.squash; d.maxa = ro->pol.max_action;
     d.W = ro->pol.W; d.W_bs = ro->pol.W_bs;
-    d.n_rewards = ro->n_rewards;
-    for (int k = 0; k < 8; ++k) d.rewards[k] = ro->rewards[k];
+    int n_joint = 0;                                  // the state terms go to rb_reward, the joint ones to rb_reward_joint
+    pilco_reward_term joint_terms[8];
+    d.n_rewards = 0;
+    for (int k = 0; k < 8; ++k) d.rewards[k] = joint_terms[k] = pilco_reward_term();
+    for (int k = 0; k < ro->n_rewards; ++k) {
+        if (reward_on_joint(ro->rewards[k].kind)) joint_terms[n_joint++] = ro->rewards[k];
+        else d.rewards[d.n_rewards++] = ro->rewards[k];
+    }
     d.traj_m = ro->traj_m; d.traj_S = ro->traj_S;
     d.risk = fws + FL.risk; d.mult_mu = ro_count_mult(ro) > 0 ? ro->mult_mu : 0.0;
     d.gm = buf(BL.gm); d.gS = buf(BL.gS); d.gMd = buf(BL.gMd); d.gSd = buf(BL.gSd); d.gVd = buf(BL.gVd);
@@ -360,6 +414,9 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
     d.gMp = buf(BL.gMp); d.gSp = buf(BL.gSp); d.gVp = buf(BL.gVp);
     d.gW = g->gW; d.gb = g->gb;
     d.rgm = buf(BL.rgm); d.rgS = buf(BL.rgS);
+    const bool joint = rb_has_joint(ro);
+    d.jgm = joint ? buf(BL.jgm) : nullptr; d.jgS = joint ? buf(BL.jgS) : nullptr;
+    d.mj0 = fws + FL.mj; d.sj0 = fws + FL.sj;
     d.tpart = ro->tape ? bws + BL.dynb : nullptr;
     d.tp_ntask = ro->dyn.E + npairs_of(ro->dyn.E);
     d.cnt = reinterpret_cast<unsigned*>(buf(BL.cnt));
@@ -368,6 +425,13 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
         d.sj = d.Vd = d.Mp = d.Sp = d.Vp = d.Mu = d.Su = d.Cq = d.Vu = nullptr;
         launch_hi(rb_reward_kernel, dim3(R, H), dim3(128), 0, st, d);     // reward gradients of every step at once
         CUDA_LAUNCH_CHECK();
+        if (joint) {
+            RbDev dj = d;
+            dj.n_rewards = n_joint;
+            for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
+            launch_hi(rb_reward_joint_kernel, dim3(R, H), dim3(128), 0, st, dj);
+            CUDA_LAUNCH_CHECK();
+        }
     }
 
     for (int t = H - 1; t >= 0; --t) {

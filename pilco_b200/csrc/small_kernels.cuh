@@ -173,6 +173,14 @@ __device__ __forceinline__ double dev_reward_value(int Ds, const pilco_reward_te
     return dev_linear_reward(Ds, rt.W, m, s, nullptr);
 }
 
+// Expected value of one term on the joint state-action Gaussian (PILCO_REWARD_*_SA) at its moments (m, s) of dimension
+// D = Ds + U: the same closed forms (SmallScratch holds MAXD x SLD either way); every thread gets the value.
+__device__ __forceinline__ double dev_joint_reward_value(int D, const pilco_reward_term& rt, const double* m, const double* s,
+                                                         SmallScratch& sc) {
+    if (rt.kind == PILCO_REWARD_EXP_SA) return dev_exp_reward(D, rt.W, rt.t, m, s, nullptr, sc);
+    return dev_linear_reward(D, rt.W, m, s, nullptr);
+}
+
 // ---------------------------------------------------------------------------------------------
 // VJPs (numpy statement: oracle/staged.py).  All "g*" outputs marked += accumulate.
 // ---------------------------------------------------------------------------------------------
@@ -321,6 +329,16 @@ __device__ __forceinline__ void dev_reward_bwd(int Ds, const pilco_reward_term& 
     else if (rt.kind == PILCO_REWARD_BOX) dev_box_risk_bwd(Ds, rt.W, m, s, scale, gm, gS);
     else {
         for (int i = threadIdx.x; i < Ds; i += blockDim.x) gm[i] += scale * rt.W[i];
+        __syncthreads();
+    }
+}
+
+// VJP of one joint state-action term (dev_joint_reward_value) with upstream weight `scale` (accumulates into gm, gS)
+__device__ __forceinline__ void dev_joint_reward_bwd(int D, const pilco_reward_term& rt, const double* m, const double* s,
+                                                     double scale, double* gm, double* gS, SmallScratch& sc) {
+    if (rt.kind == PILCO_REWARD_EXP_SA) dev_exp_reward_bwd(D, rt.W, rt.t, m, s, scale, gm, gS, sc);
+    else {
+        for (int i = threadIdx.x; i < D; i += blockDim.x) gm[i] += scale * rt.W[i];
         __syncthreads();
     }
 }

@@ -432,11 +432,25 @@ def _fill_policy(pol, policy_spec, batched=None):
 
 
 def _fill_rewards(desc, reward_terms):
-    """Fill ``desc.n_rewards`` and ``desc.rewards`` from reward-term dicts; returns the device tensors [(W, t)] they
-    point to"""
+    """Fill ``desc.n_rewards`` and ``desc.rewards`` from reward-term dicts (``desc.pol`` already filled); returns the
+    device tensors [(W, t)] they point to.  The shapes of a joint state-action term are checked against the policy
+    here, before any device work: ValueError."""
     rw = []
+    if len(reward_terms) > 8:
+        raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
     desc.n_rewards = len(reward_terms)
+    Ds, U = int(desc.pol.Ds), int(desc.pol.U)
     for k, rt in enumerate(reward_terms):
+        if rt["kind"] in _lib.JOINT_REWARDS:
+            D = Ds + U
+            if (rt.get("state_dim", Ds), rt.get("control_dim", U)) != (Ds, U):
+                raise ValueError("reward term %d is built for state_dim=%s, control_dim=%s; the policy has %d and %d"
+                                 % (k, rt.get("state_dim"), rt.get("control_dim"), Ds, U))
+            wshape = (D, D) if rt["kind"] == _lib.REWARD_EXP_SA else (D,)
+            if np.shape(rt["W"]) != wshape or (rt["kind"] == _lib.REWARD_EXP_SA and np.shape(rt.get("t")) != (D,)):
+                raise ValueError("reward term %d on the joint [x, u]: W must be %s%s for state_dim=%d, control_dim=%d, "
+                                 "got W %s, t %s" % (k, list(wshape), " and t [%d]" % D if len(wshape) == 2 else "", Ds, U,
+                                                     np.shape(rt["W"]), np.shape(rt.get("t"))))
         W = dev(rt["W"]); t = dev(rt["t"]) if rt.get("t") is not None else None
         rw.append((W, t))
         desc.rewards[k].kind = rt["kind"]
