@@ -1,12 +1,33 @@
-"""Numpy statement of the particle rollout (pilco_particles_rollout, DESIGN.md section 11) for the tests: P particles
-from the caller's x0 [P,Ds], driven by the caller's standard normals eps [P,H,Ds], through a factorised dynamics GP
-(centres C, ell, sf2, iK, beta) under a linear or RBF policy, with the reward terms evaluated at each particle's
-pre-step state.  Test infrastructure only; vectorised over particles."""
+"""Numpy statement of the particle rollouts for the tests: P particles from the caller's x0 [P,Ds], driven by the
+caller's standard normals eps [P,H,Ds], through a factorised dynamics GP (centres C, ell, sf2, iK, beta) under a linear
+or RBF policy, with the reward terms evaluated at each particle's pre-step state and action.
+
+  * ``particle_rollout``: the step-wise sampler (pilco_particles_rollout, DESIGN.md section 11), a fresh draw from the
+    latent marginal at every step;
+  * ``consistent_rollout``: the consistent sampler (pilco_particles_rollout_consistent, DESIGN.md section 14), each
+    particle following ONE function per dynamics output drawn from the latent posterior
+    k_post(a, b) = k_e(a, b) - k(a, C) iK_e k(C, b), sampled sequentially along the particle's own inputs with the
+    semidefinite Cholesky rule (a pivot d2 <= TAU sf2_e leaves its column out of later substitutions).
+
+State terms (REWARD_EXP / LINEAR / BOX) see x_t, joint terms (REWARD_EXP_SA / LINEAR_SA, DESIGN.md section 18) see
+[x_t, u_t]; within a step the state terms are added first, then the joint terms, each in term order, as on the device.
+Also the score estimator's return-to-go weights (DESIGN.md section 16).  Test infrastructure only; vectorised over
+particles and outputs."""
 import numpy as np
 
 from pilco_b200 import _lib
 
 RBF_VAR = 1e-6          # output variance of the deterministic-GP (RBF) policy at a point, as compute_action sees it
+TAU = 1e-10
+JOINT = (_lib.REWARD_EXP_SA, _lib.REWARD_LINEAR_SA)
+
+
+def is_joint(term):
+    return term["kind"] in JOINT
+
+
+def is_mult(term):
+    return int(term.get("channel", _lib.CHANNEL_ADD)) == _lib.CHANNEL_MULT
 
 
 def se_k(Xs, C, ell, sf2):
@@ -50,39 +71,157 @@ def box_point(prm, x):
     return (ok == inside).astype(np.float64)
 
 
-def reward_value(term, x):
-    """one reward term (engine dict: kind, W, t) at the points x [P,Ds] -> [P]"""
+def point_value(term, x, u=None):
+    """one reward term (engine dict: kind, W, t) at the states x [P,Ds] and, for a joint term, actions u [P,U] -> [P]"""
     W = np.asarray(term["W"], dtype=np.float64)
     if term["kind"] == _lib.REWARD_BOX:
         return box_point(W, x)
-    if term["kind"] == _lib.REWARD_LINEAR:
-        return x @ W.reshape(-1)
-    d = x - np.asarray(term["t"], dtype=np.float64).reshape(1, -1)
+    z = np.hstack([x, u]) if is_joint(term) else x
+    if term["kind"] in (_lib.REWARD_LINEAR, _lib.REWARD_LINEAR_SA):
+        return z @ W.reshape(-1)
+    d = z - np.asarray(term["t"], dtype=np.float64).reshape(1, -1)
     return np.exp(-0.5 * np.einsum("pi,ij,pj->p", d, W.reshape(d.shape[1], d.shape[1]), d))
 
 
-def particle_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0):
-    """-> traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]"""
+def step_values(terms, value, zero):
+    """(reward, risk) of one step: the sum of coef * value(term) over each channel's terms from ``zero``, state terms
+    first, then joint terms, each in term order.  Numpy or torch: ``value`` and ``zero`` decide."""
+    rew = risk = zero
+    for term in [t for t in terms if not is_joint(t)] + [t for t in terms if is_joint(t)]:
+        v = float(term.get("coef", 1.0)) * value(term)
+        if is_mult(term):
+            risk = risk + v
+        else:
+            rew = rew + v
+    return rew, risk
+
+
+def path_rewards(terms, traj, act):
+    """step_reward, step_risk [P,H] of the terms at the states traj[:, t] and actions act[:, t] of every step t < H"""
+    P, H = act.shape[:2]
+    rew, risk = np.zeros((P, H)), np.zeros((P, H))
+    for t in range(H):
+        rew[:, t], risk[:, t] = step_values(terms, lambda term: point_value(term, traj[:, t], act[:, t]), np.zeros(P))
+    return rew, risk
+
+
+def particle_return(terms, rew, risk, mult_mu):
+    """the return [P] of step rewards and risks [P,H] (numpy or torch): sum_t r_t, plus mult_mu (1 - prod_t (1 - k_t))
+    when a term is on the MULT channel"""
+    ret = rew.sum(1)
+    if any(is_mult(t) for t in terms):
+        ret = ret + mult_mu * (1.0 - (1.0 - risk).prod(1))
+    return ret
+
+
+def _rollout(pol, terms, x0, eps, mult_mu, transition):
+    """the step loop: ``transition(x, [x, u], eps_t)`` -> the next state"""
     P, H, Ds = eps.shape
     x = np.asarray(x0, dtype=np.float64).copy()
-    traj, act, rew, risk = [x], [], np.zeros((P, H)), np.zeros((P, H))
+    traj, act = [x], []
     for t in range(H):
-        for term in terms:
-            v = float(term.get("coef", 1.0)) * reward_value(term, x)
-            if int(term.get("channel", _lib.CHANNEL_ADD)) == _lib.CHANNEL_MULT:
-                risk[:, t] += v
-            else:
-                rew[:, t] += v
         u = policy_action(pol, x)
-        act.append(u)
-        mu, var = gp_latent(dyn, np.hstack([x, u]))
-        x = x + mu + np.sqrt(np.maximum(var, 0.0)) * eps[:, t]
-        traj.append(x)
-    ret = rew.sum(1)
-    if any(int(t.get("channel", 0)) == _lib.CHANNEL_MULT for t in terms):
-        ret = ret + mult_mu * (1.0 - np.prod(1.0 - risk, axis=1))
-    U = act[0].shape[1] if act else 0
-    return (np.stack(traj, 1), np.stack(act, 1) if act else np.zeros((P, 0, U)), rew, risk, ret)
+        x = transition(x, np.hstack([x, u]), eps[:, t])
+        traj.append(x); act.append(u)
+    traj, act = np.stack(traj, 1), np.stack(act, 1) if H else np.zeros((P, 0, 0))
+    rew, risk = path_rewards(terms, traj, act)
+    return traj, act, rew, risk, particle_return(terms, rew, risk, mult_mu)
+
+
+def particle_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0):
+    """-> traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P] of the step-wise sampler"""
+    def transition(x, xt, e):
+        mu, var = gp_latent(dyn, xt)
+        return x + mu + np.sqrt(np.maximum(var, 0.0)) * e
+    return _rollout(pol, terms, x0, eps, mult_mu, transition)
+
+
+def consistent_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0, swap=False):
+    """-> traj, act, step_reward, step_risk, ret of the consistent sampler (eps[:, t] is the step-t normal of every
+    output).  ``swap`` reorders the posterior's sums: the difference of the two is the sampler's own sensitivity to
+    rounding"""
+    fs = FunctionSample(dyn, eps.shape[0], swap)
+    return _rollout(pol, terms, x0, eps, mult_mu, lambda x, xt, e: x + fs.step(xt, e))
+
+
+def _posterior(dyn, A, B):
+    """latent posterior covariance k_post(A, B) per output -> [E, |A|, |B|]"""
+    C, ell, sf2, iK = (dyn[k] for k in ("C", "ell", "sf2", "iK"))
+    n = C.shape[0]
+    out = []
+    for e in range(ell.shape[0]):
+        Ka, Kb = se_k(A, C, ell[e], sf2[e]), se_k(B, C, ell[e], sf2[e])
+        out.append(se_k(A, B, ell[e], sf2[e]) - Ka @ iK[e][:n, :n] @ Kb.T)
+    return np.stack(out)
+
+
+def _posterior_pairs(dyn, A, B, swap=False):
+    """k_post(A_p, B_p) of row-wise pairs A, B [P,D] -> [P,E]; ``swap``: the quadratic form as k_A (iK k_B) instead of
+    (k_A iK) k_B, the same value with other roundings"""
+    C, ell, sf2, iK = (dyn[k] for k in ("C", "ell", "sf2", "iK"))
+    n = C.shape[0]
+    out = []
+    for e in range(ell.shape[0]):
+        Ka, Kb = se_k(A, C, ell[e], sf2[e]), se_k(B, C, ell[e], sf2[e])
+        d = (A - B) / ell[e][None, :]
+        q = (Ka * (Kb @ iK[e][:n, :n])).sum(1) if swap else ((Ka @ iK[e][:n, :n]) * Kb).sum(1)
+        out.append(sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) - q)
+    return np.stack(out, 1)
+
+
+class FunctionSample:
+    """The running state of one draw per (particle, output): the visited inputs and the packed factor rows.
+    ``step(Xt, eps_t)`` -> f(Xt) [P,E] given the draws at the earlier inputs."""
+
+    def __init__(self, dyn, P, swap=False):
+        self.dyn, self.P, self.swap = dyn, P, swap
+        self.E = dyn["ell"].shape[0]
+        self.X = []              # visited inputs, each [P,D]
+        self.L = []              # rows l [P,E,s] of the factor, below the diagonal
+        self.piv = []            # pivots [P,E] (0: degenerate column)
+        self.eps = []            # the normals [P,E] of the earlier steps
+
+    def step(self, Xt, eps_t):
+        dyn, P, E, t = self.dyn, self.P, self.E, len(self.X)
+        sf2 = np.asarray(dyn["sf2"]).reshape(1, E)
+        mu = gp_latent(dyn, Xt)[0]
+        var = _posterior_pairs(dyn, Xt, Xt, self.swap)      # [P,E]
+        l = np.zeros((P, E, t))
+        for s in range(t):                                  # forward substitution, one column at a time
+            c = _posterior_pairs(dyn, Xt, self.X[s], self.swap)
+            sub = (self.L[s] * l[:, :, :s]).sum(-1) if s else 0.0
+            piv = self.piv[s]
+            l[:, :, s] = np.where(piv > 0.0, (c - sub) / np.where(piv > 0.0, piv, 1.0), 0.0)
+        d2 = var - (l * l).sum(-1)
+        f = mu + np.sqrt(np.maximum(d2, 0.0)) * eps_t
+        if t:
+            f = f + (l * np.stack(self.eps, -1)).sum(-1)
+        self.X.append(Xt.copy()); self.L.append(l); self.eps.append(eps_t.copy())
+        self.piv.append(np.where(d2 > TAU * sf2, np.sqrt(np.maximum(d2, 0.0)), 0.0))
+        return f
+
+
+def joint_draw(dyn, Xs, eps):
+    """f at the fixed inputs Xs [T,D] from the normals eps [T,E] as mu + chol(K_post) eps, per output (K_post positive
+    definite) -> [T,E]"""
+    K = _posterior(dyn, Xs, Xs)
+    mu = gp_latent(dyn, Xs)[0]
+    return mu + np.stack([np.linalg.cholesky(K[e]) @ eps[:, e] for e in range(K.shape[0])], 1)
+
+
+def weights(terms, rew, risk, mult_mu=0.0, baseline=True):
+    """w [P, H-1]: the return-to-go G_pt of every transition t < H-1 from the step rewards and risks [P,H], minus the
+    leave-one-out mean of the other particles' G_qt when ``baseline`` (and P > 1)"""
+    P, H = rew.shape
+    mult = any(is_mult(t) for t in terms)
+    G = np.zeros((P, max(H - 1, 0)))
+    for t in range(H - 1):
+        G[:, t] = rew[:, t + 1:].sum(1)
+        if mult:
+            G[:, t] += mult_mu * np.prod(1.0 - risk[:, :t + 1], 1) * (1.0 - np.prod(1.0 - risk[:, t + 1:], 1))
+    if baseline and P > 1:
+        G = G - (G.sum(0, keepdims=True) - G) / (P - 1)
+    return G
 
 
 def moment_check(samples, mean, cov, nse=5.0):

@@ -8,31 +8,7 @@ import pytest
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-
-OK, ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_LAUNCH, ERR_UNSUP = 0, -1, -2, -3, -4, -5, -6
-FAKE = 0x10000          # 16-byte aligned, never dereferenced by the validation code
-
-
-def _gp(n=50, D=4, E=3, mode=0, iK=FAKE, ldk=64):
-    g = _lib.GpModel()
-    g.n, g.D, g.E, g.mode = n, D, E, mode
-    g.X = g.ell = g.sf2 = g.beta = FAKE
-    g.iK, g.ldk = iK, ldk
-    return g
-
-
-def _rollout(kind=_lib.POLICY_LINEAR, n_rewards=1, reward_kind=_lib.REWARD_EXP, channel=0):
-    ro = _lib.Rollout()
-    ro.R, ro.H = 2, 5
-    ro.dyn = _gp(n=50, D=4, E=3)
-    ro.pol.kind, ro.pol.Ds, ro.pol.U, ro.pol.squash = kind, 3, 1, 1
-    ro.pol.max_action = ro.pol.W = ro.pol.b = FAKE
-    ro.n_rewards = n_rewards
-    ro.rewards[0].kind, ro.rewards[0].channel, ro.rewards[0].coef = reward_kind, channel, 1.0
-    ro.rewards[0].W = ro.rewards[0].t = FAKE
-    ro.m0 = ro.S0 = ro.traj_m = ro.traj_S = ro.reward = ro.ws = FAKE
-    ro.ws_bytes = 0
-    return ro
+from abi_fakes import OK, ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_LAUNCH, ERR_UNSUP, FAKE, _gp, _rollout
 
 
 def test_status_strings():

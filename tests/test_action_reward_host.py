@@ -1,6 +1,6 @@
 """Reward terms on the joint state-action Gaussian (PILCO_REWARD_EXP_SA / PILCO_REWARD_LINEAR_SA, DESIGN.md section 18),
 checked WITHOUT a GPU: the header and ctypes constants with unchanged struct layouts, argument validation of the C ABI,
-the oracles of tests/action_reward_oracle.py against Monte Carlo, central differences and the state-term identity, the
+the moment-matching and particle oracles against Monte Carlo, central differences and the state-term identity, the
 Python classes, and the SASS of the kernels the feature added or touched."""
 import ctypes as C
 import os
@@ -13,10 +13,10 @@ import torch
 from pilco_b200 import _lib, rewards
 from pilco_b200._lib import lib
 import action_reward_oracle as aro
-from test_abi_errors import ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _rollout
+import particle_oracle as po
+from abi_fakes import ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _particles, _rollout
+from particle_grad_oracle import T, score_grad, value_and_grad
 from util import CUOBJDUMP, ROOT, make_gp_problem, sass
-
-T = aro.T
 
 
 def test_header_constants_and_unchanged_layouts():
@@ -53,7 +53,6 @@ def test_rollout_validation_of_joint_kinds():
 
 
 def test_particles_validation_of_joint_kinds():
-    from test_particles_host import _particles
     run = lambda pr: lib.pilco_particles_rollout(C.byref(pr), None)
     ok = run(_particles())                                                       # a valid description's status
     for kind in (_lib.REWARD_EXP_SA, _lib.REWARD_LINEAR_SA):
@@ -72,7 +71,7 @@ def test_particles_validation_of_joint_kinds():
 
 def _mc(term, m, s, n=400000, seed=0):
     z = np.random.RandomState(seed).multivariate_normal(m.reshape(-1), s, size=n)
-    v = aro.point_value(term, z[:, :2], z[:, 2:])
+    v = po.point_value(term, z[:, :2], z[:, 2:])
     return v.mean(), v.std() / np.sqrt(n)
 
 
@@ -142,13 +141,12 @@ def test_zero_action_block_is_the_state_term():
     assert torch.allclose(a["step_reward"], b["step_reward"], rtol=1e-12, atol=0)
     x, u = rng.rand(7, 2), rng.randn(7, 1)
     for s, j in zip(state, joint):
-        assert np.allclose(aro.point_value(s, x, u), aro.point_value(j, x, u), rtol=1e-14, atol=0)
+        assert np.allclose(po.point_value(s, x, u), po.point_value(j, x, u), rtol=1e-14, atol=0)
 
 
 def test_particle_oracles_agree_and_score_direct_term():
     """numpy rollout = torch rollout's value; the pathwise autograd gradient against central differences; the score
     oracle's direct term alone is the gradient of the joint terms at fixed states (linear term: closed form)"""
-    import particle_oracle as po
     P, terms = _small_problem(7)
     from oracle import python_port as pp
     iK, beta = pp.calculate_factorizations(P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"])
@@ -156,22 +154,22 @@ def test_particle_oracles_agree_and_score_direct_term():
     pol = dict(kind=_lib.POLICY_LINEAR, squash=True, maxa=P["maxa"], W=P["W"], b=P["b"])
     rng = np.random.RandomState(8)
     x0, eps = P["m0"][None] + 0.2 * rng.randn(40, 2), rng.randn(40, 4, 2)
-    ret = aro.particle_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[4]
-    v, g = aro.value_and_grad(dyn, pol, terms, x0, eps, mult_mu=1.5)
+    ret = po.particle_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[4]
+    v, g = value_and_grad(dyn, pol, terms, x0, eps, mult_mu=1.5)
     assert abs(v - ret.mean()) <= 1e-13 * max(1.0, abs(v))
     h = 1e-6
     d = np.zeros_like(P["W"]); d[0, 1] = h
-    vp = aro.particle_rollout(dyn, dict(pol, W=P["W"] + d), terms, x0, eps, mult_mu=1.5)[4].mean()
-    vm = aro.particle_rollout(dyn, dict(pol, W=P["W"] - d), terms, x0, eps, mult_mu=1.5)[4].mean()
+    vp = po.particle_rollout(dyn, dict(pol, W=P["W"] + d), terms, x0, eps, mult_mu=1.5)[4].mean()
+    vm = po.particle_rollout(dyn, dict(pol, W=P["W"] - d), terms, x0, eps, mult_mu=1.5)[4].mean()
     assert abs((vp - vm) / (2 * h) - g["W"][0, 1]) <= 1e-6 * max(1.0, abs(g["W"][0, 1]))
     # direct term of a lone linear action term, unsquashed policy: d/db mean_p sum_t c w_u = c w_u H
-    traj = aro.particle_rollout(dyn, dict(pol, squash=False), terms, x0, eps)[0]
+    traj = po.particle_rollout(dyn, dict(pol, squash=False), terms, x0, eps)[0]
     lone = [dict(kind=_lib.REWARD_LINEAR_SA, coef=0.3, W=np.array([0.0, 0.0, 2.0]), t=None)]
     nosq = dict(pol, squash=False)
-    gd = aro.score_grad(dyn, nosq, nosq, lone, traj, eps, transitions=False)
+    gd = score_grad(dyn, nosq, lone, traj, eps, transitions=False)
     assert abs(gd["b"][0] - 0.3 * 2.0 * 4) <= 1e-12
     assert np.allclose(gd["W"][0], 0.6 * traj[:, :4].sum(1).mean(0), rtol=1e-12)
-    assert not any(np.any(v) for v in aro.score_grad(dyn, nosq, nosq, lone, traj, eps, direct=False, transitions=False).values())
+    assert not any(np.any(v) for v in score_grad(dyn, nosq, lone, traj, eps, direct=False, transitions=False).values())
 
 
 def test_reward_classes_and_term_specs():

@@ -9,12 +9,12 @@ import torch
 
 from pilco_b200 import engine, _lib, rewards
 import action_reward_oracle as aro
-from test_gpu_particles import BOX2, _case, _draw, _dyn_np, _linear, _rbf
-from test_gpu_particles_grad import _oracle_pol
+import particle_oracle as po
+from particle_cases import BOX2, _case, _draw, _dyn_np, _linear, _oracle_pol, _rbf
+from particle_grad_oracle import T, score_grad, value_and_grad
 from util import make_gp_problem, make_rollout_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
-T = aro.T
 
 
 def _joint_terms(Ds, U, seed=0, box=True):
@@ -168,16 +168,12 @@ def test_particle_values_match_oracle(name, consistent):
     if consistent:
         # the function-sample chain has its own oracle for the states; the reward terms are checked at the device's points
         traj, act = out[0], out[1]
-        rew, risk = np.zeros((P, H)), np.zeros((P, H))
-        for t in range(H):
-            for term in aro._ordered(terms):
-                v = float(term["coef"]) * aro.point_value(term, traj[:, t], act[:, t])
-                (risk if aro._is_mult(term) else rew)[:, t] += v
-        ref = (traj, act, rew, risk, rew.sum(1) + mu * (1.0 - np.prod(1.0 - risk, axis=1)))
+        rew, risk = po.path_rewards(terms, traj, act)
+        ref = (traj, act, rew, risk, po.particle_return(terms, rew, risk, mu))
         step0 = engine.particles_rollout(gp, spec, terms, x0, eps, mult_mu=mu)
         assert np.array_equal(step0[2][:, 0].cpu().numpy(), out[2][:, 0])           # step 0 is the marginal sampler's
     else:
-        ref = aro.particle_rollout(_dyn_np(gp), pol, terms, x0, eps, mult_mu=mu)
+        ref = po.particle_rollout(_dyn_np(gp), pol, terms, x0, eps, mult_mu=mu)
     for what, o, r in zip(("traj", "act", "reward", "risk", "ret"), out, ref):
         assert scaled_err(o, r) <= 1e-9, (what, scaled_err(o, r))
 
@@ -198,7 +194,7 @@ def test_pathwise_gradient_matches_autograd(name):
     terms = [t for t in terms if t["kind"] != _lib.REWARD_BOX]
     x0, eps = _draw(m0, S0, P, H, seed=P + H + 1)
     plan, g = _grad(gp, spec, terms, x0, eps, mu)
-    v, ref = aro.value_and_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps, mu)
+    v, ref = value_and_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps, mu)
     scale = max(float(np.abs(r).max()) for r in ref.values())
     err = max(float(np.abs(g[k] - ref[k]).max()) for k in ref) / scale
     assert err <= (1e-6 if name == "fitc" else 1e-8), err
@@ -208,7 +204,7 @@ def test_pathwise_gradient_matches_autograd(name):
         assert torch.equal(a, b)
     # H = 1: the only step is the last one, which has no transition but still an action cost
     _, g1 = _grad(gp, spec, terms, x0, eps[:, :1], mu)
-    _, r1 = aro.value_and_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps[:, :1], mu)
+    _, r1 = value_and_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps[:, :1], mu)
     s1 = max(float(np.abs(r).max()) for r in r1.values())
     assert s1 > 0 and max(float(np.abs(g1[k] - r1[k]).max()) for k in r1) <= 1e-8 * s1
 
@@ -236,12 +232,12 @@ def test_score_gradient_matches_oracle_and_direct_term(name):
     plan, g = _grad(gp, spec, terms, x0, eps, mu, estimator="score")
     traj = plan.traj.cpu().numpy()
     dyn, opol = _dyn_np(gp), _oracle_pol(spec, pol)
-    ref = aro.score_grad(dyn, pol, opol, terms, traj, eps, mu)
+    ref = score_grad(dyn, opol, terms, traj, eps, mu)
     scale = max(float(np.abs(r).max()) for r in ref.values())
     assert max(float(np.abs(g[k] - ref[k]).max()) for k in ref) <= 1e-6 * scale
     # the direct term alone: H = 1 has no transition with a reward after it, so the whole gradient is the direct term
     _, g1 = _grad(gp, spec, terms, x0, eps[:, :1], mu, estimator="score")
-    d1 = aro.score_grad(dyn, pol, opol, terms, traj[:, :2], eps[:, :1], mu, transitions=False)
+    d1 = score_grad(dyn, opol, terms, traj[:, :2], eps[:, :1], mu, transitions=False)
     s1 = max(float(np.abs(r).max()) for r in d1.values())
     assert s1 > 0 and max(float(np.abs(g1[k] - d1[k]).max()) for k in d1) <= 1e-9 * s1
     pw = _grad(gp, spec, terms, x0, eps, mu)[0]

@@ -7,76 +7,11 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib
+from particle_cases import _case, _controller_np, _draw, _dyn_np, _linear, _pilco_data
 from particle_oracle import moment_check, particle_rollout
-from util import make_gp_problem, make_rollout_problem, scaled_err
+from util import make_rollout_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
-
-BOX2 = np.array([2, 1, 1.0, 0, 0.2, 0.9, 1, 0.1, 0.8])             # dims 0, 1 inside (low, high)
-BOX1C = np.array([1, 0, 1.0, 2, -np.inf, 0.6])                    # dim 2 not below 0.6
-
-
-def _dyn_np(gp):
-    return dict(C=gp.X.cpu().numpy(), ell=gp.ell.cpu().numpy(), sf2=gp.sf2.cpu().numpy(),
-                iK=gp.iK.cpu().numpy(), beta=gp.beta.cpu().numpy())
-
-
-def _rbf(Xc, Yc, lc, maxa):
-    U = Yc.shape[1]
-    pgp = engine.gp_factorize(Xc, Yc, lc, np.ones(U), 1e-4 * np.ones(U), need_iK=False, mode=1)
-    spec = dict(kind=_lib.POLICY_RBF, Ds=Xc.shape[1], U=U, squash=True, max_action=maxa, gp=pgp)
-    pol = dict(kind=_lib.POLICY_RBF, squash=True, maxa=maxa, C=Xc, ell=lc, sf2=np.ones(U), beta=pgp.beta.cpu().numpy())
-    return spec, pol
-
-
-def _linear(W, b, maxa, squash):
-    U, Ds = W.shape
-    return (dict(kind=_lib.POLICY_LINEAR, Ds=Ds, U=U, squash=squash, max_action=maxa, W=W, b=b),
-            dict(kind=_lib.POLICY_LINEAR, squash=squash, maxa=maxa, W=W, b=b))
-
-
-def _all_terms(Ds):
-    """exp, linear and box terms on both channels"""
-    rng = np.random.RandomState(Ds)
-    Wl = rng.randn(Ds)
-    return [dict(kind=_lib.REWARD_EXP, coef=1.0, W=np.eye(Ds), t=0.5 * np.ones(Ds)),
-            dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=Wl, t=None),
-            dict(kind=_lib.REWARD_BOX, coef=-2.0, W=BOX2, t=None),
-            dict(kind=_lib.REWARD_EXP, coef=0.1, channel=_lib.CHANNEL_MULT, W=2.0 * np.eye(Ds), t=np.zeros(Ds)),
-            dict(kind=_lib.REWARD_LINEAR, coef=0.01, channel=_lib.CHANNEL_MULT, W=Wl, t=None),
-            dict(kind=_lib.REWARD_BOX, coef=0.2, channel=_lib.CHANNEL_MULT, W=BOX1C, t=None)]
-
-
-def _case(name):
-    """-> dyn (DeviceGP), policy spec, oracle policy, reward terms, m0, S0, H, P, mult_mu"""
-    if name == "metric_rbf":
-        pb = make_rollout_problem(300, 10, 2, 50, 1, seed=5)
-        gp = engine.gp_factorize(pb["X"], pb["Y"], pb["ell"], pb["sf2"], pb["sn2"])
-        spec, pol = _rbf(pb["Xc"][0], pb["Yc"][0], pb["lc"][0], pb["maxa"])
-        return gp, spec, pol, _all_terms(10), pb["m0"], pb["S0"], 10, 1000, 1.5
-    if name in ("linear_squash", "linear_nosquash"):
-        X, Y, ell, sf2, sn2 = make_gp_problem(100, 5, 4, seed=6)
-        gp = engine.gp_factorize(X, 0.1 * Y, ell, 0.1 * sf2, 1e-3 * np.ones(4))
-        rng = np.random.RandomState(7)
-        spec, pol = _linear(0.5 * rng.randn(1, 4), rng.randn(1), np.array([1.3]), name == "linear_squash")
-        return gp, spec, pol, _all_terms(4), X[0, :4], 0.05 * np.eye(4), 8, 777, -3.0
-    if name == "fitc":
-        pb = make_rollout_problem(2000, 4, 1, 20, 1, seed=8)
-        Z = np.random.RandomState(9).rand(200, 5)
-        gp = engine.fitc_factorize(pb["X"], Z, pb["Y"], pb["ell"], pb["sf2"], pb["sn2"])
-        spec, pol = _rbf(pb["Xc"][0], pb["Yc"][0], pb["lc"][0], pb["maxa"])
-        return gp, spec, pol, _all_terms(4)[:3], pb["m0"], pb["S0"], 6, 300, 0.0
-    assert name == "n1_d16_h0"
-    X, Y, ell, sf2, sn2 = make_gp_problem(1, 16, 15, seed=10)
-    gp = engine.gp_factorize(X, 0.1 * Y, ell, sf2, sn2)
-    spec, pol = _linear(np.random.RandomState(11).randn(1, 15), np.zeros(1), np.ones(1), True)
-    return gp, spec, pol, _all_terms(15)[:1], X[0, :15], 0.1 * np.eye(15), 0, 50, 0.0
-
-
-def _draw(m0, S0, P, H, seed):
-    rng = np.random.RandomState(seed)
-    Ds = m0.shape[0]
-    return m0[None] + rng.randn(P, Ds) @ np.linalg.cholesky(S0).T, rng.randn(P, H, Ds)
 
 
 @pytest.mark.parametrize("name", ["metric_rbf", "linear_squash", "linear_nosquash", "fitc", "n1_d16_h0"])
@@ -178,11 +113,6 @@ def test_graph_replay_is_bitwise_equal_to_eager():
         assert torch.equal(a, b)
 
 
-def _pilco_data(seed, n=80, Ds=3, U=1):
-    rng = np.random.RandomState(seed)
-    X = rng.rand(n, Ds + U)
-    return X, 0.1 * np.sin(X).dot(rng.rand(Ds + U, Ds))
-
 
 def test_sample_trajectories_class_api():
     from pilco.models import PILCO
@@ -220,12 +150,6 @@ def test_sample_trajectories_class_api():
     ref =particle_rollout(_dyn_np(gp), _controller_np(pilco.controller), pilco.reward.terms(), f.states[:, 0], eps)
     assert scaled_err(f.states, ref[0]) <= 1e-9
 
-
-def _controller_np(ctrl):
-    U = ctrl.num_outputs
-    return dict(kind=_lib.POLICY_RBF, squash=True, maxa=np.broadcast_to(np.asarray(ctrl.max_action, dtype=np.float64), (U,)),
-                C=np.asarray(ctrl.models[0].X), ell=np.asarray(ctrl.lengthscales), sf2=np.asarray(ctrl.variance).reshape(U),
-                beta=ctrl.device_gp().beta.cpu().numpy())
 
 
 def test_sample_trajectories_smgpr_and_safe_pilco():

@@ -1,5 +1,5 @@
 """The consistent particle sampler on the device (pilco_particles_rollout_consistent through engine.particles_rollout /
-ParticlePlan and PILCO.sample_trajectories(consistent=True)): parity with the numpy oracle (tests/consistent_oracle.py)
+ParticlePlan and PILCO.sample_trajectories(consistent=True)): parity with the numpy oracle (tests/particle_oracle.py)
 given the same x0 and eps, step 0 bitwise the marginal sampler's, a revisited input reproducing its value, bitwise
 independence of a particle from P, its row and the chunking, CUDA-graph replay, and the class API."""
 import numpy as np
@@ -7,9 +7,9 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib
-from consistent_oracle import consistent_rollout
-from test_gpu_particles import _case, _controller_np, _draw, _dyn_np, _linear, _pilco_data
-from util import make_gp_problem, scaled_err
+from particle_cases import _case, _controller_np, _draw, _dyn_np, _pilco_data, _revisit_problem
+from particle_oracle import consistent_rollout
+from util import scaled_err
 
 pytestmark = pytest.mark.gpu
 
@@ -44,19 +44,6 @@ def test_first_step_is_bitwise_the_marginal_samplers(name):
     for a, b in zip(cons[:3], marg[:3]):
         assert torch.equal(a[:, :2], b[:, :2])
     assert not torch.equal(cons[0][:, 2:], marg[0][:, 2:])
-
-
-def _revisit_problem(H, P, seed):
-    """state lengthscales 1e12 (the model ignores the state) and a squashed constant action of 5, outside the data's
-    action range [0, 1): every step of a particle has the same input, where var is close to sf2"""
-    Ds, U = 3, 1
-    X, Y, ell, sf2, sn2 = make_gp_problem(60, Ds + U, Ds, seed=seed)
-    ell[:, :Ds] = 1e12
-    gp = engine.gp_factorize(X, 0.1 * Y, ell, sf2, sn2)
-    spec, _ = _linear(np.zeros((U, Ds)), np.array([np.pi / 2]), np.array([5.0]), True)
-    terms = [dict(kind=_lib.REWARD_LINEAR, coef=1.0, W=np.ones(Ds), t=None)]
-    rng = np.random.RandomState(seed)
-    return gp, spec, terms, 0.5 + 0.1 * rng.randn(P, Ds), rng.randn(P, H, Ds)
 
 
 def test_revisited_input_gives_the_same_value():

@@ -1,7 +1,7 @@
 """The consistent sampler's pathwise gradient on the device (pilco_particles_rollout_consistent_grad through
 engine.ConsistentGradPlan, PILCO.sample_policy_gradient / optimize_policy_sampled(..., consistent=True)): forward
 outputs bitwise those of pilco_particles_rollout_consistent, parity with the torch autograd oracle
-(tests/consistent_grad_oracle.py) given the same x0 and eps, a directional central difference of the device value, a
+(tests/particle_grad_oracle.py) given the same x0 and eps, a directional central difference of the device value, a
 finite gradient at a revisited input, batched restarts bitwise equal to unbatched calls, bitwise reproducibility and
 CUDA-graph replay, the workspace budget, and the class API."""
 from functools import partial
@@ -11,11 +11,8 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib, policy_opt
-from consistent_grad_oracle import value_and_grad
-from test_gpu_particles import _case, _draw, _dyn_np, _pilco_data
-from test_gpu_particles_consistent import _revisit_problem
-from test_gpu_particles_grad import _oracle_pol
-from test_gpu_particles_opt import _batch_case, _pilco
+from particle_cases import _batch_case, _case, _draw, _dyn_np, _oracle_pol, _pilco, _pilco_data, _revisit_problem
+from particle_grad_oracle import consistent_value_and_grad
 from util import make_rollout_problem
 
 pytestmark = pytest.mark.gpu
@@ -48,14 +45,14 @@ def test_parity_with_autograd_oracle(name):
     _, g, _ = _grad_run(gp, spec, terms, x0, eps, mu)
     g = {k: v.cpu().numpy() for k, v in g.items()}
     args = (_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps, mu)
-    v, ref, ratio = value_and_grad(*args)
+    v, ref, ratio = consistent_value_and_grad(*args)
     scale = max(float(np.abs(r).max()) for r in ref.values())
     if scale == 0.0:                                            # H = 0: nothing depends on the policy
         assert all(not g[k].any() for k in ref)
         err = own = 0.0
     else:
         err = max(float(np.abs(g[k].reshape(ref[k].shape) - ref[k]).max()) for k in ref) / scale
-        _, sw, _ = value_and_grad(*args, swap=True)
+        _, sw, _ = consistent_value_and_grad(*args, swap=True)
         own = max(float(np.abs(sw[k] - ref[k]).max()) for k in ref) / scale
     verr = abs(float(g["value"][0]) - v) / max(abs(v), 1e-300)
     print("consistent gradient %s (P=%d, H=%d) vs autograd oracle: %.1e of the gradient's scale, value %.1e; the "

@@ -10,7 +10,7 @@ import torch
 
 from pilco_b200 import engine, _lib
 from particle_grad_oracle import predict_vjp, value_and_grad
-from test_gpu_particles import _case, _draw, _dyn_np, _pilco_data
+from particle_cases import _case, _draw, _dyn_np, _oracle_pol, _pilco_data
 from util import make_gp_problem, make_rollout_problem
 
 pytestmark = pytest.mark.gpu
@@ -38,14 +38,6 @@ def test_predict_vjp_against_closed_form(n, D, E, T):
         perm = rng.permutation(T)
         pm = engine.gp_predict_vjp(gp, Xs[perm], gm[perm], gv[perm]).cpu().numpy()
         assert np.array_equal(pm, out[perm])
-
-
-def _oracle_pol(spec, pol):
-    if spec["kind"] == _lib.POLICY_LINEAR:
-        return pol
-    g = spec["gp"]
-    return dict(kind=_lib.POLICY_RBF, squash=pol["squash"], maxa=pol["maxa"], Xc=g.X.cpu().numpy(), Yc=g.Y.cpu().numpy(),
-                ell=g.ell.cpu().numpy(), sf2=g.sf2.cpu().numpy(), sn2=g.sn2.cpu().numpy())
 
 
 def _device_grad(gp, spec, terms, x0, eps, mu):

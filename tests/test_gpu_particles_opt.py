@@ -9,40 +9,9 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib, policy_opt
-from test_gpu_particles import _all_terms, _draw, _pilco_data
-from util import make_gp_problem, make_rollout_problem
+from particle_cases import _batch_case, _draw, _pilco, _pilco_data
 
 pytestmark = pytest.mark.gpu
-
-
-def _batch_case(kind, R):
-    """-> dyn, batched policy spec, per-restart unbatched specs, reward terms, m0, S0, H, P, mult_mu"""
-    if kind in ("rbf", "fitc"):
-        Ds, U = (6, 2) if kind == "rbf" else (4, 1)
-        pb = make_rollout_problem(300 if kind == "rbf" else 1500, Ds, U, 20, R, seed=30 + R)
-        if kind == "rbf":
-            gp = engine.gp_factorize(pb["X"], pb["Y"], pb["ell"], pb["sf2"], pb["sn2"])
-        else:
-            Z = np.random.RandomState(31).rand(150, Ds + U)
-            gp = engine.fitc_factorize(pb["X"], Z, pb["Y"], pb["ell"], pb["sf2"], pb["sn2"])
-        pgp = engine.gp_factorize(pb["Xc"], pb["Yc"], pb["lc"], np.ones((R, U)), 1e-4 * np.ones((R, U)),
-                                  need_iK=False, mode=1)
-        maxa = 0.8 + 0.4 * np.arange(U)
-        spec = dict(kind=_lib.POLICY_RBF, Ds=Ds, U=U, squash=True, max_action=maxa, gp=pgp)
-        ldw = engine.pad_n(pgp.n)
-        singles = []
-        for r in range(R):                      # restart r's arrays, as an unbatched policy
-            one = engine.DeviceGP(pgp.X[r], pgp.ell[r], pgp.sf2[r], pgp.beta[r], mode=1)
-            one.fact_ws = pgp.fact_ws[r * U * ldw * ldw:(r + 1) * U * ldw * ldw]
-            singles.append(dict(spec, gp=one))
-        return gp, spec, singles, _all_terms(Ds), pb["m0"], pb["S0"], 5, 300, 1.5
-    X, Y, ell, sf2, sn2 = make_gp_problem(100, 5, 4, seed=32)
-    gp = engine.gp_factorize(X, 0.1 * Y, ell, 0.1 * sf2, 1e-3 * np.ones(4))
-    rng = np.random.RandomState(33)
-    W, b = 0.5 * rng.randn(R, 1, 4), rng.randn(R, 1)
-    spec = dict(kind=_lib.POLICY_LINEAR, Ds=4, U=1, squash=True, max_action=np.array([1.3]), W=W, b=b)
-    singles = [dict(spec, W=W[r], b=b[r]) for r in range(R)]
-    return gp, spec, singles, _all_terms(4), X[0, :4], 0.05 * np.eye(4), 7, 777, -3.0
 
 
 def _grad_run(gp, spec, terms, x0, eps, mu, R=1):
@@ -96,16 +65,6 @@ def test_batched_call_is_reproducible_and_replays():
     torch.cuda.synchronize()
     assert all(torch.equal(first[k], plan.gbuf[k]) for k in first)
     assert torch.equal(out[0], plan.traj) and torch.equal(out[4], plan.ret)
-
-
-def _pilco(kind, seed, **kw):
-    from pilco.models import PILCO
-    from pilco.controllers import RbfController, LinearController
-    np.random.seed(seed)
-    X, Y = _pilco_data(seed)
-    ctrl = RbfController(3, 1, 10, max_action=1.2) if kind == "rbf" else LinearController(3, 1, max_action=1.0)
-    pilco = PILCO((X[:60], Y[:60]), controller=ctrl, horizon=6, m_init=X[0:1, :3], S_init=0.05 * np.eye(3), **kw)
-    return pilco, X, Y
 
 
 @pytest.mark.parametrize("kind", ["rbf", "linear"])

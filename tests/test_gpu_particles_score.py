@@ -1,18 +1,16 @@
 """Score-function gradient of the particle return on the device (pilco_particles_rollout_score_grad through
 engine.ParticlePlan(estimator="score") and PILCO.sample_policy_gradient(estimator="score")): parity with the torch
-oracle given the device's trajectories, x0 and eps (tests/score_grad_oracle.py), the forward outputs and value against
-the pathwise call, restarts against single calls, bitwise reproducibility and CUDA-graph replay, a call past one VJP
-call's row limit, unbiasedness against the moment-matching and pathwise gradients, box terms against a central
+oracle given the device's trajectories, x0 and eps (tests/particle_grad_oracle.py), the forward outputs and value
+against the pathwise call, restarts against single calls, bitwise reproducibility and CUDA-graph replay, a call past one
+VJP call's row limit, unbiasedness against the moment-matching and pathwise gradients, box terms against a central
 difference of the sampled return, and the class API."""
 import numpy as np
 import pytest
 import torch
 
 from pilco_b200 import engine, _lib
-from score_grad_oracle import score_grad
-from test_gpu_particles import BOX2, _case, _draw, _dyn_np, _pilco_data
-from test_gpu_particles_grad import _oracle_pol
-from test_gpu_particles_opt import _batch_case
+from particle_cases import BOX2, _batch_case, _case, _draw, _dyn_np, _oracle_pol, _pilco_data
+from particle_grad_oracle import score_grad
 from util import make_gp_problem, make_rollout_problem
 
 pytestmark = pytest.mark.gpu

@@ -5,7 +5,7 @@ are fake non-null addresses, as in test_abi_errors.py; only rejecting calls are 
 import ctypes as C
 
 from pilco_b200._lib import lib
-from test_abi_errors import ERR_ALIGN, ERR_DIM, ERR_NULL, FAKE, _gp
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, FAKE, _gp
 
 BIG = 1 << 30
 MS = (C.c_float * 3)()          # the timings (host memory); a rejected call never writes them

@@ -1,6 +1,6 @@
 """CPU tests of the consistent sampler's pathwise gradient (pilco_particles_rollout_consistent_grad,
 engine.ConsistentGradPlan, PILCO.sample_policy_gradient / optimize_policy_sampled(..., consistent=True)): the torch
-autograd oracle (tests/consistent_grad_oracle.py) against central differences of the numpy consistent sampler, the
+autograd oracle (tests/particle_grad_oracle.py) against central differences of the numpy consistent sampler, the
 explicit reverse steps against autograd, the oracle against the step-wise one at H <= 2, argument validation of the C
 entry point (rejecting calls only), the exact workspace layout with its 0 on overflow, the SASS, and the failures
 without a GPU or with box terms."""
@@ -16,19 +16,17 @@ import torch
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from consistent_grad_oracle import fixed_inputs_objective, reverse_steps, value_and_grad
-from consistent_oracle import consistent_rollout
-from particle_grad_oracle import rbf_pol_np, value_and_grad as stepwise_value_and_grad
-from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, ROOT, _particles
-from test_particles_grad_host import CUOBJDUMP, _grad, _problem, _sass, _terms
-from test_particles_opt_host import _batched, _linear_pilco, _safe_pilco
-
-PT_MAX_P = 65535 * 32
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from particle_cases import _linear_pilco, _problem, _safe_pilco, _terms
+from particle_grad_oracle import (consistent_value_and_grad, fixed_inputs_objective, rbf_pol_np, reverse_steps,
+                                  value_and_grad as stepwise_value_and_grad)
+from particle_oracle import consistent_rollout
+from util import CUOBJDUMP, ROOT, sass_named
 
 
 def _fd(dyn, pol, keys, rebuild, terms, x0, eps, mu, h=1e-6):
     """autograd gradient against central differences of the numpy sampler's mean return, every parameter"""
-    v, g, ratio = value_and_grad(dyn, pol, terms, x0, eps, mu)
+    v, g, ratio = consistent_value_and_grad(dyn, pol, terms, x0, eps, mu)
     worst, scale = 0.0, max(np.abs(gv).max() for gv in g.values())
     for k, src in keys.items():
         base = np.asarray(pol[src], dtype=np.float64)
@@ -104,7 +102,7 @@ def test_short_horizons_equal_the_stepwise_gradient(H):
     P, Ds = 25, 3
     pol = dict(kind=_lib.POLICY_LINEAR, squash=True, maxa=np.array([1.1]), W=0.6 * rng.randn(1, Ds), b=rng.randn(1))
     x0, eps = 0.5 + 0.2 * rng.randn(P, Ds), rng.randn(P, H, Ds)
-    v, g, _ = value_and_grad(dyn, pol, _terms(Ds), x0, eps, -1.0)
+    v, g, _ = consistent_value_and_grad(dyn, pol, _terms(Ds), x0, eps, -1.0)
     v1, g1 = stepwise_value_and_grad(dyn, pol, _terms(Ds), x0, eps, -1.0)
     assert abs(v - v1) <= 1e-15 * max(abs(v1), 1.0)
     for k in g1:
@@ -225,7 +223,7 @@ SASS_GOLDEN = os.path.join(ROOT, "tests", "golden", "predict_sass.json")
 def test_consistent_grad_and_predict_kernels_sass():
     predict = ["gp_predict_kernel", "gp_predict_vjp_kernel", "fs_predict_kernel", "fs_predict_vjp_kernel"]
     names = ["fs_cond_bwd_kernel", "fs_cond_kernel", "pg_step_kernel", "pg_param_kernel", "pg_rbf_finish_kernel"] + predict
-    sass = _sass(names)
+    sass = sass_named(names)
     assert set(sass) == set(names)
     for k, text in sass.items():
         assert not re.search(r"\b(STL|LDL)\b", text), k

@@ -1,7 +1,7 @@
 """CPU tests of the consistent particle sampler (pilco_particles_rollout_consistent, engine.particles_rollout(...,
 consistent=True), PILCO.sample_trajectories(..., consistent=True)): argument validation of the C entry point (rejecting
 calls only), the exact workspace layout with its 0 for unsupported sizes and size_t overflow, the SASS of the new
-kernels, the failure without a GPU, and the numpy oracle (tests/consistent_oracle.py) against a joint draw."""
+kernels, the failure without a GPU, and the numpy oracle (tests/particle_oracle.py) against a joint draw."""
 import ctypes as C
 import os
 import re
@@ -12,12 +12,10 @@ import torch
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from consistent_oracle import FunctionSample, consistent_rollout, joint_draw
-from particle_oracle import particle_rollout
-from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _particles
-from test_particles_grad_host import CUOBJDUMP, _problem, _sass
-
-PT_MAX_P = 65535 * 32
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _particles
+from particle_cases import _problem
+from particle_oracle import FunctionSample, consistent_rollout, joint_draw, particle_rollout
+from util import CUOBJDUMP, sass_named
 
 
 def _run(pr):
@@ -116,7 +114,7 @@ def test_consistent_workspace_bytes():
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 def test_consistent_kernels_sass():
     names = ["fs_predict_kernel", "fs_cond_kernel"]
-    sass = _sass(names)
+    sass = sass_named(names)
     assert set(sass) == set(names)
     for k, text in sass.items():
         assert not re.search(r"\b(STL|LDL)\b", text), k

@@ -14,31 +14,11 @@ import torch
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _gp, _grad, _particles
+from particle_cases import _problem, _terms
 from particle_oracle import particle_rollout
 from particle_grad_oracle import predict_vjp, rbf_pol_np, value_and_grad
-from util import CUOBJDUMP, sass
-from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, ROOT, _gp, _particles
-
-
-def _problem(seed, n=25, Ds=3, U=1):
-    rng = np.random.RandomState(seed)
-    D = Ds + U
-    C_ = rng.rand(n, D)
-    Y = 0.3 * np.sin(3.0 * C_).dot(rng.rand(D, Ds))
-    ell, sf2 = 0.5 + 0.4 * rng.rand(Ds, D), 0.05 * (1.0 + rng.rand(Ds))
-    iK, beta = [], []
-    for e in range(Ds):
-        d = (C_[:, None] - C_[None]) / ell[e]
-        K = sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) + 1e-3 * np.eye(n)
-        iK.append(np.linalg.inv(K)); beta.append(iK[-1] @ Y[:, e])
-    return dict(C=C_, ell=ell, sf2=sf2, iK=np.stack(iK), beta=np.stack(beta)), rng
-
-
-def _terms(Ds):
-    return [dict(kind=_lib.REWARD_EXP, coef=1.0, W=np.diag(np.arange(1.0, Ds + 1)) + 0.2, t=0.4 * np.ones(Ds)),
-            dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=np.linspace(-1, 1, Ds), t=None),
-            dict(kind=_lib.REWARD_EXP, coef=0.2, channel=_lib.CHANNEL_MULT, W=2.0 * np.eye(Ds), t=np.zeros(Ds)),
-            dict(kind=_lib.REWARD_LINEAR, coef=0.05, channel=_lib.CHANNEL_MULT, W=np.ones(Ds), t=None)]
+from util import CUOBJDUMP, ROOT, sass_named
 
 
 def _fd_check(dyn, pol, key_map, terms, x0, eps, mu, h=1e-6):
@@ -124,13 +104,6 @@ def test_particles_grad_struct_layout_matches_mirror(tmp_path):
     assert set(got) == set(fields)
     for f, off in got.items():
         assert getattr(_lib.ParticlesGrad, f).offset == int(off), f
-
-
-def _grad(kind=_lib.POLICY_LINEAR):
-    g = _lib.ParticlesGrad()
-    g.gW = g.gb = g.gXc = g.gYc = g.gell = g.pol_L = g.value = g.ws = FAKE
-    g.ws_bytes = 0
-    return g
 
 
 def _run(pr, g):
@@ -227,15 +200,10 @@ def test_predict_vjp_argument_validation():
     assert lib.pilco_gp_predict_vjp_workspace_bytes(50, 17, 3, 10) == 0
 
 
-def _sass(names):
-    """{name: SASS text} of the kernels whose mangled names contain one of ``names`` (keyed by the first that does)"""
-    return {next(k for k in names if k in m): text for m, text in sass("|".join(map(re.escape, names))).items()}
-
-
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 def test_gradient_kernels_sass():
     names = ["gp_predict_vjp_kernel", "pg_step_kernel", "pg_param_kernel", "pg_rbf_finish_kernel"]
-    sass = _sass(names)
+    sass = sass_named(names)
     assert set(sass) == set(names)
     for k, text in sass.items():
         assert not re.search(r"\b(STL|LDL)\b", text), k

@@ -15,36 +15,9 @@ import torch
 from oracle import python_port as pp
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _particles
 from particle_oracle import moment_check, particle_rollout
-from util import CUOBJDUMP, sass
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_UNSUP = -1, -2, -3, -4, -6
-FAKE = 0x10000          # 16-byte aligned, never dereferenced by the validation code
-
-
-def _gp(n=50, D=4, E=3, mode=0, iK=FAKE, ldk=64):
-    g = _lib.GpModel()
-    g.n, g.D, g.E, g.mode = n, D, E, mode
-    g.X = g.ell = g.sf2 = g.beta = FAKE
-    g.iK, g.ldk = iK, ldk
-    return g
-
-
-def _particles(kind=_lib.POLICY_LINEAR, reward_kind=_lib.REWARD_EXP, channel=0, P=1000, H=5):
-    pr = _lib.Particles()
-    pr.P, pr.H = P, H
-    pr.dyn = _gp()
-    pr.pol.kind, pr.pol.Ds, pr.pol.U, pr.pol.squash = kind, 3, 1, 1
-    pr.pol.max_action = pr.pol.W = pr.pol.b = FAKE
-    if kind == _lib.POLICY_RBF:
-        pr.pol.rbf = _gp(n=20, D=3, E=1, mode=1, iK=None, ldk=0)
-    pr.n_rewards = 1
-    pr.rewards[0].kind, pr.rewards[0].channel, pr.rewards[0].coef = reward_kind, channel, 1.0
-    pr.rewards[0].W = pr.rewards[0].t = FAKE
-    pr.x0 = pr.eps = pr.traj = pr.act = pr.step_reward = pr.step_risk = pr.ret = pr.ws = FAKE
-    pr.ws_bytes = 0
-    return pr
+from util import CUOBJDUMP, ROOT, sass
 
 
 def _run(pr):

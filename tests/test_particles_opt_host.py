@@ -12,21 +12,9 @@ import torch
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _particles
-from test_particles_grad_host import CUOBJDUMP, _grad, _sass
-
-PT_MAX_P = 65535 * 32
-
-
-def _batched(kind=_lib.POLICY_LINEAR, **kw):
-    """a valid description of R policies, each array with its own per-restart block"""
-    pr = _particles(kind, **kw)
-    if kind == _lib.POLICY_LINEAR:
-        pr.pol.W_bs, pr.pol.b_bs = 3, 1
-    else:
-        r = pr.pol.rbf
-        r.X_bs, r.ell_bs, r.sf2_bs, r.beta_bs = 20 * 3, 3, 1, 20
-    return pr
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from particle_cases import _linear_pilco, _safe_pilco
+from util import CUOBJDUMP, sass_named
 
 
 def _run(pr, R, g):
@@ -125,29 +113,12 @@ def test_batch_grad_workspace_bytes():
 def test_batched_kernels_sass():
     names = ["pt_step_kernel", "pg_step_kernel", "pg_param_kernel", "pg_rbf_finish_kernel", "rbf_factor_bwd_kernel",
              "gp_predict_kernel", "gp_predict_vjp_kernel"]
-    sass = _sass(names)
+    sass = sass_named(names)
     assert set(sass) == set(names)
     for k, text in sass.items():
         assert not re.search(r"\b(STL|LDL)\b", text), k
     for k in ("gp_predict_kernel", "gp_predict_vjp_kernel"):
         assert "DMMA.16x8x16" in sass[k] and "UBLKCP" in sass[k], k
-
-
-def _linear_pilco(**kw):
-    from pilco.models import PILCO
-    from pilco.controllers import LinearController
-    X = np.random.RandomState(0).rand(20, 3); Y = 0.1 * X[:, :2]
-    return PILCO((X, Y), controller=LinearController(2, 1), horizon=4, **kw), X
-
-
-def _safe_pilco():
-    from safe_pilco_extension.safe_pilco import SafePILCO
-    from safe_pilco_extension.rewards_safe import RiskOfCollision
-    from pilco.controllers import LinearController
-    from pilco.rewards import LinearReward
-    X = np.random.RandomState(1).rand(30, 5); Y = 0.1 * X[:, :4]
-    return SafePILCO((X, Y), controller=LinearController(4, 1), horizon=4, reward_add=LinearReward(4, np.ones(4)),
-                     reward_mult=RiskOfCollision(4, [0.0, 0.1], [0.6, 0.9]), mu=-4.0)
 
 
 def test_sampled_optimisation_fails_loudly_without_gpu(monkeypatch):

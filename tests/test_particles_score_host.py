@@ -1,6 +1,6 @@
 """CPU tests of the score-function gradient of the particle return (pilco_particles_rollout_score_grad,
 engine.ParticlePlan(estimator="score"), PILCO.sample_policy_gradient(estimator="score")): the torch oracle
-(tests/score_grad_oracle.py) against the moment-matching gradient where moment matching is exact and against the
+(tests/particle_grad_oracle.py) against the moment-matching gradient where moment matching is exact and against the
 pathwise oracle, the workspace size, argument validation of the C entry point (rejecting calls only, with the status
 codes of pilco_particles_rollout_batch_grad), the SASS of the new kernels, and the rejected estimator arguments."""
 import ctypes as C
@@ -13,12 +13,11 @@ import torch
 
 from pilco_b200 import _lib, engine
 from pilco_b200._lib import lib
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from particle_cases import _problem
 from particle_oracle import particle_rollout
-from particle_grad_oracle import value_and_grad
-from score_grad_oracle import score_grad
-from test_particles_host import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _particles
-from test_particles_grad_host import CUOBJDUMP, _grad, _problem, _sass
-from test_particles_opt_host import PT_MAX_P, _batched
+from particle_grad_oracle import score_grad, value_and_grad
+from util import CUOBJDUMP, sass_named
 
 F64 = torch.float64
 
@@ -212,7 +211,7 @@ def test_score_grad_argument_validation():
 @pytest.mark.skipif(not os.path.exists(CUOBJDUMP), reason="cuobjdump not available")
 def test_score_kernels_sass():
     names = ["ps_togo_kernel", "ps_base_kernel", "ps_cot_kernel", "ps_zbar_kernel"]
-    sass = _sass(names)
+    sass = sass_named(names)
     assert set(sass) == set(names)
     for k, text in sass.items():                                # no spills, no local memory (MAXD = 16 registers)
         assert not re.search(r"\b(STL|LDL)\b", text), k

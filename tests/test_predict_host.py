@@ -3,6 +3,7 @@ predict_log_density): the (iK, beta) identity the kernel relies on against GPflo
 validation of the C entry point, the workspace bound, the GPflow method surface, the no-GPU failure, and the SASS of
 the kernel."""
 import ctypes as C
+import functools
 import inspect
 import os
 import re
@@ -12,13 +13,11 @@ import pytest
 import torch
 
 from oracle import python_port as pp
-from pilco_b200 import _lib
 from pilco_b200._lib import lib
+import abi_fakes
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE
 from predict_oracle import fitc_predict_f, gpr_predict_f, ik_beta_predict
 from util import CUOBJDUMP, sass, scaled_err
-
-ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_UNSUP = -1, -2, -3, -4, -6
-FAKE = 0x10000
 
 
 def _recipe(N, seed=0, d=3, k=2):
@@ -58,13 +57,7 @@ def test_ik_beta_form_equals_gpflow_fitc_with_per_output_z():
         assert np.max(np.abs(v - v_ref)) / sf2[e] <= 1e-7
 
 
-def _gp(n=300, D=3, E=2, mode=0, iK=FAKE, ldk=320, bs=0):
-    g = _lib.GpModel()
-    g.n, g.D, g.E, g.mode = n, D, E, mode
-    g.X = g.ell = g.sf2 = g.beta = FAKE
-    g.X_bs = bs
-    g.iK, g.ldk = iK, ldk
-    return g
+_gp = functools.partial(abi_fakes._gp, n=300, D=3, E=2, ldk=320)
 
 
 def _call(g, e0=0, ne=2, T=10, Xs=FAKE, mean=FAKE, var=FAKE, full_cov=0, ws=FAKE, wsb=1 << 40):

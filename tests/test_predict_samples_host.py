@@ -13,7 +13,7 @@ import torch
 
 from pilco_b200._lib import lib
 from predict_samples_oracle import predict_f_samples
-from test_abi_errors import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _gp
+from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _gp
 from util import CUOBJDUMP, make_gp_problem, sass
 
 WSB = lambda *a: int(lib.pilco_gp_predict_samples_workspace_bytes(*a))

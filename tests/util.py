@@ -36,6 +36,11 @@ def sass(pattern):
     return {name: text for name, text in _sass_functions() if re.search(pattern, name)}
 
 
+def sass_named(names):
+    """{name: SASS text} of the kernels whose mangled names contain one of ``names`` (keyed by the first that does)"""
+    return {next(k for k in names if k in m): text for m, text in sass("|".join(map(re.escape, names))).items()}
+
+
 def relerr(a, b):
     a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
     return float(np.max(np.abs(a - b) / (np.abs(b) + 1e-300)))
