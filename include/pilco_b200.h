@@ -12,7 +12,7 @@
  *     (so every `*_forward/_backward/rollout` call is CUDA-graph capturable);
  *   - return value: 0 ok, <0 invalid argument (see pilco_status_string); numerical failures
  *     (non-PD matrices) are reported per batch element in the device `info` array
- *     (0 ok, bit0: non-PD input-covariance system, bit1: non-PD Gram matrix);
+ *     (0 ok, bit0: input outside the moment match's domain -- see pilco_mm_forward --, bit1: non-PD Gram matrix);
  *   - batch dimension R = independent rollouts ("policy restarts", pilco/models/pilco.py:98-107);
  *   - matrices are row-major; `*_bs` arguments are batch strides in doubles (0 = one array shared
  *     by all R batch elements).
@@ -58,6 +58,16 @@ typedef struct pilco_gp_model {
                                                NULL when mode==1.  Shared by the batch. */
 } pilco_gp_model;
 
+/* Moment match of N(m, s) through the GP.  Domain, checked on the device per batch element and reported as info bit0
+ * (the outputs of a flagged element are not meaningful):
+ *   - every length-scale lies in (0, inf): zero, negative, infinite and NaN length-scales are flagged (only ell^2
+ *     enters the formulas, but a negative length-scale is taken for a caller's error, not for its absolute value);
+ *   - s (its symmetric part is used) is positive semi-definite up to PILCO_MM_PSD_TOL: s = 0 and singular s are valid
+ *     inputs; an eigenvalue below -PILCO_MM_PSD_TOL x max_i |s_ii| is flagged, as is a NaN;
+ *   - s + diag(ell_a^2) and s + diag(1 / (ell_a^-2 + ell_b^-2)) are positive definite (implied by the above).
+ * The same holds for pilco_mm_forward_taped and for the dynamics step of pilco_rollout.  pilco_mm_backward has no info
+ * output: call it with inputs a forward call has accepted. */
+#define PILCO_MM_PSD_TOL 1e-6
 int pilco_mm_forward(const pilco_gp_model* gp, int R,
                      const double* m,       /* [R,D]   */
                      const double* s,       /* [R,D,D] */

@@ -28,13 +28,7 @@ static int launch_tile(const MMParams& p, cudaStream_t st) {
                          mm_tile_m16_kernel<KS>>((int)mm_tile_smem_bytes(TILE_CM, 20)))
         return PILCO_ERR_LAUNCH;
     const size_t smem = mm_tile_smem_bytes(p.L.np, p.L.ldz);
-    // row blocks per CTA: a CTA's fixed cost (TMA staging of the columns and the exp table, barrier, first-load
-    // latency: ~5 k cycles against ~16 k per 64-row sweep at the metric shape) is paid once for all its row blocks.
-    // All of a pair's row blocks go to one CTA as soon as pairs x restarts still give every SM a CTA; smaller
-    // launches keep enough CTAs to fill the machine (2 CTAs per SM).
-    int rpc = p.L.NB;
-    const long long pr = (long long)p.L.P * p.R, nsm = pilco_sm_count();
-    if (pr < nsm) { rpc = (int)(((long long)p.L.NB * pr) / (2 * nsm)); if (rpc < 1) rpc = 1; }
+    int rpc = mm_tile_rpc(p.L.NB, p.L.P, p.R, pilco_sm_count());   // row blocks per CTA
     if (rpc_env > 0) rpc = rpc_env;
     if (rpc > p.L.NB) rpc = p.L.NB;
     dim3 grid((p.L.NB + rpc - 1) / rpc, p.L.P, p.R);

@@ -84,6 +84,35 @@ static inline MMParams mm_params(const pilco_gp_model* gp, int R, const double* 
     return p;
 }
 
+// The launch decisions that follow the batch size and the machine, as functions of (shape, R, SMs) so that the host
+// suite can say which kernel branch a given case runs (tests/mm_cases.py).
+//
+// Row blocks per forward tile CTA: a CTA's fixed cost (TMA staging of the columns and the exp table, barrier,
+// first-load latency: ~5 k cycles against ~16 k per 64-row sweep at the metric shape) is paid once for all its row
+// blocks.  All NB row blocks of a pair go to one CTA as soon as pairs x restarts still give every SM a CTA; smaller
+// launches keep enough CTAs to fill the machine (2 CTAs per SM).
+static inline int mm_tile_rpc(int NB, int P, int R, int nsm) {
+    const long long pr = (long long)P * R;
+    if (pr >= nsm) return NB;
+    const int rpc = (int)(((long long)NB * pr) / (2LL * nsm));
+    return rpc < 1 ? 1 : rpc;
+}
+// Both setup stages in ONE launch while the whole launch is small -- at most half the SMs' worth of CTAs: a single
+// restart, or the RBF policy's few tasks (see mm_setup_launch)
+static inline bool mm_setup_is_fused(int ntask, int R, int nsm) { return (long long)ntask * R <= nsm / 2; }
+// Row splits of one pair over the CTAs of the taped tile kernel (mm_tape.cuh): 1 once pairs x restarts fill the machine
+// twice over, at most 4, and never fewer than 8 row octets per split
+static inline int mm_tape_splits_on(int n, int P, int R, int nsm) {
+    const int NO = (n + 7) / 8;
+    const long long pr = (long long)P * R, fill = 2LL * nsm;
+    int cs = 1;
+    if (pr < fill) cs = (int)((fill + pr - 1) / pr);
+    int cap = NO / 8;
+    if (cap < 1) cap = 1;
+    if (cap > 4) cap = 4;
+    return cs < cap ? cs : cap;
+}
+
 
 #ifdef __CUDACC__
 
@@ -148,10 +177,27 @@ __device__ __forceinline__ void setup_stage_s(const MMParams& p, int r, double* 
     }
 }
 
+// Is the symmetrised input covariance s_s positive semi-definite?  (one warp.)  The Cholesky of s + tau I, tau =
+// PILCO_MM_PSD_TOL x the largest |s_ii|, succeeds for every PSD s (zero, singular, badly conditioned: its rounding is far
+// below tau) and fails as soon as s has an eigenvalue below -tau -- an input the moment match would still evaluate to
+// finite numbers, since s + diag(ell^2) stays positive definite.
+template <int DP>
+__device__ __forceinline__ bool setup_s_is_psd(const double* s_s, int D, int lane) {
+    const int li = lane < DP ? lane : DP - 1;
+    double smax = 0.0;
+    for (int d = 0; d < D; ++d) smax = fmax(smax, fabs(s_s[d * SLD + d]));
+    const double tau = fma(PILCO_MM_PSD_TOL, smax, 1e-300);
+    double arow[DP], ipd[DP];
+#pragma unroll
+    for (int j = 0; j < DP; ++j) arow[j] = s_s[li * SLD + j] + (j == li ? tau : 0.0);
+    return chol_regs<DP>(arow, ipd, lane);
+}
+
 // stage 1 of ONE task by ONE warp (scratch Ls, Qs [MAXD*SLD], pa, pb, dinv [MAXD] private to the warp)
 template <int DP, bool BWD>
 __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int task, int lane, const double* s_s,
-                                               double* Ls, double* Qs, double* pa, double* pb, double* dinv) {
+                                               double* Ls, double* Qs, double* pa, double* pb, double* dinv,
+                                               bool check_s = true) {
     const pilco_gp_model& gp = p.gp;
     const int D = gp.D, E = gp.E;
     const MMWs& L = p.L;
@@ -163,13 +209,16 @@ __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int tas
     if (!BWD && task < E) {
         // ---------------- output task: W_a = (s + Lambda_a^2)^-1 and c_a ----------------
         const int a = task;
-        if (lane < DP) { const double l = lane < D ? ell[a * D + lane] : 1.0; pa[lane] = l * l; }
+        const double l = lane < D ? ell[a * D + lane] : 1.0;
+        const bool lbad = !(l > 0.0 && l < INFINITY);          // a length-scale outside (0, inf): reported, never used silently
+        if (lane < DP) pa[lane] = l * l;
         __syncwarp();
-        double arow[DP];
+        double arow[DP], ipd[DP];
+        // once per restart: is s itself positive semi-definite?  (two-stage form: a warp of its own, see mm_setup1_kernel)
+        const bool sbad = check_s && a == 0 && !setup_s_is_psd<DP>(s_s, D, lane);
 #pragma unroll
         for (int j = 0; j < DP; ++j) arow[j] = s_s[li * SLD + j] + (j == li ? pa[li] : 0.0);
-        double ipd[DP];
-        const bool ok = chol_regs<DP>(arow, ipd, lane);
+        const bool ok = chol_regs<DP>(arow, ipd, lane) && !sbad && !__any_sync(0xffffffffu, lbad);
         if (lane < DP) {
 #pragma unroll
             for (int j = 0; j < DP; ++j) Ls[lane * SLD + j] = arow[j];
@@ -201,8 +250,9 @@ __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int tas
     const int q = task - E;
     int a, b;
     if (BWD) { a = q / E; b = q % E; } else pair_decode(q, a, b);
+    const double la = lane < D ? ell[a * D + lane] : 1.0, lb = lane < D ? ell[b * D + lane] : 1.0;
+    const bool lbad = !(la > 0.0 && la < INFINITY && lb > 0.0 && lb < INFINITY);
     if (lane < DP) {
-        const double la = lane < D ? ell[a * D + lane] : 1.0, lb = lane < D ? ell[b * D + lane] : 1.0;
         pa[lane] = lane < D ? 1.0 / (la * la) : 0.0;
         pb[lane] = lane < D ? 1.0 / (lb * lb) : 0.0;
         dinv[lane] = lane < D ? 1.0 / (1.0 / (la * la) + 1.0 / (lb * lb)) : 0.0;      // 1/(p_a+p_b)
@@ -212,7 +262,7 @@ __device__ __forceinline__ void mm_setup1_task(const MMParams& p, int r, int tas
 #pragma unroll
     for (int j = 0; j < DP; ++j) arow[j] = s_s[li * SLD + j] + (j == li ? (li < D ? dinv[li] : 1.0) : 0.0);
     double ipd[DP];
-    const bool ok = chol_regs<DP>(arow, ipd, lane);
+    const bool ok = chol_regs<DP>(arow, ipd, lane) && !__any_sync(0xffffffffu, lbad);
     if (lane < DP) {
 #pragma unroll
         for (int j = 0; j < DP; ++j) Ls[lane * SLD + j] = arow[j];
@@ -289,7 +339,10 @@ __global__ void __launch_bounds__(32 * SETUP_WARPS) mm_setup1_kernel(MMParams p)
     PDL_ENTRY();
     const int r = blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int ntask = BWD ? p.L.P : p.gp.E + p.L.P;
+    // forward mode: the last CTA holds no task -- its warp 0 checks that s is positive semi-definite, beside the tasks
+    // instead of in front of one of them
+    const bool checker = !BWD && blockIdx.x == gridDim.x - 1;
+    const int ntask = checker ? 0 : (BWD ? p.L.P : p.gp.E + p.L.P);
     const int task0 = blockIdx.x * SETUP_WARPS + warp;
     const int task = BWD ? task0 + p.gp.E : task0;             // BWD: pair tasks only (ordered pairs)
     __shared__ double s_s[MAXD * SLD];                         // symmetrised input covariance (all warps)
@@ -299,7 +352,8 @@ __global__ void __launch_bounds__(32 * SETUP_WARPS) mm_setup1_kernel(MMParams p)
     setup_stage_s<DP>(p, r, s_s);
     __syncthreads();
     if (task0 < ntask)
-        mm_setup1_task<DP, BWD>(p, r, task, lane, s_s, sLw[warp], sQw[warp], spw[warp][0], spw[warp][1], spw[warp][2]);
+        mm_setup1_task<DP, BWD>(p, r, task, lane, s_s, sLw[warp], sQw[warp], spw[warp][0], spw[warp][1], spw[warp][2], false);
+    if (checker && warp == 0 && !setup_s_is_psd<DP>(s_s, p.gp.D, lane) && lane == 0 && p.info) atomicOr(&p.info[r], 1);
     if (!BWD) setup_publish_zeta<DP>(p, r, blockIdx.x * blockDim.x + tid, gridDim.x * blockDim.x);
 }
 
@@ -755,7 +809,7 @@ static inline void mm_setup_launch(const MMParams& p, cudaStream_t st) {
     {
         static int mode = -1;
         if (mode < 0) { const char* e = getenv("PILCO_SETUP_FUSED"); mode = (e && (e[0] == '0' || e[0] == '1')) ? e[0] - '0' : 2; }
-        const bool fused = mode == 2 ? (long long)ntask * p.R <= pilco_sm_count() / 2 : mode == 1;
+        const bool fused = mode == 2 ? mm_setup_is_fused(ntask, p.R, pilco_sm_count()) : mode == 1;
         if (fused) {
             // pair tasks are split over up to 3 CTAs, one 128-row chunk each (the stage-2 sweep is what the step waits for)
             int split = (p.L.np + 127) / 128;
@@ -765,7 +819,7 @@ static inline void mm_setup_launch(const MMParams& p, cudaStream_t st) {
             return;
         }
     }
-    launch_hi(mm_setup1_kernel<DP, BWD>, dim3((ntask + SETUP_WARPS - 1) / SETUP_WARPS, p.R), dim3(32 * SETUP_WARPS), 0, st, p);
+    launch_hi(mm_setup1_kernel<DP, BWD>, dim3((ntask + SETUP_WARPS - 1) / SETUP_WARPS + (BWD ? 0 : 1), p.R), dim3(32 * SETUP_WARPS), 0, st, p);
     if constexpr (BWD) {
         launch_hi(mm_setup2_bwd_kernel<DP>, dim3(ntask, p.R), dim3(128), 0, st, p);
     } else {

@@ -22,16 +22,7 @@
 // (host only: depends on the current device's SM count.  A tape lives in one device's memory and its forward pass and
 // reverse sweep run on that device, so both derive the same layout; every entry point also checks tape_bytes against the
 // layout of the current device, so a tape sized on a device with fewer splits is rejected, never overrun.)
-static inline int mm_tape_splits(int n, int P, int R) {
-    const int NO = (n + 7) / 8;
-    const long long pr = (long long)P * R, fill = 2LL * pilco_sm_count();
-    int cs = 1;
-    if (pr < fill) cs = (int)((fill + pr - 1) / pr);
-    int cap = NO / 8;
-    if (cap < 1) cap = 1;
-    if (cap > 4) cap = 4;
-    return cs < cap ? cs : cap;
-}
+static inline int mm_tape_splits(int n, int P, int R) { return mm_tape_splits_on(n, P, R, pilco_sm_count()); }
 
 static inline MMTapeL mm_tape_layout(int n, int D, int E, int R) {
     MMTapeL T;
@@ -344,6 +335,7 @@ __device__ __forceinline__ void tape_sweep_m16(const double* __restrict__ sZ, co
 // bench shapes: the last pass of every pair) does not fall back to one octet per warp: warps 0-3 take the octet pairs
 // {2w, 2w + 1} of the remaining block over all columns, warps 4-7 have no rows in that pass.  An octet's row-side results
 // (hr, HZ, T) are the same whichever pass form it ran in, so they do not depend on the row splits (i.e. the batch size).
+// The column sums hc do: they are stored per row split and added up by the reverse sweep (DESIGN.md section 4).
 template <int KS, bool DIAG>
 __device__ __forceinline__ void mm_tape_body_m16(const MMParams& p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];

@@ -1,5 +1,6 @@
 // Host build of the workspace-layout functions (pilco_b200/csrc/{mm_kernels,mm_backward,rollout}.cuh) so the CPU suite
-// can check their invariants (ordering, alignment, sizes) against the sizes the shared library reports.
+// can check their invariants (ordering, alignment, sizes) against the sizes the shared library reports, and of the launch
+// decisions of the moment match (tests/mm_cases.py states from them which kernel branch a case runs).
 #include "../../pilco_b200/csrc/mm_backward.cuh"
 #include "../../pilco_b200/csrc/rollout.cuh"
 
@@ -14,4 +15,9 @@ int layout_mm(int n, int D, int E, int ordered, unsigned long long* out) {
 unsigned long long layout_bwd_per_r(int n, int D, int E, int need_param) { return mm_bws_layout(n, D, E, need_param).per_r; }
 int layout_pair(int q, int* a, int* b) { int aa, bb; pair_decode(q, aa, bb); *a = aa; *b = bb; return pair_index(aa, bb); }
 int layout_misc(int D, int* ldz, int* ks) { *ldz = ldz_of(D); *ks = ksteps_of(D); return pad64(D); }
+// the launch decisions on a machine of nsm SMs: row blocks per forward tile CTA, row splits of the taped tile kernel,
+// one fused setup launch or the two-stage form
+int launch_tile_rpc(int NB, int P, int R, int nsm) { return mm_tile_rpc(NB, P, R, nsm); }
+int launch_tape_splits(int n, int P, int R, int nsm) { return mm_tape_splits_on(n, P, R, nsm); }
+int launch_setup_fused(int ntask, int R, int nsm) { return mm_setup_is_fused(ntask, R, nsm) ? 1 : 0; }
 }
