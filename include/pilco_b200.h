@@ -337,6 +337,35 @@ typedef struct pilco_rollout_grad {
 size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro);
 int    pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream);
 
+/* ---- angular state dimensions -----------------------------------------------------------------
+ * PILCO's trigonometric augmentation (gTrig in propagate.m): the angular state dimensions dims[0 .. A-1] of x [Ds]
+ * reach the policy and the dynamics GP through the feature map
+ *   phi(x) = [x_j for j not an angle, increasing j] ++ [sin x_a, cos x_a for a = dims[0], ..., dims[A-1]]   (Dh = Ds + A)
+ * whose Gaussian moments are exact.  The state itself stays raw: m0, S0, traj_m, traj_S, gm0, gS0, the state reward
+ * terms and the dynamics GP's outputs (deltas of x, angles unwrapped) are in Ds.  With angles, a pilco_rollout has
+ * pol.Ds = Dh, dyn.D = Dh + U and dyn.E = Ds, and its joint state-action terms (PILCO_REWARD_*_SA) are evaluated at
+ * the Gaussian the dynamics receive, [phi(x), u] (D = Dh + U).  Every call below with ang == NULL or ang->A == 0 is
+ * the corresponding call without angles.  Validation before any work is enqueued: PILCO_ERR_DIM for a dimension out of
+ * range or repeated, A > Ds or Dh + U > PILCO_MAX_D, otherwise the status codes of the call without angles. */
+typedef struct pilco_angles {
+    int A;                      /* number of angular dimensions, 0 .. Ds */
+    int dims[PILCO_MAX_D];      /* their state indices, distinct */
+} pilco_angles;
+
+/* moments of phi(x) for x ~ N(m, s): M [R,Dh], S [R,Dh,Dh] and C = inv(s) cov(x, phi(x)) [R,Ds,Dh] (no inverse is
+ * formed: s = 0 and singular s are valid).  With no angles: M = m, S = s, C = I. */
+int pilco_trig_moments(int Ds, int R, const pilco_angles* ang, const double* m /*[R,Ds]*/, const double* s /*[R,Ds,Ds]*/,
+                       double* M, double* S, double* C, pilco_stream_t stream);
+
+size_t pilco_rollout_angles_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang);
+size_t pilco_rollout_angles_tape_bytes(const pilco_rollout* ro, const pilco_angles* ang);
+size_t pilco_rollout_angles_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang);
+int    pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* ang, pilco_stream_t stream);
+/* policy gradients in the policy's (Dh) layout; gm0 [R,Ds] and gS0 [R,Ds,Ds] with respect to the raw initial moments,
+ * gS0 symmetric when angles are present (the gradient with respect to a symmetric S0) */
+int    pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
+                                     pilco_stream_t stream);
+
 /* ---- particle rollout -------------------------------------------------------------------------
  * Monte Carlo check of the moment-matching cascade (nothing in the reference; the PILCO papers validate moment
  * matching against particle rollouts of the same model).  P particles follow the Markov chain whose Gaussian

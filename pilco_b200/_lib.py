@@ -70,12 +70,18 @@ class ParticlesGrad(C.Structure):
                 ("value", c_dp), ("ws", c_dp), ("ws_bytes", C.c_size_t)]
 
 
+class Angles(C.Structure):
+    """mirror of ``pilco_angles``"""
+    _fields_ = [("A", C.c_int), ("dims", C.c_int * 16)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
 JOINT_REWARDS = (REWARD_EXP_SA, REWARD_LINEAR_SA)
 CHANNEL_ADD, CHANNEL_MULT = 0, 1
 ABI_VERSION = 3
+ABI_MAX_D = 16                                   # PILCO_MAX_D
 
 # name -> (restype, argtypes); every symbol declared in include/pilco_b200.h
 SIGNATURES = {
@@ -121,6 +127,12 @@ SIGNATURES = {
     "pilco_mm_backward": (C.c_int, [C.POINTER(GpModel), C.c_int] + [c_dp] * 11 + [c_dp, C.c_size_t, c_dp]),
     "pilco_rollout_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout)]),
     "pilco_rollout_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(RolloutGrad), c_dp]),
+    "pilco_trig_moments": (C.c_int, [C.c_int, C.c_int, C.POINTER(Angles)] + [c_dp] * 6),
+    "pilco_rollout_angles_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles)]),
+    "pilco_rollout_angles_tape_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles)]),
+    "pilco_rollout_angles_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles)]),
+    "pilco_rollout_angles_forward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), c_dp]),
+    "pilco_rollout_angles_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(RolloutGrad), c_dp]),
     "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
     "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
     "pilco_gp_predict_vjp_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

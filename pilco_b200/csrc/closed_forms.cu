@@ -46,6 +46,12 @@ __global__ void __launch_bounds__(32) box_risk_kernel(int Ds, const double* prm,
     }
 }
 
+__global__ void __launch_bounds__(128) tg_moments_kernel(TrigMap tm, const double* m, const double* s,
+                                                         double* M, double* S, double* C) {
+    const size_t r = blockIdx.x, Ds = tm.Ds, Dh = trig_dh(tm);
+    dev_trig(tm, m + r * Ds, s + r * Ds * Ds, M + r * Dh, S + r * Dh * Dh, C + r * Ds * Dh);
+}
+
 extern "C" {
 
 int pilco_squash_sin(int U, int R, const double* m, const double* s, const double* max_action,
@@ -82,6 +88,17 @@ int pilco_box_risk(int Ds, int R, const double* prm, const double* m, const doub
     if (!prm || !m || !s || !risk) return PILCO_ERR_NULL;
     if (Ds < 1 || Ds > MAXD || R < 1) return PILCO_ERR_DIM;
     box_risk_kernel<<<R, 32, 0, (cudaStream_t)stream>>>(Ds, prm, m, s, risk, drisk_dm, drisk_dv);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
+int pilco_trig_moments(int Ds, int R, const pilco_angles* ang, const double* m, const double* s,
+                       double* M, double* S, double* C, pilco_stream_t stream) {
+    if (!m || !s || !M || !S || !C) return PILCO_ERR_NULL;
+    TrigMap tm;
+    const int A = ang ? ang->A : 0;
+    if (R < 1 || trig_map_make(Ds, A, ang ? ang->dims : nullptr, &tm) || Ds + A > MAXD) return PILCO_ERR_DIM;
+    tg_moments_kernel<<<R, 128, 0, (cudaStream_t)stream>>>(tm, m, s, M, S, C);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }

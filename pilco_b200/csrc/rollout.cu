@@ -163,13 +163,14 @@ __global__ void __launch_bounds__(128) ro_reward_sum_kernel(RoDev p) {
     p.reward[r] = s;
 }
 
-int ro_check(const pilco_rollout* ro) {
+// validation of a rollout whose dynamics GP predicts E outputs (the state dimension): E = pol.Ds without angles
+static int ro_check_as(const pilco_rollout* ro, int E) {
     if (!ro) return PILCO_ERR_NULL;
     if (ro->R < 1 || ro->H < 0) return PILCO_ERR_DIM;
     int rc = mm_check_model(&ro->dyn);
     if (rc) return rc;
     const int Ds = ro->pol.Ds, U = ro->pol.U;
-    if (Ds < 1 || U < 1 || Ds + U != ro->dyn.D || ro->dyn.E != Ds) return PILCO_ERR_DIM;
+    if (Ds < 1 || U < 1 || Ds + U != ro->dyn.D || ro->dyn.E != E) return PILCO_ERR_DIM;
     if (ro->pol.squash && !ro->pol.max_action) return PILCO_ERR_NULL;
     if (ro->pol.kind == PILCO_POLICY_LINEAR) { if (!ro->pol.W || !ro->pol.b) return PILCO_ERR_NULL; }
     else if (ro->pol.kind == PILCO_POLICY_RBF) {
@@ -187,6 +188,17 @@ int ro_check(const pilco_rollout* ro) {
     }
     if (!ro->m0 || !ro->S0 || !ro->traj_m || !ro->traj_S || !ro->reward || !ro->ws) return PILCO_ERR_NULL;
     return PILCO_OK;
+}
+
+int ro_check(const pilco_rollout* ro) { return ro ? ro_check_as(ro, ro->pol.Ds) : PILCO_ERR_NULL; }
+
+int tg_check(const pilco_rollout* ro, const pilco_angles* ang, TrigMap* tm) {
+    if (!ro) return PILCO_ERR_NULL;
+    if (!ang || ang->A == 0) { trig_map_make(1, 0, nullptr, tm); tm->A = 0; return ro_check(ro); }
+    const int Ds = ro->dyn.E;
+    if (trig_map_make(Ds, ang->A, ang->dims, tm) || Ds + ang->A + ro->pol.U > MAXD) return PILCO_ERR_DIM;
+    if (ro->pol.Ds != Ds + ang->A) return PILCO_ERR_DIM;
+    return ro_check_as(ro, Ds);
 }
 
 extern "C" {
@@ -291,6 +303,210 @@ int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
         CUDA_LAUNCH_CHECK();
     }
     launch_hi(ro_reward_sum_kernel, dim3((R + 127) / 128), dim3(128), 0, st, d);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------
+// Angular state dimensions (pilco_rollout_angles_forward).  The state x [Ds] stays raw; the policy and the dynamics GP
+// see phi(x) [Dh] (trig_math.cuh).  Per step t:
+//   tg_state<t>   grid R : [t>0: finish dynamics MM of step t-1 + glue with cx_{t-1}] -> traj[t]; phi moments (m^, S^, C^);
+//                          linear policy on (m^, S^) + squash + joint [phi, u] + cx_t
+//   (RBF policy)  mm_setup/mm_tile on the policy GP at (m^, S^), then tg_policy<t>: finish + squash + joint + cx_t
+//   mm_setup / mm_tile on the dynamics GP with the joint Gaussian of step t (D = Dh + U)
+// cx_t = cov(x_t, [phi(x_t), u_t]) = S_x C^ [I, V_u] [Ds, Dh + U] takes the place of the first Ds rows of the joint
+// covariance in the glue: S' = S_x + S_d + cx V_d + (cx V_d)^T.  The reward launches are ro_reward's, unchanged.
+// ---------------------------------------------------------------------------------------------
+struct TgDev {
+    RoDev p;                  // p.Ds = Dh: the policy's input dimension; traj_m / traj_S / m0 / S0 in Ds
+    TrigMap tm;
+    double *mh, *Sh, *Ch, *cx;        // slots of step t [R, len]
+    const double* cx_prev;            // cx of step t-1
+};
+
+// cx = [Q, Q V_u],  Q = S_x C^  [Ds, Dh]
+__device__ __forceinline__ void tg_cross(const TgDev& g, int r, const double* sx, SmallScratch& sc) {
+    const int Ds = g.tm.Ds, Dh = g.p.Ds, U = g.p.U, D = Dh + U;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const double* Ch = g.Ch + (size_t)r * Ds * Dh;
+    const double* Vu = g.p.Vu + (size_t)r * Dh * U;
+    double* cx = g.cx + (size_t)r * Ds * D;
+    for (int e = tid; e < Ds * Dh; e += nt) {
+        const int i = e / Dh, k = e % Dh;
+        double v = 0.0;
+        for (int l = 0; l < Ds; ++l) v = fma(sx[i * Ds + l], Ch[l * Dh + k], v);
+        sc.C[i * SLD + k] = v;
+        cx[i * D + k] = v;
+    }
+    __syncthreads();
+    for (int e = tid; e < Ds * U; e += nt) {
+        const int i = e / U, j = e % U;
+        double v = 0.0;
+        for (int k = 0; k < Dh; ++k) v = fma(sc.C[i * SLD + k], Vu[k * U + j], v);
+        cx[i * D + Dh + j] = v;
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(128) tg_state_kernel(TgDev g) {
+    PDL_ENTRY();
+    __shared__ SmallScratch sc;
+    const RoDev& p = g.p;
+    const int r = blockIdx.x, t = p.t, Ds = g.tm.Ds, Dh = p.Ds, U = p.U;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    double* mx = p.traj_m + ((size_t)r * (p.H + 1) + t) * Ds;
+    double* sx = p.traj_S + ((size_t)r * (p.H + 1) + t) * Ds * Ds;
+    if (t == 0) {
+        for (int i = tid; i < Ds; i += nt) mx[i] = p.m0[(size_t)r * p.m0_bs + i];
+        for (int e = tid; e < Ds * Ds; e += nt) sx[e] = p.S0[(size_t)r * p.S0_bs + e];
+        __syncthreads();
+    } else {
+        mm_finish_device(p.dyn_prev, r);
+        __syncthreads();
+        // dev_glue reads the first Ds rows of a [., Ds + U'] matrix: cx [Ds, Dh + U] with U' = Dh + U - Ds
+        const int D = Dh + U;
+        dev_glue(Ds, D - Ds, mx - Ds, sx - Ds * Ds, g.cx_prev + (size_t)r * Ds * D,
+                 p.Md_prev + (size_t)r * Ds, p.Sd_prev + (size_t)r * Ds * Ds, p.Vd_prev + (size_t)r * D * Ds, mx, sx, sc);
+    }
+    if (t >= p.H) return;
+    double* mh = g.mh + (size_t)r * Dh;
+    double* Sh = g.Sh + (size_t)r * Dh * Dh;
+    dev_trig(g.tm, mx, sx, mh, Sh, g.Ch + (size_t)r * Ds * Dh);
+    if (p.pol_kind == PILCO_POLICY_LINEAR) {
+        dev_linear_action(Dh, U, p.W + (size_t)r * p.W_bs, p.b + (size_t)r * p.b_bs, mh, Sh,
+                          p.Mp + (size_t)r * U, p.Sp + (size_t)r * U * U, p.Vp + (size_t)r * Dh * U, sc);
+        ro_action_tail(p, r, mh, Sh, sc);
+        tg_cross(g, r, sx, sc);
+    }
+}
+
+__global__ void __launch_bounds__(128) tg_policy_kernel(TgDev g) {
+    PDL_ENTRY();
+    __shared__ SmallScratch sc;
+    const RoDev& p = g.p;
+    const int r = blockIdx.x, t = p.t, Ds = g.tm.Ds, Dh = p.Ds;
+    mm_finish_device(p.pol, r);
+    __syncthreads();
+    const double* sx = p.traj_S + ((size_t)r * (p.H + 1) + t) * Ds * Ds;
+    ro_action_tail(p, r, g.mh + (size_t)r * Dh, g.Sh + (size_t)r * Dh * Dh, sc);
+    tg_cross(g, r, sx, sc);
+}
+
+extern "C" {
+
+size_t pilco_rollout_angles_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang) {
+    if (!ang || ang->A == 0) return pilco_rollout_workspace_bytes(ro);
+    if (!ro || ro->R < 1 || ro->H < 0) return 0;
+    return tg_ws_layout(ro).total * sizeof(double);
+}
+
+size_t pilco_rollout_angles_tape_bytes(const pilco_rollout* ro, const pilco_angles* ang) {
+    (void)ang;                                        // the tape depends on the dynamics GP's shape only
+    return pilco_rollout_tape_bytes(ro);
+}
+
+int pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* ang, pilco_stream_t stream) {
+    TrigMap tm;
+    int rc = tg_check(ro, ang, &tm);
+    if (rc) return rc;
+    if (tm.A == 0) return pilco_rollout_forward(ro, stream);
+    const TgWs T = tg_ws_layout(ro);
+    const RoWs& L = T.b;
+    if (ro->ws_bytes < T.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
+    if (((uintptr_t)ro->ws) & 15) return PILCO_ERR_ALIGN;
+    if (ro->tape) {
+        const size_t need = pilco_rollout_tape_bytes(ro);
+        if (need == 0 && ro->H > 0) return PILCO_ERR_UNSUPPORTED;
+        if (ro->tape_bytes < need) return PILCO_ERR_WORKSPACE;
+        if (((uintptr_t)ro->tape) & 15) return PILCO_ERR_ALIGN;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)ro->ws;
+    const int R = ro->R, H = ro->H, Ds = tm.Ds, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U;
+    const size_t RR = (size_t)R;
+
+    TgDev g;
+    g.tm = tm;
+    RoDev& d = g.p;
+    d.R = R; d.H = H; d.Ds = Dh; d.U = U;
+    d.pol_kind = ro->pol.kind; d.squash = ro->pol.squash; d.maxa = ro->pol.max_action;
+    d.W = ro->pol.W; d.W_bs = ro->pol.W_bs; d.b = ro->pol.b; d.b_bs = ro->pol.b_bs;
+    int n_joint = 0;
+    pilco_reward_term joint_terms[8];
+    d.n_rewards = 0;
+    for (int k = 0; k < 8; ++k) d.rewards[k] = joint_terms[k] = pilco_reward_term();
+    for (int k = 0; k < ro->n_rewards; ++k) {
+        if (reward_on_joint(ro->rewards[k].kind)) joint_terms[n_joint++] = ro->rewards[k];
+        else d.rewards[d.n_rewards++] = ro->rewards[k];
+    }
+    d.m0 = ro->m0; d.m0_bs = ro->m0_bs; d.S0 = ro->S0; d.S0_bs = ro->S0_bs;
+    d.traj_m = ro->traj_m; d.traj_S = ro->traj_S; d.reward = ro->reward; d.step_reward = ro->step_reward;
+    d.risk = ws + L.risk; d.rew = ws + L.rew; d.step_risk = ro->step_risk; d.mult_mu = ro->mult_mu; d.n_mult = ro_count_mult(ro);
+
+    auto slot = [&](size_t base, size_t len, int t) { return ws + base + (size_t)t * RR * len; };
+    const MMTapeL TL = ro->tape ? mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R) : MMTapeL();
+    auto dyn_params = [&](int t) {
+        return mm_params(&ro->dyn, R, slot(L.mj, D, t), D, slot(L.sj, (size_t)D * D, t), (long long)D * D,
+                         slot(L.Md, Ds, t), slot(L.Sd, (size_t)Ds * Ds, t), slot(L.Vd, (size_t)D * Ds, t), ro->info,
+                         ws + L.dynws, ro->tape ? (double*)ro->tape + (size_t)t * RR * TL.per_r : nullptr, TL);
+    };
+    auto pol_params = [&](int t) {                   // the policy GP reads the feature moments of step t
+        return mm_params(&ro->pol.rbf, R, slot(T.mh, Dh, t), Dh, slot(T.Sh, (size_t)Dh * Dh, t), (long long)Dh * Dh,
+                         slot(L.Mp, U, t), slot(L.Sp, (size_t)U * U, t), slot(L.Vp, (size_t)Dh * U, t), ro->info,
+                         ws + L.polws);
+    };
+
+    if (ro->info) cudaMemsetAsync(ro->info, 0, sizeof(int) * RR, st);
+    for (int t = 0; t <= H; ++t) {
+        d.t = t;
+        const int tc = t < H ? t : H - 1 < 0 ? 0 : H - 1;
+        d.mj = slot(L.mj, D, tc); d.sj = slot(L.sj, (size_t)D * D, tc);
+        d.Mp = slot(L.Mp, U, tc); d.Sp = slot(L.Sp, (size_t)U * U, tc); d.Vp = slot(L.Vp, (size_t)Dh * U, tc);
+        d.Mu = slot(L.Mu, U, tc); d.Su = slot(L.Su, (size_t)U * U, tc); d.Cq = slot(L.Cq, (size_t)U * U, tc);
+        d.Vu = slot(L.Vu, (size_t)Dh * U, tc);
+        g.mh = slot(T.mh, Dh, tc); g.Sh = slot(T.Sh, (size_t)Dh * Dh, tc); g.Ch = slot(T.Ch, (size_t)Ds * Dh, tc);
+        g.cx = slot(T.cx, (size_t)Ds * D, tc);
+        if (t > 0) {
+            d.mj_prev = slot(L.mj, D, t - 1); d.sj_prev = slot(L.sj, (size_t)D * D, t - 1);
+            d.Md_prev = slot(L.Md, Ds, t - 1); d.Sd_prev = slot(L.Sd, (size_t)Ds * Ds, t - 1);
+            d.Vd_prev = slot(L.Vd, (size_t)D * Ds, t - 1);
+            g.cx_prev = slot(T.cx, (size_t)Ds * D, t - 1);
+            d.dyn_prev = dyn_params(t - 1);
+        } else {
+            d.mj_prev = d.sj_prev = d.Md_prev = d.Sd_prev = d.Vd_prev = nullptr;
+            g.cx_prev = nullptr;
+            d.dyn_prev = dyn_params(0);
+        }
+        if (ro->pol.kind == PILCO_POLICY_RBF && t < H) d.pol = pol_params(t); else d.pol = d.dyn_prev;
+        launch_hi(tg_state_kernel, dim3(R), dim3(128), 0, st, g);
+        CUDA_LAUNCH_CHECK();
+        if (t == H) break;
+        if (ro->pol.kind == PILCO_POLICY_RBF) {
+            rc = mm_forward_launch(d.pol, st, false);
+            if (rc) return rc;
+            launch_hi(tg_policy_kernel, dim3(R), dim3(128), 0, st, g);
+            CUDA_LAUNCH_CHECK();
+        }
+        rc = mm_forward_launch(dyn_params(t), st, false);
+        if (rc) return rc;
+    }
+    RoDev dr = d;                                     // the state terms read the raw trajectory
+    dr.Ds = Ds;
+    if (H > 0) {
+        launch_hi(ro_reward_kernel, dim3(H, R), dim3(128), 0, st, dr);
+        CUDA_LAUNCH_CHECK();
+    }
+    if (H > 0 && n_joint > 0) {                       // the joint terms read [phi, u]: ro_reward_joint's D = Dh + U
+        RoDev dj = d;
+        dj.n_rewards = n_joint;
+        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
+        dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
+        launch_hi(ro_reward_joint_kernel, dim3(H, R), dim3(128), 0, st, dj);
+        CUDA_LAUNCH_CHECK();
+    }
+    launch_hi(ro_reward_sum_kernel, dim3((R + 127) / 128), dim3(128), 0, st, dr);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }

@@ -20,6 +20,7 @@
 #include "mm_tape.cuh"
 #include "rollout.cuh"
 #include "small_kernels.cuh"
+#include "rollout_bwd.cuh"
 
 extern "C" size_t pilco_mm_bwd_workspace_bytes(int n, int D, int E, int R, int need_param);
 void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
@@ -29,10 +30,6 @@ struct RbWs {            // backward workspace (offsets in doubles)
     size_t gm, gS, gMd, gSd, gVd, gmj, gsj, gsjx, gMp, gSp, gVp, gbeta, gy, rgm, rgS, jgm, jgS, cnt, dynb, polb, total;
 };
 
-static bool rb_has_joint(const pilco_rollout* ro) {
-    for (int k = 0; k < ro->n_rewards && k < 8; ++k) if (reward_on_joint(ro->rewards[k].kind)) return true;
-    return false;
-}
 
 static RbWs rb_ws_layout(const pilco_rollout* ro) {
     const size_t R = ro->R, H = ro->H, Ds = ro->pol.Ds, U = ro->pol.U, D = Ds + U;
@@ -61,27 +58,6 @@ static RbWs rb_ws_layout(const pilco_rollout* ro) {
     return L;
 }
 
-struct RbDev {
-    int R, H, Ds, U, t;
-    int pol_kind, squash;
-    const double* maxa;
-    const double* W; long long W_bs;
-    int n_rewards; pilco_reward_term rewards[8];
-    const double* traj_m; const double* traj_S;
-    const double* risk; double mult_mu;       // MULT channel: per-step risks risk[t*R + r] saved by the forward
-    // forward slots of step t
-    const double *sj, *Vd, *Mp, *Sp, *Vp, *Mu, *Su, *Cq, *Vu;
-    // cotangent buffers [R, len]
-    double *gm, *gS, *gMd, *gSd, *gVd, *gmj, *gsj, *gsjx, *gMp, *gSp, *gVp;
-    double *gW, *gb;      // linear policy gradient accumulators [R,U,Ds], [R,U]
-    double *rgm, *rgS;    // reward gradients of every step (rb_reward_kernel)
-    double *jgm, *jgS;    // the joint state-action terms' gradients of every step, NULL without such terms
-    const double *mj0, *sj0;  // forward joint Gaussians of step 0; step t is R D (R D D) doubles further on
-    // taped dynamics VJP: task partials [R][ntask][MAXD + D*D] that rb_post sums into gmj / gsj itself (else NULL);
-    // then the glue cotangent gsjx is formed in shared memory too (no rb_pre launch)
-    const double* tpart; int tp_ntask;
-    unsigned* cnt;
-};
 
 // shared-memory scratch of rb_post_body (bytes), carved from a dynamic buffer
 struct RbPostSmem { SmallScratch sc; double gMu[MAXD], gSu[MAXD * MAXD], gVu[MAXD * MAXD], gB[MAXD * MAXD], gCd[MAXD], gsjx[MAXD * MAXD]; };
@@ -352,6 +328,18 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
     return PILCO_OK;
 }
 
+// rb_reward_kernel (state terms of d, at dimension ds.Ds) and, when dj is non-NULL, rb_reward_joint_kernel (joint terms, at
+// dimension dj->Ds + dj->U) for callers in other translation units (the reverse sweep with angles, rollout_angles_bwd.cu)
+int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st) {
+    launch_hi(rb_reward_kernel, dim3(ds.R, ds.H), dim3(128), 0, st, ds);
+    CUDA_LAUNCH_CHECK();
+    if (dj) {
+        launch_hi(rb_reward_joint_kernel, dim3(dj->R, dj->H), dim3(128), 0, st, *dj);
+        CUDA_LAUNCH_CHECK();
+    }
+    return PILCO_OK;
+}
+
 extern "C" {
 
 size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro) {
@@ -488,3 +476,4 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
 }
 
 }  // extern "C"
+

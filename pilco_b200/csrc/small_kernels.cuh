@@ -5,6 +5,7 @@
 #pragma once
 #include "common.cuh"
 #include "risk_math.cuh"
+#include "trig_math.cuh"
 
 #ifdef __CUDACC__
 
@@ -107,6 +108,26 @@ __device__ __forceinline__ void dev_glue(int Ds, int U, const double* mx, const 
         const int i = e / Ds, j = e % Ds;
         so[e] = Sd[e] + sx[e] + sc.A[i * SLD + j] + sc.A[j * SLD + i];
     }
+    __syncthreads();
+}
+
+// trigonometric feature map of the angular state dimensions (trig_math.cuh): N(m, s) [Ds] -> moments of phi(x) [Dh],
+// M [Dh], S [Dh,Dh], C = inv(s) cov(x, phi) [Ds,Dh].  Outputs must not alias inputs.
+__device__ __forceinline__ void dev_trig(const TrigMap& tm, const double* m, const double* s,
+                                         double* Mo, double* So, double* Co) {
+    const int tid = threadIdx.x, nt = blockDim.x, Ds = tm.Ds, Dh = trig_dh(tm);
+    for (int k = tid; k < Dh; k += nt) Mo[k] = trig_M_entry(tm, m, s, k);
+    for (int e = tid; e < Dh * Dh; e += nt) So[e] = trig_S_entry(tm, m, s, e / Dh, e % Dh);
+    for (int e = tid; e < Ds * Dh; e += nt) Co[e] = trig_C_entry(tm, m, s, e / Dh, e % Dh);
+    __syncthreads();
+}
+
+// VJP of dev_trig: gm [Ds] += d/dm, gs [Ds,Ds] += the symmetric part of d/ds, for cotangents gM, gS, gC (gC may be NULL)
+__device__ __forceinline__ void dev_trig_bwd(const TrigMap& tm, const double* m, const double* s, const double* gM,
+                                             const double* gS, const double* gC, double* gm, double* gs) {
+    const int tid = threadIdx.x, nt = blockDim.x, Ds = tm.Ds;
+    for (int i = tid; i < Ds; i += nt) gm[i] += trig_vjp_m(tm, m, s, gM, gS, gC, i);
+    for (int e = tid; e < Ds * Ds; e += nt) gs[e] += trig_vjp_s(tm, m, s, gM, gS, gC, e / Ds, e % Ds);
     __syncthreads();
 }
 

@@ -405,6 +405,50 @@ def box_risk(prm, m, s, grad=False):
     return (risk, dm, dv) if grad else risk
 
 
+def angles_struct(angle_dims, Ds):
+    """``pilco_angles`` for the angular state dimensions ``angle_dims`` of a state of dimension ``Ds`` (None or empty:
+    no angles -> None).  ValueError for a dimension out of range or repeated."""
+    if angle_dims is None or len(angle_dims) == 0:
+        return None
+    dims = [int(a) for a in angle_dims]
+    if len(set(dims)) != len(dims) or any(a < 0 or a >= Ds for a in dims):
+        raise ValueError("angle_dims %s: expected distinct indices into a state of dimension %d" % (list(angle_dims), Ds))
+    ang = _lib.Angles()
+    ang.A = len(dims)
+    for i, a in enumerate(dims):
+        ang.dims[i] = a
+    return ang
+
+
+def trig_feature_map(x, angle_dims):
+    """phi(x) on the host (numpy, last axis = state): the pass-through dimensions in increasing order, then
+    sin, cos of every angle in ``angle_dims`` order -- the map the device applies to the state Gaussian."""
+    x = np.asarray(x, dtype=np.float64)
+    Ds = x.shape[-1]
+    dims = [int(a) for a in (angle_dims or [])]
+    keep = [j for j in range(Ds) if j not in dims]
+    parts = [x[..., keep]]
+    for a in dims:
+        parts += [np.sin(x[..., a:a + 1]), np.cos(x[..., a:a + 1])]
+    return np.concatenate(parts, axis=-1)
+
+
+def trig_moments(m, s, angle_dims):
+    """pilco_trig_moments: moments of phi(x) for x ~ N(m [R,Ds], s [R,Ds,Ds]) -> M [R,Dh], S [R,Dh,Dh] and
+    C = inv(s) cov(x, phi) [R,Ds,Dh] (Dh = Ds + len(angle_dims))."""
+    m, s = dev(m), dev(s)
+    R, Ds = m.shape
+    ang = angles_struct(angle_dims, Ds)
+    Dh = Ds + (ang.A if ang is not None else 0)
+    d = device()
+    M = torch.empty((R, Dh), dtype=F64, device=d)
+    S = torch.empty((R, Dh, Dh), dtype=F64, device=d)
+    Cx = torch.empty((R, Ds, Dh), dtype=F64, device=d)
+    check(lib.pilco_trig_moments(Ds, R, C.byref(ang) if ang is not None else None, ptr(m), ptr(s), ptr(M), ptr(S),
+                                 ptr(Cx), stream_ptr()), "trig_moments")
+    return M, S, Cx
+
+
 def _max_action(policy_spec, U):
     """the policy spec's max_action (scalar or [U]) as a [U] device tensor"""
     return dev(np.broadcast_to(np.asarray(policy_spec.get("max_action", 1.0), dtype=np.float64).ravel(), (U,)).copy())
@@ -484,13 +528,25 @@ class RolloutPlan:
     pilco.py:130-134; multiplicative ones form the per-step risk of SafePILCO.predict, safe_pilco.py:29-50, and
     enter the returned reward as ``mult_mu * (1 - prod_t (1 - risk_t))``)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False):
+    def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False, angles=None):
         """``grad=True``: the forward cascade runs the TAPED dynamics tile pass (pilco_rollout.tape), so that
-        ``backward()`` needs no recomputation; without it ``backward()`` still works (recomputing path)."""
+        ``backward()`` needs no recomputation; without it ``backward()`` still works (recomputing path).
+
+        ``angles``: angular state dimensions (pilco_rollout_angles_*).  The state dimension is then the dynamics GP's
+        output count E; the policy (``policy_spec["Ds"]``) and the joint state-action terms see phi(x) of dimension
+        Dh = E + len(angles), the dynamics GP [phi(x), u]."""
         d = device()
         self.dyn = dyn
         self.R, self.H = int(R), int(H)
         self.Ds, self.U = policy_spec["Ds"], policy_spec["U"]
+        self.ang = None
+        if angles is not None and len(angles) > 0:
+            self.Ds = int(dyn.struct().E)
+            self.ang = angles_struct(angles, self.Ds)
+            Dh = self.Ds + self.ang.A
+            if int(policy_spec["Ds"]) != Dh:
+                raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
+                                 % (self.ang.A, Dh, int(policy_spec["Ds"])))
         self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
         ro = _lib.Rollout()
         ro.R, ro.H = self.R, self.H
@@ -521,7 +577,8 @@ class RolloutPlan:
         self.info = torch.zeros(self.R, dtype=torch.int32, device=d)
         ro.traj_m, ro.traj_S = self.traj_m.data_ptr(), self.traj_S.data_ptr()
         ro.reward, ro.step_reward, ro.info = self.reward.data_ptr(), self.step_reward.data_ptr(), self.info.data_ptr()
-        wsb = lib.pilco_rollout_workspace_bytes(C.byref(ro))
+        wsb = (lib.pilco_rollout_workspace_bytes(C.byref(ro)) if self.ang is None else
+               lib.pilco_rollout_angles_workspace_bytes(C.byref(ro), C.byref(self.ang)))
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         ro.ws, ro.ws_bytes = self.ws.data_ptr(), wsb
         self.tape = None
@@ -533,7 +590,11 @@ class RolloutPlan:
         self.ro = ro
 
     def forward(self):
-        check(lib.pilco_rollout_forward(C.byref(self.ro), stream_ptr()), "rollout_forward")
+        if self.ang is None:
+            check(lib.pilco_rollout_forward(C.byref(self.ro), stream_ptr()), "rollout_forward")
+        else:
+            check(lib.pilco_rollout_angles_forward(C.byref(self.ro), C.byref(self.ang), stream_ptr()),
+                  "rollout_angles_forward")
         return self.traj_m, self.traj_S, self.reward
 
     # ---- CUDA graph: the whole H-step loop (6H+1 launches forward, ~10H backward) as one graph launch -------
@@ -567,11 +628,16 @@ class RolloutPlan:
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
-            wsb = lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro))
+            wsb = (lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro)) if self.ang is None else
+                   lib.pilco_rollout_angles_bwd_workspace_bytes(C.byref(self.ro), C.byref(self.ang)))
             self.bws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.bws.data_ptr(), wsb
             self.grad = g
-        check(lib.pilco_rollout_backward(C.byref(self.ro), C.byref(self.grad), stream_ptr()), "rollout_backward")
+        if self.ang is None:
+            check(lib.pilco_rollout_backward(C.byref(self.ro), C.byref(self.grad), stream_ptr()), "rollout_backward")
+        else:
+            check(lib.pilco_rollout_angles_backward(C.byref(self.ro), C.byref(self.ang), C.byref(self.grad), stream_ptr()),
+                  "rollout_angles_backward")
         return self.gbuf
 
 
@@ -864,7 +930,8 @@ class PredictPlan:
     moments + reward + status -> pinned host memory.  Built once per (model, policy, reward, n) state by
     ``PILCO`` and replayed for every call with new initial moments (pilco/models/pilco.py:118-136)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0):
+    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0, angles=None):
+        """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``: as RolloutPlan."""
         d = device()
         self.Ds, self.n = int(Ds), int(n)
         Ds = self.Ds
@@ -872,7 +939,8 @@ class PredictPlan:
         self.h_out = torch.zeros(Ds + Ds * Ds + 2, dtype=F64).pin_memory()       # [m | S | reward | info]
         self.d_in = torch.zeros(Ds + Ds * Ds, dtype=F64, device=d)
         self.d_out = torch.zeros(Ds + Ds * Ds + 2, dtype=F64, device=d)
-        self.plan = RolloutPlan(dyn, policy_spec, reward_terms, np.zeros(Ds), np.eye(Ds), self.n, R=1, mult_mu=mult_mu)
+        self.plan = RolloutPlan(dyn, policy_spec, reward_terms, np.zeros(Ds), np.eye(Ds), self.n, R=1, mult_mu=mult_mu,
+                                angles=angles)
         self._enqueue()                                    # eager warm-up (one-time kernel attributes)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()

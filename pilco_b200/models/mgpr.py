@@ -192,6 +192,12 @@ class MGPR:
             self.models[-1]._owner = (self, i)              # predict_f uses this MGPR's factorisation
 
     def set_data(self, data):
+        """``data`` = (X, Y) in the models' input layout.  A PILCO with angle_dims trains its models on [phi(x), u]
+        (set by PILCO as ``_input_width``): raw [x, u] data of another width is a ValueError naming PILCO.set_data."""
+        w = getattr(self, "_input_width", None)
+        if w is not None and np.asarray(data[0]).shape[1] != w:
+            raise ValueError("these models take inputs [phi(x), u] of width %d, got width %d: pass raw (X = [x, u], Y) "
+                             "data to PILCO.set_data, which applies phi" % (w, np.asarray(data[0]).shape[1]))
         for i, model in enumerate(self.models):
             if isinstance(model.data[0], Parameter):
                 model.X.assign(data[0])

@@ -33,20 +33,55 @@ def _sqrt_factor(S):
     return (Q * lam.clamp(min=0.0).sqrt()[None, :]).numpy()
 
 
+def _controller_input_dim(c):
+    if isinstance(c, controllers.RbfController):
+        return int(c.policy_shapes[1])
+    if isinstance(c, controllers.LinearController):
+        return int(np.asarray(c.W).shape[1])
+    return None
+
+
 class PILCO:
     def __init__(self, data, num_induced_points=None, horizon=30, controller=None,
-                 reward=None, m_init=None, S_init=None, name=None):
+                 reward=None, m_init=None, S_init=None, name=None, *, angle_dims=None):
+        """``angle_dims``: angular state dimensions (PILCO's trigonometric augmentation, DESIGN.md section 19).  The
+        policy and the dynamics GPs then see phi(x) = [the other state dimensions, sin and cos of each angle] (Dh =
+        state_dim + len(angle_dims)), while the state, m_init / S_init, the state reward terms and the GP outputs stay
+        raw.  ``data`` stays the raw (X = [x, u], Y = delta x); the angles' deltas in Y must be continuous (unwrapped).
+        The models are trained on [phi(x), u], so ``mgpr.models[e].predict_*`` take such inputs; new raw data goes
+        through ``PILCO.set_data``.  The controller must take Dh inputs and every joint state-action reward term must
+        have state_dim = Dh (ValueError otherwise)."""
         self.name = name
-        if num_induced_points is None:
-            self.mgpr = MGPR(data)
-        else:
-            self.mgpr = SMGPR(data, num_induced_points)
         self.state_dim = data[1].shape[1]
         self.control_dim = data[0].shape[1] - data[1].shape[1]
+        self.angle_dims = None
+        if angle_dims is not None and len(angle_dims) > 0:
+            engine.angles_struct(angle_dims, self.state_dim)            # ValueError: out of range or repeated
+            self.angle_dims = [int(a) for a in angle_dims]
+            if self.policy_input_dim + self.control_dim > _lib.ABI_MAX_D:
+                raise ValueError("angle_dims: state_dim + %d angles + control_dim = %d exceeds %d"
+                                 % (len(self.angle_dims), self.policy_input_dim + self.control_dim, _lib.ABI_MAX_D))
+        gp_data = self._model_data(data)
+        if num_induced_points is None:
+            self.mgpr = MGPR(gp_data)
+        else:
+            self.mgpr = SMGPR(gp_data, num_induced_points)
+        if self.angle_dims is not None:
+            self.mgpr._input_width = self.policy_input_dim + self.control_dim
         self.horizon = horizon
         self.controller = controller if controller is not None else \
-            controllers.LinearController(self.state_dim, self.control_dim)
+            controllers.LinearController(self.policy_input_dim, self.control_dim)
         self.reward = reward if reward is not None else rewards.ExponentialReward(self.state_dim)
+        if self.angle_dims is not None:
+            Dh = self.policy_input_dim
+            cin = _controller_input_dim(self.controller)
+            if cin is not None and cin != Dh:
+                raise ValueError("with angle_dims=%s the controller must take Dh = %d inputs (phi(x)), it takes %d"
+                                 % (self.angle_dims, Dh, cin))
+            for k, t in enumerate(self.reward.terms()):
+                if t["kind"] in _lib.JOINT_REWARDS and int(t.get("state_dim", -1)) != Dh:
+                    raise ValueError("with angle_dims=%s reward term %d on the joint [phi(x), u] needs state_dim = Dh = "
+                                     "%d, got %s" % (self.angle_dims, k, Dh, t.get("state_dim")))
         if m_init is None or S_init is None:
             # first state of the data set, pilco.py:36-41
             self.m_init = data[0][0:1, 0:self.state_dim]
@@ -55,6 +90,29 @@ class PILCO:
             self.m_init = m_init
             self.S_init = S_init
         self.optimizer = None
+
+    # ---- angular state dimensions ------------------------------------------------------------------
+    @property
+    def policy_input_dim(self):
+        """Dh: the dimension of what the policy and the dynamics GPs see of the state (state_dim without angles)"""
+        return self.state_dim + (len(self.angle_dims) if self.angle_dims else 0)
+
+    def _model_data(self, data):
+        """raw (X = [x, u], Y) -> the dynamics GPs' data ([phi(x), u], Y)"""
+        if not self.angle_dims:
+            return data
+        X = np.asarray(data[0], dtype=np.float64)
+        Ds = self.state_dim
+        return (np.hstack([engine.trig_feature_map(X[:, :Ds], self.angle_dims), X[:, Ds:]]), data[1])
+
+    def set_data(self, data):
+        """New raw data (X = [x, u], Y = delta x) for the dynamics GPs; with angle_dims, phi is applied to x."""
+        self.mgpr.set_data(self._model_data(data))
+
+    def _no_angles(self, what):
+        if self.angle_dims:
+            raise ValueError("%s: the particle rollouts do not support angle_dims yet; use the moment-matching methods "
+                             "(predict, policy_gradient, optimize_policy)" % what)
 
     # ---- parameters ------------------------------------------------------------------------------
     @property
@@ -93,7 +151,7 @@ class PILCO:
         terms, mult_mu = self.reward_spec()
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(flats), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1),
-                                  np.asarray(s_x, dtype=np.float64), int(n), R=R, mult_mu=mult_mu)
+                                  np.asarray(s_x, dtype=np.float64), int(n), R=R, mult_mu=mult_mu, angles=self.angle_dims)
 
     def _reward_key(self):
         terms, mult_mu = self.reward_spec()
@@ -114,7 +172,8 @@ class PILCO:
         hit = cache.get(int(n))
         if hit is None or hit[0] != key:
             terms, mult_mu = self.reward_spec()
-            plan = engine.PredictPlan(dyn, self.policy_spec(), terms, self.state_dim, int(n), mult_mu=mult_mu)
+            plan = engine.PredictPlan(dyn, self.policy_spec(), terms, self.state_dim, int(n), mult_mu=mult_mu,
+                                      angles=self.angle_dims)
             if len(cache) >= 8:
                 cache.clear()
             cache[int(n)] = hit = (key, plan)
@@ -150,6 +209,7 @@ class PILCO:
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
         from ..params import HostArray
+        self._no_angles("sample_trajectories")
         if consistent:
             import torch
             dyn = self.mgpr.device_gp()
@@ -228,6 +288,7 @@ class PILCO:
 
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
+        self._no_angles("sample_policy_gradient")
         if estimator not in engine.ParticlePlan.ESTIMATORS:
             raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
                              % (engine.ParticlePlan.ESTIMATORS, estimator))
@@ -251,7 +312,7 @@ class PILCO:
         terms, mult_mu = self.reward_spec()
         plan = engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
-                                  int(n), R=1, mult_mu=mult_mu, grad=True)
+                                  int(n), R=1, mult_mu=mult_mu, grad=True, angles=self.angle_dims)
         plan.forward()
         g = plan.backward()
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
@@ -276,6 +337,7 @@ class PILCO:
         needs more than half the free device memory is a ValueError naming the num_samples that would fit."""
         from functools import partial
         from .. import policy_opt
+        self._no_angles("optimize_policy_sampled")
         if int(num_samples) < 1:
             raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
         terms, _ = self.reward_spec()
@@ -312,12 +374,14 @@ class PILCO:
     def compute_action(self, x_m):
         """pilco.py:115-116: the policy mean at a deterministic state (s = 0).  Served by a cached
         ``engine.ActionPlan`` (one captured CUDA graph per policy state) -- the per-control-step call of
-        examples/utils.py:32-36."""
+        examples/utils.py:32-36.  With angle_dims, x_m is the raw state and phi(x_m) is formed on the host."""
         from ..params import HostArray
         key = self.controller.state_key()
         if key != getattr(self, "_act_key", None):
             self._act_plan = engine.ActionPlan(self.policy_spec())
             self._act_key = key
+        if self.angle_dims:
+            x_m = engine.trig_feature_map(np.asarray(x_m, dtype=np.float64).reshape(1, self.state_dim), self.angle_dims)
         return self._act_plan(x_m).view(HostArray)
 
     # ---- model training (pilco.py:52-73) ------------------------------------------------------------

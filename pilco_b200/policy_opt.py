@@ -171,7 +171,8 @@ class PolicyEvaluator(_FlatEvaluator):
             self.gps.append(None if self.linear else spec["gp"])
             self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
                                                  np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
-                                                 mult_mu=mult_mu, grad=True))
+                                                 mult_mu=mult_mu, grad=True,
+                                                 angles=getattr(pilco, "angle_dims", None)))
         self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
         self._setup_io()
 
