@@ -476,6 +476,36 @@ size_t pilco_particles_score_grad_workspace_bytes(const pilco_particles* pr, int
 int    pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                           pilco_stream_t stream);
 
+/* The particle rollouts with angular state dimensions (pilco_angles above; DESIGN.md section 20).  Each call below is
+ * the call of the same name without "_angles" with the feature map phi at every particle:
+ *   u_t = squash(pi(phi(x_t))),  x~_t = [phi(x_t), u_t],  x_{t+1} = x_t + mu(x~_t) + sqrt(max(var(x~_t), 0)) o eps_t
+ * (the consistent sampler conditions on the particle's earlier x~, which hold phi).  With E = dyn.E the raw state
+ * dimension and A = ang->A: pol.Ds = Dh = E + A and dyn.D = Dh + U.  x0 [P,E], eps [P,H,E], traj [..,H+1,E] and the
+ * GP's outputs (deltas of x, angles unwrapped) stay raw; the state reward terms (EXP, LINEAR, BOX; W, t and the box's
+ * indices in E) are evaluated at the raw x_t, the joint terms (*_SA, D = Dh + U) at x~_t, so a periodic target such as
+ * "pendulum up" is an EXP_SA term on (sin, cos) = (0, -1).  Policy gradients are in the policy's Dh layout.  sin and
+ * cos are evaluated once per particle and step, and the reverse sweep reuses those values.
+ * The workspaces are those of the calls without angles at the same description, plus, for the three gradients, the
+ * phi history [R P,H+1,Dh] (the forward-only ones do not grow with H).  Every call with ang == NULL or ang->A == 0 is
+ * the call without angles.  Validation before anything is enqueued: PILCO_ERR_DIM for a repeated or out-of-range
+ * dimension, A > E, pol.Ds != E + A, dyn.D != pol.Ds + U, dyn.D > PILCO_MAX_D or an RBF policy with rbf.D != Dh;
+ * otherwise the status codes of the call without angles (a workspace query returns 0 where its call would fail on
+ * these).  batch_grad at R = 1 with an unbatched policy is the single-policy pathwise gradient. */
+size_t pilco_particles_angles_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang);
+int    pilco_particles_angles_rollout(const pilco_particles* pr, const pilco_angles* ang, pilco_stream_t stream);
+size_t pilco_particles_angles_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang);
+int    pilco_particles_angles_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                 pilco_stream_t stream);
+size_t pilco_particles_angles_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R);
+int    pilco_particles_angles_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                                 const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_angles_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R);
+int    pilco_particles_angles_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                                      const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_angles_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R);
+int    pilco_particles_angles_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                                 const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -148,6 +148,22 @@ SIGNATURES = {
                                                           c_dp]),
     "pilco_particles_score_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.c_int]),
     "pilco_particles_rollout_score_grad": (C.c_int, [C.POINTER(Particles), C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_angles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Angles)]),
+    "pilco_particles_angles_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), c_dp]),
+    "pilco_particles_angles_consistent_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Angles)]),
+    "pilco_particles_angles_consistent_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), c_dp]),
+    "pilco_particles_angles_batch_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Angles),
+                                                                       C.c_int]),
+    "pilco_particles_angles_batch_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int,
+                                                            C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_angles_consistent_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Angles),
+                                                                            C.c_int]),
+    "pilco_particles_angles_consistent_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int,
+                                                                 C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_angles_score_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Angles),
+                                                                       C.c_int]),
+    "pilco_particles_angles_score_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int,
+                                                            C.POINTER(ParticlesGrad), c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),
     "pilco_mm_forward_taped_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,

@@ -21,60 +21,10 @@
 // reward and risk after pt_step<t>, pj_grad_kernel adds their gradients to the VJP output x~_bar_t before pg_step<t> /
 // ps_zbar.  The state kernels see the state terms only (pt_policy), so they are untouched: pt_step_kernel and
 // pg_step_kernel sit at their register limits (127 and 255), and the joint terms would have spilled them.
-#include <initializer_list>
-#include "common.cuh"
-#include "risk_math.cuh"
-
-#define PT_THREADS 128
-#define PT_MAX_P   (65535 * 32)         // pilco_gp_predict's T limit
-#define PT_RBF_VAR 1e-6                 // output variance of the deterministic-GP policy (mode 1, mm_finish_device)
-#define PT_INV_PI  0.31830988618379067154
-
-// the policy and the rewards, as every per-particle kernel reads them (pt_policy)
-struct PtPolicy {
-    int P, H, Ds, U;
-    int pol_kind, squash;
-    const double* maxa;
-    const double* W; const double* b;                   // linear policy [U,Ds], [U]
-    const double* C; const double* ell; const double* sf2; const double* beta; int bf;   // RBF policy (bf = 0: linear)
-    long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;   // per-restart policy strides (0: shared)
-    int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
-};
-
-struct PtDev : PtPolicy {
-    int t;
-    const double* x0; const double* eps;                // [P,Ds], [P,H,Ds]: shared by the restarts
-    double* traj; double* act; double* step_reward; double* step_risk; double* ret;   // rows r P + p
-    double* xt;                                         // predict input [R P,D]
-    const double* mean; const double* var;              // predict outputs [R P,Ds]
-};
-
-// one reward term at the point x (registers; xg = the same point in global memory, for the box's indexed reads):
-// the closed forms of small_kernels.cuh at s = 0
-__device__ __forceinline__ double pt_reward_value(const pilco_reward_term& rt, const double (&x)[MAXD], const double* xg,
-                                                  int Ds) {
-    if (rt.kind == PILCO_REWARD_BOX) return risk_box_point(rt.W, xg);
-    if (rt.kind == PILCO_REWARD_LINEAR) {
-        double mu = 0.0;
-#pragma unroll
-        for (int i = 0; i < MAXD; ++i) if (i < Ds) mu = fma(x[i], rt.W[i], mu);
-        return mu;
-    }
-    double v[MAXD];                                     // exp(-0.5 (x-t)' W (x-t)), dev_exp_reward's order
-#pragma unroll
-    for (int i = 0; i < MAXD; ++i) v[i] = i < Ds ? x[i] - rt.t[i] : 0.0;
-    double quad = 0.0;
-#pragma unroll
-    for (int i = 0; i < MAXD; ++i) {
-        if (i < Ds) {
-            double wy = 0.0;
-#pragma unroll
-            for (int k = 0; k < MAXD; ++k) if (k < Ds) wy = fma(rt.W[i * Ds + k], v[k], wy);
-            quad = fma(v[i], wy, quad);
-        }
-    }
-    return exp(-0.5 * quad);
-}
+// Angular state dimensions (pilco_particles_angles_*, DESIGN.md section 20): pt_forward, pg_reverse and ps_run take the
+// angles' map and launch the step kernels of particles_angles.cu in place of pt_step / pg_step; the shared structs are
+// in particles.cuh.
+#include "particles.cuh"
 
 // grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y
 __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
@@ -252,15 +202,7 @@ __global__ void __launch_bounds__(PT_THREADS) pj_grad_kernel(PjDev a) {
 // a_kt = coef_k (ADD) or coef_k mult_mu prod_{s != t} (1 - risk_s) (MULT).  x_H carries no reward, so the sweep
 // starts at t = H-1 with x_bar_H = 0 and x~_bar_{H-1} = 0: H-1 VJP calls.  With joint terms pj_grad_kernel has added
 // sum_k a_kt grad v_k(x~_t) to x~_bar_t beforehand (at t = H-1 to a zeroed one, which this kernel then reads).
-struct PgDev : PtPolicy {
-    int t;
-    const double* eps; const double* traj; const double* step_risk;
-    const double* gxt;          // VJP of step t at x~_t [R P,D]; NULL at t = H-1
-    const double* var_prev;     // var_{t-1} [R P,Ds] (t > 0)
-    double* gx;                 // [R P,Ds] x_bar_{t+1} in, x_bar_t out (= the gmean of step t-1's VJP)
-    double* gvar;               // [R P,Ds] the gvar of step t-1's VJP
-    double* zbar;               // [R P,H,U]
-};
+// Its arguments: PgDev (particles.cuh).
 
 // grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y: step t of the reverse sweep
 __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
@@ -821,6 +763,7 @@ struct PtWs {
     size_t gx, gvar, gxt, zbar, s1, s2r, gbeta, gy;     // reverse sweep and the policy-parameter reduction
     size_t G, dir;                                      // reverse of the conditioning (score: G = the return-to-go)
     size_t gsum;                                        // score: the per-(restart, step) sums of G
+    size_t phi;                                         // angles, gradients: phi(x_t) [T,H+1,Dh]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -846,7 +789,7 @@ static bool pt_has_joint(const pilco_particles* pr) {
 
 // the marginal rollout: x~, the predict outputs and one predict workspace at T = P
 static PtWs pt_ws_layout(const pilco_particles* pr) {
-    const size_t P = pr->P, Ds = pr->pol.Ds, D = pr->dyn.D;
+    const size_t P = pr->P, Ds = pr->dyn.E, D = pr->dyn.D;
     PtWs L = {}; PtTake take;
     L.xt = take({P, D}); L.mean = take({P, Ds}); L.var = take({P, Ds});
     L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
@@ -858,19 +801,21 @@ static PtWs pt_ws_layout(const pilco_particles* pr) {
 // the gradient for R restarts: the forward's predict inputs and variances of EVERY step (the reverse sweep needs
 // them), the state cotangent, the VJP's cotangents and output, z_bar of every point, the RBF sums, and one predict /
 // VJP workspace at T = R P (never in use at the same time).  Rows are restart-major (row r P + p); nothing of size
-// [., n] is kept.
-static PtWs pg_ws_layout(const pilco_particles* pr, int R) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+// [., n] is kept.  State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles);
+// angles: the phi history [T,H+1,Dh] after everything else.
+static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
     L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
     L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
     L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
     const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
     const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
     L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
+    if (angles) L.phi = take({T, H + 1, Dh});
     L.total = L.pws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -879,7 +824,7 @@ static PtWs pg_ws_layout(const pilco_particles* pr, int R) {
 // mean and var [T,Ds], W_t [E,T,np], the K* history [H,E,T,np], the packed factor rows [H(H+1)/2,E,T], one predict
 // workspace at T
 static void fs_take(const pilco_particles* pr, size_t T, PtWs& L, PtTake& take) {
-    const size_t H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
+    const size_t H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
     L.xt = take({H, T, D}); L.mu = take({T, Ds}); L.s2 = take({T, Ds}); L.mean = take({T, Ds}); L.var = take({T, Ds});
     L.W = take({T, Ds, np}); L.Kh = take({H, T, Ds, np}); L.L = take({H * (H + 1) / 2, T, Ds});
     L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
@@ -896,18 +841,19 @@ static PtWs fs_ws_layout(const pilco_particles* pr) {
 // the consistent gradient for R restarts: the consistent forward's at T = R P (its W slot holds a_t in the reverse
 // sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
 // [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
-// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T
-static PtWs fg_ws_layout(const pilco_particles* pr, int R) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
+// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, as pg_ws_layout)
+static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
     fs_take(pr, T, L, take);                            // pt_batch_ok: R P <= PT_MAX_P
     L.var = take({H, T, Ds}); L.G = take({H * (H + 1) / 2, T, Ds}); L.dir = take({T, Ds, D});
     L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
     L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
     L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
     L.vws = take({L.vws_bytes / sizeof(double)});
+    if (angles) L.phi = take({T, H + 1, Dh});
     L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -921,9 +867,9 @@ static int ps_group(long long T, int H) {
 // the score gradient for R restarts: pg_ws_layout's forward part (x~ [H,T,D], mean [T,Ds], var [H,T,Ds]), then G
 // [H-1,T], the sums [R,H], gmean and gvar [H-1,T,Ds], the VJP output [H-1,T,D], z_bar [T,H,U], the RBF sums
 // [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one predict / VJP workspace for the predict at T and the largest VJP group.
-// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.
-static PtWs ps_ws_layout(const pilco_particles* pr, int R) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Ds = pr->pol.Ds, U = pr->pol.U;
+// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.  Angles: then the phi history, as pg_ws_layout.
+static PtWs ps_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+    const size_t T = (size_t)R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U;
     const size_t D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
     L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
@@ -931,13 +877,14 @@ static PtWs ps_ws_layout(const pilco_particles* pr, int R) {
     L.gx = take({Hm, T, Ds}); L.gvar = take({Hm, T, Ds});
     L.gxt = take({pt_has_joint(pr) ? H : Hm, T, D});    // joint terms: step H-1 too, for their direct term
     L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Ds}); L.s2r = take({(size_t)R, U, bf, Ds});
+    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
     L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
     const int grp = ps_group((long long)T, (int)H);
     const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
     const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T * (grp > 1 ? grp : 1));
     L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
+    if (angles) L.phi = take({T, H + 1, Dh});
     const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
     L.total = L.pws_bytes && nb * H <= 0x7fffffff ? take.bytes() : 0;
     return L;
@@ -954,8 +901,9 @@ static bool pt_batch_ok(int P, int R) {
 }
 
 // everything but the workspace (the gradients bring their own).  batched: the policy's batch strides are honoured
-// (the batch_grad and consistent_grad entry points); otherwise a batched policy is unsupported.
-static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
+// (the batch_grad and consistent_grad entry points); otherwise a batched policy is unsupported.  A: the number of
+// angular state dimensions (the policy takes dyn.E + A inputs).
+static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A = 0) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
     const pilco_gp_model& g = pr->dyn;
@@ -964,7 +912,7 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false) {
     if (g.n < 1 || g.D < 1 || g.D > MAXD || g.E < 1 || g.E > MAXE || g.ldk < pad64(g.n)) return PILCO_ERR_DIM;
     const pilco_policy& pol = pr->pol;
     const int Ds = pol.Ds, U = pol.U;
-    if (Ds < 1 || U < 1 || Ds + U != g.D || g.E != Ds) return PILCO_ERR_DIM;
+    if (Ds < 1 || U < 1 || Ds + U != g.D || g.E + A != Ds) return PILCO_ERR_DIM;
     auto strides = [batched](std::initializer_list<long long> bs) {
         for (long long b : bs) {
             if (b && !batched) return PILCO_ERR_UNSUPPORTED;
@@ -1056,10 +1004,11 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 //   pt_step<0>, predict<0>, [fs_cond<0>,] pt_step<1>, ..., pt_step<H>
 // consistent: the predict is fs_predict_kernel and fs_cond_kernel leaves the step closure (mean, var) that
 // pt_step_kernel reads unchanged.  history: var of every step is kept (the reverse sweep needs it); x~ of every step is
-// kept when either needs it.
+// kept when either needs it.  tm (angles, DESIGN.md section 20): pa_step_kernel in place of pt_step_kernel, which with
+// history also keeps phi(x_t) in L.phi.  The state width is dyn.E throughout (pol.Ds without angles).
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
-                      cudaStream_t st) {
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
+                      cudaStream_t st, const TrigMap* tm = nullptr) {
+    const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
     const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
@@ -1068,6 +1017,8 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     a.x0 = pr->x0; a.eps = pr->eps;
     a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
     a.mean = ws + L.mean;
+    PaStep pa;
+    if (tm) { pa.E = Ds; pa.tm = *tm; pa.phi = history ? ws + L.phi : nullptr; }
     FsCond c;
     c.P = P; c.T = T; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = np; c.t = 0;
     c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
@@ -1079,8 +1030,13 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
         a.t = t;
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
         a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
-        launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
+        if (tm) {
+            static_cast<PtDev&>(pa) = a;
+            if (const int rc = pa_step_launch(st, grid, pa)) return rc;
+        } else {
+            launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+            CUDA_LAUNCH_CHECK();
+        }
         if (t == H) break;
         if (joint) {
             j.t = t; j.xh = a.xt;
@@ -1110,14 +1066,15 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
                           const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
 
-// value and the policy-parameter gradient over all P H points of each restart, fixed order, from z_bar [R P,H,U]
+// value and the policy-parameter gradient over all P H points of each restart, fixed order, from z_bar [R P,H,U] and
+// the policy inputs pin [R P,H+1,Ds] (pr->traj, or with angles the phi history)
 static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_grad* g, double* ws, const PtWs& L,
-                     cudaStream_t st) {
+                     cudaStream_t st, const double* pin) {
     PgRed r;
     static_cast<PtPolicy&>(r) = pt_policy(pr);
     const bool rbf = r.pol_kind == PILCO_POLICY_RBF;
     const int Ds = r.Ds, U = r.U, bf = r.bf;
-    r.traj = pr->traj; r.zbar = ws + L.zbar; r.ret = pr->ret;
+    r.traj = pin; r.zbar = ws + L.zbar; r.ret = pr->ret;
     r.gW = g->gW; r.gb = g->gb;
     r.s1 = ws + L.s1; r.s2 = ws + L.s2r; r.gbeta = ws + L.gbeta;
     r.gXc = g->gXc; r.gell = g->gell;
@@ -1140,10 +1097,11 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // The reverse sweep after pt_forward(history) and the reduction (DESIGN.md sections 12, 15):
 //   pg_step<H-1>, [VJP<t>, pg_step<t>] for t = H-2 .. 0, then pg_reduce's launches
 // The step's VJP is pilco_gp_predict_vjp, or (consistent) fs_cond_bwd_kernel followed by fs_predict_vjp_kernel.
+// tm (angles): pa_reverse_launch's two kernels in place of pg_step, and the policy reduction over the phi history.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
-                      cudaStream_t st) {
+                      cudaStream_t st, const TrigMap* tm = nullptr) {
     double* ws = (double*)g->ws;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P;
+    const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
     const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
     if (consistent && H > 1) cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TDs * sizeof(double), st);
@@ -1186,51 +1144,63 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             CUDA_LAUNCH_CHECK();
         }
         b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * TDs : nullptr;
-        launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
-        CUDA_LAUNCH_CHECK();
+        if (tm) {
+            PaBwd ab;
+            static_cast<PgDev&>(ab) = b;
+            ab.E = Ds; ab.tm = *tm; ab.phi = ws + L.phi; ab.phib = b.gxt ? ws + L.gxt : nullptr;
+            if (const int rc = pa_reverse_launch(st, grid, ab)) return rc;
+        } else {
+            launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
+            CUDA_LAUNCH_CHECK();
+        }
     }
-    return pg_reduce(pr, R, g, ws, L, st);
+    return pg_reduce(pr, R, g, ws, L, st, tm ? ws + L.phi : pr->traj);
 }
 
 // the validated gradient of R restarts: the forward with its history, then the reverse sweep
 static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool consistent,
-                  pilco_stream_t stream) {
-    const PtWs L = consistent ? fg_ws_layout(pr, R) : pg_ws_layout(pr, R);
+                  pilco_stream_t stream, const TrigMap* tm = nullptr) {
+    const PtWs L = consistent ? fg_ws_layout(pr, R, tm != nullptr) : pg_ws_layout(pr, R, tm != nullptr);
     if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
     if (consistent) {
         if (const int rc = fs_predict_prepare()) return rc;
         if (const int rc = fs_vjp_prepare()) return rc;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st)) return rc;
-    return pg_reverse(pr, R, g, L, consistent, st);
+    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st, tm)) return rc;
+    return pg_reverse(pr, R, g, L, consistent, st, tm);
 }
 
-// the forward alone, R = 1
-static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream) {
-    if (const int rc = pt_check_desc(pr)) return rc;
+// the forward alone, R = 1 (tm: validated angles; the description is checked here)
+static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream, const TrigMap* tm = nullptr) {
+    if (const int rc = pt_check_desc(pr, false, tm ? tm->A : 0)) return rc;
     const PtWs L = consistent ? fs_ws_layout(pr) : pt_ws_layout(pr);
     if (const int rc = pt_check_ws(pr->ws, pr->ws_bytes, L.total)) return rc;
     if (consistent)
         if (const int rc = fs_predict_prepare()) return rc;
-    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream);
+    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream, tm);
 }
 
 // The score-function gradient of R restarts (validated; DESIGN.md section 16):
 //   pt_forward(history), ps_togo, ps_base, ps_cot, VJP of steps 0..H-2 in groups of whole steps, ps_zbar, pg_reduce
 // The x~ history [H-1,T,D] and the cotangents [H-1,T,Ds] are contiguous, so a group of k steps is one VJP call at k T
 // rows; a point's VJP does not depend on T or on its row, so the grouping changes no bit.
-static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
-    const PtWs L = ps_ws_layout(pr, R);
+// tm (angles): the state-width cotangents are in E (ps_cot at Ds = E); ps_zbar and the reduction read the policy
+// inputs from the phi history (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.
+static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream,
+                  const TrigMap* tm = nullptr) {
+    const PtWs L = ps_ws_layout(pr, R, tm != nullptr);
     if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     double* ws = (double*)g->ws;
-    if (const int rc = pt_forward(pr, R, ws, L, false, true, st)) return rc;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, D = pr->dyn.D, T = R * P, nb = (P + PT_THREADS - 1) / PT_THREADS;
+    if (const int rc = pt_forward(pr, R, ws, L, false, true, st, tm)) return rc;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
+    const int nb = (P + PT_THREADS - 1) / PT_THREADS;
+    const double* pin = tm ? ws + L.phi : pr->traj;
     PsDev a;
     static_cast<PtPolicy&>(a) = pt_policy(pr);
     a.T = T;
-    a.eps = pr->eps; a.traj = pr->traj; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
+    a.eps = pr->eps; a.traj = pin; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
     a.var = ws + L.var; a.G = ws + L.G; a.S = ws + L.gsum; a.gmean = ws + L.gx; a.gvar = ws + L.gvar;
     a.gxt = ws + L.gxt; a.zbar = ws + L.zbar;
     a.direct = pt_has_joint(pr);
@@ -1239,14 +1209,16 @@ static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
         CUDA_LAUNCH_CHECK();
         launch_hi(ps_base_kernel, dim3(H - 1, R), dim3(256), 0, st, a);
         CUDA_LAUNCH_CHECK();
-        launch_hi(ps_cot_kernel, dim3(nb * (H - 1), R), dim3(PT_THREADS), 0, st, a);
+        PsDev ac = a;
+        ac.Ds = E;
+        launch_hi(ps_cot_kernel, dim3(nb * (H - 1), R), dim3(PT_THREADS), 0, st, ac);
         CUDA_LAUNCH_CHECK();
         const int grp = ps_group(T, H);
         for (int t0 = 0; t0 < H - 1; t0 += grp) {
             const int k = grp < H - 1 - t0 ? grp : H - 1 - t0;
             const size_t o = (size_t)t0 * T;
-            const int rc = pilco_gp_predict_vjp(&pr->dyn, k * T, ws + L.xt + o * D, ws + L.gx + o * Ds,
-                                                ws + L.gvar + o * Ds, ws + L.gxt + o * D, ws + L.vws, L.vws_bytes, st);
+            const int rc = pilco_gp_predict_vjp(&pr->dyn, k * T, ws + L.xt + o * D, ws + L.gx + o * E,
+                                                ws + L.gvar + o * E, ws + L.gxt + o * D, ws + L.vws, L.vws_bytes, st);
             if (rc) return rc;
         }
     }
@@ -1262,20 +1234,40 @@ static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
         launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
     }
-    return pg_reduce(pr, R, g, ws, L, st);
+    return pg_reduce(pr, R, g, ws, L, st, pin);
 }
 
 // everything a gradient entry point checks before its workspace: batched honours the policy's batch strides
-static int pg_validate(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched) {
-    if (const int rc = pt_check_desc(pr, batched)) return rc;
+static int pg_validate(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, int A = 0) {
+    if (const int rc = pt_check_desc(pr, batched, A)) return rc;
     if (batched && !pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
     return pg_check(pr, g);
 }
 
 static int pg_entry(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, bool consistent,
-                    pilco_stream_t stream) {
-    if (const int rc = pg_validate(pr, R, g, batched)) return rc;
-    return pg_run(pr, R, g, consistent, stream);
+                    pilco_stream_t stream, const TrigMap* tm = nullptr) {
+    if (const int rc = pg_validate(pr, R, g, batched, tm ? tm->A : 0)) return rc;
+    return pg_run(pr, R, g, consistent, stream, tm);
+}
+
+// ---- angular state dimensions (DESIGN.md section 20) ----------------------------------------------------------------
+// The map of A >= 1 angles of the raw state (dyn.E dimensions) and the widths that go with it: PILCO_ERR_DIM for a
+// repeated or out-of-range dimension, A > E, pol.Ds != E + A, dyn.D != pol.Ds + U, dyn.D > PILCO_MAX_D or an RBF
+// policy whose input width is not pol.Ds.  pr is not NULL.
+static int pa_map(const pilco_particles* pr, const pilco_angles* ang, TrigMap* tm) {
+    const int E = pr->dyn.E, Dh = pr->pol.Ds;
+    if (trig_map_make(E, ang->A, ang->dims, tm)) return PILCO_ERR_DIM;
+    if (Dh != E + ang->A || pr->dyn.D != Dh + pr->pol.U || pr->dyn.D > MAXD) return PILCO_ERR_DIM;
+    if (pr->pol.kind == PILCO_POLICY_RBF && pr->pol.rbf.D != Dh) return PILCO_ERR_DIM;
+    return PILCO_OK;
+}
+
+static bool pa_none(const pilco_angles* ang) { return !ang || ang->A == 0; }
+
+// an angle twin's workspace: its layout with the angles' map valid, 0 otherwise
+static bool pa_sizes_ok(const pilco_particles* pr, const pilco_angles* ang) {
+    TrigMap tm;
+    return pr && pt_sizes_ok(pr) && pa_map(pr, ang, &tm) == PILCO_OK;
 }
 
 extern "C" {
@@ -1330,6 +1322,78 @@ int pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const p
                                        pilco_stream_t stream) {
     if (const int rc = pg_validate(pr, R, g, true)) return rc;
     return ps_run(pr, R, g, stream);
+}
+
+// ---- the angle twins: ang == NULL or A == 0 is the call without angles ----------------------------------------------
+size_t pilco_particles_angles_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang) {
+    if (pa_none(ang)) return pilco_particles_workspace_bytes(pr);
+    return pa_sizes_ok(pr, ang) ? pt_ws_layout(pr).total : 0;
+}
+
+int pilco_particles_angles_rollout(const pilco_particles* pr, const pilco_angles* ang, pilco_stream_t stream) {
+    if (pa_none(ang)) return pilco_particles_rollout(pr, stream);
+    if (!pr) return PILCO_ERR_NULL;
+    TrigMap tm;
+    if (const int rc = pa_map(pr, ang, &tm)) return rc;
+    return pt_run(pr, false, stream, &tm);
+}
+
+size_t pilco_particles_angles_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang) {
+    if (pa_none(ang)) return pilco_particles_consistent_workspace_bytes(pr);
+    return pa_sizes_ok(pr, ang) ? fs_ws_layout(pr).total : 0;
+}
+
+int pilco_particles_angles_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                              pilco_stream_t stream) {
+    if (pa_none(ang)) return pilco_particles_rollout_consistent(pr, stream);
+    if (!pr) return PILCO_ERR_NULL;
+    TrigMap tm;
+    if (const int rc = pa_map(pr, ang, &tm)) return rc;
+    return pt_run(pr, true, stream, &tm);
+}
+
+size_t pilco_particles_angles_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R) {
+    if (pa_none(ang)) return pilco_particles_batch_grad_workspace_bytes(pr, R);
+    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R, true).total : 0;
+}
+
+int pilco_particles_angles_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                              const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (pa_none(ang)) return pilco_particles_rollout_batch_grad(pr, R, g, stream);
+    if (!pr) return PILCO_ERR_NULL;
+    TrigMap tm;
+    if (const int rc = pa_map(pr, ang, &tm)) return rc;
+    return pg_entry(pr, R, g, true, false, stream, &tm);
+}
+
+size_t pilco_particles_angles_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                              int R) {
+    if (pa_none(ang)) return pilco_particles_consistent_grad_workspace_bytes(pr, R);
+    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R, true).total : 0;
+}
+
+int pilco_particles_angles_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                                   const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (pa_none(ang)) return pilco_particles_rollout_consistent_grad(pr, R, g, stream);
+    if (!pr) return PILCO_ERR_NULL;
+    TrigMap tm;
+    if (const int rc = pa_map(pr, ang, &tm)) return rc;
+    return pg_entry(pr, R, g, true, true, stream, &tm);
+}
+
+size_t pilco_particles_angles_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R) {
+    if (pa_none(ang)) return pilco_particles_score_grad_workspace_bytes(pr, R);
+    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R, true).total : 0;
+}
+
+int pilco_particles_angles_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
+                                              const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (pa_none(ang)) return pilco_particles_rollout_score_grad(pr, R, g, stream);
+    if (!pr) return PILCO_ERR_NULL;
+    TrigMap tm;
+    if (const int rc = pa_map(pr, ang, &tm)) return rc;
+    if (const int rc = pg_validate(pr, R, g, true, tm.A)) return rc;
+    return ps_run(pr, R, g, stream, &tm);
 }
 
 }  // extern "C"

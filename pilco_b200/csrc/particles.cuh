@@ -1,0 +1,90 @@
+// particles.cuh -- what the particle kernels of particles.cu and particles_angles.cu share: the per-particle argument
+// structs, the reward value at a point, and the angle kernels' launchers (DESIGN.md sections 11, 12 and 20).
+#pragma once
+#include <initializer_list>
+#include "common.cuh"
+#include "risk_math.cuh"
+#include "trig_math.cuh"
+
+#define PT_THREADS 128
+#define PT_MAX_P   (65535 * 32)         // pilco_gp_predict's T limit
+#define PT_RBF_VAR 1e-6                 // output variance of the deterministic-GP policy (mode 1, mm_finish_device)
+#define PT_INV_PI  0.31830988618379067154
+
+// the policy and the rewards, as every per-particle kernel reads them (pt_policy)
+struct PtPolicy {
+    int P, H, Ds, U;
+    int pol_kind, squash;
+    const double* maxa;
+    const double* W; const double* b;                   // linear policy [U,Ds], [U]
+    const double* C; const double* ell; const double* sf2; const double* beta; int bf;   // RBF policy (bf = 0: linear)
+    long long W_bs, b_bs, C_bs, ell_bs, sf2_bs, beta_bs;   // per-restart policy strides (0: shared)
+    int n_rewards, n_mult; pilco_reward_term rewards[8]; double mult_mu;
+};
+
+struct PtDev : PtPolicy {
+    int t;
+    const double* x0; const double* eps;                // [P,Ds], [P,H,Ds]: shared by the restarts
+    double* traj; double* act; double* step_reward; double* step_risk; double* ret;   // rows r P + p
+    double* xt;                                         // predict input [R P,D]
+    const double* mean; const double* var;              // predict outputs [R P,Ds]
+};
+
+// one reward term at the point x (registers; xg = the same point in global memory, for the box's indexed reads):
+// the closed forms of small_kernels.cuh at s = 0
+__device__ __forceinline__ double pt_reward_value(const pilco_reward_term& rt, const double (&x)[MAXD], const double* xg,
+                                                  int Ds) {
+    if (rt.kind == PILCO_REWARD_BOX) return risk_box_point(rt.W, xg);
+    if (rt.kind == PILCO_REWARD_LINEAR) {
+        double mu = 0.0;
+#pragma unroll
+        for (int i = 0; i < MAXD; ++i) if (i < Ds) mu = fma(x[i], rt.W[i], mu);
+        return mu;
+    }
+    double v[MAXD];                                     // exp(-0.5 (x-t)' W (x-t)), dev_exp_reward's order
+#pragma unroll
+    for (int i = 0; i < MAXD; ++i) v[i] = i < Ds ? x[i] - rt.t[i] : 0.0;
+    double quad = 0.0;
+#pragma unroll
+    for (int i = 0; i < MAXD; ++i) {
+        if (i < Ds) {
+            double wy = 0.0;
+#pragma unroll
+            for (int k = 0; k < MAXD; ++k) if (k < Ds) wy = fma(rt.W[i * Ds + k], v[k], wy);
+            quad = fma(v[i], wy, quad);
+        }
+    }
+    return exp(-0.5 * quad);
+}
+
+// the reverse sweep's step arguments (pg_step_kernel, particles.cu)
+struct PgDev : PtPolicy {
+    int t;
+    const double* eps; const double* traj; const double* step_risk;
+    const double* gxt;          // VJP of step t at x~_t [R P,D]; NULL at t = H-1
+    const double* var_prev;     // var_{t-1} [R P,Ds] (t > 0)
+    double* gx;                 // [R P,Ds] x_bar_{t+1} in, x_bar_t out (= the gmean of step t-1's VJP)
+    double* gvar;               // [R P,Ds] the gvar of step t-1's VJP
+    double* zbar;               // [R P,H,U]
+};
+
+// ---- angular state dimensions (particles_angles.cu, DESIGN.md section 20) -------------------------------------------
+// PtPolicy::Ds is the policy's input width Dh = E + A; x0, eps, traj, mean, var, gx, gvar and var_prev are in the raw
+// state width E; x~_t = [phi(x_t), u_t] has D = Dh + U.
+struct PaStep : PtDev {
+    int E;
+    TrigMap tm;                                         // tm.Ds = E
+    double* phi;                                        // phi(x_t) [R P,H+1,Dh] for the gradients, or NULL
+};
+
+struct PaBwd : PgDev {
+    int E;
+    TrigMap tm;
+    const double* phi;                                  // phi(x_t) [R P,H+1,Dh], the forward's
+    double* phib;                                       // phi_bar_t [R P,D] rows (over gxt's; NULL when gxt is)
+};
+
+// grid (ceil(P / 128), R): the angle path's forward step t (in place of pt_step_kernel)
+int pa_step_launch(cudaStream_t st, dim3 grid, const PaStep& a);
+// grid (ceil(P / 128), R): the angle path's reverse step t (in place of pg_step_kernel), two launches
+int pa_reverse_launch(cudaStream_t st, dim3 grid, const PaBwd& a);

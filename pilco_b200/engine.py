@@ -659,12 +659,17 @@ class ParticlePlan:
     ``estimator`` picks what ``launch_grad()`` estimates d E[return] with: ``"pathwise"`` (the default) differentiates
     the sampled trajectories; ``"score"`` is the score-function estimator (pilco_particles_rollout_score_grad, DESIGN.md
     section 16), which differentiates no trajectory, so box terms enter its gradient.  Both give the same rollout and
-    value.  ``"score"`` with ``consistent=True``, or an unknown estimator, is a ValueError."""
+    value.  ``"score"`` with ``consistent=True``, or an unknown estimator, is a ValueError.
+
+    ``angles``: angular state dimensions (pilco_particles_angles_*, DESIGN.md section 20).  The state x0, eps and traj
+    then have the dynamics GP's output count E as their last dimension; the policy (``policy_spec["Ds"]`` = E +
+    len(angles)) and the joint state-action terms see phi(x), the dynamics GP [phi(x), u].  The gradient of an unbatched
+    plan runs the batch-gradient call at R = 1."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
-                 estimator="pathwise"):
+                 estimator="pathwise", angles=None):
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         if consistent and estimator == "score":
@@ -675,17 +680,19 @@ class ParticlePlan:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
         self.consistent = bool(consistent)
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles)
         pr, d = self.pr, device()
         P, H = self.P, self.H
         if self.consistent:
-            wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
+            wsb = (lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)) if self.ang is None else
+                   lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(self.ang)))
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         elif not self.batched:                                  # the forward-only rollout (a batch has none)
-            wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
+            wsb = (lib.pilco_particles_workspace_bytes(C.byref(pr)) if self.ang is None else
+                   lib.pilco_particles_angles_workspace_bytes(C.byref(pr), C.byref(self.ang)))
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
@@ -698,20 +705,34 @@ class ParticlePlan:
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.ang is not None:
+            f = (lib.pilco_particles_angles_score_grad_workspace_bytes if self.estimator == "score" else
+                 lib.pilco_particles_angles_batch_grad_workspace_bytes)
+            return int(f(C.byref(pr), C.byref(self.ang), self.R))
         if self.estimator == "score":
             return int(lib.pilco_particles_score_grad_workspace_bytes(C.byref(pr), self.R))
         if self.batched:
             return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
         return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
 
-    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad):
-        """the pilco_particles description, its input and output buffers (self.pr)"""
+    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None):
+        """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
+        The angles and the policy's width are checked first, before any device work."""
+        self.ang = None
+        if angles is not None and len(angles) > 0:
+            E = int(dyn.struct().E)
+            self.ang = angles_struct(angles, E)
+            if int(policy_spec["Ds"]) != E + self.ang.A:
+                raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
+                                 % (self.ang.A, E + self.ang.A, int(policy_spec["Ds"])))
         d = device()
         self.P, self.H, self.R = int(P), int(H), int(R)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
         P, H, Ds, U, R = self.P, self.H, self.Ds, self.U, self.R
         if P < 1 or H < 0 or R < 1:
             raise ValueError("particles: needs P >= 1, H >= 0 and R >= 1 (P=%d, H=%d, R=%d)" % (P, H, R))
+        if self.ang is not None:
+            self.Ds = int(dyn.struct().E)
         rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
         self.batched = R > 1 or rbf_batched
         if self.batched and not grad:
@@ -731,7 +752,7 @@ class ParticlePlan:
         self.rw = _fill_rewards(pr, reward_terms)
         pr.mult_mu = float(mult_mu)
         mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
-        Hb = max(H, 1)                                          # H = 0: every buffer still has an address
+        Hb, Ds = max(H, 1), self.Ds                             # H = 0: every buffer still has an address
         self.x0, self.eps_buf = mk(P, Ds), mk(P, Hb, Ds)                  # shared by the R policies
         self.traj, self.act_buf = mk(*lead, P, H + 1, Ds), mk(*lead, P, Hb, U)
         self.rew_buf, self.risk_buf, self.ret = mk(*lead, P, Hb), mk(*lead, P, Hb), mk(*lead, P)
@@ -761,7 +782,16 @@ class ParticlePlan:
         ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        if self.estimator == "score":
+        if self.ang is not None:
+            if self.estimator == "score":
+                check(lib.pilco_particles_angles_score_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
+                                                                    C.byref(self.grad), stream_ptr()),
+                      "particles_angles_score_grad_rollout")
+            else:
+                check(lib.pilco_particles_angles_batch_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
+                                                                    C.byref(self.grad), stream_ptr()),
+                      "particles_angles_batch_grad_rollout")
+        elif self.estimator == "score":
             check(lib.pilco_particles_rollout_score_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
                   "particles_rollout_score_grad")
         elif self.batched:
@@ -780,6 +810,14 @@ class ParticlePlan:
     def launch(self):
         if self.batched:
             raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
+        if self.ang is not None:
+            if self.consistent:
+                check(lib.pilco_particles_angles_consistent_rollout(C.byref(self.pr), C.byref(self.ang), stream_ptr()),
+                      "particles_angles_consistent_rollout")
+            else:
+                check(lib.pilco_particles_angles_rollout(C.byref(self.pr), C.byref(self.ang), stream_ptr()),
+                      "particles_angles_rollout")
+            return
         if self.consistent:
             check(lib.pilco_particles_rollout_consistent(C.byref(self.pr), stream_ptr()), "particles_rollout_consistent")
             return
@@ -801,11 +839,13 @@ class ConsistentGradPlan(ParticlePlan):
 
     The workspace is O(R P H E n) and is not chunked: chunking the particles would reorder the gradient's fixed-order
     sums.  A plan whose workspace exceeds ``max_ws_bytes`` (default: half the free device memory) is a ValueError
-    that names the bytes needed and the number of particles that would fit, raised before anything is allocated."""
+    that names the bytes needed and the number of particles that would fit, raised before anything is allocated.
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None):
+    ``angles``: as ``ParticlePlan``."""
+
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None):
         self.consistent = True
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
@@ -823,6 +863,8 @@ class ConsistentGradPlan(ParticlePlan):
             return 0
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.ang is not None:
+            return int(lib.pilco_particles_angles_consistent_grad_workspace_bytes(C.byref(pr), C.byref(self.ang), self.R))
         return int(lib.pilco_particles_consistent_grad_workspace_bytes(C.byref(pr), self.R))
 
     def launch(self):
@@ -831,6 +873,11 @@ class ConsistentGradPlan(ParticlePlan):
     def launch_grad(self):
         """pilco_particles_rollout_consistent_grad: the consistent rollout (``outputs()``) and the pathwise gradient
         of value = mean return, returned as ``ParticlePlan.launch_grad`` returns it"""
+        if self.ang is not None:
+            check(lib.pilco_particles_angles_consistent_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
+                                                                     C.byref(self.grad), stream_ptr()),
+                  "particles_angles_consistent_grad_rollout")
+            return self.gbuf
         check(lib.pilco_particles_rollout_consistent_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
               "particles_rollout_consistent_grad")
         return self.gbuf
@@ -862,53 +909,66 @@ def gp_predict_vjp(gp, Xs, gmean, gvar):
     return out
 
 
-def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None):
+def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,
+                      angles=None):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
     step_risk [P,H], ret [P]) device tensors.
 
     ``consistent=True``: pilco_particles_rollout_consistent, one posterior function per particle.  Its workspace is
     O(P H E n), so the particles run in chunks whose workspace fits ``max_ws_bytes`` (default: half the free device
-    memory).  A particle's outputs do not depend on its batch, so the chunking does not change them."""
+    memory).  A particle's outputs do not depend on its batch, so the chunking does not change them.
+
+    ``angles``: angular state dimensions, as ``ParticlePlan``: Ds is then the dynamics GP's output count E and the
+    policy takes E + len(angles) inputs."""
     x0, eps = dev(x0), dev(eps)
     if x0.dim() != 2 or eps.dim() != 3 or eps.shape[0] != x0.shape[0] or eps.shape[2] != x0.shape[1]:
         raise ValueError("particles_rollout: x0 must be [P,Ds] and eps [P,H,Ds], got %s and %s"
                          % (tuple(x0.shape), tuple(eps.shape)))
     if consistent:
-        return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes)
-    plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu)
+        return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles)
+    plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu, angles=angles)
     plan.set_inputs(x0, eps)
     plan.launch()
     return plan.outputs()
 
 
-def consistent_workspace_bytes(dyn, Ds, U, P, H):
-    """pilco_particles_consistent_workspace_bytes of P particles over H steps (0: unsupported sizes)"""
+def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):
+    """pilco_particles_consistent_workspace_bytes of P particles over H steps (0: unsupported sizes); ``Ds`` is the
+    policy's input width (with ``angles``: E + len(angles))"""
     pr = _lib.Particles()
     pr.P, pr.H = int(P), int(H)
     pr.dyn = dyn.struct()
     pr.pol.Ds, pr.pol.U = int(Ds), int(U)
+    ang = angles_struct(angles, int(pr.dyn.E))
+    if ang is not None:
+        return int(lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(ang)))
     return int(lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)))
 
 
-def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes):
+def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None):
     P, H = int(x0.shape[0]), int(eps.shape[1])
     Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
+    if angles is not None and len(angles) > 0:                 # the policy's width, before any allocation
+        E = int(dyn.struct().E)
+        A = angles_struct(angles, E).A
+        if Ds != E + A:
+            raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d" % (A, E + A, Ds))
     if max_ws_bytes is None:
         max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
-    fits = lambda p: 0 < consistent_workspace_bytes(dyn, Ds, U, p, H) <= max_ws_bytes
+    wsb = lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles)
+    fits = lambda p: 0 < wsb(p) <= max_ws_bytes
     if not fits(1):
         raise ValueError("particles_rollout: the consistent rollout of one particle (H=%d, n=%d) needs %d workspace "
-                         "bytes, more than max_ws_bytes=%d" % (H, dyn.n, consistent_workspace_bytes(dyn, Ds, U, 1, H),
-                                                               max_ws_bytes))
+                         "bytes, more than max_ws_bytes=%d" % (H, dyn.n, wsb(1), max_ws_bytes))
     lo = _largest_fitting(fits, 1, P)
     if lo == P:
-        plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True)
+        plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles)
         plan.set_inputs(x0, eps)
         plan.launch()
         return plan.outputs()
     d = device()
-    Hb = max(H, 1)
+    Hb, Ds = max(H, 1), int(x0.shape[1])
     out = (torch.empty((P, H + 1, Ds), dtype=F64, device=d), torch.empty((P, Hb, U), dtype=F64, device=d)[:, :H],
            torch.empty((P, Hb), dtype=F64, device=d)[:, :H], torch.empty((P, Hb), dtype=F64, device=d)[:, :H],
            torch.empty(P, dtype=F64, device=d))
@@ -917,7 +977,8 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         p1 = min(P, p0 + lo)
         if plan is None or plan.P != p1 - p0:
             plan = None                                     # free the previous chunk's workspace first
-            plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True)
+            plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True,
+                                angles=angles)
         plan.set_inputs(x0[p0:p1], eps[p0:p1])
         plan.launch()
         for o, c in zip(out, plan.outputs()):
