@@ -366,6 +366,34 @@ int    pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles*
 int    pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
                                      pilco_stream_t stream);
 
+/* ---- exploration objective (the original PILCO's exploration parameter b; DESIGN.md section 21) -----------------
+ * The rollout of pilco_rollout_angles_* (ang may be NULL) with, per step t = 0 .. H-1 of restart r,
+ *   sigma_t^2 = sum_k c_k^2 Var[r_k]  over the ADD-channel terms (CombinedRewards.compute_reward's rule, covariances
+ *               between terms ignored): state terms at (m_t, S_t), joint terms (PILCO_REWARD_*_SA) at step t's joint
+ *               Gaussian; exponential: r_2 - r_1^2 (reward.m:52-56), linear: W^T S W.  MULT-channel terms do not enter.
+ *   sigma_t   = sqrt(sigma_t^2) if sigma_t^2 > 1e-12, else 0 (with zero gradient)
+ * and reward[r] = sum_t (E[r_t] + b sigma_t), summed in step order, plus the MULT channel's term.  b > 0 is optimistic
+ * under model uncertainty (exploration), b < 0 risk-averse.  step_reward stays E[r_t].  The call is inactive when
+ * ex == NULL or b == 0 with step_var == NULL: it is then the pilco_rollout_angles_* call, workspace sizes included; with
+ * b == 0 every output and gradient is bitwise that call's.  The tape is pilco_rollout_angles_tape_bytes'.  Validation
+ * before any work is enqueued: the status codes of the call without exploration, PILCO_ERR_DIM for a non-finite b,
+ * PILCO_ERR_UNSUPPORTED for an ADD-channel PILCO_REWARD_BOX term (no variance closed form), PILCO_ERR_WORKSPACE when
+ * ro->ws_bytes is below pilco_rollout_explore_workspace_bytes. */
+typedef struct pilco_exploration {
+    double  b;                  /* weight of sigma_t in the objective; finite */
+    double* step_var;           /* [R,H] sigma_t^2, or NULL */
+} pilco_exploration;
+
+size_t pilco_rollout_explore_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex);
+size_t pilco_rollout_explore_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                                 const pilco_exploration* ex);
+int    pilco_rollout_explore_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                     pilco_stream_t stream);
+/* gradient of reward[r] (with the bonus) as pilco_rollout_angles_backward gives it.  Must follow
+ * pilco_rollout_explore_forward with the same `ro`, `ang` and `ex` (it reads the sigma_t^2 that call saved in ro->ws). */
+int    pilco_rollout_explore_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                      const pilco_rollout_grad* g, pilco_stream_t stream);
+
 /* ---- particle rollout -------------------------------------------------------------------------
  * Monte Carlo check of the moment-matching cascade (nothing in the reference; the PILCO papers validate moment
  * matching against particle rollouts of the same model).  P particles follow the Markov chain whose Gaussian

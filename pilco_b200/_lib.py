@@ -75,6 +75,11 @@ class Angles(C.Structure):
     _fields_ = [("A", C.c_int), ("dims", C.c_int * 16)]
 
 
+class Exploration(C.Structure):
+    """mirror of ``pilco_exploration``"""
+    _fields_ = [("b", C.c_double), ("step_var", c_dp)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -133,6 +138,13 @@ SIGNATURES = {
     "pilco_rollout_angles_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles)]),
     "pilco_rollout_angles_forward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), c_dp]),
     "pilco_rollout_angles_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(RolloutGrad), c_dp]),
+    "pilco_rollout_explore_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles),
+                                                           C.POINTER(Exploration)]),
+    "pilco_rollout_explore_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles),
+                                                               C.POINTER(Exploration)]),
+    "pilco_rollout_explore_forward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration), c_dp]),
+    "pilco_rollout_explore_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
+                                                 C.POINTER(RolloutGrad), c_dp]),
     "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
     "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
     "pilco_gp_predict_vjp_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

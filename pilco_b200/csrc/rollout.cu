@@ -17,23 +17,6 @@
 #include "mm_tape.cuh"
 #include "small_kernels.cuh"
 
-struct RoDev {
-    int R, H, Ds, U, t;
-    int pol_kind, squash;
-    const double* maxa;
-    const double* W; long long W_bs; const double* b; long long b_bs;
-    int n_rewards; pilco_reward_term rewards[8];
-    const double* m0; long long m0_bs; const double* S0; long long S0_bs;
-    double* traj_m; double* traj_S; double* reward; double* step_reward;
-    double* risk; double* step_risk; double mult_mu; int n_mult;     // MULT channel (SafePILCO): risk[t*R + r]
-    double* rew;                                                      // additive channel per step: rew[t*R + r]
-    // per-step slots [R, len] for step t (cur) and t-1 (prev)
-    double *mj, *sj, *Mp, *Sp, *Vp, *Mu, *Su, *Cq, *Vu;
-    double *mj_prev, *sj_prev, *Md_prev, *Sd_prev, *Vd_prev;
-    MMParams dyn_prev;        // finish of the dynamics MM launched at step t-1
-    MMParams pol;             // finish of the policy MM launched at step t (RBF)
-};
-
 // squash (optional) + joint, shared by the linear and RBF paths
 __device__ __forceinline__ void ro_action_tail(const RoDev& p, int r, const double* mx, const double* sx,
                                                SmallScratch& sc) {
@@ -214,7 +197,9 @@ size_t pilco_rollout_tape_bytes(const pilco_rollout* ro) {
     return mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, ro->R).per_r * (size_t)ro->R * (size_t)ro->H * sizeof(double);
 }
 
-int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
+}  // extern "C"
+
+static int ro_forward_impl(const pilco_rollout* ro, RoRewardHook hook, const void* ctx, pilco_stream_t stream) {
     int rc = ro_check(ro);
     if (rc) return rc;
     const RoWs L = ro_ws_layout(ro);
@@ -294,20 +279,23 @@ int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
         launch_hi(ro_reward_kernel, dim3(H, R), dim3(128), 0, st, d);
         CUDA_LAUNCH_CHECK();
     }
+    RoDev dj = d;
+    dj.n_rewards = n_joint;
+    for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
+    dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
     if (H > 0 && n_joint > 0) {
-        RoDev dj = d;
-        dj.n_rewards = n_joint;
-        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
-        dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
         launch_hi(ro_reward_joint_kernel, dim3(H, R), dim3(128), 0, st, dj);
         CUDA_LAUNCH_CHECK();
     }
+    if (hook) return hook(d, n_joint > 0 ? &dj : nullptr, st, ctx);
     launch_hi(ro_reward_sum_kernel, dim3((R + 127) / 128), dim3(128), 0, st, d);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
 
-}  // extern "C"
+extern "C" int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
+    return ro_forward_impl(ro, nullptr, nullptr, stream);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Angular state dimensions (pilco_rollout_angles_forward).  The state x [Ds] stays raw; the policy and the dynamics GP
@@ -407,11 +395,13 @@ size_t pilco_rollout_angles_tape_bytes(const pilco_rollout* ro, const pilco_angl
     return pilco_rollout_tape_bytes(ro);
 }
 
-int pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* ang, pilco_stream_t stream) {
+}  // extern "C"
+
+int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t stream) {
     TrigMap tm;
     int rc = tg_check(ro, ang, &tm);
     if (rc) return rc;
-    if (tm.A == 0) return pilco_rollout_forward(ro, stream);
+    if (tm.A == 0) return ro_forward_impl(ro, hook, ctx, stream);
     const TgWs T = tg_ws_layout(ro);
     const RoWs& L = T.b;
     if (ro->ws_bytes < T.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
@@ -498,17 +488,20 @@ int pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* an
         launch_hi(ro_reward_kernel, dim3(H, R), dim3(128), 0, st, dr);
         CUDA_LAUNCH_CHECK();
     }
-    if (H > 0 && n_joint > 0) {                       // the joint terms read [phi, u]: ro_reward_joint's D = Dh + U
-        RoDev dj = d;
-        dj.n_rewards = n_joint;
-        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
-        dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
+    RoDev dj = d;                                     // the joint terms read [phi, u]: ro_reward_joint's D = Dh + U
+    dj.n_rewards = n_joint;
+    for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
+    dj.mj = slot(L.mj, D, 0); dj.sj = slot(L.sj, (size_t)D * D, 0);
+    if (H > 0 && n_joint > 0) {
         launch_hi(ro_reward_joint_kernel, dim3(H, R), dim3(128), 0, st, dj);
         CUDA_LAUNCH_CHECK();
     }
+    if (hook) return hook(dr, n_joint > 0 ? &dj : nullptr, st, ctx);
     launch_hi(ro_reward_sum_kernel, dim3((R + 127) / 128), dim3(128), 0, st, dr);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
 
-}  // extern "C"
+extern "C" int pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* ang, pilco_stream_t stream) {
+    return ro_forward_run(ro, ang, nullptr, nullptr, (cudaStream_t)stream);
+}

@@ -27,6 +27,31 @@ static inline RoWs ro_ws_layout(const pilco_rollout* ro) {
 
 int ro_check(const pilco_rollout* ro);
 
+// parameters of the forward cascade's per-step and reward kernels (rollout.cu)
+struct RoDev {
+    int R, H, Ds, U, t;
+    int pol_kind, squash;
+    const double* maxa;
+    const double* W; long long W_bs; const double* b; long long b_bs;
+    int n_rewards; pilco_reward_term rewards[8];
+    const double* m0; long long m0_bs; const double* S0; long long S0_bs;
+    double* traj_m; double* traj_S; double* reward; double* step_reward;
+    double* risk; double* step_risk; double mult_mu; int n_mult;     // MULT channel (SafePILCO): risk[t*R + r]
+    double* rew;                                                      // additive channel per step: rew[t*R + r]
+    // per-step slots [R, len] for step t (cur) and t-1 (prev)
+    double *mj, *sj, *Mp, *Sp, *Vp, *Mu, *Su, *Cq, *Vu;
+    double *mj_prev, *sj_prev, *Md_prev, *Sd_prev, *Vd_prev;
+    MMParams dyn_prev;        // finish of the dynamics MM launched at step t-1
+    MMParams pol;             // finish of the policy MM launched at step t (RBF)
+};
+
+// Optional hook of the forward (pilco_rollout_explore_forward): run after the reward launches in place of ro_reward_sum,
+// with the state terms' parameters ds (state dimension ds.Ds) and, when a joint state-action term is present, the joint
+// terms' dj (dimension dj->Ds + dj->U; dj->mj, dj->sj the joint Gaussians of step 0), else NULL.
+typedef int (*RoRewardHook)(const RoDev& ds, const RoDev* dj, cudaStream_t st, const void* ctx);
+// pilco_rollout_angles_forward (ang may be NULL) with the hook above; hook == NULL is that call
+int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t st);
+
 // ---- angular state dimensions (pilco_rollout_angles_*): state Ds = dyn.E, policy input Dh = pol.Ds = Ds + A ----
 #include "trig_math.cuh"
 // validation of a rollout with angles; fills tm.  PILCO_OK with tm.A == 0 when there are none.

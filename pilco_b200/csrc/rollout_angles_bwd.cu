@@ -248,12 +248,14 @@ size_t pilco_rollout_angles_bwd_workspace_bytes(const pilco_rollout* ro, const p
     return tb_ws_layout(ro).total * sizeof(double);
 }
 
-int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
-                                  pilco_stream_t stream) {
+}  // extern "C"
+
+int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
+                    const void* ctx, cudaStream_t stream) {
     TrigMap tm;
     int rc = tg_check(ro, ang, &tm);
     if (rc) return rc;
-    if (tm.A == 0) return pilco_rollout_backward(ro, g, stream);
+    if (tm.A == 0) return rb_backward_impl(ro, g, hook, ctx, stream);
     if (!g || !g->ws) return PILCO_ERR_NULL;
     const TgWs FT = tg_ws_layout(ro);
     const RoWs& FL = FT.b;
@@ -324,6 +326,10 @@ int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* a
         for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
         rc = rb_reward_launch(ds, joint ? &dj : nullptr, st);
         if (rc) return rc;
+        if (hook) {
+            rc = hook(ds, joint ? &dj : nullptr, st, ctx);
+            if (rc) return rc;
+        }
     }
 
     for (int t = H - 1; t >= 0; --t) {
@@ -379,4 +385,7 @@ int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* a
     return PILCO_OK;
 }
 
-}  // extern "C"
+extern "C" int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
+                                             pilco_stream_t stream) {
+    return rb_backward_run(ro, ang, g, nullptr, nullptr, (cudaStream_t)stream);
+}

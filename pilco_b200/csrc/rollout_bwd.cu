@@ -347,7 +347,10 @@ size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro) {
     return rb_ws_layout(ro).total * sizeof(double);
 }
 
-int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream) {
+}  // extern "C"
+
+int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRewardHook hook, const void* ctx,
+                     cudaStream_t stream) {
     int rc = ro_check(ro);
     if (rc) return rc;
     if (!g || !g->ws) return PILCO_ERR_NULL;
@@ -413,12 +416,16 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
         d.sj = d.Vd = d.Mp = d.Sp = d.Vp = d.Mu = d.Su = d.Cq = d.Vu = nullptr;
         launch_hi(rb_reward_kernel, dim3(R, H), dim3(128), 0, st, d);     // reward gradients of every step at once
         CUDA_LAUNCH_CHECK();
+        RbDev dj = d;
+        dj.n_rewards = n_joint;
+        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
         if (joint) {
-            RbDev dj = d;
-            dj.n_rewards = n_joint;
-            for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
             launch_hi(rb_reward_joint_kernel, dim3(R, H), dim3(128), 0, st, dj);
             CUDA_LAUNCH_CHECK();
+        }
+        if (hook) {
+            rc = hook(d, joint ? &dj : nullptr, st, ctx);
+            if (rc) return rc;
         }
     }
 
@@ -475,5 +482,7 @@ int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g,
     return PILCO_OK;
 }
 
-}  // extern "C"
+extern "C" int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream) {
+    return rb_backward_impl(ro, g, nullptr, nullptr, (cudaStream_t)stream);
+}
 

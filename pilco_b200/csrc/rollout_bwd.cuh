@@ -31,6 +31,16 @@ struct RbDev {
 };
 
 int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st);
+// Optional hook of the reverse sweep (pilco_rollout_explore_backward): run once the reward-gradient precompute
+// (rb_reward, rb_reward_joint) is enqueued and before the serial per-step chain, with the state terms' parameters ds
+// (state dimension ds.Ds) and, when a joint state-action term is present, the joint terms' dj, else NULL.
+typedef int (*RbRewardHook)(const RbDev& ds, const RbDev* dj, cudaStream_t st, const void* ctx);
+// pilco_rollout_backward with the hook above (rollout_bwd.cu); hook == NULL is that call
+int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRewardHook hook, const void* ctx,
+                     cudaStream_t st);
+// pilco_rollout_angles_backward (ang may be NULL) with the hook above (rollout_angles_bwd.cu)
+int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
+                    const void* ctx, cudaStream_t st);
 int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
                           const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
                           const double* beta, long long beta_bs, const double* gy,

@@ -287,6 +287,58 @@ __device__ __forceinline__ void dev_exp_reward_bwd(int Ds, const double* W, cons
     __syncthreads();
 }
 
+// VJP of a power of the f-scaled ExponentialReward moment (reward.m:52-66: f = 1 the mean, f = 2 the second moment)
+//   r_f = exp(-f/2 (m-t)^T W (I+f sW)^-1 (m-t)) / sqrt(det(I+f sW)),  w_f = W (I+f sW)^-1 (m-t):
+//   d r_f/dm = -f r_f w_f,  d r_f/dS = (f/2) r_f (f w_f w_f^T - W (I+f sW)^-1)
+// gm += scale d(r_f^p)/dm, gS += scale d(r_f^p)/dS (p = 1 or 2), symmetrised as dev_exp_reward_bwd; returns r_f.
+__device__ __forceinline__ double dev_exp_moment_bwd(int Ds, const double* W, const double* t, const double* m,
+                                                     const double* s, double f, int p, double scale, double* gm,
+                                                     double* gS, SmallScratch& sc) {
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    __syncthreads();
+    for (int e = tid; e < Ds * Ds; e += nt) {
+        const int i = e / Ds, j = e % Ds;
+        double v = 0.0;
+        for (int k = 0; k < Ds; ++k) v = fma(s[i * Ds + k], W[k * Ds + j], v);
+        sc.A[i * SLD + j] = f * v + (i == j ? 1.0 : 0.0);
+        sc.B[i * SLD + j] = (i == j) ? 1.0 : 0.0;
+    }
+    for (int i = tid; i < Ds; i += nt) sc.v[i] = m[i] - t[i];
+    __syncthreads();
+    if (warp == 0) {
+        double det;
+        lu_warp(sc.A, sc.perm, Ds, lane, &det);
+        lu_solve_warp(sc.A, sc.perm, sc.B, sc.C, Ds, Ds, lane);          // C = (I + f sW)^-1
+        if (lane == 0) sc.det = det;
+    }
+    __syncthreads();
+    for (int e = tid; e < Ds * Ds; e += nt) {                            // B = W (I + f sW)^-1
+        const int i = e / Ds, j = e % Ds;
+        double v = 0.0;
+        for (int k = 0; k < Ds; ++k) v = fma(W[i * Ds + k], sc.C[k * SLD + j], v);
+        sc.B[i * SLD + j] = v;
+    }
+    __syncthreads();
+    for (int i = tid; i < Ds; i += nt) {
+        double v = 0.0;
+        for (int k = 0; k < Ds; ++k) v = fma(sc.B[i * SLD + k], sc.v[k], v);
+        sc.w[i] = v;
+    }
+    __syncthreads();
+    double quad = 0.0;
+    for (int i = 0; i < Ds; ++i) quad = fma(sc.v[i], sc.w[i], quad);
+    const double rf = exp(-0.5 * f * quad) / sqrt(sc.det);
+    const double c = (p == 2 ? 2.0 * rf : 1.0) * scale * rf;              // scale d(r_f^p)/d r_f times r_f
+    for (int i = tid; i < Ds; i += nt) gm[i] += -f * c * sc.w[i];
+    for (int e = tid; e < Ds * Ds; e += nt) {
+        const int i = e / Ds, j = e % Ds;
+        const double isym = 0.5 * (sc.B[i * SLD + j] + sc.B[j * SLD + i]);
+        gS[e] += 0.5 * f * c * (f * sc.w[i] * sc.w[j] - isym);
+    }
+    __syncthreads();
+    return rf;
+}
+
 // LinearController VJP: gW += gMp m^T + (gSp+gSp^T) W s + gVp^T ; gb += gMp ; gm += W^T gMp ; gS += W^T gSp W
 __device__ __forceinline__ void dev_linear_bwd(int Ds, int U, const double* W, const double* m, const double* s,
                                                const double* gMp, const double* gSp, const double* gVp,

@@ -528,13 +528,30 @@ class RolloutPlan:
     pilco.py:130-134; multiplicative ones form the per-step risk of SafePILCO.predict, safe_pilco.py:29-50, and
     enter the returned reward as ``mult_mu * (1 - prod_t (1 - risk_t))``)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False, angles=None):
+    def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False, angles=None,
+                 exploration=None):
         """``grad=True``: the forward cascade runs the TAPED dynamics tile pass (pilco_rollout.tape), so that
         ``backward()`` needs no recomputation; without it ``backward()`` still works (recomputing path).
 
         ``angles``: angular state dimensions (pilco_rollout_angles_*).  The state dimension is then the dynamics GP's
         output count E; the policy (``policy_spec["Ds"]``) and the joint state-action terms see phi(x) of dimension
-        Dh = E + len(angles), the dynamics GP [phi(x), u]."""
+        Dh = E + len(angles), the dynamics GP [phi(x), u].
+
+        ``exploration``: a float b selects the exploration objective (pilco_rollout_explore_*, DESIGN.md section 21):
+        ``reward`` = sum_t (E[r_t] + b sigma_t) (+ the multiplicative channel's term), sigma_t^2 = sum_k c_k^2 Var[r_k]
+        over the additive terms, written to ``step_var`` [R, max(H,1)]; its gradient is ``backward()``'s.  b = 0.0 fills
+        ``step_var`` and leaves every other output and gradient as without exploration.  ``None``: no exploration.
+        A non-finite b, or an additive box term (it has no variance closed form), is a ValueError."""
+        b = None
+        if exploration is not None:
+            b = float(exploration)
+            if not np.isfinite(b):
+                raise ValueError("exploration: b must be finite, got %r" % exploration)
+            for k, rt in enumerate(reward_terms):
+                if rt["kind"] == _lib.REWARD_BOX and int(rt.get("channel", _lib.CHANNEL_ADD)) == _lib.CHANNEL_ADD:
+                    raise ValueError("exploration: reward term %d is an additive box term, which has no variance closed "
+                                     "form; use it in the multiplicative channel (SafePILCO) or leave exploration off"
+                                     % k)
         d = device()
         self.dyn = dyn
         self.R, self.H = int(R), int(H)
@@ -577,8 +594,15 @@ class RolloutPlan:
         self.info = torch.zeros(self.R, dtype=torch.int32, device=d)
         ro.traj_m, ro.traj_S = self.traj_m.data_ptr(), self.traj_S.data_ptr()
         ro.reward, ro.step_reward, ro.info = self.reward.data_ptr(), self.step_reward.data_ptr(), self.info.data_ptr()
-        wsb = (lib.pilco_rollout_workspace_bytes(C.byref(ro)) if self.ang is None else
-               lib.pilco_rollout_angles_workspace_bytes(C.byref(ro), C.byref(self.ang)))
+        self.ex, self.step_var = None, None
+        if b is not None:
+            self.step_var = torch.zeros((self.R, max(self.H, 1)), dtype=F64, device=d)
+            self.ex = _lib.Exploration(b, self.step_var.data_ptr())
+            wsb = lib.pilco_rollout_explore_workspace_bytes(C.byref(ro), self._ang_ref(), C.byref(self.ex))
+        elif self.ang is None:
+            wsb = lib.pilco_rollout_workspace_bytes(C.byref(ro))
+        else:
+            wsb = lib.pilco_rollout_angles_workspace_bytes(C.byref(ro), C.byref(self.ang))
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         ro.ws, ro.ws_bytes = self.ws.data_ptr(), wsb
         self.tape = None
@@ -589,8 +613,14 @@ class RolloutPlan:
                 ro.tape, ro.tape_bytes = self.tape.data_ptr(), tb
         self.ro = ro
 
+    def _ang_ref(self):
+        return C.byref(self.ang) if self.ang is not None else None
+
     def forward(self):
-        if self.ang is None:
+        if self.ex is not None:
+            check(lib.pilco_rollout_explore_forward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex), stream_ptr()),
+                  "rollout_explore_forward")
+        elif self.ang is None:
             check(lib.pilco_rollout_forward(C.byref(self.ro), stream_ptr()), "rollout_forward")
         else:
             check(lib.pilco_rollout_angles_forward(C.byref(self.ro), C.byref(self.ang), stream_ptr()),
@@ -628,12 +658,19 @@ class RolloutPlan:
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
-            wsb = (lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro)) if self.ang is None else
-                   lib.pilco_rollout_angles_bwd_workspace_bytes(C.byref(self.ro), C.byref(self.ang)))
+            if self.ex is not None:
+                wsb = lib.pilco_rollout_explore_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), C.byref(self.ex))
+            elif self.ang is None:
+                wsb = lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro))
+            else:
+                wsb = lib.pilco_rollout_angles_bwd_workspace_bytes(C.byref(self.ro), C.byref(self.ang))
             self.bws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.bws.data_ptr(), wsb
             self.grad = g
-        if self.ang is None:
+        if self.ex is not None:
+            check(lib.pilco_rollout_explore_backward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex),
+                                                     C.byref(self.grad), stream_ptr()), "rollout_explore_backward")
+        elif self.ang is None:
             check(lib.pilco_rollout_backward(C.byref(self.ro), C.byref(self.grad), stream_ptr()), "rollout_backward")
         else:
             check(lib.pilco_rollout_angles_backward(C.byref(self.ro), C.byref(self.ang), C.byref(self.grad), stream_ptr()),

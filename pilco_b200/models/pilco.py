@@ -43,15 +43,23 @@ def _controller_input_dim(c):
 
 class PILCO:
     def __init__(self, data, num_induced_points=None, horizon=30, controller=None,
-                 reward=None, m_init=None, S_init=None, name=None, *, angle_dims=None):
+                 reward=None, m_init=None, S_init=None, name=None, *, angle_dims=None, exploration=0.0):
         """``angle_dims``: angular state dimensions (PILCO's trigonometric augmentation, DESIGN.md section 19).  The
         policy and the dynamics GPs then see phi(x) = [the other state dimensions, sin and cos of each angle] (Dh =
         state_dim + len(angle_dims)), while the state, m_init / S_init, the state reward terms and the GP outputs stay
         raw.  ``data`` stays the raw (X = [x, u], Y = delta x); the angles' deltas in Y must be continuous (unwrapped).
         The models are trained on [phi(x), u], so ``mgpr.models[e].predict_*`` take such inputs; new raw data goes
         through ``PILCO.set_data``.  The controller must take Dh inputs and every joint state-action reward term must
-        have state_dim = Dh (ValueError otherwise)."""
+        have state_dim = Dh (ValueError otherwise).
+
+        ``exploration``: the weight b of the original PILCO's exploration objective sum_t (E[r_t] + b sigma_t), sigma_t
+        the standard deviation of step t's reward under the predicted state distribution (DESIGN.md section 21).  b > 0
+        is optimistic under model uncertainty and draws the policy to states the model does not know; b < 0 is
+        risk-averse.  ``optimize_policy``, ``policy_gradient``, ``training_loss`` and ``compute_reward`` use it;
+        ``predict`` keeps returning the expected reward.  A plain attribute: reassign ``pilco.exploration`` between
+        calls.  A reward with an additive box term has no variance closed form: b != 0 with one is a ValueError."""
         self.name = name
+        self.exploration = float(exploration)
         self.state_dim = data[1].shape[1]
         self.control_dim = data[0].shape[1] - data[1].shape[1]
         self.angle_dims = None
@@ -301,18 +309,43 @@ class PILCO:
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
 
+    def _exploration_b(self):
+        """the exploration weight for the device rollout: None at b = 0, which runs the objective without it"""
+        b = float(self.exploration)
+        return None if b == 0.0 else b
+
+    def _single_plan(self, m_x, s_x, n, grad=False, exploration=None):
+        """RolloutPlan of one n-step rollout of the current policy from N(m_x, s_x)"""
+        terms, mult_mu = self.reward_spec()
+        return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
+                                  np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
+                                  int(n), R=1, mult_mu=mult_mu, grad=grad, angles=self.angle_dims,
+                                  exploration=exploration)
+
+    def predict_reward_moments(self, m_x, s_x, n):
+        """Mean and variance of each step's reward along the n-step prediction from N(m_x, s_x): E[r_t] (the terms
+        ``predict`` sums) and sigma_t^2 = sum_k c_k^2 Var[r_k] over the additive terms (CombinedRewards' rule), how sure
+        the model is of the reward at step t (DESIGN.md section 21).  -> (mean [n], var [n]) host arrays.  A reward with
+        an additive box term is a ValueError (no variance closed form)."""
+        from ..params import HostArray
+        n = int(n)
+        plan = self._single_plan(m_x, s_x, n, exploration=0.0)
+        plan.forward()
+        if int(plan.info[0].item()) != 0:
+            raise RuntimeError("moment-matching rollout failed: covariance not positive definite")
+        return (plan.step_reward[0, :n].cpu().numpy().view(HostArray),
+                plan.step_var[0, :n].cpu().numpy().view(HostArray))
+
     def policy_gradient(self, m_x=None, s_x=None, n=None):
         """The moment-matching reward of ``predict`` (n steps from N(m_x, s_x); defaults m_init, S_init, horizon) and
         its gradient d reward / d controller.get_flat() for the current policy: the direction ``optimize_policy``
-        ascends, in the layout of ``sample_policy_gradient``.  -> (reward (float), grad host array)."""
+        ascends, in the layout of ``sample_policy_gradient``.  With ``exploration`` b != 0 the reward is the objective
+        sum_t (E[r_t] + b sigma_t).  -> (reward (float), grad host array)."""
         from ..params import HostArray
         m_x = self.m_init if m_x is None else m_x
         s_x = self.S_init if s_x is None else s_x
         n = self.horizon if n is None else n
-        terms, mult_mu = self.reward_spec()
-        plan = engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
-                                  np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
-                                  int(n), R=1, mult_mu=mult_mu, grad=True, angles=self.angle_dims)
+        plan = self._single_plan(m_x, s_x, n, grad=True, exploration=self._exploration_b())
         plan.forward()
         g = plan.backward()
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
@@ -362,7 +395,18 @@ class PILCO:
         return best_value
 
     def training_loss(self):
-        return -self.predict(self.m_init, self.S_init, self.horizon)[2]
+        """-(the objective optimize_policy maximises) from N(m_init, S_init) over the horizon: -predict's reward, or with
+        ``exploration`` b != 0, -sum_t (E[r_t] + b sigma_t) -> [1,1] host array"""
+        b = self._exploration_b()
+        if b is None:
+            return -self.predict(self.m_init, self.S_init, self.horizon)[2]
+        from ..params import HostArray
+        # the taped forward, as policy_gradient runs it: the two give the same objective to the bit
+        plan = self._single_plan(self.m_init, self.S_init, self.horizon, grad=True, exploration=b)
+        plan.forward()
+        if int(plan.info[0].item()) != 0:
+            raise RuntimeError("moment-matching rollout failed: covariance not positive definite")
+        return (-plan.reward[:1].reshape(1, 1)).cpu().numpy().view(HostArray)
 
     def compute_reward(self):
         return -self.training_loss()

@@ -149,7 +149,8 @@ class _FlatEvaluator:
 
 
 class PolicyEvaluator(_FlatEvaluator):
-    """loss(flat) = -sum_t E[r(x_t)] and its gradient for a batch of flat policy parameter vectors.
+    """loss(flat) = -sum_t E[r(x_t)] (with the PILCO's exploration b != 0: -sum_t (E[r_t] + b sigma_t)) and its
+    gradient for a batch of flat policy parameter vectors.
 
     The R restarts are dealt to ``nsplit`` sub-batches, each with its own RolloutPlan (taped forward + reverse sweep)
     on its own stream inside ONE captured CUDA graph: the latency-bound glue kernels of one sub-batch overlap the tile
@@ -166,13 +167,15 @@ class PolicyEvaluator(_FlatEvaluator):
         self.slices = [(bounds[k], bounds[k + 1]) for k in range(nsplit) if bounds[k + 1] > bounds[k]]
         self.plans, self.gps = [], []
         dyn = pilco.mgpr.device_gp()
+        b = float(getattr(pilco, "exploration", 0.0))
+        exploration = b if b != 0.0 else None                  # b = 0: the plans without exploration
         for lo, hi in self.slices:
             spec = c.policy_spec(flat0[lo:hi]) if self.linear else pilco.policy_spec(flat0[lo:hi])
             self.gps.append(None if self.linear else spec["gp"])
             self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
                                                  np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
                                                  mult_mu=mult_mu, grad=True,
-                                                 angles=getattr(pilco, "angle_dims", None)))
+                                                 angles=getattr(pilco, "angle_dims", None), exploration=exploration))
         self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
         self._setup_io()
 
