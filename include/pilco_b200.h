@@ -394,6 +394,33 @@ int    pilco_rollout_explore_forward(const pilco_rollout* ro, const pilco_angles
 int    pilco_rollout_explore_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                       const pilco_rollout_grad* g, pilco_stream_t stream);
 
+/* ---- measurement noise at the policy's input (propagate.m's noisy state measurement; DESIGN.md section 22) --------
+ * The rollout of pilco_rollout_explore_* (ang and ex may be NULL) whose policy sees a noisy measurement z = x + nu,
+ * nu ~ N(0, diag(var[0 .. Ds-1])) independent of x (Ds = dyn.E, the raw state).  Per step t of restart r:
+ *   the policy is moment-matched at the moments of phi(z) under N(m_t, S_t + diag(var)) (phi = identity without angles);
+ *   the dynamics GP receives [phi(x), u] with phi's moments under N(m_t, S_t) and cov(phi(x), u) = S^_x V_u, V_u the
+ *   policy's (squashed) input-output factor at the noisy input (propagate.m's q = S(j,i) C: the true S, the noisy C);
+ *   the next-state glue uses cov(x, [phi(x), u]) = S_t C^_x [I, V_u];
+ *   the reward terms are unchanged (state terms at (m_t, S_t), joint terms and sigma_t^2 at the joint above).
+ * With nz == NULL every call is the pilco_rollout_explore_* call, workspace sizes included.  The tape is
+ * pilco_rollout_tape_bytes'.  Validation before any work is enqueued: the status codes of the explore call's
+ * description and exploration checks, then PILCO_ERR_DIM for a non-finite or negative var[i], i < Ds, then
+ * PILCO_ERR_WORKSPACE when ro->ws_bytes is below pilco_rollout_noisy_workspace_bytes (g->ws_bytes below
+ * pilco_rollout_noisy_bwd_workspace_bytes for the backward).  The backward gives no gradient with respect to var. */
+typedef struct pilco_obs_noise {
+    double var[PILCO_MAX_D];    /* measurement noise variance of each raw state dimension, >= 0; the first Ds are used */
+} pilco_obs_noise;
+
+size_t pilco_rollout_noisy_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                           const pilco_obs_noise* nz);
+size_t pilco_rollout_noisy_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                               const pilco_exploration* ex, const pilco_obs_noise* nz);
+int    pilco_rollout_noisy_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                   const pilco_obs_noise* nz, pilco_stream_t stream);
+/* must follow pilco_rollout_noisy_forward with the same arguments (it reads the per-step moments saved in ro->ws) */
+int    pilco_rollout_noisy_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                    const pilco_obs_noise* nz, const pilco_rollout_grad* g, pilco_stream_t stream);
+
 /* ---- particle rollout -------------------------------------------------------------------------
  * Monte Carlo check of the moment-matching cascade (nothing in the reference; the PILCO papers validate moment
  * matching against particle rollouts of the same model).  P particles follow the Markov chain whose Gaussian

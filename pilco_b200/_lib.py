@@ -80,6 +80,11 @@ class Exploration(C.Structure):
     _fields_ = [("b", C.c_double), ("step_var", c_dp)]
 
 
+class ObsNoise(C.Structure):
+    """mirror of ``pilco_obs_noise``"""
+    _fields_ = [("var", C.c_double * 16)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -145,6 +150,14 @@ SIGNATURES = {
     "pilco_rollout_explore_forward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration), c_dp]),
     "pilco_rollout_explore_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
                                                  C.POINTER(RolloutGrad), c_dp]),
+    "pilco_rollout_noisy_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
+                                                         C.POINTER(ObsNoise)]),
+    "pilco_rollout_noisy_bwd_workspace_bytes": (C.c_size_t, [C.POINTER(Rollout), C.POINTER(Angles),
+                                                             C.POINTER(Exploration), C.POINTER(ObsNoise)]),
+    "pilco_rollout_noisy_forward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
+                                              C.POINTER(ObsNoise), c_dp]),
+    "pilco_rollout_noisy_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
+                                               C.POINTER(ObsNoise), C.POINTER(RolloutGrad), c_dp]),
     "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
     "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
     "pilco_gp_predict_vjp_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

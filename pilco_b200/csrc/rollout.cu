@@ -16,31 +16,7 @@
 #include "rollout.cuh"
 #include "mm_tape.cuh"
 #include "small_kernels.cuh"
-
-// squash (optional) + joint, shared by the linear and RBF paths
-__device__ __forceinline__ void ro_action_tail(const RoDev& p, int r, const double* mx, const double* sx,
-                                               SmallScratch& sc) {
-    const int Ds = p.Ds, U = p.U, D = Ds + U;
-    const int tid = threadIdx.x, nt = blockDim.x;
-    double* Mp = p.Mp + (size_t)r * U;  double* Sp = p.Sp + (size_t)r * U * U;  double* Vp = p.Vp + (size_t)r * Ds * U;
-    double* Mu = p.Mu + (size_t)r * U;  double* Su = p.Su + (size_t)r * U * U;
-    double* Cq = p.Cq + (size_t)r * U * U;  double* Vu = p.Vu + (size_t)r * Ds * U;
-    if (p.squash) {
-        dev_squash_sin(U, Mp, Sp, p.maxa, Mu, Su, Cq);
-        for (int e = tid; e < Ds * U; e += nt) {
-            const int i = e / U, j = e % U;
-            double v = 0.0;
-            for (int k = 0; k < U; ++k) v = fma(Vp[i * U + k], Cq[k * U + j], v);
-            Vu[e] = v;
-        }
-    } else {
-        for (int i = tid; i < U; i += nt) Mu[i] = Mp[i];
-        for (int e = tid; e < U * U; e += nt) { Su[e] = Sp[e]; Cq[e] = (e / U == e % U) ? 1.0 : 0.0; }
-        for (int e = tid; e < Ds * U; e += nt) Vu[e] = Vp[e];
-    }
-    __syncthreads();
-    dev_joint(Ds, U, mx, sx, Mu, Su, Vu, p.mj + (size_t)r * D, p.sj + (size_t)r * D * D, sc);
-}
+#include "rollout_step.cuh"
 
 __global__ void __launch_bounds__(128) ro_state_kernel(RoDev p) {
     PDL_ENTRY();
@@ -307,37 +283,6 @@ extern "C" int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t str
 // cx_t = cov(x_t, [phi(x_t), u_t]) = S_x C^ [I, V_u] [Ds, Dh + U] takes the place of the first Ds rows of the joint
 // covariance in the glue: S' = S_x + S_d + cx V_d + (cx V_d)^T.  The reward launches are ro_reward's, unchanged.
 // ---------------------------------------------------------------------------------------------
-struct TgDev {
-    RoDev p;                  // p.Ds = Dh: the policy's input dimension; traj_m / traj_S / m0 / S0 in Ds
-    TrigMap tm;
-    double *mh, *Sh, *Ch, *cx;        // slots of step t [R, len]
-    const double* cx_prev;            // cx of step t-1
-};
-
-// cx = [Q, Q V_u],  Q = S_x C^  [Ds, Dh]
-__device__ __forceinline__ void tg_cross(const TgDev& g, int r, const double* sx, SmallScratch& sc) {
-    const int Ds = g.tm.Ds, Dh = g.p.Ds, U = g.p.U, D = Dh + U;
-    const int tid = threadIdx.x, nt = blockDim.x;
-    const double* Ch = g.Ch + (size_t)r * Ds * Dh;
-    const double* Vu = g.p.Vu + (size_t)r * Dh * U;
-    double* cx = g.cx + (size_t)r * Ds * D;
-    for (int e = tid; e < Ds * Dh; e += nt) {
-        const int i = e / Dh, k = e % Dh;
-        double v = 0.0;
-        for (int l = 0; l < Ds; ++l) v = fma(sx[i * Ds + l], Ch[l * Dh + k], v);
-        sc.C[i * SLD + k] = v;
-        cx[i * D + k] = v;
-    }
-    __syncthreads();
-    for (int e = tid; e < Ds * U; e += nt) {
-        const int i = e / U, j = e % U;
-        double v = 0.0;
-        for (int k = 0; k < Dh; ++k) v = fma(sc.C[i * SLD + k], Vu[k * U + j], v);
-        cx[i * D + Dh + j] = v;
-    }
-    __syncthreads();
-}
-
 __global__ void __launch_bounds__(128) tg_state_kernel(TgDev g) {
     PDL_ENTRY();
     __shared__ SmallScratch sc;
@@ -397,11 +342,13 @@ size_t pilco_rollout_angles_tape_bytes(const pilco_rollout* ro, const pilco_angl
 
 }  // extern "C"
 
-int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t stream) {
+int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t stream,
+                   const NzFwd* nz) {
     TrigMap tm;
     int rc = tg_check(ro, ang, &tm);
     if (rc) return rc;
-    if (tm.A == 0) return ro_forward_impl(ro, hook, ctx, stream);
+    if (tm.A == 0 && !nz) return ro_forward_impl(ro, hook, ctx, stream);
+    if (tm.A == 0) trig_map_make(ro->dyn.E, 0, nullptr, &tm);      // measurement noise without angles: phi = identity
     const TgWs T = tg_ws_layout(ro);
     const RoWs& L = T.b;
     if (ro->ws_bytes < T.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
@@ -442,8 +389,9 @@ int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHoo
                          slot(L.Md, Ds, t), slot(L.Sd, (size_t)Ds * Ds, t), slot(L.Vd, (size_t)D * Ds, t), ro->info,
                          ws + L.dynws, ro->tape ? (double*)ro->tape + (size_t)t * RR * TL.per_r : nullptr, TL);
     };
-    auto pol_params = [&](int t) {                   // the policy GP reads the feature moments of step t
-        return mm_params(&ro->pol.rbf, R, slot(T.mh, Dh, t), Dh, slot(T.Sh, (size_t)Dh * Dh, t), (long long)Dh * Dh,
+    const size_t pmh = nz ? nz->mz : T.mh, pSh = nz ? nz->Sz : T.Sh;
+    auto pol_params = [&](int t) {                   // the policy GP reads the feature moments of step t (noisy ones with nz)
+        return mm_params(&ro->pol.rbf, R, slot(pmh, Dh, t), Dh, slot(pSh, (size_t)Dh * Dh, t), (long long)Dh * Dh,
                          slot(L.Mp, U, t), slot(L.Sp, (size_t)U * U, t), slot(L.Vp, (size_t)Dh * U, t), ro->info,
                          ws + L.polws);
     };
@@ -470,8 +418,13 @@ int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHoo
             d.dyn_prev = dyn_params(0);
         }
         if (ro->pol.kind == PILCO_POLICY_RBF && t < H) d.pol = pol_params(t); else d.pol = d.dyn_prev;
-        launch_hi(tg_state_kernel, dim3(R), dim3(128), 0, st, g);
-        CUDA_LAUNCH_CHECK();
+        if (nz) {
+            rc = nz_state_launch(g, *nz, slot(nz->mz, Dh, tc), slot(nz->Sz, (size_t)Dh * Dh, tc), st);
+            if (rc) return rc;
+        } else {
+            launch_hi(tg_state_kernel, dim3(R), dim3(128), 0, st, g);
+            CUDA_LAUNCH_CHECK();
+        }
         if (t == H) break;
         if (ro->pol.kind == PILCO_POLICY_RBF) {
             rc = mm_forward_launch(d.pol, st, false);

@@ -49,13 +49,24 @@ struct RoDev {
 // with the state terms' parameters ds (state dimension ds.Ds) and, when a joint state-action term is present, the joint
 // terms' dj (dimension dj->Ds + dj->U; dj->mj, dj->sj the joint Gaussians of step 0), else NULL.
 typedef int (*RoRewardHook)(const RoDev& ds, const RoDev* dj, cudaStream_t st, const void* ctx);
-// pilco_rollout_angles_forward (ang may be NULL) with the hook above; hook == NULL is that call
-int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t st);
+struct NzFwd;
+// pilco_rollout_angles_forward (ang may be NULL) with the hook above; hook == NULL is that call.  nz: measurement noise at
+// the policy's input (pilco_rollout_noisy_forward, validated by the caller), NULL without.
+int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t st,
+                   const NzFwd* nz = nullptr);
 
 // ---- angular state dimensions (pilco_rollout_angles_*): state Ds = dyn.E, policy input Dh = pol.Ds = Ds + A ----
 #include "trig_math.cuh"
 // validation of a rollout with angles; fills tm.  PILCO_OK with tm.A == 0 when there are none.
 int tg_check(const pilco_rollout* ro, const pilco_angles* ang, TrigMap* tm);
+
+// parameters of the angle cascade's per-step kernels (rollout.cu)
+struct TgDev {
+    RoDev p;                  // p.Ds = Dh: the policy's input dimension; traj_m / traj_S / m0 / S0 in Ds
+    TrigMap tm;
+    double *mh, *Sh, *Ch, *cx;        // slots of step t [R, len]
+    const double* cx_prev;            // cx of step t-1
+};
 
 struct TgWs {                 // offsets in doubles: ro_ws_layout's slots at the policy dimension Dh, plus per step
     RoWs b;                   // (m^, S^, C^) of the feature map and cx = cov(x, [phi, u]) [Ds, Dh + U]
@@ -85,3 +96,26 @@ static inline int ro_count_mult(const pilco_rollout* ro) {
     for (int k = 0; k < ro->n_rewards; ++k) c += ro->rewards[k].channel == PILCO_CHANNEL_MULT;
     return c;
 }
+
+// ---- measurement noise at the policy's input (pilco_rollout_noisy_*, rollout_noise.cu) ----
+// The angle cascade (A >= 0; with A = 0 phi is the identity) whose policy reads the moments (m^_z, S^_z) of phi under
+// N(m, S + diag(var)), kept per step after the angle layout (and before the exploration slot, when there is one).
+struct NzFwd {
+    double var[MAXD];         // noise variance of each raw state dimension
+    size_t mz, Sz;            // offsets in doubles in ro->ws: [H][R][Dh], [H][R][Dh][Dh]
+};
+
+// the angle layout, then the noisy moments; `total` is where an exploration slot would go
+static inline NzFwd nz_ws_layout(const pilco_rollout* ro, size_t* total) {
+    const size_t R = ro->R, H = ro->H, Dh = ro->pol.Ds;
+    NzFwd L;
+    size_t o = tg_ws_layout(ro).total;
+    auto take = [&](size_t len) { size_t at = o; o += (H * R * len + 1) & ~(size_t)1; return at; };
+    L.mz = take(Dh); L.Sz = take(Dh * Dh);
+    *total = o;
+    return L;
+}
+
+// the per-step state kernel of the noisy cascade (in place of tg_state): glue as tg_state, then both feature-moment
+// sets, the linear policy at the noisy one, squash, the joint and cx at the true one; mz / Sz the slots of step t
+int nz_state_launch(const TgDev& g, const NzFwd& nz, double* mz, double* Sz, cudaStream_t st);

@@ -50,14 +50,6 @@ static TbWs tb_ws_layout(const pilco_rollout* ro) {
     return L;
 }
 
-struct TbDev {
-    RbDev p;                  // p.Ds = Dh; p.gm / p.gS: the raw state's cotangent [R, Ds], [R, Ds, Ds]
-    TrigMap tm;
-    const double *mh, *Sh, *Ch, *cx;  // forward slots of step t
-    const double *cx_prev, *Vd_prev;  // step t-1 (NULL at t = 0)
-    double *gVd, *gcx, *gmh, *gSh, *gCh;
-};
-
 struct TbPostSmem { SmallScratch sc; double gMu[MAXD], gSu[MAXD * MAXD], gVu[MAXD * MAXD], gB[MAXD * MAXD], gCd[MAXD],
                     gQ[MAXD * MAXD]; };
 
@@ -250,17 +242,34 @@ size_t pilco_rollout_angles_bwd_workspace_bytes(const pilco_rollout* ro, const p
 
 }  // extern "C"
 
+// with measurement noise: the angle layout, then the cotangent of the noisy moments (gm^_z [R][Dh], gS^_z [R][Dh][Dh])
+static size_t nz_bwd_layout(const pilco_rollout* ro, size_t* gmz, size_t* gSz) {
+    const size_t R = ro->R, Dh = ro->pol.Ds;
+    size_t o = tb_ws_layout(ro).total;
+    *gmz = o; o += (R * Dh + 1) & ~(size_t)1;
+    *gSz = o; o += (R * Dh * Dh + 1) & ~(size_t)1;
+    return o;
+}
+
+size_t nz_bwd_ws_doubles(const pilco_rollout* ro) {
+    size_t a, b;
+    return nz_bwd_layout(ro, &a, &b);
+}
+
 int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
-                    const void* ctx, cudaStream_t stream) {
+                    const void* ctx, cudaStream_t stream, const NzFwd* nz) {
     TrigMap tm;
     int rc = tg_check(ro, ang, &tm);
     if (rc) return rc;
-    if (tm.A == 0) return rb_backward_impl(ro, g, hook, ctx, stream);
+    if (tm.A == 0 && !nz) return rb_backward_impl(ro, g, hook, ctx, stream);
+    if (tm.A == 0) trig_map_make(ro->dyn.E, 0, nullptr, &tm);      // measurement noise without angles: phi = identity
     if (!g || !g->ws) return PILCO_ERR_NULL;
     const TgWs FT = tg_ws_layout(ro);
     const RoWs& FL = FT.b;
     const TbWs BL = tb_ws_layout(ro);
-    if (g->ws_bytes < BL.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
+    size_t o_gmz = 0, o_gSz = 0;
+    const size_t need = nz ? nz_bwd_layout(ro, &o_gmz, &o_gSz) : BL.total;
+    if (g->ws_bytes < need * sizeof(double)) return PILCO_ERR_WORKSPACE;
     if (((uintptr_t)g->ws) & 15) return PILCO_ERR_ALIGN;
     const int R = ro->R, H = ro->H, Ds = tm.Ds, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U;
     const bool rbf = ro->pol.kind == PILCO_POLICY_RBF;
@@ -285,6 +294,7 @@ int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilc
         cudaMemsetAsync(g->gW, 0, sizeof(double) * RR * U * Dh, st);
         cudaMemsetAsync(g->gb, 0, sizeof(double) * RR * U, st);
     }
+    if (nz) cudaMemsetAsync(buf(o_gmz), 0, sizeof(double) * (need - o_gmz), st);     // nz_trig re-zeroes after each step
     if (!ro->tape) mm_bwd_zero_counters(mm_bws_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, 0), bws + BL.dynb, R, st);
     if (rbf) mm_bwd_zero_counters(mm_bws_layout(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, 1), bws + BL.polb, R, st);
 
@@ -317,6 +327,8 @@ int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilc
     d.cnt = reinterpret_cast<unsigned*>(buf(BL.cnt));
     d.t = 0;
     tg.gVd = buf(BL.gVd); tg.gcx = buf(BL.gcx); tg.gmh = buf(BL.gmh); tg.gSh = buf(BL.gSh); tg.gCh = buf(BL.gCh);
+    double* gmz = nz ? buf(o_gmz) : nullptr;
+    double* gSz = nz ? buf(o_gSz) : nullptr;
     if (H > 0) {
         d.sj = d.Vd = d.Mp = d.Sp = d.Vp = d.Mu = d.Su = d.Cq = d.Vu = nullptr;
         RbDev ds = d;                                 // the state terms at the raw trajectory
@@ -342,13 +354,15 @@ int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilc
         tg.cx = slot(FT.cx, (size_t)Ds * D, t);
         tg.cx_prev = t > 0 ? slot(FT.cx, (size_t)Ds * D, t - 1) : nullptr;
         tg.Vd_prev = t > 0 ? slot(FL.Vd, (size_t)D * Ds, t - 1) : nullptr;
+        TbDev tp = tg;                                // with noise, the post stage stops before the linear-policy VJP,
+        if (nz) tp.p.pol_kind = -1;                   // which nz_trig runs at the noisy moments
         if (ro->tape) {
             const MMTapeL TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
             const MMTapeBwd tb = mm_tape_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t),
                                                     (long long)D * D, slot(FL.Md, Ds, t), d.gm, d.gS, tg.gVd,
                                                     (const double*)ro->tape + (size_t)t * RR * TL.per_r, TL,
                                                     bws + BL.dynb, d.gmj, D, d.gsj, (long long)D * D);
-            rc = ks_dispatch(D, [&](auto ks) { return launch_tg_dyn_finish<4 * ks>(tb, tg, st); });
+            rc = ks_dispatch(D, [&](auto ks) { return launch_tg_dyn_finish<4 * ks>(tb, tp, st); });
             if (rc) return rc;
             CUDA_LAUNCH_CHECK();
         } else {
@@ -357,19 +371,26 @@ int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilc
                                            d.gmj, D, d.gsj, (long long)D * D, nullptr, nullptr, nullptr, 0, bws + BL.dynb);
             rc = mm_backward_launch(bp, st);
             if (rc) return rc;
-            launch_hi(tg_post_kernel, dim3(R), dim3(128), sizeof(TbPostSmem), st, tg);
+            launch_hi(tg_post_kernel, dim3(R), dim3(128), sizeof(TbPostSmem), st, tp);
             CUDA_LAUNCH_CHECK();
         }
-        if (rbf) {
-            MMBwdParams pp = mm_bwd_params(&ro->pol.rbf, R, tg.mh, Dh, tg.Sh, (long long)Dh * Dh,
+        const double* mz = nz ? slot(nz->mz, Dh, t) : nullptr;
+        const double* Sz = nz ? slot(nz->Sz, (size_t)Dh * Dh, t) : nullptr;
+        if (rbf) {                                    // the policy's input: the feature moments (the noisy ones with nz)
+            MMBwdParams pp = mm_bwd_params(&ro->pol.rbf, R, nz ? mz : tg.mh, Dh, nz ? Sz : tg.Sh, (long long)Dh * Dh,
                                            slot(FL.Mp, U, t), d.gMp, d.gSp, d.gVp,
-                                           tg.gmh, Dh, tg.gSh, (long long)Dh * Dh,
+                                           nz ? gmz : tg.gmh, Dh, nz ? gSz : tg.gSh, (long long)Dh * Dh,
                                            g->gXc, buf(BL.gbeta), g->gell, 1, bws + BL.polb);
             rc = mm_backward_launch(pp, st);
             if (rc) return rc;
         }
-        launch_hi(tg_trig_kernel, dim3(R), dim3(128), 0, st, tg);
-        CUDA_LAUNCH_CHECK();
+        if (nz) {
+            rc = nz_trig_launch(tg, *nz, mz, Sz, gmz, gSz, st);
+            if (rc) return rc;
+        } else {
+            launch_hi(tg_trig_kernel, dim3(R), dim3(128), 0, st, tg);
+            CUDA_LAUNCH_CHECK();
+        }
     }
     if (rbf) {
         const int ldw = pad64(bf);

@@ -38,10 +38,79 @@ typedef int (*RbRewardHook)(const RbDev& ds, const RbDev* dj, cudaStream_t st, c
 // pilco_rollout_backward with the hook above (rollout_bwd.cu); hook == NULL is that call
 int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRewardHook hook, const void* ctx,
                      cudaStream_t st);
-// pilco_rollout_angles_backward (ang may be NULL) with the hook above (rollout_angles_bwd.cu)
+// pilco_rollout_angles_backward (ang may be NULL) with the hook above (rollout_angles_bwd.cu).  nz: measurement noise
+// at the policy's input (pilco_rollout_noisy_backward, validated by the caller; g->ws of nz_bwd_ws_doubles), else NULL.
 int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
-                    const void* ctx, cudaStream_t st);
+                    const void* ctx, cudaStream_t st, const NzFwd* nz = nullptr);
+size_t nz_bwd_ws_doubles(const pilco_rollout* ro);
+
+// parameters of the angle cascade's reverse per-step kernels (rollout_angles_bwd.cu)
+struct TbDev {
+    RbDev p;                  // p.Ds = Dh; p.gm / p.gS: the raw state's cotangent [R, Ds], [R, Ds, Ds]
+    TrigMap tm;
+    const double *mh, *Sh, *Ch, *cx;  // forward slots of step t
+    const double *cx_prev, *Vd_prev;  // step t-1 (NULL at t = 0)
+    double *gVd, *gcx, *gmh, *gSh, *gCh;
+};
+
+#ifdef __CUDACC__
+// the per-step trig stage once the trig VJP is in the state cotangent (gm, gS) of restart r: the state reward gradients
+// of step t, then the symmetric part of gS0 (t = 0) or the seeds of step t-1.  The tail of tg_trig_kernel
+// (rollout_angles_bwd.cu), which keeps its own copy: calling this from it changes that kernel's register allocation.
+__device__ __forceinline__ void tg_trig_tail(const TbDev& g, int r, double* gm, double* gS) {
+    const RbDev& p = g.p;
+    const int Ds = g.tm.Ds, Dh = p.Ds, D = Dh + p.U, t = p.t;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    double wmult = p.mult_mu;
+    if (wmult != 0.0)
+        for (int tt = 0; tt < p.H; ++tt) if (tt != t) wmult *= 1.0 - p.risk[(size_t)tt * p.R + r];
+    const double* ra_m = p.rgm + (((size_t)t * 2) * p.R + r) * Ds;
+    const double* ra_S = p.rgS + (((size_t)t * 2) * p.R + r) * Ds * Ds;
+    const double* rm_m = ra_m + (size_t)p.R * Ds;
+    const double* rm_S = ra_S + (size_t)p.R * Ds * Ds;
+    for (int i = tid; i < Ds; i += nt) gm[i] += ra_m[i] + wmult * rm_m[i];
+    for (int e = tid; e < Ds * Ds; e += nt) gS[e] += ra_S[e] + wmult * rm_S[e];
+    __syncthreads();
+    if (t == 0) {              // gS0: the symmetric part (S0 is symmetric; the glue's gQ C^T terms are not)
+        for (int e = tid; e < Ds * Ds; e += nt) {
+            const int i = e / Ds, j = e % Ds;
+            if (i < j) { const double v = 0.5 * (gS[e] + gS[j * Ds + i]); gS[e] = v; gS[j * Ds + i] = v; }
+        }
+        return;
+    }
+    // seeds of step t-1: gV = cx^T (gS + gS^T) [D, Ds],  gcx = (gS + gS^T) V_d^T [Ds, D]
+    const double* cx = g.cx_prev + (size_t)r * Ds * D;
+    const double* Vd = g.Vd_prev + (size_t)r * D * Ds;
+    for (int e = tid; e < D * Ds; e += nt) {
+        const int k = e / Ds, j = e % Ds;
+        double v = 0.0;
+        for (int i = 0; i < Ds; ++i) v = fma(cx[i * D + k], gS[i * Ds + j] + gS[j * Ds + i], v);
+        g.gVd[(size_t)r * D * Ds + e] = v;
+    }
+    for (int e = tid; e < Ds * D; e += nt) {
+        const int i = e / D, k = e % D;
+        double v = 0.0;
+        for (int j = 0; j < Ds; ++j) v = fma(gS[i * Ds + j] + gS[j * Ds + i], Vd[k * Ds + j], v);
+        g.gcx[(size_t)r * Ds * D + e] = v;
+    }
+}
+#endif
+
+// the per-step trig stage of the noisy reverse sweep (in place of tg_trig; rollout_noise.cu): the linear-policy VJP at
+// the noisy moments (mz, Sz) into (gmz, gSz), both trig VJPs into the state cotangent, then tg_trig's reward gradients
+// and seeds of step t-1; (gmz, gSz) are left zero for the next step
+int nz_trig_launch(const TbDev& g, const NzFwd& nz, const double* mz, const double* Sz, double* gmz, double* gSz,
+                   cudaStream_t st);
 int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
                           const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
                           const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
+
+// the exploration objective on the noisy cascade (rollout_explore.cu), for an active `ex` (b != 0 or step_var) that
+// ex_terms_check accepted: sigma_t^2 goes to ro->ws + var_at
+bool ex_active(const pilco_exploration* ex);
+int ex_terms_check(const pilco_rollout* ro, const pilco_exploration* ex);
+int ex_forward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
+                     size_t var_at, cudaStream_t st);
+int ex_backward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
+                      size_t var_at, const pilco_rollout_grad* g, cudaStream_t st);

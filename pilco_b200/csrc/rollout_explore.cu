@@ -147,17 +147,23 @@ static ExWs ex_ws_layout(const pilco_rollout* ro, const pilco_angles* ang) {
     return L;
 }
 
-static bool ex_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
+bool ex_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
+
+int ex_terms_check(const pilco_rollout* ro, const pilco_exploration* ex) {
+    if (!std::isfinite(ex->b)) return PILCO_ERR_DIM;
+    for (int k = 0; k < ro->n_rewards; ++k)            // no variance closed form for a box term
+        if (ro->rewards[k].channel == PILCO_CHANNEL_ADD && ro->rewards[k].kind == PILCO_REWARD_BOX)
+            return PILCO_ERR_UNSUPPORTED;
+    return PILCO_OK;
+}
 
 // validation of an active exploration call, before anything is enqueued
 static int ex_check(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex) {
     TrigMap tm;
     int rc = tg_check(ro, ang, &tm);
     if (rc) return rc;
-    if (!std::isfinite(ex->b)) return PILCO_ERR_DIM;
-    for (int k = 0; k < ro->n_rewards; ++k)            // no variance closed form for a box term
-        if (ro->rewards[k].channel == PILCO_CHANNEL_ADD && ro->rewards[k].kind == PILCO_REWARD_BOX)
-            return PILCO_ERR_UNSUPPORTED;
+    rc = ex_terms_check(ro, ex);
+    if (rc) return rc;
     if (ro->ws_bytes < ex_ws_layout(ro, ang).total * sizeof(double)) return PILCO_ERR_WORKSPACE;
     return PILCO_OK;
 }
@@ -189,6 +195,19 @@ static int ex_backward_hook(const RbDev& ds, const RbDev* dj, cudaStream_t st, c
         CUDA_LAUNCH_CHECK();
     }
     return PILCO_OK;
+}
+
+int ex_forward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
+                     size_t var_at, cudaStream_t st) {
+    const ExCtx c = {ex->b, (double*)ro->ws + var_at, ex->step_var};
+    return ro_forward_run(ro, ang, ex_forward_hook, &c, st, nz);
+}
+
+int ex_backward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
+                      size_t var_at, const pilco_rollout_grad* g, cudaStream_t st) {
+    if (ex->b == 0.0) return rb_backward_run(ro, ang, g, nullptr, nullptr, st, nz);
+    const ExCtx c = {ex->b, (double*)ro->ws + var_at, nullptr};
+    return rb_backward_run(ro, ang, g, ex_backward_hook, &c, st, nz);
 }
 
 extern "C" {

@@ -529,7 +529,7 @@ class RolloutPlan:
     enter the returned reward as ``mult_mu * (1 - prod_t (1 - risk_t))``)."""
 
     def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False, angles=None,
-                 exploration=None):
+                 exploration=None, measurement_noise=None):
         """``grad=True``: the forward cascade runs the TAPED dynamics tile pass (pilco_rollout.tape), so that
         ``backward()`` needs no recomputation; without it ``backward()`` still works (recomputing path).
 
@@ -541,7 +541,12 @@ class RolloutPlan:
         ``reward`` = sum_t (E[r_t] + b sigma_t) (+ the multiplicative channel's term), sigma_t^2 = sum_k c_k^2 Var[r_k]
         over the additive terms, written to ``step_var`` [R, max(H,1)]; its gradient is ``backward()``'s.  b = 0.0 fills
         ``step_var`` and leaves every other output and gradient as without exploration.  ``None``: no exploration.
-        A non-finite b, or an additive box term (it has no variance closed form), is a ValueError."""
+        A non-finite b, or an additive box term (it has no variance closed form), is a ValueError.
+
+        ``measurement_noise``: variances v [Ds] >= 0 of a noisy state measurement z = x + nu, nu ~ N(0, diag(v)), that
+        the policy sees in place of the state (pilco_rollout_noisy_*, DESIGN.md section 22): the policy is moment-matched
+        at N(m, S + diag(v)) (phi of it with angles), the dynamics and the rewards see the true state's moments.  Ds is
+        the raw state dimension.  ``None``: the policy sees the state."""
         b = None
         if exploration is not None:
             b = float(exploration)
@@ -552,6 +557,11 @@ class RolloutPlan:
                     raise ValueError("exploration: reward term %d is an additive box term, which has no variance closed "
                                      "form; use it in the multiplicative channel (SafePILCO) or leave exploration off"
                                      % k)
+        nz_var = None
+        if measurement_noise is not None:
+            nz_var = np.asarray(measurement_noise, dtype=np.float64).reshape(-1)
+            if not np.all(np.isfinite(nz_var)) or np.any(nz_var < 0.0):
+                raise ValueError("measurement_noise: the variances must be finite and >= 0, got %r" % nz_var)
         d = device()
         self.dyn = dyn
         self.R, self.H = int(R), int(H)
@@ -564,6 +574,13 @@ class RolloutPlan:
             if int(policy_spec["Ds"]) != Dh:
                 raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
                                  % (self.ang.A, Dh, int(policy_spec["Ds"])))
+        self.nz = None
+        if nz_var is not None:
+            if nz_var.shape[0] != int(self.Ds):
+                raise ValueError("measurement_noise: expected %d variances (the state dimension), got %d"
+                                 % (int(self.Ds), nz_var.shape[0]))
+            self.nz = _lib.ObsNoise()
+            self.nz.var[:len(nz_var)] = nz_var.tolist()
         self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
         ro = _lib.Rollout()
         ro.R, ro.H = self.R, self.H
@@ -598,6 +615,9 @@ class RolloutPlan:
         if b is not None:
             self.step_var = torch.zeros((self.R, max(self.H, 1)), dtype=F64, device=d)
             self.ex = _lib.Exploration(b, self.step_var.data_ptr())
+        if self.nz is not None:
+            wsb = lib.pilco_rollout_noisy_workspace_bytes(C.byref(ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz))
+        elif self.ex is not None:
             wsb = lib.pilco_rollout_explore_workspace_bytes(C.byref(ro), self._ang_ref(), C.byref(self.ex))
         elif self.ang is None:
             wsb = lib.pilco_rollout_workspace_bytes(C.byref(ro))
@@ -616,8 +636,14 @@ class RolloutPlan:
     def _ang_ref(self):
         return C.byref(self.ang) if self.ang is not None else None
 
+    def _ex_ref(self):
+        return C.byref(self.ex) if self.ex is not None else None
+
     def forward(self):
-        if self.ex is not None:
+        if self.nz is not None:
+            check(lib.pilco_rollout_noisy_forward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz),
+                                                  stream_ptr()), "rollout_noisy_forward")
+        elif self.ex is not None:
             check(lib.pilco_rollout_explore_forward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex), stream_ptr()),
                   "rollout_explore_forward")
         elif self.ang is None:
@@ -658,7 +684,10 @@ class RolloutPlan:
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
-            if self.ex is not None:
+            if self.nz is not None:
+                wsb = lib.pilco_rollout_noisy_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), self._ex_ref(),
+                                                                  C.byref(self.nz))
+            elif self.ex is not None:
                 wsb = lib.pilco_rollout_explore_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), C.byref(self.ex))
             elif self.ang is None:
                 wsb = lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro))
@@ -667,7 +696,10 @@ class RolloutPlan:
             self.bws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.bws.data_ptr(), wsb
             self.grad = g
-        if self.ex is not None:
+        if self.nz is not None:
+            check(lib.pilco_rollout_noisy_backward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz),
+                                                   C.byref(self.grad), stream_ptr()), "rollout_noisy_backward")
+        elif self.ex is not None:
             check(lib.pilco_rollout_explore_backward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex),
                                                      C.byref(self.grad), stream_ptr()), "rollout_explore_backward")
         elif self.ang is None:
@@ -1028,8 +1060,8 @@ class PredictPlan:
     moments + reward + status -> pinned host memory.  Built once per (model, policy, reward, n) state by
     ``PILCO`` and replayed for every call with new initial moments (pilco/models/pilco.py:118-136)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0, angles=None):
-        """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``: as RolloutPlan."""
+    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0, angles=None, measurement_noise=None):
+        """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``, ``measurement_noise``: as RolloutPlan."""
         d = device()
         self.Ds, self.n = int(Ds), int(n)
         Ds = self.Ds
@@ -1038,7 +1070,7 @@ class PredictPlan:
         self.d_in = torch.zeros(Ds + Ds * Ds, dtype=F64, device=d)
         self.d_out = torch.zeros(Ds + Ds * Ds + 2, dtype=F64, device=d)
         self.plan = RolloutPlan(dyn, policy_spec, reward_terms, np.zeros(Ds), np.eye(Ds), self.n, R=1, mult_mu=mult_mu,
-                                angles=angles)
+                                angles=angles, measurement_noise=measurement_noise)
         self._enqueue()                                    # eager warm-up (one-time kernel attributes)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()

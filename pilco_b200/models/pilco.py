@@ -43,7 +43,8 @@ def _controller_input_dim(c):
 
 class PILCO:
     def __init__(self, data, num_induced_points=None, horizon=30, controller=None,
-                 reward=None, m_init=None, S_init=None, name=None, *, angle_dims=None, exploration=0.0):
+                 reward=None, m_init=None, S_init=None, name=None, *, angle_dims=None, exploration=0.0,
+                 measurement_noise=None):
         """``angle_dims``: angular state dimensions (PILCO's trigonometric augmentation, DESIGN.md section 19).  The
         policy and the dynamics GPs then see phi(x) = [the other state dimensions, sin and cos of each angle] (Dh =
         state_dim + len(angle_dims)), while the state, m_init / S_init, the state reward terms and the GP outputs stay
@@ -57,7 +58,17 @@ class PILCO:
         is optimistic under model uncertainty and draws the policy to states the model does not know; b < 0 is
         risk-averse.  ``optimize_policy``, ``policy_gradient``, ``training_loss`` and ``compute_reward`` use it;
         ``predict`` keeps returning the expected reward.  A plain attribute: reassign ``pilco.exploration`` between
-        calls.  A reward with an additive box term has no variance closed form: b != 0 with one is a ValueError."""
+        calls.  A reward with an additive box term has no variance closed form: b != 0 with one is a ValueError.
+
+        ``measurement_noise``: the policy acts on a noisy measurement z = x + nu of the state, nu ~ N(0, diag(v)), as
+        on the real system (the original PILCO's propagate.m; DESIGN.md section 22).  The moment-matching methods
+        (``predict``, ``propagate``, ``training_loss``, ``compute_reward``, ``policy_gradient``,
+        ``predict_reward_moments``, ``optimize_policy``) then moment-match the policy at N(m, S + diag(v)) while the
+        dynamics see the true state.  ``None``: the policy sees the state; an array v [state_dim] >= 0 (raw state
+        dimensions, angles included); or ``"model"``: v = the dynamics GPs' noise variances / 2 (a difference target
+        carries the noise of two measurements), read again at every call, so it follows ``optimize_models``.
+        ``compute_action`` is unchanged: on the system it is given the measurement.  The particle methods do not
+        support it (ValueError)."""
         self.name = name
         self.exploration = float(exploration)
         self.state_dim = data[1].shape[1]
@@ -98,6 +109,32 @@ class PILCO:
             self.m_init = m_init
             self.S_init = S_init
         self.optimizer = None
+        self.measurement_noise = self._check_noise(measurement_noise)
+
+    # ---- measurement noise ---------------------------------------------------------------------------
+    def _check_noise(self, v):
+        if v is None or (isinstance(v, str) and v == "model"):
+            return v
+        if isinstance(v, str):
+            raise ValueError("measurement_noise: expected None, 'model' or %d variances, got %r" % (self.state_dim, v))
+        a = np.asarray(v, dtype=np.float64).reshape(-1)
+        if a.shape[0] != self.state_dim or not np.all(np.isfinite(a)) or np.any(a < 0.0):
+            raise ValueError("measurement_noise: expected %d finite variances >= 0, got %r" % (self.state_dim, v))
+        return a.copy()
+
+    def _noise_var(self):
+        """the measurement-noise variances [state_dim] the device rollout gets, or None"""
+        v = self.measurement_noise
+        if v is None:
+            return None
+        if isinstance(v, str):                            # "model": propagate.m's sn2(difi) / 2
+            return np.asarray(self.mgpr.noise, dtype=np.float64).reshape(-1) / 2.0
+        return np.asarray(v, dtype=np.float64)
+
+    def _no_noise(self, what):
+        if self.measurement_noise is not None:
+            raise ValueError("%s: the particle rollouts do not support measurement_noise yet; use the moment-matching "
+                             "methods (predict, policy_gradient, optimize_policy)" % what)
 
     # ---- angular state dimensions ------------------------------------------------------------------
     @property
@@ -159,7 +196,8 @@ class PILCO:
         terms, mult_mu = self.reward_spec()
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(flats), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1),
-                                  np.asarray(s_x, dtype=np.float64), int(n), R=R, mult_mu=mult_mu, angles=self.angle_dims)
+                                  np.asarray(s_x, dtype=np.float64), int(n), R=R, mult_mu=mult_mu, angles=self.angle_dims,
+                                  measurement_noise=self._noise_var())
 
     def _reward_key(self):
         terms, mult_mu = self.reward_spec()
@@ -175,13 +213,15 @@ class PILCO:
         between calls either (tf.function), but here the cache is explicit -- any change of data, hyper-parameters,
         policy parameters or reward parameters changes the key and rebuilds the plan (a few ms)."""
         dyn = self.mgpr.device_gp()                       # (re)factorises only when data / hypers changed
-        key = (id(dyn), self.mgpr._cache_key, self.controller.state_key(), self._reward_key(), int(n))
+        v = self._noise_var()
+        key = (id(dyn), self.mgpr._cache_key, self.controller.state_key(), self._reward_key(), int(n),
+               None if v is None else v.tobytes())
         cache = self.__dict__.setdefault("_plans", {})
         hit = cache.get(int(n))
         if hit is None or hit[0] != key:
             terms, mult_mu = self.reward_spec()
             plan = engine.PredictPlan(dyn, self.policy_spec(), terms, self.state_dim, int(n), mult_mu=mult_mu,
-                                      angles=self.angle_dims)
+                                      angles=self.angle_dims, measurement_noise=v)
             if len(cache) >= 8:
                 cache.clear()
             cache[int(n)] = hit = (key, plan)
@@ -218,6 +258,7 @@ class PILCO:
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
         from ..params import HostArray
         self._no_angles("sample_trajectories")
+        self._no_noise("sample_trajectories")
         if consistent:
             import torch
             dyn = self.mgpr.device_gp()
@@ -297,6 +338,7 @@ class PILCO:
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
         self._no_angles("sample_policy_gradient")
+        self._no_noise("sample_policy_gradient")
         if estimator not in engine.ParticlePlan.ESTIMATORS:
             raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
                              % (engine.ParticlePlan.ESTIMATORS, estimator))
@@ -320,7 +362,7 @@ class PILCO:
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
                                   int(n), R=1, mult_mu=mult_mu, grad=grad, angles=self.angle_dims,
-                                  exploration=exploration)
+                                  exploration=exploration, measurement_noise=self._noise_var())
 
     def predict_reward_moments(self, m_x, s_x, n):
         """Mean and variance of each step's reward along the n-step prediction from N(m_x, s_x): E[r_t] (the terms
@@ -371,6 +413,7 @@ class PILCO:
         from functools import partial
         from .. import policy_opt
         self._no_angles("optimize_policy_sampled")
+        self._no_noise("optimize_policy_sampled")
         if int(num_samples) < 1:
             raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
         terms, _ = self.reward_spec()

@@ -169,13 +169,15 @@ class PolicyEvaluator(_FlatEvaluator):
         dyn = pilco.mgpr.device_gp()
         b = float(getattr(pilco, "exploration", 0.0))
         exploration = b if b != 0.0 else None                  # b = 0: the plans without exploration
+        noise = pilco._noise_var() if hasattr(pilco, "_noise_var") else None
         for lo, hi in self.slices:
             spec = c.policy_spec(flat0[lo:hi]) if self.linear else pilco.policy_spec(flat0[lo:hi])
             self.gps.append(None if self.linear else spec["gp"])
             self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
                                                  np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
                                                  mult_mu=mult_mu, grad=True,
-                                                 angles=getattr(pilco, "angle_dims", None), exploration=exploration))
+                                                 angles=getattr(pilco, "angle_dims", None), exploration=exploration,
+                                                 measurement_noise=noise))
         self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
         self._setup_io()
 

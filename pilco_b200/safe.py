@@ -93,11 +93,13 @@ class SafePILCO(PILCO):
     """safe_pilco.py:17-50: total = sum_t reward_add(x_t) + mu * (1 - prod_t (1 - reward_mult(x_t)))."""
 
     def __init__(self, data, num_induced_points=None, horizon=30, controller=None,
-                 reward_add=None, reward_mult=None, m_init=None, S_init=None, name=None, mu=5.0, *, exploration=0.0):
-        """``exploration``: PILCO's (the additive reward's sigma_t enters; the risk terms do not)"""
+                 reward_add=None, reward_mult=None, m_init=None, S_init=None, name=None, mu=5.0, *, exploration=0.0,
+                 measurement_noise=None):
+        """``exploration``: PILCO's (the additive reward's sigma_t enters; the risk terms do not).
+        ``measurement_noise``: PILCO's (the risk terms, like the reward, see the true state)"""
         super(SafePILCO, self).__init__(data, num_induced_points=num_induced_points, horizon=horizon,
                                         controller=controller, reward=reward_add, m_init=m_init, S_init=S_init,
-                                        exploration=exploration)
+                                        exploration=exploration, measurement_noise=measurement_noise)
         if reward_mult is None:
             raise Exception("have to define multiplicative reward")
         self.mu = Parameter(mu, trainable=False)
