@@ -1,31 +1,77 @@
-// rollout.cuh -- workspace layout of the H-step cascade shared by rollout.cu and rollout_bwd.cu.
+// rollout.cuh -- workspace layout, validation and kernel parameters of the H-step cascade, shared by its forward
+// (rollout.cu) and reverse sweep (rollout_bwd.cu) and the kernels of its options in their own translation units.
 #pragma once
 #include "mm_kernels.cuh"
 
-struct RoWs {                 // offsets in doubles
-    size_t mj, sj, Md, Sd, Vd, Mp, Sp, Vp, Mu, Su, Cq, Vu, risk, rew, dynws, polws, total;
+#include "trig_math.cuh"
+
+// The cascade runs on the features phi(x) of the state (trig_math.cuh) with angular state dimensions or measurement
+// noise: with noise and no angles phi is the identity.  Without either the policy and the dynamics see x itself.
+static inline bool ro_on_phi(const pilco_angles* ang, const pilco_obs_noise* nz) { return nz || (ang && ang->A != 0); }
+// sigma_t^2 is computed (and its slot kept) when b != 0 or step_var is set
+static inline bool ex_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
+
+struct RoWs {                 // offsets in doubles into pilco_rollout.ws; per step [H][R][len] unless noted
+    size_t mj, sj, Md, Sd, Vd, Mp, Sp, Vp, Mu, Su, Cq, Vu, risk, rew, mh, Sh, Ch, cx, dynws, polws, mz, Sz, var, total;
 };
 
-static inline RoWs ro_ws_layout(const pilco_rollout* ro) {
+// The forward workspace.  Dh = pol.Ds is the policy's input dimension and E the dynamics GP's output count: dyn.E on
+// phi, pol.Ds without.  A slot whose feature is off has length 0.
+static inline RoWs ro_ws_layout(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                const pilco_obs_noise* nz) {
+    const bool phi = ro_on_phi(ang, nz);
     const size_t R = ro->R, H = ro->H;
-    const size_t Ds = ro->pol.Ds, U = ro->pol.U, D = Ds + U, E = Ds;
+    const size_t Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U, E = phi ? (size_t)ro->dyn.E : Dh;
+    const size_t F = phi ? 1 : 0, N = nz ? 1 : 0;
     RoWs L; size_t o = 0;
     auto take = [&](size_t len) { size_t at = o; o += (H * R * len + 1) & ~(size_t)1; return at; };
     L.mj = take(D); L.sj = take(D * D);
     L.Md = take(E); L.Sd = take(E * E); L.Vd = take(D * E);
-    L.Mp = take(U); L.Sp = take(U * U); L.Vp = take(Ds * U);
-    L.Mu = take(U); L.Su = take(U * U); L.Cq = take(U * U); L.Vu = take(Ds * U);
+    L.Mp = take(U); L.Sp = take(U * U); L.Vp = take(Dh * U);
+    L.Mu = take(U); L.Su = take(U * U); L.Cq = take(U * U); L.Vu = take(Dh * U);
     L.risk = take(1);                       // per-step risk of the MULT reward channel, [H][R]
     L.rew = take(1);                        // per-step additive reward, [H][R] (summed in step order by ro_reward_sum_kernel)
+    // on phi: its moments (m^, S^, C^) and cx = cov(x, [phi, u]) [E, Dh + U]
+    L.mh = take(F * Dh); L.Sh = take(F * Dh * Dh); L.Ch = take(F * E * Dh); L.cx = take(F * E * D);
     L.dynws = o; o += pilco_mm_workspace_bytes(ro->dyn.n, ro->dyn.D, ro->dyn.E, ro->R) / 8;
     L.polws = o;
     if (ro->pol.kind == PILCO_POLICY_RBF)
         o += pilco_mm_workspace_bytes(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, ro->R) / 8;
+    L.mz = take(N * Dh); L.Sz = take(N * Dh * Dh);     // measurement noise: phi's moments at N(m, S + diag(var))
+    L.var = take(ex_active(ex) ? 1 : 0);               // exploration: sigma_t^2, [H][R]
     L.total = o;
     return L;
 }
 
-int ro_check(const pilco_rollout* ro);
+// what one validated call runs: ro_validate fills it
+struct RoOpt {
+    TrigMap tm;               // phi (the identity map of dyn.E dimensions with noise and no angles); meaningful on phi
+    bool phi;                 // ro_on_phi
+    bool noise;               // measurement noise at the policy's input, variances nzvar (0 from dyn.E on)
+    double nzvar[MAXD];
+    bool explore;             // ex_active
+    double b; double* step_var;
+};
+
+// Validation of a call of the cascade (ang, ex, nz may be NULL) before anything is enqueued: the description, the
+// angles, the exploration terms, the noise variances, then ro->ws's size (and for the forward its alignment and the
+// tape).  The reverse sweep without exploration and noise does not check ro->ws.
+int ro_validate(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const pilco_obs_noise* nz,
+                bool backward, RoOpt* o);
+
+// the state terms (for ro_reward / rb_reward; n_state of them) and the joint state-action terms (for the *_joint
+// kernels), each in term order and padded with empty terms to 8; returns the number of joint terms
+static inline int ro_split_rewards(const pilco_rollout* ro, int* n_state, pilco_reward_term state[8],
+                                   pilco_reward_term joint[8]) {
+    int n_joint = 0;
+    *n_state = 0;
+    for (int k = 0; k < 8; ++k) state[k] = joint[k] = pilco_reward_term();
+    for (int k = 0; k < ro->n_rewards; ++k) {
+        if (reward_on_joint(ro->rewards[k].kind)) joint[n_joint++] = ro->rewards[k];
+        else state[(*n_state)++] = ro->rewards[k];
+    }
+    return n_joint;
+}
 
 // parameters of the forward cascade's per-step and reward kernels (rollout.cu)
 struct RoDev {
@@ -45,22 +91,7 @@ struct RoDev {
     MMParams pol;             // finish of the policy MM launched at step t (RBF)
 };
 
-// Optional hook of the forward (pilco_rollout_explore_forward): run after the reward launches in place of ro_reward_sum,
-// with the state terms' parameters ds (state dimension ds.Ds) and, when a joint state-action term is present, the joint
-// terms' dj (dimension dj->Ds + dj->U; dj->mj, dj->sj the joint Gaussians of step 0), else NULL.
-typedef int (*RoRewardHook)(const RoDev& ds, const RoDev* dj, cudaStream_t st, const void* ctx);
-struct NzFwd;
-// pilco_rollout_angles_forward (ang may be NULL) with the hook above; hook == NULL is that call.  nz: measurement noise at
-// the policy's input (pilco_rollout_noisy_forward, validated by the caller), NULL without.
-int ro_forward_run(const pilco_rollout* ro, const pilco_angles* ang, RoRewardHook hook, const void* ctx, cudaStream_t st,
-                   const NzFwd* nz = nullptr);
-
-// ---- angular state dimensions (pilco_rollout_angles_*): state Ds = dyn.E, policy input Dh = pol.Ds = Ds + A ----
-#include "trig_math.cuh"
-// validation of a rollout with angles; fills tm.  PILCO_OK with tm.A == 0 when there are none.
-int tg_check(const pilco_rollout* ro, const pilco_angles* ang, TrigMap* tm);
-
-// parameters of the angle cascade's per-step kernels (rollout.cu)
+// parameters of the cascade's per-step kernels on phi (rollout.cu): state Ds = dyn.E, policy input Dh = pol.Ds = Ds + A
 struct TgDev {
     RoDev p;                  // p.Ds = Dh: the policy's input dimension; traj_m / traj_S / m0 / S0 in Ds
     TrigMap tm;
@@ -68,54 +99,18 @@ struct TgDev {
     const double* cx_prev;            // cx of step t-1
 };
 
-struct TgWs {                 // offsets in doubles: ro_ws_layout's slots at the policy dimension Dh, plus per step
-    RoWs b;                   // (m^, S^, C^) of the feature map and cx = cov(x, [phi, u]) [Ds, Dh + U]
-    size_t mh, Sh, Ch, cx, total;
-};
-
-static inline TgWs tg_ws_layout(const pilco_rollout* ro) {
-    const size_t R = ro->R, H = ro->H;
-    const size_t Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U, E = ro->dyn.E;
-    TgWs T; RoWs& L = T.b; size_t o = 0;
-    auto take = [&](size_t len) { size_t at = o; o += (H * R * len + 1) & ~(size_t)1; return at; };
-    L.mj = take(D); L.sj = take(D * D);
-    L.Md = take(E); L.Sd = take(E * E); L.Vd = take(D * E);
-    L.Mp = take(U); L.Sp = take(U * U); L.Vp = take(Dh * U);
-    L.Mu = take(U); L.Su = take(U * U); L.Cq = take(U * U); L.Vu = take(Dh * U);
-    L.risk = take(1); L.rew = take(1);
-    T.mh = take(Dh); T.Sh = take(Dh * Dh); T.Ch = take(E * Dh); T.cx = take(E * D);
-    L.dynws = o; o += pilco_mm_workspace_bytes(ro->dyn.n, ro->dyn.D, ro->dyn.E, ro->R) / 8;
-    L.polws = o;
-    if (ro->pol.kind == PILCO_POLICY_RBF)
-        o += pilco_mm_workspace_bytes(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, ro->R) / 8;
-    L.total = T.total = o;
-    return T;
-}
 static inline int ro_count_mult(const pilco_rollout* ro) {
     int c = 0;
     for (int k = 0; k < ro->n_rewards; ++k) c += ro->rewards[k].channel == PILCO_CHANNEL_MULT;
     return c;
 }
 
-// ---- measurement noise at the policy's input (pilco_rollout_noisy_*, rollout_noise.cu) ----
-// The angle cascade (A >= 0; with A = 0 phi is the identity) whose policy reads the moments (m^_z, S^_z) of phi under
-// N(m, S + diag(var)), kept per step after the angle layout (and before the exploration slot, when there is one).
-struct NzFwd {
-    double var[MAXD];         // noise variance of each raw state dimension
-    size_t mz, Sz;            // offsets in doubles in ro->ws: [H][R][Dh], [H][R][Dh][Dh]
-};
-
-// the angle layout, then the noisy moments; `total` is where an exploration slot would go
-static inline NzFwd nz_ws_layout(const pilco_rollout* ro, size_t* total) {
-    const size_t R = ro->R, H = ro->H, Dh = ro->pol.Ds;
-    NzFwd L;
-    size_t o = tg_ws_layout(ro).total;
-    auto take = [&](size_t len) { size_t at = o; o += (H * R * len + 1) & ~(size_t)1; return at; };
-    L.mz = take(Dh); L.Sz = take(Dh * Dh);
-    *total = o;
-    return L;
-}
-
-// the per-step state kernel of the noisy cascade (in place of tg_state): glue as tg_state, then both feature-moment
-// sets, the linear policy at the noisy one, squash, the joint and cx at the true one; mz / Sz the slots of step t
-int nz_state_launch(const TgDev& g, const NzFwd& nz, double* mz, double* Sz, cudaStream_t st);
+// the per-step state kernel of the noisy cascade (rollout_noise.cu; in place of tg_state): glue as tg_state, then both
+// feature-moment sets, the linear policy at the noisy one, squash, the joint and cx at the true one; var the noise
+// variances [MAXD], mz / Sz the slots of step t
+int nz_state_launch(const TgDev& g, const double* var, double* mz, double* Sz, cudaStream_t st);
+// the exploration objective's forward launches (rollout_explore.cu), after the reward launches in place of
+// ro_reward_sum: ro_reward_var with the state terms' ds (state dimension ds.Ds) and, when dj is non-NULL,
+// ro_reward_joint_var with the joint terms' dj (dimension dj->Ds + dj->U; dj->mj, dj->sj the joint Gaussians of step
+// 0), into sigma_t^2 var [H][R]; then ro_reward_explore_sum with step_var [R][H] if set
+int ex_reward_var_launch(const RoDev& ds, const RoDev* dj, double b, double* var, double* step_var, cudaStream_t st);

@@ -1,14 +1,10 @@
-// rollout_angles_bwd.cu -- reverse sweep of the H-step cascade with angular state dimensions
-// (pilco_rollout_angles_backward).  A translation unit of its own, so that the kernels of rollout_bwd.cu compile
-// exactly as they do without it.
+// rollout_angles_bwd.cu -- the per-step kernels of the reverse sweep on phi (angular state dimensions or measurement
+// noise; the sweep itself is rollout_bwd.cu's).  A translation unit of its own, so that the kernels of rollout_bwd.cu
+// compile exactly as they do without it.
 #include "mm_backward.cuh"
 #include "mm_tape.cuh"
 #include "rollout_bwd.cuh"
 #include "small_kernels.cuh"
-
-extern "C" size_t pilco_mm_bwd_workspace_bytes(int n, int D, int E, int R, int need_param);
-void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
-                           const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
 
 // ---------------------------------------------------------------------------------------------
 // Reverse sweep with angular state dimensions (pilco_rollout_angles_backward).  (gm, gS) is the cotangent of the raw
@@ -22,34 +18,6 @@ void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, i
 //   tg_trig: dev_trig_bwd into (gm, gS), the state reward gradients, and the seeds gV, gcx of step t-1 (a kernel of
 //            its own: folded into tg_post it made that kernel spill)
 // ---------------------------------------------------------------------------------------------
-struct TbWs {            // offsets in doubles
-    size_t gm, gS, gVd, gcx, gmj, gsj, gMp, gSp, gVp, gmh, gSh, gCh, gbeta, gy, rgm, rgS, jgm, jgS, cnt, dynb, polb, total;
-};
-
-static TbWs tb_ws_layout(const pilco_rollout* ro) {
-    const size_t R = ro->R, H = ro->H, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U, Ds = ro->dyn.E;
-    TbWs L; size_t o = 0;
-    auto take = [&](size_t len) { size_t at = o; o += (R * len + 1) & ~(size_t)1; return at; };
-    L.gm = take(Ds); L.gS = take(Ds * Ds); L.gVd = take(D * Ds); L.gcx = take(Ds * D);
-    L.gmj = take(D); L.gsj = take(D * D);
-    L.gMp = take(U); L.gSp = take(U * U); L.gVp = take(Dh * U);
-    L.gmh = take(Dh); L.gSh = take(Dh * Dh); L.gCh = take(Ds * Dh);
-    const size_t bf = ro->pol.kind == PILCO_POLICY_RBF ? ro->pol.rbf.n : 0;
-    L.gbeta = take(U * bf); L.gy = take(U * bf);
-    L.rgm = take(H * 2 * Ds); L.rgS = take(H * 2 * Ds * Ds);
-    const size_t Hj = rb_has_joint(ro) ? H : 0;
-    L.jgm = take(Hj * 2 * D); L.jgS = take(Hj * 2 * D * D);
-    L.cnt = take(1);
-    L.dynb = o;
-    if (ro->tape) o += ((size_t)ro->R * mm_tape_bwd_part_doubles(ro->dyn.D, ro->dyn.E) + 1) & ~(size_t)1;
-    else o += pilco_mm_bwd_workspace_bytes(ro->dyn.n, ro->dyn.D, ro->dyn.E, ro->R, 0) / 8;
-    L.polb = o;
-    if (ro->pol.kind == PILCO_POLICY_RBF)
-        o += pilco_mm_bwd_workspace_bytes(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, ro->R, 1) / 8;
-    L.total = o;
-    return L;
-}
-
 struct TbPostSmem { SmallScratch sc; double gMu[MAXD], gSu[MAXD * MAXD], gVu[MAXD * MAXD], gB[MAXD * MAXD], gCd[MAXD],
                     gQ[MAXD * MAXD]; };
 
@@ -232,181 +200,19 @@ static int launch_tg_dyn_finish(const MMTapeBwd& tb, const TbDev& g, cudaStream_
     return PILCO_OK;
 }
 
-extern "C" {
-
-size_t pilco_rollout_angles_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang) {
-    if (!ang || ang->A == 0) return pilco_rollout_bwd_workspace_bytes(ro);
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    return tb_ws_layout(ro).total * sizeof(double);
-}
-
-}  // extern "C"
-
-// with measurement noise: the angle layout, then the cotangent of the noisy moments (gm^_z [R][Dh], gS^_z [R][Dh][Dh])
-static size_t nz_bwd_layout(const pilco_rollout* ro, size_t* gmz, size_t* gSz) {
-    const size_t R = ro->R, Dh = ro->pol.Ds;
-    size_t o = tb_ws_layout(ro).total;
-    *gmz = o; o += (R * Dh + 1) & ~(size_t)1;
-    *gSz = o; o += (R * Dh * Dh + 1) & ~(size_t)1;
-    return o;
-}
-
-size_t nz_bwd_ws_doubles(const pilco_rollout* ro) {
-    size_t a, b;
-    return nz_bwd_layout(ro, &a, &b);
-}
-
-int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
-                    const void* ctx, cudaStream_t stream, const NzFwd* nz) {
-    TrigMap tm;
-    int rc = tg_check(ro, ang, &tm);
-    if (rc) return rc;
-    if (tm.A == 0 && !nz) return rb_backward_impl(ro, g, hook, ctx, stream);
-    if (tm.A == 0) trig_map_make(ro->dyn.E, 0, nullptr, &tm);      // measurement noise without angles: phi = identity
-    if (!g || !g->ws) return PILCO_ERR_NULL;
-    const TgWs FT = tg_ws_layout(ro);
-    const RoWs& FL = FT.b;
-    const TbWs BL = tb_ws_layout(ro);
-    size_t o_gmz = 0, o_gSz = 0;
-    const size_t need = nz ? nz_bwd_layout(ro, &o_gmz, &o_gSz) : BL.total;
-    if (g->ws_bytes < need * sizeof(double)) return PILCO_ERR_WORKSPACE;
-    if (((uintptr_t)g->ws) & 15) return PILCO_ERR_ALIGN;
-    const int R = ro->R, H = ro->H, Ds = tm.Ds, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U;
-    const bool rbf = ro->pol.kind == PILCO_POLICY_RBF;
-    if (rbf) { if (!g->gXc || !g->gYc || !g->gell || !g->pol_L) return PILCO_ERR_NULL; }
-    else { if (!g->gW || !g->gb) return PILCO_ERR_NULL; }
-    cudaStream_t st = (cudaStream_t)stream;
-    double* fws = (double*)ro->ws;
-    double* bws = (double*)g->ws;
-    const size_t RR = (size_t)R;
-    auto slot = [&](size_t base, size_t len, int t) { return fws + base + (size_t)t * RR * len; };
-    auto buf = [&](size_t base) { return bws + base; };
-
-    // zero the state cotangent and the seeds of step H-1, the counters and the parameter-gradient accumulators
-    cudaMemsetAsync(buf(BL.gm), 0, sizeof(double) * (BL.gmj - BL.gm), st);
-    cudaMemsetAsync(buf(BL.cnt), 0, sizeof(double) * (BL.dynb - BL.cnt), st);
-    const int bf = rbf ? ro->pol.rbf.n : 0;
-    if (rbf) {
-        cudaMemsetAsync(g->gXc, 0, sizeof(double) * RR * bf * Dh, st);
-        cudaMemsetAsync(g->gell, 0, sizeof(double) * RR * U * Dh, st);
-        cudaMemsetAsync(buf(BL.gbeta), 0, sizeof(double) * RR * U * bf, st);
+int tg_post_launch(const TbDev& g, const MMTapeBwd* tb, cudaStream_t st) {
+    if (tb) {
+        const int rc = ks_dispatch(g.p.Ds + g.p.U, [&](auto ks) { return launch_tg_dyn_finish<4 * ks>(*tb, g, st); });
+        if (rc) return rc;
     } else {
-        cudaMemsetAsync(g->gW, 0, sizeof(double) * RR * U * Dh, st);
-        cudaMemsetAsync(g->gb, 0, sizeof(double) * RR * U, st);
+        launch_hi(tg_post_kernel, dim3(g.p.R), dim3(128), sizeof(TbPostSmem), st, g);
     }
-    if (nz) cudaMemsetAsync(buf(o_gmz), 0, sizeof(double) * (need - o_gmz), st);     // nz_trig re-zeroes after each step
-    if (!ro->tape) mm_bwd_zero_counters(mm_bws_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, 0), bws + BL.dynb, R, st);
-    if (rbf) mm_bwd_zero_counters(mm_bws_layout(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, 1), bws + BL.polb, R, st);
-
-    TbDev tg;
-    tg.tm = tm;
-    RbDev& d = tg.p;
-    d.R = R; d.H = H; d.Ds = Dh; d.U = U;
-    d.pol_kind = ro->pol.kind; d.squash = ro->pol.squash; d.maxa = ro->pol.max_action;
-    d.W = ro->pol.W; d.W_bs = ro->pol.W_bs;
-    int n_joint = 0;
-    pilco_reward_term joint_terms[8];
-    d.n_rewards = 0;
-    for (int k = 0; k < 8; ++k) d.rewards[k] = joint_terms[k] = pilco_reward_term();
-    for (int k = 0; k < ro->n_rewards; ++k) {
-        if (reward_on_joint(ro->rewards[k].kind)) joint_terms[n_joint++] = ro->rewards[k];
-        else d.rewards[d.n_rewards++] = ro->rewards[k];
-    }
-    d.traj_m = ro->traj_m; d.traj_S = ro->traj_S;
-    d.risk = fws + FL.risk; d.mult_mu = ro_count_mult(ro) > 0 ? ro->mult_mu : 0.0;
-    d.gm = buf(BL.gm); d.gS = buf(BL.gS); d.gMd = d.gSd = d.gVd = nullptr;
-    d.gmj = buf(BL.gmj); d.gsj = buf(BL.gsj); d.gsjx = nullptr;
-    d.gMp = buf(BL.gMp); d.gSp = buf(BL.gSp); d.gVp = buf(BL.gVp);
-    d.gW = g->gW; d.gb = g->gb;
-    d.rgm = buf(BL.rgm); d.rgS = buf(BL.rgS);
-    const bool joint = rb_has_joint(ro);
-    d.jgm = joint ? buf(BL.jgm) : nullptr; d.jgS = joint ? buf(BL.jgS) : nullptr;
-    d.mj0 = fws + FL.mj; d.sj0 = fws + FL.sj;
-    d.tpart = ro->tape ? bws + BL.dynb : nullptr;
-    d.tp_ntask = ro->dyn.E + npairs_of(ro->dyn.E);
-    d.cnt = reinterpret_cast<unsigned*>(buf(BL.cnt));
-    d.t = 0;
-    tg.gVd = buf(BL.gVd); tg.gcx = buf(BL.gcx); tg.gmh = buf(BL.gmh); tg.gSh = buf(BL.gSh); tg.gCh = buf(BL.gCh);
-    double* gmz = nz ? buf(o_gmz) : nullptr;
-    double* gSz = nz ? buf(o_gSz) : nullptr;
-    if (H > 0) {
-        d.sj = d.Vd = d.Mp = d.Sp = d.Vp = d.Mu = d.Su = d.Cq = d.Vu = nullptr;
-        RbDev ds = d;                                 // the state terms at the raw trajectory
-        ds.Ds = Ds;
-        RbDev dj = d;                                 // the joint terms at [phi, u]: D = Dh + U
-        dj.n_rewards = n_joint;
-        for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
-        rc = rb_reward_launch(ds, joint ? &dj : nullptr, st);
-        if (rc) return rc;
-        if (hook) {
-            rc = hook(ds, joint ? &dj : nullptr, st, ctx);
-            if (rc) return rc;
-        }
-    }
-
-    for (int t = H - 1; t >= 0; --t) {
-        d.t = t;
-        d.sj = slot(FL.sj, (size_t)D * D, t); d.Vd = slot(FL.Vd, (size_t)D * Ds, t);
-        d.Mp = slot(FL.Mp, U, t); d.Sp = slot(FL.Sp, (size_t)U * U, t); d.Vp = slot(FL.Vp, (size_t)Dh * U, t);
-        d.Mu = slot(FL.Mu, U, t); d.Su = slot(FL.Su, (size_t)U * U, t); d.Cq = slot(FL.Cq, (size_t)U * U, t);
-        d.Vu = slot(FL.Vu, (size_t)Dh * U, t);
-        tg.mh = slot(FT.mh, Dh, t); tg.Sh = slot(FT.Sh, (size_t)Dh * Dh, t); tg.Ch = slot(FT.Ch, (size_t)Ds * Dh, t);
-        tg.cx = slot(FT.cx, (size_t)Ds * D, t);
-        tg.cx_prev = t > 0 ? slot(FT.cx, (size_t)Ds * D, t - 1) : nullptr;
-        tg.Vd_prev = t > 0 ? slot(FL.Vd, (size_t)D * Ds, t - 1) : nullptr;
-        TbDev tp = tg;                                // with noise, the post stage stops before the linear-policy VJP,
-        if (nz) tp.p.pol_kind = -1;                   // which nz_trig runs at the noisy moments
-        if (ro->tape) {
-            const MMTapeL TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
-            const MMTapeBwd tb = mm_tape_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t),
-                                                    (long long)D * D, slot(FL.Md, Ds, t), d.gm, d.gS, tg.gVd,
-                                                    (const double*)ro->tape + (size_t)t * RR * TL.per_r, TL,
-                                                    bws + BL.dynb, d.gmj, D, d.gsj, (long long)D * D);
-            rc = ks_dispatch(D, [&](auto ks) { return launch_tg_dyn_finish<4 * ks>(tb, tp, st); });
-            if (rc) return rc;
-            CUDA_LAUNCH_CHECK();
-        } else {
-            MMBwdParams bp = mm_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t), (long long)D * D,
-                                           slot(FL.Md, Ds, t), d.gm, d.gS, tg.gVd,
-                                           d.gmj, D, d.gsj, (long long)D * D, nullptr, nullptr, nullptr, 0, bws + BL.dynb);
-            rc = mm_backward_launch(bp, st);
-            if (rc) return rc;
-            launch_hi(tg_post_kernel, dim3(R), dim3(128), sizeof(TbPostSmem), st, tp);
-            CUDA_LAUNCH_CHECK();
-        }
-        const double* mz = nz ? slot(nz->mz, Dh, t) : nullptr;
-        const double* Sz = nz ? slot(nz->Sz, (size_t)Dh * Dh, t) : nullptr;
-        if (rbf) {                                    // the policy's input: the feature moments (the noisy ones with nz)
-            MMBwdParams pp = mm_bwd_params(&ro->pol.rbf, R, nz ? mz : tg.mh, Dh, nz ? Sz : tg.Sh, (long long)Dh * Dh,
-                                           slot(FL.Mp, U, t), d.gMp, d.gSp, d.gVp,
-                                           nz ? gmz : tg.gmh, Dh, nz ? gSz : tg.gSh, (long long)Dh * Dh,
-                                           g->gXc, buf(BL.gbeta), g->gell, 1, bws + BL.polb);
-            rc = mm_backward_launch(pp, st);
-            if (rc) return rc;
-        }
-        if (nz) {
-            rc = nz_trig_launch(tg, *nz, mz, Sz, gmz, gSz, st);
-            if (rc) return rc;
-        } else {
-            launch_hi(tg_trig_kernel, dim3(R), dim3(128), 0, st, tg);
-            CUDA_LAUNCH_CHECK();
-        }
-    }
-    if (rbf) {
-        const int ldw = pad64(bf);
-        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              buf(BL.gbeta), (long long)U * bf, bf, 1, buf(BL.gy), bf);
-        rc = rbf_factor_bwd_launch(st, R, bf, Dh, U, ro->pol.rbf.X, (long long)bf * Dh, ro->pol.rbf.ell, (long long)U * Dh,
-                                   ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs, ro->pol.rbf.beta, (long long)U * bf,
-                                   buf(BL.gy), g->gXc, g->gYc, g->gell);
-        if (rc) return rc;
-    }
-    if (g->gm0) cudaMemcpyAsync(g->gm0, d.gm, sizeof(double) * RR * Ds, cudaMemcpyDeviceToDevice, st);
-    if (g->gS0) cudaMemcpyAsync(g->gS0, d.gS, sizeof(double) * RR * Ds * Ds, cudaMemcpyDeviceToDevice, st);
+    CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
 
-extern "C" int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
-                                             pilco_stream_t stream) {
-    return rb_backward_run(ro, ang, g, nullptr, nullptr, (cudaStream_t)stream);
+int tg_trig_launch(const TbDev& g, cudaStream_t st) {
+    launch_hi(tg_trig_kernel, dim3(g.p.R), dim3(128), 0, st, g);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
 }

@@ -27,18 +27,25 @@ void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, i
                            const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
 
 struct RbWs {            // backward workspace (offsets in doubles)
-    size_t gm, gS, gMd, gSd, gVd, gmj, gsj, gsjx, gMp, gSp, gVp, gbeta, gy, rgm, rgS, jgm, jgS, cnt, dynb, polb, total;
+    size_t gm, gS, gMd, gSd, gVd, gcx, gmj, gsj, gsjx, gMp, gSp, gVp, gmh, gSh, gCh, gbeta, gy, rgm, rgS, jgm, jgS, cnt,
+           dynb, polb, gmz, gSz, total;
 };
 
-
-static RbWs rb_ws_layout(const pilco_rollout* ro) {
-    const size_t R = ro->R, H = ro->H, Ds = ro->pol.Ds, U = ro->pol.U, D = Ds + U;
+// Dh = pol.Ds, Ds = dyn.E on phi (pol.Ds without).  Without phi the seeds of the dynamics VJP (gMd, gSd, gVd) and the
+// glue's joint cotangent gsjx have slots of their own (rb_pre); on phi gVd and gcx are the seeds tg_trig leaves and
+// (gmh, gSh, gCh) the feature cotangent; with noise (gmz, gSz) the cotangent of the noisy moments.  A slot whose
+// feature is off has length 0.
+static RbWs rb_ws_layout(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz) {
+    const bool phi = ro_on_phi(ang, nz);
+    const size_t R = ro->R, H = ro->H, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U, Ds = phi ? (size_t)ro->dyn.E : Dh;
+    const size_t F = phi ? 1 : 0, P = 1 - F, N = nz ? 1 : 0;
     RbWs L; size_t o = 0;
     auto take = [&](size_t len) { size_t at = o; o += (R * len + 1) & ~(size_t)1; return at; };
     L.gm = take(Ds); L.gS = take(Ds * Ds);
-    L.gMd = take(Ds); L.gSd = take(Ds * Ds); L.gVd = take(D * Ds);
-    L.gmj = take(D); L.gsj = take(D * D); L.gsjx = take(D * D);
-    L.gMp = take(U); L.gSp = take(U * U); L.gVp = take(Ds * U);
+    L.gMd = take(P * Ds); L.gSd = take(P * Ds * Ds); L.gVd = take(D * Ds); L.gcx = take(F * Ds * D);
+    L.gmj = take(D); L.gsj = take(D * D); L.gsjx = take(P * D * D);
+    L.gMp = take(U); L.gSp = take(U * U); L.gVp = take(Dh * U);
+    L.gmh = take(F * Dh); L.gSh = take(F * Dh * Dh); L.gCh = take(F * Ds * Dh);
     const size_t bf = ro->pol.kind == PILCO_POLICY_RBF ? ro->pol.rbf.n : 0;
     L.gbeta = take(U * bf); L.gy = take(U * bf);
     // reward gradients of every step, per channel (0: additive, 1: multiplicative): [H][2][R][Ds], [H][2][R][Ds*Ds]
@@ -54,10 +61,10 @@ static RbWs rb_ws_layout(const pilco_rollout* ro) {
     L.polb = o;
     if (ro->pol.kind == PILCO_POLICY_RBF)
         o += pilco_mm_bwd_workspace_bytes(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, ro->R, 1) / 8;
+    L.gmz = take(N * Dh); L.gSz = take(N * Dh * Dh);
     L.total = o;
     return L;
 }
-
 
 // shared-memory scratch of rb_post_body (bytes), carved from a dynamic buffer
 struct RbPostSmem { SmallScratch sc; double gMu[MAXD], gSu[MAXD * MAXD], gVu[MAXD * MAXD], gB[MAXD * MAXD], gCd[MAXD], gsjx[MAXD * MAXD]; };
@@ -328,8 +335,6 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
     return PILCO_OK;
 }
 
-// rb_reward_kernel (state terms of d, at dimension ds.Ds) and, when dj is non-NULL, rb_reward_joint_kernel (joint terms, at
-// dimension dj->Ds + dj->U) for callers in other translation units (the reverse sweep with angles, rollout_angles_bwd.cu)
 int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st) {
     launch_hi(rb_reward_kernel, dim3(ds.R, ds.H), dim3(128), 0, st, ds);
     CUDA_LAUNCH_CHECK();
@@ -340,64 +345,67 @@ int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st) {
     return PILCO_OK;
 }
 
-extern "C" {
-
-size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro) {
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    return rb_ws_layout(ro).total * sizeof(double);
+// rb_post for step d.t: with a tape (tb) fused into rb_dyn_finish, the tape-driven dynamics VJP, else a launch of its own
+static int rb_post_launch(const RbDev& d, const MMTapeBwd* tb, cudaStream_t st) {
+    if (tb) {
+        const int rc = ks_dispatch(d.Ds + d.U, [&](auto ks) { return launch_dyn_finish<4 * ks>(*tb, d, st); });
+        if (rc) return rc;
+    } else {
+        launch_hi(rb_post_kernel, dim3(d.R), dim3(128), sizeof(RbPostSmem), st, d);
+    }
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
 }
 
-}  // extern "C"
-
-int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRewardHook hook, const void* ctx,
-                     cudaStream_t stream) {
-    int rc = ro_check(ro);
+// The reverse sweep of every call (ang, ex, nz may be NULL).  Per step the post stage is rb_post (rb_pre before the
+// recomputing dynamics VJP) or tg_post on phi, which with noise stops before the linear-policy VJP; the policy GP's
+// VJP reads x_t, phi's moments or the noisy ones; the trig stage (on phi) is tg_trig or, with noise, nz_trig.
+static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                       const pilco_obs_noise* nz, const pilco_rollout_grad* g, cudaStream_t st) {
+    RoOpt o;
+    int rc = ro_validate(ro, ang, ex, nz, true, &o);
     if (rc) return rc;
     if (!g || !g->ws) return PILCO_ERR_NULL;
-    const RoWs FL = ro_ws_layout(ro);
-    const RbWs BL = rb_ws_layout(ro);
+    const RbWs BL = rb_ws_layout(ro, ang, nz);
     if (g->ws_bytes < BL.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
     if (((uintptr_t)g->ws) & 15) return PILCO_ERR_ALIGN;
-    const int R = ro->R, H = ro->H, Ds = ro->pol.Ds, U = ro->pol.U, D = Ds + U;
+    const int R = ro->R, H = ro->H, Ds = ro->dyn.E, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U;
     const bool rbf = ro->pol.kind == PILCO_POLICY_RBF;
     if (rbf) { if (!g->gXc || !g->gYc || !g->gell || !g->pol_L) return PILCO_ERR_NULL; }
     else { if (!g->gW || !g->gb) return PILCO_ERR_NULL; }
-    cudaStream_t st = (cudaStream_t)stream;
+    const RoWs FL = ro_ws_layout(ro, ang, ex, nz);
     double* fws = (double*)ro->ws;
     double* bws = (double*)g->ws;
     const size_t RR = (size_t)R;
     auto slot = [&](size_t base, size_t len, int t) { return fws + base + (size_t)t * RR * len; };
     auto buf = [&](size_t base) { return bws + base; };
 
-    // zero the state cotangent and the parameter-gradient accumulators (and the arrival counters)
-    cudaMemsetAsync(buf(BL.gm), 0, sizeof(double) * ((BL.gMd - BL.gm)), st);
+    // zero the state cotangent (on phi with the seeds of step H-1), the parameter-gradient accumulators and the arrival
+    // counters
+    cudaMemsetAsync(buf(BL.gm), 0, sizeof(double) * ((o.phi ? BL.gmj : BL.gMd) - BL.gm), st);
     cudaMemsetAsync(buf(BL.cnt), 0, sizeof(double) * (BL.dynb - BL.cnt), st);
     const int bf = rbf ? ro->pol.rbf.n : 0;
     if (rbf) {
-        cudaMemsetAsync(g->gXc, 0, sizeof(double) * RR * bf * Ds, st);
-        cudaMemsetAsync(g->gell, 0, sizeof(double) * RR * U * Ds, st);
+        cudaMemsetAsync(g->gXc, 0, sizeof(double) * RR * bf * Dh, st);
+        cudaMemsetAsync(g->gell, 0, sizeof(double) * RR * U * Dh, st);
         cudaMemsetAsync(buf(BL.gbeta), 0, sizeof(double) * RR * U * bf, st);
     } else {
-        cudaMemsetAsync(g->gW, 0, sizeof(double) * RR * U * Ds, st);
+        cudaMemsetAsync(g->gW, 0, sizeof(double) * RR * U * Dh, st);
         cudaMemsetAsync(g->gb, 0, sizeof(double) * RR * U, st);
     }
-
+    if (o.noise) cudaMemsetAsync(buf(BL.gmz), 0, sizeof(double) * (BL.total - BL.gmz), st);   // nz_trig re-zeroes
     // arrival counters of the finish kernels (self-cleaning afterwards): zero once per reverse sweep
     if (!ro->tape) mm_bwd_zero_counters(mm_bws_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, 0), bws + BL.dynb, R, st);
     if (rbf) mm_bwd_zero_counters(mm_bws_layout(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, 1), bws + BL.polb, R, st);
 
-    RbDev d;
-    d.R = R; d.H = H; d.Ds = Ds; d.U = U;
+    TbDev tg;
+    tg.tm = o.tm;
+    RbDev& d = tg.p;
+    d.R = R; d.H = H; d.Ds = Dh; d.U = U;
     d.pol_kind = ro->pol.kind; d.squash = ro->pol.squash; d.maxa = ro->pol.max_action;
     d.W = ro->pol.W; d.W_bs = ro->pol.W_bs;
-    int n_joint = 0;                                  // the state terms go to rb_reward, the joint ones to rb_reward_joint
     pilco_reward_term joint_terms[8];
-    d.n_rewards = 0;
-    for (int k = 0; k < 8; ++k) d.rewards[k] = joint_terms[k] = pilco_reward_term();
-    for (int k = 0; k < ro->n_rewards; ++k) {
-        if (reward_on_joint(ro->rewards[k].kind)) joint_terms[n_joint++] = ro->rewards[k];
-        else d.rewards[d.n_rewards++] = ro->rewards[k];
-    }
+    const int n_joint = ro_split_rewards(ro, &d.n_rewards, d.rewards, joint_terms);
     d.traj_m = ro->traj_m; d.traj_S = ro->traj_S;
     d.risk = fws + FL.risk; d.mult_mu = ro_count_mult(ro) > 0 ? ro->mult_mu : 0.0;
     d.gm = buf(BL.gm); d.gS = buf(BL.gS); d.gMd = buf(BL.gMd); d.gSd = buf(BL.gSd); d.gVd = buf(BL.gVd);
@@ -405,26 +413,27 @@ int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRew
     d.gMp = buf(BL.gMp); d.gSp = buf(BL.gSp); d.gVp = buf(BL.gVp);
     d.gW = g->gW; d.gb = g->gb;
     d.rgm = buf(BL.rgm); d.rgS = buf(BL.rgS);
-    const bool joint = rb_has_joint(ro);
+    const bool joint = n_joint > 0;
     d.jgm = joint ? buf(BL.jgm) : nullptr; d.jgS = joint ? buf(BL.jgS) : nullptr;
     d.mj0 = fws + FL.mj; d.sj0 = fws + FL.sj;
     d.tpart = ro->tape ? bws + BL.dynb : nullptr;
     d.tp_ntask = ro->dyn.E + npairs_of(ro->dyn.E);
     d.cnt = reinterpret_cast<unsigned*>(buf(BL.cnt));
     d.t = 0;
-    if (H > 0) {
+    tg.gVd = d.gVd; tg.gcx = buf(BL.gcx); tg.gmh = buf(BL.gmh); tg.gSh = buf(BL.gSh); tg.gCh = buf(BL.gCh);
+    double* gmz = buf(BL.gmz);
+    double* gSz = buf(BL.gSz);
+    if (H > 0) {                                      // reward gradients of every step at once
         d.sj = d.Vd = d.Mp = d.Sp = d.Vp = d.Mu = d.Su = d.Cq = d.Vu = nullptr;
-        launch_hi(rb_reward_kernel, dim3(R, H), dim3(128), 0, st, d);     // reward gradients of every step at once
-        CUDA_LAUNCH_CHECK();
-        RbDev dj = d;
+        RbDev ds = d;                                 // the state terms at the raw trajectory
+        ds.Ds = Ds;
+        RbDev dj = d;                                 // the joint terms at [phi, u]: D = Dh + U
         dj.n_rewards = n_joint;
         for (int k = 0; k < 8; ++k) dj.rewards[k] = joint_terms[k];
-        if (joint) {
-            launch_hi(rb_reward_joint_kernel, dim3(R, H), dim3(128), 0, st, dj);
-            CUDA_LAUNCH_CHECK();
-        }
-        if (hook) {
-            rc = hook(d, joint ? &dj : nullptr, st, ctx);
+        rc = rb_reward_launch(ds, joint ? &dj : nullptr, st);
+        if (rc) return rc;
+        if (o.explore && o.b != 0.0) {
+            rc = rb_reward_var_launch(ds, joint ? &dj : nullptr, o.b, fws + FL.var, st);
             if (rc) return rc;
         }
     }
@@ -432,57 +441,116 @@ int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRew
     for (int t = H - 1; t >= 0; --t) {
         d.t = t;
         d.sj = slot(FL.sj, (size_t)D * D, t); d.Vd = slot(FL.Vd, (size_t)D * Ds, t);
-        d.Mp = slot(FL.Mp, U, t); d.Sp = slot(FL.Sp, (size_t)U * U, t); d.Vp = slot(FL.Vp, (size_t)Ds * U, t);
+        d.Mp = slot(FL.Mp, U, t); d.Sp = slot(FL.Sp, (size_t)U * U, t); d.Vp = slot(FL.Vp, (size_t)Dh * U, t);
         d.Mu = slot(FL.Mu, U, t); d.Su = slot(FL.Su, (size_t)U * U, t); d.Cq = slot(FL.Cq, (size_t)U * U, t);
-        d.Vu = slot(FL.Vu, (size_t)Ds * U, t);
+        d.Vu = slot(FL.Vu, (size_t)Dh * U, t);
+        tg.mh = slot(FL.mh, Dh, t); tg.Sh = slot(FL.Sh, (size_t)Dh * Dh, t); tg.Ch = slot(FL.Ch, (size_t)Ds * Dh, t);
+        tg.cx = slot(FL.cx, (size_t)Ds * D, t);
+        tg.cx_prev = t > 0 ? slot(FL.cx, (size_t)Ds * D, t - 1) : nullptr;
+        tg.Vd_prev = t > 0 ? slot(FL.Vd, (size_t)D * Ds, t - 1) : nullptr;
+        TbDev tp = tg;                                // with noise, the post stage stops before the linear-policy VJP,
+        if (o.noise) tp.p.pol_kind = -1;              // which nz_trig runs at the noisy moments
         if (ro->tape) {                              // consume the tape of step t: no exponential is recomputed
-            // seeds straight from the state cotangent (gV = s1'(gS+gS') inline); tape slot (t, :)
+            // seeds straight from the state cotangent (without phi gV = s1'(gS+gS') inline); tape slot (t, :)
             const MMTapeL TL = mm_tape_layout(ro->dyn.n, ro->dyn.D, ro->dyn.E, R);
             const MMTapeBwd tb = mm_tape_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t),
-                                                    (long long)D * D, slot(FL.Md, Ds, t), d.gm, d.gS, nullptr,
+                                                    (long long)D * D, slot(FL.Md, Ds, t), d.gm, d.gS,
+                                                    o.phi ? tg.gVd : nullptr,
                                                     (const double*)ro->tape + (size_t)t * RR * TL.per_r, TL,
                                                     bws + BL.dynb, d.gmj, D, d.gsj, (long long)D * D);
-            rc = ks_dispatch(D, [&](auto ks) { return launch_dyn_finish<4 * ks>(tb, d, st); });
+            rc = o.phi ? tg_post_launch(tp, &tb, st) : rb_post_launch(d, &tb, st);
             if (rc) return rc;
-            CUDA_LAUNCH_CHECK();
         } else {
-            launch_hi(rb_pre_kernel, dim3(R), dim3(128), 0, st, d);
-            CUDA_LAUNCH_CHECK();
+            if (!o.phi) {
+                launch_hi(rb_pre_kernel, dim3(R), dim3(128), 0, st, d);
+                CUDA_LAUNCH_CHECK();
+            }
             MMBwdParams bp = mm_bwd_params(&ro->dyn, R, slot(FL.mj, D, t), D, slot(FL.sj, (size_t)D * D, t), (long long)D * D,
-                                           slot(FL.Md, Ds, t), d.gMd, d.gSd, d.gVd,
+                                           slot(FL.Md, Ds, t), o.phi ? d.gm : d.gMd, o.phi ? d.gS : d.gSd, d.gVd,
                                            d.gmj, D, d.gsj, (long long)D * D, nullptr, nullptr, nullptr, 0, bws + BL.dynb);
             rc = mm_backward_launch(bp, st);
             if (rc) return rc;
-            launch_hi(rb_post_kernel, dim3(R), dim3(128), sizeof(RbPostSmem), st, d);
-            CUDA_LAUNCH_CHECK();
+            rc = o.phi ? tg_post_launch(tp, nullptr, st) : rb_post_launch(d, nullptr, st);
+            if (rc) return rc;
         }
-        if (rbf) {
-            MMBwdParams pp = mm_bwd_params(&ro->pol.rbf, R, ro->traj_m + (size_t)t * Ds, (long long)(H + 1) * Ds,
-                                           ro->traj_S + (size_t)t * Ds * Ds, (long long)(H + 1) * Ds * Ds,
-                                           slot(FL.Mp, U, t), d.gMp, d.gSp, d.gVp,
-                                           d.gm, Ds, d.gS, (long long)Ds * Ds,
-                                           g->gXc, buf(BL.gbeta), g->gell, 1, bws + BL.polb);
+        const double* mz = slot(FL.mz, Dh, t);
+        const double* Sz = slot(FL.Sz, (size_t)Dh * Dh, t);
+        if (rbf) {                                    // the policy's input: x_t, or phi's moments (the noisy ones)
+            MMBwdParams pp = o.phi ? mm_bwd_params(&ro->pol.rbf, R, o.noise ? mz : tg.mh, Dh, o.noise ? Sz : tg.Sh,
+                                                   (long long)Dh * Dh, slot(FL.Mp, U, t), d.gMp, d.gSp, d.gVp,
+                                                   o.noise ? gmz : tg.gmh, Dh, o.noise ? gSz : tg.gSh, (long long)Dh * Dh,
+                                                   g->gXc, buf(BL.gbeta), g->gell, 1, bws + BL.polb)
+                                   : mm_bwd_params(&ro->pol.rbf, R, ro->traj_m + (size_t)t * Ds, (long long)(H + 1) * Ds,
+                                                   ro->traj_S + (size_t)t * Ds * Ds, (long long)(H + 1) * Ds * Ds,
+                                                   slot(FL.Mp, U, t), d.gMp, d.gSp, d.gVp,
+                                                   d.gm, Dh, d.gS, (long long)Dh * Dh,
+                                                   g->gXc, buf(BL.gbeta), g->gell, 1, bws + BL.polb);
             rc = mm_backward_launch(pp, st);
             if (rc) return rc;
         }
+        if (o.noise) rc = nz_trig_launch(tg, o.nzvar, mz, Sz, gmz, gSz, st);
+        else if (o.phi) rc = tg_trig_launch(tg, st);
+        if (rc) return rc;
     }
     if (rbf) {
         // gy = (K + sn2 I)^-1 gbeta  with the Cholesky factors kept by pilco_gp_factorize
         const int ldw = pad64(bf);
         chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
                               buf(BL.gbeta), (long long)U * bf, bf, 1, buf(BL.gy), bf);
-        launch_hi(rbf_factor_bwd_kernel, dim3(R), dim3(128), 0, st, bf, Ds, U, ro->pol.rbf.X, (long long)bf * Ds,
-                                                  ro->pol.rbf.ell, (long long)U * Ds, ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs,
-                                                  ro->pol.rbf.beta, (long long)U * bf,
-                                                  buf(BL.gy), g->gXc, g->gYc, g->gell);
-        CUDA_LAUNCH_CHECK();
+        rc = rbf_factor_bwd_launch(st, R, bf, Dh, U, ro->pol.rbf.X, (long long)bf * Dh, ro->pol.rbf.ell, (long long)U * Dh,
+                                   ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs, ro->pol.rbf.beta, (long long)U * bf,
+                                   buf(BL.gy), g->gXc, g->gYc, g->gell);
+        if (rc) return rc;
     }
     if (g->gm0) cudaMemcpyAsync(g->gm0, d.gm, sizeof(double) * RR * Ds, cudaMemcpyDeviceToDevice, st);
     if (g->gS0) cudaMemcpyAsync(g->gS0, d.gS, sizeof(double) * RR * Ds * Ds, cudaMemcpyDeviceToDevice, st);
     return PILCO_OK;
 }
 
-extern "C" int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream) {
-    return rb_backward_impl(ro, g, nullptr, nullptr, (cudaStream_t)stream);
+// the size of the reverse sweep's workspace (the exploration gradient adds none): 0 for a description without a batch
+// or with H < 0
+static size_t rb_ws_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz) {
+    if (!ro || ro->R < 1 || ro->H < 0) return 0;
+    return rb_ws_layout(ro, ang, nz).total * sizeof(double);
 }
 
+extern "C" {
+
+size_t pilco_rollout_bwd_workspace_bytes(const pilco_rollout* ro) { return rb_ws_bytes(ro, nullptr, nullptr); }
+
+size_t pilco_rollout_angles_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang) {
+    return rb_ws_bytes(ro, ang, nullptr);
+}
+
+size_t pilco_rollout_explore_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                                 const pilco_exploration* ex) {
+    (void)ex;
+    return rb_ws_bytes(ro, ang, nullptr);
+}
+
+size_t pilco_rollout_noisy_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                               const pilco_exploration* ex, const pilco_obs_noise* nz) {
+    (void)ex;
+    return rb_ws_bytes(ro, ang, nz);
+}
+
+int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream) {
+    return rb_backward(ro, nullptr, nullptr, nullptr, g, (cudaStream_t)stream);
+}
+
+int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
+                                  pilco_stream_t stream) {
+    return rb_backward(ro, ang, nullptr, nullptr, g, (cudaStream_t)stream);
+}
+
+int pilco_rollout_explore_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                   const pilco_rollout_grad* g, pilco_stream_t stream) {
+    return rb_backward(ro, ang, ex, nullptr, g, (cudaStream_t)stream);
+}
+
+int pilco_rollout_noisy_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                 const pilco_obs_noise* nz, const pilco_rollout_grad* g, pilco_stream_t stream) {
+    return rb_backward(ro, ang, ex, nz, g, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -1,7 +1,9 @@
-// rollout_bwd.cuh -- parameters of the reverse sweep's per-step kernels, shared by rollout_bwd.cu and the reverse sweep
-// with angular state dimensions (rollout_angles_bwd.cu).
+// rollout_bwd.cuh -- parameters of the reverse sweep's per-step kernels, shared by its driver (rollout_bwd.cu) and the
+// kernels on phi (rollout_angles_bwd.cu), with measurement noise (rollout_noise.cu) and exploration (rollout_explore.cu).
 #pragma once
 #include "rollout.cuh"
+
+struct MMTapeBwd;
 
 static inline bool rb_has_joint(const pilco_rollout* ro) {
     for (int k = 0; k < ro->n_rewards && k < 8; ++k) if (reward_on_joint(ro->rewards[k].kind)) return true;
@@ -30,21 +32,14 @@ struct RbDev {
     unsigned* cnt;
 };
 
+// rb_reward_kernel (state terms of ds, at dimension ds.Ds) and, when dj is non-NULL, rb_reward_joint_kernel (joint terms,
+// at dimension dj->Ds + dj->U) (rollout_bwd.cu)
 int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st);
-// Optional hook of the reverse sweep (pilco_rollout_explore_backward): run once the reward-gradient precompute
-// (rb_reward, rb_reward_joint) is enqueued and before the serial per-step chain, with the state terms' parameters ds
-// (state dimension ds.Ds) and, when a joint state-action term is present, the joint terms' dj, else NULL.
-typedef int (*RbRewardHook)(const RbDev& ds, const RbDev* dj, cudaStream_t st, const void* ctx);
-// pilco_rollout_backward with the hook above (rollout_bwd.cu); hook == NULL is that call
-int rb_backward_impl(const pilco_rollout* ro, const pilco_rollout_grad* g, RbRewardHook hook, const void* ctx,
-                     cudaStream_t st);
-// pilco_rollout_angles_backward (ang may be NULL) with the hook above (rollout_angles_bwd.cu).  nz: measurement noise
-// at the policy's input (pilco_rollout_noisy_backward, validated by the caller; g->ws of nz_bwd_ws_doubles), else NULL.
-int rb_backward_run(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g, RbRewardHook hook,
-                    const void* ctx, cudaStream_t st, const NzFwd* nz = nullptr);
-size_t nz_bwd_ws_doubles(const pilco_rollout* ro);
+// the exploration gradient (rollout_explore.cu), once rb_reward_launch is enqueued and before the serial per-step
+// chain: rb_reward_var with ds and, when dj is non-NULL, rb_reward_joint_var with dj, at sigma_t^2 var [H][R]
+int rb_reward_var_launch(const RbDev& ds, const RbDev* dj, double b, const double* var, cudaStream_t st);
 
-// parameters of the angle cascade's reverse per-step kernels (rollout_angles_bwd.cu)
+// parameters of the reverse per-step kernels on phi (rollout_angles_bwd.cu)
 struct TbDev {
     RbDev p;                  // p.Ds = Dh; p.gm / p.gS: the raw state's cotangent [R, Ds], [R, Ds, Ds]
     TrigMap tm;
@@ -96,21 +91,17 @@ __device__ __forceinline__ void tg_trig_tail(const TbDev& g, int r, double* gm, 
 }
 #endif
 
+// the post stage of step g.p.t on phi (rollout_angles_bwd.cu): with a tape (tb) tg_dyn_finish, the tape-driven dynamics
+// VJP whose last CTA of a restart runs tg_post, else tg_post alone after the recomputing dynamics VJP
+int tg_post_launch(const TbDev& g, const MMTapeBwd* tb, cudaStream_t st);
+// the trig stage of step g.p.t (rollout_angles_bwd.cu): trig VJP, state reward gradients, seeds of step t-1
+int tg_trig_launch(const TbDev& g, cudaStream_t st);
 // the per-step trig stage of the noisy reverse sweep (in place of tg_trig; rollout_noise.cu): the linear-policy VJP at
 // the noisy moments (mz, Sz) into (gmz, gSz), both trig VJPs into the state cotangent, then tg_trig's reward gradients
-// and seeds of step t-1; (gmz, gSz) are left zero for the next step
-int nz_trig_launch(const TbDev& g, const NzFwd& nz, const double* mz, const double* Sz, double* gmz, double* gSz,
+// and seeds of step t-1; (gmz, gSz) are left zero for the next step.  var: the noise variances [MAXD]
+int nz_trig_launch(const TbDev& g, const double* var, const double* mz, const double* Sz, double* gmz, double* gSz,
                    cudaStream_t st);
 int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
                           const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
                           const double* beta, long long beta_bs, const double* gy,
                           double* gX, double* gY, double* gell);
-
-// the exploration objective on the noisy cascade (rollout_explore.cu), for an active `ex` (b != 0 or step_var) that
-// ex_terms_check accepted: sigma_t^2 goes to ro->ws + var_at
-bool ex_active(const pilco_exploration* ex);
-int ex_terms_check(const pilco_rollout* ro, const pilco_exploration* ex);
-int ex_forward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
-                     size_t var_at, cudaStream_t st);
-int ex_backward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
-                      size_t var_at, const pilco_rollout_grad* g, cudaStream_t st);

@@ -4,12 +4,12 @@
 //   between terms ignored; state terms at (m_t, S_t), joint terms at step t's joint Gaussian), Var = r_2 - r_1^2 for an
 //   exponential term (reward.m:52-56) and W^T S W for a linear one;  sigma_t = sqrt(sigma_t^2) above 1e-12 (reward.m:57),
 //   else 0 with zero gradient.
-// The kernels run off the serial chain, through the hooks of the forward and the reverse sweep (rollout.cuh,
-// rollout_bwd.cuh), so the launches of a rollout without exploration are exactly those it always ran:
+// The kernels run off the serial chain, launched by the forward (rollout.cu) and the reverse sweep (rollout_bwd.cu) only
+// with an active exploration, so the launches of a rollout without exploration are exactly those it always ran:
 //   forward, after the reward launches:  ro_reward_var (t, r), ro_reward_joint_var (t, r; with a joint term), then
 //            ro_reward_explore_sum in place of ro_reward_sum
-//   reverse sweep, after the reward-gradient precompute:  rb_reward_var (r, t) and rb_reward_joint_var (with a joint
-//            term) add b c_k^2 / (2 sigma_t) dVar_k/d(m, S) to the ADD-channel slots that the per-step chain consumes
+//   reverse sweep with b != 0, after the reward-gradient precompute:  rb_reward_var (r, t) and rb_reward_joint_var (with
+//            a joint term) add b c_k^2 / (2 sigma_t) dVar_k/d(m, S) to the ADD-channel slots that the per-step chain consumes
 // A translation unit of its own, so that the existing kernels compile exactly as they do without it.
 #include <cmath>
 
@@ -137,111 +137,26 @@ __global__ void __launch_bounds__(128) rb_reward_joint_var_kernel(RbDev p, doubl
     }
 }
 
-// the exploration layout: the forward workspace of the call without exploration, then sigma_t^2 [H][R]
-struct ExWs { size_t var, total; };
-
-static ExWs ex_ws_layout(const pilco_rollout* ro, const pilco_angles* ang) {
-    ExWs L;
-    L.var = (ang && ang->A > 0) ? tg_ws_layout(ro).total : ro_ws_layout(ro).total;
-    L.total = L.var + (((size_t)ro->H * ro->R + 1) & ~(size_t)1);
-    return L;
-}
-
-bool ex_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
-
-int ex_terms_check(const pilco_rollout* ro, const pilco_exploration* ex) {
-    if (!std::isfinite(ex->b)) return PILCO_ERR_DIM;
-    for (int k = 0; k < ro->n_rewards; ++k)            // no variance closed form for a box term
-        if (ro->rewards[k].channel == PILCO_CHANNEL_ADD && ro->rewards[k].kind == PILCO_REWARD_BOX)
-            return PILCO_ERR_UNSUPPORTED;
-    return PILCO_OK;
-}
-
-// validation of an active exploration call, before anything is enqueued
-static int ex_check(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex) {
-    TrigMap tm;
-    int rc = tg_check(ro, ang, &tm);
-    if (rc) return rc;
-    rc = ex_terms_check(ro, ex);
-    if (rc) return rc;
-    if (ro->ws_bytes < ex_ws_layout(ro, ang).total * sizeof(double)) return PILCO_ERR_WORKSPACE;
-    return PILCO_OK;
-}
-
-struct ExCtx { double b; double* var; double* step_var; };
-
-static int ex_forward_hook(const RoDev& ds, const RoDev* dj, cudaStream_t st, const void* ctx) {
-    const ExCtx& c = *static_cast<const ExCtx*>(ctx);
+int ex_reward_var_launch(const RoDev& ds, const RoDev* dj, double b, double* var, double* step_var, cudaStream_t st) {
     if (ds.H > 0) {
-        launch_hi(ro_reward_var_kernel, dim3(ds.H, ds.R), dim3(128), 0, st, ds, c.var);
+        launch_hi(ro_reward_var_kernel, dim3(ds.H, ds.R), dim3(128), 0, st, ds, var);
         CUDA_LAUNCH_CHECK();
         if (dj) {
-            launch_hi(ro_reward_joint_var_kernel, dim3(dj->H, dj->R), dim3(128), 0, st, *dj, c.var);
+            launch_hi(ro_reward_joint_var_kernel, dim3(dj->H, dj->R), dim3(128), 0, st, *dj, var);
             CUDA_LAUNCH_CHECK();
         }
     }
-    launch_hi(ro_reward_explore_sum_kernel, dim3((ds.R + 127) / 128), dim3(128), 0, st, ds, c.b, (const double*)c.var,
-              c.step_var);
+    launch_hi(ro_reward_explore_sum_kernel, dim3((ds.R + 127) / 128), dim3(128), 0, st, ds, b, (const double*)var, step_var);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
 
-static int ex_backward_hook(const RbDev& ds, const RbDev* dj, cudaStream_t st, const void* ctx) {
-    const ExCtx& c = *static_cast<const ExCtx*>(ctx);
-    launch_hi(rb_reward_var_kernel, dim3(ds.R, ds.H), dim3(128), 0, st, ds, c.b, (const double*)c.var);
+int rb_reward_var_launch(const RbDev& ds, const RbDev* dj, double b, const double* var, cudaStream_t st) {
+    launch_hi(rb_reward_var_kernel, dim3(ds.R, ds.H), dim3(128), 0, st, ds, b, var);
     CUDA_LAUNCH_CHECK();
     if (dj) {
-        launch_hi(rb_reward_joint_var_kernel, dim3(dj->R, dj->H), dim3(128), 0, st, *dj, c.b, (const double*)c.var);
+        launch_hi(rb_reward_joint_var_kernel, dim3(dj->R, dj->H), dim3(128), 0, st, *dj, b, var);
         CUDA_LAUNCH_CHECK();
     }
     return PILCO_OK;
 }
-
-int ex_forward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
-                     size_t var_at, cudaStream_t st) {
-    const ExCtx c = {ex->b, (double*)ro->ws + var_at, ex->step_var};
-    return ro_forward_run(ro, ang, ex_forward_hook, &c, st, nz);
-}
-
-int ex_backward_noisy(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const NzFwd* nz,
-                      size_t var_at, const pilco_rollout_grad* g, cudaStream_t st) {
-    if (ex->b == 0.0) return rb_backward_run(ro, ang, g, nullptr, nullptr, st, nz);
-    const ExCtx c = {ex->b, (double*)ro->ws + var_at, nullptr};
-    return rb_backward_run(ro, ang, g, ex_backward_hook, &c, st, nz);
-}
-
-extern "C" {
-
-size_t pilco_rollout_explore_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
-                                             const pilco_exploration* ex) {
-    if (!ex_active(ex)) return pilco_rollout_angles_workspace_bytes(ro, ang);
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    return ex_ws_layout(ro, ang).total * sizeof(double);
-}
-
-size_t pilco_rollout_explore_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
-                                                 const pilco_exploration* ex) {
-    (void)ex;                                         // the bonus's gradient goes to the slots the sweep already has
-    return pilco_rollout_angles_bwd_workspace_bytes(ro, ang);
-}
-
-int pilco_rollout_explore_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                                  pilco_stream_t stream) {
-    if (!ex_active(ex)) return pilco_rollout_angles_forward(ro, ang, stream);
-    int rc = ex_check(ro, ang, ex);
-    if (rc) return rc;
-    const ExCtx c = {ex->b, (double*)ro->ws + ex_ws_layout(ro, ang).var, ex->step_var};
-    return ro_forward_run(ro, ang, ex_forward_hook, &c, (cudaStream_t)stream);
-}
-
-int pilco_rollout_explore_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                                   const pilco_rollout_grad* g, pilco_stream_t stream) {
-    if (!ex_active(ex)) return pilco_rollout_angles_backward(ro, ang, g, stream);
-    int rc = ex_check(ro, ang, ex);
-    if (rc) return rc;
-    if (ex->b == 0.0) return pilco_rollout_angles_backward(ro, ang, g, stream);     // no bonus: nothing to add
-    const ExCtx c = {ex->b, (double*)ro->ws + ex_ws_layout(ro, ang).var, nullptr};
-    return rb_backward_run(ro, ang, g, ex_backward_hook, &c, (cudaStream_t)stream);
-}
-
-}  // extern "C"

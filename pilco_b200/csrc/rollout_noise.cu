@@ -1,12 +1,12 @@
 // rollout_noise.cu -- measurement noise at the policy's input on the moment-matching rollout (pilco_rollout_noisy_*):
 // propagate.m's noisy state measurement, ss = S + diag(sn2) for the policy and q = S(j,i) C for the joint.
-// The cascade is the angle cascade (rollout.cu, rollout_angles_bwd.cu; with no angles phi is the identity and A = 0)
-// with two kernels replaced per step:
+// The cascade is the one on phi (rollout.cu, rollout_bwd.cu; with no angles phi is the identity and A = 0) with two
+// kernels replaced per step:
 //   forward  nz_state<t> in place of tg_state: the glue, then the feature moments twice, (m^_x, S^_x, C^_x) under
 //            N(m, S) for the dynamics and (m^_z, S^_z) under N(m, S + diag(v)) for the policy (kept per step for the
 //            reverse sweep); linear policy at the noisy set, squash, the joint [phi, u] and cx at the true set.  The
-//            RBF policy's moment match reads the noisy slots; tg_policy, the dynamics and the reward launches and the
-//            exploration hook are those of the angle / exploration calls.
+//            RBF policy's moment match reads the noisy slots; tg_policy, the dynamics and the reward launches (with
+//            exploration, its launches too) are those of the angle / exploration calls.
 //   reverse  tg_post (or the taped tg_dyn_finish) without its linear-policy VJP; the RBF policy's VJP reads the noisy
 //            slots and accumulates into (gm^_z, gS^_z); nz_trig in place of tg_trig: the linear-policy VJP at the noisy
 //            set into (gm^_z, gS^_z), dev_trig_bwd at (m, S) with (gm^_x, gS^_x, gC^_x) and at (m, S + diag(v)) with
@@ -104,86 +104,21 @@ __global__ void __launch_bounds__(128) nz_trig_kernel(NzBwdDev z) {
     tg_trig_tail(g, r, gm, gS);
 }
 
-int nz_state_launch(const TgDev& g, const NzFwd& nz, double* mz, double* Sz, cudaStream_t st) {
+int nz_state_launch(const TgDev& g, const double* var, double* mz, double* Sz, cudaStream_t st) {
     NzDev z;
     z.g = g; z.mz = mz; z.Sz = Sz;
-    for (int i = 0; i < MAXD; ++i) z.var[i] = nz.var[i];
+    for (int i = 0; i < MAXD; ++i) z.var[i] = var[i];
     launch_hi(nz_state_kernel, dim3(g.p.R), dim3(128), 0, st, z);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
 
-int nz_trig_launch(const TbDev& g, const NzFwd& nz, const double* mz, const double* Sz, double* gmz, double* gSz,
+int nz_trig_launch(const TbDev& g, const double* var, const double* mz, const double* Sz, double* gmz, double* gSz,
                    cudaStream_t st) {
     NzBwdDev z;
     z.g = g; z.mz = mz; z.Sz = Sz; z.gmz = gmz; z.gSz = gSz;
-    for (int i = 0; i < MAXD; ++i) z.var[i] = nz.var[i];
+    for (int i = 0; i < MAXD; ++i) z.var[i] = var[i];
     launch_hi(nz_trig_kernel, dim3(g.p.R), dim3(128), 0, st, z);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }
-
-// validation before anything is enqueued; fills the forward layout (f) and the exploration slot's offset (var_at)
-static int nz_check(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                    const pilco_obs_noise* nz, NzFwd* f, size_t* var_at) {
-    TrigMap tm;
-    int rc = tg_check(ro, ang, &tm);
-    if (rc) return rc;
-    if (ex_active(ex)) {
-        rc = ex_terms_check(ro, ex);
-        if (rc) return rc;
-    }
-    const int Ds = ro->dyn.E;                          // <= PILCO_MAX_D - 1 once tg_check has passed
-    for (int i = 0; i < Ds; ++i)
-        if (!std::isfinite(nz->var[i]) || nz->var[i] < 0.0) return PILCO_ERR_DIM;
-    size_t total;
-    *f = nz_ws_layout(ro, &total);
-    for (int i = 0; i < MAXD; ++i) f->var[i] = i < Ds ? nz->var[i] : 0.0;
-    *var_at = total;
-    if (ex_active(ex)) total += ((size_t)ro->H * ro->R + 1) & ~(size_t)1;
-    if (ro->ws_bytes < total * sizeof(double)) return PILCO_ERR_WORKSPACE;
-    return PILCO_OK;
-}
-
-extern "C" {
-
-size_t pilco_rollout_noisy_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                                           const pilco_obs_noise* nz) {
-    if (!nz) return pilco_rollout_explore_workspace_bytes(ro, ang, ex);
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    size_t total;
-    nz_ws_layout(ro, &total);
-    if (ex_active(ex)) total += ((size_t)ro->H * ro->R + 1) & ~(size_t)1;
-    return total * sizeof(double);
-}
-
-size_t pilco_rollout_noisy_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
-                                               const pilco_exploration* ex, const pilco_obs_noise* nz) {
-    if (!nz) return pilco_rollout_explore_bwd_workspace_bytes(ro, ang, ex);
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    return nz_bwd_ws_doubles(ro) * sizeof(double);
-}
-
-int pilco_rollout_noisy_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                                const pilco_obs_noise* nz, pilco_stream_t stream) {
-    if (!nz) return pilco_rollout_explore_forward(ro, ang, ex, stream);
-    NzFwd f;
-    size_t var_at;
-    int rc = nz_check(ro, ang, ex, nz, &f, &var_at);
-    if (rc) return rc;
-    if (ex_active(ex)) return ex_forward_noisy(ro, ang, ex, &f, var_at, (cudaStream_t)stream);
-    return ro_forward_run(ro, ang, nullptr, nullptr, (cudaStream_t)stream, &f);
-}
-
-int pilco_rollout_noisy_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                                 const pilco_obs_noise* nz, const pilco_rollout_grad* g, pilco_stream_t stream) {
-    if (!nz) return pilco_rollout_explore_backward(ro, ang, ex, g, stream);
-    NzFwd f;
-    size_t var_at;
-    int rc = nz_check(ro, ang, ex, nz, &f, &var_at);
-    if (rc) return rc;
-    if (ex_active(ex)) return ex_backward_noisy(ro, ang, ex, &f, var_at, g, (cudaStream_t)stream);
-    return rb_backward_run(ro, ang, g, nullptr, nullptr, (cudaStream_t)stream, &f);
-}
-
-}  // extern "C"

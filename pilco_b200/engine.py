@@ -615,14 +615,7 @@ class RolloutPlan:
         if b is not None:
             self.step_var = torch.zeros((self.R, max(self.H, 1)), dtype=F64, device=d)
             self.ex = _lib.Exploration(b, self.step_var.data_ptr())
-        if self.nz is not None:
-            wsb = lib.pilco_rollout_noisy_workspace_bytes(C.byref(ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz))
-        elif self.ex is not None:
-            wsb = lib.pilco_rollout_explore_workspace_bytes(C.byref(ro), self._ang_ref(), C.byref(self.ex))
-        elif self.ang is None:
-            wsb = lib.pilco_rollout_workspace_bytes(C.byref(ro))
-        else:
-            wsb = lib.pilco_rollout_angles_workspace_bytes(C.byref(ro), C.byref(self.ang))
+        wsb = lib.pilco_rollout_noisy_workspace_bytes(C.byref(ro), self._ang_ref(), self._ex_ref(), self._nz_ref())
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         ro.ws, ro.ws_bytes = self.ws.data_ptr(), wsb
         self.tape = None
@@ -639,18 +632,12 @@ class RolloutPlan:
     def _ex_ref(self):
         return C.byref(self.ex) if self.ex is not None else None
 
+    def _nz_ref(self):
+        return C.byref(self.nz) if self.nz is not None else None
+
     def forward(self):
-        if self.nz is not None:
-            check(lib.pilco_rollout_noisy_forward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz),
-                                                  stream_ptr()), "rollout_noisy_forward")
-        elif self.ex is not None:
-            check(lib.pilco_rollout_explore_forward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex), stream_ptr()),
-                  "rollout_explore_forward")
-        elif self.ang is None:
-            check(lib.pilco_rollout_forward(C.byref(self.ro), stream_ptr()), "rollout_forward")
-        else:
-            check(lib.pilco_rollout_angles_forward(C.byref(self.ro), C.byref(self.ang), stream_ptr()),
-                  "rollout_angles_forward")
+        check(lib.pilco_rollout_noisy_forward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), self._nz_ref(),
+                                              stream_ptr()), "rollout_noisy_forward")
         return self.traj_m, self.traj_S, self.reward
 
     # ---- CUDA graph: the whole H-step loop (6H+1 launches forward, ~10H backward) as one graph launch -------
@@ -684,29 +671,13 @@ class RolloutPlan:
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
-            if self.nz is not None:
-                wsb = lib.pilco_rollout_noisy_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), self._ex_ref(),
-                                                                  C.byref(self.nz))
-            elif self.ex is not None:
-                wsb = lib.pilco_rollout_explore_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), C.byref(self.ex))
-            elif self.ang is None:
-                wsb = lib.pilco_rollout_bwd_workspace_bytes(C.byref(self.ro))
-            else:
-                wsb = lib.pilco_rollout_angles_bwd_workspace_bytes(C.byref(self.ro), C.byref(self.ang))
+            wsb = lib.pilco_rollout_noisy_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), self._ex_ref(),
+                                                              self._nz_ref())
             self.bws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.bws.data_ptr(), wsb
             self.grad = g
-        if self.nz is not None:
-            check(lib.pilco_rollout_noisy_backward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), C.byref(self.nz),
-                                                   C.byref(self.grad), stream_ptr()), "rollout_noisy_backward")
-        elif self.ex is not None:
-            check(lib.pilco_rollout_explore_backward(C.byref(self.ro), self._ang_ref(), C.byref(self.ex),
-                                                     C.byref(self.grad), stream_ptr()), "rollout_explore_backward")
-        elif self.ang is None:
-            check(lib.pilco_rollout_backward(C.byref(self.ro), C.byref(self.grad), stream_ptr()), "rollout_backward")
-        else:
-            check(lib.pilco_rollout_angles_backward(C.byref(self.ro), C.byref(self.ang), C.byref(self.grad), stream_ptr()),
-                  "rollout_angles_backward")
+        check(lib.pilco_rollout_noisy_backward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), self._nz_ref(),
+                                               C.byref(self.grad), stream_ptr()), "rollout_noisy_backward")
         return self.gbuf
 
 
