@@ -561,6 +561,51 @@ size_t pilco_particles_angles_score_grad_workspace_bytes(const pilco_particles* 
 int    pilco_particles_angles_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
                                                  const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* The particle rollouts with measurement noise at the policy's input (propagate.m's noisy state measurement at every
+ * particle; DESIGN.md section 23).  Each call below is the pilco_particles_angles_* call of the same name (ang may be
+ * NULL) whose policy sees a noisy measurement of the state.  Per particle p, restart r and step t < H, with E = dyn.E:
+ *   z_t = x_t + sqrt(v) o nu_t,  u_t = squash(pi(phi(z_t))),  x~_t = [phi(x_t), u_t],
+ *   x_{t+1} = x_t + mu(x~_t) + sqrt(max(var(x~_t), 0)) o eps_t
+ * (phi = identity without angles; the consistent sampler conditions on the particle's earlier x~, which hold phi(x)).
+ * The state terms are evaluated at the raw x_t and the joint terms at x~_t, as before.  traj, act, step_reward,
+ * step_risk, ret and value keep their layouts.  nu is an exogenous input like x0 and eps: each gradient is conditioned on
+ * it and estimates the derivative of the return's expectation over (x0, eps, nu); none is taken with respect to v.
+ * The forward-only workspaces are those of the angle calls; the three gradients' are those of the angle calls with
+ * angles (the phi history [R P,H+1,Dh], with A = 0 too), then the phi(z) history [R P,H+1,Dh] and, for the pathwise and
+ * consistent gradients, phi_bar_z [R P,Dh] (each slot rounded up to an even number of doubles).
+ * With nz == NULL every call is the pilco_particles_angles_* call with the same arguments, workspace sizes included.
+ * Validation before anything is enqueued: the angle call's status codes up to its workspace check, then PILCO_ERR_DIM
+ * for a non-finite or negative v.var[i] (i < E), then PILCO_ERR_NULL for nu == NULL with H > 0, then the workspace's
+ * codes (PILCO_ERR_WORKSPACE).  A workspace query returns 0 wherever its call would fail on these checks. */
+typedef struct pilco_particles_noise {
+    pilco_obs_noise v;          /* measurement variances of the raw state; the first dyn.E are used, finite, >= 0 */
+    const double*   nu;         /* [P,H,E] standard normals of the measurement noise, shared by the R restarts */
+} pilco_particles_noise;
+
+size_t pilco_particles_noisy_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz);
+int    pilco_particles_noisy_rollout(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                                     pilco_stream_t stream);
+size_t pilco_particles_noisy_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz);
+int    pilco_particles_noisy_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, pilco_stream_t stream);
+size_t pilco_particles_noisy_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R);
+int    pilco_particles_noisy_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
+                                                pilco_stream_t stream);
+size_t pilco_particles_noisy_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                             const pilco_particles_noise* nz, int R);
+int    pilco_particles_noisy_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                     const pilco_particles_noise* nz, int R,
+                                                     const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_noisy_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R);
+int    pilco_particles_noisy_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
+                                                pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

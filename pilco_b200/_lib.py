@@ -85,6 +85,11 @@ class ObsNoise(C.Structure):
     _fields_ = [("var", C.c_double * 16)]
 
 
+class ParticlesNoise(C.Structure):
+    """mirror of ``pilco_particles_noise``"""
+    _fields_ = [("v", ObsNoise), ("nu", c_dp)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -92,6 +97,8 @@ JOINT_REWARDS = (REWARD_EXP_SA, REWARD_LINEAR_SA)
 CHANNEL_ADD, CHANNEL_MULT = 0, 1
 ABI_VERSION = 3
 ABI_MAX_D = 16                                   # PILCO_MAX_D
+
+_PAN = [C.POINTER(Particles), C.POINTER(Angles), C.POINTER(ParticlesNoise)]     # the noisy particle calls' first three
 
 # name -> (restype, argtypes); every symbol declared in include/pilco_b200.h
 SIGNATURES = {
@@ -189,6 +196,16 @@ SIGNATURES = {
                                                                        C.c_int]),
     "pilco_particles_angles_score_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int,
                                                             C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_noisy_workspace_bytes": (C.c_size_t, _PAN),
+    "pilco_particles_noisy_rollout": (C.c_int, _PAN + [c_dp]),
+    "pilco_particles_noisy_consistent_workspace_bytes": (C.c_size_t, _PAN),
+    "pilco_particles_noisy_consistent_rollout": (C.c_int, _PAN + [c_dp]),
+    "pilco_particles_noisy_batch_grad_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_noisy_batch_grad_rollout": (C.c_int, _PAN + [C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_noisy_consistent_grad_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_noisy_consistent_grad_rollout": (C.c_int, _PAN + [C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_noisy_score_grad_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_noisy_score_grad_rollout": (C.c_int, _PAN + [C.c_int, C.POINTER(ParticlesGrad), c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),
     "pilco_mm_forward_taped_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,

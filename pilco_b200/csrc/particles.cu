@@ -24,6 +24,10 @@
 // Angular state dimensions (pilco_particles_angles_*, DESIGN.md section 20): pt_forward, pg_reverse and ps_run take the
 // angles' map and launch the step kernels of particles_angles.cu in place of pt_step / pg_step; the shared structs are
 // in particles.cuh.
+// Measurement noise at the policy's input (pilco_particles_noisy_*, DESIGN.md section 23): the same drivers take a
+// PnNoise next to the map (the identity map without angles) and launch the kernels of particles_noise.cu in place of the
+// angle step kernels; the policy inputs of the reductions are then the phi(z) history.
+#include <cmath>
 #include "particles.cuh"
 
 // grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y
@@ -764,6 +768,7 @@ struct PtWs {
     size_t G, dir;                                      // reverse of the conditioning (score: G = the return-to-go)
     size_t gsum;                                        // score: the per-(restart, step) sums of G
     size_t phi;                                         // angles, gradients: phi(x_t) [T,H+1,Dh]
+    size_t phiz, phibz;                                 // noise, gradients: phi(z_t) [T,H+1,Dh]; phi_bar_z [T,Dh]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -802,8 +807,9 @@ static PtWs pt_ws_layout(const pilco_particles* pr) {
 // them), the state cotangent, the VJP's cotangents and output, z_bar of every point, the RBF sums, and one predict /
 // VJP workspace at T = R P (never in use at the same time).  Rows are restart-major (row r P + p); nothing of size
 // [., n] is kept.  State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles);
-// angles: the phi history [T,H+1,Dh] after everything else.
-static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+// angles: the phi history [T,H+1,Dh] after everything else; noise (with angles = true): then the phi(z) history
+// [T,H+1,Dh] and phi_bar_z [T,Dh].
+static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -816,6 +822,7 @@ static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false) 
     L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
     if (angles) L.phi = take({T, H + 1, Dh});
+    if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
     L.total = L.pws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -841,8 +848,9 @@ static PtWs fs_ws_layout(const pilco_particles* pr) {
 // the consistent gradient for R restarts: the consistent forward's at T = R P (its W slot holds a_t in the reverse
 // sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
 // [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
-// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, as pg_ws_layout)
-static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, noise: then the
+// phi(z) history and phi_bar_z, as pg_ws_layout)
+static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -854,6 +862,7 @@ static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false) 
     L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
     L.vws = take({L.vws_bytes / sizeof(double)});
     if (angles) L.phi = take({T, H + 1, Dh});
+    if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
     L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -867,8 +876,9 @@ static int ps_group(long long T, int H) {
 // the score gradient for R restarts: pg_ws_layout's forward part (x~ [H,T,D], mean [T,Ds], var [H,T,Ds]), then G
 // [H-1,T], the sums [R,H], gmean and gvar [H-1,T,Ds], the VJP output [H-1,T,D], z_bar [T,H,U], the RBF sums
 // [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one predict / VJP workspace for the predict at T and the largest VJP group.
-// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.  Angles: then the phi history, as pg_ws_layout.
-static PtWs ps_ws_layout(const pilco_particles* pr, int R, bool angles = false) {
+// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.  Angles: then the phi history, as pg_ws_layout;
+// noise: then the phi(z) history (the score path has no phi_bar_z).
+static PtWs ps_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U;
     const size_t D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -885,6 +895,7 @@ static PtWs ps_ws_layout(const pilco_particles* pr, int R, bool angles = false) 
     L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
     if (angles) L.phi = take({T, H + 1, Dh});
+    if (noise) L.phiz = take({T, H + 1, Dh});
     const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
     L.total = L.pws_bytes && nb * H <= 0x7fffffff ? take.bytes() : 0;
     return L;
@@ -1005,9 +1016,11 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 // consistent: the predict is fs_predict_kernel and fs_cond_kernel leaves the step closure (mean, var) that
 // pt_step_kernel reads unchanged.  history: var of every step is kept (the reverse sweep needs it); x~ of every step is
 // kept when either needs it.  tm (angles, DESIGN.md section 20): pa_step_kernel in place of pt_step_kernel, which with
-// history also keeps phi(x_t) in L.phi.  The state width is dyn.E throughout (pol.Ds without angles).
+// history also keeps phi(x_t) in L.phi.  nz (noise, DESIGN.md section 23; tm then given, the identity without angles):
+// pn_step_kernel in place of pa_step_kernel, which with history also keeps phi(z_t) in L.phiz.  The state width is
+// dyn.E throughout (pol.Ds without angles).
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
-                      cudaStream_t st, const TrigMap* tm = nullptr) {
+                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
@@ -1019,6 +1032,8 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     a.mean = ws + L.mean;
     PaStep pa;
     if (tm) { pa.E = Ds; pa.tm = *tm; pa.phi = history ? ws + L.phi : nullptr; }
+    PnStep pn;
+    if (nz) { pn.nz = *nz; pn.phiz = history ? ws + L.phiz : nullptr; }
     FsCond c;
     c.P = P; c.T = T; c.H = H; c.D = D; c.Ds = Ds; c.n = pr->dyn.n; c.np = np; c.t = 0;
     c.ell = pr->dyn.ell; c.sf2 = pr->dyn.sf2;
@@ -1030,7 +1045,11 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
         a.t = t;
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
         a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
-        if (tm) {
+        if (nz) {
+            static_cast<PtDev&>(pa) = a;
+            static_cast<PaStep&>(pn) = pa;
+            if (const int rc = pn_step_launch(st, grid, pn)) return rc;
+        } else if (tm) {
             static_cast<PtDev&>(pa) = a;
             if (const int rc = pa_step_launch(st, grid, pa)) return rc;
         } else {
@@ -1098,8 +1117,9 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 //   pg_step<H-1>, [VJP<t>, pg_step<t>] for t = H-2 .. 0, then pg_reduce's launches
 // The step's VJP is pilco_gp_predict_vjp, or (consistent) fs_cond_bwd_kernel followed by fs_predict_vjp_kernel.
 // tm (angles): pa_reverse_launch's two kernels in place of pg_step, and the policy reduction over the phi history.
+// nz (noise): pn_reverse_launch's two kernels, and the policy reduction over the phi(z) history.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
-                      cudaStream_t st, const TrigMap* tm = nullptr) {
+                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1144,7 +1164,13 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             CUDA_LAUNCH_CHECK();
         }
         b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * TDs : nullptr;
-        if (tm) {
+        if (nz) {
+            PnBwd nb;
+            static_cast<PgDev&>(nb) = b;
+            nb.E = Ds; nb.tm = *tm; nb.phi = ws + L.phi; nb.phib = nullptr;
+            nb.phiz = ws + L.phiz; nb.phibz = ws + L.phibz;
+            if (const int rc = pn_reverse_launch(st, grid, nb)) return rc;
+        } else if (tm) {
             PaBwd ab;
             static_cast<PgDev&>(ab) = b;
             ab.E = Ds; ab.tm = *tm; ab.phi = ws + L.phi; ab.phib = b.gxt ? ws + L.gxt : nullptr;
@@ -1154,31 +1180,33 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             CUDA_LAUNCH_CHECK();
         }
     }
-    return pg_reduce(pr, R, g, ws, L, st, tm ? ws + L.phi : pr->traj);
+    return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj);
 }
 
 // the validated gradient of R restarts: the forward with its history, then the reverse sweep
 static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool consistent,
-                  pilco_stream_t stream, const TrigMap* tm = nullptr) {
-    const PtWs L = consistent ? fg_ws_layout(pr, R, tm != nullptr) : pg_ws_layout(pr, R, tm != nullptr);
+                  pilco_stream_t stream, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
+    const bool ang = tm != nullptr, noise = nz != nullptr;
+    const PtWs L = consistent ? fg_ws_layout(pr, R, ang, noise) : pg_ws_layout(pr, R, ang, noise);
     if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
     if (consistent) {
         if (const int rc = fs_predict_prepare()) return rc;
         if (const int rc = fs_vjp_prepare()) return rc;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st, tm)) return rc;
-    return pg_reverse(pr, R, g, L, consistent, st, tm);
+    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st, tm, nz)) return rc;
+    return pg_reverse(pr, R, g, L, consistent, st, tm, nz);
 }
 
-// the forward alone, R = 1 (tm: validated angles; the description is checked here)
-static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream, const TrigMap* tm = nullptr) {
+// the forward alone, R = 1 (tm: validated angles, nz: validated noise; the description is checked here)
+static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream, const TrigMap* tm = nullptr,
+                  const PnNoise* nz = nullptr) {
     if (const int rc = pt_check_desc(pr, false, tm ? tm->A : 0)) return rc;
     const PtWs L = consistent ? fs_ws_layout(pr) : pt_ws_layout(pr);
     if (const int rc = pt_check_ws(pr->ws, pr->ws_bytes, L.total)) return rc;
     if (consistent)
         if (const int rc = fs_predict_prepare()) return rc;
-    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream, tm);
+    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream, tm, nz);
 }
 
 // The score-function gradient of R restarts (validated; DESIGN.md section 16):
@@ -1186,17 +1214,18 @@ static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t str
 // The x~ history [H-1,T,D] and the cotangents [H-1,T,Ds] are contiguous, so a group of k steps is one VJP call at k T
 // rows; a point's VJP does not depend on T or on its row, so the grouping changes no bit.
 // tm (angles): the state-width cotangents are in E (ps_cot at Ds = E); ps_zbar and the reduction read the policy
-// inputs from the phi history (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.
+// inputs from the phi history (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.  nz (noise): the
+// policy inputs are the phi(z) history; the VJPs act on x~, which holds phi(x), unchanged.
 static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream,
-                  const TrigMap* tm = nullptr) {
-    const PtWs L = ps_ws_layout(pr, R, tm != nullptr);
+                  const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
+    const PtWs L = ps_ws_layout(pr, R, tm != nullptr, nz != nullptr);
     if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     double* ws = (double*)g->ws;
-    if (const int rc = pt_forward(pr, R, ws, L, false, true, st, tm)) return rc;
+    if (const int rc = pt_forward(pr, R, ws, L, false, true, st, tm, nz)) return rc;
     const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const int nb = (P + PT_THREADS - 1) / PT_THREADS;
-    const double* pin = tm ? ws + L.phi : pr->traj;
+    const double* pin = nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj;
     PsDev a;
     static_cast<PtPolicy&>(a) = pt_policy(pr);
     a.T = T;
@@ -1268,6 +1297,44 @@ static bool pa_none(const pilco_angles* ang) { return !ang || ang->A == 0; }
 static bool pa_sizes_ok(const pilco_particles* pr, const pilco_angles* ang) {
     TrigMap tm;
     return pr && pt_sizes_ok(pr) && pa_map(pr, ang, &tm) == PILCO_OK;
+}
+
+// ---- measurement noise at the policy's input (DESIGN.md section 23) -------------------------------------------------
+// The noise's own checks, after the description's: PILCO_ERR_DIM for a non-finite or negative var[i] (i < dyn.E), then
+// PILCO_ERR_NULL for nu == NULL with H > 0.  Fills n (sqrt(var), nu).  pr has passed its description's checks.
+static int pn_noise(const pilco_particles* pr, const pilco_particles_noise* nz, PnNoise* n) {
+    const int E = pr->dyn.E;
+    for (int i = 0; i < MAXD; ++i) {
+        const double v = i < E ? nz->v.var[i] : 0.0;
+        if (!std::isfinite(v) || v < 0.0) return PILCO_ERR_DIM;
+        n->sv[i] = std::sqrt(v);
+    }
+    if (!nz->nu && pr->H > 0) return PILCO_ERR_NULL;
+    n->nu = nz->nu;
+    return PILCO_OK;
+}
+
+// everything a noisy call checks before its workspace (nz != NULL), in order: the angles' map (A >= 1), the
+// description as the angle call checks it (grad: pg_validate with the policy's batch strides), then the noise.
+// Fills tm (without angles: the identity map, A = 0) and n.
+static int pn_validate(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz, int R,
+                       const pilco_particles_grad* g, bool grad, TrigMap* tm, PnNoise* n) {
+    if (!pr) return PILCO_ERR_NULL;
+    const bool none = pa_none(ang);
+    if (!none)
+        if (const int rc = pa_map(pr, ang, tm)) return rc;
+    const int A = none ? 0 : tm->A;
+    if (const int rc = grad ? pg_validate(pr, R, g, true, A) : pt_check_desc(pr, false, A)) return rc;
+    if (none) trig_map_make(pr->dyn.E, 0, nullptr, tm);            // 1 <= E <= PILCO_MAX_E once the description passed
+    return pn_noise(pr, nz, n);
+}
+
+// a noisy call's workspace query (nz != NULL): the sizes the angle query accepts and valid noise
+static bool pn_sizes_ok(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz) {
+    if (!pr || !pt_sizes_ok(pr) || (!pa_none(ang) && !pa_sizes_ok(pr, ang))) return false;
+    if (pr->dyn.E < 1 || pr->dyn.E > MAXE) return false;
+    PnNoise n;
+    return pn_noise(pr, nz, &n) == PILCO_OK;
 }
 
 extern "C" {
@@ -1394,6 +1461,80 @@ int pilco_particles_angles_score_grad_rollout(const pilco_particles* pr, const p
     if (const int rc = pa_map(pr, ang, &tm)) return rc;
     if (const int rc = pg_validate(pr, R, g, true, tm.A)) return rc;
     return ps_run(pr, R, g, stream, &tm);
+}
+
+// ---- the noisy twins: nz == NULL is the angle call (ang may be NULL) -----------------------------------------------
+size_t pilco_particles_noisy_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz) {
+    if (!nz) return pilco_particles_angles_workspace_bytes(pr, ang);
+    return pn_sizes_ok(pr, ang, nz) ? pt_ws_layout(pr).total : 0;
+}
+
+int pilco_particles_noisy_rollout(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                                  pilco_stream_t stream) {
+    if (!nz) return pilco_particles_angles_rollout(pr, ang, stream);
+    TrigMap tm; PnNoise n;
+    if (const int rc = pn_validate(pr, ang, nz, 1, nullptr, false, &tm, &n)) return rc;
+    return pt_run(pr, false, stream, &tm, &n);
+}
+
+size_t pilco_particles_noisy_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz) {
+    if (!nz) return pilco_particles_angles_consistent_workspace_bytes(pr, ang);
+    return pn_sizes_ok(pr, ang, nz) ? fs_ws_layout(pr).total : 0;
+}
+
+int pilco_particles_noisy_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, pilco_stream_t stream) {
+    if (!nz) return pilco_particles_angles_consistent_rollout(pr, ang, stream);
+    TrigMap tm; PnNoise n;
+    if (const int rc = pn_validate(pr, ang, nz, 1, nullptr, false, &tm, &n)) return rc;
+    return pt_run(pr, true, stream, &tm, &n);
+}
+
+size_t pilco_particles_noisy_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R) {
+    if (!nz) return pilco_particles_angles_batch_grad_workspace_bytes(pr, ang, R);
+    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R, true, true).total : 0;
+}
+
+int pilco_particles_noisy_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
+                                             pilco_stream_t stream) {
+    if (!nz) return pilco_particles_angles_batch_grad_rollout(pr, ang, R, g, stream);
+    TrigMap tm; PnNoise n;
+    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
+    return pg_run(pr, R, g, false, stream, &tm, &n);
+}
+
+size_t pilco_particles_noisy_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                             const pilco_particles_noise* nz, int R) {
+    if (!nz) return pilco_particles_angles_consistent_grad_workspace_bytes(pr, ang, R);
+    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R, true, true).total : 0;
+}
+
+int pilco_particles_noisy_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                  const pilco_particles_noise* nz, int R,
+                                                  const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (!nz) return pilco_particles_angles_consistent_grad_rollout(pr, ang, R, g, stream);
+    TrigMap tm; PnNoise n;
+    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
+    return pg_run(pr, R, g, true, stream, &tm, &n);
+}
+
+size_t pilco_particles_noisy_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R) {
+    if (!nz) return pilco_particles_angles_score_grad_workspace_bytes(pr, ang, R);
+    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R, true, true).total : 0;
+}
+
+int pilco_particles_noisy_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
+                                             pilco_stream_t stream) {
+    if (!nz) return pilco_particles_angles_score_grad_rollout(pr, ang, R, g, stream);
+    TrigMap tm; PnNoise n;
+    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
+    return ps_run(pr, R, g, stream, &tm, &n);
 }
 
 }  // extern "C"

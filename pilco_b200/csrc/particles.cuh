@@ -1,5 +1,6 @@
-// particles.cuh -- what the particle kernels of particles.cu and particles_angles.cu share: the per-particle argument
-// structs, the reward value at a point, and the angle kernels' launchers (DESIGN.md sections 11, 12 and 20).
+// particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu and particles_noise.cu share: the
+// per-particle argument structs, the reward value at a point, and the angle and noise kernels' launchers (DESIGN.md
+// sections 11, 12, 20 and 23).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -88,3 +89,26 @@ struct PaBwd : PgDev {
 int pa_step_launch(cudaStream_t st, dim3 grid, const PaStep& a);
 // grid (ceil(P / 128), R): the angle path's reverse step t (in place of pg_step_kernel), two launches
 int pa_reverse_launch(cudaStream_t st, dim3 grid, const PaBwd& a);
+
+// ---- measurement noise at the policy's input (particles_noise.cu, DESIGN.md section 23) ------------------------------
+// z_t = x_t + sqrt(v) o nu_t; the policy sees phi(z_t), the dynamics GP [phi(x_t), u_t].  Without angles tm is the
+// identity map (A = 0).
+struct PnNoise {
+    const double* nu;                                   // [P,H,E] standard normals, shared by the restarts
+    double sv[MAXD];                                    // sqrt(v_i), i < E (0 beyond)
+};
+
+struct PnStep : PaStep {
+    PnNoise nz;
+    double* phiz;                                       // phi(z_t) [R P,H+1,Dh] for the gradients, or NULL
+};
+
+struct PnBwd : PaBwd {                                  // phib = NULL: phi_bar_x stays in gxt[:Dh]
+    const double* phiz;                                 // phi(z_t) [R P,H+1,Dh], the forward's
+    double* phibz;                                      // phi_bar_z,t [R P,Dh] (written when gxt is not NULL)
+};
+
+// grid (ceil(P / 128), R): the noisy forward step t (in place of pt_step_kernel / pa_step_kernel)
+int pn_step_launch(cudaStream_t st, dim3 grid, const PnStep& a);
+// grid (ceil(P / 128), R): the noisy reverse step t (in place of pg_step_kernel / pa_reverse_launch), two launches
+int pn_reverse_launch(cudaStream_t st, dim3 grid, const PnBwd& a);

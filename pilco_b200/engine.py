@@ -704,12 +704,17 @@ class ParticlePlan:
     ``angles``: angular state dimensions (pilco_particles_angles_*, DESIGN.md section 20).  The state x0, eps and traj
     then have the dynamics GP's output count E as their last dimension; the policy (``policy_spec["Ds"]`` = E +
     len(angles)) and the joint state-action terms see phi(x), the dynamics GP [phi(x), u].  The gradient of an unbatched
-    plan runs the batch-gradient call at R = 1."""
+    plan runs the batch-gradient call at R = 1.
+
+    ``measurement_noise``: variances v [E] >= 0 of a noisy state measurement (pilco_particles_noisy_*, DESIGN.md section
+    23): the policy sees phi(z_t), z_t = x_t + sqrt(v) o nu_t, while the dynamics GP and the rewards see the true state.
+    The plan then owns a nu buffer [P,H,E] of standard normals shared by the R policies, which ``set_inputs`` fills
+    (its ``nu`` is then required).  The gradients are conditioned on nu, as on x0 and eps."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
-                 estimator="pathwise", angles=None):
+                 estimator="pathwise", angles=None, measurement_noise=None):
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         if consistent and estimator == "score":
@@ -720,19 +725,27 @@ class ParticlePlan:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
         self.consistent = bool(consistent)
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise)
         pr, d = self.pr, device()
         P, H = self.P, self.H
         if self.consistent:
-            wsb = (lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)) if self.ang is None else
-                   lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(self.ang)))
+            if self.nz is not None:
+                wsb = lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), self._ang_ref(), C.byref(self.nz))
+            elif self.ang is None:
+                wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
+            else:
+                wsb = lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(self.ang))
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         elif not self.batched:                                  # the forward-only rollout (a batch has none)
-            wsb = (lib.pilco_particles_workspace_bytes(C.byref(pr)) if self.ang is None else
-                   lib.pilco_particles_angles_workspace_bytes(C.byref(pr), C.byref(self.ang)))
+            if self.nz is not None:
+                wsb = lib.pilco_particles_noisy_workspace_bytes(C.byref(pr), self._ang_ref(), C.byref(self.nz))
+            elif self.ang is None:
+                wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
+            else:
+                wsb = lib.pilco_particles_angles_workspace_bytes(C.byref(pr), C.byref(self.ang))
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
@@ -745,6 +758,10 @@ class ParticlePlan:
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.nz is not None:
+            f = (lib.pilco_particles_noisy_score_grad_workspace_bytes if self.estimator == "score" else
+                 lib.pilco_particles_noisy_batch_grad_workspace_bytes)
+            return int(f(C.byref(pr), self._ang_ref(), C.byref(self.nz), self.R))
         if self.ang is not None:
             f = (lib.pilco_particles_angles_score_grad_workspace_bytes if self.estimator == "score" else
                  lib.pilco_particles_angles_batch_grad_workspace_bytes)
@@ -755,16 +772,17 @@ class ParticlePlan:
             return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
         return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
 
-    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None):
+    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None):
         """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
-        The angles and the policy's width are checked first, before any device work."""
-        self.ang = None
+        The angles, the policy's width and the measurement noise are checked first, before any device work."""
+        self.ang, self.nz = None, None
         if angles is not None and len(angles) > 0:
             E = int(dyn.struct().E)
             self.ang = angles_struct(angles, E)
             if int(policy_spec["Ds"]) != E + self.ang.A:
                 raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
                                  % (self.ang.A, E + self.ang.A, int(policy_spec["Ds"])))
+        nz_var = _particle_noise(measurement_noise, int(dyn.struct().E))
         d = device()
         self.P, self.H, self.R = int(P), int(H), int(R)
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
@@ -800,6 +818,16 @@ class ParticlePlan:
         pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
         pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
         self.pr = pr
+        if nz_var is not None:                                  # nu [P,H,E], shared by the R policies
+            E = len(nz_var)
+            self.nu_buf = mk(P, Hb, E)
+            self.nz = _lib.ParticlesNoise()
+            for i, v in enumerate(nz_var):
+                self.nz.v.var[i] = float(v)
+            self.nz.nu = self.nu_buf.data_ptr()
+
+    def _ang_ref(self):
+        return C.byref(self.ang) if self.ang is not None else None
 
     def _grad_buffers(self, gwsb):
         """the pilco_particles_grad outputs and a gradient workspace of gwsb bytes (self.grad)"""
@@ -822,7 +850,16 @@ class ParticlePlan:
         ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        if self.ang is not None:
+        if self.nz is not None:
+            if self.estimator == "score":
+                check(lib.pilco_particles_noisy_score_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
+                                                                   self.R, C.byref(self.grad), stream_ptr()),
+                      "particles_noisy_score_grad_rollout")
+            else:
+                check(lib.pilco_particles_noisy_batch_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
+                                                                   self.R, C.byref(self.grad), stream_ptr()),
+                      "particles_noisy_batch_grad_rollout")
+        elif self.ang is not None:
             if self.estimator == "score":
                 check(lib.pilco_particles_angles_score_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
                                                                     C.byref(self.grad), stream_ptr()),
@@ -842,14 +879,27 @@ class ParticlePlan:
                   "particles_rollout_grad")
         return self.gbuf
 
-    def set_inputs(self, x0, eps):
+    def set_inputs(self, x0, eps, nu=None):
+        """x0 [P,Ds], eps [P,H,Ds] and, with measurement noise, nu [P,H,E] (required then, and only then)"""
+        if (nu is None) != (self.nz is None):
+            raise ValueError("particles: nu [P,H,E] is required with measurement_noise and only then")
         self.x0.copy_(dev(x0).reshape(self.P, self.Ds))
         if self.H > 0:
             self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
+            if nu is not None:
+                self.nu_buf.copy_(dev(nu).reshape(self.nu_buf.shape))
 
     def launch(self):
         if self.batched:
             raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
+        if self.nz is not None:
+            if self.consistent:
+                check(lib.pilco_particles_noisy_consistent_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
+                                                                   stream_ptr()), "particles_noisy_consistent_rollout")
+            else:
+                check(lib.pilco_particles_noisy_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
+                                                        stream_ptr()), "particles_noisy_rollout")
+            return
         if self.ang is not None:
             if self.consistent:
                 check(lib.pilco_particles_angles_consistent_rollout(C.byref(self.pr), C.byref(self.ang), stream_ptr()),
@@ -881,11 +931,12 @@ class ConsistentGradPlan(ParticlePlan):
     sums.  A plan whose workspace exceeds ``max_ws_bytes`` (default: half the free device memory) is a ValueError
     that names the bytes needed and the number of particles that would fit, raised before anything is allocated.
 
-    ``angles``: as ``ParticlePlan``."""
+    ``angles``, ``measurement_noise``: as ``ParticlePlan``."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None):
+    def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
+                 measurement_noise=None):
         self.consistent = True
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
@@ -903,6 +954,9 @@ class ConsistentGradPlan(ParticlePlan):
             return 0
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.nz is not None:
+            return int(lib.pilco_particles_noisy_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
+                                                                                C.byref(self.nz), self.R))
         if self.ang is not None:
             return int(lib.pilco_particles_angles_consistent_grad_workspace_bytes(C.byref(pr), C.byref(self.ang), self.R))
         return int(lib.pilco_particles_consistent_grad_workspace_bytes(C.byref(pr), self.R))
@@ -913,6 +967,11 @@ class ConsistentGradPlan(ParticlePlan):
     def launch_grad(self):
         """pilco_particles_rollout_consistent_grad: the consistent rollout (``outputs()``) and the pathwise gradient
         of value = mean return, returned as ``ParticlePlan.launch_grad`` returns it"""
+        if self.nz is not None:
+            check(lib.pilco_particles_noisy_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
+                                                                    self.R, C.byref(self.grad), stream_ptr()),
+                  "particles_noisy_consistent_grad_rollout")
+            return self.gbuf
         if self.ang is not None:
             check(lib.pilco_particles_angles_consistent_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
                                                                      C.byref(self.grad), stream_ptr()),
@@ -949,8 +1008,21 @@ def gp_predict_vjp(gp, Xs, gmean, gvar):
     return out
 
 
+def _particle_noise(measurement_noise, E):
+    """the measurement variances v [E] of the particle plans as a numpy array (None: no noise).  ValueError for a
+    wrong length, a non-finite or a negative value"""
+    if measurement_noise is None:
+        return None
+    v = np.asarray(measurement_noise, dtype=np.float64).reshape(-1)
+    if v.shape[0] != E:
+        raise ValueError("measurement_noise: expected %d variances (the state dimension), got %d" % (E, v.shape[0]))
+    if not np.all(np.isfinite(v)) or np.any(v < 0.0):
+        raise ValueError("measurement_noise: the variances must be finite and >= 0, got %r" % v)
+    return v
+
+
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,
-                      angles=None):
+                      angles=None, measurement_noise=None, nu=None):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
     step_risk [P,H], ret [P]) device tensors.
@@ -960,15 +1032,26 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     memory).  A particle's outputs do not depend on its batch, so the chunking does not change them.
 
     ``angles``: angular state dimensions, as ``ParticlePlan``: Ds is then the dynamics GP's output count E and the
-    policy takes E + len(angles) inputs."""
+    policy takes E + len(angles) inputs.
+
+    ``measurement_noise``: variances v [E] of the policy's measurement z = x + sqrt(v) o nu, as ``ParticlePlan``; ``nu``
+    [P,H,E] are its standard normals (required with it, for both samplers)."""
     x0, eps = dev(x0), dev(eps)
     if x0.dim() != 2 or eps.dim() != 3 or eps.shape[0] != x0.shape[0] or eps.shape[2] != x0.shape[1]:
         raise ValueError("particles_rollout: x0 must be [P,Ds] and eps [P,H,Ds], got %s and %s"
                          % (tuple(x0.shape), tuple(eps.shape)))
+    if (nu is None) != (measurement_noise is None):
+        raise ValueError("particles_rollout: nu [P,H,E] is required with measurement_noise and only then")
+    if nu is not None:
+        nu = dev(nu)
+        if tuple(nu.shape) != tuple(eps.shape):
+            raise ValueError("particles_rollout: nu must be [P,H,E] like eps, got %s" % (tuple(nu.shape),))
     if consistent:
-        return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles)
-    plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu, angles=angles)
-    plan.set_inputs(x0, eps)
+        return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles,
+                                             measurement_noise, nu)
+    plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu, angles=angles,
+                        measurement_noise=measurement_noise)
+    plan.set_inputs(x0, eps, nu)
     plan.launch()
     return plan.outputs()
 
@@ -986,7 +1069,8 @@ def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):
     return int(lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)))
 
 
-def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None):
+def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None,
+                                  measurement_noise=None, nu=None):
     P, H = int(x0.shape[0]), int(eps.shape[1])
     Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
     if angles is not None and len(angles) > 0:                 # the policy's width, before any allocation
@@ -994,6 +1078,7 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         A = angles_struct(angles, E).A
         if Ds != E + A:
             raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d" % (A, E + A, Ds))
+    _particle_noise(measurement_noise, int(dyn.struct().E))
     if max_ws_bytes is None:
         max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
     wsb = lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles)
@@ -1003,8 +1088,9 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
                          "bytes, more than max_ws_bytes=%d" % (H, dyn.n, wsb(1), max_ws_bytes))
     lo = _largest_fitting(fits, 1, P)
     if lo == P:
-        plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles)
-        plan.set_inputs(x0, eps)
+        plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles,
+                            measurement_noise=measurement_noise)
+        plan.set_inputs(x0, eps, nu)
         plan.launch()
         return plan.outputs()
     d = device()
@@ -1018,8 +1104,8 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         if plan is None or plan.P != p1 - p0:
             plan = None                                     # free the previous chunk's workspace first
             plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True,
-                                angles=angles)
-        plan.set_inputs(x0[p0:p1], eps[p0:p1])
+                                angles=angles, measurement_noise=measurement_noise)
+        plan.set_inputs(x0[p0:p1], eps[p0:p1], None if nu is None else nu[p0:p1])
         plan.launch()
         for o, c in zip(out, plan.outputs()):
             o[p0:p1].copy_(c)
