@@ -606,6 +606,46 @@ int    pilco_particles_noisy_score_grad_rollout(const pilco_particles* pr, const
                                                 const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
                                                 pilco_stream_t stream);
 
+/* PILCO's exploration objective in the particle rollouts (pilco_exploration above; DESIGN.md section 24).  Each call is
+ * the pilco_particles_noisy_* gradient of the same name (ang and nz may be NULL) whose value adds the sample spread of
+ * each step's reward.  Per restart r, over its P particles, for each ADD-channel term k with coefficient c_k at step
+ * t < H (state terms at the raw x_pt, joint terms at x~_pt = [phi(x_pt), u_pt]):
+ *   rbar_kt = (1/P) sum_p r_kpt,  s_kt^2 = 1/(P-1) sum_p (r_kpt - rbar_kt)^2   (unbiased, two-pass, fixed order)
+ *   sigma_t^2 = sum_k c_k^2 s_kt^2   (section 21's rule: covariances between terms ignored; MULT terms do not enter)
+ *   sigma_t   = sqrt(sigma_t^2) if sigma_t^2 > 1e-12, else 0 (with zero gradient)
+ *   value[r]  = (1/P) sum_p ret_p + b sum_t sigma_t   (the bonus summed in step order)
+ * ex->step_var [R,H] receives sigma_t^2 when not NULL.  The gradient is pathwise: the bonus adds
+ * a_kpt grad r_kpt, a_kpt = P b c_k^2 (r_kpt - rbar_kt) / ((P-1) sigma_t), to each particle's cotangent at each step.
+ * traj, act, step_reward, step_risk and ret keep their meaning and bits.  sigma_t is the square root of an unbiased
+ * variance, so it is biased low by O(1/P).  The call is inactive when ex == NULL or b == 0 with step_var == NULL: it is
+ * then the pilco_particles_noisy_* call, workspace sizes included; with b == 0 every output and gradient is bitwise that
+ * call's.  Validation before anything is enqueued: the noisy call's status codes up to its workspace check, then
+ * PILCO_ERR_DIM for a non-finite b, PILCO_ERR_UNSUPPORTED for an ADD-channel PILCO_REWARD_BOX term, PILCO_ERR_DIM for
+ * P < 2, then the workspace's codes.  The workspace is the noisy call's (with the angle layout when ang or nz is given)
+ * followed by sigma_t [R,H] and a table [R,H,n_rewards,2] (each slot rounded up to an even number of doubles); a
+ * workspace query returns 0 wherever its call would fail on the size or exploration checks. */
+size_t pilco_particles_explore_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                          const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                          int R);
+int    pilco_particles_explore_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                  const pilco_particles_noise* nz, const pilco_exploration* ex, int R,
+                                                  const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_explore_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                               const pilco_particles_noise* nz,
+                                                               const pilco_exploration* ex, int R);
+int    pilco_particles_explore_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                       const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                       int R, const pilco_particles_grad* g, pilco_stream_t stream);
+/* The per-step sample moments above over a forward that has already run: traj [R P,H+1,E] and act [R P,H,U] of R
+ * restarts of P particles (any sampler, chunked or not).  step_mean [R,H] = sum_k c_k rbar_kt and step_var [R,H] =
+ * sigma_t^2, each skipped when NULL.  Reads P, H, dyn.E, pol.Ds (= E + A), pol.U, the reward terms, traj and act of pr
+ * and nothing else.  PILCO_ERR_DIM for P < 2, H < 0, R outside [1, 65535], a bad angle map or widths
+ * (pol.Ds != E + A, E + A + U > PILCO_MAX_D), n_rewards outside [1, 8]; PILCO_ERR_NULL / PILCO_ERR_UNSUPPORTED for
+ * the reward terms as the rollouts check them and PILCO_ERR_UNSUPPORTED for an ADD-channel box term; PILCO_ERR_NULL
+ * for traj or act NULL with H > 0.  One launch (none at H = 0), no workspace. */
+int    pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,
+                                      double* step_var, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -27,6 +27,9 @@
 // Measurement noise at the policy's input (pilco_particles_noisy_*, DESIGN.md section 23): the same drivers take a
 // PnNoise next to the map (the identity map without angles) and launch the kernels of particles_noise.cu in place of the
 // angle step kernels; the policy inputs of the reductions are then the phi(z) history.
+// The exploration objective (pilco_particles_explore_*, DESIGN.md section 24): pg_run takes a PxOpt and launches the
+// kernels of particles_explore.cu beside the others (the moments after the forward, the bonus's share before each
+// reverse step kernel, the bonus into value after the reduction).
 #include <cmath>
 #include "particles.cuh"
 
@@ -319,24 +322,6 @@ __global__ void __launch_bounds__(PT_THREADS) pg_step_kernel(PgDev a) {
             }
         }
     }
-}
-
-// fixed-order block sum of NV values per thread (256 threads): warp butterflies, then warps in order -> out[0..NV)
-template <int NV>
-__device__ __forceinline__ void pg_block_sum(double (&v)[NV], double* red, double* out) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int c = 0; c < NV; ++c) {
-        const double s = warp_sum(v[c]);
-        if (lane == 0) red[c * 8 + warp] = s;
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < NV; c += 256) {
-        double s = 0.0;
-        for (int w = 0; w < 8; ++w) s += red[c * 8 + w];
-        out[c] = s;
-    }
-    __syncthreads();
 }
 
 struct PgRed : PtPolicy {
@@ -769,6 +754,7 @@ struct PtWs {
     size_t gsum;                                        // score: the per-(restart, step) sums of G
     size_t phi;                                         // angles, gradients: phi(x_t) [T,H+1,Dh]
     size_t phiz, phibz;                                 // noise, gradients: phi(z_t) [T,H+1,Dh]; phi_bar_z [T,Dh]
+    size_t sd, tab;                                     // exploration: sigma_t [R,H]; the bonus table [R,H,K,2]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -808,8 +794,9 @@ static PtWs pt_ws_layout(const pilco_particles* pr) {
 // VJP workspace at T = R P (never in use at the same time).  Rows are restart-major (row r P + p); nothing of size
 // [., n] is kept.  State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles);
 // angles: the phi history [T,H+1,Dh] after everything else; noise (with angles = true): then the phi(z) history
-// [T,H+1,Dh] and phi_bar_z [T,Dh].
-static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
+// [T,H+1,Dh] and phi_bar_z [T,Dh]; exploration: then sigma_t [R,H] and the bonus table [R,H,K,2] (K = n_rewards).
+static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false,
+                         bool explore = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -823,6 +810,7 @@ static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false, 
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
     if (angles) L.phi = take({T, H + 1, Dh});
     if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
+    if (explore) { L.sd = take({(size_t)R, H}); L.tab = take({(size_t)R, H, (size_t)pr->n_rewards, 2}); }
     L.total = L.pws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -849,8 +837,9 @@ static PtWs fs_ws_layout(const pilco_particles* pr) {
 // sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
 // [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
 // sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, noise: then the
-// phi(z) history and phi_bar_z, as pg_ws_layout)
-static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
+// phi(z) history and phi_bar_z, exploration: then sigma_t and the bonus table, as pg_ws_layout)
+static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false,
+                         bool explore = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -863,6 +852,7 @@ static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, 
     L.vws = take({L.vws_bytes / sizeof(double)});
     if (angles) L.phi = take({T, H + 1, Dh});
     if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
+    if (explore) { L.sd = take({(size_t)R, H}); L.tab = take({(size_t)R, H, (size_t)pr->n_rewards, 2}); }
     L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
     return L;
 }
@@ -1118,8 +1108,11 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // The step's VJP is pilco_gp_predict_vjp, or (consistent) fs_cond_bwd_kernel followed by fs_predict_vjp_kernel.
 // tm (angles): pa_reverse_launch's two kernels in place of pg_step, and the policy reduction over the phi history.
 // nz (noise): pn_reverse_launch's two kernels, and the policy reduction over the phi(z) history.
+// bonus (exploration, b != 0): px_bonus_kernel after each step's VJP (and pj_grad) adds the bonus's share to x_bar_{t+1}
+// and x~_bar_t, which the step kernel then carries into x_bar_t; the sweep starts as with joint terms (x_bar_H = 0 and
+// x~_bar_{H-1} = 0 passed to the step kernel, which ignores x_bar when x~_bar is NULL).
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
-                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
+                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1137,13 +1130,19 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     const bool joint = pt_has_joint(pr);
     PjDev j = pj_dev(pr, R);
     j.xh = ws + L.xt; j.gxt = ws + L.gxt;
-    if (joint && H > 0) {                               // x_bar_H = 0 and x~_bar_{H-1} = 0, then the joint terms' share
+    PxBonus xb;
+    if (bonus) {
+        xb.P = P; xb.H = H; xb.E = Ds; xb.D = D; xb.t = 0; xb.n_rewards = pr->n_rewards;
+        for (int k = 0; k < 8; ++k) xb.rewards[k] = k < pr->n_rewards ? pr->rewards[k] : pilco_reward_term();
+        xb.traj = pr->traj; xb.tab = ws + L.tab; xb.gx = b.gx; xb.gxt = ws + L.gxt;
+    }
+    if ((joint || bonus) && H > 0) {                    // x_bar_H = 0 and x~_bar_{H-1} = 0, then the joint terms' share
         cudaMemsetAsync(b.gx, 0, TDs * sizeof(double), st);
         cudaMemsetAsync(ws + L.gxt, 0, TD * sizeof(double), st);
     }
     for (int t = H - 1; t >= 0; --t) {
         b.t = t;
-        b.gxt = joint ? ws + L.gxt : nullptr;
+        b.gxt = joint || bonus ? ws + L.gxt : nullptr;
         if (t < H - 1) {
             const double* xt = ws + L.xt + (size_t)t * TD;
             int rc;
@@ -1162,6 +1161,10 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             j.t = t;
             launch_hi(pj_grad_kernel, grid, dim3(PT_THREADS), 0, st, j);
             CUDA_LAUNCH_CHECK();
+        }
+        if (bonus) {
+            xb.t = t; xb.xh = ws + L.xt + (size_t)t * TD;
+            if (const int rc = px_bonus_launch(st, grid, xb)) return rc;
         }
         b.var_prev = t > 0 ? ws + L.var + (size_t)(t - 1) * TDs : nullptr;
         if (nz) {
@@ -1183,19 +1186,48 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj);
 }
 
-// the validated gradient of R restarts: the forward with its history, then the reverse sweep
+// exploration (DESIGN.md section 24): b and where sigma_t^2 goes (NULL: nowhere), validated
+struct PxOpt {
+    double b;
+    double* step_var;
+};
+
+// the moments kernel's arguments over the forward's traj and act (tm: the angles' map, or the identity)
+static PxMom px_mom(const pilco_particles* pr, const TrigMap& tm, double b) {
+    PxMom m;
+    m.P = pr->P; m.H = pr->H; m.U = pr->pol.U; m.n_rewards = pr->n_rewards; m.tm = tm;
+    m.traj = pr->traj; m.act = pr->act;
+    for (int k = 0; k < 8; ++k) m.rewards[k] = k < pr->n_rewards ? pr->rewards[k] : pilco_reward_term();
+    m.b = b; m.step_mean = m.step_var = m.sd = m.tab = nullptr;
+    return m;
+}
+
+// the validated gradient of R restarts: the forward with its history, then the reverse sweep.  ex (exploration): the
+// moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
 static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool consistent,
-                  pilco_stream_t stream, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
-    const bool ang = tm != nullptr, noise = nz != nullptr;
-    const PtWs L = consistent ? fg_ws_layout(pr, R, ang, noise) : pg_ws_layout(pr, R, ang, noise);
+                  pilco_stream_t stream, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
+                  const PxOpt* ex = nullptr) {
+    const bool ang = tm != nullptr, noise = nz != nullptr, explore = ex != nullptr;
+    const PtWs L = consistent ? fg_ws_layout(pr, R, ang, noise, explore) : pg_ws_layout(pr, R, ang, noise, explore);
     if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
     if (consistent) {
         if (const int rc = fs_predict_prepare()) return rc;
         if (const int rc = fs_vjp_prepare()) return rc;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (const int rc = pt_forward(pr, R, (double*)g->ws, L, consistent, true, st, tm, nz)) return rc;
-    return pg_reverse(pr, R, g, L, consistent, st, tm, nz);
+    double* ws = (double*)g->ws;
+    if (const int rc = pt_forward(pr, R, ws, L, consistent, true, st, tm, nz)) return rc;
+    const bool bonus = explore && ex->b != 0.0;
+    if (explore) {
+        TrigMap id;
+        if (!tm) trig_map_make(pr->dyn.E, 0, nullptr, &id);            // 1 <= E <= PILCO_MAX_E once validated
+        PxMom m = px_mom(pr, tm ? *tm : id, ex->b);
+        m.step_var = ex->step_var; m.sd = ws + L.sd; m.tab = bonus ? ws + L.tab : nullptr;
+        if (const int rc = px_moments_launch(st, R, m)) return rc;
+    }
+    if (const int rc = pg_reverse(pr, R, g, L, consistent, st, tm, nz, bonus)) return rc;
+    if (bonus && pr->H > 0) return px_value_launch(st, R, pr->H, ex->b, ws + L.sd, g->value);
+    return PILCO_OK;
 }
 
 // the forward alone, R = 1 (tm: validated angles, nz: validated noise; the description is checked here)
@@ -1335,6 +1367,51 @@ static bool pn_sizes_ok(const pilco_particles* pr, const pilco_angles* ang, cons
     if (pr->dyn.E < 1 || pr->dyn.E > MAXE) return false;
     PnNoise n;
     return pn_noise(pr, nz, &n) == PILCO_OK;
+}
+
+// ---- exploration objective (DESIGN.md section 24) -------------------------------------------------------------------
+static bool px_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
+
+// the exploration's own checks, after the description's: PILCO_ERR_DIM for a non-finite b, PILCO_ERR_UNSUPPORTED for
+// an ADD-channel box term (section 21's rule), PILCO_ERR_DIM for P < 2 (no sample variance).  pr is not NULL.
+static int px_check(const pilco_particles* pr, const pilco_exploration* ex) {
+    if (!std::isfinite(ex->b)) return PILCO_ERR_DIM;
+    for (int k = 0; k < pr->n_rewards && k < 8; ++k)
+        if (pr->rewards[k].channel == PILCO_CHANNEL_ADD && pr->rewards[k].kind == PILCO_REWARD_BOX)
+            return PILCO_ERR_UNSUPPORTED;
+    if (pr->P < 2) return PILCO_ERR_DIM;
+    return PILCO_OK;
+}
+
+// an active explore call's workspace (0 where the call would fail on the size or exploration checks): the noisy
+// call's layout (angles flag: angles or noise; noise flag: noise) with sigma_t and the bonus table after it
+static size_t px_ws_bytes(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                          const pilco_exploration* ex, int R, bool consistent) {
+    const size_t base = consistent ? pilco_particles_noisy_consistent_grad_workspace_bytes(pr, ang, nz, R)
+                                   : pilco_particles_noisy_batch_grad_workspace_bytes(pr, ang, nz, R);
+    if (base == 0 || px_check(pr, ex)) return 0;
+    const bool angles = nz || !pa_none(ang), noise = nz != nullptr;
+    return (consistent ? fg_ws_layout(pr, R, angles, noise, true) : pg_ws_layout(pr, R, angles, noise, true)).total;
+}
+
+// an active explore gradient: the noisy call's checks up to its workspace (nz NULL: the angle or plain call's), then
+// the exploration's, then pg_run with the path the noisy call takes
+static int px_grad(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                   const pilco_exploration* ex, int R, const pilco_particles_grad* g, bool consistent,
+                   pilco_stream_t stream) {
+    TrigMap tm; PnNoise n;
+    const bool none = pa_none(ang);
+    if (nz) {
+        if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
+    } else {
+        if (!pr) return PILCO_ERR_NULL;
+        if (!none)
+            if (const int rc = pa_map(pr, ang, &tm)) return rc;
+        if (const int rc = pg_validate(pr, R, g, true, none ? 0 : tm.A)) return rc;
+    }
+    if (const int rc = px_check(pr, ex)) return rc;
+    const PxOpt o = {ex->b, ex->step_var};
+    return pg_run(pr, R, g, consistent, stream, nz || !none ? &tm : nullptr, nz ? &n : nullptr, &o);
 }
 
 extern "C" {
@@ -1535,6 +1612,60 @@ int pilco_particles_noisy_score_grad_rollout(const pilco_particles* pr, const pi
     TrigMap tm; PnNoise n;
     if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
     return ps_run(pr, R, g, stream, &tm, &n);
+}
+
+
+// ---- the explore twins: an inactive ex (NULL, or b == 0 with step_var NULL) is the noisy call ------------------------
+size_t pilco_particles_explore_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                          const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                          int R) {
+    if (!px_active(ex)) return pilco_particles_noisy_batch_grad_workspace_bytes(pr, ang, nz, R);
+    return px_ws_bytes(pr, ang, nz, ex, R, false);
+}
+
+int pilco_particles_explore_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                               const pilco_particles_noise* nz, const pilco_exploration* ex, int R,
+                                               const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (!px_active(ex)) return pilco_particles_noisy_batch_grad_rollout(pr, ang, nz, R, g, stream);
+    return px_grad(pr, ang, nz, ex, R, g, false, stream);
+}
+
+size_t pilco_particles_explore_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                               const pilco_particles_noise* nz,
+                                                               const pilco_exploration* ex, int R) {
+    if (!px_active(ex)) return pilco_particles_noisy_consistent_grad_workspace_bytes(pr, ang, nz, R);
+    return px_ws_bytes(pr, ang, nz, ex, R, true);
+}
+
+int pilco_particles_explore_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                    const pilco_particles_noise* nz, const pilco_exploration* ex, int R,
+                                                    const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (!px_active(ex)) return pilco_particles_noisy_consistent_grad_rollout(pr, ang, nz, R, g, stream);
+    return px_grad(pr, ang, nz, ex, R, g, true, stream);
+}
+
+int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,
+                                   double* step_var, pilco_stream_t stream) {
+    if (!pr) return PILCO_ERR_NULL;
+    const int E = pr->dyn.E, U = pr->pol.U;
+    TrigMap tm;
+    const int A = pa_none(ang) ? 0 : ang->A;
+    if (pr->P < 2 || pr->H < 0 || R < 1 || R > 65535 || U < 1 || trig_map_make(E, A, A ? ang->dims : nullptr, &tm) ||
+        E > MAXE || pr->pol.Ds != E + A || E + A + U > MAXD)
+        return PILCO_ERR_DIM;
+    if (pr->n_rewards < 1 || pr->n_rewards > 8) return PILCO_ERR_DIM;
+    for (int k = 0; k < pr->n_rewards; ++k) {
+        const pilco_reward_term& rt = pr->rewards[k];
+        if (!rt.W) return PILCO_ERR_NULL;
+        if (!reward_kind_known(rt.kind)) return PILCO_ERR_UNSUPPORTED;
+        if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
+        if (reward_needs_t(rt.kind) && !rt.t) return PILCO_ERR_NULL;
+        if (rt.channel == PILCO_CHANNEL_ADD && rt.kind == PILCO_REWARD_BOX) return PILCO_ERR_UNSUPPORTED;
+    }
+    if (pr->H > 0 && (!pr->traj || !pr->act)) return PILCO_ERR_NULL;
+    PxMom m = px_mom(pr, tm, 0.0);
+    m.step_mean = step_mean; m.step_var = step_var;
+    return px_moments_launch((cudaStream_t)stream, R, m);
 }
 
 }  // extern "C"

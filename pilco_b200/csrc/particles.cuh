@@ -1,6 +1,6 @@
-// particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu and particles_noise.cu share: the
-// per-particle argument structs, the reward value at a point, and the angle and noise kernels' launchers (DESIGN.md
-// sections 11, 12, 20 and 23).
+// particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu and
+// particles_explore.cu share: the per-particle argument structs, the reward value at a point, the fixed-order block
+// sum, and the angle, noise and exploration kernels' launchers (DESIGN.md sections 11, 12, 20, 23 and 24).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -58,6 +58,24 @@ __device__ __forceinline__ double pt_reward_value(const pilco_reward_term& rt, c
     return exp(-0.5 * quad);
 }
 
+// fixed-order block sum of NV values per thread (256 threads): warp butterflies, then warps in order -> out[0..NV)
+template <int NV>
+__device__ __forceinline__ void pg_block_sum(double (&v)[NV], double* red, double* out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int c = 0; c < NV; ++c) {
+        const double s = warp_sum(v[c]);
+        if (lane == 0) red[c * 8 + warp] = s;
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < NV; c += 256) {
+        double s = 0.0;
+        for (int w = 0; w < 8; ++w) s += red[c * 8 + w];
+        out[c] = s;
+    }
+    __syncthreads();
+}
+
 // the reverse sweep's step arguments (pg_step_kernel, particles.cu)
 struct PgDev : PtPolicy {
     int t;
@@ -112,3 +130,36 @@ struct PnBwd : PaBwd {                                  // phib = NULL: phi_bar_
 int pn_step_launch(cudaStream_t st, dim3 grid, const PnStep& a);
 // grid (ceil(P / 128), R): the noisy reverse step t (in place of pg_step_kernel / pa_reverse_launch), two launches
 int pn_reverse_launch(cudaStream_t st, dim3 grid, const PnBwd& a);
+
+// ---- exploration objective (particles_explore.cu, DESIGN.md section 24) -----------------------------------------------
+// Per restart r and step t < H over the restart's P particles, for each ADD-channel term k (K = n_rewards slots; MULT
+// slots stay 0): r_kpt at x_pt (state terms, raw) or x~_pt = [phi(x_pt), u_pt] (joint terms), its mean and unbiased
+// sample variance, sigma_t^2 = sum_k c_k^2 s_kt^2 and sigma_t = sqrt(sigma_t^2) (0 at or below 1e-12).
+struct PxMom {
+    int P, H, U, n_rewards;
+    TrigMap tm;                                         // tm.Ds = E; the identity map without angles
+    const double* traj; const double* act;              // [R P,H+1,E], [R P,H,U]
+    pilco_reward_term rewards[8];
+    double b;
+    double* step_mean; double* step_var;                // [R,H] sum_k c_k mean_kt and sigma_t^2, or NULL
+    double* sd;                                         // [R,H] sigma_t, or NULL
+    double* tab;                                        // [R,H,K,2] (mean_kt, P b c_k^2 / ((P-1) sigma_t)), or NULL
+};
+
+// the bonus's share of step t's reverse step: sum_k a_kpt grad r_k, a_kpt = tab_kt.w (r_kpt - mean_kt)
+struct PxBonus {
+    int P, H, E, D, t, n_rewards;
+    pilco_reward_term rewards[8];
+    const double* traj;                                 // [R P,H+1,E]
+    const double* xh;                                   // x~_t [R P,D] (the forward's history slot of step t)
+    const double* tab;                                  // [R,H,K,2]
+    double* gx;                                         // [R P,E] state terms' share
+    double* gxt;                                        // [R P,D] joint terms' share
+};
+
+// grid (H, R), 256 threads; H = 0 launches nothing
+int px_moments_launch(cudaStream_t st, int R, const PxMom& a);
+// grid (ceil(P / 128), R)
+int px_bonus_launch(cudaStream_t st, dim3 grid, const PxBonus& a);
+// value[r] += b sum_t sd[r,t], step order
+int px_value_launch(cudaStream_t st, int R, int H, double b, const double* sd, double* value);

@@ -709,14 +709,25 @@ class ParticlePlan:
     ``measurement_noise``: variances v [E] >= 0 of a noisy state measurement (pilco_particles_noisy_*, DESIGN.md section
     23): the policy sees phi(z_t), z_t = x_t + sqrt(v) o nu_t, while the dynamics GP and the rewards see the true state.
     The plan then owns a nu buffer [P,H,E] of standard normals shared by the R policies, which ``set_inputs`` fills
-    (its ``nu`` is then required).  The gradients are conditioned on nu, as on x0 and eps."""
+    (its ``nu`` is then required).  The gradients are conditioned on nu, as on x0 and eps.
+
+    ``exploration``: a float b (0.0 included) selects PILCO's exploration objective in ``launch_grad()``
+    (pilco_particles_explore_*, DESIGN.md section 24): value = mean return + b sum_t sigma_t, sigma_t^2 the sum over the
+    additive terms of c_k^2 times the sample variance of term k over the restart's P particles at step t, with its
+    pathwise gradient.  The plan then owns ``step_var`` [R, max(H,1)], which each ``launch_grad()`` fills with
+    sigma_t^2.  At b = 0 every other output and gradient is bitwise the plan's without exploration.  It needs
+    ``grad=True``, P >= 2 and no additive box term; ``estimator="score"`` with it is a ValueError.  ``None``: no
+    exploration."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
-                 estimator="pathwise", angles=None, measurement_noise=None):
+                 estimator="pathwise", angles=None, measurement_noise=None, exploration=None):
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
+        if exploration is not None and (estimator == "score" or not grad):
+            raise ValueError("particles: exploration is an objective of the pathwise gradient: it needs grad=True and "
+                             "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
         if consistent and estimator == "score":
             raise ValueError("particles: the score-function gradient of the consistent (function-sample) rollout "
                              "is not available; use estimator='pathwise'")
@@ -725,7 +736,7 @@ class ParticlePlan:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
         self.consistent = bool(consistent)
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration)
         pr, d = self.pr, device()
         P, H = self.P, self.H
         if self.consistent:
@@ -758,6 +769,9 @@ class ParticlePlan:
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.ex is not None:
+            return int(lib.pilco_particles_explore_batch_grad_workspace_bytes(C.byref(pr), self._ang_ref(), self._nz_ref(),
+                                                                              C.byref(self.ex), self.R))
         if self.nz is not None:
             f = (lib.pilco_particles_noisy_score_grad_workspace_bytes if self.estimator == "score" else
                  lib.pilco_particles_noisy_batch_grad_workspace_bytes)
@@ -772,10 +786,13 @@ class ParticlePlan:
             return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
         return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
 
-    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None):
+    def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None,
+                  exploration=None):
         """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
-        The angles, the policy's width and the measurement noise are checked first, before any device work."""
-        self.ang, self.nz = None, None
+        The angles, the policy's width, the measurement noise and the exploration weight are checked first, before any
+        device work."""
+        self.ang, self.nz, self.ex = None, None, None
+        b = _particle_exploration(exploration, reward_terms, P)
         if angles is not None and len(angles) > 0:
             E = int(dyn.struct().E)
             self.ang = angles_struct(angles, E)
@@ -825,9 +842,15 @@ class ParticlePlan:
             for i, v in enumerate(nz_var):
                 self.nz.v.var[i] = float(v)
             self.nz.nu = self.nu_buf.data_ptr()
+        if b is not None:                                       # sigma_t^2 [R, max(H,1)], also for an unbatched plan
+            self.step_var = mk(R, Hb)
+            self.ex = _lib.Exploration(b, self.step_var.data_ptr())
 
     def _ang_ref(self):
         return C.byref(self.ang) if self.ang is not None else None
+
+    def _nz_ref(self):
+        return C.byref(self.nz) if self.nz is not None else None
 
     def _grad_buffers(self, gwsb):
         """the pilco_particles_grad outputs and a gradient workspace of gwsb bytes (self.grad)"""
@@ -847,10 +870,15 @@ class ParticlePlan:
         gradient of value = mean return w.r.t. the policy parameters with x0 and eps fixed.  Returns the device tensors
         {'value' [1], 'W' [U,Ds], 'b' [U]} (linear) or {'value', 'X' [bf,Ds], 'Y' [bf,U], 'ell' [U,Ds]} (RBF, constrained
         lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R]).
-        ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout."""
+        ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout.
+        With ``exploration``: value and gradient of the exploration objective, and sigma_t^2 in ``step_var``."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        if self.nz is not None:
+        if self.ex is not None:
+            check(lib.pilco_particles_explore_batch_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
+                                                                 C.byref(self.ex), self.R, C.byref(self.grad),
+                                                                 stream_ptr()), "particles_explore_batch_grad_rollout")
+        elif self.nz is not None:
             if self.estimator == "score":
                 check(lib.pilco_particles_noisy_score_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
                                                                    self.R, C.byref(self.grad), stream_ptr()),
@@ -931,12 +959,13 @@ class ConsistentGradPlan(ParticlePlan):
     sums.  A plan whose workspace exceeds ``max_ws_bytes`` (default: half the free device memory) is a ValueError
     that names the bytes needed and the number of particles that would fit, raised before anything is allocated.
 
-    ``angles``, ``measurement_noise``: as ``ParticlePlan``."""
+    ``angles``, ``measurement_noise``, ``exploration``: as ``ParticlePlan`` (pilco_particles_explore_consistent_grad_*
+    with exploration)."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
-                 measurement_noise=None):
+                 measurement_noise=None, exploration=None):
         self.consistent = True
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
@@ -954,6 +983,10 @@ class ConsistentGradPlan(ParticlePlan):
             return 0
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.ex is not None:
+            return int(lib.pilco_particles_explore_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
+                                                                                   self._nz_ref(), C.byref(self.ex),
+                                                                                   self.R))
         if self.nz is not None:
             return int(lib.pilco_particles_noisy_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
                                                                                 C.byref(self.nz), self.R))
@@ -966,7 +999,14 @@ class ConsistentGradPlan(ParticlePlan):
 
     def launch_grad(self):
         """pilco_particles_rollout_consistent_grad: the consistent rollout (``outputs()``) and the pathwise gradient
-        of value = mean return, returned as ``ParticlePlan.launch_grad`` returns it"""
+        of value = mean return (with ``exploration``: the exploration objective, and sigma_t^2 in ``step_var``),
+        returned as ``ParticlePlan.launch_grad`` returns it"""
+        if self.ex is not None:
+            check(lib.pilco_particles_explore_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
+                                                                      C.byref(self.ex), self.R, C.byref(self.grad),
+                                                                      stream_ptr()),
+                  "particles_explore_consistent_grad_rollout")
+            return self.gbuf
         if self.nz is not None:
             check(lib.pilco_particles_noisy_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
                                                                     self.R, C.byref(self.grad), stream_ptr()),
@@ -1019,6 +1059,61 @@ def _particle_noise(measurement_noise, E):
     if not np.all(np.isfinite(v)) or np.any(v < 0.0):
         raise ValueError("measurement_noise: the variances must be finite and >= 0, got %r" % v)
     return v
+
+
+def _particle_exploration(exploration, reward_terms, P):
+    """the exploration weight b of the particle plans as a float (None: no exploration).  ValueError for a non-finite
+    b, an additive box term (no gradient, and section 21's rule) or fewer than 2 particles (no sample variance)"""
+    if exploration is None:
+        return None
+    b = float(exploration)
+    if not np.isfinite(b):
+        raise ValueError("exploration: b must be finite, got %r" % exploration)
+    _no_additive_box(reward_terms)
+    if int(P) < 2:
+        raise ValueError("exploration: the sample variance of the step rewards needs P >= 2 particles, got %d" % int(P))
+    return b
+
+
+def _no_additive_box(reward_terms):
+    for k, rt in enumerate(reward_terms):
+        if rt["kind"] == _lib.REWARD_BOX and int(rt.get("channel", _lib.CHANNEL_ADD)) == _lib.CHANNEL_ADD:
+            raise ValueError("exploration: reward term %d is an additive box term, which the reward variance leaves "
+                             "out of its rule; use it in the multiplicative channel (SafePILCO) or leave exploration "
+                             "off" % k)
+
+
+def particle_reward_moments(reward_terms, traj, act, angles=None):
+    """pilco_particles_reward_moments: the per-step sample moments of the reward over particles that have already been
+    rolled out -> (mean [..., H], var [..., H]) device tensors.  ``traj`` [..., P, H+1, E] and ``act`` [..., P, H, U]
+    are any sampler's outputs (a leading restart dimension, or none), chunked or not.  mean_t = sum_k c_k rbar_kt and
+    var_t = sum_k c_k^2 s_kt^2 over the additive terms, s_kt^2 the unbiased variance of term k over the P particles
+    (DESIGN.md section 24): the sampled counterparts of the moment-matching rollout's E[r_t] and sigma_t^2.
+    ``angles``: the angular state dimensions the policy saw (the joint terms are evaluated at [phi(x), u])."""
+    if len(traj.shape) < 3 or len(act.shape) != len(traj.shape) or tuple(act.shape[:-2]) != tuple(traj.shape[:-2]) \
+            or act.shape[-2] != traj.shape[-2] - 1:
+        raise ValueError("particle_reward_moments: expected traj [..., P, H+1, E] and act [..., P, H, U], got %s and %s"
+                         % (tuple(traj.shape), tuple(act.shape)))
+    lead = tuple(traj.shape[:-3])
+    P, H, E, U = int(traj.shape[-3]), int(traj.shape[-2]) - 1, int(traj.shape[-1]), int(act.shape[-1])
+    if P < 2:
+        raise ValueError("particle_reward_moments: the sample variance needs P >= 2 particles, got %d" % P)
+    _no_additive_box(reward_terms)
+    traj, act = dev(traj), dev(act)
+    R = int(np.prod(lead)) if lead else 1
+    ang = angles_struct(angles, E)
+    pr = _lib.Particles()
+    pr.P, pr.H = P, H
+    pr.dyn.E = E
+    pr.pol.Ds, pr.pol.U = E + (ang.A if ang is not None else 0), U
+    keep = _fill_rewards(pr, reward_terms)                     # noqa: F841 -- the terms' device tensors stay alive
+    Hb = max(H, 1)
+    mean = torch.zeros((R, Hb), dtype=F64, device=device())
+    var = torch.zeros((R, Hb), dtype=F64, device=device())
+    pr.traj, pr.act = traj.data_ptr(), act.data_ptr()
+    check(lib.pilco_particles_reward_moments(C.byref(pr), C.byref(ang) if ang is not None else None, R, ptr(mean),
+                                             ptr(var), stream_ptr()), "particles_reward_moments")
+    return mean[:, :H].reshape(*lead, H), var[:, :H].reshape(*lead, H)
 
 
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,

@@ -273,18 +273,21 @@ class PILCO:
         out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
         return ParticleTrajectories(*out)
 
-    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False, estimator="pathwise"):
+    def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False, estimator="pathwise",
+                       exploration=None):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
         (from ``np.random`` when None): the same seed gives the same particles to every caller.  ``consistent``
-        (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``: ParticlePlan's."""
+        (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``, ``exploration``:
+        ParticlePlan's."""
         dyn = self.mgpr.device_gp()
         x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, what)
         terms, mult_mu = self.reward_spec()
         if consistent:
-            plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu)
+            plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
+                                             exploration=exploration)
         else:
             plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
-                                       grad=grad, estimator=estimator)
+                                       grad=grad, estimator=estimator, exploration=exploration)
         plan.set_inputs(x0, eps)
         return plan
 
@@ -319,7 +322,39 @@ class PILCO:
         return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
                                g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
 
-    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, estimator="pathwise"):
+    def sample_reward_moments(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
+        """Sample mean and variance of each step's reward over the particles of ``sample_trajectories`` (the same seed
+        gives the same particles): the sampled counterpart of ``predict_reward_moments``.  mean_t is the mean of the
+        step rewards (``sample_trajectories(...).rewards.mean(0)`` up to rounding) and var_t = sum_k c_k^2 s_kt^2 over
+        the additive terms, s_kt^2 the unbiased sample variance of term k at step t (covariances between terms ignored,
+        as ``predict_reward_moments``; the multiplicative terms of SafePILCO do not enter; DESIGN.md section 24).
+        ``consistent``: the particles of ``sample_trajectories(..., consistent=True)``; a chunked rollout gives the
+        statistics of all num_samples particles.  Needs num_samples >= 2; a reward with an additive box term is a
+        ValueError.  -> (mean [n], var [n]) host arrays."""
+        from ..params import HostArray
+        self._no_angles("sample_reward_moments")
+        self._no_noise("sample_reward_moments")
+        if int(num_samples) < 2:
+            raise ValueError("sample_reward_moments: the sample variance needs num_samples >= 2 (num_samples=%d)"
+                             % int(num_samples))
+        terms, mult_mu = self.reward_spec()
+        engine._no_additive_box(terms)
+        if consistent:
+            import torch
+            x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, "sample_reward_moments")
+            if eps is None:                                     # n = 0
+                eps = torch.zeros((int(num_samples), 0, self.state_dim), dtype=engine.F64, device=x0.device)
+            out = engine.particles_rollout(self.mgpr.device_gp(), self.policy_spec(), terms, x0, eps, mult_mu=mult_mu,
+                                           consistent=True)
+        else:
+            plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_reward_moments")
+            plan.launch()
+            out = plan.outputs()
+        mean, var = engine.particle_reward_moments(terms, out[0], out[1])
+        return mean.cpu().numpy().view(HostArray), var.cpu().numpy().view(HostArray)
+
+    def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, estimator="pathwise",
+                               exploration=0.0):
         """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
         are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
         d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
@@ -335,6 +370,12 @@ class PILCO:
         1 / sigma^2 where the model is confident (a small predicted variance), so it can need many more samples than
         the pathwise estimate on smooth rewards.  ``consistent=True`` with ``estimator="score"`` is a ValueError.
 
+        ``exploration``: a weight b != 0 makes value PILCO's exploration objective over the particles, mean return +
+        b sum_t sigma_t, sigma_t the sample spread of step t's reward (``sample_reward_moments``), and grad its pathwise
+        gradient (DESIGN.md section 24).  It does not read ``self.exploration``: pass ``exploration=self.exploration``
+        for the sampled counterpart of ``optimize_policy``'s objective.  b != 0 needs num_samples >= 2, the pathwise
+        estimator and no additive box term (ValueError otherwise); b = 0 is the call without it.
+
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
         self._no_angles("sample_policy_gradient")
@@ -345,8 +386,9 @@ class PILCO:
         if consistent and estimator == "score":
             raise ValueError("sample_policy_gradient: the score-function estimator is not available for the consistent "
                              "(function-sample) particles; use estimator='pathwise'")
+        b = float(exploration)
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
-                                   consistent=consistent, estimator=estimator)
+                                   consistent=consistent, estimator=estimator, exploration=None if b == 0.0 else b)
         g = plan.launch_grad()
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
@@ -392,7 +434,8 @@ class PILCO:
         g = plan.backward()
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
-    def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False):
+    def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False,
+                                exploration=0.0):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -409,13 +452,21 @@ class PILCO:
         ``consistent=True``: the particles follow one function drawn from the dynamics posterior each, as
         ``sample_trajectories(..., consistent=True)`` (Deep PILCO's objective), so model errors do not average out
         along a trajectory.  A lock-step group's workspace is O(restarts num_samples horizon^2 E n); a group that
-        needs more than half the free device memory is a ValueError naming the num_samples that would fit."""
+        needs more than half the free device memory is a ValueError naming the num_samples that would fit.
+
+        ``exploration``: a weight b != 0 optimises PILCO's exploration objective over the particles, mean return +
+        b sum_t sigma_t (``sample_policy_gradient``'s), and returns its in-sample value.  It does not read
+        ``self.exploration``: pass ``exploration=self.exploration`` for the sampled counterpart of ``optimize_policy``."""
         from functools import partial
         from .. import policy_opt
         self._no_angles("optimize_policy_sampled")
         self._no_noise("optimize_policy_sampled")
         if int(num_samples) < 1:
             raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
+        b = float(exploration)
+        if not np.isfinite(b) or (b != 0.0 and int(num_samples) < 2):
+            raise ValueError("optimize_policy_sampled: exploration needs a finite b and num_samples >= 2 (b=%r, "
+                             "num_samples=%d)" % (exploration, int(num_samples)))
         terms, _ = self.reward_spec()
         if any(t["kind"] == _lib.REWARD_BOX for t in terms):
             raise ValueError("optimize_policy_sampled: the reward has box (risk) terms, which carry no pathwise "
@@ -430,7 +481,8 @@ class PILCO:
                                             "optimize_policy_sampled")
             best_flat, best_value, _ = policy_opt.optimize(
                 self, maxiter=maxiter, restarts=restarts, flats0=flats0,
-                evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent))
+                evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent,
+                                  exploration=None if b == 0.0 else b))
             self.controller.set_flat(best_flat)
         finally:
             for p in mgpr_trainable:

@@ -211,9 +211,12 @@ class ParticleEvaluator(_FlatEvaluator):
     held fixed, so the objective is a deterministic function of the parameters: one batched device call
     (pilco_particles_rollout_batch_grad) evaluates every restart.  ``consistent=True``: each particle follows one
     function drawn from the dynamics posterior (pilco_particles_rollout_consistent_grad through
-    ``engine.ConsistentGradPlan``).  Box terms carry no pathwise gradient, so a reward with them is rejected."""
+    ``engine.ConsistentGradPlan``).  Box terms carry no pathwise gradient, so a reward with them is rejected.
+    ``exploration``: a float b makes the objective PILCO's exploration objective over the particles, mean return +
+    b sum_t sigma_t with sigma_t the sample spread of step t's reward (pilco_particles_explore_*, DESIGN.md section 24);
+    None (the default) is the mean return."""
 
-    def __init__(self, pilco, R, x0, eps, consistent=False):
+    def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None):
         terms, mult_mu = pilco.reward_spec()
         if any(t["kind"] == _lib.REWARD_BOX for t in terms):
             raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
@@ -225,10 +228,10 @@ class ParticleEvaluator(_FlatEvaluator):
         x0 = engine.dev(x0)
         if consistent:
             self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
-                                                  int(pilco.horizon), mult_mu=mult_mu, R=R)
+                                                  int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration)
         else:
             self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
-                                            mult_mu=mult_mu, grad=True, R=R)
+                                            mult_mu=mult_mu, grad=True, R=R, exploration=exploration)
         self.plan.set_inputs(x0, eps)
         self._setup_io()
 
