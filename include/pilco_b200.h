@@ -109,7 +109,10 @@ int pilco_mm_backward_taped(const pilco_gp_model* gp, int R, const double* m, co
  * iK is written with leading dimension ldk (zero padded; pass NULL to get beta only).
  * ws: scratch of pilco_gp_factorize_workspace_bytes(n, E, B) bytes; on return its first
  * B*E*ldw*ldw doubles (ldw = pilco_pad_n(n)) hold the Cholesky factors L (lower triangles), which
- * pilco_rollout_backward needs for the RBF policy (pilco_rollout_grad.pol_L).
+ * pilco_rollout_backward needs for the RBF policy (pilco_rollout_grad.pol_L), and when iK is requested the next
+ * B*E*ldw*ldw doubles hold R = L^-1 (zero above the diagonal and in the padding), which pilco_gp_append_tri extends.
+ * n <= 28000 (the substitution for beta keeps a right-hand side in shared memory); info[b] bit 1: a pivot of
+ * batch element b was not positive (its outputs are then meaningless, the other elements' are unaffected).
  */
 size_t pilco_gp_factorize_workspace_bytes(int n, int E, int B);
 int pilco_gp_factorize(int n, int D, int E, int B,
@@ -125,16 +128,20 @@ int pilco_gp_factorize(int n, int D, int E, int B,
 
 /* Incremental set_data (SURVEY section 8f-2): k rows appended to the data of a factorised model with UNCHANGED
  * hyper-parameters (pilco/models/mgpr.py:38-45; examples/inv_double_pendulum.py:102-103, swimmer.py:87-88 append the
- * rows of each new episode).  X [n0+k, D] and Y [n0+k, E] hold the old rows first; iK_old [E,ldk_old,ldk_old] is the
- * inverse pilco_gp_factorize / an earlier append produced.  Writes the new zero-padded inverse iK_new
- * [E,ldk_new,ldk_new] (ldk_new >= pilco_pad_n(n0+k), out of place) and beta_new [E,n0+k] by the block-inverse
- * (Schur complement) update: O(n^2 k) instead of O(n^3).  info[0] bit 1: Schur complement not positive definite. */
-size_t pilco_gp_append_workspace_bytes(int n0, int k, int E);
-int pilco_gp_append(int n0, int k, int D, int E,
+ * rows of each new episode).  X [n0+k, D] and Y [n0+k, E] hold the old rows first.  R_old [E,ldr_old,ldr_old] is the
+ * lower-triangular inverse Cholesky factor L^-1 of the old model (zero above the diagonal and in the padding):
+ * pilco_gp_factorize leaves it in its workspace right after the factors L (second B*E*ldw*ldw doubles), an earlier
+ * append in its R_new.  iK_old [E,ldk_old,ldk_old] is the old inverse.  Writes R_new [E,ldr_new,ldr_new] (zero
+ * padded), the new zero-padded inverse iK_new [E,ldk_new,ldk_new] (both leading dimensions >= pilco_pad_n(n0+k), out
+ * of place) and beta_new [E,n0+k] by extending R with one block row: O(n^2 k) instead of O(n^3), as accurate as a
+ * refactorisation after any number of appends.  info[0] bit 1: the new rows' Schur complement is not positive
+ * definite. */
+size_t pilco_gp_append_tri_workspace_bytes(int n0, int k, int E);
+int pilco_gp_append_tri(int n0, int k, int D, int E,
                     const double* X, const double* Y,
                     const double* ell, const double* sf2, const double* sn2,
-                    const double* iK_old, int ldk_old,
-                    double* iK_new, int ldk_new, double* beta_new, int* info,
+                    const double* R_old, int ldr_old, const double* iK_old, int ldk_old,
+                    double* R_new, int ldr_new, double* iK_new, int ldk_new, double* beta_new, int* info,
                     void* ws, size_t ws_bytes, pilco_stream_t stream);
 
 /* GP training objective (SURVEY section 8f-1): nlml[b,e] = -log p(y_e | X, theta_be) and its gradient w.r.t. the
@@ -177,7 +184,7 @@ int pilco_fitc_factorize(int N, int Mi, int D, int E,
 /* ---- prediction at deterministic inputs -------------------------------------------------------
  * Stands in for gpflow GPR.predict_f / GPRFITC.predict_f, which the reference's users call on the output models of
  * MGPR / SMGPR (pilco/models/mgpr.py:28-36, smgpr.py:16-22) to check the learnt dynamics: the posterior of outputs
- * e0 .. e0+ne-1 of an unbatched mode-0 model with iK (pilco_gp_factorize, pilco_gp_append or pilco_fitc_factorize) at
+ * e0 .. e0+ne-1 of an unbatched mode-0 model with iK (pilco_gp_factorize, pilco_gp_append_tri or pilco_fitc_factorize) at
  * T inputs Xs [T,D]:  mean = k*' beta_e,  var = sf2_e - k*' iK_e k*  (latent f; the caller adds sn2 for y), or with
  * full_cov the [ne,T,T] covariance K** - K* iK_e K*'.  A point's mean and variance do not depend on T, on its row in
  * Xs or on which outputs are requested (fixed-order reductions; diagonal path).  PILCO_ERR_UNSUPPORTED: mode != 0,

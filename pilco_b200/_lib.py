@@ -111,9 +111,9 @@ SIGNATURES = {
     "pilco_gp_factorize_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
     "pilco_gp_factorize": (C.c_int, [C.c_int] * 4 + [c_dp, c_ll] * 5 + [c_dp, C.c_int, c_dp, c_dp,
                                                                         c_dp, C.c_size_t, c_dp]),
-    "pilco_gp_append_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
-    "pilco_gp_append": (C.c_int, [C.c_int] * 4 + [c_dp] * 5 + [c_dp, C.c_int, c_dp, C.c_int, c_dp, c_dp,
-                                                            c_dp, C.c_size_t, c_dp]),
+    "pilco_gp_append_tri_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "pilco_gp_append_tri": (C.c_int, [C.c_int] * 4 + [c_dp] * 5 + [c_dp, C.c_int] * 4 + [c_dp, c_dp,
+                                                                              c_dp, C.c_size_t, c_dp]),
     "pilco_gp_nlml_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
     "pilco_gp_nlml": (C.c_int, [C.c_int] * 4 + [c_dp, c_ll] * 5 + [c_dp] * 5 + [c_dp, C.c_size_t, c_dp]),
     "pilco_fitc_nlml_workspace_bytes": (C.c_size_t, [C.c_int] * 5),

@@ -539,9 +539,17 @@ __global__ void fitc_axpy_kernel(int n, double* C, int ldc, long long cs, const 
     if (i < n && j < n) C[(size_t)e * cs + (size_t)i * ldc + j] -= a[e] * Tm[(size_t)e * ts + (size_t)i * ldt + j];
 }
 
-void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
-                           const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs) {
+// chol_solve_vec_kernel keeps the whole right-hand side in shared memory: n doubles of dynamic shared memory beside its
+// static diagonal block, opted in once up to what a CTA can hold (CHOL_SOLVE_MAX_N = 28,000 rows on sm_90).
+#define CHOL_SOLVE_STATIC_SMEM (FB * (FB + 1) * (int)sizeof(double))
+#define CHOL_SOLVE_MAX_N ((PILCO_MAX_SMEM_OPTIN - CHOL_SOLVE_STATIC_SMEM) / (int)sizeof(double))
+int chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
+                          const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs) {
+    if (n > CHOL_SOLVE_MAX_N) return PILCO_ERR_DIM;
+    if (pilco_smem_optin<chol_solve_vec_kernel>(PILCO_MAX_SMEM_OPTIN - CHOL_SOLVE_STATIC_SMEM)) return PILCO_ERR_LAUNCH;
     launch_hi(chol_solve_vec_kernel, dim3(batch), dim3(256), n * sizeof(double), st, n, L, ld, ms, E, Y, Y_bs, y_es, yinc, x, xs);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
 }
 
 extern "C" {
@@ -559,7 +567,7 @@ int pilco_gp_factorize(int n, int D, int E, int B,
                        double* iK, int ldk, double* beta, int* info,
                        void* ws, size_t ws_bytes, pilco_stream_t stream) {
     if (!X || !Y || !ell || !sf2 || !sn2 || !beta || !ws) return PILCO_ERR_NULL;
-    if (n < 1 || D < 1 || D > MAXD || E < 1 || E > MAXE || B < 1) return PILCO_ERR_DIM;
+    if (n < 1 || n > CHOL_SOLVE_MAX_N || D < 1 || D > MAXD || E < 1 || E > MAXE || B < 1) return PILCO_ERR_DIM;
     if (iK && ldk < pad64(n)) return PILCO_ERR_DIM;
     if (ws_bytes < pilco_gp_factorize_workspace_bytes(n, E, B)) return PILCO_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
@@ -577,8 +585,7 @@ int pilco_gp_factorize(int n, int D, int E, int B,
     { int rcc = chol_launch(st, batch, n, L, ldw, ms, E, info); if (rcc) return rcc; }
     CUDA_LAUNCH_CHECK();
     // beta = (L L^T)^-1 y_e   (mgpr.py:86-88)
-    launch_hi(chol_solve_vec_kernel, dim3(batch), dim3(256), n * sizeof(double), st, n, L, ldw, ms, E, Y, Y_bs, 1, E, beta, n);
-    CUDA_LAUNCH_CHECK();
+    { int rcs = chol_solve_vec_launch(st, batch, n, L, ldw, ms, E, Y, Y_bs, 1, E, beta, n); if (rcs) return rcs; }
     if (iK) {
         // iK = L^-T L^-1 through the explicit triangular inverse (mgpr.py:85)
         cudaMemsetAsync(Xi, 0, (size_t)batch * ms * sizeof(double), st);
@@ -593,60 +600,51 @@ int pilco_gp_factorize(int n, int D, int E, int B,
 
 // ---- incremental set_data: k rows appended to a factorised model, hyper-parameters unchanged -------------------
 // (SURVEY section 8f-2; pilco/models/mgpr.py:38-45 swaps the data, examples/inv_double_pendulum.py:102-103 and
-// swimmer.py:87-88 append the T rows of every new episode).  Block inverse of A1 = [[A0, K12], [K21, K22 + sn2 I]]:
-//   F = K21 A0^-1,  S = K22 + sn2 I - F K12 (Schur complement, k x k, SPD),  G = S^-1 F,
-//   A1^-1 = [[A0^-1 + F' G, -G'], [-G, S^-1]],   beta = A1^-1 y.
-// O(n^2 k) instead of O(n^3); only the old inverse is needed (no Cholesky factor of the old matrix).
-__global__ void __launch_bounds__(256) append_assemble_kernel(int n0, int k, const double* G, int ldg, long long gs,
-                                                              const double* Sinv, int lds, long long ss,
-                                                              double* iK, int ldk, long long ks) {
+// swimmer.py:87-88 append the T rows of every new episode).  The model carries R = L^-1 (the triangular inverse
+// pilco_gp_factorize builds on the way to iK) and extends it by one block row.  With K21 = k(Xnew, Xold):
+//   P = K21 R0',  S = K22 + sn2 I - P P' (= L22 L22'),  R22 = L22^-1,  W = -R22 P R0,   R1 = [[R0, 0], [W, R22]],
+//   iK1 = R1' R1 = [[iK0 + W'W, W'R22], [R22'W, R22'R22]],   beta = R1' (R1 y).
+// O(n^2 k) instead of O(n^3).  Every product is of triangular factors, so the error of one step is that of a
+// refactorisation and does not grow with cond(K) from append to append; a block-inverse (Schur complement) update of
+// iK itself multiplies the error iK0 carries by about cond(K) at every step.
+// mirror the border rows n0.. of iK into the border columns: O[j][n0+i] = O[n0+i][j], j < n0
+__global__ void __launch_bounds__(256) append_mirror_kernel(int n0, int k, double* iK, int ldk, long long ks) {
     PDL_ENTRY();
-    const int e = blockIdx.y;
-    const int n1 = n0 + k;
-    const double* Ge = G + (size_t)e * gs;
-    const double* Se = Sinv + (size_t)e * ss;
-    double* O = iK + (size_t)e * ks;
-    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < (size_t)k * n1; idx += (size_t)gridDim.x * blockDim.x) {
-        const int i = (int)(idx / n1), j = (int)(idx % n1);          // row n0 + i of the new inverse
-        if (j < n0) {
-            const double v = -Ge[(size_t)i * ldg + j];
-            O[(size_t)(n0 + i) * ldk + j] = v;
-            O[(size_t)j * ldk + n0 + i] = v;
-        } else {
-            O[(size_t)(n0 + i) * ldk + j] = Se[(size_t)i * lds + (j - n0)];
-        }
+    double* O = iK + (size_t)blockIdx.y * ks;
+    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < (size_t)k * n0; idx += (size_t)gridDim.x * blockDim.x) {
+        const int i = (int)(idx / n0), j = (int)(idx % n0);
+        O[(size_t)j * ldk + n0 + i] = O[(size_t)(n0 + i) * ldk + j];
     }
 }
 
-extern "C" size_t pilco_gp_append_workspace_bytes(int n0, int k, int E) {
+extern "C" size_t pilco_gp_append_tri_workspace_bytes(int n0, int k, int E) {
     if (n0 < 1 || k < 1 || E < 1) return 0;
-    const size_t ld0 = pad64(n0), kp = pad64(k);
-    // K21, F, G: [kp x ld0] each; S, L^-1, S^-1: [kp x kp]; T: [FB x kp]
-    return (size_t)E * (3 * kp * ld0 + 3 * kp * kp + FB * kp) * sizeof(double);
+    const size_t ld0 = pad64(n0), kp = pad64(k), n1p = pad64(n0 + k);
+    // K21 (then P R0), P: [kp x ld0] each; S: [kp x kp]; T: [FB x kp]; R1 y: [n1p]
+    return (size_t)E * (2 * kp * ld0 + kp * kp + FB * kp + n1p) * sizeof(double);
 }
 
-extern "C" int pilco_gp_append(int n0, int k, int D, int E,
+extern "C" int pilco_gp_append_tri(int n0, int k, int D, int E,
                                const double* X, const double* Y,            /* [n0+k, D], [n0+k, E]: old rows first */
                                const double* ell, const double* sf2, const double* sn2,
-                               const double* iK_old, int ldk_old,
-                               double* iK_new, int ldk_new, double* beta_new, int* info,
+                               const double* R_old, int ldr_old, const double* iK_old, int ldk_old,
+                               double* R_new, int ldr_new, double* iK_new, int ldk_new, double* beta_new, int* info,
                                void* ws, size_t ws_bytes, pilco_stream_t stream) {
-    if (!X || !Y || !ell || !sf2 || !sn2 || !iK_old || !iK_new || !beta_new || !ws) return PILCO_ERR_NULL;
+    if (!X || !Y || !ell || !sf2 || !sn2 || !R_old || !iK_old || !R_new || !iK_new || !beta_new || !ws) return PILCO_ERR_NULL;
     if (n0 < 1 || k < 1 || D < 1 || D > MAXD || E < 1 || E > MAXE) return PILCO_ERR_DIM;
     const int n1 = n0 + k;
-    if (ldk_old < pad64(n0) || ldk_new < pad64(n1)) return PILCO_ERR_DIM;
-    if (iK_old == iK_new) return PILCO_ERR_DIM;                             // out of place (leading dimensions may differ)
-    if (ws_bytes < pilco_gp_append_workspace_bytes(n0, k, E)) return PILCO_ERR_WORKSPACE;
+    if (ldr_old < pad64(n0) || ldk_old < pad64(n0) || ldr_new < pad64(n1) || ldk_new < pad64(n1)) return PILCO_ERR_DIM;
+    if (R_old == R_new || iK_old == iK_new) return PILCO_ERR_DIM;           // out of place (leading dimensions may differ)
+    if (ws_bytes < pilco_gp_append_tri_workspace_bytes(n0, k, E)) return PILCO_ERR_WORKSPACE;
     cudaStream_t st = (cudaStream_t)stream;
     const int ld0 = pad64(n0), kp = pad64(k);
     const long long rs = (long long)kp * ld0, qs = (long long)kp * kp;
     double* K21 = (double*)ws;
-    double* F = K21 + (size_t)E * rs;
-    double* G = F + (size_t)E * rs;
-    double* S = G + (size_t)E * rs;
-    double* Li = S + (size_t)E * qs;
-    double* Si = Li + (size_t)E * qs;
-    double* T = Si + (size_t)E * qs;
+    double* P = K21 + (size_t)E * rs;
+    double* S = P + (size_t)E * rs;
+    double* T = S + (size_t)E * qs;
+    double* z = T + (size_t)E * FB * kp;
+    const long long zs = pad64(n1);
     const double* Xn = X + (size_t)n0 * D;
     if (info) cudaMemsetAsync(info, 0, sizeof(int), st);
     // K21 = k(Xnew, Xold) [k x n0];  S = k(Xnew, Xnew) + sn2 I
@@ -655,32 +653,42 @@ extern "C" int pilco_gp_append(int n0, int k, int D, int E,
     GramArgs g2{k, k, D, E, Xn, 0, Xn, 0, ell, 0, sf2, 0, sn2, 0, 0.0, S, kp, qs, kp, kp, 0};
     launch_hi(gram_kernel, dim3((kp + 31) / 32, (kp + 7) / 8, E), dim3(32, 8), 0, st, g2);
     CUDA_LAUNCH_CHECK();
+    const long long ro = (long long)ldr_old * ldr_old, rn = (long long)ldr_new * ldr_new;
     const long long ko = (long long)ldk_old * ldk_old, kn = (long long)ldk_new * ldk_new;
-    int rc = gemm(st, E, k, n0, n0, 0, 0, 1.0, K21, ld0, rs, iK_old, ldk_old, ko, 0.0, F, ld0, rs);          // F = K21 A0^-1
+    int rc = gemm(st, E, k, n0, n0, 0, 1, 1.0, K21, ld0, rs, R_old, ldr_old, ro, 0.0, P, ld0, rs);            // P = K21 R0'
     if (rc) return rc;
-    rc = gemm(st, E, k, k, n0, 0, 1, -1.0, F, ld0, rs, K21, ld0, rs, 1.0, S, kp, qs);                        // S -= F K12
+    rc = gemm(st, E, k, k, n0, 0, 1, -1.0, P, ld0, rs, P, ld0, rs, 1.0, S, kp, qs);                           // S -= P P'
     if (rc) return rc;
-    { int rcc = chol_launch(st, E, k, S, kp, qs, E, info); if (rcc) return rcc; }
+    { int rcc = chol_launch(st, E, k, S, kp, qs, E, info); if (rcc) return rcc; }                             // L22
     CUDA_LAUNCH_CHECK();
-    cudaMemsetAsync(Li, 0, (size_t)E * qs * sizeof(double), st);
-    rc = tri_inverse(st, E, k, S, kp, qs, Li, kp, qs, T, (long long)FB * kp);
+    // R1: zero padded [ldr_new x ldr_new]; R0 copied, then R22 = L22^-1 and W = -R22 (P R0) written in place
+    cudaMemsetAsync(R_new, 0, (size_t)E * rn * sizeof(double), st);
+    for (int e = 0; e < E; ++e)
+        cudaMemcpy2DAsync(R_new + (size_t)e * rn, (size_t)ldr_new * sizeof(double), R_old + (size_t)e * ro,
+                          (size_t)ldr_old * sizeof(double), (size_t)n0 * sizeof(double), n0, cudaMemcpyDeviceToDevice, st);
+    double* Rrow = R_new + (size_t)n0 * ldr_new;                                                              // [W | R22]
+    double* R22 = Rrow + n0;
+    rc = tri_inverse(st, E, k, S, kp, qs, R22, ldr_new, rn, T, (long long)FB * kp);
     if (rc) return rc;
-    rc = gemm(st, E, k, k, k, 1, 0, 1.0, Li, kp, qs, Li, kp, qs, 0.0, Si, kp, qs);                           // S^-1 = L^-T L^-1
+    rc = gemm(st, E, k, n0, n0, 0, 0, 1.0, P, ld0, rs, R_old, ldr_old, ro, 0.0, K21, ld0, rs);               // P R0
     if (rc) return rc;
-    rc = gemm(st, E, k, n0, k, 0, 0, 1.0, Si, kp, qs, F, ld0, rs, 0.0, G, ld0, rs);                          // G = S^-1 F
+    rc = gemm(st, E, k, n0, k, 0, 0, -1.0, R22, ldr_new, rn, K21, ld0, rs, 0.0, Rrow, ldr_new, rn);           // W
     if (rc) return rc;
-    // new inverse: zero padded [ldk_new x ldk_new]; old block copied, then + F' G; then the border blocks
+    // iK1: zero padded [ldk_new x ldk_new]; iK0 + W'W, border rows R22' [W | R22], border columns mirrored
     cudaMemsetAsync(iK_new, 0, (size_t)E * kn * sizeof(double), st);
     for (int e = 0; e < E; ++e)
         cudaMemcpy2DAsync(iK_new + (size_t)e * kn, (size_t)ldk_new * sizeof(double), iK_old + (size_t)e * ko,
                           (size_t)ldk_old * sizeof(double), (size_t)n0 * sizeof(double), n0, cudaMemcpyDeviceToDevice, st);
-    rc = gemm(st, E, n0, n0, k, 1, 0, 1.0, F, ld0, rs, G, ld0, rs, 1.0, iK_new, ldk_new, kn);
+    rc = gemm(st, E, n0, n0, k, 1, 0, 1.0, Rrow, ldr_new, rn, Rrow, ldr_new, rn, 1.0, iK_new, ldk_new, kn);
     if (rc) return rc;
-    launch_hi(append_assemble_kernel, dim3((unsigned)min((size_t)256, ((size_t)k * n1 + 255) / 256), E), dim3(256), 0, st,
-              n0, k, (const double*)G, ld0, rs, (const double*)Si, kp, qs, iK_new, ldk_new, kn);
+    rc = gemm(st, E, k, n1, k, 1, 0, 1.0, R22, ldr_new, rn, Rrow, ldr_new, rn, 0.0, iK_new + (size_t)n0 * ldk_new, ldk_new, kn);
+    if (rc) return rc;
+    launch_hi(append_mirror_kernel, dim3((unsigned)min((size_t)256, ((size_t)k * n0 + 255) / 256), E), dim3(256), 0, st,
+              n0, k, iK_new, ldk_new, kn);
     CUDA_LAUNCH_CHECK();
-    // beta = A1^-1 y_e  (row e of beta [E, n1]; y_e = column e of Y)
-    matvec_kernel<<<dim3(n1, E), 32, 0, st>>>(n1, n1, 0, iK_new, ldk_new, kn, Y, 1, E, beta_new, n1);
+    // beta = R1' (R1 y_e)  (row e of beta [E, n1]; y_e = column e of Y)
+    matvec_kernel<<<dim3(n1, E), 32, 0, st>>>(n1, n1, 0, R_new, ldr_new, rn, Y, 1, E, z, zs);
+    matvec_kernel<<<dim3(n1, E), 32, 0, st>>>(n1, n1, 1, R_new, ldr_new, rn, z, zs, 1, beta_new, n1);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;
 }

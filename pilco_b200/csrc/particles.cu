@@ -1068,8 +1068,8 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     return PILCO_OK;
 }
 
-void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
-                           const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
+int chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
+                          const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
 int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const double* X, long long X_bs,
                           const double* ell, long long ell_bs, const double* sf2, long long sf2_bs,
                           const double* beta, long long beta_bs, const double* gy,
@@ -1094,8 +1094,8 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
         const int ldw = pad64(bf);
         launch_hi(pg_rbf_finish_kernel, dim3(R), dim3(128), 0, st, r);
         CUDA_LAUNCH_CHECK();
-        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              r.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf);
+        if (const int rcs = chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
+                                                  r.gbeta, (long long)U * bf, bf, 1, ws + L.gy, bf)) return rcs;
         const int rc = rbf_factor_bwd_launch(st, R, bf, Ds, U, r.C, r.C_bs, r.ell, r.ell_bs, r.sf2, r.sf2_bs,
                                              r.beta, r.beta_bs, ws + L.gy, g->gXc, g->gYc, g->gell);
         if (rc) return rc;

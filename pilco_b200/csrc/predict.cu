@@ -1,6 +1,6 @@
 // predict.cu -- posterior of the factorised dynamics GPs at T deterministic inputs (fp64):
 //   pilco_gp_predict   gpflow GPR.predict_f / GPRFITC.predict_f over the device factors (iK, beta) of
-//                      pilco_gp_factorize / pilco_gp_append / pilco_fitc_factorize
+//                      pilco_gp_factorize / pilco_gp_append_tri / pilco_fitc_factorize
 //   mean(x) = k*(x)' beta_e,   var(x) = sf2_e - k*(x)' iK_e k*(x),   k*(x)_i = sf2_e exp(-0.5 |(x - c_i)/ell_e|^2)
 // The diagonal path is one fused kernel (gp_predict_kernel, DESIGN.md section 10): the quadratic form runs on
 // DMMA.16x8x16 with iK tiles staged by TMA bulk copies, K* is computed in shared memory chunk by chunk and never

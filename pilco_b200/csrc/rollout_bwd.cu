@@ -23,8 +23,8 @@
 #include "rollout_bwd.cuh"
 
 extern "C" size_t pilco_mm_bwd_workspace_bytes(int n, int D, int E, int R, int need_param);
-void chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
-                           const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
+int chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, int ld, long long ms, int E,
+                          const double* Y, long long Y_bs, long long y_es, int yinc, double* x, long long xs);
 
 struct RbWs {            // backward workspace (offsets in doubles)
     size_t gm, gS, gMd, gSd, gVd, gcx, gmj, gsj, gsjx, gMp, gSp, gVp, gmh, gSh, gCh, gbeta, gy, rgm, rgS, jgm, jgS, cnt,
@@ -495,8 +495,9 @@ static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const p
     if (rbf) {
         // gy = (K + sn2 I)^-1 gbeta  with the Cholesky factors kept by pilco_gp_factorize
         const int ldw = pad64(bf);
-        chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
-                              buf(BL.gbeta), (long long)U * bf, bf, 1, buf(BL.gy), bf);
+        rc = chol_solve_vec_launch(st, R * U, bf, g->pol_L, ldw, (long long)ldw * ldw, U,
+                                   buf(BL.gbeta), (long long)U * bf, bf, 1, buf(BL.gy), bf);
+        if (rc) return rc;
         rc = rbf_factor_bwd_launch(st, R, bf, Dh, U, ro->pol.rbf.X, (long long)bf * Dh, ro->pol.rbf.ell, (long long)U * Dh,
                                    ro->pol.rbf.sf2, ro->pol.rbf.sf2_bs, ro->pol.rbf.beta, (long long)U * bf,
                                    buf(BL.gy), g->gXc, g->gYc, g->gell);

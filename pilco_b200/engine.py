@@ -90,17 +90,19 @@ def gp_factorize(X, Y, ell, sf2, sn2, need_iK=True, mode=0):
     gp = DeviceGP(X, ell, sf2, beta, iK, ldk, mode=mode, batched=batched)
     gp.info = info
     gp.fact_ws = ws            # first B*E*ldw*ldw doubles = Cholesky factors (needed by the policy VJP)
+    # with iK, the next B*E*ldw*ldw doubles = R = L^-1 (what gp_append extends)
+    gp.R = ws[B * E * ldk * ldk:2 * B * E * ldk * ldk].view(iK.shape) if need_iK else None
     gp.Y, gp.sn2 = Y, sn2
     return gp
 
 
 def gp_append(gp, X, Y):
-    """pilco_gp_append: the factorised (unbatched, exact-GP) model ``gp`` with rows appended to its data and unchanged
+    """pilco_gp_append_tri: the factorised (unbatched, exact-GP) model ``gp`` with rows appended to its data and unchanged
     hyper-parameters.  ``X`` [n1,D], ``Y`` [n1,E] hold the old rows first.  Returns a NEW DeviceGP (n changes, so do the
-    padded leading dimension and every workspace size downstream); the old inverse is consumed by the O(n^2 k)
-    block-inverse update, no Cholesky factorisation of the full matrix is done."""
-    if gp.batched or gp.iK is None or gp.mode != 0:
-        raise ValueError("gp_append needs an unbatched exact-GP model with its inverse")
+    padded leading dimension and every workspace size downstream): the old model's triangular inverse R = L^-1 is
+    extended by one block row in O(n^2 k), no Cholesky factorisation of the full matrix is done."""
+    if gp.batched or gp.iK is None or gp.mode != 0 or getattr(gp, "R", None) is None:
+        raise ValueError("gp_append needs an unbatched exact-GP model with its inverse and triangular inverse")
     X, Y = dev(X), dev(Y)
     n0, n1 = gp.n, int(X.shape[0])
     k = n1 - n0
@@ -111,14 +113,17 @@ def gp_append(gp, X, Y):
     d = device()
     beta = torch.empty((E, n1), dtype=F64, device=d)
     iK = torch.empty((E, ldk, ldk), dtype=F64, device=d)
+    R = torch.empty((E, ldk, ldk), dtype=F64, device=d)
     info = torch.zeros(1, dtype=torch.int32, device=d)
-    wsb = lib.pilco_gp_append_workspace_bytes(n0, k, E)
+    wsb = lib.pilco_gp_append_tri_workspace_bytes(n0, k, E)
     ws = torch.empty(wsb // 8, dtype=F64, device=d)
-    check(lib.pilco_gp_append(n0, k, D, E, ptr(X), ptr(Y), ptr(gp.ell), ptr(gp.sf2), ptr(gp.sn2),
-                              ptr(gp.iK), gp.ldk, ptr(iK), ldk, ptr(beta), ptr(info), ptr(ws), wsb, stream_ptr()),
+    check(lib.pilco_gp_append_tri(n0, k, D, E, ptr(X), ptr(Y), ptr(gp.ell), ptr(gp.sf2), ptr(gp.sn2),
+                              ptr(gp.R), gp.ldk, ptr(gp.iK), gp.ldk, ptr(R), ldk, ptr(iK), ldk, ptr(beta), ptr(info),
+                              ptr(ws), wsb, stream_ptr()),
           "gp_append")
     new = DeviceGP(X, gp.ell, gp.sf2, beta, iK, ldk, mode=0)
     new.info = info
+    new.R = R
     new.Y, new.sn2 = Y, gp.sn2
     new.appends = getattr(gp, "appends", 0) + 1
     return new

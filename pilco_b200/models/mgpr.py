@@ -285,8 +285,10 @@ class MGPR:
                                    need_iK=(self.mm_mode == 0), mode=self.mm_mode)
 
     # incremental set_data (SURVEY section 8f-2): rows appended + hyper-parameters unchanged -> O(n^2 k) update of the
-    # resident inverse instead of a new O(n^3) factorisation.  After MAX_APPENDS consecutive appends (round-off of
-    # the block-inverse recursion) or when more rows arrive than the model holds, it is refactorised from scratch.
+    # resident triangular inverse instead of a new O(n^3) factorisation.  After MAX_APPENDS consecutive appends or when
+    # more rows arrive than the model holds, it is refactorised from scratch.  The round-off of the appends grows
+    # slowly: on PILCO-like episodes at the noise floor (sn2 = 1e-6) eight appends of 40 rows leave iK and beta within
+    # 9 and 16 eps of their condition scales (tests/test_gpu_fact_regimes.py), where a refactorisation stays within 2.
     MAX_APPENDS = 8
     incremental = True
 
