@@ -643,6 +643,33 @@ size_t pilco_particles_explore_consistent_grad_workspace_bytes(const pilco_parti
 int    pilco_particles_explore_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                                        const pilco_particles_noise* nz, const pilco_exploration* ex,
                                                        int R, const pilco_particles_grad* g, pilco_stream_t stream);
+
+/* Score-function (likelihood-ratio) gradient over consistent function samples (DESIGN.md section 25): the contract of
+ * pilco_particles_noisy_consistent_grad_rollout (ang and nz may be NULL; R policies through the batch strides, shared
+ * x0, eps and nu, restart-major outputs, R = 1 with an unbatched policy the single-policy call; the same validation and
+ * status codes in the same order, all checked before anything is enqueued), with g->ws sized by
+ * pilco_particles_consistent_score_grad_workspace_bytes.  The forward outputs and value are bitwise those of the
+ * consistent pathwise call; the gradient, in the same layout, is that of
+ *   (1/P) sum_p sum_{t<H-1, piv_t>0} w_pt (-eps_t(theta)^2 / 2 - log piv_t(theta)),
+ *   eps_t(theta) = (f_t - mean'_t(theta)) / piv_t(theta),  mean'_t = mu(x~_t) + sum_{s<t} l_ts eps_s(theta)
+ * per output, with the increments f_t = x_{t+1} - x_t and the states x_t held fixed (theta enters through u_s = pi(x_s)
+ * inside every x~_s, s <= t): the log-density of the particle's whole path under its function draw.  w_pt is section
+ * 16's (return-to-go with the leave-one-out baseline, P = 1: w = G), and the joint terms' direct term is added as there.
+ * Its expectation is d E[return] for every reward kind, box terms included, on rollouts whose pivots are all above the
+ * forward's threshold: a step whose pivot is degenerate (d2 <= 1e-10 sf2) is deterministic given the particle's past, has
+ * no likelihood ratio and is dropped, so the estimate is biased where such steps occur.  Near the threshold nothing is
+ * clamped: 1/piv is large there and so is the variance.  H <= 1 gives a zero gradient (H = 1 with joint terms: the
+ * direct term alone).  The workspace is the consistent gradient's layout (with the angle layout when ang or nz is
+ * given, the noise slots when nz is) followed by G [H-1,R P], the sums [R,H], m_bar and v_bar [H-1,R P,E] and the x~_bar
+ * history [H,R P,D] (each slot rounded up to an even number of doubles); the query returns 0 wherever the call would
+ * fail on its sizes, and on size_t overflow.  A restart's results are bitwise independent of R and reproducible run to
+ * run; no host synchronisation (graph-capturable). */
+size_t pilco_particles_consistent_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                             const pilco_particles_noise* nz, int R);
+int    pilco_particles_consistent_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                     const pilco_particles_noise* nz, int R,
+                                                     const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* The per-step sample moments above over a forward that has already run: traj [R P,H+1,E] and act [R P,H,U] of R
  * restarts of P particles (any sampler, chunked or not).  step_mean [R,H] = sum_k c_k rbar_kt and step_var [R,H] =
  * sigma_t^2, each skipped when NULL.  Reads P, H, dyn.E, pol.Ds (= E + A), pol.U, the reward terms, traj and act of pr

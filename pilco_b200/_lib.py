@@ -212,6 +212,8 @@ SIGNATURES = {
     "pilco_particles_explore_consistent_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(Exploration), C.c_int]),
     "pilco_particles_explore_consistent_grad_rollout": (C.c_int, _PAN + [C.POINTER(Exploration), C.c_int,
                                                                          C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_consistent_score_grad_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_consistent_score_grad_rollout": (C.c_int, _PAN + [C.c_int, C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

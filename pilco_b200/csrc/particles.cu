@@ -30,6 +30,10 @@
 // The exploration objective (pilco_particles_explore_*, DESIGN.md section 24): pg_run takes a PxOpt and launches the
 // kernels of particles_explore.cu beside the others (the moments after the forward, the bonus's share before each
 // reverse step kernel, the bonus into value after the reduction).
+// The score-function gradient over consistent function samples (pilco_particles_consistent_score_grad_*, DESIGN.md
+// section 25): pc_run is ps_run's sibling on the consistent forward; pc_white_kernel (particles_cscore.cu) turns the
+// weights into the cotangents of every step's mean' and var', which the reverse of the conditioning and the predict
+// VJP carry to x~_bar_t step by step.
 #include <cmath>
 #include "particles.cuh"
 
@@ -755,6 +759,8 @@ struct PtWs {
     size_t phi;                                         // angles, gradients: phi(x_t) [T,H+1,Dh]
     size_t phiz, phibz;                                 // noise, gradients: phi(z_t) [T,H+1,Dh]; phi_bar_z [T,Dh]
     size_t sd, tab;                                     // exploration: sigma_t [R,H]; the bonus table [R,H,K,2]
+    size_t togo, mw, vw, gxh;                           // consistent score: G [H-1,T]; m_bar, v_bar [H-1,T,E];
+                                                        // the x~_bar history [H,T,D] (the sums in gsum)
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -837,9 +843,11 @@ static PtWs fs_ws_layout(const pilco_particles* pr) {
 // sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
 // [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
 // sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, noise: then the
-// phi(z) history and phi_bar_z, exploration: then sigma_t and the bonus table, as pg_ws_layout)
+// phi(z) history and phi_bar_z, exploration: then sigma_t and the bonus table, as pg_ws_layout).  score (DESIGN.md
+// section 25): then G [H-1,T], the sums [R,H], m_bar and v_bar [H-1,T,E] and the x~_bar history [H,T,D]; 0 also where
+// the per-(step, particle) grids would pass 2^31 - 1 CTAs.
 static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false,
-                         bool explore = false) {
+                         bool explore = false, bool score = false) {
     const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
     const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
@@ -853,7 +861,14 @@ static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, 
     if (angles) L.phi = take({T, H + 1, Dh});
     if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
     if (explore) { L.sd = take({(size_t)R, H}); L.tab = take({(size_t)R, H, (size_t)pr->n_rewards, 2}); }
-    L.total = L.pws_bytes && L.vws_bytes ? take.bytes() : 0;
+    bool grids = true;
+    if (score) {
+        const size_t Hm = H > 0 ? H - 1 : 0, nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
+        L.togo = take({Hm, T}); L.gsum = take({(size_t)R, H});
+        L.mw = take({Hm, T, Ds}); L.vw = take({Hm, T, Ds}); L.gxh = take({H, T, D});
+        grids = nb * H <= 0x7fffffff;
+    }
+    L.total = L.pws_bytes && L.vws_bytes && grids ? take.bytes() : 0;
     return L;
 }
 
@@ -1298,6 +1313,71 @@ static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
     return pg_reduce(pr, R, g, ws, L, st, pin);
 }
 
+// The score-function gradient over consistent function samples of R restarts (validated; DESIGN.md section 25):
+//   pt_forward(consistent, history), ps_togo, ps_base, pc_white, memset(Lambda),
+//   [fs_cond_bwd<t>, fs_vjp<t> -> x~_bar_t] for t = H-2 .. 0, (joint terms) pj_grad over all H steps, ps_zbar, pg_reduce
+// m_bar_t and v_bar_t stand where the pathwise sweep's x_bar_{t+1} and var_bar_t stand.  Nothing chains x_bar between
+// steps (x is held fixed), so there is no step kernel; Lambda accumulates over the steps, so the loop stays serial.
+// tm, nz: as ps_run (the policy inputs are the phi or phi(z) history, the direct term starts at x~ column Dh).
+static int pc_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream,
+                  const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
+    const PtWs L = fg_ws_layout(pr, R, tm != nullptr, nz != nullptr, false, true);
+    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
+    if (const int rc = fs_predict_prepare()) return rc;
+    if (const int rc = fs_vjp_prepare()) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)g->ws;
+    if (const int rc = pt_forward(pr, R, ws, L, true, true, st, tm, nz)) return rc;
+    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
+    const int nb = (P + PT_THREADS - 1) / PT_THREADS;
+    const size_t TD = (size_t)T * D, TE = (size_t)T * E;
+    const double* pin = nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj;
+    PsDev a;
+    static_cast<PtPolicy&>(a) = pt_policy(pr);
+    a.T = T;
+    a.eps = pr->eps; a.traj = pin; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
+    a.var = nullptr; a.G = ws + L.togo; a.S = ws + L.gsum; a.gmean = ws + L.mw; a.gvar = ws + L.vw;
+    a.gxt = ws + L.gxh; a.zbar = ws + L.zbar;
+    a.direct = pt_has_joint(pr);
+    if (H > 1) {
+        launch_hi(ps_togo_kernel, dim3(nb, R), dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        launch_hi(ps_base_kernel, dim3(H - 1, R), dim3(256), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+        PcWhite w;
+        w.P = P; w.T = T; w.H = H; w.Ds = E;
+        w.L = ws + L.L; w.eps = pr->eps; w.var = ws + L.var; w.G = a.G; w.S = a.S; w.mbar = a.gmean; w.vbar = a.gvar;
+        if (const int rc = pc_white_launch(st, R, w)) return rc;
+        cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TE * sizeof(double), st);
+        FsBwd q;                                        // as pg_reverse's; the cotangents come from the whitening reverse
+        q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = E; q.np = pad64(pr->dyn.n);
+        q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
+        q.xh = ws + L.xt; q.Kh = ws + L.Kh; q.L = ws + L.L; q.eps = pr->eps;
+        q.G = ws + L.G; q.A = ws + L.W; q.dir = ws + L.dir;
+        const dim3 cgrid((P + FS_WARPS - 1) / FS_WARPS, E, R);
+        for (int t = H - 2; t >= 0; --t) {
+            q.t = t; q.gx = a.gmean + (size_t)t * TE; q.gvar = a.gvar + (size_t)t * TE;
+            launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
+            CUDA_LAUNCH_CHECK();
+            const int rc = fs_vjp_launch(st, &pr->dyn, T, ws + L.xt + (size_t)t * TD, q.gx, q.A, q.dir,
+                                         ws + L.gxh + (size_t)t * TD, ws + L.vws);
+            if (rc) return rc;
+        }
+    }
+    if (H > 0 && a.direct) {                            // the direct term, as ps_run
+        cudaMemsetAsync(ws + L.gxh + (size_t)(H - 1) * TD, 0, TD * sizeof(double), st);
+        PjDev j = pj_dev(pr, R);
+        j.xh = ws + L.xt; j.gxt = ws + L.gxh; j.gstep = (long long)TD; j.first = Ds;
+        launch_hi(pj_grad_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, j);
+        CUDA_LAUNCH_CHECK();
+    }
+    if (H > 0) {
+        launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);
+        CUDA_LAUNCH_CHECK();
+    }
+    return pg_reduce(pr, R, g, ws, L, st, pin);
+}
+
 // everything a gradient entry point checks before its workspace: batched honours the policy's batch strides
 static int pg_validate(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, int A = 0) {
     if (const int rc = pt_check_desc(pr, batched, A)) return rc;
@@ -1361,6 +1441,19 @@ static int pn_validate(const pilco_particles* pr, const pilco_angles* ang, const
     return pn_noise(pr, nz, n);
 }
 
+// a gradient's checks up to its workspace with optional angles and noise: the noisy call's (nz NULL: the angle or
+// plain call's).  Fills tm when ang or nz is given (then *mapped), n when nz is.
+static int pn_grad_validate(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz, int R,
+                            const pilco_particles_grad* g, TrigMap* tm, PnNoise* n, bool* mapped) {
+    const bool none = pa_none(ang);
+    *mapped = nz || !none;
+    if (nz) return pn_validate(pr, ang, nz, R, g, true, tm, n);
+    if (!pr) return PILCO_ERR_NULL;
+    if (!none)
+        if (const int rc = pa_map(pr, ang, tm)) return rc;
+    return pg_validate(pr, R, g, true, none ? 0 : tm->A);
+}
+
 // a noisy call's workspace query (nz != NULL): the sizes the angle query accepts and valid noise
 static bool pn_sizes_ok(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz) {
     if (!pr || !pt_sizes_ok(pr) || (!pa_none(ang) && !pa_sizes_ok(pr, ang))) return false;
@@ -1399,19 +1492,11 @@ static size_t px_ws_bytes(const pilco_particles* pr, const pilco_angles* ang, co
 static int px_grad(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                    const pilco_exploration* ex, int R, const pilco_particles_grad* g, bool consistent,
                    pilco_stream_t stream) {
-    TrigMap tm; PnNoise n;
-    const bool none = pa_none(ang);
-    if (nz) {
-        if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
-    } else {
-        if (!pr) return PILCO_ERR_NULL;
-        if (!none)
-            if (const int rc = pa_map(pr, ang, &tm)) return rc;
-        if (const int rc = pg_validate(pr, R, g, true, none ? 0 : tm.A)) return rc;
-    }
+    TrigMap tm; PnNoise n; bool mapped;
+    if (const int rc = pn_grad_validate(pr, ang, nz, R, g, &tm, &n, &mapped)) return rc;
     if (const int rc = px_check(pr, ex)) return rc;
     const PxOpt o = {ex->b, ex->step_var};
-    return pg_run(pr, R, g, consistent, stream, nz || !none ? &tm : nullptr, nz ? &n : nullptr, &o);
+    return pg_run(pr, R, g, consistent, stream, mapped ? &tm : nullptr, nz ? &n : nullptr, &o);
 }
 
 extern "C" {
@@ -1642,6 +1727,22 @@ int pilco_particles_explore_consistent_grad_rollout(const pilco_particles* pr, c
                                                     const pilco_particles_grad* g, pilco_stream_t stream) {
     if (!px_active(ex)) return pilco_particles_noisy_consistent_grad_rollout(pr, ang, nz, R, g, stream);
     return px_grad(pr, ang, nz, ex, R, g, true, stream);
+}
+
+// ---- the score-function gradient over consistent function samples (DESIGN.md section 25) -------------------------
+size_t pilco_particles_consistent_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                             const pilco_particles_noise* nz, int R) {
+    const bool sizes = nz ? pn_sizes_ok(pr, ang, nz) : pr && (pa_none(ang) ? pt_sizes_ok(pr) : pa_sizes_ok(pr, ang));
+    if (!sizes || !pt_batch_ok(pr->P, R)) return 0;
+    return fg_ws_layout(pr, R, nz || !pa_none(ang), nz != nullptr, false, true).total;
+}
+
+int pilco_particles_consistent_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                  const pilco_particles_noise* nz, int R,
+                                                  const pilco_particles_grad* g, pilco_stream_t stream) {
+    TrigMap tm; PnNoise n; bool mapped;
+    if (const int rc = pn_grad_validate(pr, ang, nz, R, g, &tm, &n, &mapped)) return rc;
+    return pc_run(pr, R, g, stream, mapped ? &tm : nullptr, nz ? &n : nullptr);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,

@@ -1,6 +1,7 @@
-// particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu and
-// particles_explore.cu share: the per-particle argument structs, the reward value at a point, the fixed-order block
-// sum, and the angle, noise and exploration kernels' launchers (DESIGN.md sections 11, 12, 20, 23 and 24).
+// particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu,
+// particles_explore.cu and particles_cscore.cu share: the per-particle argument structs, the reward value at a point, the
+// fixed-order block sum, and the angle, noise, exploration and consistent-score kernels' launchers (DESIGN.md sections
+// 11, 12, 20, 23, 24 and 25).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -163,3 +164,19 @@ int px_moments_launch(cudaStream_t st, int R, const PxMom& a);
 int px_bonus_launch(cudaStream_t st, dim3 grid, const PxBonus& a);
 // value[r] += b sum_t sd[r,t], step order
 int px_value_launch(cudaStream_t st, int R, int H, double b, const double* sd, double* value);
+
+// ---- score-function gradient over consistent function samples (particles_cscore.cu, DESIGN.md section 25) ------------
+// The whitening reverse of R restarts (T = R P rows, Ds = E): from the consistent forward's packed rows and pivots, eps
+// and the weights w_pt = G_pt - (S_t - G_pt) / (P - 1) (P = 1: G_pt), the cotangents of every step's mean' and var'.
+struct PcWhite {
+    int P, T, H, Ds;
+    const double* L;                                    // [H(H+1)/2, E, T] the forward's packed rows
+    const double* eps;                                  // [P,H,E], shared by the restarts
+    const double* var;                                  // [H,T,E] var'_t = max(d2_t, 0), the forward's history
+    const double* G;                                    // [H-1,T] return-to-go (ps_togo_kernel)
+    const double* S;                                    // [R,H] its per-(restart, step) sums (ps_base_kernel)
+    double* mbar; double* vbar;                         // [H-1,T,E] m_bar_t, v_bar_t
+};
+
+// grid (ceil(P / 8), E, R), 256 threads; H < 2 launches nothing
+int pc_white_launch(cudaStream_t st, int R, const PcWhite& a);

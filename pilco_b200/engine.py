@@ -735,7 +735,7 @@ class ParticlePlan:
                              "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
         if consistent and estimator == "score":
             raise ValueError("particles: the score-function gradient of the consistent (function-sample) rollout "
-                             "is not available; use estimator='pathwise'")
+                             "is engine.ConsistentGradPlan(..., estimator='score'), not ParticlePlan")
         self.estimator = estimator
         if consistent and grad:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
@@ -965,10 +965,22 @@ class ConsistentGradPlan(ParticlePlan):
     that names the bytes needed and the number of particles that would fit, raised before anything is allocated.
 
     ``angles``, ``measurement_noise``, ``exploration``: as ``ParticlePlan`` (pilco_particles_explore_consistent_grad_*
-    with exploration)."""
+    with exploration).
+
+    ``estimator``: ``"pathwise"`` (the default) or ``"score"``, the score-function estimator over the same function
+    samples (pilco_particles_consistent_score_grad_rollout, DESIGN.md section 25), which differentiates the log-density
+    of each particle's whole path under its draw instead of the path itself, so box terms enter its gradient.  The same
+    rollout, value and output layout; its estimate is unbiased on rollouts without degenerate pivots.  ``"score"`` with
+    ``exploration``, or an unknown estimator, is a ValueError raised before any allocation."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
-                 measurement_noise=None, exploration=None):
+                 measurement_noise=None, exploration=None, estimator="pathwise"):
+        if estimator not in self.ESTIMATORS:
+            raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
+        if exploration is not None and estimator == "score":
+            raise ValueError("particles: exploration is an objective of the pathwise gradient: it needs "
+                             "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
+        self.estimator = estimator
         self.consistent = True
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration)
         need = self._grad_ws_bytes(self.P)
@@ -988,6 +1000,9 @@ class ConsistentGradPlan(ParticlePlan):
             return 0
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
+        if self.estimator == "score":
+            return int(lib.pilco_particles_consistent_score_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
+                                                                                self._nz_ref(), self.R))
         if self.ex is not None:
             return int(lib.pilco_particles_explore_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
                                                                                    self._nz_ref(), C.byref(self.ex),
@@ -1005,7 +1020,13 @@ class ConsistentGradPlan(ParticlePlan):
     def launch_grad(self):
         """pilco_particles_rollout_consistent_grad: the consistent rollout (``outputs()``) and the pathwise gradient
         of value = mean return (with ``exploration``: the exploration objective, and sigma_t^2 in ``step_var``),
-        returned as ``ParticlePlan.launch_grad`` returns it"""
+        returned as ``ParticlePlan.launch_grad`` returns it.  ``estimator="score"``: the score-function gradient
+        (pilco_particles_consistent_score_grad_rollout) in the same layout"""
+        if self.estimator == "score":
+            check(lib.pilco_particles_consistent_score_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
+                                                                    self.R, C.byref(self.grad), stream_ptr()),
+                  "particles_consistent_score_grad_rollout")
+            return self.gbuf
         if self.ex is not None:
             check(lib.pilco_particles_explore_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
                                                                       C.byref(self.ex), self.R, C.byref(self.grad),

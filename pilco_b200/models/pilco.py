@@ -384,8 +384,9 @@ class PILCO:
             raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
                              % (engine.ParticlePlan.ESTIMATORS, estimator))
         if consistent and estimator == "score":
-            raise ValueError("sample_policy_gradient: the score-function estimator is not available for the consistent "
-                             "(function-sample) particles; use estimator='pathwise'")
+            raise ValueError("sample_policy_gradient: the score-function estimator over the consistent (function-sample) "
+                             "particles is engine.ConsistentGradPlan(..., estimator='score'); this method offers "
+                             "estimator='pathwise' with them")
         b = float(exploration)
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
                                    consistent=consistent, estimator=estimator, exploration=None if b == 0.0 else b)
