@@ -27,13 +27,13 @@
 // Measurement noise at the policy's input (pilco_particles_noisy_*, DESIGN.md section 23): the same drivers take a
 // PnNoise next to the map (the identity map without angles) and launch the kernels of particles_noise.cu in place of the
 // angle step kernels; the policy inputs of the reductions are then the phi(z) history.
-// The exploration objective (pilco_particles_explore_*, DESIGN.md section 24): pg_run takes a PxOpt and launches the
-// kernels of particles_explore.cu beside the others (the moments after the forward, the bonus's share before each
-// reverse step kernel, the bonus into value after the reduction).
+// The exploration objective (pilco_particles_explore_*, DESIGN.md section 24): pt_call launches the kernels of
+// particles_explore.cu beside the others (the moments after the forward, the bonus's share before each reverse step
+// kernel, the bonus into value after the reduction).
 // The score-function gradient over consistent function samples (pilco_particles_consistent_score_grad_*, DESIGN.md
-// section 25): pc_run is ps_run's sibling on the consistent forward; pc_white_kernel (particles_cscore.cu) turns the
-// weights into the cotangents of every step's mean' and var', which the reverse of the conditioning and the predict
-// VJP carry to x~_bar_t step by step.
+// section 25): ps_run on the consistent forward; pc_white_kernel (particles_cscore.cu) turns the weights into the
+// cotangents of every step's mean' and var', which the reverse of the conditioning and the predict VJP carry to
+// x~_bar_t step by step.
 #include <cmath>
 #include "particles.cuh"
 
@@ -747,20 +747,40 @@ __global__ void __launch_bounds__(PT_THREADS) ps_zbar_kernel(PsDev a) {
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-// Offsets in doubles into a particle workspace, for all four layouts (a slot a layout does not have stays 0); the
-// predict (pws) and VJP (vws) workspaces are one slot when one call needs both.  total in bytes; 0 for unsupported
-// sizes and on size_t overflow.
+// Every entry point is one call of pt_call (or of the query pt_query): pt_validate checks the call once, in one order
+// of precedence, and fills a PtOpt; the sampler's layout (pt_ws_layout or fs_ws_layout) places the workspace; the
+// forward pt_forward, then pg_reverse (pathwise) or ps_run (score) runs it.
+
+enum PtCall { PT_FORWARD, PT_PATHWISE, PT_SCORE };
+
+// What one validated call runs.  The entry point sets the sampler, the call and batched; pt_validate the rest.
+struct PtOpt {
+    bool consistent;            // one posterior function per particle (DESIGN.md section 14), else step-wise draws
+    PtCall call;
+    bool batched;               // the policy's batch strides are honoured; otherwise a batched policy is unsupported
+    int R;
+    bool mapped;                // angles or noise: tm is the angles' map (the identity without angles)
+    TrigMap tm;
+    bool noisy;                 // measurement noise (DESIGN.md section 23)
+    PnNoise nz;
+    bool explore, bonus;        // exploration (section 24): the moments; bonus (b != 0): its share and its value
+    double b;
+    double* step_var;
+};
+
+// Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
+// (pws) and VJP (vws) workspaces are one slot when one call needs both.  total in bytes; 0 for unsupported sizes and
+// on size_t overflow.
 struct PtWs {
     size_t xt, mean, var;                               // forward: x~ [H or 1,T,D], step closure mean [T,Ds], var
     size_t mu, s2, W, Kh, L;                            // consistent forward: predict outputs, W_t, K* history, factor
     size_t gx, gvar, gxt, zbar, s1, s2r, gbeta, gy;     // reverse sweep and the policy-parameter reduction
-    size_t G, dir;                                      // reverse of the conditioning (score: G = the return-to-go)
-    size_t gsum;                                        // score: the per-(restart, step) sums of G
+    size_t G, dir;                                      // consistent: reverse of the conditioning
     size_t phi;                                         // angles, gradients: phi(x_t) [T,H+1,Dh]
     size_t phiz, phibz;                                 // noise, gradients: phi(z_t) [T,H+1,Dh]; phi_bar_z [T,Dh]
     size_t sd, tab;                                     // exploration: sigma_t [R,H]; the bonus table [R,H,K,2]
-    size_t togo, mw, vw, gxh;                           // consistent score: G [H-1,T]; m_bar, v_bar [H-1,T,E];
-                                                        // the x~_bar history [H,T,D] (the sums in gsum)
+    size_t togo, gsum, mw, vw, gxh;                     // score: G [H-1,T]; the sums [R,H]; m_bar, v_bar [H-1,T,E];
+                                                        // the x~_bar history [H-1 or H,T,D]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -784,125 +804,94 @@ static bool pt_has_joint(const pilco_particles* pr) {
     return false;
 }
 
-// the marginal rollout: x~, the predict outputs and one predict workspace at T = P
-static PtWs pt_ws_layout(const pilco_particles* pr) {
-    const size_t P = pr->P, Ds = pr->dyn.E, D = pr->dyn.D;
-    PtWs L = {}; PtTake take;
-    L.xt = take({P, D}); L.mean = take({P, Ds}); L.var = take({P, Ds});
-    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, pr->P, 0);
-    L.pws = take({L.pws_bytes / sizeof(double)});
-    L.total = L.pws_bytes ? take.bytes() : 0;
-    return L;
-}
-
-// the gradient for R restarts: the forward's predict inputs and variances of EVERY step (the reverse sweep needs
-// them), the state cotangent, the VJP's cotangents and output, z_bar of every point, the RBF sums, and one predict /
-// VJP workspace at T = R P (never in use at the same time).  Rows are restart-major (row r P + p); nothing of size
-// [., n] is kept.  State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles);
-// angles: the phi history [T,H+1,Dh] after everything else; noise (with angles = true): then the phi(z) history
-// [T,H+1,Dh] and phi_bar_z [T,Dh]; exploration: then sigma_t [R,H] and the bonus table [R,H,K,2] (K = n_rewards).
-static PtWs pg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false,
-                         bool explore = false) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
-    const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
-    PtWs L = {}; PtTake take;
-    L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
-    L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
-    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
-    const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
-    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
-    L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
-    L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
-    if (angles) L.phi = take({T, H + 1, Dh});
-    if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
-    if (explore) { L.sd = take({(size_t)R, H}); L.tab = take({(size_t)R, H, (size_t)pr->n_rewards, 2}); }
-    L.total = L.pws_bytes ? take.bytes() : 0;
-    return L;
-}
-
-// the consistent rollout at T rows: x~ of every step [H,T,D], the predict outputs mu and var and the step closure's
-// mean and var [T,Ds], W_t [E,T,np], the K* history [H,E,T,np], the packed factor rows [H(H+1)/2,E,T], one predict
-// workspace at T
-static void fs_take(const pilco_particles* pr, size_t T, PtWs& L, PtTake& take) {
-    const size_t H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, np = (size_t)pad64(pr->dyn.n);
-    L.xt = take({H, T, D}); L.mu = take({T, Ds}); L.s2 = take({T, Ds}); L.mean = take({T, Ds}); L.var = take({T, Ds});
-    L.W = take({T, Ds, np}); L.Kh = take({H, T, Ds, np}); L.L = take({H * (H + 1) / 2, T, Ds});
-    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
-    L.pws = take({L.pws_bytes / sizeof(double)});
-}
-
-static PtWs fs_ws_layout(const pilco_particles* pr) {
-    PtWs L = {}; PtTake take;
-    fs_take(pr, pr->P, L, take);
-    L.total = L.pws_bytes ? take.bytes() : 0;
-    return L;
-}
-
-// the consistent gradient for R restarts: the consistent forward's at T = R P (its W slot holds a_t in the reverse
-// sweep), then the var' history [H,T,Ds] (in place of the forward's single var slot), the packed cotangent rows
-// [H(H+1)/2,E,T], the direct sums [E,T,D], x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF
-// sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one VJP workspace at T (angles: then the phi history, noise: then the
-// phi(z) history and phi_bar_z, exploration: then sigma_t and the bonus table, as pg_ws_layout).  score (DESIGN.md
-// section 25): then G [H-1,T], the sums [R,H], m_bar and v_bar [H-1,T,E] and the x~_bar history [H,T,D]; 0 also where
-// the per-(step, particle) grids would pass 2^31 - 1 CTAs.
-static PtWs fg_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false,
-                         bool explore = false, bool score = false) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D;
-    const size_t bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
-    PtWs L = {}; PtTake take;
-    fs_take(pr, T, L, take);                            // pt_batch_ok: R P <= PT_MAX_P
-    L.var = take({H, T, Ds}); L.G = take({H * (H + 1) / 2, T, Ds}); L.dir = take({T, Ds, D});
-    L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
-    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
-    L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
-    L.vws = take({L.vws_bytes / sizeof(double)});
-    if (angles) L.phi = take({T, H + 1, Dh});
-    if (noise) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
-    if (explore) { L.sd = take({(size_t)R, H}); L.tab = take({(size_t)R, H, (size_t)pr->n_rewards, 2}); }
-    bool grids = true;
-    if (score) {
-        const size_t Hm = H > 0 ? H - 1 : 0, nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
-        L.togo = take({Hm, T}); L.gsum = take({(size_t)R, H});
-        L.mw = take({Hm, T, Ds}); L.vw = take({Hm, T, Ds}); L.gxh = take({H, T, D});
-        grids = nb * H <= 0x7fffffff;
-    }
-    L.total = L.pws_bytes && L.vws_bytes && grids ? take.bytes() : 0;
-    return L;
-}
-
 // steps per pilco_gp_predict_vjp call of the score gradient: whole steps of T rows, at most PT_MAX_P rows (T <= PT_MAX_P)
 static int ps_group(long long T, int H) {
     const long long k = PT_MAX_P / T;
     return H - 1 < k ? H - 1 : (int)k;
 }
 
-// the score gradient for R restarts: pg_ws_layout's forward part (x~ [H,T,D], mean [T,Ds], var [H,T,Ds]), then G
-// [H-1,T], the sums [R,H], gmean and gvar [H-1,T,Ds], the VJP output [H-1,T,D], z_bar [T,H,U], the RBF sums
-// [R,U,bf,Ds] x 2 and [R,U,bf] x 2, and one predict / VJP workspace for the predict at T and the largest VJP group.
-// 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs.  Angles: then the phi history, as pg_ws_layout;
-// noise: then the phi(z) history (the score path has no phi_bar_z).
-static PtWs ps_ws_layout(const pilco_particles* pr, int R, bool angles = false, bool noise = false) {
-    const size_t T = (size_t)R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U;
-    const size_t D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+// The step-wise sampler's workspace at T = R P rows (restart-major, row r P + p; nothing of size [., n] is kept).
+// State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles).
+//   forward-only: x~ [T,D], the step closure's mean and var [T,Ds], one predict workspace at T
+//   pathwise: x~ and var of EVERY step [H,T,D] and [H,T,Ds] (the reverse sweep needs them), mean [T,Ds], x_bar and
+//     var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF sums [R,U,bf,Dh] x 2 and [R,U,bf] x 2, and one
+//     predict / VJP workspace at T (never in use at the same time)
+//   score (DESIGN.md section 16): as pathwise, but G [H-1,T], the sums [R,H], m_bar and v_bar [H-1,T,Ds] and the VJP
+//     output [H-1,T,D] (joint terms: [H,T,D]) in place of x_bar .. the VJP output, and the VJP workspace for the
+//     largest VJP group; 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs
+// then, gradients only: the phi history [T,H+1,Dh] (angles or noise); the phi(z) history [T,H+1,Dh] and (pathwise)
+// phi_bar_z [T,Dh] (noise); sigma_t [R,H] and the bonus table [R,H,K,2] (exploration, K = n_rewards).
+static PtWs pt_ws_layout(const pilco_particles* pr, const PtOpt& o) {
+    const bool grad = o.call != PT_FORWARD, score = o.call == PT_SCORE;
+    const size_t R = o.R, T = R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Hx = grad ? H : 1;
+    const size_t Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
     PtWs L = {}; PtTake take;
-    L.xt = take({H, T, D}); L.mean = take({T, Ds}); L.var = take({H, T, Ds});
-    L.G = take({Hm, T}); L.gsum = take({(size_t)R, H});
-    L.gx = take({Hm, T, Ds}); L.gvar = take({Hm, T, Ds});
-    L.gxt = take({pt_has_joint(pr) ? H : Hm, T, D});    // joint terms: step H-1 too, for their direct term
-    L.zbar = take({T, H, U});
-    L.s1 = take({(size_t)R, U, bf, Dh}); L.s2r = take({(size_t)R, U, bf, Dh});
-    L.gbeta = take({(size_t)R, U, bf}); L.gy = take({(size_t)R, U, bf});
-    const int grp = ps_group((long long)T, (int)H);
+    L.xt = take({Hx, T, D}); L.mean = take({T, Ds}); L.var = take({Hx, T, Ds});
+    if (score) {
+        L.togo = take({Hm, T}); L.gsum = take({R, H});
+        L.mw = take({Hm, T, Ds}); L.vw = take({Hm, T, Ds});
+        L.gxh = take({pt_has_joint(pr) ? H : Hm, T, D});    // joint terms: step H-1 too, for their direct term
+    } else if (grad) {
+        L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D});
+    }
+    if (grad) {
+        L.zbar = take({T, H, U});
+        L.s1 = take({R, U, bf, Dh}); L.s2r = take({R, U, bf, Dh});
+        L.gbeta = take({R, U, bf}); L.gy = take({R, U, bf});
+    }
+    const int grp = score ? ps_group((long long)T, (int)H) : 1;
     const size_t pb = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
-    const size_t vb = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T * (grp > 1 ? grp : 1));
+    const size_t vb = grad ? pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E,
+                                                                  (int)T * (grp > 1 ? grp : 1)) : pb;
     L.pws_bytes = L.vws_bytes = (pb && vb) ? (pb > vb ? pb : vb) : 0;
     L.pws = L.vws = take({L.pws_bytes / sizeof(double)});
-    if (angles) L.phi = take({T, H + 1, Dh});
-    if (noise) L.phiz = take({T, H + 1, Dh});
+    if (grad && o.mapped) L.phi = take({T, H + 1, Dh});
+    if (grad && o.noisy) { L.phiz = take({T, H + 1, Dh}); if (!score) L.phibz = take({T, Dh}); }
+    if (o.explore) { L.sd = take({R, H}); L.tab = take({R, H, (size_t)pr->n_rewards, 2}); }
     const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
-    L.total = L.pws_bytes && nb * H <= 0x7fffffff ? take.bytes() : 0;
+    L.total = L.pws_bytes && (!score || nb * H <= 0x7fffffff) ? take.bytes() : 0;
+    return L;
+}
+
+// The consistent sampler's workspace at T = R P rows (DESIGN.md sections 14, 15, 25):
+//   forward: x~ of every step [H,T,D], the predict outputs mu and var and the step closure's mean and var [T,Ds], W_t
+//     [E,T,np], the K* history [H,E,T,np], the packed factor rows [H(H+1)/2,E,T], one predict workspace at T
+//   gradients: then the var' history [H,T,Ds], the packed cotangent rows [H(H+1)/2,E,T], the direct sums [E,T,D],
+//     x_bar and var_bar [T,Ds], the VJP output [T,D], z_bar [T,H,U], the RBF sums [R,U,bf,Ds] x 2 and [R,U,bf] x 2,
+//     and one VJP workspace at T (the W slot holds a_t in the reverse sweep); then the phi history (angles or noise),
+//     the phi(z) history and phi_bar_z (noise), sigma_t and the bonus table (exploration), as pt_ws_layout
+//   score: then G [H-1,T], the sums [R,H], m_bar and v_bar [H-1,T,E] and the x~_bar history [H,T,D]; 0 also where
+//     the per-(step, particle) grids would pass 2^31 - 1 CTAs
+static PtWs fs_ws_layout(const pilco_particles* pr, const PtOpt& o) {
+    const bool grad = o.call != PT_FORWARD, score = o.call == PT_SCORE;
+    const size_t R = o.R, T = R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, np = (size_t)pad64(pr->dyn.n);
+    const size_t Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+    PtWs L = {}; PtTake take;                           // pt_batch_ok: R P <= PT_MAX_P
+    L.xt = take({H, T, D}); L.mu = take({T, Ds}); L.s2 = take({T, Ds}); L.mean = take({T, Ds}); L.var = take({T, Ds});
+    L.W = take({T, Ds, np}); L.Kh = take({H, T, Ds, np}); L.L = take({H * (H + 1) / 2, T, Ds});
+    L.pws_bytes = pilco_gp_predict_workspace_bytes(pr->dyn.n, pr->dyn.D, (int)Ds, (int)T, 0);
+    L.pws = take({L.pws_bytes / sizeof(double)});
+    bool grids = true;
+    if (grad) {
+        // the var' history supersedes the forward's var slot, whose bytes stay: the sizes reported for these calls
+        // include them
+        L.var = take({H, T, Ds}); L.G = take({H * (H + 1) / 2, T, Ds}); L.dir = take({T, Ds, D});
+        L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
+        L.s1 = take({R, U, bf, Dh}); L.s2r = take({R, U, bf, Dh});
+        L.gbeta = take({R, U, bf}); L.gy = take({R, U, bf});
+        L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
+        L.vws = take({L.vws_bytes / sizeof(double)});
+        if (o.mapped) L.phi = take({T, H + 1, Dh});
+        if (o.noisy) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
+        if (o.explore) { L.sd = take({R, H}); L.tab = take({R, H, (size_t)pr->n_rewards, 2}); }
+        if (score) {
+            const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
+            L.togo = take({Hm, T}); L.gsum = take({R, H});
+            L.mw = take({Hm, T, Ds}); L.vw = take({Hm, T, Ds}); L.gxh = take({H, T, D});
+            grids = nb * H <= 0x7fffffff;
+        }
+    }
+    L.total = L.pws_bytes && (!grad || L.vws_bytes) && grids ? take.bytes() : 0;
     return L;
 }
 
@@ -914,6 +903,22 @@ static bool pt_sizes_ok(const pilco_particles* pr) {
 // R restarts of P particles: one CTA row per restart (gridDim.y) and R P predict points
 static bool pt_batch_ok(int P, int R) {
     return R >= 1 && R <= 65535 && (long long)R * P <= PT_MAX_P;
+}
+
+// the reward terms: their count, then each term's W, kind, channel and t (no_additive_box: an ADD-channel box term is
+// unsupported, section 21's rule for the reward's sample moments)
+static int pt_check_rewards(const pilco_particles* pr, bool no_additive_box) {
+    if (pr->n_rewards < 1 || pr->n_rewards > 8) return PILCO_ERR_DIM;
+    for (int k = 0; k < pr->n_rewards; ++k) {
+        const pilco_reward_term& rt = pr->rewards[k];
+        if (!rt.W) return PILCO_ERR_NULL;
+        if (!reward_kind_known(rt.kind)) return PILCO_ERR_UNSUPPORTED;
+        if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
+        if (reward_needs_t(rt.kind) && !rt.t) return PILCO_ERR_NULL;
+        if (no_additive_box && rt.channel == PILCO_CHANNEL_ADD && rt.kind == PILCO_REWARD_BOX)
+            return PILCO_ERR_UNSUPPORTED;
+    }
+    return PILCO_OK;
 }
 
 // everything but the workspace (the gradients bring their own).  batched: the policy's batch strides are honoured
@@ -947,14 +952,7 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A 
         if (r.n < 1 || r.D != Ds || r.E != U) return PILCO_ERR_DIM;
     } else return PILCO_ERR_UNSUPPORTED;
     if (pol.squash && !pol.max_action) return PILCO_ERR_NULL;
-    if (pr->n_rewards < 1 || pr->n_rewards > 8) return PILCO_ERR_DIM;
-    for (int k = 0; k < pr->n_rewards; ++k) {
-        const pilco_reward_term& rt = pr->rewards[k];
-        if (!rt.W) return PILCO_ERR_NULL;
-        if (!reward_kind_known(rt.kind)) return PILCO_ERR_UNSUPPORTED;
-        if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
-        if (reward_needs_t(rt.kind) && !rt.t) return PILCO_ERR_NULL;
-    }
+    if (const int rc = pt_check_rewards(pr, false)) return rc;
     if (!pr->x0 || !pr->eps || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret)
         return PILCO_ERR_NULL;
     if (((uintptr_t)g.iK & 15) || (g.ldk & 1)) return PILCO_ERR_ALIGN;                  // predict's TMA rows
@@ -1201,12 +1199,6 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj);
 }
 
-// exploration (DESIGN.md section 24): b and where sigma_t^2 goes (NULL: nowhere), validated
-struct PxOpt {
-    double b;
-    double* step_var;
-};
-
 // the moments kernel's arguments over the forward's traj and act (tm: the angles' map, or the identity)
 static PxMom px_mom(const pilco_particles* pr, const TrigMap& tm, double b) {
     PxMom m;
@@ -1217,154 +1209,76 @@ static PxMom px_mom(const pilco_particles* pr, const TrigMap& tm, double b) {
     return m;
 }
 
-// the validated gradient of R restarts: the forward with its history, then the reverse sweep.  ex (exploration): the
-// moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
-static int pg_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool consistent,
-                  pilco_stream_t stream, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
-                  const PxOpt* ex = nullptr) {
-    const bool ang = tm != nullptr, noise = nz != nullptr, explore = ex != nullptr;
-    const PtWs L = consistent ? fg_ws_layout(pr, R, ang, noise, explore) : pg_ws_layout(pr, R, ang, noise, explore);
-    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
-    if (consistent) {
-        if (const int rc = fs_predict_prepare()) return rc;
-        if (const int rc = fs_vjp_prepare()) return rc;
-    }
-    cudaStream_t st = (cudaStream_t)stream;
+// The score-function gradient of R restarts after pt_forward(history) (DESIGN.md sections 16, 25):
+//   ps_togo, ps_base, the cotangents of every step's predict and their VJPs, (joint terms) pj_grad over all H steps,
+//   ps_zbar, pg_reduce
+// Step-wise sampler: ps_cot, then the VJP of steps 0..H-2 in groups of whole steps.  The x~ history [H-1,T,D] and the
+// cotangents [H-1,T,Ds] are contiguous, so a group of k steps is one VJP call at k T rows; a point's VJP does not
+// depend on T or on its row, so the grouping changes no bit.
+// Consistent sampler: pc_white_kernel (particles_cscore.cu) turns the weights into m_bar_t and v_bar_t, which stand
+// where the pathwise sweep's x_bar_{t+1} and var_bar_t stand, then memset(Lambda) and [fs_cond_bwd<t>, fs_vjp<t> ->
+// x~_bar_t] for t = H-2 .. 0.  Nothing chains x_bar between steps (x is held fixed), so there is no step kernel; Lambda
+// accumulates over the steps, so the loop stays serial.
+// Angles: the state-width cotangents are in E; ps_zbar and the reduction read the policy inputs from the phi history
+// (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.  Noise: the policy inputs are the phi(z)
+// history; the VJPs act on x~, which holds phi(x), unchanged.
+static int ps_run(const pilco_particles* pr, const PtOpt& o, const pilco_particles_grad* g, const PtWs& L,
+                  cudaStream_t st) {
     double* ws = (double*)g->ws;
-    if (const int rc = pt_forward(pr, R, ws, L, consistent, true, st, tm, nz)) return rc;
-    const bool bonus = explore && ex->b != 0.0;
-    if (explore) {
-        TrigMap id;
-        if (!tm) trig_map_make(pr->dyn.E, 0, nullptr, &id);            // 1 <= E <= PILCO_MAX_E once validated
-        PxMom m = px_mom(pr, tm ? *tm : id, ex->b);
-        m.step_var = ex->step_var; m.sd = ws + L.sd; m.tab = bonus ? ws + L.tab : nullptr;
-        if (const int rc = px_moments_launch(st, R, m)) return rc;
-    }
-    if (const int rc = pg_reverse(pr, R, g, L, consistent, st, tm, nz, bonus)) return rc;
-    if (bonus && pr->H > 0) return px_value_launch(st, R, pr->H, ex->b, ws + L.sd, g->value);
-    return PILCO_OK;
-}
-
-// the forward alone, R = 1 (tm: validated angles, nz: validated noise; the description is checked here)
-static int pt_run(const pilco_particles* pr, bool consistent, pilco_stream_t stream, const TrigMap* tm = nullptr,
-                  const PnNoise* nz = nullptr) {
-    if (const int rc = pt_check_desc(pr, false, tm ? tm->A : 0)) return rc;
-    const PtWs L = consistent ? fs_ws_layout(pr) : pt_ws_layout(pr);
-    if (const int rc = pt_check_ws(pr->ws, pr->ws_bytes, L.total)) return rc;
-    if (consistent)
-        if (const int rc = fs_predict_prepare()) return rc;
-    return pt_forward(pr, 1, (double*)pr->ws, L, consistent, false, (cudaStream_t)stream, tm, nz);
-}
-
-// The score-function gradient of R restarts (validated; DESIGN.md section 16):
-//   pt_forward(history), ps_togo, ps_base, ps_cot, VJP of steps 0..H-2 in groups of whole steps, ps_zbar, pg_reduce
-// The x~ history [H-1,T,D] and the cotangents [H-1,T,Ds] are contiguous, so a group of k steps is one VJP call at k T
-// rows; a point's VJP does not depend on T or on its row, so the grouping changes no bit.
-// tm (angles): the state-width cotangents are in E (ps_cot at Ds = E); ps_zbar and the reduction read the policy
-// inputs from the phi history (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.  nz (noise): the
-// policy inputs are the phi(z) history; the VJPs act on x~, which holds phi(x), unchanged.
-static int ps_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream,
-                  const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
-    const PtWs L = ps_ws_layout(pr, R, tm != nullptr, nz != nullptr);
-    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)g->ws;
-    if (const int rc = pt_forward(pr, R, ws, L, false, true, st, tm, nz)) return rc;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
+    const int R = o.R, P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const int nb = (P + PT_THREADS - 1) / PT_THREADS;
-    const double* pin = nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj;
+    const size_t TD = (size_t)T * D, TE = (size_t)T * E;
+    const double* pin = o.noisy ? ws + L.phiz : o.mapped ? ws + L.phi : pr->traj;
     PsDev a;
     static_cast<PtPolicy&>(a) = pt_policy(pr);
     a.T = T;
     a.eps = pr->eps; a.traj = pin; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
-    a.var = ws + L.var; a.G = ws + L.G; a.S = ws + L.gsum; a.gmean = ws + L.gx; a.gvar = ws + L.gvar;
-    a.gxt = ws + L.gxt; a.zbar = ws + L.zbar;
+    a.var = o.consistent ? nullptr : ws + L.var; a.G = ws + L.togo; a.S = ws + L.gsum; a.gmean = ws + L.mw;
+    a.gvar = ws + L.vw; a.gxt = ws + L.gxh; a.zbar = ws + L.zbar;
     a.direct = pt_has_joint(pr);
     if (H > 1) {
         launch_hi(ps_togo_kernel, dim3(nb, R), dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
         launch_hi(ps_base_kernel, dim3(H - 1, R), dim3(256), 0, st, a);
         CUDA_LAUNCH_CHECK();
-        PsDev ac = a;
-        ac.Ds = E;
-        launch_hi(ps_cot_kernel, dim3(nb * (H - 1), R), dim3(PT_THREADS), 0, st, ac);
-        CUDA_LAUNCH_CHECK();
-        const int grp = ps_group(T, H);
-        for (int t0 = 0; t0 < H - 1; t0 += grp) {
-            const int k = grp < H - 1 - t0 ? grp : H - 1 - t0;
-            const size_t o = (size_t)t0 * T;
-            const int rc = pilco_gp_predict_vjp(&pr->dyn, k * T, ws + L.xt + o * D, ws + L.gx + o * E,
-                                                ws + L.gvar + o * E, ws + L.gxt + o * D, ws + L.vws, L.vws_bytes, st);
-            if (rc) return rc;
+        if (o.consistent) {
+            PcWhite w;
+            w.P = P; w.T = T; w.H = H; w.Ds = E;
+            w.L = ws + L.L; w.eps = pr->eps; w.var = ws + L.var; w.G = a.G; w.S = a.S; w.mbar = a.gmean;
+            w.vbar = a.gvar;
+            if (const int rc = pc_white_launch(st, R, w)) return rc;
+            cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TE * sizeof(double), st);
+            FsBwd q;                                    // as pg_reverse's; the cotangents come from the whitening reverse
+            q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = E; q.np = pad64(pr->dyn.n);
+            q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
+            q.xh = ws + L.xt; q.Kh = ws + L.Kh; q.L = ws + L.L; q.eps = pr->eps;
+            q.G = ws + L.G; q.A = ws + L.W; q.dir = ws + L.dir;
+            const dim3 cgrid((P + FS_WARPS - 1) / FS_WARPS, E, R);
+            for (int t = H - 2; t >= 0; --t) {
+                q.t = t; q.gx = a.gmean + (size_t)t * TE; q.gvar = a.gvar + (size_t)t * TE;
+                launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
+                CUDA_LAUNCH_CHECK();
+                const int rc = fs_vjp_launch(st, &pr->dyn, T, ws + L.xt + (size_t)t * TD, q.gx, q.A, q.dir,
+                                             ws + L.gxh + (size_t)t * TD, ws + L.vws);
+                if (rc) return rc;
+            }
+        } else {
+            PsDev ac = a;
+            ac.Ds = E;
+            launch_hi(ps_cot_kernel, dim3(nb * (H - 1), R), dim3(PT_THREADS), 0, st, ac);
+            CUDA_LAUNCH_CHECK();
+            const int grp = ps_group(T, H);
+            for (int t0 = 0; t0 < H - 1; t0 += grp) {
+                const int k = grp < H - 1 - t0 ? grp : H - 1 - t0;
+                const size_t off = (size_t)t0 * T;
+                const int rc = pilco_gp_predict_vjp(&pr->dyn, k * T, ws + L.xt + off * D, ws + L.mw + off * E,
+                                                    ws + L.vw + off * E, ws + L.gxh + off * D, ws + L.vws, L.vws_bytes,
+                                                    st);
+                if (rc) return rc;
+            }
         }
     }
     if (H > 0 && a.direct) {                            // the direct term: d v_k / d u_t of every step, on top of the VJP's
-        const size_t TD = (size_t)T * D;
-        cudaMemsetAsync(ws + L.gxt + (size_t)(H - 1) * TD, 0, TD * sizeof(double), st);
-        PjDev j = pj_dev(pr, R);
-        j.xh = ws + L.xt; j.gxt = ws + L.gxt; j.gstep = (long long)TD; j.first = Ds;
-        launch_hi(pj_grad_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, j);
-        CUDA_LAUNCH_CHECK();
-    }
-    if (H > 0) {
-        launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-    }
-    return pg_reduce(pr, R, g, ws, L, st, pin);
-}
-
-// The score-function gradient over consistent function samples of R restarts (validated; DESIGN.md section 25):
-//   pt_forward(consistent, history), ps_togo, ps_base, pc_white, memset(Lambda),
-//   [fs_cond_bwd<t>, fs_vjp<t> -> x~_bar_t] for t = H-2 .. 0, (joint terms) pj_grad over all H steps, ps_zbar, pg_reduce
-// m_bar_t and v_bar_t stand where the pathwise sweep's x_bar_{t+1} and var_bar_t stand.  Nothing chains x_bar between
-// steps (x is held fixed), so there is no step kernel; Lambda accumulates over the steps, so the loop stays serial.
-// tm, nz: as ps_run (the policy inputs are the phi or phi(z) history, the direct term starts at x~ column Dh).
-static int pc_run(const pilco_particles* pr, int R, const pilco_particles_grad* g, pilco_stream_t stream,
-                  const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
-    const PtWs L = fg_ws_layout(pr, R, tm != nullptr, nz != nullptr, false, true);
-    if (const int rc = pt_check_ws(g->ws, g->ws_bytes, L.total)) return rc;
-    if (const int rc = fs_predict_prepare()) return rc;
-    if (const int rc = fs_vjp_prepare()) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    double* ws = (double*)g->ws;
-    if (const int rc = pt_forward(pr, R, ws, L, true, true, st, tm, nz)) return rc;
-    const int P = pr->P, H = pr->H, Ds = pr->pol.Ds, E = pr->dyn.E, D = pr->dyn.D, T = R * P;
-    const int nb = (P + PT_THREADS - 1) / PT_THREADS;
-    const size_t TD = (size_t)T * D, TE = (size_t)T * E;
-    const double* pin = nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj;
-    PsDev a;
-    static_cast<PtPolicy&>(a) = pt_policy(pr);
-    a.T = T;
-    a.eps = pr->eps; a.traj = pin; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk;
-    a.var = nullptr; a.G = ws + L.togo; a.S = ws + L.gsum; a.gmean = ws + L.mw; a.gvar = ws + L.vw;
-    a.gxt = ws + L.gxh; a.zbar = ws + L.zbar;
-    a.direct = pt_has_joint(pr);
-    if (H > 1) {
-        launch_hi(ps_togo_kernel, dim3(nb, R), dim3(PT_THREADS), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        launch_hi(ps_base_kernel, dim3(H - 1, R), dim3(256), 0, st, a);
-        CUDA_LAUNCH_CHECK();
-        PcWhite w;
-        w.P = P; w.T = T; w.H = H; w.Ds = E;
-        w.L = ws + L.L; w.eps = pr->eps; w.var = ws + L.var; w.G = a.G; w.S = a.S; w.mbar = a.gmean; w.vbar = a.gvar;
-        if (const int rc = pc_white_launch(st, R, w)) return rc;
-        cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TE * sizeof(double), st);
-        FsBwd q;                                        // as pg_reverse's; the cotangents come from the whitening reverse
-        q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = E; q.np = pad64(pr->dyn.n);
-        q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2;
-        q.xh = ws + L.xt; q.Kh = ws + L.Kh; q.L = ws + L.L; q.eps = pr->eps;
-        q.G = ws + L.G; q.A = ws + L.W; q.dir = ws + L.dir;
-        const dim3 cgrid((P + FS_WARPS - 1) / FS_WARPS, E, R);
-        for (int t = H - 2; t >= 0; --t) {
-            q.t = t; q.gx = a.gmean + (size_t)t * TE; q.gvar = a.gvar + (size_t)t * TE;
-            launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
-            CUDA_LAUNCH_CHECK();
-            const int rc = fs_vjp_launch(st, &pr->dyn, T, ws + L.xt + (size_t)t * TD, q.gx, q.A, q.dir,
-                                         ws + L.gxh + (size_t)t * TD, ws + L.vws);
-            if (rc) return rc;
-        }
-    }
-    if (H > 0 && a.direct) {                            // the direct term, as ps_run
         cudaMemsetAsync(ws + L.gxh + (size_t)(H - 1) * TD, 0, TD * sizeof(double), st);
         PjDev j = pj_dev(pr, R);
         j.xh = ws + L.xt; j.gxt = ws + L.gxh; j.gstep = (long long)TD; j.first = Ds;
@@ -1376,19 +1290,6 @@ static int pc_run(const pilco_particles* pr, int R, const pilco_particles_grad* 
         CUDA_LAUNCH_CHECK();
     }
     return pg_reduce(pr, R, g, ws, L, st, pin);
-}
-
-// everything a gradient entry point checks before its workspace: batched honours the policy's batch strides
-static int pg_validate(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, int A = 0) {
-    if (const int rc = pt_check_desc(pr, batched, A)) return rc;
-    if (batched && !pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;
-    return pg_check(pr, g);
-}
-
-static int pg_entry(const pilco_particles* pr, int R, const pilco_particles_grad* g, bool batched, bool consistent,
-                    pilco_stream_t stream, const TrigMap* tm = nullptr) {
-    if (const int rc = pg_validate(pr, R, g, batched, tm ? tm->A : 0)) return rc;
-    return pg_run(pr, R, g, consistent, stream, tm);
 }
 
 // ---- angular state dimensions (DESIGN.md section 20) ----------------------------------------------------------------
@@ -1405,12 +1306,6 @@ static int pa_map(const pilco_particles* pr, const pilco_angles* ang, TrigMap* t
 
 static bool pa_none(const pilco_angles* ang) { return !ang || ang->A == 0; }
 
-// an angle twin's workspace: its layout with the angles' map valid, 0 otherwise
-static bool pa_sizes_ok(const pilco_particles* pr, const pilco_angles* ang) {
-    TrigMap tm;
-    return pr && pt_sizes_ok(pr) && pa_map(pr, ang, &tm) == PILCO_OK;
-}
-
 // ---- measurement noise at the policy's input (DESIGN.md section 23) -------------------------------------------------
 // The noise's own checks, after the description's: PILCO_ERR_DIM for a non-finite or negative var[i] (i < dyn.E), then
 // PILCO_ERR_NULL for nu == NULL with H > 0.  Fills n (sqrt(var), nu).  pr has passed its description's checks.
@@ -1426,43 +1321,8 @@ static int pn_noise(const pilco_particles* pr, const pilco_particles_noise* nz, 
     return PILCO_OK;
 }
 
-// everything a noisy call checks before its workspace (nz != NULL), in order: the angles' map (A >= 1), the
-// description as the angle call checks it (grad: pg_validate with the policy's batch strides), then the noise.
-// Fills tm (without angles: the identity map, A = 0) and n.
-static int pn_validate(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz, int R,
-                       const pilco_particles_grad* g, bool grad, TrigMap* tm, PnNoise* n) {
-    if (!pr) return PILCO_ERR_NULL;
-    const bool none = pa_none(ang);
-    if (!none)
-        if (const int rc = pa_map(pr, ang, tm)) return rc;
-    const int A = none ? 0 : tm->A;
-    if (const int rc = grad ? pg_validate(pr, R, g, true, A) : pt_check_desc(pr, false, A)) return rc;
-    if (none) trig_map_make(pr->dyn.E, 0, nullptr, tm);            // 1 <= E <= PILCO_MAX_E once the description passed
-    return pn_noise(pr, nz, n);
-}
-
-// a gradient's checks up to its workspace with optional angles and noise: the noisy call's (nz NULL: the angle or
-// plain call's).  Fills tm when ang or nz is given (then *mapped), n when nz is.
-static int pn_grad_validate(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz, int R,
-                            const pilco_particles_grad* g, TrigMap* tm, PnNoise* n, bool* mapped) {
-    const bool none = pa_none(ang);
-    *mapped = nz || !none;
-    if (nz) return pn_validate(pr, ang, nz, R, g, true, tm, n);
-    if (!pr) return PILCO_ERR_NULL;
-    if (!none)
-        if (const int rc = pa_map(pr, ang, tm)) return rc;
-    return pg_validate(pr, R, g, true, none ? 0 : tm->A);
-}
-
-// a noisy call's workspace query (nz != NULL): the sizes the angle query accepts and valid noise
-static bool pn_sizes_ok(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz) {
-    if (!pr || !pt_sizes_ok(pr) || (!pa_none(ang) && !pa_sizes_ok(pr, ang))) return false;
-    if (pr->dyn.E < 1 || pr->dyn.E > MAXE) return false;
-    PnNoise n;
-    return pn_noise(pr, nz, &n) == PILCO_OK;
-}
-
 // ---- exploration objective (DESIGN.md section 24) -------------------------------------------------------------------
+// inactive (NULL, or b == 0 with step_var NULL): the call without exploration
 static bool px_active(const pilco_exploration* ex) { return ex && (ex->b != 0.0 || ex->step_var); }
 
 // the exploration's own checks, after the description's: PILCO_ERR_DIM for a non-finite b, PILCO_ERR_UNSUPPORTED for
@@ -1476,273 +1336,268 @@ static int px_check(const pilco_particles* pr, const pilco_exploration* ex) {
     return PILCO_OK;
 }
 
-// an active explore call's workspace (0 where the call would fail on the size or exploration checks): the noisy
-// call's layout (angles flag: angles or noise; noise flag: noise) with sigma_t and the bonus table after it
-static size_t px_ws_bytes(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                          const pilco_exploration* ex, int R, bool consistent) {
-    const size_t base = consistent ? pilco_particles_noisy_consistent_grad_workspace_bytes(pr, ang, nz, R)
-                                   : pilco_particles_noisy_batch_grad_workspace_bytes(pr, ang, nz, R);
-    if (base == 0 || px_check(pr, ex)) return 0;
-    const bool angles = nz || !pa_none(ang), noise = nz != nullptr;
-    return (consistent ? fg_ws_layout(pr, R, angles, noise, true) : pg_ws_layout(pr, R, angles, noise, true)).total;
+// ---- one validator, one query, one call path --------------------------------------------------------------------------
+// Everything a call checks before its workspace, in this order: NULL pr, the angles' map (A != 0), the description
+// (the policy's batch strides as o->batched allows), R, the gradient's outputs, the noise, the exploration (active
+// only).  Each family's call is the most general call with NULL for the features it lacks, so ang == NULL or A == 0
+// is the call without angles, nz == NULL the call without noise and an inactive ex the call without exploration.
+static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                       const pilco_exploration* ex, int R, const pilco_particles_grad* g) {
+    if (!pr) return PILCO_ERR_NULL;
+    const bool angles = !pa_none(ang);
+    if (angles)
+        if (const int rc = pa_map(pr, ang, &o->tm)) return rc;
+    if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0)) return rc;
+    if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;   // the unbatched calls' R = 1 passes with the description
+    if (o->call != PT_FORWARD)
+        if (const int rc = pg_check(pr, g)) return rc;
+    if (!angles) trig_map_make(pr->dyn.E, 0, nullptr, &o->tm);     // 1 <= E <= PILCO_MAX_E once the description passed
+    if (nz)
+        if (const int rc = pn_noise(pr, nz, &o->nz)) return rc;
+    o->explore = px_active(ex);
+    if (o->explore) {
+        if (const int rc = px_check(pr, ex)) return rc;
+        o->b = ex->b; o->step_var = ex->step_var; o->bonus = ex->b != 0.0;
+    }
+    o->R = R; o->mapped = angles || nz; o->noisy = nz != nullptr;
+    return PILCO_OK;
 }
 
-// an active explore gradient: the noisy call's checks up to its workspace (nz NULL: the angle or plain call's), then
-// the exploration's, then pg_run with the path the noisy call takes
-static int px_grad(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                   const pilco_exploration* ex, int R, const pilco_particles_grad* g, bool consistent,
-                   pilco_stream_t stream) {
-    TrigMap tm; PnNoise n; bool mapped;
-    if (const int rc = pn_grad_validate(pr, ang, nz, R, g, &tm, &n, &mapped)) return rc;
-    if (const int rc = px_check(pr, ex)) return rc;
-    const PxOpt o = {ex->b, ex->step_var};
-    return pg_run(pr, R, g, consistent, stream, mapped ? &tm : nullptr, nz ? &n : nullptr, &o);
+// A call's workspace: its layout's total, 0 where the call would fail on its sizes.  The sizes accepted are the
+// description's own (pt_sizes_ok, not its width consistency), R, the angles' map, 1 <= E <= PILCO_MAX_E and valid
+// variances with noise, and the exploration's checks when active.
+static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                       const pilco_exploration* ex, int R) {
+    if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    if (!pa_none(ang) && pa_map(pr, ang, &o.tm)) return 0;
+    if (nz && (pr->dyn.E < 1 || pr->dyn.E > MAXE || pn_noise(pr, nz, &o.nz))) return 0;
+    o.explore = px_active(ex);
+    if (o.explore && px_check(pr, ex)) return 0;
+    o.R = R; o.mapped = nz || !pa_none(ang); o.noisy = nz != nullptr;
+    return (o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o)).total;
 }
+
+// Every rollout call: validate, lay out, check the workspace (pr's for the forward, g's for a gradient), prepare, then
+// the forward (with its history for a gradient) and the gradient's reverse part.  Pathwise with exploration: the
+// moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
+static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                   const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
+    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g)) return rc;
+    const bool fwd = o.call == PT_FORWARD;
+    const PtWs L = o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
+    if (const int rc = fwd ? pt_check_ws(pr->ws, pr->ws_bytes, L.total) : pt_check_ws(g->ws, g->ws_bytes, L.total))
+        return rc;
+    if (o.consistent) {
+        if (const int rc = fs_predict_prepare()) return rc;
+        if (!fwd)
+            if (const int rc = fs_vjp_prepare()) return rc;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    double* ws = (double*)(fwd ? pr->ws : g->ws);
+    const TrigMap* tm = o.mapped ? &o.tm : nullptr;
+    const PnNoise* n = o.noisy ? &o.nz : nullptr;
+    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n)) return rc;
+    if (fwd) return PILCO_OK;
+    if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
+    if (o.explore) {
+        PxMom m = px_mom(pr, o.tm, o.b);
+        m.step_var = o.step_var; m.sd = ws + L.sd; m.tab = o.bonus ? ws + L.tab : nullptr;
+        if (const int rc = px_moments_launch(st, R, m)) return rc;
+    }
+    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus)) return rc;
+    if (o.bonus && pr->H > 0) return px_value_launch(st, R, pr->H, o.b, ws + L.sd, g->value);
+    return PILCO_OK;
+}
+
+// the sampler, the call and whether the policy's batch strides are honoured, per family
+static const PtOpt FWD = {false, PT_FORWARD, false}, CFWD = {true, PT_FORWARD, false};
+static const PtOpt PATH1 = {false, PT_PATHWISE, false}, PATH = {false, PT_PATHWISE, true};
+static const PtOpt CPATH = {true, PT_PATHWISE, true}, SCORE = {false, PT_SCORE, true}, CSCORE = {true, PT_SCORE, true};
 
 extern "C" {
 
 size_t pilco_particles_workspace_bytes(const pilco_particles* pr) {
-    return pr && pt_sizes_ok(pr) ? pt_ws_layout(pr).total : 0;
+    return pt_query(FWD, pr, nullptr, nullptr, nullptr, 1);
 }
 
 int pilco_particles_rollout(const pilco_particles* pr, pilco_stream_t stream) {
-    return pt_run(pr, false, stream);
+    return pt_call(FWD, pr, nullptr, nullptr, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_grad_workspace_bytes(const pilco_particles* pr) {
-    return pr && pt_sizes_ok(pr) ? pg_ws_layout(pr, 1).total : 0;
+    return pt_query(PATH1, pr, nullptr, nullptr, nullptr, 1);
 }
 
 int pilco_particles_rollout_grad(const pilco_particles* pr, const pilco_particles_grad* g, pilco_stream_t stream) {
-    return pg_entry(pr, 1, g, false, false, stream);
+    return pt_call(PATH1, pr, nullptr, nullptr, nullptr, 1, g, stream);
 }
 
 size_t pilco_particles_batch_grad_workspace_bytes(const pilco_particles* pr, int R) {
-    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R).total : 0;
+    return pt_query(PATH, pr, nullptr, nullptr, nullptr, R);
 }
 
 int pilco_particles_rollout_batch_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                        pilco_stream_t stream) {
-    return pg_entry(pr, R, g, true, false, stream);
+    return pt_call(PATH, pr, nullptr, nullptr, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_consistent_workspace_bytes(const pilco_particles* pr) {
-    return pr && pt_sizes_ok(pr) ? fs_ws_layout(pr).total : 0;
+    return pt_query(CFWD, pr, nullptr, nullptr, nullptr, 1);
 }
 
 int pilco_particles_rollout_consistent(const pilco_particles* pr, pilco_stream_t stream) {
-    return pt_run(pr, true, stream);
+    return pt_call(CFWD, pr, nullptr, nullptr, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_consistent_grad_workspace_bytes(const pilco_particles* pr, int R) {
-    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R).total : 0;
+    return pt_query(CPATH, pr, nullptr, nullptr, nullptr, R);
 }
 
 int pilco_particles_rollout_consistent_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                             pilco_stream_t stream) {
-    return pg_entry(pr, R, g, true, true, stream);
+    return pt_call(CPATH, pr, nullptr, nullptr, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_score_grad_workspace_bytes(const pilco_particles* pr, int R) {
-    return pr && pt_sizes_ok(pr) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R).total : 0;
+    return pt_query(SCORE, pr, nullptr, nullptr, nullptr, R);
 }
 
 int pilco_particles_rollout_score_grad(const pilco_particles* pr, int R, const pilco_particles_grad* g,
                                        pilco_stream_t stream) {
-    if (const int rc = pg_validate(pr, R, g, true)) return rc;
-    return ps_run(pr, R, g, stream);
+    return pt_call(SCORE, pr, nullptr, nullptr, nullptr, R, g, stream);
 }
 
-// ---- the angle twins: ang == NULL or A == 0 is the call without angles ----------------------------------------------
 size_t pilco_particles_angles_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang) {
-    if (pa_none(ang)) return pilco_particles_workspace_bytes(pr);
-    return pa_sizes_ok(pr, ang) ? pt_ws_layout(pr).total : 0;
+    return pt_query(FWD, pr, ang, nullptr, nullptr, 1);
 }
 
 int pilco_particles_angles_rollout(const pilco_particles* pr, const pilco_angles* ang, pilco_stream_t stream) {
-    if (pa_none(ang)) return pilco_particles_rollout(pr, stream);
-    if (!pr) return PILCO_ERR_NULL;
-    TrigMap tm;
-    if (const int rc = pa_map(pr, ang, &tm)) return rc;
-    return pt_run(pr, false, stream, &tm);
+    return pt_call(FWD, pr, ang, nullptr, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_angles_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang) {
-    if (pa_none(ang)) return pilco_particles_consistent_workspace_bytes(pr);
-    return pa_sizes_ok(pr, ang) ? fs_ws_layout(pr).total : 0;
+    return pt_query(CFWD, pr, ang, nullptr, nullptr, 1);
 }
 
 int pilco_particles_angles_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                               pilco_stream_t stream) {
-    if (pa_none(ang)) return pilco_particles_rollout_consistent(pr, stream);
-    if (!pr) return PILCO_ERR_NULL;
-    TrigMap tm;
-    if (const int rc = pa_map(pr, ang, &tm)) return rc;
-    return pt_run(pr, true, stream, &tm);
+    return pt_call(CFWD, pr, ang, nullptr, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_angles_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R) {
-    if (pa_none(ang)) return pilco_particles_batch_grad_workspace_bytes(pr, R);
-    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R, true).total : 0;
+    return pt_query(PATH, pr, ang, nullptr, nullptr, R);
 }
 
 int pilco_particles_angles_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
                                               const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (pa_none(ang)) return pilco_particles_rollout_batch_grad(pr, R, g, stream);
-    if (!pr) return PILCO_ERR_NULL;
-    TrigMap tm;
-    if (const int rc = pa_map(pr, ang, &tm)) return rc;
-    return pg_entry(pr, R, g, true, false, stream, &tm);
+    return pt_call(PATH, pr, ang, nullptr, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_angles_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                               int R) {
-    if (pa_none(ang)) return pilco_particles_consistent_grad_workspace_bytes(pr, R);
-    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R, true).total : 0;
+    return pt_query(CPATH, pr, ang, nullptr, nullptr, R);
 }
 
 int pilco_particles_angles_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
                                                    const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (pa_none(ang)) return pilco_particles_rollout_consistent_grad(pr, R, g, stream);
-    if (!pr) return PILCO_ERR_NULL;
-    TrigMap tm;
-    if (const int rc = pa_map(pr, ang, &tm)) return rc;
-    return pg_entry(pr, R, g, true, true, stream, &tm);
+    return pt_call(CPATH, pr, ang, nullptr, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_angles_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang, int R) {
-    if (pa_none(ang)) return pilco_particles_score_grad_workspace_bytes(pr, R);
-    return pa_sizes_ok(pr, ang) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R, true).total : 0;
+    return pt_query(SCORE, pr, ang, nullptr, nullptr, R);
 }
 
 int pilco_particles_angles_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang, int R,
                                               const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (pa_none(ang)) return pilco_particles_rollout_score_grad(pr, R, g, stream);
-    if (!pr) return PILCO_ERR_NULL;
-    TrigMap tm;
-    if (const int rc = pa_map(pr, ang, &tm)) return rc;
-    if (const int rc = pg_validate(pr, R, g, true, tm.A)) return rc;
-    return ps_run(pr, R, g, stream, &tm);
+    return pt_call(SCORE, pr, ang, nullptr, nullptr, R, g, stream);
 }
 
-// ---- the noisy twins: nz == NULL is the angle call (ang may be NULL) -----------------------------------------------
 size_t pilco_particles_noisy_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                              const pilco_particles_noise* nz) {
-    if (!nz) return pilco_particles_angles_workspace_bytes(pr, ang);
-    return pn_sizes_ok(pr, ang, nz) ? pt_ws_layout(pr).total : 0;
+    return pt_query(FWD, pr, ang, nz, nullptr, 1);
 }
 
 int pilco_particles_noisy_rollout(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                                   pilco_stream_t stream) {
-    if (!nz) return pilco_particles_angles_rollout(pr, ang, stream);
-    TrigMap tm; PnNoise n;
-    if (const int rc = pn_validate(pr, ang, nz, 1, nullptr, false, &tm, &n)) return rc;
-    return pt_run(pr, false, stream, &tm, &n);
+    return pt_call(FWD, pr, ang, nz, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_noisy_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                         const pilco_particles_noise* nz) {
-    if (!nz) return pilco_particles_angles_consistent_workspace_bytes(pr, ang);
-    return pn_sizes_ok(pr, ang, nz) ? fs_ws_layout(pr).total : 0;
+    return pt_query(CFWD, pr, ang, nz, nullptr, 1);
 }
 
 int pilco_particles_noisy_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                              const pilco_particles_noise* nz, pilco_stream_t stream) {
-    if (!nz) return pilco_particles_angles_consistent_rollout(pr, ang, stream);
-    TrigMap tm; PnNoise n;
-    if (const int rc = pn_validate(pr, ang, nz, 1, nullptr, false, &tm, &n)) return rc;
-    return pt_run(pr, true, stream, &tm, &n);
+    return pt_call(CFWD, pr, ang, nz, nullptr, 1, nullptr, stream);
 }
 
 size_t pilco_particles_noisy_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                         const pilco_particles_noise* nz, int R) {
-    if (!nz) return pilco_particles_angles_batch_grad_workspace_bytes(pr, ang, R);
-    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? pg_ws_layout(pr, R, true, true).total : 0;
+    return pt_query(PATH, pr, ang, nz, nullptr, R);
 }
 
 int pilco_particles_noisy_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                              const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
                                              pilco_stream_t stream) {
-    if (!nz) return pilco_particles_angles_batch_grad_rollout(pr, ang, R, g, stream);
-    TrigMap tm; PnNoise n;
-    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
-    return pg_run(pr, R, g, false, stream, &tm, &n);
+    return pt_call(PATH, pr, ang, nz, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_noisy_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                              const pilco_particles_noise* nz, int R) {
-    if (!nz) return pilco_particles_angles_consistent_grad_workspace_bytes(pr, ang, R);
-    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? fg_ws_layout(pr, R, true, true).total : 0;
+    return pt_query(CPATH, pr, ang, nz, nullptr, R);
 }
 
 int pilco_particles_noisy_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                                   const pilco_particles_noise* nz, int R,
                                                   const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (!nz) return pilco_particles_angles_consistent_grad_rollout(pr, ang, R, g, stream);
-    TrigMap tm; PnNoise n;
-    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
-    return pg_run(pr, R, g, true, stream, &tm, &n);
+    return pt_call(CPATH, pr, ang, nz, nullptr, R, g, stream);
 }
 
 size_t pilco_particles_noisy_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                         const pilco_particles_noise* nz, int R) {
-    if (!nz) return pilco_particles_angles_score_grad_workspace_bytes(pr, ang, R);
-    return pn_sizes_ok(pr, ang, nz) && pt_batch_ok(pr->P, R) ? ps_ws_layout(pr, R, true, true).total : 0;
+    return pt_query(SCORE, pr, ang, nz, nullptr, R);
 }
 
 int pilco_particles_noisy_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                              const pilco_particles_noise* nz, int R, const pilco_particles_grad* g,
                                              pilco_stream_t stream) {
-    if (!nz) return pilco_particles_angles_score_grad_rollout(pr, ang, R, g, stream);
-    TrigMap tm; PnNoise n;
-    if (const int rc = pn_validate(pr, ang, nz, R, g, true, &tm, &n)) return rc;
-    return ps_run(pr, R, g, stream, &tm, &n);
+    return pt_call(SCORE, pr, ang, nz, nullptr, R, g, stream);
 }
 
-
-// ---- the explore twins: an inactive ex (NULL, or b == 0 with step_var NULL) is the noisy call ------------------------
 size_t pilco_particles_explore_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                           const pilco_particles_noise* nz, const pilco_exploration* ex,
                                                           int R) {
-    if (!px_active(ex)) return pilco_particles_noisy_batch_grad_workspace_bytes(pr, ang, nz, R);
-    return px_ws_bytes(pr, ang, nz, ex, R, false);
+    return pt_query(PATH, pr, ang, nz, ex, R);
 }
 
 int pilco_particles_explore_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                                const pilco_particles_noise* nz, const pilco_exploration* ex, int R,
                                                const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (!px_active(ex)) return pilco_particles_noisy_batch_grad_rollout(pr, ang, nz, R, g, stream);
-    return px_grad(pr, ang, nz, ex, R, g, false, stream);
+    return pt_call(PATH, pr, ang, nz, ex, R, g, stream);
 }
 
 size_t pilco_particles_explore_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                                const pilco_particles_noise* nz,
                                                                const pilco_exploration* ex, int R) {
-    if (!px_active(ex)) return pilco_particles_noisy_consistent_grad_workspace_bytes(pr, ang, nz, R);
-    return px_ws_bytes(pr, ang, nz, ex, R, true);
+    return pt_query(CPATH, pr, ang, nz, ex, R);
 }
 
 int pilco_particles_explore_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                                     const pilco_particles_noise* nz, const pilco_exploration* ex, int R,
                                                     const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (!px_active(ex)) return pilco_particles_noisy_consistent_grad_rollout(pr, ang, nz, R, g, stream);
-    return px_grad(pr, ang, nz, ex, R, g, true, stream);
+    return pt_call(CPATH, pr, ang, nz, ex, R, g, stream);
 }
 
-// ---- the score-function gradient over consistent function samples (DESIGN.md section 25) -------------------------
 size_t pilco_particles_consistent_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                              const pilco_particles_noise* nz, int R) {
-    const bool sizes = nz ? pn_sizes_ok(pr, ang, nz) : pr && (pa_none(ang) ? pt_sizes_ok(pr) : pa_sizes_ok(pr, ang));
-    if (!sizes || !pt_batch_ok(pr->P, R)) return 0;
-    return fg_ws_layout(pr, R, nz || !pa_none(ang), nz != nullptr, false, true).total;
+    return pt_query(CSCORE, pr, ang, nz, nullptr, R);
 }
 
 int pilco_particles_consistent_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
                                                   const pilco_particles_noise* nz, int R,
                                                   const pilco_particles_grad* g, pilco_stream_t stream) {
-    TrigMap tm; PnNoise n; bool mapped;
-    if (const int rc = pn_grad_validate(pr, ang, nz, R, g, &tm, &n, &mapped)) return rc;
-    return pc_run(pr, R, g, stream, mapped ? &tm : nullptr, nz ? &n : nullptr);
+    return pt_call(CSCORE, pr, ang, nz, nullptr, R, g, stream);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,
@@ -1754,15 +1609,7 @@ int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles
     if (pr->P < 2 || pr->H < 0 || R < 1 || R > 65535 || U < 1 || trig_map_make(E, A, A ? ang->dims : nullptr, &tm) ||
         E > MAXE || pr->pol.Ds != E + A || E + A + U > MAXD)
         return PILCO_ERR_DIM;
-    if (pr->n_rewards < 1 || pr->n_rewards > 8) return PILCO_ERR_DIM;
-    for (int k = 0; k < pr->n_rewards; ++k) {
-        const pilco_reward_term& rt = pr->rewards[k];
-        if (!rt.W) return PILCO_ERR_NULL;
-        if (!reward_kind_known(rt.kind)) return PILCO_ERR_UNSUPPORTED;
-        if (rt.channel != PILCO_CHANNEL_ADD && rt.channel != PILCO_CHANNEL_MULT) return PILCO_ERR_UNSUPPORTED;
-        if (reward_needs_t(rt.kind) && !rt.t) return PILCO_ERR_NULL;
-        if (rt.channel == PILCO_CHANNEL_ADD && rt.kind == PILCO_REWARD_BOX) return PILCO_ERR_UNSUPPORTED;
-    }
+    if (const int rc = pt_check_rewards(pr, true)) return rc;
     if (pr->H > 0 && (!pr->traj || !pr->act)) return PILCO_ERR_NULL;
     PxMom m = px_mom(pr, tm, 0.0);
     m.step_mean = step_mean; m.step_var = step_var;

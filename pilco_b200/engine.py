@@ -686,6 +686,19 @@ class RolloutPlan:
         return self.gbuf
 
 
+# (consistent, call) -> the C rollout and its size query (after "pilco_particles_"): the most general entry point of each
+# kind, given NULL for the angles, noise or exploration a plan lacks.  The pathwise call of an unbatched plan is the
+# batched one at R = 1 (its policy strides are 0).
+PARTICLE_CALLS = {
+    (False, "forward"): ("noisy_rollout", "noisy_workspace_bytes"),
+    (True, "forward"): ("noisy_consistent_rollout", "noisy_consistent_workspace_bytes"),
+    (False, "pathwise"): ("explore_batch_grad_rollout", "explore_batch_grad_workspace_bytes"),
+    (True, "pathwise"): ("explore_consistent_grad_rollout", "explore_consistent_grad_workspace_bytes"),
+    (False, "score"): ("noisy_score_grad_rollout", "noisy_score_grad_workspace_bytes"),
+    (True, "score"): ("consistent_score_grad_rollout", "consistent_score_grad_workspace_bytes"),
+}
+
+
 class ParticlePlan:
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
 
@@ -744,24 +757,8 @@ class ParticlePlan:
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration)
         pr, d = self.pr, device()
         P, H = self.P, self.H
-        if self.consistent:
-            if self.nz is not None:
-                wsb = lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), self._ang_ref(), C.byref(self.nz))
-            elif self.ang is None:
-                wsb = lib.pilco_particles_consistent_workspace_bytes(C.byref(pr))
-            else:
-                wsb = lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(self.ang))
-            if wsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
-            self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
-            pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
-        elif not self.batched:                                  # the forward-only rollout (a batch has none)
-            if self.nz is not None:
-                wsb = lib.pilco_particles_noisy_workspace_bytes(C.byref(pr), self._ang_ref(), C.byref(self.nz))
-            elif self.ang is None:
-                wsb = lib.pilco_particles_workspace_bytes(C.byref(pr))
-            else:
-                wsb = lib.pilco_particles_angles_workspace_bytes(C.byref(pr), C.byref(self.ang))
+        if not self.batched:                                    # the forward-only rollout (a batch has none)
+            wsb = self._query("forward", pr)
             if wsb == 0:
                 raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
@@ -770,26 +767,21 @@ class ParticlePlan:
         if grad:
             self._grad_buffers(self._grad_ws_bytes(P))
 
+    def _args(self, kind, pr):
+        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise) and R"""
+        args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
+        if kind == "pathwise":
+            args.append(C.byref(self.ex) if self.ex is not None else None)
+        return args + ([self.R] if kind != "forward" else [])
+
+    def _query(self, kind, pr):
+        return int(getattr(lib, "pilco_particles_" + PARTICLE_CALLS[self.consistent, kind][1])(*self._args(kind, pr)))
+
     def _grad_ws_bytes(self, P):
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
-        if self.ex is not None:
-            return int(lib.pilco_particles_explore_batch_grad_workspace_bytes(C.byref(pr), self._ang_ref(), self._nz_ref(),
-                                                                              C.byref(self.ex), self.R))
-        if self.nz is not None:
-            f = (lib.pilco_particles_noisy_score_grad_workspace_bytes if self.estimator == "score" else
-                 lib.pilco_particles_noisy_batch_grad_workspace_bytes)
-            return int(f(C.byref(pr), self._ang_ref(), C.byref(self.nz), self.R))
-        if self.ang is not None:
-            f = (lib.pilco_particles_angles_score_grad_workspace_bytes if self.estimator == "score" else
-                 lib.pilco_particles_angles_batch_grad_workspace_bytes)
-            return int(f(C.byref(pr), C.byref(self.ang), self.R))
-        if self.estimator == "score":
-            return int(lib.pilco_particles_score_grad_workspace_bytes(C.byref(pr), self.R))
-        if self.batched:
-            return int(lib.pilco_particles_batch_grad_workspace_bytes(C.byref(pr), self.R))
-        return int(lib.pilco_particles_grad_workspace_bytes(C.byref(pr)))
+        return self._query(self.estimator, pr)
 
     def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None,
                   exploration=None):
@@ -879,38 +871,12 @@ class ParticlePlan:
         With ``exploration``: value and gradient of the exploration objective, and sigma_t^2 in ``step_var``."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        if self.ex is not None:
-            check(lib.pilco_particles_explore_batch_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
-                                                                 C.byref(self.ex), self.R, C.byref(self.grad),
-                                                                 stream_ptr()), "particles_explore_batch_grad_rollout")
-        elif self.nz is not None:
-            if self.estimator == "score":
-                check(lib.pilco_particles_noisy_score_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
-                                                                   self.R, C.byref(self.grad), stream_ptr()),
-                      "particles_noisy_score_grad_rollout")
-            else:
-                check(lib.pilco_particles_noisy_batch_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
-                                                                   self.R, C.byref(self.grad), stream_ptr()),
-                      "particles_noisy_batch_grad_rollout")
-        elif self.ang is not None:
-            if self.estimator == "score":
-                check(lib.pilco_particles_angles_score_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
-                                                                    C.byref(self.grad), stream_ptr()),
-                      "particles_angles_score_grad_rollout")
-            else:
-                check(lib.pilco_particles_angles_batch_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
-                                                                    C.byref(self.grad), stream_ptr()),
-                      "particles_angles_batch_grad_rollout")
-        elif self.estimator == "score":
-            check(lib.pilco_particles_rollout_score_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
-                  "particles_rollout_score_grad")
-        elif self.batched:
-            check(lib.pilco_particles_rollout_batch_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
-                  "particles_rollout_batch_grad")
-        else:
-            check(lib.pilco_particles_rollout_grad(C.byref(self.pr), C.byref(self.grad), stream_ptr()),
-                  "particles_rollout_grad")
+        self._call(self.estimator, C.byref(self.grad))
         return self.gbuf
+
+    def _call(self, kind, *grad):
+        name = "particles_" + PARTICLE_CALLS[self.consistent, kind][0]
+        check(getattr(lib, "pilco_" + name)(*self._args(kind, self.pr), *grad, stream_ptr()), name)
 
     def set_inputs(self, x0, eps, nu=None):
         """x0 [P,Ds], eps [P,H,Ds] and, with measurement noise, nu [P,H,E] (required then, and only then)"""
@@ -925,26 +891,7 @@ class ParticlePlan:
     def launch(self):
         if self.batched:
             raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
-        if self.nz is not None:
-            if self.consistent:
-                check(lib.pilco_particles_noisy_consistent_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
-                                                                   stream_ptr()), "particles_noisy_consistent_rollout")
-            else:
-                check(lib.pilco_particles_noisy_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
-                                                        stream_ptr()), "particles_noisy_rollout")
-            return
-        if self.ang is not None:
-            if self.consistent:
-                check(lib.pilco_particles_angles_consistent_rollout(C.byref(self.pr), C.byref(self.ang), stream_ptr()),
-                      "particles_angles_consistent_rollout")
-            else:
-                check(lib.pilco_particles_angles_rollout(C.byref(self.pr), C.byref(self.ang), stream_ptr()),
-                      "particles_angles_rollout")
-            return
-        if self.consistent:
-            check(lib.pilco_particles_rollout_consistent(C.byref(self.pr), stream_ptr()), "particles_rollout_consistent")
-            return
-        check(lib.pilco_particles_rollout(C.byref(self.pr), stream_ptr()), "particles_rollout")
+        self._call("forward")
 
     def outputs(self):
         """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views), each
@@ -995,25 +942,6 @@ class ConsistentGradPlan(ParticlePlan):
                              "num_samples=%d would fit" % (self.R, self.P, self.H, need, max_ws_bytes, lo))
         self._grad_buffers(need)
 
-    def _grad_ws_bytes(self, P):
-        if P < 1:
-            return 0
-        pr = _lib.Particles.from_buffer_copy(self.pr)
-        pr.P = int(P)
-        if self.estimator == "score":
-            return int(lib.pilco_particles_consistent_score_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
-                                                                                self._nz_ref(), self.R))
-        if self.ex is not None:
-            return int(lib.pilco_particles_explore_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
-                                                                                   self._nz_ref(), C.byref(self.ex),
-                                                                                   self.R))
-        if self.nz is not None:
-            return int(lib.pilco_particles_noisy_consistent_grad_workspace_bytes(C.byref(pr), self._ang_ref(),
-                                                                                C.byref(self.nz), self.R))
-        if self.ang is not None:
-            return int(lib.pilco_particles_angles_consistent_grad_workspace_bytes(C.byref(pr), C.byref(self.ang), self.R))
-        return int(lib.pilco_particles_consistent_grad_workspace_bytes(C.byref(pr), self.R))
-
     def launch(self):
         raise RuntimeError("ConsistentGradPlan: the rollout runs with its gradient, launch_grad()")
 
@@ -1022,30 +950,7 @@ class ConsistentGradPlan(ParticlePlan):
         of value = mean return (with ``exploration``: the exploration objective, and sigma_t^2 in ``step_var``),
         returned as ``ParticlePlan.launch_grad`` returns it.  ``estimator="score"``: the score-function gradient
         (pilco_particles_consistent_score_grad_rollout) in the same layout"""
-        if self.estimator == "score":
-            check(lib.pilco_particles_consistent_score_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
-                                                                    self.R, C.byref(self.grad), stream_ptr()),
-                  "particles_consistent_score_grad_rollout")
-            return self.gbuf
-        if self.ex is not None:
-            check(lib.pilco_particles_explore_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), self._nz_ref(),
-                                                                      C.byref(self.ex), self.R, C.byref(self.grad),
-                                                                      stream_ptr()),
-                  "particles_explore_consistent_grad_rollout")
-            return self.gbuf
-        if self.nz is not None:
-            check(lib.pilco_particles_noisy_consistent_grad_rollout(C.byref(self.pr), self._ang_ref(), C.byref(self.nz),
-                                                                    self.R, C.byref(self.grad), stream_ptr()),
-                  "particles_noisy_consistent_grad_rollout")
-            return self.gbuf
-        if self.ang is not None:
-            check(lib.pilco_particles_angles_consistent_grad_rollout(C.byref(self.pr), C.byref(self.ang), self.R,
-                                                                     C.byref(self.grad), stream_ptr()),
-                  "particles_angles_consistent_grad_rollout")
-            return self.gbuf
-        check(lib.pilco_particles_rollout_consistent_grad(C.byref(self.pr), self.R, C.byref(self.grad), stream_ptr()),
-              "particles_rollout_consistent_grad")
-        return self.gbuf
+        return super().launch_grad()
 
 
 def _largest_fitting(fits, lo, hi):
@@ -1185,9 +1090,8 @@ def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):
     pr.dyn = dyn.struct()
     pr.pol.Ds, pr.pol.U = int(Ds), int(U)
     ang = angles_struct(angles, int(pr.dyn.E))
-    if ang is not None:
-        return int(lib.pilco_particles_angles_consistent_workspace_bytes(C.byref(pr), C.byref(ang)))
-    return int(lib.pilco_particles_consistent_workspace_bytes(C.byref(pr)))
+    return int(lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), C.byref(ang) if ang is not None else None,
+                                                                    None))
 
 
 def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None,
