@@ -680,6 +680,35 @@ int    pilco_particles_consistent_score_grad_rollout(const pilco_particles* pr, 
 int    pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,
                                       double* step_var, pilco_stream_t stream);
 
+/* Gaussian-resampled particle rollouts (Deep PILCO's refit; DESIGN.md section 26), step-wise sampler.  At every step
+ * t >= 1 each restart's particles are refitted to a Gaussian and redrawn from it (no refit at t = 0):
+ *   x'_pt = x_{p,t-1} + mu(x~_{p,t-1}) + sqrt(max(var, 0)) o eps_{p,t-1}     (pilco_particles_rollout's step)
+ *   mu^_t = (1/P) sum_p x'_pt,  S^_t = 1/(P-1) sum_p (x'_pt - mu^_t)(x'_pt - mu^_t)'   (over the restart's particles)
+ *   L^_t  = chol(S^_t) column by column; a column j whose pivot d_j <= 1e-12 S^_t,jj (or S^_t,jj <= 0) is zeroed
+ *   x_pt  = mu^_t + L^_t xi_{p,t-1}
+ * traj[:, t] holds x_t, at which the rewards, the policy and x~_t are evaluated as pilco_particles_rollout evaluates
+ * them.  xi [P,H,Ds] are standard normals shared by the restarts.  step_mean [R,H+1,Ds] and step_cov [R,H+1,Ds,Ds]
+ * receive mu^_t and S^_t (t = 0: the moments of x0), each skipped when NULL.  A restart's results do not depend on R.
+ * pilco_particles_resampled_rollout: pilco_particles_rollout's description, outputs and contract (unbatched policy,
+ * pr->ws).  pilco_particles_resampled_grad_rollout: pilco_particles_rollout_batch_grad's contract (R policies, shared
+ * x0, eps and xi, g->ws) with the pathwise gradient of value = mean return through the refit, x0, eps and xi held
+ * fixed (away from degenerate pivots a smooth function of the policy parameters).  At H <= 1 value and gradient are
+ * bitwise the call without resampling.  Validation is the call without resampling's, then PILCO_ERR_NULL for rs NULL
+ * or xi NULL with H > 0, then PILCO_ERR_DIM for P < 2, then the workspace; a size query returns 0 exactly where its
+ * call fails on sizes.  The workspace is the call without resampling's followed by O(H R P Ds + H R Ds^2). */
+typedef struct pilco_particles_resample {
+    const double* xi;           /* [P,H,Ds] standard normals of the redraw */
+    double* step_mean;          /* [R,H+1,Ds] or NULL */
+    double* step_cov;           /* [R,H+1,Ds,Ds] or NULL */
+} pilco_particles_resample;
+size_t pilco_particles_resampled_workspace_bytes(const pilco_particles* pr, const pilco_particles_resample* rs);
+int    pilco_particles_resampled_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                         pilco_stream_t stream);
+size_t pilco_particles_resampled_grad_workspace_bytes(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                      int R);
+int    pilco_particles_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs, int R,
+                                              const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -90,6 +90,11 @@ class ParticlesNoise(C.Structure):
     _fields_ = [("v", ObsNoise), ("nu", c_dp)]
 
 
+class ParticlesResample(C.Structure):
+    """mirror of ``pilco_particles_resample``"""
+    _fields_ = [("xi", c_dp), ("step_mean", c_dp), ("step_cov", c_dp)]
+
+
 POLICY_LINEAR, POLICY_RBF = 0, 1
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -214,6 +219,12 @@ SIGNATURES = {
                                                                          C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_consistent_score_grad_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
     "pilco_particles_consistent_score_grad_rollout": (C.c_int, _PAN + [C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_resampled_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(ParticlesResample)]),
+    "pilco_particles_resampled_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample), c_dp]),
+    "pilco_particles_resampled_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(ParticlesResample),
+                                                                    C.c_int]),
+    "pilco_particles_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample), C.c_int,
+                                                         C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

@@ -30,6 +30,9 @@
 // The exploration objective (pilco_particles_explore_*, DESIGN.md section 24): pt_call launches the kernels of
 // particles_explore.cu beside the others (the moments after the forward, the bonus's share before each reverse step
 // kernel, the bonus into value after the reduction).
+// Gaussian-resampled particles (pilco_particles_resampled_*, DESIGN.md section 26): pt_forward launches
+// pr_step_launch's kernels (particles_resample.cu) in place of pt_step<t> for t >= 1, and pg_reverse the refit's reverse
+// stage after the step kernel of each t = H-1 .. 1.
 // The score-function gradient over consistent function samples (pilco_particles_consistent_score_grad_*, DESIGN.md
 // section 25): ps_run on the consistent forward; pc_white_kernel (particles_cscore.cu) turns the weights into the
 // cotangents of every step's mean' and var', which the reverse of the conditioning and the predict VJP carry to
@@ -758,6 +761,7 @@ struct PtOpt {
     bool consistent;            // one posterior function per particle (DESIGN.md section 14), else step-wise draws
     PtCall call;
     bool batched;               // the policy's batch strides are honoured; otherwise a batched policy is unsupported
+    bool resampled;             // the Gaussian refit at every step (DESIGN.md section 26; step-wise sampler only)
     int R;
     bool mapped;                // angles or noise: tm is the angles' map (the identity without angles)
     TrigMap tm;
@@ -766,6 +770,7 @@ struct PtOpt {
     bool explore, bonus;        // exploration (section 24): the moments; bonus (b != 0): its share and its value
     double b;
     double* step_var;
+    pilco_particles_resample rs;
 };
 
 // Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
@@ -781,6 +786,8 @@ struct PtWs {
     size_t sd, tab;                                     // exploration: sigma_t [R,H]; the bonus table [R,H,K,2]
     size_t togo, gsum, mw, vw, gxh;                     // score: G [H-1,T]; the sums [R,H]; m_bar, v_bar [H-1,T,E];
                                                         // the x~_bar history [H-1 or H,T,D]
+    size_t xp, rmu, rL, rsc;                            // resampled: x' [H,T,Ds], mu^ [H,R,Ds], L^ [H,R,Ds,Ds]; the
+                                                        // reverse scratch [R,Ds+Ds Ds]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -821,6 +828,8 @@ static int ps_group(long long T, int H) {
 //     largest VJP group; 0 also where the per-(step, particle) grids would pass 2^31 - 1 CTAs
 // then, gradients only: the phi history [T,H+1,Dh] (angles or noise); the phi(z) history [T,H+1,Dh] and (pathwise)
 // phi_bar_z [T,Dh] (noise); sigma_t [R,H] and the bonus table [R,H,K,2] (exploration, K = n_rewards).
+// Resampled (DESIGN.md section 26), after every other slot: the x' history [H,T,Ds], mu^ [H,R,Ds], L^ [H,R,Ds,Ds] and,
+// gradients only, the reverse scratch [R,Ds+Ds Ds].
 static PtWs pt_ws_layout(const pilco_particles* pr, const PtOpt& o) {
     const bool grad = o.call != PT_FORWARD, score = o.call == PT_SCORE;
     const size_t R = o.R, T = R * pr->P, H = pr->H, Hm = H > 0 ? H - 1 : 0, Hx = grad ? H : 1;
@@ -848,6 +857,10 @@ static PtWs pt_ws_layout(const pilco_particles* pr, const PtOpt& o) {
     if (grad && o.mapped) L.phi = take({T, H + 1, Dh});
     if (grad && o.noisy) { L.phiz = take({T, H + 1, Dh}); if (!score) L.phibz = take({T, Dh}); }
     if (o.explore) { L.sd = take({R, H}); L.tab = take({R, H, (size_t)pr->n_rewards, 2}); }
+    if (o.resampled) {
+        L.xp = take({H, T, Ds}); L.rmu = take({H, R, Ds}); L.rL = take({H, R, Ds, Ds});
+        if (grad) L.rsc = take({R, Ds + Ds * Ds});
+    }
     const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
     L.total = L.pws_bytes && (!score || nb * H <= 0x7fffffff) ? take.bytes() : 0;
     return L;
@@ -1023,7 +1036,8 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 // pn_step_kernel in place of pa_step_kernel, which with history also keeps phi(z_t) in L.phiz.  The state width is
 // dyn.E throughout (pol.Ds without angles).
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
-                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr) {
+                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
+                      const pilco_particles_resample* rs = nullptr) {
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
@@ -1044,11 +1058,18 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     c.eps = pr->eps; c.L = ws + L.L; c.mean = ws + L.mean;
     const bool joint = pt_has_joint(pr);
     PjDev j = pj_dev(pr, R);
+    PrFwd f;
+    if (rs) {
+        f.P = P; f.H = H; f.Ds = Ds; f.x0 = pr->x0; f.xi = rs->xi;
+        f.xp = ws + L.xp; f.mu = ws + L.rmu; f.L = ws + L.rL; f.step_mean = rs->step_mean; f.step_cov = rs->step_cov;
+    }
     for (int t = 0; t <= H; ++t) {
         a.t = t;
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
         a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
-        if (nz) {
+        if (rs && t > 0) {
+            if (const int rc = pr_step_launch(st, grid, a, f)) return rc;
+        } else if (nz) {
             static_cast<PtDev&>(pa) = a;
             static_cast<PaStep&>(pn) = pa;
             if (const int rc = pn_step_launch(st, grid, pn)) return rc;
@@ -1058,6 +1079,8 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
         } else {
             launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
             CUDA_LAUNCH_CHECK();
+            if (rs)                                     // t = 0: the moments of x0
+                if (const int rc = pr_step_launch(st, grid, a, f)) return rc;
         }
         if (t == H) break;
         if (joint) {
@@ -1124,8 +1147,11 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // bonus (exploration, b != 0): px_bonus_kernel after each step's VJP (and pj_grad) adds the bonus's share to x_bar_{t+1}
 // and x~_bar_t, which the step kernel then carries into x_bar_t; the sweep starts as with joint terms (x_bar_H = 0 and
 // x~_bar_{H-1} = 0 passed to the step kernel, which ignores x_bar when x~_bar is NULL).
+// rs (resampled): after the step kernel of each t = H-1 .. 1, pr_reverse_launch turns x_bar_t (the cotangent of the
+// refitted particles) into that of x'_t and rewrites var_bar_{t-1}.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
-                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false) {
+                      cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false,
+                      const pilco_particles_resample* rs = nullptr) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1194,6 +1220,13 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
         } else {
             launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
             CUDA_LAUNCH_CHECK();
+        }
+        if (rs && t > 0) {
+            PrBwd q;
+            q.P = P; q.H = H; q.Ds = Ds; q.t = t; q.xi = rs->xi; q.eps = pr->eps;
+            q.xp = ws + L.xp; q.mu = ws + L.rmu; q.L = ws + L.rL; q.var_prev = b.var_prev;
+            q.gx = b.gx; q.gvar = b.gvar; q.sc = ws + L.rsc;
+            if (const int rc = pr_reverse_launch(st, grid, q)) return rc;
         }
     }
     return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj);
@@ -1341,8 +1374,11 @@ static int px_check(const pilco_particles* pr, const pilco_exploration* ex) {
 // (the policy's batch strides as o->batched allows), R, the gradient's outputs, the noise, the exploration (active
 // only).  Each family's call is the most general call with NULL for the features it lacks, so ang == NULL or A == 0
 // is the call without angles, nz == NULL the call without noise and an inactive ex the call without exploration.
+// Resampled calls (o->resampled, no angles, noise or exploration), after the gradient's outputs: PILCO_ERR_NULL for rs
+// NULL or xi NULL with H > 0, then PILCO_ERR_DIM for P < 2 (no sample covariance).
 static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                       const pilco_exploration* ex, int R, const pilco_particles_grad* g) {
+                       const pilco_exploration* ex, int R, const pilco_particles_grad* g,
+                       const pilco_particles_resample* rs = nullptr) {
     if (!pr) return PILCO_ERR_NULL;
     const bool angles = !pa_none(ang);
     if (angles)
@@ -1351,6 +1387,11 @@ static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* 
     if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;   // the unbatched calls' R = 1 passes with the description
     if (o->call != PT_FORWARD)
         if (const int rc = pg_check(pr, g)) return rc;
+    if (o->resampled) {
+        if (!rs || (!rs->xi && pr->H > 0)) return PILCO_ERR_NULL;
+        if (pr->P < 2) return PILCO_ERR_DIM;
+        o->rs = *rs;
+    }
     if (!angles) trig_map_make(pr->dyn.E, 0, nullptr, &o->tm);     // 1 <= E <= PILCO_MAX_E once the description passed
     if (nz)
         if (const int rc = pn_noise(pr, nz, &o->nz)) return rc;
@@ -1373,6 +1414,7 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
     if (nz && (pr->dyn.E < 1 || pr->dyn.E > MAXE || pn_noise(pr, nz, &o.nz))) return 0;
     o.explore = px_active(ex);
     if (o.explore && px_check(pr, ex)) return 0;
+    if (o.resampled && pr->P < 2) return 0;
     o.R = R; o.mapped = nz || !pa_none(ang); o.noisy = nz != nullptr;
     return (o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o)).total;
 }
@@ -1381,8 +1423,9 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
 // the forward (with its history for a gradient) and the gradient's reverse part.  Pathwise with exploration: the
 // moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
 static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                   const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream) {
-    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g)) return rc;
+                   const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream,
+                   const pilco_particles_resample* rs = nullptr) {
+    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs)) return rc;
     const bool fwd = o.call == PT_FORWARD;
     const PtWs L = o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
     if (const int rc = fwd ? pt_check_ws(pr->ws, pr->ws_bytes, L.total) : pt_check_ws(g->ws, g->ws_bytes, L.total))
@@ -1396,7 +1439,8 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
     double* ws = (double*)(fwd ? pr->ws : g->ws);
     const TrigMap* tm = o.mapped ? &o.tm : nullptr;
     const PnNoise* n = o.noisy ? &o.nz : nullptr;
-    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n)) return rc;
+    const pilco_particles_resample* rsv = o.resampled ? &o.rs : nullptr;
+    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv)) return rc;
     if (fwd) return PILCO_OK;
     if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
     if (o.explore) {
@@ -1404,7 +1448,7 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
         m.step_var = o.step_var; m.sd = ws + L.sd; m.tab = o.bonus ? ws + L.tab : nullptr;
         if (const int rc = px_moments_launch(st, R, m)) return rc;
     }
-    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus)) return rc;
+    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv)) return rc;
     if (o.bonus && pr->H > 0) return px_value_launch(st, R, pr->H, o.b, ws + L.sd, g->value);
     return PILCO_OK;
 }
@@ -1413,6 +1457,7 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
 static const PtOpt FWD = {false, PT_FORWARD, false}, CFWD = {true, PT_FORWARD, false};
 static const PtOpt PATH1 = {false, PT_PATHWISE, false}, PATH = {false, PT_PATHWISE, true};
 static const PtOpt CPATH = {true, PT_PATHWISE, true}, SCORE = {false, PT_SCORE, true}, CSCORE = {true, PT_SCORE, true};
+static const PtOpt RFWD = {false, PT_FORWARD, false, true}, RPATH = {false, PT_PATHWISE, true, true};
 
 extern "C" {
 
@@ -1598,6 +1643,27 @@ int pilco_particles_consistent_score_grad_rollout(const pilco_particles* pr, con
                                                   const pilco_particles_noise* nz, int R,
                                                   const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(CSCORE, pr, ang, nz, nullptr, R, g, stream);
+}
+
+size_t pilco_particles_resampled_workspace_bytes(const pilco_particles* pr, const pilco_particles_resample* rs) {
+    (void)rs;                                           // the sizes do not depend on it
+    return pt_query(RFWD, pr, nullptr, nullptr, nullptr, 1);
+}
+
+int pilco_particles_resampled_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                      pilco_stream_t stream) {
+    return pt_call(RFWD, pr, nullptr, nullptr, nullptr, 1, nullptr, stream, rs);
+}
+
+size_t pilco_particles_resampled_grad_workspace_bytes(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                      int R) {
+    (void)rs;
+    return pt_query(RPATH, pr, nullptr, nullptr, nullptr, R);
+}
+
+int pilco_particles_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs, int R,
+                                           const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(RPATH, pr, nullptr, nullptr, nullptr, R, g, stream, rs);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,

@@ -1,7 +1,7 @@
 // particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu,
-// particles_explore.cu and particles_cscore.cu share: the per-particle argument structs, the reward value at a point, the
-// fixed-order block sum, and the angle, noise, exploration and consistent-score kernels' launchers (DESIGN.md sections
-// 11, 12, 20, 23, 24 and 25).
+// particles_explore.cu, particles_cscore.cu and particles_resample.cu share: the per-particle argument structs, the
+// reward value at a point, the step's work at a given state, the fixed-order block sum, and the angle, noise,
+// exploration, consistent-score and resampling kernels' launchers (DESIGN.md sections 11, 12, 20, 23, 24, 25 and 26).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -57,6 +57,74 @@ __device__ __forceinline__ double pt_reward_value(const pilco_reward_term& rt, c
         }
     }
     return exp(-0.5 * quad);
+}
+
+// pt_step_kernel's work at step t once particle row's state x_t is known (restart r, tr = its traj[:, t] row; DESIGN.md
+// section 11): traj[:, t], and for t < H the state terms' reward and risk at x_t, x~_t and the squashed action; at
+// t = H the return.  pr_step_kernel (particles_resample.cu) runs it on x_t from the Gaussian refit.  It is a copy of
+// pt_step_kernel's code in the same order, kept apart: routing pt_step_kernel through it changes that kernel's register
+// allocation, and pt_step_kernel's SASS is pinned.  Keep the two in step.
+__device__ __forceinline__ void pt_step_at(const PtDev& a, int r, size_t row, double* tr, const double (&x)[MAXD]) {
+    const int Ds = a.Ds, U = a.U, D = Ds + U, t = a.t, H = a.H;
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) if (d < Ds) tr[d] = x[d];
+    const size_t ph = row * H;
+    if (t == H) {                                       // return: step order, as ro_reward_sum_kernel
+        double s = 0.0;
+        for (int tt = 0; tt < H; ++tt) s += a.step_reward[ph + tt];
+        if (a.n_mult > 0) {
+            double mult = 1.0;
+            for (int tt = 0; tt < H; ++tt) mult *= 1.0 - a.step_risk[ph + tt];
+            s += a.mult_mu * (1.0 - mult);
+        }
+        a.ret[row] = s;
+        return;
+    }
+    double rew = 0.0, risk = 0.0;                       // at the pre-step state (pilco.py:130-134)
+    for (int k = 0; k < a.n_rewards; ++k) {
+        const pilco_reward_term& rt = a.rewards[k];
+        const double v = pt_reward_value(rt, x, tr, Ds);
+        if (rt.channel == PILCO_CHANNEL_MULT) risk = fma(rt.coef, v, risk);
+        else rew = fma(rt.coef, v, rew);
+    }
+    a.step_reward[ph + t] = rew;
+    a.step_risk[ph + t] = risk;
+    double* xo = a.xt + row * D;
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) if (d < Ds) xo[d] = x[d];
+    double* ao = a.act + (ph + t) * U;
+    // squash_sin at a point with the policy's output variance su: maxa exp(-su/2) sin(u)  (dev_squash_sin's form).
+    // sin(u) as sinpi(u / pi): its argument reduction is exact, so the kernel carries no Payne-Hanek slow path (whose
+    // table lives in local memory); the rounding of u / pi moves the angle by |u| 1.1e-16 at most.
+    const double su = a.pol_kind == PILCO_POLICY_RBF ? PT_RBF_VAR : 0.0;
+    for (int j = 0; j < U; ++j) {
+        double u;
+        if (a.pol_kind == PILCO_POLICY_LINEAR) {        // dev_linear_action's order
+            const double* W = a.W + r * a.W_bs;
+            u = a.b[r * a.b_bs + j];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) if (d < Ds) u = fma(W[j * Ds + d], x[d], u);
+        } else {                                        // sum_i beta_ji sf2_j exp(-0.5 |(x - c_i) / ell_j|^2)
+            const double* ell = a.ell + r * a.ell_bs;
+            double il[MAXD];
+#pragma unroll
+            for (int d = 0; d < MAXD; ++d) il[d] = d < Ds ? 1.0 / ell[j * Ds + d] : 0.0;
+            const double sf2 = a.sf2[r * a.sf2_bs + j];
+            const double* be = a.beta + r * a.beta_bs + (size_t)j * a.bf;
+            const double* C = a.C + r * a.C_bs;
+            u = 0.0;
+            for (int i = 0; i < a.bf; ++i) {
+                const double* c = C + (size_t)i * Ds;
+                double d2 = 0.0;
+#pragma unroll
+                for (int d = 0; d < MAXD; ++d) if (d < Ds) { const double q = (x[d] - c[d]) * il[d]; d2 = fma(q, q, d2); }
+                u = fma(sf2 * exp(-0.5 * d2), be[i], u);
+            }
+        }
+        if (a.squash) u = a.maxa[j] * exp(-0.5 * su) * sinpi(u * PT_INV_PI);
+        ao[j] = u;
+        xo[Ds + j] = u;
+    }
 }
 
 // fixed-order block sum of NV values per thread (256 threads): warp butterflies, then warps in order -> out[0..NV)
@@ -180,3 +248,34 @@ struct PcWhite {
 
 // grid (ceil(P / 8), E, R), 256 threads; H < 2 launches nothing
 int pc_white_launch(cudaStream_t st, int R, const PcWhite& a);
+
+// ---- Gaussian-resampled particles (particles_resample.cu, DESIGN.md section 26) ----------------------------------------
+// At every step t >= 1 restart r's pre-fit particles x'_t (the step closure) are refitted to a Gaussian and redrawn:
+// x_pt = mu^_t + L^_t xi_{p,t-1}, mu^_t and S^_t = L^_t L^_t' the sample mean and unbiased covariance of x'_t over the
+// restart's P particles (pr_chol's degenerate-column rule).  The step-wise sampler only: Ds = E (no angles).
+struct PrFwd {
+    int P, H, Ds;
+    const double* x0; const double* xi;                 // [P,Ds], [P,H,Ds]: shared by the restarts
+    double* xp;                                         // x'_t at slot t-1 of [H,T,Ds]
+    double* mu; double* L;                              // mu^_t, L^_t at slot t-1 of [H,R,Ds], [H,R,Ds,Ds]
+    double* step_mean; double* step_cov;                // [R,H+1,Ds], [R,H+1,Ds,Ds] (t = 0: x0's moments), or NULL
+};
+
+// step a.t of the resampled forward, in place of the step kernel: t = 0 (after pt_step<0>) x0's moments when they are
+// asked for; t >= 1 the closure into x'_t, the moments and factor (grid R) and pr_step_kernel, which redraws x_t and
+// does pt_step_kernel's work at it.  grid = (ceil(P / 128), R).
+int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f);
+
+// the refit's reverse at step t (1 <= t <= H-1), after the reverse step kernel has left y_bar_p = the cotangent of the
+// refitted x_pt in gx: gx <- the cotangent of x'_pt, gvar <- that of var_{t-1}
+struct PrBwd {
+    int P, H, Ds, t;
+    const double* xi; const double* eps;                // [P,H,Ds]
+    const double* xp; const double* mu; const double* L;   // the forward's histories
+    const double* var_prev;                             // var_{t-1} [T,Ds]
+    double* gx; double* gvar;                           // [T,Ds]
+    double* sc;                                         // [R,Ds+Ds Ds]: mu_bar / P and (A + A') / (P-1)
+};
+
+// grid = (ceil(P / 128), R): pr_adjoint_kernel (grid R), then pr_scatter_kernel
+int pr_reverse_launch(cudaStream_t st, dim3 grid, const PrBwd& b);

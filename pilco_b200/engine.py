@@ -696,6 +696,8 @@ PARTICLE_CALLS = {
     (True, "pathwise"): ("explore_consistent_grad_rollout", "explore_consistent_grad_workspace_bytes"),
     (False, "score"): ("noisy_score_grad_rollout", "noisy_score_grad_workspace_bytes"),
     (True, "score"): ("consistent_score_grad_rollout", "consistent_score_grad_workspace_bytes"),
+    ("resampled", "forward"): ("resampled_rollout", "resampled_workspace_bytes"),
+    ("resampled", "pathwise"): ("resampled_grad_rollout", "resampled_grad_workspace_bytes"),
 }
 
 
@@ -735,14 +737,26 @@ class ParticlePlan:
     pathwise gradient.  The plan then owns ``step_var`` [R, max(H,1)], which each ``launch_grad()`` fills with
     sigma_t^2.  At b = 0 every other output and gradient is bitwise the plan's without exploration.  It needs
     ``grad=True``, P >= 2 and no additive box term; ``estimator="score"`` with it is a ValueError.  ``None``: no
-    exploration."""
+    exploration.
+
+    ``resample=True``: Deep PILCO's Gaussian refit (pilco_particles_resampled_*, DESIGN.md section 26).  At every step
+    t >= 1 each restart's particles are replaced by draws mu^_t + L^_t xi_t from the Gaussian fitted to them (sample
+    mean and unbiased covariance, L^_t its Cholesky factor with degenerate columns zeroed), and the rewards and the
+    policy are evaluated at the redrawn particles.  The plan then owns ``xi`` [P,H,Ds] (standard normals shared by the
+    R policies, which ``set_inputs`` fills: its ``xi`` is then required), ``step_mean`` [R?,H+1,Ds] and ``step_cov``
+    [R?,H+1,Ds,Ds] (the fitted moments; t = 0: those of x0), which every launch fills.  ``launch_grad()`` gives the
+    pathwise gradient through the refit.  It needs P >= 2; with ``consistent``, ``estimator="score"``, ``angles``,
+    ``measurement_noise`` or ``exploration`` it is a ValueError raised before any allocation."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
-                 estimator="pathwise", angles=None, measurement_noise=None, exploration=None):
+                 estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False):
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
+        self.resample = bool(resample)
+        if self.resample:
+            _resample_check(P, consistent, estimator, angles, measurement_noise, exploration)
         if exploration is not None and (estimator == "score" or not grad):
             raise ValueError("particles: exploration is an objective of the pathwise gradient: it needs grad=True and "
                              "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
@@ -767,15 +781,21 @@ class ParticlePlan:
         if grad:
             self._grad_buffers(self._grad_ws_bytes(P))
 
+    def _sampler(self):
+        return "resampled" if self.resample else self.consistent
+
     def _args(self, kind, pr):
-        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise) and R"""
+        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise) and R; resampled:
+        pr, the refit's buffers and R"""
+        if self.resample:
+            return [C.byref(pr), C.byref(self.rs)] + ([self.R] if kind != "forward" else [])
         args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
         if kind == "pathwise":
             args.append(C.byref(self.ex) if self.ex is not None else None)
         return args + ([self.R] if kind != "forward" else [])
 
     def _query(self, kind, pr):
-        return int(getattr(lib, "pilco_particles_" + PARTICLE_CALLS[self.consistent, kind][1])(*self._args(kind, pr)))
+        return int(getattr(lib, "pilco_particles_" + PARTICLE_CALLS[self._sampler(), kind][1])(*self._args(kind, pr)))
 
     def _grad_ws_bytes(self, P):
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
@@ -842,6 +862,13 @@ class ParticlePlan:
         if b is not None:                                       # sigma_t^2 [R, max(H,1)], also for an unbatched plan
             self.step_var = mk(R, Hb)
             self.ex = _lib.Exploration(b, self.step_var.data_ptr())
+        if self.resample:                                       # xi shared by the R policies; the fitted moments
+            self.xi_buf = mk(P, Hb, Ds)
+            self._step_mean, self._step_cov = mk(R, H + 1, Ds), mk(R, H + 1, Ds, Ds)
+            self.step_mean = self._step_mean.view(*lead, H + 1, Ds)
+            self.step_cov = self._step_cov.view(*lead, H + 1, Ds, Ds)
+            self.rs = _lib.ParticlesResample(self.xi_buf.data_ptr(), self._step_mean.data_ptr(),
+                                             self._step_cov.data_ptr())
 
     def _ang_ref(self):
         return C.byref(self.ang) if self.ang is not None else None
@@ -875,18 +902,23 @@ class ParticlePlan:
         return self.gbuf
 
     def _call(self, kind, *grad):
-        name = "particles_" + PARTICLE_CALLS[self.consistent, kind][0]
+        name = "particles_" + PARTICLE_CALLS[self._sampler(), kind][0]
         check(getattr(lib, "pilco_" + name)(*self._args(kind, self.pr), *grad, stream_ptr()), name)
 
-    def set_inputs(self, x0, eps, nu=None):
-        """x0 [P,Ds], eps [P,H,Ds] and, with measurement noise, nu [P,H,E] (required then, and only then)"""
+    def set_inputs(self, x0, eps, nu=None, xi=None):
+        """x0 [P,Ds], eps [P,H,Ds], with measurement noise nu [P,H,E] and with ``resample`` xi [P,H,Ds] (each required
+        then, and only then)"""
         if (nu is None) != (self.nz is None):
             raise ValueError("particles: nu [P,H,E] is required with measurement_noise and only then")
+        if (xi is None) == self.resample:
+            raise ValueError("particles: xi [P,H,Ds] is required with resample=True and only then")
         self.x0.copy_(dev(x0).reshape(self.P, self.Ds))
         if self.H > 0:
             self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
             if nu is not None:
                 self.nu_buf.copy_(dev(nu).reshape(self.nu_buf.shape))
+            if xi is not None:
+                self.xi_buf.copy_(dev(xi).reshape(self.P, self.H, self.Ds))
 
     def launch(self):
         if self.batched:
@@ -928,7 +960,7 @@ class ConsistentGradPlan(ParticlePlan):
             raise ValueError("particles: exploration is an objective of the pathwise gradient: it needs "
                              "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
         self.estimator = estimator
-        self.consistent = True
+        self.consistent, self.resample = True, False
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
@@ -1006,6 +1038,19 @@ def _particle_exploration(exploration, reward_terms, P):
     return b
 
 
+def _resample_check(P, consistent, estimator, angles, measurement_noise, exploration):
+    """the Gaussian refit's refusals (ValueError), before any allocation: it runs on the step-wise sampler with the
+    pathwise gradient only, without angles, measurement noise or exploration, and needs P >= 2"""
+    for on, what in ((consistent, "consistent=True (redrawing breaks a particle's identity with its function)"),
+                     (estimator == "score", "estimator='score' (the path density no longer factorises per particle)"),
+                     (angles is not None and len(angles) > 0, "angles"),
+                     (measurement_noise is not None, "measurement_noise"), (exploration is not None, "exploration")):
+        if on:
+            raise ValueError("particles: resample=True does not combine with %s" % what)
+    if int(P) < 2:
+        raise ValueError("particles: resample=True fits a covariance to the particles: it needs P >= 2, got %d" % int(P))
+
+
 def _no_additive_box(reward_terms):
     for k, rt in enumerate(reward_terms):
         if rt["kind"] == _lib.REWARD_BOX and int(rt.get("channel", _lib.CHANNEL_ADD)) == _lib.CHANNEL_ADD:
@@ -1048,7 +1093,7 @@ def particle_reward_moments(reward_terms, traj, act, angles=None):
 
 
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,
-                      angles=None, measurement_noise=None, nu=None):
+                      angles=None, measurement_noise=None, nu=None, resample=False, xi=None):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
     step_risk [P,H], ret [P]) device tensors.
@@ -1061,7 +1106,15 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     policy takes E + len(angles) inputs.
 
     ``measurement_noise``: variances v [E] of the policy's measurement z = x + sqrt(v) o nu, as ``ParticlePlan``; ``nu``
-    [P,H,E] are its standard normals (required with it, for both samplers)."""
+    [P,H,E] are its standard normals (required with it, for both samplers).
+
+    ``resample=True``: the Gaussian refit at every step, as ``ParticlePlan(resample=True)``; ``xi`` [P,H,Ds] are the
+    redraw's standard normals (required with it, and only then).  The result then also has the fitted moments:
+    (traj, act, step_reward, step_risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds])."""
+    if resample:
+        _resample_check(x0.shape[0], consistent, "pathwise", angles, measurement_noise, None)
+    if (xi is None) == bool(resample):
+        raise ValueError("particles_rollout: xi [P,H,Ds] is required with resample=True and only then")
     x0, eps = dev(x0), dev(eps)
     if x0.dim() != 2 or eps.dim() != 3 or eps.shape[0] != x0.shape[0] or eps.shape[2] != x0.shape[1]:
         raise ValueError("particles_rollout: x0 must be [P,Ds] and eps [P,H,Ds], got %s and %s"
@@ -1075,11 +1128,15 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     if consistent:
         return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles,
                                              measurement_noise, nu)
+    if resample:
+        xi = dev(xi)
+        if tuple(xi.shape) != tuple(eps.shape):
+            raise ValueError("particles_rollout: xi must be [P,H,Ds] like eps, got %s" % (tuple(xi.shape),))
     plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu, angles=angles,
-                        measurement_noise=measurement_noise)
-    plan.set_inputs(x0, eps, nu)
+                        measurement_noise=measurement_noise, resample=resample)
+    plan.set_inputs(x0, eps, nu, xi)
     plan.launch()
-    return plan.outputs()
+    return plan.outputs() + ((plan.step_mean, plan.step_cov) if resample else ())
 
 
 def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):

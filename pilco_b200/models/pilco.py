@@ -19,6 +19,16 @@ ParticleTrajectories = collections.namedtuple("ParticleTrajectories", ["states",
 ParticlePolicyGradient = collections.namedtuple("ParticlePolicyGradient", ["value", "grad", "returns"])
 
 
+def _resample_refusals(what, resample, consistent, estimator="pathwise", exploration=0.0):
+    """the Gaussian refit's refusals at the class level, as engine.ParticlePlan's (ValueError)"""
+    if not resample:
+        return
+    for on, why in ((consistent, "consistent=True"), (estimator == "score", "estimator='score'"),
+                    (float(exploration) != 0.0, "exploration")):
+        if on:
+            raise ValueError("%s: resample=True does not combine with %s" % (what, why))
+
+
 def _sqrt_factor(S):
     """F with F F' = S: the Cholesky factor, or for a positive semi-definite S (S = 0 included) the eigen-factor
     Q diag(sqrt(max(lambda, 0))).  ValueError when S has an eigenvalue below -1e-12 max|lambda|."""
@@ -239,7 +249,7 @@ class PILCO:
         M, S, _ = self.predict(m_x, s_x, 1)
         return M, S
 
-    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
+    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False):
         """Monte Carlo rollouts of the learnt dynamics under the policy, to check what ``predict``'s moment matching
         approximates: ``num_samples`` particles start at x0 ~ N(m_x, s_x) and take n steps of
         x_{t+1} = x_t + mu(x_t, u_t) + sqrt(var(x_t, u_t)) eps_t with the latent GP posterior mean and variance,
@@ -253,12 +263,18 @@ class PILCO:
         gives the same x0 and normals, so step 0 is the same in both.  Its device workspace grows as
         num_samples n^2 (and n times the model's centres); large batches run in chunks.
 
+        ``resample=True``: Deep PILCO's Gaussian refit (DESIGN.md section 26): at every step the particles are replaced
+        by draws from the Gaussian fitted to them (their sample mean and covariance), with standard normals drawn from
+        the same generator after the step normals, so a seed gives the same x0 and step normals with and without it.
+        It needs num_samples >= 2; with ``consistent=True`` it is a ValueError.
+
         -> ParticleTrajectories(states [S,n+1,Ds], actions [S,n,U], rewards [S,n], risks [S,n], returns [S]) of
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
         from ..params import HostArray
         self._no_angles("sample_trajectories")
         self._no_noise("sample_trajectories")
+        _resample_refusals("sample_trajectories", resample, consistent)
         if consistent:
             import torch
             dyn = self.mgpr.device_gp()
@@ -268,32 +284,34 @@ class PILCO:
             terms, mult_mu = self.reward_spec()
             out = engine.particles_rollout(dyn, self.policy_spec(), terms, x0, eps, mult_mu=mult_mu, consistent=True)
             return ParticleTrajectories(*[t.cpu().numpy().view(HostArray) for t in out])
-        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_trajectories")
+        plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_trajectories", resample=resample)
         plan.launch()
         out = [t.cpu().numpy().view(HostArray) for t in plan.outputs()]
         return ParticleTrajectories(*out)
 
     def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False, estimator="pathwise",
-                       exploration=None):
+                       exploration=None, resample=False):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
         (from ``np.random`` when None): the same seed gives the same particles to every caller.  ``consistent``
-        (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``, ``exploration``:
-        ParticlePlan's."""
+        (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``, ``exploration``,
+        ``resample``: ParticlePlan's (the redraw's normals come after the step normals)."""
         dyn = self.mgpr.device_gp()
-        x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, what)
+        inputs = self._particle_inputs(m_x, s_x, n, num_samples, seed, what, resample)
+        x0, eps, xi = inputs if resample else inputs + (None,)
         terms, mult_mu = self.reward_spec()
         if consistent:
             plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
                                              exploration=exploration)
         else:
             plan = engine.ParticlePlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
-                                       grad=grad, estimator=estimator, exploration=exploration)
-        plan.set_inputs(x0, eps)
+                                       grad=grad, estimator=estimator, exploration=exploration, resample=resample)
+        plan.set_inputs(x0, eps, xi=xi)
         return plan
 
-    def _particle_inputs(self, m_x, s_x, n, num_samples, seed, what):
+    def _particle_inputs(self, m_x, s_x, n, num_samples, seed, what, resample=False):
         """(x0 [S,Ds], eps [S,n,Ds]) device tensors of ``_particle_plan``: x0 = m + F eps0, then the step normals, from
-        one device generator seeded with ``seed`` (from ``np.random`` when None)."""
+        one device generator seeded with ``seed`` (from ``np.random`` when None); eps is None at n = 0.  ``resample``:
+        (x0, eps, xi), the redraw's normals xi [S,n,Ds] drawn after the step normals from the same generator."""
         import torch
         n, S = int(n), int(num_samples)
         if n < 0 or S < 1:
@@ -309,7 +327,11 @@ class PILCO:
         eps0 = torch.randn((S, Ds), dtype=engine.F64, device=d, generator=g)
         x0 = engine.dev(m)[None] + eps0 @ engine.dev(F).T
         eps = torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g) if n > 0 else None
-        return x0, eps
+        if not resample:
+            return x0, eps
+        xi = torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g) if n > 0 else \
+            torch.zeros((S, 0, Ds), dtype=engine.F64, device=d)
+        return x0, eps, xi
 
     def _flat_grad(self, g):
         """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
@@ -322,18 +344,20 @@ class PILCO:
         return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
                                g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
 
-    def sample_reward_moments(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False):
+    def sample_reward_moments(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False):
         """Sample mean and variance of each step's reward over the particles of ``sample_trajectories`` (the same seed
         gives the same particles): the sampled counterpart of ``predict_reward_moments``.  mean_t is the mean of the
         step rewards (``sample_trajectories(...).rewards.mean(0)`` up to rounding) and var_t = sum_k c_k^2 s_kt^2 over
         the additive terms, s_kt^2 the unbiased sample variance of term k at step t (covariances between terms ignored,
         as ``predict_reward_moments``; the multiplicative terms of SafePILCO do not enter; DESIGN.md section 24).
         ``consistent``: the particles of ``sample_trajectories(..., consistent=True)``; a chunked rollout gives the
-        statistics of all num_samples particles.  Needs num_samples >= 2; a reward with an additive box term is a
-        ValueError.  -> (mean [n], var [n]) host arrays."""
+        statistics of all num_samples particles.  ``resample``: the particles of ``sample_trajectories(...,
+        resample=True)``.  Needs num_samples >= 2; a reward with an additive box term is a ValueError.  -> (mean [n],
+        var [n]) host arrays."""
         from ..params import HostArray
         self._no_angles("sample_reward_moments")
         self._no_noise("sample_reward_moments")
+        _resample_refusals("sample_reward_moments", resample, consistent)
         if int(num_samples) < 2:
             raise ValueError("sample_reward_moments: the sample variance needs num_samples >= 2 (num_samples=%d)"
                              % int(num_samples))
@@ -347,14 +371,14 @@ class PILCO:
             out = engine.particles_rollout(self.mgpr.device_gp(), self.policy_spec(), terms, x0, eps, mult_mu=mult_mu,
                                            consistent=True)
         else:
-            plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_reward_moments")
+            plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_reward_moments", resample=resample)
             plan.launch()
             out = plan.outputs()
         mean, var = engine.particle_reward_moments(terms, out[0], out[1])
         return mean.cpu().numpy().view(HostArray), var.cpu().numpy().view(HostArray)
 
     def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, estimator="pathwise",
-                               exploration=0.0):
+                               exploration=0.0, resample=False):
         """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
         are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
         d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
@@ -376,6 +400,10 @@ class PILCO:
         for the sampled counterpart of ``optimize_policy``'s objective.  b != 0 needs num_samples >= 2, the pathwise
         estimator and no additive box term (ValueError otherwise); b = 0 is the call without it.
 
+        ``resample=True``: the particles of ``sample_trajectories(..., resample=True)`` and the pathwise gradient through
+        the Gaussian refit, its normals held fixed too (Deep PILCO's estimator, DESIGN.md section 26).  With
+        ``consistent=True``, ``estimator="score"`` or exploration b != 0 it is a ValueError.
+
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
         self._no_angles("sample_policy_gradient")
@@ -388,8 +416,10 @@ class PILCO:
                              "particles is engine.ConsistentGradPlan(..., estimator='score'); this method offers "
                              "estimator='pathwise' with them")
         b = float(exploration)
+        _resample_refusals("sample_policy_gradient", resample, consistent, estimator, b)
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
-                                   consistent=consistent, estimator=estimator, exploration=None if b == 0.0 else b)
+                                   consistent=consistent, estimator=estimator, exploration=None if b == 0.0 else b,
+                                   resample=resample)
         g = plan.launch_grad()
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
@@ -436,7 +466,7 @@ class PILCO:
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
     def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False,
-                                exploration=0.0):
+                                exploration=0.0, resample=False):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -457,7 +487,11 @@ class PILCO:
 
         ``exploration``: a weight b != 0 optimises PILCO's exploration objective over the particles, mean return +
         b sum_t sigma_t (``sample_policy_gradient``'s), and returns its in-sample value.  It does not read
-        ``self.exploration``: pass ``exploration=self.exploration`` for the sampled counterpart of ``optimize_policy``."""
+        ``self.exploration``: pass ``exploration=self.exploration`` for the sampled counterpart of ``optimize_policy``.
+
+        ``resample=True``: Deep PILCO's objective with its Gaussian refit at every step (``sample_policy_gradient(...,
+        resample=True)``); the refit's normals are drawn once with the others.  With ``consistent=True`` or exploration
+        b != 0 it is a ValueError."""
         from functools import partial
         from .. import policy_opt
         self._no_angles("optimize_policy_sampled")
@@ -465,6 +499,10 @@ class PILCO:
         if int(num_samples) < 1:
             raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
         b = float(exploration)
+        _resample_refusals("optimize_policy_sampled", resample, consistent, "pathwise", b)
+        if resample and int(num_samples) < 2:
+            raise ValueError("optimize_policy_sampled: resample=True needs num_samples >= 2 (num_samples=%d)"
+                             % int(num_samples))
         if not np.isfinite(b) or (b != 0.0 and int(num_samples) < 2):
             raise ValueError("optimize_policy_sampled: exploration needs a finite b and num_samples >= 2 (b=%r, "
                              "num_samples=%d)" % (exploration, int(num_samples)))
@@ -478,12 +516,13 @@ class PILCO:
             set_trainable(p, False)
         try:
             flats0 = policy_opt.initial_flats(self.controller, restarts)
-            x0, eps = self._particle_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed,
-                                            "optimize_policy_sampled")
+            inputs = self._particle_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed,
+                                           "optimize_policy_sampled", resample)
+            x0, eps, xi = inputs if resample else inputs + (None,)
             best_flat, best_value, _ = policy_opt.optimize(
                 self, maxiter=maxiter, restarts=restarts, flats0=flats0,
                 evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent,
-                                  exploration=None if b == 0.0 else b))
+                                  exploration=None if b == 0.0 else b, resample=resample, xi=xi))
             self.controller.set_flat(best_flat)
         finally:
             for p in mgpr_trainable:

@@ -214,9 +214,11 @@ class ParticleEvaluator(_FlatEvaluator):
     ``engine.ConsistentGradPlan``).  Box terms carry no pathwise gradient, so a reward with them is rejected.
     ``exploration``: a float b makes the objective PILCO's exploration objective over the particles, mean return +
     b sum_t sigma_t with sigma_t the sample spread of step t's reward (pilco_particles_explore_*, DESIGN.md section 24);
-    None (the default) is the mean return."""
+    None (the default) is the mean return.  ``resample=True``: Deep PILCO's Gaussian refit at every step
+    (pilco_particles_resampled_grad_rollout, DESIGN.md section 26) with the redraw's standard normals ``xi`` [P,H,Ds],
+    held fixed like eps."""
 
-    def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None):
+    def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None):
         terms, mult_mu = pilco.reward_spec()
         if any(t["kind"] == _lib.REWARD_BOX for t in terms):
             raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
@@ -231,8 +233,9 @@ class ParticleEvaluator(_FlatEvaluator):
                                                   int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration)
         else:
             self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
-                                            mult_mu=mult_mu, grad=True, R=R, exploration=exploration)
-        self.plan.set_inputs(x0, eps)
+                                            mult_mu=mult_mu, grad=True, R=R, exploration=exploration,
+                                            resample=resample)
+        self.plan.set_inputs(x0, eps, xi=xi)
         self._setup_io()
 
     def _enqueue(self):
