@@ -32,7 +32,11 @@ static int launch_tile(const MMParams& p, cudaStream_t st) {
     if (rpc_env > 0) rpc = rpc_env;
     if (rpc > p.L.NB) rpc = p.L.NB;
     dim3 grid((p.L.NB + rpc - 1) / rpc, p.L.P, p.R);
-    const bool hi = pilco_small_grid(grid);          // e.g. the RBF policy's 3 pairs: glue, not bulk work
+    // High priority only for a launch of at most half the SMs' worth of CTAs (the RBF policy's few pairs: glue on the step's
+    // serial path).  A dynamics tile launch of a sub-batch (220 CTAs at the metric shape) is bulk work even though it fills
+    // the machine less than twice: at high priority its queued CTAs would keep the setup and glue kernels of the other
+    // sub-batches from the slots that free up, and their steps would stall behind it (DESIGN §6).
+    const bool hi = (long long)grid.x * grid.y * grid.z <= pilco_sm_count() / 2;
     if (variant == 4) launch_pri(hi, mm_tile_m16_kernel<KS>, grid, dim3(256), smem, st, p, rpc);
     else if (variant == 3) launch_pri(hi, mm_tile_kernel<KS, 3, true>, grid, dim3(256), smem, st, p, rpc);
     else if (variant == 2) launch_pri(hi, mm_tile_kernel<KS, 4>, grid, dim3(256), smem, st, p, rpc);

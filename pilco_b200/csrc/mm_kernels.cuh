@@ -704,67 +704,81 @@ static inline __host__ __device__ int setup_pair_rows(int np, int ldz) {
     const int nch = (np + cap - 1) / cap;
     return ((np + nch - 1) / nch + 63) & ~63;
 }
-static inline __host__ __device__ size_t setup_pair_smem_bytes(int rows, int ldz) { return 16 + (size_t)PAIR_BLK * 8 + (size_t)rows * ldz * 8; }
+// Pair tasks per pair-kernel CTA.  At one pair each, a batched step launches P x R x chunks CTAs (as many as the tile
+// launch, for a few per cent of its flops), and every one of them restages the chunk's zeta rows.  A group of pairs per
+// CTA brings the launch down to about one CTA per SM, capped by what the 48 KB of shared memory holds beside the zeta
+// rows (so that 3 CTAs per SM still fit), and by P.  (Measured on the H100: half the slot time, the same bench; DESIGN §6.)
+static inline __host__ __device__ int setup_pair_group(int P, int R, int nch, int nsm, int rows, int ldz) {
+    const long long tasks = (long long)P * R * nch;
+    int grp = (int)((tasks + nsm - 1) / nsm);
+    const int cap = (48 * 1024 - 16 - rows * ldz * 8) / (PAIR_BLK * 8);
+    if (grp > cap) grp = cap;
+    if (grp > P) grp = P;
+    return grp < 1 ? 1 : grp;
+}
+static inline __host__ __device__ size_t setup_pair_smem_bytes(int rows, int ldz, int grp) {
+    return 16 + (size_t)grp * PAIR_BLK * 8 + (size_t)rows * ldz * 8;
+}
 
-// Forward stage 2, pair tasks: one CTA per (pair, row chunk, restart).  One TMA bulk copy each brings the pair block
-// and the chunk's zeta rows (written by stage 1) into shared memory on one mbarrier; after that single wait no CTA-wide
-// barrier.  Each warp sweeps octet pairs {2j, 2j+1}, j = warp, warp + 8, ..., the two octets as independent DMMA chains:
-// first their B pieces, then their row operands.  Writes B_ab, U' (DMMA A fragments) and A' in the layout the tile kernels read.
+// Forward stage 2, pair tasks: one CTA per (group of `grp` consecutive pairs, row chunk, restart).  Two TMA bulk copies
+// bring the group's pair blocks (contiguous in the workspace) and the chunk's zeta rows (written by stage 1) into shared
+// memory on one mbarrier, so zeta is staged once for all the pairs of the CTA; after that single wait no CTA-wide
+// barrier.  The CTA's items -- (pair, unit of 16 rows = octets {2j, 2j+1}) -- are dealt round-robin over the 8 warps, so
+// no sweep round runs with idle warps beyond the last.  Per item a warp loads that pair's constants from shared memory and
+// runs the two octets as independent DMMA chains: first their B pieces, then their row operands.  Writes B_ab, U' (DMMA
+// A fragments) and A' in the layout the tile kernels read.
 #define SETUP_PAIR_WARPS 8
 template <int DP>
-__global__ void __launch_bounds__(32 * SETUP_PAIR_WARPS, 3) mm_setup2_pair_kernel(MMParams p, int rows) {
+__global__ void __launch_bounds__(32 * SETUP_PAIR_WARPS, 3) mm_setup2_pair_kernel(MMParams p, int rows, int grp) {
     PDL_ENTRY();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int KS = DP / 4, NT = (DP + 7) / 8;
     constexpr int ldz = DP <= 4 ? 4 : (DP <= 12 ? 12 : 20);   // == L.ldz
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
-    double* sblk = reinterpret_cast<double*>(smem_raw + 16);   // pair block (PAIR_*)
-    double* sZ = sblk + PAIR_BLK;                              // zeta rows [c0, c0 + cm)
+    double* sblk = reinterpret_cast<double*>(smem_raw + 16);   // pair blocks q0 .. q0 + nq - 1 (PAIR_*)
+    double* sZ = sblk + (size_t)grp * PAIR_BLK;                // zeta rows [c0, c0 + cm)
     const MMWs& L = p.L;
     const int n = p.gp.n, np = L.np;
-    const int q = blockIdx.x, r = blockIdx.z, c0 = blockIdx.y * rows;
+    const int q0 = blockIdx.x * grp, r = blockIdx.z, c0 = blockIdx.y * rows;
+    const int nq = (L.P - q0) < grp ? (L.P - q0) : grp;
     const int cm = (np - c0) < rows ? (np - c0) : rows;        // multiple of 64
+    const int nu = cm >> 4;                                    // 16-row units per pair
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     double* wsr = p.ws + (size_t)r * L.per_r;
     if (tid == 0) {
         mbar_init(bar, 1); mbar_fence_init();
-        mbar_expect_tx(bar, (unsigned)(PAIR_BLK * 8 + cm * ldz * 8));
-        tma_bulk_g2s(sblk, wsr + L.Qab + (size_t)q * PAIR_BLK, (unsigned)(PAIR_BLK * 8), bar);
+        mbar_expect_tx(bar, (unsigned)(nq * PAIR_BLK * 8 + cm * ldz * 8));
+        tma_bulk_g2s(sblk, wsr + L.Qab + (size_t)q0 * PAIR_BLK, (unsigned)(nq * PAIR_BLK * 8), bar);
         tma_bulk_g2s(sZ, wsr + L.zeta + (size_t)c0 * ldz, (unsigned)(cm * ldz * 8), bar);
     }
     __syncthreads();                                           // barrier initialisation visible to the waiting warps
     mbar_wait(bar, 0);
-    double* Bq = wsr + L.Bq + (size_t)q * np + c0;
-    double* Ar = wsr + L.Arow + (size_t)q * np + c0;
-    double* uf = wsr + L.Ufrag + ((size_t)q * (np >> 3) + (c0 >> 3)) * (KS * 32);
-    // two sweeps over the warp's octet pairs, so that only one sweep's pair constants are held in registers
-    {
-        double bqb[KS][NT];                                    // B fragments: B[k][n] = Qb[n][k]
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks)
-#pragma unroll
-            for (int nt = 0; nt < NT; ++nt) {
-                const int i = 8 * nt + g;
-                bqb[ks][nt] = i < DP ? sblk[PAIR_QB + i * DP + 4 * ks + t] : 0.0;
-            }
-        const double* pb = sblk + PAIR_PB;
-        const double lsb = sblk[PAIR_SC + 2];
-        for (int j = warp; 16 * j < cm; j += SETUP_PAIR_WARPS) {
-            const double* const zr[2] = {sZ + (size_t)(16 * j + g) * ldz, sZ + (size_t)(16 * j + 8 + g) * ldz};
-            const bool live[2] = {c0 + 16 * j + g < n, c0 + 16 * j + 8 + g < n};
-            double bv[2];
-            pair_b_octets<KS, 2>(bqb, pb, lsb, zr, live, lane, bv);
-            if (t == 0) { Bq[16 * j + g] = bv[0]; Bq[16 * j + 8 + g] = bv[1]; }
-        }
-    }
-    RowOpConsts<KS> roc;
-    roc.load(sblk, lane);
-    for (int j = warp; 16 * j < cm; j += SETUP_PAIR_WARPS) {
+    for (int it = warp; it < nq * nu; it += SETUP_PAIR_WARPS) {
+        const int k = it / nu, j = it - k * nu, q = q0 + k;
+        const double* blk = sblk + (size_t)k * PAIR_BLK;
         const double* const zr[2] = {sZ + (size_t)(16 * j + g) * ldz, sZ + (size_t)(16 * j + 8 + g) * ldz};
         const bool live[2] = {c0 + 16 * j + g < n, c0 + 16 * j + 8 + g < n};
+        {
+            double bqb[KS][NT];                                // B fragments: B[k][n] = Qb[n][k]
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+                for (int nt = 0; nt < NT; ++nt) {
+                    const int i = 8 * nt + g;
+                    bqb[ks][nt] = i < DP ? blk[PAIR_QB + i * DP + 4 * ks + t] : 0.0;
+                }
+            double bv[2];
+            pair_b_octets<KS, 2>(bqb, blk + PAIR_PB, blk[PAIR_SC + 2], zr, live, lane, bv);
+            double* Bq = wsr + L.Bq + (size_t)q * np + c0;
+            if (t == 0) { Bq[16 * j + g] = bv[0]; Bq[16 * j + 8 + g] = bv[1]; }
+        }
+        RowOpConsts<KS> roc;
+        roc.load(blk, lane);
         double ua[2][KS], Apv[2];
         row_operands_octets<KS, 2>(roc, zr, live, lane, ua, Apv);
+        double* Ar = wsr + L.Arow + (size_t)q * np + c0;
         if (t == 0) { Ar[16 * j + g] = Apv[0]; Ar[16 * j + 8 + g] = Apv[1]; }
+        double* uf = wsr + L.Ufrag + ((size_t)q * (np >> 3) + (c0 >> 3)) * (KS * 32);
 #pragma unroll
         for (int o = 0; o < 2; ++o)
 #pragma unroll
@@ -823,10 +837,11 @@ static inline void mm_setup_launch(const MMParams& p, cudaStream_t st) {
     if constexpr (BWD) {
         launch_hi(mm_setup2_bwd_kernel<DP>, dim3(ntask, p.R), dim3(128), 0, st, p);
     } else {
-        const int rows = setup_pair_rows(p.L.np, p.L.ldz);
+        const int rows = setup_pair_rows(p.L.np, p.L.ldz), nch = (p.L.np + rows - 1) / rows;
+        const int grp = setup_pair_group(p.L.P, p.R, nch, pilco_sm_count(), rows, p.L.ldz);
         launch_hi(mm_setup2_out_kernel<DP>, dim3(p.gp.E, p.R), dim3(128), 0, st, p);
-        launch_hi(mm_setup2_pair_kernel<DP>, dim3(p.L.P, (p.L.np + rows - 1) / rows, p.R), dim3(32 * SETUP_PAIR_WARPS),
-                  setup_pair_smem_bytes(rows, p.L.ldz), st, p, rows);
+        launch_hi(mm_setup2_pair_kernel<DP>, dim3((p.L.P + grp - 1) / grp, nch, p.R), dim3(32 * SETUP_PAIR_WARPS),
+                  setup_pair_smem_bytes(rows, p.L.ldz, grp), st, p, rows, grp);
     }
 }
 
