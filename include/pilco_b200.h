@@ -428,6 +428,38 @@ int    pilco_rollout_noisy_forward(const pilco_rollout* ro, const pilco_angles* 
 int    pilco_rollout_noisy_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                     const pilco_obs_noise* nz, const pilco_rollout_grad* g, pilco_stream_t stream);
 
+/* ---- time-varying linear policy (probabilistic MPC's action sequences; DESIGN.md section 27) ---------------------
+ * The rollout of pilco_rollout_noisy_* (ang, ex and nz may be NULL) whose linear policy is indexed by the step: restart r
+ * at step t = 0 .. H-1 applies u_t = W_t x~ + b_t (squashed when pol.squash, x~ the policy's input as in the noisy call)
+ * with
+ *   W_t = pol.W + r pol.W_bs + t W_ts   [U, Dh],     b_t = pol.b + r pol.b_bs + t b_ts   [U].
+ * W_t = 0 at every step is an open-loop action sequence.  The schedule is active when sch != NULL and W_ts or b_ts is
+ * non-zero; an inactive call is the pilco_rollout_noisy_* call: outputs, gradients, workspace sizes and status codes.
+ * With an active schedule the backward writes the cotangents per step, g->gW [R, H, U, Dh] and g->gb [R, H, U] (their
+ * sum over t is the stationary policy's gradient), and needs the larger reverse workspace
+ * pilco_rollout_scheduled_bwd_workspace_bytes reports; the forward workspace and the tape are the noisy call's.
+ * Validation before any work is enqueued: the noisy call's status codes up to its workspace check, then PILCO_ERR_DIM
+ * for a negative stride, then PILCO_ERR_UNSUPPORTED for an active schedule with an RBF policy, then the workspace's
+ * codes.  A size query returns 0 for R < 1, H < 0 or a negative stride. */
+typedef struct pilco_policy_schedule {
+    long long W_ts;             /* step stride of pol.W in doubles (U * Dh for a dense [H, U, Dh] block), >= 0 */
+    long long b_ts;             /* step stride of pol.b in doubles (U for a dense [H, U] block), >= 0 */
+} pilco_policy_schedule;
+
+size_t pilco_rollout_scheduled_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                               const pilco_exploration* ex, const pilco_obs_noise* nz,
+                                               const pilco_policy_schedule* sch);
+int    pilco_rollout_scheduled_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                       const pilco_obs_noise* nz, const pilco_policy_schedule* sch,
+                                       pilco_stream_t stream);
+size_t pilco_rollout_scheduled_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                                   const pilco_exploration* ex, const pilco_obs_noise* nz,
+                                                   const pilco_policy_schedule* sch);
+/* must follow pilco_rollout_scheduled_forward with the same arguments */
+int    pilco_rollout_scheduled_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                        const pilco_obs_noise* nz, const pilco_policy_schedule* sch,
+                                        const pilco_rollout_grad* g, pilco_stream_t stream);
+
 /* ---- particle rollout -------------------------------------------------------------------------
  * Monte Carlo check of the moment-matching cascade (nothing in the reference; the PILCO papers validate moment
  * matching against particle rollouts of the same model).  P particles follow the Markov chain whose Gaussian

@@ -90,6 +90,11 @@ class ParticlesNoise(C.Structure):
     _fields_ = [("v", ObsNoise), ("nu", c_dp)]
 
 
+class PolicySchedule(C.Structure):
+    """mirror of ``pilco_policy_schedule``"""
+    _fields_ = [("W_ts", c_ll), ("b_ts", c_ll)]
+
+
 class ParticlesResample(C.Structure):
     """mirror of ``pilco_particles_resample``"""
     _fields_ = [("xi", c_dp), ("step_mean", c_dp), ("step_cov", c_dp)]
@@ -104,6 +109,8 @@ ABI_VERSION = 3
 ABI_MAX_D = 16                                   # PILCO_MAX_D
 
 _PAN = [C.POINTER(Particles), C.POINTER(Angles), C.POINTER(ParticlesNoise)]     # the noisy particle calls' first three
+
+_RAEN = [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration), C.POINTER(ObsNoise)]   # the noisy rollout's
 
 # name -> (restype, argtypes); every symbol declared in include/pilco_b200.h
 SIGNATURES = {
@@ -170,6 +177,10 @@ SIGNATURES = {
                                               C.POINTER(ObsNoise), c_dp]),
     "pilco_rollout_noisy_backward": (C.c_int, [C.POINTER(Rollout), C.POINTER(Angles), C.POINTER(Exploration),
                                                C.POINTER(ObsNoise), C.POINTER(RolloutGrad), c_dp]),
+    "pilco_rollout_scheduled_workspace_bytes": (C.c_size_t, _RAEN + [C.POINTER(PolicySchedule)]),
+    "pilco_rollout_scheduled_forward": (C.c_int, _RAEN + [C.POINTER(PolicySchedule), c_dp]),
+    "pilco_rollout_scheduled_bwd_workspace_bytes": (C.c_size_t, _RAEN + [C.POINTER(PolicySchedule)]),
+    "pilco_rollout_scheduled_backward": (C.c_int, _RAEN + [C.POINTER(PolicySchedule), C.POINTER(RolloutGrad), c_dp]),
     "pilco_particles_workspace_bytes": (C.c_size_t, [C.POINTER(Particles)]),
     "pilco_particles_rollout": (C.c_int, [C.POINTER(Particles), c_dp]),
     "pilco_gp_predict_vjp_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

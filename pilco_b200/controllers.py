@@ -1,4 +1,5 @@
-"""Policies (drop-in for pilco/controllers.py): ``squash_sin``, ``LinearController``, ``RbfController``.
+"""Policies (drop-in for pilco/controllers.py): ``squash_sin``, ``LinearController``, ``RbfController``, and the
+step-indexed ``TimeVaryingLinearController`` of receding-horizon planning (``PILCO.plan``).
 All moment computations run on the device through the C ABI (``pilco_squash_sin``,
 ``pilco_linear_action``, ``pilco_gp_factorize`` + ``pilco_mm_forward`` in deterministic-GP mode)."""
 import numpy as np
@@ -78,6 +79,101 @@ class LinearController:
         U, Ds = self.W.shape
         self.W.assign(np.asarray(flat[:U * Ds]).reshape(U, Ds))
         self.b.assign(np.asarray(flat[U * Ds:]).reshape(1, U))
+
+
+class TimeVaryingLinearController:
+    """u_t = W_t x + b_t, one (W_t, b_t) per step t = 0 .. horizon-1 (squashed by squash_sin in the rollout): the
+    action sequences that probabilistic MPC plans through the moment-matching cascade (Kamthe & Deisenroth 2018;
+    DESIGN.md section 27).  ``feedback=False`` is the open-loop sequence u_t = b_t: W stays 0 and is not trainable.
+    The flat vector is [W (horizon*U*Ds) | b (horizon*U)], or [b] without feedback, step-major."""
+
+    def __init__(self, state_dim, control_dim, horizon, max_action=1.0, feedback=True):
+        if int(horizon) < 1:
+            raise ValueError("TimeVaryingLinearController: horizon must be >= 1, got %r" % horizon)
+        self.horizon, self.feedback = int(horizon), bool(feedback)
+        H, U, Ds = self.horizon, int(control_dim), int(state_dim)
+        W0 = 0.1 * np.random.randn(H, U, Ds) if self.feedback else np.zeros((H, U, Ds))
+        self.W = Parameter(W0, trainable=self.feedback, name="W")
+        self.b = Parameter(0.1 * np.random.randn(H, U), name="b")
+        self.max_action = max_action
+
+    @property
+    def parameters(self):
+        return [self.W, self.b]
+
+    @property
+    def trainable_parameters(self):
+        return [p for p in self.parameters if p.trainable]
+
+    def compute_action(self, m, s, squash=True, t=0):
+        """the moments of step t's action at N(m, s) -> (M [1,U], S [U,U], V [Ds,U])"""
+        t = int(t)
+        if not 0 <= t < self.horizon:
+            raise ValueError("compute_action: step t=%d outside the schedule's %d steps" % (t, self.horizon))
+        m = np.asarray(m, dtype=np.float64).reshape(1, -1)
+        Ds = m.shape[1]
+        s = np.asarray(s, dtype=np.float64).reshape(1, Ds, Ds)
+        U = self.b.shape[1]
+        M, S, V = engine.linear_action(np.asarray(self.W)[t], np.asarray(self.b)[t], m, s)
+        if squash:
+            M, S, C = engine.squash_sin(M, S, _max_action_vec(self.max_action, U))
+            V = V @ C
+        return host(M), host(S[0]), host(V[0])
+
+    def randomize(self):
+        """small random parameters around 0: b ~ N(0, 0.1^2) (and W likewise with feedback)"""
+        if self.feedback:
+            self.W.assign(0.1 * np.random.normal(size=self.W.shape))
+        self.b.assign(0.1 * np.random.normal(size=self.b.shape))
+
+    def shift(self):
+        """the receding horizon's warm start: theta_t <- theta_{t+1}, the last step repeated"""
+        for p in self.parameters:
+            v = np.asarray(p)
+            p.assign(np.concatenate([v[1:], v[-1:]]))
+
+    def policy_spec(self, flat=None):
+        """the scheduled spec of engine.RolloutPlan(..., schedule=True): W [lead.., H, U, Ds], b [lead.., H, U]"""
+        H, U, Ds = self.W.shape
+        if flat is None:
+            W, b = np.asarray(self.W), np.asarray(self.b)
+        else:
+            flat = np.asarray(flat, dtype=np.float64)
+            lead = flat.shape[:-1]
+            nW = H * U * Ds if self.feedback else 0
+            W = flat[..., :nW].reshape(lead + (H, U, Ds)) if nW else np.zeros(lead + (H, U, Ds))
+            b = flat[..., nW:].reshape(lead + (H, U))
+        return dict(kind=_lib.POLICY_LINEAR, Ds=Ds, U=U, squash=True, max_action=_max_action_vec(self.max_action, U),
+                    W=W, b=b, schedule=True)
+
+    def state_key(self):
+        return hash((np.asarray(self.W).tobytes(), np.asarray(self.b).tobytes(),
+                     np.asarray(self.max_action, dtype=np.float64).tobytes()))
+
+    def get_flat(self):
+        b = np.asarray(self.b).ravel()
+        return np.concatenate([np.asarray(self.W).ravel(), b]) if self.feedback else b
+
+    def set_flat(self, flat):
+        H, U, Ds = self.W.shape
+        flat = np.asarray(flat, dtype=np.float64)
+        nW = H * U * Ds if self.feedback else 0
+        if nW:
+            self.W.assign(flat[:nW].reshape(H, U, Ds))
+        self.b.assign(flat[nW:].reshape(H, U))
+
+    def flat_grad(self, gW, gb):
+        """per-step cotangents gW [n, U, Ds], gb [n, U] of an n-step rollout (n <= horizon) -> the get_flat() layout,
+        zero for the steps the rollout does not reach"""
+        H, U, Ds = self.W.shape
+        n = np.shape(gb)[0]
+        fb = np.zeros((H, U))
+        fb[:n] = np.asarray(gb).reshape(n, U)
+        if not self.feedback:
+            return fb.ravel()
+        fW = np.zeros((H, U, Ds))
+        fW[:n] = np.asarray(gW).reshape(n, U, Ds)
+        return np.concatenate([fW.ravel(), fb.ravel()])
 
 
 class FakeLikelihood:

@@ -205,7 +205,7 @@ static int ro_check_as(const pilco_rollout* ro, int E) {
 }
 
 int ro_validate(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const pilco_obs_noise* nz,
-                bool backward, RoOpt* o) {
+                bool backward, RoOpt* o, const pilco_policy_schedule* sch) {
     *o = RoOpt{};
     if (!ro) return PILCO_ERR_NULL;
     const int A = ang ? ang->A : 0, Ds = ro->dyn.E;
@@ -230,6 +230,8 @@ int ro_validate(const pilco_rollout* ro, const pilco_angles* ang, const pilco_ex
     }
     o->phi = ro_on_phi(ang, nz);
     if (o->phi && A == 0) trig_map_make(Ds, 0, nullptr, &o->tm);
+    if (sch && (sch->W_ts < 0 || sch->b_ts < 0)) return PILCO_ERR_DIM;
+    if (sch_active(sch) && ro->pol.kind != PILCO_POLICY_LINEAR) return PILCO_ERR_UNSUPPORTED;
     if ((!backward || o->explore || o->noise) && ro->ws_bytes < ro_ws_layout(ro, ang, ex, nz).total * sizeof(double))
         return PILCO_ERR_WORKSPACE;
     if (backward) return PILCO_OK;
@@ -243,13 +245,15 @@ int ro_validate(const pilco_rollout* ro, const pilco_angles* ang, const pilco_ex
     return PILCO_OK;
 }
 
-// The forward of every call (ang, ex, nz may be NULL).  Per step the state kernel is ro_state, tg_state on phi or
+// The forward of every call (ang, ex, nz, sch may be NULL).  Per step the state kernel is ro_state, tg_state on phi or
 // nz_state with noise, and the policy kernel ro_policy or tg_policy (on phi); the policy GP reads x_t, phi's moments or
 // the noisy ones.  The state terms read the raw trajectory, the joint terms [phi, u]: ro_reward_joint's D = Dh + U.
+// Every state kernel reads the linear policy through its launch's W and b, so a schedule advances them by a step's
+// strides before each launch and no kernel changes.
 static int ro_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                      const pilco_obs_noise* nz, cudaStream_t st) {
+                      const pilco_obs_noise* nz, const pilco_policy_schedule* sch, cudaStream_t st) {
     RoOpt o;
-    int rc = ro_validate(ro, ang, ex, nz, false, &o);
+    int rc = ro_validate(ro, ang, ex, nz, false, &o, sch);
     if (rc) return rc;
     const RoWs L = ro_ws_layout(ro, ang, ex, nz);
     double* ws = (double*)ro->ws;
@@ -286,8 +290,10 @@ static int ro_forward(const pilco_rollout* ro, const pilco_angles* ang, const pi
     };
 
     if (ro->info) cudaMemsetAsync(ro->info, 0, sizeof(int) * RR, st);
+    const long long W_ts = sch_active(sch) ? sch->W_ts : 0, b_ts = sch_active(sch) ? sch->b_ts : 0;
     for (int t = 0; t <= H; ++t) {
         d.t = t;
+        if (W_ts || b_ts) { d.W = ro->pol.W + (t < H ? t : 0) * W_ts; d.b = ro->pol.b + (t < H ? t : 0) * b_ts; }
         const int tc = t < H ? t : H - 1 < 0 ? 0 : H - 1;      // slot used for "current" pointers (unused at t==H)
         d.mj = slot(L.mj, D, tc); d.sj = slot(L.sj, (size_t)D * D, tc);
         d.Mp = slot(L.Mp, U, tc); d.Sp = slot(L.Sp, (size_t)U * U, tc); d.Vp = slot(L.Vp, (size_t)Dh * U, tc);
@@ -348,8 +354,8 @@ static int ro_forward(const pilco_rollout* ro, const pilco_angles* ang, const pi
 
 // the size of the forward workspace: 0 for a description without a batch or with H < 0
 static size_t ro_ws_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                          const pilco_obs_noise* nz) {
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
+                          const pilco_obs_noise* nz, const pilco_policy_schedule* sch = nullptr) {
+    if (!ro || ro->R < 1 || ro->H < 0 || (sch && (sch->W_ts < 0 || sch->b_ts < 0))) return 0;
     return ro_ws_layout(ro, ang, ex, nz).total * sizeof(double);
 }
 
@@ -383,21 +389,32 @@ size_t pilco_rollout_noisy_workspace_bytes(const pilco_rollout* ro, const pilco_
 }
 
 int pilco_rollout_forward(const pilco_rollout* ro, pilco_stream_t stream) {
-    return ro_forward(ro, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+    return ro_forward(ro, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int pilco_rollout_angles_forward(const pilco_rollout* ro, const pilco_angles* ang, pilco_stream_t stream) {
-    return ro_forward(ro, ang, nullptr, nullptr, (cudaStream_t)stream);
+    return ro_forward(ro, ang, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int pilco_rollout_explore_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                   pilco_stream_t stream) {
-    return ro_forward(ro, ang, ex, nullptr, (cudaStream_t)stream);
+    return ro_forward(ro, ang, ex, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int pilco_rollout_noisy_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                 const pilco_obs_noise* nz, pilco_stream_t stream) {
-    return ro_forward(ro, ang, ex, nz, (cudaStream_t)stream);
+    return ro_forward(ro, ang, ex, nz, nullptr, (cudaStream_t)stream);
+}
+
+size_t pilco_rollout_scheduled_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                               const pilco_exploration* ex, const pilco_obs_noise* nz,
+                                               const pilco_policy_schedule* sch) {
+    return ro_ws_bytes(ro, ang, ex, nz, sch);
+}
+
+int pilco_rollout_scheduled_forward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                    const pilco_obs_noise* nz, const pilco_policy_schedule* sch, pilco_stream_t stream) {
+    return ro_forward(ro, ang, ex, nz, sch, (cudaStream_t)stream);
 }
 
 }  // extern "C"

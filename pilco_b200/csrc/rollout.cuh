@@ -55,9 +55,13 @@ struct RoOpt {
 
 // Validation of a call of the cascade (ang, ex, nz may be NULL) before anything is enqueued: the description, the
 // angles, the exploration terms, the noise variances, then ro->ws's size (and for the forward its alignment and the
-// tape).  The reverse sweep without exploration and noise does not check ro->ws.
+// tape).  The reverse sweep without exploration and noise does not check ro->ws.  A policy schedule (sch, may be NULL)
+// is checked after the noise and before the workspace.
 int ro_validate(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex, const pilco_obs_noise* nz,
-                bool backward, RoOpt* o);
+                bool backward, RoOpt* o, const pilco_policy_schedule* sch = nullptr);
+
+// a schedule that moves the policy's parameters with the step (pilco_rollout_scheduled_*); inactive: the stationary call
+static inline bool sch_active(const pilco_policy_schedule* sch) { return sch && (sch->W_ts != 0 || sch->b_ts != 0); }
 
 // the state terms (for ro_reward / rb_reward; n_state of them) and the joint state-action terms (for the *_joint
 // kernels), each in term order and padded with empty terms to 8; returns the number of joint terms

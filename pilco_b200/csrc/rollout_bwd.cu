@@ -28,14 +28,16 @@ int chol_solve_vec_launch(cudaStream_t st, int batch, int n, const double* L, in
 
 struct RbWs {            // backward workspace (offsets in doubles)
     size_t gm, gS, gMd, gSd, gVd, gcx, gmj, gsj, gsjx, gMp, gSp, gVp, gmh, gSh, gCh, gbeta, gy, rgm, rgS, jgm, jgS, cnt,
-           dynb, polb, gmz, gSz, total;
+           dynb, polb, gmz, gSz, sgW, sgb, total;
 };
 
 // Dh = pol.Ds, Ds = dyn.E on phi (pol.Ds without).  Without phi the seeds of the dynamics VJP (gMd, gSd, gVd) and the
 // glue's joint cotangent gsjx have slots of their own (rb_pre); on phi gVd and gcx are the seeds tg_trig leaves and
 // (gmh, gSh, gCh) the feature cotangent; with noise (gmz, gSz) the cotangent of the noisy moments.  A slot whose
-// feature is off has length 0.
-static RbWs rb_ws_layout(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz) {
+// feature is off has length 0.  An active policy schedule appends the per-step cotangents of W_t and b_t, step-major
+// ([H][R][U*Dh], [H][R][U]: what rb_post / tg_post / nz_trig write at step t), after every other slot.
+static RbWs rb_ws_layout(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz,
+                         const pilco_policy_schedule* sch = nullptr) {
     const bool phi = ro_on_phi(ang, nz);
     const size_t R = ro->R, H = ro->H, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U, Ds = phi ? (size_t)ro->dyn.E : Dh;
     const size_t F = phi ? 1 : 0, P = 1 - F, N = nz ? 1 : 0;
@@ -62,6 +64,8 @@ static RbWs rb_ws_layout(const pilco_rollout* ro, const pilco_angles* ang, const
     if (ro->pol.kind == PILCO_POLICY_RBF)
         o += pilco_mm_bwd_workspace_bytes(ro->pol.rbf.n, ro->pol.rbf.D, ro->pol.rbf.E, ro->R, 1) / 8;
     L.gmz = take(N * Dh); L.gSz = take(N * Dh * Dh);
+    const size_t HS = sch_active(sch) ? H : 0;
+    L.sgW = take(HS * U * Dh); L.sgb = take(HS * U);
     L.total = o;
     return L;
 }
@@ -345,6 +349,26 @@ int rb_reward_launch(const RbDev& ds, const RbDev* dj, cudaStream_t st) {
     return PILCO_OK;
 }
 
+// the per-step policy cotangents, step-major in the workspace ([H][R][n]), to the caller's restart-major [R][H][n]
+__global__ void __launch_bounds__(128) rb_sched_grad_kernel(int R, int H, int n, const double* __restrict__ src,
+                                                             double* __restrict__ dst) {
+    PDL_ENTRY();
+    const size_t total = (size_t)R * H * n;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const size_t i = e % n, rt = e / n, t = rt % H, r = rt / H;
+        dst[e] = src[(t * R + r) * n + i];
+    }
+}
+
+static int rb_sched_grad_launch(int R, int H, int n, const double* src, double* dst, cudaStream_t st) {
+    const size_t total = (size_t)R * H * n;
+    if (total == 0) return PILCO_OK;
+    const unsigned blocks = (unsigned)((total + 127) / 128 < 1024 ? (total + 127) / 128 : 1024);
+    launch_hi(rb_sched_grad_kernel, dim3(blocks), dim3(128), 0, st, R, H, n, src, dst);
+    CUDA_LAUNCH_CHECK();
+    return PILCO_OK;
+}
+
 // rb_post for step d.t: with a tape (tb) fused into rb_dyn_finish, the tape-driven dynamics VJP, else a launch of its own
 static int rb_post_launch(const RbDev& d, const MMTapeBwd* tb, cudaStream_t st) {
     if (tb) {
@@ -357,16 +381,19 @@ static int rb_post_launch(const RbDev& d, const MMTapeBwd* tb, cudaStream_t st) 
     return PILCO_OK;
 }
 
-// The reverse sweep of every call (ang, ex, nz may be NULL).  Per step the post stage is rb_post (rb_pre before the
+// The reverse sweep of every call (ang, ex, nz, sch may be NULL).  Per step the post stage is rb_post (rb_pre before the
 // recomputing dynamics VJP) or tg_post on phi, which with noise stops before the linear-policy VJP; the policy GP's
 // VJP reads x_t, phi's moments or the noisy ones; the trig stage (on phi) is tg_trig or, with noise, nz_trig.
+// With an active schedule the linear-policy VJP of step t reads W_t and accumulates into step t's own gradient slots
+// (rb_ws_layout's sgW, sgb), which rb_sched_grad reorders into g->gW, g->gb after the sweep.
 static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
-                       const pilco_obs_noise* nz, const pilco_rollout_grad* g, cudaStream_t st) {
+                       const pilco_obs_noise* nz, const pilco_policy_schedule* sch, const pilco_rollout_grad* g,
+                       cudaStream_t st) {
     RoOpt o;
-    int rc = ro_validate(ro, ang, ex, nz, true, &o);
+    int rc = ro_validate(ro, ang, ex, nz, true, &o, sch);
     if (rc) return rc;
     if (!g || !g->ws) return PILCO_ERR_NULL;
-    const RbWs BL = rb_ws_layout(ro, ang, nz);
+    const RbWs BL = rb_ws_layout(ro, ang, nz, sch);
     if (g->ws_bytes < BL.total * sizeof(double)) return PILCO_ERR_WORKSPACE;
     if (((uintptr_t)g->ws) & 15) return PILCO_ERR_ALIGN;
     const int R = ro->R, H = ro->H, Ds = ro->dyn.E, Dh = ro->pol.Ds, U = ro->pol.U, D = Dh + U;
@@ -389,6 +416,8 @@ static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const p
         cudaMemsetAsync(g->gXc, 0, sizeof(double) * RR * bf * Dh, st);
         cudaMemsetAsync(g->gell, 0, sizeof(double) * RR * U * Dh, st);
         cudaMemsetAsync(buf(BL.gbeta), 0, sizeof(double) * RR * U * bf, st);
+    } else if (sch_active(sch)) {
+        cudaMemsetAsync(buf(BL.sgW), 0, sizeof(double) * (BL.total - BL.sgW), st);
     } else {
         cudaMemsetAsync(g->gW, 0, sizeof(double) * RR * U * Dh, st);
         cudaMemsetAsync(g->gb, 0, sizeof(double) * RR * U, st);
@@ -438,8 +467,13 @@ static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const p
         }
     }
 
+    const long long W_ts = sch_active(sch) ? sch->W_ts : 0, b_ts = sch_active(sch) ? sch->b_ts : 0;
     for (int t = H - 1; t >= 0; --t) {
         d.t = t;
+        if (W_ts || b_ts) {
+            d.W = ro->pol.W + t * W_ts;
+            d.gW = buf(BL.sgW) + (size_t)t * RR * U * Dh; d.gb = buf(BL.sgb) + (size_t)t * RR * U;
+        }
         d.sj = slot(FL.sj, (size_t)D * D, t); d.Vd = slot(FL.Vd, (size_t)D * Ds, t);
         d.Mp = slot(FL.Mp, U, t); d.Sp = slot(FL.Sp, (size_t)U * U, t); d.Vp = slot(FL.Vp, (size_t)Dh * U, t);
         d.Mu = slot(FL.Mu, U, t); d.Su = slot(FL.Su, (size_t)U * U, t); d.Cq = slot(FL.Cq, (size_t)U * U, t);
@@ -503,6 +537,11 @@ static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const p
                                    buf(BL.gy), g->gXc, g->gYc, g->gell);
         if (rc) return rc;
     }
+    if (W_ts || b_ts) {
+        rc = rb_sched_grad_launch(R, H, U * Dh, buf(BL.sgW), g->gW, st);
+        if (!rc) rc = rb_sched_grad_launch(R, H, U, buf(BL.sgb), g->gb, st);
+        if (rc) return rc;
+    }
     if (g->gm0) cudaMemcpyAsync(g->gm0, d.gm, sizeof(double) * RR * Ds, cudaMemcpyDeviceToDevice, st);
     if (g->gS0) cudaMemcpyAsync(g->gS0, d.gS, sizeof(double) * RR * Ds * Ds, cudaMemcpyDeviceToDevice, st);
     return PILCO_OK;
@@ -510,9 +549,10 @@ static int rb_backward(const pilco_rollout* ro, const pilco_angles* ang, const p
 
 // the size of the reverse sweep's workspace (the exploration gradient adds none): 0 for a description without a batch
 // or with H < 0
-static size_t rb_ws_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz) {
-    if (!ro || ro->R < 1 || ro->H < 0) return 0;
-    return rb_ws_layout(ro, ang, nz).total * sizeof(double);
+static size_t rb_ws_bytes(const pilco_rollout* ro, const pilco_angles* ang, const pilco_obs_noise* nz,
+                          const pilco_policy_schedule* sch = nullptr) {
+    if (!ro || ro->R < 1 || ro->H < 0 || (sch && (sch->W_ts < 0 || sch->b_ts < 0))) return 0;
+    return rb_ws_layout(ro, ang, nz, sch).total * sizeof(double);
 }
 
 extern "C" {
@@ -536,22 +576,35 @@ size_t pilco_rollout_noisy_bwd_workspace_bytes(const pilco_rollout* ro, const pi
 }
 
 int pilco_rollout_backward(const pilco_rollout* ro, const pilco_rollout_grad* g, pilco_stream_t stream) {
-    return rb_backward(ro, nullptr, nullptr, nullptr, g, (cudaStream_t)stream);
+    return rb_backward(ro, nullptr, nullptr, nullptr, nullptr, g, (cudaStream_t)stream);
 }
 
 int pilco_rollout_angles_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_rollout_grad* g,
                                   pilco_stream_t stream) {
-    return rb_backward(ro, ang, nullptr, nullptr, g, (cudaStream_t)stream);
+    return rb_backward(ro, ang, nullptr, nullptr, nullptr, g, (cudaStream_t)stream);
 }
 
 int pilco_rollout_explore_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                    const pilco_rollout_grad* g, pilco_stream_t stream) {
-    return rb_backward(ro, ang, ex, nullptr, g, (cudaStream_t)stream);
+    return rb_backward(ro, ang, ex, nullptr, nullptr, g, (cudaStream_t)stream);
 }
 
 int pilco_rollout_noisy_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
                                  const pilco_obs_noise* nz, const pilco_rollout_grad* g, pilco_stream_t stream) {
-    return rb_backward(ro, ang, ex, nz, g, (cudaStream_t)stream);
+    return rb_backward(ro, ang, ex, nz, nullptr, g, (cudaStream_t)stream);
+}
+
+size_t pilco_rollout_scheduled_bwd_workspace_bytes(const pilco_rollout* ro, const pilco_angles* ang,
+                                                   const pilco_exploration* ex, const pilco_obs_noise* nz,
+                                                   const pilco_policy_schedule* sch) {
+    (void)ex;
+    return rb_ws_bytes(ro, ang, nz, sch);
+}
+
+int pilco_rollout_scheduled_backward(const pilco_rollout* ro, const pilco_angles* ang, const pilco_exploration* ex,
+                                     const pilco_obs_noise* nz, const pilco_policy_schedule* sch,
+                                     const pilco_rollout_grad* g, pilco_stream_t stream) {
+    return rb_backward(ro, ang, ex, nz, sch, g, (cudaStream_t)stream);
 }
 
 }  // extern "C"

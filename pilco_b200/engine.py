@@ -480,6 +480,32 @@ def _fill_policy(pol, policy_spec, batched=None):
     return max_action, W, b, rbf
 
 
+def _schedule_check(policy_spec, H, schedule):
+    """A scheduled spec (a time-varying linear policy: W [R?,Hw,U,Ds], b [R?,Hw,U]) against RolloutPlan's ``schedule``
+    and horizon H, before any allocation: ValueError.  Returns the (batched, Hw) of a scheduled spec, else None."""
+    if not schedule:
+        if isinstance(policy_spec, dict) and policy_spec.get("schedule", False):
+            raise ValueError("the policy spec is a time-varying linear policy (a schedule): pass schedule=True")
+        return None
+    if policy_spec["kind"] != _lib.POLICY_LINEAR:
+        raise ValueError("schedule=True takes a linear policy (time-varying W_t, b_t); an RBF policy has no schedule")
+    U, Ds = int(policy_spec["U"]), int(policy_spec["Ds"])
+    Ws, bs = np.shape(policy_spec["W"]), np.shape(policy_spec["b"])
+    if len(Ws) not in (3, 4) or Ws[-2:] != (U, Ds) or bs != Ws[:-2] + (U,):
+        raise ValueError("schedule=True: expected W [R?, H, U=%d, Ds=%d] and b [R?, H, U], got W %s, b %s"
+                         % (U, Ds, Ws, bs))
+    Hw = int(Ws[-3])
+    if Hw < int(H):
+        raise ValueError("schedule=True: the schedule has %d steps, fewer than the rollout's H=%d" % (Hw, int(H)))
+    return len(Ws) == 4, Hw
+
+
+def _no_schedule(policy_spec, what):
+    if isinstance(policy_spec, dict) and policy_spec.get("schedule", False):
+        raise ValueError("%s: the particle rollouts do not support a time-varying linear policy (schedule); use the "
+                         "moment-matching RolloutPlan(..., schedule=True)" % what)
+
+
 def _fill_rewards(desc, reward_terms):
     """Fill ``desc.n_rewards`` and ``desc.rewards`` from reward-term dicts (``desc.pol`` already filled); returns the
     device tensors [(W, t)] they point to.  The shapes of a joint state-action term are checked against the policy
@@ -534,7 +560,7 @@ class RolloutPlan:
     enter the returned reward as ``mult_mu * (1 - prod_t (1 - risk_t))``)."""
 
     def __init__(self, dyn, policy_spec, reward_terms, m0, S0, H, R=1, mult_mu=0.0, grad=False, angles=None,
-                 exploration=None, measurement_noise=None):
+                 exploration=None, measurement_noise=None, schedule=False):
         """``grad=True``: the forward cascade runs the TAPED dynamics tile pass (pilco_rollout.tape), so that
         ``backward()`` needs no recomputation; without it ``backward()`` still works (recomputing path).
 
@@ -551,7 +577,13 @@ class RolloutPlan:
         ``measurement_noise``: variances v [Ds] >= 0 of a noisy state measurement z = x + nu, nu ~ N(0, diag(v)), that
         the policy sees in place of the state (pilco_rollout_noisy_*, DESIGN.md section 22): the policy is moment-matched
         at N(m, S + diag(v)) (phi of it with angles), the dynamics and the rewards see the true state's moments.  Ds is
-        the raw state dimension.  ``None``: the policy sees the state."""
+        the raw state dimension.  ``None``: the policy sees the state.
+
+        ``schedule=True``: a time-varying linear policy u_t = sq(W_t x + b_t) (pilco_rollout_scheduled_*, DESIGN.md
+        section 27); the spec's W is [Hw, U, Ds] or [R, Hw, U, Ds] and b [Hw, U] or [R, Hw, U], Hw >= H (step t < H reads
+        W[..., t, :, :]).  ``backward()`` then returns the per-step cotangents W [R, H, U, Ds] and b [R, H, U].  An RBF
+        spec or Hw < H is a ValueError."""
+        sched = _schedule_check(policy_spec, H, schedule)
         b = None
         if exploration is not None:
             b = float(exploration)
@@ -590,7 +622,13 @@ class RolloutPlan:
         ro = _lib.Rollout()
         ro.R, ro.H = self.R, self.H
         ro.dyn = dyn.struct()
-        self.max_action, self.W, self.b, self.rbf = _fill_policy(ro.pol, policy_spec)
+        self.max_action, self.W, self.b, self.rbf = _fill_policy(ro.pol, policy_spec,
+                                                                 batched=None if sched is None else False)
+        self.sch = None
+        if sched is not None:                                   # step t reads W[..., t, :, :], b[..., t, :]
+            U, Ds = int(policy_spec["U"]), int(policy_spec["Ds"])
+            ro.pol.W_bs, ro.pol.b_bs = (sched[1] * U * Ds, sched[1] * U) if sched[0] else (0, 0)
+            self.sch = _lib.PolicySchedule(U * Ds, U)
         self.rw = _fill_rewards(ro, reward_terms)
         self.m0, self.S0 = dev(m0), dev(S0)
         # per-restart initial moments: leading dimension R (and R > 1); [1, ...] or unbatched = shared by the batch
@@ -620,7 +658,7 @@ class RolloutPlan:
         if b is not None:
             self.step_var = torch.zeros((self.R, max(self.H, 1)), dtype=F64, device=d)
             self.ex = _lib.Exploration(b, self.step_var.data_ptr())
-        wsb = lib.pilco_rollout_noisy_workspace_bytes(C.byref(ro), self._ang_ref(), self._ex_ref(), self._nz_ref())
+        wsb = self._call("workspace_bytes", ro)
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         ro.ws, ro.ws_bytes = self.ws.data_ptr(), wsb
         self.tape = None
@@ -640,9 +678,16 @@ class RolloutPlan:
     def _nz_ref(self):
         return C.byref(self.nz) if self.nz is not None else None
 
+    def _call(self, what, ro, *rest):
+        """pilco_rollout_noisy_<what>, or with a schedule pilco_rollout_scheduled_<what>"""
+        args = (C.byref(ro), self._ang_ref(), self._ex_ref(), self._nz_ref())
+        if self.sch is not None:
+            return getattr(lib, "pilco_rollout_scheduled_" + what)(*args, C.byref(self.sch), *rest)
+        return getattr(lib, "pilco_rollout_noisy_" + what)(*args, *rest)
+
     def forward(self):
-        check(lib.pilco_rollout_noisy_forward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), self._nz_ref(),
-                                              stream_ptr()), "rollout_noisy_forward")
+        check(self._call("forward", self.ro, stream_ptr()),
+              "rollout_noisy_forward" if self.sch is None else "rollout_scheduled_forward")
         return self.traj_m, self.traj_S, self.reward
 
     # ---- CUDA graph: the whole H-step loop (6H+1 launches forward, ~10H backward) as one graph launch -------
@@ -667,22 +712,22 @@ class RolloutPlan:
 
     def backward(self):
         """pilco_rollout_backward: d reward[r] / d policy parameters (call after forward()).
-        Linear: {'W': [R,U,Ds], 'b': [R,U]};  RBF: {'X': [R,bf,Ds], 'Y': [R,bf,U], 'ell': [R,U,Ds]}."""
+        Linear: {'W': [R,U,Ds], 'b': [R,U]} (with a schedule per step: [R,H,U,Ds], [R,H,U]);
+        RBF: {'X': [R,bf,Ds], 'Y': [R,bf,U], 'ell': [R,U,Ds]}."""
         d = device()
         if not hasattr(self, "grad"):
             g = _lib.RolloutGrad()
             R, Ds = self.R, self.Ds
-            self.gbuf = _policy_grad_buffers(g, self.ro.pol, self.rbf, (R,))
+            self.gbuf = _policy_grad_buffers(g, self.ro.pol, self.rbf, (R,) if self.sch is None else (R, self.H))
             self.gbuf["m0"] = torch.empty((R, Ds), dtype=F64, device=d)
             self.gbuf["S0"] = torch.empty((R, Ds, Ds), dtype=F64, device=d)
             g.gm0, g.gS0 = self.gbuf["m0"].data_ptr(), self.gbuf["S0"].data_ptr()
-            wsb = lib.pilco_rollout_noisy_bwd_workspace_bytes(C.byref(self.ro), self._ang_ref(), self._ex_ref(),
-                                                              self._nz_ref())
+            wsb = self._call("bwd_workspace_bytes", self.ro)
             self.bws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             g.ws, g.ws_bytes = self.bws.data_ptr(), wsb
             self.grad = g
-        check(lib.pilco_rollout_noisy_backward(C.byref(self.ro), self._ang_ref(), self._ex_ref(), self._nz_ref(),
-                                               C.byref(self.grad), stream_ptr()), "rollout_noisy_backward")
+        check(self._call("backward", self.ro, C.byref(self.grad), stream_ptr()),
+              "rollout_noisy_backward" if self.sch is None else "rollout_scheduled_backward")
         return self.gbuf
 
 
@@ -752,6 +797,7 @@ class ParticlePlan:
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
                  estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False):
+        _no_schedule(policy_spec, "ParticlePlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         self.resample = bool(resample)
@@ -954,6 +1000,7 @@ class ConsistentGradPlan(ParticlePlan):
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
                  measurement_noise=None, exploration=None, estimator="pathwise"):
+        _no_schedule(policy_spec, "ConsistentGradPlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         if exploration is not None and estimator == "score":
@@ -1111,6 +1158,7 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     ``resample=True``: the Gaussian refit at every step, as ``ParticlePlan(resample=True)``; ``xi`` [P,H,Ds] are the
     redraw's standard normals (required with it, and only then).  The result then also has the fitted moments:
     (traj, act, step_reward, step_risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds])."""
+    _no_schedule(policy_spec, "particles_rollout")
     if resample:
         _resample_check(x0.shape[0], consistent, "pathwise", angles, measurement_noise, None)
     if (xi is None) == bool(resample):
@@ -1199,8 +1247,10 @@ class PredictPlan:
     moments + reward + status -> pinned host memory.  Built once per (model, policy, reward, n) state by
     ``PILCO`` and replayed for every call with new initial moments (pilco/models/pilco.py:118-136)."""
 
-    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0, angles=None, measurement_noise=None):
-        """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``, ``measurement_noise``: as RolloutPlan."""
+    def __init__(self, dyn, policy_spec, reward_terms, Ds, n, mult_mu=0.0, angles=None, measurement_noise=None,
+                 schedule=False):
+        """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``, ``measurement_noise``, ``schedule``: as
+        RolloutPlan."""
         d = device()
         self.Ds, self.n = int(Ds), int(n)
         Ds = self.Ds
@@ -1209,7 +1259,7 @@ class PredictPlan:
         self.d_in = torch.zeros(Ds + Ds * Ds, dtype=F64, device=d)
         self.d_out = torch.zeros(Ds + Ds * Ds + 2, dtype=F64, device=d)
         self.plan = RolloutPlan(dyn, policy_spec, reward_terms, np.zeros(Ds), np.eye(Ds), self.n, R=1, mult_mu=mult_mu,
-                                angles=angles, measurement_noise=measurement_noise)
+                                angles=angles, measurement_noise=measurement_noise, schedule=schedule)
         self._enqueue()                                    # eager warm-up (one-time kernel attributes)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()

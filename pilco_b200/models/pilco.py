@@ -46,8 +46,8 @@ def _sqrt_factor(S):
 def _controller_input_dim(c):
     if isinstance(c, controllers.RbfController):
         return int(c.policy_shapes[1])
-    if isinstance(c, controllers.LinearController):
-        return int(np.asarray(c.W).shape[1])
+    if isinstance(c, (controllers.LinearController, controllers.TimeVaryingLinearController)):
+        return int(np.asarray(c.W).shape[-1])
     return None
 
 
@@ -164,6 +164,23 @@ class PILCO:
         """New raw data (X = [x, u], Y = delta x) for the dynamics GPs; with angle_dims, phi is applied to x."""
         self.mgpr.set_data(self._model_data(data))
 
+    # ---- time-varying linear policy (receding-horizon planning) ------------------------------------
+    def _scheduled(self, n=None):
+        """True for a TimeVaryingLinearController (the rollouts take schedule=True); an n-step rollout beyond its
+        horizon is a ValueError"""
+        c = self.controller
+        if not isinstance(c, controllers.TimeVaryingLinearController):
+            return False
+        if n is not None and int(n) > c.horizon:
+            raise ValueError("a rollout of n=%d steps runs beyond the TimeVaryingLinearController's horizon of %d steps"
+                             % (int(n), c.horizon))
+        return True
+
+    def _no_schedule(self, what):
+        if isinstance(self.controller, controllers.TimeVaryingLinearController):
+            raise ValueError("%s: the particle rollouts do not support the TimeVaryingLinearController; use the "
+                             "moment-matching methods (predict, policy_gradient, optimize_policy, plan)" % what)
+
     def _no_angles(self, what):
         if self.angle_dims:
             raise ValueError("%s: the particle rollouts do not support angle_dims yet; use the moment-matching methods "
@@ -178,7 +195,7 @@ class PILCO:
     def policy_spec(self, flats=None):
         """Description of the policy for ``RolloutPlan``; ``flats`` [R,P] = per-restart flat parameters."""
         c = self.controller
-        if isinstance(c, controllers.LinearController):
+        if isinstance(c, (controllers.LinearController, controllers.TimeVaryingLinearController)):
             return c.policy_spec(flats)
         if isinstance(c, controllers.RbfController):
             bf, Ds, U = c.policy_shapes
@@ -207,7 +224,7 @@ class PILCO:
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(flats), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1),
                                   np.asarray(s_x, dtype=np.float64), int(n), R=R, mult_mu=mult_mu, angles=self.angle_dims,
-                                  measurement_noise=self._noise_var())
+                                  measurement_noise=self._noise_var(), schedule=self._scheduled(n))
 
     def _reward_key(self):
         terms, mult_mu = self.reward_spec()
@@ -222,6 +239,7 @@ class PILCO:
         """Captured n-step cascade, cached per (model, policy, reward, n) state: the reference rebuilds nothing
         between calls either (tf.function), but here the cache is explicit -- any change of data, hyper-parameters,
         policy parameters or reward parameters changes the key and rebuilds the plan (a few ms)."""
+        sched = self._scheduled(n)
         dyn = self.mgpr.device_gp()                       # (re)factorises only when data / hypers changed
         v = self._noise_var()
         key = (id(dyn), self.mgpr._cache_key, self.controller.state_key(), self._reward_key(), int(n),
@@ -231,7 +249,7 @@ class PILCO:
         if hit is None or hit[0] != key:
             terms, mult_mu = self.reward_spec()
             plan = engine.PredictPlan(dyn, self.policy_spec(), terms, self.state_dim, int(n), mult_mu=mult_mu,
-                                      angles=self.angle_dims, measurement_noise=v)
+                                      angles=self.angle_dims, measurement_noise=v, schedule=sched)
             if len(cache) >= 8:
                 cache.clear()
             cache[int(n)] = hit = (key, plan)
@@ -272,6 +290,7 @@ class PILCO:
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
         from ..params import HostArray
+        self._no_schedule("sample_trajectories")
         self._no_angles("sample_trajectories")
         self._no_noise("sample_trajectories")
         _resample_refusals("sample_trajectories", resample, consistent)
@@ -337,6 +356,8 @@ class PILCO:
         """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
         derivative of the softplus transform, sigmoid(theta), as policy_opt applies it"""
         c = self.controller
+        if isinstance(c, controllers.TimeVaryingLinearController):
+            return c.flat_grad(g["W"].cpu().numpy(), g["b"].cpu().numpy())
         if isinstance(c, controllers.LinearController):
             return np.concatenate([g["W"].cpu().numpy().ravel(), g["b"].cpu().numpy().ravel()])
         bf, Ds, U = c.policy_shapes
@@ -355,6 +376,7 @@ class PILCO:
         resample=True)``.  Needs num_samples >= 2; a reward with an additive box term is a ValueError.  -> (mean [n],
         var [n]) host arrays."""
         from ..params import HostArray
+        self._no_schedule("sample_reward_moments")
         self._no_angles("sample_reward_moments")
         self._no_noise("sample_reward_moments")
         _resample_refusals("sample_reward_moments", resample, consistent)
@@ -406,6 +428,7 @@ class PILCO:
 
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
+        self._no_schedule("sample_policy_gradient")
         self._no_angles("sample_policy_gradient")
         self._no_noise("sample_policy_gradient")
         if estimator not in engine.ParticlePlan.ESTIMATORS:
@@ -435,7 +458,8 @@ class PILCO:
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(), terms,
                                   np.asarray(m_x, dtype=np.float64).reshape(-1), np.asarray(s_x, dtype=np.float64),
                                   int(n), R=1, mult_mu=mult_mu, grad=grad, angles=self.angle_dims,
-                                  exploration=exploration, measurement_noise=self._noise_var())
+                                  exploration=exploration, measurement_noise=self._noise_var(),
+                                  schedule=self._scheduled(n))
 
     def predict_reward_moments(self, m_x, s_x, n):
         """Mean and variance of each step's reward along the n-step prediction from N(m_x, s_x): E[r_t] (the terms
@@ -494,6 +518,7 @@ class PILCO:
         b != 0 it is a ValueError."""
         from functools import partial
         from .. import policy_opt
+        self._no_schedule("optimize_policy_sampled")
         self._no_angles("optimize_policy_sampled")
         self._no_noise("optimize_policy_sampled")
         if int(num_samples) < 1:
@@ -550,14 +575,24 @@ class PILCO:
     def maximum_log_likelihood_objective(self):
         return -self.training_loss()
 
-    def compute_action(self, x_m):
+    def compute_action(self, x_m, *, t=0):
         """pilco.py:115-116: the policy mean at a deterministic state (s = 0).  Served by a cached
         ``engine.ActionPlan`` (one captured CUDA graph per policy state) -- the per-control-step call of
-        examples/utils.py:32-36.  With angle_dims, x_m is the raw state and phi(x_m) is formed on the host."""
+        examples/utils.py:32-36.  With angle_dims, x_m is the raw state and phi(x_m) is formed on the host.
+        ``t``: the step whose parameters a TimeVaryingLinearController applies (0 .. horizon-1); a stationary policy
+        is the same at every step."""
         from ..params import HostArray
-        key = self.controller.state_key()
+        c = self.controller
+        sched = isinstance(c, controllers.TimeVaryingLinearController)
+        t = int(t) if sched else 0
+        if sched and not 0 <= t < c.horizon:
+            raise ValueError("compute_action: step t=%d outside the schedule's %d steps" % (t, c.horizon))
+        key = (c.state_key(), t)
         if key != getattr(self, "_act_key", None):
-            self._act_plan = engine.ActionPlan(self.policy_spec())
+            spec = self.policy_spec()
+            if sched:                                     # step t's (W_t, b_t) as a stationary linear policy
+                spec = dict(spec, W=spec["W"][t], b=spec["b"][t], schedule=False)
+            self._act_plan = engine.ActionPlan(spec)
             self._act_key = key
         if self.angle_dims:
             x_m = engine.trig_feature_map(np.asarray(x_m, dtype=np.float64).reshape(1, self.state_dim), self.angle_dims)
@@ -583,6 +618,7 @@ class PILCO:
     # ---- policy optimisation (pilco.py:75-113) --------------------------------------------------------
     def optimize_policy(self, maxiter=50, restarts=1):
         from .. import policy_opt
+        self._scheduled(self.horizon)
         start = time.time()
         mgpr_trainable = self.mgpr.trainable_parameters
         for p in mgpr_trainable:
@@ -597,3 +633,37 @@ class PILCO:
         for rwd in all_rewards:
             print("Controller's optimization: done in %.1f seconds with reward=%.3f." % (end - start, rwd))
         return best_reward
+
+    # ---- receding-horizon planning (probabilistic MPC, Kamthe & Deisenroth 2018) --------------------------------------
+    def plan(self, m_x, s_x=None, maxiter=20, restarts=1, warm_start=True):
+        """One receding-horizon step with a TimeVaryingLinearController: optimise its schedule over ``horizon`` steps
+        of the moment-matching cascade from N(m_x, s_x) (s_x = None or 0: a measured state), return the first action
+        u_0 = compute_action(m_x, t=0) [1,U], then shift the schedule one step (theta_t <- theta_{t+1}, the last step
+        repeated) so that the next call starts from the rest of this plan.  Restart 0 starts from the current schedule
+        (``warm_start=False``: from ``controller.randomize()``), the others from random draws, as ``optimize_policy``
+        chooses, batches and shards them; the objective is ``optimize_policy``'s (with ``exploration``).  m_init and
+        S_init are not touched.  A stationary controller is a TypeError."""
+        from functools import partial
+        from .. import policy_opt
+        c = self.controller
+        if not isinstance(c, controllers.TimeVaryingLinearController):
+            raise TypeError("plan: needs a TimeVaryingLinearController, the controller is a %s" % type(c).__name__)
+        self._scheduled(self.horizon)
+        Ds = self.state_dim
+        m = np.asarray(m_x, dtype=np.float64).reshape(1, Ds)
+        s = np.zeros((Ds, Ds)) if s_x is None else np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds)
+        if not warm_start:
+            c.randomize()
+        mgpr_trainable = self.mgpr.trainable_parameters
+        for p in mgpr_trainable:
+            set_trainable(p, False)
+        try:
+            best_flat, _, _ = policy_opt.optimize(self, maxiter=maxiter, restarts=restarts,
+                                                  evaluator=partial(policy_opt.PolicyEvaluator, m0=m, S0=s))
+            c.set_flat(best_flat)
+        finally:
+            for p in mgpr_trainable:
+                set_trainable(p, True)
+        u = self.compute_action(m, t=0)
+        c.shift()
+        return u

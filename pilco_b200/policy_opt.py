@@ -47,11 +47,12 @@ class _FlatEvaluator:
         self.pilco, self.R = pilco, R
         c = pilco.controller
         self.c = c
-        self.linear = isinstance(c, controllers.LinearController)
+        self.sched = isinstance(c, controllers.TimeVaryingLinearController)     # per-step W_t, b_t
+        self.linear = isinstance(c, controllers.LinearController) or self.sched
         self.flat0 = np.tile(c.get_flat(), (R, 1))
         self.P = self.flat0.shape[1]
         if self.linear:
-            U, Ds = c.W.shape
+            U, Ds = c.W.shape[-2:]
         else:
             bf, Ds, U = c.policy_shapes
             self.ell_lower = float(c.models[0].kernel.lengthscales.transform.lower)
@@ -117,6 +118,12 @@ class _FlatEvaluator:
         returns the lengthscales' unconstrained theta [R,U,Ds] (RBF) or None"""
         R = flat.shape[0]
         Ds, U = self.shape
+        if self.sched:                                         # W stays the spec's zeros without feedback
+            nW = self.c.horizon * U * Ds if self.c.feedback else 0
+            if nW:
+                plan.W.copy_(flat[:, :nW].reshape(plan.W.shape))
+            plan.b.copy_(flat[:, nW:].reshape(plan.b.shape))
+            return None
         if self.linear:
             plan.W.copy_(flat[:, :U * Ds].reshape(plan.W.shape))
             plan.b.copy_(flat[:, U * Ds:].reshape(plan.b.shape))
@@ -138,7 +145,15 @@ class _FlatEvaluator:
         Ds, U = self.shape
         out[:, 0] = -value
         out[:, 1] = info.to(torch.float64)
-        if self.linear:
+        if self.sched:                                         # steps 0 .. H-1 of the horizon's: the rest get 0
+            nW = self.c.horizon * U * Ds if self.c.feedback else 0
+            out[:, 2:] = 0.0
+            if nW:
+                gW = g["W"].reshape(R, -1)
+                out[:, 2:2 + gW.shape[1]] = -gW
+            gb = g["b"].reshape(R, -1)
+            out[:, 2 + nW:2 + nW + gb.shape[1]] = -gb
+        elif self.linear:
             out[:, 2:2 + U * Ds] = -g["W"].reshape(R, -1)
             out[:, 2 + U * Ds:] = -g["b"].reshape(R, -1)
         else:
@@ -158,7 +173,8 @@ class PolicyEvaluator(_FlatEvaluator):
 
     NSPLIT = 4
 
-    def __init__(self, pilco, R, nsplit=None):
+    def __init__(self, pilco, R, nsplit=None, m0=None, S0=None):
+        """``m0``, ``S0``: the initial state distribution (default pilco.m_init, pilco.S_init)"""
         super().__init__(pilco, R)
         c, flat0 = self.c, self.flat0
         terms, mult_mu = pilco.reward_spec()
@@ -170,14 +186,16 @@ class PolicyEvaluator(_FlatEvaluator):
         b = float(getattr(pilco, "exploration", 0.0))
         exploration = b if b != 0.0 else None                  # b = 0: the plans without exploration
         noise = pilco._noise_var() if hasattr(pilco, "_noise_var") else None
+        m0 = pilco.m_init if m0 is None else m0
+        S0 = pilco.S_init if S0 is None else S0
         for lo, hi in self.slices:
             spec = c.policy_spec(flat0[lo:hi]) if self.linear else pilco.policy_spec(flat0[lo:hi])
             self.gps.append(None if self.linear else spec["gp"])
-            self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(pilco.m_init, dtype=np.float64).reshape(-1),
-                                                 np.asarray(pilco.S_init, dtype=np.float64), int(pilco.horizon), R=hi - lo,
+            self.plans.append(engine.RolloutPlan(dyn, spec, terms, np.asarray(m0, dtype=np.float64).reshape(-1),
+                                                 np.asarray(S0, dtype=np.float64), int(pilco.horizon), R=hi - lo,
                                                  mult_mu=mult_mu, grad=True,
                                                  angles=getattr(pilco, "angle_dims", None), exploration=exploration,
-                                                 measurement_noise=noise))
+                                                 measurement_noise=noise, schedule=self.sched))
         self.side = [torch.cuda.Stream() for _ in self.plans[1:]]
         self._setup_io()
 
