@@ -1,6 +1,7 @@
 """Fake C-ABI descriptors for the tests that check argument validation without a GPU: the status codes of
 include/pilco_b200.h and builders of pilco_gp_model, pilco_rollout, pilco_particles (plain and with per-restart
-policies) and pilco_particles_grad whose pointers are fake non-null addresses.  Every entry point validates its
+policies, with angles or measurement noise) and pilco_particles_grad whose pointers are fake non-null addresses, a
+stand-in for a DeviceGP, and the rejected calls of the batched score gradient.  Every entry point validates its
 arguments on the host before it enqueues anything, so only calls that are rejected may be made with them."""
 from pilco_b200 import _lib
 
@@ -64,3 +65,88 @@ def _grad():
     g.gW = g.gb = g.gXc = g.gYc = g.gell = g.pol_L = g.value = g.ws = FAKE
     g.ws_bytes = 0
     return g
+
+
+def _angles(*dims):
+    a = _lib.Angles()
+    a.A = len(dims)
+    for i, d in enumerate(dims):
+        a.dims[i] = d
+    return a
+
+
+def _angle_particles(kind=_lib.POLICY_LINEAR, A=1, batched=False, **kw):
+    """_particles' description (E = 3 state dimensions, U = 1) with a policy of Dh = 3 + A inputs"""
+    pr = (_batched if batched else _particles)(kind, **kw)
+    pr.pol.Ds, pr.dyn.D = 3 + A, 3 + A + 1
+    if kind == _lib.POLICY_RBF:
+        pr.pol.rbf.D = 3 + A
+    return pr
+
+
+def _noise(var=(0.01, 0.02, 0.03), nu=FAKE):
+    n = _lib.ParticlesNoise()
+    for i, v in enumerate(var):
+        n.v.var[i] = v
+    n.nu = nu
+    return n
+
+
+class _FakeGP:
+    """stands in for a DeviceGP in the engine's checks before device work: struct() only"""
+    def __init__(self, n=40, D=6, E=4):
+        self.n, self.D, self.E = n, D, E
+
+    def struct(self):
+        g = _lib.GpModel()
+        g.n, g.D, g.E = self.n, self.D, self.E
+        return g
+
+
+def _score_grad_cases():
+    """(description, R, grad, expected status): every call is rejected before anything is enqueued"""
+    out = [(None, 3, _grad(), ERR_NULL), (_batched(), 3, None, ERR_NULL)]
+    for kind in (_lib.POLICY_LINEAR, _lib.POLICY_RBF):
+        for rk in (_lib.REWARD_EXP, _lib.REWARD_LINEAR, _lib.REWARD_BOX):
+            for ch in (_lib.CHANNEL_ADD, _lib.CHANNEL_MULT):
+                out.append((_batched(kind, reward_kind=rk, channel=ch), 3, _grad(), ERR_WS))
+        out.append((_particles(kind), 3, _grad(), ERR_WS))                 # stride 0: one policy shared by all
+        out.append((_particles(kind), 1, _grad(), ERR_WS))                 # R = 1, unbatched
+    out.append((_particles(H=0), 1, _grad(), ERR_WS))
+    out.append((_particles(H=1), 1, _grad(), ERR_WS))
+    for R in (0, -1, 65536):
+        out.append((_batched(), R, _grad(), ERR_DIM))
+    out.append((_batched(P=1000), PT_MAX_P // 1000 + 1, _grad(), ERR_DIM))
+    out.append((_batched(P=1), 65535, _grad(), ERR_WS))
+    for field in ("W_bs", "b_bs"):
+        pr = _batched(); setattr(pr.pol, field, -3)
+        out.append((pr, 3, _grad(), ERR_DIM))
+    for field in ("X_bs", "ell_bs", "sf2_bs", "beta_bs"):
+        pr = _batched(_lib.POLICY_RBF); setattr(pr.pol.rbf, field, -1)
+        out.append((pr, 3, _grad(), ERR_DIM))
+        pr = _batched(); setattr(pr.dyn, field, 7)                         # batched dynamics
+        out.append((pr, 3, _grad(), ERR_UNSUP))
+    for P, H in ((0, 5), (PT_MAX_P + 1, 5), (10, -1)):
+        out.append((_batched(P=P, H=H), 1, _grad(), ERR_DIM))
+    for field in ("x0", "eps", "traj", "act", "step_reward", "step_risk", "ret"):
+        pr = _batched(); setattr(pr, field, None)
+        out.append((pr, 3, _grad(), ERR_NULL))
+    pr = _batched(_lib.POLICY_RBF); pr.pol.rbf.mode = 0
+    out.append((pr, 3, _grad(), ERR_UNSUP))
+    pr = _batched(); pr.dyn.iK = None
+    out.append((pr, 3, _grad(), ERR_UNSUP))
+    out.append((_batched(kind=7), 3, _grad(), ERR_UNSUP))
+    pr = _batched(); pr.dyn.E = 4
+    out.append((pr, 3, _grad(), ERR_DIM))
+    pr = _batched(); pr.dyn.iK = FAKE + 8
+    out.append((pr, 3, _grad(), ERR_ALIGN))
+    for field in ("value", "ws", "gW", "gb"):
+        g = _grad(); setattr(g, field, None)
+        out.append((_batched(), 3, g, ERR_NULL))
+    for field in ("gXc", "gYc", "gell", "pol_L"):
+        g = _grad(); setattr(g, field, None)
+        out.append((_batched(_lib.POLICY_RBF), 3, g, ERR_NULL))
+        out.append((_batched(), 3, g, ERR_WS))                             # not needed by the linear policy
+    g = _grad(); g.ws = FAKE + 8; g.ws_bytes = 1 << 40
+    out.append((_batched(), 3, g, ERR_ALIGN))
+    return out

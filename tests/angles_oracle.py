@@ -1,7 +1,7 @@
-"""Torch statement of the moment-matching rollout with angular state dimensions (PILCO's gTrig stage in propagate.m):
-the feature map's moments written with the second moments e+- = exp(-(s_aa + s_bb +- 2 s_ab)/2) as in the PILCO
-papers (the device writes them with expm1), and the cascade of oracle/torch_port.py with that stage in front of the
-policy and the dynamics.  Autograd through it gives the reference gradients."""
+"""Torch statement of PILCO's gTrig stage in propagate.m, the moments of the angular feature map: written with the
+second moments e+- = exp(-(s_aa + s_bb +- 2 s_ab)/2) as in the PILCO papers (the device writes them with expm1).
+tests/action_reward_oracle.py puts it in front of the policy and the dynamics; autograd through it gives the
+reference gradients."""
 import torch
 
 F64 = torch.float64
@@ -63,33 +63,3 @@ def trig_moments(m, s, angle_dims):
         Ccols.append(col)
     C = torch.stack(Ccols, dim=1)
     return M, S, C
-
-
-def propagate(m_x, s_x, angle_dims, action_fn, dynamics_fn):
-    """one step: m_x [1,Ds], s_x [Ds,Ds] -> (next m [1,Ds], next s, joint m [1,D], joint s [D,D])"""
-    mh, Sh, Ch = trig_moments(m_x[0], s_x, angle_dims)
-    mh = mh[None]
-    m_u, s_u, c_xu = action_fn(mh, Sh)
-    m = torch.cat([mh, m_u], dim=1)
-    s1 = torch.cat([Sh, Sh @ c_xu], dim=1)
-    s2 = torch.cat([(Sh @ c_xu).T, s_u], dim=1)
-    s = torch.cat([s1, s2], dim=0)
-    M_dx, S_dx, C_dx = dynamics_fn(m, s)
-    Q = s_x @ Ch
-    cxx = torch.cat([Q, Q @ c_xu], dim=1)             # cov(x, [phi, u])
-    K = cxx @ C_dx
-    return M_dx + m_x, S_dx + s_x + K + K.T, m, s
-
-
-def predict(m_x, s_x, n, angle_dims, action_fn, dynamics_fn, reward_fn, joint_reward_fn=None):
-    """H-step cascade: returns (trajectory means [n+1,Ds], covariances [n+1,Ds,Ds], total reward)"""
-    total = torch.zeros((), dtype=F64)
-    ms, Ss = [m_x[0]], [s_x]
-    for _ in range(n):
-        r = reward_fn(m_x, s_x).reshape(())
-        m_x, s_x, mj, sj = propagate(m_x, s_x, angle_dims, action_fn, dynamics_fn)
-        if joint_reward_fn is not None:
-            r = r + joint_reward_fn(mj, sj).reshape(())
-        total = total + r
-        ms.append(m_x[0]); Ss.append(s_x)
-    return torch.stack(ms), torch.stack(Ss), total

@@ -2,8 +2,10 @@
 oracles' dicts), reward terms, initial states and normals, and small PILCO / SafePILCO objects.  Importing this module
 touches no device: the builders that factorise on the GPU do so when called."""
 import numpy as np
+import torch
 
 from pilco_b200 import engine, _lib
+import particle_grad_oracle as pgo
 from util import make_gp_problem, make_rollout_problem
 
 BOX2 = np.array([2, 1, 1.0, 0, 0.2, 0.9, 1, 0.1, 0.8])             # dims 0, 1 inside (low, high)
@@ -47,6 +49,48 @@ def _safe_pilco():
     X = np.random.RandomState(1).rand(30, 5); Y = 0.1 * X[:, :4]
     return SafePILCO((X, Y), controller=LinearController(4, 1), horizon=4, reward_add=LinearReward(4, np.ones(4)),
                      reward_mult=RiskOfCollision(4, [0.0, 0.1], [0.6, 0.9]), mu=-4.0)
+
+
+def _host_problem(E, A, U, seed, n=30):
+    """numpy factors of a small exact GP on [phi(x), u] (D = E + A + U inputs, E outputs)"""
+    rng = np.random.RandomState(seed)
+    D = E + A + U
+    Cx = rng.rand(n, D) * 2.0 - 1.0
+    Y = 0.1 * np.sin(2.0 * Cx).dot(rng.rand(D, E))
+    ell, sf2 = 0.7 + 0.5 * rng.rand(E, D), 0.02 * (1.0 + rng.rand(E))
+    iK, beta = [], []
+    for e in range(E):
+        d = (Cx[:, None] - Cx[None]) / ell[e]
+        K = sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) + 1e-3 * np.eye(n)
+        iK.append(np.linalg.inv(K)); beta.append(iK[-1] @ Y[:, e])
+    return dict(C=Cx, ell=ell, sf2=sf2, iK=np.stack(iK), beta=np.stack(beta)), rng
+
+
+def _joint_terms(E, A, U, other):
+    """an EXP_SA term on the first angle's (sin, cos) and a state EXP term on the raw dimension ``other``"""
+    Dh = E + A
+    W = np.zeros((Dh + U, Dh + U)); W[E - A, E - A] = W[E - A + 1, E - A + 1] = 1.0; W[Dh, Dh] = 0.1
+    t = np.zeros(Dh + U); t[E - A + 1] = -1.0
+    Ws = np.zeros((E, E)); Ws[other, other] = 2.0
+    return [dict(kind=_lib.REWARD_EXP_SA, coef=1.0, W=W, t=t),
+            dict(kind=_lib.REWARD_EXP, coef=0.5, W=Ws, t=0.3 * np.ones(E)),
+            dict(kind=_lib.REWARD_LINEAR, coef=0.2, channel=_lib.CHANNEL_MULT, W=np.eye(E)[other], t=None)]
+
+
+def _policy(kind, rng, U, Dh, squash=True):
+    if kind == "linear":
+        return dict(kind=_lib.POLICY_LINEAR, squash=squash, maxa=0.8 + rng.rand(U), W=0.5 * rng.randn(U, Dh),
+                    b=rng.randn(U))
+    bf = 8
+    return _rbf_point(dict(kind=_lib.POLICY_RBF, squash=squash, maxa=0.8 + rng.rand(U), Xc=rng.randn(bf, Dh),
+                           Yc=0.3 * rng.randn(bf, U), ell=1.0 + 0.2 * rng.rand(U, Dh), sf2=np.ones(U),
+                           sn2=1e-2 * np.ones(U)))
+
+
+def _rbf_point(pol):
+    """the numpy oracle's RBF policy (C, ell, sf2, beta) of pgo's parametrisation (Xc, Yc, ell, sf2, sn2)"""
+    beta = pgo.rbf_beta(pgo.T(pol["Xc"]), pgo.T(pol["Yc"]), pgo.T(pol["ell"]), pol["sf2"], pol["sn2"])
+    return dict(pol, C=pol["Xc"], beta=beta.detach().numpy())
 
 
 # ---- device problems --------------------------------------------------------------------------------------------------
@@ -186,3 +230,70 @@ def _pilco(kind, seed, **kw):
     ctrl = RbfController(3, 1, 10, max_action=1.2) if kind == "rbf" else LinearController(3, 1, max_action=1.0)
     pilco = PILCO((X[:60], Y[:60]), controller=ctrl, horizon=6, m_init=X[0:1, :3], S_init=0.05 * np.eye(3), **kw)
     return pilco, X, Y
+
+
+def _angle_terms(E, A, U, joint):
+    """state terms on the raw state (exp, linear, MULT box on dimension 0); with ``joint`` an EXP_SA term on the first
+    angle's (sin, cos) = (0, -1) and a LINEAR_SA term on the action"""
+    Dh, D = E + A, E + A + U
+    rng = np.random.RandomState(E + A)
+    terms = [dict(kind=_lib.REWARD_EXP, coef=1.0, W=0.5 * np.eye(E), t=0.2 * np.ones(E)),
+             dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=rng.randn(E), t=None),
+             dict(kind=_lib.REWARD_BOX, coef=0.2, channel=_lib.CHANNEL_MULT, W=np.array([1, 1, 1.0, 0, -0.5, 0.8]),
+                  t=None)]
+    if joint:
+        W = np.zeros((D, D)); k = E - A if A else 0                   # A = 0: on state dimensions 0, 1
+        W[k, k] = W[k + 1, k + 1] = 1.0; W[Dh, Dh] = 0.1
+        t = np.zeros(D); t[k + 1] = -1.0
+        terms += [dict(kind=_lib.REWARD_EXP_SA, coef=0.8, W=W, t=t),
+                  dict(kind=_lib.REWARD_LINEAR_SA, coef=-0.05, W=np.r_[np.zeros(Dh), np.ones(U)], t=None)]
+    return terms
+
+
+def _angle_case(E, dims, U=1, kind="linear", fitc=False, joint=False, n=150, R=1, seed=0):
+    """-> gp, spec (a leading R when R > 1), oracle policy dicts per restart, terms, A"""
+    A = len(dims)
+    Dh, D = E + A, E + A + U
+    X, Y, ell, sf2, sn2 = make_gp_problem(n, D, E, seed=seed + D)
+    X = 2.0 * X - 1.0
+    if fitc:
+        Z = np.random.RandomState(seed).rand(60, D) * 2.0 - 1.0
+        gp = engine.fitc_factorize(X, Z, 0.05 * Y, ell, 0.05 * sf2, 1e-3 * np.ones(E))
+    else:
+        gp = engine.gp_factorize(X, 0.05 * Y, ell, 0.05 * sf2, 1e-3 * np.ones(E))
+    rng = np.random.RandomState(seed + 7)
+    maxa = 0.8 + 0.4 * np.arange(U)
+    if kind == "linear":
+        W, b = 0.5 * rng.randn(R, U, Dh), rng.randn(R, U)
+        if R == 1:
+            spec, pol = _linear(W[0], b[0], maxa, True)
+            pols = [pol]
+        else:
+            spec = dict(kind=_lib.POLICY_LINEAR, Ds=Dh, U=U, squash=True, max_action=maxa, W=W, b=b)
+            pols = [_linear(W[r], b[r], maxa, True)[1] for r in range(R)]
+    else:
+        assert R == 1
+        spec, pol = _rbf(rng.rand(12, Dh) * 2.0 - 1.0, 0.3 * rng.randn(12, U), 1.0 + 0.2 * rng.rand(U, Dh), maxa)
+        pols = [pol]
+    return gp, spec, pols, _angle_terms(E, A, U, joint)
+
+
+def _box_case():
+    """SafePILCO-like: a linear policy, a linear additive reward and one box as the only MULT term"""
+    X, Y, ell, sf2, sn2 = make_gp_problem(100, 5, 4, seed=6)
+    gp = engine.gp_factorize(X, 0.1 * Y, ell, 0.1 * sf2, 1e-3 * np.ones(4))
+    rng = np.random.RandomState(48)
+    W, b = 0.5 * rng.randn(1, 4), rng.randn(1)
+    spec = dict(kind=_lib.POLICY_LINEAR, Ds=4, U=1, squash=True, max_action=np.array([1.3]), W=W, b=b)
+    terms = [dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=rng.randn(4), t=None),
+             dict(kind=_lib.REWARD_BOX, coef=1.0, channel=_lib.CHANNEL_MULT, W=BOX2, t=None)]
+    return gp, spec, terms, X[0, :4], 0.05 * np.eye(4), 6, -4.0
+
+
+def _seeded(P, H, Ds, m0, S0, seed):
+    d = engine.device()
+    gen = torch.Generator(device=d)
+    gen.manual_seed(seed)
+    F = engine.dev(np.linalg.cholesky(S0))
+    x0 = engine.dev(m0)[None] + torch.randn((P, Ds), dtype=engine.F64, device=d, generator=gen) @ F.T
+    return x0, torch.randn((P, H, Ds), dtype=engine.F64, device=d, generator=gen)

@@ -1,12 +1,21 @@
 """Torch statement of the particle rollouts' policy gradients for the tests: tests/particle_oracle.py transcribed to
-torch and differentiated w.r.t. the policy parameters at fixed x0 and eps.
+torch and differentiated w.r.t. the policy parameters at fixed x0 and eps, with the same optional features (angles
+``angle_dims``, measurement noise ``nu``, ``v``) and, for the pathwise gradients, the exploration bonus ``b``.
 
   * ``value_and_grad``: the step-wise sampler's pathwise gradient (pilco_particles_rollout_grad, DESIGN.md section 12);
   * ``consistent_value_and_grad``: the consistent sampler's (pilco_particles_rollout_consistent_grad, section 15), with
     the same pivot mask and the tau rule in reverse (a degenerate step's own noise is held constant), and the explicit
     numpy statement of its reverse steps 1-6 at a fixed input sequence (``reverse_steps``);
-  * ``score_grad``: the score-function gradient (pilco_particles_rollout_score_grad, section 16) plus the joint terms'
-    direct dependence on the policy (section 18).
+  * ``resampled_rollout``: the Gaussian-resampled sampler (pilco_particles_resampled_*, section 26), the step-wise
+    transition followed by the refit x_t = mu^_t + chol(S^_t) xi_{t-1} to the sample moments of the pre-fit particles;
+  * ``score_grad``: the score-function gradient (pilco_particles_rollout_score_grad, section 16, and over consistent
+    function samples with ``consistent``, section 25) plus the joint terms' direct dependence on the policy
+    (section 18).
+
+The three pathwise samplers share one step loop and differ only in their transition.  With ``b`` the value is
+PILCO's exploration objective (section 24), mean_p ret_p + b sum_t sigma_t with sigma_t^2 = sum_k c_k^2 Var_p[r_kpt]
+over the additive terms (unbiased variance), sigma_t = sqrt(sigma_t^2) if sigma_t^2 > 1e-12, else 0 (constant); at
+b = 0 the bonus is not added, so the graph is that of the call without it.
 
 The RBF policy's beta = (K + sn2 I)^-1 Yc goes through a Cholesky solve, so the gradient w.r.t. the centres, targets and
 lengthscales includes the factorisation, as the device's does.  Also the closed form of the predict VJP
@@ -19,6 +28,8 @@ import particle_oracle as po
 
 F64 = torch.float64
 T = lambda a: torch.as_tensor(np.asarray(a, dtype=np.float64))
+FLOOR = 1e-12           # the exploration bonus's floor on sigma_t^2
+CHOL_TAU = 1e-12        # the refit's degenerate-column rule (resample_math.cuh)
 
 
 def _se(Xs, C, ell, sf2):
@@ -73,6 +84,18 @@ def point_value(term, x, u):
         return z @ W.reshape(-1)
     d = z - T(term["t"]).reshape(1, -1)
     return torch.exp(-0.5 * torch.einsum("pi,ij,pj->p", d, W.reshape(d.shape[1], d.shape[1]), d))
+
+
+def feature_map_torch(x, angle_dims=None):
+    """particle_oracle.feature_map in torch (x [P,Ds]).  None or empty: x itself"""
+    if not angle_dims:
+        return x
+    dims = [int(a) for a in angle_dims]
+    keep = [j for j in range(x.shape[1]) if j not in dims]
+    parts = [x[:, keep]]
+    for a in dims:
+        parts += [torch.sin(x[:, a:a + 1]), torch.cos(x[:, a:a + 1])]
+    return torch.cat(parts, 1)
 
 
 def gp_latent(dyn, xt):
@@ -138,75 +161,226 @@ def _grads(value, prm):
     return {k: (np.zeros(prm[k].shape) if gi is None else gi.numpy()) for k, gi in zip(keys, g)}
 
 
-def _pathwise(pol, terms, x0, eps, mult_mu, transition):
-    """mean particle return and its gradient; ``transition([x, u], eps_t)`` -> (mean, var) of the step's increment"""
-    P, H, Ds = eps.shape
+def chol(S):
+    """the column-by-column factor of S's lower triangle (torch, differentiable); a column whose pivot d_j <=
+    CHOL_TAU S_jj (or S_jj <= 0) is zero, as in resample_math.cuh, so autograd differentiates the factor as executed"""
+    n = S.shape[0]
+    zero = S.new_zeros(())
+    L = [[zero] * n for _ in range(n)]
+    for j in range(n):
+        d = S[j, j]
+        for k in range(j):
+            d = d - L[j][k] * L[j][k]
+        sjj, dv = float(S[j, j].detach()), float(d.detach())
+        if not (sjj > 0.0 and dv > CHOL_TAU * sjj):
+            continue
+        piv = torch.sqrt(d)
+        L[j][j] = piv
+        for i in range(j + 1, n):
+            s = S[i, j]
+            for k in range(j):
+                s = s - L[i][k] * L[j][k]
+            L[i][j] = s / piv
+    return torch.stack([torch.stack(row) for row in L])
+
+
+def chol_np(S):
+    return chol(T(S)).numpy()
+
+
+def chol_bwd_np(S, Lb):
+    """d <Lb, chol(S)> / d S on S's lower triangle (its upper triangle is 0), by autograd"""
+    St = T(S).clone().requires_grad_()
+    L = chol(St)
+    if not L.requires_grad:
+        return np.zeros(St.shape)
+    g, = torch.autograd.grad((L * T(Lb)).sum(), St, allow_unused=True)
+    return np.zeros(St.shape) if g is None else np.tril(g.numpy())
+
+
+def _moments(x):
+    """the sample mean and unbiased covariance of the particles x [P,Ds]"""
+    m = x.mean(0)
+    c = x - m[None]
+    return m, c.T @ c / (x.shape[0] - 1)
+
+
+def step_var(terms, value):
+    """sigma_t^2 of one step: sum_k c_k^2 torch.var(r_k, unbiased=True) over the additive terms, in term order"""
+    var = torch.zeros((), dtype=F64)
+    for term in po.additive(terms):
+        c = float(term.get("coef", 1.0))
+        var = var + c * c * torch.var(value(term), unbiased=True)
+    return var
+
+
+def sigma(var):
+    """section 21's floor: sqrt above 1e-12, else a constant 0"""
+    return torch.sqrt(var) if float(var.detach()) > FLOOR else torch.zeros((), dtype=F64)
+
+
+def _step(act, terms, x, nu_t, sv, angle_dims, with_var=False):
+    """one step's work at the states x [P,Ds] (sv: the tensor sqrt(v), or None) -> (phi(x), u = pi(phi(z)), reward
+    [P], risk [P], and sigma_t^2 when ``with_var``, else None)"""
+    xf = feature_map_torch(x, angle_dims)
+    zf = xf if sv is None else feature_map_torch(po.measurement(x, nu_t, sv), angle_dims)
+    u = act(zf)
+    value = po.step_point(x, xf, u, point_value)
+    r, k = po.step_values(terms, value, torch.zeros(x.shape[0], dtype=F64))
+    return xf, u, r, k, (step_var(terms, value) if with_var else None)
+
+
+def _pathwise(pol, terms, x0, eps, mult_mu, transition, angle_dims=None, nu=None, v=None, b=None):
+    """the step loop: the mean particle return (plus b sum_t sigma_t with ``b``) and its gradient w.r.t. the policy
+    parameters; ``transition(x, [phi(x), u], eps_t)`` -> the next state.  -> (value, grads, dict(traj, act, rew, risk,
+    ret), with ``b`` also step_var [H])"""
+    P, H = eps.shape[:2]
+    sv = po._scale(v)
     prm, act = policy(pol)
     x, e = T(x0), T(eps)
-    rews, risks = [], []
-    for s in range(H):
-        u = act(x)
-        r, k = po.step_values(terms, lambda term: point_value(term, x, u), torch.zeros(P, dtype=F64))
-        rews.append(r); risks.append(k)
-        mean, var = transition(torch.cat([x, u], 1), e[:, s])
-        x = x + mean + torch.sqrt(var) * e[:, s]
-    stack = lambda v: torch.stack(v, 1) if H else torch.zeros((P, 0), dtype=F64)
-    value = po.particle_return(terms, stack(rews), stack(risks), mult_mu).mean()
-    return float(value.detach()), _grads(value, prm)
+    n, svt = (None, None) if sv is None else (T(nu), T(sv))
+    traj, acts, rews, risks, svar = [x], [], [], [], []
+    for t in range(H):
+        xf, u, r, k, var = _step(act, terms, x, None if n is None else n[:, t], svt, angle_dims, b is not None)
+        acts.append(u); rews.append(r); risks.append(k); svar.append(var)
+        x = transition(x, torch.cat([xf, u], 1), e[:, t])
+        traj.append(x)
+    stack = lambda w: torch.stack(w, 1) if H else torch.zeros((P, 0), dtype=F64)
+    rew, risk = stack(rews), stack(risks)
+    ret = po.particle_return(terms, rew, risk, mult_mu)
+    value = ret.mean()
+    if b and H:
+        bonus = torch.zeros((), dtype=F64)
+        for var in svar:
+            bonus = bonus + sigma(var)
+        value = value + b * bonus
+    nd = lambda w: w.detach().numpy()
+    hist = dict(traj=nd(torch.stack(traj, 1)), act=nd(torch.stack(acts, 1)) if H else np.zeros((P, 0, 0)),
+                rew=nd(rew), risk=nd(risk), ret=nd(ret))
+    if b is not None:
+        hist["step_var"] = np.array([float(var.detach()) for var in svar])
+    return float(value.detach()), _grads(value, prm), hist
 
 
-def value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.0):
-    """value = mean return of the step-wise sampler and its gradient w.r.t. the policy parameters at fixed x0, eps.
-    dyn = dict(C, ell, sf2, iK, beta) (numpy); pol as ``policy`` takes it.  -> (value, {'W','b'} or {'X','Y','ell'})"""
-    def transition(xt, e):
+def _stepwise(dyn):
+    """the step-wise sampler's transition: x + mu + sqrt(max(var, 0)) eps_t"""
+    def transition(x, xt, e):
         mu, var = gp_latent(dyn, xt)
-        return mu, torch.clamp(var, min=0.0)
-    return _pathwise(pol, terms, x0, eps, mult_mu, transition)
+        return x + mu + torch.sqrt(torch.clamp(var, min=0.0)) * e
+    return transition
 
 
-def consistent_value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.0, swap=False):
-    """``value_and_grad`` of the consistent sampler -> (value, grads, smallest kept pivot d2 / (TAU sf2))"""
+def value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.0, angle_dims=None, nu=None, v=None, b=None):
+    """value = mean return of the step-wise sampler and its gradient w.r.t. the policy parameters at fixed x0, eps (and
+    nu).  dyn = dict(C, ell, sf2, iK, beta) (numpy); pol as ``policy`` takes it.  -> (value, {'W','b'} or
+    {'X','Y','ell'}), with ``b`` also step_var [H]"""
+    value, grad, hist = _pathwise(pol, terms, x0, eps, mult_mu, _stepwise(dyn), angle_dims, nu, v, b)
+    return (value, grad) if b is None else (value, grad, hist["step_var"])
+
+
+def consistent_value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.0, swap=False, angle_dims=None, nu=None, v=None,
+                              b=None):
+    """``value_and_grad`` of the consistent sampler -> (value, grads, smallest kept pivot d2 / (TAU sf2)), with ``b``
+    also step_var [H]"""
     fs = TorchFunctionSample(dyn, swap)
-    return _pathwise(pol, terms, x0, eps, mult_mu, fs.step) + (fs.min_ratio,)
+
+    def transition(x, xt, e):
+        mean, var = fs.step(xt, e)
+        return x + mean + torch.sqrt(var) * e
+    value, grad, hist = _pathwise(pol, terms, x0, eps, mult_mu, transition, angle_dims, nu, v, b)
+    return (value, grad, fs.min_ratio) + (() if b is None else (hist["step_var"],))
 
 
-def score_grad(dyn, pol, terms, traj, eps, mult_mu=0.0, baseline=True, direct=True, transitions=True):
-    """The score-function gradient of the mean return over the rollout (traj [P,H+1,Ds], eps [P,H,Ds]; the device's,
-    or particle_oracle's), pol as ``policy`` takes it.  With ``transitions`` the surrogate
-
-        (1/P) sum_p sum_{t < H-1} w_pt log N(y_pt; mu(x~_t(theta)), var(x~_t(theta))),   y = mu(theta0) + s(theta0) eps
-
-    is differentiated with w (``weights``), x_t and y held fixed: its gradient at theta0 is that of
-    sum w (eps / s0 mu(theta) + (eps^2 - 1) / (2 var0) var(theta)) (0 where var0 <= 0), which is what is formed here.
-    With ``direct``, the joint terms' own dependence on the parameters through u_t = pi(x_t) at fixed states,
-    (1/P) sum_p sum_{t<H} a_kt v_k([x_pt, pi(x_pt)]), is added.  -> {'W','b'} or {'X','Y','ell'} numpy arrays"""
-    traj, eps = np.asarray(traj, dtype=np.float64), np.asarray(eps, dtype=np.float64)
+def resampled_rollout(dyn, pol, terms, x0, eps, xi, mult_mu=0.0):
+    """the step-wise sampler with the refit at every step t >= 1: x'_t = the step-wise transition of x_{t-1},
+    mu^_t, S^_t = the sample mean and unbiased covariance of x'_t, x_t = mu^_t + chol(S^_t) xi_{t-1}.  -> dict(traj
+    [P,H+1,Ds], act, rew, risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds], xp [H,P,Ds], value, grad) of one restart;
+    grad = d value / d the policy parameters, value = mean return, x0, eps and xi held fixed"""
     P, H, Ds = eps.shape
+    step, z = _stepwise(dyn), T(xi)
+    m, S = _moments(T(x0))
+    means, covs, xps = [m], [S], []
+
+    def transition(x, xt, e):
+        xp = step(x, xt, e)
+        m, S = _moments(xp)
+        means.append(m); covs.append(S); xps.append(xp)
+        return m[None] + z[:, len(xps) - 1] @ chol(S).T
+    value, grad, out = _pathwise(pol, terms, x0, eps, mult_mu, transition)
+    nd = lambda w: w.detach().numpy()
+    out.update(step_mean=nd(torch.stack(means)), step_cov=nd(torch.stack(covs)),
+               xp=nd(torch.stack(xps)) if H else np.zeros((0, P, Ds)), value=value, grad=grad)
+    return out
+
+
+def _log_density(dyn, xt, e):
+    """the step-wise transition's score term at [phi(x_t), u_t]: a mu + b var, whose gradient at theta0 is that of
+    log N(y; mu(theta), var(theta)) with y = mu(theta0) + s(theta0) eps held fixed (0 where var0 <= 0)"""
+    mu, var = gp_latent(dyn, xt)
+    v0 = var.detach()
+    pos = v0 > 0.0
+    safe = torch.where(pos, v0, torch.ones_like(v0))
+    a = torch.where(pos, e / torch.sqrt(safe), torch.zeros_like(v0))
+    b = torch.where(pos, (e * e - 1.0) / (2.0 * safe), torch.zeros_like(v0))
+    return a * mu + b * var
+
+
+def _whitened(fs, xt, e, f):
+    """the consistent transition's score term: -eps_t(theta)^2 / 2 - log piv_t(theta) with eps_t(theta) = (f_t -
+    mean'_t(theta)) / piv_t(theta), f_t = x_{t+1} - x_t held fixed; eps_t(theta) takes the caller's eps_t as its value
+    and the residual's derivative, so the rounding of f_t does not enter.  A masked step drops its term and keeps the
+    caller's eps_t, which is what the later steps' mean' reads"""
+    mean, _ = fs.step(xt, e)
+    piv = fs.piv[-1]
+    on = piv > 0.0
+    safe = torch.where(on, piv, torch.ones_like(piv))
+    r = (f - mean) / safe
+    et = torch.where(on, e + (r - r.detach()), e)
+    fs.eps[-1] = et
+    return torch.where(on, -0.5 * et * et - torch.log(safe), torch.zeros_like(et))
+
+
+def score_grad(dyn, pol, terms, traj, eps, mult_mu=0.0, baseline=True, direct=True, transitions=True, angle_dims=None,
+               nu=None, v=None, w=None, consistent=False, swap=False):
+    """The score-function gradient of the mean return over the rollout (traj [P,H+1,Ds], eps [P,H,Ds], nu [P,H,Ds]; the
+    device's, or particle_oracle's), pol as ``policy`` takes it, with x_t and nu held fixed and theta entering through
+    u_t = pi(phi(z_t)) inside every x~_t = [phi(x_t), u_t].  With ``transitions`` the surrogate
+
+        (1/P) sum_p sum_{t < H-1} w_pt s_pt(theta)
+
+    is differentiated, s_pt the transition's log-density (step-wise sampler, ``_log_density``) or, with ``consistent``,
+    the whitened log-density of the particle's function sample (``_whitened``, the factor rows and pivots of
+    TorchFunctionSample with its tau mask).  w is ``weights`` (or the caller's ``w`` [P,H-1]).  With ``direct``, the
+    joint terms' own dependence on the parameters through u_t at fixed states, (1/P) sum_p sum_{t<H} a_kt
+    v_k([phi(x_pt), u_pt]), is added.  -> {'W','b'} or {'X','Y','ell'} numpy arrays; with ``consistent`` also the
+    smallest kept pivot d2 / (TAU sf2) of the steps t < H-1"""
+    traj, eps = np.asarray(traj, dtype=np.float64), np.asarray(eps, dtype=np.float64)
+    P, H = eps.shape[:2]
+    sv = po._scale(v)
     prm, act = policy(pol)
     if H == 0:
-        return _grads(torch.zeros(()), prm)
-    xs = [T(traj[:, s]) for s in range(H)]
-    us = [act(x) for x in xs]
-    rew, risk = po.path_rewards(terms, traj, np.stack([u.detach().numpy() for u in us], 1))
-    G = po.weights(terms, rew, risk, mult_mu, baseline)
+        g = _grads(torch.zeros(()), prm)
+        return (g, np.inf) if consistent else g
+    steps = [_step(act, terms, T(traj[:, s]), None if sv is None else T(nu[:, s]), None if sv is None else T(sv),
+                   angle_dims) for s in range(H)]
+    rew, risk = po.path_rewards(terms, traj, np.stack([st[1].detach().numpy() for st in steps], 1), angle_dims)
+    G = po.weights(terms, rew, risk, mult_mu, baseline) if w is None else np.asarray(w, dtype=np.float64)
     mult = any(po.is_mult(t) for t in terms)
+    fs = TorchFunctionSample(dyn, swap) if consistent else None
     sur = torch.zeros((), dtype=F64)
-    for s, (x, u) in enumerate(zip(xs, us)):
+    for s, (x, u) in enumerate(st[:2] for st in steps):
         if transitions and s < H - 1:
-            mu, var = gp_latent(dyn, torch.cat([x, u], 1))
-            v0, e = var.detach(), T(eps[:, s])
-            pos = v0 > 0.0
-            safe = torch.where(pos, v0, torch.ones_like(v0))
-            a = torch.where(pos, e / torch.sqrt(safe), torch.zeros_like(v0))
-            b = torch.where(pos, (e * e - 1.0) / (2.0 * safe), torch.zeros_like(v0))
-            sur = sur + (T(G[:, s])[:, None] * (a * mu + b * var)).sum()
+            xt, e = torch.cat([x, u], 1), T(eps[:, s])
+            term = _whitened(fs, xt, e, T(traj[:, s + 1] - traj[:, s])) if consistent else _log_density(dyn, xt, e)
+            sur = sur + (T(G[:, s])[:, None] * term).sum()
         if direct:
             wm = mult_mu * np.prod(np.delete(1.0 - risk, s, axis=1), axis=1) if mult else np.zeros(P)
             for term in terms:
                 if po.is_joint(term):
-                    w = float(term.get("coef", 1.0)) * (T(wm) if po.is_mult(term) else 1.0)
-                    sur = sur + (w * point_value(term, x, u)).sum()
-    return _grads(sur / P, prm)
+                    c = float(term.get("coef", 1.0)) * (T(wm) if po.is_mult(term) else 1.0)
+                    sur = sur + (c * point_value(term, x, u)).sum()
+    g = _grads(sur / P, prm)
+    return (g, fs.min_ratio) if consistent else g
 
 
 def fixed_inputs_objective(dyn, Xs, eps, mbar, vbar):

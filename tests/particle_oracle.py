@@ -9,10 +9,21 @@ or RBF policy, with the reward terms evaluated at each particle's pre-step state
     k_post(a, b) = k_e(a, b) - k(a, C) iK_e k(C, b), sampled sequentially along the particle's own inputs with the
     semidefinite Cholesky rule (a pivot d2 <= TAU sf2_e leaves its column out of later substitutions).
 
+Both take the optional features of the device's particle paths:
+
+  * ``angle_dims`` (DESIGN.md section 20): the feature map
+        phi(x) = [x_j, j not an angle, increasing j] ++ [sin x_a, cos x_a for a in angle_dims order]
+    where the policy, the transition and the joint terms read the state; the state, the state terms and the GP's
+    outputs stay raw.  phi is written here, independently of the engine's;
+  * ``nu``, ``v`` (DESIGN.md section 23): the policy reads the measurement z_t = x_t + sqrt(v) o nu_t (nu [P,H,Ds]
+    standard normals, v [Ds] variances), u_t = pi(phi(z_t)), while the transition reads [phi(x_t), u_t].
+
+Without them (None, empty, or v all zero) the policy reads x_t itself and every output is that of the plain rollout.
 State terms (REWARD_EXP / LINEAR / BOX) see x_t, joint terms (REWARD_EXP_SA / LINEAR_SA, DESIGN.md section 18) see
-[x_t, u_t]; within a step the state terms are added first, then the joint terms, each in term order, as on the device.
-Also the score estimator's return-to-go weights (DESIGN.md section 16).  Test infrastructure only; vectorised over
-particles and outputs."""
+[phi(x_t), u_t]; within a step the state terms are added first, then the joint terms, each in term order, as on the
+device.  Also the sample moments of the step rewards (the exploration objective, DESIGN.md section 24) and the score
+estimator's return-to-go weights (DESIGN.md section 16).  Test infrastructure only; vectorised over particles and
+outputs."""
 import numpy as np
 
 from pilco_b200 import _lib
@@ -62,6 +73,31 @@ def policy_action(pol, x):
     return u
 
 
+def feature_map(x, angle_dims=None):
+    """phi(x) along the last axis.  None or empty: x itself (the same object)"""
+    if not angle_dims:
+        return x
+    dims = [int(a) for a in angle_dims]
+    keep = [j for j in range(x.shape[-1]) if j not in dims]
+    parts = [x[..., keep]]
+    for a in dims:
+        parts += [np.sin(x[..., a:a + 1]), np.cos(x[..., a:a + 1])]
+    return np.concatenate(parts, -1)
+
+
+def _scale(v):
+    """sqrt(v) [Ds], or None for no measurement noise (v None or all zero)"""
+    if v is None:
+        return None
+    v = np.asarray(v, dtype=np.float64).reshape(-1)
+    return np.sqrt(v) if np.any(v != 0.0) else None
+
+
+def measurement(x, nu_t, sv):
+    """z = x + sqrt(v) o nu (numpy, or torch with sv a tensor); x itself (the same object) when sv is None"""
+    return x if sv is None else x + sv[None] * nu_t
+
+
 def box_point(prm, x):
     nd, inside = int(prm[0]), prm[1] != 0.0
     ok = np.ones(x.shape[0], dtype=bool)
@@ -83,11 +119,21 @@ def point_value(term, x, u=None):
     return np.exp(-0.5 * np.einsum("pi,ij,pj->p", d, W.reshape(d.shape[1], d.shape[1]), d))
 
 
+def in_step_order(terms):
+    """the terms in the device's order within a step: state terms first, then joint terms, each in term order"""
+    return [t for t in terms if not is_joint(t)] + [t for t in terms if is_joint(t)]
+
+
+def additive(terms):
+    """the ADD-channel terms that have a variance (not box), in term order"""
+    return [t for t in terms if not is_mult(t) and t["kind"] != _lib.REWARD_BOX]
+
+
 def step_values(terms, value, zero):
-    """(reward, risk) of one step: the sum of coef * value(term) over each channel's terms from ``zero``, state terms
-    first, then joint terms, each in term order.  Numpy or torch: ``value`` and ``zero`` decide."""
+    """(reward, risk) of one step: the sum of coef * value(term) over each channel's terms from ``zero``, in
+    ``in_step_order``.  Numpy or torch: ``value`` and ``zero`` decide."""
     rew = risk = zero
-    for term in [t for t in terms if not is_joint(t)] + [t for t in terms if is_joint(t)]:
+    for term in in_step_order(terms):
         v = float(term.get("coef", 1.0)) * value(term)
         if is_mult(term):
             risk = risk + v
@@ -96,13 +142,35 @@ def step_values(terms, value, zero):
     return rew, risk
 
 
-def path_rewards(terms, traj, act):
+def step_point(x, xf, u, point_value=point_value):
+    """term -> its value at one step: a state term at the raw x, a joint term at [xf, u] (xf = phi(x))"""
+    return lambda term: point_value(term, xf if is_joint(term) else x, u)
+
+
+def path_rewards(terms, traj, act, angle_dims=None):
     """step_reward, step_risk [P,H] of the terms at the states traj[:, t] and actions act[:, t] of every step t < H"""
     P, H = act.shape[:2]
     rew, risk = np.zeros((P, H)), np.zeros((P, H))
     for t in range(H):
-        rew[:, t], risk[:, t] = step_values(terms, lambda term: point_value(term, traj[:, t], act[:, t]), np.zeros(P))
+        x = traj[:, t]
+        rew[:, t], risk[:, t] = step_values(terms, step_point(x, feature_map(x, angle_dims), act[:, t]), np.zeros(P))
     return rew, risk
+
+
+def sample_moments(terms, traj, act, angle_dims=None):
+    """(mean [H], var [H]) of the step rewards over the particles of traj [P,H+1,Ds], act [P,H,U]: mean_t =
+    sum_k c_k mean_p r_kpt and var_t = sum_k c_k^2 Var_p[r_kpt] (ddof 1) over the ``additive`` terms"""
+    H = act.shape[1]
+    mean, var = np.zeros(H), np.zeros(H)
+    for t in range(H):
+        x = traj[:, t]
+        value = step_point(x, feature_map(x, angle_dims), act[:, t])
+        for term in additive(terms):
+            c = float(term.get("coef", 1.0))
+            r = value(term)
+            mean[t] += c * r.mean()
+            var[t] += c * c * r.var(ddof=1)
+    return mean, var
 
 
 def particle_return(terms, rew, risk, mult_mu):
@@ -114,34 +182,37 @@ def particle_return(terms, rew, risk, mult_mu):
     return ret
 
 
-def _rollout(pol, terms, x0, eps, mult_mu, transition):
-    """the step loop: ``transition(x, [x, u], eps_t)`` -> the next state"""
-    P, H, Ds = eps.shape
+def _rollout(pol, terms, x0, eps, mult_mu, transition, angle_dims=None, nu=None, v=None):
+    """the step loop: u_t = pi(phi(z_t)), ``transition(x, [phi(x), u], eps_t)`` -> the next state"""
+    P, H = eps.shape[:2]
+    sv = _scale(v)
     x = np.asarray(x0, dtype=np.float64).copy()
     traj, act = [x], []
     for t in range(H):
-        u = policy_action(pol, x)
-        x = transition(x, np.hstack([x, u]), eps[:, t])
+        xf = feature_map(x, angle_dims)
+        zf = xf if sv is None else feature_map(measurement(x, nu[:, t], sv), angle_dims)
+        u = policy_action(pol, zf)
+        x = transition(x, np.hstack([xf, u]), eps[:, t])
         traj.append(x); act.append(u)
     traj, act = np.stack(traj, 1), np.stack(act, 1) if H else np.zeros((P, 0, 0))
-    rew, risk = path_rewards(terms, traj, act)
+    rew, risk = path_rewards(terms, traj, act, angle_dims)
     return traj, act, rew, risk, particle_return(terms, rew, risk, mult_mu)
 
 
-def particle_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0):
+def particle_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0, angle_dims=None, nu=None, v=None):
     """-> traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P] of the step-wise sampler"""
     def transition(x, xt, e):
         mu, var = gp_latent(dyn, xt)
         return x + mu + np.sqrt(np.maximum(var, 0.0)) * e
-    return _rollout(pol, terms, x0, eps, mult_mu, transition)
+    return _rollout(pol, terms, x0, eps, mult_mu, transition, angle_dims, nu, v)
 
 
-def consistent_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0, swap=False):
+def consistent_rollout(dyn, pol, terms, x0, eps, mult_mu=0.0, swap=False, angle_dims=None, nu=None, v=None):
     """-> traj, act, step_reward, step_risk, ret of the consistent sampler (eps[:, t] is the step-t normal of every
-    output).  ``swap`` reorders the posterior's sums: the difference of the two is the sampler's own sensitivity to
-    rounding"""
+    output; the draw conditions on the particle's earlier [phi(x), u]).  ``swap`` reorders the posterior's sums: the
+    difference of the two is the sampler's own sensitivity to rounding"""
     fs = FunctionSample(dyn, eps.shape[0], swap)
-    return _rollout(pol, terms, x0, eps, mult_mu, lambda x, xt, e: x + fs.step(xt, e))
+    return _rollout(pol, terms, x0, eps, mult_mu, lambda x, xt, e: x + fs.step(xt, e), angle_dims, nu, v)
 
 
 def _posterior(dyn, A, B):

@@ -106,8 +106,8 @@ def _small_problem(seed=3):
 
 
 def _mm_value(P, terms, W, b, H=3, mu=1.5):
-    return aro.mm_problem_rollout("linear", (W, b), P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
-                                  P["m0"], P["S0"], H, mult_mu=mu)
+    return aro.problem_rollout("linear", (W, b), P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
+                               P["m0"], P["S0"], H, mult_mu=mu)
 
 
 def test_moment_oracle_gradient_against_central_differences():

@@ -11,69 +11,15 @@ import torch
 
 from abi_fakes import ERR_DIM, ERR_NULL, FAKE, _rollout
 import angles_oracle as ao
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-dp = ctypes.POINTER(ctypes.c_double)
+from util import ROOT, TRIG_CASES, host_moments, host_vjp, trig_harness
 
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("trig") / "trig_harness.so")
-    subprocess.check_call(["g++", "-O1", "-shared", "-fPIC", "-x", "c++", "-o", so,
-                           os.path.join(ROOT, "tests", "host_harness", "trig_harness.cpp")])
-    lib = ctypes.CDLL(so)
-    ip = ctypes.POINTER(ctypes.c_int)
-    lib.trig_moments_host.argtypes = [ctypes.c_int, ctypes.c_int, ip] + [dp] * 5
-    lib.trig_vjp_host.argtypes = [ctypes.c_int, ctypes.c_int, ip] + [dp] * 7
-    lib.angles_layout.argtypes = [ctypes.POINTER(ctypes.c_size_t)]
-    return lib
+    return trig_harness(str(tmp_path_factory.mktemp("trig") / "trig_harness.so"))
 
 
-def _p(a):
-    return np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(dp)
-
-
-def host_moments(lib, m, s, dims):
-    Ds, A = len(m), len(dims)
-    Dh = Ds + A
-    M, S, C = np.zeros(Dh), np.zeros((Dh, Dh)), np.zeros((Ds, Dh))
-    m, s = np.ascontiguousarray(m, dtype=np.float64), np.ascontiguousarray(s, dtype=np.float64)
-    d = (ctypes.c_int * max(A, 1))(*dims)
-    assert lib.trig_moments_host(Ds, A, d, _p(m), _p(s), M.ctypes.data_as(dp), S.ctypes.data_as(dp),
-                                 C.ctypes.data_as(dp)) == 0
-    return M, S, C
-
-
-def host_vjp(lib, m, s, dims, gM, gS, gC):
-    Ds, A = len(m), len(dims)
-    gm, gs = np.zeros(Ds), np.zeros((Ds, Ds))
-    arrs = [np.ascontiguousarray(a, dtype=np.float64) for a in (m, s, gM, gS, gC)]
-    d = (ctypes.c_int * max(A, 1))(*dims)
-    assert lib.trig_vjp_host(Ds, A, d, *[a.ctypes.data_as(dp) for a in arrs], gm.ctypes.data_as(dp),
-                             gs.ctypes.data_as(dp)) == 0
-    return gm, gs
-
-
-def _cases():
-    rng = np.random.RandomState(7)
-    out = []
-    for Ds, dims in ((2, [0]), (4, [2]), (4, [1, 3]), (3, [2, 0, 1]), (6, [4, 1])):
-        B = rng.randn(Ds, Ds)
-        out.append(("random", rng.randn(Ds) * 2, 0.3 * B @ B.T, dims))
-    out.append(("zero_cov", np.array([0.3, -2.0, 1.1]), np.zeros((3, 3)), [1, 2]))
-    s = np.diag([0.2, 10.0, 0.5]); s[0, 2] = s[2, 0] = 0.1
-    out.append(("saa_10", np.array([0.5, 1.0, -0.7]), s, [1]))
-    L = np.array([[1.0, 0.0, 0.0], [0.999, 0.0447, 0.0], [0.2, 0.1, 0.5]])
-    out.append(("correlated_angles", np.array([0.4, -1.3, 0.2]), 0.8 * L @ L.T, [0, 1]))
-    v = rng.randn(4)
-    out.append(("singular", rng.randn(4), np.outer(v, v), [0, 3]))
-    return out
-
-
-CASES = _cases()
-
-
-@pytest.mark.parametrize("name,m,s,dims", CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(CASES)])
+@pytest.mark.parametrize("name,m,s,dims", TRIG_CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(TRIG_CASES)])
 def test_trig_moments_match_monte_carlo(harness, name, m, s, dims):
     M, S, C = host_moments(harness, m, s, dims)
     rng = np.random.RandomState(11)
@@ -97,7 +43,7 @@ def test_trig_moments_match_monte_carlo(harness, name, m, s, dims):
     assert np.all(np.abs(s @ C - cross.mean(0)) <= 5 * se_C + 1e-9), name
 
 
-@pytest.mark.parametrize("name,m,s,dims", CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(CASES)])
+@pytest.mark.parametrize("name,m,s,dims", TRIG_CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(TRIG_CASES)])
 def test_trig_moments_match_torch_oracle(harness, name, m, s, dims):
     M, S, C = host_moments(harness, m, s, dims)
     Mt, St, Ct = ao.trig_moments(torch.tensor(m), torch.tensor(s), dims)
@@ -106,7 +52,7 @@ def test_trig_moments_match_torch_oracle(harness, name, m, s, dims):
     assert np.max(np.abs(C - Ct.numpy())) < 1e-14
 
 
-@pytest.mark.parametrize("name,m,s,dims", CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(CASES)])
+@pytest.mark.parametrize("name,m,s,dims", TRIG_CASES, ids=[c[0] + "_%d" % i for i, c in enumerate(TRIG_CASES)])
 def test_trig_vjp_matches_autograd(harness, name, m, s, dims):
     Ds, Dh = len(m), len(m) + len(dims)
     rng = np.random.RandomState(3)

@@ -11,12 +11,15 @@ import numpy as np
 import pytest
 import torch
 
+from pilco_b200 import _lib
 from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _rollout
+import action_reward_oracle as aro
 import exploration_oracle as eo
+from oracle import torch_port as tp
+from particle_grad_oracle import T
 from util import CUOBJDUMP, ROOT, make_gp_problem, sass
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reward_var.npz")
-T = eo.T
 
 
 @pytest.mark.parametrize("kdim", [2, 5])
@@ -30,7 +33,7 @@ def test_variance_vjp_matches_reward_m(kdim):
                      (var, g["sR_%d" % kdim]), (dm, g["dsRdm_%d" % kdim]), (dS, g["dsRdS_%d" % kdim])):
         ref = np.asarray(ref).reshape(np.shape(got))
         assert np.max(np.abs(got - ref)) <= 1e-12 * max(1.0, np.max(np.abs(ref)))
-    assert g["sR_%d" % kdim].item() > eo.VAR_FLOOR                  # reward.m's clamp is not in play
+    assert g["sR_%d" % kdim].item() > aro.VAR_FLOOR                  # reward.m's clamp is not in play
 
 
 def _torch_vjp(fn, m, s):
@@ -48,23 +51,23 @@ def test_variance_vjp_matches_autograd():
         s = 0.3 * B @ B.T
         C = rng.randn(D, D)
         W, t, m = C @ C.T / D + 0.1 * np.eye(D), rng.randn(D), rng.randn(D)
-        term = dict(kind=eo._lib.REWARD_EXP, W=W, t=t)
+        term = dict(kind=_lib.REWARD_EXP, W=W, t=t)
         var, dm, dS = eo.exp_var_vjp(m, s, W, t)
-        rm, rS = _torch_vjp(lambda a, b: eo.term_var(term, a, b), m, s)
-        assert abs(var - float(eo.term_var(term, T(m)[None], T(s)))) < 1e-14
+        rm, rS = _torch_vjp(lambda a, b: aro.term_var(term, a, b), m, s)
+        assert abs(var - float(aro.term_var(term, T(m)[None], T(s)))) < 1e-14
         assert np.max(np.abs(dm - rm)) < 1e-12 * max(1.0, np.max(np.abs(rm)))
         assert np.max(np.abs(dS - rS)) < 1e-12 * max(1.0, np.max(np.abs(rS)))
         for f in (1.0, 2.0, 0.5):                                   # r_f is r_1 with f W
             rf, dmf, dSf = eo.exp_moment_vjp(m, s, W, t, f)
             assert abs(rf - eo.exp_moment_vjp(m, s, f * W, t, 1.0)[0]) < 1e-14
-            rm, rS = _torch_vjp(lambda a, b: eo.tp.exponential_reward(a, b, T(f * W), T(t)[None])[0, 0], m, s)
+            rm, rS = _torch_vjp(lambda a, b: tp.exponential_reward(a, b, T(f * W), T(t)[None])[0, 0], m, s)
             assert np.max(np.abs(dmf - rm)) < 1e-12 * max(1.0, np.max(np.abs(rm)))
             assert np.max(np.abs(dSf - rS)) < 1e-12 * max(1.0, np.max(np.abs(rS)))
         Wl = rng.randn(D)
-        lterm = dict(kind=eo._lib.REWARD_LINEAR, W=Wl)
+        lterm = dict(kind=_lib.REWARD_LINEAR, W=Wl)
         var, dm, dS = eo.linear_var_vjp(m, s, Wl)
-        rm, rS = _torch_vjp(lambda a, b: eo.term_var(lterm, a, b), m, s)
-        assert abs(var - float(eo.term_var(lterm, T(m)[None], T(s)))) < 1e-13
+        rm, rS = _torch_vjp(lambda a, b: aro.term_var(lterm, a, b), m, s)
+        assert abs(var - float(aro.term_var(lterm, T(m)[None], T(s)))) < 1e-13
         assert np.max(np.abs(dm - rm)) == 0.0 and np.max(np.abs(dS - rS)) < 1e-13
 
 
@@ -88,7 +91,7 @@ def test_term_variance_matches_monte_carlo(kind):
     r = f(x)
     mc = r.var()
     se = np.sqrt(np.mean((r - r.mean()) ** 4) / len(r))              # standard error of the variance estimate
-    got = float(eo.term_var(term, T(m)[None], T(s)))
+    got = float(aro.term_var(term, T(m)[None], T(s)))
     assert abs(got - mc) < 5 * se + 1e-12, (got, mc, se)
 
 
@@ -114,8 +117,8 @@ def _objective_case(angle_dims, kind, b, seed=0):
         params = [T(0.5 * rng.randn(6, Dh)), T(0.3 * rng.randn(6, U)), T(1.0 + 0.1 * rng.rand(U, Dh))]
     Bs = rng.randn(Ds, Ds)
     m0, S0 = T(0.5 * rng.rand(Ds)), T(0.05 * Bs @ Bs.T)
-    fn = lambda prm, m, S: eo.problem_rollout(kind, prm, X, 0.05 * Y, ell, sf2, sn2, maxa, terms, m, S, 4, b,
-                                              mult_mu=2.0, angle_dims=angle_dims)
+    fn = lambda prm, m, S: aro.problem_rollout(kind, prm, X, 0.05 * Y, ell, sf2, sn2, maxa, terms, m, S, 4, mult_mu=2.0,
+                                               angle_dims=angle_dims, b=b)
     return fn, params, m0, S0, terms
 
 
@@ -151,7 +154,7 @@ def test_objective_definition():
     assert torch.equal(o0["step_var"], ob["step_var"]) and torch.equal(o0["traj_m"], ob["traj_m"])
     sig = torch.sqrt(o0["step_var"])
     assert abs(float(ob["reward"] - o0["reward"] - 0.8 * sig.sum())) < 1e-13
-    assert eo.sigma(torch.tensor([0.0, 1e-12, 4e-12], dtype=torch.float64)).tolist() == [0.0, 0.0, 2e-6]
+    assert aro.sigma(torch.tensor([0.0, 1e-12, 4e-12], dtype=torch.float64)).tolist() == [0.0, 0.0, 2e-6]
 
 
 # ---- the library -----------------------------------------------------------------------------------------------------

@@ -51,8 +51,8 @@ def _mm_case(kind, R, squash, Ds=3, U=2, n=50, bf=12, seed=9):
 
 
 def _oracle(P, kind, prm_r, terms, H, mu, squash, **kw):
-    return aro.mm_problem_rollout(kind, prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
-                                  P["m0"], P["S0"], H, mult_mu=mu, squash=squash, **kw)
+    return aro.problem_rollout(kind, prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"] if squash else None,
+                               terms, P["m0"], P["S0"], H, mult_mu=mu, **kw)
 
 
 def _check_forward(plan, ref, r, H, tol=1e-10):
@@ -112,7 +112,7 @@ def test_smgpr_d16_and_long_horizon():
     plan.forward()
     fact = tp.fitc_factorizations(T(pb["X"]), T(Z), T(pb["Y"]), T(pb["ell"]), T(pb["sf2"]), T(pb["sn2"]))
     P = dict(pb, maxa=pb["maxa"])
-    ref = _oracle(P, "rbf", [T(pb[k][0]) for k in ("Xc", "Yc", "lc")], terms, 3, 0.7, True, dyn_fact=fact, centres=Z)
+    ref = _oracle(P, "rbf", [T(pb[k][0]) for k in ("Xc", "Yc", "lc")], terms, 3, 0.7, True, fact=fact, Z=Z)
     _check_forward(plan, ref, 0, 3, tol=1e-7)
     pb = make_rollout_problem(300, 10, 2, 50, 1, seed=0)
     gp = engine.gp_factorize(pb["X"], pb["Y"], pb["ell"], pb["sf2"], pb["sn2"])

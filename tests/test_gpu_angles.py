@@ -1,31 +1,25 @@
 """GPU tests of the moment-matching rollout with angular state dimensions (pilco_trig_moments,
 pilco_rollout_angles_forward / _backward through engine.RolloutPlan(angles=...)): the feature map's moments against
-the host build of the same formulas, the cascade against the torch statement in tests/angles_oracle.py, the reverse
-sweep against torch autograd (taped and recomputing), periodicity in the angles, and CUDA-graph replay."""
+the host build of the same formulas, the cascade against the torch statement in tests/action_reward_oracle.py, the
+reverse sweep against torch autograd (taped and recomputing), periodicity in the angles, and CUDA-graph replay."""
 import numpy as np
 import pytest
 import torch
 
-from util import scaled_err, make_gp_problem
-import angles_oracle as ao
+from pilco_b200 import _lib
+import action_reward_oracle as aro
+from util import TRIG_CASES, host_moments, make_gp_problem, scaled_err, trig_harness
 
 pytestmark = pytest.mark.gpu
 T = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)
 
 
 def test_trig_moments_match_host_build(tmp_path):
-    import test_angles_host as th
     from pilco_b200 import engine
-    import subprocess, ctypes, os
-    so = str(tmp_path / "trig_harness.so")
-    subprocess.check_call(["g++", "-O1", "-shared", "-fPIC", "-x", "c++", "-o", so,
-                           os.path.join(th.ROOT, "tests", "host_harness", "trig_harness.cpp")])
-    lib = ctypes.CDLL(so)
-    ip = ctypes.POINTER(ctypes.c_int)
-    lib.trig_moments_host.argtypes = [ctypes.c_int, ctypes.c_int, ip] + [th.dp] * 5
-    for name, m, s, dims in th.CASES:
+    lib = trig_harness(str(tmp_path / "trig_harness.so"))
+    for name, m, s, dims in TRIG_CASES:
         M, S, C = engine.trig_moments(m[None], s[None], dims)
-        hM, hS, hC = th.host_moments(lib, m, s, dims)
+        hM, hS, hC = host_moments(lib, m, s, dims)
         for got, ref in ((M[0], hM), (S[0], hS), (C[0], hC)):
             assert np.max(np.abs(got.cpu().numpy() - ref)) < 1e-14, name
 
@@ -71,24 +65,17 @@ def _problem(Ds, dims, U, kind, R, seed=0, singular=False, joint=False):
 
 
 def _oracle(P, r, H, params=None, m0=None, S0=None):
-    """torch cascade of restart r; params: torch leaves of the policy (else built from P)"""
-    from oracle import torch_port as tp
-    iK, beta = tp.calculate_factorizations(T(P["X"]), T(P["Y"]), T(P["ell"]), T(P["sf2"]), T(P["sn2"]))
-    maxa = T(P["maxa"])[None]
+    """torch cascade of restart r; params: torch leaves of the policy (else built from P).  -> (trajectory means
+    [H+1,Ds], covariances [H+1,Ds,Ds], total reward)"""
     if params is None:
         params = [T(P["pol"][k][r]) for k in (("W", "b") if P["kind"] == "linear" else ("X", "Y", "ell"))]
-    if P["kind"] == "linear":
-        act = lambda m, s: tp.linear_action(params[0], params[1], m, s, maxa)
-    else:
-        act = lambda m, s: tp.rbf_action(params[0], params[1], params[2], m, s, maxa)
-    dyn = lambda m, s: tp.predict_given_factorizations(T(P["X"]), T(P["ell"]), T(P["sf2"]), m, s, iK, beta)
-    rew = lambda m, s: tp.exponential_reward(m, s, T(P["Wr"]), T(P["tr"])[None])
-    jrew = None
+    terms = [dict(kind=_lib.REWARD_EXP, coef=1.0, W=P["Wr"], t=P["tr"])]
     if P["Wj"] is not None:
-        jrew = lambda m, s: -0.5 * tp.exponential_reward(m, s, T(P["Wj"]), T(P["tj"])[None])
-    m0 = T(P["m0"])[None] if m0 is None else m0
-    S0 = T(P["S0"]) if S0 is None else S0
-    return ao.predict(m0, S0, H, P["dims"], act, dyn, rew, jrew)
+        terms.append(dict(kind=_lib.REWARD_EXP_SA, coef=-0.5, W=P["Wj"], t=P["tj"]))
+    out = aro.problem_rollout(P["kind"], params, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
+                              T(P["m0"])[None] if m0 is None else m0, T(P["S0"]) if S0 is None else S0, H,
+                              angle_dims=P["dims"])
+    return out["traj_m"], out["traj_S"], out["reward"]
 
 
 SHAPES = [  # Ds, dims, U, policy, R, singular S0, joint term

@@ -1,5 +1,5 @@
 """GPU tests of the exploration objective (pilco_rollout_explore_*, DESIGN.md section 21) through engine.RolloutPlan and
-the class API: step_var and the objective against the torch oracle (tests/exploration_oracle.py), the reverse sweep
+the class API: step_var and the objective against the torch oracle (tests/action_reward_oracle.py), the reverse sweep
 against autograd (taped and recomputing, with and without angles) and central differences, the bitwise identities
 (no exploration, b = 0, batch position, graph replay, sigma_0 = 0) and PILCO(exploration=...)."""
 import ctypes
@@ -9,12 +9,12 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib, rewards
-import exploration_oracle as eo
+import action_reward_oracle as aro
 from particle_cases import BOX2
+from particle_grad_oracle import T
 from util import make_gp_problem, make_rollout_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
-T = eo.T
 
 
 def _case(kind, R, Ds=3, U=2, dims=(), seed=9, n=50, bf=12):
@@ -64,9 +64,9 @@ def _plan(P, spec, terms, H, R, b, mu=1.5, grad=False, m0=None, S0=None):
 
 
 def _oracle(P, prm_r, terms, H, b, mu=1.5, m0=None, S0=None):
-    return eo.problem_rollout(P["kind"], prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
-                              T(P["m0"]) if m0 is None else m0, T(P["S0"]) if S0 is None else S0, H, b, mult_mu=mu,
-                              angle_dims=P["dims"] or None)
+    return aro.problem_rollout(P["kind"], prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
+                               T(P["m0"]) if m0 is None else m0, T(P["S0"]) if S0 is None else S0, H, mult_mu=mu,
+                               angle_dims=P["dims"] or None, b=b)
 
 
 def _check_forward(plan, ref, r, H, tol=1e-10):
@@ -253,7 +253,7 @@ def test_zero_initial_covariance_one_step():
         out[b] = _outputs(plan, plan.backward())
         out[b]["step_var"] = plan.step_var.clone()
     torch.cuda.synchronize()
-    assert float(out[0.5]["step_var"].abs().max()) <= eo.VAR_FLOOR
+    assert float(out[0.5]["step_var"].abs().max()) <= aro.VAR_FLOOR
     for k in out[0.0]:
         assert torch.equal(out[0.0][k], out[0.5][k]), k
 

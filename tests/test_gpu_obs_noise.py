@@ -1,6 +1,6 @@
 """GPU tests of measurement noise at the policy's input (pilco_rollout_noisy_*, DESIGN.md section 22) through
 engine.RolloutPlan and the class API: trajectory, rewards and step_var against the torch oracle
-(tests/obs_noise_oracle.py), the reverse sweep against autograd (taped and recomputing) and central differences, the
+(tests/action_reward_oracle.py), the reverse sweep against autograd (taped and recomputing) and central differences, the
 identities (nz == NULL, v = 0, batch position, graph replay) and PILCO(measurement_noise=...)."""
 import ctypes
 
@@ -9,12 +9,12 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib, rewards
-import obs_noise_oracle as no
+import action_reward_oracle as aro
 from particle_cases import BOX2
+from particle_grad_oracle import T
 from util import make_gp_problem, make_rollout_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
-T = no.T
 
 
 def _case(kind, R, Ds=3, U=2, dims=(), seed=9, n=50, bf=12, squash=True):
@@ -61,9 +61,9 @@ def _plan(P, spec, terms, H, R, v, b=None, mu=1.5, grad=False, m0=None, S0=None)
 
 
 def _oracle(P, prm_r, terms, H, v, b=0.0, mu=1.5, m0=None, S0=None):
-    return no.problem_rollout(P["kind"], prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
-                              T(P["m0"]) if m0 is None else m0, T(P["S0"]) if S0 is None else S0, H, b, v, mult_mu=mu,
-                              angle_dims=P["dims"] or None)
+    return aro.problem_rollout(P["kind"], prm_r, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], terms,
+                               T(P["m0"]) if m0 is None else m0, T(P["S0"]) if S0 is None else S0, H, mult_mu=mu,
+                               angle_dims=P["dims"] or None, v=v, b=b)
 
 
 def _check_forward(plan, ref, r, H, tol=1e-10):

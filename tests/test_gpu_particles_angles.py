@@ -1,8 +1,8 @@
 """Particle rollouts with angular state dimensions on the device (pilco_particles_angles_* through engine.ParticlePlan,
 ConsistentGradPlan and particles_rollout with ``angles``, DESIGN.md section 20): forward parity of both samplers with
-the numpy oracle (tests/particle_angles_oracle.py) given the same x0 and eps, the pathwise, consistent and score gradients against torch autograd on the
-oracle, the pathwise gradient against central differences of the device forward, A = 0 / NULL against the calls
-without angles, periodicity in the angles, and the bitwise properties of the particle kernels."""
+the numpy oracle (tests/particle_oracle.py) given the same x0 and eps, the pathwise, consistent and score gradients
+against torch autograd on the oracle, the pathwise gradient against central differences of the device forward, A = 0 /
+NULL against the calls without angles, periodicity in the angles, and the bitwise properties of the particle kernels."""
 import ctypes as C
 
 import numpy as np
@@ -11,58 +11,12 @@ import torch
 
 from pilco_b200 import engine, _lib
 from pilco_b200._lib import lib
-from particle_cases import _dyn_np, _linear, _oracle_pol, _rbf
-from particle_angles_oracle import (consistent_rollout, consistent_value_and_grad, particle_rollout, score_grad,
-                                   value_and_grad)
-from util import make_gp_problem, scaled_err
+from particle_cases import _angle_case, _angle_terms, _dyn_np, _oracle_pol
+from particle_grad_oracle import consistent_value_and_grad, score_grad, value_and_grad
+from particle_oracle import consistent_rollout, particle_rollout
+from util import _rel, scaled_err
 
 pytestmark = pytest.mark.gpu
-
-
-def _terms(E, A, U, joint):
-    """state terms on the raw state (exp, linear, MULT box on dimension 0); with ``joint`` an EXP_SA term on the first
-    angle's (sin, cos) = (0, -1) and a LINEAR_SA term on the action"""
-    Dh, D = E + A, E + A + U
-    rng = np.random.RandomState(E + A)
-    terms = [dict(kind=_lib.REWARD_EXP, coef=1.0, W=0.5 * np.eye(E), t=0.2 * np.ones(E)),
-             dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=rng.randn(E), t=None),
-             dict(kind=_lib.REWARD_BOX, coef=0.2, channel=_lib.CHANNEL_MULT, W=np.array([1, 1, 1.0, 0, -0.5, 0.8]),
-                  t=None)]
-    if joint:
-        W = np.zeros((D, D)); k = E - A if A else 0                   # A = 0: on state dimensions 0, 1
-        W[k, k] = W[k + 1, k + 1] = 1.0; W[Dh, Dh] = 0.1
-        t = np.zeros(D); t[k + 1] = -1.0
-        terms += [dict(kind=_lib.REWARD_EXP_SA, coef=0.8, W=W, t=t),
-                  dict(kind=_lib.REWARD_LINEAR_SA, coef=-0.05, W=np.r_[np.zeros(Dh), np.ones(U)], t=None)]
-    return terms
-
-
-def _case(E, dims, U=1, kind="linear", fitc=False, joint=False, n=150, R=1, seed=0):
-    """-> gp, spec (a leading R when R > 1), oracle policy dicts per restart, terms, A"""
-    A = len(dims)
-    Dh, D = E + A, E + A + U
-    X, Y, ell, sf2, sn2 = make_gp_problem(n, D, E, seed=seed + D)
-    X = 2.0 * X - 1.0
-    if fitc:
-        Z = np.random.RandomState(seed).rand(60, D) * 2.0 - 1.0
-        gp = engine.fitc_factorize(X, Z, 0.05 * Y, ell, 0.05 * sf2, 1e-3 * np.ones(E))
-    else:
-        gp = engine.gp_factorize(X, 0.05 * Y, ell, 0.05 * sf2, 1e-3 * np.ones(E))
-    rng = np.random.RandomState(seed + 7)
-    maxa = 0.8 + 0.4 * np.arange(U)
-    if kind == "linear":
-        W, b = 0.5 * rng.randn(R, U, Dh), rng.randn(R, U)
-        if R == 1:
-            spec, pol = _linear(W[0], b[0], maxa, True)
-            pols = [pol]
-        else:
-            spec = dict(kind=_lib.POLICY_LINEAR, Ds=Dh, U=U, squash=True, max_action=maxa, W=W, b=b)
-            pols = [_linear(W[r], b[r], maxa, True)[1] for r in range(R)]
-    else:
-        assert R == 1
-        spec, pol = _rbf(rng.rand(12, Dh) * 2.0 - 1.0, 0.3 * rng.randn(12, U), 1.0 + 0.2 * rng.rand(U, Dh), maxa)
-        pols = [pol]
-    return gp, spec, pols, _terms(E, A, U, joint)
 
 
 def _draw_raw(E, P, H, seed):
@@ -85,7 +39,7 @@ SHAPES = {                                                      # E, dims, U, po
 @pytest.mark.parametrize("consistent", [False, True])
 def test_forward_parity_with_oracle(name, consistent):
     E, dims, U, kind, fitc, joint = SHAPES[name]
-    gp, spec, pols, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, pols, terms = _angle_case(E, dims, U, kind, fitc, joint)
     P, H, mu = (300 if consistent else 1000), 6, 1.5
     x0, eps = _draw_raw(E, P, H, seed=P + H)
     out = [t.cpu().numpy() for t in engine.particles_rollout(gp, spec, terms, x0, eps, mult_mu=mu,
@@ -116,17 +70,12 @@ def _grad_plan(gp, spec, terms, x0, eps, mu, dims, R=1, estimator="pathwise", co
     return plan, {k: v.cpu().numpy() for k, v in g.items()}
 
 
-def _rel(g, ref):
-    scale = max(float(np.abs(r).max()) for r in ref.values())
-    return max(float(np.abs(g[k].reshape(ref[k].shape) - ref[k]).max()) for k in ref) / scale
-
-
 @pytest.mark.parametrize("name", ["cartpole_linear", "cartpole_rbf", "double_pendulum", "all_angles", "joint_terms",
                                   "fitc"])
 @pytest.mark.parametrize("estimator", ["pathwise", "consistent", "score"])
 def test_gradients_match_autograd_oracle(name, estimator):
     E, dims, U, kind, fitc, joint = SHAPES[name]
-    gp, spec, pols, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, pols, terms = _angle_case(E, dims, U, kind, fitc, joint)
     P, H, mu = 200, 5, 1.5
     x0, eps = _draw_raw(E, P, H, seed=P + H + 1)
     plan, g = _grad_plan(gp, spec, terms, x0, eps, mu, dims, estimator="score" if estimator == "score" else "pathwise",
@@ -152,7 +101,7 @@ def test_gradients_match_autograd_oracle(name, estimator):
 def test_batched_gradient_restarts_match_single_policy_calls():
     """R = 3 linear policies: restart r bitwise the R = 1 call with policy r, and each against the autograd oracle"""
     E, dims, U = 4, [1], 1
-    gp, spec, pols, terms = _case(E, dims, U, "linear", joint=True, R=3)
+    gp, spec, pols, terms = _angle_case(E, dims, U, "linear", joint=True, R=3)
     x0, eps = _draw_raw(E, 150, 5, seed=5)
     plan, g = _grad_plan(gp, spec, terms, x0, eps, 0.5, dims, R=3)
     for r in range(3):
@@ -168,7 +117,7 @@ def test_batched_gradient_restarts_match_single_policy_calls():
 
 def test_pathwise_gradient_matches_central_differences_of_device_forward():
     E, dims, U = 6, [1, 2], 1
-    gp, spec, pols, terms = _case(E, dims, U, "linear", joint=True)
+    gp, spec, pols, terms = _angle_case(E, dims, U, "linear", joint=True)
     x0, eps = _draw_raw(E, 500, 6, seed=9)
     _, g = _grad_plan(gp, spec, terms, x0, eps, 1.5, dims)
     val = lambda W, b: float(engine.particles_rollout(gp, dict(spec, W=W, b=b), terms, x0, eps, mult_mu=1.5,
@@ -185,7 +134,7 @@ def test_pathwise_gradient_matches_central_differences_of_device_forward():
 def test_no_angles_is_bitwise_the_call_without_angles():
     """the angle entry points with ang = NULL and A = 0 write bitwise what the calls without angles write"""
     E, U = 4, 1
-    gp, spec, pols, terms = _case(E, [], U, "linear", joint=True)
+    gp, spec, pols, terms = _angle_case(E, [], U, "linear", joint=True)
     x0, eps = _draw_raw(E, 300, 5, seed=2)
     for consistent in (False, True):
         plan = engine.ParticlePlan(gp, spec, terms, 300, 5, mult_mu=0.5, consistent=consistent)
@@ -217,8 +166,8 @@ def test_periodic_in_the_angles(estimator):
     """x0 + 2 pi e_a: the same actions, step rewards, returns and gradients (the state terms do not read dimension a),
     the trajectory shifted by 2 pi in dimension a only"""
     E, dims, U = 4, [1, 3], 1
-    gp, spec, pols, _ = _case(E, dims, U, "rbf", joint=True)
-    terms = _terms(E, len(dims), U, True)[2:]                  # the box on dimension 0 and the joint terms
+    gp, spec, pols, _ = _angle_case(E, dims, U, "rbf", joint=True)
+    terms = _angle_terms(E, len(dims), U, True)[2:]                  # the box on dimension 0 and the joint terms
     x0, eps = _draw_raw(E, 200, 4, seed=4)
     run = lambda x: _grad_plan(gp, spec, terms, x, eps, 0.5, dims, estimator="score" if estimator == "score" else
                                "pathwise", consistent=estimator == "consistent")
@@ -236,7 +185,7 @@ def test_periodic_in_the_angles(estimator):
 
 def test_particle_is_independent_of_batch_and_row():
     E, dims, U = 6, [1, 2], 1
-    gp, spec, _, terms = _case(E, dims, U, "rbf", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, U, "rbf", joint=True)
     x0, eps = _draw_raw(E, 400, 5, seed=6)
     for consistent in (False, True):
         full = engine.particles_rollout(gp, spec, terms, x0, eps, mult_mu=0.5, consistent=consistent, angles=dims)
@@ -251,7 +200,7 @@ def test_particle_is_independent_of_batch_and_row():
 
 def test_graph_replay_is_bitwise_equal_to_eager():
     E, dims, U = 4, [1], 1
-    gp, spec, _, terms = _case(E, dims, U, "rbf", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, U, "rbf", joint=True)
     x0, eps = _draw_raw(E, 300, 5, seed=7)
     for estimator in ("pathwise", "score"):
         plan = engine.ParticlePlan(gp, spec, terms, 300, 5, mult_mu=0.5, grad=True, estimator=estimator, angles=dims)

@@ -1,19 +1,17 @@
 """Score-function gradient over consistent function samples on the device (pilco_particles_consistent_score_grad_rollout
 through engine.ConsistentGradPlan(estimator="score"), DESIGN.md section 25): parity with the torch oracle
-(tests/particle_cscore_oracle.py) given the device's trajectories, x0, eps and nu, the forward outputs and value against
-the consistent pathwise call, restarts against single calls, bitwise reproducibility and CUDA-graph replay, H = 2
-against section 16's score gradient, unbiasedness against the consistent pathwise gradient, and box terms against a
-central difference of the sampled return."""
+(tests/particle_grad_oracle.py's score_grad(consistent=True)) given the device's trajectories, x0, eps and nu, the
+forward outputs and value against the consistent pathwise call, restarts against single calls, bitwise reproducibility
+and CUDA-graph replay, H = 2 against section 16's score gradient, unbiasedness against the consistent pathwise gradient,
+and box terms against a central difference of the sampled return."""
 import numpy as np
 import pytest
 import torch
 
 from pilco_b200 import engine, _lib
-from particle_cases import _batch_case, _case, _draw, _dyn_np, _oracle_pol
-from particle_cscore_oracle import score_grad
-from particle_grad_oracle import score_grad as step_score_grad
-from test_gpu_particles_angles import _case as _angle_case
-from test_gpu_particles_score import _box_case, _seeded, _zscores
+from particle_cases import _angle_case, _batch_case, _box_case, _case, _draw, _dyn_np, _oracle_pol, _seeded
+from particle_grad_oracle import score_grad
+from util import _zscores
 
 pytestmark = pytest.mark.gpu
 
@@ -43,10 +41,11 @@ def _rel(g, ref):
 def _parity(gp, spec, pol, terms, x0, eps, mu, angles=None, v=None, nu=None):
     plan, g, out = _run(gp, spec, terms, x0, eps, mu, angles=angles, v=v, nu=nu)
     g = {k: t.cpu().numpy() for k, t in g.items()}
-    args = (_dyn_np(gp), _oracle_pol(spec, pol), terms, out[0].cpu().numpy(), eps, mu, nu, v, angles)
-    ref, ratio = score_grad(*args)
+    args = (_dyn_np(gp), _oracle_pol(spec, pol), terms, out[0].cpu().numpy(), eps, mu)
+    kw = dict(angle_dims=angles, nu=nu, v=v, consistent=True)
+    ref, ratio = score_grad(*args, **kw)
     err, scale = _rel(g, ref)
-    own = _rel(score_grad(*args, swap=True)[0], ref)[0] if scale > 0.0 else 0.0
+    own = _rel(score_grad(*args, swap=True, **kw)[0], ref)[0] if scale > 0.0 else 0.0
     return g, ref, err, own, ratio
 
 
@@ -145,7 +144,7 @@ def test_two_steps_is_the_step_wise_score_gradient(name):
     plan.set_inputs(x0, eps)
     ref = {k: t.cpu().numpy() for k, t in plan.launch_grad().items() if k != "value"}
     err, scale = _rel({k: t.cpu().numpy() for k, t in g.items()}, ref)
-    own = _rel(ref, step_score_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, plan.traj.cpu().numpy(), eps, mu))[0]
+    own = _rel(ref, score_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, plan.traj.cpu().numpy(), eps, mu))[0]
     print("H = 2 %s: consistent score vs step-wise score gradient %.1e of scale (the step-wise call against its oracle: "
           "%.1e)" % (name, err, own))
     assert torch.equal(out[0][:, :2], plan.traj[:, :2])          # step 0 is the same transition, bitwise
@@ -169,7 +168,7 @@ def test_expected_gradient_is_the_consistent_pathwise_gradient():
         if s == 0:                                              # the pivots of a subset, from the oracle
             sub = 200
             ratio = score_grad(_dyn_np(gp), _oracle_pol(spec, pol), terms, plans["score"].traj[:sub].cpu().numpy(),
-                               eps[:sub].cpu().numpy(), mu)[1]
+                               eps[:sub].cpu().numpy(), mu, consistent=True)[1]
     worst = _zscores(draws["score"], draws["pathwise"])
     print("consistent score vs pathwise gradient, paired over 16 x 2^12 particles: worst %.2f standard errors; "
           "smallest pivot d2 / (tau sf2) over %d particles %.1e" % (worst, sub, ratio))

@@ -1,7 +1,7 @@
 """PILCO's exploration objective in the particle rollouts on the device (pilco_particles_explore_* through
 engine.ParticlePlan / ConsistentGradPlan with ``exploration``, pilco_particles_reward_moments through
 engine.particle_reward_moments, and the PILCO class's sample_reward_moments and exploration keywords; DESIGN.md
-section 24): value, step_var and gradients against torch autograd on the oracle (tests/particle_explore_oracle.py)
+section 24): value, step_var and gradients against torch autograd on the oracle (tests/particle_grad_oracle.py)
 with the same x0, eps and nu, central differences of the device value, the bitwise properties (NULL and b = 0 against
 the calls without exploration, restarts, graph replay), the chunked forward's moments, and the sampled variance at
 step 0 against the moment-matching prediction."""
@@ -10,9 +10,10 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib
-from particle_cases import _dyn_np, _oracle_pol, _pilco, _safe_pilco
-from particle_explore_oracle import consistent_value_and_grad, sample_moments, value_and_grad
-from test_gpu_particles_angles import _case, _rel
+from particle_cases import _angle_case, _dyn_np, _oracle_pol, _pilco, _safe_pilco
+from particle_grad_oracle import consistent_value_and_grad, value_and_grad
+from particle_oracle import sample_moments
+from util import _rel
 
 pytestmark = pytest.mark.gpu
 
@@ -46,17 +47,18 @@ def _run(gp, spec, terms, x0, eps, nu, v, mu, dims, b, R=1, consistent=False):
 @pytest.mark.parametrize("consistent", [False, True])
 def test_value_step_var_and_gradient_match_autograd_oracle(name, consistent):
     E, dims, U, kind, fitc, joint, noisy = SHAPES[name]
-    gp, spec, pols, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, pols, terms = _angle_case(E, dims, U, kind, fitc, joint)
     P, H, mu, b = 200, 5, 1.5, 0.7
     x0, eps, nu = _draw(E, P, H, seed=P + H + 3)
     v = 0.01 + 0.02 * np.random.RandomState(4).rand(E) if noisy else None
     plan, g = _run(gp, spec, terms, x0, eps, nu, v, mu, dims, b, consistent=consistent)
-    args = (_dyn_np(gp), _oracle_pol(spec, pols[0]), terms, x0, eps, nu, v, mu)
+    args = (_dyn_np(gp), _oracle_pol(spec, pols[0]), terms, x0, eps, mu)
     f = consistent_value_and_grad if consistent else value_and_grad
-    val, ref, sv = f(*args, angle_dims=dims, b=b)
+    out = f(*args, angle_dims=dims, nu=nu, v=v, b=b)
+    val, ref, sv = out[0], out[1], out[-1]
     own = 0.0
     if consistent:
-        own = _rel(consistent_value_and_grad(*args, angle_dims=dims, b=b, swap=True)[1], ref)
+        own = _rel(consistent_value_and_grad(*args, swap=True, angle_dims=dims, nu=nu, v=v, b=b)[1], ref)
     err = _rel(g, ref)
     verr = abs(float(g["value"][0]) - val) / max(abs(val), 1e-300)
     serr = float(np.abs(plan.step_var[0, :H].cpu().numpy() - sv).max() / np.abs(sv).max())
@@ -69,7 +71,7 @@ def test_value_step_var_and_gradient_match_autograd_oracle(name, consistent):
 @pytest.mark.parametrize("b", [0.5, -0.5])
 def test_device_value_matches_central_differences(b):
     E, dims, U = 4, [1], 1
-    gp, spec, _, terms = _case(E, dims, U, "linear", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, U, "linear", joint=True)
     x0, eps, _ = _draw(E, 400, 6, seed=9)
     _, g = _run(gp, spec, terms, x0, eps, None, None, 1.5, dims, b)
     val = lambda W, bb: float(_run(gp, dict(spec, W=W, b=bb), terms, x0, eps, None, None, 1.5, dims, b)[1]["value"][0])
@@ -87,7 +89,7 @@ def test_device_value_matches_central_differences(b):
 def test_zero_b_is_bitwise_the_call_without_exploration(name, consistent):
     """b = 0 with step_var: every output and gradient is bitwise the noisy / angle / plain call's"""
     E, dims, U, kind, fitc, joint, noisy = SHAPES[name]
-    gp, spec, _, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, _, terms = _angle_case(E, dims, U, kind, fitc, joint)
     x0, eps, nu = _draw(E, 300, 5, seed=11)
     v = 0.02 * np.ones(E) if noisy else None
     outs = []
@@ -104,7 +106,7 @@ def test_zero_b_is_bitwise_the_call_without_exploration(name, consistent):
 def test_zero_spread_is_bitwise_b_zero():
     """S0 = 0 at H = 1: every particle has the same reward, sigma_0 = 0, so b = 0.5 changes nothing"""
     E = 4
-    gp, spec, _, terms = _case(E, [], 1, "linear", joint=True)
+    gp, spec, _, terms = _angle_case(E, [], 1, "linear", joint=True)
     x0 = np.tile(0.3 * np.ones(E), (100, 1))
     eps = np.random.RandomState(2).randn(100, 1, E)
     p0, g0 = _run(gp, spec, terms, x0, eps, None, None, 0.5, [], 0.0)
@@ -116,7 +118,7 @@ def test_zero_spread_is_bitwise_b_zero():
 @pytest.mark.parametrize("consistent", [False, True])
 def test_restarts_are_independent_and_graph_replay_is_bitwise(consistent):
     E, U, R = 4, 1, 3
-    gp, spec, _, terms = _case(E, [], U, "linear", joint=True, R=R)
+    gp, spec, _, terms = _angle_case(E, [], U, "linear", joint=True, R=R)
     x0, eps, _ = _draw(E, 150, 4, seed=5)
     plan, g = _run(gp, spec, terms, x0, eps, None, None, 0.5, [], 0.6, R=R, consistent=consistent)
     sv = plan.step_var.cpu().numpy()
@@ -139,7 +141,7 @@ def test_restarts_are_independent_and_graph_replay_is_bitwise(consistent):
 def test_reward_moments_over_chunked_forward_match_gradient_call():
     """pilco_particles_reward_moments over a chunked consistent forward gives the unchunked gradient call's step_var"""
     E, dims, U = 4, [1], 1
-    gp, spec, _, terms = _case(E, dims, U, "linear", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, U, "linear", joint=True)
     P, H = 300, 5
     x0, eps, _ = _draw(E, P, H, seed=13)
     plan, _ = _run(gp, spec, terms, x0, eps, None, None, 0.5, dims, 0.0, consistent=True)

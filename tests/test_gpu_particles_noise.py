@@ -1,6 +1,6 @@
 """Particle rollouts with measurement noise at the policy's input on the device (pilco_particles_noisy_* through
 engine.ParticlePlan, ConsistentGradPlan and particles_rollout with ``measurement_noise``, DESIGN.md section 23): forward
-parity of both samplers with the numpy oracle (tests/particle_noise_oracle.py) given the same x0, eps and nu, the
+parity of both samplers with the numpy oracle (tests/particle_oracle.py) given the same x0, eps and nu, the
 pathwise, consistent and score gradients against torch autograd on the oracle, the pathwise gradient against central
 differences of the device forward, nz = NULL against the angle calls, v = 0 against the calls without noise, the
 structural and bitwise properties, and the one-step moments against the noisy moment-matching rollout."""
@@ -12,12 +12,10 @@ import torch
 
 from pilco_b200 import engine, _lib
 from pilco_b200._lib import lib
-from particle_cases import _dyn_np, _linear, _oracle_pol
-from particle_noise_oracle import (consistent_rollout, consistent_value_and_grad, particle_rollout, score_grad,
-                                   value_and_grad)
-from particle_oracle import moment_check
-from test_gpu_particles_angles import _case, _rel
-from util import make_rollout_problem, scaled_err
+from particle_cases import _angle_case, _dyn_np, _linear, _oracle_pol
+from particle_grad_oracle import consistent_value_and_grad, score_grad, value_and_grad
+from particle_oracle import consistent_rollout, moment_check, particle_rollout
+from util import _rel, make_rollout_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
 
@@ -45,16 +43,16 @@ SHAPES = {                                                      # E, dims, U, po
 @pytest.mark.parametrize("consistent", [False, True])
 def test_forward_parity_with_oracle(name, consistent):
     E, dims, U, kind, fitc, joint = SHAPES[name]
-    gp, spec, pols, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, pols, terms = _angle_case(E, dims, U, kind, fitc, joint)
     P, H, mu = (300 if consistent else 1000), 6, 1.5
     x0, eps, nu = _draw(E, P, H, seed=P + H)
     v = _var(E)
     out = [t.cpu().numpy() for t in engine.particles_rollout(gp, spec, terms, x0, eps, mult_mu=mu, consistent=consistent,
                                                              angles=dims, measurement_noise=v, nu=nu)]
     f = consistent_rollout if consistent else particle_rollout
-    kw = dict(angle_dims=dims)
-    ref = f(_dyn_np(gp), pols[0], terms, x0, eps, nu, v, mu, **kw)
-    own = scaled_err(f(_dyn_np(gp), pols[0], terms, x0, eps, nu, v, mu, swap=True, **kw)[0], ref[0]) if consistent else 0.0
+    kw = dict(angle_dims=dims, nu=nu, v=v)
+    ref = f(_dyn_np(gp), pols[0], terms, x0, eps, mu, **kw)
+    own = scaled_err(f(_dyn_np(gp), pols[0], terms, x0, eps, mu, swap=True, **kw)[0], ref[0]) if consistent else 0.0
     errs = []
     for o, r in zip(out, ref):
         errs.append(scaled_err(o, r) if r.size and np.abs(r).max() > 0 else float(np.abs(o).max(initial=0.0)))
@@ -80,7 +78,7 @@ def _grad_plan(gp, spec, terms, x0, eps, nu, v, mu, dims, R=1, estimator="pathwi
 @pytest.mark.parametrize("estimator", ["pathwise", "consistent", "score"])
 def test_gradients_match_autograd_oracle(name, estimator):
     E, dims, U, kind, fitc, joint = SHAPES[name]
-    gp, spec, pols, terms = _case(E, dims, U, kind, fitc, joint)
+    gp, spec, pols, terms = _angle_case(E, dims, U, kind, fitc, joint)
     P, H, mu = 200, 5, 1.5
     x0, eps, nu = _draw(E, P, H, seed=P + H + 1)
     v = _var(E, 1)
@@ -89,13 +87,13 @@ def test_gradients_match_autograd_oracle(name, estimator):
     args = (_dyn_np(gp), _oracle_pol(spec, pols[0]), terms)
     own = 0.0
     if estimator == "pathwise":
-        val, ref = value_and_grad(*args, x0, eps, nu, v, mu, angle_dims=dims)
+        val, ref = value_and_grad(*args, x0, eps, mu, angle_dims=dims, nu=nu, v=v)
     elif estimator == "consistent":
-        val, ref, _ = consistent_value_and_grad(*args, x0, eps, nu, v, mu, angle_dims=dims)
-        own = _rel(consistent_value_and_grad(*args, x0, eps, nu, v, mu, swap=True, angle_dims=dims)[1], ref)
+        val, ref, _ = consistent_value_and_grad(*args, x0, eps, mu, angle_dims=dims, nu=nu, v=v)
+        own = _rel(consistent_value_and_grad(*args, x0, eps, mu, swap=True, angle_dims=dims, nu=nu, v=v)[1], ref)
     else:
         traj = plan.outputs()[0].cpu().numpy()
-        ref = score_grad(*args, traj, eps, nu, v, mu, angle_dims=dims)
+        ref = score_grad(*args, traj, eps, mu, angle_dims=dims, nu=nu, v=v)
         val = float(plan.outputs()[4].mean())
     err, verr = _rel(g, ref), abs(float(g["value"][0]) - val) / max(abs(val), 1e-300)
     print("noisy gradient %s %s vs autograd oracle: %.1e of scale, value %.1e (own %.1e)" % (name, estimator, err, verr,
@@ -106,7 +104,7 @@ def test_gradients_match_autograd_oracle(name, estimator):
 
 def test_pathwise_gradient_matches_central_differences_of_device_forward():
     E, dims, U = 6, [1, 2], 1
-    gp, spec, _, terms = _case(E, dims, U, "linear", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, U, "linear", joint=True)
     x0, eps, nu = _draw(E, 500, 6, seed=9)
     v = _var(E, 2)
     _, g = _grad_plan(gp, spec, terms, x0, eps, nu, v, 1.5, dims)
@@ -130,7 +128,7 @@ _GRAD = {("pathwise", False): lib.pilco_particles_noisy_batch_grad_rollout,
 def test_null_noise_is_bitwise_the_angle_call():
     """nz = NULL writes bitwise what the angle calls write, and with ang = NULL what the calls without angles write"""
     for E, dims in ((4, [1]), (4, [])):
-        gp, spec, _, terms = _case(E, dims, 1, "linear", joint=True)
+        gp, spec, _, terms = _angle_case(E, dims, 1, "linear", joint=True)
         x0, eps, _ = _draw(E, 300, 5, seed=2)
         ang = engine.angles_struct(dims, E)
         for consistent, f in zip((False, True), _FWD):
@@ -163,7 +161,7 @@ def test_null_noise_is_bitwise_the_angle_call():
 def test_zero_noise_is_the_noiseless_call(dims):
     """v = 0 with any nu: forward outputs bitwise, gradients within 1e-12 of scale (J' phi_bar is split in two sums)"""
     E = 4
-    gp, spec, _, terms = _case(E, dims, 1, "rbf", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, 1, "rbf", joint=True)
     x0, eps, nu = _draw(E, 300, 5, seed=3)
     for consistent in (False, True):
         a = engine.particles_rollout(gp, spec, terms, x0, eps, mult_mu=0.5, consistent=consistent, angles=dims)
@@ -183,7 +181,7 @@ def test_zero_noise_is_the_noiseless_call(dims):
 def test_structural_properties():
     """a linear policy with W = 0 ignores v and nu bitwise; nu in a dimension with v_i = 0 changes no bit"""
     E, dims = 4, [1]
-    gp, spec, _, terms = _case(E, dims, 1, "linear", joint=True)
+    gp, spec, _, terms = _angle_case(E, dims, 1, "linear", joint=True)
     x0, eps, nu = _draw(E, 300, 5, seed=4)
     zero = dict(spec, W=np.zeros_like(spec["W"]))
     v = _var(E)
@@ -204,7 +202,7 @@ def test_structural_properties():
 def test_restarts_rows_and_graph_replay_are_bitwise():
     """R = 3 restarts each the R = 1 call with its policy; a particle independent of P and its row; graph replay"""
     E, dims, U = 4, [1], 1
-    gp, spec, _, terms = _case(E, dims, U, "linear", joint=True, R=3)
+    gp, spec, _, terms = _angle_case(E, dims, U, "linear", joint=True, R=3)
     x0, eps, nu = _draw(E, 150, 5, seed=5)
     v = _var(E)
     for estimator, consistent in _GRAD:

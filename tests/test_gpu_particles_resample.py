@@ -1,15 +1,15 @@
 """Gaussian-resampled particle rollouts on the device (pilco_particles_resampled_* through
 engine.ParticlePlan(resample=True), DESIGN.md section 26): parity with the torch oracle
-(tests/particle_resample_oracle.py) on the same x0, eps and xi, the call without resampling at H <= 1, restarts against
-single calls, bitwise reproducibility and CUDA-graph replay, the fitted moments against the moment-matching trajectory at
-every step, a central difference of the value, and the class-level options."""
+(tests/particle_grad_oracle.py's resampled_rollout) on the same x0, eps and xi, the call without resampling at H <= 1,
+restarts against single calls, bitwise reproducibility and CUDA-graph replay, the fitted moments against the
+moment-matching trajectory at every step, a central difference of the value, and the class-level options."""
 import numpy as np
 import pytest
 import torch
 
 from pilco_b200 import engine, _lib
 from particle_cases import _batch_case, _case, _draw, _dyn_np, _linear_pilco, _oracle_pol, _pilco
-import particle_resample_oracle as pro
+import particle_grad_oracle as pgo
 from util import make_gp_problem
 
 pytestmark = pytest.mark.gpu
@@ -46,7 +46,7 @@ def test_parity_with_oracle(name):
     x0, eps = _draw(m0, S0, P, H, seed=P + H + 1)
     xi = np.random.RandomState(P + H + 2).randn(P, H, m0.shape[0])
     _, g, out = _run(gp, spec, terms, x0, eps, xi, mu)
-    ref = pro.rollout(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps, xi, mu)
+    ref = pgo.resampled_rollout(_dyn_np(gp), _oracle_pol(spec, pol), terms, x0, eps, xi, mu)
     tol = 1e-6 if name == "fitc" else 1e-9
     errs = {k: _scaled(o.cpu().numpy(), ref[k]) for k, o in zip(("traj", "act", "rew", "risk", "ret", "step_mean",
                                                                    "step_cov"), out)}

@@ -9,9 +9,9 @@ import pytest
 import torch
 
 from pilco_b200 import engine, _lib
-from particle_cases import BOX2, _batch_case, _case, _draw, _dyn_np, _oracle_pol, _pilco_data
+from particle_cases import _batch_case, _box_case, _case, _draw, _dyn_np, _oracle_pol, _pilco_data, _seeded
 from particle_grad_oracle import score_grad
-from util import make_gp_problem, make_rollout_problem
+from util import _zscores, make_gp_problem, make_rollout_problem
 
 pytestmark = pytest.mark.gpu
 
@@ -122,24 +122,6 @@ def test_past_one_vjp_call_agrees_with_oracle():
     assert err <= 1e-8
 
 
-def _seeded(P, H, Ds, m0, S0, seed):
-    d = engine.device()
-    gen = torch.Generator(device=d)
-    gen.manual_seed(seed)
-    F = engine.dev(np.linalg.cholesky(S0))
-    x0 = engine.dev(m0)[None] + torch.randn((P, Ds), dtype=engine.F64, device=d, generator=gen) @ F.T
-    return x0, torch.randn((P, H, Ds), dtype=engine.F64, device=d, generator=gen)
-
-
-def _zscores(a, b=None, ref=None):
-    """largest |mean| / standard error of a - b (paired draws) or of a against the constant ref"""
-    worst = 0.0
-    for k in a:
-        d = np.stack(a[k]) - (np.stack(b[k]) if b is not None else ref[k])
-        worst = max(worst, float(np.max(np.abs(d.mean(0)) / (d.std(0, ddof=1) / np.sqrt(d.shape[0])))))
-    return worst
-
-
 def test_expected_score_gradient_is_the_moment_matching_gradient():
     """Linear unsquashed policy, one linear reward, H = 2, where moment matching is exact (as the pathwise test)"""
     pb = make_rollout_problem(200, 4, 1, 10, 1, seed=23)
@@ -183,18 +165,6 @@ def test_expected_score_gradient_is_the_expected_pathwise_gradient():
     worst = _zscores(draws["score"], draws["pathwise"])
     print("score vs pathwise gradient, paired over 16 x 2^12 particles: worst %.2f standard errors" % worst)
     assert worst <= 5.0
-
-
-def _box_case():
-    """SafePILCO-like: a linear policy, a linear additive reward and one box as the only MULT term"""
-    X, Y, ell, sf2, sn2 = make_gp_problem(100, 5, 4, seed=6)
-    gp = engine.gp_factorize(X, 0.1 * Y, ell, 0.1 * sf2, 1e-3 * np.ones(4))
-    rng = np.random.RandomState(48)
-    W, b = 0.5 * rng.randn(1, 4), rng.randn(1)
-    spec = dict(kind=_lib.POLICY_LINEAR, Ds=4, U=1, squash=True, max_action=np.array([1.3]), W=W, b=b)
-    terms = [dict(kind=_lib.REWARD_LINEAR, coef=0.3, W=rng.randn(4), t=None),
-             dict(kind=_lib.REWARD_BOX, coef=1.0, channel=_lib.CHANNEL_MULT, W=BOX2, t=None)]
-    return gp, spec, terms, X[0, :4], 0.05 * np.eye(4), 6, -4.0
 
 
 def test_box_terms_central_difference_of_sampled_return():

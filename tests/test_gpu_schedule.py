@@ -1,8 +1,8 @@
 """GPU tests of the time-varying linear policy (pilco_rollout_scheduled_*, DESIGN.md section 27) through
 engine.RolloutPlan(schedule=True) and the class API: a constant schedule against the stationary call (bitwise forward,
-per-step gradients summing to its gradient), the torch oracle (tests/schedule_oracle.py) on the features the cascade
-combines, both reverse sweeps, a central difference, restarts against single calls and graph replay, the open-loop
-closed form, and TimeVaryingLinearController with PILCO.optimize_policy / plan / compute_action."""
+per-step gradients summing to its gradient), the torch oracle (tests/action_reward_oracle.py) on the features the
+cascade combines, both reverse sweeps, a central difference, restarts against single calls and graph replay, the
+open-loop closed form, and TimeVaryingLinearController with PILCO.optimize_policy / plan / compute_action."""
 import os
 import sys
 
@@ -12,12 +12,12 @@ import torch
 
 from pilco_b200 import engine, _lib, rewards, controllers
 from pilco_b200.models.pilco import PILCO
-import schedule_oracle as so
+import action_reward_oracle as aro
 from particle_cases import BOX2
+from particle_grad_oracle import T
 from util import make_gp_problem, scaled_err
 
 pytestmark = pytest.mark.gpu
-T = so.T
 
 
 def _case(Ds=3, U=2, H=6, R=2, dims=(), seed=5, n=50, fitc=False, mi=20):
@@ -123,11 +123,11 @@ def test_oracle_parity(shape, dims, noise, x, which, fitc, taped, n):
     g = plan.backward()
     torch.cuda.synchronize()
     assert int(plan.info.max()) == 0
-    dyn = so.dynamics(P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["Z"])
+    dyn = aro.dynamics(P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["Z"])
     for r in range(P["R"]):
         Wt, bt = T(P["W"][r]).requires_grad_(), T(P["b"][r]).requires_grad_()
-        ref = so.scheduled_rollout(dyn, Wt, bt, P["maxa"], terms, P["m0"], P["S0"], P["H"], b=x or 0.0,
-                                   v=P["v"] if noise else None, mult_mu=mu, angle_dims=P["dims"] or None)
+        ref = aro.mm_rollout(dyn, aro.step_action(Wt, bt, P["maxa"]), terms, P["m0"], P["S0"], P["H"], mult_mu=mu,
+                             angle_dims=P["dims"] or None, v=P["v"] if noise else None, b=x or 0.0)
         tol = 1e-9 if fitc else 1e-10
         assert scaled_err(plan.traj_m[r].cpu().numpy(), ref["traj_m"].detach().numpy()) <= tol
         assert scaled_err(plan.traj_S[r].cpu().numpy(), ref["traj_S"].detach().numpy()) <= tol

@@ -366,3 +366,16 @@ def test_lockstep_group_bounds():
     assert group_bounds(1) == [(0, 1)]
     assert group_bounds(64, groups=4) == [(0, 16), (16, 32), (32, 48), (48, 64)]
     assert group_bounds(17, groups=4) == [(0, 8), (8, 17)]
+
+
+def test_no_test_module_imports_another():
+    """Shared fixtures live in particle_cases.py, abi_fakes.py and util.py, and the oracles in their own modules:
+    importing a test module would run its top level and tie its private helpers to another file's tests"""
+    tests = os.path.join(ROOT, "tests")
+    pattern = re.compile(r"^\s*(import\s+test_\w*|from\s+test_\w*\s+import)\b", re.M)
+    offenders = []
+    for name in sorted(os.listdir(tests)):
+        if name.endswith(".py"):
+            src = open(os.path.join(tests, name)).read()
+            offenders += ["%s: %s" % (name, m.group(0).strip()) for m in pattern.finditer(src)]
+    assert not offenders, offenders

@@ -1,8 +1,8 @@
 """CPU tests of measurement noise at the policy's input (pilco_rollout_noisy_*, DESIGN.md section 22): the torch
-statement (tests/obs_noise_oracle.py) against propagate.m's composition (tests/golden/obs_noise.npz), bitwise the
-noiseless oracle at v = 0, against 10^6 Monte Carlo draws in the exact H = 1 case and its autograd gradient against
-central differences; and the library side that needs no GPU: exported symbols, the pilco_obs_noise layout, the new
-kernels' registers and local memory, and validation before any device work."""
+statement (tests/action_reward_oracle.py's cascade with v) against propagate.m's composition
+(tests/golden/obs_noise.npz), bitwise the cascade without v at v = 0, against 10^6 Monte Carlo draws in the exact H = 1
+case and its autograd gradient against central differences; and the library side that needs no GPU: exported symbols,
+the pilco_obs_noise layout, the new kernels' registers and local memory, and validation before any device work."""
 import ctypes
 import os
 import re
@@ -13,14 +13,13 @@ import pytest
 import torch
 
 from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _rollout
-import exploration_oracle as eo
-import obs_noise_oracle as no
+import action_reward_oracle as aro
 import particle_oracle as po
 from oracle import torch_port as tp
+from particle_grad_oracle import T
 from util import CUOBJDUMP, ROOT, make_gp_problem, sass
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "obs_noise.npz")
-T = no.T
 
 
 def _problem(kind, Ds=3, U=2, dims=(), seed=4, n=40, bf=10, squash=True):
@@ -43,9 +42,10 @@ def _problem(kind, Ds=3, U=2, dims=(), seed=4, n=40, bf=10, squash=True):
 
 
 def _run(P, H, b=0.0, v=None, prm=None, m0=None, S0=None):
-    return no.problem_rollout(P["kind"], P["prm"] if prm is None else prm, P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"],
-                              P["maxa"], P["terms"], T(P["m0"]) if m0 is None else m0, T(P["S0"]) if S0 is None else S0,
-                              H, b, P["v"] if v is None else v, angle_dims=P["dims"])
+    return aro.problem_rollout(P["kind"], P["prm"] if prm is None else prm, P["X"], P["Y"], P["ell"], P["sf2"],
+                               P["sn2"], P["maxa"], P["terms"], T(P["m0"]) if m0 is None else m0,
+                               T(P["S0"]) if S0 is None else S0, H, angle_dims=P["dims"], v=P["v"] if v is None else v,
+                               b=b)
 
 
 # ---- propagate.m ---------------------------------------------------------------------------------------------------
@@ -66,7 +66,7 @@ def test_oracle_matches_propagate_m(case):
         act = lambda mm, ss: tp.linear_action(T(g[pre + "W"]), T(g[pre + "b"]).reshape(1, -1), mm, ss, ma)
     else:
         act = lambda mm, ss: tp.rbf_action(T(g[pre + "Xc"]), T(g[pre + "Yc"]), T(g[pre + "lc"]), mm, ss, ma)
-    out = no.noisy_rollout(dyn, act, [dict(kind=1, coef=1.0, W=np.zeros(len(m)), t=None)], T(m), T(s), 1, 0.0, T(v))
+    out = aro.mm_rollout(dyn, act, [dict(kind=1, coef=1.0, W=np.zeros(len(m)), t=None)], T(m), T(s), 1, v=T(v))
     for got, ref in ((out["traj_m"][1], g[pre + "Mnext"]), (out["traj_S"][1], g[pre + "Snext"])):
         ref = np.asarray(ref).reshape(tuple(got.shape))
         assert np.max(np.abs(got.numpy() - ref)) <= 1e-12 * max(1.0, np.max(np.abs(ref)))
@@ -77,8 +77,8 @@ def test_zero_noise_is_the_noiseless_oracle_bitwise(kind, dims):
     P = _problem(kind, Ds=3, dims=dims)
     H, b = 4, 0.5
     got = _run(P, H, b=b, v=np.zeros(3))
-    ref = eo.problem_rollout(kind, P["prm"], P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], P["terms"],
-                             T(P["m0"]), T(P["S0"]), H, b, angle_dims=P["dims"])
+    ref = aro.problem_rollout(kind, P["prm"], P["X"], P["Y"], P["ell"], P["sf2"], P["sn2"], P["maxa"], P["terms"],
+                              T(P["m0"]), T(P["S0"]), H, angle_dims=P["dims"], b=b)
     for k in ("traj_m", "traj_S", "step_reward", "step_var", "reward"):
         assert torch.equal(got[k], ref[k]), k
 

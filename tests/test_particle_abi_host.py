@@ -4,7 +4,6 @@ and every pair of defects that can coexist, to valid descriptions of both policy
 {0, 1, 5}, state, joint and multiplicative terms, with and without angles, measurement noise and exploration, so each
 call's order of precedence is pinned and not only its single codes.  No call passes its workspace check: the
 workspace is 0 bytes, or 8 bytes short of the size the query reports (after that size is checked against the golden)."""
-import ctypes as C
 import itertools
 import os
 
@@ -12,7 +11,9 @@ import numpy as np
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from abi_fakes import (ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _angles, _batched, _grad,
+                       _noise, _particles)
+from util import _ref
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "particle_abi.npz")
 MISMATCH = 99           # status of a call not made because its query disagreed with the golden
@@ -47,22 +48,6 @@ CODES = {ERR_NULL, ERR_DIM, ERR_UNSUP, ERR_ALIGN, ERR_WS}
 class Case:
     def __init__(self, pr, ang=None, nz=None, ex=None, R=1, g=None, short=False):
         self.pr, self.ang, self.nz, self.ex, self.R, self.g, self.short = pr, ang, nz, ex, R, g, short
-
-
-def _angles(*dims):
-    a = _lib.Angles()
-    a.A = len(dims)
-    for i, d in enumerate(dims):
-        a.dims[i] = d
-    return a
-
-
-def _noise(var=(0.01, 0.02, 0.03), nu=FAKE):
-    n = _lib.ParticlesNoise()
-    for i, v in enumerate(var):
-        n.v.var[i] = v
-    n.nu = nu
-    return n
 
 
 def _term(pr, k, kind, channel=0, t=FAKE):
@@ -188,10 +173,6 @@ def cases():
                                                               (False, True), (False, True)):
             out.append(("H%d" % H, base(kind, False, H, "joint", angles, noise, explore, P=PT_MAX_P)))
     return out
-
-
-def _ref(x):
-    return C.byref(x) if x is not None else None
 
 
 def _args(c, sig):

@@ -1,7 +1,8 @@
 """CPU tests of the particle rollouts with angular state dimensions (pilco_particles_angles_*, DESIGN.md section 20):
-the status codes of the ten angle entry points on fake descriptors (rejected calls only), their workspace sizes
-against the calls without angles, the new kernels' registers and SASS, the angle oracle (tests/particle_angles_oracle.py)
-against the oracles without angles and against central differences, and the engine's checks before any device work."""
+the status codes of the ten angle entry points on fake descriptors (rejected calls only), their workspace sizes against
+the calls without angles, the new kernels' registers and SASS, the oracles' angles (tests/particle_oracle.py and
+particle_grad_oracle.py) against their calls without angles and against central differences, and the engine's checks
+before any device work."""
 import ctypes as C
 import os
 import re
@@ -12,33 +13,12 @@ import pytest
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, _batched, _grad, _particles
-import particle_grad_oracle as pgo
-import particle_oracle as po
-from particle_angles_oracle import (consistent_rollout, consistent_value_and_grad, feature_map, particle_rollout,
-                                   score_grad, value_and_grad)
-from util import CUOBJDUMP, ROOT, sass
-
-
-def _angles(*dims):
-    a = _lib.Angles()
-    a.A = len(dims)
-    for i, d in enumerate(dims):
-        a.dims[i] = d
-    return a
-
-
-def _angle_particles(kind=_lib.POLICY_LINEAR, A=1, batched=False, **kw):
-    """abi_fakes' description (E = 3 state dimensions, U = 1) with a policy of Dh = 3 + A inputs"""
-    pr = (_batched if batched else _particles)(kind, **kw)
-    pr.pol.Ds, pr.dyn.D = 3 + A, 3 + A + 1
-    if kind == _lib.POLICY_RBF:
-        pr.pol.rbf.D = 3 + A
-    return pr
-
-
-def _ref(x):
-    return C.byref(x) if x is not None else None
+from abi_fakes import (ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, _FakeGP, _angle_particles, _angles, _batched, _grad,
+                       _particles)
+from particle_cases import _host_problem, _joint_terms
+from particle_grad_oracle import consistent_value_and_grad, score_grad, value_and_grad
+from particle_oracle import consistent_rollout, feature_map, particle_rollout
+from util import CUOBJDUMP, ROOT, _ref, _round2, sass
 
 
 # (angle twin, call without angles, takes R and a gradient)
@@ -124,10 +104,6 @@ def test_angle_specific_dimension_errors():
     assert _calls(_angle_particles(), _angles(1), g=g)[2:] == [ERR_NULL] * 3
 
 
-def _round2(n):
-    return n + (n & 1)
-
-
 @pytest.mark.parametrize("kind", [_lib.POLICY_LINEAR, _lib.POLICY_RBF])
 def test_workspace_sizes(kind):
     """the angle layouts are those of the calls without angles at the same description, plus the phi history
@@ -182,35 +158,9 @@ def test_new_kernels_have_no_local_memory():
 
 
 # ---- the oracles ------------------------------------------------------------------------------------------------------
-def _host_problem(E, A, U, seed, n=30):
-    """numpy factors of a small exact GP on [phi(x), u] (D = E + A + U inputs, E outputs)"""
-    rng = np.random.RandomState(seed)
-    D = E + A + U
-    Cx = rng.rand(n, D) * 2.0 - 1.0
-    Y = 0.1 * np.sin(2.0 * Cx).dot(rng.rand(D, E))
-    ell, sf2 = 0.7 + 0.5 * rng.rand(E, D), 0.02 * (1.0 + rng.rand(E))
-    iK, beta = [], []
-    for e in range(E):
-        d = (Cx[:, None] - Cx[None]) / ell[e]
-        K = sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) + 1e-3 * np.eye(n)
-        iK.append(np.linalg.inv(K)); beta.append(iK[-1] @ Y[:, e])
-    return dict(C=Cx, ell=ell, sf2=sf2, iK=np.stack(iK), beta=np.stack(beta)), rng
-
-
-def _joint_terms(E, A, U, other):
-    """an EXP_SA term on the first angle's (sin, cos) and a state EXP term on the raw dimension ``other``"""
-    Dh = E + A
-    W = np.zeros((Dh + U, Dh + U)); W[E - A, E - A] = W[E - A + 1, E - A + 1] = 1.0; W[Dh, Dh] = 0.1
-    t = np.zeros(Dh + U); t[E - A + 1] = -1.0
-    Ws = np.zeros((E, E)); Ws[other, other] = 2.0
-    return [dict(kind=_lib.REWARD_EXP_SA, coef=1.0, W=W, t=t),
-            dict(kind=_lib.REWARD_EXP, coef=0.5, W=Ws, t=0.3 * np.ones(E)),
-            dict(kind=_lib.REWARD_LINEAR, coef=0.2, channel=_lib.CHANNEL_MULT, W=np.eye(E)[other], t=None)]
-
-
 def test_oracle_without_angles_is_the_oracle_without_angles():
-    """with angle_dims None or empty the angle oracle computes bitwise what particle_oracle and particle_grad_oracle
-    compute: rollouts of both samplers, the pathwise and consistent gradients, and the score gradient"""
+    """with angle_dims empty the oracles compute bitwise what they compute without angle_dims: rollouts of both
+    samplers, the pathwise and consistent gradients, and the score gradient"""
     dyn, rng = _host_problem(3, 0, 1, seed=1)
     pol = dict(kind=_lib.POLICY_LINEAR, squash=True, maxa=np.array([1.2]), W=rng.randn(1, 3), b=rng.randn(1))
     D = 4
@@ -218,16 +168,15 @@ def test_oracle_without_angles_is_the_oracle_without_angles():
     terms = _joint_terms(3, 1, 1, 0)[1:] + [joint]                 # the state terms and a joint term
     x0, eps = rng.randn(50, 3), rng.randn(50, 4, 3)
     same = lambda a, b: all(np.array_equal(u, v) for u, v in zip(a, b))
-    for mine, old in ((particle_rollout, po.particle_rollout), (consistent_rollout, po.consistent_rollout)):
-        ref = old(dyn, pol, terms, x0, eps, mult_mu=1.5)
-        for dims in ([], None):
-            assert same(mine(dyn, pol, terms, x0, eps, mult_mu=1.5, angle_dims=dims), ref)
-    for mine, old in ((value_and_grad, pgo.value_and_grad), (consistent_value_and_grad, pgo.consistent_value_and_grad)):
-        v0, g0 = old(dyn, pol, terms, x0, eps, 1.5)[:2]
-        v1, g1 = mine(dyn, pol, terms, x0, eps, 1.5, angle_dims=[])[:2]
+    for f in (particle_rollout, consistent_rollout):
+        ref = f(dyn, pol, terms, x0, eps, mult_mu=1.5)
+        assert same(f(dyn, pol, terms, x0, eps, mult_mu=1.5, angle_dims=[]), ref)
+    for f in (value_and_grad, consistent_value_and_grad):
+        v0, g0 = f(dyn, pol, terms, x0, eps, 1.5)[:2]
+        v1, g1 = f(dyn, pol, terms, x0, eps, 1.5, angle_dims=[])[:2]
         assert v0 == v1 and all(np.array_equal(g0[k], g1[k]) for k in g0)
-    traj = po.particle_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[0]
-    g0, g1 = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5), score_grad(dyn, pol, terms, traj, eps, 1.5)
+    traj = particle_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[0]
+    g0, g1 = score_grad(dyn, pol, terms, traj, eps, 1.5), score_grad(dyn, pol, terms, traj, eps, 1.5, angle_dims=[])
     assert all(np.array_equal(g0[k], g1[k]) for k in g0)
     x = rng.randn(4, 3)
     assert feature_map(x) is x
@@ -273,17 +222,6 @@ def test_oracle_pathwise_gradient_matches_central_differences():
         assert abs(fd - g["W"][0, j]) <= 1e-7 * max(1.0, abs(fd)), (j, fd, g["W"][0, j])
     fd = (val(W, b + h) - val(W, b - h)) / (2 * h)
     assert abs(fd - g["b"][0]) <= 1e-7 * max(1.0, abs(fd))
-
-
-class _FakeGP:
-    """stands in for a DeviceGP in the engine's checks before device work: struct() only"""
-    def __init__(self, n=40, D=6, E=4):
-        self.n, self.D, self.E = n, D, E
-
-    def struct(self):
-        g = _lib.GpModel()
-        g.n, g.D, g.E = self.n, self.D, self.E
-        return g
 
 
 def test_engine_checks_before_any_allocation():

@@ -1,10 +1,10 @@
 """CPU tests of the score-function gradient over consistent function samples (pilco_particles_consistent_score_grad_*,
-engine.ConsistentGradPlan(estimator="score"), DESIGN.md section 25): the torch oracle (tests/particle_cscore_oracle.py)
+engine.ConsistentGradPlan(estimator="score"), DESIGN.md section 25): the torch oracle (tests/particle_grad_oracle.py's
+score_grad(consistent=True))
 against autograd of the joint Gaussian log-density of each particle's path, against section 16's score gradient at
 H = 2 and, in expectation, against the consistent pathwise gradient; the status codes, their order and the workspace
 sizes of the C entry points on fake descriptors; the new kernel's registers and SASS; and the engine's checks before
 any allocation."""
-import ctypes as C
 import os
 import re
 import subprocess
@@ -15,32 +15,20 @@ import torch
 
 from pilco_b200 import _lib, engine
 from pilco_b200._lib import lib
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from abi_fakes import (ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _angle_particles, _angles, _batched, _grad,
+                       _noise, _particles, _score_grad_cases)
 from particle_cases import _problem, _terms
-import particle_cscore_oracle as pco
 import particle_grad_oracle as pgo
 import particle_oracle as po
-from test_particles_angles_host import _angle_particles, _angles
-from test_particles_noise_host import _noise
-from test_particles_score_host import _cases
-from util import CUOBJDUMP, ROOT, sass_named
+from util import CUOBJDUMP, ROOT, _ref, _rel, sass_named
 
 F64 = torch.float64
-
-
-def _ref(x):
-    return C.byref(x) if x is not None else None
 
 
 # ---- the oracle -------------------------------------------------------------------------------------------------------
 def _linear(rng, Ds, squash=True):
     return dict(kind=_lib.POLICY_LINEAR, squash=squash, maxa=np.array([1.2]), W=0.6 * rng.randn(1, Ds),
                 b=0.2 * rng.randn(1))
-
-
-def _rel(g, ref):
-    scale = max(float(np.abs(r).max()) for r in ref.values())
-    return max(float(np.abs(g[k] - ref[k]).max()) for k in ref) / scale
 
 
 def _joint_logdensity_grad(dyn, pol, traj):
@@ -73,7 +61,7 @@ def test_whitening_identity():
     P, H = 12, 5
     x0, eps = 0.5 + 0.2 * rng.randn(P, 3), rng.randn(P, H, 3)
     traj = po.consistent_rollout(dyn, pol, terms, x0, eps)[0]
-    g, ratio = pco.score_grad(dyn, pol, terms, traj, eps, w=np.ones((P, H - 1)), direct=False)
+    g, ratio = pgo.score_grad(dyn, pol, terms, traj, eps, w=np.ones((P, H - 1)), direct=False, consistent=True)
     ref = _joint_logdensity_grad(dyn, pol, traj)
     err = _rel(g, ref)
     print("whitening identity: %.1e of the gradient's scale, smallest pivot d2 / (tau sf2) %.1e" % (err, ratio))
@@ -90,7 +78,7 @@ def test_two_steps_is_the_step_wise_score_gradient(squash):
     P = 200
     x0, eps = 0.5 + 0.2 * rng.randn(P, 3), rng.randn(P, 2, 3)
     traj = po.consistent_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[0]
-    g, ratio = pco.score_grad(dyn, pol, terms, traj, eps, 1.5)
+    g, ratio = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5, consistent=True)
     ref = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5)
     err = _rel(g, ref)
     print("H = 2 against the step-wise score gradient: %.1e of the gradient's scale" % err)
@@ -109,7 +97,7 @@ def test_expected_gradient_is_the_consistent_pathwise_gradient():
         r = np.random.RandomState(2000 + k)
         x0, eps = 0.5 + 0.2 * r.randn(P, 3), r.randn(P, H, 3)
         traj = po.consistent_rollout(dyn, pol, terms, x0, eps, mult_mu=1.5)[0]
-        g, rt = pco.score_grad(dyn, pol, terms, traj, eps, 1.5)
+        g, rt = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5, consistent=True)
         gp = pgo.consistent_value_and_grad(dyn, pol, terms, x0, eps, 1.5)[1]
         ratio = min(ratio, rt)
         for key in score:
@@ -139,8 +127,8 @@ def test_degenerate_steps_are_dropped():
     P, H = 30, 4
     x0, eps = 0.5 + 0.1 * rng.randn(P, 3), rng.randn(P, H, 3)
     traj = po.consistent_rollout(dyn, pol, terms, x0, eps)[0]
-    g = pco.score_grad(dyn, pol, terms, traj, eps, w=np.ones((P, H - 1)), direct=False)[0]
-    one = pco.score_grad(dyn, pol, terms, traj[:, :3], eps[:, :2], w=np.ones((P, 1)), direct=False)[0]
+    g = pgo.score_grad(dyn, pol, terms, traj, eps, w=np.ones((P, H - 1)), direct=False, consistent=True)[0]
+    one = pgo.score_grad(dyn, pol, terms, traj[:, :3], eps[:, :2], w=np.ones((P, 1)), direct=False, consistent=True)[0]
     assert all(np.all(np.isfinite(g[k])) for k in g) and np.abs(one["b"]).max() > 0.0
     np.testing.assert_allclose(g["b"], one["b"], rtol=1e-12, atol=0.0)
 
@@ -165,7 +153,7 @@ def _path_ws(pr, ang, nz, R):
 def _all_cases():
     """(pr, ang, nz, R, g) rejected by the consistent pathwise call: section 16's plain cases, angles, noise and
     both, with bad variances, a missing nu and bad angle maps"""
-    out = [(pr, None, None, R, g) for pr, R, g, _ in _cases()]
+    out = [(pr, None, None, R, g) for pr, R, g, _ in _score_grad_cases()]
     for A in (1, 2):
         for kind in (_lib.POLICY_LINEAR, _lib.POLICY_RBF):
             out.append((_angle_particles(kind, A=A), _angles(*range(A)), None, 1, _grad()))

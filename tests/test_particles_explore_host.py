@@ -1,6 +1,6 @@
 """CPU tests of PILCO's exploration objective in the particle rollouts (pilco_particles_explore_*,
-pilco_particles_reward_moments, DESIGN.md section 24): the exploration oracle (tests/particle_explore_oracle.py) at
-b = 0 against the noise oracle, against central differences and, at step 0, against the closed-form reward variance;
+pilco_particles_reward_moments, DESIGN.md section 24): the exploration bonus of tests/particle_grad_oracle.py at b = 0
+against the call without it, against central differences and, at step 0, against the closed-form reward variance;
 the status codes, their order and the workspace sizes on fake descriptors; the new kernels' registers and SASS; and
 the engine's checks before any device work."""
 import ctypes as C
@@ -13,13 +13,13 @@ import pytest
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _grad, _particles
-import exploration_oracle as eo
-import particle_explore_oracle as peo
-import particle_noise_oracle as pno
-from test_particles_angles_host import _angle_particles, _angles, _host_problem, _FakeGP
-from test_particles_noise_host import _noise, _policy, _rbf_point, _ref
-from util import CUOBJDUMP, ROOT, sass
+from abi_fakes import (ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _FakeGP, _angle_particles, _angles, _batched, _grad,
+                       _noise, _particles)
+import action_reward_oracle as aro
+import particle_grad_oracle as pgo
+import particle_oracle as po
+from particle_cases import _host_problem, _policy, _rbf_point
+from util import CUOBJDUMP, ROOT, _ref, _round2, sass
 
 GRADS = ["batch_grad_", "consistent_grad_"]
 BOX_MULT = dict(kind=_lib.REWARD_BOX, coef=0.4, channel=_lib.CHANNEL_MULT,
@@ -115,10 +115,6 @@ def test_status_codes_and_order(feature):
     assert _calls(mk(), ang, nz, _ex(), g=g) == [ERR_NULL] * 2
 
 
-def _round2(n):
-    return n + (n & 1)
-
-
 @pytest.mark.parametrize("kind", [_lib.POLICY_LINEAR, _lib.POLICY_RBF])
 def test_workspace_sizes(kind):
     """the noisy / angle / plain gradient layout, then sigma_t [R,H] and the table [R,H,K,2]"""
@@ -201,10 +197,10 @@ def test_zero_b_is_the_noise_oracle_bitwise(dims, noisy):
     pol = _policy("linear", rng, U, E + A)
     x0, eps, nu = rng.randn(30, E), rng.randn(30, 4, E), rng.randn(30, 4, E)
     v = 0.02 * np.ones(E) if noisy else None
-    for mine, old in ((peo.value_and_grad, pno.value_and_grad),
-                      (peo.consistent_value_and_grad, pno.consistent_value_and_grad)):
-        v1, g1, sv = mine(dyn, pol, _terms(E, A, U), x0, eps, nu, v, 1.5, angle_dims=dims, b=0.0)
-        v0, g0 = old(dyn, pol, _terms(E, A, U), x0, eps, nu, v, 1.5, angle_dims=dims)[:2]
+    for f in (pgo.value_and_grad, pgo.consistent_value_and_grad):
+        out = f(dyn, pol, _terms(E, A, U), x0, eps, 1.5, angle_dims=dims, nu=nu, v=v, b=0.0)
+        (v1, g1), sv = out[:2], out[-1]
+        v0, g0 = f(dyn, pol, _terms(E, A, U), x0, eps, 1.5, angle_dims=dims, nu=nu, v=v)[:2]
         assert v0 == v1 and all(np.array_equal(g0[k], g1[k]) for k in g0)
         assert sv.shape == (4,) and np.all(sv > 0.0)
 
@@ -218,8 +214,8 @@ def test_oracle_gradient_matches_central_differences(kind, b):
     terms = _terms(E, A, U)
     x0, eps = rng.randn(25, E), rng.randn(25, 3, E)
     key, gkey = ("W", "W") if kind == "linear" else ("Xc", "X")
-    val = lambda p: peo.value_and_grad(dyn, p, terms, x0, eps, mult_mu=0.9, b=b)[0]
-    value, g, _ = peo.value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.9, b=b)
+    val = lambda p: pgo.value_and_grad(dyn, p, terms, x0, eps, mult_mu=0.9, b=b)[0]
+    value, g, _ = pgo.value_and_grad(dyn, pol, terms, x0, eps, mult_mu=0.9, b=b)
     h = 1e-5
     for j in range(E):
         lo, hi = dict(pol), dict(pol)
@@ -232,7 +228,7 @@ def test_oracle_gradient_matches_central_differences(kind, b):
 
 
 def test_step0_variance_matches_the_closed_form():
-    """sigma_0^2 over 10^6 draws of x0 ~ N(m0, S0) against exploration_oracle's closed-form Var at (m0, S0): exact for
+    """sigma_0^2 over 10^6 draws of x0 ~ N(m0, S0) against the closed-form Var at (m0, S0): exact for
     the state terms, and for the joint term under a linear unsquashed policy (then [x, u] is Gaussian)"""
     E, U = 3, 1
     rng = np.random.RandomState(23)
@@ -244,19 +240,19 @@ def test_step0_variance_matches_the_closed_form():
     x0 = rng.multivariate_normal(m0, S0, size=N)
     u = x0 @ W.T + bb
     traj, act = np.stack([x0, x0], 1), u[:, None]
-    got = peo.sample_moments(terms, traj, act)[1][0]
+    got = po.sample_moments(terms, traj, act)[1][0]
     mj = np.concatenate([m0, W @ m0 + bb])
     J = np.vstack([np.eye(E), W])
     Sj = J @ S0 @ J.T
-    T = eo.T
+    T = pgo.T
     want = 0.0
     q = np.zeros(N)                                          # per-draw sum_k c_k^2 (r_k - mean_k)^2: its spread is the SE
     for term in terms[:3]:
         joint = term["kind"] == _lib.REWARD_EXP_SA
         m, s = (mj, Sj) if joint else (m0, S0)
         c = term["coef"]
-        want += c * c * float(eo.term_var(term, T(m).reshape(1, -1), T(s)))
-        r = peo.po.point_value(term, x0, u)
+        want += c * c * float(aro.term_var(term, T(m).reshape(1, -1), T(s)))
+        r = po.point_value(term, x0, u)
         q += c * c * (r - r.mean()) ** 2
     se = q.std() / np.sqrt(N)
     assert abs(got - want) < 5.0 * se, (got, want, se)

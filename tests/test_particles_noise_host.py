@@ -1,8 +1,8 @@
 """CPU tests of the particle rollouts with measurement noise at the policy's input (pilco_particles_noisy_*, DESIGN.md
-section 23): the noise oracle (tests/particle_noise_oracle.py) against the angle oracle at v = 0, against central
-differences and against the exact noisy moments of one step; the status codes and workspace sizes of the ten entry
-points on fake descriptors; the pilco_particles_noise layout; the new kernels' registers and SASS; and the engine's
-checks before any device work."""
+section 23): the oracles' measurement noise (tests/particle_oracle.py and particle_grad_oracle.py) against their calls
+without it at v = 0, against central differences and against the exact noisy moments of one step; the status codes and
+workspace sizes of the ten entry points on fake descriptors; the pilco_particles_noise layout; the new kernels'
+registers and SASS; and the engine's checks before any device work."""
 import ctypes as C
 import os
 import re
@@ -13,29 +13,16 @@ import pytest
 
 from pilco_b200 import _lib
 from pilco_b200._lib import lib
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _grad, _particles
-import obs_noise_oracle as no
-import particle_angles_oracle as pao
+from abi_fakes import (ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, _FakeGP, _angle_particles, _angles, _batched, _grad,
+                       _noise, _particles)
+import action_reward_oracle as aro
 import particle_grad_oracle as pgo
-import particle_noise_oracle as pno
 import particle_oracle as po
 from oracle import torch_port as tp
-from test_particles_angles_host import _angle_particles, _angles, _host_problem, _joint_terms, _FakeGP
-from util import CUOBJDUMP, ROOT, make_gp_problem, sass
+from particle_cases import _host_problem, _joint_terms, _policy, _rbf_point
+from util import CUOBJDUMP, ROOT, _ref, _round2, make_gp_problem, sass
 
 NAMES = ["", "consistent_", "batch_grad_", "consistent_grad_", "score_grad_"]
-
-
-def _noise(var=(0.01, 0.02, 0.03), nu=FAKE):
-    n = _lib.ParticlesNoise()
-    for i, v in enumerate(var):
-        n.v.var[i] = v
-    n.nu = nu
-    return n
-
-
-def _ref(x):
-    return C.byref(x) if x is not None else None
 
 
 def _calls(pr, ang, nz, R=1, g=None):
@@ -132,10 +119,6 @@ def test_status_codes_and_order(angles):
     assert _calls(pr, ang, _noise(nu=None), g=g) == [ERR_NULL] * 5
 
 
-def _round2(n):
-    return n + (n & 1)
-
-
 @pytest.mark.parametrize("kind", [_lib.POLICY_LINEAR, _lib.POLICY_RBF])
 def test_workspace_sizes(kind):
     """forward-only: the angle call's bytes; gradients: the angle layouts with the phi history (also at A = 0), then
@@ -205,19 +188,9 @@ def test_new_kernels_have_no_local_memory():
 
 
 # ---- the oracle -------------------------------------------------------------------------------------------------------
-def _policy(kind, rng, U, Dh, squash=True):
-    if kind == "linear":
-        return dict(kind=_lib.POLICY_LINEAR, squash=squash, maxa=0.8 + rng.rand(U), W=0.5 * rng.randn(U, Dh),
-                    b=rng.randn(U))
-    bf = 8
-    return _rbf_point(dict(kind=_lib.POLICY_RBF, squash=squash, maxa=0.8 + rng.rand(U), Xc=rng.randn(bf, Dh),
-                           Yc=0.3 * rng.randn(bf, U), ell=1.0 + 0.2 * rng.rand(U, Dh), sf2=np.ones(U),
-                           sn2=1e-2 * np.ones(U)))
-
-
 @pytest.mark.parametrize("dims", [[], [1]])
 def test_zero_noise_is_the_angle_oracle_bitwise(dims):
-    """v = 0 (and v None): both samplers, the pathwise, consistent and score gradients are the angle oracle's"""
+    """v = 0 (and v None): both samplers, the pathwise, consistent and score gradients are the oracles' without v"""
     E, A, U = 3, len(dims), 1
     dyn, rng = _host_problem(E, A, U, seed=3)
     pol = _policy("linear", rng, U, E + A)
@@ -225,22 +198,20 @@ def test_zero_noise_is_the_angle_oracle_bitwise(dims):
     x0, eps, nu = rng.randn(40, E), rng.randn(40, 4, E), rng.randn(40, 4, E)
     same = lambda a, b: all(np.array_equal(u, w) for u, w in zip(a, b))
     for v in (None, np.zeros(E)):
-        assert same(pno.particle_rollout(dyn, pol, terms, x0, eps, nu, v, 1.5, dims),
-                    pao.particle_rollout(dyn, pol, terms, x0, eps, 1.5, dims))
-        assert same(pno.consistent_rollout(dyn, pol, terms, x0, eps, nu, v, 1.5, angle_dims=dims),
-                    pao.consistent_rollout(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims))
-        for mine, old in ((pno.value_and_grad, pao.value_and_grad),
-                          (pno.consistent_value_and_grad, pao.consistent_value_and_grad)):
-            v1, g1 = mine(dyn, pol, terms, x0, eps, nu, v, 1.5, angle_dims=dims)[:2]
-            v0, g0 = old(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims)[:2]
+        for f in (po.particle_rollout, po.consistent_rollout):
+            assert same(f(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims, nu=nu, v=v),
+                        f(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims))
+        for f in (pgo.value_and_grad, pgo.consistent_value_and_grad):
+            v1, g1 = f(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims, nu=nu, v=v)[:2]
+            v0, g0 = f(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims)[:2]
             assert v0 == v1 and all(np.array_equal(g0[k], g1[k]) for k in g0)
-        traj = pao.particle_rollout(dyn, pol, terms, x0, eps, 1.5, dims)[0]
-        g0 = pao.score_grad(dyn, pol, terms, traj, eps, 1.5, angle_dims=dims)
-        g1 = pno.score_grad(dyn, pol, terms, traj, eps, nu, v, 1.5, angle_dims=dims)
+        traj = po.particle_rollout(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims)[0]
+        g0 = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5, angle_dims=dims)
+        g1 = pgo.score_grad(dyn, pol, terms, traj, eps, 1.5, angle_dims=dims, nu=nu, v=v)
         assert all(np.array_equal(g0[k], g1[k]) for k in g0)
     # with noise the actions move, the first state does not
-    a = pno.particle_rollout(dyn, pol, terms, x0, eps, nu, 0.05 * np.ones(E), 1.5, dims)
-    b = pao.particle_rollout(dyn, pol, terms, x0, eps, 1.5, dims)
+    a = po.particle_rollout(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims, nu=nu, v=0.05 * np.ones(E))
+    b = po.particle_rollout(dyn, pol, terms, x0, eps, 1.5, angle_dims=dims)
     assert np.array_equal(a[0][:, 0], b[0][:, 0]) and not np.array_equal(a[1], b[1])
 
 
@@ -257,8 +228,8 @@ def test_oracle_pathwise_gradient_matches_central_differences(kind, dims):
     v = np.array([0.03, 0.0, 0.05, 0.02])
     key = "W" if kind == "linear" else "Xc"
     gkey = "W" if kind == "linear" else "X"
-    val = lambda p: pno.particle_rollout(dyn, p, terms, x0, eps, nu, v, 0.9, dims)[4].mean()
-    value, g = pno.value_and_grad(dyn, pol, terms, x0, eps, nu, v, 0.9, angle_dims=dims)
+    val = lambda p: po.particle_rollout(dyn, p, terms, x0, eps, 0.9, angle_dims=dims, nu=nu, v=v)[4].mean()
+    value, g = pgo.value_and_grad(dyn, pol, terms, x0, eps, 0.9, angle_dims=dims, nu=nu, v=v)
     assert abs(value - val(pol)) <= 1e-12 * max(1.0, abs(value))
     h = 1e-5
     for j in range(E + A):
@@ -271,15 +242,9 @@ def test_oracle_pathwise_gradient_matches_central_differences(kind, dims):
         assert abs(fd - g[gkey][0, j]) <= 1e-7 * max(1.0, abs(fd)), (j, fd, g[gkey][0, j])
 
 
-def _rbf_point(pol):
-    """the numpy oracle's RBF policy (C, ell, sf2, beta) of pgo's parametrisation (Xc, Yc, ell, sf2, sn2)"""
-    beta = pgo.rbf_beta(pgo.T(pol["Xc"]), pgo.T(pol["Yc"]), pgo.T(pol["ell"]), pol["sf2"], pol["sn2"])
-    return dict(pol, C=pol["Xc"], beta=beta.detach().numpy())
-
-
 def test_one_step_matches_the_noisy_moments():
     """H = 1, a linear unsquashed policy, no angles: x_1's sample moments over 2 10^5 particles match
-    obs_noise_oracle's exact noisy step moments; without the noise they do not"""
+    the moment-matching oracle's exact noisy step moments; without the noise they do not"""
     E, U = 3, 2
     X, Y, ell, sf2, sn2 = make_gp_problem(40, E + U, E, seed=7)
     Y = 0.1 * Y
@@ -289,16 +254,16 @@ def test_one_step_matches_the_noisy_moments():
     B = rng.randn(E, E)
     m0, S0 = X[0, :E], 0.03 * B @ B.T + 0.02 * np.eye(E)
     terms = [dict(kind=1, coef=1.0, W=np.ones(E), t=None)]
-    T = no.T
-    ref = no.problem_rollout("linear", [T(W), T(b)], X, Y, ell, sf2, sn2, None, terms, T(m0), T(S0), 1, 0.0, v)
-    bare = no.problem_rollout("linear", [T(W), T(b)], X, Y, ell, sf2, sn2, None, terms, T(m0), T(S0), 1, 0.0,
-                              np.zeros(E))
+    T = pgo.T
+    ref = aro.problem_rollout("linear", [T(W), T(b)], X, Y, ell, sf2, sn2, None, terms, T(m0), T(S0), 1, v=v)
+    bare = aro.problem_rollout("linear", [T(W), T(b)], X, Y, ell, sf2, sn2, None, terms, T(m0), T(S0), 1,
+                               v=np.zeros(E))
     iK, beta = tp.calculate_factorizations(T(X), T(Y), T(ell), T(sf2), T(sn2))
     dyn = dict(C=X, ell=ell, sf2=sf2, iK=iK.numpy(), beta=beta.numpy())
     pol = dict(kind=_lib.POLICY_LINEAR, squash=False, maxa=np.ones(U), W=W, b=b)
     N = 200000
     x0 = rng.multivariate_normal(m0, S0, size=N)
-    traj = pno.particle_rollout(dyn, pol, terms, x0, rng.randn(N, 1, E), rng.randn(N, 1, E), v)[0]
+    traj = po.particle_rollout(dyn, pol, terms, x0, rng.randn(N, 1, E), nu=rng.randn(N, 1, E), v=v)[0]
     worst = po.moment_check(traj[:, 1], ref["traj_m"][1].numpy(), ref["traj_S"][1].numpy())
     assert worst < 5.0, worst
     assert po.moment_check(traj[:, 1], bare["traj_m"][1].numpy(), bare["traj_S"][1].numpy()) > 5.0

@@ -19,14 +19,10 @@ from pilco_b200._lib import lib
 from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
 from particle_cases import _problem, _terms
 import particle_oracle as po
-import particle_resample_oracle as pro
-from util import CUOBJDUMP, ROOT, sass_named
+import particle_grad_oracle as pgo
+from util import CUOBJDUMP, ROOT, _ref, sass_named
 
 NEW_KERNELS = ["pr_close_kernel", "pr_moments_kernel", "pr_step_kernel", "pr_adjoint_kernel", "pr_scatter_kernel"]
-
-
-def _ref(x):
-    return C.byref(x) if x is not None else None
 
 
 # ---- the refit's Cholesky and its reverse, host-compiled ---------------------------------------------------------------
@@ -70,7 +66,7 @@ def test_host_cholesky_and_adjoint_are_the_oracle(chol_host, n, rank):
         S[2] = S[:, 2] = 0.0                                    # a zero variance: a degenerate column in the middle
     Lb = rng.randn(n, n)
     L, Sb = chol_host(S, Lb)
-    Lr, Sbr = pro.chol_np(S), pro.chol_bwd_np(S, np.tril(Lb))
+    Lr, Sbr = pgo.chol_np(S), pgo.chol_bwd_np(S, np.tril(Lb))
     scale = max(np.abs(Sbr).max(), 1e-300)
     print("n=%d rank=%s: factor %.1e, adjoint %.1e of scale, degenerate columns %d" % (
         n, rank, np.abs(L - Lr).max() / np.abs(Lr).max(), np.abs(Sb - Sbr).max() / scale, int((np.diag(L) == 0).sum())))
@@ -93,12 +89,12 @@ def test_oracle_gradient_is_a_central_difference():
     terms = _terms(3)
     P, H = 40, 5
     x0, eps, xi = 0.5 + 0.2 * rng.randn(P, 3), rng.randn(P, H, 3), rng.randn(P, H, 3)
-    ref = pro.rollout(dyn, pol, terms, x0, eps, xi, mult_mu=1.5)
+    ref = pgo.resampled_rollout(dyn, pol, terms, x0, eps, xi, mult_mu=1.5)
     v = {"W": rng.randn(1, 3), "b": rng.randn(1)}
     gv = sum(float((ref["grad"][k].reshape(v[k].shape) * v[k]).sum()) for k in v)
     h = 1e-6
-    val = lambda s: pro.rollout(dyn, dict(pol, W=pol["W"] + s * v["W"], b=pol["b"] + s * v["b"]), terms, x0, eps, xi,
-                                mult_mu=1.5)["value"]
+    val = lambda s: pgo.resampled_rollout(dyn, dict(pol, W=pol["W"] + s * v["W"], b=pol["b"] + s * v["b"]), terms, x0,
+                                          eps, xi, mult_mu=1.5)["value"]
     cd = (val(h) - val(-h)) / (2 * h)
     print("oracle: central difference %.12e, g'v %.12e" % (cd, gv))
     assert abs(cd - gv) <= 1e-7 * max(abs(gv), 1.0)
@@ -109,7 +105,7 @@ def test_oracle_is_the_step_wise_sampler_at_one_step():
     pol = _linear(rng, 3)
     P = 30
     x0, eps, xi = 0.5 + 0.2 * rng.randn(P, 3), rng.randn(P, 1, 3), rng.randn(P, 1, 3)
-    ref = pro.rollout(dyn, pol, _terms(3), x0, eps, xi, mult_mu=1.5)
+    ref = pgo.resampled_rollout(dyn, pol, _terms(3), x0, eps, xi, mult_mu=1.5)
     plain = po.particle_rollout(dyn, pol, _terms(3), x0, eps, mult_mu=1.5)
     np.testing.assert_allclose(ref["ret"], plain[4], rtol=1e-13, atol=1e-13)
     np.testing.assert_allclose(ref["xp"][0], plain[0][:, 1], rtol=1e-13, atol=1e-13)
@@ -124,7 +120,7 @@ def test_oracle_moments_are_the_moment_matching_trajectory():
     m0, S0 = np.array([0.5, 0.4, 0.6]), 0.02 * np.eye(3)
     x0 = m0[None] + rng.randn(P, 3) @ np.linalg.cholesky(S0).T
     eps, xi = rng.randn(P, H, 3), rng.randn(P, H, 3)
-    ref = pro.rollout(dyn, pol, terms, x0, eps, xi)
+    ref = pgo.resampled_rollout(dyn, pol, terms, x0, eps, xi)
     m, s = m0[None], S0
     C_, ell, sf2 = dyn["C"], dyn["ell"], dyn["sf2"]
     worst = po.moment_check(x0, m[0], s)

@@ -13,7 +13,7 @@ import torch
 
 from pilco_b200 import _lib, engine
 from pilco_b200._lib import lib
-from abi_fakes import ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, PT_MAX_P, _batched, _grad, _particles
+from abi_fakes import ERR_DIM, ERR_WS, PT_MAX_P, _batched, _grad, _particles, _score_grad_cases
 from particle_cases import _problem
 from particle_oracle import particle_rollout
 from particle_grad_oracle import score_grad, value_and_grad
@@ -145,57 +145,8 @@ def _batch_run(pr, R, g):
                                                   C.byref(g) if g is not None else None, None)
 
 
-def _cases():
-    """(description, R, grad, expected status): every call is rejected before anything is enqueued"""
-    out = [(None, 3, _grad(), ERR_NULL), (_batched(), 3, None, ERR_NULL)]
-    for kind in (_lib.POLICY_LINEAR, _lib.POLICY_RBF):
-        for rk in (_lib.REWARD_EXP, _lib.REWARD_LINEAR, _lib.REWARD_BOX):
-            for ch in (_lib.CHANNEL_ADD, _lib.CHANNEL_MULT):
-                out.append((_batched(kind, reward_kind=rk, channel=ch), 3, _grad(), ERR_WS))
-        out.append((_particles(kind), 3, _grad(), ERR_WS))                 # stride 0: one policy shared by all
-        out.append((_particles(kind), 1, _grad(), ERR_WS))                 # R = 1, unbatched
-    out.append((_particles(H=0), 1, _grad(), ERR_WS))
-    out.append((_particles(H=1), 1, _grad(), ERR_WS))
-    for R in (0, -1, 65536):
-        out.append((_batched(), R, _grad(), ERR_DIM))
-    out.append((_batched(P=1000), PT_MAX_P // 1000 + 1, _grad(), ERR_DIM))
-    out.append((_batched(P=1), 65535, _grad(), ERR_WS))
-    for field in ("W_bs", "b_bs"):
-        pr = _batched(); setattr(pr.pol, field, -3)
-        out.append((pr, 3, _grad(), ERR_DIM))
-    for field in ("X_bs", "ell_bs", "sf2_bs", "beta_bs"):
-        pr = _batched(_lib.POLICY_RBF); setattr(pr.pol.rbf, field, -1)
-        out.append((pr, 3, _grad(), ERR_DIM))
-        pr = _batched(); setattr(pr.dyn, field, 7)                         # batched dynamics
-        out.append((pr, 3, _grad(), ERR_UNSUP))
-    for P, H in ((0, 5), (PT_MAX_P + 1, 5), (10, -1)):
-        out.append((_batched(P=P, H=H), 1, _grad(), ERR_DIM))
-    for field in ("x0", "eps", "traj", "act", "step_reward", "step_risk", "ret"):
-        pr = _batched(); setattr(pr, field, None)
-        out.append((pr, 3, _grad(), ERR_NULL))
-    pr = _batched(_lib.POLICY_RBF); pr.pol.rbf.mode = 0
-    out.append((pr, 3, _grad(), ERR_UNSUP))
-    pr = _batched(); pr.dyn.iK = None
-    out.append((pr, 3, _grad(), ERR_UNSUP))
-    out.append((_batched(kind=7), 3, _grad(), ERR_UNSUP))
-    pr = _batched(); pr.dyn.E = 4
-    out.append((pr, 3, _grad(), ERR_DIM))
-    pr = _batched(); pr.dyn.iK = FAKE + 8
-    out.append((pr, 3, _grad(), ERR_ALIGN))
-    for field in ("value", "ws", "gW", "gb"):
-        g = _grad(); setattr(g, field, None)
-        out.append((_batched(), 3, g, ERR_NULL))
-    for field in ("gXc", "gYc", "gell", "pol_L"):
-        g = _grad(); setattr(g, field, None)
-        out.append((_batched(_lib.POLICY_RBF), 3, g, ERR_NULL))
-        out.append((_batched(), 3, g, ERR_WS))                             # not needed by the linear policy
-    g = _grad(); g.ws = FAKE + 8; g.ws_bytes = 1 << 40
-    out.append((_batched(), 3, g, ERR_ALIGN))
-    return out
-
-
 def test_score_grad_argument_validation():
-    for i, (pr, R, g, want) in enumerate(_cases()):
+    for i, (pr, R, g, want) in enumerate(_score_grad_cases()):
         assert _run(pr, R, g) == want, i
         assert _batch_run(pr, R, g) == want, i                             # the batched pathwise entry point's codes
     for kind in (_lib.POLICY_LINEAR, _lib.POLICY_RBF):                      # a workspace short of the score layout's

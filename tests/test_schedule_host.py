@@ -1,5 +1,6 @@
 """CPU tests of the time-varying linear policy (pilco_rollout_scheduled_*, DESIGN.md section 27): the torch oracle
-(tests/schedule_oracle.py) against central differences and, with a constant schedule, against the stationary oracle;
+(tests/action_reward_oracle.py's cascade under step_action) against central differences and, with a constant
+schedule, against the cascade under the stationary policy;
 and the library side that needs no GPU: exported symbols, the pilco_policy_schedule layout, status codes and their
 order on fake descriptors, workspace sizes, the new kernel's register budget, and the Python refusals raised before
 any device work."""
@@ -12,12 +13,13 @@ import numpy as np
 import pytest
 import torch
 
-import obs_noise_oracle as no
-import schedule_oracle as so
+import action_reward_oracle as aro
+import particle_grad_oracle as pgo
+from oracle import torch_port as tp
 from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _rollout
 from util import CUOBJDUMP, ROOT, make_gp_problem, sass
 
-T = so.T
+T = pgo.T
 
 
 def _problem(Ds=2, U=1, H=3, dims=(), seed=4):
@@ -28,7 +30,7 @@ def _problem(Ds=2, U=1, H=3, dims=(), seed=4):
     maxa = 0.8 + rng.rand(U)
     B = rng.randn(Ds, Ds)
     terms = [dict(kind=0, coef=1.0, W=np.diag(0.5 + rng.rand(Ds)), t=0.3 * rng.randn(Ds))]
-    return so.dynamics(X, 0.1 * Y, ell, sf2, sn2), Ws, bs, maxa, terms, X[0, :Ds], 0.05 * B @ B.T + 0.02 * np.eye(Ds)
+    return aro.dynamics(X, 0.1 * Y, ell, sf2, sn2), Ws, bs, maxa, terms, X[0, :Ds], 0.05 * B @ B.T + 0.02 * np.eye(Ds)
 
 
 @pytest.mark.parametrize("dims,v", [((), None), ((1,), [0.01, 0.02])])
@@ -36,10 +38,10 @@ def test_oracle_gradient_matches_central_differences(dims, v):
     dyn, Ws, bs, maxa, terms, m0, S0 = _problem(dims=dims)
     H = Ws.shape[0]
     Wt, bt = T(Ws).requires_grad_(), T(bs).requires_grad_()
-    out = so.scheduled_rollout(dyn, Wt, bt, maxa, terms, m0, S0, H, v=v, angle_dims=list(dims) or None)
+    out = aro.mm_rollout(dyn, aro.step_action(Wt, bt, maxa), terms, m0, S0, H, angle_dims=list(dims) or None, v=v)
     gW, gb = torch.autograd.grad(out["reward"], (Wt, bt))
-    f = lambda W, b: float(so.scheduled_rollout(dyn, T(W), T(b), maxa, terms, m0, S0, H, v=v,
-                                                angle_dims=list(dims) or None)["reward"])
+    f = lambda W, b: float(aro.mm_rollout(dyn, aro.step_action(T(W), T(b), maxa), terms, m0, S0, H,
+                                          angle_dims=list(dims) or None, v=v)["reward"])
     h = 1e-6
     for t in range(H):                                    # every step has its own derivative
         e = np.zeros_like(bs); e[t, 0] = h
@@ -54,9 +56,10 @@ def test_constant_schedule_is_the_stationary_oracle():
     dyn, Ws, bs, maxa, terms, m0, S0 = _problem()
     H = Ws.shape[0]
     W, b = Ws[0], bs[0]
-    sched = so.scheduled_rollout(dyn, T(np.repeat(W[None], H, 0)), T(np.repeat(b[None], H, 0)), maxa, terms, m0, S0, H)
-    act = lambda m, s: so.tp.linear_action(T(W), T(b).reshape(1, -1), m, s, T(maxa)[None])
-    ref = no.noisy_rollout(dyn, act, terms, T(m0), T(S0), H, 0.0, torch.zeros(len(m0), dtype=torch.float64))
+    sched = aro.mm_rollout(dyn, aro.step_action(T(np.repeat(W[None], H, 0)), T(np.repeat(b[None], H, 0)), maxa), terms,
+                           m0, S0, H)
+    act = lambda m, s: tp.linear_action(T(W), T(b).reshape(1, -1), m, s, T(maxa)[None])
+    ref = aro.mm_rollout(dyn, act, terms, T(m0), T(S0), H)
     for k in ("traj_m", "traj_S", "reward", "step_reward"):
         assert torch.equal(sched[k], ref[k]), k
 

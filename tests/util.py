@@ -1,5 +1,6 @@
 """Shared test helpers: seeded synthetic problems (SURVEY.md section 8d recipe), error metrics and the SASS of the
 built library."""
+import ctypes
 import functools
 import os
 import re
@@ -111,3 +112,88 @@ def oracle_rollout(P, r, H, dyn_fact=None, centres=None):
                       lambda m, s: pp.rbf_action(P["Xc"][r], P["Yc"][r], P["lc"][r], m, s, True, P["maxa"][None]),
                       lambda m, s: pp.predict_given_factorizations(C, P["ell"], P["sf2"], m, s, iK, beta),
                       lambda m, s: pp.exponential_reward(m, s, P["W"], P["t"][None]))
+
+
+def _rel(g, ref):
+    """the largest difference of the gradient dicts g and ref, relative to ref's largest entry"""
+    scale = max(float(np.abs(r).max()) for r in ref.values())
+    return max(float(np.abs(g[k].reshape(ref[k].shape) - ref[k]).max()) for k in ref) / scale
+
+
+def _zscores(a, b=None, ref=None):
+    """largest |mean| / standard error of a - b (paired draws) or of a against the constant ref"""
+    worst = 0.0
+    for k in a:
+        d = np.stack(a[k]) - (np.stack(b[k]) if b is not None else ref[k])
+        worst = max(worst, float(np.max(np.abs(d.mean(0)) / (d.std(0, ddof=1) / np.sqrt(d.shape[0])))))
+    return worst
+
+
+def _ref(x):
+    """a ctypes reference to x, or NULL for None"""
+    return ctypes.byref(x) if x is not None else None
+
+
+def _round2(n):
+    """n rounded up to even: the workspace slots' 16-byte alignment in doubles"""
+    return n + (n & 1)
+
+
+# ---- the host build of trig_math.cuh (tests/host_harness/trig_harness.cpp) -------------------------------------------
+_dp = ctypes.POINTER(ctypes.c_double)
+
+
+def trig_harness(so):
+    """compile the host harness of the angular feature map's closed forms into the shared library ``so`` and load it"""
+    subprocess.check_call(["g++", "-O1", "-shared", "-fPIC", "-x", "c++", "-o", so,
+                           os.path.join(ROOT, "tests", "host_harness", "trig_harness.cpp")])
+    lib = ctypes.CDLL(so)
+    ip = ctypes.POINTER(ctypes.c_int)
+    lib.trig_moments_host.argtypes = [ctypes.c_int, ctypes.c_int, ip] + [_dp] * 5
+    lib.trig_vjp_host.argtypes = [ctypes.c_int, ctypes.c_int, ip] + [_dp] * 7
+    lib.angles_layout.argtypes = [ctypes.POINTER(ctypes.c_size_t)]
+    return lib
+
+
+def _p(a):
+    return np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(_dp)
+
+
+def host_moments(lib, m, s, dims):
+    Ds, A = len(m), len(dims)
+    Dh = Ds + A
+    M, S, C = np.zeros(Dh), np.zeros((Dh, Dh)), np.zeros((Ds, Dh))
+    m, s = np.ascontiguousarray(m, dtype=np.float64), np.ascontiguousarray(s, dtype=np.float64)
+    d = (ctypes.c_int * max(A, 1))(*dims)
+    assert lib.trig_moments_host(Ds, A, d, _p(m), _p(s), M.ctypes.data_as(_dp), S.ctypes.data_as(_dp),
+                                 C.ctypes.data_as(_dp)) == 0
+    return M, S, C
+
+
+def host_vjp(lib, m, s, dims, gM, gS, gC):
+    Ds, A = len(m), len(dims)
+    gm, gs = np.zeros(Ds), np.zeros((Ds, Ds))
+    arrs = [np.ascontiguousarray(a, dtype=np.float64) for a in (m, s, gM, gS, gC)]
+    d = (ctypes.c_int * max(A, 1))(*dims)
+    assert lib.trig_vjp_host(Ds, A, d, *[a.ctypes.data_as(_dp) for a in arrs], gm.ctypes.data_as(_dp),
+                             gs.ctypes.data_as(_dp)) == 0
+    return gm, gs
+
+
+def _trig_cases():
+    rng = np.random.RandomState(7)
+    out = []
+    for Ds, dims in ((2, [0]), (4, [2]), (4, [1, 3]), (3, [2, 0, 1]), (6, [4, 1])):
+        B = rng.randn(Ds, Ds)
+        out.append(("random", rng.randn(Ds) * 2, 0.3 * B @ B.T, dims))
+    out.append(("zero_cov", np.array([0.3, -2.0, 1.1]), np.zeros((3, 3)), [1, 2]))
+    s = np.diag([0.2, 10.0, 0.5]); s[0, 2] = s[2, 0] = 0.1
+    out.append(("saa_10", np.array([0.5, 1.0, -0.7]), s, [1]))
+    L = np.array([[1.0, 0.0, 0.0], [0.999, 0.0447, 0.0], [0.2, 0.1, 0.5]])
+    out.append(("correlated_angles", np.array([0.4, -1.3, 0.2]), 0.8 * L @ L.T, [0, 1]))
+    v = rng.randn(4)
+    out.append(("singular", rng.randn(4), np.outer(v, v), [0, 3]))
+    return out
+
+
+TRIG_CASES = _trig_cases()     # (name, m [Ds], s [Ds,Ds], angle dims)
