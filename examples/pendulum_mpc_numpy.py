@@ -2,8 +2,9 @@
 examples/pendulum_numpy.py: a few episodes of random torques train the dynamics GPs (optimize_models), then at every
 control step ``PILCO.plan`` optimises a torque sequence (TimeVaryingLinearController(feedback=False)) over the horizon
 through the moment-matching cascade from the measured state, applies its first action and keeps the rest as the next
-step's warm start.  No global policy is learnt.  Usage:
-    python examples/pendulum_mpc_numpy.py [--episodes 2] [--angles]"""
+step's warm start.  No global policy is learnt.  ``--num-samples S`` plans on the mean return of S particle rollouts
+of the learnt dynamics instead of the moment-matching cascade (``PILCO.plan(num_samples=S)``).  Usage:
+    python examples/pendulum_mpc_numpy.py [--episodes 2] [--angles] [--num-samples 256]"""
 import argparse
 import os
 import sys
@@ -24,9 +25,11 @@ def task_reward(x):
     return float(np.exp(-0.5 * ((x[0] - TARGET[0]) ** 2 + 0.1 * x[1] ** 2)))
 
 
-def run(episodes=2, T=25, horizon=10, random_episodes=3, restarts=2, maxiter=10, angles=False, verbose=True, seed=0):
+def run(episodes=2, T=25, horizon=10, random_episodes=3, restarts=2, maxiter=10, angles=False, verbose=True, seed=0,
+        num_samples=None):
     """-> (the returns of the random episodes, the returns of the MPC episodes): sum over the T steps of
-    exp(-((theta - pi/3)^2 + 0.1 omega^2) / 2) at the states reached"""
+    exp(-((theta - pi/3)^2 + 0.1 omega^2) / 2) at the states reached.  ``num_samples``: plan on that many particles
+    (seeded per control step), or None for the moment-matching plan"""
     np.random.seed(seed)
     env = PendulumEnv(seed=seed)
     X, Y, random_returns = [], [], []
@@ -45,8 +48,9 @@ def run(episodes=2, T=25, horizon=10, random_episodes=3, restarts=2, maxiter=10,
     mpc_returns = []
     for ep in range(episodes):
         x, ret, Xe, Ye = env.reset(), 0.0, [], []
-        for _ in range(T):
-            u = np.asarray(pilco.plan(x, maxiter=maxiter, restarts=restarts)).reshape(control_dim)
+        for k in range(T):
+            sampled = {} if num_samples is None else dict(num_samples=num_samples, seed=seed + 1000 * ep + k)
+            u = np.asarray(pilco.plan(x, maxiter=maxiter, restarts=restarts, **sampled)).reshape(control_dim)
             x_new = env.step(u[0])
             Xe.append(np.hstack((x, u))); Ye.append(x_new - x)
             ret += task_reward(x_new)
@@ -64,5 +68,6 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--episodes", type=int, default=2)
     ap.add_argument("--angles", action="store_true", help="treat theta as an angle (sin / cos features)")
+    ap.add_argument("--num-samples", type=int, default=None, help="plan on the mean return of this many particles")
     a = ap.parse_args()
-    run(episodes=a.episodes, angles=a.angles)
+    run(episodes=a.episodes, angles=a.angles, num_samples=a.num_samples)

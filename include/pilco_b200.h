@@ -741,6 +741,71 @@ size_t pilco_particles_resampled_grad_workspace_bytes(const pilco_particles* pr,
 int    pilco_particles_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs, int R,
                                               const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* Time-varying linear policies in the particle rollouts (DESIGN.md section 28): each call is the most general call of
+ * its family (pilco_particles_noisy_*, _explore_*, _consistent_score_grad_*, _resampled_*) with a pilco_policy_schedule
+ * (section 27's) added.  Restart r at step t = 0 .. H-1 applies u_t = W_t z + b_t (squashed when pol.squash, z the
+ * policy's input as in the call without a schedule) with
+ *   W_t = pol.W + r pol.W_bs + t W_ts   [U, Dh],     b_t = pol.b + r pol.b_bs + t b_ts   [U].
+ * W_t = 0 at every step is an open-loop action sequence.  The schedule is active when sch != NULL and W_ts or b_ts is
+ * non-zero; an inactive call is the call without it: outputs, gradients, workspace sizes and status codes.  With an
+ * active schedule the gradients are per step, g->gW [R, H, U, Dh] and g->gb [R, H, U] (their sum over t is the
+ * stationary policy's gradient); value and the workspace are the call's without a schedule.  Validation before any
+ * work is enqueued: the call's status codes up to its workspace check, then PILCO_ERR_DIM for a negative stride, then
+ * PILCO_ERR_UNSUPPORTED for an active schedule with an RBF policy, then the workspace's codes.  A size query returns 0
+ * where the call's without a schedule does, and for a negative stride. */
+size_t pilco_particles_scheduled_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                 const pilco_particles_noise* nz, const pilco_policy_schedule* sch);
+int    pilco_particles_scheduled_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                         const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                         pilco_stream_t stream);
+size_t pilco_particles_scheduled_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_policy_schedule* sch);
+int    pilco_particles_scheduled_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                    const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                                    pilco_stream_t stream);
+size_t pilco_particles_scheduled_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_exploration* ex,
+                                                            const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                    const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                    const pilco_policy_schedule* sch, int R,
+                                                    const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_scheduled_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                                 const pilco_particles_noise* nz,
+                                                                 const pilco_exploration* ex,
+                                                                 const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                         const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                         const pilco_policy_schedule* sch, int R,
+                                                         const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_scheduled_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                    const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                                    int R, const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_scheduled_consistent_score_grad_workspace_bytes(const pilco_particles* pr,
+                                                                       const pilco_angles* ang,
+                                                                       const pilco_particles_noise* nz,
+                                                                       const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_consistent_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                               const pilco_particles_noise* nz,
+                                                               const pilco_policy_schedule* sch, int R,
+                                                               const pilco_particles_grad* g, pilco_stream_t stream);
+size_t pilco_particles_scheduled_resampled_workspace_bytes(const pilco_particles* pr,
+                                                           const pilco_particles_resample* rs,
+                                                           const pilco_policy_schedule* sch);
+int    pilco_particles_scheduled_resampled_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                   const pilco_policy_schedule* sch, pilco_stream_t stream);
+size_t pilco_particles_scheduled_resampled_grad_workspace_bytes(const pilco_particles* pr,
+                                                                const pilco_particles_resample* rs,
+                                                                const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                        const pilco_policy_schedule* sch, int R,
+                                                        const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -236,6 +236,38 @@ SIGNATURES = {
                                                                     C.c_int]),
     "pilco_particles_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample), C.c_int,
                                                          C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule)]),
+    "pilco_particles_scheduled_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), c_dp]),
+    "pilco_particles_scheduled_consistent_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule)]),
+    "pilco_particles_scheduled_consistent_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), c_dp]),
+    "pilco_particles_scheduled_batch_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(Exploration),
+                                                                                 C.POINTER(PolicySchedule), C.c_int]),
+    "pilco_particles_scheduled_batch_grad_rollout": (C.c_int, _PAN + [C.POINTER(Exploration), C.POINTER(PolicySchedule),
+                                                                      C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_consistent_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(Exploration),
+                                                                                      C.POINTER(PolicySchedule),
+                                                                                      C.c_int]),
+    "pilco_particles_scheduled_consistent_grad_rollout": (C.c_int, _PAN + [C.POINTER(Exploration),
+                                                                           C.POINTER(PolicySchedule), C.c_int,
+                                                                           C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_score_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule), C.c_int]),
+    "pilco_particles_scheduled_score_grad_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), C.c_int,
+                                                                      C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_consistent_score_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule),
+                                                                                            C.c_int]),
+    "pilco_particles_scheduled_consistent_score_grad_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), C.c_int,
+                                                                                 C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_resampled_workspace_bytes": (C.c_size_t, [C.POINTER(Particles),
+                                                                         C.POINTER(ParticlesResample),
+                                                                         C.POINTER(PolicySchedule)]),
+    "pilco_particles_scheduled_resampled_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample),
+                                                              C.POINTER(PolicySchedule), c_dp]),
+    "pilco_particles_scheduled_resampled_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles),
+                                                                              C.POINTER(ParticlesResample),
+                                                                              C.POINTER(PolicySchedule), C.c_int]),
+    "pilco_particles_scheduled_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample),
+                                                                   C.POINTER(PolicySchedule), C.c_int,
+                                                                   C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

@@ -37,6 +37,9 @@
 // section 25): ps_run on the consistent forward; pc_white_kernel (particles_cscore.cu) turns the weights into the
 // cotangents of every step's mean' and var', which the reverse of the conditioning and the predict VJP carry to
 // x~_bar_t step by step.
+// Time-varying linear policies (pilco_particles_scheduled_*, DESIGN.md section 28): pt_forward and pg_reverse hand step
+// t's launches W + t W_ts and b + t b_ts; ps_zbar_sched_kernel and pg_sched_kernel stand in for the two kernels that
+// cover all H steps in one grid (ps_zbar_kernel, pg_param_kernel).
 #include <cmath>
 #include "particles.cuh"
 
@@ -749,6 +752,83 @@ __global__ void __launch_bounds__(PT_THREADS) ps_zbar_kernel(PsDev a) {
     }
 }
 
+// ---- time-varying linear policy (pilco_particles_scheduled_*, DESIGN.md section 28) ---------------------------------
+// Restart r at step t applies W_t = W + r W_bs + t W_ts and b_t = b + r b_bs + t b_ts.  The per-step kernels read the
+// policy through their launch's W and b, which the drivers advance by t W_ts and t b_ts; the two kernels below cover
+// all H steps in one grid, so they take the step strides themselves.  Linear policies only.
+struct PsSched : PsDev {
+    long long W_ts, b_ts;
+};
+
+// ps_zbar_kernel under a schedule: its grid and its z_bar_t, with z_t from step t's W_t and b_t in pt_step_kernel's
+// order.  The linear policy's output variance is 0, so maxa e^{-su/2} is maxa exactly.
+__global__ void __launch_bounds__(PT_THREADS) ps_zbar_sched_kernel(PsSched a) {
+    PDL_ENTRY();
+    const int nb = (a.P + PT_THREADS - 1) / PT_THREADS;
+    const int t = blockIdx.x / nb, p = (blockIdx.x % nb) * PT_THREADS + threadIdx.x, r = blockIdx.y;
+    if (p >= a.P) return;
+    const int Ds = a.Ds, U = a.U, H = a.H;
+    const size_t row = (size_t)r * a.P + p;
+    double* zb = a.zbar + (row * H + t) * U;
+    if (t == H - 1 && !a.direct) {                      // x_H carries no reward
+        for (int j = 0; j < U; ++j) zb[j] = 0.0;
+        return;
+    }
+    const double* gx = a.gxt + ((size_t)t * a.T + row) * (Ds + U) + Ds;
+    if (!a.squash) {
+        for (int j = 0; j < U; ++j) zb[j] = gx[j];
+        return;
+    }
+    const double* xg = a.traj + (row * (H + 1) + t) * Ds;
+    double x[MAXD];
+#pragma unroll
+    for (int d = 0; d < MAXD; ++d) x[d] = d < Ds ? xg[d] : 0.0;
+    const double* W = a.W + r * a.W_bs + t * a.W_ts;
+    const double* b = a.b + r * a.b_bs + t * a.b_ts;
+    for (int j = 0; j < U; ++j) {
+        double z = b[j];
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) if (d < Ds) z = fma(W[j * Ds + d], x[d], z);
+        zb[j] = gx[j] * (a.maxa[j] * cospi(z * PT_INV_PI));
+    }
+}
+
+// The per-step policy-parameter gradient, in place of pg_param_kernel under a schedule: grid (H U + 1, R), 256
+// threads.  CTA t U + j of restart r = blockIdx.y forms sum_p z_bar_{p,t,j} [x_{p,t}, 1] over the restart's P
+// particles, thread q taking p = q, q + 256, ... in order (so a restart's sums do not depend on R), and writes
+// gW [R,H,U,Ds] and gb [R,H,U] over P.  The last CTA is pg_param_kernel's value CTA, the same code.
+__global__ void __launch_bounds__(256) pg_sched_kernel(PgRed a) {
+    PDL_ENTRY();
+    __shared__ double red[(MAXD + 1) * 8], out[MAXD + 1];
+    const int Ds = a.Ds, U = a.U, H = a.H, tid = threadIdx.x, r = blockIdx.y;
+    const size_t r0 = (size_t)r * a.P;                  // the restart's first row
+    const double invP = 1.0 / a.P;
+    if ((int)blockIdx.x == H * U) {                     // value = mean return
+        double v[1] = {0.0};
+        for (int p = tid; p < a.P; p += 256) v[0] += a.ret[r0 + p];
+        pg_block_sum<1>(v, red, out);
+        if (tid == 0) a.value[r] = out[0] * invP;
+        return;
+    }
+    const int t = blockIdx.x / U, j = blockIdx.x % U;
+    const double* traj = a.traj + (r0 * (H + 1) + t) * Ds;          // particle p's x_t at traj[p (H+1) Ds]
+    const double* zbar = a.zbar + (r0 * H + t) * U + j;             // its z_bar_{t,j} at zbar[p H U]
+    double v[MAXD + 1];
+#pragma unroll
+    for (int d = 0; d <= MAXD; ++d) v[d] = 0.0;
+    for (int p = tid; p < a.P; p += 256) {
+        const double* x = traj + (size_t)p * (H + 1) * Ds;
+        const double zb = zbar[(size_t)p * H * U];
+#pragma unroll
+        for (int d = 0; d < MAXD; ++d) if (d < Ds) v[d] = fma(zb, x[d], v[d]);
+        v[MAXD] += zb;
+    }
+    pg_block_sum<MAXD + 1>(v, red, out);
+    const size_t o = ((size_t)r * H + t) * U + j;
+    if (tid < Ds) a.gW[o * Ds + tid] = out[tid] * invP;
+    if (tid == 0) a.gb[o] = out[MAXD] * invP;
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 // Every entry point is one call of pt_call (or of the query pt_query): pt_validate checks the call once, in one order
 // of precedence, and fills a PtOpt; the sampler's layout (pt_ws_layout or fs_ws_layout) places the workspace; the
@@ -771,6 +851,8 @@ struct PtOpt {
     double b;
     double* step_var;
     pilco_particles_resample rs;
+    bool sched;                 // an active schedule (DESIGN.md section 28): step t's linear policy at t sch strides
+    pilco_policy_schedule sch;
 };
 
 // Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
@@ -1034,10 +1116,11 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 // kept when either needs it.  tm (angles, DESIGN.md section 20): pa_step_kernel in place of pt_step_kernel, which with
 // history also keeps phi(x_t) in L.phi.  nz (noise, DESIGN.md section 23; tm then given, the identity without angles):
 // pn_step_kernel in place of pa_step_kernel, which with history also keeps phi(z_t) in L.phiz.  The state width is
-// dyn.E throughout (pol.Ds without angles).
+// dyn.E throughout (pol.Ds without angles).  sch (an active schedule, DESIGN.md section 28): every step kernel reads
+// the linear policy through a.W and a.b, which step t's launch advances by t W_ts and t b_ts.
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
-                      const pilco_particles_resample* rs = nullptr) {
+                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
@@ -1065,6 +1148,7 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
     }
     for (int t = 0; t <= H; ++t) {
         a.t = t;
+        if (sch) { a.W = pr->pol.W + (t < H ? t : 0) * sch->W_ts; a.b = pr->pol.b + (t < H ? t : 0) * sch->b_ts; }
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
         a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
         if (rs && t > 0) {
@@ -1112,9 +1196,9 @@ int rbf_factor_bwd_launch(cudaStream_t st, int R, int bf, int Ds, int U, const d
                           double* gX, double* gY, double* gell);
 
 // value and the policy-parameter gradient over all P H points of each restart, fixed order, from z_bar [R P,H,U] and
-// the policy inputs pin [R P,H+1,Ds] (pr->traj, or with angles the phi history)
+// the policy inputs pin [R P,H+1,Ds] (pr->traj, or with angles the phi history); sched: per step (pg_sched_kernel)
 static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_grad* g, double* ws, const PtWs& L,
-                     cudaStream_t st, const double* pin) {
+                     cudaStream_t st, const double* pin, bool sched = false) {
     PgRed r;
     static_cast<PtPolicy&>(r) = pt_policy(pr);
     const bool rbf = r.pol_kind == PILCO_POLICY_RBF;
@@ -1124,6 +1208,11 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
     r.s1 = ws + L.s1; r.s2 = ws + L.s2r; r.gbeta = ws + L.gbeta;
     r.gXc = g->gXc; r.gell = g->gell;
     r.value = g->value;
+    if (sched) {                                        // linear (pt_validate)
+        launch_hi(pg_sched_kernel, dim3(r.H * U + 1, R), dim3(256), 0, st, r);
+        CUDA_LAUNCH_CHECK();
+        return PILCO_OK;
+    }
     launch_hi(pg_param_kernel, dim3((rbf ? U * bf : U) + 1, R), dim3(256), 0, st, r);
     CUDA_LAUNCH_CHECK();
     if (rbf) {                                          // through beta = (K + sn2 I)^-1 Yc, as pilco_rollout_backward
@@ -1149,9 +1238,10 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // x~_bar_{H-1} = 0 passed to the step kernel, which ignores x_bar when x~_bar is NULL).
 // rs (resampled): after the step kernel of each t = H-1 .. 1, pr_reverse_launch turns x_bar_t (the cotangent of the
 // refitted particles) into that of x'_t and rewrites var_bar_{t-1}.
+// sch (an active schedule): the step kernels of step t read W_t and b_t as pt_forward's, and the reduction is per step.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false,
-                      const pilco_particles_resample* rs = nullptr) {
+                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1181,6 +1271,7 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     }
     for (int t = H - 1; t >= 0; --t) {
         b.t = t;
+        if (sch) { b.W = pr->pol.W + t * sch->W_ts; b.b = pr->pol.b + t * sch->b_ts; }
         b.gxt = joint || bonus ? ws + L.gxt : nullptr;
         if (t < H - 1) {
             const double* xt = ws + L.xt + (size_t)t * TD;
@@ -1229,7 +1320,7 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             if (const int rc = pr_reverse_launch(st, grid, q)) return rc;
         }
     }
-    return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj);
+    return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj, sch != nullptr);
 }
 
 // the moments kernel's arguments over the forward's traj and act (tm: the angles' map, or the identity)
@@ -1254,7 +1345,8 @@ static PxMom px_mom(const pilco_particles* pr, const TrigMap& tm, double b) {
 // accumulates over the steps, so the loop stays serial.
 // Angles: the state-width cotangents are in E; ps_zbar and the reduction read the policy inputs from the phi history
 // (Ds = Dh), and the joint terms' direct term starts at x~ column Dh.  Noise: the policy inputs are the phi(z)
-// history; the VJPs act on x~, which holds phi(x), unchanged.
+// history; the VJPs act on x~, which holds phi(x), unchanged.  An active schedule: ps_zbar_sched and the per-step
+// reduction in place of ps_zbar and pg_param (DESIGN.md section 28).
 static int ps_run(const pilco_particles* pr, const PtOpt& o, const pilco_particles_grad* g, const PtWs& L,
                   cudaStream_t st) {
     double* ws = (double*)g->ws;
@@ -1318,11 +1410,17 @@ static int ps_run(const pilco_particles* pr, const PtOpt& o, const pilco_particl
         launch_hi(pj_grad_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, j);
         CUDA_LAUNCH_CHECK();
     }
-    if (H > 0) {
+    if (H > 0 && o.sched) {                             // step t's W_t, b_t (DESIGN.md section 28)
+        PsSched s;
+        static_cast<PsDev&>(s) = a;
+        s.W_ts = o.sch.W_ts; s.b_ts = o.sch.b_ts;
+        launch_hi(ps_zbar_sched_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, s);
+        CUDA_LAUNCH_CHECK();
+    } else if (H > 0) {
         launch_hi(ps_zbar_kernel, dim3(nb * H, R), dim3(PT_THREADS), 0, st, a);
         CUDA_LAUNCH_CHECK();
     }
-    return pg_reduce(pr, R, g, ws, L, st, pin);
+    return pg_reduce(pr, R, g, ws, L, st, pin, o.sched);
 }
 
 // ---- angular state dimensions (DESIGN.md section 20) ----------------------------------------------------------------
@@ -1369,6 +1467,10 @@ static int px_check(const pilco_particles* pr, const pilco_exploration* ex) {
     return PILCO_OK;
 }
 
+// ---- time-varying linear policy (DESIGN.md section 28) ----------------------------------------------------------------
+// active: sch not NULL and a non-zero stride; an inactive schedule is the call without it
+static bool pt_sched_active(const pilco_policy_schedule* sch) { return sch && (sch->W_ts != 0 || sch->b_ts != 0); }
+
 // ---- one validator, one query, one call path --------------------------------------------------------------------------
 // Everything a call checks before its workspace, in this order: NULL pr, the angles' map (A != 0), the description
 // (the policy's batch strides as o->batched allows), R, the gradient's outputs, the noise, the exploration (active
@@ -1376,9 +1478,11 @@ static int px_check(const pilco_particles* pr, const pilco_exploration* ex) {
 // is the call without angles, nz == NULL the call without noise and an inactive ex the call without exploration.
 // Resampled calls (o->resampled, no angles, noise or exploration), after the gradient's outputs: PILCO_ERR_NULL for rs
 // NULL or xi NULL with H > 0, then PILCO_ERR_DIM for P < 2 (no sample covariance).
+// Scheduled calls (DESIGN.md section 28), after everything else: PILCO_ERR_DIM for a negative stride, then
+// PILCO_ERR_UNSUPPORTED for an active schedule with an RBF policy.  sch NULL or both strides 0 is the call without it.
 static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                        const pilco_exploration* ex, int R, const pilco_particles_grad* g,
-                       const pilco_particles_resample* rs = nullptr) {
+                       const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
     if (!pr) return PILCO_ERR_NULL;
     const bool angles = !pa_none(ang);
     if (angles)
@@ -1401,15 +1505,23 @@ static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* 
         o->b = ex->b; o->step_var = ex->step_var; o->bonus = ex->b != 0.0;
     }
     o->R = R; o->mapped = angles || nz; o->noisy = nz != nullptr;
+    if (sch && (sch->W_ts < 0 || sch->b_ts < 0)) return PILCO_ERR_DIM;
+    o->sched = pt_sched_active(sch);
+    if (o->sched) {
+        if (pt_rbf(pr)) return PILCO_ERR_UNSUPPORTED;
+        o->sch = *sch;
+    }
     return PILCO_OK;
 }
 
 // A call's workspace: its layout's total, 0 where the call would fail on its sizes.  The sizes accepted are the
 // description's own (pt_sizes_ok, not its width consistency), R, the angles' map, 1 <= E <= PILCO_MAX_E and valid
-// variances with noise, and the exploration's checks when active.
+// variances with noise, and the exploration's checks when active; a schedule only adds non-negative strides (its
+// workspace is the call's without it).
 static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                       const pilco_exploration* ex, int R) {
+                       const pilco_exploration* ex, int R, const pilco_policy_schedule* sch = nullptr) {
     if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    if (sch && (sch->W_ts < 0 || sch->b_ts < 0)) return 0;
     if (!pa_none(ang) && pa_map(pr, ang, &o.tm)) return 0;
     if (nz && (pr->dyn.E < 1 || pr->dyn.E > MAXE || pn_noise(pr, nz, &o.nz))) return 0;
     o.explore = px_active(ex);
@@ -1424,8 +1536,8 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
 // moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
 static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                    const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream,
-                   const pilco_particles_resample* rs = nullptr) {
-    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs)) return rc;
+                   const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
+    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs, sch)) return rc;
     const bool fwd = o.call == PT_FORWARD;
     const PtWs L = o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
     if (const int rc = fwd ? pt_check_ws(pr->ws, pr->ws_bytes, L.total) : pt_check_ws(g->ws, g->ws_bytes, L.total))
@@ -1440,7 +1552,8 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
     const TrigMap* tm = o.mapped ? &o.tm : nullptr;
     const PnNoise* n = o.noisy ? &o.nz : nullptr;
     const pilco_particles_resample* rsv = o.resampled ? &o.rs : nullptr;
-    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv)) return rc;
+    const pilco_policy_schedule* sv = o.sched ? &o.sch : nullptr;
+    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv)) return rc;
     if (fwd) return PILCO_OK;
     if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
     if (o.explore) {
@@ -1448,7 +1561,7 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
         m.step_var = o.step_var; m.sd = ws + L.sd; m.tab = o.bonus ? ws + L.tab : nullptr;
         if (const int rc = px_moments_launch(st, R, m)) return rc;
     }
-    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv)) return rc;
+    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv, sv)) return rc;
     if (o.bonus && pr->H > 0) return px_value_launch(st, R, pr->H, o.b, ws + L.sd, g->value);
     return PILCO_OK;
 }
@@ -1664,6 +1777,109 @@ size_t pilco_particles_resampled_grad_workspace_bytes(const pilco_particles* pr,
 int pilco_particles_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs, int R,
                                            const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(RPATH, pr, nullptr, nullptr, nullptr, R, g, stream, rs);
+}
+
+// time-varying linear policy (DESIGN.md section 28): each family's most general call with sch
+size_t pilco_particles_scheduled_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                 const pilco_particles_noise* nz, const pilco_policy_schedule* sch) {
+    return pt_query(FWD, pr, ang, nz, nullptr, 1, sch);
+}
+
+int pilco_particles_scheduled_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                      const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                      pilco_stream_t stream) {
+    return pt_call(FWD, pr, ang, nz, nullptr, 1, nullptr, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_consistent_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_policy_schedule* sch) {
+    return pt_query(CFWD, pr, ang, nz, nullptr, 1, sch);
+}
+
+int pilco_particles_scheduled_consistent_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                 const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                                 pilco_stream_t stream) {
+    return pt_call(CFWD, pr, ang, nz, nullptr, 1, nullptr, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_exploration* ex,
+                                                            const pilco_policy_schedule* sch, int R) {
+    return pt_query(PATH, pr, ang, nz, ex, R, sch);
+}
+
+int pilco_particles_scheduled_batch_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                 const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                 const pilco_policy_schedule* sch, int R,
+                                                 const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(PATH, pr, ang, nz, ex, R, g, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                                 const pilco_particles_noise* nz,
+                                                                 const pilco_exploration* ex,
+                                                                 const pilco_policy_schedule* sch, int R) {
+    return pt_query(CPATH, pr, ang, nz, ex, R, sch);
+}
+
+int pilco_particles_scheduled_consistent_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                      const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                      const pilco_policy_schedule* sch, int R,
+                                                      const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(CPATH, pr, ang, nz, ex, R, g, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_score_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_policy_schedule* sch, int R) {
+    return pt_query(SCORE, pr, ang, nz, nullptr, R, sch);
+}
+
+int pilco_particles_scheduled_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                 const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                                 int R, const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(SCORE, pr, ang, nz, nullptr, R, g, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_consistent_score_grad_workspace_bytes(const pilco_particles* pr,
+                                                                       const pilco_angles* ang,
+                                                                       const pilco_particles_noise* nz,
+                                                                       const pilco_policy_schedule* sch, int R) {
+    return pt_query(CSCORE, pr, ang, nz, nullptr, R, sch);
+}
+
+int pilco_particles_scheduled_consistent_score_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                            const pilco_particles_noise* nz,
+                                                            const pilco_policy_schedule* sch, int R,
+                                                            const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(CSCORE, pr, ang, nz, nullptr, R, g, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_resampled_workspace_bytes(const pilco_particles* pr,
+                                                           const pilco_particles_resample* rs,
+                                                           const pilco_policy_schedule* sch) {
+    (void)rs;
+    return pt_query(RFWD, pr, nullptr, nullptr, nullptr, 1, sch);
+}
+
+int pilco_particles_scheduled_resampled_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                const pilco_policy_schedule* sch, pilco_stream_t stream) {
+    return pt_call(RFWD, pr, nullptr, nullptr, nullptr, 1, nullptr, stream, rs, sch);
+}
+
+size_t pilco_particles_scheduled_resampled_grad_workspace_bytes(const pilco_particles* pr,
+                                                                const pilco_particles_resample* rs,
+                                                                const pilco_policy_schedule* sch, int R) {
+    (void)rs;
+    return pt_query(RPATH, pr, nullptr, nullptr, nullptr, R, sch);
+}
+
+int pilco_particles_scheduled_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
+                                                     const pilco_policy_schedule* sch, int R,
+                                                     const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(RPATH, pr, nullptr, nullptr, nullptr, R, g, stream, rs, sch);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,

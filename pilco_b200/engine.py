@@ -500,10 +500,12 @@ def _schedule_check(policy_spec, H, schedule):
     return len(Ws) == 4, Hw
 
 
-def _no_schedule(policy_spec, what):
-    if isinstance(policy_spec, dict) and policy_spec.get("schedule", False):
-        raise ValueError("%s: the particle rollouts do not support a time-varying linear policy (schedule); use the "
-                         "moment-matching RolloutPlan(..., schedule=True)" % what)
+def _particle_schedule(policy_spec, H, schedule, what):
+    """``_schedule_check`` for the particle plans, before any allocation: a scheduled spec without ``schedule=True`` is
+    a ValueError that names ``what``"""
+    if not schedule and isinstance(policy_spec, dict) and policy_spec.get("schedule", False):
+        raise ValueError("%s: the policy spec is a time-varying linear policy (a schedule): pass schedule=True" % what)
+    return _schedule_check(policy_spec, H, schedule)
 
 
 def _fill_rewards(desc, reward_terms):
@@ -745,6 +747,19 @@ PARTICLE_CALLS = {
     ("resampled", "pathwise"): ("resampled_grad_rollout", "resampled_grad_workspace_bytes"),
 }
 
+# the same rows with a time-varying linear policy (DESIGN.md section 28): each call above with a pilco_policy_schedule
+# after its feature arguments
+PARTICLE_SCHEDULED_CALLS = {
+    (False, "forward"): ("scheduled_rollout", "scheduled_workspace_bytes"),
+    (True, "forward"): ("scheduled_consistent_rollout", "scheduled_consistent_workspace_bytes"),
+    (False, "pathwise"): ("scheduled_batch_grad_rollout", "scheduled_batch_grad_workspace_bytes"),
+    (True, "pathwise"): ("scheduled_consistent_grad_rollout", "scheduled_consistent_grad_workspace_bytes"),
+    (False, "score"): ("scheduled_score_grad_rollout", "scheduled_score_grad_workspace_bytes"),
+    (True, "score"): ("scheduled_consistent_score_grad_rollout", "scheduled_consistent_score_grad_workspace_bytes"),
+    ("resampled", "forward"): ("scheduled_resampled_rollout", "scheduled_resampled_workspace_bytes"),
+    ("resampled", "pathwise"): ("scheduled_resampled_grad_rollout", "scheduled_resampled_grad_workspace_bytes"),
+}
+
 
 class ParticlePlan:
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
@@ -791,13 +806,20 @@ class ParticlePlan:
     R policies, which ``set_inputs`` fills: its ``xi`` is then required), ``step_mean`` [R?,H+1,Ds] and ``step_cov``
     [R?,H+1,Ds,Ds] (the fitted moments; t = 0: those of x0), which every launch fills.  ``launch_grad()`` gives the
     pathwise gradient through the refit.  It needs P >= 2; with ``consistent``, ``estimator="score"``, ``angles``,
-    ``measurement_noise`` or ``exploration`` it is a ValueError raised before any allocation."""
+    ``measurement_noise`` or ``exploration`` it is a ValueError raised before any allocation.
+
+    ``schedule=True``: a time-varying linear policy u_t = sq(W_t x + b_t) (pilco_particles_scheduled_*, DESIGN.md
+    section 28), with every sampler, estimator and feature above.  The spec's W is [Hw, U, Ds] or [R, Hw, U, Ds] and b
+    [Hw, U] or [R, Hw, U], Hw >= H (step t < H reads W[..., t, :, :]); ``launch_grad()`` then returns the per-step
+    gradients 'W' [R?, H, U, Ds] and 'b' [R?, H, U].  An RBF spec or Hw < H is a ValueError raised before any
+    allocation, and so is a scheduled spec without ``schedule=True``."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
-                 estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False):
-        _no_schedule(policy_spec, "ParticlePlan")
+                 estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False,
+                 schedule=False):
+        sched = _particle_schedule(policy_spec, H, schedule, "ParticlePlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         self.resample = bool(resample)
@@ -814,7 +836,8 @@ class ParticlePlan:
             raise ValueError("particles: the gradient of the consistent (function-sample) rollout is "
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
         self.consistent = bool(consistent)
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration,
+                       sched)
         pr, d = self.pr, device()
         P, H = self.P, self.H
         if not self.batched:                                    # the forward-only rollout (a batch has none)
@@ -831,17 +854,22 @@ class ParticlePlan:
         return "resampled" if self.resample else self.consistent
 
     def _args(self, kind, pr):
-        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise) and R; resampled:
-        pr, the refit's buffers and R"""
+        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise), the schedule
+        (scheduled calls) and R; resampled: pr, the refit's buffers, the schedule and R"""
+        sch = [C.byref(self.sch)] if self.sch is not None else []
         if self.resample:
-            return [C.byref(pr), C.byref(self.rs)] + ([self.R] if kind != "forward" else [])
+            return [C.byref(pr), C.byref(self.rs)] + sch + ([self.R] if kind != "forward" else [])
         args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
         if kind == "pathwise":
             args.append(C.byref(self.ex) if self.ex is not None else None)
-        return args + ([self.R] if kind != "forward" else [])
+        return args + sch + ([self.R] if kind != "forward" else [])
+
+    def _names(self, kind):
+        """(rollout, size query) of kind's call, each after the prefix pilco_particles_"""
+        return (PARTICLE_CALLS if self.sch is None else PARTICLE_SCHEDULED_CALLS)[self._sampler(), kind]
 
     def _query(self, kind, pr):
-        return int(getattr(lib, "pilco_particles_" + PARTICLE_CALLS[self._sampler(), kind][1])(*self._args(kind, pr)))
+        return int(getattr(lib, "pilco_particles_" + self._names(kind)[1])(*self._args(kind, pr)))
 
     def _grad_ws_bytes(self, P):
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
@@ -850,11 +878,11 @@ class ParticlePlan:
         return self._query(self.estimator, pr)
 
     def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None,
-                  exploration=None):
+                  exploration=None, sched=None):
         """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
         The angles, the policy's width, the measurement noise and the exploration weight are checked first, before any
-        device work."""
-        self.ang, self.nz, self.ex = None, None, None
+        device work.  ``sched``: ``_schedule_check``'s (batched, Hw) of a scheduled spec, or None."""
+        self.ang, self.nz, self.ex, self.sch = None, None, None, None
         b = _particle_exploration(exploration, reward_terms, P)
         if angles is not None and len(angles) > 0:
             E = int(dyn.struct().E)
@@ -882,7 +910,14 @@ class ParticlePlan:
         pr.P, pr.H = P, H
         pr.dyn = dyn.struct()
         self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, policy_spec, self.batched)
-        if pr.pol.kind == _lib.POLICY_LINEAR:
+        if sched is not None:                                   # step t reads W[..., t, :, :], b[..., t, :]
+            Hw = sched[1]
+            if self.W.numel() != R * Hw * U * Ds or self.b.numel() != R * Hw * U:
+                raise ValueError("particles: schedule=True expects W [R,Hw,U,Ds] and b [R,Hw,U] with R=%d (unbatched: "
+                                 "[Hw,U,Ds], [Hw,U])" % R)
+            pr.pol.W_bs, pr.pol.b_bs = (Hw * U * Ds, Hw * U) if self.batched else (0, 0)
+            self.sch = _lib.PolicySchedule(U * Ds, U)
+        elif pr.pol.kind == _lib.POLICY_LINEAR:
             if self.W.numel() != R * U * Ds or self.b.numel() != R * U:
                 raise ValueError("particles: expected W [R,U,Ds] and b [R,U] with R=%d (unbatched: [U,Ds], [U])" % R)
         elif self.rbf.batched != self.batched or (self.batched and self.rbf.X.shape[0] != R):
@@ -928,7 +963,11 @@ class ParticlePlan:
         if gwsb == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, pr.dyn.D, self.R))
         g = _lib.ParticlesGrad()
-        self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead)
+        if self.sch is None:
+            self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead)
+        else:                                                   # per step; H = 0 still has an address
+            self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead + (max(self.H, 1),))
+            self.gbuf["W"], self.gbuf["b"] = self.gbuf["W"][..., :self.H, :, :], self.gbuf["b"][..., :self.H, :]
         self.gbuf["value"] = torch.zeros(self.R if self.batched else 1, dtype=F64, device=d)
         g.value = self.gbuf["value"].data_ptr()
         self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
@@ -941,14 +980,15 @@ class ParticlePlan:
         {'value' [1], 'W' [U,Ds], 'b' [U]} (linear) or {'value', 'X' [bf,Ds], 'Y' [bf,U], 'ell' [U,Ds]} (RBF, constrained
         lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R]).
         ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout.
-        With ``exploration``: value and gradient of the exploration objective, and sigma_t^2 in ``step_var``."""
+        With ``exploration``: value and gradient of the exploration objective, and sigma_t^2 in ``step_var``.  With
+        ``schedule``: 'W' [R?,H,U,Ds] and 'b' [R?,H,U], one gradient per step."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
         self._call(self.estimator, C.byref(self.grad))
         return self.gbuf
 
     def _call(self, kind, *grad):
-        name = "particles_" + PARTICLE_CALLS[self._sampler(), kind][0]
+        name = "particles_" + self._names(kind)[0]
         check(getattr(lib, "pilco_" + name)(*self._args(kind, self.pr), *grad, stream_ptr()), name)
 
     def set_inputs(self, x0, eps, nu=None, xi=None):
@@ -996,11 +1036,13 @@ class ConsistentGradPlan(ParticlePlan):
     samples (pilco_particles_consistent_score_grad_rollout, DESIGN.md section 25), which differentiates the log-density
     of each particle's whole path under its draw instead of the path itself, so box terms enter its gradient.  The same
     rollout, value and output layout; its estimate is unbiased on rollouts without degenerate pivots.  ``"score"`` with
-    ``exploration``, or an unknown estimator, is a ValueError raised before any allocation."""
+    ``exploration``, or an unknown estimator, is a ValueError raised before any allocation.
+
+    ``schedule=True``: a time-varying linear policy, as ``ParticlePlan``."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
-                 measurement_noise=None, exploration=None, estimator="pathwise"):
-        _no_schedule(policy_spec, "ConsistentGradPlan")
+                 measurement_noise=None, exploration=None, estimator="pathwise", schedule=False):
+        sched = _particle_schedule(policy_spec, H, schedule, "ConsistentGradPlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         if exploration is not None and estimator == "score":
@@ -1008,7 +1050,8 @@ class ConsistentGradPlan(ParticlePlan):
                              "estimator='pathwise' (the score-function estimate of sigma_t's gradient is not available)")
         self.estimator = estimator
         self.consistent, self.resample = True, False
-        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration)
+        self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration,
+                       sched)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
@@ -1140,7 +1183,7 @@ def particle_reward_moments(reward_terms, traj, act, angles=None):
 
 
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,
-                      angles=None, measurement_noise=None, nu=None, resample=False, xi=None):
+                      angles=None, measurement_noise=None, nu=None, resample=False, xi=None, schedule=False):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
     step_risk [P,H], ret [P]) device tensors.
@@ -1157,8 +1200,10 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
 
     ``resample=True``: the Gaussian refit at every step, as ``ParticlePlan(resample=True)``; ``xi`` [P,H,Ds] are the
     redraw's standard normals (required with it, and only then).  The result then also has the fitted moments:
-    (traj, act, step_reward, step_risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds])."""
-    _no_schedule(policy_spec, "particles_rollout")
+    (traj, act, step_reward, step_risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds]).
+
+    ``schedule=True``: a time-varying linear policy (W [Hw,U,Ds], b [Hw,U], Hw >= H), as ``ParticlePlan``."""
+    _particle_schedule(policy_spec, eps.shape[1] if len(np.shape(eps)) == 3 else 0, schedule, "particles_rollout")
     if resample:
         _resample_check(x0.shape[0], consistent, "pathwise", angles, measurement_noise, None)
     if (xi is None) == bool(resample):
@@ -1175,13 +1220,13 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
             raise ValueError("particles_rollout: nu must be [P,H,E] like eps, got %s" % (tuple(nu.shape),))
     if consistent:
         return _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles,
-                                             measurement_noise, nu)
+                                             measurement_noise, nu, schedule)
     if resample:
         xi = dev(xi)
         if tuple(xi.shape) != tuple(eps.shape):
             raise ValueError("particles_rollout: xi must be [P,H,Ds] like eps, got %s" % (tuple(xi.shape),))
     plan = ParticlePlan(dyn, policy_spec, reward_terms, x0.shape[0], eps.shape[1], mult_mu=mult_mu, angles=angles,
-                        measurement_noise=measurement_noise, resample=resample)
+                        measurement_noise=measurement_noise, resample=resample, schedule=schedule)
     plan.set_inputs(x0, eps, nu, xi)
     plan.launch()
     return plan.outputs() + ((plan.step_mean, plan.step_cov) if resample else ())
@@ -1200,7 +1245,7 @@ def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):
 
 
 def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None,
-                                  measurement_noise=None, nu=None):
+                                  measurement_noise=None, nu=None, schedule=False):
     P, H = int(x0.shape[0]), int(eps.shape[1])
     Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
     if angles is not None and len(angles) > 0:                 # the policy's width, before any allocation
@@ -1219,7 +1264,7 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     lo = _largest_fitting(fits, 1, P)
     if lo == P:
         plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles,
-                            measurement_noise=measurement_noise)
+                            measurement_noise=measurement_noise, schedule=schedule)
         plan.set_inputs(x0, eps, nu)
         plan.launch()
         return plan.outputs()
@@ -1234,7 +1279,7 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         if plan is None or plan.P != p1 - p0:
             plan = None                                     # free the previous chunk's workspace first
             plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True,
-                                angles=angles, measurement_noise=measurement_noise)
+                                angles=angles, measurement_noise=measurement_noise, schedule=schedule)
         plan.set_inputs(x0[p0:p1], eps[p0:p1], None if nu is None else nu[p0:p1])
         plan.launch()
         for o, c in zip(out, plan.outputs()):

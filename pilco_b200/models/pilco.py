@@ -635,14 +635,23 @@ class PILCO:
         return best_reward
 
     # ---- receding-horizon planning (probabilistic MPC, Kamthe & Deisenroth 2018) --------------------------------------
-    def plan(self, m_x, s_x=None, maxiter=20, restarts=1, warm_start=True):
+    def plan(self, m_x, s_x=None, maxiter=20, restarts=1, warm_start=True, num_samples=None, seed=None,
+             consistent=False):
         """One receding-horizon step with a TimeVaryingLinearController: optimise its schedule over ``horizon`` steps
         of the moment-matching cascade from N(m_x, s_x) (s_x = None or 0: a measured state), return the first action
         u_0 = compute_action(m_x, t=0) [1,U], then shift the schedule one step (theta_t <- theta_{t+1}, the last step
         repeated) so that the next call starts from the rest of this plan.  Restart 0 starts from the current schedule
         (``warm_start=False``: from ``controller.randomize()``), the others from random draws, as ``optimize_policy``
         chooses, batches and shards them; the objective is ``optimize_policy``'s (with ``exploration``).  m_init and
-        S_init are not touched.  A stationary controller is a TypeError."""
+        S_init are not touched.  A stationary controller is a TypeError.
+
+        ``num_samples=S``: optimise the schedule on the in-sample mean return of S particle rollouts of the learnt
+        dynamics instead (PETS-style trajectory sampling; DESIGN.md section 28), as ``optimize_policy_sampled`` does
+        for a stationary policy: x0 ~ N(m_x, s_x) (every particle at m_x when s_x is None) and the step normals are
+        drawn once from one generator seeded with ``seed`` and held fixed, so the objective is deterministic.
+        ``consistent=True``: each particle follows one function drawn from the dynamics posterior.  Restarts, warm
+        start and the shift are as above; ``exploration`` is not read.  Box terms, ``angle_dims`` and
+        ``measurement_noise`` are a ValueError raised before any device work."""
         from functools import partial
         from .. import policy_opt
         c = self.controller
@@ -652,14 +661,27 @@ class PILCO:
         Ds = self.state_dim
         m = np.asarray(m_x, dtype=np.float64).reshape(1, Ds)
         s = np.zeros((Ds, Ds)) if s_x is None else np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds)
+        if num_samples is not None:
+            self._no_angles("plan(num_samples=...)")
+            self._no_noise("plan(num_samples=...)")
+            if int(num_samples) < 1:
+                raise ValueError("plan: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
+            terms, _ = self.reward_spec()
+            if any(t["kind"] == _lib.REWARD_BOX for t in terms):
+                raise ValueError("plan(num_samples=...): the reward has box (risk) terms, which carry no pathwise "
+                                 "gradient; plan with the moment-matching objective (num_samples=None)")
         if not warm_start:
             c.randomize()
         mgpr_trainable = self.mgpr.trainable_parameters
         for p in mgpr_trainable:
             set_trainable(p, False)
         try:
-            best_flat, _, _ = policy_opt.optimize(self, maxiter=maxiter, restarts=restarts,
-                                                  evaluator=partial(policy_opt.PolicyEvaluator, m0=m, S0=s))
+            if num_samples is None:
+                evaluator = partial(policy_opt.PolicyEvaluator, m0=m, S0=s)
+            else:
+                x0, eps = self._particle_inputs(m, s, self.horizon, num_samples, seed, "plan")
+                evaluator = partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent)
+            best_flat, _, _ = policy_opt.optimize(self, maxiter=maxiter, restarts=restarts, evaluator=evaluator)
             c.set_flat(best_flat)
         finally:
             for p in mgpr_trainable:

@@ -234,7 +234,8 @@ class ParticleEvaluator(_FlatEvaluator):
     b sum_t sigma_t with sigma_t the sample spread of step t's reward (pilco_particles_explore_*, DESIGN.md section 24);
     None (the default) is the mean return.  ``resample=True``: Deep PILCO's Gaussian refit at every step
     (pilco_particles_resampled_grad_rollout, DESIGN.md section 26) with the redraw's standard normals ``xi`` [P,H,Ds],
-    held fixed like eps."""
+    held fixed like eps.  A ``TimeVaryingLinearController`` runs the scheduled calls (pilco_particles_scheduled_*,
+    DESIGN.md section 28), its gradient per step."""
 
     def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None):
         terms, mult_mu = pilco.reward_spec()
@@ -248,11 +249,12 @@ class ParticleEvaluator(_FlatEvaluator):
         x0 = engine.dev(x0)
         if consistent:
             self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
-                                                  int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration)
+                                                  int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration,
+                                                  schedule=self.sched)
         else:
             self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
                                             mult_mu=mult_mu, grad=True, R=R, exploration=exploration,
-                                            resample=resample)
+                                            resample=resample, schedule=self.sched)
         self.plan.set_inputs(x0, eps, xi=xi)
         self._setup_io()
 
