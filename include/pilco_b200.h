@@ -264,6 +264,7 @@ int pilco_box_risk(int Ds, int R, const double* prm, const double* m /*[R,Ds]*/,
  */
 #define PILCO_POLICY_LINEAR 0
 #define PILCO_POLICY_RBF    1
+#define PILCO_POLICY_MLP    2   /* tanh MLP, particle rollouts only: pilco_particles_mlp_* with a pilco_mlp */
 #define PILCO_REWARD_EXP    0
 #define PILCO_REWARD_LINEAR 1
 #define PILCO_REWARD_BOX    2   /* pilco_box_risk; W = its prm block, t unused */
@@ -805,6 +806,54 @@ size_t pilco_particles_scheduled_resampled_grad_workspace_bytes(const pilco_part
 int    pilco_particles_scheduled_resampled_grad_rollout(const pilco_particles* pr, const pilco_particles_resample* rs,
                                                         const pilco_policy_schedule* sch, int R,
                                                         const pilco_particles_grad* g, pilco_stream_t stream);
+
+/* Tanh MLP policies in the particle rollouts (DESIGN.md section 29), the policy class Deep PILCO trains on sampled
+ * returns.  pr->pol.kind = PILCO_POLICY_MLP, pol.Ds / U / squash / max_action as for a linear policy, the network in
+ * *mlp with L = 1 or 2 hidden layers of width[l] in 1 .. 64 units:
+ *   h_1 = tanh(A_1 [x; 1]),  h_2 = tanh(A_2 [h_1; 1])  (L = 2),  z = A_out [h_L; 1],  u = max_action o sin(z) (squash,
+ *   at output variance 0 as the linear policy) or z
+ * Each A is row-major [out, in + 1], its last column the bias; theta is A_1, (A_2,) A_out in that order:
+ *   n_theta = width[0] (Ds + 1) + (L = 2: width[1] (width[0] + 1)) + U (width[L-1] + 1)
+ * restart r's at theta + r theta_bs (the gradient calls; 0: shared).  Every other field of pr and every output has the
+ * meaning it has for a linear policy.  The gradient calls write value [R] and gtheta [R, n_theta] = d value / d theta
+ * (g's linear and RBF fields are ignored); ex may be NULL, as in pilco_particles_explore_*.  Each call is its
+ * sampler's linear-policy call (pilco_particles_rollout, _rollout_consistent, _resampled_rollout,
+ * _rollout_batch_grad / _explore_batch_grad, _explore_consistent_grad, _resampled_grad_rollout) with the MLP in place
+ * of the policy: no angles, measurement noise, schedule or score estimator.  Deterministic; a restart's results do
+ * not depend on R.  Validation before any work is enqueued: the linear call's status codes with its policy checks
+ * replaced by PILCO_ERR_UNSUPPORTED for pol.kind != PILCO_POLICY_MLP, PILCO_ERR_NULL for mlp or theta NULL,
+ * PILCO_ERR_DIM for L outside {1, 2}, a width outside 1 .. 64 or theta_bs < 0, PILCO_ERR_UNSUPPORTED for theta_bs != 0
+ * in a forward call; PILCO_ERR_NULL for gtheta NULL (gradient calls) with the gradient's outputs; then the sampler's
+ * own codes; then the workspace's.  A size query returns 0 exactly where its call fails on sizes (mlp NULL included).
+ * The linear and RBF calls return PILCO_ERR_UNSUPPORTED for PILCO_POLICY_MLP. */
+typedef struct pilco_mlp {
+    int L, width[2];
+    const double* theta; long long theta_bs;
+    double* gtheta;             /* [R, n_theta], gradient calls only */
+} pilco_mlp;
+size_t pilco_particles_mlp_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp);
+int    pilco_particles_mlp_rollout(const pilco_particles* pr, const pilco_mlp* mlp, pilco_stream_t stream);
+size_t pilco_particles_mlp_consistent_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp);
+int    pilco_particles_mlp_consistent_rollout(const pilco_particles* pr, const pilco_mlp* mlp, pilco_stream_t stream);
+size_t pilco_particles_mlp_resampled_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                     const pilco_particles_resample* rs);
+int    pilco_particles_mlp_resampled_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                             const pilco_particles_resample* rs, pilco_stream_t stream);
+size_t pilco_particles_mlp_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                      const pilco_exploration* ex, int R);
+int    pilco_particles_mlp_batch_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                              const pilco_exploration* ex, int R, const pilco_particles_grad* g,
+                                              pilco_stream_t stream);
+size_t pilco_particles_mlp_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                           const pilco_exploration* ex, int R);
+int    pilco_particles_mlp_consistent_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                   const pilco_exploration* ex, int R, const pilco_particles_grad* g,
+                                                   pilco_stream_t stream);
+size_t pilco_particles_mlp_resampled_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                          const pilco_particles_resample* rs, int R);
+int    pilco_particles_mlp_resampled_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                  const pilco_particles_resample* rs, int R,
+                                                  const pilco_particles_grad* g, pilco_stream_t stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,

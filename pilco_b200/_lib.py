@@ -100,7 +100,12 @@ class ParticlesResample(C.Structure):
     _fields_ = [("xi", c_dp), ("step_mean", c_dp), ("step_cov", c_dp)]
 
 
-POLICY_LINEAR, POLICY_RBF = 0, 1
+class Mlp(C.Structure):
+    """mirror of ``pilco_mlp``"""
+    _fields_ = [("L", C.c_int), ("width", C.c_int * 2), ("theta", c_dp), ("theta_bs", c_ll), ("gtheta", c_dp)]
+
+
+POLICY_LINEAR, POLICY_RBF, POLICY_MLP = 0, 1, 2
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
 JOINT_REWARDS = (REWARD_EXP_SA, REWARD_LINEAR_SA)
@@ -268,6 +273,28 @@ SIGNATURES = {
     "pilco_particles_scheduled_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(ParticlesResample),
                                                                    C.POINTER(PolicySchedule), C.c_int,
                                                                    C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_mlp_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp)]),
+    "pilco_particles_mlp_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), c_dp]),
+    "pilco_particles_mlp_consistent_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp)]),
+    "pilco_particles_mlp_consistent_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), c_dp]),
+    "pilco_particles_mlp_resampled_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                   C.POINTER(ParticlesResample)]),
+    "pilco_particles_mlp_resampled_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                        C.POINTER(ParticlesResample), c_dp]),
+    "pilco_particles_mlp_batch_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                    C.POINTER(Exploration), C.c_int]),
+    "pilco_particles_mlp_batch_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), C.POINTER(Exploration),
+                                                         C.c_int, C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_mlp_consistent_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                         C.POINTER(Exploration), C.c_int]),
+    "pilco_particles_mlp_consistent_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                              C.POINTER(Exploration), C.c_int,
+                                                              C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_mlp_resampled_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                        C.POINTER(ParticlesResample), C.c_int]),
+    "pilco_particles_mlp_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                             C.POINTER(ParticlesResample), C.c_int,
+                                                             C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

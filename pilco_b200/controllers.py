@@ -1,12 +1,13 @@
-"""Policies (drop-in for pilco/controllers.py): ``squash_sin``, ``LinearController``, ``RbfController``, and the
-step-indexed ``TimeVaryingLinearController`` of receding-horizon planning (``PILCO.plan``).
+"""Policies (drop-in for pilco/controllers.py): ``squash_sin``, ``LinearController``, ``RbfController``, the
+step-indexed ``TimeVaryingLinearController`` of receding-horizon planning (``PILCO.plan``), and the tanh
+``MlpController`` that the particle rollouts train (``PILCO.optimize_policy_sampled``).
 All moment computations run on the device through the C ABI (``pilco_squash_sin``,
 ``pilco_linear_action``, ``pilco_gp_factorize`` + ``pilco_mm_forward`` in deterministic-GP mode)."""
 import numpy as np
 
 from . import engine, _lib
 from .models.mgpr import MGPR, Kernel
-from .params import Parameter, Softplus, host, set_trainable
+from .params import HostArray, Parameter, Softplus, host, set_trainable
 
 
 def _max_action_vec(max_action, k):
@@ -174,6 +175,82 @@ class TimeVaryingLinearController:
         fW = np.zeros((H, U, Ds))
         fW[:n] = np.asarray(gW).reshape(n, U, Ds)
         return np.concatenate([fW.ravel(), fb.ravel()])
+
+
+class MlpController:
+    """A tanh multilayer perceptron, the policy Deep PILCO (Gal, McAllister & Rasmussen 2016) trains on sampled returns:
+    h_1 = tanh(A_1 [x; 1]), (two layers) h_2 = tanh(A_2 [h_1; 1]), z = A_out [h_L; 1], u = max_action sin(z)
+    (DESIGN.md section 29).  Each A is a Parameter [out, in + 1] with the bias as its last column; ``get_flat()`` is
+    the blocks in order, row-major, output layer last (the device's theta).  ``hidden``: one or two widths of 1 .. 64.
+
+    Moment matching has no closed form for it: the particle methods of ``PILCO`` (``sample_trajectories``,
+    ``sample_reward_moments``, ``sample_policy_gradient`` and ``optimize_policy_sampled``) run it, the moment-matching
+    ones refuse it.  ``compute_action`` evaluates it at a point."""
+
+    def __init__(self, state_dim, control_dim, hidden=(64, 64), max_action=1.0):
+        hidden = tuple(int(w) for w in hidden)
+        if len(hidden) not in (1, 2) or any(w < 1 or w > engine.MLP_MAX_WIDTH for w in hidden):
+            raise ValueError("MlpController: 1 or 2 hidden layers of 1 .. %d units, got hidden=%s"
+                             % (engine.MLP_MAX_WIDTH, hidden))
+        self.state_dim, self.control_dim, self.hidden = int(state_dim), int(control_dim), hidden
+        widths = [self.state_dim] + list(hidden) + [self.control_dim]
+        self.layers = [Parameter(np.zeros((widths[l + 1], widths[l] + 1)), name="A%d" % (l + 1))
+                       for l in range(len(widths) - 1)]
+        self.max_action = max_action
+        self.randomize()
+
+    @property
+    def parameters(self):
+        return list(self.layers)
+
+    @property
+    def trainable_parameters(self):
+        return [p for p in self.parameters if p.trainable]
+
+    def randomize(self):
+        """weights N(0, 1 / fan_in), biases 0, from np.random"""
+        for A in self.layers:
+            out, fan = A.shape[0], A.shape[1] - 1
+            W = np.random.normal(size=(out, fan)) / np.sqrt(fan)
+            A.assign(np.concatenate([W, np.zeros((out, 1))], axis=1))
+
+    def get_flat(self):
+        return np.concatenate([np.asarray(A.numpy()).ravel() for A in self.layers])
+
+    def set_flat(self, flat):
+        flat, o = np.asarray(flat, dtype=np.float64), 0
+        for A in self.layers:
+            n = int(np.prod(A.shape))
+            A.assign(flat[o:o + n].reshape(A.shape))
+            o += n
+
+    def policy_spec(self, flats=None):
+        """the device's spec: theta = ``flats`` ([n_theta] or [R, n_theta]) or the current parameters"""
+        theta = self.get_flat() if flats is None else np.asarray(flats, dtype=np.float64)
+        return dict(kind=_lib.POLICY_MLP, Ds=self.state_dim, U=self.control_dim, squash=True,
+                    max_action=_max_action_vec(self.max_action, self.control_dim), hidden=self.hidden, theta=theta)
+
+    def state_key(self):
+        return hash((self.get_flat().tobytes(), np.asarray(self.max_action, dtype=np.float64).tobytes()))
+
+    def compute_action(self, m, s=None, squash=True):
+        """the action at the point m [1, Ds] (s None or 0: an MLP has no moment closed form) -> (M [1,U], S [U,U] = 0,
+        V [Ds,U] = 0), the triple the other controllers return at s = 0.  A host fp64 evaluation of one point."""
+        m = np.asarray(m, dtype=np.float64).reshape(1, -1)
+        if s is not None and np.any(np.asarray(s, dtype=np.float64) != 0.0):
+            raise ValueError("MlpController.compute_action: evaluates at a point only (s = 0); propagate a state "
+                             "distribution with PILCO's particle methods (sample_trajectories)")
+        h = m[0]
+        for l, A in enumerate(self.layers):
+            A = np.asarray(A.numpy())
+            h = A[:, :-1] @ h + A[:, -1]
+            if l < len(self.layers) - 1:
+                h = np.tanh(h)
+        U = self.control_dim
+        if squash:
+            h = _max_action_vec(self.max_action, U) * np.sin(h)
+        return (h.reshape(1, U).view(HostArray), np.zeros((U, U)).view(HostArray),
+                np.zeros((m.shape[1], U)).view(HostArray))
 
 
 class FakeLikelihood:

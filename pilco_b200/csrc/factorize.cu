@@ -6,6 +6,7 @@
 // These run once per set_data / hyper-parameter change (dynamics GP) or once per loss evaluation
 // (RBF policy, bf<=128), never inside the H-step loop.
 #include "common.cuh"
+#include "gemm.cuh"
 
 #define FB 32                     // factorisation block size
 
@@ -306,9 +307,9 @@ __global__ void __launch_bounds__(256) gemm_dmma_kernel(GemmArgs g) {
             }
 }
 
-static int gemm(cudaStream_t st, int batch, int m, int n, int k, int ta, int tb, double alpha,
-                const double* A, int lda, long long sa, const double* B, int ldb, long long sb,
-                double beta, double* C, int ldc, long long sc) {
+int gemm(cudaStream_t st, int batch, int m, int n, int k, int ta, int tb, double alpha,
+         const double* A, int lda, long long sa, const double* B, int ldb, long long sb,
+         double beta, double* C, int ldc, long long sc) {
     if (m <= 0 || n <= 0) return PILCO_OK;
     GemmArgs g{m, n, k, ta, tb, alpha, beta, A, lda, sa, B, ldb, sb, C, ldc, sc};
     dim3 grid((n + 63) / 64, (m + 63) / 64, batch);

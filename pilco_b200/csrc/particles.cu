@@ -40,8 +40,12 @@
 // Time-varying linear policies (pilco_particles_scheduled_*, DESIGN.md section 28): pt_forward and pg_reverse hand step
 // t's launches W + t W_ts and b + t b_ts; ps_zbar_sched_kernel and pg_sched_kernel stand in for the two kernels that
 // cover all H steps in one grid (ps_zbar_kernel, pg_param_kernel).
+// Tanh MLP policies (pilco_particles_mlp_*, DESIGN.md section 29): pt_forward launches the step kernels of
+// particles_mlp.cu in place of pt_step / pr_step, pg_reverse its reverse step kernel in place of pg_step followed by one
+// batched gemm() per layer (factorize.cu) into per-chunk partials, and pm_finish_kernel in place of pg_reduce.
 #include <cmath>
 #include "particles.cuh"
+#include "gemm.cuh"
 
 // grid (ceil(P / 128), R), one thread per particle p of restart r = blockIdx.y
 __global__ void __launch_bounds__(PT_THREADS) pt_step_kernel(PtDev a) {
@@ -853,6 +857,8 @@ struct PtOpt {
     pilco_particles_resample rs;
     bool sched;                 // an active schedule (DESIGN.md section 28): step t's linear policy at t sch strides
     pilco_policy_schedule sch;
+    bool mlp;                   // an MLP call (DESIGN.md section 29): the policy is net, pol.kind must be PILCO_POLICY_MLP
+    PmNet net;
 };
 
 // Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
@@ -870,6 +876,8 @@ struct PtWs {
                                                         // the x~_bar history [H-1 or H,T,D]
     size_t xp, rmu, rL, rsc;                            // resampled: x' [H,T,Ds], mu^ [H,R,Ds], L^ [H,R,Ds,Ds]; the
                                                         // reverse scratch [R,Ds+Ds Ds]
+    size_t min0, min1, min2, md1, md2, mdo, mpart;      // MLP, gradients: the layer inputs and cotangents [., R Pp];
+                                                        // the chunk partials [R nc, n_theta]
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -899,6 +907,32 @@ static int ps_group(long long T, int H) {
     return H - 1 < k ? H - 1 : (int)k;
 }
 
+// The MLP reduction's chunks of a restart's P rows: Kc rows each (a multiple of 16, the gemm's k tile), nc <= PM_CHUNKS
+// of them, Pp = nc Kc rows with the padding
+struct PmChunks {
+    int Kc, nc;
+    long long Pp;
+};
+static PmChunks pm_chunks(int P) {
+    PmChunks c;
+    const int per = (P + PM_CHUNKS - 1) / PM_CHUNKS;
+    c.Kc = (per + 15) / 16 * 16;
+    c.nc = (P + c.Kc - 1) / c.Kc;
+    c.Pp = (long long)c.nc * c.Kc;
+    return c;
+}
+
+// the MLP gradient's slots, after every other slot: [x; 1], [h_1; 1], [h_2; 1], d_1, d_2, d_out, each [width, R Pp],
+// contiguous (one memset clears them), then the chunk partials [R nc, n_theta]
+static void pm_ws_slots(PtWs& L, PtTake& take, const pilco_particles* pr, const PtOpt& o) {
+    const PmNet& m = o.net;
+    const PmChunks c = pm_chunks(pr->P);
+    const size_t RPp = (size_t)o.R * c.Pp, Dh = pr->pol.Ds, U = pr->pol.U, w1 = m.w1, w2 = m.w2;
+    L.min0 = take({Dh + 1, RPp}); L.min1 = take({w1 + 1, RPp}); L.min2 = take({m.L == 2 ? w2 + 1 : 0, RPp});
+    L.md1 = take({w1, RPp}); L.md2 = take({w2, RPp}); L.mdo = take({U, RPp});
+    L.mpart = take({(size_t)o.R * c.nc, (size_t)m.n_theta});
+}
+
 // The step-wise sampler's workspace at T = R P rows (restart-major, row r P + p; nothing of size [., n] is kept).
 // State-width slots are in dyn.E, the RBF sums in the policy's width pol.Ds (the same without angles).
 //   forward-only: x~ [T,D], the step closure's mean and var [T,Ds], one predict workspace at T
@@ -926,7 +960,7 @@ static PtWs pt_ws_layout(const pilco_particles* pr, const PtOpt& o) {
         L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D});
     }
     if (grad) {
-        L.zbar = take({T, H, U});
+        L.zbar = take({T, H, o.mlp ? 0 : U});
         L.s1 = take({R, U, bf, Dh}); L.s2r = take({R, U, bf, Dh});
         L.gbeta = take({R, U, bf}); L.gy = take({R, U, bf});
     }
@@ -943,6 +977,7 @@ static PtWs pt_ws_layout(const pilco_particles* pr, const PtOpt& o) {
         L.xp = take({H, T, Ds}); L.rmu = take({H, R, Ds}); L.rL = take({H, R, Ds, Ds});
         if (grad) L.rsc = take({R, Ds + Ds * Ds});
     }
+    if (grad && o.mlp) pm_ws_slots(L, take, pr, o);
     const size_t nb = (pr->P + PT_THREADS - 1) / PT_THREADS;
     L.total = L.pws_bytes && (!score || nb * H <= 0x7fffffff) ? take.bytes() : 0;
     return L;
@@ -971,7 +1006,7 @@ static PtWs fs_ws_layout(const pilco_particles* pr, const PtOpt& o) {
         // the var' history supersedes the forward's var slot, whose bytes stay: the sizes reported for these calls
         // include them
         L.var = take({H, T, Ds}); L.G = take({H * (H + 1) / 2, T, Ds}); L.dir = take({T, Ds, D});
-        L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, U});
+        L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, o.mlp ? 0 : U});
         L.s1 = take({R, U, bf, Dh}); L.s2r = take({R, U, bf, Dh});
         L.gbeta = take({R, U, bf}); L.gy = take({R, U, bf});
         L.vws_bytes = pilco_gp_predict_vjp_workspace_bytes(pr->dyn.n, pr->dyn.D, pr->dyn.E, (int)T);
@@ -985,6 +1020,7 @@ static PtWs fs_ws_layout(const pilco_particles* pr, const PtOpt& o) {
             L.mw = take({Hm, T, Ds}); L.vw = take({Hm, T, Ds}); L.gxh = take({H, T, D});
             grids = nb * H <= 0x7fffffff;
         }
+        if (o.mlp) pm_ws_slots(L, take, pr, o);
     }
     L.total = L.pws_bytes && (!grad || L.vws_bytes) && grids ? take.bytes() : 0;
     return L;
@@ -1016,10 +1052,31 @@ static int pt_check_rewards(const pilco_particles* pr, bool no_additive_box) {
     return PILCO_OK;
 }
 
+// an MLP's sizes: L in {1, 2}, each hidden width in 1 .. PM_MAXW
+static bool pm_sizes_ok(const pilco_mlp* m) {
+    if (m->L < 1 || m->L > 2) return false;
+    for (int l = 0; l < m->L; ++l) if (m->width[l] < 1 || m->width[l] > PM_MAXW) return false;
+    return true;
+}
+
+// the MLP's device description (sizes checked): theta's length and block offsets
+static PmNet pm_net(const pilco_particles* pr, const pilco_mlp* m) {
+    PmNet n;
+    const int Ds = pr->pol.Ds, U = pr->pol.U;
+    n.L = m->L; n.w1 = m->width[0]; n.w2 = m->L == 2 ? m->width[1] : 0;
+    n.off2 = n.w1 * (Ds + 1);
+    n.offo = n.off2 + (m->L == 2 ? n.w2 * (n.w1 + 1) : 0);
+    n.n_theta = n.offo + U * ((m->L == 2 ? n.w2 : n.w1) + 1);
+    n.theta = m->theta; n.theta_bs = m->theta_bs;
+    return n;
+}
+
 // everything but the workspace (the gradients bring their own).  batched: the policy's batch strides are honoured
 // (the batch_grad and consistent_grad entry points); otherwise a batched policy is unsupported.  A: the number of
-// angular state dimensions (the policy takes dyn.E + A inputs).
-static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A = 0) {
+// angular state dimensions (the policy takes dyn.E + A inputs).  mlp_call: the MLP entry points, whose policy checks
+// are the MLP's (pol.kind PILCO_POLICY_MLP, mlp and theta not NULL, its sizes, theta_bs as a batch stride).
+static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A = 0, bool mlp_call = false,
+                         const pilco_mlp* mlp = nullptr) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
     const pilco_gp_model& g = pr->dyn;
@@ -1036,7 +1093,12 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A 
         }
         return PILCO_OK;
     };
-    if (pol.kind == PILCO_POLICY_LINEAR) {
+    if (mlp_call) {
+        if (pol.kind != PILCO_POLICY_MLP) return PILCO_ERR_UNSUPPORTED;
+        if (!mlp || !mlp->theta) return PILCO_ERR_NULL;
+        if (!pm_sizes_ok(mlp) || mlp->theta_bs < 0) return PILCO_ERR_DIM;
+        if (const int rc = strides({mlp->theta_bs})) return rc;
+    } else if (pol.kind == PILCO_POLICY_LINEAR) {
         if (!pol.W || !pol.b) return PILCO_ERR_NULL;
         if (const int rc = strides({pol.W_bs, pol.b_bs})) return rc;
     } else if (pol.kind == PILCO_POLICY_RBF) {
@@ -1063,9 +1125,10 @@ static int pt_check_ws(const void* ws, size_t ws_bytes, size_t total) {
     return PILCO_OK;
 }
 
-// the gradient's output pointers, after pt_check_desc
-static int pg_check(const pilco_particles* pr, const pilco_particles_grad* g) {
+// the gradient's output pointers, after pt_check_desc (mlp: the MLP's gtheta in place of the policy's fields)
+static int pg_check(const pilco_particles* pr, const pilco_particles_grad* g, const pilco_mlp* mlp = nullptr) {
     if (!g || !g->value || !g->ws) return PILCO_ERR_NULL;
+    if (mlp) return mlp->gtheta ? PILCO_OK : PILCO_ERR_NULL;
     if (pt_rbf(pr) ? (!g->gXc || !g->gYc || !g->gell || !g->pol_L) : (!g->gW || !g->gb)) return PILCO_ERR_NULL;
     return PILCO_OK;
 }
@@ -1117,10 +1180,12 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 // history also keeps phi(x_t) in L.phi.  nz (noise, DESIGN.md section 23; tm then given, the identity without angles):
 // pn_step_kernel in place of pa_step_kernel, which with history also keeps phi(z_t) in L.phiz.  The state width is
 // dyn.E throughout (pol.Ds without angles).  sch (an active schedule, DESIGN.md section 28): every step kernel reads
-// the linear policy through a.W and a.b, which step t's launch advances by t W_ts and t b_ts.
+// the linear policy through a.W and a.b, which step t's launch advances by t W_ts and t b_ts.  net (an MLP, DESIGN.md
+// section 29; no angles, noise or schedule): pm_step_kernel / pm_refit_kernel in place of pt_step / pr_step.
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
-                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
+                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
+                      const PmNet* net = nullptr) {
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
@@ -1152,7 +1217,7 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
         a.xt = ws + L.xt + (size_t)(t < H ? t : 0) * xstep;
         a.var = ws + L.var + (size_t)(t > 0 ? t - 1 : 0) * vstep;
         if (rs && t > 0) {
-            if (const int rc = pr_step_launch(st, grid, a, f)) return rc;
+            if (const int rc = pr_step_launch(st, grid, a, f, net)) return rc;
         } else if (nz) {
             static_cast<PtDev&>(pa) = a;
             static_cast<PaStep&>(pn) = pa;
@@ -1161,8 +1226,12 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
             static_cast<PtDev&>(pa) = a;
             if (const int rc = pa_step_launch(st, grid, pa)) return rc;
         } else {
-            launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
-            CUDA_LAUNCH_CHECK();
+            if (net) {
+                if (const int rc = pm_step_launch(st, grid, a, *net)) return rc;
+            } else {
+                launch_hi(pt_step_kernel, grid, dim3(PT_THREADS), 0, st, a);
+                CUDA_LAUNCH_CHECK();
+            }
             if (rs)                                     // t = 0: the moments of x0
                 if (const int rc = pr_step_launch(st, grid, a, f)) return rc;
         }
@@ -1239,9 +1308,13 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // rs (resampled): after the step kernel of each t = H-1 .. 1, pr_reverse_launch turns x_bar_t (the cotangent of the
 // refitted particles) into that of x'_t and rewrites var_bar_{t-1}.
 // sch (an active schedule): the step kernels of step t read W_t and b_t as pt_forward's, and the reduction is per step.
+// net (an MLP): pm_reverse_kernel in place of pg_step, then (where x~_bar_t exists) one gemm per layer adds step t's
+// d_l' [a_{l-1}; 1] to each chunk's partial, steps in order t = H-1 .. 0; pm_finish_kernel sums the chunks over P into
+// gtheta and writes value.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false,
-                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
+                      const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
+                      const PmNet* net = nullptr, double* gtheta = nullptr) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1264,6 +1337,15 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
         xb.P = P; xb.H = H; xb.E = Ds; xb.D = D; xb.t = 0; xb.n_rewards = pr->n_rewards;
         for (int k = 0; k < 8; ++k) xb.rewards[k] = k < pr->n_rewards ? pr->rewards[k] : pilco_reward_term();
         xb.traj = pr->traj; xb.tab = ws + L.tab; xb.gx = b.gx; xb.gxt = ws + L.gxt;
+    }
+    const PmChunks mc = pm_chunks(P);
+    PmBwd mb;
+    if (net) {                                          // the buffers' padding and the partials start at 0
+        mb.net = *net; mb.Pp = mc.Pp; mb.RPp = (long long)R * mc.Pp;
+        mb.in0 = ws + L.min0; mb.in1 = ws + L.min1; mb.in2 = ws + L.min2;
+        mb.d1 = ws + L.md1; mb.d2 = ws + L.md2; mb.dout = ws + L.mdo;
+        cudaMemsetAsync(ws + L.min0, 0, (L.mpart - L.min0) * sizeof(double), st);
+        cudaMemsetAsync(ws + L.mpart, 0, (size_t)R * mc.nc * net->n_theta * sizeof(double), st);
     }
     if ((joint || bonus) && H > 0) {                    // x_bar_H = 0 and x~_bar_{H-1} = 0, then the joint terms' share
         cudaMemsetAsync(b.gx, 0, TDs * sizeof(double), st);
@@ -1308,6 +1390,21 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             static_cast<PgDev&>(ab) = b;
             ab.E = Ds; ab.tm = *tm; ab.phi = ws + L.phi; ab.phib = b.gxt ? ws + L.gxt : nullptr;
             if (const int rc = pa_reverse_launch(st, grid, ab)) return rc;
+        } else if (net) {
+            if (const int rc = pm_reverse_launch(st, grid, b, mb)) return rc;
+            if (b.gxt) {                                // part[r, c] += d_l' [a_{l-1}; 1] over chunk c, layer by layer
+                const int Dh = pr->pol.Ds, U = pr->pol.U, w1 = net->w1, w2 = net->w2, two = net->L == 2;
+                const int wl = two ? w2 : w1;
+                const int out[3] = {w1, w2, U}, n[3] = {Dh + 1, w1 + 1, wl + 1}, off[3] = {0, net->off2, net->offo};
+                const double* dl[3] = {mb.d1, mb.d2, mb.dout};
+                const double* in[3] = {mb.in0, mb.in1, two ? mb.in2 : mb.in1};
+                for (int l = 0; l < 3; ++l) {
+                    if (l == 1 && !two) continue;
+                    const int rc = gemm(st, R * mc.nc, out[l], n[l], mc.Kc, 0, 1, 1.0, dl[l], (int)mb.RPp, mc.Kc,
+                                        in[l], (int)mb.RPp, mc.Kc, 1.0, ws + L.mpart + off[l], n[l], net->n_theta);
+                    if (rc) return rc;
+                }
+            }
         } else {
             launch_hi(pg_step_kernel, grid, dim3(PT_THREADS), 0, st, b);
             CUDA_LAUNCH_CHECK();
@@ -1320,6 +1417,7 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
             if (const int rc = pr_reverse_launch(st, grid, q)) return rc;
         }
     }
+    if (net) return pm_finish_launch(st, R, P, mc.nc, net->n_theta, ws + L.mpart, pr->ret, gtheta, g->value);
     return pg_reduce(pr, R, g, ws, L, st, nz ? ws + L.phiz : tm ? ws + L.phi : pr->traj, sch != nullptr);
 }
 
@@ -1480,17 +1578,21 @@ static bool pt_sched_active(const pilco_policy_schedule* sch) { return sch && (s
 // NULL or xi NULL with H > 0, then PILCO_ERR_DIM for P < 2 (no sample covariance).
 // Scheduled calls (DESIGN.md section 28), after everything else: PILCO_ERR_DIM for a negative stride, then
 // PILCO_ERR_UNSUPPORTED for an active schedule with an RBF policy.  sch NULL or both strides 0 is the call without it.
+// MLP calls (o->mlp, DESIGN.md section 29; no angles, noise or schedule): the description's policy checks are the
+// MLP's (pt_check_desc), and the gradient's outputs are value, ws and mlp->gtheta.
 static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                        const pilco_exploration* ex, int R, const pilco_particles_grad* g,
-                       const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
+                       const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
+                       const pilco_mlp* mlp = nullptr) {
     if (!pr) return PILCO_ERR_NULL;
     const bool angles = !pa_none(ang);
     if (angles)
         if (const int rc = pa_map(pr, ang, &o->tm)) return rc;
-    if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0)) return rc;
+    if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0, o->mlp, mlp)) return rc;
     if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;   // the unbatched calls' R = 1 passes with the description
     if (o->call != PT_FORWARD)
-        if (const int rc = pg_check(pr, g)) return rc;
+        if (const int rc = pg_check(pr, g, o->mlp ? mlp : nullptr)) return rc;
+    if (o->mlp) o->net = pm_net(pr, mlp);
     if (o->resampled) {
         if (!rs || (!rs->xi && pr->H > 0)) return PILCO_ERR_NULL;
         if (pr->P < 2) return PILCO_ERR_DIM;
@@ -1517,10 +1619,15 @@ static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* 
 // A call's workspace: its layout's total, 0 where the call would fail on its sizes.  The sizes accepted are the
 // description's own (pt_sizes_ok, not its width consistency), R, the angles' map, 1 <= E <= PILCO_MAX_E and valid
 // variances with noise, and the exploration's checks when active; a schedule only adds non-negative strides (its
-// workspace is the call's without it).
+// workspace is the call's without it); an MLP call adds mlp != NULL and its sizes (L, the widths).
 static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
-                       const pilco_exploration* ex, int R, const pilco_policy_schedule* sch = nullptr) {
+                       const pilco_exploration* ex, int R, const pilco_policy_schedule* sch = nullptr,
+                       const pilco_mlp* mlp = nullptr) {
     if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    if (o.mlp) {                                        // the MLP's sizes (NULL: none to size the workspace with)
+        if (!mlp || !pm_sizes_ok(mlp)) return 0;
+        o.net = pm_net(pr, mlp);
+    }
     if (sch && (sch->W_ts < 0 || sch->b_ts < 0)) return 0;
     if (!pa_none(ang) && pa_map(pr, ang, &o.tm)) return 0;
     if (nz && (pr->dyn.E < 1 || pr->dyn.E > MAXE || pn_noise(pr, nz, &o.nz))) return 0;
@@ -1536,8 +1643,9 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
 // moments after the forward; with b != 0 the bonus's share in the reverse sweep and the bonus in value after it.
 static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                    const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream,
-                   const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr) {
-    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs, sch)) return rc;
+                   const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
+                   const pilco_mlp* mlp = nullptr) {
+    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs, sch, mlp)) return rc;
     const bool fwd = o.call == PT_FORWARD;
     const PtWs L = o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
     if (const int rc = fwd ? pt_check_ws(pr->ws, pr->ws_bytes, L.total) : pt_check_ws(g->ws, g->ws_bytes, L.total))
@@ -1553,7 +1661,8 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
     const PnNoise* n = o.noisy ? &o.nz : nullptr;
     const pilco_particles_resample* rsv = o.resampled ? &o.rs : nullptr;
     const pilco_policy_schedule* sv = o.sched ? &o.sch : nullptr;
-    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv)) return rc;
+    const PmNet* net = o.mlp ? &o.net : nullptr;
+    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv, net)) return rc;
     if (fwd) return PILCO_OK;
     if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
     if (o.explore) {
@@ -1561,7 +1670,8 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
         m.step_var = o.step_var; m.sd = ws + L.sd; m.tab = o.bonus ? ws + L.tab : nullptr;
         if (const int rc = px_moments_launch(st, R, m)) return rc;
     }
-    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv, sv)) return rc;
+    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv, sv, net, o.mlp ? mlp->gtheta : nullptr))
+        return rc;
     if (o.bonus && pr->H > 0) return px_value_launch(st, R, pr->H, o.b, ws + L.sd, g->value);
     return PILCO_OK;
 }
@@ -1571,6 +1681,9 @@ static const PtOpt FWD = {false, PT_FORWARD, false}, CFWD = {true, PT_FORWARD, f
 static const PtOpt PATH1 = {false, PT_PATHWISE, false}, PATH = {false, PT_PATHWISE, true};
 static const PtOpt CPATH = {true, PT_PATHWISE, true}, SCORE = {false, PT_SCORE, true}, CSCORE = {true, PT_SCORE, true};
 static const PtOpt RFWD = {false, PT_FORWARD, false, true}, RPATH = {false, PT_PATHWISE, true, true};
+
+// the MLP calls (DESIGN.md section 29): a family's options with o.mlp
+static PtOpt pm_opt(PtOpt o) { o.mlp = true; return o; }
 
 extern "C" {
 
@@ -1880,6 +1993,68 @@ int pilco_particles_scheduled_resampled_grad_rollout(const pilco_particles* pr, 
                                                      const pilco_policy_schedule* sch, int R,
                                                      const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(RPATH, pr, nullptr, nullptr, nullptr, R, g, stream, rs, sch);
+}
+
+// tanh MLP policies (DESIGN.md section 29): the step-wise, consistent and resampled samplers, forward and pathwise
+size_t pilco_particles_mlp_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp) {
+    return pt_query(pm_opt(FWD), pr, nullptr, nullptr, nullptr, 1, nullptr, mlp);
+}
+
+int pilco_particles_mlp_rollout(const pilco_particles* pr, const pilco_mlp* mlp, pilco_stream_t stream) {
+    return pt_call(pm_opt(FWD), pr, nullptr, nullptr, nullptr, 1, nullptr, stream, nullptr, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_consistent_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp) {
+    return pt_query(pm_opt(CFWD), pr, nullptr, nullptr, nullptr, 1, nullptr, mlp);
+}
+
+int pilco_particles_mlp_consistent_rollout(const pilco_particles* pr, const pilco_mlp* mlp, pilco_stream_t stream) {
+    return pt_call(pm_opt(CFWD), pr, nullptr, nullptr, nullptr, 1, nullptr, stream, nullptr, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_resampled_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                     const pilco_particles_resample* rs) {
+    (void)rs;                                           // the sizes do not depend on it
+    return pt_query(pm_opt(RFWD), pr, nullptr, nullptr, nullptr, 1, nullptr, mlp);
+}
+
+int pilco_particles_mlp_resampled_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                          const pilco_particles_resample* rs, pilco_stream_t stream) {
+    return pt_call(pm_opt(RFWD), pr, nullptr, nullptr, nullptr, 1, nullptr, stream, rs, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_batch_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                      const pilco_exploration* ex, int R) {
+    return pt_query(pm_opt(PATH), pr, nullptr, nullptr, ex, R, nullptr, mlp);
+}
+
+int pilco_particles_mlp_batch_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                           const pilco_exploration* ex, int R, const pilco_particles_grad* g,
+                                           pilco_stream_t stream) {
+    return pt_call(pm_opt(PATH), pr, nullptr, nullptr, ex, R, g, stream, nullptr, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                           const pilco_exploration* ex, int R) {
+    return pt_query(pm_opt(CPATH), pr, nullptr, nullptr, ex, R, nullptr, mlp);
+}
+
+int pilco_particles_mlp_consistent_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                const pilco_exploration* ex, int R, const pilco_particles_grad* g,
+                                                pilco_stream_t stream) {
+    return pt_call(pm_opt(CPATH), pr, nullptr, nullptr, ex, R, g, stream, nullptr, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_resampled_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                          const pilco_particles_resample* rs, int R) {
+    (void)rs;
+    return pt_query(pm_opt(RPATH), pr, nullptr, nullptr, nullptr, R, nullptr, mlp);
+}
+
+int pilco_particles_mlp_resampled_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                               const pilco_particles_resample* rs, int R,
+                                               const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(pm_opt(RPATH), pr, nullptr, nullptr, nullptr, R, g, stream, rs, nullptr, mlp);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,

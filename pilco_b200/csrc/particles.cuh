@@ -1,7 +1,8 @@
 // particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu,
-// particles_explore.cu, particles_cscore.cu and particles_resample.cu share: the per-particle argument structs, the
-// reward value at a point, the step's work at a given state, the fixed-order block sum, and the angle, noise,
-// exploration, consistent-score and resampling kernels' launchers (DESIGN.md sections 11, 12, 20, 23, 24, 25 and 26).
+// particles_explore.cu, particles_cscore.cu, particles_resample.cu and particles_mlp.cu share: the per-particle argument
+// structs, the reward value at a point, the step's work at a given state, the fixed-order block sum, and the angle,
+// noise, exploration, consistent-score, resampling and MLP-policy kernels' launchers (DESIGN.md sections 11, 12, 20, 23,
+// 24, 25, 26 and 29).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -263,8 +264,10 @@ struct PrFwd {
 
 // step a.t of the resampled forward, in place of the step kernel: t = 0 (after pt_step<0>) x0's moments when they are
 // asked for; t >= 1 the closure into x'_t, the moments and factor (grid R) and pr_step_kernel, which redraws x_t and
-// does pt_step_kernel's work at it.  grid = (ceil(P / 128), R).
-int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f);
+// does pt_step_kernel's work at it.  grid = (ceil(P / 128), R).  net (an MLP policy, DESIGN.md section 29):
+// pm_refit_kernel (particles_mlp.cu) in place of pr_step_kernel.
+struct PmNet;
+int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f, const PmNet* net = nullptr);
 
 // the refit's reverse at step t (1 <= t <= H-1), after the reverse step kernel has left y_bar_p = the cotangent of the
 // refitted x_pt in gx: gx <- the cotangent of x'_pt, gvar <- that of var_{t-1}
@@ -279,3 +282,36 @@ struct PrBwd {
 
 // grid = (ceil(P / 128), R): pr_adjoint_kernel (grid R), then pr_scatter_kernel
 int pr_reverse_launch(cudaStream_t st, dim3 grid, const PrBwd& b);
+
+// ---- tanh MLP policies (particles_mlp.cu, DESIGN.md section 29) ---------------------------------------------------------
+// h_1 = tanh(A_1 [x; 1]), (L = 2) h_2 = tanh(A_2 [h_1; 1]), z = A_out [h_L; 1]; every A row-major [out, in + 1], the bias
+// its last column; theta = the A blocks in that order, restart r's at theta + r theta_bs.  The step kernels read the
+// policy from PmNet (PtPolicy's linear and RBF fields are unused); everything else is the linear path's.
+#define PM_MAXW   64                    // widest hidden layer
+#define PM_CHUNKS 16                    // the reduction's particle chunks per restart (at most)
+struct PmNet {
+    int L, w1, w2;                      // w2 = 0 when L = 1
+    int n_theta, off2, offo;            // theta's length; where A_2 (L = 2) and A_out start
+    const double* theta; long long theta_bs;
+};
+
+// The reverse step's per-particle buffers, feature-major [width, RPp] (column row = r Pp + p; Pp = the restart's rows
+// padded to whole reduction chunks, the padding zero): the layer inputs [x; 1], [h_1; 1], [h_2; 1] and the
+// pre-activation cotangents d_1, d_2, d_out (= z_bar_t) of the current step
+struct PmBwd {
+    PmNet net;
+    long long RPp, Pp;
+    double* in0; double* in1; double* in2;
+    double* d1; double* d2; double* dout;
+};
+
+// grid (ceil(P / 128), R): the MLP's forward step t, in place of pt_step_kernel
+int pm_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PmNet& m);
+// grid (ceil(P / 128), R): the MLP's refit step t >= 1, in place of pr_step_kernel
+int pm_refit_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f, const PmNet& m);
+// grid (ceil(P / 128), R): the MLP's reverse step t, in place of pg_step_kernel (x_bar_t, var_bar_{t-1}; with a.gxt the
+// step's layer inputs and cotangents into b's buffers)
+int pm_reverse_launch(cudaStream_t st, dim3 grid, const PgDev& a, const PmBwd& b);
+// gtheta [R, n_theta] = (1/P) sum of the chunk partials part [R, nc, n_theta] in chunk order; value [R] = the mean return
+int pm_finish_launch(cudaStream_t st, int R, int P, int nc, int n_theta, const double* part, const double* ret,
+                     double* gtheta, double* value);

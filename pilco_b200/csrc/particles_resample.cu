@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(PT_THREADS) pr_scatter_kernel(PrBwd b) {
     }
 }
 
-int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f) {
+int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f, const PmNet* net) {
     const int R = grid.y, t = a.t;
     PrMom m;
     m.P = f.P; m.Ds = f.Ds; m.t = t; m.H = f.H;
@@ -211,6 +211,7 @@ int pr_step_launch(cudaStream_t st, dim3 grid, const PtDev& a, const PrFwd& f) {
     m.x = f.xp + (size_t)(t - 1) * R * f.P * f.Ds; m.rs = (long long)f.P * f.Ds; m.mu = f.mu; m.L = f.L;
     launch_hi(pr_moments_kernel, dim3(R), dim3(256), 0, st, m);
     CUDA_LAUNCH_CHECK();
+    if (net) return pm_refit_launch(st, grid, a, f, *net);
     launch_hi(pr_step_kernel, grid, dim3(PT_THREADS), 0, st, a, f);
     CUDA_LAUNCH_CHECK();
     return PILCO_OK;

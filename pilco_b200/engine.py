@@ -474,10 +474,54 @@ def _fill_policy(pol, policy_spec, batched=None):
         bat = W.dim() == 3 if batched is None else batched
         pol.W, pol.W_bs = W.data_ptr(), U * Ds if bat else 0
         pol.b, pol.b_bs = b.data_ptr(), U if bat else 0
-    else:
+    elif pol.kind == _lib.POLICY_RBF:
         rbf = policy_spec["gp"]
         pol.rbf = rbf.struct()
     return max_action, W, b, rbf
+
+
+MLP_MAX_WIDTH = 64                                       # the widest hidden layer the MLP kernels take
+
+
+def mlp_theta_size(Ds, U, hidden):
+    """the length of a tanh MLP's flat parameter vector: A_1 [w1, Ds+1], (A_2 [w2, w1+1],) A_out [U, w_L+1]"""
+    widths = [int(Ds)] + [int(w) for w in hidden]
+    return sum(widths[l + 1] * (widths[l] + 1) for l in range(len(hidden))) + int(U) * (widths[-1] + 1)
+
+
+def _is_mlp(policy_spec):
+    return isinstance(policy_spec, dict) and policy_spec.get("kind") == _lib.POLICY_MLP
+
+
+def _refuse_mlp(policy_spec, what):
+    """the moment-matching plans take no MLP spec (it has no closed-form moments): ValueError before any allocation"""
+    if _is_mlp(policy_spec):
+        raise ValueError("%s: an MLP policy runs in the particle rollouts only (ParticlePlan, ConsistentGradPlan, "
+                         "particles_rollout); moment matching has no closed form for it" % what)
+
+
+def _particle_mlp(policy_spec, what, R=1, angles=None, measurement_noise=None, schedule=False, estimator="pathwise"):
+    """An MLP spec's refusals and checks for the particle plans, before any allocation (ValueError): no angles,
+    measurement noise, schedule or score estimator; 1 or 2 hidden layers of 1 .. 64 units; theta [n_theta] or
+    [R, n_theta].  Returns (L, widths, n_theta, batched) for an MLP spec, else None."""
+    if not _is_mlp(policy_spec):
+        return None
+    for on, feat in ((angles is not None and len(angles) > 0, "angles"),
+                     (measurement_noise is not None, "measurement_noise"), (bool(schedule), "schedule=True"),
+                     (estimator == "score", "estimator='score'")):
+        if on:
+            raise ValueError("%s: an MLP policy does not combine with %s" % (what, feat))
+    hidden = tuple(int(w) for w in policy_spec["hidden"])
+    if len(hidden) not in (1, 2) or any(w < 1 or w > MLP_MAX_WIDTH for w in hidden):
+        raise ValueError("%s: an MLP policy has 1 or 2 hidden layers of 1 .. %d units, got hidden=%s"
+                         % (what, MLP_MAX_WIDTH, hidden))
+    n = mlp_theta_size(policy_spec["Ds"], policy_spec["U"], hidden)
+    shape = tuple(np.shape(policy_spec["theta"]))
+    if shape not in ((n,), (int(R), n)) or (int(R) > 1 and shape != (int(R), n)):
+        raise ValueError("%s: the MLP (Ds=%d, hidden=%s, U=%d) has %d parameters: theta must be [%s%d], got %s"
+                         % (what, int(policy_spec["Ds"]), hidden, int(policy_spec["U"]), n,
+                            "%d, " % int(R) if int(R) > 1 else "R?, ", n, shape))
+    return len(hidden), hidden, n, len(shape) == 2
 
 
 def _schedule_check(policy_spec, H, schedule):
@@ -585,6 +629,7 @@ class RolloutPlan:
         section 27); the spec's W is [Hw, U, Ds] or [R, Hw, U, Ds] and b [Hw, U] or [R, Hw, U], Hw >= H (step t < H reads
         W[..., t, :, :]).  ``backward()`` then returns the per-step cotangents W [R, H, U, Ds] and b [R, H, U].  An RBF
         spec or Hw < H is a ValueError."""
+        _refuse_mlp(policy_spec, "RolloutPlan")
         sched = _schedule_check(policy_spec, H, schedule)
         b = None
         if exploration is not None:
@@ -760,6 +805,17 @@ PARTICLE_SCHEDULED_CALLS = {
     ("resampled", "pathwise"): ("scheduled_resampled_grad_rollout", "scheduled_resampled_grad_workspace_bytes"),
 }
 
+# the rows a tanh MLP policy runs (DESIGN.md section 29): each sampler's forward and pathwise call with a pilco_mlp
+# after pr (then the exploration for the step-wise and consistent gradients, the refit's buffers for the resampled)
+PARTICLE_MLP_CALLS = {
+    (False, "forward"): ("mlp_rollout", "mlp_workspace_bytes"),
+    (True, "forward"): ("mlp_consistent_rollout", "mlp_consistent_workspace_bytes"),
+    (False, "pathwise"): ("mlp_batch_grad_rollout", "mlp_batch_grad_workspace_bytes"),
+    (True, "pathwise"): ("mlp_consistent_grad_rollout", "mlp_consistent_grad_workspace_bytes"),
+    ("resampled", "forward"): ("mlp_resampled_rollout", "mlp_resampled_workspace_bytes"),
+    ("resampled", "pathwise"): ("mlp_resampled_grad_rollout", "mlp_resampled_grad_workspace_bytes"),
+}
+
 
 class ParticlePlan:
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
@@ -812,13 +868,21 @@ class ParticlePlan:
     section 28), with every sampler, estimator and feature above.  The spec's W is [Hw, U, Ds] or [R, Hw, U, Ds] and b
     [Hw, U] or [R, Hw, U], Hw >= H (step t < H reads W[..., t, :, :]); ``launch_grad()`` then returns the per-step
     gradients 'W' [R?, H, U, Ds] and 'b' [R?, H, U].  An RBF spec or Hw < H is a ValueError raised before any
-    allocation, and so is a scheduled spec without ``schedule=True``."""
+    allocation, and so is a scheduled spec without ``schedule=True``.
+
+    A tanh MLP policy (pilco_particles_mlp_*, DESIGN.md section 29): ``dict(kind=POLICY_MLP, Ds, U, squash,
+    max_action, hidden=(w1[, w2]), theta)``, theta [n_theta] or [R, n_theta] in ``mlp_theta_size``'s flat layout (A_1,
+    (A_2,) A_out, each row-major [out, in + 1] with the bias last).  Every sampler, forward and pathwise, with
+    exploration; ``launch_grad()`` returns {'value', 'theta' [R?, n_theta]}.  With ``angles``, ``measurement_noise``,
+    ``schedule=True`` or ``estimator="score"``, or a theta of the wrong length, it is a ValueError raised before any
+    allocation."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
                  estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False,
                  schedule=False):
+        mlp = _particle_mlp(policy_spec, "ParticlePlan", R, angles, measurement_noise, schedule, estimator)
         sched = _particle_schedule(policy_spec, H, schedule, "ParticlePlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
@@ -837,7 +901,7 @@ class ParticlePlan:
                              "ConsistentGradPlan, not ParticlePlan(grad=True)")
         self.consistent = bool(consistent)
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration,
-                       sched)
+                       sched, mlp)
         pr, d = self.pr, device()
         P, H = self.P, self.H
         if not self.batched:                                    # the forward-only rollout (a batch has none)
@@ -857,6 +921,10 @@ class ParticlePlan:
         """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise), the schedule
         (scheduled calls) and R; resampled: pr, the refit's buffers, the schedule and R"""
         sch = [C.byref(self.sch)] if self.sch is not None else []
+        if self.mlp is not None:
+            feat = [C.byref(self.rs)] if self.resample else \
+                [] if kind == "forward" else [C.byref(self.ex) if self.ex is not None else None]
+            return [C.byref(pr), C.byref(self.mlp)] + feat + ([self.R] if kind != "forward" else [])
         if self.resample:
             return [C.byref(pr), C.byref(self.rs)] + sch + ([self.R] if kind != "forward" else [])
         args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
@@ -866,7 +934,9 @@ class ParticlePlan:
 
     def _names(self, kind):
         """(rollout, size query) of kind's call, each after the prefix pilco_particles_"""
-        return (PARTICLE_CALLS if self.sch is None else PARTICLE_SCHEDULED_CALLS)[self._sampler(), kind]
+        table = PARTICLE_MLP_CALLS if self.mlp is not None else \
+            PARTICLE_CALLS if self.sch is None else PARTICLE_SCHEDULED_CALLS
+        return table[self._sampler(), kind]
 
     def _query(self, kind, pr):
         return int(getattr(lib, "pilco_particles_" + self._names(kind)[1])(*self._args(kind, pr)))
@@ -878,11 +948,12 @@ class ParticlePlan:
         return self._query(self.estimator, pr)
 
     def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None,
-                  exploration=None, sched=None):
+                  exploration=None, sched=None, mlp=None):
         """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
         The angles, the policy's width, the measurement noise and the exploration weight are checked first, before any
-        device work.  ``sched``: ``_schedule_check``'s (batched, Hw) of a scheduled spec, or None."""
-        self.ang, self.nz, self.ex, self.sch = None, None, None, None
+        device work.  ``sched``: ``_schedule_check``'s (batched, Hw) of a scheduled spec, or None; ``mlp``:
+        ``_particle_mlp``'s (L, widths, n_theta, batched) of an MLP spec, or None."""
+        self.ang, self.nz, self.ex, self.sch, self.mlp = None, None, None, None, None
         b = _particle_exploration(exploration, reward_terms, P)
         if angles is not None and len(angles) > 0:
             E = int(dyn.struct().E)
@@ -900,7 +971,7 @@ class ParticlePlan:
         if self.ang is not None:
             self.Ds = int(dyn.struct().E)
         rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
-        self.batched = R > 1 or rbf_batched
+        self.batched = R > 1 or rbf_batched or (mlp is not None and mlp[3])
         if self.batched and not grad:
             raise ValueError("particles: a batch of policies runs the gradient path only (grad=True)")
         lead = (R,) if self.batched else ()
@@ -917,6 +988,12 @@ class ParticlePlan:
                                  "[Hw,U,Ds], [Hw,U])" % R)
             pr.pol.W_bs, pr.pol.b_bs = (Hw * U * Ds, Hw * U) if self.batched else (0, 0)
             self.sch = _lib.PolicySchedule(U * Ds, U)
+        elif mlp is not None:                                   # theta [R?, n_theta] (its length checked)
+            L, hidden, n_theta, _ = mlp
+            self.theta = dev(policy_spec["theta"])
+            self.n_theta = n_theta
+            self.mlp = _lib.Mlp(L, (C.c_int * 2)(hidden[0], hidden[-1] if L == 2 else 0), self.theta.data_ptr(),
+                                n_theta if self.batched else 0, None)
         elif pr.pol.kind == _lib.POLICY_LINEAR:
             if self.W.numel() != R * U * Ds or self.b.numel() != R * U:
                 raise ValueError("particles: expected W [R,U,Ds] and b [R,U] with R=%d (unbatched: [U,Ds], [U])" % R)
@@ -963,7 +1040,10 @@ class ParticlePlan:
         if gwsb == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, pr.dyn.D, self.R))
         g = _lib.ParticlesGrad()
-        if self.sch is None:
+        if self.mlp is not None:                                # d value / d theta [R?, n_theta]
+            self.gbuf = {"theta": torch.zeros((*self.lead, self.n_theta), dtype=F64, device=d)}
+            self.mlp.gtheta = self.gbuf["theta"].data_ptr()
+        elif self.sch is None:
             self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead)
         else:                                                   # per step; H = 0 still has an address
             self.gbuf = _policy_grad_buffers(g, pr.pol, self.rbf, self.lead + (max(self.H, 1),))
@@ -981,7 +1061,8 @@ class ParticlePlan:
         lengthscales), like ``RolloutPlan.backward``.  A batched plan returns them with a leading R ('value' [R]).
         ``estimator="score"``: the score-function gradient (pilco_particles_rollout_score_grad) in the same layout.
         With ``exploration``: value and gradient of the exploration objective, and sigma_t^2 in ``step_var``.  With
-        ``schedule``: 'W' [R?,H,U,Ds] and 'b' [R?,H,U], one gradient per step."""
+        ``schedule``: 'W' [R?,H,U,Ds] and 'b' [R?,H,U], one gradient per step.  An MLP policy: {'value', 'theta'
+        [R?, n_theta]}."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
         self._call(self.estimator, C.byref(self.grad))
@@ -1038,10 +1119,11 @@ class ConsistentGradPlan(ParticlePlan):
     rollout, value and output layout; its estimate is unbiased on rollouts without degenerate pivots.  ``"score"`` with
     ``exploration``, or an unknown estimator, is a ValueError raised before any allocation.
 
-    ``schedule=True``: a time-varying linear policy, as ``ParticlePlan``."""
+    ``schedule=True``: a time-varying linear policy, as ``ParticlePlan``.  A tanh MLP policy: as ``ParticlePlan``."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
                  measurement_noise=None, exploration=None, estimator="pathwise", schedule=False):
+        mlp = _particle_mlp(policy_spec, "ConsistentGradPlan", R, angles, measurement_noise, schedule, estimator)
         sched = _particle_schedule(policy_spec, H, schedule, "ConsistentGradPlan")
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
@@ -1051,7 +1133,7 @@ class ConsistentGradPlan(ParticlePlan):
         self.estimator = estimator
         self.consistent, self.resample = True, False
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, True, angles, measurement_noise, exploration,
-                       sched)
+                       sched, mlp)
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
@@ -1202,7 +1284,10 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     redraw's standard normals (required with it, and only then).  The result then also has the fitted moments:
     (traj, act, step_reward, step_risk, ret, step_mean [H+1,Ds], step_cov [H+1,Ds,Ds]).
 
-    ``schedule=True``: a time-varying linear policy (W [Hw,U,Ds], b [Hw,U], Hw >= H), as ``ParticlePlan``."""
+    ``schedule=True``: a time-varying linear policy (W [Hw,U,Ds], b [Hw,U], Hw >= H), as ``ParticlePlan``.
+
+    A tanh MLP spec (theta [n_theta]) runs every sampler, as ``ParticlePlan``."""
+    _particle_mlp(policy_spec, "particles_rollout", 1, angles, measurement_noise, schedule)
     _particle_schedule(policy_spec, eps.shape[1] if len(np.shape(eps)) == 3 else 0, schedule, "particles_rollout")
     if resample:
         _resample_check(x0.shape[0], consistent, "pathwise", angles, measurement_noise, None)
@@ -1296,6 +1381,7 @@ class PredictPlan:
                  schedule=False):
         """``Ds``: the state dimension (the dynamics GP's outputs); ``angles``, ``measurement_noise``, ``schedule``: as
         RolloutPlan."""
+        _refuse_mlp(policy_spec, "PredictPlan")
         d = device()
         self.Ds, self.n = int(Ds), int(n)
         Ds = self.Ds
@@ -1400,6 +1486,7 @@ class ActionPlan:
     one stream synchronisation instead of ~10 allocations and 4-6 separate launches."""
 
     def __init__(self, policy_spec):
+        _refuse_mlp(policy_spec, "ActionPlan")
         d = device()
         self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
         Ds, U = self.Ds, self.U

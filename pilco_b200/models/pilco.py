@@ -48,6 +48,8 @@ def _controller_input_dim(c):
         return int(c.policy_shapes[1])
     if isinstance(c, (controllers.LinearController, controllers.TimeVaryingLinearController)):
         return int(np.asarray(c.W).shape[-1])
+    if isinstance(c, controllers.MlpController):
+        return c.state_dim
     return None
 
 
@@ -181,6 +183,12 @@ class PILCO:
             raise ValueError("%s: the particle rollouts do not support the TimeVaryingLinearController; use the "
                              "moment-matching methods (predict, policy_gradient, optimize_policy, plan)" % what)
 
+    def _no_mlp(self, what):
+        """the moment-matching methods refuse an MlpController (no closed-form moments), before any device work"""
+        if isinstance(self.controller, controllers.MlpController):
+            raise TypeError("%s: an MlpController has no moment-matching closed form; train it on the sampled return "
+                            "with optimize_policy_sampled (and inspect it with sample_trajectories)" % what)
+
     def _no_angles(self, what):
         if self.angle_dims:
             raise ValueError("%s: the particle rollouts do not support angle_dims yet; use the moment-matching methods "
@@ -195,7 +203,8 @@ class PILCO:
     def policy_spec(self, flats=None):
         """Description of the policy for ``RolloutPlan``; ``flats`` [R,P] = per-restart flat parameters."""
         c = self.controller
-        if isinstance(c, (controllers.LinearController, controllers.TimeVaryingLinearController)):
+        if isinstance(c, (controllers.LinearController, controllers.TimeVaryingLinearController,
+                          controllers.MlpController)):
             return c.policy_spec(flats)
         if isinstance(c, controllers.RbfController):
             bf, Ds, U = c.policy_shapes
@@ -219,6 +228,7 @@ class PILCO:
         return self.reward.terms(), 0.0
 
     def rollout_plan(self, m_x, s_x, n, flats=None):
+        self._no_mlp("rollout_plan")
         R = 1 if flats is None else int(np.asarray(flats).shape[0])
         terms, mult_mu = self.reward_spec()
         return engine.RolloutPlan(self.mgpr.device_gp(), self.policy_spec(flats), terms,
@@ -258,12 +268,14 @@ class PILCO:
     def predict(self, m_x, s_x, n):
         """n-step cascade (pilco.py:118-136) -> (m [1,Ds], S [Ds,Ds], reward [1,1]): one replay of a cached
         CUDA graph (host moments in, host moments out)."""
+        self._no_mlp("predict")
         from ..params import HostArray
         M, S, rew = self._predict_plan(n)(m_x, s_x)
         return M.view(HostArray), S.view(HostArray), rew.view(HostArray)
 
     def propagate(self, m_x, s_x):
         """one step (pilco.py:138-153) -> (M_x [1,Ds], S_x [Ds,Ds])"""
+        self._no_mlp("propagate")
         M, S, _ = self.predict(m_x, s_x, 1)
         return M, S
 
@@ -356,6 +368,8 @@ class PILCO:
         """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
         derivative of the softplus transform, sigmoid(theta), as policy_opt applies it"""
         c = self.controller
+        if isinstance(c, controllers.MlpController):
+            return g["theta"].cpu().numpy().ravel()
         if isinstance(c, controllers.TimeVaryingLinearController):
             return c.flat_grad(g["W"].cpu().numpy(), g["b"].cpu().numpy())
         if isinstance(c, controllers.LinearController):
@@ -434,6 +448,8 @@ class PILCO:
         if estimator not in engine.ParticlePlan.ESTIMATORS:
             raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
                              % (engine.ParticlePlan.ESTIMATORS, estimator))
+        if estimator == "score":
+            self._no_mlp("sample_policy_gradient(estimator='score')")
         if consistent and estimator == "score":
             raise ValueError("sample_policy_gradient: the score-function estimator over the consistent (function-sample) "
                              "particles is engine.ConsistentGradPlan(..., estimator='score'); this method offers "
@@ -466,6 +482,7 @@ class PILCO:
         ``predict`` sums) and sigma_t^2 = sum_k c_k^2 Var[r_k] over the additive terms (CombinedRewards' rule), how sure
         the model is of the reward at step t (DESIGN.md section 21).  -> (mean [n], var [n]) host arrays.  A reward with
         an additive box term is a ValueError (no variance closed form)."""
+        self._no_mlp("predict_reward_moments")
         from ..params import HostArray
         n = int(n)
         plan = self._single_plan(m_x, s_x, n, exploration=0.0)
@@ -480,6 +497,7 @@ class PILCO:
         its gradient d reward / d controller.get_flat() for the current policy: the direction ``optimize_policy``
         ascends, in the layout of ``sample_policy_gradient``.  With ``exploration`` b != 0 the reward is the objective
         sum_t (E[r_t] + b sigma_t).  -> (reward (float), grad host array)."""
+        self._no_mlp("policy_gradient")
         from ..params import HostArray
         m_x = self.m_init if m_x is None else m_x
         s_x = self.S_init if s_x is None else s_x
@@ -557,6 +575,7 @@ class PILCO:
     def training_loss(self):
         """-(the objective optimize_policy maximises) from N(m_init, S_init) over the horizon: -predict's reward, or with
         ``exploration`` b != 0, -sum_t (E[r_t] + b sigma_t) -> [1,1] host array"""
+        self._no_mlp("training_loss")
         b = self._exploration_b()
         if b is None:
             return -self.predict(self.m_init, self.S_init, self.horizon)[2]
@@ -569,6 +588,7 @@ class PILCO:
         return (-plan.reward[:1].reshape(1, 1)).cpu().numpy().view(HostArray)
 
     def compute_reward(self):
+        self._no_mlp("compute_reward")
         return -self.training_loss()
 
     @property
@@ -580,9 +600,14 @@ class PILCO:
         ``engine.ActionPlan`` (one captured CUDA graph per policy state) -- the per-control-step call of
         examples/utils.py:32-36.  With angle_dims, x_m is the raw state and phi(x_m) is formed on the host.
         ``t``: the step whose parameters a TimeVaryingLinearController applies (0 .. horizon-1); a stationary policy
-        is the same at every step."""
+        is the same at every step.  An MlpController: its host fp64 evaluation at the point (MlpController.compute_action)."""
         from ..params import HostArray
         c = self.controller
+        if isinstance(c, controllers.MlpController):
+            if self.angle_dims:
+                x_m = engine.trig_feature_map(np.asarray(x_m, dtype=np.float64).reshape(1, self.state_dim),
+                                              self.angle_dims)
+            return c.compute_action(np.asarray(x_m, dtype=np.float64).reshape(1, -1))[0].view(HostArray)
         sched = isinstance(c, controllers.TimeVaryingLinearController)
         t = int(t) if sched else 0
         if sched and not 0 <= t < c.horizon:
@@ -617,6 +642,7 @@ class PILCO:
 
     # ---- policy optimisation (pilco.py:75-113) --------------------------------------------------------
     def optimize_policy(self, maxiter=50, restarts=1):
+        self._no_mlp("optimize_policy")
         from .. import policy_opt
         self._scheduled(self.horizon)
         start = time.time()
@@ -654,6 +680,7 @@ class PILCO:
         ``measurement_noise`` are a ValueError raised before any device work."""
         from functools import partial
         from .. import policy_opt
+        self._no_mlp("plan")
         c = self.controller
         if not isinstance(c, controllers.TimeVaryingLinearController):
             raise TypeError("plan: needs a TimeVaryingLinearController, the controller is a %s" % type(c).__name__)

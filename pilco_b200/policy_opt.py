@@ -49,9 +49,12 @@ class _FlatEvaluator:
         self.c = c
         self.sched = isinstance(c, controllers.TimeVaryingLinearController)     # per-step W_t, b_t
         self.linear = isinstance(c, controllers.LinearController) or self.sched
+        self.mlp = isinstance(c, controllers.MlpController)                      # theta as the flat vector itself
         self.flat0 = np.tile(c.get_flat(), (R, 1))
         self.P = self.flat0.shape[1]
-        if self.linear:
+        if self.mlp:
+            U, Ds = c.control_dim, c.state_dim
+        elif self.linear:
             U, Ds = c.W.shape[-2:]
         else:
             bf, Ds, U = c.policy_shapes
@@ -118,6 +121,9 @@ class _FlatEvaluator:
         returns the lengthscales' unconstrained theta [R,U,Ds] (RBF) or None"""
         R = flat.shape[0]
         Ds, U = self.shape
+        if self.mlp:
+            plan.theta.copy_(flat.reshape(plan.theta.shape))
+            return None
         if self.sched:                                         # W stays the spec's zeros without feedback
             nW = self.c.horizon * U * Ds if self.c.feedback else 0
             if nW:
@@ -145,7 +151,9 @@ class _FlatEvaluator:
         Ds, U = self.shape
         out[:, 0] = -value
         out[:, 1] = info.to(torch.float64)
-        if self.sched:                                         # steps 0 .. H-1 of the horizon's: the rest get 0
+        if self.mlp:
+            out[:, 2:] = -g["theta"].reshape(R, -1)
+        elif self.sched:                                         # steps 0 .. H-1 of the horizon's: the rest get 0
             nW = self.c.horizon * U * Ds if self.c.feedback else 0
             out[:, 2:] = 0.0
             if nW:
@@ -235,7 +243,8 @@ class ParticleEvaluator(_FlatEvaluator):
     None (the default) is the mean return.  ``resample=True``: Deep PILCO's Gaussian refit at every step
     (pilco_particles_resampled_grad_rollout, DESIGN.md section 26) with the redraw's standard normals ``xi`` [P,H,Ds],
     held fixed like eps.  A ``TimeVaryingLinearController`` runs the scheduled calls (pilco_particles_scheduled_*,
-    DESIGN.md section 28), its gradient per step."""
+    DESIGN.md section 28), its gradient per step; an ``MlpController`` the MLP calls (pilco_particles_mlp_*, section 29),
+    its flat vector being the device's theta."""
 
     def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None):
         terms, mult_mu = pilco.reward_spec()
@@ -244,8 +253,8 @@ class ParticleEvaluator(_FlatEvaluator):
                              "almost everywhere, so optimising it would ignore the constraint")
         super().__init__(pilco, R)
         c, flat0 = self.c, self.flat0
-        spec = c.policy_spec(flat0) if self.linear else pilco.policy_spec(flat0)
-        self.gp = None if self.linear else spec["gp"]
+        spec = c.policy_spec(flat0) if self.linear or self.mlp else pilco.policy_spec(flat0)
+        self.gp = None if self.linear or self.mlp else spec["gp"]
         x0 = engine.dev(x0)
         if consistent:
             self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
@@ -262,7 +271,7 @@ class ParticleEvaluator(_FlatEvaluator):
         self.d_flat.copy_(self.h_flat, non_blocking=True)
         th = self._unpack(self.d_flat, self.plan, self.gp)
         g = self.plan.launch_grad()
-        info = self.gp.info if not self.linear else torch.zeros_like(g["value"])
+        info = self.gp.info if self.gp is not None else torch.zeros_like(g["value"])
         self._pack(self.d_out, g["value"].reshape(self.R), info.reshape(self.R), g, th)
         self.h_out.copy_(self.d_out, non_blocking=True)
 
