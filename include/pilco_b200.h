@@ -855,6 +855,65 @@ int    pilco_particles_mlp_resampled_grad_rollout(const pilco_particles* pr, con
                                                   const pilco_particles_resample* rs, int R,
                                                   const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* ---- function samples from random-feature draws (DESIGN.md section 30) -----------------------------------------
+ * The consistent sampler's process (one dynamics function per particle and output, x_{t+1} = x_t + f_p(x~_t)) with
+ * each function drawn once as a random-feature prior plus an exact data update (Wilson et al. 2020):
+ *   omega_ei = zeta_ei / ell_e,  phi_e(x) = sqrt(sf2_e / F) [cos(omega_e x); sin(omega_e x)]  (2F features)
+ *   v_pe = beta_e - iK_e (Phi_e(X) w_pe + sqrt(sn2_e) eps_pe),  f_pe(x~) = phi_e(x~)' w_pe + k_e(x~, X) v_pe
+ * Given the frequencies, the sample's covariance is the posterior's with the F-feature prior in place of k; its cost
+ * per particle, output and step is O(F + n), and no buffer grows with the horizon beyond the outputs and the
+ * gradient's x~ history.  dyn must be the exact GP pilco_gp_factorize leaves (iK = (K + sn2 I)^-1 and sn2 the noise
+ * variances it was factorised with): the C layer cannot tell a FITC model apart, and for one the update is wrong.
+ *
+ * pilco_particles_features_draw: omega [E,F,D] and v [P,E,n] from the caller's standard normals zeta [E,F,D] (shared
+ * by all particles), w [P,E,2F] and eps_y [P,E,n]; sn2 [E] on the device.  Once per set of normals, not per rollout.
+ * A particle's v is bitwise independent of P.  PILCO_ERR_NULL for a NULL pointer (dyn, its arrays, sn2, zeta, w,
+ * eps_y, omega, v), PILCO_ERR_UNSUPPORTED for a model that is not unbatched mode 0 with iK, PILCO_ERR_DIM for sizes
+ * out of range (P, F in 1 .. PILCO_MAX_FEATURES, n, D, E, ldk), then the workspace's codes.
+ *
+ * The rollouts take the draws in place of pr->eps (not read; it may be NULL) and otherwise are the consistent calls
+ * they mirror: pilco_particles_features_rollout as pilco_particles_noisy_consistent_rollout,
+ * _features_grad_rollout as pilco_particles_explore_consistent_grad_rollout (R restarts share the draws; restart r
+ * is bitwise the R = 1 call with policy r), and the _mlp_ calls as pilco_particles_mlp_consistent_rollout /
+ * _mlp_consistent_grad_rollout.  Same outputs, angles, noise and exploration rules (ang, nz, ex NULL: without them).
+ * Validation before any work is enqueued: the mirrored call's codes up to its workspace check (pr->eps excepted),
+ * then PILCO_ERR_NULL for fd, omega, w or v NULL, PILCO_ERR_DIM for F outside 1 .. PILCO_MAX_FEATURES, then the
+ * workspace's codes.  A size query returns 0 exactly where its call fails on sizes (fd NULL included).
+ * Deterministic, no host synchronisation (graph-capturable); a particle's outputs depend neither on P nor on its row. */
+#define PILCO_MAX_FEATURES 8192
+typedef struct pilco_feature_draws {
+    int F;                      /* 1 .. 8192 frequency pairs per output */
+    const double* omega;        /* [E,F,D] written by the draw call */
+    const double* w;            /* [P,E,2F] the caller's standard normals */
+    const double* v;            /* [P,E,n]  written by the draw call */
+} pilco_feature_draws;
+size_t pilco_particles_features_draw_workspace_bytes(const pilco_gp_model* dyn, int P, int F);
+int    pilco_particles_features_draw(const pilco_gp_model* dyn, const double* sn2, int P, int F, const double* zeta,
+                                     const double* w, const double* eps_y, double* omega, double* v,
+                                     void* ws, size_t ws_bytes, pilco_stream_t stream);
+size_t pilco_particles_features_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, const pilco_feature_draws* fd);
+int    pilco_particles_features_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                        const pilco_particles_noise* nz, const pilco_feature_draws* fd,
+                                        pilco_stream_t stream);
+size_t pilco_particles_features_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                     const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                     const pilco_feature_draws* fd, int R);
+int    pilco_particles_features_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                             const pilco_feature_draws* fd, int R, const pilco_particles_grad* g,
+                                             pilco_stream_t stream);
+size_t pilco_particles_mlp_features_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                    const pilco_feature_draws* fd);
+int    pilco_particles_mlp_features_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                            const pilco_feature_draws* fd, pilco_stream_t stream);
+size_t pilco_particles_mlp_features_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                         const pilco_exploration* ex, const pilco_feature_draws* fd,
+                                                         int R);
+int    pilco_particles_mlp_features_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                 const pilco_exploration* ex, const pilco_feature_draws* fd, int R,
+                                                 const pilco_particles_grad* g, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

@@ -105,6 +105,12 @@ class Mlp(C.Structure):
     _fields_ = [("L", C.c_int), ("width", C.c_int * 2), ("theta", c_dp), ("theta_bs", c_ll), ("gtheta", c_dp)]
 
 
+class FeatureDraws(C.Structure):
+    """mirror of ``pilco_feature_draws``"""
+    _fields_ = [("F", C.c_int), ("omega", c_dp), ("w", c_dp), ("v", c_dp)]
+
+
+MAX_FEATURES = 8192                              # PILCO_MAX_FEATURES
 POLICY_LINEAR, POLICY_RBF, POLICY_MLP = 0, 1, 2
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -295,6 +301,25 @@ SIGNATURES = {
     "pilco_particles_mlp_resampled_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
                                                              C.POINTER(ParticlesResample), C.c_int,
                                                              C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_features_draw_workspace_bytes": (C.c_size_t, [C.POINTER(GpModel), C.c_int, C.c_int]),
+    "pilco_particles_features_draw": (C.c_int, [C.POINTER(GpModel), c_dp, C.c_int, C.c_int] + [c_dp] * 6
+                                      + [C.c_size_t, c_dp]),
+    "pilco_particles_features_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(FeatureDraws)]),
+    "pilco_particles_features_rollout": (C.c_int, _PAN + [C.POINTER(FeatureDraws), c_dp]),
+    "pilco_particles_features_grad_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(Exploration),
+                                                                          C.POINTER(FeatureDraws), C.c_int]),
+    "pilco_particles_features_grad_rollout": (C.c_int, _PAN + [C.POINTER(Exploration), C.POINTER(FeatureDraws), C.c_int,
+                                                               C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_mlp_features_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                  C.POINTER(FeatureDraws)]),
+    "pilco_particles_mlp_features_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), C.POINTER(FeatureDraws),
+                                                       c_dp]),
+    "pilco_particles_mlp_features_grad_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                       C.POINTER(Exploration), C.POINTER(FeatureDraws),
+                                                                       C.c_int]),
+    "pilco_particles_mlp_features_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                            C.POINTER(Exploration), C.POINTER(FeatureDraws), C.c_int,
+                                                            C.POINTER(ParticlesGrad), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

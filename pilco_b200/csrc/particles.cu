@@ -43,6 +43,9 @@
 // Tanh MLP policies (pilco_particles_mlp_*, DESIGN.md section 29): pt_forward launches the step kernels of
 // particles_mlp.cu in place of pt_step / pr_step, pg_reverse its reverse step kernel in place of pg_step followed by one
 // batched gemm() per layer (factorize.cu) into per-chunk partials, and pm_finish_kernel in place of pg_reduce.
+// Function samples from random-feature draws (pilco_particles_features_* and _mlp_features_*, DESIGN.md section 30):
+// pt_forward launches pf_eval_kernel (particles_features.cu) in place of the predict, which leaves mean = f(x~_t) and
+// var = 0 for the unchanged step kernels, and pg_reverse pf_vjp_kernel in place of the predict VJP.
 #include <cmath>
 #include "particles.cuh"
 #include "gemm.cuh"
@@ -859,6 +862,8 @@ struct PtOpt {
     pilco_policy_schedule sch;
     bool mlp;                   // an MLP call (DESIGN.md section 29): the policy is net, pol.kind must be PILCO_POLICY_MLP
     PmNet net;
+    bool features;              // function samples from random-feature draws (DESIGN.md section 30): fd's, not eps
+    pilco_feature_draws fd;
 };
 
 // Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
@@ -878,6 +883,7 @@ struct PtWs {
                                                         // reverse scratch [R,Ds+Ds Ds]
     size_t min0, min1, min2, md1, md2, mdo, mpart;      // MLP, gradients: the layer inputs and cotangents [., R Pp];
                                                         // the chunk partials [R nc, n_theta]
+    size_t fz;                                          // features: the zero eps [P,H,Ds] the step kernels read
     size_t pws, pws_bytes, vws, vws_bytes, total;
 };
 
@@ -1026,6 +1032,33 @@ static PtWs fs_ws_layout(const pilco_particles* pr, const PtOpt& o) {
     return L;
 }
 
+// The feature sampler's workspace at T = R P rows (DESIGN.md section 30): pt_ws_layout's forward and pathwise slots
+// without the predict and VJP workspaces, then the zero eps [P,H,Ds] with which the unchanged step kernels close each
+// step (x + f + sqrt(0) 0 = x + f exactly).
+static PtWs pf_ws_layout(const pilco_particles* pr, const PtOpt& o) {
+    const bool grad = o.call != PT_FORWARD;
+    const size_t R = o.R, T = R * pr->P, H = pr->H, Hx = grad ? H : 1;
+    const size_t Ds = pr->dyn.E, Dh = pr->pol.Ds, U = pr->pol.U, D = pr->dyn.D, bf = pt_rbf(pr) ? pr->pol.rbf.n : 0;
+    PtWs L = {}; PtTake take;
+    L.xt = take({Hx, T, D}); L.mean = take({T, Ds}); L.var = take({Hx, T, Ds});
+    if (grad) {
+        L.gx = take({T, Ds}); L.gvar = take({T, Ds}); L.gxt = take({T, D}); L.zbar = take({T, H, o.mlp ? 0 : U});
+        L.s1 = take({R, U, bf, Dh}); L.s2r = take({R, U, bf, Dh});
+        L.gbeta = take({R, U, bf}); L.gy = take({R, U, bf});
+        if (o.mapped) L.phi = take({T, H + 1, Dh});
+        if (o.noisy) { L.phiz = take({T, H + 1, Dh}); L.phibz = take({T, Dh}); }
+        if (o.explore) { L.sd = take({R, H}); L.tab = take({R, H, (size_t)pr->n_rewards, 2}); }
+    }
+    L.fz = take({(size_t)pr->P, H, Ds});
+    if (grad && o.mlp) pm_ws_slots(L, take, pr, o);
+    L.total = take.bytes();
+    return L;
+}
+
+static PtWs pt_layout(const pilco_particles* pr, const PtOpt& o) {
+    return o.features ? pf_ws_layout(pr, o) : o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
+}
+
 static bool pt_sizes_ok(const pilco_particles* pr) {
     return pr->P >= 1 && pr->P <= PT_MAX_P && pr->H >= 0 && pr->dyn.n >= 1 && pr->dyn.D >= 1 && pr->dyn.D <= MAXD &&
            pr->pol.Ds >= 1 && pr->pol.U >= 1 && pr->pol.Ds <= MAXE;
@@ -1074,9 +1107,10 @@ static PmNet pm_net(const pilco_particles* pr, const pilco_mlp* m) {
 // everything but the workspace (the gradients bring their own).  batched: the policy's batch strides are honoured
 // (the batch_grad and consistent_grad entry points); otherwise a batched policy is unsupported.  A: the number of
 // angular state dimensions (the policy takes dyn.E + A inputs).  mlp_call: the MLP entry points, whose policy checks
-// are the MLP's (pol.kind PILCO_POLICY_MLP, mlp and theta not NULL, its sizes, theta_bs as a batch stride).
+// are the MLP's (pol.kind PILCO_POLICY_MLP, mlp and theta not NULL, its sizes, theta_bs as a batch stride).  need_eps
+// = false (the feature sampler): pr->eps is not read and may be NULL.
 static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A = 0, bool mlp_call = false,
-                         const pilco_mlp* mlp = nullptr) {
+                         const pilco_mlp* mlp = nullptr, bool need_eps = true) {
     if (!pr) return PILCO_ERR_NULL;
     if (pr->P < 1 || pr->P > PT_MAX_P || pr->H < 0) return PILCO_ERR_DIM;
     const pilco_gp_model& g = pr->dyn;
@@ -1110,7 +1144,7 @@ static int pt_check_desc(const pilco_particles* pr, bool batched = false, int A 
     } else return PILCO_ERR_UNSUPPORTED;
     if (pol.squash && !pol.max_action) return PILCO_ERR_NULL;
     if (const int rc = pt_check_rewards(pr, false)) return rc;
-    if (!pr->x0 || !pr->eps || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret)
+    if (!pr->x0 || (need_eps && !pr->eps) || !pr->traj || !pr->act || !pr->step_reward || !pr->step_risk || !pr->ret)
         return PILCO_ERR_NULL;
     if (((uintptr_t)g.iK & 15) || (g.ldk & 1)) return PILCO_ERR_ALIGN;                  // predict's TMA rows
     return PILCO_OK;
@@ -1181,18 +1215,21 @@ int fs_vjp_launch(cudaStream_t st, const pilco_gp_model* gp, int T, const double
 // pn_step_kernel in place of pa_step_kernel, which with history also keeps phi(z_t) in L.phiz.  The state width is
 // dyn.E throughout (pol.Ds without angles).  sch (an active schedule, DESIGN.md section 28): every step kernel reads
 // the linear policy through a.W and a.b, which step t's launch advances by t W_ts and t b_ts.  net (an MLP, DESIGN.md
-// section 29; no angles, noise or schedule): pm_step_kernel / pm_refit_kernel in place of pt_step / pr_step.
+// section 29; no angles, noise or schedule): pm_step_kernel / pm_refit_kernel in place of pt_step / pr_step.  pf
+// (feature draws, DESIGN.md section 30; not consistent, no refit or schedule): pf_eval_kernel in place of the predict,
+// and the step kernels read the zero eps in L.fz.
 static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& L, bool consistent, bool history,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr,
                       const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
-                      const PmNet* net = nullptr) {
+                      const PmNet* net = nullptr, const PfDev* pf = nullptr) {
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P, np = pad64(pr->dyn.n);
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds, slot = TDs * np;
     const size_t xstep = consistent || history ? TD : 0, vstep = history ? TDs : 0;
     const dim3 grid((P + PT_THREADS - 1) / PT_THREADS, R), cgrid((P + FS_WARPS - 1) / FS_WARPS, Ds, R);
     PtDev a;
     static_cast<PtPolicy&>(a) = pt_policy(pr);
-    a.x0 = pr->x0; a.eps = pr->eps;
+    a.x0 = pr->x0; a.eps = pf ? ws + L.fz : pr->eps;
+    if (pf && H > 0) cudaMemsetAsync(ws + L.fz, 0, (size_t)P * H * Ds * sizeof(double), st);
     a.traj = pr->traj; a.act = pr->act; a.step_reward = pr->step_reward; a.step_risk = pr->step_risk; a.ret = pr->ret;
     a.mean = ws + L.mean;
     PaStep pa;
@@ -1249,6 +1286,10 @@ static int pt_forward(const pilco_particles* pr, int R, double* ws, const PtWs& 
             c.t = t; c.var = var;
             launch_hi(fs_cond_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, c);
             CUDA_LAUNCH_CHECK();
+        } else if (pf) {
+            PfDev q = *pf;
+            q.xh = a.xt; q.mean = ws + L.mean; q.var = var;
+            if (const int rc = pf_eval_launch(st, q)) return rc;
         } else {
             const int rc = pilco_gp_predict(&pr->dyn, 0, Ds, T, a.xt, ws + L.mean, var, 0, ws + L.pws, L.pws_bytes, st);
             if (rc) return rc;
@@ -1311,10 +1352,12 @@ static int pg_reduce(const pilco_particles* pr, int R, const pilco_particles_gra
 // net (an MLP): pm_reverse_kernel in place of pg_step, then (where x~_bar_t exists) one gemm per layer adds step t's
 // d_l' [a_{l-1}; 1] to each chunk's partial, steps in order t = H-1 .. 0; pm_finish_kernel sums the chunks over P into
 // gtheta and writes value.
+// pf (feature draws): pf_vjp_kernel is the step's VJP (var = 0, so var_bar has no share), and the step kernels read
+// the forward's zero eps.
 static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_grad* g, const PtWs& L, bool consistent,
                       cudaStream_t st, const TrigMap* tm = nullptr, const PnNoise* nz = nullptr, bool bonus = false,
                       const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
-                      const PmNet* net = nullptr, double* gtheta = nullptr) {
+                      const PmNet* net = nullptr, double* gtheta = nullptr, const PfDev* pf = nullptr) {
     double* ws = (double*)g->ws;
     const int P = pr->P, H = pr->H, Ds = pr->dyn.E, D = pr->dyn.D, T = R * P;
     const size_t TD = (size_t)T * D, TDs = (size_t)T * Ds;
@@ -1322,7 +1365,7 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
     if (consistent && H > 1) cudaMemsetAsync(ws + L.G, 0, (size_t)H * (H + 1) / 2 * TDs * sizeof(double), st);
     PgDev b;
     static_cast<PtPolicy&>(b) = pt_policy(pr);
-    b.eps = pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
+    b.eps = pf ? ws + L.fz : pr->eps; b.traj = pr->traj; b.step_risk = pr->step_risk;
     b.gx = ws + L.gx; b.gvar = ws + L.gvar; b.zbar = ws + L.zbar;
     FsBwd q;                                            // the cotangent rows G accumulate from zero
     q.P = P; q.T = T; q.H = H; q.D = D; q.Ds = Ds; q.np = pad64(pr->dyn.n); q.t = 0;
@@ -1363,6 +1406,10 @@ static int pg_reverse(const pilco_particles* pr, int R, const pilco_particles_gr
                 launch_hi(fs_cond_bwd_kernel, cgrid, dim3(FS_WARPS * 32), 0, st, q);
                 CUDA_LAUNCH_CHECK();
                 rc = fs_vjp_launch(st, &pr->dyn, T, xt, b.gx, q.A, q.dir, ws + L.gxt, ws + L.vws);
+            } else if (pf) {
+                PfDev v = *pf;
+                v.xh = xt; v.gmean = b.gx; v.gxt = ws + L.gxt;
+                rc = pf_vjp_launch(st, v);
             } else {
                 rc = pilco_gp_predict_vjp(&pr->dyn, T, xt, b.gx, b.gvar, ws + L.gxt, ws + L.vws, L.vws_bytes, st);
             }
@@ -1580,15 +1627,19 @@ static bool pt_sched_active(const pilco_policy_schedule* sch) { return sch && (s
 // PILCO_ERR_UNSUPPORTED for an active schedule with an RBF policy.  sch NULL or both strides 0 is the call without it.
 // MLP calls (o->mlp, DESIGN.md section 29; no angles, noise or schedule): the description's policy checks are the
 // MLP's (pt_check_desc), and the gradient's outputs are value, ws and mlp->gtheta.
+// Feature calls (o->features, DESIGN.md section 30; no refit, schedule or score estimator): pr->eps is not checked,
+// and after everything else PILCO_ERR_NULL for fd, omega, w or v NULL, then PILCO_ERR_DIM for F out of range.
+static bool pf_F_ok(int F) { return F >= 1 && F <= PILCO_MAX_FEATURES; }
+
 static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                        const pilco_exploration* ex, int R, const pilco_particles_grad* g,
                        const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
-                       const pilco_mlp* mlp = nullptr) {
+                       const pilco_mlp* mlp = nullptr, const pilco_feature_draws* fd = nullptr) {
     if (!pr) return PILCO_ERR_NULL;
     const bool angles = !pa_none(ang);
     if (angles)
         if (const int rc = pa_map(pr, ang, &o->tm)) return rc;
-    if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0, o->mlp, mlp)) return rc;
+    if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0, o->mlp, mlp, !o->features)) return rc;
     if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;   // the unbatched calls' R = 1 passes with the description
     if (o->call != PT_FORWARD)
         if (const int rc = pg_check(pr, g, o->mlp ? mlp : nullptr)) return rc;
@@ -1613,17 +1664,24 @@ static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* 
         if (pt_rbf(pr)) return PILCO_ERR_UNSUPPORTED;
         o->sch = *sch;
     }
+    if (o->features) {
+        if (!fd || !fd->omega || !fd->w || !fd->v) return PILCO_ERR_NULL;
+        if (!pf_F_ok(fd->F)) return PILCO_ERR_DIM;
+        o->fd = *fd;
+    }
     return PILCO_OK;
 }
 
 // A call's workspace: its layout's total, 0 where the call would fail on its sizes.  The sizes accepted are the
 // description's own (pt_sizes_ok, not its width consistency), R, the angles' map, 1 <= E <= PILCO_MAX_E and valid
 // variances with noise, and the exploration's checks when active; a schedule only adds non-negative strides (its
-// workspace is the call's without it); an MLP call adds mlp != NULL and its sizes (L, the widths).
+// workspace is the call's without it); an MLP call adds mlp != NULL and its sizes (L, the widths); a feature call fd !=
+// NULL and F in range.
 static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                        const pilco_exploration* ex, int R, const pilco_policy_schedule* sch = nullptr,
-                       const pilco_mlp* mlp = nullptr) {
+                       const pilco_mlp* mlp = nullptr, const pilco_feature_draws* fd = nullptr) {
     if (!pr || !pt_sizes_ok(pr) || !pt_batch_ok(pr->P, R)) return 0;
+    if (o.features && (!fd || !pf_F_ok(fd->F))) return 0;
     if (o.mlp) {                                        // the MLP's sizes (NULL: none to size the workspace with)
         if (!mlp || !pm_sizes_ok(mlp)) return 0;
         o.net = pm_net(pr, mlp);
@@ -1635,7 +1693,7 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
     if (o.explore && px_check(pr, ex)) return 0;
     if (o.resampled && pr->P < 2) return 0;
     o.R = R; o.mapped = nz || !pa_none(ang); o.noisy = nz != nullptr;
-    return (o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o)).total;
+    return pt_layout(pr, o).total;
 }
 
 // Every rollout call: validate, lay out, check the workspace (pr's for the forward, g's for a gradient), prepare, then
@@ -1644,10 +1702,10 @@ static size_t pt_query(PtOpt o, const pilco_particles* pr, const pilco_angles* a
 static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
                    const pilco_exploration* ex, int R, const pilco_particles_grad* g, pilco_stream_t stream,
                    const pilco_particles_resample* rs = nullptr, const pilco_policy_schedule* sch = nullptr,
-                   const pilco_mlp* mlp = nullptr) {
-    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs, sch, mlp)) return rc;
+                   const pilco_mlp* mlp = nullptr, const pilco_feature_draws* fd = nullptr) {
+    if (const int rc = pt_validate(&o, pr, ang, nz, ex, R, g, rs, sch, mlp, fd)) return rc;
     const bool fwd = o.call == PT_FORWARD;
-    const PtWs L = o.consistent ? fs_ws_layout(pr, o) : pt_ws_layout(pr, o);
+    const PtWs L = pt_layout(pr, o);
     if (const int rc = fwd ? pt_check_ws(pr->ws, pr->ws_bytes, L.total) : pt_check_ws(g->ws, g->ws_bytes, L.total))
         return rc;
     if (o.consistent) {
@@ -1662,7 +1720,13 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
     const pilco_particles_resample* rsv = o.resampled ? &o.rs : nullptr;
     const pilco_policy_schedule* sv = o.sched ? &o.sch : nullptr;
     const PmNet* net = o.mlp ? &o.net : nullptr;
-    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv, net)) return rc;
+    PfDev q = {};
+    if (o.features) {
+        q.T = (long long)R * pr->P; q.P = pr->P; q.D = pr->dyn.D; q.E = pr->dyn.E; q.F = o.fd.F; q.n = pr->dyn.n;
+        q.omega = o.fd.omega; q.X = pr->dyn.X; q.ell = pr->dyn.ell; q.sf2 = pr->dyn.sf2; q.w = o.fd.w; q.v = o.fd.v;
+    }
+    const PfDev* pf = o.features ? &q : nullptr;
+    if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv, net, pf)) return rc;
     if (fwd) return PILCO_OK;
     if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
     if (o.explore) {
@@ -1670,7 +1734,8 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
         m.step_var = o.step_var; m.sd = ws + L.sd; m.tab = o.bonus ? ws + L.tab : nullptr;
         if (const int rc = px_moments_launch(st, R, m)) return rc;
     }
-    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv, sv, net, o.mlp ? mlp->gtheta : nullptr))
+    if (const int rc = pg_reverse(pr, R, g, L, o.consistent, st, tm, n, o.bonus, rsv, sv, net,
+                                  o.mlp ? mlp->gtheta : nullptr, pf))
         return rc;
     if (o.bonus && pr->H > 0) return px_value_launch(st, R, pr->H, o.b, ws + L.sd, g->value);
     return PILCO_OK;
@@ -1684,6 +1749,9 @@ static const PtOpt RFWD = {false, PT_FORWARD, false, true}, RPATH = {false, PT_P
 
 // the MLP calls (DESIGN.md section 29): a family's options with o.mlp
 static PtOpt pm_opt(PtOpt o) { o.mlp = true; return o; }
+
+// the feature calls (DESIGN.md section 30): the step-wise forward and pathwise options with o.features
+static PtOpt pf_opt(PtOpt o) { o.features = true; return o; }
 
 extern "C" {
 
@@ -2055,6 +2123,53 @@ int pilco_particles_mlp_resampled_grad_rollout(const pilco_particles* pr, const 
                                                const pilco_particles_resample* rs, int R,
                                                const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(pm_opt(RPATH), pr, nullptr, nullptr, nullptr, R, g, stream, rs, nullptr, mlp);
+}
+
+// function samples from random-feature draws (DESIGN.md section 30); the draw call is in particles_features.cu
+size_t pilco_particles_features_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, const pilco_feature_draws* fd) {
+    return pt_query(pf_opt(FWD), pr, ang, nz, nullptr, 1, nullptr, nullptr, fd);
+}
+
+int pilco_particles_features_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                     const pilco_particles_noise* nz, const pilco_feature_draws* fd,
+                                     pilco_stream_t stream) {
+    return pt_call(pf_opt(FWD), pr, ang, nz, nullptr, 1, nullptr, stream, nullptr, nullptr, nullptr, fd);
+}
+
+size_t pilco_particles_features_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                     const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                                     const pilco_feature_draws* fd, int R) {
+    return pt_query(pf_opt(PATH), pr, ang, nz, ex, R, nullptr, nullptr, fd);
+}
+
+int pilco_particles_features_grad_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                          const pilco_particles_noise* nz, const pilco_exploration* ex,
+                                          const pilco_feature_draws* fd, int R, const pilco_particles_grad* g,
+                                          pilco_stream_t stream) {
+    return pt_call(pf_opt(PATH), pr, ang, nz, ex, R, g, stream, nullptr, nullptr, nullptr, fd);
+}
+
+size_t pilco_particles_mlp_features_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                    const pilco_feature_draws* fd) {
+    return pt_query(pf_opt(pm_opt(FWD)), pr, nullptr, nullptr, nullptr, 1, nullptr, mlp, fd);
+}
+
+int pilco_particles_mlp_features_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                         const pilco_feature_draws* fd, pilco_stream_t stream) {
+    return pt_call(pf_opt(pm_opt(FWD)), pr, nullptr, nullptr, nullptr, 1, nullptr, stream, nullptr, nullptr, mlp, fd);
+}
+
+size_t pilco_particles_mlp_features_grad_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp,
+                                                         const pilco_exploration* ex, const pilco_feature_draws* fd,
+                                                         int R) {
+    return pt_query(pf_opt(pm_opt(PATH)), pr, nullptr, nullptr, ex, R, nullptr, mlp, fd);
+}
+
+int pilco_particles_mlp_features_grad_rollout(const pilco_particles* pr, const pilco_mlp* mlp,
+                                              const pilco_exploration* ex, const pilco_feature_draws* fd, int R,
+                                              const pilco_particles_grad* g, pilco_stream_t stream) {
+    return pt_call(pf_opt(pm_opt(PATH)), pr, nullptr, nullptr, ex, R, g, stream, nullptr, nullptr, mlp, fd);
 }
 
 int pilco_particles_reward_moments(const pilco_particles* pr, const pilco_angles* ang, int R, double* step_mean,

@@ -1,8 +1,8 @@
 // particles.cuh -- what the particle kernels of particles.cu, particles_angles.cu, particles_noise.cu,
-// particles_explore.cu, particles_cscore.cu, particles_resample.cu and particles_mlp.cu share: the per-particle argument
-// structs, the reward value at a point, the step's work at a given state, the fixed-order block sum, and the angle,
-// noise, exploration, consistent-score, resampling and MLP-policy kernels' launchers (DESIGN.md sections 11, 12, 20, 23,
-// 24, 25, 26 and 29).
+// particles_explore.cu, particles_cscore.cu, particles_resample.cu, particles_mlp.cu and particles_features.cu share: the
+// per-particle argument structs, the reward value at a point, the step's work at a given state, the fixed-order block
+// sum, and the angle, noise, exploration, consistent-score, resampling, MLP-policy and feature-sample kernels' launchers
+// (DESIGN.md sections 11, 12, 20, 23, 24, 25, 26, 29 and 30).
 #pragma once
 #include <initializer_list>
 #include "common.cuh"
@@ -315,3 +315,23 @@ int pm_reverse_launch(cudaStream_t st, dim3 grid, const PgDev& a, const PmBwd& b
 // gtheta [R, n_theta] = (1/P) sum of the chunk partials part [R, nc, n_theta] in chunk order; value [R] = the mean return
 int pm_finish_launch(cudaStream_t st, int R, int P, int nc, int n_theta, const double* part, const double* ret,
                      double* gtheta, double* value);
+
+// ---- function samples from random-feature draws (particles_features.cu, DESIGN.md section 30) -------------------------
+// f_pe(x~) = phi_e(x~)' w_pe + sum_j sf2_e exp(-0.5 |(x~ - X_j) / ell_e|^2) v_pe,j at the T = R P rows of x~ (row r P + p
+// reads particle p's draws: the restarts share them)
+struct PfDev {
+    long long T;
+    int P, D, E, F, n;
+    const double* omega;                                // [E,F,D]
+    const double* X; const double* ell; const double* sf2;   // the dynamics GP's [n,D], [E,D], [E]
+    const double* w; const double* v;                   // [P,E,2F], [P,E,n]
+    const double* xh;                                   // x~_t [T,D]
+    double* mean; double* var;                          // [T,E] eval: f and 0
+    const double* gmean;                                // [T,E] VJP: m_bar
+    double* gxt;                                        // [T,D] VJP: x~_bar
+};
+
+// grid (ceil(T / 8), E): mean = f(x~_t), var = 0
+int pf_eval_launch(cudaStream_t st, const PfDev& a);
+// grid ceil(T / 8): gxt = sum_e gmean_e d f_e / d x~ at x~_t
+int pf_vjp_launch(cudaStream_t st, const PfDev& a);

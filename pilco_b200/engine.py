@@ -792,6 +792,13 @@ PARTICLE_CALLS = {
     ("resampled", "pathwise"): ("resampled_grad_rollout", "resampled_grad_workspace_bytes"),
 }
 
+# the feature sampler's rows (DESIGN.md section 30): the forward and pathwise call with a pilco_feature_draws after
+# the angles, noise and (pathwise) exploration
+PARTICLE_FEATURE_CALLS = {
+    ("features", "forward"): ("features_rollout", "features_workspace_bytes"),
+    ("features", "pathwise"): ("features_grad_rollout", "features_grad_workspace_bytes"),
+}
+
 # the same rows with a time-varying linear policy (DESIGN.md section 28): each call above with a pilco_policy_schedule
 # after its feature arguments
 PARTICLE_SCHEDULED_CALLS = {
@@ -814,7 +821,63 @@ PARTICLE_MLP_CALLS = {
     (True, "pathwise"): ("mlp_consistent_grad_rollout", "mlp_consistent_grad_workspace_bytes"),
     ("resampled", "forward"): ("mlp_resampled_rollout", "mlp_resampled_workspace_bytes"),
     ("resampled", "pathwise"): ("mlp_resampled_grad_rollout", "mlp_resampled_grad_workspace_bytes"),
+    ("features", "forward"): ("mlp_features_rollout", "mlp_features_workspace_bytes"),
+    ("features", "pathwise"): ("mlp_features_grad_rollout", "mlp_features_grad_workspace_bytes"),
 }
+
+
+class FeatureDraws:
+    """What ``feature_draws`` returns: the device tensors of P particles' function draws (DESIGN.md section 30),
+    omega [E,F,D], w [P,E,2F] and v [P,E,n].  A plan draws once and rolls out many times on them."""
+
+    def __init__(self, F, omega, w, v):
+        self.F, self.omega, self.w, self.v = int(F), omega, w, v
+        self.P, self.E, self.n = int(w.shape[0]), int(w.shape[1]), int(v.shape[2])
+        self.D = int(omega.shape[2]) if len(np.shape(omega)) == 3 else -1
+        if tuple(np.shape(omega)) != (self.E, self.F, self.D) or tuple(np.shape(w)) != (self.P, self.E, 2 * self.F) \
+                or tuple(np.shape(v)) != (self.P, self.E, self.n):
+            raise ValueError("FeatureDraws: expected omega [E,F,D], w [P,E,2F] and v [P,E,n], got %s, %s and %s"
+                             % (tuple(np.shape(omega)), tuple(np.shape(w)), tuple(np.shape(v))))
+
+    def struct(self, p0=0):
+        """the pilco_feature_draws of the particles from p0 on (the draws of one particle are contiguous)"""
+        return _lib.FeatureDraws(self.F, self.omega.data_ptr(), self.w[p0:].data_ptr(), self.v[p0:].data_ptr())
+
+
+def _features_check(dyn, num_features):
+    """the feature sampler's refusals on the model and F (ValueError), before any allocation"""
+    F = int(num_features)
+    if getattr(dyn, "sn2", None) is None or dyn.mode != 0 or dyn.iK is None or dyn.batched:
+        raise ValueError("features: the function draws need the exact GP gp_factorize returns (with its sn2); a FITC "
+                         "(SMGPR) model is not supported")
+    if F < 1 or F > _lib.MAX_FEATURES:
+        raise ValueError("features: num_features must be in 1 .. %d, got %d" % (_lib.MAX_FEATURES, F))
+    return F
+
+
+def feature_draws(dyn, P, F, zeta, w, eps_y):
+    """pilco_particles_features_draw: P particles' dynamics functions f_pe = phi_e' w_pe + k_e(., X) v_pe drawn from
+    the caller's standard normals zeta [E,F,D] (the frequencies, shared by all particles), w [P,E,2F] (the feature
+    weights) and eps_y [P,E,n] (the data update's noise), through the exact GP ``dyn`` (``gp_factorize``'s, with its
+    sn2) -> ``FeatureDraws``.  ValueError, before any allocation, for a model without sn2 (FITC), F outside
+    1 .. 8192 or a wrong shape."""
+    F = _features_check(dyn, F)
+    P, E, n, D = int(P), dyn.E, dyn.n, dyn.D
+    for a, shape, what in ((zeta, (E, F, D), "zeta"), (w, (P, E, 2 * F), "w"), (eps_y, (P, E, n), "eps_y")):
+        if tuple(np.shape(a)) != shape:
+            raise ValueError("feature_draws: %s must be %s, got %s" % (what, shape, tuple(np.shape(a))))
+    g = dyn.struct()
+    wsb = int(lib.pilco_particles_features_draw_workspace_bytes(C.byref(g), P, F))
+    if wsb == 0:
+        raise ValueError("feature_draws: unsupported sizes (P=%d, F=%d, n=%d, D=%d, E=%d)" % (P, F, n, D, E))
+    zeta, w, eps_y = dev(zeta).contiguous(), dev(w).contiguous(), dev(eps_y).contiguous()
+    d = device()
+    omega = torch.empty((E, F, D), dtype=F64, device=d)
+    v = torch.empty((P, E, n), dtype=F64, device=d)
+    ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+    check(lib.pilco_particles_features_draw(C.byref(g), ptr(dyn.sn2), P, F, ptr(zeta), ptr(w), ptr(eps_y), ptr(omega),
+                                            ptr(v), ptr(ws), wsb, stream_ptr()), "particles_features_draw")
+    return FeatureDraws(F, omega, w, v)
 
 
 class ParticlePlan:
@@ -875,15 +938,22 @@ class ParticlePlan:
     (A_2,) A_out, each row-major [out, in + 1] with the bias last).  Every sampler, forward and pathwise, with
     exploration; ``launch_grad()`` returns {'value', 'theta' [R?, n_theta]}.  With ``angles``, ``measurement_noise``,
     ``schedule=True`` or ``estimator="score"``, or a theta of the wrong length, it is a ValueError raised before any
-    allocation."""
+    allocation.
+
+    ``num_features=F`` with ``consistent=True``: each particle's functions are random-feature draws with an exact
+    data update (pilco_particles_features_*, DESIGN.md section 30), which ``set_inputs(x0, None, features=draws)``
+    takes from ``feature_draws`` in place of eps; the workspace does not grow with n or F.  Its gradient is
+    ``ConsistentGradPlan(num_features=F)``.  Without ``consistent=True``, with ``estimator="score"``, ``resample``
+    or ``schedule``, or with a model without sn2 (FITC), it is a ValueError raised before any allocation."""
 
     ESTIMATORS = ("pathwise", "score")
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, grad=False, R=1, consistent=False,
                  estimator="pathwise", angles=None, measurement_noise=None, exploration=None, resample=False,
-                 schedule=False):
+                 schedule=False, num_features=None):
         mlp = _particle_mlp(policy_spec, "ParticlePlan", R, angles, measurement_noise, schedule, estimator)
         sched = _particle_schedule(policy_spec, H, schedule, "ParticlePlan")
+        self.fd = _features_plan_check(dyn, num_features, consistent, estimator, resample, schedule)
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         self.resample = bool(resample)
@@ -915,26 +985,27 @@ class ParticlePlan:
             self._grad_buffers(self._grad_ws_bytes(P))
 
     def _sampler(self):
-        return "resampled" if self.resample else self.consistent
+        return "resampled" if self.resample else "features" if self.fd is not None else self.consistent
 
     def _args(self, kind, pr):
         """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise), the schedule
         (scheduled calls) and R; resampled: pr, the refit's buffers, the schedule and R"""
         sch = [C.byref(self.sch)] if self.sch is not None else []
+        fd = [C.byref(self.fd)] if self.fd is not None else []
         if self.mlp is not None:
             feat = [C.byref(self.rs)] if self.resample else \
                 [] if kind == "forward" else [C.byref(self.ex) if self.ex is not None else None]
-            return [C.byref(pr), C.byref(self.mlp)] + feat + ([self.R] if kind != "forward" else [])
+            return [C.byref(pr), C.byref(self.mlp)] + feat + fd + ([self.R] if kind != "forward" else [])
         if self.resample:
             return [C.byref(pr), C.byref(self.rs)] + sch + ([self.R] if kind != "forward" else [])
         args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
         if kind == "pathwise":
             args.append(C.byref(self.ex) if self.ex is not None else None)
-        return args + sch + ([self.R] if kind != "forward" else [])
+        return args + sch + fd + ([self.R] if kind != "forward" else [])
 
     def _names(self, kind):
         """(rollout, size query) of kind's call, each after the prefix pilco_particles_"""
-        table = PARTICLE_MLP_CALLS if self.mlp is not None else \
+        table = PARTICLE_MLP_CALLS if self.mlp is not None else PARTICLE_FEATURE_CALLS if self.fd is not None else \
             PARTICLE_CALLS if self.sch is None else PARTICLE_SCHEDULED_CALLS
         return table[self._sampler(), kind]
 
@@ -1072,16 +1143,29 @@ class ParticlePlan:
         name = "particles_" + self._names(kind)[0]
         check(getattr(lib, "pilco_" + name)(*self._args(kind, self.pr), *grad, stream_ptr()), name)
 
-    def set_inputs(self, x0, eps, nu=None, xi=None):
+    def set_inputs(self, x0, eps, nu=None, xi=None, features=None):
         """x0 [P,Ds], eps [P,H,Ds], with measurement noise nu [P,H,E] and with ``resample`` xi [P,H,Ds] (each required
-        then, and only then)"""
+        then, and only then).  With ``num_features``: ``features`` (``feature_draws`` of P particles at that F) in
+        place of eps, which is then not read (None)."""
+        if (features is None) != (self.fd is None):
+            raise ValueError("particles: features (feature_draws) are required with num_features and only then")
+        if features is not None:
+            dyn = self.pr.dyn
+            have, want = (features.P, features.F, features.E, features.n, features.D), \
+                (self.P, self.fd.F, dyn.E, dyn.n, dyn.D)
+            if have != want:
+                raise ValueError("particles: the feature draws are for (P, F, E, n, D) = %s; the plan has %s"
+                                 % (have, want))
+            self.features = features                            # keeps the draws alive
+            self.fd = features.struct()
         if (nu is None) != (self.nz is None):
             raise ValueError("particles: nu [P,H,E] is required with measurement_noise and only then")
         if (xi is None) == self.resample:
             raise ValueError("particles: xi [P,H,Ds] is required with resample=True and only then")
         self.x0.copy_(dev(x0).reshape(self.P, self.Ds))
         if self.H > 0:
-            self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
+            if features is None:
+                self.eps_buf.copy_(dev(eps).reshape(self.P, self.H, self.Ds))
             if nu is not None:
                 self.nu_buf.copy_(dev(nu).reshape(self.nu_buf.shape))
             if xi is not None:
@@ -1119,12 +1203,17 @@ class ConsistentGradPlan(ParticlePlan):
     rollout, value and output layout; its estimate is unbiased on rollouts without degenerate pivots.  ``"score"`` with
     ``exploration``, or an unknown estimator, is a ValueError raised before any allocation.
 
-    ``schedule=True``: a time-varying linear policy, as ``ParticlePlan``.  A tanh MLP policy: as ``ParticlePlan``."""
+    ``schedule=True``: a time-varying linear policy, as ``ParticlePlan``.  A tanh MLP policy: as ``ParticlePlan``.
+
+    ``num_features=F``: the functions are random-feature draws with an exact data update (DESIGN.md section 30), taken
+    by ``set_inputs(x0, None, nu=None, features=draws)``; the workspace is O(R P H (D + E)), whatever n and F.  With
+    ``estimator="score"`` or ``schedule`` it is a ValueError raised before any allocation."""
 
     def __init__(self, dyn, policy_spec, reward_terms, P, H, mult_mu=0.0, R=1, max_ws_bytes=None, angles=None,
-                 measurement_noise=None, exploration=None, estimator="pathwise", schedule=False):
+                 measurement_noise=None, exploration=None, estimator="pathwise", schedule=False, num_features=None):
         mlp = _particle_mlp(policy_spec, "ConsistentGradPlan", R, angles, measurement_noise, schedule, estimator)
         sched = _particle_schedule(policy_spec, H, schedule, "ConsistentGradPlan")
+        self.fd = _features_plan_check(dyn, num_features, True, estimator, False, schedule)
         if estimator not in self.ESTIMATORS:
             raise ValueError("particles: estimator must be one of %s, not %r" % (self.ESTIMATORS, estimator))
         if exploration is not None and estimator == "score":
@@ -1155,6 +1244,19 @@ class ConsistentGradPlan(ParticlePlan):
         returned as ``ParticlePlan.launch_grad`` returns it.  ``estimator="score"``: the score-function gradient
         (pilco_particles_consistent_score_grad_rollout) in the same layout"""
         return super().launch_grad()
+
+
+def _features_plan_check(dyn, num_features, consistent, estimator, resample, schedule):
+    """a plan's feature sampler (ValueError before any allocation): None without num_features, else the
+    pilco_feature_draws its size queries take (F set; set_inputs points it at the draws)"""
+    if num_features is None:
+        return None
+    for on, what in ((not consistent, "consistent=False (the draws are whole functions: consistent=True)"),
+                     (estimator == "score", "estimator='score' (a function sample has no per-step path density)"),
+                     (resample, "resample=True"), (schedule, "schedule=True")):
+        if on:
+            raise ValueError("particles: num_features does not combine with %s" % what)
+    return _lib.FeatureDraws(_features_check(dyn, num_features), None, None, None)
 
 
 def _largest_fitting(fits, lo, hi):
@@ -1265,7 +1367,8 @@ def particle_reward_moments(reward_terms, traj, act, angles=None):
 
 
 def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, consistent=False, max_ws_bytes=None,
-                      angles=None, measurement_noise=None, nu=None, resample=False, xi=None, schedule=False):
+                      angles=None, measurement_noise=None, nu=None, resample=False, xi=None, schedule=False,
+                      features=None, horizon=None):
     """pilco_particles_rollout: P particles from x0 [P,Ds] driven by the standard normals eps [P,H,Ds] through the
     factorised dynamics ``dyn`` under the (unbatched) policy -> (traj [P,H+1,Ds], act [P,H,U], step_reward [P,H],
     step_risk [P,H], ret [P]) device tensors.
@@ -1286,7 +1389,15 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
 
     ``schedule=True``: a time-varying linear policy (W [Hw,U,Ds], b [Hw,U], Hw >= H), as ``ParticlePlan``.
 
-    A tanh MLP spec (theta [n_theta]) runs every sampler, as ``ParticlePlan``."""
+    A tanh MLP spec (theta [n_theta]) runs every sampler, as ``ParticlePlan``.
+
+    ``features`` (``feature_draws`` of the P particles) with ``consistent=True``: the functions are those random-feature
+    draws with an exact data update (DESIGN.md section 30) and eps is not read: pass None and the horizon as
+    ``horizon``.  The particles run in chunks under ``max_ws_bytes`` as with the exact consistent sampler.  Without
+    ``consistent=True``, or with ``resample`` or ``schedule``, it is a ValueError."""
+    if features is not None:
+        return _particles_rollout_features(dyn, policy_spec, reward_terms, x0, mult_mu, consistent, max_ws_bytes,
+                                           angles, measurement_noise, nu, resample, schedule, features, horizon)
     _particle_mlp(policy_spec, "particles_rollout", 1, angles, measurement_noise, schedule)
     _particle_schedule(policy_spec, eps.shape[1] if len(np.shape(eps)) == 3 else 0, schedule, "particles_rollout")
     if resample:
@@ -1317,21 +1428,46 @@ def particles_rollout(dyn, policy_spec, reward_terms, x0, eps, mult_mu=0.0, cons
     return plan.outputs() + ((plan.step_mean, plan.step_cov) if resample else ())
 
 
-def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None):
+def _particles_rollout_features(dyn, policy_spec, reward_terms, x0, mult_mu, consistent, max_ws_bytes, angles,
+                                measurement_noise, nu, resample, schedule, features, horizon):
+    """particles_rollout with feature draws: every check on the host shapes first, then the chunked consistent path
+    with no eps"""
+    _features_plan_check(dyn, features.F, consistent, "pathwise", resample, schedule)
+    _particle_mlp(policy_spec, "particles_rollout", 1, angles, measurement_noise, schedule)
+    if horizon is None or int(horizon) < 0:
+        raise ValueError("particles_rollout: with features the horizon (>= 0) is required, got %r" % (horizon,))
+    H = int(horizon)
+    if len(np.shape(x0)) != 2 or np.shape(x0)[0] != features.P:
+        raise ValueError("particles_rollout: x0 must be [P,Ds] with P=%d (the draws'), got %s"
+                         % (features.P, tuple(np.shape(x0))))
+    if (nu is None) != (measurement_noise is None):
+        raise ValueError("particles_rollout: nu [P,H,E] is required with measurement_noise and only then")
+    if nu is not None and tuple(np.shape(nu)) != (features.P, H, int(np.shape(x0)[1])):
+        raise ValueError("particles_rollout: nu must be [P,H,E], got %s" % (tuple(np.shape(nu)),))
+    return _particles_rollout_consistent(dyn, policy_spec, reward_terms, dev(x0), None, mult_mu, max_ws_bytes, angles,
+                                         measurement_noise, None if nu is None else dev(nu), schedule, features, H)
+
+
+def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None, num_features=None):
     """pilco_particles_consistent_workspace_bytes of P particles over H steps (0: unsupported sizes); ``Ds`` is the
-    policy's input width (with ``angles``: E + len(angles))"""
+    policy's input width (with ``angles``: E + len(angles)).  ``num_features``: the feature sampler's
+    (pilco_particles_features_workspace_bytes)."""
     pr = _lib.Particles()
     pr.P, pr.H = int(P), int(H)
     pr.dyn = dyn.struct()
     pr.pol.Ds, pr.pol.U = int(Ds), int(U)
     ang = angles_struct(angles, int(pr.dyn.E))
-    return int(lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), C.byref(ang) if ang is not None else None,
-                                                                    None))
+    ang = C.byref(ang) if ang is not None else None
+    if num_features is not None:
+        fd = _lib.FeatureDraws(int(num_features), None, None, None)
+        return int(lib.pilco_particles_features_workspace_bytes(C.byref(pr), ang, None, C.byref(fd)))
+    return int(lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), ang, None))
 
 
 def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None,
-                                  measurement_noise=None, nu=None, schedule=False):
-    P, H = int(x0.shape[0]), int(eps.shape[1])
+                                  measurement_noise=None, nu=None, schedule=False, features=None, H=None):
+    """the consistent rollout in chunks of particles; with ``features`` eps is None and H is given"""
+    P, H = int(x0.shape[0]), int(eps.shape[1]) if H is None else int(H)
     Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
     if angles is not None and len(angles) > 0:                 # the policy's width, before any allocation
         E = int(dyn.struct().E)
@@ -1341,7 +1477,8 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     _particle_noise(measurement_noise, int(dyn.struct().E))
     if max_ws_bytes is None:
         max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
-    wsb = lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles)
+    F = features.F if features is not None else None
+    wsb = lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles, F)
     fits = lambda p: 0 < wsb(p) <= max_ws_bytes
     if not fits(1):
         raise ValueError("particles_rollout: the consistent rollout of one particle (H=%d, n=%d) needs %d workspace "
@@ -1349,8 +1486,8 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     lo = _largest_fitting(fits, 1, P)
     if lo == P:
         plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles,
-                            measurement_noise=measurement_noise, schedule=schedule)
-        plan.set_inputs(x0, eps, nu)
+                            measurement_noise=measurement_noise, schedule=schedule, num_features=F)
+        plan.set_inputs(x0, None if F else eps, nu, features=features)
         plan.launch()
         return plan.outputs()
     d = device()
@@ -1364,8 +1501,9 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
         if plan is None or plan.P != p1 - p0:
             plan = None                                     # free the previous chunk's workspace first
             plan = ParticlePlan(dyn, policy_spec, reward_terms, p1 - p0, H, mult_mu=mult_mu, consistent=True,
-                                angles=angles, measurement_noise=measurement_noise, schedule=schedule)
-        plan.set_inputs(x0[p0:p1], eps[p0:p1], None if nu is None else nu[p0:p1])
+                                angles=angles, measurement_noise=measurement_noise, schedule=schedule, num_features=F)
+        part = None if features is None else FeatureDraws(F, features.omega, features.w[p0:p1], features.v[p0:p1])
+        plan.set_inputs(x0[p0:p1], None if F else eps[p0:p1], None if nu is None else nu[p0:p1], features=part)
         plan.launch()
         for o, c in zip(out, plan.outputs()):
             o[p0:p1].copy_(c)

@@ -29,6 +29,23 @@ def _resample_refusals(what, resample, consistent, estimator="pathwise", explora
             raise ValueError("%s: resample=True does not combine with %s" % (what, why))
 
 
+def _feature_refusals(what, num_features, consistent, model, estimator="pathwise"):
+    """the random-feature sampler's refusals at the class level (ValueError), before any device work: it draws whole
+    functions (consistent=True), from the exact GP (not SMGPR's FITC), for the pathwise estimator, with 1 .. 8192
+    frequency pairs"""
+    if num_features is None:
+        return None
+    for on, why in ((not consistent, "consistent=False (the draws are whole functions: pass consistent=True)"),
+                    (isinstance(model, SMGPR), "an SMGPR (FITC) dynamics model"),
+                    (estimator == "score", "estimator='score' (a function sample has no per-step path density)")):
+        if on:
+            raise ValueError("%s: num_features does not combine with %s" % (what, why))
+    F = int(num_features)
+    if F < 1 or F > _lib.MAX_FEATURES:
+        raise ValueError("%s: num_features must be in 1 .. %d, got %d" % (what, _lib.MAX_FEATURES, F))
+    return F
+
+
 def _sqrt_factor(S):
     """F with F F' = S: the Cholesky factor, or for a positive semi-definite S (S = 0 included) the eigen-factor
     Q diag(sqrt(max(lambda, 0))).  ValueError when S has an eigenvalue below -1e-12 max|lambda|."""
@@ -279,7 +296,8 @@ class PILCO:
         M, S, _ = self.predict(m_x, s_x, 1)
         return M, S
 
-    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False):
+    def sample_trajectories(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False,
+                            num_features=None):
         """Monte Carlo rollouts of the learnt dynamics under the policy, to check what ``predict``'s moment matching
         approximates: ``num_samples`` particles start at x0 ~ N(m_x, s_x) and take n steps of
         x_{t+1} = x_t + mu(x_t, u_t) + sqrt(var(x_t, u_t)) eps_t with the latent GP posterior mean and variance,
@@ -298,6 +316,12 @@ class PILCO:
         the same generator after the step normals, so a seed gives the same x0 and step normals with and without it.
         It needs num_samples >= 2; with ``consistent=True`` it is a ValueError.
 
+        ``num_features=F`` with ``consistent=True``: each particle's functions are drawn once as a prior of F random
+        Fourier features plus an exact data update (DESIGN.md section 30), in time linear in n and with a workspace
+        that does not grow with the model's centres.  The same seed gives the same x0; the draws' normals (the
+        frequencies, the feature weights, the update's noise) follow from the same generator.  ``None``: the exact
+        sampler.  With ``consistent=False`` or an SMGPR model it is a ValueError.
+
         -> ParticleTrajectories(states [S,n+1,Ds], actions [S,n,U], rewards [S,n], risks [S,n], returns [S]) of
         host arrays; ``risks`` is the multiplicative channel of SafePILCO (zeros otherwise) and
         returns = rewards.sum(1) (+ mu (1 - prod_t (1 - risks)) for SafePILCO)."""
@@ -306,6 +330,10 @@ class PILCO:
         self._no_angles("sample_trajectories")
         self._no_noise("sample_trajectories")
         _resample_refusals("sample_trajectories", resample, consistent)
+        F = _feature_refusals("sample_trajectories", num_features, consistent, self.mgpr)
+        if F is not None:
+            out = self._feature_rollout(m_x, s_x, n, num_samples, seed, F, "sample_trajectories")
+            return ParticleTrajectories(*[t.cpu().numpy().view(HostArray) for t in out])
         if consistent:
             import torch
             dyn = self.mgpr.device_gp()
@@ -321,12 +349,20 @@ class PILCO:
         return ParticleTrajectories(*out)
 
     def _particle_plan(self, m_x, s_x, n, num_samples, seed, what, grad=False, consistent=False, estimator="pathwise",
-                       exploration=None, resample=False):
+                       exploration=None, resample=False, num_features=None):
         """ParticlePlan with x0 = m + F eps0 and the step normals drawn from one device generator seeded with ``seed``
         (from ``np.random`` when None): the same seed gives the same particles to every caller.  ``consistent``
         (with ``grad``): the ConsistentGradPlan over the same particles.  ``estimator``, ``exploration``,
-        ``resample``: ParticlePlan's (the redraw's normals come after the step normals)."""
+        ``resample``: ParticlePlan's (the redraw's normals come after the step normals).  ``num_features`` (with
+        ``consistent`` and ``grad``): the ConsistentGradPlan of the random-feature sampler over ``_feature_inputs``."""
         dyn = self.mgpr.device_gp()
+        if num_features is not None:
+            x0, draws = self._feature_inputs(m_x, s_x, n, num_samples, seed, num_features, what)
+            terms, mult_mu = self.reward_spec()
+            plan = engine.ConsistentGradPlan(dyn, self.policy_spec(), terms, int(num_samples), int(n), mult_mu=mult_mu,
+                                             exploration=exploration, num_features=num_features)
+            plan.set_inputs(x0, None, features=draws)
+            return plan
         inputs = self._particle_inputs(m_x, s_x, n, num_samples, seed, what, resample)
         x0, eps, xi = inputs if resample else inputs + (None,)
         terms, mult_mu = self.reward_spec()
@@ -339,14 +375,10 @@ class PILCO:
         plan.set_inputs(x0, eps, xi=xi)
         return plan
 
-    def _particle_inputs(self, m_x, s_x, n, num_samples, seed, what, resample=False):
-        """(x0 [S,Ds], eps [S,n,Ds]) device tensors of ``_particle_plan``: x0 = m + F eps0, then the step normals, from
-        one device generator seeded with ``seed`` (from ``np.random`` when None); eps is None at n = 0.  ``resample``:
-        (x0, eps, xi), the redraw's normals xi [S,n,Ds] drawn after the step normals from the same generator."""
+    def _start_states(self, m_x, s_x, S, seed):
+        """(x0 = m + F eps0 [S,Ds], the device generator seeded with ``seed`` (from ``np.random`` when None) after
+        eps0): the first draws of every particle method"""
         import torch
-        n, S = int(n), int(num_samples)
-        if n < 0 or S < 1:
-            raise ValueError("%s: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (what, n, S))
         Ds = self.state_dim
         m = np.asarray(m_x, dtype=np.float64).reshape(Ds)
         F = _sqrt_factor(np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds))
@@ -356,13 +388,48 @@ class PILCO:
         g = torch.Generator(device=d)
         g.manual_seed(int(seed))
         eps0 = torch.randn((S, Ds), dtype=engine.F64, device=d, generator=g)
-        x0 = engine.dev(m)[None] + eps0 @ engine.dev(F).T
+        return engine.dev(m)[None] + eps0 @ engine.dev(F).T, g
+
+    def _particle_inputs(self, m_x, s_x, n, num_samples, seed, what, resample=False):
+        """(x0 [S,Ds], eps [S,n,Ds]) device tensors of ``_particle_plan``: x0 = m + F eps0, then the step normals, from
+        one device generator seeded with ``seed`` (from ``np.random`` when None); eps is None at n = 0.  ``resample``:
+        (x0, eps, xi), the redraw's normals xi [S,n,Ds] drawn after the step normals from the same generator."""
+        import torch
+        n, S = int(n), int(num_samples)
+        if n < 0 or S < 1:
+            raise ValueError("%s: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (what, n, S))
+        Ds = self.state_dim
+        x0, g = self._start_states(m_x, s_x, S, seed)
+        d = x0.device
         eps = torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g) if n > 0 else None
         if not resample:
             return x0, eps
         xi = torch.randn((S, n, Ds), dtype=engine.F64, device=d, generator=g) if n > 0 else \
             torch.zeros((S, 0, Ds), dtype=engine.F64, device=d)
         return x0, eps, xi
+
+    def _feature_inputs(self, m_x, s_x, n, num_samples, seed, F, what):
+        """(x0 [S,Ds], draws) of the random-feature sampler: x0 exactly as ``_particle_inputs`` draws it for the same
+        seed, then from the same generator zeta [E,F,D], w [S,E,2F] and eps_y [S,E,N] (N training points), which
+        ``engine.feature_draws`` turns into the draws; no step normals are drawn"""
+        import torch
+        n, S = int(n), int(num_samples)
+        if n < 0 or S < 1:
+            raise ValueError("%s: needs n >= 0 and num_samples >= 1 (n=%d, num_samples=%d)" % (what, n, S))
+        dyn = self.mgpr.device_gp()
+        x0, g = self._start_states(m_x, s_x, S, seed)
+        d = x0.device
+        zeta = torch.randn((dyn.E, F, dyn.D), dtype=engine.F64, device=d, generator=g)
+        w = torch.randn((S, dyn.E, 2 * F), dtype=engine.F64, device=d, generator=g)
+        eps_y = torch.randn((S, dyn.E, dyn.n), dtype=engine.F64, device=d, generator=g)
+        return x0, engine.feature_draws(dyn, S, F, zeta, w, eps_y)
+
+    def _feature_rollout(self, m_x, s_x, n, num_samples, seed, F, what):
+        """the random-feature sampler's forward outputs over ``_feature_inputs``'s particles (chunked when large)"""
+        x0, draws = self._feature_inputs(m_x, s_x, n, num_samples, seed, F, what)
+        terms, mult_mu = self.reward_spec()
+        return engine.particles_rollout(self.mgpr.device_gp(), self.policy_spec(), terms, x0, None, mult_mu=mult_mu,
+                                        consistent=True, features=draws, horizon=int(n))
 
     def _flat_grad(self, g):
         """policy gradient blocks (device tensors) -> d / d controller.get_flat(): the lengthscale block times the
@@ -379,7 +446,8 @@ class PILCO:
         return np.concatenate([g["X"].cpu().numpy().ravel(), g["Y"].cpu().numpy().ravel(),
                                g["ell"].cpu().numpy().ravel() / (1.0 + np.exp(-th))])
 
-    def sample_reward_moments(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False):
+    def sample_reward_moments(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, resample=False,
+                              num_features=None):
         """Sample mean and variance of each step's reward over the particles of ``sample_trajectories`` (the same seed
         gives the same particles): the sampled counterpart of ``predict_reward_moments``.  mean_t is the mean of the
         step rewards (``sample_trajectories(...).rewards.mean(0)`` up to rounding) and var_t = sum_k c_k^2 s_kt^2 over
@@ -387,19 +455,23 @@ class PILCO:
         as ``predict_reward_moments``; the multiplicative terms of SafePILCO do not enter; DESIGN.md section 24).
         ``consistent``: the particles of ``sample_trajectories(..., consistent=True)``; a chunked rollout gives the
         statistics of all num_samples particles.  ``resample``: the particles of ``sample_trajectories(...,
-        resample=True)``.  Needs num_samples >= 2; a reward with an additive box term is a ValueError.  -> (mean [n],
+        resample=True)``.  ``num_features``: the particles of ``sample_trajectories(..., consistent=True,
+        num_features=F)``.  Needs num_samples >= 2; a reward with an additive box term is a ValueError.  -> (mean [n],
         var [n]) host arrays."""
         from ..params import HostArray
         self._no_schedule("sample_reward_moments")
         self._no_angles("sample_reward_moments")
         self._no_noise("sample_reward_moments")
         _resample_refusals("sample_reward_moments", resample, consistent)
+        F = _feature_refusals("sample_reward_moments", num_features, consistent, self.mgpr)
         if int(num_samples) < 2:
             raise ValueError("sample_reward_moments: the sample variance needs num_samples >= 2 (num_samples=%d)"
                              % int(num_samples))
         terms, mult_mu = self.reward_spec()
         engine._no_additive_box(terms)
-        if consistent:
+        if F is not None:
+            out = self._feature_rollout(m_x, s_x, n, num_samples, seed, F, "sample_reward_moments")
+        elif consistent:
             import torch
             x0, eps = self._particle_inputs(m_x, s_x, n, num_samples, seed, "sample_reward_moments")
             if eps is None:                                     # n = 0
@@ -414,7 +486,7 @@ class PILCO:
         return mean.cpu().numpy().view(HostArray), var.cpu().numpy().view(HostArray)
 
     def sample_policy_gradient(self, m_x, s_x, n, num_samples=1000, seed=None, consistent=False, estimator="pathwise",
-                               exploration=0.0, resample=False):
+                               exploration=0.0, resample=False, num_features=None):
         """Pathwise (reparameterisation) gradient of the Monte Carlo return of ``sample_trajectories``: the particles
         are drawn exactly as there (the same seed gives the same particles), value = mean of their returns, and grad =
         d value / d controller.get_flat() with x0 and the step normals held fixed -- the ascent direction of the
@@ -440,6 +512,11 @@ class PILCO:
         the Gaussian refit, its normals held fixed too (Deep PILCO's estimator, DESIGN.md section 26).  With
         ``consistent=True``, ``estimator="score"`` or exploration b != 0 it is a ValueError.
 
+        ``num_features=F`` with ``consistent=True``: the particles of ``sample_trajectories(..., consistent=True,
+        num_features=F)`` and the pathwise gradient over their random-feature draws (DESIGN.md section 30), whose
+        workspace does not grow with the model's centres.  With ``consistent=False``, an SMGPR model or
+        ``estimator="score"`` it is a ValueError.
+
         -> ParticlePolicyGradient(value (float), grad [len(get_flat())], returns [num_samples]) host arrays."""
         from ..params import HostArray
         self._no_schedule("sample_policy_gradient")
@@ -448,6 +525,7 @@ class PILCO:
         if estimator not in engine.ParticlePlan.ESTIMATORS:
             raise ValueError("sample_policy_gradient: estimator must be one of %s, not %r"
                              % (engine.ParticlePlan.ESTIMATORS, estimator))
+        F = _feature_refusals("sample_policy_gradient", num_features, consistent, self.mgpr, estimator)
         if estimator == "score":
             self._no_mlp("sample_policy_gradient(estimator='score')")
         if consistent and estimator == "score":
@@ -458,7 +536,7 @@ class PILCO:
         _resample_refusals("sample_policy_gradient", resample, consistent, estimator, b)
         plan = self._particle_plan(m_x, s_x, n, num_samples, seed, "sample_policy_gradient", grad=True,
                                    consistent=consistent, estimator=estimator, exploration=None if b == 0.0 else b,
-                                   resample=resample)
+                                   resample=resample, num_features=F)
         g = plan.launch_grad()
         return ParticlePolicyGradient(float(g["value"].item()), self._flat_grad(g).view(HostArray),
                                       plan.ret.cpu().numpy().view(HostArray))
@@ -508,7 +586,7 @@ class PILCO:
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
     def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False,
-                                exploration=0.0, resample=False):
+                                exploration=0.0, resample=False, num_features=None):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -533,7 +611,12 @@ class PILCO:
 
         ``resample=True``: Deep PILCO's objective with its Gaussian refit at every step (``sample_policy_gradient(...,
         resample=True)``); the refit's normals are drawn once with the others.  With ``consistent=True`` or exploration
-        b != 0 it is a ValueError."""
+        b != 0 it is a ValueError.
+
+        ``num_features=F`` with ``consistent=True``: the particles follow random-feature function draws (DESIGN.md
+        section 30), made once as ``sample_trajectories(..., num_features=F)`` makes them; a lock-step group's workspace
+        is then O(restarts num_samples horizon (D + E)) whatever the model's size.  With ``consistent=False`` or an
+        SMGPR model it is a ValueError."""
         from functools import partial
         from .. import policy_opt
         self._no_schedule("optimize_policy_sampled")
@@ -543,6 +626,7 @@ class PILCO:
             raise ValueError("optimize_policy_sampled: needs num_samples >= 1 (num_samples=%d)" % int(num_samples))
         b = float(exploration)
         _resample_refusals("optimize_policy_sampled", resample, consistent, "pathwise", b)
+        F = _feature_refusals("optimize_policy_sampled", num_features, consistent, self.mgpr)
         if resample and int(num_samples) < 2:
             raise ValueError("optimize_policy_sampled: resample=True needs num_samples >= 2 (num_samples=%d)"
                              % int(num_samples))
@@ -559,13 +643,19 @@ class PILCO:
             set_trainable(p, False)
         try:
             flats0 = policy_opt.initial_flats(self.controller, restarts)
-            inputs = self._particle_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed,
-                                           "optimize_policy_sampled", resample)
-            x0, eps, xi = inputs if resample else inputs + (None,)
+            draws = None
+            if F is not None:
+                x0, draws = self._feature_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed, F,
+                                                 "optimize_policy_sampled")
+                eps, xi = None, None
+            else:
+                inputs = self._particle_inputs(self.m_init, self.S_init, self.horizon, num_samples, seed,
+                                               "optimize_policy_sampled", resample)
+                x0, eps, xi = inputs if resample else inputs + (None,)
             best_flat, best_value, _ = policy_opt.optimize(
                 self, maxiter=maxiter, restarts=restarts, flats0=flats0,
                 evaluator=partial(policy_opt.ParticleEvaluator, x0=x0, eps=eps, consistent=consistent,
-                                  exploration=None if b == 0.0 else b, resample=resample, xi=xi))
+                                  exploration=None if b == 0.0 else b, resample=resample, xi=xi, features=draws))
             self.controller.set_flat(best_flat)
         finally:
             for p in mgpr_trainable:

@@ -244,9 +244,11 @@ class ParticleEvaluator(_FlatEvaluator):
     (pilco_particles_resampled_grad_rollout, DESIGN.md section 26) with the redraw's standard normals ``xi`` [P,H,Ds],
     held fixed like eps.  A ``TimeVaryingLinearController`` runs the scheduled calls (pilco_particles_scheduled_*,
     DESIGN.md section 28), its gradient per step; an ``MlpController`` the MLP calls (pilco_particles_mlp_*, section 29),
-    its flat vector being the device's theta."""
+    its flat vector being the device's theta.  ``features``: ``engine.feature_draws`` of the P particles, with
+    ``consistent=True``: the functions are those random-feature draws (pilco_particles_features_grad_rollout, DESIGN.md
+    section 30) and eps is not read (None)."""
 
-    def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None):
+    def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None, features=None):
         terms, mult_mu = pilco.reward_spec()
         if any(t["kind"] == _lib.REWARD_BOX for t in terms):
             raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
@@ -259,12 +261,14 @@ class ParticleEvaluator(_FlatEvaluator):
         if consistent:
             self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
                                                   int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration,
-                                                  schedule=self.sched)
+                                                  schedule=self.sched,
+                                                  num_features=None if features is None else features.F)
         else:
             self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
                                             mult_mu=mult_mu, grad=True, R=R, exploration=exploration,
-                                            resample=resample, schedule=self.sched)
-        self.plan.set_inputs(x0, eps, xi=xi)
+                                            resample=resample, schedule=self.sched,
+                                            num_features=None if features is None else features.F)
+        self.plan.set_inputs(x0, eps, xi=xi, features=features)
         self._setup_io()
 
     def _enqueue(self):
