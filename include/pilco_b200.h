@@ -914,6 +914,62 @@ int    pilco_particles_mlp_features_grad_rollout(const pilco_particles* pr, cons
                                                  const pilco_exploration* ex, const pilco_feature_draws* fd, int R,
                                                  const pilco_particles_grad* g, pilco_stream_t stream);
 
+/* ---- batched forward-only scheduled rollouts and the cross-entropy method (DESIGN.md section 31) ------------------
+ * pilco_particles_scheduled_batch_rollout / _scheduled_consistent_batch_rollout: the forward of
+ * pilco_particles_scheduled_batch_grad_rollout / _scheduled_consistent_grad_rollout (ex NULL) without the reverse sweep
+ * or its histories.  R restarts share x0, eps (and nu); restart r runs the schedule at pol.W + r pol.W_bs + t W_ts and
+ * pol.b + r pol.b_bs + t b_ts.  The outputs have a leading R as in the gradient calls, and value [R] is the fixed-order
+ * mean return.  Outputs and value are bitwise the gradient call's; restart r is bitwise
+ * pilco_particles_scheduled_rollout (_consistent_rollout) with restart r's schedule.  ang and nz may be NULL.  The
+ * workspace is pr->ws.  Validation before any work is enqueued: the gradient call's codes with PILCO_ERR_NULL for value
+ * NULL in place of its gradient-output checks, then the workspace's codes.  A size query returns 0 exactly where its
+ * call fails on sizes.  Deterministic, no host synchronisation (graph-capturable).
+ *
+ * pilco_cem_update: one iteration of the cross-entropy method over K candidate sequences cand [K,H,U] scored value
+ * [K] (a batched rollout's value with b = cand, b_bs = H U, b_ts = U), in this order:
+ *   1. rank: value descending, NaN last, ties to the lower index; the elites are the first n_elite in rank order
+ *   2. refit per (t, u): m_e, v_e the elites' mean and biased variance (two passes, summed in rank order);
+ *      mean <- alpha mean + (1 - alpha) m_e, std <- sqrt(alpha std^2 + (1 - alpha) v_e)
+ *   3. best so far: when the top value is strictly above *best_value, it and its candidate go to best_value and best
+ *   4. next candidates (xi not NULL): row 0 = clip(mean, lo, hi), row k >= 1 = clip(mean + std o xi_k, lo, hi)
+ *   5. trace (not NULL): trace[0] = the top value, trace[1] = the elites' mean value (rank-order sum / n_elite)
+ * pilco_cem_draw: step 4 alone (the first candidates); it reads cand, xi, mean, std, K, H, U, lo and hi.
+ * Validation before any work is enqueued: PILCO_ERR_NULL for c or a pointer the call uses (update: value, cand, mean,
+ * std, best_value, best; draw: cand, xi, mean, std), then PILCO_ERR_DIM for K outside 1 .. 8192, H < 1, U < 1,
+ * H U > 2^24, lo >= hi (or a NaN bound) and (update) n_elite outside 1 .. K or alpha outside [0, 1), then the
+ * workspace's codes (NULL, PILCO_ERR_ALIGN below 16-byte alignment, PILCO_ERR_WORKSPACE).  The workspace query returns
+ * 0 exactly for K outside 1 .. 8192.  Deterministic (no atomics), no host synchronisation (graph-capturable). */
+size_t pilco_particles_scheduled_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                       const pilco_particles_noise* nz,
+                                                       const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                               const pilco_particles_noise* nz, const pilco_policy_schedule* sch,
+                                               int R, double* value, pilco_stream_t stream);
+size_t pilco_particles_scheduled_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                                  const pilco_particles_noise* nz,
+                                                                  const pilco_policy_schedule* sch, int R);
+int    pilco_particles_scheduled_consistent_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                          const pilco_particles_noise* nz,
+                                                          const pilco_policy_schedule* sch, int R, double* value,
+                                                          pilco_stream_t stream);
+typedef struct pilco_cem {
+    int K, H, U;                /* candidates, steps, action width */
+    int n_elite;                /* 1 .. K */
+    double alpha;               /* smoothing in [0, 1) */
+    double lo, hi;              /* the candidates' bounds, lo < hi */
+    const double* value;        /* [K] the candidates' values */
+    double* cand;               /* [K,H,U] in: the scored candidates; out: the next ones */
+    const double* xi;           /* [K,H,U] standard normals of the next candidates (row 0 unread); NULL: no draw */
+    double* mean;               /* [H,U] the sampling mean, updated in place */
+    double* std;                /* [H,U] the sampling standard deviation, updated in place */
+    double* best_value;         /* [1] the best value so far (-inf before the first iteration) */
+    double* best;               /* [H,U] its candidate */
+    double* trace;              /* [2] this iteration's (top value, elites' mean value), or NULL */
+} pilco_cem;
+size_t pilco_cem_update_workspace_bytes(int K);
+int    pilco_cem_update(const pilco_cem* c, void* ws, size_t ws_bytes, pilco_stream_t stream);
+int    pilco_cem_draw(const pilco_cem* c, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

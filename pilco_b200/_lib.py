@@ -110,7 +110,16 @@ class FeatureDraws(C.Structure):
     _fields_ = [("F", C.c_int), ("omega", c_dp), ("w", c_dp), ("v", c_dp)]
 
 
+class Cem(C.Structure):
+    """mirror of ``pilco_cem``"""
+    _fields_ = [("K", C.c_int), ("H", C.c_int), ("U", C.c_int), ("n_elite", C.c_int),
+                ("alpha", C.c_double), ("lo", C.c_double), ("hi", C.c_double),
+                ("value", c_dp), ("cand", c_dp), ("xi", c_dp), ("mean", c_dp), ("std", c_dp),
+                ("best_value", c_dp), ("best", c_dp), ("trace", c_dp)]
+
+
 MAX_FEATURES = 8192                              # PILCO_MAX_FEATURES
+CEM_MAX_K = 8192                                 # pilco_cem_update's largest K
 POLICY_LINEAR, POLICY_RBF, POLICY_MLP = 0, 1, 2
 REWARD_EXP, REWARD_LINEAR, REWARD_BOX = 0, 1, 2
 REWARD_EXP_SA, REWARD_LINEAR_SA = 3, 4           # on the joint state-action Gaussian [x, u], D = Ds + U
@@ -320,6 +329,15 @@ SIGNATURES = {
     "pilco_particles_mlp_features_grad_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp),
                                                             C.POINTER(Exploration), C.POINTER(FeatureDraws), C.c_int,
                                                             C.POINTER(ParticlesGrad), c_dp]),
+    "pilco_particles_scheduled_batch_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule), C.c_int]),
+    "pilco_particles_scheduled_batch_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), C.c_int, c_dp, c_dp]),
+    "pilco_particles_scheduled_consistent_batch_workspace_bytes": (C.c_size_t, _PAN + [C.POINTER(PolicySchedule),
+                                                                                       C.c_int]),
+    "pilco_particles_scheduled_consistent_batch_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), C.c_int, c_dp,
+                                                                            c_dp]),
+    "pilco_cem_update_workspace_bytes": (C.c_size_t, [C.c_int]),
+    "pilco_cem_update": (C.c_int, [C.POINTER(Cem), c_dp, C.c_size_t, c_dp]),
+    "pilco_cem_draw": (C.c_int, [C.POINTER(Cem), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

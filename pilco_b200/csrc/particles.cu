@@ -843,7 +843,8 @@ __global__ void __launch_bounds__(256) pg_sched_kernel(PgRed a) {
 
 enum PtCall { PT_FORWARD, PT_PATHWISE, PT_SCORE };
 
-// What one validated call runs.  The entry point sets the sampler, the call and batched; pt_validate the rest.
+// What one validated call runs.  The entry point sets the sampler, the call, batched (and a batched forward's value);
+// pt_validate the rest.
 struct PtOpt {
     bool consistent;            // one posterior function per particle (DESIGN.md section 14), else step-wise draws
     PtCall call;
@@ -864,6 +865,8 @@ struct PtOpt {
     PmNet net;
     bool features;              // function samples from random-feature draws (DESIGN.md section 30): fd's, not eps
     pilco_feature_draws fd;
+    double* value;              // a batched forward (call PT_FORWARD with batched, DESIGN.md section 31): the mean
+                                // return per restart [R], set by the entry point
 };
 
 // Offsets in doubles into a particle workspace, for both layouts (a slot a call does not have stays 0); the predict
@@ -1618,9 +1621,10 @@ static bool pt_sched_active(const pilco_policy_schedule* sch) { return sch && (s
 
 // ---- one validator, one query, one call path --------------------------------------------------------------------------
 // Everything a call checks before its workspace, in this order: NULL pr, the angles' map (A != 0), the description
-// (the policy's batch strides as o->batched allows), R, the gradient's outputs, the noise, the exploration (active
-// only).  Each family's call is the most general call with NULL for the features it lacks, so ang == NULL or A == 0
-// is the call without angles, nz == NULL the call without noise and an inactive ex the call without exploration.
+// (the policy's batch strides as o->batched allows), R, the gradient's outputs (a batched forward's: value), the
+// noise, the exploration (active only).  Each family's call is the most general call with NULL for the features it
+// lacks, so ang == NULL or A == 0 is the call without angles, nz == NULL the call without noise and an inactive ex the
+// call without exploration.
 // Resampled calls (o->resampled, no angles, noise or exploration), after the gradient's outputs: PILCO_ERR_NULL for rs
 // NULL or xi NULL with H > 0, then PILCO_ERR_DIM for P < 2 (no sample covariance).
 // Scheduled calls (DESIGN.md section 28), after everything else: PILCO_ERR_DIM for a negative stride, then
@@ -1641,8 +1645,9 @@ static int pt_validate(PtOpt* o, const pilco_particles* pr, const pilco_angles* 
         if (const int rc = pa_map(pr, ang, &o->tm)) return rc;
     if (const int rc = pt_check_desc(pr, o->batched, angles ? o->tm.A : 0, o->mlp, mlp, !o->features)) return rc;
     if (!pt_batch_ok(pr->P, R)) return PILCO_ERR_DIM;   // the unbatched calls' R = 1 passes with the description
-    if (o->call != PT_FORWARD)
+    if (o->call != PT_FORWARD) {
         if (const int rc = pg_check(pr, g, o->mlp ? mlp : nullptr)) return rc;
+    } else if (o->batched && !o->value) return PILCO_ERR_NULL;
     if (o->mlp) o->net = pm_net(pr, mlp);
     if (o->resampled) {
         if (!rs || (!rs->xi && pr->H > 0)) return PILCO_ERR_NULL;
@@ -1727,7 +1732,9 @@ static int pt_call(PtOpt o, const pilco_particles* pr, const pilco_angles* ang, 
     }
     const PfDev* pf = o.features ? &q : nullptr;
     if (const int rc = pt_forward(pr, R, ws, L, o.consistent, !fwd, st, tm, n, rsv, sv, net, pf)) return rc;
-    if (fwd) return PILCO_OK;
+    // a batched forward's value: pm_finish_kernel with no parameters is its value CTA alone, the same fixed-order mean
+    // as pg_param_kernel's and pg_sched_kernel's
+    if (fwd) return o.batched ? pm_finish_launch(st, R, pr->P, 0, 0, nullptr, pr->ret, nullptr, o.value) : PILCO_OK;
     if (o.call == PT_SCORE) return ps_run(pr, o, g, L, st);
     if (o.explore) {
         PxMom m = px_mom(pr, o.tm, o.b);
@@ -1746,6 +1753,7 @@ static const PtOpt FWD = {false, PT_FORWARD, false}, CFWD = {true, PT_FORWARD, f
 static const PtOpt PATH1 = {false, PT_PATHWISE, false}, PATH = {false, PT_PATHWISE, true};
 static const PtOpt CPATH = {true, PT_PATHWISE, true}, SCORE = {false, PT_SCORE, true}, CSCORE = {true, PT_SCORE, true};
 static const PtOpt RFWD = {false, PT_FORWARD, false, true}, RPATH = {false, PT_PATHWISE, true, true};
+static const PtOpt BFWD = {false, PT_FORWARD, true}, CBFWD = {true, PT_FORWARD, true};
 
 // the MLP calls (DESIGN.md section 29): a family's options with o.mlp
 static PtOpt pm_opt(PtOpt o) { o.mlp = true; return o; }
@@ -1996,6 +2004,36 @@ int pilco_particles_scheduled_batch_grad_rollout(const pilco_particles* pr, cons
                                                  const pilco_policy_schedule* sch, int R,
                                                  const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(PATH, pr, ang, nz, ex, R, g, stream, nullptr, sch);
+}
+
+// batched forward-only rollouts (DESIGN.md section 31): the scheduled gradient calls' forward without their histories
+size_t pilco_particles_scheduled_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                       const pilco_particles_noise* nz,
+                                                       const pilco_policy_schedule* sch, int R) {
+    return pt_query(BFWD, pr, ang, nz, nullptr, R, sch);
+}
+
+int pilco_particles_scheduled_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                            const pilco_particles_noise* nz, const pilco_policy_schedule* sch, int R,
+                                            double* value, pilco_stream_t stream) {
+    PtOpt o = BFWD;
+    o.value = value;
+    return pt_call(o, pr, ang, nz, nullptr, R, nullptr, stream, nullptr, sch);
+}
+
+size_t pilco_particles_scheduled_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                                  const pilco_particles_noise* nz,
+                                                                  const pilco_policy_schedule* sch, int R) {
+    return pt_query(CBFWD, pr, ang, nz, nullptr, R, sch);
+}
+
+int pilco_particles_scheduled_consistent_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                       const pilco_particles_noise* nz,
+                                                       const pilco_policy_schedule* sch, int R, double* value,
+                                                       pilco_stream_t stream) {
+    PtOpt o = CBFWD;
+    o.value = value;
+    return pt_call(o, pr, ang, nz, nullptr, R, nullptr, stream, nullptr, sch);
 }
 
 size_t pilco_particles_scheduled_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,

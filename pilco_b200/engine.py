@@ -1510,6 +1510,202 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     return out
 
 
+# the batched forward-only rollouts (DESIGN.md section 31) per sampler: (rollout, size query) after "pilco_particles_"
+PARTICLE_BATCH_CALLS = {
+    False: ("scheduled_batch_rollout", "scheduled_batch_workspace_bytes"),
+    True: ("scheduled_consistent_batch_rollout", "scheduled_consistent_batch_workspace_bytes"),
+}
+
+CEM_BOUND = 0.5 * np.pi          # the candidates' b lie in [-pi/2, pi/2], where u = maxa sin(b) is monotone and onto
+
+
+class CemPlan:
+    """The cross-entropy method (CEM) over open-loop action sequences on the sampled return, as trajectory-sampling MPC
+    plans on a learnt model (PETS, Chua et al. 2018; DESIGN.md section 31), every iteration on the device.
+
+    ``spec`` is a scheduled linear policy: W [Hw,U,Ds] (Hw >= H), shared by every candidate and held fixed (zero for the
+    open-loop sequences u_t = maxa sin(b_t)), and b [Hw,U], whose first H steps are the initial sampling mean.  Each of
+    ``iters`` iterations rolls out the ``population`` = K candidate schedules b [K,H,U] over the same P particles (x0,
+    eps and, with ``measurement_noise``, nu; pilco_particles_scheduled_batch_rollout, or _consistent_ with
+    ``consistent=True``), scores each by its mean return and refits a diagonal Gaussian to the ``elites`` best with
+    smoothing ``alpha`` (pilco_cem_update).  The candidates are clipped to [-pi/2, pi/2]; row 0 of every population is
+    the clipped sampling mean, so the plan is at least as good as its warm start on the same particles.  Every reward
+    term works, box terms and the SafePILCO channel (``mult_mu``) included, since nothing is differentiated.
+    ``angles``: as ``ParticlePlan`` (the state is then the dynamics GP's E outputs, the policy takes E + len(angles)).
+
+    ``set_inputs(x0, eps, xi, nu=None, std0=None)`` fills the static buffers; ``launch()`` enqueues the whole loop (a
+    draw, then per iteration the batched rollout and the update) and ``capture()`` records it as one CUDA graph that
+    ``replay()`` runs.  Afterwards ``best_b`` [H,U] and ``best_value`` [1] hold the best candidate so far and its value,
+    ``mean`` and ``std`` [H,U] the sampling distribution, ``trace`` [iters,2] each iteration's top value and elites'
+    mean value, and ``outputs()`` the last population's rollouts.
+
+    ``consistent=True`` rolls the candidates out in chunks whose O(R P H E n) workspace fits ``max_ws_bytes`` (default:
+    half the free device memory); restarts are independent, so the chunking changes no bit.  An RBF or MLP spec, a W
+    with a leading batch dimension, an unsquashed policy, ``num_features``, ``resample``, any ``estimator``, K outside
+    1 .. 8192, elites outside 1 .. K, iters < 1, alpha outside [0, 1) or H < 1 is a ValueError raised before any
+    allocation."""
+
+    def __init__(self, dyn, spec, reward_terms, P, H, population, elites, iters, mult_mu=0.0, consistent=False,
+                 angles=None, measurement_noise=None, alpha=0.1, max_ws_bytes=None, num_features=None, resample=False,
+                 estimator=None):
+        if _is_mlp(spec) or spec.get("kind") != _lib.POLICY_LINEAR:
+            raise ValueError("CemPlan: the candidates are the b of a scheduled linear policy; an %s policy has none"
+                             % ("MLP" if _is_mlp(spec) else "RBF"))
+        for on, what in ((num_features is not None, "num_features (the feature sampler)"),
+                         (bool(resample), "resample=True"),
+                         (estimator is not None, "an estimator (estimator=%r): CEM differentiates nothing" % (estimator,))):
+            if on:
+                raise ValueError("CemPlan: the batched forward rollout does not combine with %s" % what)
+        K, ke, iters, P, H, alpha = int(population), int(elites), int(iters), int(P), int(H), float(alpha)
+        if not 1 <= K <= _lib.CEM_MAX_K:
+            raise ValueError("CemPlan: population must be in 1 .. %d, got %d" % (_lib.CEM_MAX_K, K))
+        if not 1 <= ke <= K:
+            raise ValueError("CemPlan: elites must be in 1 .. population=%d, got %d" % (K, ke))
+        if iters < 1 or P < 1 or H < 1:
+            raise ValueError("CemPlan: needs iters >= 1, P >= 1 and H >= 1 (iters=%d, P=%d, H=%d)" % (iters, P, H))
+        if not 0.0 <= alpha < 1.0:
+            raise ValueError("CemPlan: alpha must be in [0, 1), got %r" % alpha)
+        batched, _ = _schedule_check(spec, H, True)
+        if batched:
+            raise ValueError("CemPlan: W [Hw,U,Ds] is shared by every candidate: no leading batch dimension")
+        if not spec.get("squash", True):
+            raise ValueError("CemPlan: the bounds [-pi/2, pi/2] need the squashed policy u = maxa sin(b)")
+        E = int(dyn.struct().E)
+        Ds, U = int(spec["Ds"]), int(spec["U"])
+        ang = angles_struct(angles, E) if angles is not None and len(angles) > 0 else None
+        if Ds != E + (ang.A if ang is not None else 0):
+            raise ValueError("CemPlan: the policy must take %d inputs (the state%s), got %d"
+                             % (E + (ang.A if ang is not None else 0), " with its angles" if ang is not None else "", Ds))
+        nz_var = _particle_noise(measurement_noise, E)
+        self.P, self.H, self.K, self.elites, self.iters, self.alpha = P, H, K, ke, iters, alpha
+        self.E, self.U, self.consistent = E, U, bool(consistent)
+        self.ang, self.keep = ang, [dyn, spec, reward_terms]
+        pr = _lib.Particles()
+        pr.P, pr.H = P, H
+        pr.dyn = dyn.struct()
+        pr.pol.kind, pr.pol.Ds, pr.pol.U = _lib.POLICY_LINEAR, Ds, U      # what the size queries read
+        self.sch = _lib.PolicySchedule(U * Ds, U)              # step t: W[t], cand[r, t]
+        self.nz = None
+        if nz_var is not None:
+            self.nz = _lib.ParticlesNoise()
+            for i, v in enumerate(nz_var):
+                self.nz.v.var[i] = float(v)
+        names = PARTICLE_BATCH_CALLS[self.consistent]
+        self._roll = getattr(lib, "pilco_particles_" + names[0])
+        qz = None                                               # the sizes' noise: nu is checked, not read
+        if self.nz is not None:
+            qz = _lib.ParticlesNoise.from_buffer_copy(self.nz)
+            qz.nu = 16
+        query = lambda R: int(getattr(lib, "pilco_particles_" + names[1])(
+            C.byref(pr), self._ang_ref(), C.byref(qz) if qz is not None else None, C.byref(self.sch), int(R)))
+        if query(1) == 0:
+            raise ValueError("CemPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, pr.dyn.D))
+        if len(reward_terms) > 8:
+            raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
+        if max_ws_bytes is None:
+            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+        fits = lambda R: 0 < query(R) <= max_ws_bytes
+        if not fits(1):
+            raise ValueError("CemPlan: the rollout of one candidate (P=%d, H=%d, n=%d) needs %d workspace bytes, more "
+                             "than max_ws_bytes=%d" % (P, H, pr.dyn.n, query(1), max_ws_bytes))
+        Rc = _largest_fitting(fits, 1, K)
+        self.max_action, self.W, b, _ = _fill_policy(pr.pol, spec, batched=False)
+        self.rw = _fill_rewards(pr, reward_terms)
+        pr.mult_mu = float(mult_mu)
+        d = device()
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
+        self.x0, self.eps_buf = mk(P, E), mk(P, H, E)           # shared by the candidates
+        self.traj, self.act_buf = mk(K, P, H + 1, E), mk(K, P, H, U)
+        self.rew_buf, self.risk_buf, self.ret, self.value = mk(K, P, H), mk(K, P, H), mk(K, P), mk(K)
+        self.cand, self.xi = mk(K, H, U), mk(iters, K, H, U)
+        self.mean0, self.std0 = b[:H].clone(), mk(H, U)
+        self.mean, self.std, self.best_b = mk(H, U), mk(H, U), mk(H, U)
+        self.best_value, self.trace = mk(1), mk(iters, 2)
+        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
+        pr.pol.b_bs = H * U
+        if self.nz is not None:
+            self.nu_buf = mk(P, H, E)
+            self.nz.nu = self.nu_buf.data_ptr()
+        self.ws = torch.empty(max(query(Rc) // 8, 2), dtype=F64, device=d)
+        pr.ws, pr.ws_bytes = self.ws.data_ptr(), query(Rc)
+        self.chunks = []                                        # (description, R, value) of each chunk of candidates
+        for r0 in range(0, K, Rc):
+            c = _lib.Particles.from_buffer_copy(pr)
+            c.pol.b = self.cand[r0].data_ptr()
+            c.traj, c.act = self.traj[r0].data_ptr(), self.act_buf[r0].data_ptr()
+            c.step_reward, c.step_risk = self.rew_buf[r0].data_ptr(), self.risk_buf[r0].data_ptr()
+            c.ret = self.ret[r0].data_ptr()
+            self.chunks.append((c, min(Rc, K - r0), self.value[r0].data_ptr()))
+        self.chunk = Rc
+        cem = lambda xi, trace: _lib.Cem(K, H, U, ke, alpha, -CEM_BOUND, CEM_BOUND, self.value.data_ptr(),
+                                         self.cand.data_ptr(), xi, self.mean.data_ptr(), self.std.data_ptr(),
+                                         self.best_value.data_ptr(), self.best_b.data_ptr(), trace)
+        self.draw = cem(self.xi[0].data_ptr(), None)            # the first population, then each update's next one
+        self.updates = [cem(self.xi[i + 1].data_ptr() if i + 1 < iters else None, self.trace[i].data_ptr())
+                        for i in range(iters)]
+        self.uws_bytes = int(lib.pilco_cem_update_workspace_bytes(K))
+        self.uws = torch.empty(max(self.uws_bytes // 8, 2), dtype=F64, device=d)
+        self.graph = None
+
+    def _ang_ref(self):
+        return C.byref(self.ang) if self.ang is not None else None
+
+    def _nz_ref(self):
+        return C.byref(self.nz) if self.nz is not None else None
+
+    def set_inputs(self, x0, eps, xi, nu=None, std0=None):
+        """x0 [P,E], eps [P,H,E], xi [iters,K,H,U] (iteration i's population draws xi[i]; row 0 is unread), with
+        measurement noise nu [P,H,E] (required then, and only then); std0: the initial sampling std (a scalar or
+        [H,U]; default (hi - lo) / 4 = pi/4)"""
+        if (nu is None) != (self.nz is None):
+            raise ValueError("CemPlan: nu [P,H,E] is required with measurement_noise and only then")
+        self.x0.copy_(dev(x0).reshape(self.P, self.E))
+        self.eps_buf.copy_(dev(eps).reshape(self.eps_buf.shape))
+        self.xi.copy_(dev(xi).reshape(self.xi.shape))
+        if nu is not None:
+            self.nu_buf.copy_(dev(nu).reshape(self.nu_buf.shape))
+        self.std0.copy_(dev(np.broadcast_to(np.asarray(0.5 * CEM_BOUND if std0 is None else std0, dtype=np.float64),
+                                            (self.H, self.U)).copy()))
+
+    def rollout(self):
+        """the batched rollout of the current population: value [K] and ``outputs()``"""
+        for c, R, value in self.chunks:
+            check(self._roll(C.byref(c), self._ang_ref(), self._nz_ref(), C.byref(self.sch), R, value, stream_ptr()),
+                  "particles_batch_rollout")
+        return self.value
+
+    def launch(self):
+        """the whole plan on the current stream, from the initial mean and std0: no host synchronisation"""
+        self.mean.copy_(self.mean0)
+        self.std.copy_(self.std0)
+        self.best_b.copy_(self.mean0)
+        self.best_value.fill_(-float("inf"))
+        check(lib.pilco_cem_draw(C.byref(self.draw), stream_ptr()), "cem_draw")
+        for u in self.updates:
+            self.rollout()
+            check(lib.pilco_cem_update(C.byref(u), self.uws.data_ptr(), self.uws_bytes, stream_ptr()), "cem_update")
+        return self.best_b, self.best_value
+
+    def capture(self):
+        """record ``launch()`` as one CUDA graph (after an eager warm-up that sets one-time kernel attributes)"""
+        self.launch()
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.launch()
+        self.graph = g
+        return g
+
+    def replay(self):
+        self.graph.replay()
+        return self.best_b, self.best_value
+
+    def outputs(self):
+        """(traj [K,P,H+1,E], act [K,P,H,U], step_reward [K,P,H], step_risk [K,P,H], ret [K,P]) of the last population
+        rolled out"""
+        return self.traj, self.act_buf, self.rew_buf, self.risk_buf, self.ret
+
+
 class PredictPlan:
     """``PILCO.predict(m, S, n)`` as ONE graph launch: host moments -> device, n-step cascade (R = 1), final
     moments + reward + status -> pinned host memory.  Built once per (model, policy, reward, n) state by

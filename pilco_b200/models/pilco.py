@@ -752,7 +752,7 @@ class PILCO:
 
     # ---- receding-horizon planning (probabilistic MPC, Kamthe & Deisenroth 2018) --------------------------------------
     def plan(self, m_x, s_x=None, maxiter=20, restarts=1, warm_start=True, num_samples=None, seed=None,
-             consistent=False):
+             consistent=False, optimizer="lbfgsb", population=400, elites=40):
         """One receding-horizon step with a TimeVaryingLinearController: optimise its schedule over ``horizon`` steps
         of the moment-matching cascade from N(m_x, s_x) (s_x = None or 0: a measured state), return the first action
         u_0 = compute_action(m_x, t=0) [1,U], then shift the schedule one step (theta_t <- theta_{t+1}, the last step
@@ -767,7 +767,17 @@ class PILCO:
         drawn once from one generator seeded with ``seed`` and held fixed, so the objective is deterministic.
         ``consistent=True``: each particle follows one function drawn from the dynamics posterior.  Restarts, warm
         start and the shift are as above; ``exploration`` is not read.  Box terms, ``angle_dims`` and
-        ``measurement_noise`` are a ValueError raised before any device work."""
+        ``measurement_noise`` are a ValueError raised before any device work.
+
+        ``optimizer="cem"`` (with ``num_samples``, ``restarts=1``): the cross-entropy method over the schedule's b on
+        the same sampled return, every iteration on the device (``engine.CemPlan``, DESIGN.md section 31), as PETS
+        plans.  ``maxiter`` is its iteration count; each iteration rolls out ``population`` candidate schedules and
+        refits the sampling distribution to the ``elites`` best.  The candidates start from the controller's current
+        schedule (W held fixed), its b clipped to [-pi/2, pi/2], with std pi/4.  The seeded generator draws x0 and the
+        step normals exactly as the default optimizer does (the same particles for the same seed), then the
+        measurement noise's normals, then the candidates' normals.  Nothing is differentiated, so box terms,
+        SafePILCO's risk channel, ``angle_dims`` and ``measurement_noise`` all work.  The controller's b then holds the
+        best candidate, and ``cem_plan`` the plan (its ``trace``, ``best_value`` and particles)."""
         from functools import partial
         from .. import policy_opt
         self._no_mlp("plan")
@@ -778,6 +788,11 @@ class PILCO:
         Ds = self.state_dim
         m = np.asarray(m_x, dtype=np.float64).reshape(1, Ds)
         s = np.zeros((Ds, Ds)) if s_x is None else np.asarray(s_x, dtype=np.float64).reshape(Ds, Ds)
+        if optimizer == "cem":
+            return self._plan_cem(m, s, maxiter, restarts, warm_start, num_samples, seed, consistent, population,
+                                  elites)
+        if optimizer != "lbfgsb":
+            raise ValueError("plan: optimizer must be 'lbfgsb' or 'cem', not %r" % (optimizer,))
         if num_samples is not None:
             self._no_angles("plan(num_samples=...)")
             self._no_noise("plan(num_samples=...)")
@@ -803,6 +818,44 @@ class PILCO:
         finally:
             for p in mgpr_trainable:
                 set_trainable(p, True)
+        u = self.compute_action(m, t=0)
+        c.shift()
+        return u
+
+    def _plan_cem(self, m, s, maxiter, restarts, warm_start, num_samples, seed, consistent, population, elites):
+        """plan(optimizer="cem"): every refusal before any device work, then one engine.CemPlan"""
+        import torch
+        if num_samples is None or int(num_samples) < 1:
+            raise ValueError("plan(optimizer='cem'): needs num_samples >= 1 (num_samples=%r)" % (num_samples,))
+        if int(restarts) != 1:
+            raise ValueError("plan(optimizer='cem'): takes restarts=1 (the population is the search), got %d"
+                             % int(restarts))
+        K, ke, iters = int(population), int(elites), int(maxiter)
+        if not 1 <= K <= _lib.CEM_MAX_K or not 1 <= ke <= K or iters < 1:
+            raise ValueError("plan(optimizer='cem'): needs 1 <= population <= %d, 1 <= elites <= population and "
+                             "maxiter >= 1 (population=%d, elites=%d, maxiter=%d)" % (_lib.CEM_MAX_K, K, ke, iters))
+        c, H, S, U, Ds = self.controller, int(self.horizon), int(num_samples), self.control_dim, self.state_dim
+        if H < 1:
+            raise ValueError("plan(optimizer='cem'): needs horizon >= 1")
+        if not warm_start:
+            c.randomize()
+        spec = c.policy_spec()
+        spec["b"] = np.clip(spec["b"], -engine.CEM_BOUND, engine.CEM_BOUND)
+        terms, mult_mu = self.reward_spec()
+        noise = self._noise_var()
+        x0, g = self._start_states(m, s, S, seed)
+        draw = lambda *shape: torch.randn(shape, dtype=engine.F64, device=x0.device, generator=g)
+        eps = draw(S, H, Ds)                                    # _particle_inputs' step normals
+        nu = draw(S, H, Ds) if noise is not None else None
+        xi = draw(iters, K, H, U)
+        plan = engine.CemPlan(self.mgpr.device_gp(), spec, terms, S, H, K, ke, iters, mult_mu=mult_mu,
+                              consistent=consistent, angles=self.angle_dims, measurement_noise=noise)
+        plan.set_inputs(x0, eps, xi, nu=nu)
+        plan.launch()
+        b = np.array(c.b, dtype=np.float64)
+        b[:H] = plan.best_b.cpu().numpy()
+        c.b.assign(b)
+        self.cem_plan = plan
         u = self.compute_action(m, t=0)
         c.shift()
         return u
