@@ -970,6 +970,52 @@ size_t pilco_cem_update_workspace_bytes(int K);
 int    pilco_cem_update(const pilco_cem* c, void* ws, size_t ws_bytes, pilco_stream_t stream);
 int    pilco_cem_draw(const pilco_cem* c, pilco_stream_t stream);
 
+/* ---- counter-based normals and the Adam step (DESIGN.md section 32) -----------------------------------------------
+ * pilco_normals: out[0 .. n) standard normals.  Normal i is a pure function of (seed, stream_id, *iter, i): Philox4x32-10
+ * (curand's Philox4_32_10) of the counter (j low 32 bits, j high 32 bits, stream_id, low 32 bits of *iter), j = i / 2,
+ * under the key (seed low 32 bits, seed high 32 bits) gives x0..x3; u1 = (((x0 << 32 | x1) >> 11) + 0.5) 2^-53 and u2
+ * likewise from (x2, x3), both in (0, 1); r = sqrt(-2 log u1), element 2j = r cospi(2 u2), element 2j + 1 =
+ * r sinpi(2 u2).  *iter is read on the device when the kernel runs, so a captured graph draws new normals at every
+ * replay after something advances it (pilco_adam_update does).  The bits depend neither on the grid nor on n (a call's
+ * first n elements are the n call's).  Validation before any work is enqueued: PILCO_ERR_NULL for iter or out NULL,
+ * PILCO_ERR_DIM for n < 0; n = 0 enqueues nothing.  Deterministic, no host synchronisation (graph-capturable).
+ *
+ * pilco_adam_update: one Adam step of R restarts' flat parameters theta [R, n] (row stride ld_theta) from the packed rows
+ * [loss | status | gradient of loss [n]] (row stride ld_packed, read only), then *iter += 1.  For each restart r:
+ *   ok_r = status_r == 0, loss_r finite and every gradient entry finite
+ *   if ok_r:  max_norm > 0 and ||g_r|| > max_norm: g_r <- g_r (max_norm / ||g_r||)   (||.||^2 summed in a fixed order)
+ *             t_r += 1, b1t_r <- b1t_r b1, b2t_r <- b2t_r b2                           (running products b^t, no pow)
+ *             m_r <- b1 m_r + (1 - b1) g_r,  v_r <- b2 v_r + (1 - b2) g_r o g_r
+ *             theta_r <- theta_r - lr (m_r / (1 - b1t_r)) / (sqrt(v_r / (1 - b2t_r)) + eps)
+ *   k = *iter (read before the increment): when 0 <= k < trace_rows, trace[k, r] = -loss_r and ok[k, r] = ok_r
+ * A restart that is not ok keeps theta, m, v, t and its running products; no restart reads another's row.  Every
+ * product, sum, quotient and square root is rounded once (no fma), so a host build of sgd_math.cuh gives the same bits.
+ * Start a run with m = v = 0, t = 0, b1t = b2t = 1.  Validation before any work is enqueued: PILCO_ERR_NULL for a NULL
+ * a, theta, packed, m, v, t, b1t, b2t or iter (trace and ok too when trace_rows > 0), then PILCO_ERR_DIM for R < 1,
+ * n < 1, ld_theta < n, ld_packed < n + 2, trace_rows < 0, lr <= 0 or not finite, b1 or b2 outside [0, 1), eps <= 0
+ * (or NaN) and max_norm < 0 (or NaN).  Deterministic (no atomics), no host synchronisation (graph-capturable). */
+int pilco_normals(unsigned long long seed, unsigned stream_id, const long long* iter, long long n, double* out,
+                  pilco_stream_t stream);
+typedef struct pilco_adam {
+    int R, n;                   /* restarts, parameters per restart */
+    double lr, b1, b2, eps;     /* step size > 0, moment decays in [0, 1), eps > 0 */
+    double max_norm;            /* clip ||g|| to it when > 0; 0: no clipping */
+    double* theta;              /* [R, ld_theta] the parameters, updated in place */
+    int ld_theta;               /* >= n */
+    const double* packed;       /* [R, ld_packed] rows [loss | status | gradient of loss] */
+    int ld_packed;              /* >= n + 2 */
+    double* m;                  /* [R, n] first moments */
+    double* v;                  /* [R, n] second moments */
+    long long* t;               /* [R] steps taken */
+    double* b1t;                /* [R] b1^t */
+    double* b2t;                /* [R] b2^t */
+    long long* iter;            /* [1] the iteration counter k */
+    double* trace;              /* [trace_rows, R] -loss of iteration k */
+    int* ok;                    /* [trace_rows, R] whether iteration k stepped */
+    int trace_rows;             /* >= 0 */
+} pilco_adam;
+int pilco_adam_update(const pilco_adam* a, pilco_stream_t stream);
+
 /* ---- diagnostics ------------------------------------------------------------------------------
  * fp64 pipe microbenchmark used for the roofline denominators (DESIGN.md "Roofline"): which = 0 DFMA,
  * 1 DMMA m8n8k4, 2 both interleaved, 3 table exp, 4 libdevice exp, 5 DMMA m16n8k8, 6 DMMA m16n8k16;

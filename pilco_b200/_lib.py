@@ -118,6 +118,14 @@ class Cem(C.Structure):
                 ("best_value", c_dp), ("best", c_dp), ("trace", c_dp)]
 
 
+class Adam(C.Structure):
+    """mirror of ``pilco_adam``"""
+    _fields_ = [("R", C.c_int), ("n", C.c_int), ("lr", C.c_double), ("b1", C.c_double), ("b2", C.c_double),
+                ("eps", C.c_double), ("max_norm", C.c_double), ("theta", c_dp), ("ld_theta", C.c_int),
+                ("packed", c_dp), ("ld_packed", C.c_int), ("m", c_dp), ("v", c_dp), ("t", c_dp), ("b1t", c_dp),
+                ("b2t", c_dp), ("iter", c_dp), ("trace", c_dp), ("ok", c_dp), ("trace_rows", C.c_int)]
+
+
 MAX_FEATURES = 8192                              # PILCO_MAX_FEATURES
 CEM_MAX_K = 8192                                 # pilco_cem_update's largest K
 POLICY_LINEAR, POLICY_RBF, POLICY_MLP = 0, 1, 2
@@ -338,6 +346,8 @@ SIGNATURES = {
     "pilco_cem_update_workspace_bytes": (C.c_size_t, [C.c_int]),
     "pilco_cem_update": (C.c_int, [C.POINTER(Cem), c_dp, C.c_size_t, c_dp]),
     "pilco_cem_draw": (C.c_int, [C.POINTER(Cem), c_dp]),
+    "pilco_normals": (C.c_int, [C.c_ulonglong, C.c_uint, c_dp, c_ll, c_dp, c_dp]),
+    "pilco_adam_update": (C.c_int, [C.POINTER(Adam), c_dp]),
     "pilco_particles_reward_moments": (C.c_int, [C.POINTER(Particles), C.POINTER(Angles), C.c_int, c_dp, c_dp, c_dp]),
     "pilco_mm_forward_profile": (C.c_int, [C.POINTER(GpModel), C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                            c_dp, C.c_size_t, C.POINTER(C.c_float), c_dp]),

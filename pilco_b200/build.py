@@ -15,7 +15,7 @@ SOURCES = ["abi.cu", "mm_forward.cu", "mm_backward.cu", "mm_tape.cu", "closed_fo
            "rollout_bwd.cu", "rollout_angles_bwd.cu", "rollout_explore.cu", "rollout_noise.cu", "microbench.cu", "predict.cu",
            "particles.cu", "particles_angles.cu", "particles_noise.cu", "particles_explore.cu",
            "particles_cscore.cu", "particles_resample.cu", "particles_mlp.cu", "particles_features.cu",
-           "particles_cem.cu"]
+           "particles_cem.cu", "particles_sgd.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-rdc=false"]

@@ -855,12 +855,13 @@ def _features_check(dyn, num_features):
     return F
 
 
-def feature_draws(dyn, P, F, zeta, w, eps_y):
+def feature_draws(dyn, P, F, zeta, w, eps_y, out=None):
     """pilco_particles_features_draw: P particles' dynamics functions f_pe = phi_e' w_pe + k_e(., X) v_pe drawn from
     the caller's standard normals zeta [E,F,D] (the frequencies, shared by all particles), w [P,E,2F] (the feature
     weights) and eps_y [P,E,n] (the data update's noise), through the exact GP ``dyn`` (``gp_factorize``'s, with its
     sn2) -> ``FeatureDraws``.  ValueError, before any allocation, for a model without sn2 (FITC), F outside
-    1 .. 8192 or a wrong shape."""
+    1 .. 8192 or a wrong shape.  ``out``: an earlier call's draws of the same sizes over the same w tensor, redrawn in
+    place with nothing allocated, so that the call can be captured in a CUDA graph."""
     F = _features_check(dyn, F)
     P, E, n, D = int(P), dyn.E, dyn.n, dyn.D
     for a, shape, what in ((zeta, (E, F, D), "zeta"), (w, (P, E, 2 * F), "w"), (eps_y, (P, E, n), "eps_y")):
@@ -871,13 +872,17 @@ def feature_draws(dyn, P, F, zeta, w, eps_y):
     if wsb == 0:
         raise ValueError("feature_draws: unsupported sizes (P=%d, F=%d, n=%d, D=%d, E=%d)" % (P, F, n, D, E))
     zeta, w, eps_y = dev(zeta).contiguous(), dev(w).contiguous(), dev(eps_y).contiguous()
-    d = device()
-    omega = torch.empty((E, F, D), dtype=F64, device=d)
-    v = torch.empty((P, E, n), dtype=F64, device=d)
-    ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
-    check(lib.pilco_particles_features_draw(C.byref(g), ptr(dyn.sn2), P, F, ptr(zeta), ptr(w), ptr(eps_y), ptr(omega),
-                                            ptr(v), ptr(ws), wsb, stream_ptr()), "particles_features_draw")
-    return FeatureDraws(F, omega, w, v)
+    if out is None:
+        d = device()
+        out = FeatureDraws(F, torch.empty((E, F, D), dtype=F64, device=d), w,
+                           torch.empty((P, E, n), dtype=F64, device=d))
+        out.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+    elif (out.P, out.F, out.E, out.n, out.D) != (P, F, E, n, D) or out.w.data_ptr() != w.data_ptr():
+        raise ValueError("feature_draws: out holds the draws of other sizes or another w")
+    check(lib.pilco_particles_features_draw(C.byref(g), ptr(dyn.sn2), P, F, ptr(zeta), ptr(w), ptr(eps_y),
+                                            ptr(out.omega), ptr(out.v), ptr(out.ws), wsb, stream_ptr()),
+          "particles_features_draw")
+    return out
 
 
 class ParticlePlan:
@@ -1704,6 +1709,84 @@ class CemPlan:
         """(traj [K,P,H+1,E], act [K,P,H,U], step_reward [K,P,H], step_risk [K,P,H], ret [K,P]) of the last population
         rolled out"""
         return self.traj, self.act_buf, self.rew_buf, self.risk_buf, self.ret
+
+
+def _device_tensor(t, dtype, what):
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_cuda or not t.is_contiguous():
+        raise ValueError("%s must be a contiguous %s CUDA tensor" % (what, dtype))
+
+
+def normals(out, seed, stream_id, iter):
+    """pilco_normals (DESIGN.md section 32): fill ``out`` (a contiguous fp64 CUDA tensor) with standard normals, each a
+    pure function of (seed, stream_id, iteration, its index): Philox4x32-10 and Box-Muller.  The iteration is read from
+    ``iter`` (an int64 CUDA tensor of one element) when the kernel runs, so a captured graph draws new normals at every
+    replay once something advances it (``AdamState.step``).  seed is taken modulo 2^64; stream_id must be in
+    0 .. 2^32 - 1.  The first k elements do not depend on out's size.  Returns out; ValueError before any device work
+    for a bad tensor or stream_id."""
+    _device_tensor(out, F64, "normals: out")
+    if not isinstance(iter, torch.Tensor) or iter.dtype != torch.int64 or iter.numel() != 1 or not iter.is_cuda:
+        raise ValueError("normals: iter must be an int64 CUDA tensor of one element")
+    if not 0 <= int(stream_id) < 2 ** 32:
+        raise ValueError("normals: stream_id must be in 0 .. 2^32 - 1, got %d" % int(stream_id))
+    check(lib.pilco_normals(int(seed) % 2 ** 64, int(stream_id), iter.data_ptr(), out.numel(), out.data_ptr(),
+                            stream_ptr()), "normals")
+    return out
+
+
+def adam_hyperparameters(lr, betas, eps, max_norm):
+    """(lr, b1, b2, eps, max_norm) as pilco_adam_update takes them, max_norm None -> 0 (no clipping); ValueError
+    outside its ranges: lr > 0 finite, b1 and b2 in [0, 1), eps > 0, max_norm >= 0"""
+    lr, eps = float(lr), float(eps)
+    b1, b2 = (float(b) for b in betas)
+    max_norm = 0.0 if max_norm is None else float(max_norm)
+    for bad, what in ((not (0.0 < lr < float("inf")), "learning_rate must be finite and > 0"),
+                      (not (0.0 <= b1 < 1.0 and 0.0 <= b2 < 1.0), "betas must be in [0, 1)"),
+                      (not eps > 0.0, "eps must be > 0"), (not max_norm >= 0.0, "max_grad_norm must be >= 0")):
+        if bad:
+            raise ValueError("adam: %s (learning_rate=%r, betas=%r, eps=%r, max_grad_norm=%r)"
+                             % (what, lr, tuple(betas), eps, max_norm))
+    return lr, b1, b2, eps, max_norm
+
+
+class AdamState:
+    """Adam's state for R restarts of n flat parameters on the device (pilco_adam_update, DESIGN.md section 32): the
+    moments ``m``, ``v`` [R,n], the step counts ``t`` [R], the running products ``b1t``, ``b2t`` [R], the iteration
+    counter ``iter`` [1] (int64: ``normals`` reads it), and ``trace`` / ``ok`` [trace_rows,R], iteration k's -loss and
+    whether it stepped.  ``step(theta, packed)`` enqueues one update of theta [R,>=n] from the rows packed [R,>=n+2] =
+    [loss | status | gradient of loss], then advances the counter: no host synchronisation, graph-capturable.
+    ``reset()`` restores the start (zero moments, counts and counter, unit products, a NaN trace).  Hyper-parameters
+    out of range are a ValueError (``adam_hyperparameters``) raised before any allocation."""
+
+    def __init__(self, R, n, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, max_norm=None, trace_rows=0):
+        self.lr, self.b1, self.b2, self.eps, self.max_norm = adam_hyperparameters(lr, betas, eps, max_norm)
+        self.R, self.n, self.trace_rows = int(R), int(n), int(trace_rows)
+        if self.R < 1 or self.n < 1 or self.trace_rows < 0:
+            raise ValueError("AdamState: needs R >= 1, n >= 1 and trace_rows >= 0 (R=%d, n=%d, trace_rows=%d)"
+                             % (self.R, self.n, self.trace_rows))
+        d, R, rows = device(), self.R, max(self.trace_rows, 1)
+        mk = lambda *shape, dtype=F64: torch.zeros(shape, dtype=dtype, device=d)
+        self.m, self.v, self.b1t, self.b2t, self.trace = mk(R, self.n), mk(R, self.n), mk(R), mk(R), mk(rows, R)
+        self.t, self.iter, self.ok = mk(R, dtype=torch.int64), mk(1, dtype=torch.int64), mk(rows, R, dtype=torch.int32)
+        self.reset()
+
+    def reset(self):
+        for z in (self.m, self.v, self.t, self.iter, self.ok):
+            z.zero_()
+        self.b1t.fill_(1.0)
+        self.b2t.fill_(1.0)
+        self.trace.fill_(float("nan"))
+
+    def step(self, theta, packed):
+        for a, w, what in ((theta, self.n, "theta"), (packed, self.n + 2, "packed")):
+            if not isinstance(a, torch.Tensor) or a.dtype != F64 or not a.is_cuda or a.dim() != 2 or \
+                    a.shape[0] != self.R or a.shape[1] < w or a.stride(1) != 1:
+                raise ValueError("AdamState.step: %s must be an fp64 CUDA tensor [%d, >=%d] with unit column stride"
+                                 % (what, self.R, w))
+        a = _lib.Adam(self.R, self.n, self.lr, self.b1, self.b2, self.eps, self.max_norm, theta.data_ptr(),
+                      theta.stride(0), packed.data_ptr(), packed.stride(0), self.m.data_ptr(), self.v.data_ptr(),
+                      self.t.data_ptr(), self.b1t.data_ptr(), self.b2t.data_ptr(), self.iter.data_ptr(),
+                      self.trace.data_ptr(), self.ok.data_ptr(), self.trace_rows)
+        check(lib.pilco_adam_update(C.byref(a), stream_ptr()), "adam_update")
 
 
 class PredictPlan:

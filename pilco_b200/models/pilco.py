@@ -17,6 +17,7 @@ from .smgpr import SMGPR
 
 ParticleTrajectories = collections.namedtuple("ParticleTrajectories", ["states", "actions", "rewards", "risks", "returns"])
 ParticlePolicyGradient = collections.namedtuple("ParticlePolicyGradient", ["value", "grad", "returns"])
+AdamTrace = collections.namedtuple("AdamTrace", ["value", "ok"])
 
 
 def _resample_refusals(what, resample, consistent, estimator="pathwise", exploration=0.0):
@@ -586,7 +587,8 @@ class PILCO:
         return float(plan.reward[0].item()), self._flat_grad({k: v[0] for k, v in g.items()}).view(HostArray)
 
     def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False,
-                                exploration=0.0, resample=False, num_features=None):
+                                exploration=0.0, resample=False, num_features=None, optimizer="lbfgsb",
+                                learning_rate=1e-3, betas=(0.9, 0.999), eps=1e-8, max_grad_norm=None):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -616,9 +618,24 @@ class PILCO:
         ``num_features=F`` with ``consistent=True``: the particles follow random-feature function draws (DESIGN.md
         section 30), made once as ``sample_trajectories(..., num_features=F)`` makes them; a lock-step group's workspace
         is then O(restarts num_samples horizon (D + E)) whatever the model's size.  With ``consistent=False`` or an
-        SMGPR model it is a ValueError."""
+        SMGPR model it is a ValueError.
+
+        ``optimizer="adam"``: stochastic gradient ascent on the expected return instead (Deep PILCO, PIPPS; DESIGN.md
+        section 32).  Each of the ``maxiter`` Adam steps (``learning_rate``, ``betas``, ``eps``, the gradient's norm
+        clipped to ``max_grad_norm`` when given) draws ``num_samples`` fresh particles on the device from a
+        counter-based generator seeded with ``seed``, so the optimiser cannot fit the policy to one sample; the whole
+        run is one CUDA graph per lock-step group replayed ``maxiter`` times.  ``consistent``, ``num_features``,
+        ``resample`` and ``exploration`` mean what they mean above.  Every restart's final policy is then scored on one
+        held-out sample from the same generator; the controller is set to the best, and its held-out value is returned
+        (an out-of-sample estimate).  ``adam_trace`` keeps each step's in-sample values [maxiter, restarts] and whether
+        each restart stepped (a restart whose value or gradient is not finite keeps its parameters).  The refusals
+        above apply, and so do ValueErrors for maxiter < 1 and hyper-parameters out of range (learning_rate finite and
+        > 0, betas in [0, 1), eps > 0, max_grad_norm >= 0), all raised before any device work.  The default
+        optimizer ignores the four Adam arguments."""
         from functools import partial
         from .. import policy_opt
+        if optimizer not in ("lbfgsb", "adam"):
+            raise ValueError("optimize_policy_sampled: optimizer must be 'lbfgsb' or 'adam', not %r" % (optimizer,))
         self._no_schedule("optimize_policy_sampled")
         self._no_angles("optimize_policy_sampled")
         self._no_noise("optimize_policy_sampled")
@@ -638,6 +655,13 @@ class PILCO:
             raise ValueError("optimize_policy_sampled: the reward has box (risk) terms, which carry no pathwise "
                              "gradient; use optimize_policy")
         restarts = max(int(restarts), 1)
+        if optimizer == "adam":
+            if int(maxiter) < 1:
+                raise ValueError("optimize_policy_sampled: optimizer='adam' needs maxiter >= 1 (maxiter=%d)"
+                                 % int(maxiter))
+            engine.adam_hyperparameters(learning_rate, betas, eps, max_grad_norm)
+            return self._optimize_policy_adam(maxiter, restarts, num_samples, seed, consistent, b, resample, F,
+                                              learning_rate, betas, eps, max_grad_norm)
         mgpr_trainable = self.mgpr.trainable_parameters
         for p in mgpr_trainable:
             set_trainable(p, False)
@@ -660,6 +684,29 @@ class PILCO:
         finally:
             for p in mgpr_trainable:
                 set_trainable(p, True)
+        return best_value
+
+    def _optimize_policy_adam(self, maxiter, restarts, num_samples, seed, consistent, b, resample, F, learning_rate,
+                              betas, eps, max_grad_norm):
+        """optimize_policy_sampled(optimizer="adam") after its refusals"""
+        from .. import policy_opt
+        mgpr_trainable = self.mgpr.trainable_parameters
+        for p in mgpr_trainable:
+            set_trainable(p, False)
+        try:
+            flats0 = policy_opt.initial_flats(self.controller, restarts)
+            if seed is None:
+                seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+            best_flat, best_value, _, trace, ok = policy_opt.optimize_stochastic(
+                self, int(maxiter), restarts, int(num_samples), int(seed), consistent=consistent,
+                exploration=None if b == 0.0 else b, resample=resample, num_features=F, lr=learning_rate, betas=betas,
+                eps=eps, max_norm=max_grad_norm, flats0=flats0)
+            self.controller.set_flat(best_flat)
+        finally:
+            for p in mgpr_trainable:
+                set_trainable(p, True)
+        from ..params import HostArray
+        self.adam_trace = AdamTrace(trace.view(HostArray), ok)
         return best_value
 
     def training_loss(self):

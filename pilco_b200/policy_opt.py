@@ -144,6 +144,24 @@ class _FlatEvaluator:
         engine.gp_refactorize(gp)
         return th
 
+    def _particle_plan(self, P, consistent, exploration, resample, num_features, measurement_noise=None):
+        """self.plan, the batched pathwise-gradient plan of the R restarts over P particles (``ConsistentGradPlan``
+        with ``consistent``, else ``ParticlePlan``), and self.gp, the RBF policy it refactorises (None otherwise)"""
+        pilco, c, flat0 = self.pilco, self.c, self.flat0
+        terms, mult_mu = pilco.reward_spec()
+        spec = c.policy_spec(flat0) if self.linear or self.mlp else pilco.policy_spec(flat0)
+        self.gp = None if self.linear or self.mlp else spec["gp"]
+        if consistent:
+            self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, P, int(pilco.horizon),
+                                                  mult_mu=mult_mu, R=self.R, exploration=exploration,
+                                                  measurement_noise=measurement_noise, schedule=self.sched,
+                                                  num_features=num_features)
+        else:
+            self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, P, int(pilco.horizon),
+                                            mult_mu=mult_mu, grad=True, R=self.R, exploration=exploration,
+                                            measurement_noise=measurement_noise, resample=resample,
+                                            schedule=self.sched, num_features=num_features)
+
     def _pack(self, out, value, info, g, th):
         """out [R,P+2] = [-value | status | -gradient in the flat layout]; the lengthscale block goes through the
         softplus: d ell / d theta = sigmoid(theta)"""
@@ -249,25 +267,11 @@ class ParticleEvaluator(_FlatEvaluator):
     section 30) and eps is not read (None)."""
 
     def __init__(self, pilco, R, x0, eps, consistent=False, exploration=None, resample=False, xi=None, features=None):
-        terms, mult_mu = pilco.reward_spec()
-        if any(t["kind"] == _lib.REWARD_BOX for t in terms):
-            raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
-                             "almost everywhere, so optimising it would ignore the constraint")
+        _no_box(pilco)
         super().__init__(pilco, R)
-        c, flat0 = self.c, self.flat0
-        spec = c.policy_spec(flat0) if self.linear or self.mlp else pilco.policy_spec(flat0)
-        self.gp = None if self.linear or self.mlp else spec["gp"]
         x0 = engine.dev(x0)
-        if consistent:
-            self.plan = engine.ConsistentGradPlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]),
-                                                  int(pilco.horizon), mult_mu=mult_mu, R=R, exploration=exploration,
-                                                  schedule=self.sched,
-                                                  num_features=None if features is None else features.F)
-        else:
-            self.plan = engine.ParticlePlan(pilco.mgpr.device_gp(), spec, terms, int(x0.shape[0]), int(pilco.horizon),
-                                            mult_mu=mult_mu, grad=True, R=R, exploration=exploration,
-                                            resample=resample, schedule=self.sched,
-                                            num_features=None if features is None else features.F)
+        self._particle_plan(int(x0.shape[0]), consistent, exploration, resample,
+                            None if features is None else features.F)
         self.plan.set_inputs(x0, eps, xi=xi, features=features)
         self._setup_io()
 
@@ -278,6 +282,168 @@ class ParticleEvaluator(_FlatEvaluator):
         info = self.gp.info if self.gp is not None else torch.zeros_like(g["value"])
         self._pack(self.d_out, g["value"].reshape(self.R), info.reshape(self.R), g, th)
         self.h_out.copy_(self.d_out, non_blocking=True)
+
+
+class StochasticEvaluator(_FlatEvaluator):
+    """One lock-step group of R restarts trained by Adam on particles drawn afresh at every iteration (DESIGN.md
+    section 32): the objective is the expected return itself, not one fixed sample of it (Deep PILCO, PIPPS).
+
+    The plan is the one ``ParticleEvaluator`` builds for the same arguments (``consistent``, ``exploration``,
+    ``resample``, ``num_features``; also ``measurement_noise``).  ``iteration()`` enqueues, on the current stream and
+    without host synchronisation:
+      1. the draws, each with ``engine.normals`` into a persistent buffer at the counter ``adam.iter``, under its stream
+         id: 0 eps0 [P,Ds] (then x0 = m0 + eps0 F', F = the factor of S0 the class's particle methods use), 1 eps
+         [P,H,Ds] (not with features), 2 nu (with measurement noise), 3 xi (with ``resample``), 4, 5, 6 zeta, w, eps_y
+         and the feature draws (with ``num_features``);
+      2. ``_unpack`` of the device parameters ``theta`` [R,n], the plan's ``launch_grad``, ``_pack`` into ``packed``
+         [R,n+2];
+      3. ``adam.step(theta, packed)``, which advances the counter.
+    ``capture()`` runs one eager iteration (warm-up), restores the start and records one iteration as a CUDA graph that
+    ``replay()`` runs.  ``held_out()`` returns each restart's value at the current theta on the held-out sample, the
+    same draws under stream ids 16 + j at iteration 0."""
+
+    HELD_OUT = 16
+
+    def __init__(self, pilco, R, flats0, num_samples, seed, m0, F0, consistent=False, exploration=None, resample=False,
+                 num_features=None, measurement_noise=None, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, max_norm=None,
+                 trace_rows=0):
+        _no_box(pilco)
+        engine.adam_hyperparameters(lr, betas, eps, max_norm)
+        super().__init__(pilco, R)
+        P, self.seed = int(num_samples), int(seed)
+        self._particle_plan(P, consistent, exploration, resample, num_features, measurement_noise)
+        p, d = self.plan, engine.device()
+        mk = lambda *shape: torch.zeros(shape, dtype=torch.float64, device=d)
+        self.flats0 = engine.dev(np.asarray(flats0, dtype=np.float64).reshape(R, self.P))
+        self.theta, self.packed = self.flats0.clone(), mk(R, self.P + 2)
+        self.adam = engine.AdamState(R, self.P, lr, betas, eps, max_norm, trace_rows)
+        self.zero = torch.zeros(1, dtype=torch.int64, device=d)            # the held-out sample's iteration
+        self.m0, self.Ft = engine.dev(m0)[None], engine.dev(F0).T
+        self.eps0 = mk(P, p.Ds)
+        self.draws = None
+        if num_features is not None:
+            dyn = pilco.mgpr.device_gp()
+            self.feat = (mk(dyn.E, int(num_features), dyn.D), mk(P, dyn.E, 2 * int(num_features)), mk(P, dyn.E, dyn.n))
+            self.draws = engine.feature_draws(dyn, P, num_features, *self.feat)
+            p.set_inputs(p.x0, None, nu=p.nu_buf if p.nz is not None else None, features=self.draws)
+        self.graph, self.stream = None, torch.cuda.Stream()
+
+    def _draw(self, it, base):
+        """the draws of one iteration at the counter ``it``, under stream ids base + 0 .. 6"""
+        p, s = self.plan, self.seed
+        engine.normals(self.eps0, s, base, it)
+        p.x0.copy_(self.m0 + self.eps0 @ self.Ft)
+        if p.H > 0:
+            if self.draws is not None:
+                for j, buf in enumerate(self.feat):
+                    engine.normals(buf, s, base + 4 + j, it)
+                engine.feature_draws(self.pilco.mgpr.device_gp(), p.P, self.draws.F, *self.feat, out=self.draws)
+            else:
+                engine.normals(p.eps_buf, s, base + 1, it)
+            if p.nz is not None:
+                engine.normals(p.nu_buf, s, base + 2, it)
+            if p.resample:
+                engine.normals(p.xi_buf, s, base + 3, it)
+
+    def _evaluate(self, it, base):
+        """the draws at ``it``, then the pathwise gradient of every restart at theta, packed -> value [R]"""
+        self._draw(it, base)
+        th = self._unpack(self.theta, self.plan, self.gp)
+        g = self.plan.launch_grad()
+        info = self.gp.info if self.gp is not None else torch.zeros_like(g["value"])
+        self._pack(self.packed, g["value"].reshape(self.R), info.reshape(self.R), g, th)
+        return g["value"].reshape(self.R)
+
+    def iteration(self):
+        self._evaluate(self.adam.iter, 0)
+        self.adam.step(self.theta, self.packed)
+
+    def restart(self):
+        """theta back to the starting points and Adam's state to its start"""
+        self.theta.copy_(self.flats0)
+        self.adam.reset()
+
+    def capture(self):
+        self.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.stream):
+            self.iteration()
+            self.restart()
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.iteration()
+        self.graph = g
+
+    def replay(self):
+        with torch.cuda.stream(self.stream):
+            self.graph.replay()
+
+    def held_out(self):
+        """-> value [R] (device) of the current theta on the held-out sample, enqueued on the group's stream"""
+        cur = torch.cuda.current_stream()
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            value = self._evaluate(self.zero, self.HELD_OUT).clone()
+        cur.wait_stream(self.stream)
+        return value
+
+
+def optimize_stochastic(pilco, maxiter, restarts, num_samples, seed, consistent=False, exploration=None,
+                        resample=False, num_features=None, measurement_noise=None, lr=1e-3, betas=(0.9, 0.999),
+                        eps=1e-8, max_norm=None, flats0=None, m0=None, S0=None):
+    """Adam on the sampled return with fresh particles at every step (DESIGN.md section 32).  The restarts start from
+    ``flats0`` (default ``initial_flats``), are sharded over ranks with ``shard_restarts`` and dealt to lock-step groups
+    (``StochasticEvaluator``), each of which captures one iteration as a CUDA graph and replays it ``maxiter`` times
+    with no host synchronisation until the end.  Every restart's final parameters are then scored once on the common
+    held-out sample, and the winner is picked by ``gather_table`` + ``select_best`` on [-held-out value | theta].
+    ``m0``, ``S0``: the initial state distribution (default pilco.m_init, pilco.S_init).
+    Returns (best_flat, best held-out value, per-restart held-out values, trace [maxiter, restarts] of the in-sample
+    values, ok [maxiter, restarts]); the trace's columns of restarts on other ranks are NaN (ok False)."""
+    from .models.pilco import _sqrt_factor
+    maxiter, restarts = int(maxiter), max(int(restarts), 1)
+    if maxiter < 1:
+        raise ValueError("optimize_stochastic: needs maxiter >= 1 (maxiter=%d)" % maxiter)
+    engine.adam_hyperparameters(lr, betas, eps, max_norm)
+    dist, rank, world = _dist()
+    flats0 = initial_flats(pilco.controller, restarts) if flats0 is None else np.asarray(flats0, dtype=np.float64)
+    m0 = np.asarray(pilco.m_init if m0 is None else m0, dtype=np.float64).reshape(-1)
+    S0 = np.asarray(pilco.S_init if S0 is None else S0, dtype=np.float64).reshape(m0.size, m0.size)
+    F0 = _sqrt_factor(S0)
+    mine = shard_restarts(restarts, rank, world)
+    P = flats0.shape[1]
+    local = np.full((restarts, 1 + P), np.nan)
+    trace, ok = np.full((maxiter, restarts), np.nan), np.zeros((maxiter, restarts), dtype=bool)
+    if mine:
+        bounds = group_bounds(len(mine))
+        evs = [StochasticEvaluator(pilco, hi - lo, flats0[mine][lo:hi], num_samples, seed, m0, F0,
+                                   consistent=consistent, exploration=exploration, resample=resample,
+                                   num_features=num_features, measurement_noise=measurement_noise, lr=lr, betas=betas,
+                                   eps=eps, max_norm=max_norm, trace_rows=maxiter) for lo, hi in bounds]
+        for ev in evs:
+            ev.capture()
+        for _ in range(maxiter):
+            for ev in evs:
+                ev.replay()
+        values = [ev.held_out() for ev in evs]
+        torch.cuda.synchronize()
+        cols = np.asarray(mine)
+        for ev, (lo, hi), v in zip(evs, bounds, values):
+            local[cols[lo:hi], 0] = -v.cpu().numpy()
+            local[cols[lo:hi], 1:] = ev.theta.cpu().numpy()
+            trace[:, cols[lo:hi]] = ev.adam.trace.cpu().numpy()
+            ok[:, cols[lo:hi]] = ev.adam.ok.cpu().numpy() != 0
+        LAST_STATS.update(evals=maxiter, restarts_local=len(mine), horizon=int(pilco.horizon), groups=len(evs),
+                          rollout_steps=maxiter * len(mine) * int(pilco.horizon))
+    local = gather_table(local, restarts, rank, world, dist)
+    best = select_best(local)
+    return local[best, 1:], -float(local[best, 0]), [-float(v) for v in local[:, 0]], trace, ok
+
+
+def _no_box(pilco):
+    terms, _ = pilco.reward_spec()
+    if any(t["kind"] == _lib.REWARD_BOX for t in terms):
+        raise ValueError("the sampled return's pathwise gradient ignores box (risk) terms: their indicator is flat "
+                         "almost everywhere, so optimising it would ignore the constraint")
 
 
 class LockstepLBFGS:
