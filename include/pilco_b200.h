@@ -970,6 +970,36 @@ size_t pilco_cem_update_workspace_bytes(int K);
 int    pilco_cem_update(const pilco_cem* c, void* ws, size_t ws_bytes, pilco_stream_t stream);
 int    pilco_cem_draw(const pilco_cem* c, pilco_stream_t stream);
 
+/* ---- batched forward-only rollouts of stationary policies (DESIGN.md section 33) ------------------------------------
+ * pilco_particles_batch_rollout / _consistent_batch_rollout: the forward of pilco_particles_explore_batch_grad_rollout /
+ * _explore_consistent_grad_rollout (ex NULL) without the reverse sweep or its histories, for a linear or RBF policy.
+ * pilco_particles_mlp_batch_rollout / _mlp_consistent_batch_rollout: the same of pilco_particles_mlp_batch_grad_rollout
+ * / _mlp_consistent_grad_rollout (ex NULL) for a tanh MLP policy (no angles or noise, as every MLP call).  R restarts
+ * share x0, eps (and nu); restart r reads its policy at the batch strides (linear W_bs, b_bs; RBF the batched policy
+ * model's strides; MLP theta_bs).  The outputs have a leading R as in the gradient calls, and value [R] is the
+ * fixed-order mean return of the gradient calls' value CTA.  Outputs and value are bitwise the gradient call's; restart
+ * r is bitwise the single forward call (pilco_particles_noisy_rollout / _noisy_consistent_rollout,
+ * pilco_particles_mlp_rollout / _mlp_consistent_rollout) with restart r's policy.  ang and nz may be NULL.  The
+ * workspace is pr->ws; the step-wise sampler's does not grow with H.  Validation before any work is enqueued: the
+ * gradient call's codes with PILCO_ERR_NULL for value NULL in place of its gradient-output checks, then the workspace's
+ * codes.  A size query returns 0 exactly where its call fails on sizes.  Deterministic, no host synchronisation
+ * (graph-capturable). */
+size_t pilco_particles_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, int R);
+int    pilco_particles_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                     const pilco_particles_noise* nz, int R, double* value, pilco_stream_t stream);
+size_t pilco_particles_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R);
+int    pilco_particles_consistent_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                                const pilco_particles_noise* nz, int R, double* value,
+                                                pilco_stream_t stream);
+size_t pilco_particles_mlp_batch_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp, int R);
+int    pilco_particles_mlp_batch_rollout(const pilco_particles* pr, const pilco_mlp* mlp, int R, double* value,
+                                         pilco_stream_t stream);
+size_t pilco_particles_mlp_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp, int R);
+int    pilco_particles_mlp_consistent_batch_rollout(const pilco_particles* pr, const pilco_mlp* mlp, int R,
+                                                    double* value, pilco_stream_t stream);
+
 /* ---- counter-based normals and the Adam step (DESIGN.md section 32) -----------------------------------------------
  * pilco_normals: out[0 .. n) standard normals.  Normal i is a pure function of (seed, stream_id, *iter, i): Philox4x32-10
  * (curand's Philox4_32_10) of the counter (j low 32 bits, j high 32 bits, stream_id, low 32 bits of *iter), j = i / 2,

@@ -343,6 +343,16 @@ SIGNATURES = {
                                                                                        C.c_int]),
     "pilco_particles_scheduled_consistent_batch_rollout": (C.c_int, _PAN + [C.POINTER(PolicySchedule), C.c_int, c_dp,
                                                                             c_dp]),
+    "pilco_particles_batch_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_batch_rollout": (C.c_int, _PAN + [C.c_int, c_dp, c_dp]),
+    "pilco_particles_consistent_batch_workspace_bytes": (C.c_size_t, _PAN + [C.c_int]),
+    "pilco_particles_consistent_batch_rollout": (C.c_int, _PAN + [C.c_int, c_dp, c_dp]),
+    "pilco_particles_mlp_batch_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp), C.c_int]),
+    "pilco_particles_mlp_batch_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), C.c_int, c_dp, c_dp]),
+    "pilco_particles_mlp_consistent_batch_workspace_bytes": (C.c_size_t, [C.POINTER(Particles), C.POINTER(Mlp),
+                                                                          C.c_int]),
+    "pilco_particles_mlp_consistent_batch_rollout": (C.c_int, [C.POINTER(Particles), C.POINTER(Mlp), C.c_int, c_dp,
+                                                               c_dp]),
     "pilco_cem_update_workspace_bytes": (C.c_size_t, [C.c_int]),
     "pilco_cem_update": (C.c_int, [C.POINTER(Cem), c_dp, C.c_size_t, c_dp]),
     "pilco_cem_draw": (C.c_int, [C.POINTER(Cem), c_dp]),

@@ -2036,6 +2036,33 @@ int pilco_particles_scheduled_consistent_batch_rollout(const pilco_particles* pr
     return pt_call(o, pr, ang, nz, nullptr, R, nullptr, stream, nullptr, sch);
 }
 
+// batched forward-only rollouts of stationary policies (DESIGN.md section 33): the explore gradient calls' forward
+// (ex NULL) without their histories; the same options as section 31's with no schedule
+size_t pilco_particles_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, int R) {
+    return pt_query(BFWD, pr, ang, nz, nullptr, R);
+}
+
+int pilco_particles_batch_rollout(const pilco_particles* pr, const pilco_angles* ang, const pilco_particles_noise* nz,
+                                  int R, double* value, pilco_stream_t stream) {
+    PtOpt o = BFWD;
+    o.value = value;
+    return pt_call(o, pr, ang, nz, nullptr, R, nullptr, stream);
+}
+
+size_t pilco_particles_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
+                                                        const pilco_particles_noise* nz, int R) {
+    return pt_query(CBFWD, pr, ang, nz, nullptr, R);
+}
+
+int pilco_particles_consistent_batch_rollout(const pilco_particles* pr, const pilco_angles* ang,
+                                             const pilco_particles_noise* nz, int R, double* value,
+                                             pilco_stream_t stream) {
+    PtOpt o = CBFWD;
+    o.value = value;
+    return pt_call(o, pr, ang, nz, nullptr, R, nullptr, stream);
+}
+
 size_t pilco_particles_scheduled_consistent_grad_workspace_bytes(const pilco_particles* pr, const pilco_angles* ang,
                                                                  const pilco_particles_noise* nz,
                                                                  const pilco_exploration* ex,
@@ -2161,6 +2188,29 @@ int pilco_particles_mlp_resampled_grad_rollout(const pilco_particles* pr, const 
                                                const pilco_particles_resample* rs, int R,
                                                const pilco_particles_grad* g, pilco_stream_t stream) {
     return pt_call(pm_opt(RPATH), pr, nullptr, nullptr, nullptr, R, g, stream, rs, nullptr, mlp);
+}
+
+// batched forward-only MLP rollouts (DESIGN.md section 33): the MLP gradient calls' forward (ex NULL)
+size_t pilco_particles_mlp_batch_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp, int R) {
+    return pt_query(pm_opt(BFWD), pr, nullptr, nullptr, nullptr, R, nullptr, mlp);
+}
+
+int pilco_particles_mlp_batch_rollout(const pilco_particles* pr, const pilco_mlp* mlp, int R, double* value,
+                                      pilco_stream_t stream) {
+    PtOpt o = pm_opt(BFWD);
+    o.value = value;
+    return pt_call(o, pr, nullptr, nullptr, nullptr, R, nullptr, stream, nullptr, nullptr, mlp);
+}
+
+size_t pilco_particles_mlp_consistent_batch_workspace_bytes(const pilco_particles* pr, const pilco_mlp* mlp, int R) {
+    return pt_query(pm_opt(CBFWD), pr, nullptr, nullptr, nullptr, R, nullptr, mlp);
+}
+
+int pilco_particles_mlp_consistent_batch_rollout(const pilco_particles* pr, const pilco_mlp* mlp, int R, double* value,
+                                                 pilco_stream_t stream) {
+    PtOpt o = pm_opt(CBFWD);
+    o.value = value;
+    return pt_call(o, pr, nullptr, nullptr, nullptr, R, nullptr, stream, nullptr, nullptr, mlp);
 }
 
 // function samples from random-feature draws (DESIGN.md section 30); the draw call is in particles_features.cu

@@ -1711,6 +1711,176 @@ class CemPlan:
         return self.traj, self.act_buf, self.rew_buf, self.risk_buf, self.ret
 
 
+# the batched forward-only rollouts of stationary policies (DESIGN.md section 33) per (MLP, consistent): (rollout, size
+# query) after "pilco_particles_"
+PARTICLE_STATIONARY_BATCH_CALLS = {
+    (False, False): ("batch_rollout", "batch_workspace_bytes"),
+    (False, True): ("consistent_batch_rollout", "consistent_batch_workspace_bytes"),
+    (True, False): ("mlp_batch_rollout", "mlp_batch_workspace_bytes"),
+    (True, True): ("mlp_consistent_batch_rollout", "mlp_consistent_batch_workspace_bytes"),
+}
+
+
+class ParticleBatchPlan:
+    """R stationary policies rolled out forward only over the same P particles (DESIGN.md section 33): the value of
+    each, without the reverse sweep or its histories, for the cross-entropy method over policy parameters
+    (``policy_opt.CemPolicySearch``).
+
+    ``spec`` is a linear (W [R,U,Ds], b [R,U]), RBF (``gp`` factorised with a leading R) or tanh MLP (theta
+    [R,n_theta]) policy spec, as ``ParticlePlan`` takes for a batch.  The plan owns x0 [P,E], eps [P,H,E] and, with
+    ``measurement_noise``, nu [P,H,E], shared by the R policies and filled by ``set_inputs``; and the policies' device
+    buffers under the names ``policy_opt``'s flat-row unpacking writes: ``W`` and ``b``, ``theta``, or the batched
+    RBF model ``rbf``.  ``launch()`` enqueues the R rollouts (pilco_particles_batch_rollout, _consistent_batch_rollout
+    with ``consistent=True``, or their MLP calls) with no host synchronisation, and returns ``value`` [R], each
+    policy's mean return.
+
+    The policies run in chunks of ``chunk`` whose workspace plus their trajectory buffers fit ``max_ws_bytes`` (default:
+    half the free device memory); those buffers are the chunk's and are reused, so memory does not grow with R.  The
+    restarts are independent, so the chunking changes no bit.  ``outputs()`` are the last chunk's rollouts;
+    ``bytes_needed(r)`` is what a chunk of r policies needs.
+
+    ``angles`` and ``measurement_noise``: as ``ParticlePlan``, for linear and RBF policies.  A scheduled spec, an MLP
+    with angles or noise, ``num_features``, ``resample``, ``exploration``, a spec of the wrong shape, or R, P or H below 1
+    is a ValueError raised before any allocation."""
+
+    def __init__(self, dyn, spec, reward_terms, P, H, R, mult_mu=0.0, consistent=False, angles=None,
+                 measurement_noise=None, max_ws_bytes=None, num_features=None, resample=False, exploration=None):
+        P, H, R = int(P), int(H), int(R)
+        if R < 1 or P < 1 or H < 1:
+            raise ValueError("ParticleBatchPlan: needs R >= 1, P >= 1 and H >= 1 (R=%d, P=%d, H=%d)" % (R, P, H))
+        if isinstance(spec, dict) and spec.get("schedule", False):
+            raise ValueError("ParticleBatchPlan: the policies are stationary; a time-varying linear policy (a schedule) "
+                             "runs in engine.CemPlan")
+        for on, what in ((num_features is not None, "num_features (the feature sampler)"),
+                         (bool(resample), "resample=True"), (exploration is not None, "exploration")):
+            if on:
+                raise ValueError("ParticleBatchPlan: the batched forward rollout does not combine with %s" % what)
+        mlp = _particle_mlp(spec, "ParticleBatchPlan", R, angles, measurement_noise)
+        E = int(dyn.struct().E)
+        Ds, U = int(spec["Ds"]), int(spec["U"])
+        ang = angles_struct(angles, E) if angles is not None and len(angles) > 0 else None
+        if Ds != E + (ang.A if ang is not None else 0):
+            raise ValueError("ParticleBatchPlan: the policy must take %d inputs (the state%s), got %d"
+                             % (E + (ang.A if ang is not None else 0), " with its angles" if ang is not None else "", Ds))
+        kind = spec["kind"]
+        if kind == _lib.POLICY_LINEAR:
+            if np.shape(spec["W"]) != (R, U, Ds) or np.shape(spec["b"]) != (R, U):
+                raise ValueError("ParticleBatchPlan: expected W [R,U,Ds] = %s and b [R,U] = %s, got %s and %s"
+                                 % ((R, U, Ds), (R, U), np.shape(spec["W"]), np.shape(spec["b"])))
+        elif kind == _lib.POLICY_RBF:
+            g = spec["gp"]
+            if not g.batched or tuple(g.X.shape[:1]) != (R,) or g.D != Ds or g.E != U:
+                raise ValueError("ParticleBatchPlan: the RBF policy must be factorised with a leading R=%d, Ds=%d "
+                                 "inputs and U=%d outputs" % (R, Ds, U))
+        elif mlp is None:
+            raise ValueError("ParticleBatchPlan: unknown policy kind %r" % (kind,))
+        nz_var = _particle_noise(measurement_noise, E)
+        if len(reward_terms) > 8:
+            raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
+        self.P, self.H, self.R, self.E, self.Ds, self.U = P, H, R, E, Ds, U
+        self.consistent, self.ang, self.keep = bool(consistent), ang, [dyn, spec, reward_terms]
+        pr = _lib.Particles()
+        pr.P, pr.H = P, H
+        pr.dyn = dyn.struct()
+        pr.pol.kind, pr.pol.Ds, pr.pol.U = kind, Ds, U                   # what the size queries read
+        self.mlp = None
+        if mlp is not None:
+            L, hidden, self.n_theta, _ = mlp
+            self.mlp = _lib.Mlp(L, (C.c_int * 2)(hidden[0], hidden[-1] if L == 2 else 0), None, self.n_theta, None)
+        elif kind == _lib.POLICY_RBF:
+            pr.pol.rbf = spec["gp"].struct()
+        self.nz = None
+        if nz_var is not None:
+            self.nz = _lib.ParticlesNoise()
+            for i, v in enumerate(nz_var):
+                self.nz.v.var[i] = float(v)
+        names = PARTICLE_STATIONARY_BATCH_CALLS[mlp is not None, self.consistent]
+        self._roll = getattr(lib, "pilco_particles_" + names[0])
+        qz = None                                               # the sizes' noise: nu is checked, not read
+        if self.nz is not None:
+            qz = _lib.ParticlesNoise.from_buffer_copy(self.nz)
+            qz.nu = 16
+        if self.mlp is not None:
+            query = lambda r: int(getattr(lib, "pilco_particles_" + names[1])(C.byref(pr), C.byref(self.mlp), int(r)))
+        else:
+            query = lambda r: int(getattr(lib, "pilco_particles_" + names[1])(
+                C.byref(pr), self._ang_ref(), C.byref(qz) if qz is not None else None, int(r)))
+        if query(1) == 0:
+            raise ValueError("ParticleBatchPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, pr.dyn.D))
+        per = 8 * P * ((H + 1) * E + H * U + 2 * H + 1)          # one restart's trajectory buffers, in bytes
+        need = lambda r: query(r) + r * per
+        if max_ws_bytes is None:
+            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+        fits = lambda r: 0 < query(r) and need(r) <= max_ws_bytes
+        if not fits(1):
+            raise ValueError("ParticleBatchPlan: the rollout of one policy (P=%d, H=%d, n=%d) needs %d bytes, more than "
+                             "max_ws_bytes=%d" % (P, H, pr.dyn.n, need(1), max_ws_bytes))
+        Rc = _largest_fitting(fits, 1, R)
+        self.bytes_needed = need
+        self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, spec, batched=True)
+        if self.mlp is not None:
+            self.theta = dev(spec["theta"]).reshape(R, self.n_theta)
+        self.rw = _fill_rewards(pr, reward_terms)
+        pr.mult_mu = float(mult_mu)
+        d = device()
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
+        self.x0, self.eps_buf = mk(P, E), mk(P, H, E)           # shared by the policies
+        self.traj, self.act_buf = mk(Rc, P, H + 1, E), mk(Rc, P, H, U)
+        self.rew_buf, self.risk_buf, self.ret, self.value = mk(Rc, P, H), mk(Rc, P, H), mk(Rc, P), mk(R)
+        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
+        pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
+        pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
+        if self.nz is not None:
+            self.nu_buf = mk(P, H, E)
+            self.nz.nu = self.nu_buf.data_ptr()
+        wsb = query(Rc)
+        self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+        pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        self.pr, self.chunk, self.chunks = pr, Rc, []           # (description, MLP, R, value) of each chunk
+        for r0 in range(0, R, Rc):
+            c, m = _lib.Particles.from_buffer_copy(pr), None
+            if self.mlp is not None:
+                m = _lib.Mlp.from_buffer_copy(self.mlp)
+                m.theta = self.theta[r0].data_ptr()
+            elif kind == _lib.POLICY_LINEAR:
+                c.pol.W, c.pol.b = self.W[r0].data_ptr(), self.b[r0].data_ptr()
+            else:
+                g = self.rbf
+                c.pol.rbf.X, c.pol.rbf.ell = g.X[r0].data_ptr(), g.ell[r0].data_ptr()
+                c.pol.rbf.sf2, c.pol.rbf.beta = g.sf2[r0].data_ptr(), g.beta[r0].data_ptr()
+            self.chunks.append((c, m, min(Rc, R - r0), self.value[r0].data_ptr()))
+
+    def _ang_ref(self):
+        return C.byref(self.ang) if self.ang is not None else None
+
+    def _nz_ref(self):
+        return C.byref(self.nz) if self.nz is not None else None
+
+    def set_inputs(self, x0, eps, nu=None):
+        """x0 [P,E], eps [P,H,E] and, with measurement noise, nu [P,H,E] (required then, and only then)"""
+        if (nu is None) != (self.nz is None):
+            raise ValueError("ParticleBatchPlan: nu [P,H,E] is required with measurement_noise and only then")
+        self.x0.copy_(dev(x0).reshape(self.P, self.E))
+        self.eps_buf.copy_(dev(eps).reshape(self.eps_buf.shape))
+        if nu is not None:
+            self.nu_buf.copy_(dev(nu).reshape(self.nu_buf.shape))
+
+    def launch(self):
+        """the R rollouts on the current stream, chunk by chunk: no host synchronisation -> value [R]"""
+        for c, m, R, value in self.chunks:
+            if m is not None:
+                rc = self._roll(C.byref(c), C.byref(m), R, value, stream_ptr())
+            else:
+                rc = self._roll(C.byref(c), self._ang_ref(), self._nz_ref(), R, value, stream_ptr())
+            check(rc, "particles_batch_rollout")
+        return self.value
+
+    def outputs(self):
+        """(traj [Rc,P,H+1,E], act [Rc,P,H,U], step_reward [Rc,P,H], step_risk [Rc,P,H], ret [Rc,P]) of the last chunk
+        rolled out (Rc = ``chunk``; the first R - r0 rows of a shorter last chunk)"""
+        return self.traj, self.act_buf, self.rew_buf, self.risk_buf, self.ret
+
+
 def _device_tensor(t, dtype, what):
     if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_cuda or not t.is_contiguous():
         raise ValueError("%s must be a contiguous %s CUDA tensor" % (what, dtype))

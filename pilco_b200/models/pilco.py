@@ -588,7 +588,8 @@ class PILCO:
 
     def optimize_policy_sampled(self, maxiter=50, restarts=1, num_samples=1000, seed=None, consistent=False,
                                 exploration=0.0, resample=False, num_features=None, optimizer="lbfgsb",
-                                learning_rate=1e-3, betas=(0.9, 0.999), eps=1e-8, max_grad_norm=None):
+                                learning_rate=1e-3, betas=(0.9, 0.999), eps=1e-8, max_grad_norm=None, population=400,
+                                elites=40, cem_std=0.5):
         """Optimise the policy on the sampled return instead of the moment-matching reward (Deep PILCO, PIPPS): the
         objective is the mean return of ``num_samples`` particle rollouts of the learnt dynamics from N(m_init, S_init)
         over ``horizon`` steps, with x0 and the step normals drawn once, exactly as ``sample_trajectories`` and
@@ -631,11 +632,31 @@ class PILCO:
         each restart stepped (a restart whose value or gradient is not finite keeps its parameters).  The refusals
         above apply, and so do ValueErrors for maxiter < 1 and hyper-parameters out of range (learning_rate finite and
         > 0, betas in [0, 1), eps > 0, max_grad_norm >= 0), all raised before any device work.  The default
-        optimizer ignores the four Adam arguments."""
+        optimizer ignores the four Adam arguments.
+
+        ``optimizer="cem"``: the cross-entropy method over the flat policy vector on the same in-sample objective,
+        every iteration on the device (``policy_opt.CemPolicySearch``, DESIGN.md section 33).  ``maxiter`` is its
+        iteration count; each iteration rolls out ``population`` candidate policies over the fixed particles and
+        refits a diagonal Gaussian to the ``elites`` best.  The search starts at the controller's current vector with
+        std ``cem_std`` (a scalar or one value per parameter, finite and > 0); ``restarts`` must be 1 (the population
+        is the search).  The seeded generator draws x0 and the step normals exactly as the default optimizer does (the
+        same particles for the same seed), then the measurement noise's normals; the candidates' normals come from the
+        counter-based generator under the same seed.  Only forward values are needed, so box terms, SafePILCO's risk
+        channel, ``consistent``, and with linear and RBF controllers ``angle_dims`` and ``measurement_noise`` all work.
+        The controller is set to the best candidate, whose in-sample value is returned (biased upwards, as the default
+        optimizer's), and ``cem_search`` keeps the search (``trace`` [maxiter, 2] of each iteration's top value and
+        elites' mean value, ``best_value``, ``mean``, ``std``).  A TimeVaryingLinearController (use ``plan``), an
+        MlpController with angles or measurement noise, exploration b != 0, ``resample``, ``num_features``, restarts
+        != 1, population outside 1 .. 8192, elites outside 1 .. population, maxiter < 1 or a bad ``cem_std`` is a
+        ValueError raised before any device work."""
         from functools import partial
         from .. import policy_opt
+        if optimizer == "cem":
+            return self._optimize_policy_cem(maxiter, restarts, num_samples, seed, consistent, exploration, resample,
+                                             num_features, population, elites, cem_std)
         if optimizer not in ("lbfgsb", "adam"):
-            raise ValueError("optimize_policy_sampled: optimizer must be 'lbfgsb' or 'adam', not %r" % (optimizer,))
+            raise ValueError("optimize_policy_sampled: optimizer must be 'lbfgsb', 'adam' or 'cem', not %r"
+                             % (optimizer,))
         self._no_schedule("optimize_policy_sampled")
         self._no_angles("optimize_policy_sampled")
         self._no_noise("optimize_policy_sampled")
@@ -708,6 +729,54 @@ class PILCO:
         from ..params import HostArray
         self.adam_trace = AdamTrace(trace.view(HostArray), ok)
         return best_value
+
+    def _optimize_policy_cem(self, maxiter, restarts, num_samples, seed, consistent, exploration, resample,
+                             num_features, population, elites, cem_std):
+        """optimize_policy_sampled(optimizer="cem"): every refusal before any device work, then one
+        policy_opt.CemPolicySearch"""
+        import torch
+        from .. import policy_opt
+        what = "optimize_policy_sampled(optimizer='cem')"
+        c = self.controller
+        if isinstance(c, controllers.TimeVaryingLinearController):
+            raise ValueError("%s: a TimeVaryingLinearController plans with plan(optimizer='cem')" % what)
+        if isinstance(c, controllers.MlpController):
+            for on, feat in ((bool(self.angle_dims), "angles"), (self.measurement_noise is not None,
+                                                                 "measurement_noise")):
+                if on:
+                    raise ValueError("%s: an MLP policy does not combine with %s" % (what, feat))
+        for on, feat in ((float(exploration) != 0.0, "exploration (CEM's objective is the mean return)"),
+                         (bool(resample), "resample=True"), (num_features is not None, "num_features")):
+            if on:
+                raise ValueError("%s: does not combine with %s" % (what, feat))
+        if int(restarts) != 1:
+            raise ValueError("%s: takes restarts=1 (the population is the search), got %d" % (what, int(restarts)))
+        K, ke, iters, S, H = int(population), int(elites), int(maxiter), int(num_samples), int(self.horizon)
+        if not 1 <= K <= _lib.CEM_MAX_K or not 1 <= ke <= K or iters < 1:
+            raise ValueError("%s: needs 1 <= population <= %d, 1 <= elites <= population and maxiter >= 1 "
+                             "(population=%d, elites=%d, maxiter=%d)" % (what, _lib.CEM_MAX_K, K, ke, iters))
+        if S < 1 or H < 1:
+            raise ValueError("%s: needs num_samples >= 1 and horizon >= 1 (num_samples=%d, horizon=%d)" % (what, S, H))
+        n = c.get_flat().size
+        std = np.asarray(cem_std, dtype=np.float64)
+        if std.shape not in ((), (n,)) or not np.all(np.isfinite(std)) or not np.all(std > 0.0):
+            raise ValueError("%s: cem_std must be finite and > 0, a scalar or %d values (len(get_flat())), got shape %s"
+                             % (what, n, std.shape))
+        noise = self._noise_var()
+        if seed is None:
+            seed = int(np.random.randint(0, 2 ** 63 - 1, dtype=np.int64))
+        Ds = self.state_dim
+        x0, g = self._start_states(self.m_init, self.S_init, S, seed)
+        draw = lambda *shape: torch.randn(shape, dtype=engine.F64, device=x0.device, generator=g)
+        eps = draw(S, H, Ds)                                    # _particle_inputs' step normals
+        nu = draw(S, H, Ds) if noise is not None else None
+        search = policy_opt.CemPolicySearch(self, K, ke, iters, S, seed, std0=std, consistent=consistent,
+                                            angles=self.angle_dims, measurement_noise=noise)
+        search.set_inputs(x0, eps, nu)
+        best, best_value = search.run()
+        c.set_flat(best.cpu().numpy())
+        self.cem_search = search
+        return float(best_value.item())
 
     def training_loss(self):
         """-(the objective optimize_policy maximises) from N(m_init, S_init) over the horizon: -predict's reward, or with

@@ -13,6 +13,8 @@
   ``all_gather`` of ``[loss | flat parameters]`` lets every rank pick the same winner (ties -> lowest
   restart index, the sequential ``>`` comparison of pilco.py:105).  No other collective is used.
 """
+import ctypes as C
+import gc
 import os
 import threading
 import time
@@ -437,6 +439,109 @@ def optimize_stochastic(pilco, maxiter, restarts, num_samples, seed, consistent=
     local = gather_table(local, restarts, rank, world, dist)
     best = select_best(local)
     return local[best, 1:], -float(local[best, 0]), [-float(v) for v in local[:, 0]], trace, ok
+
+
+class CemPolicySearch(_FlatEvaluator):
+    """The cross-entropy method over a stationary policy's flat parameter vector (``controller.get_flat()`` layout, n
+    long) on the sampled return, every iteration on the device (DESIGN.md section 33).
+
+    ``K`` candidates are rolled out over the same P particles (``engine.ParticleBatchPlan``: x0, eps and, with
+    ``measurement_noise``, nu, filled by ``set_inputs``) and scored by their mean return.  A diagonal Gaussian over the
+    n parameters, started at the controller's current vector with std ``std0`` (a scalar or [n]), is refitted to the
+    ``elites`` best with smoothing ``alpha`` (pilco_cem_update at H = 1, U = n and unbounded candidates).
+    ``launch()`` enqueues, with no host synchronisation:
+      1. population 0: ``engine.normals`` into xi [K,n] under ``seed`` and stream id ``STREAM`` at iteration 0, then
+         pilco_cem_draw (row k = mean + std xi_k, row 0 = mean);
+      2. per iteration i: ``_unpack`` of the K rows into the plan's policy buffers (RBF: the batched refactorisation),
+         the plan's ``launch()`` (an RBF candidate whose factorisation failed gets a NaN value), the normals of
+         population i + 1 at iteration i + 1 (read from a device arange), and pilco_cem_update, which keeps the best
+         candidate so far, writes trace row i and draws the next population.
+    Row 0 of every population is the mean, so ``best_value`` is never below the start's value on the same particles; a
+    candidate with a NaN value ranks last and never becomes the best.  ``run()`` runs ``launch()`` eagerly once (the
+    warm-up), captures it as one CUDA graph and replays it once.  Afterwards ``best`` [n] and ``best_value`` [1] hold the
+    best candidate and its value, ``mean`` and ``std`` [n] the sampling distribution and ``trace`` [iters,2] each
+    iteration's top value and elites' mean value."""
+
+    STREAM = 32              # the candidates' normals (the Adam draws use stream ids 0 .. 6 and 16 .. 22)
+    ALPHA = 0.1              # engine.CemPlan's smoothing
+
+    def __init__(self, pilco, K, elites, iters, num_samples, seed, std0=0.5, consistent=False, angles=None,
+                 measurement_noise=None, alpha=ALPHA, max_ws_bytes=None):
+        super().__init__(pilco, int(K))
+        if self.sched:
+            raise ValueError("CemPolicySearch: a TimeVaryingLinearController plans with PILCO.plan(optimizer='cem')")
+        K, ke, iters, n = self.R, int(elites), int(iters), self.P
+        if not 1 <= K <= _lib.CEM_MAX_K or not 1 <= ke <= K or iters < 1:
+            raise ValueError("CemPolicySearch: needs 1 <= population <= %d, 1 <= elites <= population and iters >= 1 "
+                             "(population=%d, elites=%d, iters=%d)" % (_lib.CEM_MAX_K, K, ke, iters))
+        std0 = np.broadcast_to(np.asarray(std0, dtype=np.float64), (n,)).copy()
+        if not (np.isfinite(std0).all() and (std0 > 0.0).all()):
+            raise ValueError("CemPolicySearch: the initial std must be finite and > 0 (a scalar or %d values)" % n)
+        self.K, self.elites, self.iters, self.seed, self.alpha = K, ke, iters, int(seed), float(alpha)
+        terms, mult_mu = pilco.reward_spec()
+        spec = self.c.policy_spec(self.flat0) if self.linear or self.mlp else pilco.policy_spec(self.flat0)
+        self.plan = engine.ParticleBatchPlan(pilco.mgpr.device_gp(), spec, terms, int(num_samples), int(pilco.horizon),
+                                             K, mult_mu=mult_mu, consistent=consistent, angles=angles,
+                                             measurement_noise=measurement_noise, max_ws_bytes=max_ws_bytes)
+        self.gp = self.plan.rbf
+        d = engine.device()
+        mk = lambda *shape: torch.zeros(shape, dtype=torch.float64, device=d)
+        self.mean0, self.std0 = engine.dev(self.flat0[0]), engine.dev(std0)
+        self.cand, self.xi = mk(K, n), mk(K, n)
+        self.mean, self.std, self.best, self.best_value, self.trace = mk(n), mk(n), mk(n), mk(1), mk(iters, 2)
+        self.its = torch.arange(iters, dtype=torch.int64, device=d)       # population i's normals: iteration i
+        value = self.plan.value
+        cem = lambda xi, trace: _lib.Cem(K, 1, n, ke, self.alpha, -np.inf, np.inf, value.data_ptr(),
+                                         self.cand.data_ptr(), xi, self.mean.data_ptr(), self.std.data_ptr(),
+                                         self.best_value.data_ptr(), self.best.data_ptr(), trace)
+        self.draw = cem(self.xi.data_ptr(), None)
+        self.updates = [cem(self.xi.data_ptr() if i + 1 < iters else None, self.trace[i].data_ptr())
+                        for i in range(iters)]
+        self.uws_bytes = int(_lib.lib.pilco_cem_update_workspace_bytes(K))
+        self.uws = torch.empty(max(self.uws_bytes // 8, 2), dtype=torch.float64, device=d)
+
+    def set_inputs(self, x0, eps, nu=None):
+        self.plan.set_inputs(x0, eps, nu)
+
+    def evaluate(self):
+        """the plan's rollouts of the current population -> value [K]; a candidate whose RBF factorisation failed
+        gets NaN"""
+        self._unpack(self.cand, self.plan, self.gp)
+        value = self.plan.launch()
+        if self.gp is not None:
+            value.masked_fill_(self.gp.info.reshape(self.K) != 0, float("nan"))
+        return value
+
+    def launch(self):
+        """the whole search on the current stream, from the start: no host synchronisation"""
+        self.mean.copy_(self.mean0)
+        self.std.copy_(self.std0)
+        self.best.copy_(self.mean0)
+        self.best_value.fill_(-float("inf"))
+        engine.normals(self.xi, self.seed, self.STREAM, self.its[0:1])
+        _lib.check(_lib.lib.pilco_cem_draw(C.byref(self.draw), engine.stream_ptr()), "cem_draw")
+        for i, u in enumerate(self.updates):
+            self.evaluate()
+            if i + 1 < self.iters:
+                engine.normals(self.xi, self.seed, self.STREAM, self.its[i + 1:i + 2])
+            _lib.check(_lib.lib.pilco_cem_update(C.byref(u), self.uws.data_ptr(), self.uws_bytes, engine.stream_ptr()),
+                       "cem_update")
+        return self.best, self.best_value
+
+    def run(self):
+        """``launch()`` eagerly (warm-up), then captured as one CUDA graph and replayed once -> (best [n], best_value
+        [1]).  Unreachable cycles are collected first: one that holds an earlier graph would otherwise be freed inside
+        the capture, and freeing a graph's memory there invalidates it.  The graph is released after its replay."""
+        self.launch()
+        torch.cuda.synchronize()
+        gc.collect()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.launch()
+        g.replay()
+        torch.cuda.synchronize()
+        del g
+        return self.best, self.best_value
 
 
 def _no_box(pilco):
