@@ -5,6 +5,7 @@ CUDA tensors (the API classes convert to host arrays at the boundary).  There is
 ``device()`` raises when no CUDA device is present.
 """
 import ctypes as C
+import gc
 
 import numpy as np
 import torch
@@ -268,15 +269,10 @@ def gp_predict_samples(gp, Xnew, eps, e0=0, ne=None, full_cov=True, jitter=1e-6,
     wsb = predict_samples_workspace_bytes(gp, T, S, ne, full_cov)
     if wsb == 0:
         raise ValueError("gp_predict_samples: unsupported sizes (n=%d, D=%d, ne=%d, T=%d, S=%d)" % (gp.n, gp.D, ne, T, S))
+    _largest_fitting(lambda t: predict_samples_workspace_bytes(gp, t, S, ne, full_cov), T, max_ws_bytes,
+                     "gp_predict_samples: %d samples of %d outputs at T=%d points (full_cov=%s)"
+                     % (S, ne, T, bool(full_cov)), whole="T")
     d = device()
-    if max_ws_bytes is None:
-        max_ws_bytes = torch.cuda.mem_get_info(d)[0] // 2
-    if wsb > max_ws_bytes:
-        lo = _largest_fitting(lambda t: 0 < predict_samples_workspace_bytes(gp, t, S, ne, full_cov) <= max_ws_bytes,
-                              0, T - 1)
-        raise ValueError("gp_predict_samples: %d samples of %d outputs at T=%d points (full_cov=%s) need %d workspace "
-                         "bytes, more than max_ws_bytes=%d (half the free device memory by default); T=%d would fit"
-                         % (S, ne, T, bool(full_cov), wsb, max_ws_bytes, lo))
     samples = torch.empty((S, T, ne), dtype=F64, device=d)
     info = torch.empty(ne, dtype=torch.int32, device=d)
     ws = torch.empty(wsb // 8, dtype=F64, device=d)
@@ -552,13 +548,17 @@ def _particle_schedule(policy_spec, H, schedule, what):
     return _schedule_check(policy_spec, H, schedule)
 
 
+def _reward_count(reward_terms):
+    if len(reward_terms) > 8:
+        raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
+
+
 def _fill_rewards(desc, reward_terms):
     """Fill ``desc.n_rewards`` and ``desc.rewards`` from reward-term dicts (``desc.pol`` already filled); returns the
     device tensors [(W, t)] they point to.  The shapes of a joint state-action term are checked against the policy
     here, before any device work: ValueError."""
     rw = []
-    if len(reward_terms) > 8:
-        raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
+    _reward_count(reward_terms)
     desc.n_rewards = len(reward_terms)
     Ds, U = int(desc.pol.Ds), int(desc.pol.U)
     for k, rt in enumerate(reward_terms):
@@ -778,52 +778,209 @@ class RolloutPlan:
         return self.gbuf
 
 
-# (consistent, call) -> the C rollout and its size query (after "pilco_particles_"): the most general entry point of each
-# kind, given NULL for the angles, noise or exploration a plan lacks.  The pathwise call of an unbatched plan is the
-# batched one at R = 1 (its policy strides are 0).
-PARTICLE_CALLS = {
-    (False, "forward"): ("noisy_rollout", "noisy_workspace_bytes"),
-    (True, "forward"): ("noisy_consistent_rollout", "noisy_consistent_workspace_bytes"),
-    (False, "pathwise"): ("explore_batch_grad_rollout", "explore_batch_grad_workspace_bytes"),
-    (True, "pathwise"): ("explore_consistent_grad_rollout", "explore_consistent_grad_workspace_bytes"),
-    (False, "score"): ("noisy_score_grad_rollout", "noisy_score_grad_workspace_bytes"),
-    (True, "score"): ("consistent_score_grad_rollout", "consistent_score_grad_workspace_bytes"),
-    ("resampled", "forward"): ("resampled_rollout", "resampled_workspace_bytes"),
-    ("resampled", "pathwise"): ("resampled_grad_rollout", "resampled_grad_workspace_bytes"),
-}
+# (policy family, sampler, call) -> the C rollout and its size query, pilco_particles_<stem>_rollout and
+# pilco_particles_<stem>_workspace_bytes.  Families: "plain" (linear or RBF), "scheduled" (a time-varying linear policy,
+# DESIGN.md section 28) and "mlp" (section 29); samplers: "step", "consistent" (section 14), "resampled" (section 26) and
+# "features" (section 30); calls: "forward", the gradients "pathwise" and "score", and "batch", R policies forward only
+# (sections 31 and 33).  Each row is the most general entry point of its kind, given NULL for the angles, noise or
+# exploration a plan lacks; the pathwise call of an unbatched plan is the batched one at R = 1.
+PARTICLE_ENTRY_POINTS = {key: ("pilco_particles_%s_rollout" % stem, "pilco_particles_%s_workspace_bytes" % stem)
+                         for key, stem in {
+    ("plain", "step", "forward"): "noisy",
+    ("plain", "consistent", "forward"): "noisy_consistent",
+    ("plain", "step", "pathwise"): "explore_batch_grad",
+    ("plain", "consistent", "pathwise"): "explore_consistent_grad",
+    ("plain", "step", "score"): "noisy_score_grad",
+    ("plain", "consistent", "score"): "consistent_score_grad",
+    ("plain", "resampled", "forward"): "resampled",
+    ("plain", "resampled", "pathwise"): "resampled_grad",
+    ("plain", "features", "forward"): "features",
+    ("plain", "features", "pathwise"): "features_grad",
+    ("plain", "step", "batch"): "batch",
+    ("plain", "consistent", "batch"): "consistent_batch",
+    ("scheduled", "step", "forward"): "scheduled",
+    ("scheduled", "consistent", "forward"): "scheduled_consistent",
+    ("scheduled", "step", "pathwise"): "scheduled_batch_grad",
+    ("scheduled", "consistent", "pathwise"): "scheduled_consistent_grad",
+    ("scheduled", "step", "score"): "scheduled_score_grad",
+    ("scheduled", "consistent", "score"): "scheduled_consistent_score_grad",
+    ("scheduled", "resampled", "forward"): "scheduled_resampled",
+    ("scheduled", "resampled", "pathwise"): "scheduled_resampled_grad",
+    ("scheduled", "step", "batch"): "scheduled_batch",
+    ("scheduled", "consistent", "batch"): "scheduled_consistent_batch",
+    ("mlp", "step", "forward"): "mlp",
+    ("mlp", "consistent", "forward"): "mlp_consistent",
+    ("mlp", "step", "pathwise"): "mlp_batch_grad",
+    ("mlp", "consistent", "pathwise"): "mlp_consistent_grad",
+    ("mlp", "resampled", "forward"): "mlp_resampled",
+    ("mlp", "resampled", "pathwise"): "mlp_resampled_grad",
+    ("mlp", "features", "forward"): "mlp_features",
+    ("mlp", "features", "pathwise"): "mlp_features_grad",
+    ("mlp", "step", "batch"): "mlp_batch",
+    ("mlp", "consistent", "batch"): "mlp_consistent_batch",
+}.items()}
 
-# the feature sampler's rows (DESIGN.md section 30): the forward and pathwise call with a pilco_feature_draws after
-# the angles, noise and (pathwise) exploration
-PARTICLE_FEATURE_CALLS = {
-    ("features", "forward"): ("features_rollout", "features_workspace_bytes"),
-    ("features", "pathwise"): ("features_grad_rollout", "features_grad_workspace_bytes"),
-}
 
-# the same rows with a time-varying linear policy (DESIGN.md section 28): each call above with a pilco_policy_schedule
-# after its feature arguments
-PARTICLE_SCHEDULED_CALLS = {
-    (False, "forward"): ("scheduled_rollout", "scheduled_workspace_bytes"),
-    (True, "forward"): ("scheduled_consistent_rollout", "scheduled_consistent_workspace_bytes"),
-    (False, "pathwise"): ("scheduled_batch_grad_rollout", "scheduled_batch_grad_workspace_bytes"),
-    (True, "pathwise"): ("scheduled_consistent_grad_rollout", "scheduled_consistent_grad_workspace_bytes"),
-    (False, "score"): ("scheduled_score_grad_rollout", "scheduled_score_grad_workspace_bytes"),
-    (True, "score"): ("scheduled_consistent_score_grad_rollout", "scheduled_consistent_score_grad_workspace_bytes"),
-    ("resampled", "forward"): ("scheduled_resampled_rollout", "scheduled_resampled_workspace_bytes"),
-    ("resampled", "pathwise"): ("scheduled_resampled_grad_rollout", "scheduled_resampled_grad_workspace_bytes"),
-}
+def _view(keep, key):
+    """the rows of PARTICLE_ENTRY_POINTS that keep(family, sampler, call) selects, under key(family, sampler, call),
+    their names after "pilco_particles_": the per-family tables that callers index"""
+    return {key(*k): tuple(n[len("pilco_particles_"):] for n in v) for k, v in PARTICLE_ENTRY_POINTS.items() if keep(*k)}
 
-# the rows a tanh MLP policy runs (DESIGN.md section 29): each sampler's forward and pathwise call with a pilco_mlp
-# after pr (then the exploration for the step-wise and consistent gradients, the refit's buffers for the resampled)
-PARTICLE_MLP_CALLS = {
-    (False, "forward"): ("mlp_rollout", "mlp_workspace_bytes"),
-    (True, "forward"): ("mlp_consistent_rollout", "mlp_consistent_workspace_bytes"),
-    (False, "pathwise"): ("mlp_batch_grad_rollout", "mlp_batch_grad_workspace_bytes"),
-    (True, "pathwise"): ("mlp_consistent_grad_rollout", "mlp_consistent_grad_workspace_bytes"),
-    ("resampled", "forward"): ("mlp_resampled_rollout", "mlp_resampled_workspace_bytes"),
-    ("resampled", "pathwise"): ("mlp_resampled_grad_rollout", "mlp_resampled_grad_workspace_bytes"),
-    ("features", "forward"): ("mlp_features_rollout", "mlp_features_workspace_bytes"),
-    ("features", "pathwise"): ("mlp_features_grad_rollout", "mlp_features_grad_workspace_bytes"),
-}
+
+_SAMPLER_KEY = {"step": False, "consistent": True}             # the views' sampler keys: the consistent flag, or the name
+PARTICLE_CALLS = _view(lambda f, s, c: f == "plain" and s != "features" and c != "batch",
+                       lambda f, s, c: (_SAMPLER_KEY.get(s, s), c))
+PARTICLE_FEATURE_CALLS = _view(lambda f, s, c: f == "plain" and s == "features", lambda f, s, c: (s, c))
+PARTICLE_SCHEDULED_CALLS = _view(lambda f, s, c: f == "scheduled" and c != "batch",
+                                 lambda f, s, c: (_SAMPLER_KEY.get(s, s), c))
+PARTICLE_MLP_CALLS = _view(lambda f, s, c: f == "mlp" and c != "batch", lambda f, s, c: (_SAMPLER_KEY.get(s, s), c))
+PARTICLE_BATCH_CALLS = _view(lambda f, s, c: f == "scheduled" and c == "batch", lambda f, s, c: s == "consistent")
+PARTICLE_STATIONARY_BATCH_CALLS = _view(lambda f, s, c: f != "scheduled" and c == "batch",
+                                        lambda f, s, c: (f == "mlp", s == "consistent"))
+
+# the slot each argtype of a particle entry point takes (a rollout's final c_dp is the stream, which each launch passes)
+_SLOTS = {C.POINTER(_lib.Particles): "pr", C.POINTER(_lib.Angles): "ang", C.POINTER(_lib.ParticlesNoise): "nz",
+          C.POINTER(_lib.Exploration): "ex", C.POINTER(_lib.PolicySchedule): "sch", C.POINTER(_lib.Mlp): "mlp",
+          C.POINTER(_lib.ParticlesResample): "rs", C.POINTER(_lib.FeatureDraws): "fd",
+          C.POINTER(_lib.ParticlesGrad): "grad", C.c_int: "R", _lib.c_dp: "value"}
+
+
+def particle_args(name, **slots):
+    """The arguments of the particle entry point ``name`` before its stream, in the order of its ``_lib.SIGNATURES``
+    argtypes (the header's): the structs ``pr`` (the pilco_particles description), ``ang``, ``nz``, ``ex``, ``sch``,
+    ``mlp``, ``rs``, ``fd`` and ``grad`` by reference, NULL where ``slots`` has none; ``R`` for the c_int; ``value``
+    for a c_dp before the stream."""
+    res, types = _lib.SIGNATURES[name]
+    args = [slots.get(_SLOTS[t]) for t in (types[:-1] if res is C.c_int else types)]
+    return tuple(C.byref(a) if isinstance(a, C.Structure) else a for a in args)
+
+
+class _Entry:
+    """Row ``key`` of PARTICLE_ENTRY_POINTS with its arguments bound once (``particle_args``): ``query()`` is the
+    workspace size, a call enqueues the rollout on the current stream."""
+
+    def __init__(self, key, **slots):
+        run, query = PARTICLE_ENTRY_POINTS[key]
+        self.name = run[len("pilco_"):]
+        self.run, self.args = getattr(lib, run), particle_args(run, **slots)
+        self.size, self.size_args = getattr(lib, query), particle_args(query, **slots)
+
+    def query(self):
+        return int(self.size(*self.size_args))
+
+    def __call__(self):
+        check(self.run(*self.args, stream_ptr()), self.name)
+
+
+def _policy_width(dyn, spec, angles, what):
+    """(E, the pilco_angles of ``angles`` or None): the policy takes the state's E dimensions and one more per angle
+    (phi(x)); ValueError otherwise, before any allocation"""
+    E = int(dyn.struct().E)
+    ang = angles_struct(angles, E) if angles is not None and len(angles) > 0 else None
+    A = ang.A if ang is not None else 0
+    if int(spec["Ds"]) != E + A:
+        raise ValueError("%s: with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
+                         % (what, A, E + A, int(spec["Ds"])))
+    return E, ang
+
+
+def _noise_struct(measurement_noise, E):
+    """the pilco_particles_noise of the measurement variances (None: no noise; ``_particle_noise``'s refusals).  Its
+    nu is a placeholder, which the size queries check but do not read, until ``_buffers`` points it at the plan's nu"""
+    v = _particle_noise(measurement_noise, E)
+    if v is None:
+        return None
+    nz = _lib.ParticlesNoise()
+    for i, x in enumerate(v):
+        nz.v.var[i] = float(x)
+    nz.nu = 16
+    return nz
+
+
+class _Particles:
+    """What the particle plans share: one ``pilco_particles`` description ``pr``, the structs the entry points take
+    beside it and the device tensors they point to.  ``_structs`` allocates nothing, so that a plan can query sizes and
+    refuse before any allocation; ``_buffers`` allocates."""
+
+    ang = nz = ex = sch = mlp = rs = fd = grad = None
+    R = 1
+
+    def _structs(self, dyn, spec, P, H, ang=None, nz=None, schedule=False, mlp=None, batched=False):
+        """the description with what the size queries read (sizes, model, the policy's kind and widths, an RBF
+        policy's model), the schedule (step t reads W[t], b[t]) and the MLP (``_particle_mlp``'s (L, widths,
+        n_theta, _); theta strides by n_theta when ``batched``)"""
+        self.keep = [dyn, spec]                                 # keep device tensors alive
+        self.P, self.H, self.E, self.U = int(P), int(H), int(dyn.struct().E), int(spec["U"])
+        self.ang, self.nz = ang, nz
+        pr = self.pr = _lib.Particles()
+        pr.P, pr.H = self.P, self.H
+        pr.dyn = dyn.struct()
+        pr.pol.kind, pr.pol.Ds, pr.pol.U = spec.get("kind", _lib.POLICY_LINEAR), int(spec["Ds"]), self.U
+        if pr.pol.kind == _lib.POLICY_RBF:
+            pr.pol.rbf = spec["gp"].struct()
+        if schedule:
+            self.sch = _lib.PolicySchedule(self.U * pr.pol.Ds, self.U)
+        if mlp is not None:
+            L, hidden, self.n_theta, _ = mlp
+            self.mlp = _lib.Mlp(L, (C.c_int * 2)(hidden[0], hidden[-1] if L == 2 else 0), None,
+                                self.n_theta if batched else 0, None)
+
+    def _buffers(self, spec, reward_terms, mult_mu, lead, batched):
+        """the policy's device tensors (``_fill_policy``; a batched schedule strides by its steps, an MLP's theta is
+        [R?, n_theta]), the reward terms and mult_mu, the inputs x0 [P,E], eps [P,Hb,E] and with measurement noise nu
+        [P,Hb,E], shared by the policies, and the outputs traj [*lead,P,H+1,E], act_buf [*lead,P,Hb,U], rew_buf and
+        risk_buf [*lead,P,Hb] and ret [*lead,P] (Hb = max(H, 1): H = 0 still has addresses)"""
+        pr, d = self.pr, device()
+        P, H, Hb, E, U = self.P, self.H, max(self.H, 1), self.E, self.U
+        self.keep.append(reward_terms)
+        self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, spec, batched)
+        if self.sch is not None and batched:                    # W [R,Hw,U,Ds], b [R,Hw,U]
+            pr.pol.W_bs, pr.pol.b_bs = self.W[0].numel(), self.b[0].numel()
+        if self.mlp is not None:
+            self.theta = dev(spec["theta"]).reshape(*((self.R,) if batched else ()), self.n_theta)
+            self.mlp.theta = self.theta.data_ptr()
+        self.rw = _fill_rewards(pr, reward_terms)
+        pr.mult_mu = float(mult_mu)
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
+        self.x0, self.eps_buf = mk(P, E), mk(P, Hb, E)
+        self.traj, self.act_buf = mk(*lead, P, H + 1, E), mk(*lead, P, Hb, U)
+        self.rew_buf, self.risk_buf, self.ret = mk(*lead, P, Hb), mk(*lead, P, Hb), mk(*lead, P)
+        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
+        pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
+        pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
+        if self.nz is not None:
+            self.nu_buf = mk(P, Hb, E)
+            self.nz.nu = self.nu_buf.data_ptr()
+
+    def _ang_ref(self):
+        return C.byref(self.ang) if self.ang is not None else None
+
+    def _nz_ref(self):
+        return C.byref(self.nz) if self.nz is not None else None
+
+    def _entry(self, key, **slots):
+        """row ``key`` of PARTICLE_ENTRY_POINTS bound to this description's structs (``slots`` replace them)"""
+        return _Entry(key, **dict(dict(pr=self.pr, ang=self.ang, nz=self.nz, ex=self.ex, sch=self.sch, mlp=self.mlp,
+                                       rs=self.rs, fd=self.fd, grad=self.grad, R=self.R), **slots))
+
+
+def _largest_fitting(need, n, max_ws_bytes, what, whole=None):
+    """The largest count c in 1 .. n whose workspace of need(c) bytes fits max_ws_bytes (default: half the free device
+    memory), by bisection: need(c) grows with c and is 0 for sizes the call does not support.  Not even c = 1 fitting
+    is a ValueError that names ``what`` and the bytes needed.  ``whole`` (the count's name): all n must fit, and the
+    ValueError also names the largest count that would."""
+    if max_ws_bytes is None:
+        max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+    fits = lambda c: 0 < need(c) <= max_ws_bytes
+    lo, hi = (n, n) if fits(n) else (0, n - 1)
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    if lo < (n if whole else 1):
+        raise ValueError("%s: need %d workspace bytes, more than max_ws_bytes=%d (half the free device memory by "
+                         "default)%s" % (what, need(n if whole else 1), max_ws_bytes,
+                                         "; %s=%d would fit" % (whole, lo) if whole else ""))
+    return lo
 
 
 class FeatureDraws:
@@ -885,7 +1042,7 @@ def feature_draws(dyn, P, F, zeta, w, eps_y, out=None):
     return out
 
 
-class ParticlePlan:
+class ParticlePlan(_Particles):
     """Owns the buffers of one ``pilco_particles`` description (P particles, horizon H) and launches it.
 
     ``x0`` [P,Ds] and ``eps`` [P,H,Ds] are static device buffers: fill them (``set_inputs``) and ``launch()``, or
@@ -978,137 +1135,74 @@ class ParticlePlan:
         self._describe(dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles, measurement_noise, exploration,
                        sched, mlp)
         pr, d = self.pr, device()
-        P, H = self.P, self.H
         if not self.batched:                                    # the forward-only rollout (a batch has none)
-            wsb = self._query("forward", pr)
+            self.fwd = self._entry(self._key("forward"))
+            wsb = self.fwd.query()
             if wsb == 0:
-                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, dyn.D))
+                raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d)" % (self.P, self.H, dyn.D))
             self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
             pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
         self.grad = None
         if grad:
-            self._grad_buffers(self._grad_ws_bytes(P))
+            self._grad_buffers(self._grad_ws_bytes(self.P))
 
-    def _sampler(self):
-        return "resampled" if self.resample else "features" if self.fd is not None else self.consistent
-
-    def _args(self, kind, pr):
-        """the arguments of kind's call up to R: pr, the angles, the noise, the exploration (pathwise), the schedule
-        (scheduled calls) and R; resampled: pr, the refit's buffers, the schedule and R"""
-        sch = [C.byref(self.sch)] if self.sch is not None else []
-        fd = [C.byref(self.fd)] if self.fd is not None else []
-        if self.mlp is not None:
-            feat = [C.byref(self.rs)] if self.resample else \
-                [] if kind == "forward" else [C.byref(self.ex) if self.ex is not None else None]
-            return [C.byref(pr), C.byref(self.mlp)] + feat + fd + ([self.R] if kind != "forward" else [])
-        if self.resample:
-            return [C.byref(pr), C.byref(self.rs)] + sch + ([self.R] if kind != "forward" else [])
-        args = [C.byref(pr), self._ang_ref(), self._nz_ref()]
-        if kind == "pathwise":
-            args.append(C.byref(self.ex) if self.ex is not None else None)
-        return args + sch + fd + ([self.R] if kind != "forward" else [])
-
-    def _names(self, kind):
-        """(rollout, size query) of kind's call, each after the prefix pilco_particles_"""
-        table = PARTICLE_MLP_CALLS if self.mlp is not None else PARTICLE_FEATURE_CALLS if self.fd is not None else \
-            PARTICLE_CALLS if self.sch is None else PARTICLE_SCHEDULED_CALLS
-        return table[self._sampler(), kind]
-
-    def _query(self, kind, pr):
-        return int(getattr(lib, "pilco_particles_" + self._names(kind)[1])(*self._args(kind, pr)))
+    def _key(self, call):
+        """the PARTICLE_ENTRY_POINTS row of this plan's ``call``"""
+        family = "mlp" if self.mlp is not None else "scheduled" if self.sch is not None else "plain"
+        sampler = "resampled" if self.resample else "features" if self.fd is not None else \
+            "consistent" if self.consistent else "step"
+        return family, sampler, call
 
     def _grad_ws_bytes(self, P):
         """the gradient workspace of this plan's call with P particles per restart (0: unsupported sizes)"""
         pr = _lib.Particles.from_buffer_copy(self.pr)
         pr.P = int(P)
-        return self._query(self.estimator, pr)
+        return self._entry(self._key(self.estimator), pr=pr).query()
 
     def _describe(self, dyn, policy_spec, reward_terms, P, H, mult_mu, R, grad, angles=None, measurement_noise=None,
                   exploration=None, sched=None, mlp=None):
         """the pilco_particles description, its input and output buffers (self.pr); self.Ds is the state's width.
-        The angles, the policy's width, the measurement noise and the exploration weight are checked first, before any
-        device work.  ``sched``: ``_schedule_check``'s (batched, Hw) of a scheduled spec, or None; ``mlp``:
-        ``_particle_mlp``'s (L, widths, n_theta, batched) of an MLP spec, or None."""
-        self.ang, self.nz, self.ex, self.sch, self.mlp = None, None, None, None, None
+        The angles, the policy's width, the measurement noise, the exploration weight and the policy's shapes are
+        checked first, before any device work.  ``sched``: ``_schedule_check``'s (batched, Hw) of a scheduled spec, or
+        None; ``mlp``: ``_particle_mlp``'s (L, widths, n_theta, batched) of an MLP spec, or None."""
         b = _particle_exploration(exploration, reward_terms, P)
-        if angles is not None and len(angles) > 0:
-            E = int(dyn.struct().E)
-            self.ang = angles_struct(angles, E)
-            if int(policy_spec["Ds"]) != E + self.ang.A:
-                raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d"
-                                 % (self.ang.A, E + self.ang.A, int(policy_spec["Ds"])))
-        nz_var = _particle_noise(measurement_noise, int(dyn.struct().E))
-        d = device()
-        self.P, self.H, self.R = int(P), int(H), int(R)
-        self.Ds, self.U = int(policy_spec["Ds"]), int(policy_spec["U"])
-        P, H, Ds, U, R = self.P, self.H, self.Ds, self.U, self.R
+        E, ang = _policy_width(dyn, policy_spec, angles, "particles")
+        nz = _noise_struct(measurement_noise, E)
+        P, H, R = int(P), int(H), int(R)
         if P < 1 or H < 0 or R < 1:
             raise ValueError("particles: needs P >= 1, H >= 0 and R >= 1 (P=%d, H=%d, R=%d)" % (P, H, R))
-        if self.ang is not None:
-            self.Ds = int(dyn.struct().E)
+        Ds, U = E + (ang.A if ang is not None else 0), int(policy_spec["U"])
         rbf_batched = policy_spec["kind"] == _lib.POLICY_RBF and policy_spec["gp"].batched
-        self.batched = R > 1 or rbf_batched or (mlp is not None and mlp[3])
+        self.R, self.batched = R, R > 1 or rbf_batched or (mlp is not None and mlp[3])
         if self.batched and not grad:
             raise ValueError("particles: a batch of policies runs the gradient path only (grad=True)")
-        lead = (R,) if self.batched else ()
-        self.lead = lead
-        self.keep = [dyn, policy_spec, reward_terms]            # keep device tensors alive
-        pr = _lib.Particles()
-        pr.P, pr.H = P, H
-        pr.dyn = dyn.struct()
-        self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, policy_spec, self.batched)
+        size = lambda k: int(np.prod(np.shape(policy_spec[k])))
         if sched is not None:                                   # step t reads W[..., t, :, :], b[..., t, :]
             Hw = sched[1]
-            if self.W.numel() != R * Hw * U * Ds or self.b.numel() != R * Hw * U:
+            if size("W") != R * Hw * U * Ds or size("b") != R * Hw * U:
                 raise ValueError("particles: schedule=True expects W [R,Hw,U,Ds] and b [R,Hw,U] with R=%d (unbatched: "
                                  "[Hw,U,Ds], [Hw,U])" % R)
-            pr.pol.W_bs, pr.pol.b_bs = (Hw * U * Ds, Hw * U) if self.batched else (0, 0)
-            self.sch = _lib.PolicySchedule(U * Ds, U)
-        elif mlp is not None:                                   # theta [R?, n_theta] (its length checked)
-            L, hidden, n_theta, _ = mlp
-            self.theta = dev(policy_spec["theta"])
-            self.n_theta = n_theta
-            self.mlp = _lib.Mlp(L, (C.c_int * 2)(hidden[0], hidden[-1] if L == 2 else 0), self.theta.data_ptr(),
-                                n_theta if self.batched else 0, None)
-        elif pr.pol.kind == _lib.POLICY_LINEAR:
-            if self.W.numel() != R * U * Ds or self.b.numel() != R * U:
+        elif mlp is None and policy_spec["kind"] == _lib.POLICY_LINEAR:
+            if size("W") != R * U * Ds or size("b") != R * U:
                 raise ValueError("particles: expected W [R,U,Ds] and b [R,U] with R=%d (unbatched: [U,Ds], [U])" % R)
-        elif self.rbf.batched != self.batched or (self.batched and self.rbf.X.shape[0] != R):
+        elif mlp is None and (rbf_batched != self.batched or (self.batched and policy_spec["gp"].X.shape[0] != R)):
             raise ValueError("particles: the RBF policy must be factorised with a leading R=%d (unbatched: none)" % R)
-        self.rw = _fill_rewards(pr, reward_terms)
-        pr.mult_mu = float(mult_mu)
-        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
-        Hb, Ds = max(H, 1), self.Ds                             # H = 0: every buffer still has an address
-        self.x0, self.eps_buf = mk(P, Ds), mk(P, Hb, Ds)                  # shared by the R policies
-        self.traj, self.act_buf = mk(*lead, P, H + 1, Ds), mk(*lead, P, Hb, U)
-        self.rew_buf, self.risk_buf, self.ret = mk(*lead, P, Hb), mk(*lead, P, Hb), mk(*lead, P)
-        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
-        pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
-        pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
-        self.pr = pr
-        if nz_var is not None:                                  # nu [P,H,E], shared by the R policies
-            E = len(nz_var)
-            self.nu_buf = mk(P, Hb, E)
-            self.nz = _lib.ParticlesNoise()
-            for i, v in enumerate(nz_var):
-                self.nz.v.var[i] = float(v)
-            self.nz.nu = self.nu_buf.data_ptr()
+        self.lead = (R,) if self.batched else ()
+        self._structs(dyn, policy_spec, P, H, ang, nz, sched is not None, mlp, self.batched)
+        self.Ds = E
+        self._buffers(policy_spec, reward_terms, mult_mu, self.lead, self.batched)
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=device())
+        Hb, lead = max(H, 1), self.lead
         if b is not None:                                       # sigma_t^2 [R, max(H,1)], also for an unbatched plan
             self.step_var = mk(R, Hb)
             self.ex = _lib.Exploration(b, self.step_var.data_ptr())
         if self.resample:                                       # xi shared by the R policies; the fitted moments
-            self.xi_buf = mk(P, Hb, Ds)
-            self._step_mean, self._step_cov = mk(R, H + 1, Ds), mk(R, H + 1, Ds, Ds)
-            self.step_mean = self._step_mean.view(*lead, H + 1, Ds)
-            self.step_cov = self._step_cov.view(*lead, H + 1, Ds, Ds)
+            self.xi_buf = mk(P, Hb, E)
+            self._step_mean, self._step_cov = mk(R, H + 1, E), mk(R, H + 1, E, E)
+            self.step_mean = self._step_mean.view(*lead, H + 1, E)
+            self.step_cov = self._step_cov.view(*lead, H + 1, E, E)
             self.rs = _lib.ParticlesResample(self.xi_buf.data_ptr(), self._step_mean.data_ptr(),
                                              self._step_cov.data_ptr())
-
-    def _ang_ref(self):
-        return C.byref(self.ang) if self.ang is not None else None
-
-    def _nz_ref(self):
-        return C.byref(self.nz) if self.nz is not None else None
 
     def _grad_buffers(self, gwsb):
         """the pilco_particles_grad outputs and a gradient workspace of gwsb bytes (self.grad)"""
@@ -1129,6 +1223,7 @@ class ParticlePlan:
         self.gws = torch.empty(max(gwsb // 8, 2), dtype=F64, device=d)
         g.ws, g.ws_bytes = self.gws.data_ptr(), gwsb
         self.grad = g
+        self.bwd = self._entry(self._key(self.estimator))
 
     def launch_grad(self):
         """pilco_particles_rollout_grad: the rollout (``outputs()`` as after ``launch()``, bitwise) and the pathwise
@@ -1141,12 +1236,8 @@ class ParticlePlan:
         [R?, n_theta]}."""
         if self.grad is None:
             raise RuntimeError("ParticlePlan: constructed without grad=True")
-        self._call(self.estimator, C.byref(self.grad))
+        self.bwd()
         return self.gbuf
-
-    def _call(self, kind, *grad):
-        name = "particles_" + self._names(kind)[0]
-        check(getattr(lib, "pilco_" + name)(*self._args(kind, self.pr), *grad, stream_ptr()), name)
 
     def set_inputs(self, x0, eps, nu=None, xi=None, features=None):
         """x0 [P,Ds], eps [P,H,Ds], with measurement noise nu [P,H,E] and with ``resample`` xi [P,H,Ds] (each required
@@ -1162,7 +1253,8 @@ class ParticlePlan:
                 raise ValueError("particles: the feature draws are for (P, F, E, n, D) = %s; the plan has %s"
                                  % (have, want))
             self.features = features                            # keeps the draws alive
-            self.fd = features.struct()
+            st = features.struct()                              # in place: the bound calls point at self.fd
+            self.fd.omega, self.fd.w, self.fd.v = st.omega, st.w, st.v
         if (nu is None) != (self.nz is None):
             raise ValueError("particles: nu [P,H,E] is required with measurement_noise and only then")
         if (xi is None) == self.resample:
@@ -1179,7 +1271,7 @@ class ParticlePlan:
     def launch(self):
         if self.batched:
             raise RuntimeError("ParticlePlan: a batch of policies runs launch_grad()")
-        self._call("forward")
+        self.fwd()
 
     def outputs(self):
         """(traj [P,H+1,Ds], act [P,H,U], step_reward [P,H], step_risk [P,H], ret [P]) device tensors (views), each
@@ -1231,13 +1323,8 @@ class ConsistentGradPlan(ParticlePlan):
         need = self._grad_ws_bytes(self.P)
         if need == 0:
             raise ValueError("particles: unsupported sizes (P=%d, H=%d, D=%d, R=%d)" % (self.P, self.H, dyn.D, self.R))
-        if max_ws_bytes is None:
-            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
-        if need > max_ws_bytes:
-            lo = _largest_fitting(lambda p: 0 < self._grad_ws_bytes(p) <= max_ws_bytes, 0, self.P - 1)
-            raise ValueError("particles: the consistent gradient of %d restarts x %d particles over H=%d steps needs %d "
-                             "workspace bytes, more than max_ws_bytes=%d (half the free device memory by default); "
-                             "num_samples=%d would fit" % (self.R, self.P, self.H, need, max_ws_bytes, lo))
+        _largest_fitting(self._grad_ws_bytes, self.P, max_ws_bytes, "particles: the consistent gradient of %d restarts "
+                         "x %d particles over H=%d steps" % (self.R, self.P, self.H), whole="num_samples")
         self._grad_buffers(need)
 
     def launch(self):
@@ -1262,14 +1349,6 @@ def _features_plan_check(dyn, num_features, consistent, estimator, resample, sch
         if on:
             raise ValueError("particles: num_features does not combine with %s" % what)
     return _lib.FeatureDraws(_features_check(dyn, num_features), None, None, None)
-
-
-def _largest_fitting(fits, lo, hi):
-    """the largest p in [lo, hi] with fits(p), by bisection; fits must be monotone and hold at lo (or lo is returned)"""
-    while lo < hi:
-        mid = (lo + hi + 1) // 2
-        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
-    return lo
 
 
 def gp_predict_vjp(gp, Xs, gmean, gvar):
@@ -1457,16 +1536,11 @@ def consistent_workspace_bytes(dyn, Ds, U, P, H, angles=None, num_features=None)
     """pilco_particles_consistent_workspace_bytes of P particles over H steps (0: unsupported sizes); ``Ds`` is the
     policy's input width (with ``angles``: E + len(angles)).  ``num_features``: the feature sampler's
     (pilco_particles_features_workspace_bytes)."""
-    pr = _lib.Particles()
-    pr.P, pr.H = int(P), int(H)
-    pr.dyn = dyn.struct()
-    pr.pol.Ds, pr.pol.U = int(Ds), int(U)
-    ang = angles_struct(angles, int(pr.dyn.E))
-    ang = C.byref(ang) if ang is not None else None
+    d = _Particles()
+    d._structs(dyn, dict(Ds=Ds, U=U), P, H, angles_struct(angles, int(dyn.struct().E)))
     if num_features is not None:
-        fd = _lib.FeatureDraws(int(num_features), None, None, None)
-        return int(lib.pilco_particles_features_workspace_bytes(C.byref(pr), ang, None, C.byref(fd)))
-    return int(lib.pilco_particles_noisy_consistent_workspace_bytes(C.byref(pr), ang, None))
+        d.fd = _lib.FeatureDraws(int(num_features), None, None, None)
+    return d._entry(("plain", "consistent" if d.fd is None else "features", "forward")).query()
 
 
 def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_mu, max_ws_bytes, angles=None,
@@ -1474,21 +1548,11 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     """the consistent rollout in chunks of particles; with ``features`` eps is None and H is given"""
     P, H = int(x0.shape[0]), int(eps.shape[1]) if H is None else int(H)
     Ds, U = int(policy_spec["Ds"]), int(policy_spec["U"])
-    if angles is not None and len(angles) > 0:                 # the policy's width, before any allocation
-        E = int(dyn.struct().E)
-        A = angles_struct(angles, E).A
-        if Ds != E + A:
-            raise ValueError("with %d angle dimension(s) the policy must take %d inputs (phi(x)), got %d" % (A, E + A, Ds))
-    _particle_noise(measurement_noise, int(dyn.struct().E))
-    if max_ws_bytes is None:
-        max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
+    E, _ = _policy_width(dyn, policy_spec, angles, "particles_rollout")
+    _particle_noise(measurement_noise, E)
     F = features.F if features is not None else None
-    wsb = lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles, F)
-    fits = lambda p: 0 < wsb(p) <= max_ws_bytes
-    if not fits(1):
-        raise ValueError("particles_rollout: the consistent rollout of one particle (H=%d, n=%d) needs %d workspace "
-                         "bytes, more than max_ws_bytes=%d" % (H, dyn.n, wsb(1), max_ws_bytes))
-    lo = _largest_fitting(fits, 1, P)
+    lo = _largest_fitting(lambda p: consistent_workspace_bytes(dyn, Ds, U, p, H, angles, F), P, max_ws_bytes,
+                          "particles_rollout: the consistent rollout of one particle (H=%d, n=%d)" % (H, dyn.n))
     if lo == P:
         plan = ParticlePlan(dyn, policy_spec, reward_terms, P, H, mult_mu=mult_mu, consistent=True, angles=angles,
                             measurement_noise=measurement_noise, schedule=schedule, num_features=F)
@@ -1515,16 +1579,62 @@ def _particles_rollout_consistent(dyn, policy_spec, reward_terms, x0, eps, mult_
     return out
 
 
-# the batched forward-only rollouts (DESIGN.md section 31) per sampler: (rollout, size query) after "pilco_particles_"
-PARTICLE_BATCH_CALLS = {
-    False: ("scheduled_batch_rollout", "scheduled_batch_workspace_bytes"),
-    True: ("scheduled_consistent_batch_rollout", "scheduled_consistent_batch_workspace_bytes"),
-}
+class CemLoop:
+    """The cross-entropy method's loop on the device (DESIGN.md sections 31 and 33), shared by ``CemPlan`` and
+    ``policy_opt.CemPolicySearch``: the K candidates ``cand`` [K,H,U], the diagonal Gaussian ``mean`` and ``std`` [H,U]
+    they are drawn from, the best so far (``best`` [H,U], ``best_value`` [1]) and ``trace`` [iters,2], with the
+    pilco_cem structs of the first draw and of every iteration's update and the update's workspace.  The candidates'
+    values are ``value`` [K]; population i is drawn from the normals ``xi[i]`` (i < iters), clipped to [-bound,
+    bound]."""
+
+    def __init__(self, K, H, U, elites, iters, alpha, bound, value, xi, mean0, std0):
+        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=device())
+        self.mean0, self.std0 = mean0, std0
+        self.cand, self.mean, self.std, self.best = mk(K, H, U), mk(H, U), mk(H, U), mk(H, U)
+        self.best_value, self.trace = mk(1), mk(iters, 2)
+        cem = lambda xi, trace: _lib.Cem(K, H, U, elites, alpha, -bound, bound, value.data_ptr(), self.cand.data_ptr(),
+                                         xi, self.mean.data_ptr(), self.std.data_ptr(), self.best_value.data_ptr(),
+                                         self.best.data_ptr(), trace)
+        self.draw = cem(xi[0].data_ptr(), None)                 # the first population, then each update's next one
+        self.updates = [cem(xi[i + 1].data_ptr() if i + 1 < iters else None, self.trace[i].data_ptr())
+                        for i in range(iters)]
+        self.uws_bytes = int(lib.pilco_cem_update_workspace_bytes(K))
+        self.uws = torch.empty(max(self.uws_bytes // 8, 2), dtype=F64, device=device())
+
+    def launch(self, evaluate, redraw=None):
+        """the whole loop on the current stream, with no host synchronisation: mean, std and the best back to the
+        start, (``redraw(0)``,) the first draw, then per iteration i ``evaluate()`` (the candidates' values), (before
+        every update but the last ``redraw(i + 1)``, the normals of the next population,) and the update"""
+        self.mean.copy_(self.mean0)
+        self.std.copy_(self.std0)
+        self.best.copy_(self.mean0)
+        self.best_value.fill_(-float("inf"))
+        if redraw is not None:
+            redraw(0)
+        check(lib.pilco_cem_draw(C.byref(self.draw), stream_ptr()), "cem_draw")
+        for i, u in enumerate(self.updates):
+            evaluate()
+            if redraw is not None and i + 1 < len(self.updates):
+                redraw(i + 1)
+            check(lib.pilco_cem_update(C.byref(u), self.uws.data_ptr(), self.uws_bytes, stream_ptr()), "cem_update")
+
+    def capture(self, evaluate, redraw=None):
+        """``launch`` eagerly (a warm-up that sets one-time kernel attributes), then recorded as one CUDA graph, which
+        is returned.  Unreachable cycles are collected first: one that holds an earlier graph would otherwise be freed
+        inside the capture, and freeing a graph's memory there invalidates it."""
+        self.launch(evaluate, redraw)
+        torch.cuda.synchronize()
+        gc.collect()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.launch(evaluate, redraw)
+        return g
+
 
 CEM_BOUND = 0.5 * np.pi          # the candidates' b lie in [-pi/2, pi/2], where u = maxa sin(b) is monotone and onto
 
 
-class CemPlan:
+class CemPlan(_Particles):
     """The cross-entropy method (CEM) over open-loop action sequences on the sampled return, as trajectory-sampling MPC
     plans on a learnt model (PETS, Chua et al. 2018; DESIGN.md section 31), every iteration on the device.
 
@@ -1575,88 +1685,41 @@ class CemPlan:
             raise ValueError("CemPlan: W [Hw,U,Ds] is shared by every candidate: no leading batch dimension")
         if not spec.get("squash", True):
             raise ValueError("CemPlan: the bounds [-pi/2, pi/2] need the squashed policy u = maxa sin(b)")
-        E = int(dyn.struct().E)
-        Ds, U = int(spec["Ds"]), int(spec["U"])
-        ang = angles_struct(angles, E) if angles is not None and len(angles) > 0 else None
-        if Ds != E + (ang.A if ang is not None else 0):
-            raise ValueError("CemPlan: the policy must take %d inputs (the state%s), got %d"
-                             % (E + (ang.A if ang is not None else 0), " with its angles" if ang is not None else "", Ds))
-        nz_var = _particle_noise(measurement_noise, E)
-        self.P, self.H, self.K, self.elites, self.iters, self.alpha = P, H, K, ke, iters, alpha
-        self.E, self.U, self.consistent = E, U, bool(consistent)
-        self.ang, self.keep = ang, [dyn, spec, reward_terms]
-        pr = _lib.Particles()
-        pr.P, pr.H = P, H
-        pr.dyn = dyn.struct()
-        pr.pol.kind, pr.pol.Ds, pr.pol.U = _lib.POLICY_LINEAR, Ds, U      # what the size queries read
-        self.sch = _lib.PolicySchedule(U * Ds, U)              # step t: W[t], cand[r, t]
-        self.nz = None
-        if nz_var is not None:
-            self.nz = _lib.ParticlesNoise()
-            for i, v in enumerate(nz_var):
-                self.nz.v.var[i] = float(v)
-        names = PARTICLE_BATCH_CALLS[self.consistent]
-        self._roll = getattr(lib, "pilco_particles_" + names[0])
-        qz = None                                               # the sizes' noise: nu is checked, not read
-        if self.nz is not None:
-            qz = _lib.ParticlesNoise.from_buffer_copy(self.nz)
-            qz.nu = 16
-        query = lambda R: int(getattr(lib, "pilco_particles_" + names[1])(
-            C.byref(pr), self._ang_ref(), C.byref(qz) if qz is not None else None, C.byref(self.sch), int(R)))
-        if query(1) == 0:
-            raise ValueError("CemPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, pr.dyn.D))
-        if len(reward_terms) > 8:
-            raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
-        if max_ws_bytes is None:
-            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
-        fits = lambda R: 0 < query(R) <= max_ws_bytes
-        if not fits(1):
-            raise ValueError("CemPlan: the rollout of one candidate (P=%d, H=%d, n=%d) needs %d workspace bytes, more "
-                             "than max_ws_bytes=%d" % (P, H, pr.dyn.n, query(1), max_ws_bytes))
-        Rc = _largest_fitting(fits, 1, K)
-        self.max_action, self.W, b, _ = _fill_policy(pr.pol, spec, batched=False)
-        self.rw = _fill_rewards(pr, reward_terms)
-        pr.mult_mu = float(mult_mu)
-        d = device()
-        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
-        self.x0, self.eps_buf = mk(P, E), mk(P, H, E)           # shared by the candidates
-        self.traj, self.act_buf = mk(K, P, H + 1, E), mk(K, P, H, U)
-        self.rew_buf, self.risk_buf, self.ret, self.value = mk(K, P, H), mk(K, P, H), mk(K, P), mk(K)
-        self.cand, self.xi = mk(K, H, U), mk(iters, K, H, U)
-        self.mean0, self.std0 = b[:H].clone(), mk(H, U)
-        self.mean, self.std, self.best_b = mk(H, U), mk(H, U), mk(H, U)
-        self.best_value, self.trace = mk(1), mk(iters, 2)
-        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
-        pr.pol.b_bs = H * U
-        if self.nz is not None:
-            self.nu_buf = mk(P, H, E)
-            self.nz.nu = self.nu_buf.data_ptr()
-        self.ws = torch.empty(max(query(Rc) // 8, 2), dtype=F64, device=d)
-        pr.ws, pr.ws_bytes = self.ws.data_ptr(), query(Rc)
-        self.chunks = []                                        # (description, R, value) of each chunk of candidates
+        E, ang = _policy_width(dyn, spec, angles, "CemPlan")
+        nz = _noise_struct(measurement_noise, E)
+        self.K, self.elites, self.iters, self.alpha, self.consistent = K, ke, iters, alpha, bool(consistent)
+        self._structs(dyn, spec, P, H, ang, nz, schedule=True)
+        entry = lambda R, **slots: self._entry(("scheduled", "consistent" if self.consistent else "step", "batch"),
+                                               R=int(R), **slots)
+        if entry(1).query() == 0:
+            raise ValueError("CemPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, self.pr.dyn.D))
+        _reward_count(reward_terms)
+        Rc = _largest_fitting(lambda R: entry(R).query(), K, max_ws_bytes,
+                              "CemPlan: the rollout of one candidate (P=%d, H=%d, n=%d)" % (P, H, self.pr.dyn.n))
+        self._buffers(spec, reward_terms, mult_mu, (K,), False)
+        pr, U, d = self.pr, self.U, device()
+        pr.pol.b_bs = H * U                                     # step t: W[t], cand[r, t]
+        self.value = torch.zeros(K, dtype=F64, device=d)
+        self.xi = torch.zeros((iters, K, H, U), dtype=F64, device=d)
+        self.mean0, self.std0 = self.b[:H].clone(), torch.zeros((H, U), dtype=F64, device=d)
+        self.loop = CemLoop(K, H, U, ke, iters, alpha, CEM_BOUND, self.value, list(self.xi), self.mean0, self.std0)
+        self.cand, self.mean, self.std, self.best_b = self.loop.cand, self.loop.mean, self.loop.std, self.loop.best
+        self.best_value, self.trace = self.loop.best_value, self.loop.trace
+        self.draw, self.updates, self.uws, self.uws_bytes = self.loop.draw, self.loop.updates, self.loop.uws, \
+            self.loop.uws_bytes
+        wsb = entry(Rc).query()
+        self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
+        pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
+        self.chunks = []                                        # the bound rollout of each chunk of candidates
         for r0 in range(0, K, Rc):
             c = _lib.Particles.from_buffer_copy(pr)
             c.pol.b = self.cand[r0].data_ptr()
             c.traj, c.act = self.traj[r0].data_ptr(), self.act_buf[r0].data_ptr()
             c.step_reward, c.step_risk = self.rew_buf[r0].data_ptr(), self.risk_buf[r0].data_ptr()
             c.ret = self.ret[r0].data_ptr()
-            self.chunks.append((c, min(Rc, K - r0), self.value[r0].data_ptr()))
+            self.chunks.append(entry(min(Rc, K - r0), pr=c, value=self.value[r0].data_ptr()))
         self.chunk = Rc
-        cem = lambda xi, trace: _lib.Cem(K, H, U, ke, alpha, -CEM_BOUND, CEM_BOUND, self.value.data_ptr(),
-                                         self.cand.data_ptr(), xi, self.mean.data_ptr(), self.std.data_ptr(),
-                                         self.best_value.data_ptr(), self.best_b.data_ptr(), trace)
-        self.draw = cem(self.xi[0].data_ptr(), None)            # the first population, then each update's next one
-        self.updates = [cem(self.xi[i + 1].data_ptr() if i + 1 < iters else None, self.trace[i].data_ptr())
-                        for i in range(iters)]
-        self.uws_bytes = int(lib.pilco_cem_update_workspace_bytes(K))
-        self.uws = torch.empty(max(self.uws_bytes // 8, 2), dtype=F64, device=d)
         self.graph = None
-
-    def _ang_ref(self):
-        return C.byref(self.ang) if self.ang is not None else None
-
-    def _nz_ref(self):
-        return C.byref(self.nz) if self.nz is not None else None
 
     def set_inputs(self, x0, eps, xi, nu=None, std0=None):
         """x0 [P,E], eps [P,H,E], xi [iters,K,H,U] (iteration i's population draws xi[i]; row 0 is unread), with
@@ -1674,32 +1737,19 @@ class CemPlan:
 
     def rollout(self):
         """the batched rollout of the current population: value [K] and ``outputs()``"""
-        for c, R, value in self.chunks:
-            check(self._roll(C.byref(c), self._ang_ref(), self._nz_ref(), C.byref(self.sch), R, value, stream_ptr()),
-                  "particles_batch_rollout")
+        for c in self.chunks:
+            c()
         return self.value
 
     def launch(self):
         """the whole plan on the current stream, from the initial mean and std0: no host synchronisation"""
-        self.mean.copy_(self.mean0)
-        self.std.copy_(self.std0)
-        self.best_b.copy_(self.mean0)
-        self.best_value.fill_(-float("inf"))
-        check(lib.pilco_cem_draw(C.byref(self.draw), stream_ptr()), "cem_draw")
-        for u in self.updates:
-            self.rollout()
-            check(lib.pilco_cem_update(C.byref(u), self.uws.data_ptr(), self.uws_bytes, stream_ptr()), "cem_update")
+        self.loop.launch(self.rollout)
         return self.best_b, self.best_value
 
     def capture(self):
-        """record ``launch()`` as one CUDA graph (after an eager warm-up that sets one-time kernel attributes)"""
-        self.launch()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self.launch()
-        self.graph = g
-        return g
+        """record ``launch()`` as one CUDA graph (``CemLoop.capture``)"""
+        self.graph = self.loop.capture(self.rollout)
+        return self.graph
 
     def replay(self):
         self.graph.replay()
@@ -1721,7 +1771,7 @@ PARTICLE_STATIONARY_BATCH_CALLS = {
 }
 
 
-class ParticleBatchPlan:
+class ParticleBatchPlan(_Particles):
     """R stationary policies rolled out forward only over the same P particles (DESIGN.md section 33): the value of
     each, without the reverse sweep or its histories, for the cross-entropy method over policy parameters
     (``policy_opt.CemPolicySearch``).
@@ -1756,13 +1806,8 @@ class ParticleBatchPlan:
             if on:
                 raise ValueError("ParticleBatchPlan: the batched forward rollout does not combine with %s" % what)
         mlp = _particle_mlp(spec, "ParticleBatchPlan", R, angles, measurement_noise)
-        E = int(dyn.struct().E)
-        Ds, U = int(spec["Ds"]), int(spec["U"])
-        ang = angles_struct(angles, E) if angles is not None and len(angles) > 0 else None
-        if Ds != E + (ang.A if ang is not None else 0):
-            raise ValueError("ParticleBatchPlan: the policy must take %d inputs (the state%s), got %d"
-                             % (E + (ang.A if ang is not None else 0), " with its angles" if ang is not None else "", Ds))
-        kind = spec["kind"]
+        E, ang = _policy_width(dyn, spec, angles, "ParticleBatchPlan")
+        Ds, U, kind = int(spec["Ds"]), int(spec["U"]), spec["kind"]
         if kind == _lib.POLICY_LINEAR:
             if np.shape(spec["W"]) != (R, U, Ds) or np.shape(spec["b"]) != (R, U):
                 raise ValueError("ParticleBatchPlan: expected W [R,U,Ds] = %s and b [R,U] = %s, got %s and %s"
@@ -1774,69 +1819,26 @@ class ParticleBatchPlan:
                                  "inputs and U=%d outputs" % (R, Ds, U))
         elif mlp is None:
             raise ValueError("ParticleBatchPlan: unknown policy kind %r" % (kind,))
-        nz_var = _particle_noise(measurement_noise, E)
-        if len(reward_terms) > 8:
-            raise ValueError("at most 8 reward terms per rollout, got %d" % len(reward_terms))
-        self.P, self.H, self.R, self.E, self.Ds, self.U = P, H, R, E, Ds, U
-        self.consistent, self.ang, self.keep = bool(consistent), ang, [dyn, spec, reward_terms]
-        pr = _lib.Particles()
-        pr.P, pr.H = P, H
-        pr.dyn = dyn.struct()
-        pr.pol.kind, pr.pol.Ds, pr.pol.U = kind, Ds, U                   # what the size queries read
-        self.mlp = None
-        if mlp is not None:
-            L, hidden, self.n_theta, _ = mlp
-            self.mlp = _lib.Mlp(L, (C.c_int * 2)(hidden[0], hidden[-1] if L == 2 else 0), None, self.n_theta, None)
-        elif kind == _lib.POLICY_RBF:
-            pr.pol.rbf = spec["gp"].struct()
-        self.nz = None
-        if nz_var is not None:
-            self.nz = _lib.ParticlesNoise()
-            for i, v in enumerate(nz_var):
-                self.nz.v.var[i] = float(v)
-        names = PARTICLE_STATIONARY_BATCH_CALLS[mlp is not None, self.consistent]
-        self._roll = getattr(lib, "pilco_particles_" + names[0])
-        qz = None                                               # the sizes' noise: nu is checked, not read
-        if self.nz is not None:
-            qz = _lib.ParticlesNoise.from_buffer_copy(self.nz)
-            qz.nu = 16
-        if self.mlp is not None:
-            query = lambda r: int(getattr(lib, "pilco_particles_" + names[1])(C.byref(pr), C.byref(self.mlp), int(r)))
-        else:
-            query = lambda r: int(getattr(lib, "pilco_particles_" + names[1])(
-                C.byref(pr), self._ang_ref(), C.byref(qz) if qz is not None else None, int(r)))
-        if query(1) == 0:
-            raise ValueError("ParticleBatchPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, pr.dyn.D))
+        nz = _noise_struct(measurement_noise, E)
+        _reward_count(reward_terms)
+        self.R, self.Ds, self.consistent = R, Ds, bool(consistent)
+        self._structs(dyn, spec, P, H, ang, nz, mlp=mlp, batched=True)
+        entry = lambda r, **slots: self._entry(("mlp" if mlp is not None else "plain",
+                                                "consistent" if self.consistent else "step", "batch"), R=int(r),
+                                               **slots)
+        if entry(1).query() == 0:
+            raise ValueError("ParticleBatchPlan: unsupported sizes (P=%d, H=%d, D=%d)" % (P, H, self.pr.dyn.D))
         per = 8 * P * ((H + 1) * E + H * U + 2 * H + 1)          # one restart's trajectory buffers, in bytes
-        need = lambda r: query(r) + r * per
-        if max_ws_bytes is None:
-            max_ws_bytes = torch.cuda.mem_get_info(device())[0] // 2
-        fits = lambda r: 0 < query(r) and need(r) <= max_ws_bytes
-        if not fits(1):
-            raise ValueError("ParticleBatchPlan: the rollout of one policy (P=%d, H=%d, n=%d) needs %d bytes, more than "
-                             "max_ws_bytes=%d" % (P, H, pr.dyn.n, need(1), max_ws_bytes))
-        Rc = _largest_fitting(fits, 1, R)
-        self.bytes_needed = need
-        self.max_action, self.W, self.b, self.rbf = _fill_policy(pr.pol, spec, batched=True)
-        if self.mlp is not None:
-            self.theta = dev(spec["theta"]).reshape(R, self.n_theta)
-        self.rw = _fill_rewards(pr, reward_terms)
-        pr.mult_mu = float(mult_mu)
-        d = device()
-        mk = lambda *shape: torch.zeros(shape, dtype=F64, device=d)
-        self.x0, self.eps_buf = mk(P, E), mk(P, H, E)           # shared by the policies
-        self.traj, self.act_buf = mk(Rc, P, H + 1, E), mk(Rc, P, H, U)
-        self.rew_buf, self.risk_buf, self.ret, self.value = mk(Rc, P, H), mk(Rc, P, H), mk(Rc, P), mk(R)
-        pr.x0, pr.eps = self.x0.data_ptr(), self.eps_buf.data_ptr()
-        pr.traj, pr.act = self.traj.data_ptr(), self.act_buf.data_ptr()
-        pr.step_reward, pr.step_risk, pr.ret = self.rew_buf.data_ptr(), self.risk_buf.data_ptr(), self.ret.data_ptr()
-        if self.nz is not None:
-            self.nu_buf = mk(P, H, E)
-            self.nz.nu = self.nu_buf.data_ptr()
-        wsb = query(Rc)
+        self.bytes_needed = lambda r: q + r * per if (q := entry(r).query()) else 0
+        Rc = _largest_fitting(self.bytes_needed, R, max_ws_bytes, "ParticleBatchPlan: the rollout of one policy (P=%d, "
+                              "H=%d, n=%d)" % (P, H, self.pr.dyn.n))
+        self._buffers(spec, reward_terms, mult_mu, (Rc,), True)
+        pr, d = self.pr, device()
+        self.value = torch.zeros(R, dtype=F64, device=d)
+        wsb = entry(Rc).query()
         self.ws = torch.empty(max(wsb // 8, 2), dtype=F64, device=d)
         pr.ws, pr.ws_bytes = self.ws.data_ptr(), wsb
-        self.pr, self.chunk, self.chunks = pr, Rc, []           # (description, MLP, R, value) of each chunk
+        self.chunk, self.chunks = Rc, []                        # the bound rollout of each chunk
         for r0 in range(0, R, Rc):
             c, m = _lib.Particles.from_buffer_copy(pr), None
             if self.mlp is not None:
@@ -1848,13 +1850,7 @@ class ParticleBatchPlan:
                 g = self.rbf
                 c.pol.rbf.X, c.pol.rbf.ell = g.X[r0].data_ptr(), g.ell[r0].data_ptr()
                 c.pol.rbf.sf2, c.pol.rbf.beta = g.sf2[r0].data_ptr(), g.beta[r0].data_ptr()
-            self.chunks.append((c, m, min(Rc, R - r0), self.value[r0].data_ptr()))
-
-    def _ang_ref(self):
-        return C.byref(self.ang) if self.ang is not None else None
-
-    def _nz_ref(self):
-        return C.byref(self.nz) if self.nz is not None else None
+            self.chunks.append(entry(min(Rc, R - r0), pr=c, mlp=m, value=self.value[r0].data_ptr()))
 
     def set_inputs(self, x0, eps, nu=None):
         """x0 [P,E], eps [P,H,E] and, with measurement noise, nu [P,H,E] (required then, and only then)"""
@@ -1867,12 +1863,8 @@ class ParticleBatchPlan:
 
     def launch(self):
         """the R rollouts on the current stream, chunk by chunk: no host synchronisation -> value [R]"""
-        for c, m, R, value in self.chunks:
-            if m is not None:
-                rc = self._roll(C.byref(c), C.byref(m), R, value, stream_ptr())
-            else:
-                rc = self._roll(C.byref(c), self._ang_ref(), self._nz_ref(), R, value, stream_ptr())
-            check(rc, "particles_batch_rollout")
+        for c in self.chunks:
+            c()
         return self.value
 
     def outputs(self):

@@ -13,8 +13,6 @@
   ``all_gather`` of ``[loss | flat parameters]`` lets every rank pick the same winner (ties -> lowest
   restart index, the sequential ``>`` comparison of pilco.py:105).  No other collective is used.
 """
-import ctypes as C
-import gc
 import os
 import threading
 import time
@@ -485,20 +483,15 @@ class CemPolicySearch(_FlatEvaluator):
                                              measurement_noise=measurement_noise, max_ws_bytes=max_ws_bytes)
         self.gp = self.plan.rbf
         d = engine.device()
-        mk = lambda *shape: torch.zeros(shape, dtype=torch.float64, device=d)
         self.mean0, self.std0 = engine.dev(self.flat0[0]), engine.dev(std0)
-        self.cand, self.xi = mk(K, n), mk(K, n)
-        self.mean, self.std, self.best, self.best_value, self.trace = mk(n), mk(n), mk(n), mk(1), mk(iters, 2)
+        self.xi = torch.zeros((K, n), dtype=torch.float64, device=d)
         self.its = torch.arange(iters, dtype=torch.int64, device=d)       # population i's normals: iteration i
-        value = self.plan.value
-        cem = lambda xi, trace: _lib.Cem(K, 1, n, ke, self.alpha, -np.inf, np.inf, value.data_ptr(),
-                                         self.cand.data_ptr(), xi, self.mean.data_ptr(), self.std.data_ptr(),
-                                         self.best_value.data_ptr(), self.best.data_ptr(), trace)
-        self.draw = cem(self.xi.data_ptr(), None)
-        self.updates = [cem(self.xi.data_ptr() if i + 1 < iters else None, self.trace[i].data_ptr())
-                        for i in range(iters)]
-        self.uws_bytes = int(_lib.lib.pilco_cem_update_workspace_bytes(K))
-        self.uws = torch.empty(max(self.uws_bytes // 8, 2), dtype=torch.float64, device=d)
+        self.loop = engine.CemLoop(K, 1, n, ke, iters, self.alpha, np.inf, self.plan.value, [self.xi] * iters,
+                                   self.mean0, self.std0)
+        self.cand, self.mean, self.std = self.loop.cand.view(K, n), self.loop.mean.view(n), self.loop.std.view(n)
+        self.best, self.best_value, self.trace = self.loop.best.view(n), self.loop.best_value, self.loop.trace
+        self.draw, self.updates, self.uws, self.uws_bytes = self.loop.draw, self.loop.updates, self.loop.uws, \
+            self.loop.uws_bytes
 
     def set_inputs(self, x0, eps, nu=None):
         self.plan.set_inputs(x0, eps, nu)
@@ -512,32 +505,19 @@ class CemPolicySearch(_FlatEvaluator):
             value.masked_fill_(self.gp.info.reshape(self.K) != 0, float("nan"))
         return value
 
+    def _redraw(self, i):
+        """population i's normals: iteration i under ``seed`` and stream id ``STREAM``"""
+        engine.normals(self.xi, self.seed, self.STREAM, self.its[i:i + 1])
+
     def launch(self):
         """the whole search on the current stream, from the start: no host synchronisation"""
-        self.mean.copy_(self.mean0)
-        self.std.copy_(self.std0)
-        self.best.copy_(self.mean0)
-        self.best_value.fill_(-float("inf"))
-        engine.normals(self.xi, self.seed, self.STREAM, self.its[0:1])
-        _lib.check(_lib.lib.pilco_cem_draw(C.byref(self.draw), engine.stream_ptr()), "cem_draw")
-        for i, u in enumerate(self.updates):
-            self.evaluate()
-            if i + 1 < self.iters:
-                engine.normals(self.xi, self.seed, self.STREAM, self.its[i + 1:i + 2])
-            _lib.check(_lib.lib.pilco_cem_update(C.byref(u), self.uws.data_ptr(), self.uws_bytes, engine.stream_ptr()),
-                       "cem_update")
+        self.loop.launch(self.evaluate, self._redraw)
         return self.best, self.best_value
 
     def run(self):
-        """``launch()`` eagerly (warm-up), then captured as one CUDA graph and replayed once -> (best [n], best_value
-        [1]).  Unreachable cycles are collected first: one that holds an earlier graph would otherwise be freed inside
-        the capture, and freeing a graph's memory there invalidates it.  The graph is released after its replay."""
-        self.launch()
-        torch.cuda.synchronize()
-        gc.collect()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self.launch()
+        """``launch()`` eagerly (warm-up), then captured as one CUDA graph (``engine.CemLoop.capture``) and replayed
+        once -> (best [n], best_value [1]).  The graph is released after its replay."""
+        g = self.loop.capture(self.evaluate, self._redraw)
         g.replay()
         torch.cuda.synchronize()
         del g

@@ -1,13 +1,25 @@
 """Fake C-ABI descriptors for the tests that check argument validation without a GPU: the status codes of
 include/pilco_b200.h and builders of pilco_gp_model, pilco_rollout, pilco_particles (plain and with per-restart
 policies, with angles or measurement noise) and pilco_particles_grad whose pointers are fake non-null addresses, a
-stand-in for a DeviceGP, and the rejected calls of the batched score gradient.  Every entry point validates its
-arguments on the host before it enqueues anything, so only calls that are rejected may be made with them."""
-from pilco_b200 import _lib
+stand-in for a DeviceGP, the rejected calls of the batched score gradient, and the rows of the engine's particle entry
+points called with the engine's own argument order.  Every entry point validates its arguments on the host before it
+enqueues anything, so only calls that are rejected may be made with them."""
+from pilco_b200 import _lib, engine
 
 OK, ERR_NULL, ERR_DIM, ERR_WS, ERR_ALIGN, ERR_LAUNCH, ERR_UNSUP = 0, -1, -2, -3, -4, -5, -6
 FAKE = 0x10000          # 16-byte aligned, never dereferenced by the validation code
 PT_MAX_P = 65535 * 32   # the particle kernels' largest P (and R P)
+
+
+def entry_call(key, query=False, **slots):
+    """row ``key`` of engine.PARTICLE_ENTRY_POINTS with the arguments engine.particle_args binds to ``slots`` and a
+    NULL stream -> its status; ``query``: its size query's result"""
+    name = engine.PARTICLE_ENTRY_POINTS[key][1 if query else 0]
+    args = engine.particle_args(name, **slots)
+    return getattr(_lib.lib, name)(*args) if query else getattr(_lib.lib, name)(*args, None)
+
+
+SAMPLER = {False: "step", True: "consistent", "resampled": "resampled"}     # the host tests' sampler keys
 
 
 def _gp(n=50, D=4, E=3, mode=0, iK=FAKE, ldk=64, bs=0):

@@ -2,7 +2,6 @@
 forward bitwise against the scheduled gradient calls' forward and against single calls, chunking, rerun and graph
 replay; the update fed the device's own values against the numpy oracle; the whole loop against the particle oracle
 and the numpy update; monotonicity; SafePILCO's risk channel; PILCO.plan(optimizer="cem"); the example."""
-import ctypes as C
 import os
 import sys
 
@@ -15,7 +14,6 @@ import particle_oracle as po
 import particle_schedule_oracle as pso
 from particle_cases import _angle_case, _dyn_np
 from pilco_b200 import _lib, controllers, engine, rewards
-from pilco_b200._lib import check, lib
 from pilco_b200.models.pilco import PILCO
 from util import ROOT
 
@@ -44,21 +42,17 @@ class _Batch:
     """the batched forward on a plan's description and output buffers (its own workspace and value)"""
 
     def __init__(self, plan, consistent, R):
-        names = engine.PARTICLE_BATCH_CALLS[consistent]
-        self.fn = getattr(lib, "pilco_particles_" + names[0])
-        self.plan, self.R = plan, R
+        key = ("scheduled", "consistent" if consistent else "step", "batch")
         self.pr = _lib.Particles.from_buffer_copy(plan.pr)
-        wsb = getattr(lib, "pilco_particles_" + names[1])(C.byref(self.pr), plan._ang_ref(), plan._nz_ref(),
-                                                         C.byref(plan.sch), R)
+        wsb = plan._entry(key, pr=self.pr, R=R).query()
         assert wsb > 0
         self.ws = torch.empty(wsb // 8 + 2, dtype=torch.float64, device=engine.device())
         self.pr.ws, self.pr.ws_bytes = self.ws.data_ptr(), wsb
         self.value = torch.zeros(R, dtype=torch.float64, device=engine.device())
+        self.call = plan._entry(key, pr=self.pr, R=R, value=self.value.data_ptr())
 
     def __call__(self):
-        p = self.plan
-        check(self.fn(C.byref(self.pr), p._ang_ref(), p._nz_ref(), C.byref(p.sch), self.R, self.value.data_ptr(),
-                      engine.stream_ptr()), "particles_batch_rollout")
+        self.call()
 
 
 FORWARD = [(False, False), (False, True), (True, False), (True, True)]      # consistent, angles and noise

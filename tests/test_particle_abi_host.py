@@ -225,3 +225,31 @@ def test_golden_has_every_status_of_every_call():
     for j, (call, _, _) in enumerate(CALLS):
         assert set(gold["status"][:, j].tolist()) == CODES, call
     assert (gold["size"] > 0).any(axis=0).all() and (gold["size"] == 0).any(axis=0).all()
+
+
+def test_every_engine_row_binds_its_argtypes():
+    """every row of the engine's PARTICLE_ENTRY_POINTS: the size query is its rollout's pair, and the arguments
+    engine.particle_args binds follow each one's argtypes, one per argtype (the rollout's final stream left out): each
+    struct by reference to the slot of its type (NULL without one), R for the c_int and value for a c_dp"""
+    import ctypes as C
+    from pilco_b200 import engine
+    structs = {t: t._type_ for t in engine._SLOTS if isinstance(getattr(t, "_type_", None), type)}
+    slots = {engine._SLOTS[t]: s() for t, s in structs.items()}
+    slots.update(R=7, value=FAKE)
+    assert len(engine.PARTICLE_ENTRY_POINTS) == 32
+    for key, (run, query) in engine.PARTICLE_ENTRY_POINTS.items():
+        assert run.endswith("_rollout") and query == run[:-len("rollout")] + "workspace_bytes", key
+        for name in (run, query):
+            res, types = _lib.SIGNATURES[name]
+            if res is C.c_int:
+                assert types[-1] is _lib.c_dp, name
+                types = types[:-1]
+            else:
+                assert res is C.c_size_t and _lib.c_dp not in types, name
+            args = engine.particle_args(name, **slots)
+            assert len(args) == len(types) and types[0] is C.POINTER(_lib.Particles), name
+            for a, t in zip(args, types):
+                want = {C.c_int: 7, _lib.c_dp: FAKE}.get(t)
+                assert (a == want) if want is not None else (a._obj is slots[engine._SLOTS[t]]), (name, t)
+            bare = engine.particle_args(name, R=7, value=FAKE)
+            assert all(a is None for a, t in zip(bare, types) if t in structs), name

@@ -15,7 +15,7 @@ import pytest
 
 import cem_oracle as co
 from abi_fakes import (ERR_ALIGN, ERR_DIM, ERR_NULL, ERR_WS, FAKE, PT_MAX_P, _FakeGP, _angles, _batched,
-                       _grad, _noise, _particles)
+                       _grad, _noise, _particles, entry_call)
 from pilco_b200 import _lib, controllers, engine
 from pilco_b200._lib import lib
 from util import CUOBJDUMP, ROOT
@@ -23,7 +23,6 @@ from util import CUOBJDUMP, ROOT
 CALLS = ["pilco_particles_batch_rollout", "pilco_particles_consistent_batch_rollout"]
 MLP_CALLS = ["pilco_particles_mlp_batch_rollout", "pilco_particles_mlp_consistent_batch_rollout"]
 GRAD = ["pilco_particles_explore_batch_grad_rollout", "pilco_particles_explore_consistent_grad_rollout"]
-MLP_GRAD = ["pilco_particles_mlp_batch_grad_rollout", "pilco_particles_mlp_consistent_grad_rollout"]
 N_THETA = 8 * 4 + 6 * 9 + 1 * 7                       # _mlp(): Ds = 3, widths (8, 6), U = 1
 
 
@@ -37,8 +36,8 @@ def test_library_exports_the_entry_points():
         for s in (name, _size(name)):
             assert hasattr(lib, s) and s in _lib.SIGNATURES and s + "(" in header, s
     assert lib.pilco_version() == 3
-    assert sorted(engine.PARTICLE_STATIONARY_BATCH_CALLS.values()) == sorted(
-        (n[len("pilco_particles_"):], _size(n)[len("pilco_particles_"):]) for n in CALLS + MLP_CALLS)
+    assert sorted(v for k, v in engine.PARTICLE_ENTRY_POINTS.items() if k[0] != "scheduled" and k[2] == "batch") == \
+        sorted((n, _size(n)) for n in CALLS + MLP_CALLS)
 
 
 # ---- status codes ------------------------------------------------------------------------------------------------------
@@ -49,27 +48,25 @@ def _mlp(theta=FAKE, bs=N_THETA, L=2, widths=(8, 6)):
     return _lib.Mlp(L, (C.c_int * 2)(*widths), theta, bs, FAKE)
 
 
+def _row(family, consistent, call):
+    return family, "consistent" if consistent else "step", call
+
+
 def _fwd(consistent, pr, R=3, value=FAKE, ang=None, nz=None, query=False):
-    name = CALLS[consistent]
-    if query:
-        return getattr(lib, _size(name))(ref(pr), ref(ang), ref(nz), R)
-    return getattr(lib, name)(ref(pr), ref(ang), ref(nz), R, value, None)
+    return entry_call(_row("plain", consistent, "batch"), query, pr=pr, ang=ang, nz=nz, R=R, value=value)
 
 
 def _grad_call(consistent, pr, R=3, g="default", ang=None, nz=None):
-    return getattr(lib, GRAD[consistent])(ref(pr), ref(ang), ref(nz), None, R, ref(_grad() if g == "default" else g),
-                                          None)
+    return entry_call(_row("plain", consistent, "pathwise"), pr=pr, ang=ang, nz=nz, R=R,
+                      grad=_grad() if g == "default" else g)
 
 
 def _mfwd(consistent, pr, mlp, R=3, value=FAKE, query=False):
-    name = MLP_CALLS[consistent]
-    if query:
-        return getattr(lib, _size(name))(ref(pr), ref(mlp), R)
-    return getattr(lib, name)(ref(pr), ref(mlp), R, value, None)
+    return entry_call(_row("mlp", consistent, "batch"), query, pr=pr, mlp=mlp, R=R, value=value)
 
 
 def _mgrad(consistent, pr, mlp, R=3, g="default"):
-    return getattr(lib, MLP_GRAD[consistent])(ref(pr), ref(mlp), None, R, ref(_grad() if g == "default" else g), None)
+    return entry_call(_row("mlp", consistent, "pathwise"), pr=pr, mlp=mlp, R=R, grad=_grad() if g == "default" else g)
 
 
 def _broken():

@@ -14,7 +14,7 @@ import pytest
 import particle_features_oracle as pfo
 import particle_grad_oracle as pgo
 import particle_oracle as po
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _gp, _grad, _particles
+from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _gp, _grad, _particles, entry_call
 from particle_cases import _problem, _terms
 from pilco_b200 import _lib, engine
 from pilco_b200._lib import lib
@@ -141,22 +141,10 @@ def _mlp(theta=FAKE, gtheta=FAKE):
 
 
 def _call(key, pr, fd, g=None, R=3, query=False, ang=None, nz=None, ex=None, mlp="default"):
-    """row ("features", kind) of engine.PARTICLE_FEATURE_CALLS (lin) or PARTICLE_MLP_CALLS (mlp), as ParticlePlan
-    passes it"""
+    """row (plain (lin) or mlp, "features", kind) of engine.PARTICLE_ENTRY_POINTS"""
     pol, kind = key
-    table = engine.PARTICLE_FEATURE_CALLS if pol == "lin" else engine.PARTICLE_MLP_CALLS
-    names = table["features", kind]
-    ref = lambda s: C.byref(s) if s is not None else None
-    args = [ref(pr)] + ([ref(ang), ref(nz)] if pol == "lin" else [ref(_mlp() if mlp == "default" else mlp)])
-    if kind != "forward":
-        args.append(ref(ex))
-    args.append(ref(fd))
-    if kind != "forward":
-        args.append(R)
-    fn = getattr(lib, "pilco_particles_" + names[1 if query else 0])
-    if query:
-        return fn(*args)
-    return fn(*args, *([ref(g)] if kind != "forward" else []), None)
+    return entry_call(("plain" if pol == "lin" else "mlp", "features", kind), query, pr=pr, ang=ang, nz=nz,
+                      mlp=_mlp() if mlp == "default" else mlp, ex=ex, fd=fd, grad=g, R=R)
 
 
 def _desc(key):

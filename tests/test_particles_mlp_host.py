@@ -14,7 +14,7 @@ import torch
 import particle_grad_oracle as pgo
 import particle_mlp_oracle as pmo
 import particle_oracle as po
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _grad, _particles
+from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, SAMPLER, _batched, _grad, _particles, entry_call
 from particle_cases import _problem, _terms
 from pilco_b200 import _lib, controllers, engine
 from pilco_b200._lib import lib
@@ -112,22 +112,11 @@ def _rs(xi=FAKE):
     return _lib.ParticlesResample(xi, None, None)
 
 
-def _call(key, pr, mlp, g=None, R=3, query=False, rs="default", ex=None):
-    """row ``key`` of engine.PARTICLE_MLP_CALLS, with the arguments ParticlePlan passes"""
+def _call(key, pr, mlp, g=None, R=3, query=False, rs="default", ex=None, family="mlp"):
+    """row (``family``, ``key``) of engine.PARTICLE_ENTRY_POINTS"""
     sampler, kind = key
-    names = engine.PARTICLE_MLP_CALLS[key]
-    ref = lambda s: C.byref(s) if s is not None else None
-    args = [ref(pr), ref(mlp)]
-    if sampler == "resampled":
-        args.append(ref(_rs() if rs == "default" else rs))
-    elif kind != "forward":
-        args.append(ref(ex))
-    if kind != "forward":
-        args.append(R)
-    fn = getattr(lib, "pilco_particles_" + names[1 if query else 0])
-    if query:
-        return fn(*args)
-    return fn(*args, *([ref(g)] if kind != "forward" else []), None)
+    return entry_call((family, SAMPLER[sampler], kind), query, pr=pr, mlp=mlp, grad=g, R=R, ex=ex,
+                      rs=_rs() if rs == "default" else rs)
 
 
 def _desc(key, kind=_lib.POLICY_MLP):
@@ -179,31 +168,19 @@ def test_status_codes_and_their_order(key):
 
 @pytest.mark.parametrize("key", KEYS, ids=lambda k: "%s-%s" % k)
 def test_existing_calls_refuse_the_mlp_kind(key):
-    names = engine.PARTICLE_CALLS[key]
-    sampler, kind = key
-    args = [C.byref(_desc(key))] + ([C.byref(_rs())] if sampler == "resampled" else [None, None])
-    if kind == "pathwise" and sampler != "resampled":
-        args.append(None)
-    if kind != "forward":
-        args.append(3)
-    fn = getattr(lib, "pilco_particles_" + names[0])
-    assert fn(*args, *([C.byref(_grad())] if kind != "forward" else []), None) == ERR_UNSUP
+    assert _call(key, _desc(key), None, _grad(), family="plain") == ERR_UNSUP
 
 
 @pytest.mark.parametrize("key", KEYS, ids=lambda k: "%s-%s" % k)
 def test_workspace_sizes(key):
     """forward: the linear call's workspace; gradients: more, growing with the widths; 0 exactly where the call
     fails on sizes"""
-    lin = engine.PARTICLE_CALLS[key]
     for P, H in ((1000, 5), (7, 0), (300, 12)):
         pr = _desc(key)
         pr.P, pr.H = P, H
         m1, m2, m3 = _call(key, pr, _mlp(L=1, widths=(8, 0)), query=True), _call(key, pr, _mlp(), query=True), \
             _call(key, pr, _mlp(widths=(64, 64)), query=True)
-        args = [C.byref(pr)] + ([C.byref(_rs())] if key[0] == "resampled" else [None, None])
-        if key[1] == "pathwise" and key[0] != "resampled":
-            args.append(None)
-        base = getattr(lib, "pilco_particles_" + lin[1])(*(args + ([3] if key[1] != "forward" else [])))
+        base = _call(key, pr, None, query=True, family="plain")
         assert base > 0
         if key[1] == "forward":
             assert m1 == m2 == m3 == base

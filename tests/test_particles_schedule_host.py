@@ -3,7 +3,6 @@
 policy, the torch gradient per step against central differences of the numpy rollout), and the library side that needs no GPU: exported symbols,
 status codes and their order on fake descriptors, workspace sizes, the new kernels' register budget, and the Python
 refusals raised before any device work."""
-import ctypes as C
 import os
 import re
 import subprocess
@@ -14,7 +13,7 @@ import pytest
 import particle_grad_oracle as pgo
 import particle_oracle as po
 import particle_schedule_oracle as pso
-from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, _batched, _grad, _particles
+from abi_fakes import ERR_DIM, ERR_NULL, ERR_UNSUP, ERR_WS, FAKE, SAMPLER, _batched, _grad, _particles, entry_call
 from particle_cases import _problem, _terms
 from pilco_b200 import _lib, engine
 from pilco_b200._lib import lib
@@ -88,15 +87,17 @@ def test_oracle_gradient_matches_central_differences():
             assert abs(fd - g[k][idx]) <= 1e-7 * max(1.0, abs(fd)), (k, idx, fd, g[k][idx])
 
 
-def _names(scheduled):
-    return (engine.PARTICLE_SCHEDULED_CALLS if scheduled else engine.PARTICLE_CALLS).values()
+def _rows(family):
+    """(sampler, call) -> (rollout, size query) of the family's rows of engine.PARTICLE_ENTRY_POINTS, the batched
+    forward calls (DESIGN.md sections 31 and 33) left out"""
+    return {k[1:]: v for k, v in engine.PARTICLE_ENTRY_POINTS.items() if k[0] == family and k[2] != "batch"}
 
 
 def test_library_exports_the_entry_points():
     header = open(os.path.join(ROOT, "include", "pilco_b200.h")).read()
-    new = [n for pair in _names(True) for n in pair]
-    assert len(set(new)) == 16 and set(engine.PARTICLE_SCHEDULED_CALLS) == set(engine.PARTICLE_CALLS)
-    for name in ("pilco_particles_" + n for n in new):
+    new = [n for pair in _rows("scheduled").values() for n in pair]
+    assert len(set(new)) == 16 and set(_rows("scheduled")) == {k for k in _rows("plain") if k[0] != "features"}
+    for name in new:
         assert hasattr(lib, name) and name in _lib.SIGNATURES and name + "(" in header
 
 
@@ -105,22 +106,10 @@ def _rs():
 
 
 def _call(key, pr, sch, g=None, R=3, scheduled=True, query=False):
-    """the row ``key`` of engine.PARTICLE_CALLS (scheduled: PARTICLE_SCHEDULED_CALLS) with NULL angles, noise and
-    exploration, as ParticlePlan passes them"""
+    """the row (scheduled or plain, ``key``) of engine.PARTICLE_ENTRY_POINTS with NULL angles, noise and exploration"""
     sampler, kind = key
-    names = (engine.PARTICLE_SCHEDULED_CALLS if scheduled else engine.PARTICLE_CALLS)[key]
-    ref = lambda s: C.byref(s) if s is not None else None
-    args = [ref(pr)] + ([C.byref(_rs())] if sampler == "resampled" else [None, None])
-    if kind == "pathwise" and sampler != "resampled":
-        args.append(None)
-    if scheduled:
-        args.append(ref(sch))
-    if kind != "forward":
-        args.append(R)
-    fn = getattr(lib, "pilco_particles_" + names[1 if query else 0])
-    if query:
-        return fn(*args)
-    return fn(*args, *([ref(g)] if kind != "forward" else []), None)
+    return entry_call(("scheduled" if scheduled else "plain", SAMPLER[sampler], kind), query, pr=pr, sch=sch, grad=g,
+                      R=R, rs=_rs())
 
 
 def _desc(key, kind=_lib.POLICY_LINEAR):
