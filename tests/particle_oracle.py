@@ -226,49 +226,56 @@ def _posterior(dyn, A, B):
     return np.stack(out)
 
 
-def _posterior_pairs(dyn, A, B, swap=False):
-    """k_post(A_p, B_p) of row-wise pairs A, B [P,D] -> [P,E]; ``swap``: the quadratic form as k_A (iK k_B) instead of
-    (k_A iK) k_B, the same value with other roundings"""
-    C, ell, sf2, iK = (dyn[k] for k in ("C", "ell", "sf2", "iK"))
-    n = C.shape[0]
-    out = []
-    for e in range(ell.shape[0]):
-        Ka, Kb = se_k(A, C, ell[e], sf2[e]), se_k(B, C, ell[e], sf2[e])
-        d = (A - B) / ell[e][None, :]
-        q = (Ka * (Kb @ iK[e][:n, :n])).sum(1) if swap else ((Ka @ iK[e][:n, :n]) * Kb).sum(1)
-        out.append(sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) - q)
-    return np.stack(out, 1)
-
-
 class FunctionSample:
-    """The running state of one draw per (particle, output): the visited inputs and the packed factor rows.
-    ``step(Xt, eps_t)`` -> f(Xt) [P,E] given the draws at the earlier inputs."""
+    """The running state of one draw per (particle, output): the visited inputs, their K* rows and the packed factor
+    rows.  ``step(Xt, eps_t)`` -> f(Xt) [P,E] given the draws at the earlier inputs.  Written over numpy's generic
+    arithmetic: with ``np.longdouble`` factors, inputs and normals it runs in extended precision."""
 
     def __init__(self, dyn, P, swap=False):
         self.dyn, self.P, self.swap = dyn, P, swap
         self.E = dyn["ell"].shape[0]
         self.X = []              # visited inputs, each [P,D]
+        self.K, self.KiK = [], []    # their K* [E,P,n] and K* iK [E,P,n]
         self.L = []              # rows l [P,E,s] of the factor, below the diagonal
         self.piv = []            # pivots [P,E] (0: degenerate column)
         self.eps = []            # the normals [P,E] of the earlier steps
+        self.mean, self.var = [], []     # each step's mean' = mu + sum_s l_s eps_s and d2 = var - sum_s l_s^2, [P,E]
+
+    def _pairs(self, Xt, K, KiK, s):
+        """k_post(Xt_p, X_s,p) [P,E] (s None: Xt itself).  ``swap``: the quadratic form as k_t (iK k_s) instead of
+        (k_t iK) k_s, the same value with other roundings"""
+        ell, sf2 = self.dyn["ell"], self.dyn["sf2"]
+        Xs, Ks, KiKs = (Xt, K, KiK) if s is None else (self.X[s], self.K[s], self.KiK[s])
+        out = []
+        for e in range(self.E):
+            d = (Xt - Xs) / ell[e][None, :]
+            q = (K[e] * KiKs[e]).sum(1) if self.swap else (KiK[e] * Ks[e]).sum(1)
+            out.append(sf2[e] * np.exp(-0.5 * (d * d).sum(-1)) - q)
+        return np.stack(out, 1)
 
     def step(self, Xt, eps_t):
         dyn, P, E, t = self.dyn, self.P, self.E, len(self.X)
-        sf2 = np.asarray(dyn["sf2"]).reshape(1, E)
-        mu = gp_latent(dyn, Xt)[0]
-        var = _posterior_pairs(dyn, Xt, Xt, self.swap)      # [P,E]
-        l = np.zeros((P, E, t))
+        C, ell, sf2, iK, beta = (dyn[k] for k in ("C", "ell", "sf2", "iK", "beta"))
+        n = C.shape[0]
+        K = np.stack([se_k(Xt, C, ell[e], sf2[e]) for e in range(E)])
+        KiK = np.stack([K[e] @ iK[e][:n, :n] for e in range(E)])
+        mu = np.stack([K[e] @ beta[e] for e in range(E)], 1)
+        var = self._pairs(Xt, K, KiK, None)                 # [P,E]
+        l = np.zeros((P, E, t), dtype=var.dtype)
         for s in range(t):                                  # forward substitution, one column at a time
-            c = _posterior_pairs(dyn, Xt, self.X[s], self.swap)
+            c = self._pairs(Xt, K, KiK, s)
             sub = (self.L[s] * l[:, :, :s]).sum(-1) if s else 0.0
             piv = self.piv[s]
             l[:, :, s] = np.where(piv > 0.0, (c - sub) / np.where(piv > 0.0, piv, 1.0), 0.0)
         d2 = var - (l * l).sum(-1)
         f = mu + np.sqrt(np.maximum(d2, 0.0)) * eps_t
+        mean = mu
         if t:
-            f = f + (l * np.stack(self.eps, -1)).sum(-1)
-        self.X.append(Xt.copy()); self.L.append(l); self.eps.append(eps_t.copy())
-        self.piv.append(np.where(d2 > TAU * sf2, np.sqrt(np.maximum(d2, 0.0)), 0.0))
+            le = (l * np.stack(self.eps, -1)).sum(-1)
+            f, mean = f + le, mu + le
+        self.X.append(Xt.copy()); self.K.append(K); self.KiK.append(KiK)
+        self.L.append(l); self.eps.append(eps_t.copy()); self.mean.append(mean); self.var.append(d2)
+        self.piv.append(np.where(d2 > TAU * np.asarray(sf2).reshape(1, E), np.sqrt(np.maximum(d2, 0.0)), 0.0))
         return f
 
 
